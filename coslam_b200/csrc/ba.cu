@@ -20,7 +20,6 @@
 #include <vector>
 
 #include "ba_kernels.cuh"
-#include "ba_schur_blk.cuh"
 #include "ba_tile.cuh"
 #include "common.cuh"
 
@@ -102,7 +101,7 @@ struct cosl_ba_solver {
   BaBwdEntry* d_bwd = nullptr;
   BaSumEntry* d_sum = nullptr;
   double* d_rhsS = nullptr;
-  int *d_blkRows = nullptr, *d_blkRow0 = nullptr, *d_tileIdx = nullptr, *d_diagBlk = nullptr,
+  int *d_blkRows = nullptr, *d_diagBlk = nullptr,
       *d_blkCam0 = nullptr, *d_order = nullptr, *d_solIdx = nullptr;
   BaTileDev td;
   std::vector<BaTask> taskOrder;  // as uploaded: [POTRF / BACKWARD | TRSM / UPDATE / SUM]
@@ -113,30 +112,14 @@ struct cosl_ba_solver {
   double* d_sc = nullptr;
   unsigned char* d_outlier = nullptr;
   BaPairItem* d_items = nullptr;
-  BaRowDst* d_rowDst = nullptr;
-  int4* d_visit = nullptr;
-  int* d_cptrFree = nullptr;
   double* d_Vinv = nullptr;
-  int nSlots = 1;
-  size_t rowsSmem = 0;
-  bool useRows = false;
-  cudaEvent_t evBlock = nullptr;  // blocking-sync event of the multi-GPU scalar read-back
   bool costDone = false;         // solve_trial already evaluated the trial cost (ba_finish_cost)
   bool statsPending = false;     // |g|_inf / max diag of the last linearisation still to be computed (prep kernel)
   unsigned long long scSeq = 0;  // sequence number of the last scalar read-back (ba_publish_sc)
-  bool useBlk = false;     // camera-block DMMA contraction (COSL_BA_SCHUR_BLK=1)
-  BaVisit* d_bvis = nullptr;
-  BaBlkItem* d_bitems = nullptr;
-  BaBlkDst* d_btabs = nullptr;
-  int nBItems = 0;
-  long long nVisits = 0;
-  bool schurSimt = false;  // COSL_BA_SCHUR_SIMT=1: scalar-gather pair kernel instead of the staged one
-  int rowSplits = 1;
   int4* d_entries = nullptr;
   int nItems = 0;
   long long nEntries = 0;
   double* h_sc = nullptr;  // pinned
-  bool smallSolve = true;
   bool twoSolve = false;  // <= 2 blocks: single-CTA resident solve (ba_tile_two)
   int two00 = -1, two10 = -1, two11 = -1;
   SectionTimer timer;
@@ -325,13 +308,11 @@ void free_solver(cosl_ba_solver* s) {
                   s->d_cam, s->d_pt, s->d_cobs, s->d_ccam, s->d_xy, s->d_wgt, s->d_ptr, s->d_W,
                   s->d_V, s->d_S, s->d_y, s->d_x, s->d_sc, s->d_outlier,
                   s->d_items, s->d_entries, s->d_Linv, s->d_cnt, s->d_tasks, s->d_bwd, s->d_blkRows,
-                  s->d_blkRow0, s->d_tileIdx, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_solIdx,
-                  s->d_trace, s->d_sum, s->d_rhsS, s->d_rowDst, s->d_cptrFree, s->d_Vinv, s->d_visit,
-                  s->d_bvis, s->d_bitems, s->d_btabs};
+                  s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_solIdx,
+                  s->d_trace, s->d_sum, s->d_rhsS, s->d_Vinv};
   for (void* b : bufs)
     if (b) cudaFreeAsync(b, s->stream);
   if (s->stream) cudaStreamSynchronize(s->stream);
-  if (s->evBlock) cudaEventDestroy(s->evBlock);
   if (s->h_sc) pinned_slots().put(s->h_sc);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
@@ -439,13 +420,6 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   for (int ja = 0; ja < mf; ++ja)
     for (int jb = ja; jb < mf; ++jb)
       if (poff[(size_t)ja * mf + jb + 1] > poff[(size_t)ja * mf + jb]) adj[(size_t)ja * mf + jb] = adj[(size_t)jb * mf + ja] = 1;
-  auto run_threads = [&](int T, auto&& body) {
-    std::vector<std::thread> th;
-    for (int t = 1; t < T; ++t) th.emplace_back(body, t);
-    body(0);
-    for (auto& x : th) x.join();
-  };
-  (void)run_threads;
   if (s->comm && s->comm->nranks > 1 && mf > 0) {
     uint8_t* d_adj = nullptr;
     COSL_TRY(tmp.alloc(&d_adj, adj.size()));
@@ -456,10 +430,8 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     COSL_CUDA(cudaStreamSynchronize(s->stream));
   }
   {
-    int ndDepth = -1;
-    if (const char* e = std::getenv("COSL_BA_ND_DEPTH")) ndDepth = std::atoi(e);
     const double tPlan0 = now_s();
-    s->plan = ba_make_plan(mf, adj, ndDepth);
+    s->plan = ba_make_plan(mf, adj);
     if (ba_timing()) std::fprintf(stderr, "[ba timing] plan %.1f ms\n", 1e3 * (now_s() - tPlan0));
     if (s->plan.nb < 0) return set_error(COSL_E_INVALID, "solve plan: dependency cycle (internal error)");
   }
@@ -477,207 +449,40 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     rOff = bLater ? oB : oA;
     return true;
   };
-  // band of the reduced camera system in the natural camera order -> camera-row Schur kernel
-  int bandw = 0;
-  for (int ja = 0; ja < mf; ++ja)
-    for (int jb = mf - 1; jb > ja + bandw; --jb)
-      if (adj[(size_t)ja * mf + jb]) {
-        bandw = jb - ja;
-        break;
-      }
-  s->nSlots = bandw + 1;
-  s->rowsSmem = sizeof(double) * (size_t)BA_ROWS_WARPS * ((size_t)s->nSlots * 36 + 8);
-  // The camera-row kernel halves the DRAM traffic and needs no atomics but is L1TEX-bound on its
-  // 24-byte row reads: 0.75 ms vs 0.50 ms for the staged pair lists (Schur time per LM trial at c4 on
-  // an H100 80GB HBM3, 700 W), so the pair-list kernel stays the default; COSL_BA_SCHUR_ROWS=1 selects it.
-  s->useRows = mf > 0 && s->rowsSmem <= 160 * 1024 && std::getenv("COSL_BA_SCHUR_ROWS") != nullptr;
-  // few cameras with long observation lists (local BA): split each list over several CTAs
-  s->rowSplits = (mf > 0 && mf < 296) ? std::max(1, std::min(64, 296 / mf)) : 1;
-  if (Nc / std::max(1, mf * s->rowSplits) < 64) s->rowSplits = std::max(1, (int)(Nc / 64 / std::max(1, mf)));
-  std::vector<BaRowDst> rowDst;
-  std::vector<int> cptrFree(mf + 1, 0);
-  std::vector<int4> visit;
+  // pair lists: one bucket per camera pair (offsets counted on the device above); a work item is
+  // a run of <= 512 entries of one bucket; the entries themselves are placed by ba_pairs_build.
+  // Fewer entries per item when the problem is small (local BA: a few dozen camera pairs with
+  // thousands of entries each), so that the grid still fills the GPU; ba_schur_pairs_st works in
+  // batches of 32 entries and sums 32 lanes per item: multiples of 32, >= 128
   std::vector<BaPairItem> items;
-  long long nEntries = 0;
-  if (s->useRows) {
-    rowDst.assign((size_t)mf * s->nSlots, BaRowDst{-1, 0, 0, 0});
-    for (int ja = 0; ja < mf; ++ja)
-      for (int sl = 0; sl < s->nSlots && ja + sl < mf; ++sl)
-        if (adj[(size_t)ja * mf + ja + sl]) {
-          BaRowDst& r = rowDst[(size_t)ja * s->nSlots + sl];
-          if (!pair_dst(ja, ja + sl, r.dst, r.rOff, r.cOff, r.trans))
-            return set_error(COSL_E_INVALID, "solve plan: missing tile");
-        }
-    for (int jf = 0; jf <= mf; ++jf) cptrFree[jf] = (int)cptr[std::min(m, jf + mcon)];
-    visit.resize((size_t)Nc);
-    for (long long q = 0; q < Nc; ++q) {
-      const int o = cobs[q], i = pt[o];
-      visit[q] = make_int4(o, i, (int)p->ptr[i], (int)(p->ptr[i + 1] - p->ptr[i]));
-    }
-  }
-  // camera-block visits (ba_schur_blk.cuh): default contraction unless a point touches too many blocks
-  // Correct, but 0.86 ms vs 0.50 ms for the staged pair lists (Schur time per LM trial at c4 on an H100
-  // 80GB HBM3, 700 W) -- in the benchmark scene a point is seen by ~13 of ~36 candidate cameras, so even with
-  // co-visibility blocking a visit holds only 3.5 of 16 possible pairs (DMMAs mostly multiply zeros and
-  // the per-visit staging overhead dominates).  COSL_BA_SCHUR_BLK=1 selects it; pair lists stay the default.
-  s->useBlk = !s->useRows && mf > 0 && std::getenv("COSL_BA_SCHUR_BLK") != nullptr;
-  if (s->useBlk) {
-    // blocks of <= BA_CB cameras by co-visibility: seed = first unassigned camera, then repeatedly the
-    // unassigned camera sharing the most points with the block so far (pair counts from the bucket scan)
-    std::vector<int> camBlock(mf, -1), camSlot(mf, 0), blkCams;
-    auto pairCnt = [&](int a, int b) -> long long {
-      if (a > b) std::swap(a, b);
-      return (long long)poff[(size_t)a * mf + b + 1] - (long long)poff[(size_t)a * mf + b];
-    };
-    int nB = 0;
-    {
-      std::vector<long long> score(mf);
-      for (int j = 0; j < mf; ++j) {
-        if (camBlock[j] >= 0) continue;
-        camBlock[j] = nB;
-        camSlot[j] = 0;
-        blkCams.push_back(j);
-        std::fill(score.begin(), score.end(), 0);
-        int last = j;
-        int filled = 1;
-        for (; filled < BA_CB; ++filled) {
-          long long best = 0;
-          int bestK = -1;
-          for (int k = 0; k < mf; ++k) {
-            if (camBlock[k] >= 0) continue;
-            score[k] += pairCnt(last, k);
-            if (score[k] > best) {
-              best = score[k];
-              bestK = k;
-            }
-          }
-          if (bestK < 0) break;
-          camBlock[bestK] = nB;
-          camSlot[bestK] = filled;
-          blkCams.push_back(bestK);
-          last = bestK;
-        }
-        for (; filled < BA_CB; ++filled) blkCams.push_back(-1);
-        ++nB;
+  const long long nEntries = poff[nBuckets];
+  const int chunk = (int)(32 * std::max<long long>(4, std::min<long long>(16, nEntries / (4096 * 32))));
+  for (int ja = 0; ja < mf; ++ja)
+    for (int jb = ja; jb < mf; ++jb) {
+      const long long b0 = poff[(size_t)ja * mf + jb], b1 = poff[(size_t)ja * mf + jb + 1];
+      if (b1 == b0) continue;
+      BaPairItem it;
+      std::memset(&it, 0, sizeof(it));
+      it.rowCam = ja;
+      it.colCam = jb;
+      if (!pair_dst(ja, jb, it.dst, it.rOff, it.cOff, it.trans))
+        return set_error(COSL_E_INVALID, "solve plan: missing tile");
+      it.rhsIdx = P.camBlk[ja] * BA_TB + P.camOff[ja];
+      for (long long b = b0; b < b1; b += chunk) {
+        it.begin = (int)b;
+        it.end = (int)std::min(b1, b + chunk);
+        items.push_back(it);
       }
     }
-    int *d_camBlock = nullptr, *d_camSlot = nullptr;
-    COSL_TRY(tmp.alloc(&d_camBlock, (size_t)mf));
-    COSL_TRY(tmp.alloc(&d_camSlot, (size_t)mf));
-    COSL_CUDA(cudaMemcpyAsync(d_camBlock, camBlock.data(), sizeof(int) * mf, cudaMemcpyHostToDevice, s->stream));
-    COSL_CUDA(cudaMemcpyAsync(d_camSlot, camSlot.data(), sizeof(int) * mf, cudaMemcpyHostToDevice, s->stream));
-    const size_t nBB = (size_t)nB * nB;
-    unsigned *d_vcnt = nullptr, *d_voff = nullptr;
-    int* d_ovf = nullptr;
-    COSL_TRY(tmp.alloc(&d_vcnt, nBB + 1));
-    COSL_TRY(tmp.alloc(&d_voff, nBB + 1));
-    COSL_TRY(tmp.alloc(&d_ovf, (size_t)1));
-    COSL_CUDA(cudaMemsetAsync(d_vcnt, 0, sizeof(unsigned) * (nBB + 1), s->stream));
-    COSL_CUDA(cudaMemsetAsync(d_ovf, 0, sizeof(int), s->stream));
-    BaDev dv = db;
-    dv.n = n;
-    std::vector<unsigned> voff(nBB + 1, 0u);
-    int ovf = 0;
-    if (n > ncon) {
-      COSL_LAUNCH(ba_visits_build<false>, (unsigned)div_up(n - ncon, 128), 128, 0, s->stream, dv, nB, d_camBlock, d_camSlot,
-                  d_vcnt, d_voff, nullptr, d_ovf);
-      COSL_LAUNCH(ba_scan_u32, 1, 1024, 0, s->stream, d_vcnt, d_voff, (long long)nBB);
-      COSL_CUDA(cudaMemcpyAsync(voff.data(), d_voff, sizeof(unsigned) * (nBB + 1), cudaMemcpyDeviceToHost, s->stream));
-      COSL_CUDA(cudaMemcpyAsync(&ovf, d_ovf, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
-    }
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
-    if (ovf) {
-      s->useBlk = false;  // a point seen from > BA_VIS_MAXB camera blocks: pair lists handle any structure
-    } else {
-      s->nVisits = voff[nBB];
-      // a work item = a run of visits of one block pair (one warp); aim at >= ~8 items per SM-resident warp
-      const long long chunkV = 4 * std::max<long long>(8, std::min<long long>(64, s->nVisits / (4096 * 4)));
-      std::vector<BaBlkItem> bitems;
-      std::vector<BaBlkDst> btabs;
-      for (int A = 0; A < nB; ++A)
-        for (int B = A; B < nB; ++B) {
-          const long long b0 = voff[(size_t)A * nB + B], b1 = voff[(size_t)A * nB + B + 1];
-          if (b1 == b0) continue;
-          BaBlkDst tab;
-          for (int a = 0; a < BA_CB; ++a) {
-            const int ja = blkCams[(size_t)A * BA_CB + a];
-            tab.rhsIdx[a] = ja >= 0 ? P.camBlk[ja] * BA_TB + P.camOff[ja] : -1;
-            for (int b = 0; b < BA_CB; ++b) {
-              const int jb = blkCams[(size_t)B * BA_CB + b], t = a * BA_CB + b;
-              tab.dst[t] = -1;
-              tab.rOff[t] = tab.cOff[t] = tab.trans[t] = 0;
-              if (ja < 0 || jb < 0 || (A == B && a > b) || !adj[(size_t)ja * mf + jb]) continue;
-              if (!pair_dst(ja, jb, tab.dst[t], tab.rOff[t], tab.cOff[t], tab.trans[t]))
-                return set_error(COSL_E_INVALID, "solve plan: missing tile");
-            }
-          }
-          BaBlkItem it;
-          std::memset(&it, 0, sizeof(it));
-          it.A = A;
-          it.B = B;
-          it.tab = (int)btabs.size();
-          btabs.push_back(tab);
-          for (long long b = b0; b < b1; b += chunkV) {
-            it.begin = (int)b;
-            it.end = (int)std::min(b1, b + chunkV);
-            bitems.push_back(it);
-          }
-        }
-      s->nBItems = (int)bitems.size();
-      COSL_TRY(dev_alloc(s->stream, &s->d_bvis, (size_t)std::max<long long>(1, s->nVisits)));
-      COSL_TRY(dev_alloc(s->stream, &s->d_bitems, std::max<size_t>(1, bitems.size())));
-      COSL_TRY(dev_alloc(s->stream, &s->d_btabs, std::max<size_t>(1, btabs.size())));
-      if (!bitems.empty()) {
-        COSL_CUDA(cudaMemcpyAsync(s->d_bitems, bitems.data(), sizeof(BaBlkItem) * bitems.size(), cudaMemcpyHostToDevice, s->stream));
-        COSL_CUDA(cudaMemcpyAsync(s->d_btabs, btabs.data(), sizeof(BaBlkDst) * btabs.size(), cudaMemcpyHostToDevice, s->stream));
-        COSL_CUDA(cudaMemsetAsync(d_vcnt, 0, sizeof(unsigned) * (nBB + 1), s->stream));
-        COSL_LAUNCH(ba_visits_build<true>, (unsigned)div_up(n - ncon, 128), 128, 0, s->stream, dv, nB, d_camBlock, d_camSlot,
-                    d_vcnt, d_voff, s->d_bvis, d_ovf);
-        COSL_CUDA(cudaStreamSynchronize(s->stream));  // bitems / btabs are host vectors of this scope
-      }
-      nEntries = poff[nBuckets];
-    }
-    if (ba_timing())
-      std::fprintf(stderr, "[ba timing] camera-block visits: %d blocks, %lld visits (%.2f pair entries per visit), %d items\n",
-                   nB, s->nVisits, s->nVisits ? (double)poff[nBuckets] / (double)s->nVisits : 0.0, s->nBItems);
-  }
-  if (!s->useRows && !s->useBlk) {
-    // pair lists: one bucket per camera pair (offsets counted on the device above); a work item is
-    // a run of <= 512 entries of one bucket; the entries themselves are placed by ba_pairs_build
-    nEntries = poff[nBuckets];
-    // <= 512 entries per work item (one warp); fewer when the problem is small (local BA: a few
-    // dozen camera pairs with thousands of entries each), so that the grid still fills the GPU
-    s->schurSimt = std::getenv("COSL_BA_SCHUR_SIMT") != nullptr;
-    // the staged kernel works in batches of 32 entries and sums 32 lanes per item: multiples of 32, >= 128
-    const int chunk = s->schurSimt ? (int)std::max<long long>(64, std::min<long long>(512, nEntries / 4096))
-                                   : (int)(32 * std::max<long long>(4, std::min<long long>(16, nEntries / (4096 * 32))));
-    for (int ja = 0; ja < mf; ++ja)
-      for (int jb = ja; jb < mf; ++jb) {
-        const long long b0 = poff[(size_t)ja * mf + jb], b1 = poff[(size_t)ja * mf + jb + 1];
-        if (b1 == b0) continue;
-        BaPairItem it;
-        std::memset(&it, 0, sizeof(it));
-        it.rowCam = ja;
-        it.colCam = jb;
-        if (!pair_dst(ja, jb, it.dst, it.rOff, it.cOff, it.trans))
-          return set_error(COSL_E_INVALID, "solve plan: missing tile");
-        it.rhsIdx = P.camBlk[ja] * BA_TB + P.camOff[ja];
-        for (long long b = b0; b < b1; b += chunk) {
-          it.begin = (int)b;
-          it.end = (int)std::min(b1, b + chunk);
-          items.push_back(it);
-        }
-      }
-    COSL_TRY(dev_alloc(s->stream, &s->d_entries, (size_t)nEntries));
-    COSL_CUDA(cudaMemsetAsync(d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->stream));
-    if (nEntries)
-      COSL_LAUNCH(ba_pairs_build<true>, (unsigned)div_up64(Nc, 256), 256, 0, s->stream, db, d_pcnt, d_poff, s->d_entries);
-  }
+  COSL_TRY(dev_alloc(s->stream, &s->d_entries, (size_t)nEntries));
+  COSL_CUDA(cudaMemsetAsync(d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->stream));
+  if (nEntries)
+    COSL_LAUNCH(ba_pairs_build<true>, (unsigned)div_up64(Nc, 256), 256, 0, s->stream, db, d_pcnt, d_poff, s->d_entries);
   s->nEntries = nEntries;
   s->nItems = (int)items.size();
   if (ba_timing())
-    std::fprintf(stderr, "[ba timing] co-visibility + Schur work lists %.1f ms (%s, band %d, %lld pair entries, %d threads)\n",
-                 1e3 * (now_s() - tPair0), s->useRows ? "camera rows" : "pair lists", bandw, nEntries, host_threads());
+    std::fprintf(stderr, "[ba timing] co-visibility + Schur work lists %.1f ms (%lld pair entries, %d threads)\n",
+                 1e3 * (now_s() - tPair0), nEntries, host_threads());
   // intrinsics: only K0,K1,K2,K4,K5 are used (as BundleRTS packs them, app/SL_CoSLAMBA.cpp:337-343)
   std::vector<double> camK((size_t)m * 5);
   for (int j = 0; j < m; ++j) {
@@ -719,24 +524,16 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   COSL_TRY(dev_alloc(s->stream, &s->d_tasks, P.tasks.size()));
   COSL_TRY(dev_alloc(s->stream, &s->d_bwd, P.bwdList.size()));
   COSL_TRY(dev_alloc(s->stream, &s->d_blkRows, (size_t)nb));
-  COSL_TRY(dev_alloc(s->stream, &s->d_blkRow0, (size_t)nb + 1));
-  COSL_TRY(dev_alloc(s->stream, &s->d_tileIdx, (size_t)nb * nb));
   COSL_TRY(dev_alloc(s->stream, &s->d_diagBlk, (size_t)nTiles));
   COSL_TRY(dev_alloc(s->stream, &s->d_blkCam0, (size_t)nb + 1));
   COSL_TRY(dev_alloc(s->stream, &s->d_order, (size_t)std::max(1, mf)));
   COSL_TRY(dev_alloc(s->stream, &s->d_solIdx, (size_t)std::max(1, mf)));
-  std::vector<int> h_blkRow0(nb + 1, 0), h_diagBlk(nTiles, -1), h_solIdx(std::max(1, mf), 0);
-  for (int k = 0; k < P.nb; ++k) {
-    h_blkRow0[k + 1] = h_blkRow0[k] + P.blkRows[k];
-    h_diagBlk[P.tileIdx[(size_t)k * P.nb + k]] = k;
-  }
+  std::vector<int> h_diagBlk(nTiles, -1), h_solIdx(std::max(1, mf), 0);
+  for (int k = 0; k < P.nb; ++k) h_diagBlk[P.tileIdx[(size_t)k * P.nb + k]] = k;
   for (int j = 0; j < mf; ++j) h_solIdx[j] = P.camBlk[j] * BA_TB + P.camOff[j];
   COSL_TRY(dev_alloc(s->stream, &s->d_sc, (size_t)SC_NTOT));
   COSL_TRY(dev_alloc(s->stream, &s->d_outlier, (size_t)N));
   COSL_TRY(dev_alloc(s->stream, &s->d_items, items.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_rowDst, rowDst.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_visit, visit.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_cptrFree, cptrFree.size()));
   COSL_TRY(dev_alloc(s->stream, &s->d_Vinv, (size_t)n * 6));
   static_assert(SC_NTOT <= 16, "pinned slot size");
   s->h_sc = pinned_slots().get();
@@ -748,9 +545,6 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   UP(s->d_camK, camK.data(), sizeof(double) * 5 * m);
   UP(s->d_xy, p->xy, sizeof(double) * 2 * (size_t)N);
   if (!items.empty()) UP(s->d_items, items.data(), sizeof(BaPairItem) * items.size());
-  if (!rowDst.empty()) UP(s->d_rowDst, rowDst.data(), sizeof(BaRowDst) * rowDst.size());
-  if (!visit.empty()) UP(s->d_visit, visit.data(), sizeof(int4) * visit.size());
-  UP(s->d_cptrFree, cptrFree.data(), sizeof(int) * cptrFree.size());
   // two ticket lists (each keeps the critical-path-first order, hence stays topological)
   s->taskOrder.clear();
   for (const BaTask& t : P.tasks)
@@ -761,7 +555,6 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   {
     // hot successors of every POTRF(k): TRSM(j, k) and the diagonal UPD(j, j, k) of j = first block
     // of struct(k) -- the next pivot of the dependency chain (ba_tile.cuh)
-    const bool hotOn = std::getenv("COSL_BA_NO_HOT") == nullptr;
     std::vector<int> firstTrsm(P.nb, -1), firstRow(P.nb, 1 << 30);
     for (int t = 0; t < (int)s->taskOrder.size(); ++t) {
       const BaTask& k = s->taskOrder[t];
@@ -777,8 +570,8 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     }
     for (BaTask& k : s->taskOrder)
       if (k.type == BA_T_POTRF) {
-        k.l0 = hotOn ? firstTrsm[k.k] : -1;
-        k.l1 = hotOn ? diagUpd[k.k] : -1;
+        k.l0 = firstTrsm[k.k];
+        k.l1 = diagUpd[k.k];
       }
   }
   if (!s->taskOrder.empty()) UP(s->d_tasks, s->taskOrder.data(), sizeof(BaTask) * s->taskOrder.size());
@@ -786,11 +579,9 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   if (!P.sumList.empty()) UP(s->d_sum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
   if (P.nb) {
     UP(s->d_blkRows, P.blkRows.data(), sizeof(int) * P.nb);
-    UP(s->d_tileIdx, P.tileIdx.data(), sizeof(int) * (size_t)P.nb * P.nb);
     UP(s->d_blkCam0, P.blkCam0.data(), sizeof(int) * (P.nb + 1));
     UP(s->d_order, P.order.data(), sizeof(int) * mf);
   }
-  UP(s->d_blkRow0, h_blkRow0.data(), sizeof(int) * (nb + 1));
   UP(s->d_diagBlk, h_diagBlk.data(), sizeof(int) * nTiles);
   UP(s->d_solIdx, h_solIdx.data(), sizeof(int) * std::max(1, mf));
 #undef UP
@@ -844,32 +635,19 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   td.sc = s->d_sc;
   td.scFail = (int)SC_FAIL;
   td.trace = nullptr;
-  // small systems (local BA) are factored inside one CTA (ns*ns doubles of shared memory)
-  const size_t smallBytes = sizeof(double) * (size_t)s->ns * s->ns;
-  // For the 72 x 72 system of the c3 local BA the one-CTA dense kernel needs 96 us per LM trial (72
-  // pivots x 3 CTA barriers), the task kernel 43 us and ba_tile_two (below) 26 us (H100 80GB HBM3,
-  // 700 W), so the task kernels are the default everywhere.  COSL_BA_SMALL_KERNEL=1 selects
-  // the dense kernel.
-  if (P.nb >= 1 && P.nb <= 2 && std::getenv("COSL_BA_NO_TWO_KERNEL") == nullptr) {
+  // Systems of one or two blocks (local BA) are solved by one resident CTA: for the 72 x 72 system of
+  // the c3 local BA, ba_tile_two needs 26 us per LM trial and the task kernel 42 us (H100 80GB HBM3, 400 W).
+  if (P.nb >= 1 && P.nb <= 2) {
     s->twoSolve = true;
     s->two00 = P.tileIdx[0];
     s->two10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
     s->two11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
     if (s->two00 < 0 || (P.nb == 2 && s->two11 < 0)) s->twoSolve = false;
   }
-  s->smallSolve = (smallBytes <= 200 * 1024) && s->ns <= 1024 && std::getenv("COSL_BA_SMALL_KERNEL") != nullptr;
-  // (the kernel also has ~8 KB of static shared memory, so opt in well below the 48 KB default)
-  if (s->smallSolve && smallBytes > 32 * 1024)
-    COSL_CUDA(cudaFuncSetAttribute(ba_tile_small, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)smallBytes));
   COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_schur_pairs_st, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_ST_SMEM));
-  COSL_CUDA(cudaFuncSetAttribute(ba_schur_blk, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_BLK_SMEM));
-  if (s->useRows && s->rowsSmem > 40 * 1024)
-    COSL_CUDA(cudaFuncSetAttribute(ba_schur_rows, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)s->rowsSmem));
   {
     // persistent grid: never more CTAs than can be co-resident (the ticket scheduler spins)
     int nsm = 0, perSm = 0;
@@ -877,12 +655,10 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     s->numSM = std::max(1, nsm);
     COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS,
                                                             BA_TILE_SMEM));
-    int grid = nsm * std::max(1, std::min(perSm, 1));
-    if (const char* e = std::getenv("COSL_BA_SOLVE_GRID")) grid = std::max(2, std::min(std::atoi(e), nsm * std::max(1, perSm)));
+    const int grid = nsm * std::max(1, std::min(perSm, 1));
     s->solveGrid = std::max(2, std::min(grid, td.nTasks + 1));
     // CTAs that only ever run the diagonal-block tasks (see BaTileDev::nSpecial)
-    int nsp = std::min(24, std::max(1, s->solveGrid / 6));
-    if (const char* e = std::getenv("COSL_BA_SPECIAL")) nsp = std::atoi(e);
+    const int nsp = std::min(24, std::max(1, s->solveGrid / 6));
     td.nSpecial = std::max(1, std::min(nsp, s->solveGrid - 1));
   }
   s->secLin = s->timer.section("ba_linearize");
@@ -917,7 +693,7 @@ int zero_sc(cosl_ba_solver* s, int first, int count) {
 // Scalars of a trial -> host.  Instead of a copy-engine transfer + stream synchronise (microseconds of latency per
 // LM trial), a 32-thread kernel stores the 16 scalars into MAPPED pinned host memory, fences, and stores a
 // sequence number; the host spins on that word.  Falls back to a stream synchronise if the flag does not
-// arrive (error on the stream) or with COSL_BA_SYNC_READBACK=1.
+// arrive (error on the stream).
 __global__ void ba_publish_sc(const double* __restrict__ sc, volatile double* host, unsigned long long seq) {
   if (threadIdx.x < SC_NTOT) host[threadIdx.x] = sc[threadIdx.x];
   __threadfence_system();
@@ -929,22 +705,14 @@ __global__ void ba_publish_sc(const double* __restrict__ sc, volatile double* ho
 }
 
 int read_sc(cosl_ba_solver* s) {
-  static const bool syncReadback = std::getenv("COSL_BA_SYNC_READBACK") != nullptr;
-  // multi-GPU on a crowded host (fewer than 3 usable cores per rank, e.g. 8 ranks in a 16-thread cgroup): the
-  // copy-engine read-back + stream synchronise of round 1 is kept there (N ranks polling mapped memory
-  // compete with NCCL's proxy threads for the cores; with enough cores per rank the polling read-back wins).  COSL_BA_BLOCKING_READBACK=1: core-yielding wait.
-  static const bool forceBlock = std::getenv("COSL_BA_BLOCKING_READBACK") != nullptr;
+  // multi-GPU on a crowded host (fewer than 3 usable cores per rank, e.g. 8 ranks in a 16-thread cgroup): a
+  // copy-engine read-back + stream synchronise (N ranks polling mapped memory compete with NCCL's proxy
+  // threads for the cores; with enough cores per rank the polling read-back wins)
   const bool crowded = multi(s) && host_threads_all() < 3 * s->comm->nranks;
-  if (syncReadback || crowded || (forceBlock && multi(s))) {
+  if (crowded) {
     COSL_CUDA(cudaMemcpyAsync(s->h_sc, s->d_sc, sizeof(double) * SC_NTOT, cudaMemcpyDeviceToHost,
                               s->stream));
-    if (forceBlock) {
-      if (!s->evBlock) COSL_CUDA(cudaEventCreateWithFlags(&s->evBlock, cudaEventBlockingSync | cudaEventDisableTiming));
-      COSL_CUDA(cudaEventRecord(s->evBlock, s->stream));
-      COSL_CUDA(cudaEventSynchronize(s->evBlock));
-    } else {
-      COSL_CUDA(cudaStreamSynchronize(s->stream));
-    }
+    COSL_CUDA(cudaStreamSynchronize(s->stream));
     return COSL_OK;
   }
   const unsigned long long seq = ++s->scSeq;
@@ -1032,9 +800,6 @@ int dense_solve(cosl_ba_solver* s) {
   s->timer.begin(s->secSolve, s->stream);
   if (s->twoSolve) {
     COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s->stream, s->td, s->two00, s->two10, s->two11);
-  } else if (s->smallSolve) {
-    COSL_LAUNCH(ba_tile_small, 1, 256, sizeof(double) * (size_t)ns * ns, s->stream, s->td,
-                s->d_tileIdx, s->d_blkRow0, ns);
   } else {
     COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, s->stream, s->td);
   }
@@ -1065,37 +830,17 @@ int solve_trial(cosl_ba_solver* s, double mu, bool* solved) {
     const bool doStats = s->statsPending;
     s->statsPending = false;
     COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->stream, s->d,
-                mu, r0 ? 1 : 0, s->d_diagBlk, s->d_blkCam0, s->d_order, s->smallSolve ? (int*)nullptr : s->d_cnt,
-                s->smallSolve ? 0 : s->td.nCounters + 2 + s->td.nTasks, nTilesInit, s->d_Vinv, doStats ? 1 : 0,
+                mu, r0 ? 1 : 0, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt,
+                s->td.nCounters + 2 + s->td.nTasks, nTilesInit, s->d_Vinv, doStats ? 1 : 0,
                 s->d_dpb, 3LL * s->n);
     if (doStats) COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
     if (fineSchur) {
       s->timer.end(s->stream);
       s->timer.begin(s->secSchur, s->stream);
     }
-    if (s->useRows) {
-      if (s->Nc)
-        COSL_LAUNCH(ba_schur_rows, s->mf * s->rowSplits, 32 * BA_ROWS_WARPS, s->rowsSmem, s->stream, s->d,
-                    s->d_cptrFree, s->d_visit, s->d_rowDst, s->nSlots, s->d_Vinv, s->d_solIdx, s->rowSplits);
-    } else if (s->useBlk) {
-      if (s->nBItems)
-        COSL_LAUNCH(ba_schur_blk, div_up(s->nBItems, BA_BLK_WARPS), 32 * BA_BLK_WARPS, BA_BLK_SMEM, s->stream, s->d,
-                    s->d_bitems, s->nBItems, s->d_bvis, s->d_btabs, s->d_Vinv);
-    } else if (s->nItems) {
-      // fp64 tensor-core variant (ba_schur_mma, DMMA m8n8k4 over smem-staged entry rows): correct and
-      // parity-tested, but 1.49 ms vs 0.50 ms per LM trial at c4 (H100 80GB HBM3, 700 W) -- its staging
-      // spends ~100 instructions per entry on index arithmetic.
-      // COSL_BA_SCHUR_MMA=1 selects it; the SIMT kernel is the default.
-      if (std::getenv("COSL_BA_SCHUR_MMA") != nullptr)
-        COSL_LAUNCH(ba_schur_mma, div_up(s->nItems, 4), 128, 0, s->stream, s->d, s->d_items, s->nItems,
-                    s->d_entries, s->d_Vinv);
-      else if (s->schurSimt)
-        COSL_LAUNCH(ba_schur_pairs_t<4>, div_up(s->nItems, 4), 128, 0, s->stream, s->d, s->d_items,
-                    s->nItems, s->d_entries, s->d_Vinv);
-      else
-        COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, s->stream,
-                    s->d, s->d_items, s->nItems, s->d_entries, s->d_Vinv);
-    }
+    if (s->nItems)
+      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, s->stream,
+                  s->d, s->d_items, s->nItems, s->d_entries, s->d_Vinv);
   }
   s->timer.end(s->stream);
   // the one exchange of an LM trial: [rhs | Schur-structure tiles] is contiguous, no packing
@@ -1471,7 +1216,7 @@ int cosl_ba_solver_stats(cosl_ba_solver* s, double out[8]) {
   for (int k = 0; k < 8; ++k) out[k] = 0.0;
   out[0] = (double)s->ns;
   out[1] = (double)s->reduceCount;
-  out[2] = s->smallSolve ? (double)s->ns * s->ns * s->ns / 3.0 : 0.5 * s->factorFlops;
+  out[2] = 0.5 * s->factorFlops;
   out[5] = (double)s->plan.nb;
   out[6] = (double)s->plan.nTiles;
   out[7] = (double)s->plan.tasks.size();
@@ -1489,7 +1234,7 @@ int cosl_ba_solver_plan_info(cosl_ba_solver* s, int out[8]) {
   out[4] = s->plan.ndDepth;
   out[5] = s->plan.criticalPathTasks;
   out[6] = s->solveGrid;
-  out[7] = s->smallSolve ? 1 : 0;
+  out[7] = s->twoSolve ? 1 : 0;
   return COSL_OK;
 }
 

@@ -392,8 +392,8 @@ __device__ __forceinline__ void ba_tile_init_body(const BaDev& d, double mu, int
 // ------------------------------------------------------------------------------------------
 // Schur contraction over camera pairs.  Work item = a run of (obsA, obsB) entries that belong to
 // one camera pair (j <= k): block(j,k) -= sum_i W_ij V*_i^-1 W_ik^T (and, for j == k,
-// rhs_j -= sum_i W_ij V*_i^-1 eb_i).  One warp per item; two lanes share an entry (3 block columns
-// each), 18 accumulators per lane, butterfly reduction, 18 atomics per lane-parity per item.
+// rhs_j -= sum_i W_ij V*_i^-1 eb_i).  One warp per item (ba_schur_pairs_st below); the items of a
+// pair add into its block with atomics.
 // ------------------------------------------------------------------------------------------
 struct BaPairItem {
   int rowCam, colCam;  // free-camera indices (0-based in the reduced system)
@@ -476,95 +476,12 @@ ba_prep_kernel(BaDev d, double mu, int addU, const int* __restrict__ diagBlk, co
   }
 }
 
-// Entries carry the point index ({obsA, obsB, point, -}) and the damped inverses V*^-1 are computed
-// once per trial (ba_vinv_kernel), so the loads of an entry are ONE dependent level below the entry
-// itself; the next entry is fetched while the current one is processed.
-template <int MINB>
-__global__ void __launch_bounds__(128, MINB)
-ba_schur_pairs_t(BaDev d, const BaPairItem* __restrict__ items, int nItems,
-                 const int4* __restrict__ entries, const double* __restrict__ Vinv) {
-  const int item = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (item >= nItems) return;
-  const int lane = threadIdx.x & 31;
-  const int half = lane & 1;  // which 3 columns of the 6x6 block
-  const BaPairItem it = items[item];
-  double acc[18];
-#pragma unroll
-  for (int k = 0; k < 18; ++k) acc[k] = 0;
-  double racc[3] = {0, 0, 0};
-  const bool diag = (it.rowCam == it.colCam);
-  int e = it.begin + (lane >> 1);
-  int4 nxt = (e < it.end) ? __ldg(&entries[e]) : make_int4(0, 0, 0, 0);
-  for (; e < it.end; e += 16) {
-    const int4 ob = nxt;
-    if (e + 16 < it.end) nxt = __ldg(&entries[e + 16]);
-    const double* Wa = d.W + 18 * (size_t)ob.x;
-    const double* Wb = d.W + 18 * (size_t)ob.y;
-    const int i = ob.z;
-    const double* Vi = Vinv + 6 * (size_t)i;
-    double Iv[6];
-#pragma unroll
-    for (int k = 0; k < 6; ++k) Iv[k] = Vi[k];
-    double wa[18];
-#pragma unroll
-    for (int k = 0; k < 18; ++k) wa[k] = Wa[k];
-#pragma unroll
-    for (int cc = 0; cc < 3; ++cc) {
-      const int c = 3 * half + cc;
-      const double b0 = Wb[3 * c], b1 = Wb[3 * c + 1], b2 = Wb[3 * c + 2];
-      const double t0 = Iv[0] * b0 + Iv[1] * b1 + Iv[2] * b2;
-      const double t1 = Iv[1] * b0 + Iv[3] * b1 + Iv[4] * b2;
-      const double t2 = Iv[2] * b0 + Iv[4] * b1 + Iv[5] * b2;
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
-        acc[3 * r + cc] += wa[3 * r] * t0 + wa[3 * r + 1] * t1 + wa[3 * r + 2] * t2;
-    }
-    if (diag) {
-      const double* eb = d.eb + 3 * (size_t)i;
-      const double t0 = Iv[0] * eb[0] + Iv[1] * eb[1] + Iv[2] * eb[2];
-      const double t1 = Iv[1] * eb[0] + Iv[3] * eb[1] + Iv[4] * eb[2];
-      const double t2 = Iv[2] * eb[0] + Iv[4] * eb[1] + Iv[5] * eb[2];
-#pragma unroll
-      for (int rr = 0; rr < 3; ++rr) {
-        const double* wr = Wa + 3 * (3 * half + rr);  // row (3*half + rr) of W_a
-        racc[rr] += wr[0] * t0 + wr[1] * t1 + wr[2] * t2;
-      }
-    }
-  }
-  // butterfly over lanes of equal parity
-#pragma unroll
-  for (int o = 2; o < 32; o <<= 1) {
-#pragma unroll
-    for (int k = 0; k < 18; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) racc[k] += __shfl_xor_sync(0xffffffffu, racc[k], o);
-  }
-  if (lane < 2) {
-    double* T = d.tiles + it.dst;
-#pragma unroll
-    for (int r = 0; r < 6; ++r)
-#pragma unroll
-      for (int cc = 0; cc < 3; ++cc) {
-        const int c = 3 * half + cc;
-        // only the lower part (row >= col of the tile, i.e. c >= r) of diagonal blocks is kept
-        if (!diag || c >= r) {
-          const int col = it.cOff + (it.trans ? c : r), row = it.rOff + (it.trans ? r : c);
-          atomicAdd(&T[col * 64 + row], -acc[3 * r + cc]);
-        }
-      }
-    if (diag) {
-#pragma unroll
-      for (int rr = 0; rr < 3; ++rr) atomicAdd(&d.rhs[it.rhsIdx + 3 * half + rr], -racc[rr]);
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------
-// Staged variant of the pair-list contraction (default).  ba_schur_pairs_t gathers the rows of an entry
-// with scalar 8-byte loads issued by the lanes that consume them: 33 load instructions per 16 entries,
-// each touching ~16 different 128-byte lines -> ~33 L1TEX wavefronts per entry, which is what bounds it
-// (0.52 ms per LM trial at c4 for 1.7 GFLOP against 0.50 for this kernel, H100 80GB HBM3, 700 W;
-// COSL_BA_SCHUR_SIMT=1 selects it).  Here a warp works on 32 entries at a time:
+// Pair-list contraction.  The damped inverses V*^-1 are computed once per trial (ba_prep_kernel) and an
+// entry carries its point index ({obsA, obsB, point, -}), so the rows of an entry are one dependent load
+// below its descriptor.  Gathering those rows with scalar 8-byte loads by the lanes that consume them
+// touches ~16 different 128-byte lines per load instruction, and L1TEX wavefronts bound such a kernel;
+// the rows are therefore staged.  A warp works on 32 entries at a time:
 //   1. STAGE: the 21 16-byte segments of every entry -- W_a (9), W_b (9), V*^-1 (3) -- are copied with
 //      cp.async in SEGMENT-major order (consecutive lanes copy consecutive segments of the same row, so
 //      one instruction touches ~8 lines instead of 32: ~5 wavefronts per entry), into a row of 42
@@ -760,228 +677,6 @@ __global__ void __launch_bounds__(1024) ba_scan_u32(const unsigned* __restrict__
     run += cnt[k];
   }
   if (tid == 1023) off[n] = s_sum[1023];
-}
-
-// ------------------------------------------------------------------------------------------
-// Schur contraction on the fp64 tensor cores (DMMA m8n8k4).  Same work items as ba_schur_pairs_t
-// (one warp per run of <= 512 entries of one camera pair); the 6x6 block
-//     sum_i W_ia V*_i^-1 W_ib^T  =  [W_ia]_(6 x 3n) . [V*_i^-1 W_ib^T]_(3n x 6)
-// is ONE dense contraction with the entries stacked along k.  Per chunk of 16 entries:
-//   1. the rows W_a, W_b (144 B each), V*^-1 (48 B) and e_b of the entries are staged in shared
-//      memory with 16-byte loads of contiguous segments (the scalar gathers of the SIMT kernel are
-//      what bound it: L1TEX wavefronts, see profiles/);
-//   2. T_i = V*_i^-1 W_ib^T (3 x 6) and the right-hand-side column V*_i^-1 e_b,i are formed in place;
-//   3. 12 DMMAs accumulate C(8x8) += A(8x4) B(4x8): A(r, k) = W_ia(r, c) with k = 3 i + c (rows 6, 7
-//      are zero), B(k, n) = T_i(c, n) for n < 6 and B(k, 6) = (V*^-1 e_b)(c): column 6 of the
-//      accumulator is the right-hand side of diagonal items for free.
-// ------------------------------------------------------------------------------------------
-constexpr int BA_MMA_CHUNK = 16;                      // entries per chunk
-constexpr int BA_MMA_ESTRIDE = 18 + 24 + 2;           // doubles per entry: W_a | T (3 x 8) | pad
-
-__device__ __forceinline__ void ba_dmma884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
-
-__global__ void __launch_bounds__(128, 6)
-ba_schur_mma(BaDev d, const BaPairItem* __restrict__ items, int nItems, const int4* __restrict__ entries,
-             const double* __restrict__ Vinv) {
-  __shared__ __align__(16) double s_e[4][BA_MMA_CHUNK * BA_MMA_ESTRIDE];  // per warp
-  __shared__ __align__(16) double s_wb[4][BA_MMA_CHUNK * 28];             // W_b (18) | Vinv (6) | e_b (3) | pad
-  __shared__ int4 s_ob[4][BA_MMA_CHUNK];
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int item = blockIdx.x * 4 + w;
-  if (item >= nItems) return;
-  const BaPairItem it = items[item];
-  const bool diag = (it.rowCam == it.colCam);
-  double* se = s_e[w];
-  double* sb = s_wb[w];
-  double c0 = 0.0, c1 = 0.0;
-  const int lr = lane >> 2, lk = lane & 3;
-  for (int e0 = it.begin; e0 < it.end; e0 += BA_MMA_CHUNK) {
-    const int ne = min(BA_MMA_CHUNK, it.end - e0);
-    // ---- 1. stage: 21 (+2) 16-byte segments per entry: W_a (9), W_b (9), Vinv (3), e_b (1.5)
-    if (lane < BA_MMA_CHUNK) s_ob[w][lane] = (lane < ne) ? __ldg(&entries[e0 + lane]) : make_int4(0, 0, 0, 0);
-    __syncwarp();
-#pragma unroll 4
-    for (int t = lane; t < BA_MMA_CHUNK * 23; t += 32) {
-      const int j = t / 23, part = t - 23 * j;
-      double2 v = make_double2(0.0, 0.0);
-      if (j < ne) {
-        const int4 ob = s_ob[w][j];
-        if (part < 9) v = *reinterpret_cast<const double2*>(d.W + 18 * (size_t)ob.x + 2 * part);
-        else if (part < 18) v = *reinterpret_cast<const double2*>(d.W + 18 * (size_t)ob.y + 2 * (part - 9));
-        else if (part < 21) v = *reinterpret_cast<const double2*>(Vinv + 6 * (size_t)ob.z + 2 * (part - 18));
-        else if (diag) {
-          const double* eb = d.eb + 3 * (size_t)ob.z;
-          v = (part == 21) ? make_double2(eb[0], eb[1]) : make_double2(eb[2], 0.0);
-        }
-      }
-      if (part < 9) *reinterpret_cast<double2*>(se + j * BA_MMA_ESTRIDE + 2 * part) = v;
-      else *reinterpret_cast<double2*>(sb + j * 28 + 2 * (part - 9)) = v;
-    }
-    __syncwarp();
-    // ---- 2. T_i(c, n) = sum_c' Vinv(c, c') W_b(n, c')  (n < 6),  T_i(c, 6) = (Vinv e_b)(c), T_i(c, 7) = 0
-    for (int t = lane; t < BA_MMA_CHUNK * 24; t += 32) {
-      const int j = t / 24, cn = t - 24 * j, c = cn >> 3, n = cn & 7;
-      const double* q = sb + j * 28;
-      const double* Vi = q + 18;
-      const double v0 = (c == 0) ? Vi[0] : (c == 1) ? Vi[1] : Vi[2];
-      const double v1 = (c == 0) ? Vi[1] : (c == 1) ? Vi[3] : Vi[4];
-      const double v2 = (c == 0) ? Vi[2] : (c == 1) ? Vi[4] : Vi[5];
-      double r = 0.0;
-      if (n < 6) r = v0 * q[3 * n] + v1 * q[3 * n + 1] + v2 * q[3 * n + 2];
-      else if (n == 6) r = v0 * q[24] + v1 * q[25] + v2 * q[26];
-      se[j * BA_MMA_ESTRIDE + 18 + cn] = r;
-    }
-    __syncwarp();
-    // ---- 3. 12 k-steps of 4: k = 3 j + c
-#pragma unroll
-    for (int ks = 0; ks < 3 * BA_MMA_CHUNK / 4; ++ks) {
-      const int k = 4 * ks + lk, j = k / 3, c = k - 3 * j;
-      const double a = (lr < 6) ? se[j * BA_MMA_ESTRIDE + 3 * lr + c] : 0.0;  // W_a(r = lr, c)
-      const double b = se[j * BA_MMA_ESTRIDE + 18 + 8 * c + lr];             // T(c, n = lr)
-      ba_dmma884(c0, c1, a, b);
-    }
-    __syncwarp();
-  }
-  // C(r = lr, n = 2 lk, 2 lk + 1): block element (r, n) for n < 6; column 6 = rhs
-  if (lr < 6) {
-    double* T = d.tiles + it.dst;
-    const double cv[2] = {c0, c1};
-#pragma unroll
-    for (int h2 = 0; h2 < 2; ++h2) {
-      const int n = 2 * lk + h2, r = lr;
-      if (n < 6) {
-        if (!diag || n >= r) {
-          const int col = it.cOff + (it.trans ? n : r), row = it.rOff + (it.trans ? r : n);
-          atomicAdd(&T[col * 64 + row], -cv[h2]);
-        }
-      } else if (n == 6 && diag) {
-        atomicAdd(&d.rhs[it.rhsIdx + r], -cv[h2]);
-      }
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// Schur contraction, camera-row form (the default): CTA = one free camera a.  It walks a's
-// observations (camera-major list); for each point i it reads the point's W rows -- ONE contiguous
-// segment of the point-major W array -- and accumulates Y_a(i) W_b(i)^T for every free camera
-// b >= a that sees i into warp-private shared-memory accumulators indexed by b - a (the band of
-// the reduced camera system), plus Y_a(i) eb_i for the right-hand side.  At the end the four warp
-// copies are summed in a fixed order and subtracted from the tiles: every 6x6 block (a, b) has
-// exactly one owner, so there are no atomics and the result is deterministic.  Traffic: W is read
-// ~(k_i + 1)/2 times per row from L2 in contiguous 144-byte rows (the pair-list kernel gathered
-// 288 B per pair entry through index lists).  Used when the band (nSlots = max(b - a) + 1) fits
-// shared memory; ba_schur_pairs remains for arbitrary co-visibility.
-// ------------------------------------------------------------------------------------------
-struct BaRowDst {
-  int dst, rOff, cOff, trans;  // as in BaPairItem; dst < 0: cameras (a, a + slot) share no point
-};
-
-
-constexpr int BA_ROWS_WARPS = 4;
-
-// visit = one (camera a, point i) pair of the camera-major list: {observation o, point i, first
-// observation of i, number of observations of i}.  The records and the camera lists of the NEXT
-// visits are prefetched while the current one is processed, so the dependent chain per visit is
-// one level of loads (W rows) instead of four (cobs -> pt -> ptr -> cam -> W).
-__global__ void __launch_bounds__(32 * BA_ROWS_WARPS)
-ba_schur_rows(BaDev d, const int* __restrict__ cptr, const int4* __restrict__ visit,
-              const BaRowDst* __restrict__ rowDst, int nSlots, const double* __restrict__ Vinv,
-              const int* __restrict__ rhsIdx, int splits) {
-  extern __shared__ double sacc[];  // [BA_ROWS_WARPS][stride]
-  __shared__ int s_list[BA_ROWS_WARPS][32], s_slot[BA_ROWS_WARPS][32];
-  __shared__ double s_Y[BA_ROWS_WARPS][18];
-  // splits > 1 (few cameras, many observations: local BA): several CTAs share a camera's
-  // observation list and add their partial blocks with atomics
-  const int af = blockIdx.x / splits, part = blockIdx.x - af * splits;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int stride = nSlots * 36 + 8;
-  double* acc = sacc + (size_t)w * stride;
-  for (int e = lane; e < stride; e += 32) acc[e] = 0.0;
-  __syncwarp();
-  const int qend = cptr[af + 1], step = BA_ROWS_WARPS * splits;
-  int q = cptr[af] + part * BA_ROWS_WARPS + w;
-  const int4 none = make_int4(0, -1, 0, 0);
-  int4 r0 = (q < qend) ? visit[q] : none;
-  int4 r1 = (q + step < qend) ? visit[q + step] : none;
-  int camCur = (r0.y >= 0 && lane < r0.w) ? d.cam[r0.z + lane] : -1;
-  for (; q < qend; q += step) {
-    const int4 r2 = (q + 2 * step < qend) ? visit[q + 2 * step] : none;
-    const int camNext = (r1.y >= 0 && lane < r1.w) ? d.cam[r1.z + lane] : -1;
-    const int o = r0.x, i = r0.y;
-    if (i >= d.ncon) {  // fixed points do not enter the reduced system (warp-uniform)
-      const double* Vi = Vinv + 6 * (size_t)i;
-      const double i0 = Vi[0], i1 = Vi[1], i2 = Vi[2], i3 = Vi[3], i4 = Vi[4], i5 = Vi[5];
-      if (lane < 18) {  // Y = W_o Vinv_i, entry (r, c) = lane
-        const int r = lane / 3, c = lane - 3 * r;
-        const double* wr = d.W + 18 * (size_t)o + 3 * r;
-        const double v0 = (c == 0) ? i0 : (c == 1) ? i1 : i2;
-        const double v1 = (c == 0) ? i1 : (c == 1) ? i3 : i4;
-        const double v2 = (c == 0) ? i2 : (c == 1) ? i4 : i5;
-        s_Y[w][lane] = wr[0] * v0 + wr[1] * v1 + wr[2] * v2;
-      }
-      __syncwarp();
-      double Y[18];
-#pragma unroll
-      for (int k = 0; k < 18; ++k) Y[k] = s_Y[w][k];
-      if (lane < 6) {  // rhs_a -= Y eb_i
-        const double* eb = d.eb + 3 * (size_t)i;
-        const double* yr = &s_Y[w][3 * lane];
-        acc[nSlots * 36 + lane] += yr[0] * eb[0] + yr[1] * eb[1] + yr[2] * eb[2];
-      }
-      const int p0 = r0.z, p1 = r0.z + r0.w;
-      for (int base = p0; base < p1; base += 32) {
-        const int ob = base + lane;
-        const int cm = (base == p0) ? camCur : ((ob < p1) ? d.cam[ob] : -1);
-        const int bf = (ob < p1) ? cm - d.mcon : -1;
-        const bool ok = bf >= af;
-        const unsigned mask = __ballot_sync(0xffffffffu, ok);
-        const int nq = __popc(mask);
-        if (ok) {
-          const int pos = __popc(mask & ((1u << lane) - 1u));
-          s_list[w][pos] = ob;
-          s_slot[w][pos] = bf - af;
-        }
-        __syncwarp();
-        for (int t = lane; t < 6 * nq; t += 32) {
-          const int j = t / 6, sc = t - 6 * j;
-          const double* wb = d.W + 18 * (size_t)s_list[w][j] + 3 * sc;
-          const double w0 = wb[0], w1 = wb[1], w2 = wb[2];
-          double* ap = acc + s_slot[w][j] * 36 + sc;
-#pragma unroll
-          for (int r = 0; r < 6; ++r) ap[6 * r] += Y[3 * r] * w0 + Y[3 * r + 1] * w1 + Y[3 * r + 2] * w2;
-        }
-        __syncwarp();
-      }
-    }
-    r0 = r1;
-    r1 = r2;
-    camCur = camNext;
-  }
-  __syncthreads();
-  for (int e = threadIdx.x; e < nSlots * 36; e += 32 * BA_ROWS_WARPS) {
-    const int slot = e / 36, rs = e - 36 * slot, r = rs / 6, sc = rs - 6 * r;
-    const BaRowDst rd = rowDst[(size_t)af * nSlots + slot];
-    if (rd.dst < 0) continue;
-    if (slot == 0 && sc < r) continue;  // diagonal block: lower part of the tile only
-    double v = 0;
-#pragma unroll
-    for (int ww = 0; ww < BA_ROWS_WARPS; ++ww) v += sacc[(size_t)ww * stride + e];
-    const int col = rd.cOff + (rd.trans ? sc : r), row = rd.rOff + (rd.trans ? r : sc);
-    if (splits > 1) atomicAdd(&d.tiles[rd.dst + col * 64 + row], -v);
-    else d.tiles[rd.dst + col * 64 + row] -= v;
-  }
-  if (threadIdx.x < 6) {
-    double v = 0;
-#pragma unroll
-    for (int ww = 0; ww < BA_ROWS_WARPS; ++ww) v += sacc[(size_t)ww * stride + nSlots * 36 + threadIdx.x];
-    if (splits > 1) atomicAdd(&d.rhs[rhsIdx[af] + threadIdx.x], -v);
-    else d.rhs[rhsIdx[af] + threadIdx.x] -= v;
-  }
 }
 
 // ------------------------------------------------------------------------------------------

@@ -31,7 +31,6 @@
 #pragma once
 #include <algorithm>
 #include <cstdint>
-#include <cstdlib>
 #include <vector>
 
 namespace coslam {
@@ -255,7 +254,7 @@ inline BaPlan ba_make_plan(int mf, const std::vector<uint8_t>& adj, int ndDepthO
   // order would serialise a separator tile behind the slowest interior; instead the order follows
   // the estimated time at which each update's operands become available (pass 1 below).
   auto T = [&](int i, int j) { return P.tileIdx[(size_t)i * nb + j]; };
-  const bool useScratch = (regions.size() > 1) && (std::getenv("COSL_BA_NO_SCRATCH") == nullptr);
+  const bool useScratch = regions.size() > 1;
   // scratch slot per (target tile, pivot region): created on first use
   std::vector<std::vector<std::pair<int, int>>> scratchOf(nt);  // target tile -> (region, scratch tile)
   int nScratch = 0;

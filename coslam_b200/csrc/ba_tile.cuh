@@ -843,75 +843,4 @@ __global__ void __launch_bounds__(BA_NTHREADS, 1) ba_tile_two(BaTileDev d, int t
   if (tid == 0 && s_fail) d.sc[d.scFail] = 1.0;
 }
 
-// ---------------------------------------------------------------------------------------------
-// Small systems (local BA: a handful of blocks): everything inside ONE CTA's shared memory,
-// dense column-major lower with leading dimension ns (rows of block k start at 60*k: every block
-// but the last is full when the plan has a single region).
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-ba_tile_small(BaTileDev d, const int* __restrict__ tileIdx, const int* __restrict__ blkRow0, int ns) {
-  extern __shared__ double sL[];
-  __shared__ int s_fail;
-  __shared__ double sx[1024];
-  const int tid = threadIdx.x, nt = blockDim.x;
-  for (int bj = 0; bj < d.nb; ++bj)
-    for (int bi = bj; bi < d.nb; ++bi) {
-      const int t = tileIdx[bi * d.nb + bj];
-      const int ri = d.blkRows[bi], rj = d.blkRows[bj], r0 = blkRow0[bi], c0 = blkRow0[bj];
-      for (int e = tid; e < ri * rj; e += nt) {
-        const int c = e / ri, r = e - c * ri;
-        const double v = (t >= 0) ? d.tiles[(size_t)t * BA_TILE + c * BA_TB + r] : 0.0;
-        sL[(c0 + c) * ns + r0 + r] = (r0 + r >= c0 + c) ? v : 0.0;
-      }
-    }
-  for (int bi = 0; bi < d.nb; ++bi)
-    for (int r = tid; r < d.blkRows[bi]; r += nt) sx[blkRow0[bi] + r] = d.rhs[(size_t)bi * BA_TB + r];
-  if (tid == 0) s_fail = 0;
-  __syncthreads();
-  for (int k = 0; k < ns; ++k) {
-    const double dkk = sL[k * ns + k];
-    if (!(dkk > 0) || !isfinite(dkk)) {
-      if (tid == 0) s_fail = 1;
-      break;  // uniform: every thread reads the same dkk
-    }
-    const double rs = 1.0 / sqrt(dkk);
-    __syncthreads();
-    for (int i = k + tid; i < ns; i += nt) sL[k * ns + i] = (i == k) ? sqrt(dkk) : sL[k * ns + i] * rs;
-    __syncthreads();
-    const int tj = tid >> 4, ti = tid & 15;
-    for (int j = k + 1 + tj; j < ns; j += 16) {
-      const double ljk = sL[k * ns + j];
-      for (int i = j + ti; i < ns; i += 16) sL[j * ns + i] -= sL[k * ns + i] * ljk;
-    }
-    __syncthreads();
-  }
-  __syncthreads();
-  if (s_fail) {
-    if (tid == 0) d.sc[d.scFail] = 1.0;
-    return;
-  }
-  if (tid < 32) {
-    for (int k = 0; k < ns; ++k) {
-      const double xk = sx[k] / sL[k * ns + k];
-      __syncwarp();
-      if (tid == 0) sx[k] = xk;
-      for (int i = k + 1 + tid; i < ns; i += 32) sx[i] -= sL[k * ns + i] * xk;
-      __syncwarp();
-    }
-    for (int k = ns - 1; k >= 0; --k) {
-      double part = 0;
-      for (int i = k + 1 + tid; i < ns; i += 32) part += sL[k * ns + i] * sx[i];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-      __syncwarp();
-      if (tid == 0) sx[k] = (sx[k] - part) / sL[k * ns + k];
-      __syncwarp();
-    }
-  }
-  __syncthreads();
-  for (int bi = 0; bi < d.nb; ++bi)
-    for (int r = tid; r < BA_TB; r += nt)
-      d.x[(size_t)bi * BA_TB + r] = (r < d.blkRows[bi]) ? sx[blkRow0[bi] + r] : 0.0;
-}
-
 }  // namespace coslam

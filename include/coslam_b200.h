@@ -308,12 +308,13 @@ const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* ca
 int cosl_ba_solver_profile_enable(cosl_ba_solver* s, int on);
 /* Structure of the reduced camera system, for the roofline arithmetic of bench.py:
  * out[0] = order ns, out[1] = doubles in the all-reduce payload [rhs | Schur-structure tiles],
- * out[2] = multiply-adds of the tile Cholesky + substitutions on the used rows (ns^3/3 for the
- * single-CTA small solve), out[3] = Schur pair entries, out[4] = pair work items, out[5] = blocks,
+ * out[2] = multiply-adds of the tile Cholesky + substitutions on the used rows,
+ * out[3] = Schur pair entries, out[4] = pair work items, out[5] = blocks,
  * out[6] = tiles incl. fill, out[7] = tasks of the solve DAG. */
 int cosl_ba_solver_stats(cosl_ba_solver* s, double out[8]);
 /* Plan of the reduced-system solve: out = {blocks, Schur-structure tiles, tiles incl. fill, tasks,
- * nested-dissection depth, longest dependency chain (tasks), persistent grid size, small-solve}. */
+ * nested-dissection depth, longest dependency chain (tasks), persistent grid size, small-solve}.
+ * small-solve = 1: the system has at most two blocks and one CTA solves it (ba_tile_two). */
 int cosl_ba_solver_plan_info(cosl_ba_solver* s, int out[8]);
 /* Diagnostic timeline of the persistent solve kernel.  enable != 0: arm tracing for the following
  * solves (returns the task count).  enable == 0: copy the timeline of the LAST solve into
