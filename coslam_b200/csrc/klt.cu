@@ -44,6 +44,7 @@ struct cosl_klt {
   // device memory
   uint8_t* d_img = nullptr;
   float4* d_pyr[2] = {nullptr, nullptr};
+  bool lv0Stored[2] = {true, true};  // level 0 of d_pyr[b] holds its frame (see build_pyramid)
   int cur = 1;  // pyr1 == d_pyr[cur]
   float* d_corn = nullptr;
   float4 *d_src = nullptr, *d_dst = nullptr, *d_ping = nullptr, *d_pong = nullptr, *d_res = nullptr;
@@ -111,6 +112,19 @@ static void update_detect_window(cosl_klt* g) {
   const float Wf = (float)g->W, Hf = (float)g->H;
   bounds(g->W, mg / Wf, 1.0f - mg / Wf, g->detXlo, g->detXhi);
   bounds(g->H, mg / Hf, 1.0f - mg / Hf, g->detYlo, g->detYhi);
+}
+
+// the gain tracker's instantiation for this group's window (compile-time width when it is the live one)
+using FusedFn = void (*)(const float4*, const float4*, long long, KltLevels, int, const float4*, float4*,
+                         unsigned long long*, const int*, float4*, int, KltTrackParams, KltTrackParams, int,
+                         KltTail);
+using PassFn = void (*)(const float4*, const float4*, long long, long long, int, int, const float4*,
+                        const float4*, float4*, const int*, float, float, KltTrackParams, int);
+static FusedFn fused_kernel(const cosl_klt* g) {
+  return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE> : klt_gain_fused<0>;
+}
+static PassFn pass_kernel(const cosl_klt* g) {
+  return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE> : klt_gain_pass<0>;
 }
 
 int alloc_group(cosl_klt* g) {
@@ -200,7 +214,7 @@ int alloc_group(cosl_klt* g) {
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
     cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
     g->numSM = std::max(1, nsm);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, klt_gain_fused, KLT_FUSED_THREADS, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fused_kernel(g), KLT_FUSED_THREADS, 0);
     g->fusedOK = ok && coop && perSM > 0 && !(g->cfg.compat & COSL_KLT_PASS_KERNELS);
     const int T = F * C;
     g->fusedBlocks = std::max(1, std::min(div_up(T, KLT_GPB), nsm * perSM));
@@ -335,9 +349,18 @@ static void launch_prefilter(cosl_klt* g, cudaStream_t st) {
                 g->prelimCap, g->d_counters);
 }
 
+// true when the tracker's level list (L-1, L-1-levelSkip, ...) contains level 0
+static bool tracker_reads_level0(const cosl_klt* g) { return (g->L - 1) % g->levelSkip == 0; }
+
 // PyramidWithDerivativesCreator::buildPyramidForGrayscaleImage (v3d_gpupyramid.cpp:366-429)
-int build_pyramid(cosl_klt* g, bool wantCorn) {
+// trackOnly: the frame is built for the tracker.  With the cornerness fused into the front pass as
+// well, nothing but a tracker that visits level 0 reads that level, so it is stored only then: at
+// 16 B/px it is larger than the L2, and writing it would evict the pyramid levels the tracker that
+// follows reads.
+int build_pyramid(cosl_klt* g, bool wantCorn, bool trackOnly = false) {
   float4* P = g->d_pyr[g->cur];
+  const bool storeL0 = !(trackOnly && wantCorn) || tracker_reads_level0(g);
+  g->lv0Stored[g->cur] = storeL0;
   g->timer.begin(g->secPyr, g->stream);
   // level 0 + level 1 + (optionally) the detector's cornerness map in one pass over the image
   FrontParams fp;
@@ -353,6 +376,7 @@ int build_pyramid(cosl_klt* g, bool wantCorn) {
   fp.nStrips = div_up(g->W, FS_SW);
   fp.nChunks = div_up(g->H, FS_R);
   fp.wantL1 = g->L > 1 ? 1 : 0;
+  const auto front = storeL0 ? klt_front<true> : klt_front<false>;
   fp.wantCorn = wantCorn ? 1 : 0;
   fp.minC = g->cfg.minCornerness;
   fp.ixlo = g->detXlo;
@@ -369,12 +393,12 @@ int build_pyramid(cosl_klt* g, bool wantCorn) {
       COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evImg[c0 + nc - 1], 0));
       fp.camBase = c0;
       dim3 g1(div_up(fp.nStrips * fp.nChunks, FS_WARPS), nc);
-      COSL_LAUNCH(klt_front, g1, 32 * FS_WARPS, 0, g->stream, fp);
+      COSL_LAUNCH(front, g1, 32 * FS_WARPS, 0, g->stream, fp);
     }
   } else {
     fp.camBase = 0;
     dim3 g0(div_up(fp.nStrips * fp.nChunks, FS_WARPS), g->C);
-    COSL_LAUNCH(klt_front, g0, 32 * FS_WARPS, 0, g->stream, fp);
+    COSL_LAUNCH(front, g0, 32 * FS_WARPS, 0, g->stream, fp);
   }
   if (g->evFront) {
     COSL_CUDA(cudaEventRecord(g->evFront, g->stream));
@@ -473,7 +497,7 @@ int run_tracker(cosl_klt* g) {
                     (void*)&nIter,       (void*)&g->d_src, (void*)&g->d_state, (void*)&g->d_ver,
                     (void*)&g->d_waitset, (void*)&g->d_res, (void*)&C,        (void*)&Plax,
                     (void*)&Pstrict,     (void*)&verBase, (void*)&tail};
-    COSL_CUDA(cudaLaunchCooperativeKernel((const void*)klt_gain_fused, dim3(g->fusedBlocks),
+    COSL_CUDA(cudaLaunchCooperativeKernel((const void*)fused_kernel(g), dim3(g->fusedBlocks),
                                           dim3(KLT_FUSED_THREADS), args, 0, g->stream));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     g->verBase += nPass;
@@ -510,6 +534,7 @@ int run_tracker(cosl_klt* g) {
   } else if (g->cfg.trackWithGain) {
     const float4* in = g->d_src;
     float4* bufs[2] = {g->d_ping, g->d_pong};
+    const PassFn pass = pass_kernel(g);
     int which = 0, first = 1;
     bool strict = false;
     for (int level = g->L - 1; level >= 0; level -= g->levelSkip) {
@@ -523,7 +548,7 @@ int run_tracker(cosl_klt* g) {
         const bool last =
             (level - g->levelSkip < 0) && (iter == g->cfg.nIterations);
         float4* out = last ? g->d_res : bufs[which];
-        COSL_LAUNCH(klt_gain_pass, gridHalf, 256, 0, g->stream, P0, P1, g->pyrStride,
+        COSL_LAUNCH(pass, gridHalf, 256, 0, g->stream, P0, P1, g->pyrStride,
                     g->lvOff[level], w, h, g->d_src, in, out, g->d_nbr, dsx, dsy,
                     track_params(g, strict), first);
         in = out;
@@ -579,6 +604,9 @@ int run_detector(cosl_klt* g, int mode, int nPresentExt) {
   const float Wf = (float)g->W, Hf = (float)g->H, mg = g->detectMargin;
   g->timer.begin(g->secDetect, g->stream);
   if (!g->cornValid) {
+    // a pyramid without level 0 always comes with its cornerness map (build_pyramid)
+    if (!g->lv0Stored[g->cur])
+      return set_error(COSL_E_STATE, "detector: level 0 of the current pyramid was not stored");
     dim3 gc(div_up(g->W, DC_TW), div_up(g->H, DC_TH), g->C);
     COSL_LAUNCH(klt_cornerness, gc, 256, 0, g->stream, g->d_pyr[g->cur], g->pyrStride, g->d_corn,
                 g->W, g->H, g->cfg.minCornerness, mg / Wf, mg / Hf, 1.0f - mg / Wf, 1.0f - mg / Hf);
@@ -640,7 +668,7 @@ int advance(cosl_klt* g) {
 
 int do_track(cosl_klt* g, bool wantCorn = false) {
   COSL_TRY(zero_counters(g));  // before the front pass: the early prefilter counts into them
-  COSL_TRY(build_pyramid(g, wantCorn));
+  COSL_TRY(build_pyramid(g, wantCorn, true));
   g->statusDone = g->suppressDone = false;
   g->wantTail = true;  // the persistent gain tracker writes the feature table itself
   COSL_TRY(run_tracker(g));
@@ -1006,9 +1034,13 @@ int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* ou
   if (w) *w = lw;
   if (ht) *ht = lh;
   if (!out3) return COSL_OK;
+  const int buf = which ? h->cur : 1 - h->cur;
+  if (level == 0 && !h->lv0Stored[buf])
+    return set_error(COSL_E_INVALID,
+                     "debug_pyramid: level 0 of this pyramid was not stored (a tracked frame keeps only "
+                     "the levels its tracker visits; detect() and first() store every level)");
   std::vector<float4> tmp((size_t)lw * lh);
-  const float4* src =
-      h->d_pyr[which ? h->cur : 1 - h->cur] + (size_t)cam * h->pyrStride + h->lvOff[level];
+  const float4* src = h->d_pyr[buf] + (size_t)cam * h->pyrStride + h->lvOff[level];
   COSL_CUDA(cudaStreamSynchronize(h->stream));
   COSL_CUDA(cudaMemcpy(tmp.data(), src, sizeof(float4) * tmp.size(), cudaMemcpyDeviceToHost));
   for (size_t i = 0; i < tmp.size(); ++i) {

@@ -3,8 +3,10 @@
 //   * pyramid level 1 ([1 3 3 1]^2 / 64)   [pyramid_with_derivative_pass2.cg]
 //   * the detector's cornerness map        [klt_detector_pass1.cg + klt_detector_pass2.cg]
 // so the 16 B/px level-0 texels are written once and never re-read from HBM by the pyramid or the
-// detector.  Every output is computed with the same operations, in the same order, as the
-// stand-alone kernels (klt_pyr_level0, klt_pyr_down, klt_cornerness) and the oracle: bit-exact.
+// detector.  When nothing will read level 0 (STORE_L0 = false: a tracking frame whose cornerness
+// is fused here and whose tracker skips level 0), it is not written at all.  Every output is
+// computed with the same operations, in the same order, as the stand-alone kernels
+// (klt_pyr_level0, klt_pyr_down, klt_cornerness) and the oracle: bit-exact.
 // (The level-0 taps 1/8, 1/4, 1/2 are powers of two, so fma(k, x, acc) rounds exactly like
 // acc + k*x; the [1 3 3 1] taps and the structure-tensor sums keep separate mul / add.)
 //
@@ -50,6 +52,8 @@ struct FrontParams {
   int ixlo, ixhi, iylo, iyhi;  // detector window (pixels whose centre lies inside the margins)
 };
 
+// STORE_L0 = false: level 0 is computed (every other output derives from it) but not written
+template <bool STORE_L0>
 __global__ void __launch_bounds__(32 * FS_WARPS, FS_MINB)
 klt_front(const FrontParams P) {
   const int lane = threadIdx.x & 31;
@@ -148,7 +152,7 @@ klt_front(const FrontParams P) {
         }
       }
       // ---- level 0 out
-      if (yy >= r0 && yy < r1) {
+      if (STORE_L0 && yy >= r0 && yy < r1) {
         float4* o = out0 + (size_t)yy * W + xa;
         if (wa) o[0] = make_float4(A[0], A[1], A[2], 0.0f);
         if (wb) o[1] = make_float4(B[0], B[1], B[2], 0.0f);

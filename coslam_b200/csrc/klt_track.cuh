@@ -49,6 +49,29 @@ constexpr int KLT_TP = 15;
 constexpr int KLT_G = 8;        // lanes per feature slot
 constexpr int KLT_ROUNDS = 7;   // window pixels per lane on the fast path (<= 56 pixels)
 
+// Texel (a, b) = (column, row) of the I1 tile that lane gl of a group loads in load u (0..8) of a
+// tile half (rows 0..5 or 6..11): each load covers two rows x four columns, so the indices are
+// constants plus (gl >> 2, gl & 3) and cost no registers across the passes.
+static_assert(KLT_TW == 12 && KLT_G == 8, "tile load mapping: 3 x 3 loads of 2 rows x 4 columns per half");
+__device__ __forceinline__ int2 klt_tile_texel(int gl, int half, int u) {
+  return make_int2(4 * (u % 3) + (gl & 3), half * (KLT_TW / 2) + 2 * (u / 3) + (gl >> 2));
+}
+
+// L2 prefetch of the texels (x .. x + n - 1, y) of a level, clamped to the level like the loads
+// that will read them (one bulk prefetch: a row segment is contiguous)
+__device__ __forceinline__ void klt_prefetch_row(const float4* lv, int w, int h, int x, int y, int n) {
+  const int xa = clampi(x, 0, w - 1), xb = clampi(x + n - 1, 0, w - 1);
+  const float4* p = lv + (size_t)clampi(y, 0, h - 1) * w + xa;
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"((xb - xa + 1) * 16) : "memory");
+}
+
+// A copy of v the compiler cannot see through: what is derived from it is computed where it is
+// used instead of being hoisted out of a loop and held in registers (or spilled) across it.
+__device__ __forceinline__ int klt_opaque(int v) {
+  asm volatile("" : "+r"(v));
+  return v;
+}
+
 struct KltCentre {
   float ax, ay;  // bilinear weights shared by the whole window
   int xi, yi;    // unclamped integer texel coordinates of the centre's top-left tap
@@ -190,10 +213,17 @@ __device__ __forceinline__ float klt_nbterm(float bn, float beta, int gl, int gr
 }
 
 
+// Both gain-tracker drivers are instantiated for a window half-width known at compile time (HWC,
+// the live CoSLAM setting hw = 3) and for any width (HWC = 0: P.halfWidth at run time).  With the
+// width fixed, the window size, the pixel guards and the fast-path test fold to constants; the
+// arithmetic is the same in both instantiations.
+constexpr int KLT_HW_LIVE = 3;
+
 // ------------------------------------------------------------------------------------------
 // One pass per launch (diagnostic / fallback).  Grid: x = ceil(F / 32) blocks of 256 threads
 // (32 lane groups), y = camera.
 // ------------------------------------------------------------------------------------------
+template <int HWC>
 __global__ void __launch_bounds__(256)
 klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, long long pyrStride,
               long long lvOff, int w, int h, const float4* __restrict__ X0buf,
@@ -216,7 +246,7 @@ klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
   const float bn = firstPass ? 1.0f : in[fb + nbr[slot * 8 + gl]].z;
   const float nbterm = klt_nbterm(bn, beta, gl, grpBase);
   const bool pre_invalid = (cur.x < 0.f) || (x0.x < 0.f);
-  const int hw = P.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
+  const int hw = HWC > 0 ? HWC : P.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
   const float halfW = 0.5f * (float)P.W, halfH = 0.5f * (float)P.H;
   const KltCentre c0 = klt_centre(w, h, x0.x, x0.y);
   const KltCentre c1 = klt_centre(w, h, cur.x, cur.y);
@@ -286,6 +316,7 @@ struct KltTail {
 constexpr int KLT_FUSED_THREADS = KLT_FUSED_THREADS_N;  // 16 lane groups per CTA
 constexpr int KLT_GPB = KLT_FUSED_THREADS / KLT_G;
 
+template <int HWC>
 __global__ void __launch_bounds__(KLT_FUSED_THREADS, KLT_FUSED_MINBLOCKS)
 klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                long long pyrStride, KltLevels LV, int nIter, const float4* __restrict__ X0buf,
@@ -300,7 +331,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   const int Q = gridDim.x * KLT_GPB;
   const int F = Plax.F;
   const int T = C * F;
-  const int hw = Plax.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
+  const int hw = HWC > 0 ? HWC : Plax.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
   const bool fast = (npx <= KLT_G * KLT_ROUNDS) && (2 * hw + 2 + 2 <= KLT_TW) && (2 * hw + 2 <= 8);
   const float halfW = 0.5f * (float)Plax.W, halfH = 0.5f * (float)Plax.H;
   float4* tile = s_tile[grpInBlock];
@@ -313,14 +344,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   const int cam0 = item0 / F, slot0 = item0 - cam0 * F;
   const float4 x00 = X0buf[item0];
   const int wsA0 = waitset[slot0 * 16 + gl], wsB0 = waitset[slot0 * 16 + 8 + gl];
-  // tile offset of this lane's window pixels
-  int toff[KLT_ROUNDS];
-#pragma unroll
-  for (int r = 0; r < KLT_ROUNDS; ++r) {
-    const int p = min(gl + KLT_G * r, npx - 1);
-    const int py = p / fwid, px = p - py * fwid;
-    toff[r] = (py - hw) * KLT_TP + (px - hw);
-  }
   float3 I0r[KLT_ROUNDS];
   float f0 = 0.f;  // group sum of klt_d2_term of the resident item at the current level
   float4 cur0 = make_float4(-1.f, -1.f, -1.f, 0.f);
@@ -332,6 +355,15 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   unsigned long long gt0;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt0));
 #endif
+  // The I0 block of every level depends only on X0: all of them are requested into L2 now, so the
+  // per-level staging below finds them there (lane gl: row gl of each 8x8 block)
+  if (fast && active0 && x00.x >= 0.f) {
+    for (int li = 0; li < LV.n; ++li) {
+      const KltCentre c0 = klt_centre(LV.w[li], LV.h[li], x00.x, x00.y);
+      klt_prefetch_row(pyr0 + (size_t)cam0 * pyrStride + LV.off[li], LV.w[li], LV.h[li], c0.xi - hw,
+                       c0.yi - hw + gl, 8);
+    }
+  }
   int pass = 0;
   for (int li = 0; li < LV.n; ++li) {
     const int w = LV.w[li], h = LV.h[li];
@@ -372,6 +404,15 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         const float beta = cur.z;
         const bool pre_invalid = (cur.x < 0.f) || (x0.x < 0.f);
         const KltCentre c1 = klt_centre(w, h, cur.x, cur.y);
+        // last iteration of a level: request the next level's I1 tile around the current estimate
+        // into L2 (rows gl and gl + 8), so its staging does not wait on HBM
+        if (staged && it == nIter && li + 1 < LV.n && !pre_invalid) {
+          const int wn = LV.w[li + 1], hn = LV.h[li + 1];
+          const KltCentre cn = klt_centre(wn, hn, cur.x, cur.y);
+          const float4* Ln = pyr1 + (size_t)cam * pyrStride + LV.off[li + 1];
+          klt_prefetch_row(Ln, wn, hn, cn.xi - hw - 2, cn.yi - hw - 2 + gl, KLT_TW);
+          if (gl + KLT_G < KLT_TW) klt_prefetch_row(Ln, wn, hn, cn.xi - hw - 2, cn.yi - hw - 2 + gl + KLT_G, KLT_TW);
+        }
         // ---- per-level staging (first iteration of a level): I0 samples + I1 tile.
         // Three memory round trips with all loads of a trip in flight together: (A) the 8x8 texels
         // under the I0 window and the upper half of the I1 tile, (B) the I0 samples interpolated
@@ -395,32 +436,32 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
               t0[u] = __ldg(&L0[(size_t)clampi(c0.yi - hw + u, 0, h - 1) * w + clampi(c0.xi - hw + gl, 0, w - 1)]);
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
-              const int i = gl + KLT_G * u;
-              const int b = i / KLT_TW, a = i - b * KLT_TW;
+              const int2 ba = klt_tile_texel(gl, 0, u);
+              const int b = ba.y, a = ba.x;
               tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
             }
 #pragma unroll
             for (int u = 0; u < 8; ++u) tile[I0B + u * 8 + gl] = t0[u];
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
-              const int i = gl + KLT_G * u;
-              const int b = i / KLT_TW, a = i - b * KLT_TW;
+              const int2 ba = klt_tile_texel(gl, 0, u);
+              const int b = ba.y, a = ba.x;
               tile[b * KLT_TP + a] = tv[u];
             }
           }
           __syncwarp();
-          if (!pre_invalid) {
+          // I0r is written on every path (a dead slot never reads it), so the previous level's
+          // samples are not live across the loads above
 #pragma unroll
-            for (int r = 0; r < KLT_ROUNDS; ++r) {
-              const int p = gl + KLT_G * r;
-              if (p < npx) {
-                const int py = p / fwid, px = p - py * fwid;
-                const float4* t4 = tile + I0B + py * 8 + px;
-                I0r[r] = klt_lerp4(t4[0], t4[1], t4[8], t4[9], c0.ax, c0.ay);
-                d2 = __fadd_rn(d2, klt_d2_term(I0r[r], Plax.lambda, Plax.delta));
-              } else {
-                I0r[r] = make_float3(0.f, 0.f, 0.f);
-              }
+          for (int r = 0; r < KLT_ROUNDS; ++r) {
+            const int p = gl + KLT_G * r;
+            if (!pre_invalid && p < npx) {
+              const int py = p / fwid, px = p - py * fwid;
+              const float4* t4 = tile + I0B + py * 8 + px;
+              I0r[r] = klt_lerp4(t4[0], t4[1], t4[8], t4[9], c0.ax, c0.ay);
+              d2 = __fadd_rn(d2, klt_d2_term(I0r[r], Plax.lambda, Plax.delta));
+            } else {
+              I0r[r] = make_float3(0.f, 0.f, 0.f);
             }
           }
           __syncwarp();
@@ -428,14 +469,14 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
             float4 tw[NLD];
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
-              const int i = gl + KLT_G * (u + NLD);
-              const int b = i / KLT_TW, a = i - b * KLT_TW;
+              const int2 ba = klt_tile_texel(gl, 1, u);
+              const int b = ba.y, a = ba.x;
               tw[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
             }
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
-              const int i = gl + KLT_G * (u + NLD);
-              const int b = i / KLT_TW, a = i - b * KLT_TW;
+              const int2 ba = klt_tile_texel(gl, 1, u);
+              const int b = ba.y, a = ba.x;
               tile[b * KLT_TP + a] = tw[u];
             }
           }
@@ -467,14 +508,14 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                 float4 tv[NLD];
 #pragma unroll
                 for (int u = 0; u < NLD; ++u) {
-                  const int i = gl + KLT_G * (u + half * NLD);
-                  const int b = i / KLT_TW, a = i - b * KLT_TW;
+                  const int2 ba = klt_tile_texel(gl, half, u);
+                  const int b = ba.y, a = ba.x;
                   tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
                 }
 #pragma unroll
                 for (int u = 0; u < NLD; ++u) {
-                  const int i = gl + KLT_G * (u + half * NLD);
-                  const int b = i / KLT_TW, a = i - b * KLT_TW;
+                  const int2 ba = klt_tile_texel(gl, half, u);
+                  const int b = ba.y, a = ba.x;
                   tile[b * KLT_TP + a] = tv[u];
                 }
               }
@@ -488,6 +529,9 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         if (!pre_invalid) {
           if (inTile) {
             const float4* tc = tile + b0 * KLT_TP + a0;
+            // the tap offsets of this lane are recomputed every pass: held across the passes,
+            // they do not fit the register budget of 4 CTAs per SM
+            const int glp = klt_opaque(gl);
 #pragma unroll
             for (int r = 0; r < KLT_ROUNDS; ++r) {
               if (r == KLT_ROUNDS / 2 && pass > 1 && active) {
@@ -497,7 +541,8 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                 vb = ld_hint_u64(rb);
               }
               if (gl + KLT_G * r < npx) {
-                const float4* t4 = tc + toff[r];
+                const int p = glp + KLT_G * r, py = p / fwid, px = p - py * fwid;
+                const float4* t4 = tc + ((py - hw) * KLT_TP + (px - hw));
                 const float3 I1 = klt_lerp4(t4[0], t4[1], t4[KLT_TP], t4[KLT_TP + 1], c1.ax, c1.ay);
                 klt_acc_pixel(A, I0r[r], I1, beta, halfW, halfH, Plax.lambda);
               }

@@ -161,7 +161,9 @@ void* cosl_klt_stream(cosl_klt* h);
 
 /* Test/inspection hooks (not part of the reference surface). */
 /* Copy pyramid level `level` of camera `cam` to host as interleaved (I, Ix, Iy) floats.
- * which: 0 = previous frame (pyr0), 1 = current frame (pyr1). */
+ * which: 0 = previous frame (pyr0), 1 = current frame (pyr1).  Level 0 of a frame built by
+ * next()/redetect() is not stored when the tracker does not visit level 0 (levels L-1, L-1-levelSkip,
+ * ...); reading it then returns COSL_E_INVALID.  detect()/first() and track() store every level. */
 int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* out3, int* w,
                            int* ht);
 /* Copy the cornerness map after non-max suppression input stage (W*H floats) of camera cam. */
