@@ -165,11 +165,43 @@ __device__ __forceinline__ void klt_acc_pixel(KltAcc& A, const float3 I0, const 
   A.ssd = __fmaf_rn(e, e, A.ssd);
 }
 
+// The tracker parameters klt_gain_finish reads, held by value.  The fused kernel picks the lax or
+// strict threshold field by field on the warp-uniform `strict`: a reference to one of two by-value
+// kernel-parameter structs (strict ? Pstrict : Plax) cannot be formed as a pointer, so every field
+// read through it compiled to a chain of predicated constant loads over all candidate offsets.
+struct KltFinishParams {
+  float delta, W, H;         // the same in the lax and the strict set
+  float ssdThr, sqrConv;
+  float vr0, vr1, vr2, vr3;  // validRegion
+};
+
+// c ? a : b as a bit mask, with the mask opaque to the compiler: a plain select of two
+// kernel parameters compiles to a load of one and a predicated constant load of the other
+__device__ __forceinline__ float klt_select(bool c, float a, float b) {
+  const unsigned m = (unsigned)klt_opaque(-(int)c);
+  return __uint_as_float((__float_as_uint(a) & m) | (__float_as_uint(b) & ~m));
+}
+
+__device__ __forceinline__ KltFinishParams klt_finish_params(const KltTrackParams& lax,
+                                                             const KltTrackParams& str, bool strict) {
+  KltFinishParams T;
+  T.delta = lax.delta;
+  T.W = (float)lax.W;
+  T.H = (float)lax.H;
+  T.ssdThr = klt_select(strict, str.ssdThr, lax.ssdThr);
+  T.sqrConv = klt_select(strict, str.sqrConv, lax.sqrConv);
+  T.vr0 = klt_select(strict, str.vr0, lax.vr0);
+  T.vr1 = klt_select(strict, str.vr1, lax.vr1);
+  T.vr2 = klt_select(strict, str.vr2, lax.vr2);
+  T.vr3 = klt_select(strict, str.vr3, lax.vr3);
+  return T;
+}
+
 // reduce over the lane group, solve, test (klt_tracker_with_gain.cg:12-40,124-147)
 // f = group sum of klt_d2_term over the window
 __device__ __forceinline__ float4 klt_gain_finish(KltAcc A, float f, float nbterm, float npxf,
                                                   float X1x, float X1y, float beta,
-                                                  const KltTrackParams& P) {
+                                                  const KltFinishParams P) {
   const float a = grp_sum(A.a0), b = grp_sum(A.a1), c = grp_sum(A.a2);
   const float d = grp_sum(A.d0), e = grp_sum(A.d1);
   const float r0 = grp_sum(A.r0), r1 = grp_sum(A.r1);
@@ -188,8 +220,8 @@ __device__ __forceinline__ float4 klt_gain_finish(KltAcc A, float f, float nbter
   const float ub = __fmul_rn(__fmaf_rn(Ff, r2, __fmaf_rn(Ee, r1, __fmul_rn(Cc, r0))), rdet);
   X1x = __fadd_rn(X1x, ux);
   X1y = __fadd_rn(X1y, uy);
-  ux = __fmul_rn(ux, (float)P.W);
-  uy = __fmul_rn(uy, (float)P.H);
+  ux = __fmul_rn(ux, P.W);
+  uy = __fmul_rn(uy, P.H);
   const float sqrLen = __fmaf_rn(ux, ux, __fmul_rn(uy, uy));
   bool invalid = (det < 0.00001f);
   invalid = invalid || (ssd > P.ssdThr);
@@ -260,7 +292,8 @@ klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
     d2 = __fadd_rn(d2, klt_d2_term(I0, P.lambda, P.delta));
     klt_acc_pixel(A, I0, I1, beta, halfW, halfH, P.lambda);
   }
-  float4 res = klt_gain_finish(A, grp_sum(d2), nbterm, (float)npx, cur.x, cur.y, beta, P);
+  float4 res = klt_gain_finish(A, grp_sum(d2), nbterm, (float)npx, cur.x, cur.y, beta,
+                               klt_finish_params(P, P, false));  // the host chose P per pass
   if (pre_invalid) res = make_float4(-1.f, -1.f, -1.f, 0.f);
   if (gl == 0 && active) out[fb + slot] = res;
 }
@@ -603,7 +636,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         KLT_CLK(c3p);
         const float nbterm = klt_nbterm(bn, beta, gl, grpBase);
         float4 res = klt_gain_finish(A, f, nbterm, (float)npx, cur.x, cur.y, beta,
-                                     strict ? Pstrict : Plax);
+                                     klt_finish_params(Plax, Pstrict, strict));
         if (pre_invalid) res = make_float4(-1.f, -1.f, -1.f, 0.f);
         if (staged) cur0 = res;
         if (gl == 0 && active) {
