@@ -44,6 +44,9 @@ def _load():
         f.argtypes = [vp, cf]
     L.cosl_klt_group_next.argtypes = [vp, vp, C.c_size_t, vp, vp]
     L.cosl_klt_group_first.argtypes = [vp, vp, C.c_size_t, vp, vp]
+    L.cosl_klt_group_first_present.argtypes = [vp, vp, C.c_size_t, vp, vp, vp, vp]
+    L.cosl_klt_group_feed.argtypes = [vp, vp, vp, vp, vp]
+    L.cosl_klt_group_advance_cams.argtypes = [vp, vp]
     L.cosl_klt_group_next_dev.argtypes = [vp, vp, C.c_size_t]
     L.cosl_klt_group_fetch.argtypes = [vp, vp, vp]
     L.cosl_klt_group_sync.argtypes = [vp]
@@ -227,10 +230,47 @@ class KltGroup:
             assert im.dtype == np.uint8 and im.strides[0] == pitch and im.shape == (self.H, self.W)
         return (C.c_void_p * self.C)(*[im.ctypes.data for im in imgs]), pitch
 
-    def first(self, imgs):
+    def _per_cam(self, lists):
+        """Per-camera (n, 3) float32 point lists (None: camera not addressed) -> (counts with -1
+        for None, the arrays, a pointer array)."""
+        assert len(lists) == self.C
+        arrs = [None if p is None else np.ascontiguousarray(p, np.float32).reshape(-1, 3) for p in lists]
+        n = np.array([-1 if a is None else len(a) for a in arrs], np.int32)
+        ptrs = (C.c_void_p * self.C)(*[None if a is None or not len(a) else a.ctypes.data for a in arrs])
+        return n, arrs, ptrs
+
+    def first(self, imgs, present=None):
+        """Batched GPUKLT::first.  present: per-camera (n, 3) point lists (None or empty: no present
+        points for that camera), as in KltTracker.detect."""
         arr, pitch = self._imgs(imgs)
-        _ck(LIB.cosl_klt_group_first(self.h, arr, pitch, self._dest, _ptr(self.counts)))
+        if present is None:
+            _ck(LIB.cosl_klt_group_first(self.h, arr, pitch, self._dest, _ptr(self.counts)))
+        else:
+            n, _arrs, ptrs = self._per_cam(present)
+            n = np.maximum(n, 0)
+            _ck(LIB.cosl_klt_group_first_present(self.h, arr, pitch, _ptr(n), ptrs, self._dest,
+                                                 _ptr(self.counts)))
         return self.feats, self.counts
+
+    def feed(self, pts):
+        """cosl_klt_group_feed: pts[c] = (n, 3) points for camera c, or None to leave it alone.
+        Returns (trackIds per camera, None where not addressed; nFed per camera, 0 where not
+        addressed).  No advance: call advance(cams) after it, as GPUKLT::feedExternFeatPoints does."""
+        n, arrs, ptrs = self._per_cam(pts)
+        ids = [None if a is None else np.full(len(a), -1, np.int32) for a in arrs]
+        idp = (C.c_void_p * self.C)(*[None if i is None or not len(i) else i.ctypes.data for i in ids])
+        fed = np.zeros(self.C, np.int32)
+        _ck(LIB.cosl_klt_group_feed(self.h, _ptr(n), ptrs, idp, _ptr(fed)))
+        return ids, fed
+
+    def advance(self, cams=None):
+        """advanceFrame for the cameras in `cams` (indices; None: every camera, cosl_klt_advance)."""
+        if cams is None:
+            _ck(LIB.cosl_klt_advance(self.h))
+            return
+        mask = np.zeros(self.C, np.uint8)
+        mask[list(cams)] = 1
+        _ck(LIB.cosl_klt_group_advance_cams(self.h, _ptr(mask)))
 
     def next(self, imgs):
         arr, pitch = self._imgs(imgs)

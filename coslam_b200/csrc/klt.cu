@@ -44,24 +44,28 @@ struct cosl_klt {
   // device memory
   uint8_t* d_img = nullptr;
   float4* d_pyr[2] = {nullptr, nullptr};
-  bool lv0Stored[2] = {true, true};  // level 0 of d_pyr[b] holds its frame (see build_pyramid)
+  // level 0 of camera c's slice of d_pyr[b] holds its frame (see build_pyramid); per camera because
+  // cosl_klt_group_advance_cams exchanges single cameras' slices between the buffers
+  bool lv0Stored[2][64];
   int cur = 1;  // pyr1 == d_pyr[cur]
   float* d_corn = nullptr;
   float4 *d_src = nullptr, *d_dst = nullptr, *d_ping = nullptr, *d_pong = nullptr, *d_res = nullptr;
   float4* d_present = nullptr;
+  int* d_nPresent = nullptr;  // [C] lengths of the present lists in d_present
   int* d_nbr = nullptr;
   unsigned long long* d_cand = nullptr;
   unsigned* d_prelim = nullptr;  // [C][prelimCap] packed (y << 16 | x) of 3x3 local maxima
   int prelimCap = 0;
   int* d_counters = nullptr;
   cosl_klt_feature* d_feat = nullptr;
-  float* d_feedpts = nullptr;
-  int* d_feedids = nullptr;
-  int feedCap = 0;
+  // fed points (3 floats each), then their slots and the per-camera placed counts (ints)
+  void* d_feedbuf = nullptr;
+  size_t feedCap = 0;  // bytes
   // pinned host mirrors
   cosl_klt_feature* h_feat = nullptr;
   int* h_counters = nullptr;
   float4* h_present = nullptr;
+  int* h_nPresent = nullptr;
   // frame-pipelined ingest (cosl_klt_group_submit / _collect): two result slots, completion events
   cosl_klt_feature* h_featQ[2] = {nullptr, nullptr};
   int* h_cntQ[2] = {nullptr, nullptr};
@@ -147,6 +151,7 @@ int alloc_group(cosl_klt* g) {
   g->candCap = cap;
   g->smemKeys = std::min(cap, 16384);
   COSL_CUDA(cudaMalloc(&g->d_img, g->imgStride * C));
+  std::fill(&g->lv0Stored[0][0], &g->lv0Stored[0][0] + 2 * 64, true);
   for (int b = 0; b < 2; ++b) {
     COSL_CUDA(cudaMalloc(&g->d_pyr[b], sizeof(float4) * g->pyrStride * C));
     COSL_CUDA(cudaMemsetAsync(g->d_pyr[b], 0, sizeof(float4) * g->pyrStride * C, g->stream));
@@ -169,6 +174,8 @@ int alloc_group(cosl_klt* g) {
   COSL_CUDA(cudaMallocHost(&g->h_feat, sizeof(cosl_klt_feature) * (size_t)F * C));
   COSL_CUDA(cudaMallocHost(&g->h_counters, sizeof(int) * 8 * C));
   COSL_CUDA(cudaMallocHost(&g->h_present, fbytes));
+  COSL_CUDA(cudaMalloc(&g->d_nPresent, sizeof(int) * C));
+  COSL_CUDA(cudaMallocHost(&g->h_nPresent, sizeof(int) * C));
   // neighbour slots of the gain smoothness term (klt_tracker_with_gain.cg:64-75): NEAREST,
   // CLAMP_TO_EDGE lookups in the featW x featH slot texture at st0 +- ds0; betaN1 adds the SCALAR
   // ds0.x (resp. ds0.y) to both coordinates.
@@ -281,6 +288,7 @@ void free_group(cosl_klt* g) {
   cudaFree(g->d_pong);
   cudaFree(g->d_res);
   cudaFree(g->d_present);
+  cudaFree(g->d_nPresent);
   cudaFree(g->d_nbr);
   if (g->auxStream) cudaStreamDestroy(g->auxStream);
   if (g->evPre) cudaEventDestroy(g->evPre);
@@ -292,14 +300,14 @@ void free_group(cosl_klt* g) {
   cudaFree(g->d_prelim);
   cudaFree(g->d_counters);
   cudaFree(g->d_feat);
-  cudaFree(g->d_feedpts);
-  cudaFree(g->d_feedids);
+  cudaFree(g->d_feedbuf);
   cudaFree(g->d_state);
   cudaFree(g->d_ver);
   cudaFree(g->d_waitset);
   cudaFreeHost(g->h_feat);
   cudaFreeHost(g->h_counters);
   cudaFreeHost(g->h_present);
+  cudaFreeHost(g->h_nPresent);
   for (int i = 0; i < 2; ++i) {
     if (g->h_featQ[i]) cudaFreeHost(g->h_featQ[i]);
     if (g->h_cntQ[i]) cudaFreeHost(g->h_cntQ[i]);
@@ -360,7 +368,7 @@ static bool tracker_reads_level0(const cosl_klt* g) { return (g->L - 1) % g->lev
 int build_pyramid(cosl_klt* g, bool wantCorn, bool trackOnly = false) {
   float4* P = g->d_pyr[g->cur];
   const bool storeL0 = !(trackOnly && wantCorn) || tracker_reads_level0(g);
-  g->lv0Stored[g->cur] = storeL0;
+  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = storeL0;
   g->timer.begin(g->secPyr, g->stream);
   // level 0 + level 1 + (optionally) the detector's cornerness map in one pass over the image
   FrontParams fp;
@@ -599,14 +607,16 @@ int run_status(cosl_klt* g) {
 }
 
 // KLT_Detector::detectCorners + extractCorners (v3d_gpuklt.cpp:423-588) and the slot logic of
-// detect/redetect (:651-805).  mode 0: detect (present = external points), 1: redetect.
-int run_detector(cosl_klt* g, int mode, int nPresentExt) {
+// detect/redetect (:651-805).  mode 0: detect (present = the external points of upload_present,
+// maxPresent = the longest list), 1: redetect.
+int run_detector(cosl_klt* g, int mode, int maxPresent) {
   const float Wf = (float)g->W, Hf = (float)g->H, mg = g->detectMargin;
   g->timer.begin(g->secDetect, g->stream);
   if (!g->cornValid) {
     // a pyramid without level 0 always comes with its cornerness map (build_pyramid)
-    if (!g->lv0Stored[g->cur])
-      return set_error(COSL_E_STATE, "detector: level 0 of the current pyramid was not stored");
+    for (int c = 0; c < g->C; ++c)
+      if (!g->lv0Stored[g->cur][c])
+        return set_error(COSL_E_STATE, "detector: level 0 of the current pyramid was not stored");
     dim3 gc(div_up(g->W, DC_TW), div_up(g->H, DC_TH), g->C);
     COSL_LAUNCH(klt_cornerness, gc, 256, 0, g->stream, g->d_pyr[g->cur], g->pyrStride, g->d_corn,
                 g->W, g->H, g->cfg.minCornerness, mg / Wf, mg / Hf, 1.0f - mg / Wf, 1.0f - mg / Hf);
@@ -616,10 +626,11 @@ int run_detector(cosl_klt* g, int mode, int nPresentExt) {
     g->suppressDone = false;  // the tracker's last pass already marked the live tracks
   } else if (mode == 1) {
     dim3 gs(div_up(g->F, 256), g->C);
-    COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_res, g->F, g->F, g->d_corn, g->W, g->H);
-  } else if (nPresentExt > 0) {
-    dim3 gs(div_up(nPresentExt, 256), g->C);
-    COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_present, nPresentExt, g->F, g->d_corn,
+    COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F, g->d_corn,
+                g->W, g->H);
+  } else if (maxPresent > 0) {
+    dim3 gs(div_up(maxPresent, 256), g->C);
+    COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F, g->d_corn,
                 g->W, g->H);
   }
   const int r = std::max(1, g->cfg.minDistance);
@@ -637,8 +648,8 @@ int run_detector(cosl_klt* g, int mode, int nPresentExt) {
   COSL_LAUNCH(klt_select_refill, g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
               g->d_cand, g->candCap, g->plCap, g->d_counters, g->d_feat, g->d_dst,
               g->foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
-              nPresentExt, g->F, g->W, g->H, mode, g->cfg.trackWithGain ? 1 : 0, g->smemKeys,
-              (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
+              maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, g->W, g->H, mode,
+              g->cfg.trackWithGain ? 1 : 0, g->smemKeys, (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
   g->timer.end(g->stream);
   g->advanceDone = g->foldAdvance;
   COSL_CUDA(cudaGetLastError());
@@ -666,6 +677,90 @@ int advance(cosl_klt* g) {
   return COSL_OK;
 }
 
+// advance() for the cameras with cams[c] != 0 only.  A strict subset cannot flip `cur`: the cameras'
+// slices of the two pyramid buffers are exchanged instead (klt_advance_cams), and their level-0 flags
+// move with the slices.
+int advance_cams(cosl_klt* g, const uint8_t* cams) {
+  KltCamList L;
+  L.n = 0;
+  for (int c = 0; c < g->C; ++c)
+    if (cams[c]) L.cam[L.n++] = c;
+  if (L.n == g->C) return advance(g);
+  if (L.n == 0) return COSL_OK;
+  dim3 grid((unsigned)std::min<long long>(div_up64(g->pyrStride, 256), 2 * g->numSM), L.n);
+  COSL_LAUNCH(klt_advance_cams, grid, 256, 0, g->stream, g->d_pyr[0], g->d_pyr[1], g->pyrStride, g->d_dst,
+              g->d_src, g->F, L);
+  for (int k = 0; k < L.n; ++k) std::swap(g->lv0Stored[0][L.cam[k]], g->lv0Stored[1][L.cam[k]]);
+  return COSL_OK;
+}
+
+// The present lists of a detect: camera c's nPresent[c] points (x, y, ignored) -> d_present[c][.],
+// the lengths -> d_nPresent.  *maxPresent = the longest list (0: nothing uploaded).
+int upload_present(cosl_klt* g, const int* nPresent, const float* const* present3, int* maxPresent) {
+  int mx = 0;
+  size_t n4 = 0;  // float4s up to the end of the last non-empty list
+  for (int c = 0; c < g->C; ++c) {
+    const int n = nPresent[c];
+    for (int i = 0; i < n; ++i)
+      g->h_present[(size_t)c * g->F + i] = make_float4(present3[c][3 * i], present3[c][3 * i + 1], 0.f, 0.f);
+    g->h_nPresent[c] = n;
+    if (n > 0) n4 = (size_t)c * g->F + n;
+    mx = std::max(mx, n);
+  }
+  *maxPresent = mx;
+  if (mx == 0) return COSL_OK;
+  COSL_CUDA(cudaMemcpyAsync(g->d_present, g->h_present, sizeof(float4) * n4, cudaMemcpyHostToDevice, g->stream));
+  COSL_CUDA(cudaMemcpyAsync(g->d_nPresent, g->h_nPresent, sizeof(int) * g->C, cudaMemcpyHostToDevice, g->stream));
+  return COSL_OK;
+}
+
+// feedExternFeaturePoints (v3d_gpuklt.cpp:808-855) for every camera with npts[c] >= 0, into d_dst:
+// one launch of klt_feed_kill and klt_feed_place for all cameras with points, one H2D copy, one D2H
+// copy, one synchronise.  No advance.
+int feed_cams(cosl_klt* g, const int* npts, const float* const* pts3, int* const* trackIds, int* nFed) {
+  KltFeedList L;
+  L.n = 0;
+  L.off[0] = 0;
+  long long total = 0;
+  for (int c = 0; c < g->C; ++c) {
+    if (npts[c] >= 0) nFed[c] = 0;
+    if (npts[c] <= 0) continue;
+    total += npts[c];
+    if (total > (1 << 26)) return set_error(COSL_E_INVALID, "feed: too many points (%lld)", total);
+    L.cam[L.n] = c;
+    L.off[++L.n] = (int)total;
+  }
+  if (L.n == 0) return COSL_OK;
+  const size_t ptsBytes = sizeof(float) * 3 * total, idsCount = (size_t)total + L.n;
+  const size_t bytes = ptsBytes + sizeof(int) * idsCount;
+  if (bytes > g->feedCap) {
+    cudaFree(g->d_feedbuf);
+    g->d_feedbuf = nullptr;
+    g->feedCap = 0;
+    COSL_CUDA(cudaMalloc(&g->d_feedbuf, bytes));
+    g->feedCap = bytes;
+  }
+  std::vector<float> pts((size_t)3 * total);
+  for (int k = 0; k < L.n; ++k)
+    std::memcpy(pts.data() + (size_t)3 * L.off[k], pts3[L.cam[k]], sizeof(float) * 3 * (L.off[k + 1] - L.off[k]));
+  float* d_pts = (float*)g->d_feedbuf;
+  int* d_ids = (int*)((char*)g->d_feedbuf + ptsBytes);
+  COSL_CUDA(cudaMemcpyAsync(d_pts, pts.data(), ptsBytes, cudaMemcpyHostToDevice, g->stream));
+  COSL_CUDA(cudaMemsetAsync(d_ids, 0xff, sizeof(int) * idsCount, g->stream));
+  COSL_LAUNCH(klt_feed_kill, dim3(div_up(g->F, 256), L.n), 256, 0, g->stream, g->d_dst, g->F, d_pts, L,
+              (g->cfg.compat & COSL_KLT_COMPAT_FEED_STRIDE2) ? 2 : 3);
+  COSL_LAUNCH(klt_feed_place, L.n, 32, 0, g->stream, g->d_dst, g->F, d_pts, L, d_ids, d_ids + total);
+  std::vector<int> ids(idsCount);
+  COSL_CUDA(cudaMemcpyAsync(ids.data(), d_ids, sizeof(int) * idsCount, cudaMemcpyDeviceToHost, g->stream));
+  COSL_CUDA(cudaStreamSynchronize(g->stream));
+  for (int k = 0; k < L.n; ++k) {
+    const int c = L.cam[k];
+    std::memcpy(trackIds[c], ids.data() + L.off[k], sizeof(int) * (L.off[k + 1] - L.off[k]));
+    nFed[c] = ids[total + k];
+  }
+  return COSL_OK;
+}
+
 int do_track(cosl_klt* g, bool wantCorn = false) {
   COSL_TRY(zero_counters(g));  // before the front pass: the early prefilter counts into them
   COSL_TRY(build_pyramid(g, wantCorn, true));
@@ -686,10 +781,10 @@ int do_redetect(cosl_klt* g) {
   return COSL_OK;
 }
 
-int do_detect(cosl_klt* g, int nPresentExt) {
+int do_detect(cosl_klt* g, int maxPresent) {
   COSL_TRY(build_pyramid(g, true));
   COSL_TRY(zero_counters(g));
-  COSL_TRY(run_detector(g, 0, nPresentExt));
+  COSL_TRY(run_detector(g, 0, maxPresent));
   return COSL_OK;
 }
 
@@ -811,14 +906,11 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   if (!img || !dest || !nDetected || nPresent < 0 || nPresent > h->F || (nPresent && !present3) ||
       pitch < (size_t)h->W)
     return set_error(COSL_E_INVALID, "cosl_klt_detect: bad argument");
-  for (int i = 0; i < nPresent; ++i)
-    h->h_present[i] = make_float4(present3[3 * i], present3[3 * i + 1], 0.f, 0.f);
-  if (nPresent)
-    COSL_CUDA(cudaMemcpyAsync(h->d_present, h->h_present, sizeof(float4) * nPresent,
-                              cudaMemcpyHostToDevice, h->stream));
+  int maxPresent = 0;
+  COSL_TRY(upload_present(h, &nPresent, &present3, &maxPresent));
   const uint8_t* imgs[1] = {img};
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(do_detect(h, nPresent));
+  COSL_TRY(do_detect(h, maxPresent));
   COSL_TRY(fetch_results(h));
   copy_out(h, 0, dest);
   *nDetected = h->h_counters[2];
@@ -860,32 +952,7 @@ int cosl_klt_feed(cosl_klt* h, int npts, const float* pts3, int* trackIds, int* 
   KLT_SINGLE(h)
   if (npts < 0 || (npts && (!pts3 || !trackIds)) || !nFed)
     return set_error(COSL_E_INVALID, "cosl_klt_feed: bad argument");
-  *nFed = 0;
-  if (npts == 0) return COSL_OK;
-  if (npts > h->feedCap) {
-    cudaFree(h->d_feedpts);
-    cudaFree(h->d_feedids);
-    h->d_feedpts = nullptr;
-    h->d_feedids = nullptr;
-    h->feedCap = 0;
-    COSL_CUDA(cudaMalloc(&h->d_feedpts, sizeof(float) * 3 * npts));
-    COSL_CUDA(cudaMalloc(&h->d_feedids, sizeof(int) * (npts + 1)));
-    h->feedCap = npts;
-  }
-  COSL_CUDA(cudaMemcpyAsync(h->d_feedpts, pts3, sizeof(float) * 3 * npts, cudaMemcpyHostToDevice,
-                            h->stream));
-  COSL_CUDA(cudaMemsetAsync(h->d_feedids, 0xff, sizeof(int) * (npts + 1), h->stream));
-  COSL_LAUNCH(klt_feed_kill, div_up(h->F, 256), 256, 0, h->stream, h->d_dst, h->F, h->d_feedpts,
-              npts, (h->cfg.compat & COSL_KLT_COMPAT_FEED_STRIDE2) ? 2 : 3);
-  COSL_LAUNCH(klt_feed_place, 1, 32, 0, h->stream, h->d_dst, h->F, h->d_feedpts, npts,
-              h->d_feedids, h->d_feedids + npts);
-  std::vector<int> ids(npts + 1);
-  COSL_CUDA(cudaMemcpyAsync(ids.data(), h->d_feedids, sizeof(int) * (npts + 1),
-                            cudaMemcpyDeviceToHost, h->stream));
-  COSL_CUDA(cudaStreamSynchronize(h->stream));
-  std::memcpy(trackIds, ids.data(), sizeof(int) * npts);
-  *nFed = ids[npts];
-  return COSL_OK;
+  return feed_cams(h, &npts, &pts3, &trackIds, nFed);
 }
 
 int cosl_klt_advance(cosl_klt* h) {
@@ -913,13 +980,18 @@ int cosl_klt_set_ssd(cosl_klt* h, float t) {
   return COSL_OK;
 }
 
-int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
-                         cosl_klt_feature* const* dest, int* nDetected) {
-  KLT_ENTER(h)
-  if (!imgs || pitch < (size_t)h->W) return set_error(COSL_E_INVALID, "group_first: bad argument");
+#define KLT_NOT_IN_FLIGHT(h, name) \
+  if ((h)->nInFlight > 0) return set_error(COSL_E_STATE, name ": submitted frames not yet collected");
+
+// batched GPUKLT::first(f, img[, present, ips]) (tracking/GPUKLT.cpp:111-135): detect + advanceFrame;
+// nPresent == nullptr: no present lists
+static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, const int* nPresent,
+                       const float* const* present3, cosl_klt_feature* const* dest, int* nDetected) {
+  int maxPresent = 0;
+  if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
   h->foldAdvance = true;  // the provided set goes to both feature buffers in one launch
-  const int rcDet = do_detect(h, 0);
+  const int rcDet = do_detect(h, maxPresent);
   h->foldAdvance = false;
   if (rcDet != COSL_OK) return rcDet;
   COSL_TRY(advance(h));
@@ -928,6 +1000,46 @@ int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
     if (dest && dest[c]) copy_out(h, c, dest[c]);
     if (nDetected) nDetected[c] = h->h_counters[8 * c + 2];
   }
+  return COSL_OK;
+}
+
+int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
+                         cosl_klt_feature* const* dest, int* nDetected) {
+  KLT_ENTER(h)
+  if (!imgs || pitch < (size_t)h->W) return set_error(COSL_E_INVALID, "group_first: bad argument");
+  return group_first(h, imgs, pitch, nullptr, nullptr, dest, nDetected);
+}
+
+int cosl_klt_group_first_present(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
+                                 const int* nPresent, const float* const* present3,
+                                 cosl_klt_feature* const* dest, int* nDetected) {
+  KLT_ENTER(h)
+  KLT_NOT_IN_FLIGHT(h, "group_first_present")
+  if (!imgs || pitch < (size_t)h->W || !nPresent)
+    return set_error(COSL_E_INVALID, "group_first_present: bad argument");
+  for (int c = 0; c < h->C; ++c)
+    if (nPresent[c] < 0 || nPresent[c] > h->F || (nPresent[c] > 0 && (!present3 || !present3[c])))
+      return set_error(COSL_E_INVALID, "group_first_present: bad present list of camera %d", c);
+  return group_first(h, imgs, pitch, nPresent, present3, dest, nDetected);
+}
+
+int cosl_klt_group_feed(cosl_klt* h, const int* npts, const float* const* pts3, int* const* trackIds,
+                        int* nFed) {
+  KLT_ENTER(h)
+  KLT_NOT_IN_FLIGHT(h, "group_feed")
+  if (!npts || !nFed) return set_error(COSL_E_INVALID, "group_feed: bad argument");
+  for (int c = 0; c < h->C; ++c)
+    if (npts[c] > 0 && (!pts3 || !pts3[c] || !trackIds || !trackIds[c]))
+      return set_error(COSL_E_INVALID, "group_feed: null point or id list for camera %d", c);
+  return feed_cams(h, npts, pts3, trackIds, nFed);
+}
+
+int cosl_klt_group_advance_cams(cosl_klt* h, const uint8_t* cams) {
+  KLT_ENTER(h)
+  KLT_NOT_IN_FLIGHT(h, "group_advance_cams")
+  if (!cams) return set_error(COSL_E_INVALID, "group_advance_cams: null camera mask");
+  COSL_TRY(advance_cams(h, cams));
+  COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
 
@@ -1035,7 +1147,7 @@ int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* ou
   if (ht) *ht = lh;
   if (!out3) return COSL_OK;
   const int buf = which ? h->cur : 1 - h->cur;
-  if (level == 0 && !h->lv0Stored[buf])
+  if (level == 0 && !h->lv0Stored[buf][cam])
     return set_error(COSL_E_INVALID,
                      "debug_pyramid: level 0 of this pyramid was not stored (a tracked frame keeps only "
                      "the levels its tracker visits; detect() and first() store every level)");

@@ -352,12 +352,13 @@ klt_cornerness(const float4* __restrict__ pyr, long long pyrStride, float* __res
 }
 
 // Suppress detection at the pixel of every live point (presentFeaturesShader, v3d_gpuklt.cpp:475-500).
-// pts: float4 (x, y, .., ..) per slot, x < 0 == dead (clipped).
-__global__ void klt_suppress(const float4* __restrict__ pts, int n, int ptsStride,
-                             float* __restrict__ corn, int W, int H) {
+// pts: float4 (x, y, .., ..) per slot, x < 0 == dead (clipped).  Camera c reads nPer[c] points when
+// nPer is given (present lists of different lengths), else n.
+__global__ void klt_suppress(const float4* __restrict__ pts, int n, const int* __restrict__ nPer,
+                             int ptsStride, float* __restrict__ corn, int W, int H) {
   const int cam = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= (nPer ? nPer[cam] : n)) return;
   const float4 p = pts[(size_t)cam * ptsStride + i];
   if (!(p.x >= 0.0f && p.x < 1.0f && p.y >= 0.0f && p.y < 1.0f)) return;
   const int ix = (int)floorf(__fmul_rn(p.x, (float)W)), iy = (int)floorf(__fmul_rn(p.y, (float)H));
@@ -515,6 +516,7 @@ klt_nm_verify(const float* __restrict__ corn, int W, int H, int r,
 // Single-CTA per camera: sort the candidate keys (bitonic, shared memory when they fit), then do
 // the slot logic of KLT_SequenceTracker::{detect, redetect} (v3d_gpuklt.cpp:651-805) on the device:
 //   mode 0 (detect):   slots [0, nDet) <- strongest corners, [nDet, nDet+nPresent) <- present pts
+//                      (nPresent = nPresentExt[cam], 0 when nPresentExt is null)
 //   mode 1 (redetect): dead slots, in increasing slot index, <- strongest corners
 // and "provide" the new feature table (dst buffer).  counters[cam*8+2] = returned count
 // (nDetected / nNewFeatures as the reference defines them), [3] = raw candidate count.
@@ -562,12 +564,13 @@ __global__ void __launch_bounds__(1024)
 klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
                   int* __restrict__ counters, cosl_klt_feature* __restrict__ dest,
                   float4* __restrict__ dstbuf, float4* __restrict__ alsoSrc,
-                  const float4* __restrict__ present, int nPresentExt,
+                  const float4* __restrict__ present, const int* __restrict__ nPresentPer,
                   int F, int W, int H, int mode, int withGain, int smemKeys, int histo) {
   extern __shared__ unsigned long long s_keys[];
   __shared__ int s_scan[1024];
   __shared__ int s_base;
   const int cam = blockIdx.x;
+  const int nPresentExt = (mode == 0 && nPresentPer) ? nPresentPer[cam] : 0;
   int* cnt = counters + cam * 8;
   unsigned long long* ck = cand + (size_t)cam * candCap;
   const int nCandRaw = cnt[1];
@@ -742,47 +745,100 @@ __global__ void klt_copy_f4(const float4* __restrict__ a, float4* __restrict__ b
 // ------------------------------------------------------------------------------------------
 // feedExternFeaturePoints (v3d_gpuklt.cpp:808-855): (1) kill KLT points within normalised
 // distance^2 < 1e-4 of any fed point, (2) place fed points into dead slots in increasing index.
+// One launch serves every addressed camera of a group: the points of list k (camera cam[k]) are
+// pts3[3 * off[k], 3 * off[k + 1]), their slots go to trackIds[off[k] + j] and the count of placed
+// points to nFed[k].
 // ------------------------------------------------------------------------------------------
-// stride = 3 (default) or 2 (COSL_KLT_COMPAT_FEED_STRIDE2: the reference's reads at :826-827)
+struct KltFeedList {
+  int n;         // addressed cameras
+  int cam[64];
+  int off[65];   // point offsets, off[n] = total
+};
+
+// grid (div_up(F, blockDim.x), n).  stride = 3 (default) or 2 (COSL_KLT_COMPAT_FEED_STRIDE2: the
+// reference's reads at :826-827, within the camera's own list)
 __global__ void klt_feed_kill(float4* __restrict__ buf, int F, const float* __restrict__ pts3,
-                              int npts, int stride) {
+                              KltFeedList L, int stride) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= F) return;
-  float4 c = buf[i];
+  const int k0 = L.off[blockIdx.y], npts = L.off[blockIdx.y + 1] - k0;
+  const float* p = pts3 + 3 * (size_t)k0;
+  float4* b = buf + (size_t)L.cam[blockIdx.y] * F;
+  float4 c = b[i];
   if (c.x < 0.f) return;
   for (int k = 0; k < npts; ++k) {
-    const double dx = (double)(pts3[stride * k] - c.x), dy = (double)(pts3[stride * k + 1] - c.y);
+    const double dx = (double)(p[stride * k] - c.x), dy = (double)(p[stride * k + 1] - c.y);
     if (dx * dx + dy * dy < 1e-4) {
       c.x = -1.0f;
-      buf[i] = c;
+      b[i] = c;
       return;
     }
   }
 }
 
-__global__ void klt_feed_place(float4* __restrict__ buf, int F, const float* __restrict__ pts3,
-                               int npts, int* __restrict__ trackIds, int* __restrict__ nFed) {
-  // single thread block, sequential scan semantics via one warp-stride loop of ballots
-  __shared__ int s_k;
-  if (threadIdx.x == 0) s_k = 0;
-  __syncthreads();
-  for (int start = 0; start < F; start += 32) {
-    if (threadIdx.x < 32) {
-      const int i = start + threadIdx.x;
-      const bool dead = (i < F) && (buf[i].x < 0.f);
-      const unsigned bal = __ballot_sync(0xffffffffu, dead);
-      const int k = s_k + __popc(bal & ((1u << threadIdx.x) - 1));
-      if (dead && k < npts) {
-        buf[i] = make_float4(pts3[3 * k], pts3[3 * k + 1], 1.0f, 0.f);
-        trackIds[k] = i;
-      }
-      __syncwarp();
-      if (threadIdx.x == 0) s_k = min(npts, s_k + __popc(bal));
-      __syncwarp();
+// grid n, one warp per camera: sequential scan semantics via a warp-stride loop of ballots
+__global__ void __launch_bounds__(32) klt_feed_place(float4* __restrict__ buf, int F,
+                                                     const float* __restrict__ pts3, KltFeedList L,
+                                                     int* __restrict__ trackIds, int* __restrict__ nFed) {
+  const int k0 = L.off[blockIdx.x], npts = L.off[blockIdx.x + 1] - k0;
+  const float* p = pts3 + 3 * (size_t)k0;
+  float4* b = buf + (size_t)L.cam[blockIdx.x] * F;
+  int* ids = trackIds + k0;
+  const int lane = threadIdx.x;
+  int base = 0;  // fed points placed so far (warp-uniform)
+  for (int start = 0; start < F && base < npts; start += 32) {
+    const int i = start + lane;
+    const bool dead = (i < F) && (b[i].x < 0.f);
+    const unsigned bal = __ballot_sync(0xffffffffu, dead);
+    const int k = base + __popc(bal & ((1u << lane) - 1));
+    if (dead && k < npts) {
+      b[i] = make_float4(p[3 * k], p[3 * k + 1], 1.0f, 0.f);
+      ids[k] = i;
+    }
+    base = min(npts, base + __popc(bal));
+  }
+  if (lane == 0) nFed[blockIdx.x] = base;
+}
+
+// ------------------------------------------------------------------------------------------
+// advanceFrame (v3d_gpuklt.h:252-259) for a strict subset of a group's cameras: the O(1) flip of
+// the pyramid buffers cannot apply to part of a group, so the cameras' slices of the two buffers
+// are exchanged (an exchange, not a copy: a second advance swaps them back, as the reference's
+// double swap does) and their feature slice is copied dst -> src.  grid (any, n).
+// ------------------------------------------------------------------------------------------
+struct KltCamList {
+  int n;
+  int cam[64];
+};
+
+__global__ void klt_advance_cams(float4* __restrict__ pyrA, float4* __restrict__ pyrB, long long pyrStride,
+                                 const float4* __restrict__ dst, float4* __restrict__ src, int F,
+                                 KltCamList L) {
+  const int cam = L.cam[blockIdx.y];
+  float4* a = pyrA + (size_t)cam * pyrStride;
+  float4* b = pyrB + (size_t)cam * pyrStride;
+  const long long step = (long long)gridDim.x * blockDim.x;
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  for (; i + 3 * step < pyrStride; i += 4 * step) {  // 8 loads in flight per thread
+    float4 ta[4], tb[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      ta[u] = a[i + u * step];
+      tb[u] = b[i + u * step];
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      a[i + u * step] = tb[u];
+      b[i + u * step] = ta[u];
     }
   }
-  __syncthreads();
-  if (threadIdx.x == 0) *nFed = s_k;
+  for (; i < pyrStride; i += step) {
+    const float4 t = a[i];
+    a[i] = b[i];
+    b[i] = t;
+  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < F; i += step)
+    src[(size_t)cam * F + i] = dst[(size_t)cam * F + i];
 }
 
 }  // namespace coslam

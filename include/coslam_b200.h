@@ -147,6 +147,33 @@ int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                          cosl_klt_feature* const* dest, int* nDetected);
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew);
 int cosl_klt_group_sync(cosl_klt* h);
+/* Per-camera forms of the calls a multi-camera CoSLAM loop makes besides next().  Each camera of the
+ * group behaves bit for bit like a single-camera tracker that receives the same calls; cameras a
+ * call does not address keep their state.  All three return COSL_E_STATE while frames submitted
+ * with cosl_klt_group_submit are not yet collected.
+ *
+ * KLT_SequenceTracker::feedExternFeaturePoints (v3d_gpuklt.cpp:808-855) for the cameras with
+ * npts[c] >= 0; what NewMapPtsNCC::output -> SingleSLAM::feedExtraFeatPtsToTracker ->
+ * GPUKLT::feedExternFeatPoints does for one CoSLAM camera group (app/SL_NewMapPointsInterCam.cpp:540-544,
+ * app/SL_SingleSLAM.cpp:1168-1171, tracking/GPUKLT.cpp:163-190), without its advanceFrame.
+ * npts[c] < 0: camera not addressed, pts3[c] / trackIds[c] not read, nFed[c] not written.
+ * pts3[c] = npts[c] float triples as in cosl_klt_feed; trackIds[c] receives npts[c] slots (-1: no
+ * dead slot left); nFed[c] = points placed.  One launch per kernel for all addressed cameras, one
+ * H2D and one D2H copy, one synchronise. */
+int cosl_klt_group_feed(cosl_klt* h, const int* npts, const float* const* pts3, int* const* trackIds,
+                        int* nFed);
+/* KLT_SequenceTracker::advanceFrame (v3d_gpuklt.h:252-259) for the cameras with cams[c] != 0 (C
+ * entries).  All cameras marked is exactly cosl_klt_advance; a strict subset exchanges those
+ * cameras' pyramid slices between the two buffers on the device (a second call swaps them back). */
+int cosl_klt_group_advance_cams(cosl_klt* h, const uint8_t* cams);
+/* GPUKLT::first(f, img, present, ips) (tracking/GPUKLT.cpp:111-135, called per camera by
+ * CoSLAM::initMapMultiCam, app/SL_CoSLAM.cpp:258-262) for the whole group: detect with camera c's
+ * nPresent[c] in [0, featW*featH] present points present3[c] (float triples as in cosl_klt_detect,
+ * may be NULL when nPresent[c] == 0) + advanceFrame.  All nPresent[c] == 0 is exactly
+ * cosl_klt_group_first. */
+int cosl_klt_group_first_present(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
+                                 const int* nPresent, const float* const* present3,
+                                 cosl_klt_feature* const* dest, int* nDetected);
 /* Frame-pipelined form of cosl_klt_group_next (ingest half of SURVEY.md 8f-4; what
  * SingleSLAM::grabReadFrame + GPUKLT::next become when the next frame is already decoded,
  * app/SL_SingleSLAM.cpp:317-327, tracking/GPUKLT.cpp:144-161): submit() enqueues upload, kernels and
@@ -163,7 +190,8 @@ void* cosl_klt_stream(cosl_klt* h);
 /* Copy pyramid level `level` of camera `cam` to host as interleaved (I, Ix, Iy) floats.
  * which: 0 = previous frame (pyr0), 1 = current frame (pyr1).  Level 0 of a frame built by
  * next()/redetect() is not stored when the tracker does not visit level 0 (levels L-1, L-1-levelSkip,
- * ...); reading it then returns COSL_E_INVALID.  detect()/first() and track() store every level. */
+ * ...); reading it then returns COSL_E_INVALID.  detect()/first() and track() store every level.
+ * The record of what was stored follows each camera through cosl_klt_group_advance_cams. */
 int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* out3, int* w,
                            int* ht);
 /* Copy the cornerness map after non-max suppression input stage (W*H floats) of camera cam. */
