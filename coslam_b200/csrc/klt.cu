@@ -34,7 +34,6 @@ struct cosl_klt {
   // suppression marks can only remove candidates, and klt_nm_verify reads the marked map)
   cudaStream_t auxStream = nullptr;
   cudaEvent_t evPre = nullptr;
-  bool earlyPrefilter = false, prefilterDone = false;
   // geometry
   int lvW[8], lvH[8];
   long long lvOff[8];
@@ -73,7 +72,6 @@ struct cosl_klt {
   unsigned subSeq = 0;
   int nInFlight = 0;
   bool havePrev = false;
-  bool cornValid = false;  // cornerness of the current frame already produced by klt_front
   // persistent fused gain tracker (klt_gain_fused)
   float4* d_state = nullptr;             // [C*F]
   unsigned long long* d_ver = nullptr;   // [2][C*F] (pass << 32 | beta bits)
@@ -81,15 +79,11 @@ struct cosl_klt {
   bool fusedOK = false;
   int fusedBlocks = 0;
   int numSM = 132;
-  // launch folding on the combined next() path
-  bool wantTail = false, statusDone = false, suppressDone = false;
-  bool foldAdvance = false, advanceDone = false;
   int detXlo = 0, detXhi = -1, detYlo = 0, detYhi = -1;  // detector window in pixels
   int verBase = 0;
   // TMA descriptors of every pyramid level of both buffers: [buffer][level], load box (source of
   // level + 1) and store box (destination of level - 1 -> level); klt_pyr_tma.cuh
   CUtensorMap tmLoad[2][8], tmStore[2][8];
-  bool tmaOK = false;
   SectionTimer timer;
   int secPyr = 0, secTrack = 0, secDetect = 0, secSelect = 0;
 };
@@ -97,8 +91,9 @@ struct cosl_klt {
 namespace {
 
 // Detector window (klt_detector_pass2.cg: the pixel centre (i + 0.5) / n must lie inside
-// [margin / n, 1 - margin / n]); evaluated with the same fp32 expressions the stand-alone
-// cornerness kernel evaluates per pixel, so the integer bounds select exactly the same pixels.
+// [margin / n, 1 - margin / n]); evaluated with the fp32 expressions the oracle's margin mask
+// evaluates per pixel (sx = (x + 0.5f) / W against margin / W and 1 - margin / W,
+// oracle/klt_oracle.cpp), so the integer bounds select exactly the same pixels.
 static void update_detect_window(cosl_klt* g) {
   const float mg = g->detectMargin;
   auto bounds = [](int n, float lo, float hi, int& i0, int& i1) {
@@ -133,6 +128,12 @@ static PassFn pass_kernel(const cosl_klt* g) {
 
 int alloc_group(cosl_klt* g) {
   const int C = g->C, W = g->W, H = g->H, F = g->F;
+  COSL_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
+  COSL_CUDA(cudaStreamCreateWithFlags(&g->copyStream, cudaStreamNonBlocking));
+  COSL_CUDA(cudaEventCreateWithFlags(&g->evFront, cudaEventDisableTiming));
+  for (int c = 0; c < C; ++c) COSL_CUDA(cudaEventCreateWithFlags(&g->evImg[c], cudaEventDisableTiming));
+  COSL_CUDA(cudaStreamCreateWithFlags(&g->auxStream, cudaStreamNonBlocking));
+  COSL_CUDA(cudaEventCreateWithFlags(&g->evPre, cudaEventDisableTiming));
   long long off = 0;
   for (int l = 0; l < g->L; ++l) {
     g->lvW[l] = W >> l;
@@ -233,33 +234,32 @@ int alloc_group(cosl_klt* g) {
     g->verBase = 0;
   }
   // tensor maps for the TMA pyramid kernel (driver entry point through the runtime: no -lcuda)
-  g->tmaOK = false;
-  if (!std::getenv("COSL_KLT_NO_TMA") && g->L > 2) {
+  if (g->L > 2) {
     typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) == cudaSuccess && fn &&
-        qr == cudaDriverEntryPointSuccess) {
-      bool ok = true;
-      for (int b = 0; b < 2 && ok; ++b)
-        for (int l = 1; l < g->L && ok; ++l) {
-          // a level of the whole camera group: x = texels as pairs of 8-byte elements, y, camera
-          const cuuint64_t dims[3] = {2ull * g->lvW[l], (cuuint64_t)g->lvH[l], (cuuint64_t)C};
-          const cuuint64_t strides[2] = {16ull * g->lvW[l], 16ull * (cuuint64_t)g->pyrStride};
-          const cuuint32_t es[3] = {1, 1, 1};
-          const cuuint32_t boxL[3] = {2 * PT_SW, PT_SH, 1}, boxS[3] = {2 * PT_TW, PT_TH, 1};
-          void* base = (void*)(g->d_pyr[b] + g->lvOff[l]);
-          ok = ok && ((EncodeFn)fn)(&g->tmLoad[b][l], CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, base, dims, strides, boxL,
-                                    es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                    CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-          ok = ok && ((EncodeFn)fn)(&g->tmStore[b][l], CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, base, dims, strides, boxS,
-                                    es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                    CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-        }
-      g->tmaOK = ok;
-    }
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || !fn ||
+        qr != cudaDriverEntryPointSuccess)
+      return set_error(COSL_E_CUDA, "KLT pyramid: cuTensorMapEncodeTiled is not available");
+    for (int b = 0; b < 2; ++b)
+      for (int l = 1; l < g->L; ++l) {
+        // a level of the whole camera group: x = texels as pairs of 8-byte elements, y, camera
+        const cuuint64_t dims[3] = {2ull * g->lvW[l], (cuuint64_t)g->lvH[l], (cuuint64_t)C};
+        const cuuint64_t strides[2] = {16ull * g->lvW[l], 16ull * (cuuint64_t)g->pyrStride};
+        const cuuint32_t es[3] = {1, 1, 1};
+        const cuuint32_t boxL[3] = {2 * PT_SW, PT_SH, 1}, boxS[3] = {2 * PT_TW, PT_TH, 1};
+        void* base = (void*)(g->d_pyr[b] + g->lvOff[l]);
+        if (((EncodeFn)fn)(&g->tmLoad[b][l], CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, base, dims, strides, boxL, es,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS ||
+            ((EncodeFn)fn)(&g->tmStore[b][l], CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, base, dims, strides, boxS, es,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+          return set_error(COSL_E_CUDA, "KLT pyramid: cannot encode the tensor maps of level %d (%dx%d)", l,
+                           g->lvW[l], g->lvH[l]);
+      }
   }
   // dynamic shared memory opt-ins
   COSL_CUDA(cudaFuncSetAttribute(klt_select_refill, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -320,7 +320,7 @@ void free_group(cosl_klt* g) {
 // ---- stages (all asynchronous on g->stream) ----
 
 int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind kind) {
-  if (kind == cudaMemcpyHostToDevice && g->C > 1 && g->copyStream) {
+  if (kind == cudaMemcpyHostToDevice && g->C > 1) {
     // the previous frame's front pass must have consumed d_img before it is overwritten
     if (g->frontRecorded) COSL_CUDA(cudaStreamWaitEvent(g->copyStream, g->evFront, 0));
     const bool flat = (pitch == (size_t)g->W) && (g->imgPitch == (size_t)g->W);  // one contiguous block
@@ -357,18 +357,44 @@ static void launch_prefilter(cosl_klt* g, cudaStream_t st) {
                 g->prelimCap, g->d_counters);
 }
 
-// true when the tracker's level list (L-1, L-1-levelSkip, ...) contains level 0
+// The tracker's level list: L-1, L-1-levelSkip, ... down to >= 0.  scaled: the 2x2 tracker's
+// window step at each level (2^level); 1 for the gain trackers.
+static KltLevels tracker_levels(const cosl_klt* g, bool scaled) {
+  KltLevels LV;
+  LV.n = 0;
+  float mult = scaled ? (float)(1 << (g->L - 1)) : 1.0f;
+  for (int level = g->L - 1; level >= 0; level -= g->levelSkip) {
+    LV.level[LV.n] = level;
+    LV.w[LV.n] = g->lvW[level];
+    LV.h[LV.n] = g->lvH[level];
+    LV.off[LV.n] = g->lvOff[level];
+    LV.mult[LV.n] = mult;
+    if (scaled) mult /= (float)(1 << g->levelSkip);
+    ++LV.n;
+  }
+  return LV;
+}
+
+// true when the tracker's level list contains level 0
 static bool tracker_reads_level0(const cosl_klt* g) { return (g->L - 1) % g->levelSkip == 0; }
 
+// the persistent gain tracker (klt_gain_fused) runs, not the per-pass kernels or the 2x2 tracker
+static bool fused_tracker(const cosl_klt* g) { return g->cfg.trackWithGain && g->fusedOK; }
+
+// What the stages of one frame fold together; run_frame decides it for the frame's kind.
+struct FramePlan {
+  bool wantCorn;        // klt_front also produces the detector's cornerness map
+  bool storeL0;         // klt_front stores pyramid level 0
+  bool earlyPrefilter;  // the detector's prefilter runs on auxStream right after klt_front
+  bool trackerTail;     // the tracker writes the feature table (klt_status) and, with wantCorn, the
+                        // suppression marks of the live tracks (klt_suppress) itself
+  bool foldAdvance;     // klt_select_refill also writes the provided set to d_src (the advance copy)
+};
+
 // PyramidWithDerivativesCreator::buildPyramidForGrayscaleImage (v3d_gpupyramid.cpp:366-429)
-// trackOnly: the frame is built for the tracker.  With the cornerness fused into the front pass as
-// well, nothing but a tracker that visits level 0 reads that level, so it is stored only then: at
-// 16 B/px it is larger than the L2, and writing it would evict the pyramid levels the tracker that
-// follows reads.
-int build_pyramid(cosl_klt* g, bool wantCorn, bool trackOnly = false) {
+int build_pyramid(cosl_klt* g, const FramePlan& p) {
   float4* P = g->d_pyr[g->cur];
-  const bool storeL0 = !(trackOnly && wantCorn) || tracker_reads_level0(g);
-  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = storeL0;
+  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = p.storeL0;
   g->timer.begin(g->secPyr, g->stream);
   // level 0 + level 1 + (optionally) the detector's cornerness map in one pass over the image
   FrontParams fp;
@@ -384,8 +410,8 @@ int build_pyramid(cosl_klt* g, bool wantCorn, bool trackOnly = false) {
   fp.nStrips = div_up(g->W, FS_SW);
   fp.nChunks = div_up(g->H, FS_R);
   fp.wantL1 = g->L > 1 ? 1 : 0;
-  const auto front = storeL0 ? klt_front<true> : klt_front<false>;
-  fp.wantCorn = wantCorn ? 1 : 0;
+  const auto front = p.storeL0 ? klt_front<true> : klt_front<false>;
+  fp.wantCorn = p.wantCorn ? 1 : 0;
   fp.minC = g->cfg.minCornerness;
   fp.ixlo = g->detXlo;
   fp.ixhi = g->detXhi;
@@ -408,25 +434,18 @@ int build_pyramid(cosl_klt* g, bool wantCorn, bool trackOnly = false) {
     dim3 g0(div_up(fp.nStrips * fp.nChunks, FS_WARPS), g->C);
     COSL_LAUNCH(front, g0, 32 * FS_WARPS, 0, g->stream, fp);
   }
-  if (g->evFront) {
-    COSL_CUDA(cudaEventRecord(g->evFront, g->stream));
-    g->frontRecorded = true;
-  }
-  if (g->earlyPrefilter && wantCorn && g->auxStream && g->evFront && g->evPre) {
+  COSL_CUDA(cudaEventRecord(g->evFront, g->stream));
+  g->frontRecorded = true;
+  if (p.earlyPrefilter) {
     COSL_CUDA(cudaStreamWaitEvent(g->auxStream, g->evFront, 0));
     launch_prefilter(g, g->auxStream);
     COSL_CUDA(cudaEventRecord(g->evPre, g->auxStream));
-    g->prefilterDone = true;
   }
-  g->cornValid = wantCorn;
+  // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh)
   for (int l = 2; l < g->L; ++l) {
-    dim3 gl(div_up(g->lvW[l], PD_TW), div_up(g->lvH[l], PD_TH), g->C);
-    if (g->tmaOK)  // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh)
-      COSL_LAUNCH(klt_pyr_down_tma, gl, 256, 0, g->stream, g->tmLoad[g->cur][l - 1], g->tmStore[g->cur][l],
-                  g->lvW[l - 1], g->lvH[l - 1]);
-    else
-      COSL_LAUNCH(klt_pyr_down, gl, 256, 0, g->stream, P + g->lvOff[l - 1], P + g->lvOff[l],
-                  g->pyrStride, g->lvW[l - 1], g->lvH[l - 1], g->lvW[l], g->lvH[l]);
+    dim3 gl(div_up(g->lvW[l], PT_TW), div_up(g->lvH[l], PT_TH), g->C);
+    COSL_LAUNCH(klt_pyr_down_tma, gl, 256, 0, g->stream, g->tmLoad[g->cur][l - 1], g->tmStore[g->cur][l],
+                g->lvW[l - 1], g->lvH[l - 1]);
   }
   g->timer.end(g->stream);
   COSL_CUDA(cudaGetLastError());
@@ -462,24 +481,15 @@ KltTrackParams track_params(const cosl_klt* g, bool strict) {
 
 // KLT_TrackerWithGain::trackFeaturesAndGain (v3d_gpuklt.cpp:205-305) /
 // KLT_Tracker::trackFeatures (:99-161); result -> d_res
-int run_tracker(cosl_klt* g) {
+int run_tracker(cosl_klt* g, const FramePlan& p) {
   const float4* P0 = g->d_pyr[1 - g->cur];
   const float4* P1 = g->d_pyr[g->cur];
   const int wpb = 8;  // warps per block (2x2 tracker: one warp per slot)
   dim3 grid(div_up(g->F, wpb), g->C);
   dim3 gridHalf(div_up(g->F, 256 / KLT_G), g->C);  // gain tracker: one lane group per slot
+  KltLevels LV = tracker_levels(g, !g->cfg.trackWithGain);
   g->timer.begin(g->secTrack, g->stream);
-  if (g->cfg.trackWithGain && g->fusedOK) {
-    KltLevels LV;
-    LV.n = 0;
-    for (int level = g->L - 1; level >= 0; level -= g->levelSkip) {
-      LV.level[LV.n] = level;
-      LV.w[LV.n] = g->lvW[level];
-      LV.h[LV.n] = g->lvH[level];
-      LV.off[LV.n] = g->lvOff[level];
-      LV.mult[LV.n] = 1.0f;
-      ++LV.n;
-    }
+  if (fused_tracker(g)) {
     int nIter = g->cfg.nIterations, C = g->C;
     const int nPass = LV.n * nIter;
     if (g->verBase > 2000000000 - 2 * nPass) {  // version wrap: restart the counters
@@ -490,17 +500,8 @@ int run_tracker(cosl_klt* g) {
     long long pyrStride = g->pyrStride;
     KltTrackParams Plax = track_params(g, false), Pstrict = track_params(g, true);
     int verBase = g->verBase;
-    KltTail tail = {nullptr, nullptr, nullptr, 0, 0, 0};
-    if (g->wantTail) {
-      tail.dest = g->d_feat;
-      tail.counters = g->d_counters;
-      tail.corn = g->d_corn;
-      tail.W = g->W;
-      tail.H = g->H;
-      tail.suppress = g->cornValid ? 1 : 0;  // only a map of THIS frame may be marked
-      g->statusDone = true;
-      g->suppressDone = tail.suppress != 0;
-    }
+    // the feature table and, when this frame produced a cornerness map, its suppression marks
+    KltTail tail = {g->d_feat, g->d_counters, g->d_corn, g->W, g->H, p.wantCorn ? 1 : 0};
     void* args[] = {(void*)&P0,          (void*)&P1,     (void*)&pyrStride, (void*)&LV,
                     (void*)&nIter,       (void*)&g->d_src, (void*)&g->d_state, (void*)&g->d_ver,
                     (void*)&g->d_waitset, (void*)&g->d_res, (void*)&C,        (void*)&Plax,
@@ -545,19 +546,18 @@ int run_tracker(cosl_klt* g) {
     const PassFn pass = pass_kernel(g);
     int which = 0, first = 1;
     bool strict = false;
-    for (int level = g->L - 1; level >= 0; level -= g->levelSkip) {
-      const int w = g->lvW[level], h = g->lvH[level];
+    for (int li = 0; li < LV.n; ++li) {
+      const int w = LV.w[li], h = LV.h[li];
       const float dsx = 1.0f / (float)w, dsy = 1.0f / (float)h;
       for (int iter = 1; iter <= g->cfg.nIterations; ++iter) {
         if (iter == 1)
           strict = false;
         else if (iter == g->cfg.nIterations)
           strict = true;
-        const bool last =
-            (level - g->levelSkip < 0) && (iter == g->cfg.nIterations);
+        const bool last = (li == LV.n - 1) && (iter == g->cfg.nIterations);
         float4* out = last ? g->d_res : bufs[which];
         COSL_LAUNCH(pass, gridHalf, 256, 0, g->stream, P0, P1, g->pyrStride,
-                    g->lvOff[level], w, h, g->d_src, in, out, g->d_nbr, dsx, dsy,
+                    LV.off[li], w, h, g->d_src, in, out, g->d_nbr, dsx, dsy,
                     track_params(g, strict), first);
         in = out;
         which ^= 1;
@@ -565,18 +565,6 @@ int run_tracker(cosl_klt* g) {
       }
     }
   } else {
-    KltLevels LV;
-    LV.n = 0;
-    float mult = (float)(1 << (g->L - 1));
-    for (int level = g->L - 1; level >= 0; level -= g->levelSkip) {
-      LV.level[LV.n] = level;
-      LV.w[LV.n] = g->lvW[level];
-      LV.h[LV.n] = g->lvH[level];
-      LV.off[LV.n] = g->lvOff[level];
-      LV.mult[LV.n] = mult;
-      mult /= (float)(1 << g->levelSkip);
-      ++LV.n;
-    }
     const int nIter = (g->cfg.compat & COSL_KLT_COMPAT_ITER5) ? 5 : g->cfg.nIterations;
     const int hw2 = g->halfWidth, npx2 = (2 * hw2 + 1) * (2 * hw2 + 1);
     const bool tiled = (npx2 <= KLT_G * KLT_ROUNDS) && (2 * hw2 + 4 <= KLT_TW) && (2 * hw2 + 2 <= 8) &&
@@ -595,51 +583,25 @@ int run_tracker(cosl_klt* g) {
   return COSL_OK;
 }
 
-int zero_counters(cosl_klt* g) {
-  COSL_CUDA(cudaMemsetAsync(g->d_counters, 0, sizeof(int) * 8 * g->C, g->stream));
-  return COSL_OK;
-}
-
-int run_status(cosl_klt* g) {
-  dim3 grid(div_up(g->F, 256), g->C);
-  COSL_LAUNCH(klt_status, grid, 256, 0, g->stream, g->d_res, g->d_feat, g->d_counters, g->F);
-  return COSL_OK;
-}
-
 // KLT_Detector::detectCorners + extractCorners (v3d_gpuklt.cpp:423-588) and the slot logic of
-// detect/redetect (:651-805).  mode 0: detect (present = the external points of upload_present,
-// maxPresent = the longest list), 1: redetect.
-int run_detector(cosl_klt* g, int mode, int maxPresent) {
-  const float Wf = (float)g->W, Hf = (float)g->H, mg = g->detectMargin;
+// detect/redetect (:651-805) on the cornerness map klt_front produced for this frame.  mode 0: detect
+// (present = the external points of upload_present, maxPresent = the longest list), 1: redetect.
+int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
   g->timer.begin(g->secDetect, g->stream);
-  if (!g->cornValid) {
-    // a pyramid without level 0 always comes with its cornerness map (build_pyramid)
-    for (int c = 0; c < g->C; ++c)
-      if (!g->lv0Stored[g->cur][c])
-        return set_error(COSL_E_STATE, "detector: level 0 of the current pyramid was not stored");
-    dim3 gc(div_up(g->W, DC_TW), div_up(g->H, DC_TH), g->C);
-    COSL_LAUNCH(klt_cornerness, gc, 256, 0, g->stream, g->d_pyr[g->cur], g->pyrStride, g->d_corn,
-                g->W, g->H, g->cfg.minCornerness, mg / Wf, mg / Hf, 1.0f - mg / Wf, 1.0f - mg / Hf);
-  }
-  g->cornValid = false;  // the suppression below modifies the map
-  if (mode == 1 && g->suppressDone) {
-    g->suppressDone = false;  // the tracker's last pass already marked the live tracks
-  } else if (mode == 1) {
+  if (mode == 1 && !p.trackerTail) {
     dim3 gs(div_up(g->F, 256), g->C);
     COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F, g->d_corn,
                 g->W, g->H);
-  } else if (maxPresent > 0) {
+  } else if (mode == 0 && maxPresent > 0) {
     dim3 gs(div_up(maxPresent, 256), g->C);
     COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F, g->d_corn,
                 g->W, g->H);
   }
   const int r = std::max(1, g->cfg.minDistance);
-  if (g->prefilterDone) {
-    g->prefilterDone = false;
+  if (p.earlyPrefilter)
     COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evPre, 0));
-  } else {
+  else
     launch_prefilter(g, g->stream);
-  }
   dim3 gv(2 * g->numSM, g->C);
   COSL_LAUNCH(klt_nm_verify, gv, 256, 0, g->stream, g->d_corn, g->W, g->H, r, g->d_prelim,
               g->prelimCap, g->d_cand, g->candCap, g->d_counters);
@@ -647,11 +609,10 @@ int run_detector(cosl_klt* g, int mode, int maxPresent) {
   g->timer.begin(g->secSelect, g->stream);
   COSL_LAUNCH(klt_select_refill, g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
               g->d_cand, g->candCap, g->plCap, g->d_counters, g->d_feat, g->d_dst,
-              g->foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
+              p.foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
               maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, g->W, g->H, mode,
               g->cfg.trackWithGain ? 1 : 0, g->smemKeys, (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
   g->timer.end(g->stream);
-  g->advanceDone = g->foldAdvance;
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
@@ -669,10 +630,7 @@ int advance(cosl_klt* g) {
   // swapFeatureBuffers + swap pyramids (v3d_gpuklt.h:252-259); the feature buffer is copied, not
   // swapped, so a later feed() still sees the provided set (see DESIGN.md, quirk list)
   const size_t n = (size_t)g->F * g->C;
-  if (g->advanceDone)
-    g->advanceDone = false;  // klt_select_refill already wrote the provided set to both buffers
-  else
-    COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, g->stream, g->d_dst, g->d_src, n);
+  COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, g->stream, g->d_dst, g->d_src, n);
   g->cur = 1 - g->cur;
   return COSL_OK;
 }
@@ -761,35 +719,56 @@ int feed_cams(cosl_klt* g, const int* npts, const float* const* pts3, int* const
   return COSL_OK;
 }
 
-int do_track(cosl_klt* g, bool wantCorn = false) {
-  COSL_TRY(zero_counters(g));  // before the front pass: the early prefilter counts into them
-  COSL_TRY(build_pyramid(g, wantCorn, true));
-  g->statusDone = g->suppressDone = false;
-  g->wantTail = true;  // the persistent gain tracker writes the feature table itself
-  COSL_TRY(run_tracker(g));
-  g->wantTail = false;
-  if (!g->statusDone) COSL_TRY(run_status(g));
+enum FrameKind {
+  FRAME_DETECT,    // detect, first: pyramid with the cornerness map, detector, slot refill
+  FRAME_TRACK,     // track: pyramid, tracker; the tracked set becomes the next frame's table
+  FRAME_REDETECT,  // redetect, next, next_dev, submit: as FRAME_TRACK, then the detector refills
+};
+
+// One frame through its stages, all asynchronous on g->stream.  This is the one place that decides
+// which launches the frame folds together.  maxPresent: the longest present list of a detect
+// (upload_present).  foldAdvance (detector kinds): advanceFrame follows the frame, and
+// klt_select_refill writes the provided set to both feature buffers, so the advance is the pyramid
+// flip alone.  Nothing of the plan outlives the call.
+int run_frame(cosl_klt* g, FrameKind kind, int maxPresent, bool foldAdvance) {
+  FramePlan p;
+  p.wantCorn = kind != FRAME_TRACK;
+  // A re-detect frame has its cornerness fused into the front pass, so nothing but a tracker that
+  // visits level 0 reads that level.  It is stored only then: at 16 B/px it is larger than the L2,
+  // and writing it would evict the pyramid levels the tracker that follows reads.
+  p.storeL0 = kind != FRAME_REDETECT || tracker_reads_level0(g);
+  p.earlyPrefilter = kind == FRAME_REDETECT;
+  p.trackerTail = fused_tracker(g);
+  p.foldAdvance = foldAdvance;
+  // zeroed first on every kind: the early prefilter counts into them, and a detect frame launches
+  // nothing that reads them before its detector
+  COSL_CUDA(cudaMemsetAsync(g->d_counters, 0, sizeof(int) * 8 * g->C, g->stream));
+  COSL_TRY(build_pyramid(g, p));
+  if (kind != FRAME_DETECT) {
+    COSL_TRY(run_tracker(g, p));
+    if (!p.trackerTail) {
+      dim3 grid(div_up(g->F, 256), g->C);
+      COSL_LAUNCH(klt_status, grid, 256, 0, g->stream, g->d_res, g->d_feat, g->d_counters, g->F);
+    }
+  }
+  if (kind == FRAME_TRACK) {
+    // provide: the tracked set becomes the feature table of the next frame
+    const size_t n = (size_t)g->F * g->C;
+    COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, g->stream, g->d_res, g->d_dst, n);
+  } else {
+    COSL_TRY(run_detector(g, kind == FRAME_REDETECT ? 1 : 0, maxPresent, p));
+  }
+  if (foldAdvance) g->cur = 1 - g->cur;
   return COSL_OK;
 }
 
-int do_redetect(cosl_klt* g) {
-  g->earlyPrefilter = true;
-  const int rcTrack = do_track(g, true);
-  g->earlyPrefilter = false;
-  if (rcTrack != COSL_OK) return rcTrack;
-  COSL_TRY(run_detector(g, 1, 0));
-  return COSL_OK;
-}
-
-int do_detect(cosl_klt* g, int maxPresent) {
-  COSL_TRY(build_pyramid(g, true));
-  COSL_TRY(zero_counters(g));
-  COSL_TRY(run_detector(g, 0, maxPresent));
-  return COSL_OK;
-}
-
-void copy_out(cosl_klt* g, int cam, cosl_klt_feature* dest) {
-  std::memcpy(dest, g->h_feat + (size_t)cam * g->F, sizeof(cosl_klt_feature) * g->F);
+// Camera c's table of `feat` -> dest[c] and its count counters[8c + 2] -> n[c], each where given.
+void copy_out(const cosl_klt* g, const cosl_klt_feature* feat, const int* counters,
+              cosl_klt_feature* const* dest, int* n) {
+  for (int c = 0; c < g->C; ++c) {
+    if (dest && dest[c]) std::memcpy(dest[c], feat + (size_t)c * g->F, sizeof(cosl_klt_feature) * g->F);
+    if (n) n[c] = counters[8 * c + 2];
+  }
 }
 
 }  // namespace
@@ -852,27 +831,6 @@ int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int 
   g->conv = cfg->convergenceThreshold;
   g->ssd = cfg->SSD_Threshold;
   g->detectMargin = 10.0f;  // KLT_Detector::_margin default (v3d_gpuklt.h:113-114)
-  cudaError_t e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) {
-    delete g;
-    return set_error(COSL_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
-  }
-  if (cudaStreamCreateWithFlags(&g->copyStream, cudaStreamNonBlocking) == cudaSuccess) {
-    bool ok = cudaEventCreateWithFlags(&g->evFront, cudaEventDisableTiming) == cudaSuccess;
-    for (int c = 0; c < g->C && ok; ++c)
-      ok = cudaEventCreateWithFlags(&g->evImg[c], cudaEventDisableTiming) == cudaSuccess;
-    if (!ok) {  // fall back to uploads on the compute stream
-      cudaStreamDestroy(g->copyStream);
-      g->copyStream = nullptr;
-    }
-  } else {
-    g->copyStream = nullptr;
-  }
-  if (cudaStreamCreateWithFlags(&g->auxStream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&g->evPre, cudaEventDisableTiming) != cudaSuccess) {
-    if (g->auxStream) cudaStreamDestroy(g->auxStream);
-    g->auxStream = nullptr;
-  }
   int rc = alloc_group(g);
   if (rc != COSL_OK) {
     free_group(g);
@@ -910,10 +868,9 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   COSL_TRY(upload_present(h, &nPresent, &present3, &maxPresent));
   const uint8_t* imgs[1] = {img};
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(do_detect(h, maxPresent));
+  COSL_TRY(run_frame(h, FRAME_DETECT, maxPresent, false));
   COSL_TRY(fetch_results(h));
-  copy_out(h, 0, dest);
-  *nDetected = h->h_counters[2];
+  copy_out(h, h->h_feat, h->h_counters, &dest, nDetected);
   return COSL_OK;
 }
 
@@ -924,10 +881,9 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
     return set_error(COSL_E_INVALID, "cosl_klt_redetect: bad argument");
   const uint8_t* imgs[1] = {img};
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(do_redetect(h));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, 0, false));
   COSL_TRY(fetch_results(h));
-  copy_out(h, 0, dest);
-  *nNewFeatures = h->h_counters[2];
+  copy_out(h, h->h_feat, h->h_counters, &dest, nNewFeatures);
   return COSL_OK;
 }
 
@@ -938,12 +894,9 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
     return set_error(COSL_E_INVALID, "cosl_klt_track: bad argument");
   const uint8_t* imgs[1] = {img};
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(do_track(h));
-  // provide: the tracked set becomes the feature table of the next frame
-  const size_t n = (size_t)h->F;
-  COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, h->stream, h->d_res, h->d_dst, n);
+  COSL_TRY(run_frame(h, FRAME_TRACK, 0, false));
   COSL_TRY(fetch_results(h));
-  copy_out(h, 0, dest);
+  copy_out(h, h->h_feat, h->h_counters, &dest, nullptr);
   *nPresent = h->h_counters[0];
   return COSL_OK;
 }
@@ -990,16 +943,9 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
   int maxPresent = 0;
   if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  h->foldAdvance = true;  // the provided set goes to both feature buffers in one launch
-  const int rcDet = do_detect(h, maxPresent);
-  h->foldAdvance = false;
-  if (rcDet != COSL_OK) return rcDet;
-  COSL_TRY(advance(h));
+  COSL_TRY(run_frame(h, FRAME_DETECT, maxPresent, true));
   COSL_TRY(fetch_results(h));
-  for (int c = 0; c < h->C; ++c) {
-    if (dest && dest[c]) copy_out(h, c, dest[c]);
-    if (nDetected) nDetected[c] = h->h_counters[8 * c + 2];
-  }
+  copy_out(h, h->h_feat, h->h_counters, dest, nDetected);
   return COSL_OK;
 }
 
@@ -1048,16 +994,9 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
   KLT_ENTER(h)
   if (!imgs || pitch < (size_t)h->W) return set_error(COSL_E_INVALID, "group_next: bad argument");
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  h->foldAdvance = true;  // the provided set goes to both feature buffers in one launch
-  const int rcDet = do_redetect(h);
-  h->foldAdvance = false;
-  if (rcDet != COSL_OK) return rcDet;
-  COSL_TRY(advance(h));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, 0, true));
   COSL_TRY(fetch_results(h));
-  for (int c = 0; c < h->C; ++c) {
-    if (dest && dest[c]) copy_out(h, c, dest[c]);
-    if (nNew) nNew[c] = h->h_counters[8 * c + 2];
-  }
+  copy_out(h, h->h_feat, h->h_counters, dest, nNew);
   return COSL_OK;
 }
 
@@ -1066,21 +1005,13 @@ int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pit
   if (!dimgs || pitch < (size_t)h->W)
     return set_error(COSL_E_INVALID, "group_next_dev: bad argument");
   COSL_TRY(upload_images(h, dimgs, pitch, cudaMemcpyDeviceToDevice));
-  h->foldAdvance = true;  // the provided set goes to both feature buffers in one launch
-  const int rcDet = do_redetect(h);
-  h->foldAdvance = false;
-  if (rcDet != COSL_OK) return rcDet;
-  COSL_TRY(advance(h));
-  return COSL_OK;
+  return run_frame(h, FRAME_REDETECT, 0, true);
 }
 
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
   COSL_TRY(fetch_results(h));
-  for (int c = 0; c < h->C; ++c) {
-    if (dest && dest[c]) copy_out(h, c, dest[c]);
-    if (nNew) nNew[c] = h->h_counters[8 * c + 2];
-  }
+  copy_out(h, h->h_feat, h->h_counters, dest, nNew);
   return COSL_OK;
 }
 
@@ -1100,11 +1031,7 @@ int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch)
     COSL_CUDA(cudaEventCreateWithFlags(&h->evDone[slot], cudaEventDisableTiming));
   }
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  h->foldAdvance = true;
-  const int rcDet = do_redetect(h);
-  h->foldAdvance = false;
-  if (rcDet != COSL_OK) return rcDet;
-  COSL_TRY(advance(h));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, 0, true));
   COSL_CUDA(cudaMemcpyAsync(h->h_featQ[slot], h->d_feat, sizeof(cosl_klt_feature) * (size_t)h->F * h->C,
                             cudaMemcpyDeviceToHost, h->stream));
   COSL_CUDA(cudaMemcpyAsync(h->h_cntQ[slot], h->d_counters, sizeof(int) * 8 * h->C, cudaMemcpyDeviceToHost,
@@ -1121,11 +1048,7 @@ int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew
   const int slot = (int)((h->subSeq - (unsigned)h->nInFlight) & 1u);
   COSL_CUDA(cudaEventSynchronize(h->evDone[slot]));
   --h->nInFlight;
-  for (int c = 0; c < h->C; ++c) {
-    if (dest && dest[c])
-      std::memcpy(dest[c], h->h_featQ[slot] + (size_t)c * h->F, sizeof(cosl_klt_feature) * h->F);
-    if (nNew) nNew[c] = h->h_cntQ[slot][8 * c + 2];
-  }
+  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], dest, nNew);
   return COSL_OK;
 }
 
@@ -1181,8 +1104,7 @@ double cosl_klt_algorithmic_bytes(cosl_klt* h) {
   if (!h) return 0;
   // SURVEY.md 8(d): B_frame = C * (25 W H + 4640 F); the 4640 B/feature generalise to
   // n_lvl * 2 * (w+1)^2 * 12 + 32 for other window sizes / level sets
-  int nlv = 0;
-  for (int level = h->L - 1; level >= 0; level -= h->levelSkip) ++nlv;
+  const int nlv = tracker_levels(h, false).n;
   const double w1 = 2 * h->halfWidth + 2;
   double pyr = 1.0;
   for (int l = 0; l < h->L; ++l) pyr += 12.0 / (double)(1 << (2 * l));

@@ -5,8 +5,8 @@
 // so the 16 B/px level-0 texels are written once and never re-read from HBM by the pyramid or the
 // detector.  When nothing will read level 0 (STORE_L0 = false: a tracking frame whose cornerness
 // is fused here and whose tracker skips level 0), it is not written at all.  Every output is
-// computed with the same operations, in the same order, as the stand-alone kernels
-// (klt_pyr_level0, klt_pyr_down, klt_cornerness) and the oracle: bit-exact.
+// computed with the same operations, in the same order, as the oracle (oracle/klt_oracle.cpp):
+// bit-exact.
 // (The level-0 taps 1/8, 1/4, 1/2 are powers of two, so fma(k, x, acc) rounds exactly like
 // acc + k*x; the [1 3 3 1] taps and the structure-tensor sums keep separate mul / add.)
 //

@@ -22,116 +22,14 @@ namespace coslam {
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
 
-// ------------------------------------------------------------------------------------------
-// Pyramid level 0: u8 image -> (I, Ix, Iy).  pyramid_with_derivative_pass1v.cg:63-83 (vertical
-// [1 2 1]/4 and [-1 -2 0 2 1]/8 on the 0..255 image) + pass1h.cg:96-128 (horizontal), fused through
-// shared memory.  Tile: 64 x 16 outputs per 256-thread CTA; the u8 tile (+2 halo) is read once.
-// ------------------------------------------------------------------------------------------
-constexpr int P0_TW = 64, P0_TH = 16;
-
-__global__ void __launch_bounds__(256)
-klt_pyr_level0(const uint8_t* __restrict__ img, size_t imgPitch, size_t imgStride,
-               float4* __restrict__ pyr, long long pyrStride, int W, int H) {
-  __shared__ uint8_t s_img[P0_TH + 4][P0_TW + 4 + 4];
-  __shared__ float s_v[P0_TH][P0_TW + 4];
-  __shared__ float s_dv[P0_TH][P0_TW + 4];
-  const int cam = blockIdx.z;
-  const int x0 = blockIdx.x * P0_TW, y0 = blockIdx.y * P0_TH;
-  const uint8_t* im = img + (size_t)cam * imgStride;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < (P0_TH + 4) * (P0_TW + 4); i += 256) {
-    const int ty = i / (P0_TW + 4), tx = i - ty * (P0_TW + 4);
-    const int gy = clampi(y0 + ty - 2, 0, H - 1), gx = clampi(x0 + tx - 2, 0, W - 1);
-    s_img[ty][tx] = im[(size_t)gy * imgPitch + gx];
-  }
-  __syncthreads();
-  for (int i = tid; i < P0_TH * (P0_TW + 4); i += 256) {
-    const int ty = i / (P0_TW + 4), tx = i - ty * (P0_TW + 4);
-    const float gm2 = s_img[ty][tx], gm1 = s_img[ty + 1][tx], g0 = s_img[ty + 2][tx];
-    const float gp1 = s_img[ty + 3][tx], gp2 = s_img[ty + 4][tx];
-    float vv = __fmul_rn(0.25f, gm1);
-    vv = __fadd_rn(vv, __fmul_rn(0.5f, g0));
-    vv = __fadd_rn(vv, __fmul_rn(0.25f, gp1));
-    float dd = __fmul_rn(-0.125f, gm2);
-    dd = __fadd_rn(dd, __fmul_rn(-0.25f, gm1));
-    dd = __fadd_rn(dd, __fmul_rn(0.25f, gp1));
-    dd = __fadd_rn(dd, __fmul_rn(0.125f, gp2));
-    s_v[ty][tx] = vv;
-    s_dv[ty][tx] = dd;
-  }
-  __syncthreads();
-  float4* out = pyr + (size_t)cam * pyrStride;
-  for (int i = tid; i < P0_TH * P0_TW; i += 256) {
-    const int ty = i / P0_TW, tx = i - ty * P0_TW;
-    const int gx = x0 + tx, gy = y0 + ty;
-    if (gx >= W || gy >= H) continue;
-    // the smem tile was loaded with clamped global coordinates, so tx+2+k indexes the clamped
-    // neighbour directly
-    const float* rv = &s_v[ty][tx];
-    const float* rd = &s_dv[ty][tx];
-    float I = __fmul_rn(0.25f, rv[1]);
-    I = __fadd_rn(I, __fmul_rn(0.5f, rv[2]));
-    I = __fadd_rn(I, __fmul_rn(0.25f, rv[3]));
-    float Ix = __fmul_rn(-0.125f, rv[0]);
-    Ix = __fadd_rn(Ix, __fmul_rn(-0.25f, rv[1]));
-    Ix = __fadd_rn(Ix, __fmul_rn(0.25f, rv[3]));
-    Ix = __fadd_rn(Ix, __fmul_rn(0.125f, rv[4]));
-    float Iy = __fmul_rn(0.25f, rd[1]);
-    Iy = __fadd_rn(Iy, __fmul_rn(0.5f, rd[2]));
-    Iy = __fadd_rn(Iy, __fmul_rn(0.25f, rd[3]));
-    out[(size_t)gy * W + gx] = make_float4(I, Ix, Iy, 0.0f);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// Pyramid level l >= 1: [1 3 3 1]/8 vertical then horizontal with decimation by 2 on all three
-// channels (pyramid_with_derivative_pass2.cg:1-15, host v3d_gpupyramid.cpp:402-420), fused.
-// Tile: 32 x 8 outputs per 256-thread CTA; source tile (66 x 18) staged in shared memory.
-// ------------------------------------------------------------------------------------------
-constexpr int PD_TW = 32, PD_TH = 8;
-
+// [1 3 3 1] / 8 tap of the pyramid levels l >= 1 (pyramid_with_derivative_pass2.cg:1-15, host
+// v3d_gpupyramid.cpp:402-420), applied vertically then horizontally with decimation by 2 on all three
+// channels by klt_front (level 1) and klt_pyr_down_tma (levels >= 2).
 __device__ __forceinline__ float tap1331(float a, float b, float c, float d) {
   float r = __fadd_rn(a, __fmul_rn(3.0f, b));
   r = __fadd_rn(r, __fmul_rn(3.0f, c));
   r = __fadd_rn(r, d);
   return __fmul_rn(r, 0.125f);  // == r / 8 exactly
-}
-
-__global__ void __launch_bounds__(256)
-klt_pyr_down(const float4* __restrict__ src, float4* __restrict__ dst, long long pyrStride, int sw,
-             int sh, int dw, int dh) {
-  __shared__ float4 s_in[2 * PD_TH + 2][2 * PD_TW + 2];
-  __shared__ float4 s_t[PD_TH][2 * PD_TW + 2];
-  const int cam = blockIdx.z;
-  const float4* S = src + (size_t)cam * pyrStride;
-  float4* D = dst + (size_t)cam * pyrStride;
-  const int ox = blockIdx.x * PD_TW, oy = blockIdx.y * PD_TH;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < (2 * PD_TH + 2) * (2 * PD_TW + 2); i += 256) {
-    const int ty = i / (2 * PD_TW + 2), tx = i - ty * (2 * PD_TW + 2);
-    const int gy = clampi(2 * oy - 1 + ty, 0, sh - 1), gx = clampi(2 * ox - 1 + tx, 0, sw - 1);
-    s_in[ty][tx] = S[(size_t)gy * sw + gx];
-  }
-  __syncthreads();
-  for (int i = tid; i < PD_TH * (2 * PD_TW + 2); i += 256) {
-    const int ty = i / (2 * PD_TW + 2), tx = i - ty * (2 * PD_TW + 2);
-    const float4 a = s_in[2 * ty][tx], b = s_in[2 * ty + 1][tx], c = s_in[2 * ty + 2][tx],
-                 d = s_in[2 * ty + 3][tx];
-    s_t[ty][tx] = make_float4(tap1331(a.x, b.x, c.x, d.x), tap1331(a.y, b.y, c.y, d.y),
-                              tap1331(a.z, b.z, c.z, d.z), 0.0f);
-  }
-  __syncthreads();
-  {
-    const int ty = tid / PD_TW, tx = tid - ty * PD_TW;
-    const int gx = ox + tx, gy = oy + ty;
-    if (gx < dw && gy < dh) {
-      const float4 a = s_t[ty][2 * tx], b = s_t[ty][2 * tx + 1], c = s_t[ty][2 * tx + 2],
-                   d = s_t[ty][2 * tx + 3];
-      D[(size_t)gy * dw + gx] =
-          make_float4(tap1331(a.x, b.x, c.x, d.x), tap1331(a.y, b.y, c.y, d.y),
-                      tap1331(a.z, b.z, c.z, d.z), 0.0f);
-    }
-  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -287,68 +185,6 @@ __global__ void klt_status(const float4* __restrict__ res, cosl_klt_feature* __r
   }
   const unsigned m = __ballot_sync(0xffffffffu, live);
   if ((threadIdx.x & 31) == 0 && m) atomicAdd(&counters[cam * 8 + 0], __popc(m));
-}
-
-// ------------------------------------------------------------------------------------------
-// Detector: 7x7 structure tensor of the level-0 gradients, min-eigenvalue cornerness minus
-// threshold, margin mask (klt_detector_pass1.cg, klt_detector_pass2.cg) fused through shared
-// memory; identical operation order to the oracle (bit-exact).  Tile 64 x 16 per 256 threads.
-// ------------------------------------------------------------------------------------------
-constexpr int DC_TW = 64, DC_TH = 16;
-
-__global__ void __launch_bounds__(256)
-klt_cornerness(const float4* __restrict__ pyr, long long pyrStride, float* __restrict__ corn,
-               int W, int H, float minC, float vr0, float vr1, float vr2, float vr3) {
-  __shared__ float2 s_g[DC_TH + 6][DC_TW + 6];
-  __shared__ float s_c0[DC_TH][DC_TW + 6], s_c1[DC_TH][DC_TW + 6], s_c2[DC_TH][DC_TW + 6];
-  const int cam = blockIdx.z;
-  const float4* L0 = pyr + (size_t)cam * pyrStride;
-  const int x0 = blockIdx.x * DC_TW, y0 = blockIdx.y * DC_TH;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < (DC_TH + 6) * (DC_TW + 6); i += 256) {
-    const int ty = i / (DC_TW + 6), tx = i - ty * (DC_TW + 6);
-    const int gy = clampi(y0 + ty - 3, 0, H - 1), gx = clampi(x0 + tx - 3, 0, W - 1);
-    const float4 p = __ldg(&L0[(size_t)gy * W + gx]);
-    s_g[ty][tx] = make_float2(p.y, p.z);
-  }
-  __syncthreads();
-  for (int i = tid; i < DC_TH * (DC_TW + 6); i += 256) {
-    const int ty = i / (DC_TW + 6), tx = i - ty * (DC_TW + 6);
-    float r0 = 0.f, r1 = 0.f, r2 = 0.f;
-#pragma unroll
-    for (int k = 0; k < 7; ++k) {
-      const float2 g = s_g[ty + k][tx];
-      r0 = __fadd_rn(r0, __fmul_rn(g.x, g.x));
-      r1 = __fadd_rn(r1, __fmul_rn(g.x, g.y));
-      r2 = __fadd_rn(r2, __fmul_rn(g.y, g.y));
-    }
-    s_c0[ty][tx] = r0;
-    s_c1[ty][tx] = r1;
-    s_c2[ty][tx] = r2;
-  }
-  __syncthreads();
-  float* out = corn + (size_t)cam * W * H;
-  const float Wf = (float)W, Hf = (float)H;
-  for (int i = tid; i < DC_TH * DC_TW; i += 256) {
-    const int ty = i / DC_TW, tx = i - ty * DC_TW;
-    const int gx = x0 + tx, gy = y0 + ty;
-    if (gx >= W || gy >= H) continue;
-    float a = 0.f, b = 0.f, c = 0.f;
-#pragma unroll
-    for (int k = 0; k < 7; ++k) {
-      a = __fadd_rn(a, s_c0[ty][tx + k]);
-      b = __fadd_rn(b, s_c1[ty][tx + k]);
-      c = __fadd_rn(c, s_c2[ty][tx + k]);
-    }
-    const float amc = __fsub_rn(a, c);
-    const float rad = __fadd_rn(__fmul_rn(amc, amc), __fmul_rn(4.0f, __fmul_rn(b, b)));
-    float cs = __fmul_rn(0.5f, __fsub_rn(__fadd_rn(a, c), __fsqrt_rn(rad)));
-    cs = fmaxf(__fsub_rn(cs, minC), 0.0f);
-    const float sx = __fdiv_rn(__fadd_rn((float)gx, 0.5f), Wf);
-    const float sy = __fdiv_rn(__fadd_rn((float)gy, 0.5f), Hf);
-    const bool inside = (sx >= vr0 && sy >= vr1) && (sx <= vr2 && sy <= vr3);
-    out[(size_t)gy * W + gx] = inside ? cs : 0.0f;
-  }
 }
 
 // Suppress detection at the pixel of every live point (presentFeaturesShader, v3d_gpuklt.cpp:475-500).

@@ -1,7 +1,8 @@
 // klt_pyr_tma.cuh -- pyramid levels >= 2 with the source tile staged into shared memory by TMA.
 //
-// Same arithmetic, in the same order, as klt_pyr_down (pyramid_with_derivative_pass2.cg, host
-// CGKLT/v3d_gpupyramid.cpp:402-420): bit-exact.  What changes is the data movement:
+// [1 3 3 1] / 8 vertically, then horizontally with decimation by 2 (tap1331;
+// pyramid_with_derivative_pass2.cg, host CGKLT/v3d_gpupyramid.cpp:402-420), in the oracle's order:
+// bit-exact.  The data movement is TMA:
 //   * the (2*TW+2) x (2*TH+2) source tile of float4 texels arrives through ONE
 //     cp.async.bulk.tensor.3d (SASS: UTMALDG) issued by one thread and completes on an mbarrier; no
 //     thread computes addresses or clamps coordinates for the load.  The tensor map describes one
