@@ -23,9 +23,11 @@ $(LIB): $(OBJS)
 
 oracle:
 	$(MAKE) -s -C oracle
+	$(MAKE) -s -C oracle -f Makefile.pg_general
 
 clean:
 	rm -f $(CSRC)/*.o $(CSRC)/*.ptxas.log $(LIB)
 	$(MAKE) -C oracle clean
+	$(MAKE) -C oracle -f Makefile.pg_general clean
 
 .PHONY: all oracle clean

@@ -90,6 +90,8 @@ def _load():
     L.cosl_ba_solver_trace.argtypes = [vp, ci, vp, vp, ci]
     L.cosl_ba_solver_tasks.argtypes = [vp, vp, ci, vp, ci]
     L.cosl_posegraph_spread_chains.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, vp, ci]
+    L.cosl_posegraph_solve.argtypes = [ci, vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci]
+    L.cosl_posegraph_last_host_ms.restype = cd
     return L
 
 
@@ -408,6 +410,34 @@ def posegraph_spread_chains(chain_off, fixed, R, t, eR, et, device=0):
     _ck(LIB.cosl_posegraph_spread_chains(len(off) - 1, _ptr(off), _ptr(fx), _ptr(R), _ptr(t),
                                          _ptr(eR), _ptr(et), _ptr(nR), _ptr(nt), int(device)))
     return nR, nt
+
+
+def posegraph_solve(fixed, R, t, id1, id2, eR, et, scale_col=None, n_scale=0, device=0):
+    """cosl_posegraph_solve: GlobalPoseGraph::computeNewCameraRotations + ::computeNewCameraTranslations4
+    on an arbitrary edge set (the camera-group merge).  fixed[n]; R (n,3,3); t (n,3); edges id1 -> id2 with
+    eR (e,3,3), et (e,3); scale_col[e] = shared scale column of edge e (-1: known scale; None: all known).
+    Returns newR (n,3,3), newt (n,3), scale (n_scale,)."""
+    fx = np.ascontiguousarray(fixed, np.uint8)
+    n = fx.size
+    R = np.ascontiguousarray(R, np.float64).reshape(n, 3, 3)
+    t = np.ascontiguousarray(t, np.float64).reshape(n, 3)
+    id1 = np.ascontiguousarray(id1, np.int32)
+    id2 = np.ascontiguousarray(id2, np.int32)
+    ne = id1.size
+    assert id2.size == ne
+    eR = np.ascontiguousarray(eR, np.float64).reshape(ne, 3, 3)
+    et = np.ascontiguousarray(et, np.float64).reshape(ne, 3)
+    sc = None if scale_col is None else np.ascontiguousarray(scale_col, np.int32)
+    assert sc is None or sc.size == ne
+    nR, nt, s = np.empty((n, 3, 3)), np.empty((n, 3)), np.empty(max(1, int(n_scale)))
+    _ck(LIB.cosl_posegraph_solve(n, _ptr(fx), _ptr(R), _ptr(t), ne, _ptr(id1), _ptr(id2), _ptr(eR), _ptr(et),
+                                 _ptr(sc), int(n_scale), _ptr(nR), _ptr(nt), _ptr(s), int(device)))
+    return nR, nt, s[:int(n_scale)]
+
+
+def posegraph_last_host_ms():
+    """Host time (ms) of this thread's last posegraph_solve: validation, numbering, planning, lists."""
+    return float(LIB.cosl_posegraph_last_host_ms())
 
 
 def nccl_unique_id():

@@ -22,8 +22,89 @@
 #include "ba_kernels.cuh"
 #include "ba_tile.cuh"
 #include "common.cuh"
+#include "tile_solve.h"
 
 using namespace coslam;
+
+/* ---------------------------------------------------------------- the tile solve for other callers */
+namespace coslam {
+
+int tile_task_order(const BaPlan& P, std::vector<BaTask>& order) {
+  // two ticket lists (each keeps the critical-path-first order, hence stays topological)
+  order.clear();
+  for (const BaTask& t : P.tasks)
+    if (t.type == BA_T_POTRF || t.type == BA_T_BWD) order.push_back(t);
+  const int nA = (int)order.size();
+  for (const BaTask& t : P.tasks)
+    if (!(t.type == BA_T_POTRF || t.type == BA_T_BWD)) order.push_back(t);
+  // hot successors of every POTRF(k): TRSM(j, k) and the diagonal UPD(j, j, k) of j = first block
+  // of struct(k) -- the next pivot of the dependency chain (ba_tile.cuh)
+  std::vector<int> firstTrsm(P.nb, -1), firstRow(P.nb, 1 << 30);
+  for (int t = 0; t < (int)order.size(); ++t) {
+    const BaTask& k = order[t];
+    if (k.type == BA_T_TRSM && k.i < firstRow[k.k]) {
+      firstRow[k.k] = k.i;
+      firstTrsm[k.k] = t;
+    }
+  }
+  std::vector<int> diagUpd(P.nb, -1);
+  for (int t = 0; t < (int)order.size(); ++t) {
+    const BaTask& k = order[t];
+    if (k.type == BA_T_UPD && (k.flags & 1) && firstTrsm[k.k] >= 0 && k.i == firstRow[k.k]) diagUpd[k.k] = t;
+  }
+  for (BaTask& k : order)
+    if (k.type == BA_T_POTRF) {
+      k.l0 = firstTrsm[k.k];
+      k.l1 = diagUpd[k.k];
+    }
+  return nA;
+}
+
+int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int device, cudaStream_t s) {
+  if (P.nb <= 0) return COSL_OK;
+  BaTileDev td = {};
+  td.rhs = b.rhs;
+  td.tiles = b.tiles;
+  td.rhsS = b.rhsS;
+  td.Linv = b.Linv;
+  td.y = b.y;
+  td.x = b.x;
+  td.cnt = b.cnt;
+  td.tasks = b.tasks;
+  td.bwd = b.bwd;
+  td.sum = b.sum;
+  td.blkRows = b.blkRows;
+  td.nTasks = (int)P.tasks.size();
+  td.nA = nA;
+  td.nb = P.nb;
+  td.nTiles = P.nTiles;
+  td.nCounters = P.nCounters;
+  td.xdoneBase = P.nTiles + P.nScratch;
+  td.sc = b.fail;
+  td.scFail = 0;
+  td.trace = nullptr;
+  const int t00 = P.tileIdx[0];
+  const int t10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
+  const int t11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
+  if (P.nb <= 2 && t00 >= 0 && (P.nb == 1 || t11 >= 0)) {
+    COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+    COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s, td, t00, t10, t11);
+  } else {
+    // same grid rule as the BA solver: never more CTAs than can be co-resident (the tickets spin)
+    COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+    int nsm = 0, perSm = 0;
+    COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+    COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS, BA_TILE_SMEM));
+    if (perSm < 1) return set_error(COSL_E_CUDA, "tile solve: the kernel does not fit on a multiprocessor");
+    const int grid = std::max(2, std::min(std::max(1, nsm), td.nTasks + 1));
+    td.nSpecial = std::max(1, std::min(std::min(24, std::max(1, grid / 6)), grid - 1));
+    COSL_LAUNCH(ba_tile_solve, grid, BA_NTHREADS, BA_TILE_SMEM, s, td);
+  }
+  COSL_CUDA(cudaGetLastError());
+  return COSL_OK;
+}
+
+}  // namespace coslam
 
 /* ---------------------------------------------------------------- NCCL through dlopen */
 namespace {
@@ -545,35 +626,7 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   UP(s->d_camK, camK.data(), sizeof(double) * 5 * m);
   UP(s->d_xy, p->xy, sizeof(double) * 2 * (size_t)N);
   if (!items.empty()) UP(s->d_items, items.data(), sizeof(BaPairItem) * items.size());
-  // two ticket lists (each keeps the critical-path-first order, hence stays topological)
-  s->taskOrder.clear();
-  for (const BaTask& t : P.tasks)
-    if (t.type == BA_T_POTRF || t.type == BA_T_BWD) s->taskOrder.push_back(t);
-  const int nA = (int)s->taskOrder.size();
-  for (const BaTask& t : P.tasks)
-    if (!(t.type == BA_T_POTRF || t.type == BA_T_BWD)) s->taskOrder.push_back(t);
-  {
-    // hot successors of every POTRF(k): TRSM(j, k) and the diagonal UPD(j, j, k) of j = first block
-    // of struct(k) -- the next pivot of the dependency chain (ba_tile.cuh)
-    std::vector<int> firstTrsm(P.nb, -1), firstRow(P.nb, 1 << 30);
-    for (int t = 0; t < (int)s->taskOrder.size(); ++t) {
-      const BaTask& k = s->taskOrder[t];
-      if (k.type == BA_T_TRSM && k.i < firstRow[k.k]) {
-        firstRow[k.k] = k.i;
-        firstTrsm[k.k] = t;
-      }
-    }
-    std::vector<int> diagUpd(P.nb, -1);
-    for (int t = 0; t < (int)s->taskOrder.size(); ++t) {
-      const BaTask& k = s->taskOrder[t];
-      if (k.type == BA_T_UPD && (k.flags & 1) && firstTrsm[k.k] >= 0 && k.i == firstRow[k.k]) diagUpd[k.k] = t;
-    }
-    for (BaTask& k : s->taskOrder)
-      if (k.type == BA_T_POTRF) {
-        k.l0 = firstTrsm[k.k];
-        k.l1 = diagUpd[k.k];
-      }
-  }
+  const int nA = tile_task_order(P, s->taskOrder);
   if (!s->taskOrder.empty()) UP(s->d_tasks, s->taskOrder.data(), sizeof(BaTask) * s->taskOrder.size());
   if (!P.bwdList.empty()) UP(s->d_bwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
   if (!P.sumList.empty()) UP(s->d_sum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());

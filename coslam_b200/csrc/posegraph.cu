@@ -19,11 +19,19 @@
 // Kernel: one CTA per chain, each thread owns a contiguous chunk of nodes; chunk composites are scanned
 // across the CTA in shared memory; newR/newt hold (P_k, q_k) between the two passes.
 // Algorithmic bytes / node: 216 read (R, t, edge R, edge t, flag) + 96 written.
+//
+// The second half of the file solves GENERAL graphs with shared unknown scales (cosl_posegraph_solve,
+// the camera-group merge): normal equations on the BA's tile Cholesky, see the comment above PgItem.
+#include <algorithm>
+#include <chrono>
 #include <cmath>
+#include <map>
 #include <mutex>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
+#include "tile_solve.h"
 
 namespace coslam {
 namespace {
@@ -316,6 +324,246 @@ posegraph_chain_kernel(const int* __restrict__ chainOff, const unsigned char* __
   }
 }
 
+// Stream-ordered allocation from the device's default pool: after the first call a slab comes out of
+// the pool without a device synchronisation (cudaMalloc / cudaFree cost more than the kernels).
+void keep_pool(int device) {
+  static std::mutex mu;
+  static bool kept[64] = {};
+  std::lock_guard<std::mutex> lk(mu);
+  if (device >= 0 && device < 64 && !kept[device]) {
+    kept[device] = true;
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
+      unsigned long long keep = ~0ull;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+  }
+}
+
+// =====================================================================================================
+// General pose graphs (cosl_posegraph_solve): the normal equations of the rotation and translation
+// least-squares systems of GlobalPoseGraph (slam/SL_GlobalPoseEstimation.cpp:52-218, :361-525) as ONE
+// SPD system in the tile layout of ba_plan.h, solved by the BA's tile Cholesky (tile_solve.h).
+//
+// Every edge e = (i -> j) with a row contributes, per 3-vector unknown ("slot") of its end nodes,
+//     x_j - R_e x_i (- s_c t_e for the translation slot of an uncertain edge) = b_e
+// where the slots are the three columns of R_k (rotations) and t_k (translations).  All four slots
+// share the 3x3 blocks of R_e, so the unknowns of a free node form two planner "cameras" (units) of
+// six rows: unit 2f = [col 0 | col 1], unit 2f+1 = [col 2 | t].  Scale column c lives in row c % 6
+// of unit 2 nF + c / 6; unused rows of the last scale unit hold a 1 on the diagonal and a zero rhs.
+// =====================================================================================================
+struct PgItem {  // one 6x6 block of the lower triangle: rows of unit uR, columns of unit uC
+  int uR, uC, rOff, cOff;
+  int e0, e1;  // edges between two different nodes: range in PgDev::pairEdges
+};
+
+struct PgDev {
+  const double *R, *t, *eR, *et;
+  const unsigned char* fixed;
+  const int *id1, *id2, *scaleCol;  // scaleCol: -1 = known scale
+  const int *freeNode, *freeOf;     // free index <-> node
+  const int *nodeOff, *nodeEdges;   // per free node: its edges (all have rows), by edge index
+  const int *colOff, *colEdges;     // per scale column: its edges with rows, by edge index
+  const int* pairEdges;
+  const int* unitPos;                // unit -> index of its first row in the block-padded vector
+  const PgItem* items;
+  const int *itemOff, *diagBlk, *order, *blkCam0, *blkRows;
+  int nF, nScale;
+};
+
+// index of slot s (0..2: column s of R_k, 3: t_k) of free node k in the block-padded vector
+__device__ __forceinline__ int pg_pos(const PgDev& d, int k, int s) {
+  return d.unitPos[2 * d.freeOf[k] + (s >> 1)] + 3 * (s & 1);
+}
+__device__ __forceinline__ int pg_scale_pos(const PgDev& d, int c) {
+  return d.unitPos[2 * d.nF + c / 6] + c % 6;
+}
+
+// residual b_e - (A x0)_e of slot s of edge e (x0 == nullptr: x0 = 0, i.e. the right-hand side b_e)
+__device__ void pg_edge_res(const PgDev& d, const double* __restrict__ x0, int e, int s, double v[3]) {
+  const int i = d.id1[e], j = d.id2[e];
+  const double* Re = d.eR + 9 * (size_t)e;
+  const int c = (s == 3 && d.scaleCol) ? d.scaleCol[e] : -1;
+  double xi[3] = {0, 0, 0}, xj[3] = {0, 0, 0};
+  for (int u = 0; u < 3; ++u) {
+    if (s < 3) {
+      xi[u] = d.fixed[i] ? d.R[9 * (size_t)i + 3 * u + s] : (x0 ? x0[pg_pos(d, i, s) + u] : 0.0);
+      xj[u] = d.fixed[j] ? d.R[9 * (size_t)j + 3 * u + s] : (x0 ? x0[pg_pos(d, j, s) + u] : 0.0);
+    } else {
+      xi[u] = d.fixed[i] ? d.t[3 * (size_t)i + u] : (x0 ? x0[pg_pos(d, i, 3) + u] : 0.0);
+      xj[u] = d.fixed[j] ? d.t[3 * (size_t)j + u] : (x0 ? x0[pg_pos(d, j, 3) + u] : 0.0);
+    }
+  }
+  const double sc = (c >= 0 && x0) ? x0[pg_scale_pos(d, c)] : 0.0;
+  for (int u = 0; u < 3; ++u) {
+    double r = (s == 3 && c < 0) ? d.et[3 * (size_t)e + u] : 0.0;
+    r += Re[3 * u] * xi[0] + Re[3 * u + 1] * xi[1] + Re[3 * u + 2] * xi[2] - xj[u];
+    if (c >= 0) r += sc * d.et[3 * (size_t)e + u];
+    v[u] = r;
+  }
+}
+
+// entry (row r of unit uA, column c of unit uB) of the normal matrix
+__device__ double pg_entry(const PgDev& d, int uA, int r, int uB, int c, int e0, int e1) {
+  const int nodeUnits = 2 * d.nF;
+  if (uA >= nodeUnits && uB >= nodeUnits) {  // scale x scale: diagonal
+    const int ca = 6 * (uA - nodeUnits) + r, cb = 6 * (uB - nodeUnits) + c;
+    if (ca != cb) return 0.0;
+    if (ca >= d.nScale) return 1.0;
+    double v = 0.0;
+    for (int q = d.colOff[ca]; q < d.colOff[ca + 1]; ++q) {
+      const double* te = d.et + 3 * (size_t)d.colEdges[q];
+      v += te[0] * te[0] + te[1] * te[1] + te[2] * te[2];
+    }
+    return v;
+  }
+  if (uA >= nodeUnits || uB >= nodeUnits) {  // translation slot x scale column
+    int un = uA, rn = r, us = uB, cs = c;
+    if (uA >= nodeUnits) {
+      un = uB;
+      rn = c;
+      us = uA;
+      cs = r;
+    }
+    const int col = 6 * (us - nodeUnits) + cs;
+    if (!(un & 1) || rn < 3 || col >= d.nScale) return 0.0;
+    const int f = un >> 1, p = d.freeNode[f], u = rn - 3;
+    double v = 0.0;
+    for (int q = d.nodeOff[f]; q < d.nodeOff[f + 1]; ++q) {
+      const int e = d.nodeEdges[q];
+      if (d.scaleCol[e] != col) continue;
+      const double* te = d.et + 3 * (size_t)e;
+      const double* Re = d.eR + 9 * (size_t)e;
+      v += (d.id2[e] == p) ? -te[u] : Re[u] * te[0] + Re[3 + u] * te[1] + Re[6 + u] * te[2];
+    }
+    return v;
+  }
+  // node x node: the same 3x3 block for every slot, zero between different slots
+  if (2 * (uA & 1) + r / 3 != 2 * (uB & 1) + c / 3) return 0.0;
+  const int p = d.freeNode[uA >> 1], q2 = d.freeNode[uB >> 1], a = r % 3, b = c % 3;
+  double v = 0.0;
+  if (p == q2) {
+    const int f = uA >> 1;
+    for (int q = d.nodeOff[f]; q < d.nodeOff[f + 1]; ++q) {
+      const int e = d.nodeEdges[q];
+      if (d.id2[e] == p) {
+        v += (a == b) ? 1.0 : 0.0;
+      } else {  // (R_e^T R_e)(a, b)
+        const double* Re = d.eR + 9 * (size_t)e;
+        v += Re[a] * Re[b] + Re[3 + a] * Re[3 + b] + Re[6 + a] * Re[6 + b];
+      }
+    }
+  } else {
+    for (int q = e0; q < e1; ++q) {
+      const int e = d.pairEdges[q];
+      const double* Re = d.eR + 9 * (size_t)e;
+      v -= (d.id1[e] == p) ? Re[3 * b + a] : Re[3 * a + b];  // p -> q2: -R_e^T; q2 -> p: -R_e
+    }
+  }
+  return v;
+}
+
+// right-hand side (A^T (b - A x0)) of row r of unit u
+__device__ double pg_rhs(const PgDev& d, const double* __restrict__ x0, int u, int r) {
+  const int nodeUnits = 2 * d.nF;
+  double v = 0.0, res[3];
+  if (u >= nodeUnits) {
+    const int col = 6 * (u - nodeUnits) + r;
+    if (col >= d.nScale) return 0.0;
+    for (int q = d.colOff[col]; q < d.colOff[col + 1]; ++q) {
+      const int e = d.colEdges[q];
+      pg_edge_res(d, x0, e, 3, res);
+      const double* te = d.et + 3 * (size_t)e;
+      v -= te[0] * res[0] + te[1] * res[1] + te[2] * res[2];
+    }
+    return v;
+  }
+  const int f = u >> 1, p = d.freeNode[f], s = 2 * (u & 1) + r / 3, a = r % 3;
+  for (int q = d.nodeOff[f]; q < d.nodeOff[f + 1]; ++q) {
+    const int e = d.nodeEdges[q];
+    pg_edge_res(d, x0, e, s, res);
+    if (d.id2[e] == p) {
+      v += res[a];
+    } else {
+      const double* Re = d.eR + 9 * (size_t)e;
+      v -= Re[a] * res[0] + Re[3 + a] * res[1] + Re[6 + a] * res[2];
+    }
+  }
+  return v;
+}
+
+// One CTA per tile of the plan (fill included): zero it, then write the blocks that land in it and,
+// for a diagonal tile, the block's right-hand side (padding rows 0), as ba_prep_kernel leaves them.
+// Every entry is one thread's sum over a CSR list in a fixed order: no atomics, bit-reproducible.
+__global__ void __launch_bounds__(256)
+pg_assemble(PgDev d, const double* __restrict__ x0, double* __restrict__ tiles, double* __restrict__ rhs) {
+  const int tl = blockIdx.x, tid = threadIdx.x;
+  double2* tile2 = reinterpret_cast<double2*>(tiles + (size_t)tl * 4096);
+#pragma unroll
+  for (int u = 0; u < 8; ++u) tile2[tid + 256 * u] = make_double2(0.0, 0.0);
+  __syncthreads();
+  double* tile = tiles + (size_t)tl * 4096;
+  const int i0 = d.itemOff[tl], n = (d.itemOff[tl + 1] - i0) * 36;
+  for (int q = tid; q < n; q += 256) {
+    const PgItem it = d.items[i0 + q / 36];
+    const int r = (q % 36) / 6, c = q % 6;
+    if (it.uR == it.uC && r < c) continue;  // diagonal block: lower half
+    tile[(it.cOff + c) * 64 + it.rOff + r] = pg_entry(d, it.uR, r, it.uC, c, it.e0, it.e1);
+  }
+  const int k = d.diagBlk[tl];
+  if (k >= 0 && tid < 64) {
+    double v = 0.0;
+    if (tid < d.blkRows[k]) v = pg_rhs(d, x0, d.order[d.blkCam0[k] + tid / 6], tid % 6);
+    rhs[(size_t)k * 64 + tid] = v;
+  }
+}
+
+// x = x1 + x2 (solve + refinement); per node: nearest rotation of the free nodes, copies of the fixed
+// ones (slam/SL_GlobalPoseEstimation.cpp:205-216, :505-513); the scales; out[.. + 1] = 1 on a
+// non-finite result.
+__global__ void __launch_bounds__(128)
+pg_finish(PgDev d, int nNodes, const double* __restrict__ x1, const double* __restrict__ x2,
+          double* __restrict__ newR, double* __restrict__ newt, double* __restrict__ scale,
+          double* __restrict__ nonFinite) {
+  const int k = blockIdx.x * 128 + threadIdx.x;
+  bool bad = false;
+  if (k < nNodes) {
+    if (d.fixed[k]) {
+#pragma unroll
+      for (int i = 0; i < 9; ++i) newR[9 * (size_t)k + i] = d.R[9 * (size_t)k + i];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) newt[3 * (size_t)k + i] = d.t[3 * (size_t)k + i];
+    } else {
+      double M[9], Rn[9];
+      for (int a = 0; a < 3; ++a) {
+        const int p = pg_pos(d, k, a);
+        for (int u = 0; u < 3; ++u) M[3 * u + a] = x1[p + u] + x2[p + u];  // column a of R_k
+      }
+      for (int i = 0; i < 9; ++i) bad |= !isfinite(M[i]);
+      nearest_rotation(M, Rn);
+      const int p = pg_pos(d, k, 3);
+      for (int i = 0; i < 9; ++i) {
+        newR[9 * (size_t)k + i] = Rn[i];
+        bad |= !isfinite(Rn[i]);
+      }
+      for (int u = 0; u < 3; ++u) {
+        const double v = x1[p + u] + x2[p + u];
+        newt[3 * (size_t)k + u] = v;
+        bad |= !isfinite(v);
+      }
+    }
+  }
+  if (k < d.nScale) {
+    const int p = pg_scale_pos(d, k);
+    const double v = x1[p] + x2[p];
+    scale[k] = v;
+    bad |= !isfinite(v);
+  }
+  if (bad) *nonFinite = 1.0;
+}
+
+thread_local double g_pgHostMs = 0.0;
+
 }  // namespace
 }  // namespace coslam
 
@@ -337,21 +585,7 @@ extern "C" int cosl_posegraph_spread_chains(int nChains, const int* chainOff, co
   // one device slab: [R 9N | t 3N | eR 9N | et 3N | newR 9N | newt 3N] doubles, [anchor 2N | off C+1 | status] ints, flags
   const size_t nd = (size_t)36 * N, ni = (size_t)2 * N + nChains + 2;
   const size_t bytes = nd * 8 + ni * 4 + (size_t)N;
-  // stream-ordered allocation from the device's default pool: after the first call the slab comes out of
-  // the pool without a device synchronisation (cudaMalloc / cudaFree cost more than the kernel)
-  {
-    static std::mutex mu;
-    static bool kept[64] = {};
-    std::lock_guard<std::mutex> lk(mu);
-    if (device >= 0 && device < 64 && !kept[device]) {
-      kept[device] = true;
-      cudaMemPool_t pool;
-      if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
-        unsigned long long keep = ~0ull;
-        cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-      }
-    }
-  }
+  keep_pool(device);
   cudaStream_t s = cudaStreamPerThread;
   char* slab = nullptr;
   COSL_CUDA(cudaMallocAsync(&slab, bytes, s));
@@ -391,5 +625,304 @@ extern "C" int cosl_posegraph_spread_chains(int nChains, const int* chainOff, co
   if (status != 0)
     return set_error(COSL_E_INVALID, "cosl_posegraph_spread_chains: chain %d has no fixed node (rank-deficient system)",
                      status - 1);
+  return COSL_OK;
+}
+
+namespace {
+
+// aligned bump layout of one device slab (the same offsets index the host staging buffer)
+struct SlabLayout {
+  size_t bytes = 0;
+  size_t take(size_t n) {
+    const size_t at = (bytes + 255) & ~(size_t)255;
+    bytes = at + n;
+    return at;
+  }
+};
+
+int pg_find(std::vector<int>& parent, int a) {
+  while (parent[a] != a) a = parent[a] = parent[parent[a]];
+  return a;
+}
+
+}  // namespace
+
+extern "C" double cosl_posegraph_last_host_ms(void) { return g_pgHostMs; }
+
+extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const double* R, const double* t,
+                                    int nEdges, const int* id1, const int* id2, const double* eR,
+                                    const double* et, const int* scaleCol, int nScale, double* newR,
+                                    double* newt, double* scale, int device) {
+  const auto tHost0 = std::chrono::steady_clock::now();
+  g_pgHostMs = 0.0;
+  const char* fn = "cosl_posegraph_solve";
+  if (nNodes < 0 || nEdges < 0 || nScale < 0) return set_error(COSL_E_INVALID, "%s: negative count", fn);
+  if (nNodes > 0 && (!fixed || !R || !t || !newR || !newt)) return set_error(COSL_E_INVALID, "%s: null node array", fn);
+  if (nEdges > 0 && (!id1 || !id2 || !eR || !et)) return set_error(COSL_E_INVALID, "%s: null edge array", fn);
+  if (nScale > 0 && !scale) return set_error(COSL_E_INVALID, "%s: null scale array", fn);
+  const int N = nNodes, E = nEdges;
+  // ---- validation: indices, self-loops, rows of the scale columns, components without a fixed node
+  std::vector<int> parent(N), colRows(nScale, 0);
+  for (int k = 0; k < N; ++k) parent[k] = k;
+  for (int e = 0; e < E; ++e) {
+    const int i = id1[e], j = id2[e], c = scaleCol ? scaleCol[e] : -1;
+    if (i < 0 || i >= N || j < 0 || j >= N)
+      return set_error(COSL_E_INVALID, "%s: edge %d joins node %d to node %d (%d nodes)", fn, e, i, j, N);
+    if (i == j) return set_error(COSL_E_INVALID, "%s: edge %d is a self-loop on node %d", fn, e, i);
+    if (c < -1 || c >= nScale)
+      return set_error(COSL_E_INVALID, "%s: edge %d has scale column %d (%d columns)", fn, e, c, nScale);
+    if (fixed[i] && fixed[j]) continue;  // no rows (:59, :368)
+    if (c >= 0) ++colRows[c];
+    const int a = pg_find(parent, i), b = pg_find(parent, j);
+    if (a != b) parent[std::max(a, b)] = std::min(a, b);
+  }
+  for (int c = 0; c < nScale; ++c)
+    if (!colRows[c]) return set_error(COSL_E_INVALID, "%s: scale column %d gets no row", fn, c);
+  {
+    std::vector<uint8_t> anchored(N, 0);
+    for (int k = 0; k < N; ++k)
+      if (fixed[k]) anchored[pg_find(parent, k)] = 1;
+    for (int k = 0; k < N; ++k)
+      if (!fixed[k] && !anchored[pg_find(parent, k)])
+        return set_error(COSL_E_INVALID,
+                         "%s: node %d lies in a connected component without a fixed node (rank-deficient system)",
+                         fn, k);
+  }
+  // ---- numbering: free nodes, units (two per free node, one per 6 scale columns)
+  std::vector<int> freeNode, freeOf(N, -1);
+  for (int k = 0; k < N; ++k)
+    if (!fixed[k]) {
+      freeOf[k] = (int)freeNode.size();
+      freeNode.push_back(k);
+    }
+  const int nF = (int)freeNode.size();
+  if (nF == 0) {  // nothing to solve (and no scale column can have a row): fixed nodes are copied
+    std::memcpy(newR, R, sizeof(double) * 9 * (size_t)N);
+    std::memcpy(newt, t, sizeof(double) * 3 * (size_t)N);
+    return COSL_OK;
+  }
+  const int nG = (nScale + 5) / 6, mf = 2 * nF + nG;
+  // ---- CSR lists in edge order: per free node, per scale column, per node pair
+  std::vector<int> nodeOff(nF + 1, 0), colOff(nScale + 1, 0);
+  for (int e = 0; e < E; ++e) {
+    const int i = id1[e], j = id2[e], c = scaleCol ? scaleCol[e] : -1;
+    if (fixed[i] && fixed[j]) continue;
+    if (!fixed[i]) ++nodeOff[freeOf[i] + 1];
+    if (!fixed[j]) ++nodeOff[freeOf[j] + 1];
+    if (c >= 0) ++colOff[c + 1];
+  }
+  for (int f = 0; f < nF; ++f) nodeOff[f + 1] += nodeOff[f];
+  for (int c = 0; c < nScale; ++c) colOff[c + 1] += colOff[c];
+  std::vector<int> nodeEdges(std::max(1, nodeOff[nF])), colEdges(std::max(1, colOff[nScale]));
+  std::map<std::pair<int, int>, std::vector<int>> pairs;  // free-free edges per unordered free pair
+  std::vector<std::pair<int, int>> scaleAdj;             // (scale group, free node) with an uncertain edge
+  {
+    std::vector<int> nf(nodeOff.begin(), nodeOff.end() - 1), cf(colOff.begin(), colOff.end() - 1);
+    for (int e = 0; e < E; ++e) {
+      const int i = id1[e], j = id2[e], c = scaleCol ? scaleCol[e] : -1;
+      if (fixed[i] && fixed[j]) continue;
+      if (!fixed[i]) nodeEdges[nf[freeOf[i]]++] = e;
+      if (!fixed[j]) nodeEdges[nf[freeOf[j]]++] = e;
+      if (c >= 0) {
+        colEdges[cf[c]++] = e;
+        if (!fixed[i]) scaleAdj.push_back({c / 6, freeOf[i]});
+        if (!fixed[j]) scaleAdj.push_back({c / 6, freeOf[j]});
+      }
+      if (!fixed[i] && !fixed[j]) pairs[{std::min(freeOf[i], freeOf[j]), std::max(freeOf[i], freeOf[j])}].push_back(e);
+    }
+    std::sort(scaleAdj.begin(), scaleAdj.end());
+    scaleAdj.erase(std::unique(scaleAdj.begin(), scaleAdj.end()), scaleAdj.end());
+  }
+  // ---- unit adjacency and the plan
+  std::vector<uint8_t> adj((size_t)mf * mf, 0);
+  auto link = [&](int a, int b) {
+    adj[(size_t)a * mf + b] = 1;
+    adj[(size_t)b * mf + a] = 1;
+  };
+  for (const auto& pr : pairs) {
+    link(2 * pr.first.first, 2 * pr.first.second);
+    link(2 * pr.first.first + 1, 2 * pr.first.second + 1);
+  }
+  for (const auto& sa : scaleAdj) link(2 * nF + sa.first, 2 * sa.second + 1);
+  const BaPlan P = ba_make_plan(mf, adj);
+  if (P.nb <= 0) return set_error(COSL_E_NUMERIC, "%s: planning the solve failed", fn);
+  std::vector<BaTask> tasks;
+  const int nA = tile_task_order(P, tasks);
+  // ---- items: every structurally non-zero 6x6 block of the lower triangle, grouped by tile
+  std::vector<int> unitPos(mf);
+  for (int u = 0; u < mf; ++u) unitPos[u] = P.camBlk[u] * 64 + P.camOff[u];
+  std::vector<int> pairEdges;
+  std::vector<PgItem> raw;
+  auto addItem = [&](int a, int b, int e0, int e1) {
+    // the unit later in the elimination order owns the rows
+    if (unitPos[a] < unitPos[b]) std::swap(a, b);
+    raw.push_back({a, b, P.camOff[a], P.camOff[b], e0, e1});
+  };
+  for (int u = 0; u < mf; ++u) addItem(u, u, 0, 0);
+  for (const auto& pr : pairs) {
+    const int e0 = (int)pairEdges.size();
+    pairEdges.insert(pairEdges.end(), pr.second.begin(), pr.second.end());
+    const int e1 = (int)pairEdges.size();
+    addItem(2 * pr.first.first, 2 * pr.first.second, e0, e1);
+    addItem(2 * pr.first.first + 1, 2 * pr.first.second + 1, e0, e1);
+  }
+  for (const auto& sa : scaleAdj) addItem(2 * nF + sa.first, 2 * sa.second + 1, 0, 0);
+  if (pairEdges.empty()) pairEdges.push_back(0);
+  const int nTiles = P.nTiles, nb = P.nb;
+  auto tileOf = [&](const PgItem& it) { return P.tileIdx[(size_t)P.camBlk[it.uR] * nb + P.camBlk[it.uC]]; };
+  std::vector<int> itemOff(nTiles + 1, 0), diagBlk(nTiles, -1);
+  for (const PgItem& it : raw) ++itemOff[tileOf(it) + 1];
+  for (int q = 0; q < nTiles; ++q) itemOff[q + 1] += itemOff[q];
+  std::vector<PgItem> items(raw.size());
+  {
+    std::vector<int> fill(itemOff.begin(), itemOff.end() - 1);
+    for (const PgItem& it : raw) items[fill[tileOf(it)]++] = it;
+  }
+  for (int k = 0; k < nb; ++k) diagBlk[P.tileIdx[(size_t)k * nb + k]] = k;
+  std::vector<int> sc(E);
+  for (int e = 0; e < E; ++e) sc[e] = scaleCol ? scaleCol[e] : -1;
+  // ---- one slab: inputs (uploaded in one copy, counters included as zeros), work, outputs
+  const size_t nTilesAll = (size_t)nTiles + P.nScratch, nCnt = (size_t)P.nCounters + 2 + tasks.size();
+  SlabLayout L;
+  auto put = [&](size_t bytes) { return L.take(std::max<size_t>(bytes, 8)); };
+  const size_t oR = put(72 * (size_t)N), ot = put(24 * (size_t)N), oeR = put(72 * (size_t)E), oet = put(24 * (size_t)E);
+  const size_t oFixed = put(N), oId1 = put(4 * (size_t)E), oId2 = put(4 * (size_t)E), oSc = put(4 * (size_t)E);
+  const size_t oFreeNode = put(4 * (size_t)nF), oFreeOf = put(4 * (size_t)N);
+  const size_t oNodeOff = put(4 * nodeOff.size()), oNodeEdges = put(4 * nodeEdges.size());
+  const size_t oColOff = put(4 * colOff.size()), oColEdges = put(4 * colEdges.size());
+  const size_t oPair = put(4 * pairEdges.size()), oUnitPos = put(4 * (size_t)mf);
+  const size_t oItems = put(sizeof(PgItem) * items.size()), oItemOff = put(4 * itemOff.size());
+  const size_t oDiag = put(4 * (size_t)nTiles), oOrder = put(4 * (size_t)mf), oBlkCam0 = put(4 * (size_t)(nb + 1));
+  const size_t oBlkRows = put(4 * (size_t)nb), oTasks = put(sizeof(BaTask) * tasks.size());
+  const size_t oBwd = put(sizeof(BaBwdEntry) * P.bwdList.size()), oSum = put(sizeof(BaSumEntry) * P.sumList.size());
+  const size_t oCnt = put(4 * nCnt);
+  const size_t inputBytes = L.bytes;
+  const size_t oRhs = put(8 * (size_t)nb * 64), oTiles = put(8 * nTilesAll * 4096);
+  const size_t oRhsS = put(8 * (size_t)std::max(1, P.nScratch) * 64), oLinv = put(8 * (size_t)nb * 4096);
+  const size_t oY = put(8 * (size_t)nb * 64), oX = put(8 * (size_t)nb * 64), oX1 = put(8 * (size_t)nb * 64);
+  // outputs, contiguous: [newR 9N | newt 3N | scale | pivot failure | non-finite]
+  const size_t nOut = 12 * (size_t)N + nScale + 2;
+  const size_t oOut = put(8 * nOut);
+  std::vector<char> host(inputBytes, 0);
+  auto stage = [&](size_t off, const void* src, size_t bytes) {
+    if (bytes) std::memcpy(host.data() + off, src, bytes);
+  };
+  stage(oR, R, 72 * (size_t)N);
+  stage(ot, t, 24 * (size_t)N);
+  stage(oeR, eR, 72 * (size_t)E);
+  stage(oet, et, 24 * (size_t)E);
+  stage(oFixed, fixed, N);
+  stage(oId1, id1, 4 * (size_t)E);
+  stage(oId2, id2, 4 * (size_t)E);
+  stage(oSc, sc.data(), 4 * (size_t)E);
+  stage(oFreeNode, freeNode.data(), 4 * (size_t)nF);
+  stage(oFreeOf, freeOf.data(), 4 * (size_t)N);
+  stage(oNodeOff, nodeOff.data(), 4 * nodeOff.size());
+  stage(oNodeEdges, nodeEdges.data(), 4 * nodeEdges.size());
+  stage(oColOff, colOff.data(), 4 * colOff.size());
+  stage(oColEdges, colEdges.data(), 4 * colEdges.size());
+  stage(oPair, pairEdges.data(), 4 * pairEdges.size());
+  stage(oUnitPos, unitPos.data(), 4 * (size_t)mf);
+  stage(oItems, items.data(), sizeof(PgItem) * items.size());
+  stage(oItemOff, itemOff.data(), 4 * itemOff.size());
+  stage(oDiag, diagBlk.data(), 4 * (size_t)nTiles);
+  stage(oOrder, P.order.data(), 4 * (size_t)mf);
+  stage(oBlkCam0, P.blkCam0.data(), 4 * (size_t)(nb + 1));
+  stage(oBlkRows, P.blkRows.data(), 4 * (size_t)nb);
+  stage(oTasks, tasks.data(), sizeof(BaTask) * tasks.size());
+  stage(oBwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
+  stage(oSum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
+  g_pgHostMs = 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - tHost0).count();
+  // ---- device
+  COSL_CUDA(cudaSetDevice(device));
+  keep_pool(device);
+  cudaStream_t s = cudaStreamPerThread;
+  char* slab = nullptr;
+  {
+    const cudaError_t e = cudaMallocAsync(&slab, L.bytes, s);
+    if (e == cudaErrorMemoryAllocation) {
+      cudaGetLastError();
+      return set_error(COSL_E_NOMEM, "%s: device allocation of %zu bytes failed", fn, L.bytes);
+    }
+    if (e != cudaSuccess) return set_error(COSL_E_CUDA, "%s: cudaMallocAsync: %s", fn, cudaGetErrorString(e));
+  }
+  auto at = [&](size_t off) { return slab + off; };
+  PgDev d;
+  d.R = reinterpret_cast<const double*>(at(oR));
+  d.t = reinterpret_cast<const double*>(at(ot));
+  d.eR = reinterpret_cast<const double*>(at(oeR));
+  d.et = reinterpret_cast<const double*>(at(oet));
+  d.fixed = reinterpret_cast<const unsigned char*>(at(oFixed));
+  d.id1 = reinterpret_cast<const int*>(at(oId1));
+  d.id2 = reinterpret_cast<const int*>(at(oId2));
+  d.scaleCol = reinterpret_cast<const int*>(at(oSc));
+  d.freeNode = reinterpret_cast<const int*>(at(oFreeNode));
+  d.freeOf = reinterpret_cast<const int*>(at(oFreeOf));
+  d.nodeOff = reinterpret_cast<const int*>(at(oNodeOff));
+  d.nodeEdges = reinterpret_cast<const int*>(at(oNodeEdges));
+  d.colOff = reinterpret_cast<const int*>(at(oColOff));
+  d.colEdges = reinterpret_cast<const int*>(at(oColEdges));
+  d.pairEdges = reinterpret_cast<const int*>(at(oPair));
+  d.unitPos = reinterpret_cast<const int*>(at(oUnitPos));
+  d.items = reinterpret_cast<const PgItem*>(at(oItems));
+  d.itemOff = reinterpret_cast<const int*>(at(oItemOff));
+  d.diagBlk = reinterpret_cast<const int*>(at(oDiag));
+  d.order = reinterpret_cast<const int*>(at(oOrder));
+  d.blkCam0 = reinterpret_cast<const int*>(at(oBlkCam0));
+  d.blkRows = reinterpret_cast<const int*>(at(oBlkRows));
+  d.nF = nF;
+  d.nScale = nScale;
+  double* out = reinterpret_cast<double*>(at(oOut));
+  TileSolveBufs b;
+  b.rhs = reinterpret_cast<double*>(at(oRhs));
+  b.tiles = reinterpret_cast<double*>(at(oTiles));
+  b.rhsS = reinterpret_cast<double*>(at(oRhsS));
+  b.Linv = reinterpret_cast<double*>(at(oLinv));
+  b.y = reinterpret_cast<double*>(at(oY));
+  b.x = reinterpret_cast<double*>(at(oX));
+  b.cnt = reinterpret_cast<int*>(at(oCnt));
+  b.tasks = reinterpret_cast<const BaTask*>(at(oTasks));
+  b.bwd = reinterpret_cast<const BaBwdEntry*>(at(oBwd));
+  b.sum = reinterpret_cast<const BaSumEntry*>(at(oSum));
+  b.blkRows = d.blkRows;
+  b.fail = out + 12 * (size_t)N + nScale;
+  double* x1 = reinterpret_cast<double*>(at(oX1));
+  std::vector<double> hout(nOut);
+  int rc = COSL_OK;
+  auto cuda_step = [&](cudaError_t e, const char* what) {
+    if (rc == COSL_OK && e != cudaSuccess)
+      rc = set_error(COSL_E_CUDA, "%s: %s: %s", fn, what, cudaGetErrorString(e));
+  };
+  cuda_step(cudaMemcpyAsync(slab, host.data(), inputBytes, cudaMemcpyHostToDevice, s), "H2D");
+  cuda_step(cudaMemsetAsync(b.fail, 0, 16, s), "memset");
+  // Normal equations square the condition number (chains of n free nodes: ~n^2), so the solve is
+  // followed by one refinement step: assemble again with the residual A^T (b - A x1) as rhs, solve,
+  // x = x1 + x2 (the same step as oracle/posegraph_general_oracle.cpp).
+  for (int pass = 0; pass < 2 && rc == COSL_OK; ++pass) {
+    if (pass == 1) {
+      cuda_step(cudaMemcpyAsync(x1, b.x, 8 * (size_t)nb * 64, cudaMemcpyDeviceToDevice, s), "D2D");
+      cuda_step(cudaMemsetAsync(b.cnt, 0, 4 * nCnt, s), "memset");
+    }
+    if (rc != COSL_OK) break;
+    COSL_LAUNCH(pg_assemble, nTiles, 256, 0, s, d, pass ? x1 : nullptr, b.tiles, b.rhs);
+    cuda_step(cudaGetLastError(), "pg_assemble");
+    if (rc == COSL_OK) rc = tile_solve_launch(P, nA, b, device, s);
+  }
+  if (rc == COSL_OK) {
+    const int nThr = std::max(N, nScale);
+    COSL_LAUNCH(pg_finish, (unsigned)div_up(nThr, 128), 128, 0, s, d, N, x1, b.x, out, out + 9 * (size_t)N,
+                out + 12 * (size_t)N, out + 12 * (size_t)N + nScale + 1);
+    cuda_step(cudaGetLastError(), "pg_finish");
+  }
+  cuda_step(cudaMemcpyAsync(hout.data(), out, 8 * nOut, cudaMemcpyDeviceToHost, s), "D2H");
+  cuda_step(cudaStreamSynchronize(s), "sync");
+  cudaFreeAsync(slab, s);
+  if (rc != COSL_OK) return rc;
+  if (hout[12 * (size_t)N + nScale] != 0.0)
+    return set_error(COSL_E_NUMERIC, "%s: non-positive pivot in the normal equations", fn);
+  if (hout[12 * (size_t)N + nScale + 1] != 0.0) return set_error(COSL_E_NUMERIC, "%s: non-finite result", fn);
+  std::memcpy(newR, hout.data(), sizeof(double) * 9 * (size_t)N);
+  std::memcpy(newt, hout.data() + 9 * (size_t)N, sizeof(double) * 3 * (size_t)N);
+  if (nScale) std::memcpy(scale, hout.data() + 12 * (size_t)N, sizeof(double) * nScale);
   return COSL_OK;
 }

@@ -8,6 +8,15 @@
 // Supported graphs: what constructCameraGraphs builds -- edge e runs from node e to node e+1, no
 // uncertain-scale edges.  Anything else throws std::runtime_error (the constrained variants
 // computeNewCamera*2/3/4 and save/load are not on the post-BA path and are not provided).
+//
+// With COSL_POSEGRAPH_GENERAL defined (for EVERY translation unit of the program: the class layout and
+// its inline methods differ, so mixing breaks the one-definition rule) the header also serves
+// MergeCameraGroup (app/SL_MergeCameraGroup.cpp:907-1102): computeNewCameraRotations /
+// computeNewCameraTranslations accept any edge set without uncertain-scale edges, and
+// computeNewCameraTranslations4() solves the shared-scale translations.  Chain graphs without
+// uncertain edges still go to cosl_posegraph_spread_chains (the same bits as without the definition);
+// every other graph goes to cosl_posegraph_solve.  A rotations call followed by a translations call is
+// one ABI call either way.
 #ifndef SL_GLOBALPOSEESTIMATION_H_
 #define SL_GLOBALPOSEESTIMATION_H_
 #include <cassert>
@@ -131,6 +140,11 @@ public:
 	// slam/SL_GlobalPoseEstimation.cpp:220-359: newt = spread translations (newR of free nodes untouched,
 	// fixed nodes get copies of R, t as at :339-343)
 	void computeNewCameraTranslations() {
+#ifdef COSL_POSEGRAPH_GENERAL
+		for (int e = 0; e < nEdges; ++e)
+			if (poseEdges[e].uncertainScale)
+				throw std::runtime_error("GlobalPoseGraph (coslam_b200): computeNewCameraTranslations with uncertain-scale edges is not supported (use computeNewCameraTranslations4)");
+#endif
 		if (!m_haveT)
 			solve();
 		for (int k = 0; k < nNodes; ++k) {
@@ -140,8 +154,30 @@ public:
 		}
 		m_haveT = false;
 	}
+#ifdef COSL_POSEGRAPH_GENERAL
+	// slam/SL_GlobalPoseEstimation.cpp:361-525: newt = translations with one unknown scale per scale id of
+	// the constraint edges (:383-403); fixed nodes get copies of R, t (:505-513); CamPoseEdge::s of every
+	// uncertain-scale edge = its solved scale (:515-522)
+	void computeNewCameraTranslations4() {
+		if (!m_haveT)
+			solve();
+		for (int k = 0; k < nNodes; ++k) {
+			if (poseNodes[k].fixed)
+				std::memcpy(poseNodes[k].newR, poseNodes[k].R, sizeof(double) * 9);
+			std::memcpy(poseNodes[k].newt, &m_newt[3 * (size_t) k], sizeof(double) * 3);
+		}
+		for (int e = 0; e < nEdges; ++e)
+			if (poseEdges[e].uncertainScale && poseEdges[e].scaleId >= 0)
+				poseEdges[e].s = m_scale[m_scaleCol[e]];
+		m_haveT = false;
+	}
+#endif
 private:
 	std::vector<double> m_newR, m_newt;
+#ifdef COSL_POSEGRAPH_GENERAL
+	std::vector<double> m_scale;
+	std::vector<int> m_scaleCol;
+#endif
 	bool m_haveT;
 	GlobalPoseGraph(const GlobalPoseGraph&);
 	GlobalPoseGraph& operator=(const GlobalPoseGraph&);
@@ -152,6 +188,15 @@ private:
 		m_newt.assign(3 * n, 0.0);
 		if (nNodes == 0)
 			return;
+#ifdef COSL_POSEGRAPH_GENERAL
+		bool chain = nEdges == nNodes - 1;
+		for (int e = 0; chain && e < nEdges; ++e)
+			chain = poseEdges[e].id1 == e && poseEdges[e].id2 == e + 1 && !poseEdges[e].uncertainScale;
+		if (!chain) {
+			solveGeneral();
+			return;
+		}
+#endif
 		if (nEdges != nNodes - 1)
 			throw std::runtime_error("GlobalPoseGraph (coslam_b200): only chain graphs are supported (nEdges != nNodes-1)");
 		std::vector<double> R(9 * n), t(3 * n), eR(9 * n, 0.0), et(3 * n, 0.0);
@@ -176,6 +221,52 @@ private:
 		if (rc != COSL_OK)
 			throw std::runtime_error(std::string("GlobalPoseGraph (coslam_b200): ") + cosl_last_error());
 	}
+#ifdef COSL_POSEGRAPH_GENERAL
+	// any edge set: scale ids -> columns as :383-403 (the distinct ids of the constraint edges, in
+	// increasing order); an uncertain edge whose id no constraint edge carries is refused (the reference
+	// reads column -1 there, which aliases the last translation unknown)
+	void solveGeneral() {
+		const size_t n = (size_t) nNodes, ne = (size_t) nEdges;
+		std::vector<int> colOfId(ne, -1), id1(ne), id2(ne);
+		for (int e = 0; e < nEdges; ++e)
+			if (poseEdges[e].constraint) {
+				const int sId = poseEdges[e].scaleId;
+				if (sId < 0 || sId >= nEdges)
+					throw std::runtime_error("GlobalPoseGraph (coslam_b200): constraint edge with a scale id outside [0, nEdges)");
+				colOfId[sId] = 0;
+			}
+		int nScale = 0;
+		for (int k = 0; k < nEdges; ++k)
+			if (colOfId[k] >= 0)
+				colOfId[k] = nScale++;
+		m_scaleCol.assign(ne, -1);
+		std::vector<double> R(9 * n), t(3 * n), eR(9 * ne), et(3 * ne);
+		std::vector<uint8_t> fixed(n);
+		for (int k = 0; k < nNodes; ++k) {
+			std::memcpy(&R[9 * (size_t) k], poseNodes[k].R, sizeof(double) * 9);
+			std::memcpy(&t[3 * (size_t) k], poseNodes[k].t, sizeof(double) * 3);
+			fixed[k] = poseNodes[k].fixed ? 1 : 0;
+		}
+		for (int e = 0; e < nEdges; ++e) {
+			const CamPoseEdge& ed = poseEdges[e];
+			id1[e] = ed.id1;
+			id2[e] = ed.id2;
+			std::memcpy(&eR[9 * (size_t) e], ed.R, sizeof(double) * 9);
+			std::memcpy(&et[3 * (size_t) e], ed.t, sizeof(double) * 3);
+			if (ed.uncertainScale) {
+				const int c = (ed.scaleId >= 0 && ed.scaleId < nEdges) ? colOfId[ed.scaleId] : -1;
+				if (c < 0)
+					throw std::runtime_error("GlobalPoseGraph (coslam_b200): an uncertain-scale edge has a scale id that no constraint edge carries");
+				m_scaleCol[e] = c;
+			}
+		}
+		m_scale.assign(nScale > 0 ? nScale : 1, 0.0);
+		const int rc = cosl_posegraph_solve(nNodes, fixed.data(), R.data(), t.data(), nEdges, id1.data(), id2.data(),
+				eR.data(), et.data(), m_scaleCol.data(), nScale, m_newR.data(), m_newt.data(), m_scale.data(), device);
+		if (rc != COSL_OK)
+			throw std::runtime_error(std::string("GlobalPoseGraph (coslam_b200): ") + cosl_last_error());
+	}
+#endif
 };
 
 // All cameras' graphs in ONE launch (what updateNonKeyCameraPoses' loop over cameras becomes when the

@@ -297,3 +297,167 @@ def make_pose_chains(lengths, key_every=8, seed=0, shift=0.03, lead_free=0, fixe
     return dict(chain_off=off, fixed=fixed, R=R, t=t, eR=eR, et=et, id1=id1, id2=id2,
                 eR_list=eR[id1] if len(id1) else np.zeros((0, 3, 3)),
                 et_list=et[id1] if len(id1) else np.zeros((0, 3)))
+
+
+def _rel(Ra, ta, Rb, tb):
+    """Rigid transform from pose a to pose b (getRigidTransFromTo): x_b = R x_a + t."""
+    R = Rb @ Ra.T
+    return R, tb - R @ ta
+
+
+def scale_columns(scale_id):
+    """Scale column of every edge the way computeNewCameraTranslations4 numbers them
+    (slam/SL_GlobalPoseEstimation.cpp:383-403): the distinct scale ids of the constraint edges in
+    increasing order; -1 for an edge without one.  Returns (columns, number of columns)."""
+    sid = np.asarray(scale_id, np.int64)
+    ids = np.unique(sid[sid >= 0])
+    col = np.full(sid.shape, -1, np.int32)
+    for c, s in enumerate(ids):
+        col[sid == s] = c
+    return col, len(ids)
+
+
+def _trajectories(rng, n_frames, n_cams):
+    R, t = np.zeros((n_frames, n_cams, 3, 3)), np.zeros((n_frames, n_cams, 3))
+    for c in range(n_cams):
+        R[0, c] = _rodrigues(rng.normal(size=3))
+        t[0, c] = rng.normal(size=3)
+        for k in range(1, n_frames):
+            R[k, c] = _rodrigues(rng.normal(size=3) * 0.05) @ R[k - 1, c]
+            t[k, c] = t[k - 1, c] + rng.normal(size=3) * 0.1
+    return R, t
+
+
+def _noisy(rng, R, t, noise):
+    if noise <= 0:
+        return R, t
+    return _rodrigues(rng.normal(size=3) * noise) @ R, t + rng.normal(size=3) * noise
+
+
+def make_merge_graph(n_key, n_cams, seed=0, groups=None, merge_frame=None, n_constraints=1, n_scale_ids=1,
+                     noise=0.0):
+    """Synthetic key-frame graph of a camera-group merge, shaped as MergeCameraGroup::
+    _constructGraphForKeyFrms builds it (reference app/SL_MergeCameraGroup.cpp:907-1035): node
+    k * n_cams + c = camera c at key frame k, the first key frame's nodes fixed; up to the merge frame,
+    edges between the cameras of each group (a ring when a group has more than 2); per camera, edges
+    between successive key frames; n_constraints merge edges between the groups near the merge frame,
+    uncertain scale, scale id = edge index % n_scale_ids.  A constraint edge's t is the true translation
+    divided by the true scale of its id, so with noise = 0 every edge is consistent with the input poses
+    and the solution is the input with those scales.  noise > 0 perturbs every edge measurement.
+    Returns dict(fixed, R, t, id1, id2, eR, et, scale_id, scale_col, n_scale, true_scale)."""
+    rng = np.random.default_rng(seed)
+    if groups is None:
+        h = (n_cams + 1) // 2
+        groups = [list(range(h)), list(range(h, n_cams))]
+    if merge_frame is None:
+        merge_frame = max(1, (2 * n_key) // 3)
+    Rt, tt = _trajectories(rng, n_key, n_cams)
+    node = lambda k, c: k * n_cams + c  # noqa: E731
+    fixed = np.zeros(n_key * n_cams, np.uint8)
+    fixed[:n_cams] = 1
+    id1, id2, eR, et, sid = [], [], [], [], []
+
+    def edge(a, b, R, t, s=-1):
+        R, t = _noisy(rng, R, t, noise)
+        id1.append(a)
+        id2.append(b)
+        eR.append(R)
+        et.append(t)
+        sid.append(s)
+
+    for k in range(n_key):
+        if k <= merge_frame:
+            for g in groups:
+                if len(g) < 2:
+                    continue
+                ring = list(zip(g[:-1], g[1:])) + ([(g[-1], g[0])] if len(g) > 2 else [])
+                for c1, c2 in ring:
+                    edge(node(k, c1), node(k, c2), *_rel(Rt[k, c1], tt[k, c1], Rt[k, c2], tt[k, c2]))
+        if k > 0:
+            for c in range(n_cams):
+                edge(node(k - 1, c), node(k, c), *_rel(Rt[k - 1, c], tt[k - 1, c], Rt[k, c], tt[k, c]))
+    true_scale = 0.5 + rng.uniform(size=n_scale_ids)
+    for q in range(n_constraints):
+        ga, gb = groups[0], groups[-1]
+        c1, c2 = ga[q % len(ga)], gb[(q * 7 + 1) % len(gb)]
+        f1 = merge_frame
+        f2 = max(1, merge_frame - (q % 3))
+        R, t = _rel(Rt[f1, c1], tt[f1, c1], Rt[f2, c2], tt[f2, c2])
+        s = q % n_scale_ids
+        edge(node(f1, c1), node(f2, c2), R, t / true_scale[s], s)
+    sid = np.asarray(sid, np.int32)
+    col, ns = scale_columns(sid)
+    return dict(fixed=fixed, R=Rt.reshape(-1, 3, 3).copy(), t=tt.reshape(-1, 3).copy(),
+                id1=np.asarray(id1, np.int32), id2=np.asarray(id2, np.int32), eR=np.asarray(eR).reshape(-1, 3, 3),
+                et=np.asarray(et).reshape(-1, 3), scale_id=sid, scale_col=col, n_scale=ns,
+                true_scale=true_scale[:ns])
+
+
+def make_pose_graph(n_nodes, seed=0, components=1, fixed_every=0, loops=0, parallel=0, reverse=0,
+                    fixed_pairs=0, n_scale=0, uncertain=0, noise=0.02):
+    """A general pose graph: `components` disjoint chains over n_nodes (each with its first node fixed,
+    and every fixed_every-th when > 0), plus per component `loops` random loop closures, `parallel`
+    duplicated edges, `reverse` edges in the opposite direction, `fixed_pairs` edges between two fixed
+    nodes, and `uncertain` extra edges with scale columns 0 .. n_scale-1 (each column used at least once).
+    Edges are measured from the true poses with `noise`; the fixed nodes are then moved by ~noise.
+    Returns dict(fixed, R, t, id1, id2, eR, et, scale_col, n_scale)."""
+    rng = np.random.default_rng(seed)
+    Rt, tt = _trajectories(rng, n_nodes, 1)
+    Rt, tt = Rt[:, 0], tt[:, 0]
+    bounds = np.linspace(0, n_nodes, components + 1).astype(int)
+    fixed = np.zeros(n_nodes, np.uint8)
+    id1, id2, eR, et, col = [], [], [], [], []
+
+    def edge(a, b, c=-1):
+        R, t = _rel(Rt[a], tt[a], Rt[b], tt[b])
+        s = 1.0
+        if c >= 0:
+            s = 0.5 + 0.25 * c
+            t = t / s
+        R, t = _noisy(rng, R, t, noise)
+        id1.append(a)
+        id2.append(b)
+        eR.append(R)
+        et.append(t)
+        col.append(c)
+
+    n_unc = max(uncertain, n_scale)
+    for q in range(components):
+        a, b = int(bounds[q]), int(bounds[q + 1])
+        if b <= a:
+            continue
+        fixed[a] = 1
+        if fixed_every > 0:
+            fixed[a:b:fixed_every] = 1
+        for k in range(a, b - 1):
+            edge(k, k + 1)
+        n = b - a
+        if n < 3:
+            continue
+        for _ in range(loops):
+            i, j = sorted(rng.choice(n, 2, replace=False) + a)
+            edge(int(i), int(j))
+        for _ in range(parallel):
+            k = int(rng.integers(a, b - 1))
+            edge(k, k + 1)
+        for _ in range(reverse):
+            k = int(rng.integers(a, b - 1))
+            edge(k + 1, k)
+        fx = np.nonzero(fixed[a:b])[0] + a
+        if len(fx) >= 2:
+            for _ in range(fixed_pairs):
+                i, j = rng.choice(fx, 2, replace=False)
+                edge(int(i), int(j))
+        if q == 0:
+            for u in range(n_unc):
+                i, j = rng.choice(n, 2, replace=False) + a
+                if fixed[i] and fixed[j]:
+                    j = a + 1 + (j - a) % (n - 1) if not fixed[a + 1] else i
+                edge(int(i), int(j), u % n_scale if n_scale else -1)
+    R, t = Rt.copy(), tt.copy()
+    for k in np.nonzero(fixed)[0]:
+        R[k] = _rodrigues(rng.normal(size=3) * noise) @ R[k]
+        t[k] += rng.normal(size=3) * noise
+    return dict(fixed=fixed, R=R, t=t, id1=np.asarray(id1, np.int32), id2=np.asarray(id2, np.int32),
+                eR=np.asarray(eR).reshape(-1, 3, 3), et=np.asarray(et).reshape(-1, 3),
+                scale_col=np.asarray(col, np.int32), n_scale=n_scale)

@@ -377,6 +377,38 @@ int cosl_posegraph_spread_chains(int nChains, const int* chainOff, const uint8_t
                                  const double* R, const double* t, const double* eR,
                                  const double* et, double* newR, double* newt, int device);
 
+/* ================= general pose graphs (SURVEY.md 8f-2; the camera-group merge) =================
+ * Replaces, on an ARBITRARY edge set, GlobalPoseGraph::computeNewCameraRotations
+ * (slam/SL_GlobalPoseEstimation.cpp:52-218: least squares, then the nearest rotation of every free node)
+ * together with ::computeNewCameraTranslations4 (:361-525: translations with shared unknown scales),
+ * as MergeCameraGroup::recomputeKeyCamPoses calls them (app/SL_MergeCameraGroup.cpp:1083-1086) on the
+ * graph _constructGraphForKeyFrms builds (:907-1035).  Both systems are solved by ONE call; the
+ * translation system uses the edges' R, not the new rotations, as the reference's does.
+ *   fixed[nNodes]          1 = fixed node (CamPoseNode::fixed): copied to newR / newt (:205-216, :505-513)
+ *   R[9n], t[3n]           node poses, row-major (CamPoseNode::R, ::t)
+ *   id1/id2[nEdges]        edge e runs from node id1[e] to node id2[e] (CamPoseEdge::id1, ::id2)
+ *   eR[9e], et[3e]         rigid transform of edge e (CamPoseEdge::R, ::t)
+ *   scaleCol[nEdges]       scale column of edge e: t_j - R_e t_i = s[scaleCol[e]] et_e; -1 = known
+ *                          scale (t_j - R_e t_i = et_e).  NULL: every scale is known.  The shim maps
+ *                          CamPoseEdge::scaleId to columns as :383-403 does.
+ *   newR[9n], newt[3n]     out: CamPoseNode::newR, ::newt
+ *   scale[nScale]          out: the solved scales (CamPoseEdge::s of the uncertain edges, :515-522)
+ * Edges joining two fixed nodes give no rows (:59, :368); parallel edges and edges in both directions
+ * are allowed; a disjoint union of graphs is one call.  Never throws.  Returns
+ *   COSL_E_INVALID  a node or scale index out of range, a self-loop, a scale column without a row, or a
+ *                   connected component with free nodes but no fixed node (the message names one such
+ *                   node; the reference's system is rank deficient there);
+ *   COSL_E_NUMERIC  a non-positive pivot of the normal equations or a non-finite result;
+ *   COSL_E_NOMEM / COSL_E_CUDA  allocation failure / no usable device.
+ * A graph without free nodes is answered on the host (copies). */
+int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const double* R, const double* t,
+                         int nEdges, const int* id1, const int* id2, const double* eR, const double* et,
+                         const int* scaleCol, int nScale, double* newR, double* newt, double* scale,
+                         int device);
+/* Diagnostic: host time (validation, numbering, planning, CSR lists; ms) of the calling thread's last
+ * cosl_posegraph_solve call. */
+double cosl_posegraph_last_host_ms(void);
+
 #ifdef __cplusplus
 }
 #endif
