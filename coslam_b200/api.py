@@ -34,6 +34,7 @@ def _load():
     L.cosl_klt_config_default.argtypes = [C.POINTER(KltConfig)]
     L.cosl_klt_create.argtypes = [C.POINTER(KltConfig)] + [ci] * 8 + [C.POINTER(vp)]
     L.cosl_klt_group_create.argtypes = [C.POINTER(KltConfig)] + [ci] * 9 + [C.POINTER(vp)]
+    L.cosl_klt_group_create_sizes.argtypes = [C.POINTER(KltConfig), ci, vp, vp] + [ci] * 6 + [C.POINTER(vp)]
     L.cosl_klt_destroy.argtypes = [vp]
     L.cosl_klt_detect.argtypes = [vp, vp, C.c_size_t, ci, vp, vp, pint]
     L.cosl_klt_redetect.argtypes = [vp, vp, C.c_size_t, vp, pint]
@@ -203,15 +204,28 @@ class KltTracker:
 
 
 class KltGroup:
-    """C cameras of equal geometry, one launch per kernel for the whole group (batched
-    GPUKLT::first / GPUKLT::next)."""
+    """C cameras, one launch per kernel for the whole group (batched GPUKLT::first / GPUKLT::next).
+
+    width, height: one size for every camera (cosl_klt_group_create), or one per camera
+    (sequences of n_cams entries: cosl_klt_group_create_sizes).  self.sizes lists each camera's
+    (width, height); self.W, self.H are the largest width and height."""
 
     def __init__(self, cfg, n_cams, width, height, n_levels, feat_w, feat_h, device=0):
-        self.cfg, self.C, self.W, self.H, self.nl = cfg, n_cams, width, height, n_levels
+        self.mixed = not (np.isscalar(width) and np.isscalar(height))
+        ws = [int(v) for v in np.broadcast_to(width, (n_cams,))]
+        hs = [int(v) for v in np.broadcast_to(height, (n_cams,))]
+        self.cfg, self.C, self.nl = cfg, n_cams, n_levels
+        self.sizes = list(zip(ws, hs))
+        self.W, self.H = max(ws), max(hs)
         self.fw, self.fh, self.F = feat_w, feat_h, feat_w * feat_h
         h = C.c_void_p()
-        _ck(LIB.cosl_klt_group_create(C.byref(cfg), n_cams, width, height, n_levels, feat_w,
-                                      feat_h, 0, 0, device, C.byref(h)))
+        if self.mixed:
+            wa, ha = np.asarray(ws, np.int32), np.asarray(hs, np.int32)
+            _ck(LIB.cosl_klt_group_create_sizes(C.byref(cfg), n_cams, _ptr(wa), _ptr(ha), n_levels,
+                                                feat_w, feat_h, 0, 0, device, C.byref(h)))
+        else:
+            _ck(LIB.cosl_klt_group_create(C.byref(cfg), n_cams, width, height, n_levels, feat_w,
+                                          feat_h, 0, 0, device, C.byref(h)))
         self.h = h
         self.feats = np.zeros((n_cams, self.F), FEAT_DTYPE)
         self.counts = np.zeros(n_cams, np.int32)
@@ -226,10 +240,19 @@ class KltGroup:
         self.close()
 
     def _imgs(self, imgs):
+        """(pointer array, pitch).  Camera c's frame is (H_c, W_c) uint8.  One row pitch shared by
+        every frame is passed as is; on a group made with per-camera sizes, frames whose rows are
+        each their own width apart (C-contiguous) pass pitch 0."""
         assert len(imgs) == self.C
-        pitch = imgs[0].strides[0]
-        for im in imgs:
-            assert im.dtype == np.uint8 and im.strides[0] == pitch and im.shape == (self.H, self.W)
+        for im, (w, h) in zip(imgs, self.sizes):
+            assert im.dtype == np.uint8 and im.shape == (h, w) and im.strides[1] == 1
+        pitches = {im.strides[0] for im in imgs}
+        if len(pitches) == 1:
+            pitch = pitches.pop()
+        else:
+            assert self.mixed and all(im.strides[0] == w for im, (w, _) in zip(imgs, self.sizes)), \
+                "frames of different pitches: give each camera's frame rows of its own width"
+            pitch = 0
         return (C.c_void_p * self.C)(*[im.ctypes.data for im in imgs]), pitch
 
     def _per_cam(self, lists):
@@ -334,9 +357,15 @@ class KltGroup:
         return out
 
     def pyramid(self, cam, which, level):
-        w, h = self.W >> level, self.H >> level
+        w, h = self.sizes[cam][0] >> level, self.sizes[cam][1] >> level
         out = np.empty((h, w, 3), np.float32)
         _ck(LIB.cosl_klt_debug_pyramid(self.h, cam, which, level, _ptr(out), None, None))
+        return out
+
+    def cornerness(self, cam):
+        w, h = self.sizes[cam]
+        out = np.empty((h, w), np.float32)
+        _ck(LIB.cosl_klt_debug_cornerness(self.h, cam, _ptr(out)))
         return out
 
 

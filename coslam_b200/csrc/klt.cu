@@ -19,7 +19,13 @@ using namespace coslam;
 
 struct cosl_klt {
   cosl_klt_config cfg;
+  // W x H: the group's largest geometry (maximum width, maximum height); every buffer slice is laid
+  // out at it and camera c uses the top-left hcam[c].W x hcam[c].H of its slice (klt_kernels.cuh)
   int C = 1, W = 0, H = 0, L = 0, fw = 0, fh = 0, F = 0, plCap = 0, device = 0;
+  bool mixed = false;        // the cameras differ in size: kernels read the per-camera table
+  bool pitchZeroOK = false;  // made by cosl_klt_group_create_sizes: pitch 0 = each camera's own width
+  KltCam hcam[64];           // per camera: extent and detector window (camera 0's: the uniform case)
+  KltCam* d_cams = nullptr;  // device copy of hcam, read by the kernels of a mixed group
   int levelSkip = 1, halfWidth = 3;
   float trackMargin = 4.f, conv = 0.1f, ssd = 5000.f, detectMargin = 10.f;
   cudaStream_t stream = nullptr;
@@ -79,7 +85,6 @@ struct cosl_klt {
   bool fusedOK = false;
   int fusedBlocks = 0;
   int numSM = 132;
-  int detXlo = 0, detXhi = -1, detYlo = 0, detYhi = -1;  // detector window in pixels
   int verBase = 0;
   // TMA descriptors of every pyramid level of both buffers: [buffer][level], load box (source of
   // level + 1) and store box (destination of level - 1 -> level); klt_pyr_tma.cuh
@@ -90,11 +95,13 @@ struct cosl_klt {
 
 namespace {
 
+// Detector window of every camera, then hcam -> d_cams on the group's stream (the margin can change
+// between frames).
 // Detector window (klt_detector_pass2.cg: the pixel centre (i + 0.5) / n must lie inside
 // [margin / n, 1 - margin / n]); evaluated with the fp32 expressions the oracle's margin mask
 // evaluates per pixel (sx = (x + 0.5f) / W against margin / W and 1 - margin / W,
 // oracle/klt_oracle.cpp), so the integer bounds select exactly the same pixels.
-static void update_detect_window(cosl_klt* g) {
+static int update_cameras(cosl_klt* g) {
   const float mg = g->detectMargin;
   auto bounds = [](int n, float lo, float hi, int& i0, int& i1) {
     const float nf = (float)n;
@@ -108,23 +115,33 @@ static void update_detect_window(cosl_klt* g) {
       }
     }
   };
-  const float Wf = (float)g->W, Hf = (float)g->H;
-  bounds(g->W, mg / Wf, 1.0f - mg / Wf, g->detXlo, g->detXhi);
-  bounds(g->H, mg / Hf, 1.0f - mg / Hf, g->detYlo, g->detYhi);
+  for (int c = 0; c < g->C; ++c) {
+    KltCam& K = g->hcam[c];
+    const float Wf = (float)K.W, Hf = (float)K.H;
+    bounds(K.W, mg / Wf, 1.0f - mg / Wf, K.ixlo, K.ixhi);
+    bounds(K.H, mg / Hf, 1.0f - mg / Hf, K.iylo, K.iyhi);
+  }
+  // pageable source: the copy is staged before the call returns, so hcam may change again
+  COSL_CUDA(cudaMemcpyAsync(g->d_cams, g->hcam, sizeof(KltCam) * g->C, cudaMemcpyHostToDevice, g->stream));
+  return COSL_OK;
 }
 
 // the gain tracker's instantiation for this group's window (compile-time width when it is the live one)
-using FusedFn = void (*)(const float4*, const float4*, long long, KltLevels, int, const float4*, float4*,
-                         unsigned long long*, const int*, float4*, int, KltTrackParams, KltTrackParams, int,
-                         KltTail);
-using PassFn = void (*)(const float4*, const float4*, long long, long long, int, int, const float4*,
-                        const float4*, float4*, const int*, float, float, KltTrackParams, int);
+using FusedFn = void (*)(const float4*, const float4*, long long, KltLevels, const KltCam*, int, const float4*,
+                         float4*, unsigned long long*, const int*, float4*, int, KltTrackParams, KltTrackParams,
+                         int, KltTail);
+using PassFn = void (*)(const float4*, const float4*, long long, long long, int, int, const KltCam*,
+                        const float4*, const float4*, float4*, const int*, KltTrackParams, int);
 static FusedFn fused_kernel(const cosl_klt* g) {
-  return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE> : klt_gain_fused<0>;
+  if (g->mixed) return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE, true> : klt_gain_fused<0, true>;
+  return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE, false> : klt_gain_fused<0, false>;
 }
 static PassFn pass_kernel(const cosl_klt* g) {
-  return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE> : klt_gain_pass<0>;
+  if (g->mixed) return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE, true> : klt_gain_pass<0, true>;
+  return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE, false> : klt_gain_pass<0, false>;
 }
+// the instantiation of a kernel for this group's sizes (klt_kernels.cuh, KltCam)
+#define KLT_SIZED(g, ...) ((g)->mixed ? __VA_ARGS__<true> : __VA_ARGS__<false>)
 
 int alloc_group(cosl_klt* g) {
   const int C = g->C, W = g->W, H = g->H, F = g->F;
@@ -144,13 +161,15 @@ int alloc_group(cosl_klt* g) {
   g->pyrStride = off;
   g->imgPitch = ((size_t)W + 15) & ~(size_t)15;
   g->imgStride = g->imgPitch * H;
+  COSL_CUDA(cudaMalloc(&g->d_cams, sizeof(KltCam) * C));
   // candidate capacity: a strict (2r+1)^2 maximum admits at most one survivor per (r+1)^2 pixels
+  // (of the largest camera, which bounds every camera's count)
   const int r = std::max(1, g->cfg.minDistance);
   long long maxCand = ((long long)(W + r) / (r + 1) + 1) * ((long long)(H + r) / (r + 1) + 1);
   int cap = 1024;
   while (cap < maxCand) cap <<= 1;
   g->candCap = cap;
-  g->smemKeys = std::min(cap, 16384);
+  g->smemKeys = std::min(cap, KLT_MAX_SMEM_KEYS);
   COSL_CUDA(cudaMalloc(&g->d_img, g->imgStride * C));
   std::fill(&g->lv0Stored[0][0], &g->lv0Stored[0][0] + 2 * 64, true);
   for (int b = 0; b < 2; ++b) {
@@ -261,10 +280,11 @@ int alloc_group(cosl_klt* g) {
                            g->lvW[l], g->lvH[l]);
       }
   }
-  // dynamic shared memory opt-ins
-  COSL_CUDA(cudaFuncSetAttribute(klt_select_refill, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 g->smemKeys * (int)sizeof(unsigned long long)));
-  update_detect_window(g);
+  // dynamic shared memory opt-in: the attribute belongs to the kernel, not to this group, so it is
+  // the largest any group uses (a group created later must not lower it below an earlier one's)
+  COSL_CUDA(cudaFuncSetAttribute(KLT_SIZED(g, klt_select_refill), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 KLT_MAX_SMEM_KEYS * (int)sizeof(unsigned long long)));
+  COSL_TRY(update_cameras(g));
   g->secPyr = g->timer.section("klt_pyramid");
   g->secTrack = g->timer.section("klt_track");
   g->secDetect = g->timer.section("klt_detect");
@@ -279,6 +299,7 @@ void free_group(cosl_klt* g) {
   if (g->stream) cudaStreamSynchronize(g->stream);
   g->timer.destroy();
   cudaFree(g->d_img);
+  cudaFree(g->d_cams);
   cudaFree(g->d_pyr[0]);
   cudaFree(g->d_pyr[1]);
   cudaFree(g->d_corn);
@@ -319,26 +340,27 @@ void free_group(cosl_klt* g) {
 
 // ---- stages (all asynchronous on g->stream) ----
 
+// camera c's image: hcam[c].W x hcam[c].H bytes, rows `pitch` bytes apart (0: hcam[c].W, pitch_ok)
 int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind kind) {
   if (kind == cudaMemcpyHostToDevice && g->C > 1) {
     // the previous frame's front pass must have consumed d_img before it is overwritten
     if (g->frontRecorded) COSL_CUDA(cudaStreamWaitEvent(g->copyStream, g->evFront, 0));
-    const bool flat = (pitch == (size_t)g->W) && (g->imgPitch == (size_t)g->W);  // one contiguous block
     for (int c = 0; c < g->C; ++c) {
-      if (flat)
-        COSL_CUDA(cudaMemcpyAsync(g->d_img + (size_t)c * g->imgStride, imgs[c], (size_t)g->W * g->H,
-                                  kind, g->copyStream));
+      const size_t w = (size_t)g->hcam[c].W, sp = pitch ? pitch : w;
+      if (sp == w && g->imgPitch == w)  // one contiguous block
+        COSL_CUDA(cudaMemcpyAsync(g->d_img + (size_t)c * g->imgStride, imgs[c], w * g->hcam[c].H, kind,
+                                  g->copyStream));
       else
-        COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c],
-                                    pitch, g->W, g->H, kind, g->copyStream));
+        COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c], sp, w,
+                                    g->hcam[c].H, kind, g->copyStream));
       COSL_CUDA(cudaEventRecord(g->evImg[c], g->copyStream));
     }
     g->imgPerCam = true;
     return COSL_OK;
   }
   for (int c = 0; c < g->C; ++c)
-    COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c], pitch,
-                                g->W, g->H, kind, g->stream));
+    COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c],
+                                pitch ? pitch : (size_t)g->hcam[c].W, g->hcam[c].W, g->hcam[c].H, kind, g->stream));
   return COSL_OK;
 }
 
@@ -346,15 +368,12 @@ int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMem
 static void launch_prefilter(cosl_klt* g, cudaStream_t st) {
   const int pr = std::min(std::max(1, g->cfg.minDistance), 3);
   dim3 gp(div_up(g->W, 32 - 2 * pr), div_up(g->H, 8 * NP_ROWS), g->C);
-  if (pr == 3)
-    COSL_LAUNCH(klt_nm_prefilter<3>, gp, 256, 0, st, g->d_corn, g->W, g->H, g->d_prelim,
-                g->prelimCap, g->d_counters);
-  else if (pr == 2)
-    COSL_LAUNCH(klt_nm_prefilter<2>, gp, 256, 0, st, g->d_corn, g->W, g->H, g->d_prelim,
-                g->prelimCap, g->d_counters);
-  else
-    COSL_LAUNCH(klt_nm_prefilter<1>, gp, 256, 0, st, g->d_corn, g->W, g->H, g->d_prelim,
-                g->prelimCap, g->d_counters);
+  const long long cs = (long long)g->W * g->H;
+  const auto kern = pr == 3 ? (g->mixed ? klt_nm_prefilter<3, true> : klt_nm_prefilter<3, false>)
+                  : pr == 2 ? (g->mixed ? klt_nm_prefilter<2, true> : klt_nm_prefilter<2, false>)
+                            : (g->mixed ? klt_nm_prefilter<1, true> : klt_nm_prefilter<1, false>);
+  COSL_LAUNCH(kern, gp, 256, 0, st, g->d_corn, g->W, cs, g->d_cams, g->W, g->H, g->d_prelim, g->prelimCap,
+              g->d_counters);
 }
 
 // The tracker's level list: L-1, L-1-levelSkip, ... down to >= 0.  scaled: the 2x2 tracker's
@@ -405,18 +424,23 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   fp.pyrStride = g->pyrStride;
   fp.lv1Off = g->L > 1 ? g->lvOff[1] : 0;
   fp.corn = g->d_corn;
+  fp.cornStride = (long long)g->W * g->H;
   fp.W = g->W;
   fp.H = g->H;
   fp.nStrips = div_up(g->W, FS_SW);
   fp.nChunks = div_up(g->H, FS_R);
   fp.wantL1 = g->L > 1 ? 1 : 0;
-  const auto front = p.storeL0 ? klt_front<true> : klt_front<false>;
+  const auto front = p.storeL0 ? (g->mixed ? klt_front<true, true> : klt_front<true, false>)
+                                : (g->mixed ? klt_front<false, true> : klt_front<false, false>);
   fp.wantCorn = p.wantCorn ? 1 : 0;
   fp.minC = g->cfg.minCornerness;
-  fp.ixlo = g->detXlo;
-  fp.ixhi = g->detXhi;
-  fp.iylo = g->detYlo;
-  fp.iyhi = g->detYhi;
+  fp.ixlo = g->hcam[0].ixlo;
+  fp.ixhi = g->hcam[0].ixhi;
+  fp.iylo = g->hcam[0].iylo;
+  fp.iyhi = g->hcam[0].iyhi;
+  fp.cams = g->d_cams;
+  // the grid covers the largest camera; a smaller camera's surplus warps exit
+  const int nWarps = fp.nStrips * fp.nChunks;
   if (g->imgPerCam) {
     // two half-groups: the front pass of the first half overlaps the upload of the second (a launch
     // per camera would leave the SMs mostly empty: 500 warps per 1280x720 camera)
@@ -426,12 +450,12 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
       const int nc = std::min(half, g->C - c0);
       COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evImg[c0 + nc - 1], 0));
       fp.camBase = c0;
-      dim3 g1(div_up(fp.nStrips * fp.nChunks, FS_WARPS), nc);
+      dim3 g1(div_up(nWarps, FS_WARPS), nc);
       COSL_LAUNCH(front, g1, 32 * FS_WARPS, 0, g->stream, fp);
     }
   } else {
     fp.camBase = 0;
-    dim3 g0(div_up(fp.nStrips * fp.nChunks, FS_WARPS), g->C);
+    dim3 g0(div_up(nWarps, FS_WARPS), g->C);
     COSL_LAUNCH(front, g0, 32 * FS_WARPS, 0, g->stream, fp);
   }
   COSL_CUDA(cudaEventRecord(g->evFront, g->stream));
@@ -444,21 +468,24 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh)
   for (int l = 2; l < g->L; ++l) {
     dim3 gl(div_up(g->lvW[l], PT_TW), div_up(g->lvH[l], PT_TH), g->C);
-    COSL_LAUNCH(klt_pyr_down_tma, gl, 256, 0, g->stream, g->tmLoad[g->cur][l - 1], g->tmStore[g->cur][l],
-                g->lvW[l - 1], g->lvH[l - 1]);
+    COSL_LAUNCH(KLT_SIZED(g, klt_pyr_down_tma), gl, 256, 0, g->stream, g->tmLoad[g->cur][l - 1],
+                g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], g->d_cams, l);
   }
   g->timer.end(g->stream);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
 
+// W, H, vr*: camera 0's, which are every camera's unless the group is mixed (klt_vr_lo / _hi)
 KltTrackParams track_params(const cosl_klt* g, bool strict) {
   KltTrackParams P;
-  P.W = g->W;
-  P.H = g->H;
+  P.W = g->hcam[0].W;
+  P.H = g->hcam[0].H;
   P.F = g->F;
   P.halfWidth = g->halfWidth;
-  const float Wf = (float)g->W, Hf = (float)g->H, m = g->trackMargin;
+  P.strict = strict ? 1 : 0;
+  P.margin = g->trackMargin;
+  const float Wf = (float)P.W, Hf = (float)P.H, m = g->trackMargin;
   if (strict) {
     P.sqrConv = g->conv * g->conv;
     P.ssdThr = g->ssd;
@@ -501,11 +528,11 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
     KltTrackParams Plax = track_params(g, false), Pstrict = track_params(g, true);
     int verBase = g->verBase;
     // the feature table and, when this frame produced a cornerness map, its suppression marks
-    KltTail tail = {g->d_feat, g->d_counters, g->d_corn, g->W, g->H, p.wantCorn ? 1 : 0};
-    void* args[] = {(void*)&P0,          (void*)&P1,     (void*)&pyrStride, (void*)&LV,
-                    (void*)&nIter,       (void*)&g->d_src, (void*)&g->d_state, (void*)&g->d_ver,
-                    (void*)&g->d_waitset, (void*)&g->d_res, (void*)&C,        (void*)&Plax,
-                    (void*)&Pstrict,     (void*)&verBase, (void*)&tail};
+    KltTail tail = {g->d_feat, g->d_counters, g->d_corn, (long long)g->W * g->H, g->W, p.wantCorn ? 1 : 0};
+    void* args[] = {(void*)&P0,          (void*)&P1,       (void*)&pyrStride,  (void*)&LV,
+                    (void*)&g->d_cams,   (void*)&nIter,    (void*)&g->d_src,   (void*)&g->d_state,
+                    (void*)&g->d_ver,    (void*)&g->d_waitset, (void*)&g->d_res, (void*)&C,
+                    (void*)&Plax,        (void*)&Pstrict,  (void*)&verBase,    (void*)&tail};
     COSL_CUDA(cudaLaunchCooperativeKernel((const void*)fused_kernel(g), dim3(g->fusedBlocks),
                                           dim3(KLT_FUSED_THREADS), args, 0, g->stream));
     g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -547,8 +574,6 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
     int which = 0, first = 1;
     bool strict = false;
     for (int li = 0; li < LV.n; ++li) {
-      const int w = LV.w[li], h = LV.h[li];
-      const float dsx = 1.0f / (float)w, dsy = 1.0f / (float)h;
       for (int iter = 1; iter <= g->cfg.nIterations; ++iter) {
         if (iter == 1)
           strict = false;
@@ -556,9 +581,8 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
           strict = true;
         const bool last = (li == LV.n - 1) && (iter == g->cfg.nIterations);
         float4* out = last ? g->d_res : bufs[which];
-        COSL_LAUNCH(pass, gridHalf, 256, 0, g->stream, P0, P1, g->pyrStride,
-                    LV.off[li], w, h, g->d_src, in, out, g->d_nbr, dsx, dsy,
-                    track_params(g, strict), first);
+        COSL_LAUNCH(pass, gridHalf, 256, 0, g->stream, P0, P1, g->pyrStride, LV.off[li], LV.level[li],
+                    LV.w[li], g->d_cams, g->d_src, in, out, g->d_nbr, track_params(g, strict), first);
         in = out;
         which ^= 1;
         first = 0;
@@ -571,11 +595,11 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
                        !(g->cfg.compat & COSL_KLT_PASS_KERNELS);
     if (tiled) {
       dim3 gt(div_up(g->F, 16), g->C);
-      COSL_LAUNCH(klt_track_2x2_tiled, gt, 128, 0, g->stream, P0, P1, g->pyrStride, LV, g->d_src,
-                  g->d_res, track_params(g, true), nIter);
+      COSL_LAUNCH(KLT_SIZED(g, klt_track_2x2_tiled), gt, 128, 0, g->stream, P0, P1, g->pyrStride, LV, g->d_cams,
+                  g->d_src, g->d_res, track_params(g, true), nIter);
     } else {
-      COSL_LAUNCH(klt_track_2x2, grid, wpb * 32, 0, g->stream, P0, P1, g->pyrStride, LV, g->d_src,
-                  g->d_res, track_params(g, true), nIter);
+      COSL_LAUNCH(KLT_SIZED(g, klt_track_2x2), grid, wpb * 32, 0, g->stream, P0, P1, g->pyrStride, LV, g->d_cams,
+                  g->d_src, g->d_res, track_params(g, true), nIter);
     }
   }
   g->timer.end(g->stream);
@@ -588,14 +612,15 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
 // (present = the external points of upload_present, maxPresent = the longest list), 1: redetect.
 int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
   g->timer.begin(g->secDetect, g->stream);
+  const long long cs = (long long)g->W * g->H;
   if (mode == 1 && !p.trackerTail) {
     dim3 gs(div_up(g->F, 256), g->C);
-    COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F, g->d_corn,
-                g->W, g->H);
+    COSL_LAUNCH(KLT_SIZED(g, klt_suppress), gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F,
+                g->d_corn, g->W, cs, g->d_cams, g->W, g->H);
   } else if (mode == 0 && maxPresent > 0) {
     dim3 gs(div_up(maxPresent, 256), g->C);
-    COSL_LAUNCH(klt_suppress, gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F, g->d_corn,
-                g->W, g->H);
+    COSL_LAUNCH(KLT_SIZED(g, klt_suppress), gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F,
+                g->d_corn, g->W, cs, g->d_cams, g->W, g->H);
   }
   const int r = std::max(1, g->cfg.minDistance);
   if (p.earlyPrefilter)
@@ -603,14 +628,14 @@ int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
   else
     launch_prefilter(g, g->stream);
   dim3 gv(2 * g->numSM, g->C);
-  COSL_LAUNCH(klt_nm_verify, gv, 256, 0, g->stream, g->d_corn, g->W, g->H, r, g->d_prelim,
-              g->prelimCap, g->d_cand, g->candCap, g->d_counters);
+  COSL_LAUNCH(KLT_SIZED(g, klt_nm_verify), gv, 256, 0, g->stream, g->d_corn, g->W, cs, g->d_cams, g->W, g->H, r,
+              g->d_prelim, g->prelimCap, g->d_cand, g->candCap, g->d_counters);
   g->timer.end(g->stream);
   g->timer.begin(g->secSelect, g->stream);
-  COSL_LAUNCH(klt_select_refill, g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
+  COSL_LAUNCH(KLT_SIZED(g, klt_select_refill), g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
               g->d_cand, g->candCap, g->plCap, g->d_counters, g->d_feat, g->d_dst,
               p.foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
-              maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, g->W, g->H, mode,
+              maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, g->d_cams, g->W, g->H, mode,
               g->cfg.trackWithGain ? 1 : 0, g->smemKeys, (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
   g->timer.end(g->stream);
   COSL_CUDA(cudaGetLastError());
@@ -792,16 +817,23 @@ void cosl_klt_config_default(cosl_klt_config* c) {
   c->compat = COSL_KLT_COMPAT_ITER5;
 }
 
-int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int height,
-                          int nLevels, int featW, int featH, int plW, int plH, int device,
-                          cosl_klt** out) {
-  if (!cfg || !out) return set_error(COSL_E_INVALID, "null argument");
+int cosl_klt_group_create_sizes(const cosl_klt_config* cfg, int nCams, const int* widths,
+                                const int* heights, int nLevels, int featW, int featH, int plW, int plH,
+                                int device, cosl_klt** out) {
+  if (!cfg || !out || !widths || !heights) return set_error(COSL_E_INVALID, "null argument");
   *out = nullptr;
-  if (nCams < 1 || nCams > 64 || width < 16 || height < 16 || width > 65535 || height > 65535 ||
-      nLevels < 1 || nLevels > 8 || featW < 1 || featH < 1 || (width >> (nLevels - 1)) < 2 ||
-      (height >> (nLevels - 1)) < 2)
-    return set_error(COSL_E_INVALID, "bad tracker geometry %dx%d L=%d feat=%dx%d C=%d", width,
-                     height, nLevels, featW, featH, nCams);
+  if (nCams < 1 || nCams > 64 || nLevels < 1 || nLevels > 8 || featW < 1 || featH < 1)
+    return set_error(COSL_E_INVALID, "bad tracker geometry L=%d feat=%dx%d C=%d", nLevels, featW, featH, nCams);
+  int maxW = 0, maxH = 0;
+  for (int c = 0; c < nCams; ++c) {
+    const int width = widths[c], height = heights[c];
+    if (width < 16 || height < 16 || width > 65535 || height > 65535 || (width >> (nLevels - 1)) < 2 ||
+        (height >> (nLevels - 1)) < 2)
+      return set_error(COSL_E_INVALID, "bad tracker geometry of camera %d: %dx%d L=%d", c, width, height,
+                       nLevels);
+    maxW = std::max(maxW, width);
+    maxH = std::max(maxH, height);
+  }
   if (cfg->windowWidth < 1 || cfg->windowWidth > 31 || cfg->minDistance < 1 ||
       cfg->minDistance > 32 || cfg->nIterations < 1)
     return set_error(COSL_E_INVALID, "bad tracker config");
@@ -814,8 +846,13 @@ int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int 
   g->cfg = *cfg;
   g->cfg.nLevels = nLevels;
   g->C = nCams;
-  g->W = width;
-  g->H = height;
+  g->W = maxW;
+  g->H = maxH;
+  for (int c = 0; c < nCams; ++c) {
+    g->hcam[c].W = widths[c];
+    g->hcam[c].H = heights[c];
+    g->mixed = g->mixed || widths[c] != widths[0] || heights[c] != heights[0];
+  }
   g->L = nLevels;
   g->fw = featW;
   g->fh = featH;
@@ -824,6 +861,7 @@ int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int 
   if (plH <= 0) plH = 2 * featH;
   g->plCap = plW * plH;
   g->device = device;
+  g->pitchZeroOK = true;
   g->levelSkip = cfg->levelSkip > 0 ? cfg->levelSkip : (nLevels - 1);
   if (g->levelSkip < 1) g->levelSkip = 1;
   g->halfWidth = cfg->windowWidth / 2;
@@ -837,6 +875,22 @@ int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int 
     return rc;
   }
   *out = g;
+  return COSL_OK;
+}
+
+int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int height,
+                          int nLevels, int featW, int featH, int plW, int plH, int device,
+                          cosl_klt** out) {
+  if (!out) return set_error(COSL_E_INVALID, "null argument");
+  *out = nullptr;
+  if (nCams < 1 || nCams > 64)
+    return set_error(COSL_E_INVALID, "bad tracker geometry %dx%d L=%d feat=%dx%d C=%d", width, height, nLevels,
+                     featW, featH, nCams);
+  int widths[64], heights[64];
+  std::fill(widths, widths + nCams, width);
+  std::fill(heights, heights + nCams, height);
+  COSL_TRY(cosl_klt_group_create_sizes(cfg, nCams, widths, heights, nLevels, featW, featH, plW, plH, device, out));
+  (*out)->pitchZeroOK = false;  // the images of an equal-size group are always given a pitch
   return COSL_OK;
 }
 
@@ -854,6 +908,10 @@ int cosl_klt_destroy(cosl_klt* h) {
   if (!(h)) return set_error(COSL_E_INVALID, "null tracker handle"); \
   COSL_CUDA(cudaSetDevice((h)->device));
 
+// Row pitch of the images a call takes: at least the widest camera's width, or 0 on a group made with
+// cosl_klt_group_create_sizes (camera c's rows are its own width apart)
+static bool pitch_ok(const cosl_klt* g, size_t pitch) { return pitch ? pitch >= (size_t)g->W : g->pitchZeroOK; }
+
 #define KLT_SINGLE(h) \
   KLT_ENTER(h)        \
   if ((h)->C != 1) return set_error(COSL_E_STATE, "single-camera call on a %d-camera group", (h)->C);
@@ -862,7 +920,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
                     const float* present3, cosl_klt_feature* dest, int* nDetected) {
   KLT_SINGLE(h)
   if (!img || !dest || !nDetected || nPresent < 0 || nPresent > h->F || (nPresent && !present3) ||
-      pitch < (size_t)h->W)
+      !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_detect: bad argument");
   int maxPresent = 0;
   COSL_TRY(upload_present(h, &nPresent, &present3, &maxPresent));
@@ -877,7 +935,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
 int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_feature* dest,
                       int* nNewFeatures) {
   KLT_SINGLE(h)
-  if (!img || !dest || !nNewFeatures || pitch < (size_t)h->W)
+  if (!img || !dest || !nNewFeatures || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_redetect: bad argument");
   const uint8_t* imgs[1] = {img};
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
@@ -890,7 +948,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
 int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_feature* dest,
                    int* nPresent) {
   KLT_SINGLE(h)
-  if (!img || !dest || !nPresent || pitch < (size_t)h->W)
+  if (!img || !dest || !nPresent || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_track: bad argument");
   const uint8_t* imgs[1] = {img};
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
@@ -919,8 +977,7 @@ int cosl_klt_set_margin(cosl_klt* h, float m) {  // tracker AND detector (v3d_gp
   KLT_ENTER(h)
   h->trackMargin = m;
   h->detectMargin = m;
-  update_detect_window(h);
-  return COSL_OK;
+  return update_cameras(h);
 }
 int cosl_klt_set_conv(cosl_klt* h, float t) {
   KLT_ENTER(h)
@@ -952,7 +1009,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
 int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                          cosl_klt_feature* const* dest, int* nDetected) {
   KLT_ENTER(h)
-  if (!imgs || pitch < (size_t)h->W) return set_error(COSL_E_INVALID, "group_first: bad argument");
+  if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_first: bad argument");
   return group_first(h, imgs, pitch, nullptr, nullptr, dest, nDetected);
 }
 
@@ -961,7 +1018,7 @@ int cosl_klt_group_first_present(cosl_klt* h, const uint8_t* const* imgs, size_t
                                  cosl_klt_feature* const* dest, int* nDetected) {
   KLT_ENTER(h)
   KLT_NOT_IN_FLIGHT(h, "group_first_present")
-  if (!imgs || pitch < (size_t)h->W || !nPresent)
+  if (!imgs || !pitch_ok(h, pitch) || !nPresent)
     return set_error(COSL_E_INVALID, "group_first_present: bad argument");
   for (int c = 0; c < h->C; ++c)
     if (nPresent[c] < 0 || nPresent[c] > h->F || (nPresent[c] > 0 && (!present3 || !present3[c])))
@@ -992,7 +1049,7 @@ int cosl_klt_group_advance_cams(cosl_klt* h, const uint8_t* cams) {
 int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                         cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
-  if (!imgs || pitch < (size_t)h->W) return set_error(COSL_E_INVALID, "group_next: bad argument");
+  if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
   COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(run_frame(h, FRAME_REDETECT, 0, true));
   COSL_TRY(fetch_results(h));
@@ -1002,7 +1059,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
 
 int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pitch) {
   KLT_ENTER(h)
-  if (!dimgs || pitch < (size_t)h->W)
+  if (!dimgs || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "group_next_dev: bad argument");
   COSL_TRY(upload_images(h, dimgs, pitch, cudaMemcpyDeviceToDevice));
   return run_frame(h, FRAME_REDETECT, 0, true);
@@ -1022,7 +1079,7 @@ int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) 
 // pass, which is the last reader of the image buffer).
 int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch) {
   KLT_ENTER(h)
-  if (!imgs || pitch < (size_t)h->W) return set_error(COSL_E_INVALID, "group_submit: bad argument");
+  if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_submit: bad argument");
   if (h->nInFlight >= 2) return set_error(COSL_E_STATE, "group_submit: two frames in flight, collect one first");
   const int slot = (int)(h->subSeq & 1u);
   if (!h->h_featQ[slot]) {
@@ -1065,7 +1122,7 @@ int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* ou
   KLT_ENTER(h)
   if (cam < 0 || cam >= h->C || level < 0 || level >= h->L)
     return set_error(COSL_E_INVALID, "debug_pyramid: bad argument");
-  const int lw = h->lvW[level], lh = h->lvH[level];
+  const int lw = h->hcam[cam].W >> level, lh = h->hcam[cam].H >> level;
   if (w) *w = lw;
   if (ht) *ht = lh;
   if (!out3) return COSL_OK;
@@ -1077,7 +1134,8 @@ int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* ou
   std::vector<float4> tmp((size_t)lw * lh);
   const float4* src = h->d_pyr[buf] + (size_t)cam * h->pyrStride + h->lvOff[level];
   COSL_CUDA(cudaStreamSynchronize(h->stream));
-  COSL_CUDA(cudaMemcpy(tmp.data(), src, sizeof(float4) * tmp.size(), cudaMemcpyDeviceToHost));
+  COSL_CUDA(cudaMemcpy2D(tmp.data(), sizeof(float4) * lw, src, sizeof(float4) * h->lvW[level], sizeof(float4) * lw,
+                         lh, cudaMemcpyDeviceToHost));
   for (size_t i = 0; i < tmp.size(); ++i) {
     out3[3 * i] = tmp[i].x;
     out3[3 * i + 1] = tmp[i].y;
@@ -1090,8 +1148,9 @@ int cosl_klt_debug_cornerness(cosl_klt* h, int cam, float* out) {
   KLT_ENTER(h)
   if (cam < 0 || cam >= h->C || !out) return set_error(COSL_E_INVALID, "debug_cornerness");
   COSL_CUDA(cudaStreamSynchronize(h->stream));
-  COSL_CUDA(cudaMemcpy(out, h->d_corn + (size_t)cam * h->W * h->H,
-                       sizeof(float) * (size_t)h->W * h->H, cudaMemcpyDeviceToHost));
+  COSL_CUDA(cudaMemcpy2D(out, sizeof(float) * h->hcam[cam].W, h->d_corn + (size_t)cam * h->W * h->H,
+                         sizeof(float) * h->W, sizeof(float) * h->hcam[cam].W, h->hcam[cam].H,
+                         cudaMemcpyDeviceToHost));
   return COSL_OK;
 }
 
@@ -1109,7 +1168,9 @@ double cosl_klt_algorithmic_bytes(cosl_klt* h) {
   double pyr = 1.0;
   for (int l = 0; l < h->L; ++l) pyr += 12.0 / (double)(1 << (2 * l));
   const double perFeat = nlv * 2.0 * w1 * w1 * 12.0 + 32.0;
-  return (double)h->C * ((pyr + 8.0) * h->W * h->H + perFeat * h->F);
+  double px = 0.0;  // pixels of all cameras (exact)
+  for (int c = 0; c < h->C; ++c) px += (double)h->hcam[c].W * h->hcam[c].H;
+  return (double)h->C * ((pyr + 8.0) * (px / h->C) + perFeat * h->F);
 }
 
 int cosl_klt_profile_enable(cosl_klt* h, int on) {

@@ -19,7 +19,9 @@
 //
 // CLAMP_TO_EDGE of every pass is reproduced by construction: lanes / rows outside the image hold
 // the values of the clamped coordinate (u8 loads are clamped; level-0 values of out-of-image
-// columns are replaced by those of column 0 / W-1, out-of-image rows re-use row 0 / H-1).
+// columns are replaced by those of column 0 / W-1, out-of-image rows re-use row 0 / H-1).  W x H is
+// the camera's own extent (MIXED: its KltCam entry); the grid covers the group's largest camera and
+// the warps past a smaller camera's strips and chunks exit.
 #pragma once
 #include "klt_kernels.cuh"
 
@@ -46,22 +48,26 @@ struct FrontParams {
   float4* pyr;
   long long pyrStride, lv1Off;
   float* corn;
-  int W, H, nStrips, nChunks, wantL1, wantCorn;
+  long long cornStride;  // floats per camera; rows are W floats apart
+  int W, H, nStrips, nChunks, wantL1, wantCorn;  // W x H: the group's (largest) geometry
   int camBase;  // first camera of this launch (per-camera launches pipeline with the uploads)
   float minC;
   int ixlo, ixhi, iylo, iyhi;  // detector window (pixels whose centre lies inside the margins)
+  const KltCam* cams;          // MIXED: every camera's extent and detector window
 };
 
 // STORE_L0 = false: level 0 is computed (every other output derives from it) but not written
-template <bool STORE_L0>
+template <bool STORE_L0, bool MIXED>
 __global__ void __launch_bounds__(32 * FS_WARPS, FS_MINB)
 klt_front(const FrontParams P) {
   const int lane = threadIdx.x & 31;
   const int wid = blockIdx.x * FS_WARPS + (threadIdx.x >> 5);
-  if (wid >= P.nStrips * P.nChunks) return;
   const int cam = blockIdx.y + P.camBase;
-  const int chunk = wid / P.nStrips, strip = wid - chunk * P.nStrips;
-  const int W = P.W, H = P.H;
+  const int2 ext = klt_extent<MIXED>(P.cams, cam, P.W, P.H);
+  const int W = ext.x, H = ext.y;
+  const int nStrips = MIXED ? (W + FS_SW - 1) / FS_SW : P.nStrips;
+  if (wid >= nStrips * (MIXED ? (H + FS_R - 1) / FS_R : P.nChunks)) return;
+  const int chunk = wid / nStrips, strip = wid - chunk * nStrips;
   const int X0 = strip * FS_SW - FS_HL;
   const int xa = X0 + 2 * lane, xb = xa + 1;
   const int r0 = chunk * FS_R, r1 = min(H, r0 + FS_R);
@@ -75,9 +81,10 @@ klt_front(const FrontParams P) {
   const uint8_t* im = P.img + (size_t)cam * P.imgStride;
   float4* out0 = P.pyr + (size_t)cam * P.pyrStride;
   float4* out1 = out0 + P.lv1Off;
-  float* outc = P.corn + (size_t)cam * W * H;
-  const int dw = W >> 1, dh = H >> 1;
+  float* outc = P.corn + (size_t)cam * P.cornStride;
+  const int dh = H >> 1;
   const int j0 = r0 >> 1, j1 = min(dh, (r0 + FS_R) >> 1);  // level-1 rows of this chunk
+  const bool w1 = owner && (xa >> 1) < (W >> 1);            // this lane writes a level-1 column
 
   float ga[5], gb[5];  // image rows yc-2 .. yc+2 (clamped) at columns xa, xb
   // raw pixel pair (xa | xb << 8) of a clamped image row
@@ -153,7 +160,7 @@ klt_front(const FrontParams P) {
       }
       // ---- level 0 out
       if (STORE_L0 && yy >= r0 && yy < r1) {
-        float4* o = out0 + (size_t)yy * W + xa;
+        float4* o = out0 + (size_t)yy * P.W + xa;
         if (wa) o[0] = make_float4(A[0], A[1], A[2], 0.0f);
         if (wb) o[1] = make_float4(B[0], B[1], B[2], 0.0f);
       }
@@ -172,7 +179,7 @@ klt_front(const FrontParams P) {
               r[c] = tap1331(tl, ta, tb, tr);
             }
             const int i = xa >> 1;
-            if (owner && i < dw) out1[(size_t)j * dw + i] = make_float4(r[0], r[1], r[2], 0.0f);
+            if (w1) out1[(size_t)j * (P.W >> 1) + i] = make_float4(r[0], r[1], r[2], 0.0f);
           }
 #pragma unroll
           for (int c = 0; c < 3; ++c) {
@@ -210,6 +217,16 @@ klt_front(const FrontParams P) {
             for (int k = 0; k < 7; ++k) t = __fadd_rn(t, prod[(u + 1 + k) % 7][c]);  // top row first
             s[c] = t;
           }
+          // a mixed group's detector window, read here rather than held across the row loop,
+          // which is at the register limit (the camera index is re-read for the same reason)
+          int ixlo = P.ixlo, ixhi = P.ixhi, iylo = P.iylo, iyhi = P.iyhi;
+          if (MIXED) {
+            const KltCam* K = P.cams + klt_opaque((int)blockIdx.y) + P.camBase;
+            ixlo = __ldg(&K->ixlo);
+            ixhi = __ldg(&K->ixhi);
+            iylo = __ldg(&K->iylo);
+            iyhi = __ldg(&K->iyhi);
+          }
           float cs[2];
           float h[2][3];
 #pragma unroll
@@ -242,10 +259,10 @@ klt_front(const FrontParams P) {
             float v = __fmul_rn(0.5f, __fsub_rn(__fadd_rn(a, c), __fsqrt_rn(rad)));
             v = fmaxf(__fsub_rn(v, P.minC), 0.0f);
             const int gx = xa + q;
-            const bool inside = (gx >= P.ixlo && gx <= P.ixhi) && (yo >= P.iylo && yo <= P.iyhi);
+            const bool inside = (gx >= ixlo && gx <= ixhi) && (yo >= iylo && yo <= iyhi);
             cs[q] = inside ? v : 0.0f;
           }
-          float* o = outc + (size_t)yo * W + xa;
+          float* o = outc + (size_t)yo * P.W + xa;
           if (wa) o[0] = cs[0];
           if (wb) o[1] = cs[1];
         }

@@ -1,8 +1,12 @@
 // klt_kernels.cuh -- device code of the pyramidal KLT tracker (sm_90a).
 //
-// Data layout in HBM (per tracker group, C cameras of equal geometry, camera-major):
+// Data layout in HBM (per tracker group, C cameras, camera-major).  W x H is the group's largest
+// geometry (the maximum width and the maximum height over its cameras); every camera's slice is laid
+// out at it, and camera c's data occupies the top-left W_c x H_c (level l: (W_c >> l) x (H_c >> l))
+// of its slice.  Nothing reads the rest (KltCam):
 //   image    u8   [C][H][imgPitch]
-//   pyramid  float4 (I, Ix, Iy, 0) [2 buffers][C][sum_l w_l*h_l]   level l at offset lvOff[l]
+//   pyramid  float4 (I, Ix, Iy, 0) [2 buffers][C][sum_l w_l*h_l]   level l at offset lvOff[l], rows
+//                                                                   w_l = W >> l texels apart
 //   cornerness float [C][H][W]
 //   feature buffers float4 (x, y, gain, _) [C][F]: src (X0), dst (provided), ping/pong/res
 //   candidates u64 keys [C][candCap]: (~cornerness_bits << 32) | y << 16 | x  (ascending sort ==
@@ -22,6 +26,37 @@ namespace coslam {
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
 
+// A copy of v the compiler cannot see through: what is derived from it is computed where it is
+// used instead of being hoisted out of a loop and held in registers (or spilled) across it.
+__device__ __forceinline__ int klt_opaque(int v) {
+  asm volatile("" : "+r"(v));
+  return v;
+}
+
+// One camera of a group whose cameras differ in size (cosl_klt_group_create_sizes): its level-0
+// extent (level l is (W >> l) x (H >> l)) and its detector window.  Every kernel clamps its accesses
+// to the camera's own level border, so the padding of a smaller camera's slice is never read as data.
+//
+// Each kernel that needs an extent is instantiated twice, selected by the group's sizes:
+//   MIXED = false  the cameras are of one size: the kernel reads it from scalar kernel parameters (the
+//                  group's W, H, detector window, validRegion), as for a single camera;
+//   MIXED = true   the kernel reads its camera's entry of the table in global memory (the camera index
+//                  may differ between the lane groups of a warp: a parameter array indexed with it
+//                  would compile to chains of predicated constant loads).
+// A table of kernel parameters indexed per block was measured too: its size slowed the launches of
+// the uniform case, and a table read in every kernel added a memory round trip to each block.
+struct KltCam {
+  int W, H;
+  int ixlo, ixhi, iylo, iyhi;  // detector window: pixels whose centre lies inside the margins
+};
+
+// extent of camera `cam`: its table entry, or the group's W x H when all cameras share it
+template <bool MIXED>
+__device__ __forceinline__ int2 klt_extent(const KltCam* __restrict__ cams, int cam, int W, int H) {
+  if (MIXED) return make_int2(__ldg(&cams[cam].W), __ldg(&cams[cam].H));
+  return make_int2(W, H);
+}
+
 // [1 3 3 1] / 8 tap of the pyramid levels l >= 1 (pyramid_with_derivative_pass2.cg:1-15, host
 // v3d_gpupyramid.cpp:402-420), applied vertically then horizontally with decimation by 2 on all three
 // channels by klt_front (level 1) and klt_pyr_down_tma (levels >= 2).
@@ -35,8 +70,9 @@ __device__ __forceinline__ float tap1331(float a, float b, float c, float d) {
 // ------------------------------------------------------------------------------------------
 // Bilinear sampling of a pyramid level with clamp-to-edge (SURVEY Appendix A.3).
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float3 klt_sample(const float4* __restrict__ lv, int w, int h, float s,
-                                             float t) {
+// pitch: row pitch of the level in texels; w x h: the camera's extent of the level
+__device__ __forceinline__ float3 klt_sample(const float4* __restrict__ lv, int pitch, int w, int h,
+                                             float s, float t) {
   float u = s * (float)w - 0.5f;
   float v = t * (float)h - 0.5f;
   u = fminf(fmaxf(u, -2.0f), (float)w + 1.0f);
@@ -46,10 +82,10 @@ __device__ __forceinline__ float3 klt_sample(const float4* __restrict__ lv, int 
   const int xi = (int)fu, yi = (int)fv;
   const int x0 = clampi(xi, 0, w - 1), x1 = clampi(xi + 1, 0, w - 1);
   const int y0 = clampi(yi, 0, h - 1), y1 = clampi(yi + 1, 0, h - 1);
-  const float4 p00 = __ldg(&lv[(size_t)y0 * w + x0]);
-  const float4 p10 = __ldg(&lv[(size_t)y0 * w + x1]);
-  const float4 p01 = __ldg(&lv[(size_t)y1 * w + x0]);
-  const float4 p11 = __ldg(&lv[(size_t)y1 * w + x1]);
+  const float4 p00 = __ldg(&lv[(size_t)y0 * pitch + x0]);
+  const float4 p10 = __ldg(&lv[(size_t)y0 * pitch + x1]);
+  const float4 p01 = __ldg(&lv[(size_t)y1 * pitch + x0]);
+  const float4 p11 = __ldg(&lv[(size_t)y1 * pitch + x1]);
   float3 r;
   {
     const float top = p00.x + ax * (p10.x - p00.x), bot = p01.x + ax * (p11.x - p01.x);
@@ -72,13 +108,25 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// W, H, vr*: the group's (MIXED = false); a mixed group's kernels use the camera's extent and derive
+// the strict validRegion from `margin` (klt_vr_lo / klt_vr_hi)
 struct KltTrackParams {
   int W, H, F, halfWidth;
   float sqrConv, ssdThr;
   float vr0, vr1, vr2, vr3;  // validRegion
   float lambda, delta;
+  int strict;    // this set holds the strict validRegion (not the lax one, -1 .. 2)
+  float margin;  // trackBorderMargin (pixels)
 };
 
+// validRegion of a strict pass for a camera of n pixels along the axis: margin / n and
+// 1 - margin / n, the same correctly rounded fp32 values the host computes (v3d_gpuklt.cpp:266-270)
+__device__ __forceinline__ float klt_vr_lo(float margin, int n) { return __fdiv_rn(margin, (float)n); }
+__device__ __forceinline__ float klt_vr_hi(float margin, int n) {
+  return __fsub_rn(1.0f, __fdiv_rn(margin, (float)n));
+}
+
+// w, h: the group's level sizes (largest camera), also the row pitch of the level in texels
 struct KltLevels {
   int n;             // number of levels visited
   int level[8];
@@ -92,11 +140,14 @@ struct KltLevels {
 // feature.  Output (X1.x, X1.y, X0.x) or -1.
 // ------------------------------------------------------------------------------------------
 
+template <bool MIXED>
 __global__ void __launch_bounds__(256)
 klt_track_2x2(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, long long pyrStride,
-              KltLevels LV, const float4* __restrict__ X0buf, float4* __restrict__ out,
-              KltTrackParams P, int nIter) {
+              KltLevels LV, const KltCam* __restrict__ cams, const float4* __restrict__ X0buf,
+              float4* __restrict__ out, KltTrackParams P, int nIter) {
   const int cam = blockIdx.y;
+  const int2 ext = klt_extent<MIXED>(cams, cam, P.W, P.H);
+  const int Wc = ext.x, Hc = ext.y;
   const int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (slot >= P.F) return;
@@ -106,13 +157,14 @@ klt_track_2x2(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
   float X1x = X0x, X1y = X0y;
   bool invalid = (X1x < 0.f);
   const int hw = P.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
-  const float Wf = (float)P.W, Hf = (float)P.H;
+  const float Wf = (float)Wc, Hf = (float)Hc;
   const float dsx = 1.0f / Wf, dsy = 1.0f / Hf;
   float sqrLen = 0.f, ssd = 0.f;
   for (int li = 0; li < LV.n; ++li) {
     const float4* L0 = pyr0 + (size_t)cam * pyrStride + LV.off[li];
     const float4* L1 = pyr1 + (size_t)cam * pyrStride + LV.off[li];
-    const int w = LV.w[li], h = LV.h[li];
+    const int pitch = LV.w[li];
+    const int w = MIXED ? Wc >> LV.level[li] : LV.w[li], h = MIXED ? Hc >> LV.level[li] : LV.h[li];
     const float dx = dsx * LV.mult[li], dy = dsy * LV.mult[li];
     for (int it = 0; it < nIter; ++it) {
       float a = 0, b = 0, c = 0, r0 = 0, r1 = 0;
@@ -120,8 +172,8 @@ klt_track_2x2(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
       for (int p = lane; p < npx; p += 32) {
         const int py = p / fwid, px = p - py * fwid;
         const float fx = (float)(px - hw), fy = (float)(py - hw);
-        const float3 I0 = klt_sample(L0, w, h, X0x + fx * dx, X0y + fy * dy);
-        const float3 I1 = klt_sample(L1, w, h, X1x + fx * dx, X1y + fy * dy);
+        const float3 I0 = klt_sample(L0, pitch, w, h, X0x + fx * dx, X0y + fy * dy);
+        const float3 I1 = klt_sample(L1, pitch, w, h, X1x + fx * dx, X1y + fy * dy);
         const float e = I0.x - I1.x;
         const float Jx = (I0.y + I1.y) * Wf * 0.5f;
         const float Jy = (I0.z + I1.z) * Hf * 0.5f;
@@ -152,7 +204,11 @@ klt_track_2x2(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
     invalid = invalid || (sqrLen > P.sqrConv);
     invalid = invalid || (ssd > P.ssdThr);
   }
-  invalid = invalid || (X1x < P.vr0 || X1y < P.vr1) || (X1x > P.vr2 || X1y > P.vr3);
+  if (MIXED)
+    invalid = invalid || (X1x < klt_vr_lo(P.margin, Wc) || X1y < klt_vr_lo(P.margin, Hc)) ||
+              (X1x > klt_vr_hi(P.margin, Wc) || X1y > klt_vr_hi(P.margin, Hc));
+  else
+    invalid = invalid || (X1x < P.vr0 || X1y < P.vr1) || (X1x > P.vr2 || X1y > P.vr3);
   if (lane == 0)
     out[fb + slot] = invalid ? make_float4(-1.f, -1.f, -1.f, 0.f) : make_float4(X1x, X1y, X0x, 0.f);
 }
@@ -190,15 +246,22 @@ __global__ void klt_status(const float4* __restrict__ res, cosl_klt_feature* __r
 // Suppress detection at the pixel of every live point (presentFeaturesShader, v3d_gpuklt.cpp:475-500).
 // pts: float4 (x, y, .., ..) per slot, x < 0 == dead (clipped).  Camera c reads nPer[c] points when
 // nPer is given (present lists of different lengths), else n.
+// The cornerness map of camera c: rows `pitch` floats apart, `cornStride` floats per camera.
+template <bool MIXED>
 __global__ void klt_suppress(const float4* __restrict__ pts, int n, const int* __restrict__ nPer,
-                             int ptsStride, float* __restrict__ corn, int W, int H) {
+                             int ptsStride, float* __restrict__ corn, int pitch, long long cornStride,
+                             const KltCam* __restrict__ cams, int W, int H) {
   const int cam = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (nPer ? nPer[cam] : n)) return;
   const float4 p = pts[(size_t)cam * ptsStride + i];
   if (!(p.x >= 0.0f && p.x < 1.0f && p.y >= 0.0f && p.y < 1.0f)) return;
+  if (MIXED) {
+    W = __ldg(&cams[cam].W);
+    H = __ldg(&cams[cam].H);
+  }
   const int ix = (int)floorf(__fmul_rn(p.x, (float)W)), iy = (int)floorf(__fmul_rn(p.y, (float)H));
-  if (ix >= 0 && ix < W && iy >= 0 && iy < H) corn[(size_t)cam * W * H + (size_t)iy * W + ix] = -1e30f;
+  if (ix >= 0 && ix < W && iy >= 0 && iy < H) corn[(size_t)cam * cornStride + (size_t)iy * pitch + ix] = -1e30f;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -221,13 +284,19 @@ __global__ void klt_suppress(const float4* __restrict__ pts, int n, const int* _
 constexpr int NP_ROWS = 16;  // rows per warp in klt_nm_prefilter
 
 // PR = prefilter radius (1..3, <= the suppression radius r): lanes PR .. 31-PR produce outputs.
-template <int PR>
+template <int PR, bool MIXED>
 __global__ void __launch_bounds__(256)
-klt_nm_prefilter(const float* __restrict__ corn, int W, int H, unsigned* __restrict__ prelim,
+klt_nm_prefilter(const float* __restrict__ corn, int pitch, long long cornStride,
+                 const KltCam* __restrict__ cams, int W, int H, unsigned* __restrict__ prelim,
                  int prelimCap, int* __restrict__ counters) {
   constexpr int NCOLS = 32 - 2 * PR, NR = 2 * PR + 1;
   const int cam = blockIdx.z;
-  const float* cm = corn + (size_t)cam * W * H;
+  if (MIXED) {
+    W = __ldg(&cams[cam].W);
+    H = __ldg(&cams[cam].H);
+    if ((int)blockIdx.x * NCOLS >= W) return;  // the block's output columns lie outside this camera
+  }
+  const float* cm = corn + (size_t)cam * cornStride;
   const int lane = threadIdx.x & 31;
   const int x = blockIdx.x * NCOLS - PR + lane;                        // unclamped column
   const int y0 = (blockIdx.y * 8 + (threadIdx.x >> 5)) * NP_ROWS;      // first output row
@@ -237,7 +306,7 @@ klt_nm_prefilter(const float* __restrict__ corn, int W, int H, unsigned* __restr
   float v[NP_ROWS + 2 * PR];
 #pragma unroll
   for (int k = 0; k < NP_ROWS + 2 * PR; ++k)
-    v[k] = fabsf(__ldg(&cm[(size_t)clampi(y0 - PR + k, 0, H - 1) * W + cx]));
+    v[k] = fabsf(__ldg(&cm[(size_t)clampi(y0 - PR + k, 0, H - 1) * pitch + cx]));
   // The clamped loads make the window of a pixel near the image border contain copies of the edge
   // texels, which is exactly what the reference's CLAMP_TO_EDGE window contains there.
   const bool colOK = (lane >= PR) && (lane < PR + NCOLS) && (x < W);
@@ -296,12 +365,17 @@ klt_nm_prefilter(const float* __restrict__ corn, int W, int H, unsigned* __restr
 
 constexpr int NV_BATCH = 4;  // candidates a warp examines together (independent loads in flight)
 
+template <bool MIXED>
 __global__ void __launch_bounds__(256)
-klt_nm_verify(const float* __restrict__ corn, int W, int H, int r,
-              const unsigned* __restrict__ prelim, int prelimCap,
-              unsigned long long* __restrict__ cand, int candCap, int* __restrict__ counters) {
+klt_nm_verify(const float* __restrict__ corn, int pitch, long long cornStride,
+              const KltCam* __restrict__ cams, int W, int H, int r, const unsigned* __restrict__ prelim,
+              int prelimCap, unsigned long long* __restrict__ cand, int candCap, int* __restrict__ counters) {
   const int cam = blockIdx.y;
-  const float* cm = corn + (size_t)cam * W * H;
+  if (MIXED) {
+    W = __ldg(&cams[cam].W);
+    H = __ldg(&cams[cam].H);
+  }
+  const float* cm = corn + (size_t)cam * cornStride;
   const int lane = threadIdx.x & 31;
   const int warp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int nwarps = gridDim.x * (blockDim.x >> 5);
@@ -312,7 +386,7 @@ klt_nm_verify(const float* __restrict__ corn, int W, int H, int r,
     if (k >= nwin) return false;
     const int ri = k / side, dx = k - ri * side - r;
     const int dy = (ri & 1) ? -((ri + 1) >> 1) : (ri >> 1);
-    const float v = __ldg(&cm[(size_t)clampi(y + dy, 0, H - 1) * W + clampi(x + dx, 0, W - 1)]);
+    const float v = __ldg(&cm[(size_t)clampi(y + dy, 0, H - 1) * pitch + clampi(x + dx, 0, W - 1)]);
     return ((dx | dy) != 0) && !(c > fabsf(v));
   };
   for (int i0 = warp * NV_BATCH; i0 < n; i0 += nwarps * NV_BATCH) {
@@ -323,7 +397,7 @@ klt_nm_verify(const float* __restrict__ corn, int W, int H, int r,
     for (int j = 0; j < NV_BATCH; ++j) p[j] = (i0 + j < n) ? prelim[(size_t)cam * prelimCap + i0 + j] : 0u;
 #pragma unroll
     for (int j = 0; j < NV_BATCH; ++j)  // signed value: negative if suppressed meanwhile
-      c[j] = (i0 + j < n) ? __ldg(&cm[(size_t)(p[j] >> 16) * W + (p[j] & 0xffffu)]) : -1.0f;
+      c[j] = (i0 + j < n) ? __ldg(&cm[(size_t)(p[j] >> 16) * pitch + (p[j] & 0xffffu)]) : -1.0f;
     // first 32 texels (the centre row and most of the one above) of every candidate of the batch in
     // one memory round trip; the few candidates that are still unbeaten walk the rest of their
     // window 32 texels at a time and leave at the first larger value (reading whole windows
@@ -396,16 +470,24 @@ __device__ __forceinline__ unsigned klt_compact1by1(unsigned v) {
   return v;
 }
 
+constexpr int KLT_MAX_SMEM_KEYS = 16384;  // keys sorted in shared memory; more sort in global memory
+
+template <bool MIXED>
 __global__ void __launch_bounds__(1024)
 klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
                   int* __restrict__ counters, cosl_klt_feature* __restrict__ dest,
                   float4* __restrict__ dstbuf, float4* __restrict__ alsoSrc,
                   const float4* __restrict__ present, const int* __restrict__ nPresentPer,
-                  int F, int W, int H, int mode, int withGain, int smemKeys, int histo) {
+                  int F, const KltCam* __restrict__ cams, int W, int H, int mode, int withGain,
+                  int smemKeys, int histo) {
   extern __shared__ unsigned long long s_keys[];
   __shared__ int s_scan[1024];
   __shared__ int s_base;
   const int cam = blockIdx.x;
+  if (MIXED) {
+    W = __ldg(&cams[cam].W);
+    H = __ldg(&cams[cam].H);
+  }
   const int nPresentExt = (mode == 0 && nPresentPer) ? nPresentPer[cam] : 0;
   int* cnt = counters + cam * 8;
   unsigned long long* ck = cand + (size_t)cam * candCap;

@@ -13,6 +13,11 @@
 //     always lies inside the box.
 //   * the TW x TH output tile is written back with a TMA store (SASS: UTMASTG), which clips the
 //     tile at the level border by itself.
+// In a group of cameras of different sizes the tensor maps describe the group's largest level, and
+// the kernel clamps to the camera's own source level (sw x sh = the camera's extent of level - 1): the
+// box may cover padding of a smaller camera's slice, but only clamped coordinates are read.  The
+// store clips at the largest level, so a tile that straddles the camera's border also writes into
+// its padding (values derived from clamped data, never read); blocks wholly outside the camera exit.
 #pragma once
 #include <cuda.h>
 
@@ -27,15 +32,24 @@ __device__ __forceinline__ unsigned smem_u32(const void* p) {
   return (unsigned)__cvta_generic_to_shared(p);
 }
 
+// sw x sh: the source level of the group's cameras (MIXED: of the largest; each block reads its own
+// camera's from `cams`); level: the destination level
+template <bool MIXED>
 __global__ void __launch_bounds__(256)
 klt_pyr_down_tma(const __grid_constant__ CUtensorMap srcMap, const __grid_constant__ CUtensorMap dstMap,
-                 int sw, int sh) {
+                 int sw, int sh, const KltCam* __restrict__ cams, int level) {
   __shared__ __align__(128) float4 s_in[PT_SH][PT_SW];
   __shared__ __align__(128) float4 s_out[PT_TH][PT_TW];
   __shared__ float4 s_t[PT_TH][PT_SW];
   __shared__ __align__(8) unsigned long long s_bar;
   const int cam = blockIdx.z;
   const int ox = blockIdx.x * PT_TW, oy = blockIdx.y * PT_TH;
+  if (MIXED) {
+    const int Wc = __ldg(&cams[cam].W), Hc = __ldg(&cams[cam].H);
+    if (ox >= (Wc >> level) || oy >= (Hc >> level)) return;
+    sw = Wc >> (level - 1);
+    sh = Hc >> (level - 1);
+  }
   const int tid = threadIdx.x;
   const int x0 = 2 * ox - 1, y0 = 2 * oy - 1;  // tile origin in the source level (may be -1)
   if (tid == 0) {

@@ -57,19 +57,13 @@ __device__ __forceinline__ int2 klt_tile_texel(int gl, int half, int u) {
   return make_int2(4 * (u % 3) + (gl & 3), half * (KLT_TW / 2) + 2 * (u / 3) + (gl >> 2));
 }
 
-// L2 prefetch of the texels (x .. x + n - 1, y) of a level, clamped to the level like the loads
-// that will read them (one bulk prefetch: a row segment is contiguous)
-__device__ __forceinline__ void klt_prefetch_row(const float4* lv, int w, int h, int x, int y, int n) {
+// L2 prefetch of the texels (x .. x + n - 1, y) of a level, clamped to the camera's w x h of the
+// level like the loads that will read them (one bulk prefetch: a row segment is contiguous)
+__device__ __forceinline__ void klt_prefetch_row(const float4* lv, int pitch, int w, int h, int x, int y,
+                                                 int n) {
   const int xa = clampi(x, 0, w - 1), xb = clampi(x + n - 1, 0, w - 1);
-  const float4* p = lv + (size_t)clampi(y, 0, h - 1) * w + xa;
+  const float4* p = lv + (size_t)clampi(y, 0, h - 1) * pitch + xa;
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"((xb - xa + 1) * 16) : "memory");
-}
-
-// A copy of v the compiler cannot see through: what is derived from it is computed where it is
-// used instead of being hoisted out of a loop and held in registers (or spilled) across it.
-__device__ __forceinline__ int klt_opaque(int v) {
-  asm volatile("" : "+r"(v));
-  return v;
 }
 
 struct KltCentre {
@@ -107,13 +101,14 @@ __device__ __forceinline__ float3 klt_lerp4(const float4 p00, const float4 p10, 
   return r;
 }
 
-// tap (xi, yi) of a level with clamp-to-edge, weights (ax, ay)
-__device__ __forceinline__ float3 klt_fetch_global(const float4* __restrict__ lv, int w, int h,
+// tap (xi, yi) of a level (rows `pitch` texels apart) with clamp-to-edge at the camera's w x h,
+// weights (ax, ay)
+__device__ __forceinline__ float3 klt_fetch_global(const float4* __restrict__ lv, int pitch, int w, int h,
                                                    int xi, int yi, float ax, float ay) {
   const int x0 = clampi(xi, 0, w - 1), x1 = clampi(xi + 1, 0, w - 1);
   const int y0 = clampi(yi, 0, h - 1), y1 = clampi(yi + 1, 0, h - 1);
-  return klt_lerp4(__ldg(&lv[(size_t)y0 * w + x0]), __ldg(&lv[(size_t)y0 * w + x1]),
-                   __ldg(&lv[(size_t)y1 * w + x0]), __ldg(&lv[(size_t)y1 * w + x1]), ax, ay);
+  return klt_lerp4(__ldg(&lv[(size_t)y0 * pitch + x0]), __ldg(&lv[(size_t)y0 * pitch + x1]),
+                   __ldg(&lv[(size_t)y1 * pitch + x0]), __ldg(&lv[(size_t)y1 * pitch + x1]), ax, ay);
 }
 
 __device__ __forceinline__ float grp_sum(float v) {
@@ -170,7 +165,7 @@ __device__ __forceinline__ void klt_acc_pixel(KltAcc& A, const float3 I0, const 
 // kernel-parameter structs (strict ? Pstrict : Plax) cannot be formed as a pointer, so every field
 // read through it compiled to a chain of predicated constant loads over all candidate offsets.
 struct KltFinishParams {
-  float delta, W, H;         // the same in the lax and the strict set
+  float delta, W, H;         // the same in the lax and the strict set; W, H: the slot's camera
   float ssdThr, sqrConv;
   float vr0, vr1, vr2, vr3;  // validRegion
 };
@@ -182,18 +177,29 @@ __device__ __forceinline__ float klt_select(bool c, float a, float b) {
   return __uint_as_float((__float_as_uint(a) & m) | (__float_as_uint(b) & ~m));
 }
 
+// MIXED: the slot's camera is Wc x Hc (the lane groups of a warp may serve two cameras), and the
+// strict validRegion is derived from it; otherwise every field comes from the parameter sets
+template <bool MIXED>
 __device__ __forceinline__ KltFinishParams klt_finish_params(const KltTrackParams& lax,
-                                                             const KltTrackParams& str, bool strict) {
+                                                             const KltTrackParams& str, bool strict,
+                                                             int Wc, int Hc) {
   KltFinishParams T;
   T.delta = lax.delta;
-  T.W = (float)lax.W;
-  T.H = (float)lax.H;
+  T.W = (float)(MIXED ? Wc : lax.W);
+  T.H = (float)(MIXED ? Hc : lax.H);
   T.ssdThr = klt_select(strict, str.ssdThr, lax.ssdThr);
   T.sqrConv = klt_select(strict, str.sqrConv, lax.sqrConv);
-  T.vr0 = klt_select(strict, str.vr0, lax.vr0);
-  T.vr1 = klt_select(strict, str.vr1, lax.vr1);
-  T.vr2 = klt_select(strict, str.vr2, lax.vr2);
-  T.vr3 = klt_select(strict, str.vr3, lax.vr3);
+  if (MIXED) {
+    T.vr0 = klt_select(strict, klt_vr_lo(str.margin, Wc), lax.vr0);
+    T.vr1 = klt_select(strict, klt_vr_lo(str.margin, Hc), lax.vr1);
+    T.vr2 = klt_select(strict, klt_vr_hi(str.margin, Wc), lax.vr2);
+    T.vr3 = klt_select(strict, klt_vr_hi(str.margin, Hc), lax.vr3);
+  } else {
+    T.vr0 = klt_select(strict, str.vr0, lax.vr0);
+    T.vr1 = klt_select(strict, str.vr1, lax.vr1);
+    T.vr2 = klt_select(strict, str.vr2, lax.vr2);
+    T.vr3 = klt_select(strict, str.vr3, lax.vr3);
+  }
   return T;
 }
 
@@ -253,17 +259,18 @@ constexpr int KLT_HW_LIVE = 3;
 
 // ------------------------------------------------------------------------------------------
 // One pass per launch (diagnostic / fallback).  Grid: x = ceil(F / 32) blocks of 256 threads
-// (32 lane groups), y = camera.
+// (32 lane groups), y = camera.  level, lvOff, pitch: the pyramid level of the pass.
 // ------------------------------------------------------------------------------------------
-template <int HWC>
+template <int HWC, bool MIXED>
 __global__ void __launch_bounds__(256)
 klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, long long pyrStride,
-              long long lvOff, int w, int h, const float4* __restrict__ X0buf,
-              const float4* __restrict__ in, float4* __restrict__ out,
-              const int* __restrict__ nbr, float dsx, float dsy, KltTrackParams P, int firstPass) {
-  (void)dsx;
-  (void)dsy;
+              long long lvOff, int level, int pitch, const KltCam* __restrict__ cams,
+              const float4* __restrict__ X0buf, const float4* __restrict__ in, float4* __restrict__ out,
+              const int* __restrict__ nbr, KltTrackParams P, int firstPass) {
   const int cam = blockIdx.y;
+  const int2 ext = klt_extent<MIXED>(cams, cam, P.W, P.H);
+  const int Wc = ext.x, Hc = ext.y;
+  const int w = Wc >> level, h = Hc >> level;
   const int gl = threadIdx.x & (KLT_G - 1), grpBase = threadIdx.x & (32 - KLT_G);
   int slot = blockIdx.x * (blockDim.x / KLT_G) + (threadIdx.x / KLT_G);
   const bool active = slot < P.F;
@@ -279,7 +286,7 @@ klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
   const float nbterm = klt_nbterm(bn, beta, gl, grpBase);
   const bool pre_invalid = (cur.x < 0.f) || (x0.x < 0.f);
   const int hw = HWC > 0 ? HWC : P.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
-  const float halfW = 0.5f * (float)P.W, halfH = 0.5f * (float)P.H;
+  const float halfW = 0.5f * (float)Wc, halfH = 0.5f * (float)Hc;
   const KltCentre c0 = klt_centre(w, h, x0.x, x0.y);
   const KltCentre c1 = klt_centre(w, h, cur.x, cur.y);
   KltAcc A = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -287,13 +294,14 @@ klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
   for (int p = gl; p < npx; p += KLT_G) {
     const int py = p / fwid, px = p - py * fwid;
     const int dx = px - hw, dy = py - hw;
-    const float3 I0 = klt_fetch_global(L0, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
-    const float3 I1 = klt_fetch_global(L1, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
+    const float3 I0 = klt_fetch_global(L0, pitch, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
+    const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
     d2 = __fadd_rn(d2, klt_d2_term(I0, P.lambda, P.delta));
     klt_acc_pixel(A, I0, I1, beta, halfW, halfH, P.lambda);
   }
+  // the host chose P per pass: its validRegion is the strict or the lax one as P.strict says
   float4 res = klt_gain_finish(A, grp_sum(d2), nbterm, (float)npx, cur.x, cur.y, beta,
-                               klt_finish_params(P, P, false));  // the host chose P per pass
+                               klt_finish_params<MIXED>(P, P, P.strict != 0, Wc, Hc));
   if (pre_invalid) res = make_float4(-1.f, -1.f, -1.f, 0.f);
   if (gl == 0 && active) out[fb + slot] = res;
 }
@@ -343,16 +351,18 @@ struct KltTail {
   cosl_klt_feature* dest;
   int* counters;
   float* corn;
-  int W, H, suppress;
+  long long cornStride;  // floats per camera; rows are `pitch` floats apart
+  int pitch, suppress;
 };
 
 constexpr int KLT_FUSED_THREADS = KLT_FUSED_THREADS_N;  // 16 lane groups per CTA
 constexpr int KLT_GPB = KLT_FUSED_THREADS / KLT_G;
 
-template <int HWC>
+template <int HWC, bool MIXED>
 __global__ void __launch_bounds__(KLT_FUSED_THREADS, KLT_FUSED_MINBLOCKS)
 klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
-               long long pyrStride, KltLevels LV, int nIter, const float4* __restrict__ X0buf,
+               long long pyrStride, KltLevels LV, const KltCam* __restrict__ cams, int nIter,
+               const float4* __restrict__ X0buf,
                float4* __restrict__ state, unsigned long long* __restrict__ rec,
                const int* __restrict__ waitset,
                float4* __restrict__ out, int C, KltTrackParams Plax, KltTrackParams Pstrict,
@@ -366,7 +376,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   const int T = C * F;
   const int hw = HWC > 0 ? HWC : Plax.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
   const bool fast = (npx <= KLT_G * KLT_ROUNDS) && (2 * hw + 2 + 2 <= KLT_TW) && (2 * hw + 2 <= 8);
-  const float halfW = 0.5f * (float)Plax.W, halfH = 0.5f * (float)Plax.H;
   float4* tile = s_tile[grpInBlock];
   // all groups of a warp must execute the same number of outer iterations (full-mask shuffles)
   const int nOwn = (T + Q - 1) / Q;
@@ -377,6 +386,8 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   const int cam0 = item0 / F, slot0 = item0 - cam0 * F;
   const float4 x00 = X0buf[item0];
   const int wsA0 = waitset[slot0 * 16 + gl], wsB0 = waitset[slot0 * 16 + 8 + gl];
+  // MIXED: the resident item's camera, packed W | H << 16 into one register
+  const unsigned wh0 = MIXED ? (unsigned)__ldg(&cams[cam0].W) | ((unsigned)__ldg(&cams[cam0].H) << 16) : 0u;
   float3 I0r[KLT_ROUNDS];
   float f0 = 0.f;  // group sum of klt_d2_term of the resident item at the current level
   float4 cur0 = make_float4(-1.f, -1.f, -1.f, 0.f);
@@ -392,14 +403,16 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   // per-level staging below finds them there (lane gl: row gl of each 8x8 block)
   if (fast && active0 && x00.x >= 0.f) {
     for (int li = 0; li < LV.n; ++li) {
-      const KltCentre c0 = klt_centre(LV.w[li], LV.h[li], x00.x, x00.y);
-      klt_prefetch_row(pyr0 + (size_t)cam0 * pyrStride + LV.off[li], LV.w[li], LV.h[li], c0.xi - hw,
+      const int w = MIXED ? (int)(wh0 & 0xffffu) >> LV.level[li] : LV.w[li];
+      const int h = MIXED ? (int)(wh0 >> 16) >> LV.level[li] : LV.h[li];
+      const KltCentre c0 = klt_centre(w, h, x00.x, x00.y);
+      klt_prefetch_row(pyr0 + (size_t)cam0 * pyrStride + LV.off[li], LV.w[li], w, h, c0.xi - hw,
                        c0.yi - hw + gl, 8);
     }
   }
   int pass = 0;
   for (int li = 0; li < LV.n; ++li) {
-    const int w = LV.w[li], h = LV.h[li];
+    const int pitch = LV.w[li], level = LV.level[li];
     for (int it = 1; it <= nIter; ++it) {
       ++pass;
       // thresholds are lax except on the last iteration of a level (v3d_gpuklt.cpp:266-279)
@@ -421,6 +434,16 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
           wsA = waitset[slot * 16 + gl];
           wsB = waitset[slot * 16 + 8 + gl];
         }
+        // the item's camera: the lane groups of a warp may serve two cameras (F % 4 != 0)
+        int Wc = Plax.W, Hc = Plax.H, w = pitch, h = LV.h[li];
+        if (MIXED) {
+          const unsigned wh =
+              (own == 0) ? wh0 : (unsigned)__ldg(&cams[cam].W) | ((unsigned)__ldg(&cams[cam].H) << 16);
+          Wc = wh & 0xffffu;
+          Hc = wh >> 16;
+          w = Wc >> level;
+          h = Hc >> level;
+        }
         // own state; the neighbours' gains are needed only after the pixel loop (klt_gain_finish)
         float4 cur;
         if (pass == 1)
@@ -440,11 +463,12 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         // last iteration of a level: request the next level's I1 tile around the current estimate
         // into L2 (rows gl and gl + 8), so its staging does not wait on HBM
         if (staged && it == nIter && li + 1 < LV.n && !pre_invalid) {
-          const int wn = LV.w[li + 1], hn = LV.h[li + 1];
+          const int pn = LV.w[li + 1];
+          const int wn = MIXED ? Wc >> LV.level[li + 1] : pn, hn = MIXED ? Hc >> LV.level[li + 1] : LV.h[li + 1];
           const KltCentre cn = klt_centre(wn, hn, cur.x, cur.y);
           const float4* Ln = pyr1 + (size_t)cam * pyrStride + LV.off[li + 1];
-          klt_prefetch_row(Ln, wn, hn, cn.xi - hw - 2, cn.yi - hw - 2 + gl, KLT_TW);
-          if (gl + KLT_G < KLT_TW) klt_prefetch_row(Ln, wn, hn, cn.xi - hw - 2, cn.yi - hw - 2 + gl + KLT_G, KLT_TW);
+          klt_prefetch_row(Ln, pn, wn, hn, cn.xi - hw - 2, cn.yi - hw - 2 + gl, KLT_TW);
+          if (gl + KLT_G < KLT_TW) klt_prefetch_row(Ln, pn, wn, hn, cn.xi - hw - 2, cn.yi - hw - 2 + gl + KLT_G, KLT_TW);
         }
         // ---- per-level staging (first iteration of a level): I0 samples + I1 tile.
         // Three memory round trips with all loads of a trip in flight together: (A) the 8x8 texels
@@ -466,12 +490,12 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
             float4 t0[8], tv[NLD];
 #pragma unroll
             for (int u = 0; u < 8; ++u)  // lane gl loads column gl of the 8x8 block
-              t0[u] = __ldg(&L0[(size_t)clampi(c0.yi - hw + u, 0, h - 1) * w + clampi(c0.xi - hw + gl, 0, w - 1)]);
+              t0[u] = __ldg(&L0[(size_t)clampi(c0.yi - hw + u, 0, h - 1) * pitch + clampi(c0.xi - hw + gl, 0, w - 1)]);
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
               const int2 ba = klt_tile_texel(gl, 0, u);
               const int b = ba.y, a = ba.x;
-              tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
+              tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * pitch + clampi(tx0 + a, 0, w - 1)]);
             }
 #pragma unroll
             for (int u = 0; u < 8; ++u) tile[I0B + u * 8 + gl] = t0[u];
@@ -504,7 +528,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
             for (int u = 0; u < NLD; ++u) {
               const int2 ba = klt_tile_texel(gl, 1, u);
               const int b = ba.y, a = ba.x;
-              tw[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
+              tw[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * pitch + clampi(tx0 + a, 0, w - 1)]);
             }
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
@@ -520,6 +544,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         KLT_CLK(c2k);
         KltAcc A = {0, 0, 0, 0, 0, 0, 0, 0, 0};
         float f = f0;
+        const float halfW = 0.5f * (float)Wc, halfH = 0.5f * (float)Hc;
         // tile[b * KLT_TP + a] == level[clamp(ty0 + b)][clamp(tx0 + a)]: indexing with the
         // unclamped tap coordinates reproduces the clamped fetches exactly
         int a0 = c1.xi - tx0, b0 = c1.yi - ty0;
@@ -543,7 +568,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                 for (int u = 0; u < NLD; ++u) {
                   const int2 ba = klt_tile_texel(gl, half, u);
                   const int b = ba.y, a = ba.x;
-                  tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
+                  tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * pitch + clampi(tx0 + a, 0, w - 1)]);
                 }
 #pragma unroll
                 for (int u = 0; u < NLD; ++u) {
@@ -587,7 +612,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
               const int p = gl + KLT_G * r;
               if (p < npx) {
                 const int py = p / fwid, px = p - py * fwid;
-                const float3 I1 = klt_fetch_global(L1, w, h, c1.xi + px - hw, c1.yi + py - hw, c1.ax, c1.ay);
+                const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + px - hw, c1.yi + py - hw, c1.ax, c1.ay);
                 // I0r is indexed dynamically only on this rare path
                 float3 I0 = I0r[0];
 #pragma unroll
@@ -604,8 +629,8 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
             for (int p = gl; p < npx; p += KLT_G) {
               const int py = p / fwid, px = p - py * fwid;
               const int dx = px - hw, dy = py - hw;
-              const float3 I0 = klt_fetch_global(L0, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
-              const float3 I1 = klt_fetch_global(L1, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
+              const float3 I0 = klt_fetch_global(L0, pitch, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
+              const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
               d2 = __fadd_rn(d2, klt_d2_term(I0, Plax.lambda, Plax.delta));
               klt_acc_pixel(A, I0, I1, beta, halfW, halfH, Plax.lambda);
             }
@@ -636,7 +661,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         KLT_CLK(c3p);
         const float nbterm = klt_nbterm(bn, beta, gl, grpBase);
         float4 res = klt_gain_finish(A, f, nbterm, (float)npx, cur.x, cur.y, beta,
-                                     klt_finish_params(Plax, Pstrict, strict));
+                                     klt_finish_params<MIXED>(Plax, Pstrict, strict, Wc, Hc));
         if (pre_invalid) res = make_float4(-1.f, -1.f, -1.f, 0.f);
         if (staged) cur0 = res;
         if (gl == 0 && active) {
@@ -654,10 +679,10 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
               if (live) {
                 atomicAdd(&tail.counters[cam * 8 + 0], 1);
                 if (tail.suppress && res.x < 1.0f && res.y >= 0.0f && res.y < 1.0f) {
-                  const int ix = (int)floorf(__fmul_rn(res.x, (float)tail.W));
-                  const int iy = (int)floorf(__fmul_rn(res.y, (float)tail.H));
-                  if (ix >= 0 && ix < tail.W && iy >= 0 && iy < tail.H)
-                    tail.corn[(size_t)cam * tail.W * tail.H + (size_t)iy * tail.W + ix] = -1e30f;
+                  const int ix = (int)floorf(__fmul_rn(res.x, (float)Wc));
+                  const int iy = (int)floorf(__fmul_rn(res.y, (float)Hc));
+                  if (ix >= 0 && ix < Wc && iy >= 0 && iy < Hc)
+                    tail.corn[(size_t)cam * tail.cornStride + (size_t)iy * tail.pitch + ix] = -1e30f;
                 }
               }
             }
@@ -706,10 +731,12 @@ namespace coslam {
 // klt_track_2x2 (thresholds from the last iteration of every level, validity region at the end);
 // used when the window fits the tile (hw <= 3), klt_track_2x2 otherwise.
 // ------------------------------------------------------------------------------------------
+template <bool MIXED>
 __global__ void __launch_bounds__(128)
 klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
-                    long long pyrStride, KltLevels LV, const float4* __restrict__ X0buf,
-                    float4* __restrict__ out, KltTrackParams P, int nIter) {
+                    long long pyrStride, KltLevels LV, const KltCam* __restrict__ cams,
+                    const float4* __restrict__ X0buf, float4* __restrict__ out, KltTrackParams P,
+                    int nIter) {
   __shared__ float4 s_tile[16][KLT_TW * KLT_TP];
   const int gl = threadIdx.x & (KLT_G - 1);
   const int grp = threadIdx.x / KLT_G;
@@ -724,7 +751,9 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
   bool invalid = (x0.x < 0.f);
   const bool dead = invalid;  // no samples are fetched for a dead slot
   const int hw = P.halfWidth, fwid = 2 * hw + 1, npx = fwid * fwid;
-  const float halfW = 0.5f * (float)P.W, halfH = 0.5f * (float)P.H;
+  const int2 ext = klt_extent<MIXED>(cams, cam, P.W, P.H);
+  const int Wc = ext.x, Hc = ext.y;
+  const float halfW = 0.5f * (float)Wc, halfH = 0.5f * (float)Hc;
   int toff[KLT_ROUNDS];
 #pragma unroll
   for (int r = 0; r < KLT_ROUNDS; ++r) {
@@ -735,7 +764,8 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
   float3 I0r[KLT_ROUNDS];
   float sqrLen = 0.f, ssd = 0.f;
   for (int li = 0; li < LV.n; ++li) {
-    const int w = LV.w[li], h = LV.h[li];
+    const int pitch = LV.w[li];
+    const int w = MIXED ? Wc >> LV.level[li] : LV.w[li], h = MIXED ? Hc >> LV.level[li] : LV.h[li];
     const float4* L0 = pyr0 + (size_t)cam * pyrStride + LV.off[li];
     const float4* L1 = pyr1 + (size_t)cam * pyrStride + LV.off[li];
     constexpr int NLD = KLT_TW * KLT_TW / KLT_G / 2;
@@ -751,12 +781,12 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
         float4 t0[8], tv[NLD];
 #pragma unroll
         for (int u = 0; u < 8; ++u)
-          t0[u] = __ldg(&L0[(size_t)clampi(c0.yi - hw + u, 0, h - 1) * w + clampi(c0.xi - hw + gl, 0, w - 1)]);
+          t0[u] = __ldg(&L0[(size_t)clampi(c0.yi - hw + u, 0, h - 1) * pitch + clampi(c0.xi - hw + gl, 0, w - 1)]);
 #pragma unroll
         for (int u = 0; u < NLD; ++u) {
           const int i = gl + KLT_G * u;
           const int b = i / KLT_TW, a = i - b * KLT_TW;
-          tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
+          tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * pitch + clampi(tx0 + a, 0, w - 1)]);
         }
 #pragma unroll
         for (int u = 0; u < 8; ++u) tile[I0B + u * 8 + gl] = t0[u];
@@ -788,7 +818,7 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
         for (int u = 0; u < NLD; ++u) {
           const int i = gl + KLT_G * (u + NLD);
           const int b = i / KLT_TW, a = i - b * KLT_TW;
-          tw[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
+          tw[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * pitch + clampi(tx0 + a, 0, w - 1)]);
         }
 #pragma unroll
         for (int u = 0; u < NLD; ++u) {
@@ -815,7 +845,7 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
             for (int u = 0; u < NLD; ++u) {
               const int i = gl + KLT_G * (u + half * NLD);
               const int b = i / KLT_TW, a = i - b * KLT_TW;
-              tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * w + clampi(tx0 + a, 0, w - 1)]);
+              tv[u] = __ldg(&L1[(size_t)clampi(ty0 + b, 0, h - 1) * pitch + clampi(tx0 + a, 0, w - 1)]);
             }
 #pragma unroll
             for (int u = 0; u < NLD; ++u) {
@@ -863,14 +893,18 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
       float uy = __fmul_rn(rdet, __fmaf_rn(a, r1, -__fmul_rn(b, r0)));
       X1x = __fadd_rn(X1x, ux);
       X1y = __fadd_rn(X1y, uy);
-      ux = __fmul_rn(ux, (float)P.W);
-      uy = __fmul_rn(uy, (float)P.H);
+      ux = __fmul_rn(ux, (float)Wc);
+      uy = __fmul_rn(uy, (float)Hc);
       sqrLen = __fmaf_rn(ux, ux, __fmul_rn(uy, uy));
     }
     invalid = invalid || (sqrLen > P.sqrConv);
     invalid = invalid || (ssd > P.ssdThr);
   }
-  invalid = invalid || (X1x < P.vr0 || X1y < P.vr1) || (X1x > P.vr2 || X1y > P.vr3);
+  if (MIXED)
+    invalid = invalid || (X1x < klt_vr_lo(P.margin, Wc) || X1y < klt_vr_lo(P.margin, Hc)) ||
+              (X1x > klt_vr_hi(P.margin, Wc) || X1y > klt_vr_hi(P.margin, Hc));
+  else
+    invalid = invalid || (X1x < P.vr0 || X1y < P.vr1) || (X1x > P.vr2 || X1y > P.vr3);
   if (gl == 0 && active)
     out[fb + slot] = invalid ? make_float4(-1.f, -1.f, -1.f, 0.f) : make_float4(X1x, X1y, x0.x, 0.f);
 }

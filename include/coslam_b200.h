@@ -90,7 +90,7 @@ typedef struct cosl_klt_feature {
   int fed;      /* >=0: index of the externally fed point */
 } cosl_klt_feature;
 
-typedef struct cosl_klt cosl_klt; /* opaque: one tracker group = C cameras of equal geometry */
+typedef struct cosl_klt cosl_klt; /* opaque: one tracker group = C cameras */
 
 void cosl_klt_config_default(cosl_klt_config* cfg);
 
@@ -105,6 +105,18 @@ int cosl_klt_create(const cosl_klt_config* cfg, int width, int height, int nLeve
 int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int height,
                           int nLevels, int featW, int featH, int plW, int plH, int device,
                           cosl_klt** out);
+/* Extension: a group whose camera c is widths[c] x heights[c] (each SingleSLAM's tracker takes its
+ * size from its own video, app/SL_SingleSLAM.cpp:267-300); the configuration, level count and
+ * feature grid are shared.  Every camera must satisfy the per-camera checks of
+ * cosl_klt_group_create, the smallest one included ((W >> (nLevels-1)) >= 2).  Every group call
+ * works on such a group, and each camera behaves bit for bit like a single-camera tracker of its own
+ * size.  Image-taking calls accept pitch == 0 on such a group: camera c's rows are then widths[c]
+ * bytes apart; a pitch > 0 must be at least the largest width.  Buffers are laid out at the largest
+ * width and the largest height for every camera.  cosl_klt_group_create is this call with equal
+ * sizes, except that it keeps rejecting pitch == 0. */
+int cosl_klt_group_create_sizes(const cosl_klt_config* cfg, int nCams, const int* widths,
+                                const int* heights, int nLevels, int featW, int featH, int plW, int plH,
+                                int device, cosl_klt** out);
 /* KLT_SequenceTracker::deallocate (v3d_gpuklt.cpp:626-648). */
 int cosl_klt_destroy(cosl_klt* h);
 
@@ -187,14 +199,15 @@ int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew
 void* cosl_klt_stream(cosl_klt* h);
 
 /* Test/inspection hooks (not part of the reference surface). */
-/* Copy pyramid level `level` of camera `cam` to host as interleaved (I, Ix, Iy) floats.
+/* Copy pyramid level `level` of camera `cam` to host as interleaved (I, Ix, Iy) floats: the camera's
+ * own (W_c >> level) x (H_c >> level) texels, returned in *w, *ht.
  * which: 0 = previous frame (pyr0), 1 = current frame (pyr1).  Level 0 of a frame built by
  * next()/redetect() is not stored when the tracker does not visit level 0 (levels L-1, L-1-levelSkip,
  * ...); reading it then returns COSL_E_INVALID.  detect()/first() and track() store every level.
  * The record of what was stored follows each camera through cosl_klt_group_advance_cams. */
 int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* out3, int* w,
                            int* ht);
-/* Copy the cornerness map after non-max suppression input stage (W*H floats) of camera cam. */
+/* Copy the cornerness map after non-max suppression input stage (W_c*H_c floats) of camera cam. */
 int cosl_klt_debug_cornerness(cosl_klt* h, int cam, float* out);
 /* Raw number of detector candidates of the last detect/redetect fetched to the host. */
 int cosl_klt_debug_num_candidates(cosl_klt* h, int cam);
