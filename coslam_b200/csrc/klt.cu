@@ -29,6 +29,12 @@ struct cosl_klt {
   int levelSkip = 1, halfWidth = 3;
   float trackMargin = 4.f, conv = 0.1f, ssd = 5000.f, detectMargin = 10.f;
   cudaStream_t stream = nullptr;
+  // image copies, klt_front and the pyramid tail run on the front stream, so that frame n+1's
+  // pyramid is built while frame n's detector runs on `stream`.  The front stream starts a frame
+  // after evFence, which `stream` records behind the last stage that reads what the front stream
+  // overwrites (run_frame); `stream` waits for evTail before the frame's tracker or detector.
+  cudaStream_t frontStream = nullptr;
+  cudaEvent_t evFence = nullptr, evTail = nullptr;
   // host uploads run on their own stream, one event per camera, so that klt_front of camera c
   // overlaps the copy of camera c+1 (cosl_klt_group_next path)
   cudaStream_t copyStream = nullptr;
@@ -53,15 +59,22 @@ struct cosl_klt {
   // cosl_klt_group_advance_cams exchanges single cameras' slices between the buffers
   bool lv0Stored[2][64];
   int cur = 1;  // pyr1 == d_pyr[cur]
-  float* d_corn = nullptr;
+  // Two sets of what the front stream of frame n+1 writes while the detector of frame n still reads
+  // it: cornerness map, prelim list and counters.  A frame with a cornerness map switches to the
+  // other set; `par` is the set of the last frame (the one fetch and the debug reads see).
+  int par = 0;
+  float* d_corn[2] = {nullptr, nullptr};
   float4 *d_src = nullptr, *d_dst = nullptr, *d_ping = nullptr, *d_pong = nullptr, *d_res = nullptr;
   float4* d_present = nullptr;
   int* d_nPresent = nullptr;  // [C] lengths of the present lists in d_present
   int* d_nbr = nullptr;
   unsigned long long* d_cand = nullptr;
-  unsigned* d_prelim = nullptr;  // [C][prelimCap] packed (y << 16 | x) of 3x3 local maxima
+  unsigned* d_prelim[2] = {nullptr, nullptr};  // [C][prelimCap] packed (y << 16 | x) of 3x3 local maxima
   int prelimCap = 0;
-  int* d_counters = nullptr;
+  // [C][8]: [0] live tracks, [1] candidates, [2] returned count, [3] raw candidates, [4] prelim
+  // (klt_kernels.cuh).  `stream` zeroes [0..3] of a frame; [4] belongs to the prefilter, which may
+  // count before `stream` gets to the frame, so the front stream zeroes it.
+  int* d_counters[2] = {nullptr, nullptr};
   cosl_klt_feature* d_feat = nullptr;
   // fed points (3 floats each), then their slots and the per-camera placed counts (ints)
   void* d_feedbuf = nullptr;
@@ -123,6 +136,8 @@ static int update_cameras(cosl_klt* g) {
   }
   // pageable source: the copy is staged before the call returns, so hcam may change again
   COSL_CUDA(cudaMemcpyAsync(g->d_cams, g->hcam, sizeof(KltCam) * g->C, cudaMemcpyHostToDevice, g->stream));
+  // the next frame's front pass reads d_cams
+  COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
   return COSL_OK;
 }
 
@@ -146,6 +161,9 @@ static PassFn pass_kernel(const cosl_klt* g) {
 int alloc_group(cosl_klt* g) {
   const int C = g->C, W = g->W, H = g->H, F = g->F;
   COSL_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
+  COSL_CUDA(cudaStreamCreateWithFlags(&g->frontStream, cudaStreamNonBlocking));
+  COSL_CUDA(cudaEventCreateWithFlags(&g->evFence, cudaEventDisableTiming));
+  COSL_CUDA(cudaEventCreateWithFlags(&g->evTail, cudaEventDisableTiming));
   COSL_CUDA(cudaStreamCreateWithFlags(&g->copyStream, cudaStreamNonBlocking));
   COSL_CUDA(cudaEventCreateWithFlags(&g->evFront, cudaEventDisableTiming));
   for (int c = 0; c < C; ++c) COSL_CUDA(cudaEventCreateWithFlags(&g->evImg[c], cudaEventDisableTiming));
@@ -176,7 +194,7 @@ int alloc_group(cosl_klt* g) {
     COSL_CUDA(cudaMalloc(&g->d_pyr[b], sizeof(float4) * g->pyrStride * C));
     COSL_CUDA(cudaMemsetAsync(g->d_pyr[b], 0, sizeof(float4) * g->pyrStride * C, g->stream));
   }
-  COSL_CUDA(cudaMalloc(&g->d_corn, sizeof(float) * (size_t)W * H * C));
+  for (int b = 0; b < 2; ++b) COSL_CUDA(cudaMalloc(&g->d_corn[b], sizeof(float) * (size_t)W * H * C));
   const size_t fbytes = sizeof(float4) * (size_t)F * C;
   float4** bufs[] = {&g->d_src, &g->d_dst, &g->d_ping, &g->d_pong, &g->d_res, &g->d_present};
   std::vector<float4> init((size_t)F * C, make_float4(-1.f, -1.f, 1.f, 0.f));
@@ -187,9 +205,11 @@ int alloc_group(cosl_klt* g) {
   COSL_CUDA(cudaMalloc(&g->d_cand, sizeof(unsigned long long) * (size_t)cap * C));
   // strict 3x3 maxima cannot be 8-adjacent: at most one per 2x2 block
   g->prelimCap = ((W + 1) / 2) * ((H + 1) / 2);
-  COSL_CUDA(cudaMalloc(&g->d_prelim, sizeof(unsigned) * (size_t)g->prelimCap * C));
-  COSL_CUDA(cudaMalloc(&g->d_counters, sizeof(int) * 8 * C));
-  COSL_CUDA(cudaMemset(g->d_counters, 0, sizeof(int) * 8 * C));
+  for (int b = 0; b < 2; ++b) {
+    COSL_CUDA(cudaMalloc(&g->d_prelim[b], sizeof(unsigned) * (size_t)g->prelimCap * C));
+    COSL_CUDA(cudaMalloc(&g->d_counters[b], sizeof(int) * 8 * C));
+    COSL_CUDA(cudaMemset(g->d_counters[b], 0, sizeof(int) * 8 * C));
+  }
   COSL_CUDA(cudaMalloc(&g->d_feat, sizeof(cosl_klt_feature) * (size_t)F * C));
   COSL_CUDA(cudaMallocHost(&g->h_feat, sizeof(cosl_klt_feature) * (size_t)F * C));
   COSL_CUDA(cudaMallocHost(&g->h_counters, sizeof(int) * 8 * C));
@@ -302,7 +322,8 @@ void free_group(cosl_klt* g) {
   cudaFree(g->d_cams);
   cudaFree(g->d_pyr[0]);
   cudaFree(g->d_pyr[1]);
-  cudaFree(g->d_corn);
+  cudaFree(g->d_corn[0]);
+  cudaFree(g->d_corn[1]);
   cudaFree(g->d_src);
   cudaFree(g->d_dst);
   cudaFree(g->d_ping);
@@ -313,13 +334,18 @@ void free_group(cosl_klt* g) {
   cudaFree(g->d_nbr);
   if (g->auxStream) cudaStreamDestroy(g->auxStream);
   if (g->evPre) cudaEventDestroy(g->evPre);
+  if (g->frontStream) cudaStreamDestroy(g->frontStream);
+  if (g->evFence) cudaEventDestroy(g->evFence);
+  if (g->evTail) cudaEventDestroy(g->evTail);
   if (g->copyStream) cudaStreamDestroy(g->copyStream);
   if (g->evFront) cudaEventDestroy(g->evFront);
   for (int c = 0; c < 64; ++c)
     if (g->evImg[c]) cudaEventDestroy(g->evImg[c]);
   cudaFree(g->d_cand);
-  cudaFree(g->d_prelim);
-  cudaFree(g->d_counters);
+  for (int b = 0; b < 2; ++b) {
+    cudaFree(g->d_prelim[b]);
+    cudaFree(g->d_counters[b]);
+  }
   cudaFree(g->d_feat);
   cudaFree(g->d_feedbuf);
   cudaFree(g->d_state);
@@ -338,9 +364,10 @@ void free_group(cosl_klt* g) {
   delete g;
 }
 
-// ---- stages (all asynchronous on g->stream) ----
+// ---- stages (all asynchronous; the streams of each are in run_frame) ----
 
-// camera c's image: hcam[c].W x hcam[c].H bytes, rows `pitch` bytes apart (0: hcam[c].W, pitch_ok)
+// camera c's image: hcam[c].W x hcam[c].H bytes, rows `pitch` bytes apart (0: hcam[c].W, pitch_ok);
+// on the front stream, or for a multi-camera host upload on the copy stream
 int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind kind) {
   if (kind == cudaMemcpyHostToDevice && g->C > 1) {
     // the previous frame's front pass must have consumed d_img before it is overwritten
@@ -360,7 +387,8 @@ int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMem
   }
   for (int c = 0; c < g->C; ++c)
     COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c],
-                                pitch ? pitch : (size_t)g->hcam[c].W, g->hcam[c].W, g->hcam[c].H, kind, g->stream));
+                                pitch ? pitch : (size_t)g->hcam[c].W, g->hcam[c].W, g->hcam[c].H, kind,
+                                g->frontStream));
   return COSL_OK;
 }
 
@@ -372,8 +400,8 @@ static void launch_prefilter(cosl_klt* g, cudaStream_t st) {
   const auto kern = pr == 3 ? (g->mixed ? klt_nm_prefilter<3, true> : klt_nm_prefilter<3, false>)
                   : pr == 2 ? (g->mixed ? klt_nm_prefilter<2, true> : klt_nm_prefilter<2, false>)
                             : (g->mixed ? klt_nm_prefilter<1, true> : klt_nm_prefilter<1, false>);
-  COSL_LAUNCH(kern, gp, 256, 0, st, g->d_corn, g->W, cs, g->d_cams, g->W, g->H, g->d_prelim, g->prelimCap,
-              g->d_counters);
+  COSL_LAUNCH(kern, gp, 256, 0, st, g->d_corn[g->par], g->W, cs, g->d_cams, g->W, g->H, g->d_prelim[g->par],
+              g->prelimCap, g->d_counters[g->par]);
 }
 
 // The tracker's level list: L-1, L-1-levelSkip, ... down to >= 0.  scaled: the 2x2 tracker's
@@ -410,11 +438,13 @@ struct FramePlan {
   bool foldAdvance;     // klt_select_refill also writes the provided set to d_src (the advance copy)
 };
 
-// PyramidWithDerivativesCreator::buildPyramidForGrayscaleImage (v3d_gpupyramid.cpp:366-429)
+// PyramidWithDerivativesCreator::buildPyramidForGrayscaleImage (v3d_gpupyramid.cpp:366-429), on the
+// front stream
 int build_pyramid(cosl_klt* g, const FramePlan& p) {
+  cudaStream_t st = g->frontStream;
   float4* P = g->d_pyr[g->cur];
   for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = p.storeL0;
-  g->timer.begin(g->secPyr, g->stream);
+  g->timer.begin(g->secPyr, st);
   // level 0 + level 1 + (optionally) the detector's cornerness map in one pass over the image
   FrontParams fp;
   fp.img = g->d_img;
@@ -423,7 +453,7 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   fp.pyr = P;
   fp.pyrStride = g->pyrStride;
   fp.lv1Off = g->L > 1 ? g->lvOff[1] : 0;
-  fp.corn = g->d_corn;
+  fp.corn = g->d_corn[g->par];
   fp.cornStride = (long long)g->W * g->H;
   fp.W = g->W;
   fp.H = g->H;
@@ -448,17 +478,17 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
     const int half = (g->C + 1) / 2;
     for (int c0 = 0; c0 < g->C; c0 += half) {
       const int nc = std::min(half, g->C - c0);
-      COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evImg[c0 + nc - 1], 0));
+      COSL_CUDA(cudaStreamWaitEvent(st, g->evImg[c0 + nc - 1], 0));
       fp.camBase = c0;
       dim3 g1(div_up(nWarps, FS_WARPS), nc);
-      COSL_LAUNCH(front, g1, 32 * FS_WARPS, 0, g->stream, fp);
+      COSL_LAUNCH(front, g1, 32 * FS_WARPS, 0, st, fp);
     }
   } else {
     fp.camBase = 0;
     dim3 g0(div_up(nWarps, FS_WARPS), g->C);
-    COSL_LAUNCH(front, g0, 32 * FS_WARPS, 0, g->stream, fp);
+    COSL_LAUNCH(front, g0, 32 * FS_WARPS, 0, st, fp);
   }
-  COSL_CUDA(cudaEventRecord(g->evFront, g->stream));
+  COSL_CUDA(cudaEventRecord(g->evFront, st));
   g->frontRecorded = true;
   if (p.earlyPrefilter) {
     COSL_CUDA(cudaStreamWaitEvent(g->auxStream, g->evFront, 0));
@@ -468,10 +498,10 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh)
   for (int l = 2; l < g->L; ++l) {
     dim3 gl(div_up(g->lvW[l], PT_TW), div_up(g->lvH[l], PT_TH), g->C);
-    COSL_LAUNCH(KLT_SIZED(g, klt_pyr_down_tma), gl, 256, 0, g->stream, g->tmLoad[g->cur][l - 1],
+    COSL_LAUNCH(KLT_SIZED(g, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->cur][l - 1],
                 g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], g->d_cams, l);
   }
-  g->timer.end(g->stream);
+  g->timer.end(st);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
@@ -528,7 +558,8 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
     KltTrackParams Plax = track_params(g, false), Pstrict = track_params(g, true);
     int verBase = g->verBase;
     // the feature table and, when this frame produced a cornerness map, its suppression marks
-    KltTail tail = {g->d_feat, g->d_counters, g->d_corn, (long long)g->W * g->H, g->W, p.wantCorn ? 1 : 0};
+    KltTail tail = {g->d_feat, g->d_counters[g->par], g->d_corn[g->par], (long long)g->W * g->H, g->W,
+                    p.wantCorn ? 1 : 0};
     void* args[] = {(void*)&P0,          (void*)&P1,       (void*)&pyrStride,  (void*)&LV,
                     (void*)&g->d_cams,   (void*)&nIter,    (void*)&g->d_src,   (void*)&g->d_state,
                     (void*)&g->d_ver,    (void*)&g->d_waitset, (void*)&g->d_res, (void*)&C,
@@ -613,14 +644,16 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
 int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
   g->timer.begin(g->secDetect, g->stream);
   const long long cs = (long long)g->W * g->H;
+  float* corn = g->d_corn[g->par];
+  int* counters = g->d_counters[g->par];
   if (mode == 1 && !p.trackerTail) {
     dim3 gs(div_up(g->F, 256), g->C);
     COSL_LAUNCH(KLT_SIZED(g, klt_suppress), gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F,
-                g->d_corn, g->W, cs, g->d_cams, g->W, g->H);
+                corn, g->W, cs, g->d_cams, g->W, g->H);
   } else if (mode == 0 && maxPresent > 0) {
     dim3 gs(div_up(maxPresent, 256), g->C);
     COSL_LAUNCH(KLT_SIZED(g, klt_suppress), gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F,
-                g->d_corn, g->W, cs, g->d_cams, g->W, g->H);
+                corn, g->W, cs, g->d_cams, g->W, g->H);
   }
   const int r = std::max(1, g->cfg.minDistance);
   if (p.earlyPrefilter)
@@ -628,12 +661,12 @@ int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
   else
     launch_prefilter(g, g->stream);
   dim3 gv(2 * g->numSM, g->C);
-  COSL_LAUNCH(KLT_SIZED(g, klt_nm_verify), gv, 256, 0, g->stream, g->d_corn, g->W, cs, g->d_cams, g->W, g->H, r,
-              g->d_prelim, g->prelimCap, g->d_cand, g->candCap, g->d_counters);
+  COSL_LAUNCH(KLT_SIZED(g, klt_nm_verify), gv, 256, 0, g->stream, corn, g->W, cs, g->d_cams, g->W, g->H, r,
+              g->d_prelim[g->par], g->prelimCap, g->d_cand, g->candCap, counters);
   g->timer.end(g->stream);
   g->timer.begin(g->secSelect, g->stream);
   COSL_LAUNCH(KLT_SIZED(g, klt_select_refill), g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
-              g->d_cand, g->candCap, g->plCap, g->d_counters, g->d_feat, g->d_dst,
+              g->d_cand, g->candCap, g->plCap, counters, g->d_feat, g->d_dst,
               p.foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
               maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, g->d_cams, g->W, g->H, mode,
               g->cfg.trackWithGain ? 1 : 0, g->smemKeys, (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
@@ -645,7 +678,7 @@ int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
 int fetch_results(cosl_klt* g) {
   COSL_CUDA(cudaMemcpyAsync(g->h_feat, g->d_feat, sizeof(cosl_klt_feature) * (size_t)g->F * g->C,
                             cudaMemcpyDeviceToHost, g->stream));
-  COSL_CUDA(cudaMemcpyAsync(g->h_counters, g->d_counters, sizeof(int) * 8 * g->C,
+  COSL_CUDA(cudaMemcpyAsync(g->h_counters, g->d_counters[g->par], sizeof(int) * 8 * g->C,
                             cudaMemcpyDeviceToHost, g->stream));
   COSL_CUDA(cudaStreamSynchronize(g->stream));
   return COSL_OK;
@@ -673,6 +706,8 @@ int advance_cams(cosl_klt* g, const uint8_t* cams) {
   dim3 grid((unsigned)std::min<long long>(div_up64(g->pyrStride, 256), 2 * g->numSM), L.n);
   COSL_LAUNCH(klt_advance_cams, grid, 256, 0, g->stream, g->d_pyr[0], g->d_pyr[1], g->pyrStride, g->d_dst,
               g->d_src, g->F, L);
+  // the next frame's front pass overwrites one of the two exchanged buffers
+  COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
   for (int k = 0; k < L.n; ++k) std::swap(g->lv0Stored[0][L.cam[k]], g->lv0Stored[1][L.cam[k]]);
   return COSL_OK;
 }
@@ -750,12 +785,27 @@ enum FrameKind {
   FRAME_REDETECT,  // redetect, next, next_dev, submit: as FRAME_TRACK, then the detector refills
 };
 
-// One frame through its stages, all asynchronous on g->stream.  This is the one place that decides
-// which launches the frame folds together.  maxPresent: the longest present list of a detect
-// (upload_present).  foldAdvance (detector kinds): advanceFrame follows the frame, and
-// klt_select_refill writes the provided set to both feature buffers, so the advance is the pyramid
-// flip alone.  Nothing of the plan outlives the call.
-int run_frame(cosl_klt* g, FrameKind kind, int maxPresent, bool foldAdvance) {
+// One frame through its stages, asynchronous on g->stream and, joined into it before the call
+// returns, the front stream (image copies, klt_front, pyramid tail) and auxStream (the early
+// prefilter).  This is the one place that decides how a frame is scheduled and which launches it
+// folds together.  imgs, pitch, copyKind: the frame's images (upload_images).  maxPresent: the
+// longest present list of a detect (upload_present).  foldAdvance (detector kinds): advanceFrame
+// follows the frame, and klt_select_refill writes the provided set to both feature buffers, so the
+// advance is the pyramid flip alone.  Nothing of the plan outlives the call.
+//
+// Frame n+1's image copies wait only for frame n's front pass; its front pass and pyramid tail wait
+// for evFence, which frame n records right after its tracker, so they run next to frame n's
+// klt_nm_verify and klt_select_refill.  What the front stream writes and who else touches it:
+//   d_img                    read by the front passes only (same stream; copy stream: evFront)
+//   d_pyr[cur]               frame n+1 builds into frame n's P0, whose last reader is frame n's
+//                            tracker: the fence
+//   d_corn, d_prelim,        frame n's tracker marks, klt_suppress, verify and select use set `par`;
+//   d_counters[.][8c + 4]    frame n+1 (a frame with a cornerness map) switches to the other set,
+//                            whose last users are frame n-1's, ahead of the fence
+// and it reads d_cams, which update_cameras rewrites on g->stream (it records the fence after);
+// klt_advance_cams also exchanges pyramid slices on g->stream and records the fence after.
+int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind,
+              int maxPresent, bool foldAdvance) {
   FramePlan p;
   p.wantCorn = kind != FRAME_TRACK;
   // A re-detect frame has its cornerness fused into the front pass, so nothing but a tracker that
@@ -765,15 +815,25 @@ int run_frame(cosl_klt* g, FrameKind kind, int maxPresent, bool foldAdvance) {
   p.earlyPrefilter = kind == FRAME_REDETECT;
   p.trackerTail = fused_tracker(g);
   p.foldAdvance = foldAdvance;
-  // zeroed first on every kind: the early prefilter counts into them, and a detect frame launches
-  // nothing that reads them before its detector
-  COSL_CUDA(cudaMemsetAsync(g->d_counters, 0, sizeof(int) * 8 * g->C, g->stream));
+  if (p.wantCorn) g->par ^= 1;
+  int* counters = g->d_counters[g->par];
+  // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below
+  COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
+  // the images ahead of the fence: d_img is read by the front passes alone, so they run under the
+  // previous frame's tracker
+  COSL_TRY(upload_images(g, imgs, pitch, copyKind));
+  COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evFence, 0));
+  if (p.wantCorn)
+    COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
   COSL_TRY(build_pyramid(g, p));
+  COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
+  COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
   if (kind != FRAME_DETECT) {
     COSL_TRY(run_tracker(g, p));
+    COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
     if (!p.trackerTail) {
       dim3 grid(div_up(g->F, 256), g->C);
-      COSL_LAUNCH(klt_status, grid, 256, 0, g->stream, g->d_res, g->d_feat, g->d_counters, g->F);
+      COSL_LAUNCH(klt_status, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F);
     }
   }
   if (kind == FRAME_TRACK) {
@@ -783,6 +843,7 @@ int run_frame(cosl_klt* g, FrameKind kind, int maxPresent, bool foldAdvance) {
   } else {
     COSL_TRY(run_detector(g, kind == FRAME_REDETECT ? 1 : 0, maxPresent, p));
   }
+  if (kind == FRAME_DETECT) COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
   if (foldAdvance) g->cur = 1 - g->cur;
   return COSL_OK;
 }
@@ -925,8 +986,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   int maxPresent = 0;
   COSL_TRY(upload_present(h, &nPresent, &present3, &maxPresent));
   const uint8_t* imgs[1] = {img};
-  COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(run_frame(h, FRAME_DETECT, maxPresent, false));
+  COSL_TRY(run_frame(h, FRAME_DETECT, imgs, pitch, cudaMemcpyHostToDevice, maxPresent, false));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, &dest, nDetected);
   return COSL_OK;
@@ -938,8 +998,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
   if (!img || !dest || !nNewFeatures || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_redetect: bad argument");
   const uint8_t* imgs[1] = {img};
-  COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(run_frame(h, FRAME_REDETECT, 0, false));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, false));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, &dest, nNewFeatures);
   return COSL_OK;
@@ -951,8 +1010,7 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
   if (!img || !dest || !nPresent || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_track: bad argument");
   const uint8_t* imgs[1] = {img};
-  COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(run_frame(h, FRAME_TRACK, 0, false));
+  COSL_TRY(run_frame(h, FRAME_TRACK, imgs, pitch, cudaMemcpyHostToDevice, 0, false));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, &dest, nullptr);
   *nPresent = h->h_counters[0];
@@ -999,8 +1057,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
                        const float* const* present3, cosl_klt_feature* const* dest, int* nDetected) {
   int maxPresent = 0;
   if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
-  COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(run_frame(h, FRAME_DETECT, maxPresent, true));
+  COSL_TRY(run_frame(h, FRAME_DETECT, imgs, pitch, cudaMemcpyHostToDevice, maxPresent, true));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, dest, nDetected);
   return COSL_OK;
@@ -1050,8 +1107,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                         cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
-  COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(run_frame(h, FRAME_REDETECT, 0, true));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, dest, nNew);
   return COSL_OK;
@@ -1061,8 +1117,7 @@ int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pit
   KLT_ENTER(h)
   if (!dimgs || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "group_next_dev: bad argument");
-  COSL_TRY(upload_images(h, dimgs, pitch, cudaMemcpyDeviceToDevice));
-  return run_frame(h, FRAME_REDETECT, 0, true);
+  return run_frame(h, FRAME_REDETECT, dimgs, pitch, cudaMemcpyDeviceToDevice, 0, true);
 }
 
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {
@@ -1076,7 +1131,8 @@ int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) 
 // n + 1, its kernels and the D2H copy of its feature table and returns; collect() waits for the OLDEST
 // submitted frame.  With submit(n+1) called before collect(n), the image upload of frame n + 1 runs on
 // the copy stream under the tracker / detector kernels of frame n (it only waits for frame n's front
-// pass, which is the last reader of the image buffer).
+// pass, which is the last reader of the image buffer), and its pyramid under frame n's detector
+// (run_frame).
 int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch) {
   KLT_ENTER(h)
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_submit: bad argument");
@@ -1087,12 +1143,11 @@ int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch)
     COSL_CUDA(cudaMallocHost(&h->h_cntQ[slot], sizeof(int) * 8 * h->C));
     COSL_CUDA(cudaEventCreateWithFlags(&h->evDone[slot], cudaEventDisableTiming));
   }
-  COSL_TRY(upload_images(h, imgs, pitch, cudaMemcpyHostToDevice));
-  COSL_TRY(run_frame(h, FRAME_REDETECT, 0, true));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
   COSL_CUDA(cudaMemcpyAsync(h->h_featQ[slot], h->d_feat, sizeof(cosl_klt_feature) * (size_t)h->F * h->C,
                             cudaMemcpyDeviceToHost, h->stream));
-  COSL_CUDA(cudaMemcpyAsync(h->h_cntQ[slot], h->d_counters, sizeof(int) * 8 * h->C, cudaMemcpyDeviceToHost,
-                            h->stream));
+  COSL_CUDA(cudaMemcpyAsync(h->h_cntQ[slot], h->d_counters[h->par], sizeof(int) * 8 * h->C,
+                            cudaMemcpyDeviceToHost, h->stream));
   COSL_CUDA(cudaEventRecord(h->evDone[slot], h->stream));
   ++h->subSeq;
   ++h->nInFlight;
@@ -1148,7 +1203,7 @@ int cosl_klt_debug_cornerness(cosl_klt* h, int cam, float* out) {
   KLT_ENTER(h)
   if (cam < 0 || cam >= h->C || !out) return set_error(COSL_E_INVALID, "debug_cornerness");
   COSL_CUDA(cudaStreamSynchronize(h->stream));
-  COSL_CUDA(cudaMemcpy2D(out, sizeof(float) * h->hcam[cam].W, h->d_corn + (size_t)cam * h->W * h->H,
+  COSL_CUDA(cudaMemcpy2D(out, sizeof(float) * h->hcam[cam].W, h->d_corn[h->par] + (size_t)cam * h->W * h->H,
                          sizeof(float) * h->W, sizeof(float) * h->hcam[cam].W, h->hcam[cam].H,
                          cudaMemcpyDeviceToHost));
   return COSL_OK;

@@ -153,7 +153,11 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
 /* Same, but images already resident in device memory (dimgs[c] = device pointers, tightly packed
  * rows of `pitch` bytes) and the feature table left on the device: no host transfer, no
  * synchronise; used for the kernel-only throughput number.  Results can be fetched later with
- * cosl_klt_group_fetch. */
+ * cosl_klt_group_fetch.
+ * The device images must hold the frame when the call is made, as the host images of next() and
+ * submit() do: the group copies them on a stream of its own that runs ahead of the group's stream
+ * (cosl_klt_stream) and is NOT ordered after work the caller enqueued there since the previous call.
+ * They must stay unchanged until work enqueued on the group's stream after this call has run. */
 int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pitch);
 int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                          cosl_klt_feature* const* dest, int* nDetected);
@@ -195,7 +199,9 @@ int cosl_klt_group_first_present(cosl_klt* h, const uint8_t* const* imgs, size_t
  * buffers of a submitted frame must stay untouched until that frame has been collected. */
 int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch);
 int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew);
-/* CUDA stream (cudaStream_t as void*) the group launches on; lets callers time with events. */
+/* CUDA stream (cudaStream_t as void*) the group launches on; lets callers time with events.  Parts of
+ * a frame run on side streams, but every call joins them into this stream before it returns: work
+ * enqueued here after a call sees the whole frame. */
 void* cosl_klt_stream(cosl_klt* h);
 
 /* Test/inspection hooks (not part of the reference surface). */

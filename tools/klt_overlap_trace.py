@@ -1,0 +1,94 @@
+"""torch.profiler trace of back-to-back KLT frames (bench.py's c3 workload, frames resident in HBM).
+
+  python tools/klt_overlap_trace.py OUT_DIR [--frames 20]
+
+Writes OUT_DIR/klt_next_dev.json (Chrome trace) and prints, per frame pair, whether frame n+1's
+klt_front overlaps frame n's klt_nm_verify / klt_select_refill, the device time per frame, and the host
+time to enqueue one cosl_klt_group_next_dev call (measured without the profiler).  The host must
+enqueue a frame faster than the device runs it, or the queue drains and the overlap is lost."""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import bench  # noqa: E402
+from coslam_b200 import api  # noqa: E402
+
+
+def kernels(trace, name):
+    return sorted((e["ts"], e["ts"] + e["dur"]) for e in trace["traceEvents"]
+                  if e.get("cat") == "kernel" and name in e.get("name", ""))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("out")
+    ap.add_argument("--frames", type=int, default=20)
+    args = ap.parse_args()
+    os.makedirs(args.out, exist_ok=True)
+    C, W, H = bench.KLT_C, bench.KLT_W, bench.KLT_H
+    seqs = bench.make_sequences(0)
+    grp = api.KltGroup(bench.klt_cfg(), C, W, H, bench.KLT_L, bench.KLT_FW, bench.KLT_FH)
+    stream = torch.cuda.ExternalStream(grp.stream())
+    dev = [[torch.from_numpy(seqs[c].frames[k]).cuda() for c in range(C)] for k in range(bench.KLT_FRAMES)]
+    ptrs = [[t.data_ptr() for t in row] for row in dev]
+    torch.cuda.synchronize()
+    grp.first([seqs[c].frames[0] for c in range(C)])
+    fidx = seqs[0].frame_index
+    i = 1
+
+    def run(n, host_times=None):
+        nonlocal i
+        for _ in range(n):
+            t0 = time.perf_counter()
+            grp.next_dev(ptrs[fidx(i)], W)
+            if host_times is not None:
+                host_times.append(time.perf_counter() - t0)
+            i += 1
+
+    run(10)
+    grp.sync()
+    # device time per frame, profiler off
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    run(200)
+    e1.record(stream)
+    grp.sync()
+    dev_ms = e0.elapsed_time(e1) / 200
+    # host enqueue time, in bursts of 8 calls from an idle queue: in a long run the host gets ahead of
+    # the device until the launch queue is full, and from then on each call waits for a frame to finish
+    host = []
+    for _ in range(25):
+        run(8, host)
+        grp.sync()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU,
+                                            torch.profiler.ProfilerActivity.CUDA]) as prof:
+        run(args.frames)
+        grp.sync()
+    path = os.path.join(args.out, "klt_next_dev.json")
+    prof.export_chrome_trace(path)
+    trace = json.load(open(path))
+    front, verify, select = (kernels(trace, k) for k in ("klt_front", "klt_nm_verify", "klt_select_refill"))
+    n = min(len(front), len(verify), len(select))
+    overl = 0
+    for k in range(n - 1):
+        f0, f1 = front[k + 1]
+        ov = any(f0 < b and a < f1 for a, b in (verify[k], select[k]))
+        overl += ov
+    print(json.dumps({
+        "gpu": bench.gpu_identity(torch.cuda.current_device()),
+        "frames_traced": n,
+        "front_overlaps_previous_detector": f"{overl} of {n - 1} frame pairs",
+        "device_ms_per_frame": dev_ms,
+        "host_enqueue_ms_per_call": {"median": 1e3 * float(np.median(host)), "p90": 1e3 * float(np.percentile(host, 90))},
+        "trace": path}))
+    grp.close()
+
+
+if __name__ == "__main__":
+    main()
