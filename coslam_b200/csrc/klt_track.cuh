@@ -2,10 +2,13 @@
 // v3d_gpuklt.cpp:205-305) for sm_90a.
 //
 // Mapping: one QUARTER-WARP (KLT_G = 8 lanes) per feature slot, four slots per warp.  The (2hw+1)^2
-// window pixels are spread over the 8 lanes in ROUNDS rounds (49 pixels -> 7 rounds, 87.5 % lane
-// use), the running sums are reduced with width-8 butterfly shuffles and every lane solves the 3x3
-// system in closed form (adjugate), so control flow is uniform.  The per-pass overhead (neighbour
-// wait, reduction, solve, publish) is paid once per warp, i.e. shared by four slots.
+// window pixels are spread over the 8 lanes in ROUNDS rounds: for the live hw = 3, lane gl < 7 owns
+// window column gl and walks its 7 rows (lane 7 idles, 87.5 % lane use), so the horizontal stage of
+// the bilinear sample is shared by two vertically adjacent pixels; for any other width the pixels
+// p = gl + 8r are taken in row-major order.  The running sums are reduced with width-8 butterfly
+// shuffles and every lane solves the 3x3 system in closed form (adjugate), so control flow is
+// uniform.  The per-pass overhead (neighbour wait, reduction, solve, publish) is paid once per
+// warp, i.e. shared by four slots.
 //
 // Window sampling.  The window samples of a level are one texel apart (ds = 1 / w_level), so all
 // (2hw+1)^2 bilinear taps of a window share the fractional offsets of the window centre and their
@@ -24,8 +27,7 @@
 //       12x12-texel tile of the current-frame pyramid around the feature is staged in shared memory
 //       (clamped 128-bit loads; TMA box loads cannot reproduce CLAMP_TO_EDGE, and at the coarse
 //       levels most windows straddle the border) -- the iterations then sample from shared memory;
-//       if a window drifts out of its tile the pass falls back to clamped global loads (same
-//       values, same arithmetic);
+//       a window that drifts out of its tile gets the tile re-centred on it;
 //     * the only coupling between slots, the gain-smoothness term that reads beta of <= 8
 //       neighbour slots from the PREVIOUS pass, is synchronised without grid barriers and without
 //       fences: each slot publishes (pass number, beta) as ONE naturally atomic 8-byte word into a
@@ -41,10 +43,11 @@
 namespace coslam {
 
 constexpr int KLT_TW = 12;      // staged I1 tile side (texels): 2*hw + 2 + 2*margin with hw = 3
-// Row pitch of the tile in shared memory.  A lane group reads 8 consecutive window pixels
-// p = 7*py + px per LDS.128, i.e. float4 index p + py*(pitch - 7); with pitch = 15 that is
-// p (mod 8), so the 8 lanes of a quarter-warp hit 8 distinct 16-byte bank groups (pitch 12 gave
-// 2-way conflicts on every tap).
+// Row pitch of the tile in shared memory.  On the hw = 3 path the lanes of a group read 7
+// consecutive texels of one tile row per LDS.128, which is conflict-free at any pitch.  The
+// any-width path reads 8 consecutive window pixels in row-major order per LDS.128; for a 7-wide
+// window (p = 7*py + px) that is float4 index p + py*(pitch - 7), which pitch 15 makes p (mod 8):
+// the 8 lanes of a quarter-warp hit 8 distinct 16-byte bank groups (pitch 12 gave 2-way conflicts).
 constexpr int KLT_TP = 15;
 constexpr int KLT_G = 8;        // lanes per feature slot
 constexpr int KLT_ROUNDS = 7;   // window pixels per lane on the fast path (<= 56 pixels)
@@ -92,13 +95,20 @@ __device__ __forceinline__ float lerp1(float p0, float p1, float a) {
   return __fmaf_rn(a, __fsub_rn(p1, p0), p0);
 }
 
+// The two stages of the bilinear sample: along a tap row, then between two tap rows.  The hw = 3
+// window walks share one horizontal stage between the two pixels above and below a tap row; every
+// sample is still lerp1(lerp1(p00, p10, ax), lerp1(p01, p11, ax), ay), bit for bit.
+__device__ __forceinline__ float3 klt_hlerp(const float4 p0, const float4 p1, float ax) {
+  return make_float3(lerp1(p0.x, p1.x, ax), lerp1(p0.y, p1.y, ax), lerp1(p0.z, p1.z, ax));
+}
+
+__device__ __forceinline__ float3 klt_vlerp(const float3 h0, const float3 h1, float ay) {
+  return make_float3(lerp1(h0.x, h1.x, ay), lerp1(h0.y, h1.y, ay), lerp1(h0.z, h1.z, ay));
+}
+
 __device__ __forceinline__ float3 klt_lerp4(const float4 p00, const float4 p10, const float4 p01,
                                             const float4 p11, float ax, float ay) {
-  float3 r;
-  r.x = lerp1(lerp1(p00.x, p10.x, ax), lerp1(p01.x, p11.x, ax), ay);
-  r.y = lerp1(lerp1(p00.y, p10.y, ax), lerp1(p01.y, p11.y, ax), ay);
-  r.z = lerp1(lerp1(p00.z, p10.z, ax), lerp1(p01.z, p11.z, ax), ay);
-  return r;
+  return klt_vlerp(klt_hlerp(p00, p10, ax), klt_hlerp(p01, p11, ax), ay);
 }
 
 // tap (xi, yi) of a level (rows `pitch` texels apart) with clamp-to-edge at the camera's w x h,
@@ -253,9 +263,45 @@ __device__ __forceinline__ float klt_nbterm(float bn, float beta, int gl, int gr
 
 // Both gain-tracker drivers are instantiated for a window half-width known at compile time (HWC,
 // the live CoSLAM setting hw = 3) and for any width (HWC = 0: P.halfWidth at run time).  With the
-// width fixed, the window size, the pixel guards and the fast-path test fold to constants; the
-// arithmetic is the same in both instantiations.
+// width fixed, the window size, the pixel guards and the fast-path test fold to constants, and the
+// window is walked column per lane (see the top of the file); the arithmetic of a pixel is the same
+// in both instantiations.  Every path of both drivers walks a window in the same lane assignment
+// and order, so that their sums round alike.
 constexpr int KLT_HW_LIVE = 3;
+static_assert(2 * KLT_HW_LIVE + 1 <= KLT_G && 2 * KLT_HW_LIVE + 1 <= KLT_ROUNDS,
+              "hw = 3 walk: one window column per lane, one row per round");
+
+// A window walked with clamped global loads (the per-pass kernel; the fused kernel's items without
+// a tile): adds every pixel to A and returns this lane's sum of klt_d2_term, in the lane
+// assignment and order of the tile path
+template <int HWC>
+__device__ __forceinline__ float klt_window_global(KltAcc& A, const float4* __restrict__ L0,
+                                                   const float4* __restrict__ L1, int pitch, int w, int h,
+                                                   const KltCentre c0, const KltCentre c1, int gl, int hw,
+                                                   float beta, float halfW, float halfH, float lambda,
+                                                   float delta) {
+  const int fwid = 2 * hw + 1, npx = fwid * fwid;
+  float d2 = 0.f;
+  auto pixel = [&](int px, int py) {
+    const int dx = px - hw, dy = py - hw;
+    const float3 I0 = klt_fetch_global(L0, pitch, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
+    const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
+    d2 = __fadd_rn(d2, klt_d2_term(I0, lambda, delta));
+    klt_acc_pixel(A, I0, I1, beta, halfW, halfH, lambda);
+  };
+  if constexpr (HWC == KLT_HW_LIVE) {
+    // a trip count known only at run time, like the any-width loop: fully unrolled, the loads of
+    // 7 rows in flight push the fused kernel past its register budget
+    const int rows = gl < fwid ? fwid : 0;
+    for (int py = 0; py < rows; ++py) pixel(gl, py);
+  } else {
+    for (int p = gl; p < npx; p += KLT_G) {
+      const int py = p / fwid;
+      pixel(p - py * fwid, py);
+    }
+  }
+  return d2;
+}
 
 // ------------------------------------------------------------------------------------------
 // One pass per launch (diagnostic / fallback).  Grid: x = ceil(F / 32) blocks of 256 threads
@@ -290,15 +336,8 @@ klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
   const KltCentre c0 = klt_centre(w, h, x0.x, x0.y);
   const KltCentre c1 = klt_centre(w, h, cur.x, cur.y);
   KltAcc A = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  float d2 = 0.f;
-  for (int p = gl; p < npx; p += KLT_G) {
-    const int py = p / fwid, px = p - py * fwid;
-    const int dx = px - hw, dy = py - hw;
-    const float3 I0 = klt_fetch_global(L0, pitch, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
-    const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
-    d2 = __fadd_rn(d2, klt_d2_term(I0, P.lambda, P.delta));
-    klt_acc_pixel(A, I0, I1, beta, halfW, halfH, P.lambda);
-  }
+  const float d2 = klt_window_global<HWC>(A, L0, L1, pitch, w, h, c0, c1, gl, hw, beta, halfW, halfH,
+                                          P.lambda, P.delta);
   // the host chose P per pass: its validRegion is the strict or the lax one as P.strict says
   float4 res = klt_gain_finish(A, grp_sum(d2), nbterm, (float)npx, cur.x, cur.y, beta,
                                klt_finish_params<MIXED>(P, P, P.strict != 0, Wc, Hc));
@@ -509,16 +548,34 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
           __syncwarp();
           // I0r is written on every path (a dead slot never reads it), so the previous level's
           // samples are not live across the loads above
+          if constexpr (HWC == KLT_HW_LIVE) {
+            // I0r[r] = pixel (gl, r): lane gl walks column gl of the 8x8 block, one tap row per row
+            if (!pre_invalid && gl < fwid) {
+              const float4* t4 = tile + I0B + gl;
+              float3 hp = klt_hlerp(t4[0], t4[1], c0.ax);
 #pragma unroll
-          for (int r = 0; r < KLT_ROUNDS; ++r) {
-            const int p = gl + KLT_G * r;
-            if (!pre_invalid && p < npx) {
-              const int py = p / fwid, px = p - py * fwid;
-              const float4* t4 = tile + I0B + py * 8 + px;
-              I0r[r] = klt_lerp4(t4[0], t4[1], t4[8], t4[9], c0.ax, c0.ay);
-              d2 = __fadd_rn(d2, klt_d2_term(I0r[r], Plax.lambda, Plax.delta));
+              for (int r = 0; r < KLT_ROUNDS; ++r) {
+                const float3 hn = klt_hlerp(t4[8 * (r + 1)], t4[8 * (r + 1) + 1], c0.ax);
+                I0r[r] = klt_vlerp(hp, hn, c0.ay);
+                d2 = __fadd_rn(d2, klt_d2_term(I0r[r], Plax.lambda, Plax.delta));
+                hp = hn;
+              }
             } else {
-              I0r[r] = make_float3(0.f, 0.f, 0.f);
+#pragma unroll
+              for (int r = 0; r < KLT_ROUNDS; ++r) I0r[r] = make_float3(0.f, 0.f, 0.f);
+            }
+          } else {
+#pragma unroll
+            for (int r = 0; r < KLT_ROUNDS; ++r) {
+              const int p = gl + KLT_G * r;
+              if (!pre_invalid && p < npx) {
+                const int py = p / fwid, px = p - py * fwid;
+                const float4* t4 = tile + I0B + py * 8 + px;
+                I0r[r] = klt_lerp4(t4[0], t4[1], t4[8], t4[9], c0.ax, c0.ay);
+                d2 = __fadd_rn(d2, klt_d2_term(I0r[r], Plax.lambda, Plax.delta));
+              } else {
+                I0r[r] = make_float3(0.f, 0.f, 0.f);
+              }
             }
           }
           __syncwarp();
@@ -548,12 +605,11 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         // tile[b * KLT_TP + a] == level[clamp(ty0 + b)][clamp(tx0 + a)]: indexing with the
         // unclamped tap coordinates reproduces the clamped fetches exactly
         int a0 = c1.xi - tx0, b0 = c1.yi - ty0;
-        bool inTile = staged && (a0 - hw >= 0) && (a0 + hw + 1 < KLT_TW) && (b0 - hw >= 0) &&
-                      (b0 + hw + 1 < KLT_TW);
         // A window that drifted out of its tile gets the tile re-centred (two batches of loads)
         // rather than paying clamped global loads for the rest of the level; the slow warp would
         // otherwise hold up every slot that waits on it.
         if (staged && it != 1) {
+          const bool inTile = (a0 - hw >= 0) && (a0 + hw + 1 < KLT_TW) && (b0 - hw >= 0) && (b0 + hw + 1 < KLT_TW);
           const bool need = !pre_invalid && !inTile;
           if (__any_sync(0xffffffffu, need)) {
             if (need) {
@@ -577,15 +633,47 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                   tile[b * KLT_TP + a] = tv[u];
                 }
               }
-              a0 = c1.xi - tx0;
+              a0 = c1.xi - tx0;  // the window now lies in the tile: 2 * hw + 2 + 2 <= KLT_TW when staged
               b0 = c1.yi - ty0;
-              inTile = true;  // 2 * hw + 2 + 2 <= KLT_TW on the staged path
             }
             __syncwarp();
           }
         }
         if (!pre_invalid) {
-          if (inTile) {
+          // a staged window is in its tile here: the tile was staged around it on the first
+          // iteration of the level or re-centred on it above
+          if (staged && HWC == KLT_HW_LIVE) {
+            // lane gl < 7: window column gl.  Tap row j (taps (gl, j) and (gl + 1, j): 7 lanes read
+            // 8 consecutive texels of one tile row) is interpolated along x once and serves the
+            // pixels of rows j - 1 and j: 16 LDS.128 and 45 lerps per lane for 7 pixels
+            const float4* tc = tile + (b0 - hw) * KLT_TP + (a0 - hw) + gl;
+            const bool col = gl < fwid;
+            constexpr int JP = 5;  // tap rows 0..4 (pixel rows 0..3), the record poll, tap rows 5..7
+            float3 hp;
+            if (col) {
+              hp = klt_hlerp(tc[0], tc[1], c1.ax);
+#pragma unroll
+              for (int j = 1; j < JP; ++j) {
+                const float3 hn = klt_hlerp(tc[j * KLT_TP], tc[j * KLT_TP + 1], c1.ax);
+                klt_acc_pixel(A, I0r[j - 1], klt_vlerp(hp, hn, c1.ay), beta, halfW, halfH, Plax.lambda);
+                hp = hn;
+              }
+            }
+            if (pass > 1 && active) {
+              // early, non-binding look at the records: usually published by now, and the L2
+              // round trip overlaps the rest of the window
+              va = ld_hint_u64(ra);
+              vb = ld_hint_u64(rb);
+            }
+            if (col) {
+#pragma unroll
+              for (int j = JP; j <= 2 * KLT_HW_LIVE + 1; ++j) {
+                const float3 hn = klt_hlerp(tc[j * KLT_TP], tc[j * KLT_TP + 1], c1.ax);
+                klt_acc_pixel(A, I0r[j - 1], klt_vlerp(hp, hn, c1.ay), beta, halfW, halfH, Plax.lambda);
+                hp = hn;
+              }
+            }
+          } else if (staged) {
             const float4* tc = tile + b0 * KLT_TP + a0;
             // the tap offsets of this lane are recomputed every pass: held across the passes,
             // they do not fit the register budget of 4 CTAs per SM
@@ -605,36 +693,12 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                 klt_acc_pixel(A, I0r[r], I1, beta, halfW, halfH, Plax.lambda);
               }
             }
-          } else if (staged) {
-            const float4* L1 = pyr1 + (size_t)cam * pyrStride + LV.off[li];
-#pragma unroll 1
-            for (int r = 0; r < KLT_ROUNDS; ++r) {
-              const int p = gl + KLT_G * r;
-              if (p < npx) {
-                const int py = p / fwid, px = p - py * fwid;
-                const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + px - hw, c1.yi + py - hw, c1.ax, c1.ay);
-                // I0r is indexed dynamically only on this rare path
-                float3 I0 = I0r[0];
-#pragma unroll
-                for (int k = 1; k < KLT_ROUNDS; ++k)
-                  if (r == k) I0 = I0r[k];
-                klt_acc_pixel(A, I0, I1, beta, halfW, halfH, Plax.lambda);
-              }
-            }
           } else {
             const float4* L0 = pyr0 + (size_t)cam * pyrStride + LV.off[li];
             const float4* L1 = pyr1 + (size_t)cam * pyrStride + LV.off[li];
             const KltCentre c0 = klt_centre(w, h, x0.x, x0.y);
-            float d2 = 0.f;
-            for (int p = gl; p < npx; p += KLT_G) {
-              const int py = p / fwid, px = p - py * fwid;
-              const int dx = px - hw, dy = py - hw;
-              const float3 I0 = klt_fetch_global(L0, pitch, w, h, c0.xi + dx, c0.yi + dy, c0.ax, c0.ay);
-              const float3 I1 = klt_fetch_global(L1, pitch, w, h, c1.xi + dx, c1.yi + dy, c1.ax, c1.ay);
-              d2 = __fadd_rn(d2, klt_d2_term(I0, Plax.lambda, Plax.delta));
-              klt_acc_pixel(A, I0, I1, beta, halfW, halfH, Plax.lambda);
-            }
-            f = d2;
+            f = klt_window_global<HWC>(A, L0, L1, pitch, w, h, c0, c1, gl, hw, beta, halfW, halfH,
+                                       Plax.lambda, Plax.delta);
           }
         }
         KLT_CLK(c3k);
