@@ -40,6 +40,28 @@ extern std::atomic<uint64_t> g_launches;
     coslam::g_launches.fetch_add(1, std::memory_order_relaxed);          \
   } while (0)
 
+// COSL_LAUNCH as a programmatic dependent launch: the kernel may be scheduled as soon as every CTA
+// of the kernel before it on stream `strm` has executed griddepcontrol.launch_dependents or exited,
+// so its launch and prologue overlap that kernel's drain.  The kernel must execute griddepcontrol.wait
+// (it returns once the earlier grid has completed and its memory is visible) before it touches
+// anything that grid or the work ahead of it on `strm` writes or reads.  Returns from the
+// enclosing function on a launch error.
+#define COSL_LAUNCH_PDL(kernel, grid, block, smem, strm, ...)                      \
+  do {                                                                             \
+    cudaLaunchAttribute _attr[1];                                                  \
+    _attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;              \
+    _attr[0].val.programmaticStreamSerializationAllowed = 1;                       \
+    cudaLaunchConfig_t _cfg = {};                                                  \
+    _cfg.gridDim = (grid);                                                         \
+    _cfg.blockDim = (block);                                                       \
+    _cfg.dynamicSmemBytes = (smem);                                                \
+    _cfg.stream = (strm);                                                          \
+    _cfg.attrs = _attr;                                                            \
+    _cfg.numAttrs = 1;                                                             \
+    coslam::g_launches.fetch_add(1, std::memory_order_relaxed);                    \
+    COSL_CUDA(cudaLaunchKernelEx(&_cfg, kernel, __VA_ARGS__));                     \
+  } while (0)
+
 inline int div_up(int a, int b) { return (a + b - 1) / b; }
 inline int64_t div_up64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -495,11 +495,15 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
     launch_prefilter(g, g->auxStream);
     COSL_CUDA(cudaEventRecord(g->evPre, g->auxStream));
   }
-  // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh)
+  // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh).  Each level is a
+  // programmatic dependent launch of the kernel before it (klt_front, then the level above): its
+  // CTAs are scheduled before that kernel ends and wait in the kernel for the source level.
+  // The front passes themselves are plain launches: they read the image copies and the counter
+  // reset ahead of them on this stream and have no grid-dependency wait.
   for (int l = 2; l < g->L; ++l) {
     dim3 gl(div_up(g->lvW[l], PT_TW), div_up(g->lvH[l], PT_TH), g->C);
-    COSL_LAUNCH(KLT_SIZED(g, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->cur][l - 1],
-                g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], g->d_cams, l);
+    COSL_LAUNCH_PDL(KLT_SIZED(g, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->cur][l - 1],
+                    g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], g->d_cams, l);
   }
   g->timer.end(st);
   COSL_CUDA(cudaGetLastError());

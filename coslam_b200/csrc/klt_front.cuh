@@ -270,6 +270,12 @@ klt_front(const FrontParams P) {
     }
     if (r0 - 3 + base + 7 > r1 + 2) break;  // the rows that remain feed nothing of this chunk
   }
+  // Level 2 of the pyramid tail is a programmatic dependent launch of this kernel: it is scheduled
+  // once every CTA has a warp here or has exited, and its griddepcontrol.wait still waits for the
+  // whole grid.  Not at kernel start: this pass shares the SMs with the previous frame's detector,
+  // and level-2 CTAs launched then would sit in their wait through the whole pass, holding slots
+  // and shared memory the detector could use.
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
 }  // namespace coslam

@@ -55,8 +55,21 @@ klt_pyr_down_tma(const __grid_constant__ CUtensorMap srcMap, const __grid_consta
   if (tid == 0) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&s_bar)));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&srcMap) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&dstMap) : "memory");
   }
   __syncthreads();
+  // Launched as a programmatic dependent of the kernel that writes the source level (klt_front or
+  // the level above), whose CTAs may still run: everything above reads only the tensor maps and the
+  // camera table.  The wait returns once that grid has completed and its stores, TMA stores
+  // included, are visible; nothing of this level is read or written before it.  The level-0 flag,
+  // the mixed-group clamping and the zero-fill reasoning above do not depend on it.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  // The next level may be scheduled once every CTA of this one has passed here: by then all of them
+  // hold their slots, so its CTAs (which wait above) take only slots this level does not need.
+  // Triggering here rather than after the store gets them resident ahead of the side stream's
+  // prefilter, which otherwise fills the SMs as level 2 drains and delays level 3 by about 4 us.
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (tid == 0) {
     constexpr unsigned bytes = PT_SH * PT_SW * sizeof(float4);
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&s_bar)), "r"(bytes)

@@ -1,10 +1,11 @@
 """torch.profiler trace of back-to-back KLT frames (bench.py's c3 workload, frames resident in HBM).
 
-  python tools/klt_overlap_trace.py OUT_DIR [--frames 20]
+  python tools/klt_overlap_trace.py OUT_DIR [--frames 20] [--no-gain]
 
 Writes OUT_DIR/klt_next_dev.json (Chrome trace) and prints, per frame pair, whether frame n+1's
-klt_front overlaps frame n's klt_nm_verify / klt_select_refill, the device time per frame, and the host
-time to enqueue one cosl_klt_group_next_dev call (measured without the profiler).  The host must
+klt_front overlaps frame n's klt_nm_verify / klt_select_refill, the device time per frame, the host
+time to enqueue one cosl_klt_group_next_dev call (measured without the profiler) and the split of
+the pyramid chain into kernels and the gaps between them (chain_split).  The host must
 enqueue a frame faster than the device runs it, or the queue drains and the overlap is lost."""
 import argparse
 import json
@@ -25,15 +26,48 @@ def kernels(trace, name):
                   if e.get("cat") == "kernel" and name in e.get("name", ""))
 
 
+def chain_split(front, pyr, track):
+    """Median per frame, in us, of the pyramid chain klt_front -> klt_pyr_down_tma x (L - 2) -> tracker
+    on the device timeline: the gap from the front pass's end to the first level's start, each
+    level's duration and the gap before the next, the tail (front pass end to last level end) and
+    the gap from the tail's end to the tracker's start.  A programmatic dependent launch starts
+    before the kernel ahead of it ends, so its gap can be negative and its duration includes the
+    wait."""
+    rows = []
+    for k, (f0, f1) in enumerate(front):
+        nxt = front[k + 1][0] if k + 1 < len(front) else float("inf")
+        lv = [p for p in pyr if f0 <= p[0] < nxt]
+        tr = [t for t in track if t[0] >= f1]
+        if not lv or not tr:
+            continue
+        r = {"front_to_level2_gap": lv[0][0] - f1, "tail": lv[-1][1] - f1,
+             "tail_to_tracker_gap": tr[0][0] - lv[-1][1]}
+        for i, (a, b) in enumerate(lv):
+            r[f"level{i + 2}_dur"] = b - a
+            if i + 1 < len(lv):
+                r[f"level{i + 2}_to_{i + 3}_gap"] = lv[i + 1][0] - b
+        rows.append(r)
+    if not rows:
+        return {}
+    keys = [k for k in rows[0] if all(k in r for r in rows)]
+    return {"frames": len(rows), **{k: round(float(np.median([r[k] for r in rows])), 2) for k in keys}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("out")
     ap.add_argument("--frames", type=int, default=20)
+    ap.add_argument("--no-gain", action="store_true", help="the 2x2 tracker (bench.py's klt_2x2 line)")
     args = ap.parse_args()
     os.makedirs(args.out, exist_ok=True)
     C, W, H = bench.KLT_C, bench.KLT_W, bench.KLT_H
     seqs = bench.make_sequences(0)
-    grp = api.KltGroup(bench.klt_cfg(), C, W, H, bench.KLT_L, bench.KLT_FW, bench.KLT_FH)
+    if args.no_gain:
+        from coslam_b200.ctypes_defs import KltConfig
+        cfg, tracker = KltConfig.coslam_live(with_gain=False), "klt_track_2x2"
+    else:
+        cfg, tracker = bench.klt_cfg(), "klt_gain_fused"
+    grp = api.KltGroup(cfg, C, W, H, bench.KLT_L, bench.KLT_FW, bench.KLT_FH)
     stream = torch.cuda.ExternalStream(grp.stream())
     dev = [[torch.from_numpy(seqs[c].frames[k]).cuda() for c in range(C)] for k in range(bench.KLT_FRAMES)]
     ptrs = [[t.data_ptr() for t in row] for row in dev]
@@ -86,6 +120,7 @@ def main():
         "front_overlaps_previous_detector": f"{overl} of {n - 1} frame pairs",
         "device_ms_per_frame": dev_ms,
         "host_enqueue_ms_per_call": {"median": 1e3 * float(np.median(host)), "p90": 1e3 * float(np.percentile(host, 90))},
+        "pyramid_chain_us": chain_split(front, kernels(trace, "klt_pyr_down_tma"), kernels(trace, tracker)),
         "trace": path}))
     grp.close()
 
