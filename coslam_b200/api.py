@@ -8,8 +8,8 @@ import os
 
 import numpy as np
 
-from .ctypes_defs import (COSL_BA_INFOSZ, FEAT_DTYPE, BaOptions, BaProblem, KltConfig, KltFeature,
-                          PoseOpt)
+from .ctypes_defs import (COSL_BA_INFOSZ, COSL_KLT_OP_SKIP, FEAT_DTYPE, BaOptions, BaProblem, KltConfig,
+                          KltFeature, PoseOpt)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # COSLAM_B200_LIB selects another build of the same library (kernel tuning experiments)
@@ -49,6 +49,8 @@ def _load():
     L.cosl_klt_group_feed.argtypes = [vp, vp, vp, vp, vp]
     L.cosl_klt_group_advance_cams.argtypes = [vp, vp]
     L.cosl_klt_group_next_dev.argtypes = [vp, vp, C.c_size_t]
+    L.cosl_klt_group_step.argtypes = [vp, vp, vp, C.c_size_t, vp, vp]
+    L.cosl_klt_group_step_dev.argtypes = [vp, vp, vp, C.c_size_t]
     L.cosl_klt_group_fetch.argtypes = [vp, vp, vp]
     L.cosl_klt_group_sync.argtypes = [vp]
     L.cosl_klt_group_submit.argtypes = [vp, vp, C.c_size_t]
@@ -316,6 +318,50 @@ class KltGroup:
     def next_dev(self, dev_ptrs, pitch):
         arr = (C.c_void_p * self.C)(*dev_ptrs)
         _ck(LIB.cosl_klt_group_next_dev(self.h, arr, pitch))
+
+    def _ops(self, ops):
+        ops = np.ascontiguousarray(ops, np.uint8)
+        assert ops.shape == (self.C,)
+        return ops
+
+    def _step_result(self, ops):
+        """(tables, counts) of the addressed cameras, None for a skipped one"""
+        tables = [None if o == COSL_KLT_OP_SKIP else self.feats[c] for c, o in enumerate(ops)]
+        counts = [None if o == COSL_KLT_OP_SKIP else int(self.counts[c]) for c, o in enumerate(ops)]
+        return tables, counts
+
+    def step(self, ops, imgs):
+        """cosl_klt_group_step: ops[c] in COSL_KLT_OP_* for camera c; imgs[c] its frame, or None
+        for a skipped camera.  Returns (tables, counts), None for a skipped camera."""
+        ops = self._ops(ops)
+        addr = [im for im, o in zip(imgs, ops) if o != COSL_KLT_OP_SKIP]
+        ptrs = (C.c_void_p * self.C)()
+        pitch = self.W  # read by no camera when every camera is skipped
+        if addr:
+            for im, (w, h), o in zip(imgs, self.sizes, ops):
+                if o != COSL_KLT_OP_SKIP:
+                    assert im.dtype == np.uint8 and im.shape == (h, w) and im.strides[1] == 1
+            # one pitch must hold the widest camera, which need not be addressed: frames whose rows
+            # are each their own camera's width apart pass 0 instead (per-camera sizes only)
+            pitches = {im.strides[0] for im in addr}
+            if len(pitches) == 1 and min(pitches) >= self.W:
+                pitch = pitches.pop()
+            else:
+                assert self.mixed and all(im.strides[0] == w for im, (w, _), o in zip(imgs, self.sizes, ops)
+                                          if o != COSL_KLT_OP_SKIP), \
+                    "give every frame one row pitch >= the widest camera, or rows of its camera's own width"
+                pitch = 0
+            for c, (im, o) in enumerate(zip(imgs, ops)):
+                ptrs[c] = None if o == COSL_KLT_OP_SKIP else im.ctypes.data
+        _ck(LIB.cosl_klt_group_step(self.h, _ptr(ops), ptrs, pitch, self._dest, _ptr(self.counts)))
+        return self._step_result(ops)
+
+    def step_dev(self, ops, dev_ptrs, pitch):
+        """cosl_klt_group_step_dev: device frames (None or 0 for a skipped camera); fetch() hands
+        back the result."""
+        ops = self._ops(ops)
+        arr = (C.c_void_p * self.C)(*[p or None for p in dev_ptrs])
+        _ck(LIB.cosl_klt_group_step_dev(self.h, _ptr(ops), arr, pitch))
 
     def fetch(self):
         _ck(LIB.cosl_klt_group_fetch(self.h, self._dest, _ptr(self.counts)))

@@ -26,6 +26,16 @@ struct cosl_klt {
   bool pitchZeroOK = false;  // made by cosl_klt_group_create_sizes: pitch 0 = each camera's own width
   KltCam hcam[64];           // per camera: extent and detector window (camera 0's: the uniform case)
   KltCam* d_cams = nullptr;  // device copy of hcam, read by the kernels of a mixed group
+  // cosl_klt_group_step: hcam with each camera's stages, written to one of two pinned tables and
+  // copied to the device table of the same index, in turn (the front pass of a step runs while the
+  // previous step's detector still reads its table); evStepTab[t] follows the last copy from table t
+  KltCam* h_stepCams[2] = {nullptr, nullptr};
+  KltCam* d_stepCams[2] = {nullptr, nullptr};
+  cudaEvent_t evStepTab[2] = {nullptr, nullptr};
+  int stepTab = 0;
+  // the ops of the last frame call when it was a step: what cosl_klt_group_fetch hands back
+  uint8_t stepOps[64];
+  bool stepOpsValid = false;
   int levelSkip = 1, halfWidth = 3;
   float trackMargin = 4.f, conv = 0.1f, ssd = 5000.f, detectMargin = 10.f;
   cudaStream_t stream = nullptr;
@@ -97,6 +107,7 @@ struct cosl_klt {
   int* d_waitset = nullptr;   // [F][16]
   bool fusedOK = false;
   int fusedBlocks = 0;
+  int fusedBlocksMixed = 0;  // of the MIXED instantiation, which steps run on every group
   int numSM = 132;
   int verBase = 0;
   // TMA descriptors of every pyramid level of both buffers: [buffer][level], load box (source of
@@ -133,6 +144,7 @@ static int update_cameras(cosl_klt* g) {
     const float Wf = (float)K.W, Hf = (float)K.H;
     bounds(K.W, mg / Wf, 1.0f - mg / Wf, K.ixlo, K.ixhi);
     bounds(K.H, mg / Hf, 1.0f - mg / Hf, K.iylo, K.iyhi);
+    K.stages = KLT_STAGE_ALL;
   }
   // pageable source: the copy is staged before the call returns, so hcam may change again
   COSL_CUDA(cudaMemcpyAsync(g->d_cams, g->hcam, sizeof(KltCam) * g->C, cudaMemcpyHostToDevice, g->stream));
@@ -147,16 +159,16 @@ using FusedFn = void (*)(const float4*, const float4*, long long, KltLevels, con
                          int, KltTail);
 using PassFn = void (*)(const float4*, const float4*, long long, long long, int, int, const KltCam*,
                         const float4*, const float4*, float4*, const int*, KltTrackParams, int);
-static FusedFn fused_kernel(const cosl_klt* g) {
-  if (g->mixed) return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE, true> : klt_gain_fused<0, true>;
+static FusedFn fused_kernel(const cosl_klt* g, bool mixed) {
+  if (mixed) return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE, true> : klt_gain_fused<0, true>;
   return g->halfWidth == KLT_HW_LIVE ? klt_gain_fused<KLT_HW_LIVE, false> : klt_gain_fused<0, false>;
 }
-static PassFn pass_kernel(const cosl_klt* g) {
-  if (g->mixed) return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE, true> : klt_gain_pass<0, true>;
+static PassFn pass_kernel(const cosl_klt* g, bool mixed) {
+  if (mixed) return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE, true> : klt_gain_pass<0, true>;
   return g->halfWidth == KLT_HW_LIVE ? klt_gain_pass<KLT_HW_LIVE, false> : klt_gain_pass<0, false>;
 }
-// the instantiation of a kernel for this group's sizes (klt_kernels.cuh, KltCam)
-#define KLT_SIZED(g, ...) ((g)->mixed ? __VA_ARGS__<true> : __VA_ARGS__<false>)
+// the instantiation of a kernel that reads the camera table (mixed) or not (klt_kernels.cuh, KltCam)
+#define KLT_SIZED(mixed, ...) ((mixed) ? __VA_ARGS__<true> : __VA_ARGS__<false>)
 
 int alloc_group(cosl_klt* g) {
   const int C = g->C, W = g->W, H = g->H, F = g->F;
@@ -180,6 +192,11 @@ int alloc_group(cosl_klt* g) {
   g->imgPitch = ((size_t)W + 15) & ~(size_t)15;
   g->imgStride = g->imgPitch * H;
   COSL_CUDA(cudaMalloc(&g->d_cams, sizeof(KltCam) * C));
+  for (int t = 0; t < 2; ++t) {
+    COSL_CUDA(cudaMalloc(&g->d_stepCams[t], sizeof(KltCam) * C));
+    COSL_CUDA(cudaMallocHost(&g->h_stepCams[t], sizeof(KltCam) * C));
+    COSL_CUDA(cudaEventCreateWithFlags(&g->evStepTab[t], cudaEventDisableTiming));
+  }
   // candidate capacity: a strict (2r+1)^2 maximum admits at most one survivor per (r+1)^2 pixels
   // (of the largest camera, which bounds every camera's count)
   const int r = std::max(1, g->cfg.minDistance);
@@ -256,15 +273,17 @@ int alloc_group(cosl_klt* g) {
         }
         ws[(size_t)j * 16 + 8 + nrev[j]++] = i;
       }
-    int dev = 0, coop = 0, nsm = 0, perSM = 0;
+    int dev = 0, coop = 0, nsm = 0, perSM = 0, perSMMixed = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
     cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
     g->numSM = std::max(1, nsm);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fused_kernel(g), KLT_FUSED_THREADS, 0);
-    g->fusedOK = ok && coop && perSM > 0 && !(g->cfg.compat & COSL_KLT_PASS_KERNELS);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, fused_kernel(g, g->mixed), KLT_FUSED_THREADS, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSMMixed, fused_kernel(g, true), KLT_FUSED_THREADS, 0);
+    g->fusedOK = ok && coop && perSM > 0 && perSMMixed > 0 && !(g->cfg.compat & COSL_KLT_PASS_KERNELS);
     const int T = F * C;
     g->fusedBlocks = std::max(1, std::min(div_up(T, KLT_GPB), nsm * perSM));
+    g->fusedBlocksMixed = std::max(1, std::min(div_up(T, KLT_GPB), nsm * perSMMixed));
     COSL_CUDA(cudaMalloc(&g->d_waitset, sizeof(int) * ws.size()));
     COSL_CUDA(cudaMemcpy(g->d_waitset, ws.data(), sizeof(int) * ws.size(), cudaMemcpyHostToDevice));
     COSL_CUDA(cudaMalloc(&g->d_state, sizeof(float4) * 2 * (size_t)T));
@@ -302,8 +321,9 @@ int alloc_group(cosl_klt* g) {
   }
   // dynamic shared memory opt-in: the attribute belongs to the kernel, not to this group, so it is
   // the largest any group uses (a group created later must not lower it below an earlier one's)
-  COSL_CUDA(cudaFuncSetAttribute(KLT_SIZED(g, klt_select_refill), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 KLT_MAX_SMEM_KEYS * (int)sizeof(unsigned long long)));
+  for (const bool mixed : {false, true})
+    COSL_CUDA(cudaFuncSetAttribute(KLT_SIZED(mixed, klt_select_refill), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   KLT_MAX_SMEM_KEYS * (int)sizeof(unsigned long long)));
   COSL_TRY(update_cameras(g));
   g->secPyr = g->timer.section("klt_pyramid");
   g->secTrack = g->timer.section("klt_track");
@@ -320,6 +340,11 @@ void free_group(cosl_klt* g) {
   g->timer.destroy();
   cudaFree(g->d_img);
   cudaFree(g->d_cams);
+  for (int t = 0; t < 2; ++t) {
+    cudaFree(g->d_stepCams[t]);
+    if (g->h_stepCams[t]) cudaFreeHost(g->h_stepCams[t]);
+    if (g->evStepTab[t]) cudaEventDestroy(g->evStepTab[t]);
+  }
   cudaFree(g->d_pyr[0]);
   cudaFree(g->d_pyr[1]);
   cudaFree(g->d_corn[0]);
@@ -367,12 +392,19 @@ void free_group(cosl_klt* g) {
 // ---- stages (all asynchronous; the streams of each are in run_frame) ----
 
 // camera c's image: hcam[c].W x hcam[c].H bytes, rows `pitch` bytes apart (0: hcam[c].W, pitch_ok);
-// on the front stream, or for a multi-camera host upload on the copy stream
-int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind kind) {
+// on the front stream, or for a multi-camera host upload on the copy stream.  ops (a step, else
+// nullptr): the cameras with COSL_KLT_OP_SKIP are not copied; their events are still recorded, so
+// the front pass can wait for any camera's.
+int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind kind,
+                  const uint8_t* ops) {
   if (kind == cudaMemcpyHostToDevice && g->C > 1) {
     // the previous frame's front pass must have consumed d_img before it is overwritten
     if (g->frontRecorded) COSL_CUDA(cudaStreamWaitEvent(g->copyStream, g->evFront, 0));
     for (int c = 0; c < g->C; ++c) {
+      if (ops && ops[c] == COSL_KLT_OP_SKIP) {
+        COSL_CUDA(cudaEventRecord(g->evImg[c], g->copyStream));
+        continue;
+      }
       const size_t w = (size_t)g->hcam[c].W, sp = pitch ? pitch : w;
       if (sp == w && g->imgPitch == w)  // one contiguous block
         COSL_CUDA(cudaMemcpyAsync(g->d_img + (size_t)c * g->imgStride, imgs[c], w * g->hcam[c].H, kind,
@@ -386,21 +418,22 @@ int upload_images(cosl_klt* g, const uint8_t* const* imgs, size_t pitch, cudaMem
     return COSL_OK;
   }
   for (int c = 0; c < g->C; ++c)
-    COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c],
-                                pitch ? pitch : (size_t)g->hcam[c].W, g->hcam[c].W, g->hcam[c].H, kind,
-                                g->frontStream));
+    if (!ops || ops[c] != COSL_KLT_OP_SKIP)
+      COSL_CUDA(cudaMemcpy2DAsync(g->d_img + (size_t)c * g->imgStride, g->imgPitch, imgs[c],
+                                  pitch ? pitch : (size_t)g->hcam[c].W, g->hcam[c].W, g->hcam[c].H, kind,
+                                  g->frontStream));
   return COSL_OK;
 }
 
 // klt_nm_prefilter on `st` (prefilter radius = min(minDistance, 3))
-static void launch_prefilter(cosl_klt* g, cudaStream_t st) {
+static void launch_prefilter(cosl_klt* g, cudaStream_t st, bool mixed, const KltCam* cams) {
   const int pr = std::min(std::max(1, g->cfg.minDistance), 3);
   dim3 gp(div_up(g->W, 32 - 2 * pr), div_up(g->H, 8 * NP_ROWS), g->C);
   const long long cs = (long long)g->W * g->H;
-  const auto kern = pr == 3 ? (g->mixed ? klt_nm_prefilter<3, true> : klt_nm_prefilter<3, false>)
-                  : pr == 2 ? (g->mixed ? klt_nm_prefilter<2, true> : klt_nm_prefilter<2, false>)
-                            : (g->mixed ? klt_nm_prefilter<1, true> : klt_nm_prefilter<1, false>);
-  COSL_LAUNCH(kern, gp, 256, 0, st, g->d_corn[g->par], g->W, cs, g->d_cams, g->W, g->H, g->d_prelim[g->par],
+  const auto kern = pr == 3 ? (mixed ? klt_nm_prefilter<3, true> : klt_nm_prefilter<3, false>)
+                  : pr == 2 ? (mixed ? klt_nm_prefilter<2, true> : klt_nm_prefilter<2, false>)
+                            : (mixed ? klt_nm_prefilter<1, true> : klt_nm_prefilter<1, false>);
+  COSL_LAUNCH(kern, gp, 256, 0, st, g->d_corn[g->par], g->W, cs, cams, g->W, g->H, g->d_prelim[g->par],
               g->prelimCap, g->d_counters[g->par]);
 }
 
@@ -428,9 +461,14 @@ static bool tracker_reads_level0(const cosl_klt* g) { return (g->L - 1) % g->lev
 // the persistent gain tracker (klt_gain_fused) runs, not the per-pass kernels or the 2x2 tracker
 static bool fused_tracker(const cosl_klt* g) { return g->cfg.trackWithGain && g->fusedOK; }
 
-// What the stages of one frame fold together; run_frame decides it for the frame's kind.
+// What the stages of one frame fold together; run_frame decides it for the frame's kind, run_step
+// for the union of its cameras' ops.
 struct FramePlan {
-  bool wantCorn;        // klt_front also produces the detector's cornerness map
+  const KltCam* cams;   // the camera table the kernels read: the group's, or a step's (stages)
+  bool mixed;           // the kernels' MIXED instantiation runs (reads `cams`)
+  bool tracked;         // the tracker runs (for some camera)
+  int cornMode;         // FrontParams::wantCorn: 0, 1, or KLT_CORN_PER_CAM (a step)
+  bool wantCorn;        // klt_front also produces the detector's cornerness map (for some camera)
   bool storeL0;         // klt_front stores pyramid level 0
   bool earlyPrefilter;  // the detector's prefilter runs on auxStream right after klt_front
   bool trackerTail;     // the tracker writes the feature table (klt_status) and, with wantCorn, the
@@ -443,7 +481,6 @@ struct FramePlan {
 int build_pyramid(cosl_klt* g, const FramePlan& p) {
   cudaStream_t st = g->frontStream;
   float4* P = g->d_pyr[g->cur];
-  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = p.storeL0;
   g->timer.begin(g->secPyr, st);
   // level 0 + level 1 + (optionally) the detector's cornerness map in one pass over the image
   FrontParams fp;
@@ -460,15 +497,15 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   fp.nStrips = div_up(g->W, FS_SW);
   fp.nChunks = div_up(g->H, FS_R);
   fp.wantL1 = g->L > 1 ? 1 : 0;
-  const auto front = p.storeL0 ? (g->mixed ? klt_front<true, true> : klt_front<true, false>)
-                                : (g->mixed ? klt_front<false, true> : klt_front<false, false>);
-  fp.wantCorn = p.wantCorn ? 1 : 0;
+  const auto front = p.storeL0 ? (p.mixed ? klt_front<true, true> : klt_front<true, false>)
+                                : (p.mixed ? klt_front<false, true> : klt_front<false, false>);
+  fp.wantCorn = p.cornMode;
   fp.minC = g->cfg.minCornerness;
   fp.ixlo = g->hcam[0].ixlo;
   fp.ixhi = g->hcam[0].ixhi;
   fp.iylo = g->hcam[0].iylo;
   fp.iyhi = g->hcam[0].iyhi;
-  fp.cams = g->d_cams;
+  fp.cams = p.cams;
   // the grid covers the largest camera; a smaller camera's surplus warps exit
   const int nWarps = fp.nStrips * fp.nChunks;
   if (g->imgPerCam) {
@@ -492,7 +529,7 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   g->frontRecorded = true;
   if (p.earlyPrefilter) {
     COSL_CUDA(cudaStreamWaitEvent(g->auxStream, g->evFront, 0));
-    launch_prefilter(g, g->auxStream);
+    launch_prefilter(g, g->auxStream, p.mixed, p.cams);
     COSL_CUDA(cudaEventRecord(g->evPre, g->auxStream));
   }
   // source tile by TMA load, destination tile by TMA store (klt_pyr_tma.cuh).  Each level is a
@@ -502,8 +539,8 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   // reset ahead of them on this stream and have no grid-dependency wait.
   for (int l = 2; l < g->L; ++l) {
     dim3 gl(div_up(g->lvW[l], PT_TW), div_up(g->lvH[l], PT_TH), g->C);
-    COSL_LAUNCH_PDL(KLT_SIZED(g, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->cur][l - 1],
-                    g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], g->d_cams, l);
+    COSL_LAUNCH_PDL(KLT_SIZED(p.mixed, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->cur][l - 1],
+                    g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], p.cams, l);
   }
   g->timer.end(st);
   COSL_CUDA(cudaGetLastError());
@@ -565,10 +602,11 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
     KltTail tail = {g->d_feat, g->d_counters[g->par], g->d_corn[g->par], (long long)g->W * g->H, g->W,
                     p.wantCorn ? 1 : 0};
     void* args[] = {(void*)&P0,          (void*)&P1,       (void*)&pyrStride,  (void*)&LV,
-                    (void*)&g->d_cams,   (void*)&nIter,    (void*)&g->d_src,   (void*)&g->d_state,
+                    (void*)&p.cams,      (void*)&nIter,    (void*)&g->d_src,   (void*)&g->d_state,
                     (void*)&g->d_ver,    (void*)&g->d_waitset, (void*)&g->d_res, (void*)&C,
                     (void*)&Plax,        (void*)&Pstrict,  (void*)&verBase,    (void*)&tail};
-    COSL_CUDA(cudaLaunchCooperativeKernel((const void*)fused_kernel(g), dim3(g->fusedBlocks),
+    COSL_CUDA(cudaLaunchCooperativeKernel((const void*)fused_kernel(g, p.mixed),
+                                          dim3(p.mixed ? g->fusedBlocksMixed : g->fusedBlocks),
                                           dim3(KLT_FUSED_THREADS), args, 0, g->stream));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     g->verBase += nPass;
@@ -605,7 +643,7 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
   } else if (g->cfg.trackWithGain) {
     const float4* in = g->d_src;
     float4* bufs[2] = {g->d_ping, g->d_pong};
-    const PassFn pass = pass_kernel(g);
+    const PassFn pass = pass_kernel(g, p.mixed);
     int which = 0, first = 1;
     bool strict = false;
     for (int li = 0; li < LV.n; ++li) {
@@ -617,7 +655,7 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
         const bool last = (li == LV.n - 1) && (iter == g->cfg.nIterations);
         float4* out = last ? g->d_res : bufs[which];
         COSL_LAUNCH(pass, gridHalf, 256, 0, g->stream, P0, P1, g->pyrStride, LV.off[li], LV.level[li],
-                    LV.w[li], g->d_cams, g->d_src, in, out, g->d_nbr, track_params(g, strict), first);
+                    LV.w[li], p.cams, g->d_src, in, out, g->d_nbr, track_params(g, strict), first);
         in = out;
         which ^= 1;
         first = 0;
@@ -630,10 +668,10 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
                        !(g->cfg.compat & COSL_KLT_PASS_KERNELS);
     if (tiled) {
       dim3 gt(div_up(g->F, 16), g->C);
-      COSL_LAUNCH(KLT_SIZED(g, klt_track_2x2_tiled), gt, 128, 0, g->stream, P0, P1, g->pyrStride, LV, g->d_cams,
+      COSL_LAUNCH(KLT_SIZED(p.mixed, klt_track_2x2_tiled), gt, 128, 0, g->stream, P0, P1, g->pyrStride, LV, p.cams,
                   g->d_src, g->d_res, track_params(g, true), nIter);
     } else {
-      COSL_LAUNCH(KLT_SIZED(g, klt_track_2x2), grid, wpb * 32, 0, g->stream, P0, P1, g->pyrStride, LV, g->d_cams,
+      COSL_LAUNCH(KLT_SIZED(p.mixed, klt_track_2x2), grid, wpb * 32, 0, g->stream, P0, P1, g->pyrStride, LV, p.cams,
                   g->d_src, g->d_res, track_params(g, true), nIter);
     }
   }
@@ -644,35 +682,36 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
 
 // KLT_Detector::detectCorners + extractCorners (v3d_gpuklt.cpp:423-588) and the slot logic of
 // detect/redetect (:651-805) on the cornerness map klt_front produced for this frame.  mode 0: detect
-// (present = the external points of upload_present, maxPresent = the longest list), 1: redetect.
+// (present = the external points of upload_present, maxPresent = the longest list), 1: redetect,
+// 2: per camera of a step (klt_select_refill).
 int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
   g->timer.begin(g->secDetect, g->stream);
   const long long cs = (long long)g->W * g->H;
   float* corn = g->d_corn[g->par];
   int* counters = g->d_counters[g->par];
-  if (mode == 1 && !p.trackerTail) {
+  if (mode != 0 && p.tracked && !p.trackerTail) {  // the live tracks of the re-detecting cameras
     dim3 gs(div_up(g->F, 256), g->C);
-    COSL_LAUNCH(KLT_SIZED(g, klt_suppress), gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F,
-                corn, g->W, cs, g->d_cams, g->W, g->H);
+    COSL_LAUNCH(KLT_SIZED(p.mixed, klt_suppress), gs, 256, 0, g->stream, g->d_res, g->F, (const int*)nullptr, g->F,
+                corn, g->W, cs, p.cams, g->W, g->H, KLT_STAGE_TRACK | KLT_STAGE_DETECT);
   } else if (mode == 0 && maxPresent > 0) {
     dim3 gs(div_up(maxPresent, 256), g->C);
-    COSL_LAUNCH(KLT_SIZED(g, klt_suppress), gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F,
-                corn, g->W, cs, g->d_cams, g->W, g->H);
+    COSL_LAUNCH(KLT_SIZED(p.mixed, klt_suppress), gs, 256, 0, g->stream, g->d_present, 0, g->d_nPresent, g->F,
+                corn, g->W, cs, p.cams, g->W, g->H, KLT_STAGE_DETECT);
   }
   const int r = std::max(1, g->cfg.minDistance);
   if (p.earlyPrefilter)
     COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evPre, 0));
   else
-    launch_prefilter(g, g->stream);
+    launch_prefilter(g, g->stream, p.mixed, p.cams);
   dim3 gv(2 * g->numSM, g->C);
-  COSL_LAUNCH(KLT_SIZED(g, klt_nm_verify), gv, 256, 0, g->stream, corn, g->W, cs, g->d_cams, g->W, g->H, r,
+  COSL_LAUNCH(KLT_SIZED(p.mixed, klt_nm_verify), gv, 256, 0, g->stream, corn, g->W, cs, p.cams, g->W, g->H, r,
               g->d_prelim[g->par], g->prelimCap, g->d_cand, g->candCap, counters);
   g->timer.end(g->stream);
   g->timer.begin(g->secSelect, g->stream);
-  COSL_LAUNCH(KLT_SIZED(g, klt_select_refill), g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
+  COSL_LAUNCH(KLT_SIZED(p.mixed, klt_select_refill), g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
               g->d_cand, g->candCap, g->plCap, counters, g->d_feat, g->d_dst,
               p.foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
-              maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, g->d_cams, g->W, g->H, mode,
+              maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, p.cams, g->W, g->H, mode,
               g->cfg.trackWithGain ? 1 : 0, g->smemKeys, (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
   g->timer.end(g->stream);
   COSL_CUDA(cudaGetLastError());
@@ -811,7 +850,11 @@ enum FrameKind {
 int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind,
               int maxPresent, bool foldAdvance) {
   FramePlan p;
+  p.cams = g->d_cams;
+  p.mixed = g->mixed;
+  p.tracked = kind != FRAME_DETECT;
   p.wantCorn = kind != FRAME_TRACK;
+  p.cornMode = p.wantCorn ? 1 : 0;
   // A re-detect frame has its cornerness fused into the front pass, so nothing but a tracker that
   // visits level 0 reads that level.  It is stored only then: at 16 B/px it is larger than the L2,
   // and writing it would evict the pyramid levels the tracker that follows reads.
@@ -819,16 +862,18 @@ int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pi
   p.earlyPrefilter = kind == FRAME_REDETECT;
   p.trackerTail = fused_tracker(g);
   p.foldAdvance = foldAdvance;
+  g->stepOpsValid = false;
   if (p.wantCorn) g->par ^= 1;
   int* counters = g->d_counters[g->par];
   // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below
   COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
   // the images ahead of the fence: d_img is read by the front passes alone, so they run under the
   // previous frame's tracker
-  COSL_TRY(upload_images(g, imgs, pitch, copyKind));
+  COSL_TRY(upload_images(g, imgs, pitch, copyKind, nullptr));
   COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evFence, 0));
   if (p.wantCorn)
     COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
+  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = p.storeL0;
   COSL_TRY(build_pyramid(g, p));
   COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
   COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
@@ -837,7 +882,7 @@ int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pi
     COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
     if (!p.trackerTail) {
       dim3 grid(div_up(g->F, 256), g->C);
-      COSL_LAUNCH(klt_status, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F);
+      COSL_LAUNCH(klt_status<false>, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, g->d_cams);
     }
   }
   if (kind == FRAME_TRACK) {
@@ -852,12 +897,139 @@ int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pi
   return COSL_OK;
 }
 
+// the stages of a cosl_klt_group_step op (KltCam::stages)
+static int op_stages(int op) {
+  return op == COSL_KLT_OP_FIRST   ? KLT_STAGE_PYR | KLT_STAGE_DETECT
+         : op == COSL_KLT_OP_TRACK ? KLT_STAGE_PYR | KLT_STAGE_TRACK
+         : op == COSL_KLT_OP_NEXT  ? KLT_STAGE_ALL
+                                   : 0;
+}
+
+// exchange the cameras' slices of the two pyramid buffers (and their level-0 records) on g->stream
+static int exchange_slices(cosl_klt* g, const KltCamList& L) {
+  if (L.n == 0) return COSL_OK;
+  dim3 grid((unsigned)std::min<long long>(div_up64(g->pyrStride, 256), 2 * g->numSM), L.n);
+  COSL_LAUNCH(klt_advance_cams, grid, 256, 0, g->stream, g->d_pyr[0], g->d_pyr[1], g->pyrStride, g->d_dst,
+              g->d_src, 0, L);
+  for (int k = 0; k < L.n; ++k) std::swap(g->lv0Stored[0][L.cam[k]], g->lv0Stored[1][L.cam[k]]);
+  return COSL_OK;
+}
+
+// One step of cosl_klt_group_step: camera c gets ops[c] followed by advanceFrame, or nothing.
+// Every camera with the same op: the frame of that kind (run_frame), exactly as group_first /
+// group_next / track + advance run it.  Otherwise one frame whose kernels are the MIXED
+// instantiations on a table of the step's own (KltCam::stages), so each launch covers the group
+// and a camera's blocks exit in the stages its op does not have:
+//   pyramid (front pass, tail)       FIRST, TRACK, NEXT
+//   tracker, status                  TRACK, NEXT
+//   cornerness, non-max, selection   FIRST, NEXT      (klt_select_refill: mode per camera)
+//   provide (klt_provide_cams)       TRACK
+// The frame's schedule is run_frame's, with the plan of the union of the ops: the front pass stores
+// level 0 when one of its cameras needs it, the prefilter runs early, and a step with a detecting
+// camera switches the counter set (a switch is always safe: the set it leaves is the one the
+// fence protects).  The front pass of the next frame waits for the fence as ever.
+//
+// Advance of a strict subset: the pyramid slices of either the skipped or the addressed cameras
+// are exchanged, whichever are fewer.  Skipped ones: `cur` flips for the group and their slices
+// are exchanged ahead of the tracker (nothing of the step touches them); addressed ones: `cur`
+// stays and their slices are exchanged after the tracker, ahead of the fence.  The feature-buffer
+// half of the advance is folded into klt_select_refill and klt_provide_cams.
+int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
+  const int C = g->C;
+  int nOp[4] = {0, 0, 0, 0};
+  for (int c = 0; c < C; ++c) ++nOp[ops[c]];
+  if (nOp[COSL_KLT_OP_NEXT] == C) {
+    COSL_TRY(run_frame(g, FRAME_REDETECT, imgs, pitch, copyKind, 0, true));
+  } else if (nOp[COSL_KLT_OP_FIRST] == C) {
+    COSL_TRY(run_frame(g, FRAME_DETECT, imgs, pitch, copyKind, 0, true));
+  } else if (nOp[COSL_KLT_OP_TRACK] == C) {
+    COSL_TRY(run_frame(g, FRAME_TRACK, imgs, pitch, copyKind, 0, false));
+    COSL_TRY(advance(g));
+  } else if (nOp[COSL_KLT_OP_SKIP] < C) {
+    KltCamList addr, skip, provide;
+    addr.n = skip.n = provide.n = 0;
+    bool anyTrack = false, anyDetect = false, storeL0 = false;
+    bool lv0[64];  // what a single tracker records for the frame of the camera's op
+    // the pinned table's previous copy was enqueued two steps ago: the host waits here only when
+    // it runs more than a step ahead of the front stream (cosl_klt_group_step_dev)
+    const int tab = g->stepTab ^= 1;
+    COSL_CUDA(cudaEventSynchronize(g->evStepTab[tab]));
+    KltCam* hstep = g->h_stepCams[tab];
+    for (int c = 0; c < C; ++c) {
+      const int st = op_stages(ops[c]);
+      hstep[c] = g->hcam[c];
+      hstep[c].stages = st;
+      if (!st) {
+        skip.cam[skip.n++] = c;
+        continue;
+      }
+      addr.cam[addr.n++] = c;
+      if (ops[c] == COSL_KLT_OP_TRACK) provide.cam[provide.n++] = c;
+      anyTrack = anyTrack || (st & KLT_STAGE_TRACK);
+      anyDetect = anyDetect || (st & KLT_STAGE_DETECT);
+      lv0[c] = ops[c] != COSL_KLT_OP_NEXT || tracker_reads_level0(g);
+      storeL0 = storeL0 || lv0[c];
+    }
+    const bool flip = skip.n <= addr.n;
+    FramePlan p;
+    p.cams = g->d_stepCams[tab];
+    p.mixed = true;
+    p.tracked = anyTrack;
+    p.wantCorn = anyDetect;
+    p.cornMode = anyDetect ? KLT_CORN_PER_CAM : 0;
+    p.storeL0 = storeL0;
+    p.earlyPrefilter = anyDetect;
+    p.trackerTail = fused_tracker(g);
+    p.foldAdvance = true;
+    if (p.wantCorn) g->par ^= 1;
+    int* counters = g->d_counters[g->par];
+    COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), C, g->stream));
+    if (flip) COSL_TRY(exchange_slices(g, skip));
+    COSL_TRY(upload_images(g, imgs, pitch, copyKind, ops));
+    COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evFence, 0));
+    // the device table's last readers belong to the step before the previous one, ahead of the fence
+    COSL_CUDA(cudaMemcpyAsync(g->d_stepCams[tab], hstep, sizeof(KltCam) * C, cudaMemcpyHostToDevice, g->frontStream));
+    COSL_CUDA(cudaEventRecord(g->evStepTab[tab], g->frontStream));
+    if (p.wantCorn)
+      COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), C, g->frontStream));
+    for (int k = 0; k < addr.n; ++k) g->lv0Stored[g->cur][addr.cam[k]] = lv0[addr.cam[k]];
+    COSL_TRY(build_pyramid(g, p));
+    COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
+    COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
+    if (anyTrack) {
+      COSL_TRY(run_tracker(g, p));
+      if (!flip) COSL_TRY(exchange_slices(g, addr));
+      COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
+      if (!p.trackerTail) {
+        dim3 grid(div_up(g->F, 256), C);
+        COSL_LAUNCH(klt_status<true>, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, p.cams);
+      }
+    }
+    if (provide.n)
+      COSL_LAUNCH(klt_provide_cams, dim3(div_up(g->F, 256), provide.n), 256, 0, g->stream, g->d_res, g->d_dst,
+                  g->d_src, g->F, provide);
+    if (anyDetect) COSL_TRY(run_detector(g, 2, 0, p));
+    if (!anyTrack) {
+      if (!flip) COSL_TRY(exchange_slices(g, addr));
+      COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
+    }
+    if (flip) g->cur = 1 - g->cur;
+  }
+  std::memcpy(g->stepOps, ops, C);
+  g->stepOpsValid = true;
+  return COSL_OK;
+}
+
 // Camera c's table of `feat` -> dest[c] and its count counters[8c + 2] -> n[c], each where given.
+// After a step (g->stepOpsValid): the addressed cameras only, a tracked-only camera's count being
+// its live tracks (counters[8c + 0], what track() returns).
 void copy_out(const cosl_klt* g, const cosl_klt_feature* feat, const int* counters,
               cosl_klt_feature* const* dest, int* n) {
   for (int c = 0; c < g->C; ++c) {
+    const int op = g->stepOpsValid ? g->stepOps[c] : COSL_KLT_OP_NEXT;
+    if (op == COSL_KLT_OP_SKIP) continue;
     if (dest && dest[c]) std::memcpy(dest[c], feat + (size_t)c * g->F, sizeof(cosl_klt_feature) * g->F);
-    if (n) n[c] = counters[8 * c + 2];
+    if (n) n[c] = counters[8 * c + (op == COSL_KLT_OP_TRACK ? 0 : 2)];
   }
 }
 
@@ -1122,6 +1294,36 @@ int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pit
   if (!dimgs || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "group_next_dev: bad argument");
   return run_frame(h, FRAME_REDETECT, dimgs, pitch, cudaMemcpyDeviceToDevice, 0, true);
+}
+
+// ops[c] in COSL_KLT_OP_*, an image for every addressed camera
+static int check_step(const cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch,
+                      const char* name) {
+  if (!ops || !imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "%s: bad argument", name);
+  for (int c = 0; c < h->C; ++c) {
+    if (ops[c] > COSL_KLT_OP_NEXT) return set_error(COSL_E_INVALID, "%s: bad op %d of camera %d", name, ops[c], c);
+    if (ops[c] != COSL_KLT_OP_SKIP && !imgs[c])
+      return set_error(COSL_E_INVALID, "%s: no image for camera %d", name, c);
+  }
+  return COSL_OK;
+}
+
+int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch,
+                        cosl_klt_feature* const* dest, int* n) {
+  KLT_ENTER(h)
+  KLT_NOT_IN_FLIGHT(h, "group_step")
+  COSL_TRY(check_step(h, ops, imgs, pitch, "group_step"));
+  COSL_TRY(run_step(h, ops, imgs, pitch, cudaMemcpyHostToDevice));
+  COSL_TRY(fetch_results(h));
+  copy_out(h, h->h_feat, h->h_counters, dest, n);
+  return COSL_OK;
+}
+
+int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* const* dimgs, size_t pitch) {
+  KLT_ENTER(h)
+  KLT_NOT_IN_FLIGHT(h, "group_step_dev")
+  COSL_TRY(check_step(h, ops, dimgs, pitch, "group_step_dev"));
+  return run_step(h, ops, dimgs, pitch, cudaMemcpyDeviceToDevice);
 }
 
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {

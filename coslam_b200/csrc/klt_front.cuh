@@ -42,6 +42,8 @@ constexpr int FS_WARPS = 4;  // warps per CTA (independent of each other)
 #define FS_PF 3           // image rows in flight ahead of the row loop
 #endif
 
+constexpr int KLT_CORN_PER_CAM = 2;  // FrontParams::wantCorn: each camera of the detector stage (MIXED)
+
 struct FrontParams {
   const uint8_t* img;
   size_t imgPitch, imgStride;
@@ -63,6 +65,7 @@ klt_front(const FrontParams P) {
   const int lane = threadIdx.x & 31;
   const int wid = blockIdx.x * FS_WARPS + (threadIdx.x >> 5);
   const int cam = blockIdx.y + P.camBase;
+  if (!klt_in_stage<MIXED>(P.cams, cam, KLT_STAGE_PYR)) return;
   const int2 ext = klt_extent<MIXED>(P.cams, cam, P.W, P.H);
   const int W = ext.x, H = ext.y;
   const int nStrips = MIXED ? (W + FS_SW - 1) / FS_SW : P.nStrips;
@@ -200,7 +203,12 @@ klt_front(const FrontParams P) {
         }
       }
       // ---- cornerness of row yy - 3 (klt_detector_pass1.cg / pass2.cg)
-      if (P.wantCorn) {
+      // MIXED, wantCorn == KLT_CORN_PER_CAM: the cameras of the detector stage (re-read per row for
+      // the register limit, see below)
+      if (MIXED ? (P.wantCorn == KLT_CORN_PER_CAM
+                       ? klt_in_stage<MIXED>(P.cams, klt_opaque((int)blockIdx.y) + P.camBase, KLT_STAGE_DETECT)
+                       : P.wantCorn != 0)
+                : P.wantCorn != 0) {
         prod[u][0] = __fmul_rn(A[1], A[1]);
         prod[u][1] = __fmul_rn(A[1], A[2]);
         prod[u][2] = __fmul_rn(A[2], A[2]);

@@ -48,7 +48,20 @@ __device__ __forceinline__ int klt_opaque(int v) {
 struct KltCam {
   int W, H;
   int ixlo, ixhi, iylo, iyhi;  // detector window: pixels whose centre lies inside the margins
+  int stages;                  // KLT_STAGE_* bits this camera takes part in (cosl_klt_group_step)
 };
+
+// Stages of a frame, per camera.  The group's own table has every bit set; cosl_klt_group_step
+// runs the MIXED instantiations on a table of its own in which each camera carries the stages of
+// its op (FIRST = PYR | DETECT, TRACK = PYR | TRACK, NEXT = all three, SKIP = none), and every
+// kernel's blocks of a camera that does not take part in its stage exit.
+enum { KLT_STAGE_PYR = 1, KLT_STAGE_TRACK = 2, KLT_STAGE_DETECT = 4, KLT_STAGE_ALL = 7 };
+
+// MIXED: camera `cam` takes part in the stages `bits` (all of them); always true otherwise
+template <bool MIXED>
+__device__ __forceinline__ bool klt_in_stage(const KltCam* __restrict__ cams, int cam, int bits) {
+  return !MIXED || (__ldg(&cams[cam].stages) & bits) == bits;
+}
 
 // extent of camera `cam`: its table entry, or the group's W x H when all cameras share it
 template <bool MIXED>
@@ -146,6 +159,7 @@ klt_track_2x2(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
               KltLevels LV, const KltCam* __restrict__ cams, const float4* __restrict__ X0buf,
               float4* __restrict__ out, KltTrackParams P, int nIter) {
   const int cam = blockIdx.y;
+  if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) return;
   const int2 ext = klt_extent<MIXED>(cams, cam, P.W, P.H);
   const int Wc = ext.x, Hc = ext.y;
   const int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -216,10 +230,13 @@ klt_track_2x2(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
 // ------------------------------------------------------------------------------------------
 // KLT_SequenceTracker::track host loop (v3d_gpuklt.cpp:872-888) on the device: tracker output ->
 // dest entries + per-camera count of present features.  counters[cam*8 + 0] = nPresent.
+// MIXED: only the cameras of the tracker stage (cams, KltCam::stages).
 // ------------------------------------------------------------------------------------------
+template <bool MIXED>
 __global__ void klt_status(const float4* __restrict__ res, cosl_klt_feature* __restrict__ dest,
-                           int* __restrict__ counters, int F) {
+                           int* __restrict__ counters, int F, const KltCam* __restrict__ cams) {
   const int cam = blockIdx.y;
+  if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   bool live = false;
   if (i < F) {
@@ -247,11 +264,13 @@ __global__ void klt_status(const float4* __restrict__ res, cosl_klt_feature* __r
 // pts: float4 (x, y, .., ..) per slot, x < 0 == dead (clipped).  Camera c reads nPer[c] points when
 // nPer is given (present lists of different lengths), else n.
 // The cornerness map of camera c: rows `pitch` floats apart, `cornStride` floats per camera.
+// MIXED: only the cameras that take part in all of the stages `bits`.
 template <bool MIXED>
 __global__ void klt_suppress(const float4* __restrict__ pts, int n, const int* __restrict__ nPer,
                              int ptsStride, float* __restrict__ corn, int pitch, long long cornStride,
-                             const KltCam* __restrict__ cams, int W, int H) {
+                             const KltCam* __restrict__ cams, int W, int H, int bits) {
   const int cam = blockIdx.y;
+  if (!klt_in_stage<MIXED>(cams, cam, bits)) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (nPer ? nPer[cam] : n)) return;
   const float4 p = pts[(size_t)cam * ptsStride + i];
@@ -295,6 +314,7 @@ klt_nm_prefilter(const float* __restrict__ corn, int pitch, long long cornStride
     W = __ldg(&cams[cam].W);
     H = __ldg(&cams[cam].H);
     if ((int)blockIdx.x * NCOLS >= W) return;  // the block's output columns lie outside this camera
+    if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_DETECT)) return;
   }
   const float* cm = corn + (size_t)cam * cornStride;
   const int lane = threadIdx.x & 31;
@@ -372,6 +392,7 @@ klt_nm_verify(const float* __restrict__ corn, int pitch, long long cornStride,
               int prelimCap, unsigned long long* __restrict__ cand, int candCap, int* __restrict__ counters) {
   const int cam = blockIdx.y;
   if (MIXED) {
+    if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_DETECT)) return;
     W = __ldg(&cams[cam].W);
     H = __ldg(&cams[cam].H);
   }
@@ -428,6 +449,8 @@ klt_nm_verify(const float* __restrict__ corn, int pitch, long long cornStride,
 //   mode 0 (detect):   slots [0, nDet) <- strongest corners, [nDet, nDet+nPresent) <- present pts
 //                      (nPresent = nPresentExt[cam], 0 when nPresentExt is null)
 //   mode 1 (redetect): dead slots, in increasing slot index, <- strongest corners
+//   mode 2 (MIXED):    per camera, 1 for a camera of the tracker stage, else 0
+//                      (cosl_klt_group_step; the cameras outside the detector stage exit)
 // and "provide" the new feature table (dst buffer).  counters[cam*8+2] = returned count
 // (nDetected / nNewFeatures as the reference defines them), [3] = raw candidate count.
 // ------------------------------------------------------------------------------------------
@@ -485,6 +508,9 @@ klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
   __shared__ int s_base;
   const int cam = blockIdx.x;
   if (MIXED) {
+    const int stages = __ldg(&cams[cam].stages);
+    if (!(stages & KLT_STAGE_DETECT)) return;
+    if (mode == 2) mode = (stages & KLT_STAGE_TRACK) ? 1 : 0;  // per camera: re-detect after a track
     W = __ldg(&cams[cam].W);
     H = __ldg(&cams[cam].H);
   }
@@ -660,6 +686,23 @@ __global__ void klt_copy_f4(const float4* __restrict__ a, float4* __restrict__ b
   if (i < n) b[i] = a[i];
 }
 
+struct KltCamList {
+  int n;
+  int cam[64];
+};
+
+// "provide" and advanceFrame of the tracked-only cameras of a cosl_klt_group_step: dst and src
+// <- tracker result for the cameras of the list.  grid (div_up(F, blockDim.x), n).
+__global__ void klt_provide_cams(const float4* __restrict__ res, float4* __restrict__ dst,
+                                 float4* __restrict__ src, int F, KltCamList L) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= F) return;
+  const size_t k = (size_t)L.cam[blockIdx.y] * F + i;
+  const float4 v = res[k];
+  dst[k] = v;
+  src[k] = v;
+}
+
 // ------------------------------------------------------------------------------------------
 // feedExternFeaturePoints (v3d_gpuklt.cpp:808-855): (1) kill KLT points within normalised
 // distance^2 < 1e-4 of any fed point, (2) place fed points into dead slots in increasing index.
@@ -722,13 +765,9 @@ __global__ void __launch_bounds__(32) klt_feed_place(float4* __restrict__ buf, i
 // advanceFrame (v3d_gpuklt.h:252-259) for a strict subset of a group's cameras: the O(1) flip of
 // the pyramid buffers cannot apply to part of a group, so the cameras' slices of the two buffers
 // are exchanged (an exchange, not a copy: a second advance swaps them back, as the reference's
-// double swap does) and their feature slice is copied dst -> src.  grid (any, n).
+// double swap does) and their feature slice is copied dst -> src (F = 0: pyramids only).
+// grid (any, n).
 // ------------------------------------------------------------------------------------------
-struct KltCamList {
-  int n;
-  int cam[64];
-};
-
 __global__ void klt_advance_cams(float4* __restrict__ pyrA, float4* __restrict__ pyrB, long long pyrStride,
                                  const float4* __restrict__ dst, float4* __restrict__ src, int F,
                                  KltCamList L) {

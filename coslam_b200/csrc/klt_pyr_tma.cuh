@@ -46,7 +46,7 @@ klt_pyr_down_tma(const __grid_constant__ CUtensorMap srcMap, const __grid_consta
   const int ox = blockIdx.x * PT_TW, oy = blockIdx.y * PT_TH;
   if (MIXED) {
     const int Wc = __ldg(&cams[cam].W), Hc = __ldg(&cams[cam].H);
-    if (ox >= (Wc >> level) || oy >= (Hc >> level)) return;
+    if (ox >= (Wc >> level) || oy >= (Hc >> level) || !klt_in_stage<MIXED>(cams, cam, KLT_STAGE_PYR)) return;
     sw = Wc >> (level - 1);
     sh = Hc >> (level - 1);
   }

@@ -314,6 +314,7 @@ klt_gain_pass(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1, 
               const float4* __restrict__ X0buf, const float4* __restrict__ in, float4* __restrict__ out,
               const int* __restrict__ nbr, KltTrackParams P, int firstPass) {
   const int cam = blockIdx.y;
+  if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) return;
   const int2 ext = klt_extent<MIXED>(cams, cam, P.W, P.H);
   const int Wc = ext.x, Hc = ext.y;
   const int w = Wc >> level, h = Hc >> level;
@@ -397,6 +398,17 @@ struct KltTail {
 constexpr int KLT_FUSED_THREADS = KLT_FUSED_THREADS_N;  // 16 lane groups per CTA
 constexpr int KLT_GPB = KLT_FUSED_THREADS / KLT_G;
 
+// X0 of an item of klt_gain_fused.  MIXED: an item of a camera outside the tracker stage reads as a
+// dead slot (x < 0), so it stages, loads and accumulates nothing; it also neither waits for nor
+// publishes records and writes no result (the stage is re-read there, see below).
+template <bool MIXED>
+__device__ __forceinline__ float4 klt_fused_x0(const float4* __restrict__ X0buf, const KltCam* __restrict__ cams,
+                                               int item, int cam) {
+  float4 x0 = X0buf[item];
+  if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) x0.x = -1.0f;
+  return x0;
+}
+
 template <int HWC, bool MIXED>
 __global__ void __launch_bounds__(KLT_FUSED_THREADS, KLT_FUSED_MINBLOCKS)
 klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
@@ -423,7 +435,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   const bool active0 = q < T;
   const int item0 = active0 ? q : T - 1;
   const int cam0 = item0 / F, slot0 = item0 - cam0 * F;
-  const float4 x00 = X0buf[item0];
+  const float4 x00 = klt_fused_x0<MIXED>(X0buf, cams, item0, cam0);
   const int wsA0 = waitset[slot0 * 16 + gl], wsB0 = waitset[slot0 * 16 + 8 + gl];
   // MIXED: the resident item's camera, packed W | H << 16 into one register
   const unsigned wh0 = MIXED ? (unsigned)__ldg(&cams[cam0].W) | ((unsigned)__ldg(&cams[cam0].H) << 16) : 0u;
@@ -469,7 +481,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
           if (!active) item = T - 1;
           cam = item / F;
           const int slot = item - cam * F;
-          x0 = X0buf[item];
+          x0 = klt_fused_x0<MIXED>(X0buf, cams, item, cam);
           wsA = waitset[slot * 16 + gl];
           wsB = waitset[slot * 16 + 8 + gl];
         }
@@ -707,7 +719,9 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         float bn = 1.0f;
         if (pass > 1) {
           bn = -1.0f;
-          if (active) {
+          // an item of a camera outside the tracker stage (MIXED) neither waits nor writes; the
+          // stage is read where it is needed, not held in a register across the pixel loop
+          if (active && klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) {
             while ((int)(va >> 32) < need) {
               va = ld_relaxed_u64(ra);
               if ((int)(va >> 32) >= need) break;
@@ -728,7 +742,7 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                                      klt_finish_params<MIXED>(Plax, Pstrict, strict, Wc, Hc));
         if (pre_invalid) res = make_float4(-1.f, -1.f, -1.f, 0.f);
         if (staged) cur0 = res;
-        if (gl == 0 && active) {
+        if (gl == 0 && active && klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) {
           if (pass == LV.n * nIter) {
             out[item] = res;
             if (tail.dest) {  // v3d_gpuklt.cpp:872-888 and :475-500, see klt_status / klt_suppress
@@ -805,6 +819,7 @@ klt_track_2x2_tiled(const float4* __restrict__ pyr0, const float4* __restrict__ 
   const int gl = threadIdx.x & (KLT_G - 1);
   const int grp = threadIdx.x / KLT_G;
   const int cam = blockIdx.y;
+  if (!klt_in_stage<MIXED>(cams, cam, KLT_STAGE_TRACK)) return;
   int slot = blockIdx.x * 16 + grp;
   const bool active = slot < P.F;
   if (!active) slot = P.F - 1;  // keep the warp complete for the shuffles

@@ -7,6 +7,11 @@ import numpy as np
 COSL_OK = 0
 COSL_BA_INFOSZ = 16
 COSL_KLT_COMPAT_ITER5 = 1
+# ops of cosl_klt_group_step
+COSL_KLT_OP_SKIP = 0
+COSL_KLT_OP_FIRST = 1
+COSL_KLT_OP_TRACK = 2
+COSL_KLT_OP_NEXT = 3
 
 
 class KltConfig(C.Structure):

@@ -190,6 +190,31 @@ int cosl_klt_group_advance_cams(cosl_klt* h, const uint8_t* cams);
 int cosl_klt_group_first_present(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                                  const int* nPresent, const float* const* present3,
                                  cosl_klt_feature* const* dest, int* nDetected);
+/* A frame with an op of its own for each camera: GPUKLT::next with a track / re-detect cadence
+ * (tracking/GPUKLT.cpp:144-161 picks track() or redetect() from a frame counter), or a rig whose
+ * cameras do not all have a frame at every step.  ops[c] is one of: */
+enum { COSL_KLT_OP_SKIP = 0,   /* camera not addressed: image not read, state untouched          */
+       COSL_KLT_OP_FIRST = 1,  /* detect + advanceFrame      (GPUKLT::first, GPUKLT.cpp:133-142)  */
+       COSL_KLT_OP_TRACK = 2,  /* track + advanceFrame       (GPUKLT::next, track branch :153-158) */
+       COSL_KLT_OP_NEXT = 3 }; /* redetect + advanceFrame    (GPUKLT::next, :149-152)             */
+/* Camera c addressed with an op behaves bit for bit like a single-camera tracker that receives the
+ * matching call followed by cosl_klt_advance: its table, its count and every later frame.  n[c] is
+ * what that call returns (FIRST: nDetected, TRACK: nPresent, NEXT: nNewFeatures).  A skipped camera
+ * keeps all of its state (both pyramids, feature table, gains, the level-0 record of
+ * cosl_klt_debug_pyramid); imgs[c] may then be NULL and dest[c] / n[c] are not written.  Every op
+ * equal is exactly cosl_klt_group_first / group_next (or track + advance for every camera); all
+ * SKIP returns COSL_OK and launches nothing.  Otherwise one launch per kernel serves every
+ * addressed camera, and a camera gets the work of its op's stages only.  An op outside the four
+ * values or a NULL image of an addressed camera gives COSL_E_INVALID; frames submitted with
+ * cosl_klt_group_submit and not yet collected give COSL_E_STATE.  imgs, pitch, dest: as in
+ * cosl_klt_group_next. */
+int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch,
+                        cosl_klt_feature* const* dest, int* n);
+/* Same with device images, as cosl_klt_group_next_dev: no host transfer, no synchronise (a step
+ * whose ops differ copies its small per-camera op table from one of two pinned buffers, and waits
+ * for the copy made two such steps earlier only when the host runs that far ahead of the group's
+ * streams).  cosl_klt_group_fetch then hands back the tables and counts of the addressed cameras. */
+int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* const* dimgs, size_t pitch);
 /* Frame-pipelined form of cosl_klt_group_next (ingest half of SURVEY.md 8f-4; what
  * SingleSLAM::grabReadFrame + GPUKLT::next become when the next frame is already decoded,
  * app/SL_SingleSLAM.cpp:317-327, tracking/GPUKLT.cpp:144-161): submit() enqueues upload, kernels and
