@@ -3,6 +3,7 @@
 This is plumbing for tests/ and bench.py -- the product is the shared library.  There is NO CPU
 fallback: if the library is missing, importing this module raises; if no CUDA device is present,
 the first call that needs one returns COSL_E_CUDA and raises CoslError."""
+import collections
 import ctypes as C
 import os
 
@@ -54,6 +55,7 @@ def _load():
     L.cosl_klt_group_fetch.argtypes = [vp, vp, vp]
     L.cosl_klt_group_sync.argtypes = [vp]
     L.cosl_klt_group_submit.argtypes = [vp, vp, C.c_size_t]
+    L.cosl_klt_group_submit_step.argtypes = [vp, vp, vp, C.c_size_t]
     L.cosl_klt_group_collect.argtypes = [vp, vp, vp]
     L.cosl_klt_stream.argtypes = [vp]
     L.cosl_klt_stream.restype = vp
@@ -232,6 +234,8 @@ class KltGroup:
         self.feats = np.zeros((n_cams, self.F), FEAT_DTYPE)
         self.counts = np.zeros(n_cams, np.int32)
         self._dest = (C.c_void_p * n_cams)(*[self.feats[c].ctypes.data for c in range(n_cams)])
+        # ops of each submitted frame not yet collected, oldest first (None: a submit)
+        self._in_flight = collections.deque()
 
     def close(self):
         if getattr(self, "h", None):
@@ -330,9 +334,8 @@ class KltGroup:
         counts = [None if o == COSL_KLT_OP_SKIP else int(self.counts[c]) for c, o in enumerate(ops)]
         return tables, counts
 
-    def step(self, ops, imgs):
-        """cosl_klt_group_step: ops[c] in COSL_KLT_OP_* for camera c; imgs[c] its frame, or None
-        for a skipped camera.  Returns (tables, counts), None for a skipped camera."""
+    def _step_args(self, ops, imgs):
+        """(ops, pointer array, pitch) of a step: imgs[c] is camera c's frame, None if skipped"""
         ops = self._ops(ops)
         addr = [im for im, o in zip(imgs, ops) if o != COSL_KLT_OP_SKIP]
         ptrs = (C.c_void_p * self.C)()
@@ -353,6 +356,12 @@ class KltGroup:
                 pitch = 0
             for c, (im, o) in enumerate(zip(imgs, ops)):
                 ptrs[c] = None if o == COSL_KLT_OP_SKIP else im.ctypes.data
+        return ops, ptrs, pitch
+
+    def step(self, ops, imgs):
+        """cosl_klt_group_step: ops[c] in COSL_KLT_OP_* for camera c; imgs[c] its frame, or None
+        for a skipped camera.  Returns (tables, counts), None for a skipped camera."""
+        ops, ptrs, pitch = self._step_args(ops, imgs)
         _ck(LIB.cosl_klt_group_step(self.h, _ptr(ops), ptrs, pitch, self._dest, _ptr(self.counts)))
         return self._step_result(ops)
 
@@ -373,14 +382,26 @@ class KltGroup:
     def submit_raw(self, ptrs_pitch):
         """cosl_klt_group_submit: enqueue one frame (pointer array from host_ptrs()) and return."""
         _ck(LIB.cosl_klt_group_submit(self.h, ptrs_pitch[0], ptrs_pitch[1]))
+        self._in_flight.append(None)
 
     def submit(self, imgs):
         self.submit_raw(self._imgs(imgs))
 
+    def submit_step(self, ops, imgs):
+        """cosl_klt_group_submit_step: enqueue the step of step(ops, imgs) and return; collect()
+        hands back its tables.  The addressed frames must stay untouched until then."""
+        ops, ptrs, pitch = self._step_args(ops, imgs)
+        _ck(LIB.cosl_klt_group_submit_step(self.h, _ptr(ops), ptrs, pitch))
+        self._in_flight.append(ops)
+
     def collect(self):
-        """cosl_klt_group_collect: wait for the oldest submitted frame, return its tables."""
+        """cosl_klt_group_collect: wait for the oldest submitted frame and return its tables: (feats,
+        counts) for a submit, (tables, counts) with None for a skipped camera for a submit_step."""
         _ck(LIB.cosl_klt_group_collect(self.h, self._dest, _ptr(self.counts)))
-        return self.feats, self.counts
+        ops = self._in_flight.popleft()
+        if ops is None:
+            return self.feats, self.counts
+        return self._step_result(ops)
 
     def stream(self):
         return LIB.cosl_klt_stream(self.h)

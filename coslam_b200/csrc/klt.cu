@@ -94,10 +94,12 @@ struct cosl_klt {
   int* h_counters = nullptr;
   float4* h_present = nullptr;
   int* h_nPresent = nullptr;
-  // frame-pipelined ingest (cosl_klt_group_submit / _collect): two result slots, completion events
+  // frame-pipelined ingest (cosl_klt_group_submit / _submit_step / _collect): two result slots,
+  // completion events, and the ops of the frame each slot holds (all NEXT for a submit)
   cosl_klt_feature* h_featQ[2] = {nullptr, nullptr};
   int* h_cntQ[2] = {nullptr, nullptr};
   cudaEvent_t evDone[2] = {nullptr, nullptr};
+  uint8_t opsQ[2][64];
   unsigned subSeq = 0;
   int nInFlight = 0;
   bool havePrev = false;
@@ -1021,12 +1023,13 @@ int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t
 }
 
 // Camera c's table of `feat` -> dest[c] and its count counters[8c + 2] -> n[c], each where given.
-// After a step (g->stepOpsValid): the addressed cameras only, a tracked-only camera's count being
-// its live tracks (counters[8c + 0], what track() returns).
-void copy_out(const cosl_klt* g, const cosl_klt_feature* feat, const int* counters,
+// ops: the step the tables come from (nullptr: a frame of one kind for every camera): the addressed
+// cameras only, a tracked-only camera's count being its live tracks (counters[8c + 0], what track()
+// returns).
+void copy_out(const cosl_klt* g, const cosl_klt_feature* feat, const int* counters, const uint8_t* ops,
               cosl_klt_feature* const* dest, int* n) {
   for (int c = 0; c < g->C; ++c) {
-    const int op = g->stepOpsValid ? g->stepOps[c] : COSL_KLT_OP_NEXT;
+    const int op = ops ? ops[c] : COSL_KLT_OP_NEXT;
     if (op == COSL_KLT_OP_SKIP) continue;
     if (dest && dest[c]) std::memcpy(dest[c], feat + (size_t)c * g->F, sizeof(cosl_klt_feature) * g->F);
     if (n) n[c] = counters[8 * c + (op == COSL_KLT_OP_TRACK ? 0 : 2)];
@@ -1164,7 +1167,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, FRAME_DETECT, imgs, pitch, cudaMemcpyHostToDevice, maxPresent, false));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, &dest, nDetected);
+  copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nDetected);
   return COSL_OK;
 }
 
@@ -1176,7 +1179,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, false));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, &dest, nNewFeatures);
+  copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nNewFeatures);
   return COSL_OK;
 }
 
@@ -1188,7 +1191,7 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, FRAME_TRACK, imgs, pitch, cudaMemcpyHostToDevice, 0, false));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, &dest, nullptr);
+  copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nullptr);
   *nPresent = h->h_counters[0];
   return COSL_OK;
 }
@@ -1235,7 +1238,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
   if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
   COSL_TRY(run_frame(h, FRAME_DETECT, imgs, pitch, cudaMemcpyHostToDevice, maxPresent, true));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, dest, nDetected);
+  copy_out(h, h->h_feat, h->h_counters, nullptr, dest, nDetected);
   return COSL_OK;
 }
 
@@ -1285,7 +1288,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
   COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, dest, nNew);
+  copy_out(h, h->h_feat, h->h_counters, nullptr, dest, nNew);
   return COSL_OK;
 }
 
@@ -1315,7 +1318,7 @@ int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* i
   COSL_TRY(check_step(h, ops, imgs, pitch, "group_step"));
   COSL_TRY(run_step(h, ops, imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, dest, n);
+  copy_out(h, h->h_feat, h->h_counters, ops, dest, n);
   return COSL_OK;
 }
 
@@ -1329,7 +1332,7 @@ int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* cons
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, dest, nNew);
+  copy_out(h, h->h_feat, h->h_counters, h->stepOpsValid ? h->stepOps : nullptr, dest, nNew);
   return COSL_OK;
 }
 
@@ -1338,26 +1341,61 @@ int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) 
 // submitted frame.  With submit(n+1) called before collect(n), the image upload of frame n + 1 runs on
 // the copy stream under the tracker / detector kernels of frame n (it only waits for frame n's front
 // pass, which is the last reader of the image buffer), and its pyramid under frame n's detector
-// (run_frame).
-int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch) {
-  KLT_ENTER(h)
-  if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_submit: bad argument");
-  if (h->nInFlight >= 2) return set_error(COSL_E_STATE, "group_submit: two frames in flight, collect one first");
-  const int slot = (int)(h->subSeq & 1u);
-  if (!h->h_featQ[slot]) {
-    COSL_CUDA(cudaMallocHost(&h->h_featQ[slot], sizeof(cosl_klt_feature) * (size_t)h->F * h->C));
-    COSL_CUDA(cudaMallocHost(&h->h_cntQ[slot], sizeof(int) * 8 * h->C));
-    COSL_CUDA(cudaEventCreateWithFlags(&h->evDone[slot], cudaEventDisableTiming));
+// (run_frame).  submit_step() does the same for a step (run_step); both share the two slots and the
+// FIFO, and the slot keeps the frame's ops for collect().
+//
+// The result slot of the next submitted frame, allocated on first use.
+static int submit_slot(cosl_klt* h, const char* name, int* slot) {
+  if (h->nInFlight >= 2) return set_error(COSL_E_STATE, "%s: two frames in flight, collect one first", name);
+  const int s = (int)(h->subSeq & 1u);
+  if (!h->h_featQ[s]) {
+    COSL_CUDA(cudaMallocHost(&h->h_featQ[s], sizeof(cosl_klt_feature) * (size_t)h->F * h->C));
+    COSL_CUDA(cudaMallocHost(&h->h_cntQ[s], sizeof(int) * 8 * h->C));
+    COSL_CUDA(cudaEventCreateWithFlags(&h->evDone[s], cudaEventDisableTiming));
   }
-  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
-  COSL_CUDA(cudaMemcpyAsync(h->h_featQ[slot], h->d_feat, sizeof(cosl_klt_feature) * (size_t)h->F * h->C,
-                            cudaMemcpyDeviceToHost, h->stream));
-  COSL_CUDA(cudaMemcpyAsync(h->h_cntQ[slot], h->d_counters[h->par], sizeof(int) * 8 * h->C,
-                            cudaMemcpyDeviceToHost, h->stream));
+  *slot = s;
+  return COSL_OK;
+}
+
+// The read-back of the frame just enqueued into `slot` (whose opsQ is set) and its place in the
+// FIFO.  An all-SKIP step has nothing to read back: its event alone keeps the order.
+static int submit_readback(cosl_klt* h, int slot) {
+  bool any = false;
+  for (int c = 0; c < h->C; ++c) any = any || h->opsQ[slot][c] != COSL_KLT_OP_SKIP;
+  if (any) {
+    COSL_CUDA(cudaMemcpyAsync(h->h_featQ[slot], h->d_feat, sizeof(cosl_klt_feature) * (size_t)h->F * h->C,
+                              cudaMemcpyDeviceToHost, h->stream));
+    COSL_CUDA(cudaMemcpyAsync(h->h_cntQ[slot], h->d_counters[h->par], sizeof(int) * 8 * h->C,
+                              cudaMemcpyDeviceToHost, h->stream));
+  }
   COSL_CUDA(cudaEventRecord(h->evDone[slot], h->stream));
   ++h->subSeq;
   ++h->nInFlight;
   return COSL_OK;
+}
+
+int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch) {
+  KLT_ENTER(h)
+  if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_submit: bad argument");
+  int slot = 0;
+  COSL_TRY(submit_slot(h, "group_submit", &slot));
+  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
+  std::memset(h->opsQ[slot], COSL_KLT_OP_NEXT, h->C);
+  return submit_readback(h, slot);
+}
+
+// A step's op table comes from one of two pinned host tables (run_step); the host waits for the copy
+// out of the table it reuses, made two mixed steps earlier.  At most two frames are in flight, so when
+// that step was submitted it has been collected (the copy is done); only a step_dev can leave it
+// pending, and its copy is already enqueued.
+int cosl_klt_group_submit_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch) {
+  KLT_ENTER(h)
+  COSL_TRY(check_step(h, ops, imgs, pitch, "group_submit_step"));
+  int slot = 0;
+  COSL_TRY(submit_slot(h, "group_submit_step", &slot));
+  COSL_TRY(run_step(h, ops, imgs, pitch, cudaMemcpyHostToDevice));
+  std::memcpy(h->opsQ[slot], ops, h->C);
+  return submit_readback(h, slot);
 }
 
 int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {
@@ -1366,7 +1404,7 @@ int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew
   const int slot = (int)((h->subSeq - (unsigned)h->nInFlight) & 1u);
   COSL_CUDA(cudaEventSynchronize(h->evDone[slot]));
   --h->nInFlight;
-  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], dest, nNew);
+  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], h->opsQ[slot], dest, nNew);
   return COSL_OK;
 }
 

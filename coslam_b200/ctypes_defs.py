@@ -7,7 +7,7 @@ import numpy as np
 COSL_OK = 0
 COSL_BA_INFOSZ = 16
 COSL_KLT_COMPAT_ITER5 = 1
-# ops of cosl_klt_group_step
+# ops of cosl_klt_group_step / _submit_step
 COSL_KLT_OP_SKIP = 0
 COSL_KLT_OP_FIRST = 1
 COSL_KLT_OP_TRACK = 2

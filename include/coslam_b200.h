@@ -166,7 +166,7 @@ int cosl_klt_group_sync(cosl_klt* h);
 /* Per-camera forms of the calls a multi-camera CoSLAM loop makes besides next().  Each camera of the
  * group behaves bit for bit like a single-camera tracker that receives the same calls; cameras a
  * call does not address keep their state.  All three return COSL_E_STATE while frames submitted
- * with cosl_klt_group_submit are not yet collected.
+ * with cosl_klt_group_submit or _submit_step are not yet collected.
  *
  * KLT_SequenceTracker::feedExternFeaturePoints (v3d_gpuklt.cpp:808-855) for the cameras with
  * npts[c] >= 0; what NewMapPtsNCC::output -> SingleSLAM::feedExtraFeatPtsToTracker ->
@@ -206,8 +206,8 @@ enum { COSL_KLT_OP_SKIP = 0,   /* camera not addressed: image not read, state un
  * SKIP returns COSL_OK and launches nothing.  Otherwise one launch per kernel serves every
  * addressed camera, and a camera gets the work of its op's stages only.  An op outside the four
  * values or a NULL image of an addressed camera gives COSL_E_INVALID; frames submitted with
- * cosl_klt_group_submit and not yet collected give COSL_E_STATE.  imgs, pitch, dest: as in
- * cosl_klt_group_next. */
+ * cosl_klt_group_submit or _submit_step and not yet collected give COSL_E_STATE.  imgs, pitch,
+ * dest: as in cosl_klt_group_next. */
 int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch,
                         cosl_klt_feature* const* dest, int* n);
 /* Same with device images, as cosl_klt_group_next_dev: no host transfer, no synchronise (a step
@@ -223,6 +223,20 @@ int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* cons
  * before collect(n) overlaps the upload of frame n+1 with the kernels of frame n.  The image
  * buffers of a submitted frame must stay untouched until that frame has been collected. */
 int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch);
+/* Frame-pipelined form of cosl_klt_group_step: enqueues what group_step does plus the read-back of
+ * the step, and returns.  ops, imgs, pitch and their checks (COSL_E_INVALID) are group_step's.  It
+ * shares the two frames in flight and their order with cosl_klt_group_submit, and the two may be
+ * mixed; a third frame gives COSL_E_STATE.  An all-SKIP step launches nothing but still counts as a
+ * submitted frame, whose collect writes nothing.  The image buffers of the addressed cameras must
+ * stay untouched until the step has been collected.  Like submit it does not wait for the device,
+ * with one exception: a step whose ops differ reuses the pinned op table of the step two such steps
+ * earlier, and when that step was given to cosl_klt_group_step_dev and its front pass has not yet
+ * started, this call waits for it (as step_dev itself does). */
+int cosl_klt_group_submit_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch);
+/* Waits for the oldest frame submitted by either call.  For a submit, every camera's dest[c] / nNew[c]
+ * are written as by cosl_klt_group_next; for a submit_step only the addressed cameras' are, with n[c]
+ * as cosl_klt_group_step documents it (FIRST: nDetected, TRACK: nPresent, NEXT: nNewFeatures); a
+ * skipped camera's entries are left untouched.  COSL_E_STATE when nothing is in flight. */
 int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew);
 /* CUDA stream (cudaStream_t as void*) the group launches on; lets callers time with events.  Parts of
  * a frame run on side streams, but every call joins them into this stream before it returns: work

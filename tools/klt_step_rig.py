@@ -1,4 +1,4 @@
-"""Per-camera frame ops (cosl_klt_group_step) on c3: 4 x 1280x720, 2000 slots, live settings.
+"""Per-camera frame ops (cosl_klt_group_step, _submit_step) on c3: 4 x 1280x720, 2000 slots, live settings.
 Prints one JSON line (card name and power limit included).
 
   all_next   all-NEXT steps against cosl_klt_group_next of the same build, and (--parent-lib) of
@@ -8,11 +8,15 @@ Prints one JSON line (card name and power limit included).
              all-NEXT group_next frames
   skip_rig   camera 3 skipped on every other step (the others re-detect): group_step against
              4 single trackers that get the same frames, and against all-NEXT
+  pipelined  the cadence and the skip rig through cosl_klt_group_submit_step / _collect (step n+1
+             submitted before step n is collected), against their group_step arms; and all-NEXT
+             frames through cosl_klt_group_submit / _collect, the pipelined form of group_next
   exchange   device time (CUDA events) of exchanging one camera's pyramid slices
              (cosl_klt_group_advance_cams of camera 3), which a step skipping one camera of four pays
 
-Frames come from pinned host buffers; every arm synchronises once per frame set.  Round 0 of each
-arm is a warm-up; the arms alternate within a round.
+Frames come from pinned host buffers; every synchronous arm synchronises once per frame set, every
+pipelined arm collects (reads back and waits for) every frame set.  Round 0 of each arm is a
+warm-up; the arms alternate within a round.
 
   python tools/klt_step_rig.py [--frames 40] [--rounds 3] [--parent-lib PATH]"""
 import argparse
@@ -72,6 +76,28 @@ def main():
             step(ops, f + 1)
         return time.perf_counter() - t0, grp.feats.copy()
 
+    def submit_step(ops, k):
+        ptrs, pitch = args[fidx(k)]
+        api._ck(api.LIB.cosl_klt_group_submit_step(grp.h, ops.ctypes.data, ptrs, pitch))
+
+    def submit_next(_ops, k):
+        ptrs, pitch = args[fidx(k)]
+        api._ck(api.LIB.cosl_klt_group_submit(grp.h, ptrs, pitch))
+
+    def collect():
+        api._ck(api.LIB.cosl_klt_group_collect(grp.h, dest, counts))
+
+    def group_pipelined(sched, submit):
+        """frame set f + 1 submitted before f is collected; every frame set collected"""
+        grp.first(host[0])
+        t0 = time.perf_counter()
+        submit(sched[0], 1)
+        for f in range(1, len(sched)):
+            submit(sched[f], f + 1)
+            collect()
+        collect()
+        return time.perf_counter() - t0, grp.feats.copy()
+
     def group_next():
         grp.first(host[0])
         t0 = time.perf_counter()
@@ -126,12 +152,16 @@ def main():
         "cadence_singles": lambda: singles_sched(cadence),
         "skip_rig_step": lambda: group_sched(skip_rig),
         "skip_rig_singles": lambda: singles_sched(skip_rig),
+        "cadence_submit_step": lambda: group_pipelined(cadence, submit_step),
+        "skip_rig_submit_step": lambda: group_pipelined(skip_rig, submit_step),
+        "all_next_submit": lambda: group_pipelined([ops_next] * n_frames, submit_next),
     }
     if parent:
         arms["all_next_parent_group_next"] = parent_next
     times = {k: [] for k in arms}
     same = {"all_next_step_vs_group_next": True, "cadence_step_vs_singles": True,
-            "skip_rig_step_vs_singles": True}
+            "skip_rig_step_vs_singles": True, "cadence_submit_step_vs_step": True,
+            "skip_rig_submit_step_vs_step": True, "all_next_submit_vs_group_next": True}
     if parent:
         same["all_next_group_next_vs_parent"] = True
     stream = torch.cuda.ExternalStream(grp.stream(), device=a.device)
@@ -157,6 +187,11 @@ def main():
         same["all_next_step_vs_group_next"] &= out["all_next_step"].tobytes() == out["all_next_group_next"].tobytes()
         same["cadence_step_vs_singles"] &= out["cadence_step"].tobytes() == out["cadence_singles"].tobytes()
         same["skip_rig_step_vs_singles"] &= out["skip_rig_step"].tobytes() == out["skip_rig_singles"].tobytes()
+        same["cadence_submit_step_vs_step"] &= out["cadence_submit_step"].tobytes() == out["cadence_step"].tobytes()
+        same["skip_rig_submit_step_vs_step"] &= (out["skip_rig_submit_step"].tobytes()
+                                                 == out["skip_rig_step"].tobytes())
+        same["all_next_submit_vs_group_next"] &= (out["all_next_submit"].tobytes()
+                                                  == out["all_next_group_next"].tobytes())
         if r:
             exch.append(exchange_ms())
         if parent:
@@ -177,12 +212,16 @@ def main():
                    "cadence_step_over_all_next": m["cadence_step"] / m["all_next_group_next"],
                    "skip_rig_singles_over_step": m["skip_rig_singles"] / m["skip_rig_step"],
                    "skip_rig_step_over_all_next": m["skip_rig_step"] / m["all_next_group_next"],
+                   "cadence_submit_step_over_step": m["cadence_submit_step"] / m["cadence_step"],
+                   "skip_rig_submit_step_over_step": m["skip_rig_submit_step"] / m["skip_rig_step"],
+                   "cadence_submit_step_over_all_next_submit": m["cadence_submit_step"] / m["all_next_submit"],
                    **({"group_next_over_parent": m["all_next_group_next"] / m["all_next_parent_group_next"]}
                       if parent else {})},
         "exchange_one_camera_device_ms": {"ms": float(np.mean(exch)), "range": [min(exch), max(exch)]},
         "bit_identical": same,
         "config": {"workload": f"c3 ({KC} x {W}x{H}, {F} slots, live settings), first + {n_frames} frame sets "
-                               "through pinned host buffers, one synchronise per frame set",
+                               "through pinned host buffers, one synchronise (synchronous arms) or one "
+                               "collect (pipelined arms) per frame set",
                    "cadence": "4 x TRACK + 1 x NEXT on every camera",
                    "skip_rig": "camera 3 skipped on every other step, the others NEXT",
                    "rounds": a.rounds, "parent_lib": bool(parent)},
