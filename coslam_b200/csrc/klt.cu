@@ -26,12 +26,14 @@ struct cosl_klt {
   bool pitchZeroOK = false;  // made by cosl_klt_group_create_sizes: pitch 0 = each camera's own width
   KltCam hcam[64];           // per camera: extent and detector window (camera 0's: the uniform case)
   KltCam* d_cams = nullptr;  // device copy of hcam, read by the kernels of a mixed group
-  // cosl_klt_group_step: hcam with each camera's stages, written to one of two pinned tables and
-  // copied to the device table of the same index, in turn (the front pass of a step runs while the
-  // previous step's detector still reads its table); evStepTab[t] follows the last copy from table t
-  KltCam* h_stepCams[2] = {nullptr, nullptr};
-  KltCam* d_stepCams[2] = {nullptr, nullptr};
-  cudaEvent_t evStepTab[2] = {nullptr, nullptr};
+  // cosl_klt_group_step: hcam with each camera's stages, written to one of three pinned tables and
+  // copied to the device table of the same index, in turn (the front pass of a step may run while
+  // the detectors of the two steps before it still read their tables); evStepTab[t] follows the last
+  // copy from table t, evStepFence[t] the last group-stream reader of device table t
+  KltCam* h_stepCams[3] = {nullptr, nullptr, nullptr};
+  KltCam* d_stepCams[3] = {nullptr, nullptr, nullptr};
+  cudaEvent_t evStepTab[3] = {nullptr, nullptr, nullptr};
+  cudaEvent_t evStepFence[3] = {nullptr, nullptr, nullptr};
   int stepTab = 0;
   // the ops of the last frame call when it was a step: what cosl_klt_group_fetch hands back
   uint8_t stepOps[64];
@@ -40,11 +42,15 @@ struct cosl_klt {
   float trackMargin = 4.f, conv = 0.1f, ssd = 5000.f, detectMargin = 10.f;
   cudaStream_t stream = nullptr;
   // image copies, klt_front and the pyramid tail run on the front stream, so that frame n+1's
-  // pyramid is built while frame n's detector runs on `stream`.  The front stream starts a frame
-  // after evFence, which `stream` records behind the last stage that reads what the front stream
-  // overwrites (run_frame); `stream` waits for evTail before the frame's tracker or detector.
+  // pyramid is built while frames n and n-1 still run on `stream`.  Before a frame, the front stream
+  // waits for the fence of each buffer it writes (evPyr, evPar, evStepFence), which `stream` records
+  // behind the last stage that reads or writes that buffer (run_frame), and for evCams when
+  // update_cameras has rewritten d_cams since; `stream` waits for evTail before the frame's tracker
+  // or detector.
   cudaStream_t frontStream = nullptr;
-  cudaEvent_t evFence = nullptr, evTail = nullptr;
+  cudaEvent_t evPyr[3] = {nullptr, nullptr, nullptr}, evPar[3] = {nullptr, nullptr, nullptr};
+  cudaEvent_t evCams = nullptr, evTail = nullptr;
+  bool camsDirty = false;
   // host uploads run on their own stream, one event per camera, so that klt_front of camera c
   // overlaps the copy of camera c+1 (cosl_klt_group_next path)
   cudaStream_t copyStream = nullptr;
@@ -64,27 +70,34 @@ struct cosl_klt {
   int candCap = 0, smemKeys = 0;
   // device memory
   uint8_t* d_img = nullptr;
-  float4* d_pyr[2] = {nullptr, nullptr};
+  // Three pyramid buffers.  p0 holds the previous frame's pyramid (the tracker's P0) and p1 the
+  // current one (P1), as in the reference's two-buffer tracker; `nxt` is the buffer the next front
+  // pass writes, p1 itself or, after an advance, the third buffer.  An advance makes p1 the new p0
+  // and the old p0 the new p1 (the reference's swap), and points nxt at the third buffer, whose last
+  // reader is the tracker of two frames back: so frame n+1's pyramid is built while frame n's tracker
+  // runs.  A front pass writes nxt and then p1 = nxt.
+  float4* d_pyr[3] = {nullptr, nullptr, nullptr};
+  int p0 = 0, p1 = 1, nxt = 1;
   // level 0 of camera c's slice of d_pyr[b] holds its frame (see build_pyramid); per camera because
   // cosl_klt_group_advance_cams exchanges single cameras' slices between the buffers
-  bool lv0Stored[2][64];
-  int cur = 1;  // pyr1 == d_pyr[cur]
-  // Two sets of what the front stream of frame n+1 writes while the detector of frame n still reads
-  // it: cornerness map, prelim list and counters.  A frame with a cornerness map switches to the
-  // other set; `par` is the set of the last frame (the one fetch and the debug reads see).
+  bool lv0Stored[3][64];
+  // Three sets of what the front stream of frame n+1 writes while the detectors of frames n and n-1
+  // may still read it: cornerness map, prelim list and counters.  A frame with a cornerness map
+  // moves on to the next set; `par` is the set of the last frame (the one fetch and the debug reads
+  // see).
   int par = 0;
-  float* d_corn[2] = {nullptr, nullptr};
+  float* d_corn[3] = {nullptr, nullptr, nullptr};
   float4 *d_src = nullptr, *d_dst = nullptr, *d_ping = nullptr, *d_pong = nullptr, *d_res = nullptr;
   float4* d_present = nullptr;
   int* d_nPresent = nullptr;  // [C] lengths of the present lists in d_present
   int* d_nbr = nullptr;
   unsigned long long* d_cand = nullptr;
-  unsigned* d_prelim[2] = {nullptr, nullptr};  // [C][prelimCap] packed (y << 16 | x) of 3x3 local maxima
+  unsigned* d_prelim[3] = {nullptr, nullptr, nullptr};  // [C][prelimCap] packed (y << 16 | x) of 3x3 maxima
   int prelimCap = 0;
   // [C][8]: [0] live tracks, [1] candidates, [2] returned count, [3] raw candidates, [4] prelim
   // (klt_kernels.cuh).  `stream` zeroes [0..3] of a frame; [4] belongs to the prefilter, which may
   // count before `stream` gets to the frame, so the front stream zeroes it.
-  int* d_counters[2] = {nullptr, nullptr};
+  int* d_counters[3] = {nullptr, nullptr, nullptr};
   cosl_klt_feature* d_feat = nullptr;
   // fed points (3 floats each), then their slots and the per-camera placed counts (ints)
   void* d_feedbuf = nullptr;
@@ -112,9 +125,9 @@ struct cosl_klt {
   int fusedBlocksMixed = 0;  // of the MIXED instantiation, which steps run on every group
   int numSM = 132;
   int verBase = 0;
-  // TMA descriptors of every pyramid level of both buffers: [buffer][level], load box (source of
-  // level + 1) and store box (destination of level - 1 -> level); klt_pyr_tma.cuh
-  CUtensorMap tmLoad[2][8], tmStore[2][8];
+  // TMA descriptors of every pyramid level of the three buffers: [buffer][level], load box (source
+  // of level + 1) and store box (destination of level - 1 -> level); klt_pyr_tma.cuh
+  CUtensorMap tmLoad[3][8], tmStore[3][8];
   SectionTimer timer;
   int secPyr = 0, secTrack = 0, secDetect = 0, secSelect = 0;
 };
@@ -151,7 +164,35 @@ static int update_cameras(cosl_klt* g) {
   // pageable source: the copy is staged before the call returns, so hcam may change again
   COSL_CUDA(cudaMemcpyAsync(g->d_cams, g->hcam, sizeof(KltCam) * g->C, cudaMemcpyHostToDevice, g->stream));
   // the next frame's front pass reads d_cams
-  COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
+  COSL_CUDA(cudaEventRecord(g->evCams, g->stream));
+  g->camsDirty = true;
+  return COSL_OK;
+}
+
+// the pyramid buffer b's fence: its last group-stream reader or writer so far
+static int fence_pyr(cosl_klt* g, int b) {
+  COSL_CUDA(cudaEventRecord(g->evPyr[b], g->stream));
+  return COSL_OK;
+}
+
+// The front stream's waits ahead of a frame whose front pass writes pyramid buffer nxt, the
+// counter set par (wantCorn) and, for a step, op table tab (-1: none).
+static int front_waits(cosl_klt* g, bool wantCorn, int tab) {
+  COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evPyr[g->nxt], 0));
+  if (wantCorn) COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evPar[g->par], 0));
+  if (tab >= 0) COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evStepFence[tab], 0));
+  if (g->camsDirty) {
+    COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evCams, 0));
+    g->camsDirty = false;
+  }
+  return COSL_OK;
+}
+
+// A frame with a cornerness map moves on to the next counter set; the set it leaves is fenced behind
+// everything enqueued on `stream` so far, which includes the read-back of the frame before.
+static int next_par(cosl_klt* g) {
+  COSL_CUDA(cudaEventRecord(g->evPar[g->par], g->stream));
+  g->par = (g->par + 1) % 3;
   return COSL_OK;
 }
 
@@ -176,7 +217,11 @@ int alloc_group(cosl_klt* g) {
   const int C = g->C, W = g->W, H = g->H, F = g->F;
   COSL_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
   COSL_CUDA(cudaStreamCreateWithFlags(&g->frontStream, cudaStreamNonBlocking));
-  COSL_CUDA(cudaEventCreateWithFlags(&g->evFence, cudaEventDisableTiming));
+  for (int b = 0; b < 3; ++b) {
+    COSL_CUDA(cudaEventCreateWithFlags(&g->evPyr[b], cudaEventDisableTiming));
+    COSL_CUDA(cudaEventCreateWithFlags(&g->evPar[b], cudaEventDisableTiming));
+  }
+  COSL_CUDA(cudaEventCreateWithFlags(&g->evCams, cudaEventDisableTiming));
   COSL_CUDA(cudaEventCreateWithFlags(&g->evTail, cudaEventDisableTiming));
   COSL_CUDA(cudaStreamCreateWithFlags(&g->copyStream, cudaStreamNonBlocking));
   COSL_CUDA(cudaEventCreateWithFlags(&g->evFront, cudaEventDisableTiming));
@@ -194,10 +239,11 @@ int alloc_group(cosl_klt* g) {
   g->imgPitch = ((size_t)W + 15) & ~(size_t)15;
   g->imgStride = g->imgPitch * H;
   COSL_CUDA(cudaMalloc(&g->d_cams, sizeof(KltCam) * C));
-  for (int t = 0; t < 2; ++t) {
+  for (int t = 0; t < 3; ++t) {
     COSL_CUDA(cudaMalloc(&g->d_stepCams[t], sizeof(KltCam) * C));
     COSL_CUDA(cudaMallocHost(&g->h_stepCams[t], sizeof(KltCam) * C));
     COSL_CUDA(cudaEventCreateWithFlags(&g->evStepTab[t], cudaEventDisableTiming));
+    COSL_CUDA(cudaEventCreateWithFlags(&g->evStepFence[t], cudaEventDisableTiming));
   }
   // candidate capacity: a strict (2r+1)^2 maximum admits at most one survivor per (r+1)^2 pixels
   // (of the largest camera, which bounds every camera's count)
@@ -208,12 +254,12 @@ int alloc_group(cosl_klt* g) {
   g->candCap = cap;
   g->smemKeys = std::min(cap, KLT_MAX_SMEM_KEYS);
   COSL_CUDA(cudaMalloc(&g->d_img, g->imgStride * C));
-  std::fill(&g->lv0Stored[0][0], &g->lv0Stored[0][0] + 2 * 64, true);
-  for (int b = 0; b < 2; ++b) {
+  std::fill(&g->lv0Stored[0][0], &g->lv0Stored[0][0] + 3 * 64, true);
+  for (int b = 0; b < 3; ++b) {
     COSL_CUDA(cudaMalloc(&g->d_pyr[b], sizeof(float4) * g->pyrStride * C));
     COSL_CUDA(cudaMemsetAsync(g->d_pyr[b], 0, sizeof(float4) * g->pyrStride * C, g->stream));
   }
-  for (int b = 0; b < 2; ++b) COSL_CUDA(cudaMalloc(&g->d_corn[b], sizeof(float) * (size_t)W * H * C));
+  for (int b = 0; b < 3; ++b) COSL_CUDA(cudaMalloc(&g->d_corn[b], sizeof(float) * (size_t)W * H * C));
   const size_t fbytes = sizeof(float4) * (size_t)F * C;
   float4** bufs[] = {&g->d_src, &g->d_dst, &g->d_ping, &g->d_pong, &g->d_res, &g->d_present};
   std::vector<float4> init((size_t)F * C, make_float4(-1.f, -1.f, 1.f, 0.f));
@@ -224,7 +270,7 @@ int alloc_group(cosl_klt* g) {
   COSL_CUDA(cudaMalloc(&g->d_cand, sizeof(unsigned long long) * (size_t)cap * C));
   // strict 3x3 maxima cannot be 8-adjacent: at most one per 2x2 block
   g->prelimCap = ((W + 1) / 2) * ((H + 1) / 2);
-  for (int b = 0; b < 2; ++b) {
+  for (int b = 0; b < 3; ++b) {
     COSL_CUDA(cudaMalloc(&g->d_prelim[b], sizeof(unsigned) * (size_t)g->prelimCap * C));
     COSL_CUDA(cudaMalloc(&g->d_counters[b], sizeof(int) * 8 * C));
     COSL_CUDA(cudaMemset(g->d_counters[b], 0, sizeof(int) * 8 * C));
@@ -303,7 +349,7 @@ int alloc_group(cosl_klt* g) {
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || !fn ||
         qr != cudaDriverEntryPointSuccess)
       return set_error(COSL_E_CUDA, "KLT pyramid: cuTensorMapEncodeTiled is not available");
-    for (int b = 0; b < 2; ++b)
+    for (int b = 0; b < 3; ++b)
       for (int l = 1; l < g->L; ++l) {
         // a level of the whole camera group: x = texels as pairs of 8-byte elements, y, camera
         const cuuint64_t dims[3] = {2ull * g->lvW[l], (cuuint64_t)g->lvH[l], (cuuint64_t)C};
@@ -342,15 +388,18 @@ void free_group(cosl_klt* g) {
   g->timer.destroy();
   cudaFree(g->d_img);
   cudaFree(g->d_cams);
-  for (int t = 0; t < 2; ++t) {
+  for (int t = 0; t < 3; ++t) {
     cudaFree(g->d_stepCams[t]);
     if (g->h_stepCams[t]) cudaFreeHost(g->h_stepCams[t]);
     if (g->evStepTab[t]) cudaEventDestroy(g->evStepTab[t]);
+    if (g->evStepFence[t]) cudaEventDestroy(g->evStepFence[t]);
+    cudaFree(g->d_pyr[t]);
+    cudaFree(g->d_corn[t]);
+    cudaFree(g->d_prelim[t]);
+    cudaFree(g->d_counters[t]);
+    if (g->evPyr[t]) cudaEventDestroy(g->evPyr[t]);
+    if (g->evPar[t]) cudaEventDestroy(g->evPar[t]);
   }
-  cudaFree(g->d_pyr[0]);
-  cudaFree(g->d_pyr[1]);
-  cudaFree(g->d_corn[0]);
-  cudaFree(g->d_corn[1]);
   cudaFree(g->d_src);
   cudaFree(g->d_dst);
   cudaFree(g->d_ping);
@@ -362,17 +411,13 @@ void free_group(cosl_klt* g) {
   if (g->auxStream) cudaStreamDestroy(g->auxStream);
   if (g->evPre) cudaEventDestroy(g->evPre);
   if (g->frontStream) cudaStreamDestroy(g->frontStream);
-  if (g->evFence) cudaEventDestroy(g->evFence);
+  if (g->evCams) cudaEventDestroy(g->evCams);
   if (g->evTail) cudaEventDestroy(g->evTail);
   if (g->copyStream) cudaStreamDestroy(g->copyStream);
   if (g->evFront) cudaEventDestroy(g->evFront);
   for (int c = 0; c < 64; ++c)
     if (g->evImg[c]) cudaEventDestroy(g->evImg[c]);
   cudaFree(g->d_cand);
-  for (int b = 0; b < 2; ++b) {
-    cudaFree(g->d_prelim[b]);
-    cudaFree(g->d_counters[b]);
-  }
   cudaFree(g->d_feat);
   cudaFree(g->d_feedbuf);
   cudaFree(g->d_state);
@@ -482,7 +527,7 @@ struct FramePlan {
 // front stream
 int build_pyramid(cosl_klt* g, const FramePlan& p) {
   cudaStream_t st = g->frontStream;
-  float4* P = g->d_pyr[g->cur];
+  float4* P = g->d_pyr[g->nxt];
   g->timer.begin(g->secPyr, st);
   // level 0 + level 1 + (optionally) the detector's cornerness map in one pass over the image
   FrontParams fp;
@@ -541,11 +586,12 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   // reset ahead of them on this stream and have no grid-dependency wait.
   for (int l = 2; l < g->L; ++l) {
     dim3 gl(div_up(g->lvW[l], PT_TW), div_up(g->lvH[l], PT_TH), g->C);
-    COSL_LAUNCH_PDL(KLT_SIZED(p.mixed, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->cur][l - 1],
-                    g->tmStore[g->cur][l], g->lvW[l - 1], g->lvH[l - 1], p.cams, l);
+    COSL_LAUNCH_PDL(KLT_SIZED(p.mixed, klt_pyr_down_tma), gl, 256, 0, st, g->tmLoad[g->nxt][l - 1],
+                    g->tmStore[g->nxt][l], g->lvW[l - 1], g->lvH[l - 1], p.cams, l);
   }
   g->timer.end(st);
   COSL_CUDA(cudaGetLastError());
+  g->p1 = g->nxt;
   return COSL_OK;
 }
 
@@ -580,10 +626,10 @@ KltTrackParams track_params(const cosl_klt* g, bool strict) {
 }
 
 // KLT_TrackerWithGain::trackFeaturesAndGain (v3d_gpuklt.cpp:205-305) /
-// KLT_Tracker::trackFeatures (:99-161); result -> d_res
+// KLT_Tracker::trackFeatures (:99-161); result -> d_res.  The caller fences both buffers after it.
 int run_tracker(cosl_klt* g, const FramePlan& p) {
-  const float4* P0 = g->d_pyr[1 - g->cur];
-  const float4* P1 = g->d_pyr[g->cur];
+  const float4* P0 = g->d_pyr[g->p0];
+  const float4* P1 = g->d_pyr[g->p1];
   const int wpb = 8;  // warps per block (2x2 tracker: one warp per slot)
   dim3 grid(div_up(g->F, wpb), g->C);
   dim3 gridHalf(div_up(g->F, 256 / KLT_G), g->C);  // gain tracker: one lane group per slot
@@ -729,32 +775,45 @@ int fetch_results(cosl_klt* g) {
   return COSL_OK;
 }
 
+// The pyramid half of advanceFrame: p1 becomes p0, and the old p0 becomes p1, as the reference swaps
+// its two pyramids.  The next front pass writes the third buffer, not p1, so it does not wait for
+// the tracker that read p0 and p1 (whose last frame might still be running).
+static void advance_pyramids(cosl_klt* g) {
+  std::swap(g->p0, g->p1);
+  g->nxt = 3 - g->p0 - g->p1;
+}
+
 int advance(cosl_klt* g) {
   // swapFeatureBuffers + swap pyramids (v3d_gpuklt.h:252-259); the feature buffer is copied, not
   // swapped, so a later feed() still sees the provided set (see DESIGN.md, quirk list)
   const size_t n = (size_t)g->F * g->C;
   COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, g->stream, g->d_dst, g->d_src, n);
-  g->cur = 1 - g->cur;
+  advance_pyramids(g);
   return COSL_OK;
 }
 
-// advance() for the cameras with cams[c] != 0 only.  A strict subset cannot flip `cur`: the cameras'
-// slices of the two pyramid buffers are exchanged instead (klt_advance_cams), and their level-0 flags
-// move with the slices.
+// Exchange the cameras' slices of p0 and p1 (and their level-0 records) and copy their provided
+// feature sets to d_src (nFeat = F; 0: no copy), on g->stream; both buffers are fenced after it.
+static int exchange_slices(cosl_klt* g, const KltCamList& L, int nFeat) {
+  if (L.n == 0) return COSL_OK;
+  dim3 grid((unsigned)std::min<long long>(div_up64(g->pyrStride, 256), 2 * g->numSM), L.n);
+  COSL_LAUNCH(klt_advance_cams, grid, 256, 0, g->stream, g->d_pyr[g->p0], g->d_pyr[g->p1], g->pyrStride,
+              g->d_dst, g->d_src, nFeat, L);
+  for (int k = 0; k < L.n; ++k) std::swap(g->lv0Stored[g->p0][L.cam[k]], g->lv0Stored[g->p1][L.cam[k]]);
+  COSL_TRY(fence_pyr(g, g->p0));
+  return fence_pyr(g, g->p1);
+}
+
+// advance() for the cameras with cams[c] != 0 only.  A strict subset cannot move the buffer
+// indices: the cameras' slices of p0 and p1 are exchanged instead (klt_advance_cams), as advance()
+// exchanges the roles of the two buffers.  nxt stays: the third buffer holds nothing any camera keeps.
 int advance_cams(cosl_klt* g, const uint8_t* cams) {
   KltCamList L;
   L.n = 0;
   for (int c = 0; c < g->C; ++c)
     if (cams[c]) L.cam[L.n++] = c;
   if (L.n == g->C) return advance(g);
-  if (L.n == 0) return COSL_OK;
-  dim3 grid((unsigned)std::min<long long>(div_up64(g->pyrStride, 256), 2 * g->numSM), L.n);
-  COSL_LAUNCH(klt_advance_cams, grid, 256, 0, g->stream, g->d_pyr[0], g->d_pyr[1], g->pyrStride, g->d_dst,
-              g->d_src, g->F, L);
-  // the next frame's front pass overwrites one of the two exchanged buffers
-  COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
-  for (int k = 0; k < L.n; ++k) std::swap(g->lv0Stored[0][L.cam[k]], g->lv0Stored[1][L.cam[k]]);
-  return COSL_OK;
+  return exchange_slices(g, L, g->F);
 }
 
 // The present lists of a detect: camera c's nPresent[c] points (x, y, ignored) -> d_present[c][.],
@@ -838,17 +897,20 @@ enum FrameKind {
 // follows the frame, and klt_select_refill writes the provided set to both feature buffers, so the
 // advance is the pyramid flip alone.  Nothing of the plan outlives the call.
 //
-// Frame n+1's image copies wait only for frame n's front pass; its front pass and pyramid tail wait
-// for evFence, which frame n records right after its tracker, so they run next to frame n's
-// klt_nm_verify and klt_select_refill.  What the front stream writes and who else touches it:
-//   d_img                    read by the front passes only (same stream; copy stream: evFront)
-//   d_pyr[cur]               frame n+1 builds into frame n's P0, whose last reader is frame n's
-//                            tracker: the fence
-//   d_corn, d_prelim,        frame n's tracker marks, klt_suppress, verify and select use set `par`;
-//   d_counters[.][8c + 4]    frame n+1 (a frame with a cornerness map) switches to the other set,
-//                            whose last users are frame n-1's, ahead of the fence
-// and it reads d_cams, which update_cameras rewrites on g->stream (it records the fence after);
-// klt_advance_cams also exchanges pyramid slices on g->stream and records the fence after.
+// Frame n+1's image copies wait only for frame n's front pass.  Its front pass and pyramid tail wait
+// only for the fences of the buffers they write, each recorded on g->stream behind that buffer's
+// last reader or writer there.  Between frames that advance, that is frame n-1's tracker, so the
+// steady state of back-to-back frames is
+//   tracker(n-1) | front(n+1) next to detector(n-1) | tracker(n) next to tail(n+1) | front(n+2) ...
+// What the front stream writes, its ring and its fence:
+//   d_img                    one; read by the front passes only (same stream; copy stream: evFront)
+//   d_pyr[nxt]               three (p0, p1, nxt); evPyr[b], recorded after each tracker for the two
+//                            buffers it reads and after each exchange of slices (klt_advance_cams)
+//   d_corn, d_prelim,        three sets; the tracker's marks, klt_suppress, verify, select and the
+//   d_counters[.][8c + 4]    read-backs use set `par`.  A frame with a cornerness map moves on to the
+//                            next set and records the fence evPar of the set it leaves (next_par)
+//   d_stepCams[tab]          three (run_step); evStepFence[t], recorded at the end of the step
+// and it reads d_cams, which update_cameras rewrites on g->stream (evCams).
 int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind,
               int maxPresent, bool foldAdvance) {
   FramePlan p;
@@ -865,23 +927,24 @@ int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pi
   p.trackerTail = fused_tracker(g);
   p.foldAdvance = foldAdvance;
   g->stepOpsValid = false;
-  if (p.wantCorn) g->par ^= 1;
+  if (p.wantCorn) COSL_TRY(next_par(g));
   int* counters = g->d_counters[g->par];
   // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below
   COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
-  // the images ahead of the fence: d_img is read by the front passes alone, so they run under the
+  // the images ahead of the fences: d_img is read by the front passes alone, so they run under the
   // previous frame's tracker
   COSL_TRY(upload_images(g, imgs, pitch, copyKind, nullptr));
-  COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evFence, 0));
+  COSL_TRY(front_waits(g, p.wantCorn, -1));
   if (p.wantCorn)
     COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
-  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->cur][c] = p.storeL0;
+  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->nxt][c] = p.storeL0;
   COSL_TRY(build_pyramid(g, p));
   COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
   COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
   if (kind != FRAME_DETECT) {
     COSL_TRY(run_tracker(g, p));
-    COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
+    COSL_TRY(fence_pyr(g, g->p0));
+    COSL_TRY(fence_pyr(g, g->p1));
     if (!p.trackerTail) {
       dim3 grid(div_up(g->F, 256), g->C);
       COSL_LAUNCH(klt_status<false>, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, g->d_cams);
@@ -894,8 +957,7 @@ int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pi
   } else {
     COSL_TRY(run_detector(g, kind == FRAME_REDETECT ? 1 : 0, maxPresent, p));
   }
-  if (kind == FRAME_DETECT) COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
-  if (foldAdvance) g->cur = 1 - g->cur;
+  if (foldAdvance) advance_pyramids(g);
   return COSL_OK;
 }
 
@@ -905,16 +967,6 @@ static int op_stages(int op) {
          : op == COSL_KLT_OP_TRACK ? KLT_STAGE_PYR | KLT_STAGE_TRACK
          : op == COSL_KLT_OP_NEXT  ? KLT_STAGE_ALL
                                    : 0;
-}
-
-// exchange the cameras' slices of the two pyramid buffers (and their level-0 records) on g->stream
-static int exchange_slices(cosl_klt* g, const KltCamList& L) {
-  if (L.n == 0) return COSL_OK;
-  dim3 grid((unsigned)std::min<long long>(div_up64(g->pyrStride, 256), 2 * g->numSM), L.n);
-  COSL_LAUNCH(klt_advance_cams, grid, 256, 0, g->stream, g->d_pyr[0], g->d_pyr[1], g->pyrStride, g->d_dst,
-              g->d_src, 0, L);
-  for (int k = 0; k < L.n; ++k) std::swap(g->lv0Stored[0][L.cam[k]], g->lv0Stored[1][L.cam[k]]);
-  return COSL_OK;
 }
 
 // One step of cosl_klt_group_step: camera c gets ops[c] followed by advanceFrame, or nothing.
@@ -928,14 +980,16 @@ static int exchange_slices(cosl_klt* g, const KltCamList& L) {
 //   provide (klt_provide_cams)       TRACK
 // The frame's schedule is run_frame's, with the plan of the union of the ops: the front pass stores
 // level 0 when one of its cameras needs it, the prefilter runs early, and a step with a detecting
-// camera switches the counter set (a switch is always safe: the set it leaves is the one the
-// fence protects).  The front pass of the next frame waits for the fence as ever.
+// camera moves on to the next counter set.
 //
 // Advance of a strict subset: the pyramid slices of either the skipped or the addressed cameras
-// are exchanged, whichever are fewer.  Skipped ones: `cur` flips for the group and their slices
-// are exchanged ahead of the tracker (nothing of the step touches them); addressed ones: `cur`
-// stays and their slices are exchanged after the tracker, ahead of the fence.  The feature-buffer
-// half of the advance is folded into klt_select_refill and klt_provide_cams.
+// are exchanged, whichever are fewer.  Skipped ones: p0 and p1 change roles for the group and their
+// slices are exchanged ahead of the tracker (nothing of the step touches them); addressed ones: the
+// roles stay and their slices are exchanged after the tracker.  Such a step builds into p1, as the
+// two-buffer tracker does, not into the third buffer: then the skipped cameras would need their
+// slices of all three buffers rotated, where one exchange of two buffers moves the same bytes.  So
+// it waits for the tracker before it, and the next step for its own.  The feature-buffer half of the
+// advance is folded into klt_select_refill and klt_provide_cams.
 int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
   const int C = g->C;
   int nOp[4] = {0, 0, 0, 0};
@@ -952,9 +1006,9 @@ int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t
     addr.n = skip.n = provide.n = 0;
     bool anyTrack = false, anyDetect = false, storeL0 = false;
     bool lv0[64];  // what a single tracker records for the frame of the camera's op
-    // the pinned table's previous copy was enqueued two steps ago: the host waits here only when
-    // it runs more than a step ahead of the front stream (cosl_klt_group_step_dev)
-    const int tab = g->stepTab ^= 1;
+    // the pinned table's previous copy was enqueued three steps ago: the host waits here only when
+    // it runs more than two steps ahead of the front stream (cosl_klt_group_step_dev)
+    const int tab = g->stepTab = (g->stepTab + 1) % 3;
     COSL_CUDA(cudaEventSynchronize(g->evStepTab[tab]));
     KltCam* hstep = g->h_stepCams[tab];
     for (int c = 0; c < C; ++c) {
@@ -983,25 +1037,31 @@ int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t
     p.earlyPrefilter = anyDetect;
     p.trackerTail = fused_tracker(g);
     p.foldAdvance = true;
-    if (p.wantCorn) g->par ^= 1;
+    if (p.wantCorn) COSL_TRY(next_par(g));
     int* counters = g->d_counters[g->par];
     COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), C, g->stream));
-    if (flip) COSL_TRY(exchange_slices(g, skip));
     COSL_TRY(upload_images(g, imgs, pitch, copyKind, ops));
-    COSL_CUDA(cudaStreamWaitEvent(g->frontStream, g->evFence, 0));
-    // the device table's last readers belong to the step before the previous one, ahead of the fence
+    g->nxt = g->p1;
+    COSL_TRY(front_waits(g, p.wantCorn, tab));
+    // enqueued after the front stream's waits, which it must not join: the front pass writes the
+    // addressed cameras' slices only
+    if (flip) COSL_TRY(exchange_slices(g, skip, 0));
     COSL_CUDA(cudaMemcpyAsync(g->d_stepCams[tab], hstep, sizeof(KltCam) * C, cudaMemcpyHostToDevice, g->frontStream));
     COSL_CUDA(cudaEventRecord(g->evStepTab[tab], g->frontStream));
     if (p.wantCorn)
       COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), C, g->frontStream));
-    for (int k = 0; k < addr.n; ++k) g->lv0Stored[g->cur][addr.cam[k]] = lv0[addr.cam[k]];
+    for (int k = 0; k < addr.n; ++k) g->lv0Stored[g->nxt][addr.cam[k]] = lv0[addr.cam[k]];
     COSL_TRY(build_pyramid(g, p));
     COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
     COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
     if (anyTrack) {
       COSL_TRY(run_tracker(g, p));
-      if (!flip) COSL_TRY(exchange_slices(g, addr));
-      COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
+      if (!flip) {
+        COSL_TRY(exchange_slices(g, addr, 0));
+      } else {
+        COSL_TRY(fence_pyr(g, g->p0));
+        COSL_TRY(fence_pyr(g, g->p1));
+      }
       if (!p.trackerTail) {
         dim3 grid(div_up(g->F, 256), C);
         COSL_LAUNCH(klt_status<true>, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, p.cams);
@@ -1011,11 +1071,10 @@ int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t
       COSL_LAUNCH(klt_provide_cams, dim3(div_up(g->F, 256), provide.n), 256, 0, g->stream, g->d_res, g->d_dst,
                   g->d_src, g->F, provide);
     if (anyDetect) COSL_TRY(run_detector(g, 2, 0, p));
-    if (!anyTrack) {
-      if (!flip) COSL_TRY(exchange_slices(g, addr));
-      COSL_CUDA(cudaEventRecord(g->evFence, g->stream));
-    }
-    if (flip) g->cur = 1 - g->cur;
+    if (!anyTrack && !flip) COSL_TRY(exchange_slices(g, addr, 0));
+    COSL_CUDA(cudaEventRecord(g->evStepFence[tab], g->stream));
+    if (flip) std::swap(g->p0, g->p1);
+    g->nxt = g->p1;
   }
   std::memcpy(g->stepOps, ops, C);
   g->stepOpsValid = true;
@@ -1384,10 +1443,10 @@ int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch)
   return submit_readback(h, slot);
 }
 
-// A step's op table comes from one of two pinned host tables (run_step); the host waits for the copy
-// out of the table it reuses, made two mixed steps earlier.  At most two frames are in flight, so when
-// that step was submitted it has been collected (the copy is done); only a step_dev can leave it
-// pending, and its copy is already enqueued.
+// A step's op table comes from one of three pinned host tables (run_step); the host waits for the
+// copy out of the table it reuses, made three mixed steps earlier.  At most two frames are in flight,
+// so when that step was submitted it has been collected (the copy is done); only a step_dev can leave
+// it pending, and its copy is already enqueued.
 int cosl_klt_group_submit_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch) {
   KLT_ENTER(h)
   COSL_TRY(check_step(h, ops, imgs, pitch, "group_submit_step"));
@@ -1425,7 +1484,7 @@ int cosl_klt_debug_pyramid(cosl_klt* h, int cam, int which, int level, float* ou
   if (w) *w = lw;
   if (ht) *ht = lh;
   if (!out3) return COSL_OK;
-  const int buf = which ? h->cur : 1 - h->cur;
+  const int buf = which ? h->p1 : h->p0;
   if (level == 0 && !h->lv0Stored[buf][cam])
     return set_error(COSL_E_INVALID,
                      "debug_pyramid: level 0 of this pyramid was not stored (a tracked frame keeps only "

@@ -101,7 +101,11 @@ int cosl_klt_create(const cosl_klt_config* cfg, int width, int height, int nLeve
                     int featH, int plW, int plH, int device, cosl_klt** out);
 /* Extension: C cameras of identical geometry that are always advanced together; every kernel is
  * launched once for the whole group (camera = grid.z).  Single-camera calls below address
- * camera 0 of a group. */
+ * camera 0 of a group.
+ * Device memory: a tracker keeps three pyramids per camera, not the reference's two, and three
+ * cornerness maps and corner lists, so that the next frame's pyramid is built while the current
+ * frame is tracked.  The third set costs about 24 MB per 1280x720 camera (19.7 MB of it the
+ * pyramid) and about 55 MB per 1920x1080 camera (44 MB). */
 int cosl_klt_group_create(const cosl_klt_config* cfg, int nCams, int width, int height,
                           int nLevels, int featW, int featH, int plW, int plH, int device,
                           cosl_klt** out);
@@ -180,7 +184,8 @@ int cosl_klt_group_feed(cosl_klt* h, const int* npts, const float* const* pts3, 
                         int* nFed);
 /* KLT_SequenceTracker::advanceFrame (v3d_gpuklt.h:252-259) for the cameras with cams[c] != 0 (C
  * entries).  All cameras marked is exactly cosl_klt_advance; a strict subset exchanges those
- * cameras' pyramid slices between the two buffers on the device (a second call swaps them back). */
+ * cameras' slices of the previous and the current pyramid on the device (a second call swaps them
+ * back). */
 int cosl_klt_group_advance_cams(cosl_klt* h, const uint8_t* cams);
 /* GPUKLT::first(f, img, present, ips) (tracking/GPUKLT.cpp:111-135, called per camera by
  * CoSLAM::initMapMultiCam, app/SL_CoSLAM.cpp:258-262) for the whole group: detect with camera c's

@@ -5,7 +5,8 @@
 Writes OUT_DIR/klt_next_dev.json (Chrome trace) and prints, per frame pair, whether frame n+1's
 klt_front overlaps frame n's klt_nm_verify / klt_select_refill, the device time per frame, the host
 time to enqueue one cosl_klt_group_next_dev call (measured without the profiler) and the split of
-the pyramid chain into kernels and the gaps between them (chain_split).  The host must
+the pyramid chain into kernels and the gaps between them (chain_split), and how far each front pass
+runs ahead of the tracker before it (lookahead).  The host must
 enqueue a frame faster than the device runs it, or the queue drains and the overlap is lost."""
 import argparse
 import json
@@ -51,6 +52,28 @@ def chain_split(front, pyr, track):
         return {}
     keys = [k for k in rows[0] if all(k in r for r in rows)]
     return {"frames": len(rows), **{k: round(float(np.median([r[k] for r in rows])), 2) for k in keys}}
+
+
+def lookahead(front, pyr, track, verify, select, n_levels):
+    """Per frame pair (n, n+1), from the k-th launch of each kernel being frame k's: whether front(n+1)
+    starts before tracker(n) does, the detector span (klt_nm_verify start -> klt_select_refill end)
+    of frame n and front(n+1)'s duration, the time from tail(n+1)'s end to tracker(n)'s end (> 0: the
+    tail is done before the next tracker can start) and from tracker(n)'s end to tracker(n+1)'s start.
+    Medians in us, and the count of frame pairs where front(n+1) runs ahead.  With fewer than 3
+    levels there is no tail kernel and the front pass's end stands for the tail's."""
+    per = n_levels - 2
+    tails = [pyr[i + per - 1] for i in range(0, len(pyr) - per + 1, per)] if per > 0 else front
+    n = min(len(front), len(track), len(verify), len(select), len(tails))
+    rows, ahead = [], 0
+    for k in range(n - 1):
+        ahead += front[k + 1][0] < track[k][0]
+        rows.append({"detector_span": select[k][1] - verify[k][0], "front_dur": front[k + 1][1] - front[k + 1][0],
+                     "tail_end_to_tracker_end": track[k][1] - tails[k + 1][1],
+                     "tracker_end_to_next_tracker_start": track[k + 1][0] - track[k][1]})
+    if not rows:
+        return {}
+    return {"front_ahead_of_tracker": f"{ahead} of {len(rows)} frame pairs",
+            **{k: round(float(np.median([r[k] for r in rows])), 2) for k in rows[0]}}
 
 
 def main():
@@ -121,6 +144,8 @@ def main():
         "device_ms_per_frame": dev_ms,
         "host_enqueue_ms_per_call": {"median": 1e3 * float(np.median(host)), "p90": 1e3 * float(np.percentile(host, 90))},
         "pyramid_chain_us": chain_split(front, kernels(trace, "klt_pyr_down_tma"), kernels(trace, tracker)),
+        "lookahead_us": lookahead(front, kernels(trace, "klt_pyr_down_tma"), kernels(trace, tracker), verify, select,
+                                  bench.KLT_L),
         "trace": path}))
     grp.close()
 
