@@ -94,6 +94,7 @@ def _load():
     L.cosl_ba_solver_plan_info.argtypes = [vp, pint]
     L.cosl_ba_solver_trace.argtypes = [vp, ci, vp, vp, ci]
     L.cosl_ba_solver_tasks.argtypes = [vp, vp, ci, vp, ci]
+    L.cosl_ba_debug_tile_solve.argtypes = [ci, vp, ci, vp, vp, vp, pint, pint]
     L.cosl_posegraph_spread_chains.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, vp, ci]
     L.cosl_posegraph_solve.argtypes = [ci, vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci]
     L.cosl_posegraph_last_host_ms.restype = cd
@@ -489,6 +490,27 @@ def ba_solve_multi(prob, opt, n_gpus, devices=None):
     return info
 
 
+PLAN_INFO_KEYS = ("blocks", "tiles_schur", "tiles", "tasks", "nd_depth", "critical_tasks", "grid",
+                  "small_solve")
+
+
+def ba_debug_tile_solve(S, b, adj, nd_depth=-1):
+    """cosl_ba_debug_tile_solve: x = S^-1 b with the BA's reduced-system solve (S dense 6mf x 6mf, lower
+    triangle read; adj the mf x mf block pattern).  Returns (x, fail flag, plan info dict)."""
+    adj = np.ascontiguousarray(adj, np.uint8)
+    mf = adj.shape[0]
+    assert adj.shape == (mf, mf)
+    S = np.ascontiguousarray(S, np.float64)
+    b = np.ascontiguousarray(b, np.float64)
+    assert S.shape == (6 * mf, 6 * mf) and b.shape == (6 * mf,)
+    x = np.empty(6 * mf)
+    fail = C.c_int(0)
+    out = (C.c_int * 8)()
+    _ck(LIB.cosl_ba_debug_tile_solve(mf, _ptr(adj), int(nd_depth), _ptr(S), _ptr(b), _ptr(x), C.byref(fail),
+                                     out))
+    return x, fail.value, dict(zip(PLAN_INFO_KEYS, [int(v) for v in out]))
+
+
 def posegraph_spread_chains(chain_off, fixed, R, t, eR, et, device=0):
     """cosl_posegraph_spread_chains: post-BA spreading of the non-key-frame poses of all cameras
     (GlobalPoseGraph::computeNewCameraRotations + ::computeNewCameraTranslations on the chain
@@ -612,9 +634,7 @@ class BaSolver:
     def plan_info(self):
         out = (C.c_int * 8)()
         _ck(LIB.cosl_ba_solver_plan_info(self.h, out))
-        keys = ("blocks", "tiles_schur", "tiles", "tasks", "nd_depth", "critical_tasks", "grid",
-                "small_solve")
-        return dict(zip(keys, [int(v) for v in out]))
+        return dict(zip(PLAN_INFO_KEYS, [int(v) for v in out]))
 
     def tasks(self):
         """Task list of the solve plan: (tasks [n,16] int32, wait lists [m,2] int32)."""

@@ -60,7 +60,8 @@ int tile_task_order(const BaPlan& P, std::vector<BaTask>& order) {
   return nA;
 }
 
-int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int device, cudaStream_t s) {
+int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int device, cudaStream_t s, int* gridOut) {
+  if (gridOut) *gridOut = 0;
   if (P.nb <= 0) return COSL_OK;
   BaTileDev td = {};
   td.rhs = b.rhs;
@@ -89,6 +90,7 @@ int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int devic
   if (P.nb <= 2 && t00 >= 0 && (P.nb == 1 || t11 >= 0)) {
     COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
     COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s, td, t00, t10, t11);
+    if (gridOut) *gridOut = 1;
   } else {
     // same grid rule as the BA solver: never more CTAs than can be co-resident (the tickets spin)
     COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
@@ -99,6 +101,7 @@ int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int devic
     const int grid = std::max(2, std::min(std::max(1, nsm), td.nTasks + 1));
     td.nSpecial = std::max(1, std::min(std::min(24, std::max(1, grid / 6)), grid - 1));
     COSL_LAUNCH(ba_tile_solve, grid, BA_NTHREADS, BA_TILE_SMEM, s, td);
+    if (gridOut) *gridOut = grid;
   }
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
@@ -361,6 +364,26 @@ static double now_s() {
   return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
+// ptr monotone from 0, camera indices in range, and no (point, camera) pair twice.  The Schur
+// contraction relies on the last: its pair lists hold one entry per ordered pair of a point's
+// observations with the second camera >= the first, which covers each pair of cameras once only
+// when a point has at most one observation per camera (sba's vmask cannot express more either).
+int check_observations(const cosl_ba_problem* p) {
+  if (p->n && p->ptr[0] != 0) return set_error(COSL_E_INVALID, "ptr[0] != 0");
+  std::vector<int> seen((size_t)p->m, -1);  // last point that camera j observed
+  for (int i = 0; i < p->n; ++i) {
+    if (p->ptr[i + 1] < p->ptr[i]) return set_error(COSL_E_INVALID, "ptr not monotone at %d", i);
+    for (long long o = p->ptr[i]; o < p->ptr[i + 1]; ++o) {
+      const int j = p->cam[o];
+      if (j < 0 || j >= p->m) return set_error(COSL_E_INVALID, "camera index out of range");
+      if (seen[j] == i)
+        return set_error(COSL_E_INVALID, "point %d is observed twice by camera %d (one observation per pair)", i, j);
+      seen[j] = i;
+    }
+  }
+  return COSL_OK;
+}
+
 int upload_params(cosl_ba_solver* s, const cosl_ba_problem* p) {
   const int m = s->m;
   std::vector<double> R0((size_t)m * 9), pa((size_t)m * 6, 0.0);
@@ -428,16 +451,11 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   s->mf = m - mcon;
   s->ns = 6 * s->mf;
   s->N = N;
-  // host-side index structures
+  // host-side index structures (the observation lists were validated by check_observations)
   std::vector<int> pt((size_t)N), cam((size_t)N);
-  for (int i = 0; i < n; ++i) {
-    if (p->ptr[i + 1] < p->ptr[i]) return set_error(COSL_E_INVALID, "ptr not monotone at %d", i);
+  for (int i = 0; i < n; ++i)
     for (long long o = p->ptr[i]; o < p->ptr[i + 1]; ++o) pt[o] = i;
-  }
-  for (long long o = 0; o < N; ++o) {
-    cam[o] = p->cam[o];
-    if (cam[o] < 0 || cam[o] >= m) return set_error(COSL_E_INVALID, "camera index out of range");
-  }
+  for (long long o = 0; o < N; ++o) cam[o] = p->cam[o];
   // camera-major list of the free-camera observations
   std::vector<long long> cptr(m + 1, 0);
   for (long long o = 0; o < N; ++o)
@@ -1202,6 +1220,7 @@ int cosl_ba_solver_create(const cosl_ba_problem* prob, const cosl_ba_options* op
     return set_error(COSL_E_INVALID, "cosl_ba_solver_create: bad problem");
   if (prob->n && prob->ptr[prob->n] != prob->nobs)
     return set_error(COSL_E_INVALID, "ptr[n] != nobs");
+  COSL_TRY(check_observations(prob));
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || opt->device < 0 || opt->device >= ndev)
     return set_error(COSL_E_CUDA, "CUDA device %d not available", opt->device);
@@ -1343,6 +1362,93 @@ int cosl_ba_solver_tasks(cosl_ba_solver* s, int32_t* tasks, int cap, int32_t* li
     if (tasks) std::memcpy(tasks + 16 * (size_t)t, &k, sizeof(BaTask));
   }
   return nt;
+}
+
+// diagnostic: one solve of a dense SPD system with the reduced-camera-system solve of the BA, from the
+// plan to the unpermuted solution, so that the tile kernels can be checked against a dense reference
+int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const double* S, const double* b,
+                             double* x, int* fail, int out[8]) {
+  if (mf < 1 || !adj || !S || !b || !x || !fail || !out)
+    return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_solve: bad argument");
+  const BaPlan P = ba_make_plan(mf, std::vector<uint8_t>(adj, adj + (size_t)mf * mf), nd_depth);
+  if (P.nb <= 0) return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_solve: planning failed");
+  std::vector<BaTask> tasks;
+  const int nA = tile_task_order(P, tasks);
+  const int nb = P.nb;
+  const size_t ns = 6 * (size_t)mf, nScratch = (size_t)std::max(1, P.nScratch);
+  const size_t nCnt = (size_t)P.nCounters + 2 + tasks.size();
+  // the lower triangle of the permuted system, placed as build_solver's pair_dst places the Schur
+  // blocks: the camera later in the elimination order owns the rows; fill and padding stay zero
+  std::vector<double> hTiles((size_t)P.nTiles * BA_TILE, 0.0), hRhs((size_t)nb * BA_TB, 0.0);
+  for (int a = 0; a < mf; ++a)
+    for (int c = 0; c < mf; ++c) {
+      if (a != c && !adj[(size_t)a * mf + c] && !adj[(size_t)c * mf + a]) continue;
+      const int bA = P.camBlk[a], bC = P.camBlk[c];
+      if (bA < bC || (bA == bC && P.camOff[a] < P.camOff[c])) continue;
+      double* T = &hTiles[(size_t)P.tileIdx[(size_t)bA * nb + bC] * BA_TILE];
+      for (int r = 0; r < 6; ++r)
+        for (int q = 0; q < 6; ++q) {
+          if (a == c && q > r) continue;
+          const size_t i = 6 * (size_t)a + r, j = 6 * (size_t)c + q;
+          T[(size_t)(P.camOff[c] + q) * BA_TB + P.camOff[a] + r] = i >= j ? S[i * ns + j] : S[j * ns + i];
+        }
+    }
+  for (int a = 0; a < mf; ++a)
+    for (int r = 0; r < 6; ++r) hRhs[(size_t)P.camBlk[a] * BA_TB + P.camOff[a] + r] = b[6 * a + r];
+  int device = 0;
+  COSL_CUDA(cudaGetDevice(&device));
+  cudaStream_t s = cudaStreamPerThread;
+  TmpDeviceBufs tmp(s);
+  double *dRhs, *dTiles, *dRhsS, *dLinv, *dY, *dX, *dFail;
+  int *dCnt, *dBlkRows;
+  BaTask* dTasks;
+  BaBwdEntry* dBwd;
+  BaSumEntry* dSum;
+  COSL_TRY(tmp.alloc(&dRhs, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dTiles, ((size_t)P.nTiles + P.nScratch) * BA_TILE));
+  COSL_TRY(tmp.alloc(&dRhsS, nScratch * BA_TB));
+  COSL_TRY(tmp.alloc(&dLinv, (size_t)nb * BA_TILE));
+  COSL_TRY(tmp.alloc(&dY, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dX, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dFail, 1));
+  COSL_TRY(tmp.alloc(&dCnt, nCnt));
+  COSL_TRY(tmp.alloc(&dBlkRows, (size_t)nb));
+  COSL_TRY(tmp.alloc(&dTasks, tasks.size()));
+  COSL_TRY(tmp.alloc(&dBwd, P.bwdList.size()));
+  COSL_TRY(tmp.alloc(&dSum, P.sumList.size()));
+  COSL_CUDA(cudaMemcpyAsync(dRhs, hRhs.data(), 8 * hRhs.size(), cudaMemcpyHostToDevice, s));
+  COSL_CUDA(cudaMemcpyAsync(dTiles, hTiles.data(), 8 * hTiles.size(), cudaMemcpyHostToDevice, s));
+  // scratch tiles and their rhs parts start as NaN: their first update must overwrite them
+  COSL_CUDA(cudaMemsetAsync(dTiles + (size_t)P.nTiles * BA_TILE, 0xff, 8 * (size_t)P.nScratch * BA_TILE, s));
+  COSL_CUDA(cudaMemsetAsync(dRhsS, 0xff, 8 * nScratch * BA_TB, s));
+  COSL_CUDA(cudaMemsetAsync(dCnt, 0, 4 * nCnt, s));
+  COSL_CUDA(cudaMemsetAsync(dFail, 0, 8, s));
+  COSL_CUDA(cudaMemcpyAsync(dBlkRows, P.blkRows.data(), 4 * (size_t)nb, cudaMemcpyHostToDevice, s));
+  COSL_CUDA(cudaMemcpyAsync(dTasks, tasks.data(), sizeof(BaTask) * tasks.size(), cudaMemcpyHostToDevice, s));
+  if (!P.bwdList.empty())
+    COSL_CUDA(cudaMemcpyAsync(dBwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size(), cudaMemcpyHostToDevice, s));
+  if (!P.sumList.empty())
+    COSL_CUDA(cudaMemcpyAsync(dSum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size(), cudaMemcpyHostToDevice, s));
+  const TileSolveBufs tb = {dRhs, dTiles, dRhsS, dLinv, dY, dX, dCnt, dTasks, dBwd, dSum, dBlkRows, dFail};
+  int grid = 0;
+  COSL_TRY(tile_solve_launch(P, nA, tb, device, s, &grid));
+  std::vector<double> hX((size_t)nb * BA_TB);
+  double hFail = 0.0;
+  COSL_CUDA(cudaMemcpyAsync(hX.data(), dX, 8 * hX.size(), cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(&hFail, dFail, 8, cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaStreamSynchronize(s));
+  for (int a = 0; a < mf; ++a)
+    for (int r = 0; r < 6; ++r) x[6 * a + r] = hX[(size_t)P.camBlk[a] * BA_TB + P.camOff[a] + r];
+  *fail = hFail != 0.0 ? 1 : 0;
+  out[0] = P.nb;
+  out[1] = P.nTilesOrig;
+  out[2] = P.nTiles;
+  out[3] = (int)P.tasks.size();
+  out[4] = P.ndDepth;
+  out[5] = P.criticalPathTasks;
+  out[6] = grid;
+  out[7] = grid == 1 ? 1 : 0;
+  return COSL_OK;
 }
 
 int cosl_ba_solver_profile_enable(cosl_ba_solver* s, int on) {

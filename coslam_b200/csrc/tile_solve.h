@@ -36,7 +36,8 @@ struct TileSolveBufs {
 
 // Enqueues the solve of the assembled system on `s`: x = S^-1 rhs, block padded in the plan's
 // order.  The counters and tickets (cnt) must be zero.  One CTA for one or two blocks (ba_tile_two),
-// the persistent dataflow kernel (ba_tile_solve) otherwise.
-int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int device, cudaStream_t s);
+// the persistent dataflow kernel (ba_tile_solve) otherwise.  gridOut (optional): CTAs launched.
+int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int device, cudaStream_t s,
+                      int* gridOut = nullptr);
 
 }  // namespace coslam

@@ -310,7 +310,9 @@ int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const do
  *   bundleAdjustRobust(nCamsCon, Ks, Rs, Ts, nPtsCon, pts, meas, maxErr, maxIter, nInnerMaxIter)
  * (LibVisualSLAM geometry/SL_BundleAdjust.h; call app/SL_CoSLAMRobustBA.cpp:174-175).
  * Observations are CSR by point: point i owns obs [ptr[i], ptr[i+1]), sorted by camera index,
- * exactly the order of vector<vector<Meas2D>> built at app/SL_CoSLAMRobustBA.cpp:109-165. */
+ * exactly the order of vector<vector<Meas2D>> built at app/SL_CoSLAMRobustBA.cpp:109-165.
+ * ptr[0] = 0, and a camera observes a point at most once (as sba's vmask); a problem with a
+ * repeated (point, camera) pair is refused with COSL_E_INVALID. */
 typedef struct cosl_ba_problem {
   int m;              /* cameras (poses)                                   */
   int n;              /* points                                            */
@@ -420,6 +422,14 @@ int cosl_ba_solver_trace(cosl_ba_solver* s, int enable, uint64_t* out, int32_t* 
  * coslam_b200/csrc/ba_plan.h) and the wait lists of the BACKWARD / SUM tasks as (counter, value)
  * pairs; returns the number of tasks. */
 int cosl_ba_solver_tasks(cosl_ba_solver* s, int32_t* tasks, int cap, int32_t* lists, int listCap);
+/* Diagnostic: solve S x = b with the BA's tile Cholesky on the current device.  S is dense (6mf x 6mf,
+ * row-major, only the lower triangle read); the co-visibility of the 6x6 blocks is taken from adj
+ * (mf x mf), and entries of S outside those blocks are ignored.  nd_depth < 0: automatic.  *fail = the
+ * solver's failure flag (a pivot outside (1e-30, 1e30) or NaN: x is then meaningless, the call still
+ * returns COSL_OK).  out as cosl_ba_solver_plan_info, with out[6] = CTAs launched.  Returns COSL_OK or
+ * COSL_E_*. */
+int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const double* S,
+                             const double* b, double* x, int* fail, int out[8]);
 
 /* ================= post-BA pose-graph spreading (SURVEY.md 8f-2) =================
  * Replaces, for chain graphs, GlobalPoseGraph::computeNewCameraRotations

@@ -629,9 +629,21 @@ struct BA {
   }
 };
 
+// a camera observes a point at most once (sba's vmask cannot say more); the library refuses the rest
+bool observations_valid(const cosl_ba_problem* p) {
+  std::vector<int> seen((size_t)p->m, -1);
+  for (int i = 0; i < p->n; ++i)
+    for (int64_t o = p->ptr[i]; o < p->ptr[i + 1]; ++o) {
+      const int j = p->cam[o];
+      if (j < 0 || j >= p->m || seen[j] == i) return false;
+      seen[j] = i;
+    }
+  return true;
+}
+
 int run_robust(cosl_ba_problem* prob, const cosl_ba_options* opt, int fixed_trials,
                double info[COSL_BA_INFOSZ]) {
-  if (!prob || !opt || prob->m < 1 || prob->n < 0) return COSL_E_INVALID;
+  if (!prob || !opt || prob->m < 1 || prob->n < 0 || !observations_valid(prob)) return COSL_E_INVALID;
   BA ba;
   ba.init(prob);
   double sinfo[10] = {0};

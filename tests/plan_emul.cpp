@@ -229,10 +229,18 @@ int main(int argc, char** argv) {
       err = std::fmax(err, std::fabs(xv - xr[6 * a + r]));
       nrm = std::fmax(nrm, std::fabs(xr[6 * a + r]));
     }
+  // SUM tasks of diagonal tiles (they also add the rhs parts of their scratch tiles) and BWD tasks
+  // whose wait list is not a whole number of the kernel's chunks of 4
+  int diagSums = 0, bwdNot4 = 0;
+  for (const BaTask& t : P.tasks) {
+    diagSums += (t.type == BA_T_SUM && (t.flags & 1)) ? 1 : 0;
+    bwdNot4 += (t.type == BA_T_BWD && (t.l1 - t.l0) % 4 != 0) ? 1 : 0;
+  }
   std::printf("{\"mf\": %d, \"nb\": %d, \"nd_depth\": %d, \"tiles_orig\": %d, \"tiles\": %d, \"scratch\": %d, "
-              "\"tasks\": %d, \"critical_tasks\": %d, \"critical_cost\": %.1f, \"gflop\": %.4f, \"rel_err\": %.3e}\n",
+              "\"tasks\": %d, \"critical_tasks\": %d, \"critical_cost\": %.1f, \"gflop\": %.4f, \"rel_err\": %.3e, "
+              "\"diag_sums\": %d, \"bwd_not4\": %d}\n",
               mf, nb, P.ndDepth, P.nTilesOrig, P.nTiles, P.nScratch, (int)P.tasks.size(), P.criticalPathTasks,
-              P.criticalPathCost, P.flops * 1e-9, err / nrm);
+              P.criticalPathCost, P.flops * 1e-9, err / nrm, diagSums, bwdNot4);
   if (!(err / nrm < 1e-9)) {
     std::printf("FAIL: solution differs\n");
     return 1;

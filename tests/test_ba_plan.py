@@ -49,3 +49,12 @@ def test_nested_dissection_shortens_the_critical_path(emul):
     assert flat["nd_depth"] == 0 and auto["nd_depth"] >= 2
     assert auto["critical_cost"] < 0.5 * flat["critical_cost"]
     assert auto["gflop"] < 4 * flat["gflop"]  # bounded fill
+    assert auto["diag_sums"] > 0 and auto["bwd_not4"] > 0
+
+
+def test_band_plans_reach_the_scratch_and_chunk_edges(emul):
+    """The band patterns of tests/test_gpu_ba_tile_solve.py reach the SUM of diagonal scratch tiles
+    (their rhs parts) and BWD wait lists that end in a partial chunk of 4."""
+    st = _run(emul, 121, "band", 29, 1)
+    assert st["nd_depth"] == 1 and st["scratch"] > 0
+    assert st["diag_sums"] > 0 and st["bwd_not4"] > 0
