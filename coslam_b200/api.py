@@ -83,6 +83,9 @@ def _load():
     L.cosl_ba_solver_reset.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_run.argtypes = [vp, vp]
     L.cosl_ba_solver_run_fixed.argtypes = [vp, ci, vp]
+    L.cosl_ba_solver_submit.argtypes = [vp]
+    L.cosl_ba_solver_query.argtypes = [vp, pint]
+    L.cosl_ba_solver_collect.argtypes = [vp, vp]
     L.cosl_ba_solver_download.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_destroy.argtypes = [vp]
     L.cosl_ba_solver_stream.argtypes = [vp]
@@ -610,6 +613,22 @@ class BaSolver:
     def run_fixed(self, trials):
         info = np.zeros(COSL_BA_INFOSZ)
         _ck(LIB.cosl_ba_solver_run_fixed(self.h, int(trials), _ptr(info)))
+        return info
+
+    def submit(self):
+        """cosl_ba_solver_submit: enqueue run()'s robust loop on the solver's stream and return at once."""
+        _ck(LIB.cosl_ba_solver_submit(self.h))
+
+    def done(self):
+        """cosl_ba_solver_query: True once the submitted loop has finished (never waits)."""
+        d = C.c_int(0)
+        _ck(LIB.cosl_ba_solver_query(self.h, C.byref(d)))
+        return bool(d.value)
+
+    def collect(self):
+        """cosl_ba_solver_collect: wait for the submitted loop; the info vector of run()."""
+        info = np.zeros(COSL_BA_INFOSZ)
+        _ck(LIB.cosl_ba_solver_collect(self.h, _ptr(info)))
         return info
 
     def download(self, into=None):

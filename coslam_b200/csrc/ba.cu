@@ -19,6 +19,7 @@
 #include <thread>
 #include <vector>
 
+#include "ba_ctl.cuh"
 #include "ba_kernels.cuh"
 #include "ba_tile.cuh"
 #include "common.cuh"
@@ -210,6 +211,13 @@ struct cosl_ba_solver {
   int secLin = 0, secSchur = 0, secSolve = 0, secBack = 0, secCost = 0, secComm = 0;
   // statistics
   int nfev = 0, njev = 0, nlss = 0;
+  // submitted robust loop (cosl_ba_solver_submit): the graph with the device-side LM control, the
+  // parameter buffers it was built for, and the events that time and mark one submission
+  BaCtl* d_ctl = nullptr;
+  cudaGraphExec_t graphExec = nullptr;
+  const double *graphPa = nullptr, *graphNa = nullptr, *graphPb = nullptr, *graphNb = nullptr;
+  cudaEvent_t evSubmit = nullptr, evDone = nullptr;
+  bool inFlight = false;
 };
 
 namespace {
@@ -408,12 +416,15 @@ void free_solver(cosl_ba_solver* s) {
   cudaSetDevice(s->device);
   if (s->stream) cudaStreamSynchronize(s->stream);
   s->timer.destroy();
+  if (s->graphExec) cudaGraphExecDestroy(s->graphExec);
+  if (s->evSubmit) cudaEventDestroy(s->evSubmit);
+  if (s->evDone) cudaEventDestroy(s->evDone);
   void* bufs[] = {s->d_camK, s->d_camR0, s->d_pa, s->d_na, s->d_dpa, s->d_pb, s->d_nb, s->d_dpb,
                   s->d_cam, s->d_pt, s->d_cobs, s->d_ccam, s->d_xy, s->d_wgt, s->d_ptr, s->d_W,
                   s->d_V, s->d_S, s->d_y, s->d_x, s->d_sc, s->d_outlier,
                   s->d_items, s->d_entries, s->d_Linv, s->d_cnt, s->d_tasks, s->d_bwd, s->d_blkRows,
                   s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_solIdx,
-                  s->d_trace, s->d_sum, s->d_rhsS, s->d_Vinv};
+                  s->d_trace, s->d_sum, s->d_rhsS, s->d_Vinv, s->d_ctl};
   for (void* b : bufs)
     if (b) cudaFreeAsync(b, s->stream);
   if (s->stream) cudaStreamSynchronize(s->stream);
@@ -1149,6 +1160,175 @@ int download(cosl_ba_solver* s, cosl_ba_problem* p) {
   return COSL_OK;
 }
 
+/* ---------------------------------------------------------------- submitted robust loop (ba_ctl.cuh) */
+// Add a conditional node after the current capture position of `cs`; the capture continues behind it.
+int capture_conditional(cudaStream_t cs, cudaGraphConditionalHandle h, cudaGraphConditionalNodeType type,
+                        cudaGraph_t* body) {
+  cudaStreamCaptureStatus st;
+  cudaGraph_t cg = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t nd = 0;
+  COSL_CUDA(cudaStreamGetCaptureInfo(cs, &st, nullptr, &cg, &deps, &nd));
+  cudaGraphNodeParams np = {};
+  np.type = cudaGraphNodeTypeConditional;
+  np.conditional.handle = h;
+  np.conditional.type = type;
+  np.conditional.size = 1;
+  cudaGraphNode_t node;
+  COSL_CUDA(cudaGraphAddNode(&node, cg, deps, nd, &np));
+  *body = np.conditional.phGraph_out[0];
+  COSL_CUDA(cudaStreamUpdateCaptureDependencies(cs, &node, 1, cudaStreamSetCaptureDependencies));
+  return COSL_OK;
+}
+
+// the kernels of one stage of the loop body, enqueued on the capturing stream cs
+int enqueue_stage(cosl_ba_solver* s, cudaStream_t cs, int stage) {
+  const unsigned gN = (unsigned)div_up64(s->N, 256);
+  if (stage == BA_STAGE_ROUND) {  // compute_weights + levmar's initial cost
+    if (s->opt.max_err > 0) {
+      if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, cs, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+    } else if (s->N) {
+      COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, cs, s->d_wgt, s->N, 1.0);
+    }
+    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, cs, s->d, s->d_pa, s->d_pb, 0, 0.0, nullptr);
+  } else if (stage == BA_STAGE_LIN0 || stage == BA_STAGE_LIN) {  // linearize()
+    const long long nV = 9LL * s->n + 27LL * s->m;
+    COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, cs, s->d_V, nV, 0.0);
+    if (s->N) COSL_LAUNCH(ba_linearize_points, gN, 256, 0, cs, s->d, s->d_pa, s->d_pb);
+    if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, cs, s->d, s->d_pa, s->d_pb);
+    // at itno > 0 the prep kernel of the next trial computes the statistics, unless there is none
+    if (stage == BA_STAGE_LIN0 || !s->ns)
+      COSL_LAUNCH(ba_stats_kernel, (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, cs, s->d);
+  } else if (s->ns) {  // solve_trial + the trial cost, free cameras
+    const int nTilesInit = std::max(1, s->plan.nTiles);
+    COSL_LAUNCH(ba_prep_kernel_ctl, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, cs, s->d,
+                s->d_ctl, 1, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks,
+                nTilesInit, s->d_Vinv, s->d_dpb, 3LL * s->n);
+    if (s->nItems)
+      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, cs, s->d,
+                  s->d_items, s->nItems, s->d_entries, s->d_Vinv);
+    if (s->twoSolve)
+      COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, cs, s->td, s->two00, s->two10, s->two11);
+    else
+      COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, cs, s->td);
+    const int nCamBlocks = div_up(6 * s->m, 256);
+    COSL_LAUNCH(ba_back_cams_points_ctl, nCamBlocks + gN, 256, 0, cs, s->d, s->d_ctl, s->d_pa, s->d_x, s->d_dpa,
+                s->d_na, 1, nCamBlocks, s->d_dpb);
+    COSL_LAUNCH(ba_finish_cost_ctl, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, cs, s->d, s->d_ctl,
+                s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv);
+  } else {  // solve_trial + the trial cost, no free camera
+    COSL_LAUNCH(ba_cam_update_ctl,
+                std::max(div_up(6 * s->m, 256), (int)std::min<long long>(s->numSM, div_up64(3LL * s->n, 1024))), 256,
+                0, cs, s->d, s->d_ctl, s->d_pa, s->d_x, s->d_dpa, s->d_na, 1, s->d_nb, 3LL * s->n);
+    if (s->N) COSL_LAUNCH(ba_back_subst, gN, 256, 0, cs, s->d, s->d_dpa, s->d_nb);
+    if (s->n)
+      COSL_LAUNCH(ba_back_finish_ctl, (unsigned)div_up64(s->n, 256), 256, 0, cs, s->d, s->d_ctl, s->d_pb, s->d_nb,
+                  s->d_dpb);
+    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, cs, s->d, s->d_na, s->d_nb, 0, 0.0, nullptr);
+  }
+  COSL_CUDA(cudaGetLastError());
+  return COSL_OK;
+}
+
+// capture into `g` on cs, leaving an empty node in a body that has no kernel (e.g. no observations)
+template <typename F>
+int capture_into(cudaStream_t cs, cudaGraph_t g, F&& enqueue) {
+  COSL_CUDA(cudaStreamBeginCaptureToGraph(cs, g, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+  const int rc = enqueue();
+  cudaGraph_t out = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(cs, &out);
+  COSL_TRY(rc);
+  if (e != cudaSuccess) return set_error(COSL_E_CUDA, "graph capture: %s", cudaGetErrorString(e));
+  size_t nn = 0;
+  COSL_CUDA(cudaGraphGetNodes(g, nullptr, &nn));
+  if (nn == 0) {
+    cudaGraphNode_t empty;
+    COSL_CUDA(cudaGraphAddEmptyNode(&empty, g, nullptr, 0));
+  }
+  return COSL_OK;
+}
+
+// The graph of the submitted robust loop:
+//   ba_ctl_init -> WHILE(loop) { IF(round) -> IF(lin0) -> IF(lin) -> IF(trial) -> ba_ctl_step -> ba_ctl_accept }
+//   -> outlier pass
+int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
+  BaCtlParams P = {};
+  const double* o = s->opt.opts;
+  P.tau = o[0];
+  P.eps1 = o[1];
+  P.eps2 = o[2];
+  P.eps3 = o[3];
+  P.eps4 = o[4];
+  P.rounds = std::max(1, s->opt.outer_iters);
+  P.itmax = s->opt.inner_iters;
+  P.ns = s->ns;
+  P.hasObs = s->N > 0;
+  P.outliers = s->opt.max_err > 0;
+  COSL_CUDA(cudaGraphConditionalHandleCreate(&P.hLoop, g, 1, cudaGraphCondAssignDefault));
+  for (int k = 0; k < BA_NSTAGES; ++k)
+    COSL_CUDA(cudaGraphConditionalHandleCreate(&P.hStage[k], g, k == BA_STAGE_ROUND ? 1 : 0, cudaGraphCondAssignDefault));
+  cudaGraph_t loopBody = nullptr, stageBody[BA_NSTAGES] = {};
+  COSL_TRY(capture_into(cs, g, [&]() -> int {
+    COSL_LAUNCH(ba_ctl_init, 1, 32, 0, cs, s->d_ctl, s->d_sc);
+    COSL_TRY(capture_conditional(cs, P.hLoop, cudaGraphCondTypeWhile, &loopBody));
+    if (s->opt.max_err > 0) {  // the outlier pass of run_robust; ba_ctl_step cleared the count
+      if (s->N)
+        COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, cs, s->d, s->d_pa, s->d_pb, 2,
+                    s->opt.max_err, s->d_outlier);
+    } else {
+      COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, cs));
+    }
+    COSL_CUDA(cudaGetLastError());
+    return COSL_OK;
+  }));
+  COSL_TRY(capture_into(cs, loopBody, [&]() -> int {
+    for (int k = 0; k < BA_NSTAGES; ++k) COSL_TRY(capture_conditional(cs, P.hStage[k], cudaGraphCondTypeIf, &stageBody[k]));
+    COSL_LAUNCH(ba_ctl_step, 1, 32, 0, cs, s->d_ctl, s->d_sc, P);
+    const long long nA = 6LL * s->m, nB = 3LL * s->n;
+    COSL_LAUNCH(ba_ctl_accept, (unsigned)std::max<long long>(1, std::min<long long>(4LL * s->numSM, div_up64(nA + nB, 256))),
+                256, 0, cs, s->d_ctl, s->d_pa, s->d_na, nA, s->d_pb, s->d_nb, nB);
+    COSL_CUDA(cudaGetLastError());
+    return COSL_OK;
+  }));
+  for (int k = 0; k < BA_NSTAGES; ++k) COSL_TRY(capture_into(cs, stageBody[k], [&]() { return enqueue_stage(s, cs, k); }));
+  return COSL_OK;
+}
+
+int build_graph(cosl_ba_solver* s) {
+  if (s->graphExec) {
+    COSL_CUDA(cudaStreamSynchronize(s->stream));
+    cudaGraphExecDestroy(s->graphExec);
+    s->graphExec = nullptr;
+  }
+  int drv = 0;
+  COSL_CUDA(cudaDriverGetVersion(&drv));
+  if (drv < 12040)
+    return set_error(COSL_E_CUDA,
+                     "cosl_ba_solver_submit: the CUDA driver (version %d) has no conditional graph nodes (12.4 or "
+                     "newer is needed)", drv);
+  if (!s->d_ctl) COSL_TRY(dev_alloc(s->stream, &s->d_ctl, 1));
+  cudaStream_t cs = nullptr;
+  COSL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+  cudaGraph_t g = nullptr;
+  cudaError_t e = cudaGraphCreate(&g, 0);
+  int rc = e == cudaSuccess ? build_graph_nodes(s, cs, g) : set_error(COSL_E_CUDA, "cudaGraphCreate: %s", cudaGetErrorString(e));
+  if (rc == COSL_OK) {
+    e = cudaGraphInstantiate(&s->graphExec, g, 0);
+    if (e != cudaSuccess) {
+      s->graphExec = nullptr;
+      rc = set_error(COSL_E_CUDA, "cosl_ba_solver_submit: graph instantiation failed: %s", cudaGetErrorString(e));
+    }
+  }
+  if (g) cudaGraphDestroy(g);
+  cudaStreamDestroy(cs);
+  if (rc != COSL_OK) return rc;
+  s->graphPa = s->d_pa;
+  s->graphNa = s->d_na;
+  s->graphPb = s->d_pb;
+  s->graphNb = s->d_nb;
+  return COSL_OK;
+}
+
 }  // namespace
 
 /* ================================================================ C-ABI */
@@ -1251,8 +1431,12 @@ int cosl_ba_solver_create(const cosl_ba_problem* prob, const cosl_ba_options* op
   if (!(s)) return set_error(COSL_E_INVALID, "null solver handle"); \
   COSL_CUDA(cudaSetDevice((s)->device));
 
+#define BA_IDLE(s, what) \
+  if ((s)->inFlight) return set_error(COSL_E_STATE, what ": a submitted solve is not collected yet");
+
 int cosl_ba_solver_reset(cosl_ba_solver* s, const cosl_ba_problem* prob) {
   BA_ENTER(s)
+  BA_IDLE(s, "cosl_ba_solver_reset")
   if (!prob || prob->m != s->m || prob->n != s->n)
     return set_error(COSL_E_INVALID, "cosl_ba_solver_reset: problem shape changed");
   s->timer.reset();
@@ -1261,23 +1445,93 @@ int cosl_ba_solver_reset(cosl_ba_solver* s, const cosl_ba_problem* prob) {
 
 int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
+  BA_IDLE(s, "cosl_ba_solver_run")
   return run_robust(s, 0, info);
 }
 
 int cosl_ba_solver_run_fixed(cosl_ba_solver* s, int trials, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
+  BA_IDLE(s, "cosl_ba_solver_run_fixed")
   return run_robust(s, trials < 1 ? 1 : trials, info);
 }
 
 int cosl_ba_solver_download(cosl_ba_solver* s, cosl_ba_problem* prob) {
   BA_ENTER(s)
+  BA_IDLE(s, "cosl_ba_solver_download")
   if (!prob || prob->m != s->m || prob->n != s->n)
     return set_error(COSL_E_INVALID, "cosl_ba_solver_download: problem shape changed");
   return download(s, prob);
 }
 
+int cosl_ba_solver_submit(cosl_ba_solver* s) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID,
+                     "cosl_ba_solver_submit: a multi-rank solver exchanges over NCCL between host-ordered steps; "
+                     "use cosl_ba_solver_run");
+  BA_IDLE(s, "cosl_ba_solver_submit")
+  // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
+  if (!s->graphExec || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
+      s->graphNb != s->d_nb)
+    COSL_TRY(build_graph(s));
+  if (!s->evSubmit) COSL_CUDA(cudaEventCreate(&s->evSubmit));
+  if (!s->evDone) COSL_CUDA(cudaEventCreate(&s->evDone));
+  COSL_CUDA(cudaEventRecord(s->evSubmit, s->stream));
+  COSL_CUDA(cudaGraphLaunch(s->graphExec, s->stream));
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  COSL_CUDA(cudaEventRecord(s->evDone, s->stream));
+  s->inFlight = true;
+  return COSL_OK;
+}
+
+int cosl_ba_solver_query(cosl_ba_solver* s, int* done) {
+  BA_ENTER(s)
+  if (!done) return set_error(COSL_E_INVALID, "cosl_ba_solver_query: null argument");
+  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_ba_solver_query: nothing submitted");
+  const cudaError_t e = cudaEventQuery(s->evDone);
+  if (e == cudaErrorNotReady) {
+    *done = 0;
+    return COSL_OK;
+  }
+  COSL_CUDA(e);
+  *done = 1;
+  return COSL_OK;
+}
+
+int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
+  BA_ENTER(s)
+  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_ba_solver_collect: nothing submitted");
+  s->inFlight = false;
+  COSL_CUDA(cudaEventSynchronize(s->evDone));
+  BaCtl c;
+  double nout = 0;
+  COSL_CUDA(cudaMemcpyAsync(&c, s->d_ctl, sizeof(c), cudaMemcpyDeviceToHost, s->stream));
+  COSL_CUDA(cudaMemcpyAsync(&nout, s->d_sc + SC_COST, sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  float ms = 0.f;
+  COSL_CUDA(cudaEventElapsedTime(&ms, s->evSubmit, s->evDone));
+  if (info) {  // the fields of run_robust
+    for (int k = 0; k < COSL_BA_INFOSZ; ++k) info[k] = 0;
+    info[0] = c.first_e0;
+    info[1] = c.p_eL2;
+    info[2] = c.ginf;
+    info[3] = c.dp_L2;
+    info[4] = c.maxdiag > 0 ? c.mu / c.maxdiag : 0;
+    info[5] = c.itno;
+    info[6] = c.stop;
+    info[7] = c.nfev;
+    info[8] = c.njev;
+    info[9] = c.nlss;
+    info[10] = c.totalTrials;
+    info[11] = 1e-3 * ms;
+    info[12] = c.p_eL2;
+    info[13] = s->opt.max_err > 0 ? nout : 0.0;
+  }
+  return COSL_OK;
+}
+
 int cosl_ba_solver_destroy(cosl_ba_solver* s) {
-  free_solver(s);
+  free_solver(s);  // waits for a submitted solve that is still in flight
   return COSL_OK;
 }
 

@@ -715,9 +715,8 @@ ba_back_subst(BaDev d, const double* __restrict__ dpa, double* __restrict__ acc3
 
 // Back substitution, step 2, one point per thread: nb holds t_i on entry; db_i = V*_i^-1 (eb_i - t_i),
 // nb <- pb + db, plus the point-side parts of |dp|^2, dL, |p|^2.
-__global__ void __launch_bounds__(256)
-ba_back_finish(BaDev d, const double* __restrict__ pb, double* __restrict__ nb,
-               double* __restrict__ dpb, double mu) {
+__device__ __forceinline__ void ba_back_finish_body(const BaDev& d, const double* __restrict__ pb,
+                                                    double* __restrict__ nb, double* __restrict__ dpb, double mu) {
   __shared__ double s_red[8];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double dp2 = 0, dl = 0, p2 = 0;
@@ -753,12 +752,18 @@ ba_back_finish(BaDev d, const double* __restrict__ pb, double* __restrict__ nb,
   if (threadIdx.x == 0 && t != 0) atomicAdd(&d.sc[SC_P_L2], t);
 }
 
+__global__ void __launch_bounds__(256)
+ba_back_finish(BaDev d, const double* __restrict__ pb, double* __restrict__ nb,
+               double* __restrict__ dpb, double mu) {
+  ba_back_finish_body(d, pb, nb, dpb, mu);
+}
+
 // Trial camera parameters na = pa + dpa and the camera-side parts of |dp|^2, dL, |p|^2.
 // addSums: only one rank contributes the (replicated) camera-side sums.
-__global__ void __launch_bounds__(256)
-ba_cam_update(BaDev d, const double* __restrict__ pa, const double* __restrict__ sol,
-              double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums,
-              double* __restrict__ zeroBuf, long long zeroCount) {
+__device__ __forceinline__ void ba_cam_update_body(const BaDev& d, const double* __restrict__ pa,
+                                                   const double* __restrict__ sol, double* __restrict__ dpa,
+                                                   double* __restrict__ na, double mu, int addSums,
+                                                   double* __restrict__ zeroBuf, long long zeroCount) {
   __shared__ double s_red[8];
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   for (long long q = t; q < zeroCount; q += (long long)gridDim.x * blockDim.x) zeroBuf[q] = 0.0;
@@ -783,6 +788,13 @@ ba_cam_update(BaDev d, const double* __restrict__ pa, const double* __restrict__
   if (threadIdx.x == 0 && addSums && s != 0) atomicAdd(&d.sc[SC_P_L2], s);
 }
 
+__global__ void __launch_bounds__(256)
+ba_cam_update(BaDev d, const double* __restrict__ pa, const double* __restrict__ sol,
+              double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums,
+              double* __restrict__ zeroBuf, long long zeroCount) {
+  ba_cam_update_body(d, pa, sol, dpa, na, mu, addSums, zeroBuf, zeroCount);
+}
+
 // ------------------------------------------------------------------------------------------
 // Back substitution in two launches (instead of cam update | memset | point accumulate | point finish | cost):
 //  ba_back_cams_points: blocks [0, nCamBlocks) form the trial camera parameters na = pa + da and the camera-side
@@ -794,10 +806,10 @@ ba_cam_update(BaDev d, const double* __restrict__ pa, const double* __restrict__
 //    point-side sums), then the weighted squared residual at (na, nb_i) -> cost.  Extra threads finish the
 //    points that have no observation.
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-ba_back_cams_points(BaDev d, const double* __restrict__ pa, const double* __restrict__ sol,
-                    double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums, int nCamBlocks,
-                    double* __restrict__ acc3) {
+__device__ __forceinline__ void ba_back_cams_points_body(const BaDev& d, const double* __restrict__ pa,
+                                                         const double* __restrict__ sol, double* __restrict__ dpa,
+                                                         double* __restrict__ na, double mu, int addSums,
+                                                         int nCamBlocks, double* __restrict__ acc3) {
   __shared__ double s_red[8];
   if ((int)blockIdx.x < nCamBlocks) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -851,8 +863,16 @@ ba_back_cams_points(BaDev d, const double* __restrict__ pa, const double* __rest
 }
 
 __global__ void __launch_bounds__(256)
-ba_finish_cost(BaDev d, const double* __restrict__ na, const double* __restrict__ pb, double* __restrict__ nb,
-               const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu) {
+ba_back_cams_points(BaDev d, const double* __restrict__ pa, const double* __restrict__ sol,
+                    double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums, int nCamBlocks,
+                    double* __restrict__ acc3) {
+  ba_back_cams_points_body(d, pa, sol, dpa, na, mu, addSums, nCamBlocks, acc3);
+}
+
+__device__ __forceinline__ void ba_finish_cost_body(const BaDev& d, const double* __restrict__ na,
+                                                    const double* __restrict__ pb, double* __restrict__ nb,
+                                                    const double* __restrict__ acc3,
+                                                    const double* __restrict__ Vinv, double mu) {
   __shared__ double s_red[8];
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double dp2 = 0, dl = 0, p2 = 0, c = 0;
@@ -916,6 +936,12 @@ ba_finish_cost(BaDev d, const double* __restrict__ na, const double* __restrict_
   if (threadIdx.x == 0 && s != 0) atomicAdd(&d.sc[SC_DL], s);
   s = block_sum_1(p2, s_red);
   if (threadIdx.x == 0 && s != 0) atomicAdd(&d.sc[SC_P_L2], s);
+}
+
+__global__ void __launch_bounds__(256)
+ba_finish_cost(BaDev d, const double* __restrict__ na, const double* __restrict__ pb, double* __restrict__ nb,
+               const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu) {
+  ba_finish_cost_body(d, na, pb, nb, acc3, Vinv, mu);
 }
 
 }  // namespace coslam

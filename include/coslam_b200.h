@@ -396,6 +396,16 @@ int cosl_ba_solver_run_fixed(cosl_ba_solver* s, int trials, double info[COSL_BA_
 int cosl_ba_solver_download(cosl_ba_solver* s, cosl_ba_problem* prob);
 int cosl_ba_solver_destroy(cosl_ba_solver* s);
 void* cosl_ba_solver_stream(cosl_ba_solver* s);
+/* Non-blocking form of cosl_ba_solver_run.  submit enqueues the same robust loop on the solver's
+ * stream and returns at once: the device takes every LM decision (no host read-back until collect).
+ * query sets *done = 1 once it has finished, without waiting.  collect waits for it and writes the
+ * info fields of run; [11] is the device time from submit to the end of the loop.  download then
+ * returns the result.  While a submit is in flight, run, run_fixed, reset, download and submit give
+ * COSL_E_STATE; query and collect with nothing in flight give COSL_E_STATE; destroy waits for it.
+ * A solver with a multi-rank comm gives COSL_E_INVALID; opt->verbose is ignored. */
+int cosl_ba_solver_submit(cosl_ba_solver* s);
+int cosl_ba_solver_query(cosl_ba_solver* s, int* done);
+int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]);
 /* Per-kernel accumulated device time in ms since create/reset, by name (NULL-terminated list via
  * index): returns name or NULL when idx is out of range. */
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls);
