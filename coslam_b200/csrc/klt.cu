@@ -4,7 +4,6 @@
 // frame costs one H2D copy per camera, one D2H copy of the feature table and one synchronise.
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <new>
 #include <vector>
@@ -508,19 +507,33 @@ static bool tracker_reads_level0(const cosl_klt* g) { return (g->L - 1) % g->lev
 // the persistent gain tracker (klt_gain_fused) runs, not the per-pass kernels or the 2x2 tracker
 static bool fused_tracker(const cosl_klt* g) { return g->cfg.trackWithGain && g->fusedOK; }
 
-// What the stages of one frame fold together; run_frame decides it for the frame's kind, run_step
-// for the union of its cameras' ops.
+// Everything that differs between the frames run_frame enqueues: plan_frame decides it for a frame of
+// one kind, plan_step for a step whose cameras have different ops.
 struct FramePlan {
   const KltCam* cams;   // the camera table the kernels read: the group's, or a step's (stages)
   bool mixed;           // the kernels' MIXED instantiation runs (reads `cams`)
   bool tracked;         // the tracker runs (for some camera)
   int cornMode;         // FrontParams::wantCorn: 0, 1, or KLT_CORN_PER_CAM (a step)
-  bool wantCorn;        // klt_front also produces the detector's cornerness map (for some camera)
+  bool wantCorn;        // klt_front also produces the detector's cornerness map, and the detector runs
+                        // (for some camera)
   bool storeL0;         // klt_front stores pyramid level 0
+  bool lv0[64];         // the record of camera c's slice of the buffer the front pass writes (lv0Stored)
   bool earlyPrefilter;  // the detector's prefilter runs on auxStream right after klt_front
   bool trackerTail;     // the tracker writes the feature table (klt_status) and, with wantCorn, the
                         // suppression marks of the live tracks (klt_suppress) itself
-  bool foldAdvance;     // klt_select_refill also writes the provided set to d_src (the advance copy)
+  bool foldAdvance;     // klt_select_refill also writes the provided set to d_src (the advance copy),
+                        // and the frame ends with the pyramid half of the advance
+  int detectMode = 0;   // run_detector's mode
+  int maxPresent = 0;   // detect: the longest present list (upload_present)
+  bool provideAll = false;  // track: the tracked set becomes every camera's feature table (klt_copy_f4)
+  KltCamList provide{};     // a step's TRACK cameras: their tracked sets go to both feature buffers
+  // a step's only (plan_step)
+  const uint8_t* ops = nullptr;  // the cameras with COSL_KLT_OP_SKIP are neither uploaded nor built
+  int tab = -1;                  // its op table: h_stepCams[tab] -> d_stepCams[tab] == cams
+  bool intoP1 = false;           // the front pass writes p1, not the third buffer, and so does the next
+  bool flip = false;             // intoP1: p0 and p1 change roles at the end of the frame
+  KltCamList exchangeEarly{};    // slices of p0 and p1 exchanged ahead of the front pass
+  KltCamList exchangeLate{};     // ... after the tracker, or after the detector when nothing is tracked
 };
 
 // PyramidWithDerivativesCreator::buildPyramidForGrayscaleImage (v3d_gpupyramid.cpp:366-429), on the
@@ -658,36 +671,6 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
                                           dim3(KLT_FUSED_THREADS), args, 0, g->stream));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     g->verBase += nPass;
-#if KLT_EXP_CLOCK
-    {
-      static int calls = 0;
-      if (++calls == 50) {
-        cudaStreamSynchronize(g->stream);
-        const int nw = g->fusedBlocks * KLT_FUSED_THREADS / 32;
-        std::vector<float> hs((size_t)nw * 12);
-        cudaMemcpy(hs.data(), g->d_state, sizeof(float) * hs.size(), cudaMemcpyDeviceToHost);
-        double acc[6] = {0, 0, 0, 0, 0, 0}, mx = 0;
-        unsigned s0 = ~0u, s1 = 0, e0 = ~0u, e1 = 0;
-        for (int i = 0; i < nw; ++i) {
-          for (int k = 0; k < 6; ++k) acc[k] += hs[(size_t)i * 12 + k];
-          mx = std::max(mx, (double)hs[(size_t)i * 12 + 5]);
-          unsigned a, b;
-          memcpy(&a, &hs[(size_t)i * 12 + 6], 4);
-          memcpy(&b, &hs[(size_t)i * 12 + 7], 4);
-          s0 = std::min(s0, a); s1 = std::max(s1, a); e0 = std::min(e0, b); e1 = std::max(e1, b);
-        }
-        if (const char* dump = std::getenv("COSL_KLT_CLOCK_DUMP")) {
-          if (FILE* f = fopen(dump, "wb")) {
-            fwrite(hs.data(), sizeof(float), hs.size(), f);
-            fclose(f);
-          }
-        }
-        fprintf(stderr, "[klt clock] globaltimer ns: start spread %u, end spread %u, first start -> last end %u, last start -> first end %u\n", s1 - s0, e1 - e0, e1 - s0, e0 - s1);
-        fprintf(stderr, "[klt clock] warps %d  mean cycles: poll %.0f  pre+stage %.0f  loop %.0f  finish %.0f  (stage-only %.0f)  total %.0f max %.0f\n", nw,
-                acc[0] / nw, acc[1] / nw, acc[2] / nw, acc[3] / nw, acc[4] / nw, acc[5] / nw, mx);
-      }
-    }
-#endif
   } else if (g->cfg.trackWithGain) {
     const float4* in = g->d_src;
     float4* bufs[2] = {g->d_ping, g->d_pong};
@@ -729,10 +712,11 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
 }
 
 // KLT_Detector::detectCorners + extractCorners (v3d_gpuklt.cpp:423-588) and the slot logic of
-// detect/redetect (:651-805) on the cornerness map klt_front produced for this frame.  mode 0: detect
-// (present = the external points of upload_present, maxPresent = the longest list), 1: redetect,
-// 2: per camera of a step (klt_select_refill).
-int run_detector(cosl_klt* g, int mode, int maxPresent, const FramePlan& p) {
+// detect/redetect (:651-805) on the cornerness map klt_front produced for this frame.  p.detectMode
+// 0: detect (present = the external points of upload_present, p.maxPresent = the longest list),
+// 1: redetect, 2: per camera of a step (klt_select_refill).
+int run_detector(cosl_klt* g, const FramePlan& p) {
+  const int mode = p.detectMode, maxPresent = p.maxPresent;
   g->timer.begin(g->secDetect, g->stream);
   const long long cs = (long long)g->W * g->H;
   float* corn = g->d_corn[g->par];
@@ -889,30 +873,11 @@ enum FrameKind {
   FRAME_REDETECT,  // redetect, next, next_dev, submit: as FRAME_TRACK, then the detector refills
 };
 
-// One frame through its stages, asynchronous on g->stream and, joined into it before the call
-// returns, the front stream (image copies, klt_front, pyramid tail) and auxStream (the early
-// prefilter).  This is the one place that decides how a frame is scheduled and which launches it
-// folds together.  imgs, pitch, copyKind: the frame's images (upload_images).  maxPresent: the
-// longest present list of a detect (upload_present).  foldAdvance (detector kinds): advanceFrame
-// follows the frame, and klt_select_refill writes the provided set to both feature buffers, so the
-// advance is the pyramid flip alone.  Nothing of the plan outlives the call.
-//
-// Frame n+1's image copies wait only for frame n's front pass.  Its front pass and pyramid tail wait
-// only for the fences of the buffers they write, each recorded on g->stream behind that buffer's
-// last reader or writer there.  Between frames that advance, that is frame n-1's tracker, so the
-// steady state of back-to-back frames is
-//   tracker(n-1) | front(n+1) next to detector(n-1) | tracker(n) next to tail(n+1) | front(n+2) ...
-// What the front stream writes, its ring and its fence:
-//   d_img                    one; read by the front passes only (same stream; copy stream: evFront)
-//   d_pyr[nxt]               three (p0, p1, nxt); evPyr[b], recorded after each tracker for the two
-//                            buffers it reads and after each exchange of slices (klt_advance_cams)
-//   d_corn, d_prelim,        three sets; the tracker's marks, klt_suppress, verify, select and the
-//   d_counters[.][8c + 4]    read-backs use set `par`.  A frame with a cornerness map moves on to the
-//                            next set and records the fence evPar of the set it leaves (next_par)
-//   d_stepCams[tab]          three (run_step); evStepFence[t], recorded at the end of the step
-// and it reads d_cams, which update_cameras rewrites on g->stream (evCams).
-int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind,
-              int maxPresent, bool foldAdvance) {
+// The plan of a frame of one kind for every camera.  maxPresent: the longest present list of a
+// detect (upload_present).  foldAdvance (detector kinds): advanceFrame follows the frame, and
+// klt_select_refill writes the provided set to both feature buffers, so the advance is the pyramid
+// flip alone.
+static FramePlan plan_frame(const cosl_klt* g, FrameKind kind, int maxPresent, bool foldAdvance) {
   FramePlan p;
   p.cams = g->d_cams;
   p.mixed = g->mixed;
@@ -923,42 +888,14 @@ int run_frame(cosl_klt* g, FrameKind kind, const uint8_t* const* imgs, size_t pi
   // visits level 0 reads that level.  It is stored only then: at 16 B/px it is larger than the L2,
   // and writing it would evict the pyramid levels the tracker that follows reads.
   p.storeL0 = kind != FRAME_REDETECT || tracker_reads_level0(g);
+  std::fill(p.lv0, p.lv0 + g->C, p.storeL0);
   p.earlyPrefilter = kind == FRAME_REDETECT;
   p.trackerTail = fused_tracker(g);
   p.foldAdvance = foldAdvance;
-  g->stepOpsValid = false;
-  if (p.wantCorn) COSL_TRY(next_par(g));
-  int* counters = g->d_counters[g->par];
-  // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below
-  COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
-  // the images ahead of the fences: d_img is read by the front passes alone, so they run under the
-  // previous frame's tracker
-  COSL_TRY(upload_images(g, imgs, pitch, copyKind, nullptr));
-  COSL_TRY(front_waits(g, p.wantCorn, -1));
-  if (p.wantCorn)
-    COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
-  for (int c = 0; c < g->C; ++c) g->lv0Stored[g->nxt][c] = p.storeL0;
-  COSL_TRY(build_pyramid(g, p));
-  COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
-  COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
-  if (kind != FRAME_DETECT) {
-    COSL_TRY(run_tracker(g, p));
-    COSL_TRY(fence_pyr(g, g->p0));
-    COSL_TRY(fence_pyr(g, g->p1));
-    if (!p.trackerTail) {
-      dim3 grid(div_up(g->F, 256), g->C);
-      COSL_LAUNCH(klt_status<false>, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, g->d_cams);
-    }
-  }
-  if (kind == FRAME_TRACK) {
-    // provide: the tracked set becomes the feature table of the next frame
-    const size_t n = (size_t)g->F * g->C;
-    COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, g->stream, g->d_res, g->d_dst, n);
-  } else {
-    COSL_TRY(run_detector(g, kind == FRAME_REDETECT ? 1 : 0, maxPresent, p));
-  }
-  if (foldAdvance) advance_pyramids(g);
-  return COSL_OK;
+  p.detectMode = kind == FRAME_REDETECT ? 1 : 0;
+  p.maxPresent = maxPresent;
+  p.provideAll = kind == FRAME_TRACK;
+  return p;
 }
 
 // the stages of a cosl_klt_group_step op (KltCam::stages)
@@ -969,112 +906,170 @@ static int op_stages(int op) {
                                    : 0;
 }
 
-// One step of cosl_klt_group_step: camera c gets ops[c] followed by advanceFrame, or nothing.
-// Every camera with the same op: the frame of that kind (run_frame), exactly as group_first /
-// group_next / track + advance run it.  Otherwise one frame whose kernels are the MIXED
-// instantiations on a table of the step's own (KltCam::stages), so each launch covers the group
-// and a camera's blocks exit in the stages its op does not have:
+// The plan of a step whose cameras do not all have the same op, and its op table: the group's table
+// with each camera's stages, written to h_stepCams[tab].  The kernels are the MIXED instantiations on
+// that table, so each launch covers the group and a camera's blocks exit in the stages its op does
+// not have:
 //   pyramid (front pass, tail)       FIRST, TRACK, NEXT
 //   tracker, status                  TRACK, NEXT
 //   cornerness, non-max, selection   FIRST, NEXT      (klt_select_refill: mode per camera)
 //   provide (klt_provide_cams)       TRACK
-// The frame's schedule is run_frame's, with the plan of the union of the ops: the front pass stores
-// level 0 when one of its cameras needs it, the prefilter runs early, and a step with a detecting
-// camera moves on to the next counter set.
+// The folds are those of the union of the ops: the front pass stores level 0 when one of its cameras
+// needs it (each camera's record is what its single tracker records), the prefilter runs early, and
+// a step with a detecting camera moves on to the next counter set.
 //
 // Advance of a strict subset: the pyramid slices of either the skipped or the addressed cameras
 // are exchanged, whichever are fewer.  Skipped ones: p0 and p1 change roles for the group and their
-// slices are exchanged ahead of the tracker (nothing of the step touches them); addressed ones: the
-// roles stay and their slices are exchanged after the tracker.  Such a step builds into p1, as the
-// two-buffer tracker does, not into the third buffer: then the skipped cameras would need their
+// slices are exchanged ahead of the front pass (nothing of the step touches them); addressed ones:
+// the roles stay and their slices are exchanged after the tracker.  Such a step builds into p1, as
+// the two-buffer tracker does, not into the third buffer: then the skipped cameras would need their
 // slices of all three buffers rotated, where one exchange of two buffers moves the same bytes.  So
 // it waits for the tracker before it, and the next step for its own.  The feature-buffer half of the
 // advance is folded into klt_select_refill and klt_provide_cams.
+static FramePlan plan_step(cosl_klt* g, const uint8_t* ops, int tab) {
+  FramePlan p;
+  p.cams = g->d_stepCams[tab];
+  p.mixed = true;
+  p.tracked = p.wantCorn = p.storeL0 = false;
+  KltCamList addr, skip;
+  addr.n = skip.n = 0;
+  KltCam* hstep = g->h_stepCams[tab];
+  for (int c = 0; c < g->C; ++c) {
+    const int st = op_stages(ops[c]);
+    hstep[c] = g->hcam[c];
+    hstep[c].stages = st;
+    if (!st) {
+      skip.cam[skip.n++] = c;
+      continue;
+    }
+    addr.cam[addr.n++] = c;
+    if (ops[c] == COSL_KLT_OP_TRACK) p.provide.cam[p.provide.n++] = c;
+    p.tracked = p.tracked || (st & KLT_STAGE_TRACK);
+    p.wantCorn = p.wantCorn || (st & KLT_STAGE_DETECT);
+    p.lv0[c] = ops[c] != COSL_KLT_OP_NEXT || tracker_reads_level0(g);
+    p.storeL0 = p.storeL0 || p.lv0[c];
+  }
+  p.cornMode = p.wantCorn ? KLT_CORN_PER_CAM : 0;
+  p.earlyPrefilter = p.wantCorn;
+  p.trackerTail = fused_tracker(g);
+  p.foldAdvance = true;
+  p.detectMode = 2;
+  p.ops = ops;
+  p.tab = tab;
+  p.intoP1 = true;
+  p.flip = skip.n <= addr.n;
+  if (p.flip)
+    p.exchangeEarly = skip;
+  else
+    p.exchangeLate = addr;
+  return p;
+}
+
+// One frame through its stages, asynchronous on g->stream and, joined into it before the call
+// returns, the front stream (image copies, klt_front, pyramid tail) and auxStream (the early
+// prefilter).  Every entry point that processes a frame, the per-camera steps included, enqueues it
+// here; what differs between frames is decided before, in the plan (plan_frame, plan_step).  imgs,
+// pitch, copyKind: the frame's images (upload_images).  Nothing of the plan outlives the call.
+//
+// Frame n+1's image copies wait only for frame n's front pass.  Its front pass and pyramid tail wait
+// only for the fences of the buffers they write, each recorded on g->stream behind that buffer's
+// last reader or writer there.  Between frames that advance, that is frame n-1's tracker, so the
+// steady state of back-to-back frames is
+//   tracker(n-1) | front(n+1) next to detector(n-1) | tracker(n) next to tail(n+1) | front(n+2) ...
+// What the front stream writes, its ring and its fence:
+//   d_img                    one; read by the front passes only (same stream; copy stream: evFront)
+//   d_pyr[nxt]               three (p0, p1, nxt; a step's nxt is p1); evPyr[b], recorded after each
+//                            tracker for the two buffers it reads and after each exchange of slices
+//   d_corn, d_prelim,        three sets; the tracker's marks, klt_suppress, verify, select and the
+//   d_counters[.][8c + 4]    read-backs use set `par`.  A frame with a cornerness map moves on to the
+//                            next set and records the fence evPar of the set it leaves (next_par)
+//   d_stepCams[tab]          three, a step's op table: copied from h_stepCams[tab] after the waits
+//                            (evStepTab[tab] follows the copy); evStepFence[tab], recorded at the end
+//                            of the step
+// and it reads d_cams, which update_cameras rewrites on g->stream (evCams).  A step exchanges pyramid
+// slices of p0 and p1 (klt_advance_cams, which fences both) on g->stream: exchangeEarly is enqueued
+// after the front stream's waits, which must not wait for it (the front pass writes the other
+// cameras' slices only); exchangeLate takes the place of the tracker's fences, or follows the
+// detector when nothing is tracked.
+int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
+  g->stepOpsValid = false;
+  if (p.wantCorn) COSL_TRY(next_par(g));
+  int* counters = g->d_counters[g->par];
+  // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below
+  COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
+  // the images ahead of the fences: d_img is read by the front passes alone, so they run under the
+  // previous frame's tracker
+  COSL_TRY(upload_images(g, imgs, pitch, copyKind, p.ops));
+  if (p.intoP1) g->nxt = g->p1;
+  COSL_TRY(front_waits(g, p.wantCorn, p.tab));
+  COSL_TRY(exchange_slices(g, p.exchangeEarly, 0));
+  if (p.tab >= 0) {
+    COSL_CUDA(cudaMemcpyAsync(g->d_stepCams[p.tab], g->h_stepCams[p.tab], sizeof(KltCam) * g->C,
+                              cudaMemcpyHostToDevice, g->frontStream));
+    COSL_CUDA(cudaEventRecord(g->evStepTab[p.tab], g->frontStream));
+  }
+  if (p.wantCorn)
+    COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
+  for (int c = 0; c < g->C; ++c)
+    if (!p.ops || p.ops[c] != COSL_KLT_OP_SKIP) g->lv0Stored[g->nxt][c] = p.lv0[c];
+  COSL_TRY(build_pyramid(g, p));
+  COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
+  COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
+  if (p.tracked) {
+    COSL_TRY(run_tracker(g, p));
+    if (p.exchangeLate.n) {
+      COSL_TRY(exchange_slices(g, p.exchangeLate, 0));
+    } else {
+      COSL_TRY(fence_pyr(g, g->p0));
+      COSL_TRY(fence_pyr(g, g->p1));
+    }
+    if (!p.trackerTail) {
+      // on a step's table the cameras outside the tracker stage exit
+      const auto status = p.tab < 0 ? klt_status<false> : klt_status<true>;
+      dim3 grid(div_up(g->F, 256), g->C);
+      COSL_LAUNCH(status, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, p.cams);
+    }
+  }
+  // provide: the tracked set becomes the feature table of the next frame
+  if (p.provideAll) {
+    const size_t n = (size_t)g->F * g->C;
+    COSL_LAUNCH(klt_copy_f4, (unsigned)div_up64(n, 256), 256, 0, g->stream, g->d_res, g->d_dst, n);
+  }
+  if (p.provide.n)
+    COSL_LAUNCH(klt_provide_cams, dim3(div_up(g->F, 256), p.provide.n), 256, 0, g->stream, g->d_res, g->d_dst,
+                g->d_src, g->F, p.provide);
+  if (p.wantCorn) COSL_TRY(run_detector(g, p));
+  if (!p.tracked) COSL_TRY(exchange_slices(g, p.exchangeLate, 0));
+  if (p.tab >= 0) COSL_CUDA(cudaEventRecord(g->evStepFence[p.tab], g->stream));
+  if (p.intoP1) {
+    if (p.flip) std::swap(g->p0, g->p1);
+    g->nxt = g->p1;
+  } else if (p.foldAdvance) {
+    advance_pyramids(g);
+  }
+  return COSL_OK;
+}
+
+// One step of cosl_klt_group_step: camera c gets ops[c] followed by advanceFrame, or nothing.
+// Every camera with the same op: the frame of that kind, exactly as group_first / group_next /
+// track + advance run it.  Otherwise one frame with plan_step's plan, on the next op table.
 int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
   const int C = g->C;
   int nOp[4] = {0, 0, 0, 0};
   for (int c = 0; c < C; ++c) ++nOp[ops[c]];
   if (nOp[COSL_KLT_OP_NEXT] == C) {
-    COSL_TRY(run_frame(g, FRAME_REDETECT, imgs, pitch, copyKind, 0, true));
+    COSL_TRY(run_frame(g, plan_frame(g, FRAME_REDETECT, 0, true), imgs, pitch, copyKind));
   } else if (nOp[COSL_KLT_OP_FIRST] == C) {
-    COSL_TRY(run_frame(g, FRAME_DETECT, imgs, pitch, copyKind, 0, true));
+    COSL_TRY(run_frame(g, plan_frame(g, FRAME_DETECT, 0, true), imgs, pitch, copyKind));
   } else if (nOp[COSL_KLT_OP_TRACK] == C) {
-    COSL_TRY(run_frame(g, FRAME_TRACK, imgs, pitch, copyKind, 0, false));
+    COSL_TRY(run_frame(g, plan_frame(g, FRAME_TRACK, 0, false), imgs, pitch, copyKind));
     COSL_TRY(advance(g));
   } else if (nOp[COSL_KLT_OP_SKIP] < C) {
-    KltCamList addr, skip, provide;
-    addr.n = skip.n = provide.n = 0;
-    bool anyTrack = false, anyDetect = false, storeL0 = false;
-    bool lv0[64];  // what a single tracker records for the frame of the camera's op
     // the pinned table's previous copy was enqueued three steps ago: the host waits here only when
     // it runs more than two steps ahead of the front stream (cosl_klt_group_step_dev)
     const int tab = g->stepTab = (g->stepTab + 1) % 3;
     COSL_CUDA(cudaEventSynchronize(g->evStepTab[tab]));
-    KltCam* hstep = g->h_stepCams[tab];
-    for (int c = 0; c < C; ++c) {
-      const int st = op_stages(ops[c]);
-      hstep[c] = g->hcam[c];
-      hstep[c].stages = st;
-      if (!st) {
-        skip.cam[skip.n++] = c;
-        continue;
-      }
-      addr.cam[addr.n++] = c;
-      if (ops[c] == COSL_KLT_OP_TRACK) provide.cam[provide.n++] = c;
-      anyTrack = anyTrack || (st & KLT_STAGE_TRACK);
-      anyDetect = anyDetect || (st & KLT_STAGE_DETECT);
-      lv0[c] = ops[c] != COSL_KLT_OP_NEXT || tracker_reads_level0(g);
-      storeL0 = storeL0 || lv0[c];
-    }
-    const bool flip = skip.n <= addr.n;
-    FramePlan p;
-    p.cams = g->d_stepCams[tab];
-    p.mixed = true;
-    p.tracked = anyTrack;
-    p.wantCorn = anyDetect;
-    p.cornMode = anyDetect ? KLT_CORN_PER_CAM : 0;
-    p.storeL0 = storeL0;
-    p.earlyPrefilter = anyDetect;
-    p.trackerTail = fused_tracker(g);
-    p.foldAdvance = true;
-    if (p.wantCorn) COSL_TRY(next_par(g));
-    int* counters = g->d_counters[g->par];
-    COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), C, g->stream));
-    COSL_TRY(upload_images(g, imgs, pitch, copyKind, ops));
-    g->nxt = g->p1;
-    COSL_TRY(front_waits(g, p.wantCorn, tab));
-    // enqueued after the front stream's waits, which it must not join: the front pass writes the
-    // addressed cameras' slices only
-    if (flip) COSL_TRY(exchange_slices(g, skip, 0));
-    COSL_CUDA(cudaMemcpyAsync(g->d_stepCams[tab], hstep, sizeof(KltCam) * C, cudaMemcpyHostToDevice, g->frontStream));
-    COSL_CUDA(cudaEventRecord(g->evStepTab[tab], g->frontStream));
-    if (p.wantCorn)
-      COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), C, g->frontStream));
-    for (int k = 0; k < addr.n; ++k) g->lv0Stored[g->nxt][addr.cam[k]] = lv0[addr.cam[k]];
-    COSL_TRY(build_pyramid(g, p));
-    COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
-    COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
-    if (anyTrack) {
-      COSL_TRY(run_tracker(g, p));
-      if (!flip) {
-        COSL_TRY(exchange_slices(g, addr, 0));
-      } else {
-        COSL_TRY(fence_pyr(g, g->p0));
-        COSL_TRY(fence_pyr(g, g->p1));
-      }
-      if (!p.trackerTail) {
-        dim3 grid(div_up(g->F, 256), C);
-        COSL_LAUNCH(klt_status<true>, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, p.cams);
-      }
-    }
-    if (provide.n)
-      COSL_LAUNCH(klt_provide_cams, dim3(div_up(g->F, 256), provide.n), 256, 0, g->stream, g->d_res, g->d_dst,
-                  g->d_src, g->F, provide);
-    if (anyDetect) COSL_TRY(run_detector(g, 2, 0, p));
-    if (!anyTrack && !flip) COSL_TRY(exchange_slices(g, addr, 0));
-    COSL_CUDA(cudaEventRecord(g->evStepFence[tab], g->stream));
-    if (flip) std::swap(g->p0, g->p1);
-    g->nxt = g->p1;
+    COSL_TRY(run_frame(g, plan_step(g, ops, tab), imgs, pitch, copyKind));
   }
   std::memcpy(g->stepOps, ops, C);
   g->stepOpsValid = true;
@@ -1224,7 +1219,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   int maxPresent = 0;
   COSL_TRY(upload_present(h, &nPresent, &present3, &maxPresent));
   const uint8_t* imgs[1] = {img};
-  COSL_TRY(run_frame(h, FRAME_DETECT, imgs, pitch, cudaMemcpyHostToDevice, maxPresent, false));
+  COSL_TRY(run_frame(h, plan_frame(h, FRAME_DETECT, maxPresent, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nDetected);
   return COSL_OK;
@@ -1236,7 +1231,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
   if (!img || !dest || !nNewFeatures || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_redetect: bad argument");
   const uint8_t* imgs[1] = {img};
-  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, false));
+  COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nNewFeatures);
   return COSL_OK;
@@ -1248,7 +1243,7 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
   if (!img || !dest || !nPresent || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_track: bad argument");
   const uint8_t* imgs[1] = {img};
-  COSL_TRY(run_frame(h, FRAME_TRACK, imgs, pitch, cudaMemcpyHostToDevice, 0, false));
+  COSL_TRY(run_frame(h, plan_frame(h, FRAME_TRACK, 0, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nullptr);
   *nPresent = h->h_counters[0];
@@ -1295,7 +1290,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
                        const float* const* present3, cosl_klt_feature* const* dest, int* nDetected) {
   int maxPresent = 0;
   if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
-  COSL_TRY(run_frame(h, FRAME_DETECT, imgs, pitch, cudaMemcpyHostToDevice, maxPresent, true));
+  COSL_TRY(run_frame(h, plan_frame(h, FRAME_DETECT, maxPresent, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, nullptr, dest, nDetected);
   return COSL_OK;
@@ -1345,7 +1340,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                         cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
-  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
+  COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
   copy_out(h, h->h_feat, h->h_counters, nullptr, dest, nNew);
   return COSL_OK;
@@ -1355,7 +1350,7 @@ int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pit
   KLT_ENTER(h)
   if (!dimgs || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "group_next_dev: bad argument");
-  return run_frame(h, FRAME_REDETECT, dimgs, pitch, cudaMemcpyDeviceToDevice, 0, true);
+  return run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), dimgs, pitch, cudaMemcpyDeviceToDevice);
 }
 
 // ops[c] in COSL_KLT_OP_*, an image for every addressed camera
@@ -1438,7 +1433,7 @@ int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch)
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_submit: bad argument");
   int slot = 0;
   COSL_TRY(submit_slot(h, "group_submit", &slot));
-  COSL_TRY(run_frame(h, FRAME_REDETECT, imgs, pitch, cudaMemcpyHostToDevice, 0, true));
+  COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), imgs, pitch, cudaMemcpyHostToDevice));
   std::memset(h->opsQ[slot], COSL_KLT_OP_NEXT, h->C);
   return submit_readback(h, slot);
 }

@@ -371,20 +371,6 @@ __device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned l
   asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
-#ifndef KLT_EXP_CLOCK
-#define KLT_EXP_CLOCK 0  // per-section cycle counters written to state[] (experiment builds)
-#endif
-#if KLT_EXP_CLOCK
-#define KLT_CLK(v) const long long v = clock64()
-#else
-#define KLT_CLK(v)
-#endif
-#ifndef KLT_FUSED_THREADS_N
-#define KLT_FUSED_THREADS_N 128
-#endif
-#ifndef KLT_FUSED_MINBLOCKS
-#define KLT_FUSED_MINBLOCKS 4
-#endif
 // Optional tail of the last pass: what klt_status (feature table + live count) and klt_suppress
 // (-1e30 at the pixel of every live track) would do in two more launches.  dest == nullptr: off.
 struct KltTail {
@@ -395,7 +381,8 @@ struct KltTail {
   int pitch, suppress;
 };
 
-constexpr int KLT_FUSED_THREADS = KLT_FUSED_THREADS_N;  // 16 lane groups per CTA
+constexpr int KLT_FUSED_THREADS = 128;  // 16 lane groups per CTA
+constexpr int KLT_FUSED_MINBLOCKS = 4;
 constexpr int KLT_GPB = KLT_FUSED_THREADS / KLT_G;
 
 // X0 of an item of klt_gain_fused.  MIXED: an item of a camera outside the tracker stage reads as a
@@ -444,12 +431,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
   float4 cur0 = make_float4(-1.f, -1.f, -1.f, 0.f);
   int tx0 = 0, ty0 = 0;
 
-#if KLT_EXP_CLOCK
-  long long ck[6] = {0, 0, 0, 0, 0, 0};
-  const long long ckStart = clock64();
-  unsigned long long gt0;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt0));
-#endif
   // The I0 block of every level depends only on X0: all of them are requested into L2 now, so the
   // per-level staging below finds them there (lane gl: row gl of each 8x8 block)
   if (fast && active0 && x00.x >= 0.f) {
@@ -470,7 +451,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
       const bool strict = (it == nIter) && (it != 1);
       const int rd = (pass - 1) & 1, wr = pass & 1;
       for (int own = 0; own < nOwn; ++own) {
-        KLT_CLK(c0);
         const bool staged = fast && (own == 0);
         int item = item0, cam = cam0, wsA = wsA0, wsB = wsB0;
         bool active = active0;
@@ -507,7 +487,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
         const unsigned long long* rb = rec + (size_t)rd * T + (size_t)cam * F + (wsB >= 0 ? wsB : wsA);
         const int need = verBase + pass - 1;
         unsigned long long va = 0, vb = 0;  // version 0 < need for every pass >= 2
-        KLT_CLK(c1k);
         const float beta = cur.z;
         const bool pre_invalid = (cur.x < 0.f) || (x0.x < 0.f);
         const KltCentre c1 = klt_centre(w, h, cur.x, cur.y);
@@ -610,7 +589,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
           __syncwarp();
         }
         // ---- the iteration
-        KLT_CLK(c2k);
         KltAcc A = {0, 0, 0, 0, 0, 0, 0, 0, 0};
         float f = f0;
         const float halfW = 0.5f * (float)Wc, halfH = 0.5f * (float)Hc;
@@ -713,7 +691,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                                        Plax.lambda, Plax.delta);
           }
         }
-        KLT_CLK(c3k);
         if (!staged) f = grp_sum(f);  // warp-uniform branch: staged depends on own only
         // ---- wait for the pass-(p-1) records, get the neighbour gains with the poll itself
         float bn = 1.0f;
@@ -736,7 +713,6 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
           }
           __syncwarp();
         }
-        KLT_CLK(c3p);
         const float nbterm = klt_nbterm(bn, beta, gl, grpBase);
         float4 res = klt_gain_finish(A, f, nbterm, (float)npx, cur.x, cur.y, beta,
                                      klt_finish_params<MIXED>(Plax, Pstrict, strict, Wc, Hc));
@@ -771,30 +747,9 @@ klt_gain_fused(const float4* __restrict__ pyr0, const float4* __restrict__ pyr1,
                              (unsigned long long)__float_as_uint(res.z));
         }
         __syncwarp();
-#if KLT_EXP_CLOCK
-        const long long c4k = clock64();
-        ck[0] += c3p - c3k;
-        ck[1] += c2k - c0;
-        ck[2] += c3k - c2k;
-        ck[3] += c4k - c3p;
-        if (it == 1) ck[4] += c2k - c1k;
-#endif
       }
     }
   }
-#if KLT_EXP_CLOCK
-  if ((threadIdx.x & 31) == 0) {
-    const int wg = (blockIdx.x * KLT_FUSED_THREADS + threadIdx.x) >> 5;
-    unsigned long long gt1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt1));
-    unsigned smid, warpid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    asm volatile("mov.u32 %0, %%warpid;" : "=r"(warpid));
-    state[3 * wg] = make_float4((float)ck[0], (float)ck[1], (float)ck[2], (float)ck[3]);
-    state[3 * wg + 1] = make_float4((float)ck[4], (float)(clock64() - ckStart), __uint_as_float((unsigned)(gt0 & 0xffffffffu)), __uint_as_float((unsigned)(gt1 & 0xffffffffu)));
-    state[3 * wg + 2] = make_float4((float)smid, (float)warpid, (float)blockIdx.x, 0.f);
-  }
-#endif
 }
 
 }  // namespace coslam
