@@ -143,7 +143,10 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
 int cosl_klt_feed(cosl_klt* h, int npts, const float* pts3, int* trackIds, int* nFed);
 /* KLT_SequenceTracker::advanceFrame (v3d_gpuklt.h:252-259). */
 int cosl_klt_advance(cosl_klt* h);
-/* setBorderMargin / setConvergenceThreshold / setSSD_Threshold (v3d_gpuklt.h:217-239). */
+/* setBorderMargin / setConvergenceThreshold / setSSD_Threshold (v3d_gpuklt.h:217-239).  A new value
+ * applies to every frame enqueued after the call, on every path: a frame already submitted with
+ * cosl_klt_group_submit / _submit_step and not yet collected keeps the values it was enqueued with,
+ * and the next submitted frame is the first to use the new one. */
 int cosl_klt_set_margin(cosl_klt* h, float margin);
 int cosl_klt_set_conv(cosl_klt* h, float thr);
 int cosl_klt_set_ssd(cosl_klt* h, float thr);

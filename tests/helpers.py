@@ -1,4 +1,5 @@
 """Shared helpers of the parity tests."""
+import collections
 import os
 import subprocess
 import tempfile
@@ -6,11 +7,55 @@ import tempfile
 import numpy as np
 
 from coslam_b200 import synth
-from coslam_b200.ctypes_defs import KltConfig
+from coslam_b200.ctypes_defs import COSL_KLT_COMPAT_ITER5, KltConfig
 
 
 def live_cfg(gain=True, min_corner=3000.0):
     c = KltConfig.coslam_live(with_gain=gain)
+    c.minCornerness = min_corner
+    return c
+
+
+KltRow = collections.namedtuple("KltRow", "id gain window n_levels level_skip n_iter iter5 fw fh")
+
+# Tracker configurations beyond the live CoSLAM settings, one per code path of the trackers: window
+# half-width 1, 2, 3, 4, 7 and 15, level lists with and without level 0 (levelSkip 0 = nLevels - 1),
+# 1, 2, 5, 7, 8 and 12 iterations, ITER5 on and off, and slot grids whose gain-tracker wait sets
+# overflow (32x4, 4x64, 1x16: the per-pass kernels run) or whose neighbour lookups land exactly on
+# slot boundaries (10x15).  The ref_defaults rows are KLT_SequenceTrackerConfig()'s own defaults.
+KLT_CONFIG_ROWS = [
+    KltRow("ref_defaults", False, 5, 3, 2, 12, True, 32, 32),
+    KltRow("ref_defaults_gain", True, 5, 3, 2, 12, False, 32, 32),
+    KltRow("iter_exact", False, 5, 3, 2, 7, False, 32, 32),
+    KltRow("hw1_every_level", True, 3, 4, 1, 12, False, 20, 12),
+    KltRow("hw4_gain", True, 9, 5, 2, 12, False, 32, 32),
+    KltRow("hw4_2x2", False, 9, 5, 2, 12, False, 32, 32),
+    KltRow("hw7", True, 15, 4, 3, 8, False, 16, 16),
+    KltRow("hw15_gain", True, 31, 3, 2, 5, False, 12, 12),
+    KltRow("hw15_2x2", False, 31, 3, 2, 5, False, 12, 12),
+    KltRow("one_iter", True, 6, 6, 2, 1, False, 32, 32),
+    KltRow("two_iter", True, 6, 6, 2, 2, False, 32, 32),
+    KltRow("top_only", True, 6, 4, 5, 12, False, 32, 32),
+    KltRow("default_skip", True, 6, 5, 0, 12, False, 32, 32),
+    KltRow("single_level_gain", True, 5, 1, 2, 12, False, 32, 32),
+    KltRow("single_level_2x2", False, 5, 1, 2, 12, False, 32, 32),
+    KltRow("wait_set_32x4", True, 6, 6, 2, 12, False, 32, 4),
+    KltRow("wait_set_4x64", True, 6, 6, 2, 12, False, 4, 64),
+    KltRow("wait_set_1x16", True, 6, 6, 2, 12, False, 1, 16),
+    KltRow("texel_tie_10x15", True, 6, 6, 2, 12, False, 10, 15),
+]
+
+
+def row_cfg(row, min_corner):
+    """The KltConfig of a KLT_CONFIG_ROWS row: the reference defaults' thresholds for ref_defaults*,
+    the live CoSLAM thresholds otherwise."""
+    c = KltConfig.reference_defaults() if row.id.startswith("ref_defaults") else KltConfig.coslam_live()
+    c.trackWithGain = int(row.gain)
+    c.windowWidth = row.window
+    c.nLevels = row.n_levels
+    c.levelSkip = row.level_skip
+    c.nIterations = row.n_iter
+    c.compat = COSL_KLT_COMPAT_ITER5 if row.iter5 else 0
     c.minCornerness = min_corner
     return c
 

@@ -2,73 +2,14 @@
 [1 3 3 1] reduction, Shi-Tomasi cornerness, separable non-max suppression), written from the shader
 formulas in float64 with np.pad(mode="edge") for CLAMP_TO_EDGE, against the C++ oracle.  A second
 implementation in another language that agrees with the oracle to fp32 rounding is the strongest
-pin available for the front end: the reference ships no golden vectors (parity unpinned)."""
+pin available for the front end: the reference ships no golden vectors (parity unpinned).  The
+restatement itself is tests/klt_numpy.py; tests/test_oracle_klt_config.py runs it across the
+tracker configurations."""
 import numpy as np
 import pytest
 
 from helpers import live_cfg, seq
-
-
-def _tap_v(a, taps, lo):
-    """out[y] = sum_k taps[k] * a[clamp(y + lo + k)] along axis 0."""
-    n = len(taps)
-    hi = lo + n - 1
-    p = np.pad(a, ((max(0, -lo), max(0, hi)), (0, 0)), mode="edge")
-    off = max(0, -lo)
-    H = a.shape[0]
-    return sum(t * p[off + lo + k: off + lo + k + H] for k, t in enumerate(taps))
-
-
-def _tap_h(a, taps, lo):
-    return _tap_v(a.T, taps, lo).T
-
-
-def level0(img):
-    g = img.astype(np.float64)
-    v = _tap_v(g, [0.25, 0.5, 0.25], -1)                    # pass1v.cg:63-83
-    dv = _tap_v(g, [-0.125, -0.25, 0.0, 0.25, 0.125], -2)
-    I = _tap_h(v, [0.25, 0.5, 0.25], -1)                    # pass1h.cg:96-128
-    Ix = _tap_h(v, [-0.125, -0.25, 0.0, 0.25, 0.125], -2)
-    Iy = _tap_h(dv, [0.25, 0.5, 0.25], -1)
-    return np.stack([I, Ix, Iy], -1)
-
-
-def reduce1331(P):
-    """pass2.cg: rows 2j-1..2j+2 then columns 2i-1..2i+2, weights [1 3 3 1] / 8, size >> 1."""
-    H, W, _ = P.shape
-    h, w = H >> 1, W >> 1
-    out = np.empty((h, w, 3))
-    for c in range(3):
-        a = P[..., c]
-        t = _tap_v(a, [0.125, 0.375, 0.375, 0.125], -1)[0:2 * h:2]      # row 2j: taps 2j-1..2j+2
-        out[..., c] = _tap_h(t, [0.125, 0.375, 0.375, 0.125], -1)[:, 0:2 * w:2]
-    return out
-
-
-def cornerness(P0, min_c, margin, W, H):
-    gx, gy = P0[..., 1], P0[..., 2]
-    box = lambda a: _tap_h(_tap_v(a, [1.0] * 7, -3), [1.0] * 7, -3)     # detector_pass1/2.cg
-    a, b, c = box(gx * gx), box(gx * gy), box(gy * gy)
-    cs = np.maximum(0.5 * (a + c - np.sqrt((a - c) ** 2 + 4 * b * b)) - min_c, 0.0)
-    sx = (np.arange(W) + 0.5) / W
-    sy = (np.arange(H) + 0.5) / H
-    inside = ((sx >= margin / W) & (sx <= 1 - margin / W))[None, :] & \
-             ((sy >= margin / H) & (sy <= 1 - margin / H))[:, None]
-    return np.where(inside, cs, 0.0)
-
-
-def nonmax_survivors(c, r):
-    """klt_detector_nonmax.cg: strictly greatest |.| in the clamped (2r+1)^2 window, ties kill."""
-    H, W = c.shape
-    a = np.abs(c)
-    p = np.pad(a, r, mode="edge")
-    best = np.zeros_like(a)
-    for dy in range(-r, r + 1):
-        for dx in range(-r, r + 1):
-            if dx == 0 and dy == 0:
-                continue
-            best = np.maximum(best, p[r + dy: r + dy + H, r + dx: r + dx + W])
-    return (c > 0) & (a > best)
+from klt_numpy import cornerness, level0, nonmax_survivors, reduce1331, track_2x2, track_gain
 
 
 @pytest.mark.parametrize("W,H,L", [(328, 250, 4), (97, 61, 3)])
@@ -107,112 +48,6 @@ def test_cornerness_and_nonmax_match_numpy_restatement(orc):
     # strongest first
     cs = np.array([got[int(np.floor(py * H)), int(np.floor(px * W))] for px, py in feats["pos"][live]])
     assert np.all(np.diff(cs) <= 0)
-
-
-# --------------------------------------------------------------------------------------------
-# Trackers: Appendix A.3 (sampling), A.4 (2x2 LK) and A.5 (3x3 LK with gain) in float64 numpy,
-# run on the oracle's own pyramids of two frames.
-# --------------------------------------------------------------------------------------------
-def _sample(P, s, t):
-    """Bilinear sample of level array P[h][w][3] at normalised (s, t), clamp-to-edge (A.3)."""
-    h, w, _ = P.shape
-    u = np.clip(s * w - 0.5, -2.0, w + 1.0)
-    v = np.clip(t * h - 0.5, -2.0, h + 1.0)
-    x0 = np.floor(u).astype(int)
-    y0 = np.floor(v).astype(int)
-    ax, ay = (u - x0)[..., None], (v - y0)[..., None]
-    cx0, cx1 = np.clip(x0, 0, w - 1), np.clip(x0 + 1, 0, w - 1)
-    cy0, cy1 = np.clip(y0, 0, h - 1), np.clip(y0 + 1, 0, h - 1)
-    top = P[cy0, cx0] + ax * (P[cy0, cx1] - P[cy0, cx0])
-    bot = P[cy1, cx0] + ax * (P[cy1, cx1] - P[cy1, cx0])
-    return top + ay * (bot - top)
-
-
-def _window(hw):
-    d = np.arange(-hw, hw + 1, dtype=np.float64)
-    dx, dy = np.meshgrid(d, d)
-    return dx.ravel(), dy.ravel()
-
-
-def track_2x2(P0, P1, X0, W, H, levels, n_iter, hw, conv, ssd_thr, margin):
-    """A.4.  P0/P1: dict level -> array; X0: (F, 2) normalised, x < 0 = dead."""
-    dx, dy = _window(hw)
-    out = np.full((len(X0), 3), -1.0)
-    for f, (x0, y0) in enumerate(X0):
-        if x0 < 0:
-            continue
-        x1, y1, invalid = x0, y0, False
-        for lv in levels:
-            sx, sy = (2.0 ** lv) / W, (2.0 ** lv) / H
-            len2 = ssd = 0.0
-            for _ in range(n_iter):
-                a0 = _sample(P0[lv], x0 + dx * sx, y0 + dy * sy)
-                a1 = _sample(P1[lv], x1 + dx * sx, y1 + dy * sy)
-                e = a0[:, 0] - a1[:, 0]
-                jx = (a0[:, 1] + a1[:, 1]) * W / 2
-                jy = (a0[:, 2] + a1[:, 2]) * H / 2
-                a, b, c = (jx * jx).sum(), (jx * jy).sum(), (jy * jy).sum()
-                r0, r1, ssd = (e * jx).sum(), (e * jy).sum(), (e * e).sum()
-                det = a * c - b * b
-                invalid |= det < 1e-5
-                if det == 0:
-                    break
-                ux, uy = (c * r0 - b * r1) / det, (-b * r0 + a * r1) / det
-                x1, y1 = x1 + ux, y1 + uy
-                len2 = (ux * W) ** 2 + (uy * H) ** 2
-            invalid |= (len2 > conv * conv) or (ssd > ssd_thr)
-        invalid |= x1 < margin / W or y1 < margin / H or x1 > 1 - margin / W or y1 > 1 - margin / H
-        if not invalid:
-            out[f] = (x1, y1, x0)
-    return out
-
-
-def track_gain(P0, P1, X0, W, H, fw, fh, levels, n_iter, hw, conv, ssd_thr, margin, lam=1.0, delta=200.0):
-    """A.5: one pass over all slots per (level, iteration); neighbours' gains from the previous pass."""
-    dx, dy = _window(hw)
-    F = fw * fh
-    cur = np.column_stack([X0[:, 0], X0[:, 1], np.ones(F)])      # X1 <- X0, beta <- 1
-    offs = [(1, 1), (-1, -1), (1, 1), (-1, -1), (1, 0), (-1, 0), (0, 1), (0, -1)]  # fw == fh
-    for lv in levels:
-        w, h = W >> lv, H >> lv
-        for it in range(1, n_iter + 1):
-            strict = (it == n_iter) and (it != 1)
-            conv2, ssd_t = (conv * conv, ssd_thr) if strict else (1e6, 1e6)
-            vr = (margin / W, margin / H, 1 - margin / W, 1 - margin / H) if strict else (-1, -1, 2, 2)
-            nxt = np.full((F, 3), -1.0)
-            for f in range(F):
-                x0, y0 = X0[f]
-                x1, y1, beta = cur[f]
-                if x1 < 0 or x0 < 0:
-                    continue
-                sy_, sx_ = divmod(f, fw)
-                nb = 0.0
-                for ox, oy in offs:
-                    g = cur[min(max(sy_ + oy, 0), fh - 1) * fw + min(max(sx_ + ox, 0), fw - 1), 2]
-                    nb += beta if g < 0 else g
-                a0 = _sample(P0[lv], x0 + dx / w, y0 + dy / h)
-                a1 = _sample(P1[lv], x1 + dx / w, y1 + dy / h)
-                e = beta * a0[:, 0] - a1[:, 0]
-                jx = (beta * a0[:, 1] + a1[:, 1]) * W / 2
-                jy = (beta * a0[:, 2] + a1[:, 2]) * H / 2
-                g0 = np.hypot(a0[:, 1], a0[:, 2])
-                g1 = np.hypot(a1[:, 1], a1[:, 2])
-                J = np.stack([jx, jy, -a0[:, 0]])
-                M = J @ J.T
-                M[2, 2] = (a0[:, 0] ** 2 + lam * g0 * g0 + 8 * delta).sum()
-                r = J @ e
-                r[2] = (-e * a0[:, 0] + lam * g0 * (g1 - beta * g0) + delta * (nb - 8 * beta)).sum()
-                det = np.linalg.det(M)
-                if det == 0:
-                    continue
-                u = np.linalg.solve(M, r)
-                x1, y1, nbeta = x1 + u[0], y1 + u[1], beta + u[2]
-                bad = det < 1e-5 or (e * e).sum() > ssd_t or (u[0] * W) ** 2 + (u[1] * H) ** 2 > conv2
-                bad |= x1 < vr[0] or y1 < vr[1] or x1 > vr[2] or y1 > vr[3]
-                if not bad:
-                    nxt[f] = (x1, y1, nbeta)
-            cur = nxt
-    return cur
 
 
 def _two_frames(orc, gain, W=192, H=144, L=4, fw=8, fh=8):
