@@ -57,6 +57,10 @@ def _load():
     L.cosl_klt_group_submit.argtypes = [vp, vp, C.c_size_t]
     L.cosl_klt_group_submit_step.argtypes = [vp, vp, vp, C.c_size_t]
     L.cosl_klt_group_collect.argtypes = [vp, vp, vp]
+    L.cosl_klt_group_prefetch.argtypes = [vp, vp, vp, C.c_size_t]
+    L.cosl_klt_group_run_prefetched.argtypes = [vp, vp, vp]
+    L.cosl_klt_group_submit_prefetched.argtypes = [vp]
+    L.cosl_klt_group_discard_prefetch.argtypes = [vp]
     L.cosl_klt_stream.argtypes = [vp]
     L.cosl_klt_stream.restype = vp
     L.cosl_klt_debug_pyramid.argtypes = [vp, ci, ci, ci, vp, pint, pint]
@@ -240,6 +244,8 @@ class KltGroup:
         self._dest = (C.c_void_p * n_cams)(*[self.feats[c].ctypes.data for c in range(n_cams)])
         # ops of each submitted frame not yet collected, oldest first (None: a submit)
         self._in_flight = collections.deque()
+        # ops of the pending prefetch (None: prefetched without ops, as next / submit)
+        self._prefetched = None
 
     def close(self):
         if getattr(self, "h", None):
@@ -406,6 +412,38 @@ class KltGroup:
         if ops is None:
             return self.feats, self.counts
         return self._step_result(ops)
+
+    def prefetch(self, imgs, ops=None):
+        """cosl_klt_group_prefetch: enqueue the image half (upload, pyramid, cornerness map) of the
+        frame next(imgs) (ops None) or step(ops, imgs) would run, and return.  Feeds and advances may
+        follow; run_prefetched() or submit_prefetched() then runs the rest on the state they leave.
+        The frames must stay untouched until then."""
+        if ops is None:
+            ptrs, pitch = self._imgs(imgs)
+            _ck(LIB.cosl_klt_group_prefetch(self.h, None, ptrs, pitch))
+        else:
+            ops, ptrs, pitch = self._step_args(ops, imgs)
+            _ck(LIB.cosl_klt_group_prefetch(self.h, _ptr(ops), ptrs, pitch))
+        self._prefetched = ops
+
+    def run_prefetched(self):
+        """cosl_klt_group_run_prefetched: what next() (prefetched without ops) or step() returns."""
+        _ck(LIB.cosl_klt_group_run_prefetched(self.h, self._dest, _ptr(self.counts)))
+        ops, self._prefetched = self._prefetched, None
+        if ops is None:
+            return self.feats, self.counts
+        return self._step_result(ops)
+
+    def submit_prefetched(self):
+        """cosl_klt_group_submit_prefetched: enqueue the rest of the prefetched frame as a submitted
+        frame; collect() hands back its tables."""
+        _ck(LIB.cosl_klt_group_submit_prefetched(self.h))
+        self._in_flight.append(self._prefetched)
+        self._prefetched = None
+
+    def discard_prefetch(self):
+        _ck(LIB.cosl_klt_group_discard_prefetch(self.h))
+        self._prefetched = None
 
     def stream(self):
         return LIB.cosl_klt_stream(self.h)

@@ -16,6 +16,49 @@
 
 using namespace coslam;
 
+// Everything that differs between the frames run_frame enqueues: plan_frame decides it for a frame of
+// one kind, plan_step for a step whose cameras have different ops.
+struct FramePlan {
+  const KltCam* cams;   // the camera table the kernels read: the group's, or a step's (stages)
+  bool mixed;           // the kernels' MIXED instantiation runs (reads `cams`)
+  bool tracked;         // the tracker runs (for some camera)
+  int cornMode;         // FrontParams::wantCorn: 0, 1, or KLT_CORN_PER_CAM (a step)
+  bool wantCorn;        // klt_front also produces the detector's cornerness map, and the detector runs
+                        // (for some camera)
+  bool storeL0;         // klt_front stores pyramid level 0
+  bool lv0[64];         // the record of camera c's slice of the buffer the front pass writes (lv0Stored)
+  bool earlyPrefilter;  // the detector's prefilter runs on auxStream right after klt_front
+  bool trackerTail;     // the tracker writes the feature table (klt_status) and, with wantCorn, the
+                        // suppression marks of the live tracks (klt_suppress) itself
+  bool foldAdvance;     // klt_select_refill also writes the provided set to d_src (the advance copy),
+                        // and the frame ends with the pyramid half of the advance
+  int detectMode = 0;   // run_detector's mode
+  int maxPresent = 0;   // detect: the longest present list (upload_present)
+  bool provideAll = false;  // track: the tracked set becomes every camera's feature table (klt_copy_f4)
+  KltCamList provide{};     // a step's TRACK cameras: their tracked sets go to both feature buffers
+  // a step's only (plan_step)
+  const uint8_t* ops = nullptr;  // the cameras with COSL_KLT_OP_SKIP are neither uploaded nor built
+  int tab = -1;                  // its op table: h_stepCams[tab] -> d_stepCams[tab] == cams
+  bool intoP1 = false;           // the front pass writes p1, not the third buffer, and so does the next
+  bool flip = false;             // intoP1: p0 and p1 change roles at the end of the frame
+  KltCamList exchangeEarly{};    // slices of p0 and p1 exchanged ahead of the front pass
+  KltCamList exchangeLate{};     // ... after the tracker, or after the detector when nothing is tracked
+};
+
+// A frame whose image half cosl_klt_group_prefetch has enqueued and whose dependent half has not run
+// (run_frame): what the second half needs of the first.  Until the frame is consumed, the handle's
+// par, nxt, p1 and level-0 records stay those of the last consumed frame, so feeds, advances, fetch
+// and the debug reads in between see the group as if nothing had been prefetched.
+struct KltPrefetch {
+  bool pending = false;
+  FramePlan plan;
+  uint8_t ops[64];            // the frame's ops (all NEXT when none were given); plan.ops points here
+  bool step = false;          // ops were given: the frame is a step, as cosl_klt_group_step runs it
+  bool advanceAfter = false;  // every camera TRACK: advance() follows the frame (run_step)
+  int par = 0;                // the counter set next_par moved the frame to
+  int buf = 0;                // the pyramid buffer its front pass wrote: p1 once consumed
+};
+
 struct cosl_klt {
   cosl_klt_config cfg;
   // W x H: the group's largest geometry (maximum width, maximum height); every buffer slice is laid
@@ -74,7 +117,7 @@ struct cosl_klt {
   // pass writes, p1 itself or, after an advance, the third buffer.  An advance makes p1 the new p0
   // and the old p0 the new p1 (the reference's swap), and points nxt at the third buffer, whose last
   // reader is the tracker of two frames back: so frame n+1's pyramid is built while frame n's tracker
-  // runs.  A front pass writes nxt and then p1 = nxt.
+  // runs.  A front pass writes nxt, and the frame's dependent half then sets p1 = nxt (run_frame).
   float4* d_pyr[3] = {nullptr, nullptr, nullptr};
   int p0 = 0, p1 = 1, nxt = 1;
   // level 0 of camera c's slice of d_pyr[b] holds its frame (see build_pyramid); per camera because
@@ -115,6 +158,7 @@ struct cosl_klt {
   unsigned subSeq = 0;
   int nInFlight = 0;
   bool havePrev = false;
+  KltPrefetch pf;
   // persistent fused gain tracker (klt_gain_fused)
   float4* d_state = nullptr;             // [C*F]
   unsigned long long* d_ver = nullptr;   // [2][C*F] (pass << 32 | beta bits)
@@ -384,6 +428,9 @@ void free_group(cosl_klt* g) {
   if (!g) return;
   cudaSetDevice(g->device);
   if (g->stream) cudaStreamSynchronize(g->stream);
+  // a pending prefetch is not joined into `stream` (cosl_klt_group_prefetch)
+  for (cudaStream_t st : {g->copyStream, g->frontStream, g->auxStream})
+    if (st) cudaStreamSynchronize(st);
   g->timer.destroy();
   cudaFree(g->d_img);
   cudaFree(g->d_cams);
@@ -507,35 +554,6 @@ static bool tracker_reads_level0(const cosl_klt* g) { return (g->L - 1) % g->lev
 // the persistent gain tracker (klt_gain_fused) runs, not the per-pass kernels or the 2x2 tracker
 static bool fused_tracker(const cosl_klt* g) { return g->cfg.trackWithGain && g->fusedOK; }
 
-// Everything that differs between the frames run_frame enqueues: plan_frame decides it for a frame of
-// one kind, plan_step for a step whose cameras have different ops.
-struct FramePlan {
-  const KltCam* cams;   // the camera table the kernels read: the group's, or a step's (stages)
-  bool mixed;           // the kernels' MIXED instantiation runs (reads `cams`)
-  bool tracked;         // the tracker runs (for some camera)
-  int cornMode;         // FrontParams::wantCorn: 0, 1, or KLT_CORN_PER_CAM (a step)
-  bool wantCorn;        // klt_front also produces the detector's cornerness map, and the detector runs
-                        // (for some camera)
-  bool storeL0;         // klt_front stores pyramid level 0
-  bool lv0[64];         // the record of camera c's slice of the buffer the front pass writes (lv0Stored)
-  bool earlyPrefilter;  // the detector's prefilter runs on auxStream right after klt_front
-  bool trackerTail;     // the tracker writes the feature table (klt_status) and, with wantCorn, the
-                        // suppression marks of the live tracks (klt_suppress) itself
-  bool foldAdvance;     // klt_select_refill also writes the provided set to d_src (the advance copy),
-                        // and the frame ends with the pyramid half of the advance
-  int detectMode = 0;   // run_detector's mode
-  int maxPresent = 0;   // detect: the longest present list (upload_present)
-  bool provideAll = false;  // track: the tracked set becomes every camera's feature table (klt_copy_f4)
-  KltCamList provide{};     // a step's TRACK cameras: their tracked sets go to both feature buffers
-  // a step's only (plan_step)
-  const uint8_t* ops = nullptr;  // the cameras with COSL_KLT_OP_SKIP are neither uploaded nor built
-  int tab = -1;                  // its op table: h_stepCams[tab] -> d_stepCams[tab] == cams
-  bool intoP1 = false;           // the front pass writes p1, not the third buffer, and so does the next
-  bool flip = false;             // intoP1: p0 and p1 change roles at the end of the frame
-  KltCamList exchangeEarly{};    // slices of p0 and p1 exchanged ahead of the front pass
-  KltCamList exchangeLate{};     // ... after the tracker, or after the detector when nothing is tracked
-};
-
 // PyramidWithDerivativesCreator::buildPyramidForGrayscaleImage (v3d_gpupyramid.cpp:366-429), on the
 // front stream
 int build_pyramid(cosl_klt* g, const FramePlan& p) {
@@ -604,7 +622,6 @@ int build_pyramid(cosl_klt* g, const FramePlan& p) {
   }
   g->timer.end(st);
   COSL_CUDA(cudaGetLastError());
-  g->p1 = g->nxt;
   return COSL_OK;
 }
 
@@ -965,11 +982,20 @@ static FramePlan plan_step(cosl_klt* g, const uint8_t* ops, int tab) {
   return p;
 }
 
+// The halves of a frame in run_frame.  The image half depends on the frame's images alone: upload,
+// front pass (levels 0 / 1, cornerness map), pyramid tail and early prefilter, on the copy, front and
+// aux streams.  The dependent half reads the feature tables and p0 / p1 as the calls before it left
+// them: tracker, provide, detector and refill on g->stream, which first joins the image half.
+enum FrameHalf { HALF_IMAGES = 1, HALF_DEPENDENT = 2, HALF_BOTH = 3 };
+
 // One frame through its stages, asynchronous on g->stream and, joined into it before the call
 // returns, the front stream (image copies, klt_front, pyramid tail) and auxStream (the early
 // prefilter).  Every entry point that processes a frame, the per-camera steps included, enqueues it
 // here; what differs between frames is decided before, in the plan (plan_frame, plan_step).  imgs,
-// pitch, copyKind: the frame's images (upload_images).  Nothing of the plan outlives the call.
+// pitch, copyKind: the frame's images (upload_images).  Nothing of the plan outlives the call, unless
+// the halves run in two calls (cosl_klt_group_prefetch): then the image half leaves g->par and g->nxt
+// on the set and the buffer it wrote, the caller keeps them with the plan (KltPrefetch) and puts them
+// back before the dependent half.  Run back to back, the halves enqueue exactly the undivided frame.
 //
 // Frame n+1's image copies wait only for frame n's front pass.  Its front pass and pyramid tail wait
 // only for the fences of the buffers they write, each recorded on g->stream behind that buffer's
@@ -991,29 +1017,40 @@ static FramePlan plan_step(cosl_klt* g, const uint8_t* ops, int tab) {
 // after the front stream's waits, which must not wait for it (the front pass writes the other
 // cameras' slices only); exchangeLate takes the place of the tracker's fences, or follows the
 // detector when nothing is tracked.
-int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
-  g->stepOpsValid = false;
-  if (p.wantCorn) COSL_TRY(next_par(g));
-  int* counters = g->d_counters[g->par];
-  // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below
-  COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
-  // the images ahead of the fences: d_img is read by the front passes alone, so they run under the
-  // previous frame's tracker
-  COSL_TRY(upload_images(g, imgs, pitch, copyKind, p.ops));
-  if (p.intoP1) g->nxt = g->p1;
-  COSL_TRY(front_waits(g, p.wantCorn, p.tab));
-  COSL_TRY(exchange_slices(g, p.exchangeEarly, 0));
-  if (p.tab >= 0) {
-    COSL_CUDA(cudaMemcpyAsync(g->d_stepCams[p.tab], g->h_stepCams[p.tab], sizeof(KltCam) * g->C,
-                              cudaMemcpyHostToDevice, g->frontStream));
-    COSL_CUDA(cudaEventRecord(g->evStepTab[p.tab], g->frontStream));
+int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind,
+              int halves = HALF_BOTH) {
+  if (halves & HALF_IMAGES) {
+    if (p.wantCorn) COSL_TRY(next_par(g));
+    int* counters = g->d_counters[g->par];
+    // counters [0..3] of every camera, zeroed first on every kind; [4] on the front stream below.  A
+    // prefetched frame zeroes them at consume: a frame without a cornerness map keeps the last
+    // frame's set, whose counts group_fetch still returns until then
+    if (halves & HALF_DEPENDENT)
+      COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
+    // the images ahead of the fences: d_img is read by the front passes alone, so they run under the
+    // previous frame's tracker
+    COSL_TRY(upload_images(g, imgs, pitch, copyKind, p.ops));
+    if (p.intoP1) g->nxt = g->p1;
+    COSL_TRY(front_waits(g, p.wantCorn, p.tab));
+    COSL_TRY(exchange_slices(g, p.exchangeEarly, 0));
+    if (p.tab >= 0) {
+      COSL_CUDA(cudaMemcpyAsync(g->d_stepCams[p.tab], g->h_stepCams[p.tab], sizeof(KltCam) * g->C,
+                                cudaMemcpyHostToDevice, g->frontStream));
+      COSL_CUDA(cudaEventRecord(g->evStepTab[p.tab], g->frontStream));
+    }
+    if (p.wantCorn)
+      COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
+    COSL_TRY(build_pyramid(g, p));
+    COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
   }
-  if (p.wantCorn)
-    COSL_CUDA(cudaMemset2DAsync(counters + 4, 8 * sizeof(int), 0, sizeof(int), g->C, g->frontStream));
+  if (!(halves & HALF_DEPENDENT)) return COSL_OK;
+  g->stepOpsValid = false;
+  int* counters = g->d_counters[g->par];
+  if (!(halves & HALF_IMAGES))
+    COSL_CUDA(cudaMemset2DAsync(counters, 8 * sizeof(int), 0, 4 * sizeof(int), g->C, g->stream));
   for (int c = 0; c < g->C; ++c)
     if (!p.ops || p.ops[c] != COSL_KLT_OP_SKIP) g->lv0Stored[g->nxt][c] = p.lv0[c];
-  COSL_TRY(build_pyramid(g, p));
-  COSL_CUDA(cudaEventRecord(g->evTail, g->frontStream));
+  g->p1 = g->nxt;
   COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
   if (p.tracked) {
     COSL_TRY(run_tracker(g, p));
@@ -1050,29 +1087,67 @@ int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_
   return COSL_OK;
 }
 
-// One step of cosl_klt_group_step: camera c gets ops[c] followed by advanceFrame, or nothing.
-// Every camera with the same op: the frame of that kind, exactly as group_first / group_next /
-// track + advance run it.  Otherwise one frame with plan_step's plan, on the next op table.
-int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
+// The frame of a step (cosl_klt_group_step): camera c gets ops[c] followed by advanceFrame, or
+// nothing.  Every camera with the same op: the frame of that kind, exactly as group_first /
+// group_next / track + advance run it (*advanceAfter: the advance after track).  Otherwise
+// plan_step's plan, on the next op table.  *any = false: every camera skips, and nothing runs.
+static int plan_ops(cosl_klt* g, const uint8_t* ops, FramePlan* p, bool* advanceAfter, bool* any) {
   const int C = g->C;
   int nOp[4] = {0, 0, 0, 0};
   for (int c = 0; c < C; ++c) ++nOp[ops[c]];
+  *advanceAfter = false;
+  *any = nOp[COSL_KLT_OP_SKIP] < C;
   if (nOp[COSL_KLT_OP_NEXT] == C) {
-    COSL_TRY(run_frame(g, plan_frame(g, FRAME_REDETECT, 0, true), imgs, pitch, copyKind));
+    *p = plan_frame(g, FRAME_REDETECT, 0, true);
   } else if (nOp[COSL_KLT_OP_FIRST] == C) {
-    COSL_TRY(run_frame(g, plan_frame(g, FRAME_DETECT, 0, true), imgs, pitch, copyKind));
+    *p = plan_frame(g, FRAME_DETECT, 0, true);
   } else if (nOp[COSL_KLT_OP_TRACK] == C) {
-    COSL_TRY(run_frame(g, plan_frame(g, FRAME_TRACK, 0, false), imgs, pitch, copyKind));
-    COSL_TRY(advance(g));
-  } else if (nOp[COSL_KLT_OP_SKIP] < C) {
+    *p = plan_frame(g, FRAME_TRACK, 0, false);
+    *advanceAfter = true;
+  } else if (*any) {
     // the pinned table's previous copy was enqueued three steps ago: the host waits here only when
     // it runs more than two steps ahead of the front stream (cosl_klt_group_step_dev)
     const int tab = g->stepTab = (g->stepTab + 1) % 3;
     COSL_CUDA(cudaEventSynchronize(g->evStepTab[tab]));
-    COSL_TRY(run_frame(g, plan_step(g, ops, tab), imgs, pitch, copyKind));
+    *p = plan_step(g, ops, tab);
   }
-  std::memcpy(g->stepOps, ops, C);
+  return COSL_OK;
+}
+
+// One step of cosl_klt_group_step
+int run_step(cosl_klt* g, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch, cudaMemcpyKind copyKind) {
+  FramePlan p;
+  bool advanceAfter = false, any = false;
+  COSL_TRY(plan_ops(g, ops, &p, &advanceAfter, &any));
+  if (any) COSL_TRY(run_frame(g, p, imgs, pitch, copyKind));
+  if (advanceAfter) COSL_TRY(advance(g));
+  std::memcpy(g->stepOps, ops, g->C);
   g->stepOpsValid = true;
+  return COSL_OK;
+}
+
+// The dependent half of the prefetched frame (cosl_klt_group_prefetch), on the feature tables and
+// p0 / p1 the feeds and advances since have left, then what run_step or group_next does after it.
+static int consume_prefetch(cosl_klt* g) {
+  KltPrefetch& f = g->pf;
+  f.pending = false;
+  g->par = f.par;
+  g->nxt = f.buf;
+  COSL_TRY(run_frame(g, f.plan, nullptr, 0, cudaMemcpyHostToDevice, HALF_DEPENDENT));
+  if (f.advanceAfter) COSL_TRY(advance(g));
+  if (f.step) {
+    std::memcpy(g->stepOps, f.ops, g->C);
+    g->stepOpsValid = true;
+  }
+  return COSL_OK;
+}
+
+// Waits on the host for everything a dropped prefetch enqueued: its upload, which still reads the
+// caller's image buffers, and its prefilter on auxStream, which may still write the counter set the
+// next frame moves to.  A discard is rare (a camera restarts), so it need not return early.
+static int drop_prefetch(cosl_klt* g) {
+  g->pf.pending = false;
+  for (cudaStream_t st : {g->copyStream, g->frontStream, g->auxStream}) COSL_CUDA(cudaStreamSynchronize(st));
   return COSL_OK;
 }
 
@@ -1206,6 +1281,11 @@ int cosl_klt_destroy(cosl_klt* h) {
 // cosl_klt_group_create_sizes (camera c's rows are its own width apart)
 static bool pitch_ok(const cosl_klt* g, size_t pitch) { return pitch ? pitch >= (size_t)g->W : g->pitchZeroOK; }
 
+// the calls that process a frame of their own, and set_margin (the margin enters the cornerness map
+// the prefetched front pass already made), wait until a prefetched frame is consumed or discarded
+#define KLT_NOT_PREFETCHED(h, name) \
+  if ((h)->pf.pending) return set_error(COSL_E_STATE, name ": a prefetched frame is pending");
+
 #define KLT_SINGLE(h) \
   KLT_ENTER(h)        \
   if ((h)->C != 1) return set_error(COSL_E_STATE, "single-camera call on a %d-camera group", (h)->C);
@@ -1213,6 +1293,7 @@ static bool pitch_ok(const cosl_klt* g, size_t pitch) { return pitch ? pitch >= 
 int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
                     const float* present3, cosl_klt_feature* dest, int* nDetected) {
   KLT_SINGLE(h)
+  KLT_NOT_PREFETCHED(h, "cosl_klt_detect")
   if (!img || !dest || !nDetected || nPresent < 0 || nPresent > h->F || (nPresent && !present3) ||
       !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_detect: bad argument");
@@ -1228,6 +1309,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
 int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_feature* dest,
                       int* nNewFeatures) {
   KLT_SINGLE(h)
+  KLT_NOT_PREFETCHED(h, "cosl_klt_redetect")
   if (!img || !dest || !nNewFeatures || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_redetect: bad argument");
   const uint8_t* imgs[1] = {img};
@@ -1240,6 +1322,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
 int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_feature* dest,
                    int* nPresent) {
   KLT_SINGLE(h)
+  KLT_NOT_PREFETCHED(h, "cosl_klt_track")
   if (!img || !dest || !nPresent || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "cosl_klt_track: bad argument");
   const uint8_t* imgs[1] = {img};
@@ -1266,6 +1349,7 @@ int cosl_klt_advance(cosl_klt* h) {
 
 int cosl_klt_set_margin(cosl_klt* h, float m) {  // tracker AND detector (v3d_gpuklt.h:217-224)
   KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "cosl_klt_set_margin")
   h->trackMargin = m;
   h->detectMargin = m;
   return update_cameras(h);
@@ -1299,6 +1383,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
 int cosl_klt_group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                          cosl_klt_feature* const* dest, int* nDetected) {
   KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "group_first")
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_first: bad argument");
   return group_first(h, imgs, pitch, nullptr, nullptr, dest, nDetected);
 }
@@ -1308,6 +1393,7 @@ int cosl_klt_group_first_present(cosl_klt* h, const uint8_t* const* imgs, size_t
                                  cosl_klt_feature* const* dest, int* nDetected) {
   KLT_ENTER(h)
   KLT_NOT_IN_FLIGHT(h, "group_first_present")
+  KLT_NOT_PREFETCHED(h, "group_first_present")
   if (!imgs || !pitch_ok(h, pitch) || !nPresent)
     return set_error(COSL_E_INVALID, "group_first_present: bad argument");
   for (int c = 0; c < h->C; ++c)
@@ -1339,6 +1425,7 @@ int cosl_klt_group_advance_cams(cosl_klt* h, const uint8_t* cams) {
 int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
                         cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "group_next")
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
@@ -1348,6 +1435,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
 
 int cosl_klt_group_next_dev(cosl_klt* h, const uint8_t* const* dimgs, size_t pitch) {
   KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "group_next_dev")
   if (!dimgs || !pitch_ok(h, pitch))
     return set_error(COSL_E_INVALID, "group_next_dev: bad argument");
   return run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), dimgs, pitch, cudaMemcpyDeviceToDevice);
@@ -1369,6 +1457,7 @@ int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* i
                         cosl_klt_feature* const* dest, int* n) {
   KLT_ENTER(h)
   KLT_NOT_IN_FLIGHT(h, "group_step")
+  KLT_NOT_PREFETCHED(h, "group_step")
   COSL_TRY(check_step(h, ops, imgs, pitch, "group_step"));
   COSL_TRY(run_step(h, ops, imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
@@ -1379,6 +1468,7 @@ int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* i
 int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* const* dimgs, size_t pitch) {
   KLT_ENTER(h)
   KLT_NOT_IN_FLIGHT(h, "group_step_dev")
+  KLT_NOT_PREFETCHED(h, "group_step_dev")
   COSL_TRY(check_step(h, ops, dimgs, pitch, "group_step_dev"));
   return run_step(h, ops, dimgs, pitch, cudaMemcpyDeviceToDevice);
 }
@@ -1430,6 +1520,7 @@ static int submit_readback(cosl_klt* h, int slot) {
 
 int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch) {
   KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "group_submit")
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_submit: bad argument");
   int slot = 0;
   COSL_TRY(submit_slot(h, "group_submit", &slot));
@@ -1444,6 +1535,7 @@ int cosl_klt_group_submit(cosl_klt* h, const uint8_t* const* imgs, size_t pitch)
 // it pending, and its copy is already enqueued.
 int cosl_klt_group_submit_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch) {
   KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "group_submit_step")
   COSL_TRY(check_step(h, ops, imgs, pitch, "group_submit_step"));
   int slot = 0;
   COSL_TRY(submit_slot(h, "group_submit_step", &slot));
@@ -1462,9 +1554,77 @@ int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew
   return COSL_OK;
 }
 
+// The image half of a frame now, its dependent half later (cosl_klt_group_run_prefetched /
+// _submit_prefetched), with feeds and advances in between.  The front pass writes the third buffer,
+// the one neither p0 nor p1 holds, which no feed or advance touches; an advance only exchanges p0 and
+// p1 (or slices of them).  A step whose ops differ would build into p1 (plan_step); without skipped
+// cameras nothing of p1 needs keeping, so it builds into the third buffer like a frame of one kind.
+int cosl_klt_group_prefetch(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch) {
+  KLT_ENTER(h)
+  KLT_NOT_PREFETCHED(h, "group_prefetch")
+  if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_prefetch: bad argument");
+  for (int c = 0; c < h->C; ++c) {
+    if (ops && (ops[c] == COSL_KLT_OP_SKIP || ops[c] > COSL_KLT_OP_NEXT))
+      return set_error(COSL_E_INVALID, "group_prefetch: op %d of camera %d (SKIP cannot be prefetched)", ops[c], c);
+    if (!imgs[c]) return set_error(COSL_E_INVALID, "group_prefetch: no image for camera %d", c);
+  }
+  KltPrefetch& f = h->pf;
+  f.step = ops != nullptr;
+  if (ops)
+    std::memcpy(f.ops, ops, h->C);
+  else
+    std::memset(f.ops, COSL_KLT_OP_NEXT, h->C);
+  bool any = true;
+  COSL_TRY(plan_ops(h, f.ops, &f.plan, &f.advanceAfter, &any));
+  f.plan.intoP1 = f.plan.flip = false;
+  const int par = h->par, nxt = h->nxt;
+  h->nxt = 3 - h->p0 - h->p1;
+  const int rc = run_frame(h, f.plan, imgs, pitch, cudaMemcpyHostToDevice, HALF_IMAGES);
+  f.par = h->par;
+  f.buf = h->nxt;
+  h->par = par;
+  h->nxt = nxt;
+  if (rc != COSL_OK) {
+    drop_prefetch(h);
+    return rc;
+  }
+  f.pending = true;
+  return COSL_OK;
+}
+
+int cosl_klt_group_run_prefetched(cosl_klt* h, cosl_klt_feature* const* dest, int* n) {
+  KLT_ENTER(h)
+  if (!h->pf.pending) return set_error(COSL_E_STATE, "group_run_prefetched: nothing prefetched");
+  if (h->pf.step) KLT_NOT_IN_FLIGHT(h, "group_run_prefetched")
+  COSL_TRY(consume_prefetch(h));
+  COSL_TRY(fetch_results(h));
+  copy_out(h, h->h_feat, h->h_counters, h->pf.step ? h->pf.ops : nullptr, dest, n);
+  return COSL_OK;
+}
+
+int cosl_klt_group_submit_prefetched(cosl_klt* h) {
+  KLT_ENTER(h)
+  if (!h->pf.pending) return set_error(COSL_E_STATE, "group_submit_prefetched: nothing prefetched");
+  int slot = 0;
+  COSL_TRY(submit_slot(h, "group_submit_prefetched", &slot));
+  COSL_TRY(consume_prefetch(h));
+  std::memcpy(h->opsQ[slot], h->pf.ops, h->C);
+  return submit_readback(h, slot);
+}
+
+int cosl_klt_group_discard_prefetch(cosl_klt* h) {
+  KLT_ENTER(h)
+  if (!h->pf.pending) return set_error(COSL_E_STATE, "group_discard_prefetch: nothing prefetched");
+  return drop_prefetch(h);
+}
+
 int cosl_klt_group_sync(cosl_klt* h) {
   KLT_ENTER(h)
   COSL_CUDA(cudaStreamSynchronize(h->stream));
+  if (h->pf.pending) {
+    COSL_CUDA(cudaStreamSynchronize(h->frontStream));
+    COSL_CUDA(cudaStreamSynchronize(h->auxStream));
+  }
   return COSL_OK;
 }
 

@@ -246,9 +246,51 @@ int cosl_klt_group_submit_step(cosl_klt* h, const uint8_t* ops, const uint8_t* c
  * as cosl_klt_group_step documents it (FIRST: nDetected, TRACK: nPresent, NEXT: nNewFeatures); a
  * skipped camera's entries are left untouched.  COSL_E_STATE when nothing is in flight. */
 int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew);
+/* A frame in two halves, for a loop that maps between frames (CoSLAM::genNewMapPoints feeds new
+ * points to one camera group and advances those cameras, app/SL_CoSLAM.cpp:1368-1371): prefetch
+ * enqueues the half that depends on the images alone -- upload, pyramid, cornerness map, the
+ * detector's prefilter -- and returns without waiting for the device; feeds and advances may follow;
+ * run_prefetched or submit_prefetched then runs the rest (tracker, detector, refill) on the state
+ * they left.  The tables, counts and every later frame are bit for bit those of the synchronous call
+ * made at consume time: cosl_klt_group_next (ops == NULL, NEXT for every camera, as submit) or
+ * cosl_klt_group_step with the same ops.
+ *
+ * ops: FIRST, TRACK or NEXT for each camera, or NULL.  A SKIP op gives COSL_E_INVALID: a step with
+ * skipped cameras builds into the current pyramid, which a feed's advance may still exchange, not
+ * into the third buffer, so it cannot be prefetched.  An image for every camera; imgs and pitch as in
+ * cosl_klt_group_next.  The upload may still read the image buffers after any call returns except
+ * these three: they must stay untouched until run_prefetched returns, until the frame
+ * submit_prefetched enqueued has been collected (as for submit), or until discard_prefetch returns.
+ * Until the prefetch is consumed, group_fetch and the debug reads show the last consumed frame.  At
+ * most one prefetch may be pending (COSL_E_STATE).  While one is, every call that
+ * processes a frame of its own images (first*, next*, track, redetect, detect, step*, submit*) and
+ * cosl_klt_set_margin (the margin enters the cornerness map) give COSL_E_STATE and change nothing;
+ * set_conv / set_ssd act on the tracker, which runs at consume time.  Feeds and advances
+ * (cosl_klt_feed, _advance, cosl_klt_group_feed, _advance_cams) are allowed and do not wait for the
+ * prefetched work; they still refuse while submitted frames are uncollected.  A prefetch may be made
+ * while frames are submitted: the steady state of a loop that maps is
+ *   submit_prefetched(n), prefetch(n+1), collect(n), map + feed + advance, submit_prefetched(n+1). */
+int cosl_klt_group_prefetch(cosl_klt* h, const uint8_t* ops, const uint8_t* const* imgs, size_t pitch);
+/* The dependent half of the pending prefetch, then the read-back: dest / n as group_next (ops ==
+ * NULL) or group_step (and, like group_step, COSL_E_STATE while submitted frames are uncollected)
+ * would write them.  COSL_E_STATE when nothing is prefetched. */
+int cosl_klt_group_run_prefetched(cosl_klt* h, cosl_klt_feature* const* dest, int* n);
+/* The same, enqueued as a submitted frame: it shares the two frames in flight and their order with
+ * submit / submit_step, and cosl_klt_group_collect returns it.  COSL_E_STATE when nothing is
+ * prefetched or two frames are in flight (the prefetch then stays pending). */
+int cosl_klt_group_submit_prefetched(cosl_klt* h);
+/* Drops the pending prefetch (e.g. a camera must restart with FIRST): every later table, pyramid
+ * (cosl_klt_debug_pyramid, its level-0 record), count (cosl_klt_group_fetch) and cornerness map is
+ * as if it had never been made.  It waits on the host for the dropped work, the upload included, so
+ * the image buffers may be reused when it returns; since that work waits for the submitted frames'
+ * trackers that last read its pyramid buffer, a discard may wait for those too.  COSL_E_STATE when
+ * nothing is prefetched.  destroy and cosl_klt_group_sync wait for a pending prefetch. */
+int cosl_klt_group_discard_prefetch(cosl_klt* h);
 /* CUDA stream (cudaStream_t as void*) the group launches on; lets callers time with events.  Parts of
  * a frame run on side streams, but every call joins them into this stream before it returns: work
- * enqueued here after a call sees the whole frame. */
+ * enqueued here after a call sees the whole frame.  The one exception is a pending prefetch: its
+ * image half joins this stream only when it is consumed, so work enqueued here in between (feeds and
+ * advances included) neither waits for it nor is seen by it, and the consumed frame runs after it. */
 void* cosl_klt_stream(cosl_klt* h);
 
 /* Test/inspection hooks (not part of the reference surface). */
