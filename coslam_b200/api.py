@@ -85,6 +85,7 @@ def _load():
     L.cosl_ba_solver_create.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp,
                                         C.POINTER(vp)]
     L.cosl_ba_solver_reset.argtypes = [vp, C.POINTER(BaProblem)]
+    L.cosl_ba_solver_load.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_run.argtypes = [vp, vp]
     L.cosl_ba_solver_run_fixed.argtypes = [vp, ci, vp]
     L.cosl_ba_solver_submit.argtypes = [vp]
@@ -642,6 +643,13 @@ class BaSolver:
             self.prob = prob
             self._s = prob.struct()
         _ck(LIB.cosl_ba_solver_reset(self.h, C.byref(self._s)))
+
+    def load(self, prob):
+        """cosl_ba_solver_load: make `prob` (any shape) the solver's problem without waiting for the device;
+        download() then writes into `prob`."""
+        s = prob.struct()
+        _ck(LIB.cosl_ba_solver_load(self.h, C.byref(s)))
+        self.prob, self._s = prob, s
 
     def run(self):
         info = np.zeros(COSL_BA_INFOSZ)

@@ -9,6 +9,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -17,6 +18,7 @@
 #include <new>
 #include <sched.h>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "ba_ctl.cuh"
@@ -166,13 +168,26 @@ struct cosl_ba_solver {
   int m = 0, n = 0, mcon = 0, ncon = 0, mf = 0, ns = 0;
   long long N = 0, Nc = 0;
   std::vector<double> q0;  // m x 4
-  // device buffers
-  double *d_camK = nullptr, *d_camR0 = nullptr;
+  // device buffers: every allocation is in `cap` (bytes), kept while a loaded problem fits in it
+  std::unordered_map<void*, size_t> cap;
+  // the read-only arrays of the loaded problem, uploaded as one block (load_problem): ptr, cam, xy, camK,
+  // the Schur work items and the solve plan's lists point into d_in
+  unsigned char* d_in = nullptr;
+  const double* d_camK = nullptr;
+  double* d_camR0 = nullptr;
   double *d_pa = nullptr, *d_na = nullptr, *d_dpa = nullptr;
   double *d_pb = nullptr, *d_nb = nullptr, *d_dpb = nullptr;
-  int *d_cam = nullptr, *d_pt = nullptr, *d_cobs = nullptr, *d_ccam = nullptr;
-  double *d_xy = nullptr, *d_wgt = nullptr;
-  long long* d_ptr = nullptr;
+  const int* d_cam = nullptr;
+  int *d_pt = nullptr, *d_cobs = nullptr, *d_ccam = nullptr;
+  const double* d_xy = nullptr;
+  double* d_wgt = nullptr;
+  const long long* d_ptr = nullptr;
+  unsigned *d_hist = nullptr, *d_pcnt = nullptr;  // set-up scratch of the index kernels
+  // pinned staging buffer of the uploads: [R0 | pa | X] (upload_params) then the block of d_in; evStaged
+  // marks the end of the last copy out of it
+  unsigned char* h_stage = nullptr;
+  size_t stageBytes = 0;
+  cudaEvent_t evStaged = nullptr;
   double *d_W = nullptr, *d_V = nullptr, *d_eb = nullptr;
   double* d_Uea = nullptr;   // [U (m x 21) | ea (m x 6)] contiguous for one all-reduce
   // reduced camera system: [rhs (nb*64) | tiles]; the leading part [rhs | Schur-structure tiles]
@@ -182,12 +197,12 @@ struct cosl_ba_solver {
   long long reduceCount = 0;  // doubles in the all-reduce payload
   double *d_Linv = nullptr, *d_y = nullptr, *d_x = nullptr;
   int* d_cnt = nullptr;
-  BaTask* d_tasks = nullptr;
-  BaBwdEntry* d_bwd = nullptr;
-  BaSumEntry* d_sum = nullptr;
+  const BaTask* d_tasks = nullptr;
+  const BaBwdEntry* d_bwd = nullptr;
+  const BaSumEntry* d_sum = nullptr;
   double* d_rhsS = nullptr;
-  int *d_blkRows = nullptr, *d_diagBlk = nullptr,
-      *d_blkCam0 = nullptr, *d_order = nullptr, *d_solIdx = nullptr;
+  const int *d_blkRows = nullptr, *d_diagBlk = nullptr, *d_blkCam0 = nullptr, *d_order = nullptr,
+            *d_solIdx = nullptr;
   BaTileDev td;
   std::vector<BaTask> taskOrder;  // as uploaded: [POTRF / BACKWARD | TRSM / UPDATE / SUM]
   unsigned long long* d_trace = nullptr;
@@ -196,7 +211,7 @@ struct cosl_ba_solver {
   double factorFlops = 0.0;
   double* d_sc = nullptr;
   unsigned char* d_outlier = nullptr;
-  BaPairItem* d_items = nullptr;
+  const BaPairItem* d_items = nullptr;
   double* d_Vinv = nullptr;
   bool costDone = false;         // solve_trial already evaluated the trial cost (ba_finish_cost)
   bool statsPending = false;     // |g|_inf / max diag of the last linearisation still to be computed (prep kernel)
@@ -215,6 +230,7 @@ struct cosl_ba_solver {
   // parameter buffers it was built for, and the events that time and mark one submission
   BaCtl* d_ctl = nullptr;
   cudaGraphExec_t graphExec = nullptr;
+  bool graphStale = false;  // a load changed the problem since the graph was built
   const double *graphPa = nullptr, *graphNa = nullptr, *graphPb = nullptr, *graphNb = nullptr;
   cudaEvent_t evSubmit = nullptr, evDone = nullptr;
   bool inFlight = false;
@@ -392,22 +408,93 @@ int check_observations(const cosl_ba_problem* p) {
   return COSL_OK;
 }
 
+// Library-owned pinned staging buffers: a load copies every array it uploads into one first, so that
+// the uploads are asynchronous whatever memory the caller's arrays live in.  cudaHostAlloc costs
+// milliseconds and cosl_ba_solve creates a solver per call, so released buffers are pooled.
+struct PinnedStaging {
+  std::mutex mu;
+  std::vector<std::pair<unsigned char*, size_t>> free_;
+  // a buffer of at least `bytes`: the largest pooled one, replaced by a new one when it is too small
+  int get(size_t bytes, unsigned char** p, size_t* size) {
+    std::pair<unsigned char*, size_t> b(nullptr, 0);
+    {
+      std::lock_guard<std::mutex> lk(mu);
+      auto it = std::max_element(free_.begin(), free_.end(),
+                                 [](const std::pair<unsigned char*, size_t>& a,
+                                    const std::pair<unsigned char*, size_t>& c) { return a.second < c.second; });
+      if (it != free_.end()) {
+        b = *it;
+        free_.erase(it);
+      }
+    }
+    if (b.first && b.second < bytes) {
+      cudaFreeHost(b.first);
+      b = {nullptr, 0};
+    }
+    if (!b.first) {
+      const size_t sz = std::max<size_t>(bytes + bytes / 4, (size_t)1 << 20);
+      void* q = nullptr;
+      if (cudaHostAlloc(&q, sz, cudaHostAllocPortable) != cudaSuccess)
+        return set_error(COSL_E_NOMEM, "pinned staging buffer of %zu bytes", sz);
+      b = {(unsigned char*)q, sz};
+    }
+    *p = b.first;
+    *size = b.second;
+    return COSL_OK;
+  }
+  void put(unsigned char* p, size_t size) {
+    if (!p) return;
+    std::lock_guard<std::mutex> lk(mu);
+    free_.emplace_back(p, size);
+  }
+};
+static PinnedStaging& pinned_staging() {
+  static PinnedStaging* p = new PinnedStaging();  // never destroyed, as pinned_slots()
+  return *p;
+}
+
+// A device buffer of at least `count` elements: kept while it is large enough, otherwise replaced by a
+// stream-ordered allocation with some headroom.  Neither waits for the device.
+template <typename T>
+int grow(cosl_ba_solver* s, T** p, size_t count) {
+  const size_t bytes = sizeof(T) * std::max<size_t>(count, 1);
+  if (*p) {
+    auto it = s->cap.find((void*)*p);
+    if (it != s->cap.end() && it->second >= bytes) return COSL_OK;
+    s->cap.erase((void*)*p);
+    COSL_CUDA(cudaFreeAsync((void*)*p, s->stream));
+    *p = nullptr;
+  }
+  const size_t want = bytes + bytes / 4;
+  COSL_CUDA(cudaMallocAsync((void**)p, want, s->stream));
+  s->cap[(void*)*p] = want;
+  return COSL_OK;
+}
+
+inline bool multi(const cosl_ba_solver* s) { return s->comm && s->comm->nranks > 1; }
+inline int rank_of(const cosl_ba_solver* s) { return s->comm ? s->comm->rank : 0; }
+
+// R, t, X -> camR0, pa, pb through the parameter part of the staging buffer.  The caller has waited for
+// evStaged (the staging buffer is free) and records it after its own copies.
 int upload_params(cosl_ba_solver* s, const cosl_ba_problem* p) {
   const int m = s->m;
-  std::vector<double> R0((size_t)m * 9), pa((size_t)m * 6, 0.0);
+  double* R0 = reinterpret_cast<double*>(s->h_stage);
+  double* pa = R0 + 9 * (size_t)m;
+  double* X = pa + 6 * (size_t)m;
   s->q0.resize((size_t)m * 4);
   for (int j = 0; j < m; ++j) {
     mat2quat(p->R + 9 * j, &s->q0[4 * j]);
     quat2mat(&s->q0[4 * j], &R0[9 * j]);
-    for (int k = 0; k < 3; ++k) pa[6 * j + 3 + k] = p->t[3 * j + k];
+    for (int k = 0; k < 3; ++k) {
+      pa[6 * j + k] = 0.0;
+      pa[6 * j + 3 + k] = p->t[3 * j + k];
+    }
   }
-  COSL_CUDA(cudaMemcpyAsync(s->d_camR0, R0.data(), sizeof(double) * 9 * m, cudaMemcpyHostToDevice,
-                            s->stream));
-  COSL_CUDA(cudaMemcpyAsync(s->d_pa, pa.data(), sizeof(double) * 6 * m, cudaMemcpyHostToDevice,
-                            s->stream));
-  COSL_CUDA(cudaMemcpyAsync(s->d_pb, p->X, sizeof(double) * 3 * (size_t)s->n,
-                            cudaMemcpyHostToDevice, s->stream));
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  if (s->n) std::memcpy(X, p->X, sizeof(double) * 3 * (size_t)s->n);
+  COSL_CUDA(cudaMemcpyAsync(s->d_camR0, R0, sizeof(double) * 9 * m, cudaMemcpyHostToDevice, s->stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_pa, pa, sizeof(double) * 6 * m, cudaMemcpyHostToDevice, s->stream));
+  if (s->n)
+    COSL_CUDA(cudaMemcpyAsync(s->d_pb, X, sizeof(double) * 3 * (size_t)s->n, cudaMemcpyHostToDevice, s->stream));
   return COSL_OK;
 }
 
@@ -419,16 +506,11 @@ void free_solver(cosl_ba_solver* s) {
   if (s->graphExec) cudaGraphExecDestroy(s->graphExec);
   if (s->evSubmit) cudaEventDestroy(s->evSubmit);
   if (s->evDone) cudaEventDestroy(s->evDone);
-  void* bufs[] = {s->d_camK, s->d_camR0, s->d_pa, s->d_na, s->d_dpa, s->d_pb, s->d_nb, s->d_dpb,
-                  s->d_cam, s->d_pt, s->d_cobs, s->d_ccam, s->d_xy, s->d_wgt, s->d_ptr, s->d_W,
-                  s->d_V, s->d_S, s->d_y, s->d_x, s->d_sc, s->d_outlier,
-                  s->d_items, s->d_entries, s->d_Linv, s->d_cnt, s->d_tasks, s->d_bwd, s->d_blkRows,
-                  s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_solIdx,
-                  s->d_trace, s->d_sum, s->d_rhsS, s->d_Vinv, s->d_ctl};
-  for (void* b : bufs)
-    if (b) cudaFreeAsync(b, s->stream);
+  if (s->evStaged) cudaEventDestroy(s->evStaged);
+  for (const auto& b : s->cap) cudaFreeAsync(b.first, s->stream);
   if (s->stream) cudaStreamSynchronize(s->stream);
   if (s->h_sc) pinned_slots().put(s->h_sc);
+  pinned_staging().put(s->h_stage, s->stageBytes);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
@@ -450,87 +532,107 @@ struct TmpDeviceBufs {
   }
 };
 
-int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
-  TmpDeviceBufs tmp(s->stream);
-  const double tBuild0 = now_s();
-  const int m = p->m, n = p->n, mcon = p->m_con, ncon = p->n_con;
-  const long long N = p->nobs;
-  s->m = m;
-  s->n = n;
-  s->mcon = mcon;
-  s->ncon = ncon;
-  s->mf = m - mcon;
-  s->ns = 6 * s->mf;
-  s->N = N;
-  // host-side index structures (the observation lists were validated by check_observations)
-  std::vector<int> pt((size_t)N), cam((size_t)N);
-  for (int i = 0; i < n; ++i)
-    for (long long o = p->ptr[i]; o < p->ptr[i + 1]; ++o) pt[o] = i;
-  for (long long o = 0; o < N; ++o) cam[o] = p->cam[o];
-  // camera-major list of the free-camera observations
-  std::vector<long long> cptr(m + 1, 0);
-  for (long long o = 0; o < N; ++o)
-    if (cam[o] >= mcon) cptr[cam[o] + 1]++;
-  for (int j = 0; j < m; ++j) cptr[j + 1] += cptr[j];
-  const long long Nc = cptr[m];
-  s->Nc = Nc;
-  std::vector<int> cobs((size_t)Nc), ccam((size_t)Nc);
-  {
-    std::vector<long long> fill(cptr.begin(), cptr.end() - 1);
-    for (long long o = 0; o < N; ++o)
-      if (cam[o] >= mcon) {
-        const long long q = fill[cam[o]]++;
-        cobs[q] = (int)o;
-        ccam[q] = cam[o];
+// The arguments of a problem (cosl_ba_solver_create / _load)
+int check_problem(const cosl_ba_problem* prob, const char* what) {
+  if (!prob) return set_error(COSL_E_INVALID, "%s: null problem", what);
+  if (prob->m < 1 || prob->n < 0 || prob->nobs < 0 || prob->m_con < 0 || prob->m_con > prob->m ||
+      prob->n_con < 0 || prob->n_con > prob->n || !prob->K || !prob->R || !prob->t ||
+      (prob->n && (!prob->X || !prob->ptr)) || (prob->nobs && (!prob->cam || !prob->xy)) ||
+      prob->nobs >= (1ll << 31))
+    return set_error(COSL_E_INVALID, "%s: bad problem", what);
+  if (prob->n && prob->ptr[prob->n] != prob->nobs) return set_error(COSL_E_INVALID, "ptr[n] != nobs");
+  return check_observations(prob);
+}
+
+// What the host derives from the observation lists (validated by check_problem) to plan a problem
+// without a device round trip: the start of each free camera in the camera-major list and the start of
+// each camera-pair bucket (ja <= jb, row-major over mf x mf) in the Schur pair entries.
+struct BaIndex {
+  long long Nc = 0, nEntries = 0;
+  std::vector<unsigned> camStart;  // mf + 1
+  std::vector<unsigned> poff;      // mf * mf + 1
+};
+
+int index_problem(const cosl_ba_problem* p, BaIndex& x) {
+  const int mcon = p->m_con, mf = p->m - p->m_con, n = p->n, ncon = p->n_con;
+  std::vector<long long> perCam((size_t)mf, 0);
+  long long ne = 0;
+  for (int i = 0; i < n; ++i) {
+    long long k = 0;
+    for (long long o = p->ptr[i]; o < p->ptr[i + 1]; ++o)
+      if (p->cam[o] >= mcon) {
+        ++perCam[p->cam[o] - mcon];
+        ++k;
       }
+    // ba_pairs_build: a free point with k free-camera observations gives k (k + 1) / 2 entries
+    if (i >= ncon) ne += k * (k + 1) / 2;
   }
-  if (ba_timing()) std::fprintf(stderr, "[ba timing] observation index lists %.1f ms\n", 1e3 * (now_s() - tBuild0));
-  // camera co-visibility (which pairs of free cameras share a free point) -> plan of the
-  // reduced-system solve (ordering, tiles, task DAG) and the work lists of the Schur contraction.
-  // In the multi-GPU case every rank must derive the SAME structure although it only sees the
-  // pairs of its own point shard: the presence bitmap is all-reduced (max) first.
-  const int mf = s->mf;
-  const double tPair0 = now_s();
-  // the observation index arrays go to the device first: the pair buckets are counted there
-  COSL_TRY(dev_alloc(s->stream, &s->d_cam, (size_t)N));
-  COSL_TRY(dev_alloc(s->stream, &s->d_pt, (size_t)N));
-  COSL_TRY(dev_alloc(s->stream, &s->d_ptr, (size_t)n + 1));
-  COSL_TRY(dev_alloc(s->stream, &s->d_cobs, (size_t)Nc));
-  COSL_TRY(dev_alloc(s->stream, &s->d_ccam, (size_t)Nc));
+  if (ne > INT_MAX)
+    return set_error(COSL_E_INVALID, "%lld Schur pair entries: more than the solver's 32-bit offsets can address", ne);
+  x.nEntries = ne;
+  x.camStart.assign((size_t)mf + 1, 0u);
+  for (int j = 0; j < mf; ++j) x.camStart[j + 1] = x.camStart[j] + (unsigned)perCam[j];
+  x.Nc = x.camStart[mf];
+  // entries per bucket; large problems (the c4 global BA) split the points over a few threads
   const size_t nBuckets = (size_t)mf * mf;
-  unsigned *d_pcnt = nullptr, *d_poff = nullptr;
-  COSL_TRY(tmp.alloc(&d_pcnt, nBuckets + 1));
-  COSL_TRY(tmp.alloc(&d_poff, nBuckets + 1));
-  COSL_CUDA(cudaMemcpyAsync(s->d_cam, cam.data(), sizeof(int) * (size_t)N, cudaMemcpyHostToDevice, s->stream));
-  COSL_CUDA(cudaMemcpyAsync(s->d_pt, pt.data(), sizeof(int) * (size_t)N, cudaMemcpyHostToDevice, s->stream));
-  COSL_CUDA(cudaMemcpyAsync(s->d_ptr, p->ptr, sizeof(long long) * ((size_t)n + 1), cudaMemcpyHostToDevice, s->stream));
-  if (Nc) {
-    COSL_CUDA(cudaMemcpyAsync(s->d_cobs, cobs.data(), sizeof(int) * (size_t)Nc, cudaMemcpyHostToDevice, s->stream));
-    COSL_CUDA(cudaMemcpyAsync(s->d_ccam, ccam.data(), sizeof(int) * (size_t)Nc, cudaMemcpyHostToDevice, s->stream));
+  auto count = [&](int i0, int i1, unsigned* c) {
+    std::vector<int> js;
+    for (int i = i0; i < i1; ++i) {
+      js.clear();
+      for (long long o = p->ptr[i]; o < p->ptr[i + 1]; ++o)
+        if (p->cam[o] >= mcon) js.push_back(p->cam[o] - mcon);
+      for (size_t a = 0; a < js.size(); ++a)
+        for (size_t b = a; b < js.size(); ++b) ++c[(size_t)std::min(js[a], js[b]) * mf + std::max(js[a], js[b])];
+    }
+  };
+  std::vector<unsigned> cnt(nBuckets, 0u);
+  const int T = (int)std::min<long long>({(long long)host_threads(), 1 + ne / (1 << 20), (long long)std::max(1, n - ncon)});
+  if (T <= 1) {
+    count(ncon, n, cnt.data());
+  } else {
+    std::vector<std::vector<unsigned>> part(T);
+    std::vector<std::thread> th;
+    for (int t = 0; t < T; ++t)
+      th.emplace_back([&, t] {
+        part[t].assign(nBuckets, 0u);
+        count(ncon + (int)((long long)(n - ncon) * t / T), ncon + (int)((long long)(n - ncon) * (t + 1) / T),
+              part[t].data());
+      });
+    for (auto& h : th) h.join();
+    th.clear();
+    for (int t = 0; t < T; ++t)
+      th.emplace_back([&, t] {
+        const size_t b0 = nBuckets * t / T, b1 = nBuckets * (t + 1) / T;
+        for (int u = 0; u < T; ++u)
+          for (size_t b = b0; b < b1; ++b) cnt[b] += part[u][b];
+      });
+    for (auto& h : th) h.join();
   }
-  BaDev db;  // just what ba_pairs_build reads
-  std::memset(&db, 0, sizeof(db));
-  db.mcon = mcon;
-  db.ncon = ncon;
-  db.mf = mf;
-  db.Nc = Nc;
-  db.cam = s->d_cam;
-  db.pt = s->d_pt;
-  db.ptr = s->d_ptr;
-  db.cobs = s->d_cobs;
-  std::vector<unsigned> poff(nBuckets + 1, 0u);
-  COSL_CUDA(cudaMemsetAsync(d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->stream));
-  if (Nc && mf) {
-    COSL_LAUNCH(ba_pairs_build<false>, (unsigned)div_up64(Nc, 256), 256, 0, s->stream, db, d_pcnt, d_poff, nullptr);
-    COSL_LAUNCH(ba_scan_u32, 1, 1024, 0, s->stream, d_pcnt, d_poff, (long long)nBuckets);
-    COSL_CUDA(cudaMemcpyAsync(poff.data(), d_poff, sizeof(unsigned) * (nBuckets + 1), cudaMemcpyDeviceToHost, s->stream));
-  }
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  x.poff.assign(nBuckets + 1, 0u);
+  for (size_t b = 0; b < nBuckets; ++b) x.poff[b + 1] = x.poff[b] + cnt[b];
+  return COSL_OK;
+}
+
+// Replace the solver's problem with `p` (validated by check_problem, indexed by index_problem).  The
+// host plans the reduced-system solve and the Schur work items from the bucket counts, copies everything
+// the device needs into the staging buffer and enqueues the rest on the solver's stream: the upload, the
+// observation index kernels (ba_index_*) and the pair entries (ba_pairs_build).  Waits for nothing on the
+// device except, for a multi-rank solver, the all-reduce of the co-visibility bitmap.
+int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) {
+  const double tLoad0 = now_s();
+  const int m = p->m, n = p->n, mcon = p->m_con, ncon = p->n_con, mf = m - mcon;
+  const long long N = p->nobs, Nc = x.Nc, nEntries = x.nEntries;
+  const size_t nBuckets = (size_t)mf * mf;
+  // camera co-visibility (which pairs of free cameras share a free point) -> plan of the reduced-system
+  // solve (ordering, tiles, task DAG) and the work lists of the Schur contraction.  In the multi-GPU case
+  // every rank must derive the SAME structure although it only sees the pairs of its own point shard:
+  // the presence bitmap is all-reduced (max) first.
   std::vector<uint8_t> adj(nBuckets, 0);
   for (int ja = 0; ja < mf; ++ja)
     for (int jb = ja; jb < mf; ++jb)
-      if (poff[(size_t)ja * mf + jb + 1] > poff[(size_t)ja * mf + jb]) adj[(size_t)ja * mf + jb] = adj[(size_t)jb * mf + ja] = 1;
-  if (s->comm && s->comm->nranks > 1 && mf > 0) {
+      if (x.poff[(size_t)ja * mf + jb + 1] > x.poff[(size_t)ja * mf + jb]) adj[(size_t)ja * mf + jb] = adj[(size_t)jb * mf + ja] = 1;
+  if (multi(s) && mf > 0) {
+    TmpDeviceBufs tmp(s->stream);
     uint8_t* d_adj = nullptr;
     COSL_TRY(tmp.alloc(&d_adj, adj.size()));
     COSL_CUDA(cudaMemcpyAsync(d_adj, adj.data(), adj.size(), cudaMemcpyHostToDevice, s->stream));
@@ -539,13 +641,10 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     COSL_CUDA(cudaMemcpyAsync(adj.data(), d_adj, adj.size(), cudaMemcpyDeviceToHost, s->stream));
     COSL_CUDA(cudaStreamSynchronize(s->stream));
   }
-  {
-    const double tPlan0 = now_s();
-    s->plan = ba_make_plan(mf, adj);
-    if (ba_timing()) std::fprintf(stderr, "[ba timing] plan %.1f ms\n", 1e3 * (now_s() - tPlan0));
-    if (s->plan.nb < 0) return set_error(COSL_E_INVALID, "solve plan: dependency cycle (internal error)");
-  }
-  const BaPlan& P = s->plan;
+  const double tPlan0 = now_s();
+  BaPlan P = ba_make_plan(mf, adj);
+  if (ba_timing()) std::fprintf(stderr, "[ba timing] plan %.1f ms\n", 1e3 * (now_s() - tPlan0));
+  if (P.nb < 0) return set_error(COSL_E_INVALID, "solve plan: dependency cycle (internal error)");
   // destination of the 6x6 block of camera pair (ja <= jb) in the tile storage: the lower
   // triangle of the permuted system, i.e. the later camera (block, offset) gives the row
   auto pair_dst = [&](int ja, int jb, int& dst, int& rOff, int& cOff, int& trans) {
@@ -559,17 +658,16 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     rOff = bLater ? oB : oA;
     return true;
   };
-  // pair lists: one bucket per camera pair (offsets counted on the device above); a work item is
-  // a run of <= 512 entries of one bucket; the entries themselves are placed by ba_pairs_build.
-  // Fewer entries per item when the problem is small (local BA: a few dozen camera pairs with
-  // thousands of entries each), so that the grid still fills the GPU; ba_schur_pairs_st works in
-  // batches of 32 entries and sums 32 lanes per item: multiples of 32, >= 128
+  // pair lists: one bucket per camera pair; a work item is a run of <= 512 entries of one bucket; the
+  // entries themselves are placed by ba_pairs_build.  Fewer entries per item when the problem is small
+  // (local BA: a few dozen camera pairs with thousands of entries each), so that the grid still fills
+  // the GPU; ba_schur_pairs_st works in batches of 32 entries and sums 32 lanes per item: multiples of
+  // 32, >= 128
   std::vector<BaPairItem> items;
-  const long long nEntries = poff[nBuckets];
   const int chunk = (int)(32 * std::max<long long>(4, std::min<long long>(16, nEntries / (4096 * 32))));
   for (int ja = 0; ja < mf; ++ja)
     for (int jb = ja; jb < mf; ++jb) {
-      const long long b0 = poff[(size_t)ja * mf + jb], b1 = poff[(size_t)ja * mf + jb + 1];
+      const long long b0 = x.poff[(size_t)ja * mf + jb], b1 = x.poff[(size_t)ja * mf + jb + 1];
       if (b1 == b0) continue;
       BaPairItem it;
       std::memset(&it, 0, sizeof(it));
@@ -584,15 +682,12 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
         items.push_back(it);
       }
     }
-  COSL_TRY(dev_alloc(s->stream, &s->d_entries, (size_t)nEntries));
-  COSL_CUDA(cudaMemsetAsync(d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->stream));
-  if (nEntries)
-    COSL_LAUNCH(ba_pairs_build<true>, (unsigned)div_up64(Nc, 256), 256, 0, s->stream, db, d_pcnt, d_poff, s->d_entries);
-  s->nEntries = nEntries;
-  s->nItems = (int)items.size();
-  if (ba_timing())
-    std::fprintf(stderr, "[ba timing] co-visibility + Schur work lists %.1f ms (%lld pair entries, %d threads)\n",
-                 1e3 * (now_s() - tPair0), nEntries, host_threads());
+  std::vector<BaTask> taskOrder;
+  const int nA = tile_task_order(P, taskOrder);
+  const int nb = std::max(1, P.nb), nTiles = std::max(1, P.nTiles);
+  std::vector<int> h_diagBlk(nTiles, -1), h_solIdx(std::max(1, mf), 0);
+  for (int k = 0; k < P.nb; ++k) h_diagBlk[P.tileIdx[(size_t)k * P.nb + k]] = k;
+  for (int j = 0; j < mf; ++j) h_solIdx[j] = P.camBlk[j] * BA_TB + P.camOff[j];
   // intrinsics: only K0,K1,K2,K4,K5 are used (as BundleRTS packs them, app/SL_CoSLAMBA.cpp:337-343)
   std::vector<double> camK((size_t)m * 5);
   for (int j = 0; j < m; ++j) {
@@ -603,78 +698,129 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
     camK[5 * j + 3] = K[4];
     camK[5 * j + 4] = K[5];
   }
-  // device allocations
-  COSL_TRY(dev_alloc(s->stream, &s->d_camK, (size_t)m * 5));
-  COSL_TRY(dev_alloc(s->stream, &s->d_camR0, (size_t)m * 9));
-  COSL_TRY(dev_alloc(s->stream, &s->d_pa, (size_t)m * 6));
-  COSL_TRY(dev_alloc(s->stream, &s->d_na, (size_t)m * 6));
-  COSL_TRY(dev_alloc(s->stream, &s->d_dpa, (size_t)m * 6));
-  COSL_TRY(dev_alloc(s->stream, &s->d_pb, (size_t)n * 3));
-  COSL_TRY(dev_alloc(s->stream, &s->d_nb, (size_t)n * 3));
-  COSL_TRY(dev_alloc(s->stream, &s->d_dpb, (size_t)n * 3));
-  COSL_TRY(dev_alloc(s->stream, &s->d_xy, (size_t)N * 2));
-  COSL_TRY(dev_alloc(s->stream, &s->d_wgt, (size_t)N));
-  COSL_TRY(dev_alloc(s->stream, &s->d_W, (size_t)N * 18));
+  // the block of read-only arrays that becomes d_in: sections of whole 256-byte lines
+  struct Sec {
+    const void* src;
+    size_t bytes, off;
+  };
+  std::vector<Sec> secs;
+  size_t inBytes = 0;
+  auto sec = [&](const void* src, size_t bytes) {
+    secs.push_back({src, bytes, inBytes});
+    inBytes += std::max<size_t>(256, (bytes + 255) & ~(size_t)255);
+    return secs.back().off;
+  };
+  const long long zeroPtr = 0;
+  const size_t oPtr = sec(n ? (const void*)p->ptr : (const void*)&zeroPtr, sizeof(long long) * ((size_t)n + 1));
+  const size_t oCam = sec(p->cam, sizeof(int) * (size_t)N);
+  const size_t oXy = sec(p->xy, sizeof(double) * 2 * (size_t)N);
+  const size_t oK = sec(camK.data(), sizeof(double) * camK.size());
+  const size_t oItems = sec(items.data(), sizeof(BaPairItem) * items.size());
+  const size_t oTasks = sec(taskOrder.data(), sizeof(BaTask) * taskOrder.size());
+  const size_t oBwd = sec(P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
+  const size_t oSum = sec(P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
+  const size_t oBlkRows = sec(P.blkRows.data(), sizeof(int) * P.nb);
+  const size_t oBlkCam0 = sec(P.blkCam0.data(), P.nb ? sizeof(int) * (P.nb + 1) : 0);
+  const size_t oOrder = sec(P.order.data(), P.nb ? sizeof(int) * mf : 0);
+  const size_t oDiag = sec(h_diagBlk.data(), sizeof(int) * h_diagBlk.size());
+  const size_t oSol = sec(h_solIdx.data(), sizeof(int) * h_solIdx.size());
+  const size_t oCamStart = sec(x.camStart.data(), sizeof(unsigned) * x.camStart.size());
+  const size_t oPoff = sec(x.poff.data(), sizeof(unsigned) * x.poff.size());
+  const size_t parBytes = (sizeof(double) * (15 * (size_t)m + 3 * (size_t)n) + 255) & ~(size_t)255;
+  // the staging buffer is free once the last copy out of it has run (at once, unless a load was
+  // enqueued behind other work and is loaded over right away)
+  if (s->evStaged) COSL_CUDA(cudaEventSynchronize(s->evStaged));
+  if (parBytes + inBytes > s->stageBytes) {
+    pinned_staging().put(s->h_stage, s->stageBytes);
+    s->h_stage = nullptr;
+    s->stageBytes = 0;
+    COSL_TRY(pinned_staging().get(parBytes + inBytes, &s->h_stage, &s->stageBytes));
+  }
+  for (const Sec& q : secs)
+    if (q.bytes) std::memcpy(s->h_stage + parBytes + q.off, q.src, q.bytes);
+  // from here on the handle holds the new problem
+  s->m = m;
+  s->n = n;
+  s->mcon = mcon;
+  s->ncon = ncon;
+  s->mf = mf;
+  s->ns = 6 * mf;
+  s->N = N;
+  s->Nc = Nc;
+  s->nEntries = nEntries;
+  s->nItems = (int)items.size();
+  s->plan = std::move(P);
+  s->taskOrder = std::move(taskOrder);
+  const BaPlan& PL = s->plan;
+  s->reduceCount = (long long)nb * BA_TB + (long long)PL.nTilesOrig * BA_TILE;
+  s->factorFlops = PL.flops;
+  s->graphStale = true;
+  COSL_TRY(grow(s, &s->d_in, inBytes));
+  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_stage + parBytes, inBytes, cudaMemcpyHostToDevice, s->stream));
+  s->d_ptr = reinterpret_cast<const long long*>(s->d_in + oPtr);
+  s->d_cam = reinterpret_cast<const int*>(s->d_in + oCam);
+  s->d_xy = reinterpret_cast<const double*>(s->d_in + oXy);
+  s->d_camK = reinterpret_cast<const double*>(s->d_in + oK);
+  s->d_items = reinterpret_cast<const BaPairItem*>(s->d_in + oItems);
+  s->d_tasks = reinterpret_cast<const BaTask*>(s->d_in + oTasks);
+  s->d_bwd = reinterpret_cast<const BaBwdEntry*>(s->d_in + oBwd);
+  s->d_sum = reinterpret_cast<const BaSumEntry*>(s->d_in + oSum);
+  s->d_blkRows = reinterpret_cast<const int*>(s->d_in + oBlkRows);
+  s->d_blkCam0 = reinterpret_cast<const int*>(s->d_in + oBlkCam0);
+  s->d_order = reinterpret_cast<const int*>(s->d_in + oOrder);
+  s->d_diagBlk = reinterpret_cast<const int*>(s->d_in + oDiag);
+  s->d_solIdx = reinterpret_cast<const int*>(s->d_in + oSol);
+  const unsigned* d_camStart = reinterpret_cast<const unsigned*>(s->d_in + oCamStart);
+  const unsigned* d_poff = reinterpret_cast<const unsigned*>(s->d_in + oPoff);
+  // the buffers the solver writes
+  COSL_TRY(grow(s, &s->d_camR0, (size_t)m * 9));
+  COSL_TRY(grow(s, &s->d_pa, (size_t)m * 6));
+  COSL_TRY(grow(s, &s->d_na, (size_t)m * 6));
+  COSL_TRY(grow(s, &s->d_dpa, (size_t)m * 6));
+  COSL_TRY(grow(s, &s->d_pb, (size_t)n * 3));
+  COSL_TRY(grow(s, &s->d_nb, (size_t)n * 3));
+  COSL_TRY(grow(s, &s->d_dpb, (size_t)n * 3));
+  COSL_TRY(grow(s, &s->d_pt, (size_t)N));
+  COSL_TRY(grow(s, &s->d_cobs, (size_t)Nc));
+  COSL_TRY(grow(s, &s->d_ccam, (size_t)Nc));
+  COSL_TRY(grow(s, &s->d_wgt, (size_t)N));
+  COSL_TRY(grow(s, &s->d_W, (size_t)N * 18));
   // [V (n x 6) | e_b (n x 3) | U (m x 21) | e_a (m x 6)] in one slab: one memset per linearisation
-  COSL_TRY(dev_alloc(s->stream, &s->d_V, (size_t)n * 9 + (size_t)m * 27));
+  COSL_TRY(grow(s, &s->d_V, (size_t)n * 9 + (size_t)m * 27));
   s->d_eb = s->d_V + (size_t)n * 6;
   s->d_Uea = s->d_eb + (size_t)n * 3;
-  const double tAlloc0 = now_s();
-  const int nb = std::max(1, P.nb), nTiles = std::max(1, P.nTiles);
   const size_t rhsLen = (size_t)nb * BA_TB;
-  s->reduceCount = (long long)rhsLen + (long long)P.nTilesOrig * BA_TILE;
-  s->factorFlops = P.flops;
-  COSL_TRY(dev_alloc(s->stream, &s->d_S, rhsLen + ((size_t)nTiles + P.nScratch) * BA_TILE));
-  COSL_TRY(dev_alloc(s->stream, &s->d_rhsS, (size_t)std::max(1, P.nScratch) * BA_TB));
-  COSL_TRY(dev_alloc(s->stream, &s->d_sum, P.sumList.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_Linv, (size_t)nb * BA_TILE));
-  COSL_TRY(dev_alloc(s->stream, &s->d_y, rhsLen));
-  COSL_TRY(dev_alloc(s->stream, &s->d_x, rhsLen));
-  COSL_TRY(dev_alloc(s->stream, &s->d_cnt, (size_t)P.nCounters + 2 + P.tasks.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_tasks, P.tasks.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_bwd, P.bwdList.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_blkRows, (size_t)nb));
-  COSL_TRY(dev_alloc(s->stream, &s->d_diagBlk, (size_t)nTiles));
-  COSL_TRY(dev_alloc(s->stream, &s->d_blkCam0, (size_t)nb + 1));
-  COSL_TRY(dev_alloc(s->stream, &s->d_order, (size_t)std::max(1, mf)));
-  COSL_TRY(dev_alloc(s->stream, &s->d_solIdx, (size_t)std::max(1, mf)));
-  std::vector<int> h_diagBlk(nTiles, -1), h_solIdx(std::max(1, mf), 0);
-  for (int k = 0; k < P.nb; ++k) h_diagBlk[P.tileIdx[(size_t)k * P.nb + k]] = k;
-  for (int j = 0; j < mf; ++j) h_solIdx[j] = P.camBlk[j] * BA_TB + P.camOff[j];
-  COSL_TRY(dev_alloc(s->stream, &s->d_sc, (size_t)SC_NTOT));
-  COSL_TRY(dev_alloc(s->stream, &s->d_outlier, (size_t)N));
-  COSL_TRY(dev_alloc(s->stream, &s->d_items, items.size()));
-  COSL_TRY(dev_alloc(s->stream, &s->d_Vinv, (size_t)n * 6));
-  static_assert(SC_NTOT <= 16, "pinned slot size");
-  s->h_sc = pinned_slots().get();
-  if (!s->h_sc) return set_error(COSL_E_NOMEM, "pinned host allocation failed");
-  *reinterpret_cast<volatile unsigned long long*>(s->h_sc + SC_NTOT) = 0;  // a pooled slot keeps its last flag
-  s->scSeq = 0;
-#define UP(dst, src, bytes) \
-  COSL_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s->stream))
-  UP(s->d_camK, camK.data(), sizeof(double) * 5 * m);
-  UP(s->d_xy, p->xy, sizeof(double) * 2 * (size_t)N);
-  if (!items.empty()) UP(s->d_items, items.data(), sizeof(BaPairItem) * items.size());
-  const int nA = tile_task_order(P, s->taskOrder);
-  if (!s->taskOrder.empty()) UP(s->d_tasks, s->taskOrder.data(), sizeof(BaTask) * s->taskOrder.size());
-  if (!P.bwdList.empty()) UP(s->d_bwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
-  if (!P.sumList.empty()) UP(s->d_sum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
-  if (P.nb) {
-    UP(s->d_blkRows, P.blkRows.data(), sizeof(int) * P.nb);
-    UP(s->d_blkCam0, P.blkCam0.data(), sizeof(int) * (P.nb + 1));
-    UP(s->d_order, P.order.data(), sizeof(int) * mf);
+  COSL_TRY(grow(s, &s->d_S, rhsLen + ((size_t)nTiles + PL.nScratch) * BA_TILE));
+  COSL_TRY(grow(s, &s->d_rhsS, (size_t)std::max(1, PL.nScratch) * BA_TB));
+  COSL_TRY(grow(s, &s->d_Linv, (size_t)nb * BA_TILE));
+  COSL_TRY(grow(s, &s->d_y, rhsLen));
+  COSL_TRY(grow(s, &s->d_x, rhsLen));
+  COSL_TRY(grow(s, &s->d_cnt, (size_t)PL.nCounters + 2 + PL.tasks.size()));
+  COSL_TRY(grow(s, &s->d_outlier, (size_t)N));
+  COSL_TRY(grow(s, &s->d_Vinv, (size_t)n * 6));
+  COSL_TRY(grow(s, &s->d_entries, (size_t)nEntries));
+  COSL_TRY(upload_params(s, p));
+  COSL_CUDA(cudaEventRecord(s->evStaged, s->stream));
+  // observation index lists and Schur pair entries
+  if (n) COSL_LAUNCH(ba_index_points, div_up(n, 256), 256, 0, s->stream, s->d_ptr, n, s->d_pt);
+  if (Nc) {
+    const int chunk = (int)std::max<long long>(256, 32 * div_up64(div_up64(N, 256), 32));
+    const int nChunks = (int)div_up64(N, chunk);
+    COSL_TRY(grow(s, &s->d_hist, (size_t)nChunks * mf));
+    COSL_CUDA(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * (size_t)nChunks * mf, s->stream));
+    const unsigned gW = (unsigned)div_up64(32LL * nChunks, 256);
+    COSL_LAUNCH(ba_index_cams<false>, gW, 256, 0, s->stream, s->d_cam, N, mcon, mf, chunk, s->d_hist, s->d_cobs,
+                s->d_ccam);
+    COSL_LAUNCH(ba_index_cam_base, div_up(mf, 256), 256, 0, s->stream, s->d_hist, nChunks, mf, d_camStart);
+    COSL_LAUNCH(ba_index_cams<true>, gW, 256, 0, s->stream, s->d_cam, N, mcon, mf, chunk, s->d_hist, s->d_cobs,
+                s->d_ccam);
   }
-  UP(s->d_diagBlk, h_diagBlk.data(), sizeof(int) * nTiles);
-  UP(s->d_solIdx, h_solIdx.data(), sizeof(int) * std::max(1, mf));
-#undef UP
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
-  if (ba_timing()) std::fprintf(stderr, "[ba timing] allocations + uploads %.1f ms\n", 1e3 * (now_s() - tAlloc0));
   BaDev& d = s->d;
   d.m = m;
   d.n = n;
   d.mcon = mcon;
   d.ncon = ncon;
-  d.mf = s->mf;
+  d.mf = mf;
   d.ns = s->ns;
   d.N = N;
   d.Nc = Nc;
@@ -696,6 +842,13 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   d.tiles = s->d_S + rhsLen;
   d.solIdx = s->d_solIdx;
   d.sc = s->d_sc;
+  if (nEntries) {
+    COSL_TRY(grow(s, &s->d_pcnt, nBuckets + 1));
+    COSL_CUDA(cudaMemsetAsync(s->d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->stream));
+    COSL_LAUNCH(ba_pairs_build<true>, (unsigned)div_up64(Nc, 256), 256, 0, s->stream, d, s->d_pcnt, d_poff,
+                s->d_entries);
+  }
+  COSL_CUDA(cudaGetLastError());
   BaTileDev& td = s->td;
   td.rhs = d.rhs;
   td.tiles = d.tiles;
@@ -707,54 +860,80 @@ int build_solver(cosl_ba_solver* s, const cosl_ba_problem* p) {
   td.bwd = s->d_bwd;
   td.sum = s->d_sum;
   td.rhsS = s->d_rhsS;
-  td.xdoneBase = P.nTiles + P.nScratch;
+  td.xdoneBase = PL.nTiles + PL.nScratch;
   td.blkRows = s->d_blkRows;
-  td.nTasks = (int)P.tasks.size();
+  td.nTasks = (int)PL.tasks.size();
   td.nA = nA;
-  td.nb = P.nb;
-  td.nTiles = P.nTiles;
-  td.nCounters = P.nCounters;
+  td.nb = PL.nb;
+  td.nTiles = PL.nTiles;
+  td.nCounters = PL.nCounters;
   td.sc = s->d_sc;
   td.scFail = (int)SC_FAIL;
   td.trace = nullptr;
   // Systems of one or two blocks (local BA) are solved by one resident CTA: for the 72 x 72 system of
   // the c3 local BA, ba_tile_two needs 26 us per LM trial and the task kernel 42 us (H100 80GB HBM3, 400 W).
-  if (P.nb >= 1 && P.nb <= 2) {
+  s->twoSolve = false;
+  s->two00 = s->two10 = s->two11 = -1;
+  if (PL.nb >= 1 && PL.nb <= 2) {
     s->twoSolve = true;
-    s->two00 = P.tileIdx[0];
-    s->two10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
-    s->two11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
-    if (s->two00 < 0 || (P.nb == 2 && s->two11 < 0)) s->twoSolve = false;
+    s->two00 = PL.tileIdx[0];
+    s->two10 = PL.nb == 2 ? PL.tileIdx[(size_t)1 * PL.nb + 0] : -1;
+    s->two11 = PL.nb == 2 ? PL.tileIdx[(size_t)1 * PL.nb + 1] : -1;
+    if (s->two00 < 0 || (PL.nb == 2 && s->two11 < 0)) s->twoSolve = false;
   }
-  COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 BA_TILE_SMEM));
-  COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
-  COSL_CUDA(cudaFuncSetAttribute(ba_schur_pairs_st, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_ST_SMEM));
   {
     // persistent grid: never more CTAs than can be co-resident (the ticket scheduler spins)
-    int nsm = 0, perSm = 0;
-    COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, s->device));
-    s->numSM = std::max(1, nsm);
-    COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS,
-                                                            BA_TILE_SMEM));
-    const int grid = nsm * std::max(1, std::min(perSm, 1));
+    int perSm = 0;
+    COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS, BA_TILE_SMEM));
+    const int grid = s->numSM * std::max(1, std::min(perSm, 1));
     s->solveGrid = std::max(2, std::min(grid, td.nTasks + 1));
     // CTAs that only ever run the diagonal-block tasks (see BaTileDev::nSpecial)
     const int nsp = std::min(24, std::max(1, s->solveGrid / 6));
     td.nSpecial = std::max(1, std::min(nsp, s->solveGrid - 1));
   }
+  if (ba_timing())
+    std::fprintf(stderr, "[ba timing] load: host %.2f ms (%lld pair entries, %d items)\n", 1e3 * (now_s() - tLoad0),
+                 nEntries, s->nItems);
+  return COSL_OK;
+}
+
+// A solver handle without a problem: stream, scalar slots, the kernel attributes of the solve
+int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver** out) {
+  cosl_ba_solver* s = new (std::nothrow) cosl_ba_solver();
+  if (!s) return set_error(COSL_E_NOMEM, "host allocation failed");
+  s->opt = *opt;
+  s->comm = comm;
+  s->device = opt->device;
+  cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
+  if (e != cudaSuccess) {
+    delete s;
+    return set_error(COSL_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
+  }
+  *out = s;
+  pool_keep(opt->device);
+  static_assert(SC_NTOT <= 16, "pinned slot size");
+  s->h_sc = pinned_slots().get();
+  if (!s->h_sc) return set_error(COSL_E_NOMEM, "pinned host allocation failed");
+  *reinterpret_cast<volatile unsigned long long*>(s->h_sc + SC_NTOT) = 0;  // a pooled slot keeps its last flag
+  s->scSeq = 0;
+  COSL_CUDA(cudaEventCreateWithFlags(&s->evStaged, cudaEventDisableTiming));
+  COSL_TRY(grow(s, &s->d_sc, (size_t)SC_NTOT));
+  COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+  COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+  COSL_CUDA(cudaFuncSetAttribute(ba_schur_pairs_st, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_ST_SMEM));
+  int nsm = 0;
+  COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, s->device));
+  s->numSM = std::max(1, nsm);
   s->secLin = s->timer.section("ba_linearize");
   s->secSchur = s->timer.section("ba_schur");
   s->secSolve = s->timer.section("ba_solve");
   s->secBack = s->timer.section("ba_backsub");
   s->secCost = s->timer.section("ba_cost");
   s->secComm = s->timer.section("ba_allreduce");
-  return upload_params(s, p);
+  return COSL_OK;
 }
 
 /* ---------------------------------------------------------------- device steps */
-inline bool multi(const cosl_ba_solver* s) { return s->comm && s->comm->nranks > 1; }
-inline int rank_of(const cosl_ba_solver* s) { return s->comm ? s->comm->rank : 0; }
 
 int allreduce(cosl_ba_solver* s, double* buf, size_t count, int op) {
   if (!multi(s)) return COSL_OK;
@@ -1214,8 +1393,9 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t cs, int stage) {
     const int nCamBlocks = div_up(6 * s->m, 256);
     COSL_LAUNCH(ba_back_cams_points_ctl, nCamBlocks + gN, 256, 0, cs, s->d, s->d_ctl, s->d_pa, s->d_x, s->d_dpa,
                 s->d_na, 1, nCamBlocks, s->d_dpb);
-    COSL_LAUNCH(ba_finish_cost_ctl, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, cs, s->d, s->d_ctl,
-                s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv);
+    if (s->N + s->n)  // a problem without points never reaches a trial (|g| = 0 stops it), but is captured
+      COSL_LAUNCH(ba_finish_cost_ctl, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, cs, s->d, s->d_ctl,
+                  s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv);
   } else {  // solve_trial + the trial cost, no free camera
     COSL_LAUNCH(ba_cam_update_ctl,
                 std::max(div_up(6 * s->m, 256), (int)std::min<long long>(s->numSM, div_up64(3LL * s->n, 1024))), 256,
@@ -1294,25 +1474,35 @@ int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
   return COSL_OK;
 }
 
+// (Re)builds the graph for the loaded problem.  An existing executable graph is updated in place when
+// the driver accepts the new topology, and instantiated afresh otherwise; neither waits for the device
+// (an executable graph that is destroyed while it runs is released when it completes).
 int build_graph(cosl_ba_solver* s) {
-  if (s->graphExec) {
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
-    cudaGraphExecDestroy(s->graphExec);
-    s->graphExec = nullptr;
-  }
+  const double t0 = now_s();
   int drv = 0;
   COSL_CUDA(cudaDriverGetVersion(&drv));
   if (drv < 12040)
     return set_error(COSL_E_CUDA,
                      "cosl_ba_solver_submit: the CUDA driver (version %d) has no conditional graph nodes (12.4 or "
                      "newer is needed)", drv);
-  if (!s->d_ctl) COSL_TRY(dev_alloc(s->stream, &s->d_ctl, 1));
+  COSL_TRY(grow(s, &s->d_ctl, 1));
   cudaStream_t cs = nullptr;
   COSL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaGraphCreate(&g, 0);
   int rc = e == cudaSuccess ? build_graph_nodes(s, cs, g) : set_error(COSL_E_CUDA, "cudaGraphCreate: %s", cudaGetErrorString(e));
-  if (rc == COSL_OK) {
+  const double t1 = now_s();
+  bool updated = false;
+  if (rc == COSL_OK && s->graphExec) {
+    cudaGraphExecUpdateResultInfo ui;
+    updated = cudaGraphExecUpdate(s->graphExec, g, &ui) == cudaSuccess;
+    if (!updated) {
+      cudaGetLastError();  // a refused update is not an error: instantiate instead
+      cudaGraphExecDestroy(s->graphExec);
+      s->graphExec = nullptr;
+    }
+  }
+  if (rc == COSL_OK && !updated) {
     e = cudaGraphInstantiate(&s->graphExec, g, 0);
     if (e != cudaSuccess) {
       s->graphExec = nullptr;
@@ -1322,6 +1512,10 @@ int build_graph(cosl_ba_solver* s) {
   if (g) cudaGraphDestroy(g);
   cudaStreamDestroy(cs);
   if (rc != COSL_OK) return rc;
+  if (ba_timing())
+    std::fprintf(stderr, "[ba timing] graph: capture %.2f ms, %s %.2f ms\n", 1e3 * (t1 - t0),
+                 updated ? "exec update" : "instantiate", 1e3 * (now_s() - t1));
+  s->graphStale = false;
   s->graphPa = s->d_pa;
   s->graphNa = s->d_na;
   s->graphPb = s->d_pb;
@@ -1393,32 +1587,20 @@ int cosl_ba_solver_create(const cosl_ba_problem* prob, const cosl_ba_options* op
                           cosl_ba_comm* comm, cosl_ba_solver** out) {
   if (!prob || !opt || !out) return set_error(COSL_E_INVALID, "null argument");
   *out = nullptr;
-  if (prob->m < 1 || prob->n < 0 || prob->nobs < 0 || prob->m_con < 0 || prob->m_con > prob->m ||
-      prob->n_con < 0 || prob->n_con > prob->n || !prob->K || !prob->R || !prob->t ||
-      (prob->n && (!prob->X || !prob->ptr)) || (prob->nobs && (!prob->cam || !prob->xy)) ||
-      prob->nobs >= (1ll << 31))
-    return set_error(COSL_E_INVALID, "cosl_ba_solver_create: bad problem");
-  if (prob->n && prob->ptr[prob->n] != prob->nobs)
-    return set_error(COSL_E_INVALID, "ptr[n] != nobs");
-  COSL_TRY(check_observations(prob));
+  COSL_TRY(check_problem(prob, "cosl_ba_solver_create"));
+  const double t0 = now_s();
+  BaIndex x;
+  COSL_TRY(index_problem(prob, x));
+  if (ba_timing()) std::fprintf(stderr, "[ba timing] index %.2f ms\n", 1e3 * (now_s() - t0));
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || opt->device < 0 || opt->device >= ndev)
     return set_error(COSL_E_CUDA, "CUDA device %d not available", opt->device);
   COSL_CUDA(cudaSetDevice(opt->device));
-  cosl_ba_solver* s = new (std::nothrow) cosl_ba_solver();
-  if (!s) return set_error(COSL_E_NOMEM, "host allocation failed");
-  s->opt = *opt;
-  s->comm = comm;
-  s->device = opt->device;
-  cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) {
-    delete s;
-    return set_error(COSL_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
-  }
-  pool_keep(opt->device);
-  const double tBuild0 = now_s();
-  const int rc = build_solver(s, prob);
-  if (ba_timing()) std::fprintf(stderr, "[ba timing] build_solver %.1f ms\n", 1e3 * (now_s() - tBuild0));
+  cosl_ba_solver* s = nullptr;
+  int rc = make_handle(opt, comm, &s);
+  if (rc == COSL_OK) rc = load_problem(s, prob, x);
+  if (rc == COSL_OK && cudaStreamSynchronize(s->stream) != cudaSuccess)
+    rc = set_error(COSL_E_CUDA, "cosl_ba_solver_create: %s", cudaGetErrorString(cudaGetLastError()));
   if (rc != COSL_OK) {
     free_solver(s);
     return rc;
@@ -1440,7 +1622,23 @@ int cosl_ba_solver_reset(cosl_ba_solver* s, const cosl_ba_problem* prob) {
   if (!prob || prob->m != s->m || prob->n != s->n)
     return set_error(COSL_E_INVALID, "cosl_ba_solver_reset: problem shape changed");
   s->timer.reset();
-  return upload_params(s, prob);
+  COSL_CUDA(cudaEventSynchronize(s->evStaged));
+  COSL_TRY(upload_params(s, prob));
+  COSL_CUDA(cudaEventRecord(s->evStaged, s->stream));
+  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  return COSL_OK;
+}
+
+int cosl_ba_solver_load(cosl_ba_solver* s, const cosl_ba_problem* prob) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_load: a multi-rank solver plans over all ranks; create one");
+  BA_IDLE(s, "cosl_ba_solver_load")
+  COSL_TRY(check_problem(prob, "cosl_ba_solver_load"));
+  BaIndex x;
+  COSL_TRY(index_problem(prob, x));
+  s->timer.reset();
+  return load_problem(s, prob, x);
 }
 
 int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
@@ -1471,7 +1669,7 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
                      "use cosl_ba_solver_run");
   BA_IDLE(s, "cosl_ba_solver_submit")
   // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
-  if (!s->graphExec || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
+  if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
       s->graphNb != s->d_nb)
     COSL_TRY(build_graph(s));
   if (!s->evSubmit) COSL_CUDA(cudaEventCreate(&s->evSubmit));
@@ -1571,7 +1769,7 @@ int cosl_ba_solver_trace(cosl_ba_solver* s, int enable, uint64_t* out, int32_t* 
   BA_ENTER(s)
   const int nt = (int)s->plan.tasks.size();
   if (enable) {
-    if (!s->d_trace) COSL_TRY(dev_alloc(s->stream, &s->d_trace, (size_t)std::max(1, nt) * 8));
+    COSL_TRY(grow(s, &s->d_trace, (size_t)std::max(1, nt) * 8));
     COSL_CUDA(cudaMemsetAsync(s->d_trace, 0, sizeof(unsigned long long) * 8 * std::max(1, nt), s->stream));
     s->td.trace = s->d_trace;
     return nt;

@@ -629,8 +629,8 @@ ba_schur_pairs_st(BaDev d, const BaPairItem* __restrict__ items, int nItems, con
 // ------------------------------------------------------------------------------------------
 // Pair work lists built on the device (solver set-up).  For every free observation a = (camera ja,
 // point i) of the camera-major list and every observation b of the same point with camera jb > ja,
-// or jb == ja and b >= a: one entry in bucket (ja, jb).  Pass 1 counts per bucket, ba_scan_u32 turns
-// the counts into offsets, pass 2 places {a, b, i} at offset + running index.  (A host version
+// or jb == ja and b >= a: one entry in bucket (ja, jb).  The bucket offsets come from the host's
+// count (cosl_ba_solver_load); FILL places {a, b, i} at offset + running index.  (A host version
 // wrote 81 MB of entries at c4 and uploaded them, which dominated solver creation.)  The order
 // inside a bucket depends on the atomics; the contraction sums the same terms in a different order.
 // ------------------------------------------------------------------------------------------
@@ -654,29 +654,59 @@ ba_pairs_build(BaDev d, unsigned* __restrict__ cnt, const unsigned* __restrict__
   }
 }
 
-// exclusive prefix sum of n unsigned counts into off[0 .. n] (one CTA; n is the number of camera
-// pairs, a few 10^5)
-__global__ void __launch_bounds__(1024) ba_scan_u32(const unsigned* __restrict__ cnt, unsigned* __restrict__ off,
-                                                     long long n) {
-  __shared__ unsigned s_sum[1024];
-  const int tid = threadIdx.x;
-  const long long chunk = (n + 1023) / 1024, lo = tid * chunk, hi = min(n, lo + chunk);
-  unsigned acc = 0;
-  for (long long k = lo; k < hi; ++k) acc += cnt[k];
-  s_sum[tid] = acc;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {
-    const unsigned v = (tid >= o) ? s_sum[tid - o] : 0u;
-    __syncthreads();
-    s_sum[tid] += v;
-    __syncthreads();
+// ------------------------------------------------------------------------------------------
+// Observation index lists built on the device (cosl_ba_solver_load).  ba_index_points expands the
+// point-major CSR into pt[o].  ba_index_cams builds the camera-major list of the free-camera
+// observations (cobs, ccam) as a STABLE counting sort, so that every camera's observations stay in
+// ascending o, the order in which ba_linearize_cams sums them: one warp per chunk of `chunk`
+// consecutive observations.  Pass PLACE = false counts each free camera's observations of the chunk
+// into hist[chunk][mf] (zeroed before); ba_index_cam_base turns every column into the offsets of the
+// chunk in cobs (the camera's start + the counts of the earlier chunks); PLACE = true puts each
+// observation at its chunk offset + its rank among the camera's earlier observations of the chunk.
+// A warp owns its row of hist, so the running counts need no atomics.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+ba_index_points(const long long* __restrict__ ptr, int n, int* __restrict__ pt) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (long long o = ptr[i]; o < ptr[i + 1]; ++o) pt[o] = i;
+}
+
+template <bool PLACE>
+__global__ void __launch_bounds__(256)
+ba_index_cams(const int* __restrict__ cam, long long N, int mcon, int mf, int chunk, unsigned* __restrict__ hist,
+              int* __restrict__ cobs, int* __restrict__ ccam) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const long long o0 = w * chunk;
+  if (o0 >= N) return;  // warp-uniform
+  const long long o1 = min(N, o0 + chunk);
+  unsigned* row = hist + w * mf;
+  for (long long b = o0; b < o1; b += 32) {
+    const long long o = b + lane;
+    const int j = o < o1 ? cam[o] - mcon : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, j);
+    if (PLACE && j >= 0) {
+      const unsigned q = row[j] + __popc(peers & ((1u << lane) - 1u));
+      cobs[q] = (int)o;
+      ccam[q] = j + mcon;
+    }
+    __syncwarp();
+    if (j >= 0 && lane == 31 - __clz(peers)) row[j] += __popc(peers);
+    __syncwarp();
   }
-  unsigned run = (tid > 0) ? s_sum[tid - 1] : 0u;
-  for (long long k = lo; k < hi; ++k) {
-    off[k] = run;
-    run += cnt[k];
+}
+
+__global__ void __launch_bounds__(256)
+ba_index_cam_base(unsigned* __restrict__ hist, int nChunks, int mf, const unsigned* __restrict__ camStart) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= mf) return;
+  unsigned run = camStart[j];
+  for (int c = 0; c < nChunks; ++c) {
+    const unsigned v = hist[(size_t)c * mf + j];
+    hist[(size_t)c * mf + j] = run;
+    run += v;
   }
-  if (tid == 1023) off[n] = s_sum[1023];
 }
 
 // ------------------------------------------------------------------------------------------

@@ -432,6 +432,13 @@ int cosl_ba_solver_create(const cosl_ba_problem* prob, const cosl_ba_options* op
                           cosl_ba_comm* comm /* NULL = single GPU */, cosl_ba_solver** out);
 /* Re-upload parameters (R, t, X) from the problem struct -- resets the solver to its start. */
 int cosl_ba_solver_reset(cosl_ba_solver* s, const cosl_ba_problem* prob);
+/* Replace the solver's problem with `prob`, of any size (m, n, nobs, m_con, n_con).  Validates on the
+ * calling thread, copies what it needs (the caller may reuse its arrays on return), enqueues the
+ * set-up on the solver's stream and returns without waiting for the device.  Afterwards the handle
+ * behaves as if cosl_ba_solver_create(prob) had made it: run / run_fixed / submit / download /
+ * reset see the loaded problem.  COSL_E_STATE while a submit is in flight; COSL_E_INVALID for a
+ * malformed problem (the handle keeps its previous problem) or a multi-rank solver. */
+int cosl_ba_solver_load(cosl_ba_solver* s, const cosl_ba_problem* prob);
 /* Run the robust loop (outer_iters x inner_iters) on the resident problem. */
 int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]);
 /* Run exactly `trials` LM trials (linear solves) of one weighted inner loop without any stop test
