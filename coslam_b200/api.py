@@ -75,6 +75,13 @@ def _load():
     L.cosl_pose_intracam.argtypes = [vp, vp, vp, ci, vp, vp, vp, cd, vp, vp, C.POINTER(PoseOpt),
                                      pint]
     L.cosl_pose_intracam_batch.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, cd, vp, vp, vp, vp, ci]
+    L.cosl_pose_solver_create.argtypes = [ci, ci, ci, C.POINTER(vp)]
+    L.cosl_pose_solver_destroy.argtypes = [vp]
+    L.cosl_pose_solver_submit.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, cd, vp]
+    L.cosl_pose_solver_query.argtypes = [vp, pint]
+    L.cosl_pose_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.cosl_pose_solver_stream.argtypes = [vp]
+    L.cosl_pose_solver_stream.restype = vp
     L.cosl_ba_options_default.argtypes = [C.POINTER(BaOptions)]
     L.cosl_ba_solve.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp]
     L.cosl_ba_solve_multi.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), ci, vp, vp]
@@ -494,7 +501,9 @@ def pose_intracam(K, R0, t0, Ms, ms, tau, prev_errs=None, opt=None):
     return bool(ok.value), R.reshape(3, 3), t, opt
 
 
-def pose_intracam_batch(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, device=0):
+def _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts):
+    """C-ABI arguments of a batched pose solve up to tau, then opts (C PoseOpts; defaults when None).
+    The arrays behind the pointers live in the returned tuple."""
     Cn = len(Ms_list)
     Ks = np.ascontiguousarray(Ks, np.float64).reshape(Cn, 9)
     R0s = np.ascontiguousarray(R0s, np.float64).reshape(Cn, 9)
@@ -509,10 +518,62 @@ def pose_intracam_batch(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opt
         prev_list = [None if a is None else np.ascontiguousarray(a, np.float64) for a in prev_list]
         pp = (C.c_void_p * Cn)(*[None if a is None else a.ctypes.data for a in prev_list])
     opts = opts if opts is not None else (PoseOpt * Cn)(*[PoseOpt.defaults() for _ in range(Cn)])
+    keep = (Ks, R0s, t0s, Ms_list, ms_list, prev_list)
+    return (Cn, _ptr(Ks), _ptr(R0s), _ptr(t0s), _ptr(npts), Mp, mp, pp, float(tau)), opts, keep
+
+
+def pose_intracam_batch(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, device=0):
+    args, opts, _keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
+    Cn = args[0]
     R, t, ok = np.empty((Cn, 9)), np.empty((Cn, 3)), np.zeros(Cn, np.int32)
-    _ck(LIB.cosl_pose_intracam_batch(Cn, _ptr(Ks), _ptr(R0s), _ptr(t0s), _ptr(npts), Mp, mp, pp,
-                                     float(tau), _ptr(R), _ptr(t), opts, _ptr(ok), device))
+    _ck(LIB.cosl_pose_intracam_batch(*args, _ptr(R), _ptr(t), opts, _ptr(ok), device))
     return ok.astype(bool), R.reshape(Cn, 3, 3), t, opts
+
+
+class PoseSolver:
+    """cosl_pose_solver: pose_intracam_batch without blocking, on a stream and buffers of its own for at
+    most max_cams cameras and max_pts points (all cameras together) per submit."""
+
+    def __init__(self, device, max_cams, max_pts):
+        h = C.c_void_p()
+        _ck(LIB.cosl_pose_solver_create(int(device), int(max_cams), int(max_pts), C.byref(h)))
+        self.h, self.device, self.max_cams, self.max_pts = h, device, max_cams, max_pts
+        self._opts = None
+
+    def close(self):
+        """cosl_pose_solver_destroy: waits for a solve in flight."""
+        if getattr(self, "h", None):
+            LIB.cosl_pose_solver_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None):
+        """cosl_pose_solver_submit: enqueue pose_intracam_batch's solve and return at once; the input arrays
+        may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills."""
+        args, opts, _keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
+        _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
+        self._opts = opts
+
+    def done(self):
+        """cosl_pose_solver_query: True once the submitted solve has finished (never waits)."""
+        d = C.c_int(0)
+        _ck(LIB.cosl_pose_solver_query(self.h, C.byref(d)))
+        return bool(d.value)
+
+    def collect(self):
+        """cosl_pose_solver_collect: wait for the submitted solve.  Returns (ok, R, t, opts) as
+        pose_intracam_batch does, then the device time of its copies and kernel in ms."""
+        opts = self._opts if self._opts is not None else (PoseOpt * 1)()
+        Cn = len(opts)
+        R, t, ok, ms = np.empty((Cn, 9)), np.empty((Cn, 3)), np.zeros(Cn, np.int32), C.c_double(0)
+        _ck(LIB.cosl_pose_solver_collect(self.h, _ptr(R), _ptr(t), opts, _ptr(ok), C.byref(ms)))
+        self._opts = None
+        return ok.astype(bool), R.reshape(Cn, 3, 3), t, opts, ms.value
+
+    def stream(self):
+        return LIB.cosl_pose_solver_stream(self.h)
 
 
 def ba_solve(prob, opt):

@@ -9,9 +9,11 @@
 // fp64 operations (this file is compiled with -fmad=false) so that the differences see the same
 // roundings as the oracle.
 #include <algorithm>
+#include <climits>
 #include <cmath>
+#include <map>
 #include <mutex>
-#include <vector>
+#include <new>
 
 #include "common.cuh"
 
@@ -32,17 +34,6 @@ struct PoseOut {
   double R[9], t[3];
   double lambda0, lambda, err0, err, errRW;
   int retTypeLM, npts, nIterLM, nIterRW, ok;
-};
-
-struct PoseOut;
-struct PoseCam;
-struct PoseWorkspace {
-  cudaStream_t stream = nullptr;
-  PoseCam* d_cams = nullptr;
-  double *d_M = nullptr, *d_m = nullptr, *d_p = nullptr, *d_W = nullptr;
-  PoseOut* d_out = nullptr;
-  int capC = 0;
-  long long capPts = 0;
 };
 
 struct PoseCfg {
@@ -379,6 +370,94 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
   }
 }
 
+// Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
+// cameras.
+int check_cameras(const char* fn, int C, const int* npts, const double* const* Ms, const double* const* ms,
+                  const cosl_pose_opt* opts, long long* tot) {
+  long long n = 0;
+  for (int c = 0; c < C; ++c) {
+    if (npts[c] < 0 || (npts[c] && (!Ms[c] || !ms[c])))
+      return set_error(COSL_E_INVALID, "%s: bad camera %d", fn, c);
+    n += npts[c];
+  }
+  if (n > INT_MAX) return set_error(COSL_E_INVALID, "%s: %lld points exceed one solve", fn, n);
+  // all opts share the solver settings of opts[0] except lambda0, which is per camera in the
+  // reference (carried across calls by the caller); kernel cfg takes opts[0], lambda0 is uniform
+  for (int c = 1; c < C; ++c)
+    if (opts[c].lambda0 != opts[0].lambda0 || opts[c].maxIterLM != opts[0].maxIterLM ||
+        opts[c].maxIterRW != opts[0].maxIterRW || opts[c].epsErrorChangeLM != opts[0].epsErrorChangeLM ||
+        opts[c].epsParamChangeLM != opts[0].epsParamChangeLM ||
+        opts[c].epsErrorChangeRW != opts[0].epsErrorChangeRW)
+      return set_error(COSL_E_INVALID, "batched pose solve needs identical options per camera");
+  *tot = n;
+  return COSL_OK;
+}
+
+}  // namespace
+
+// A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out as
+// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] (tot = points of the solve); the PoseOuts come back into
+// pinned memory.  Capacity is fixed at create: everything is allocated once.
+struct cosl_pose_solver {
+  int device = 0, maxCams = 0, maxPts = 0;
+  cudaStream_t stream = nullptr;
+  cudaEvent_t evStart = nullptr, evDone = nullptr;
+  unsigned char* h_in = nullptr;
+  unsigned char* d_in = nullptr;
+  double* d_W = nullptr;
+  PoseOut* d_out = nullptr;
+  PoseOut* h_out = nullptr;
+  int C = 0;  // cameras of the solve in flight
+  bool inFlight = false;
+};
+
+namespace {
+
+size_t input_bytes(int C, long long tot) { return sizeof(PoseCam) * C + sizeof(double) * 6 * tot; }
+
+void free_pose_solver(cosl_pose_solver* s) {
+  cudaSetDevice(s->device);
+  if (s->stream) cudaStreamSynchronize(s->stream);  // a solve in flight reads and writes the buffers below
+  if (s->evStart) cudaEventDestroy(s->evStart);
+  if (s->evDone) cudaEventDestroy(s->evDone);
+  if (s->h_in) cudaFreeHost(s->h_in);
+  if (s->h_out) cudaFreeHost(s->h_out);
+  cudaFree(s->d_in);
+  cudaFree(s->d_W);
+  cudaFree(s->d_out);
+  if (s->stream) cudaStreamDestroy(s->stream);
+  delete s;
+}
+
+int alloc_pose_solver(cosl_pose_solver* s) {
+  COSL_CUDA(cudaSetDevice(s->device));
+  COSL_CUDA(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
+  COSL_CUDA(cudaEventCreate(&s->evStart));
+  COSL_CUDA(cudaEventCreate(&s->evDone));
+  const size_t in = input_bytes(s->maxCams, s->maxPts);
+  COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
+  COSL_CUDA(cudaHostAlloc(&s->h_out, sizeof(PoseOut) * s->maxCams, cudaHostAllocPortable));
+  COSL_CUDA(cudaMalloc(&s->d_in, in));
+  COSL_CUDA(cudaMalloc(&s->d_W, sizeof(double) * std::max(s->maxPts, 1)));
+  COSL_CUDA(cudaMalloc(&s->d_out, sizeof(PoseOut) * s->maxCams));
+  return COSL_OK;
+}
+
+// The staged inputs of C cameras and tot points: copy, kernel, read-back, between the two events.
+int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg) {
+  const PoseCam* d_cams = reinterpret_cast<const PoseCam*>(s->d_in);
+  const double* d_M = reinterpret_cast<const double*>(s->d_in + sizeof(PoseCam) * C);
+  const double* d_m = d_M + 3 * tot;
+  const double* d_p = d_m + 2 * tot;
+  COSL_CUDA(cudaEventRecord(s->evStart, s->stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, input_bytes(C, tot), cudaMemcpyHostToDevice, s->stream));
+  COSL_LAUNCH(pose_intracam_kernel, C, POSE_THREADS, 0, s->stream, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out);
+  COSL_CUDA(cudaGetLastError());
+  COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, s->stream));
+  COSL_CUDA(cudaEventRecord(s->evDone, s->stream));
+  return COSL_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -394,39 +473,68 @@ void cosl_pose_opt_default(cosl_pose_opt* o) {
   o->lambda0 = 1e-3;
 }
 
-int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const double* t0,
-                             const int* npts, const double* const* Ms, const double* const* ms,
-                             const double* const* prevErrs, double tau, double* R_opt,
-                             double* t_opt, cosl_pose_opt* opts, int* ok, int device) {
-  if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !R_opt || !t_opt || !opts)
-    return set_error(COSL_E_INVALID, "cosl_pose_intracam_batch: null argument");
+int cosl_pose_solver_create(int device, int maxCams, int maxPts, cosl_pose_solver** out) {
+  if (!out || device < 0 || maxCams < 1 || maxPts < 0)
+    return set_error(COSL_E_INVALID, "cosl_pose_solver_create: bad argument");
+  *out = nullptr;
   int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device >= ndev)
     return set_error(COSL_E_CUDA, "CUDA device %d not available", device);
-  COSL_CUDA(cudaSetDevice(device));
-  std::vector<PoseCam> cams(C);
+  cosl_pose_solver* s = new (std::nothrow) cosl_pose_solver;
+  if (!s) return set_error(COSL_E_NOMEM, "cosl_pose_solver_create: out of host memory");
+  s->device = device;
+  s->maxCams = maxCams;
+  s->maxPts = maxPts;
+  const int rc = alloc_pose_solver(s);
+  if (rc != COSL_OK) {
+    free_pose_solver(s);
+    return rc;
+  }
+  *out = s;
+  return COSL_OK;
+}
+
+int cosl_pose_solver_destroy(cosl_pose_solver* s) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  free_pose_solver(s);
+  return COSL_OK;
+}
+
+int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
+                            const int* npts, const double* const* Ms, const double* const* ms,
+                            const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  if (s->inFlight) return set_error(COSL_E_STATE, "cosl_pose_solver_submit: a submitted solve is not collected yet");
+  if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !opts)
+    return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: null argument");
+  if (C > s->maxCams)
+    return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: %d cameras exceed the handle's %d", C, s->maxCams);
   long long tot = 0;
+  COSL_TRY(check_cameras("cosl_pose_solver_submit", C, npts, Ms, ms, opts, &tot));
+  if (tot > s->maxPts)
+    return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: %lld points exceed the handle's %d", tot, s->maxPts);
+  COSL_CUDA(cudaSetDevice(s->device));
+  // nothing is in flight, so no copy reads the staging buffer any more
+  PoseCam* cams = reinterpret_cast<PoseCam*>(s->h_in);
+  double* hM = reinterpret_cast<double*>(s->h_in + sizeof(PoseCam) * C);
+  double* hm = hM + 3 * tot;
+  double* hp = hm + 2 * tot;
+  long long off = 0;
   for (int c = 0; c < C; ++c) {
-    if (npts[c] < 0 || (npts[c] && (!Ms[c] || !ms[c])))
-      return set_error(COSL_E_INVALID, "cosl_pose_intracam_batch: bad camera %d", c);
     std::memcpy(cams[c].K, K9 + 9 * c, sizeof(double) * 9);
     std::memcpy(cams[c].R0, R0 + 9 * c, sizeof(double) * 9);
     std::memcpy(cams[c].t0, t0 + 3 * c, sizeof(double) * 3);
     cams[c].npts = npts[c];
     cams[c].hasPrev = (prevErrs && prevErrs[c]) ? 1 : 0;
-    cams[c].off = tot;
-    tot += npts[c];
+    cams[c].off = off;
+    if (npts[c]) {
+      std::memcpy(hM + 3 * off, Ms[c], sizeof(double) * 3 * npts[c]);
+      std::memcpy(hm + 2 * off, ms[c], sizeof(double) * 2 * npts[c]);
+      // a camera without prevErrs leaves its slice unset: the kernel does not read it
+      if (cams[c].hasPrev) std::memcpy(hp + off, prevErrs[c], sizeof(double) * npts[c]);
+    }
+    off += npts[c];
   }
-  const long long totA = tot > 0 ? tot : 1;
-  std::vector<double> hM(3 * totA), hm(2 * totA), hp(totA, 0.0);
-  for (int c = 0; c < C; ++c) {
-    if (!npts[c]) continue;
-    std::memcpy(&hM[3 * cams[c].off], Ms[c], sizeof(double) * 3 * npts[c]);
-    std::memcpy(&hm[2 * cams[c].off], ms[c], sizeof(double) * 2 * npts[c]);
-    if (cams[c].hasPrev) std::memcpy(&hp[cams[c].off], prevErrs[c], sizeof(double) * npts[c]);
-  }
-  // all opts share the solver settings of opts[0] except lambda0, which is per camera in the
-  // reference (carried across calls by the caller); kernel cfg takes opts[0], lambda0 is uniform
   PoseCfg cfg;
   cfg.maxIterLM = opts[0].maxIterLM;
   cfg.maxIterRW = opts[0].maxIterRW;
@@ -435,62 +543,45 @@ int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const do
   cfg.epsRW = opts[0].epsErrorChangeRW;
   cfg.lambda0 = opts[0].lambda0;
   cfg.tau = tau;
-  for (int c = 1; c < C; ++c)
-    if (opts[c].lambda0 != opts[0].lambda0 || opts[c].maxIterLM != opts[0].maxIterLM ||
-        opts[c].maxIterRW != opts[0].maxIterRW || opts[c].epsErrorChangeLM != opts[0].epsErrorChangeLM ||
-        opts[c].epsParamChangeLM != opts[0].epsParamChangeLM ||
-        opts[c].epsErrorChangeRW != opts[0].epsErrorChangeRW)
-      return set_error(COSL_E_INVALID, "batched pose solve needs identical options per camera");
-  // per-device workspace, reused across calls: the solve is latency-bound, a cudaMalloc/cudaFree
-  // pair per call would cost more than the kernel
-  static std::mutex mtx;
-  static PoseWorkspace ws[64];
-  std::lock_guard<std::mutex> lock(mtx);
-  PoseWorkspace& W = ws[device & 63];
-  int rc = COSL_OK;
-  std::vector<PoseOut> outs(C);
-#define POSE_CK(expr)                                                               \
-  if (rc == COSL_OK) {                                                              \
-    cudaError_t _e = (expr);                                                        \
-    if (_e != cudaSuccess) rc = set_error(COSL_E_CUDA, "%s: %s", #expr, cudaGetErrorString(_e)); \
+  const int rc = enqueue_solve(s, C, tot, cfg);
+  if (rc != COSL_OK) {
+    cudaStreamSynchronize(s->stream);  // a copy that was enqueued may still read the staging buffer
+    return rc;
   }
-  if (!W.stream) POSE_CK(cudaStreamCreateWithFlags(&W.stream, cudaStreamNonBlocking));
-  if (rc == COSL_OK && (W.capC < C || W.capPts < totA)) {
-    cudaFree(W.d_cams);
-    cudaFree(W.d_M);
-    cudaFree(W.d_m);
-    cudaFree(W.d_p);
-    cudaFree(W.d_W);
-    cudaFree(W.d_out);
-    W = PoseWorkspace{W.stream};
-    const int capC = std::max(C, 16);
-    const long long capP = std::max<long long>(totA, 4096);
-    POSE_CK(cudaMalloc(&W.d_cams, sizeof(PoseCam) * capC));
-    POSE_CK(cudaMalloc(&W.d_M, sizeof(double) * 3 * capP));
-    POSE_CK(cudaMalloc(&W.d_m, sizeof(double) * 2 * capP));
-    POSE_CK(cudaMalloc(&W.d_p, sizeof(double) * capP));
-    POSE_CK(cudaMalloc(&W.d_W, sizeof(double) * capP));
-    POSE_CK(cudaMalloc(&W.d_out, sizeof(PoseOut) * capC));
-    if (rc == COSL_OK) {
-      W.capC = capC;
-      W.capPts = capP;
-    }
+  s->C = C;
+  s->inFlight = true;
+  return COSL_OK;
+}
+
+int cosl_pose_solver_query(cosl_pose_solver* s, int* done) {
+  if (!s || !done) return set_error(COSL_E_INVALID, "cosl_pose_solver_query: null argument");
+  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_pose_solver_query: nothing submitted");
+  COSL_CUDA(cudaSetDevice(s->device));
+  const cudaError_t e = cudaEventQuery(s->evDone);
+  if (e == cudaErrorNotReady) {
+    *done = 0;
+    return COSL_OK;
   }
-  cudaStream_t st = W.stream;
-  POSE_CK(cudaMemcpyAsync(W.d_cams, cams.data(), sizeof(PoseCam) * C, cudaMemcpyHostToDevice, st));
-  POSE_CK(cudaMemcpyAsync(W.d_M, hM.data(), sizeof(double) * 3 * totA, cudaMemcpyHostToDevice, st));
-  POSE_CK(cudaMemcpyAsync(W.d_m, hm.data(), sizeof(double) * 2 * totA, cudaMemcpyHostToDevice, st));
-  POSE_CK(cudaMemcpyAsync(W.d_p, hp.data(), sizeof(double) * totA, cudaMemcpyHostToDevice, st));
-  if (rc == COSL_OK) {
-    COSL_LAUNCH(pose_intracam_kernel, C, POSE_THREADS, 0, st, W.d_cams, W.d_M, W.d_m, W.d_p, W.d_W,
-                cfg, W.d_out);
+  COSL_CUDA(e);
+  *done = 1;
+  return COSL_OK;
+}
+
+int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, cosl_pose_opt* opts, int* ok,
+                             double* device_ms) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_pose_solver_collect: nothing submitted");
+  if (!R_opt || !t_opt || !opts) return set_error(COSL_E_INVALID, "cosl_pose_solver_collect: null argument");
+  COSL_CUDA(cudaSetDevice(s->device));
+  s->inFlight = false;
+  COSL_CUDA(cudaEventSynchronize(s->evDone));
+  if (device_ms) {
+    float ms = 0.f;
+    COSL_CUDA(cudaEventElapsedTime(&ms, s->evStart, s->evDone));
+    *device_ms = ms;
   }
-  POSE_CK(cudaGetLastError());
-  POSE_CK(cudaMemcpyAsync(outs.data(), W.d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, st));
-  POSE_CK(cudaStreamSynchronize(st));
-#undef POSE_CK
-  if (rc != COSL_OK) return rc;
-  for (int c = 0; c < C; ++c) {
+  const PoseOut* outs = s->h_out;
+  for (int c = 0; c < s->C; ++c) {
     std::memcpy(R_opt + 9 * c, outs[c].R, sizeof(double) * 9);
     std::memcpy(t_opt + 3 * c, outs[c].t, sizeof(double) * 3);
     opts[c].lambda0 = outs[c].lambda0;
@@ -505,6 +596,37 @@ int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const do
     if (ok) ok[c] = outs[c].ok;
   }
   return COSL_OK;
+}
+
+void* cosl_pose_solver_stream(cosl_pose_solver* s) { return s ? (void*)s->stream : nullptr; }
+
+int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const double* t0,
+                             const int* npts, const double* const* Ms, const double* const* ms,
+                             const double* const* prevErrs, double tau, double* R_opt,
+                             double* t_opt, cosl_pose_opt* opts, int* ok, int device) {
+  if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !R_opt || !t_opt || !opts)
+    return set_error(COSL_E_INVALID, "cosl_pose_intracam_batch: null argument");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
+    return set_error(COSL_E_CUDA, "CUDA device %d not available", device);
+  long long tot = 0;
+  COSL_TRY(check_cameras("cosl_pose_intracam_batch", C, npts, Ms, ms, opts, &tot));
+  // one library-owned handle per device, reused across calls (the solve is latency-bound: an allocation per
+  // call would cost more than the kernel); it is replaced by a larger one when a call does not fit.  The lock
+  // serialises the callers of these shared handles only.
+  static std::mutex mtx;
+  static std::map<int, cosl_pose_solver*> shared;
+  std::lock_guard<std::mutex> lock(mtx);
+  cosl_pose_solver*& s = shared[device];
+  if (!s || s->maxCams < C || s->maxPts < tot) {
+    const int capC = std::max(C, s ? s->maxCams : 16);
+    const int capP = (int)std::max<long long>(tot, s ? s->maxPts : 4096);
+    if (s) cosl_pose_solver_destroy(s);
+    s = nullptr;
+    COSL_TRY(cosl_pose_solver_create(device, capC, capP, &s));
+  }
+  COSL_TRY(cosl_pose_solver_submit(s, C, K9, R0, t0, npts, Ms, ms, prevErrs, tau, opts));
+  return cosl_pose_solver_collect(s, R_opt, t_opt, opts, ok, nullptr);
 }
 
 int cosl_pose_intracam(const double K[9], const double R0[9], const double t0[3], int npts,

@@ -349,6 +349,42 @@ int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const do
                              const double* const* prevErrs, double tau, double* R_opt,
                              double* t_opt, cosl_pose_opt* opts, int* ok, int device);
 
+/* A pose solver handle: the batched solve above without blocking the calling thread, what
+ * CoSLAM::parallelPoseUpdate (app/SL_CoSLAM.cpp:398-417) needs to keep tracking while the poses of
+ * a frame are refined.  A handle owns a non-blocking stream, its device buffers, a pinned staging
+ * buffer for the inputs, a pinned buffer for the results and its events, all allocated by create
+ * for at most maxCams cameras and maxPts points (all cameras together) per submit; nothing is
+ * allocated afterwards.  Without a usable device create gives COSL_E_CUDA; there is no CPU path.
+ *
+ * submit takes the arguments of cosl_pose_intracam_batch less the outputs and the device, runs its
+ * checks on the calling thread with its codes (COSL_E_INVALID for a NULL argument, a bad camera or
+ * options that differ between cameras), and COSL_E_INVALID when C > maxCams or the points exceed
+ * maxPts (the handle stays usable).  It packs the inputs into the pinned buffer, so the caller may
+ * reuse its arrays when it returns, enqueues one host-to-device copy, the batch call's kernel and
+ * the read-back of the results on the handle's stream, and returns without waiting for the device.
+ * query sets *done = 1 once the solve has finished, without waiting.  collect waits for it and
+ * writes R_opt, t_opt, the opts fields and ok (nullable) exactly as cosl_pose_intracam_batch does
+ * for the same inputs, bit for bit; *device_ms (nullable) is the device time of the copies and the
+ * kernel, from CUDA events.
+ *
+ * One solve may be in flight per handle: a second submit gives COSL_E_STATE, and so do query and
+ * collect with nothing in flight.  destroy waits for a solve in flight.  A handle is not
+ * re-entrant; different handles, on any threads and devices, share no lock.  Every call makes the
+ * handle's device current on the calling thread. */
+typedef struct cosl_pose_solver cosl_pose_solver;
+int cosl_pose_solver_create(int device, int maxCams, int maxPts, cosl_pose_solver** out);
+int cosl_pose_solver_destroy(cosl_pose_solver* s);
+int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const double* R0,
+                            const double* t0, const int* npts, const double* const* Ms,
+                            const double* const* ms, const double* const* prevErrs, double tau,
+                            const cosl_pose_opt* opts);
+int cosl_pose_solver_query(cosl_pose_solver* s, int* done);
+int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, cosl_pose_opt* opts,
+                             int* ok, double* device_ms);
+/* CUDA stream (cudaStream_t as void*) the handle's solves run on; work enqueued there after a
+ * submit runs after that solve. */
+void* cosl_pose_solver_stream(cosl_pose_solver* s);
+
 /* ================================================================ bundle adjustment */
 
 /* Flat form of the arguments of
