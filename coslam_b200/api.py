@@ -113,6 +113,14 @@ def _load():
     L.cosl_posegraph_spread_chains.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, vp, ci]
     L.cosl_posegraph_solve.argtypes = [ci, vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci]
     L.cosl_posegraph_last_host_ms.restype = cd
+    L.cosl_posegraph_solver_create.argtypes = [ci, C.POINTER(vp)]
+    L.cosl_posegraph_solver_destroy.argtypes = [vp]
+    L.cosl_posegraph_solver_submit_chains.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp]
+    L.cosl_posegraph_solver_submit.argtypes = [vp, ci, vp, vp, vp, ci, vp, vp, vp, vp, vp, ci]
+    L.cosl_posegraph_solver_query.argtypes = [vp, pint]
+    L.cosl_posegraph_solver_collect.argtypes = [vp, vp, vp, vp, vp]
+    L.cosl_posegraph_solver_stream.argtypes = [vp]
+    L.cosl_posegraph_solver_stream.restype = vp
     return L
 
 
@@ -614,11 +622,9 @@ def ba_debug_tile_solve(S, b, adj, nd_depth=-1):
     return x, fail.value, dict(zip(PLAN_INFO_KEYS, [int(v) for v in out]))
 
 
-def posegraph_spread_chains(chain_off, fixed, R, t, eR, et, device=0):
-    """cosl_posegraph_spread_chains: post-BA spreading of the non-key-frame poses of all cameras
-    (GlobalPoseGraph::computeNewCameraRotations + ::computeNewCameraTranslations on the chain
-    graphs of RobustBundleRTS::constructCameraGraphs).  chain_off[nChains+1]; fixed[N]; R (N,3,3);
-    t (N,3); eR (N,3,3), et (N,3): edge k = node k -> k+1.  Returns newR (N,3,3), newt (N,3)."""
+def _chain_args(chain_off, fixed, R, t, eR, et):
+    """C-ABI arguments of a chain spread from nChains on, and N.  The arrays behind the pointers live in the
+    returned tuple."""
     off = np.ascontiguousarray(chain_off, np.int32)
     N = int(off[-1])
     fx = np.ascontiguousarray(fixed, np.uint8)
@@ -627,17 +633,24 @@ def posegraph_spread_chains(chain_off, fixed, R, t, eR, et, device=0):
     eR = np.ascontiguousarray(eR, np.float64).reshape(N, 3, 3)
     et = np.ascontiguousarray(et, np.float64).reshape(N, 3)
     assert fx.size == N
+    keep = (off, fx, R, t, eR, et)
+    return (len(off) - 1, _ptr(off), _ptr(fx), _ptr(R), _ptr(t), _ptr(eR), _ptr(et)), N, keep
+
+
+def posegraph_spread_chains(chain_off, fixed, R, t, eR, et, device=0):
+    """cosl_posegraph_spread_chains: post-BA spreading of the non-key-frame poses of all cameras
+    (GlobalPoseGraph::computeNewCameraRotations + ::computeNewCameraTranslations on the chain
+    graphs of RobustBundleRTS::constructCameraGraphs).  chain_off[nChains+1]; fixed[N]; R (N,3,3);
+    t (N,3); eR (N,3,3), et (N,3): edge k = node k -> k+1.  Returns newR (N,3,3), newt (N,3)."""
+    args, N, _keep = _chain_args(chain_off, fixed, R, t, eR, et)
     nR, nt = np.empty((N, 3, 3)), np.empty((N, 3))
-    _ck(LIB.cosl_posegraph_spread_chains(len(off) - 1, _ptr(off), _ptr(fx), _ptr(R), _ptr(t),
-                                         _ptr(eR), _ptr(et), _ptr(nR), _ptr(nt), int(device)))
+    _ck(LIB.cosl_posegraph_spread_chains(*args, _ptr(nR), _ptr(nt), int(device)))
     return nR, nt
 
 
-def posegraph_solve(fixed, R, t, id1, id2, eR, et, scale_col=None, n_scale=0, device=0):
-    """cosl_posegraph_solve: GlobalPoseGraph::computeNewCameraRotations + ::computeNewCameraTranslations4
-    on an arbitrary edge set (the camera-group merge).  fixed[n]; R (n,3,3); t (n,3); edges id1 -> id2 with
-    eR (e,3,3), et (e,3); scale_col[e] = shared scale column of edge e (-1: known scale; None: all known).
-    Returns newR (n,3,3), newt (n,3), scale (n_scale,)."""
+def _graph_args(fixed, R, t, id1, id2, eR, et, scale_col, n_scale):
+    """C-ABI arguments of a general pose graph from nNodes to nScale, and nNodes.  The arrays behind the
+    pointers live in the returned tuple."""
     fx = np.ascontiguousarray(fixed, np.uint8)
     n = fx.size
     R = np.ascontiguousarray(R, np.float64).reshape(n, 3, 3)
@@ -650,10 +663,74 @@ def posegraph_solve(fixed, R, t, id1, id2, eR, et, scale_col=None, n_scale=0, de
     et = np.ascontiguousarray(et, np.float64).reshape(ne, 3)
     sc = None if scale_col is None else np.ascontiguousarray(scale_col, np.int32)
     assert sc is None or sc.size == ne
+    keep = (fx, R, t, id1, id2, eR, et, sc)
+    return (n, _ptr(fx), _ptr(R), _ptr(t), ne, _ptr(id1), _ptr(id2), _ptr(eR), _ptr(et), _ptr(sc),
+            int(n_scale)), n, keep
+
+
+def posegraph_solve(fixed, R, t, id1, id2, eR, et, scale_col=None, n_scale=0, device=0):
+    """cosl_posegraph_solve: GlobalPoseGraph::computeNewCameraRotations + ::computeNewCameraTranslations4
+    on an arbitrary edge set (the camera-group merge).  fixed[n]; R (n,3,3); t (n,3); edges id1 -> id2 with
+    eR (e,3,3), et (e,3); scale_col[e] = shared scale column of edge e (-1: known scale; None: all known).
+    Returns newR (n,3,3), newt (n,3), scale (n_scale,)."""
+    args, n, _keep = _graph_args(fixed, R, t, id1, id2, eR, et, scale_col, n_scale)
     nR, nt, s = np.empty((n, 3, 3)), np.empty((n, 3)), np.empty(max(1, int(n_scale)))
-    _ck(LIB.cosl_posegraph_solve(n, _ptr(fx), _ptr(R), _ptr(t), ne, _ptr(id1), _ptr(id2), _ptr(eR), _ptr(et),
-                                 _ptr(sc), int(n_scale), _ptr(nR), _ptr(nt), _ptr(s), int(device)))
+    _ck(LIB.cosl_posegraph_solve(*args, _ptr(nR), _ptr(nt), _ptr(s), int(device)))
     return nR, nt, s[:int(n_scale)]
+
+
+class PoseGraphSolver:
+    """cosl_posegraph_solver: posegraph_spread_chains and posegraph_solve without blocking, on a stream and
+    buffers of its own that grow with the largest request."""
+
+    def __init__(self, device):
+        h = C.c_void_p()
+        _ck(LIB.cosl_posegraph_solver_create(int(device), C.byref(h)))
+        self.h, self.device = h, device
+        self._shape = None  # (nodes, scale columns or None for a chain spread) of the request in flight
+
+    def close(self):
+        """cosl_posegraph_solver_destroy: waits for a request in flight."""
+        if getattr(self, "h", None):
+            LIB.cosl_posegraph_solver_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def submit_chains(self, chain_off, fixed, R, t, eR, et):
+        """cosl_posegraph_solver_submit_chains: enqueue posegraph_spread_chains' spread and return at once; the
+        input arrays may be reused when it returns."""
+        args, N, _keep = _chain_args(chain_off, fixed, R, t, eR, et)
+        _ck(LIB.cosl_posegraph_solver_submit_chains(self.h, *args))
+        self._shape = (N, None)
+
+    def submit(self, fixed, R, t, id1, id2, eR, et, scale_col=None, n_scale=0):
+        """cosl_posegraph_solver_submit: enqueue posegraph_solve's solve and return at once; the input arrays
+        may be reused when it returns."""
+        args, n, _keep = _graph_args(fixed, R, t, id1, id2, eR, et, scale_col, n_scale)
+        _ck(LIB.cosl_posegraph_solver_submit(self.h, *args))
+        self._shape = (n, int(n_scale))
+
+    def done(self):
+        """cosl_posegraph_solver_query: True once the submitted request has finished (never waits)."""
+        d = C.c_int(0)
+        _ck(LIB.cosl_posegraph_solver_query(self.h, C.byref(d)))
+        return bool(d.value)
+
+    def collect(self):
+        """cosl_posegraph_solver_collect: wait for the submitted request.  Returns (newR, newt, scale, device_ms):
+        what posegraph_spread_chains (scale None) or posegraph_solve returns, then the device time of the
+        copies and kernels in ms.  Raises CoslError as those calls do."""
+        n, ns = self._shape if self._shape is not None else (0, 0)
+        nR, nt, s = np.empty((n, 3, 3)), np.empty((n, 3)), np.empty(max(1, ns or 0))
+        ms = C.c_double(0)
+        self._shape = None  # a collect that reports an error consumes the request as well
+        _ck(LIB.cosl_posegraph_solver_collect(self.h, _ptr(nR), _ptr(nt), _ptr(s), C.byref(ms)))
+        return nR, nt, (None if ns is None else s[:ns]), ms.value
+
+    def stream(self):
+        return LIB.cosl_posegraph_solver_stream(self.h)
 
 
 def posegraph_last_host_ms():

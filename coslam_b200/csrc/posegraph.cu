@@ -25,8 +25,10 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <functional>
 #include <map>
 #include <mutex>
+#include <new>
 #include <utility>
 #include <vector>
 
@@ -564,73 +566,7 @@ pg_finish(PgDev d, int nNodes, const double* __restrict__ x1, const double* __re
 
 thread_local double g_pgHostMs = 0.0;
 
-}  // namespace
-}  // namespace coslam
-
-using namespace coslam;
-
-extern "C" int cosl_posegraph_spread_chains(int nChains, const int* chainOff, const uint8_t* fixed,
-                                            const double* R, const double* t, const double* eR,
-                                            const double* et, double* newR, double* newt, int device) {
-  if (nChains < 0 || !chainOff) return set_error(COSL_E_INVALID, "cosl_posegraph_spread_chains: bad chain table");
-  if (nChains == 0) return COSL_OK;
-  const int N = chainOff[nChains];
-  for (int c = 0; c < nChains; ++c)
-    if (chainOff[c + 1] < chainOff[c] || chainOff[0] != 0)
-      return set_error(COSL_E_INVALID, "cosl_posegraph_spread_chains: chainOff must start at 0 and be non-decreasing");
-  if (N == 0) return COSL_OK;
-  if (!fixed || !R || !t || !eR || !et || !newR || !newt)
-    return set_error(COSL_E_INVALID, "cosl_posegraph_spread_chains: null array");
-  COSL_CUDA(cudaSetDevice(device));
-  // one device slab: [R 9N | t 3N | eR 9N | et 3N | newR 9N | newt 3N] doubles, [anchor 2N | off C+1 | status] ints, flags
-  const size_t nd = (size_t)36 * N, ni = (size_t)2 * N + nChains + 2;
-  const size_t bytes = nd * 8 + ni * 4 + (size_t)N;
-  keep_pool(device);
-  cudaStream_t s = cudaStreamPerThread;
-  char* slab = nullptr;
-  COSL_CUDA(cudaMallocAsync(&slab, bytes, s));
-  double* dR = reinterpret_cast<double*>(slab);
-  double *dt = dR + 9 * (size_t)N, *deR = dt + 3 * (size_t)N, *det = deR + 9 * (size_t)N;
-  double *dnR = det + 3 * (size_t)N, *dnt = dnR + 9 * (size_t)N;
-  int* dAnchor = reinterpret_cast<int*>(dnt + 3 * (size_t)N);
-  int *dOff = dAnchor + 2 * (size_t)N, *dStatus = dOff + nChains + 1;
-  unsigned char* dFixed = reinterpret_cast<unsigned char*>(dStatus + 1);
-  int rc = COSL_OK;
-  auto fail = [&](cudaError_t e, const char* what) {
-    rc = set_error(COSL_E_CUDA, "cosl_posegraph_spread_chains: %s: %s", what, cudaGetErrorString(e));
-  };
-  cudaError_t e;
-#define PG_CP(dst, src, n)                                                              \
-  if (rc == COSL_OK && (e = cudaMemcpyAsync(dst, src, (n), cudaMemcpyHostToDevice, s)) != cudaSuccess) fail(e, "H2D")
-  PG_CP(dR, R, 72 * (size_t)N);
-  PG_CP(dt, t, 24 * (size_t)N);
-  PG_CP(deR, eR, 72 * (size_t)N);
-  PG_CP(det, et, 24 * (size_t)N);
-  PG_CP(dOff, chainOff, 4 * (size_t)(nChains + 1));
-  PG_CP(dFixed, fixed, (size_t)N);
-#undef PG_CP
-  if (rc == COSL_OK && (e = cudaMemsetAsync(dStatus, 0, 4, s)) != cudaSuccess) fail(e, "memset");
-  int status = 0;
-  if (rc == COSL_OK) {
-    COSL_LAUNCH(posegraph_chain_kernel, nChains, PG_THREADS, 0, s, dOff, dFixed, dR, dt, deR, det, dnR, dnt,
-                dAnchor, dStatus);
-    if ((e = cudaGetLastError()) != cudaSuccess) fail(e, "launch");
-  }
-  if (rc == COSL_OK && (e = cudaMemcpyAsync(newR, dnR, 72 * (size_t)N, cudaMemcpyDeviceToHost, s)) != cudaSuccess) fail(e, "D2H");
-  if (rc == COSL_OK && (e = cudaMemcpyAsync(newt, dnt, 24 * (size_t)N, cudaMemcpyDeviceToHost, s)) != cudaSuccess) fail(e, "D2H");
-  if (rc == COSL_OK && (e = cudaMemcpyAsync(&status, dStatus, 4, cudaMemcpyDeviceToHost, s)) != cudaSuccess) fail(e, "D2H");
-  if (rc == COSL_OK && (e = cudaStreamSynchronize(s)) != cudaSuccess) fail(e, "sync");
-  cudaFreeAsync(slab, s);
-  if (rc != COSL_OK) return rc;
-  if (status != 0)
-    return set_error(COSL_E_INVALID, "cosl_posegraph_spread_chains: chain %d has no fixed node (rank-deficient system)",
-                     status - 1);
-  return COSL_OK;
-}
-
-namespace {
-
-// aligned bump layout of one device slab (the same offsets index the host staging buffer)
+// aligned bump layout of one device slab (the same offsets index the host staging buffers)
 struct SlabLayout {
   size_t bytes = 0;
   size_t take(size_t n) {
@@ -640,40 +576,174 @@ struct SlabLayout {
   }
 };
 
+// Where a prepare step packs a request's inputs: stage(bytes, &buf) points buf at a host buffer of at least
+// `bytes` bytes (pageable for the synchronous calls, the handle's pinned buffer for a submit) or returns an
+// error code.
+using StageFn = std::function<int(size_t, char**)>;
+
+// ---- chain spreading: prepare (checks, layout, packing) and enqueue (copies, kernel), shared by
+// cosl_posegraph_spread_chains and cosl_posegraph_solver_submit_chains.
+// Slab: inputs [R 9N | t 3N | eR 9N | et 3N | chainOff C+1 | fixed N], outputs [newR 9N | newt 3N | status]
+// (read back together), then the anchors [2N].
+struct ChainJob {
+  int nChains = 0, N = 0;  // N == 0: nothing to solve and nothing to write
+  size_t oR = 0, ot = 0, oeR = 0, oet = 0, oOff = 0, oFixed = 0, inBytes = 0, oOut = 0, oAnchor = 0, bytes = 0;
+  const int* chainOff = nullptr;  // the caller's arrays
+  const uint8_t* fixed = nullptr;
+  const double *R = nullptr, *t = nullptr, *eR = nullptr, *et = nullptr;
+  const char* staged = nullptr;  // the packed inputs (bytes [0, inBytes) of the slab), or nullptr
+};
+
+size_t chain_out_bytes(int N) { return 96 * (size_t)N + 4; }
+
+// outs: the synchronous call's {newR, newt}, checked with the inputs; nullptr for a submit (collect takes
+// them).  Without `stage` nothing is packed and the copies read the caller's arrays, which outlive the
+// synchronous call: that saves it a host copy of its inputs.
+int chain_prepare(const char* fn, int nChains, const int* chainOff, const uint8_t* fixed, const double* R,
+                  const double* t, const double* eR, const double* et, const double* const* outs,
+                  const StageFn& stage, ChainJob& j) {
+  j = ChainJob();
+  if (nChains < 0 || !chainOff) return set_error(COSL_E_INVALID, "%s: bad chain table", fn);
+  if (nChains == 0) return COSL_OK;
+  const int N = chainOff[nChains];
+  for (int c = 0; c < nChains; ++c)
+    if (chainOff[c + 1] < chainOff[c] || chainOff[0] != 0)
+      return set_error(COSL_E_INVALID, "%s: chainOff must start at 0 and be non-decreasing", fn);
+  if (N == 0) return COSL_OK;
+  if (!fixed || !R || !t || !eR || !et || (outs && (!outs[0] || !outs[1])))
+    return set_error(COSL_E_INVALID, "%s: null array", fn);
+  SlabLayout L;
+  j.oR = L.take(72 * (size_t)N);
+  j.ot = L.take(24 * (size_t)N);
+  j.oeR = L.take(72 * (size_t)N);
+  j.oet = L.take(24 * (size_t)N);
+  j.oOff = L.take(4 * (size_t)(nChains + 1));
+  j.oFixed = L.take((size_t)N);
+  j.inBytes = L.bytes;
+  j.oOut = L.take(chain_out_bytes(N));
+  j.oAnchor = L.take(8 * (size_t)N);
+  j.bytes = L.bytes;
+  j.nChains = nChains;
+  j.N = N;
+  j.chainOff = chainOff;
+  j.fixed = fixed;
+  j.R = R;
+  j.t = t;
+  j.eR = eR;
+  j.et = et;
+  if (stage) {
+    char* h = nullptr;
+    COSL_TRY(stage(j.inBytes, &h));
+    std::memcpy(h + j.oR, R, 72 * (size_t)N);
+    std::memcpy(h + j.ot, t, 24 * (size_t)N);
+    std::memcpy(h + j.oeR, eR, 72 * (size_t)N);
+    std::memcpy(h + j.oet, et, 24 * (size_t)N);
+    std::memcpy(h + j.oOff, chainOff, 4 * (size_t)(nChains + 1));
+    std::memcpy(h + j.oFixed, fixed, (size_t)N);
+    j.staged = h;
+  }
+  return COSL_OK;
+}
+
+// The spread (j.N > 0) on `s` into `slab` (j.bytes): the inputs in one copy from j.staged or section by section
+// from the caller's arrays, the kernel, and the outputs in one copy into hostOut (chain_out_bytes, laid out
+// as the slab's output region) or into newR, newt and *status.
+int chain_enqueue(const char* fn, const ChainJob& j, char* slab, cudaStream_t s, char* hostOut, double* newR,
+                  double* newt, int* status) {
+  const int N = j.N;
+  double *dR = reinterpret_cast<double*>(slab + j.oR), *dt = reinterpret_cast<double*>(slab + j.ot);
+  double *deR = reinterpret_cast<double*>(slab + j.oeR), *det = reinterpret_cast<double*>(slab + j.oet);
+  int* dOff = reinterpret_cast<int*>(slab + j.oOff);
+  unsigned char* dFixed = reinterpret_cast<unsigned char*>(slab + j.oFixed);
+  double* dnR = reinterpret_cast<double*>(slab + j.oOut);
+  double* dnt = dnR + 9 * (size_t)N;
+  int* dStatus = reinterpret_cast<int*>(dnt + 3 * (size_t)N);
+  int* dAnchor = reinterpret_cast<int*>(slab + j.oAnchor);
+  int rc = COSL_OK;
+  auto step = [&](cudaError_t e, const char* what) {
+    if (rc == COSL_OK && e != cudaSuccess)
+      rc = set_error(COSL_E_CUDA, "%s: %s: %s", fn, what, cudaGetErrorString(e));
+  };
+  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
+  if (j.staged) {
+    step(cudaMemcpyAsync(slab, j.staged, j.inBytes, h2d, s), "H2D");
+  } else {
+    step(cudaMemcpyAsync(dR, j.R, 72 * (size_t)N, h2d, s), "H2D");
+    step(cudaMemcpyAsync(dt, j.t, 24 * (size_t)N, h2d, s), "H2D");
+    step(cudaMemcpyAsync(deR, j.eR, 72 * (size_t)N, h2d, s), "H2D");
+    step(cudaMemcpyAsync(det, j.et, 24 * (size_t)N, h2d, s), "H2D");
+    step(cudaMemcpyAsync(dOff, j.chainOff, 4 * (size_t)(j.nChains + 1), h2d, s), "H2D");
+    step(cudaMemcpyAsync(dFixed, j.fixed, (size_t)N, h2d, s), "H2D");
+  }
+  step(cudaMemsetAsync(dStatus, 0, 4, s), "memset");
+  if (rc != COSL_OK) return rc;
+  COSL_LAUNCH(posegraph_chain_kernel, j.nChains, PG_THREADS, 0, s, dOff, dFixed, dR, dt, deR, det, dnR, dnt,
+              dAnchor, dStatus);
+  step(cudaGetLastError(), "launch");
+  if (hostOut) {
+    step(cudaMemcpyAsync(hostOut, dnR, chain_out_bytes(N), d2h, s), "D2H");
+  } else {
+    step(cudaMemcpyAsync(newR, dnR, 72 * (size_t)N, d2h, s), "D2H");
+    step(cudaMemcpyAsync(newt, dnt, 24 * (size_t)N, d2h, s), "D2H");
+    step(cudaMemcpyAsync(status, dStatus, 4, d2h, s), "D2H");
+  }
+  return rc;
+}
+
+// the error the kernel reports through its status word
+int chain_status(const char* fn, int status) {
+  if (status != 0)
+    return set_error(COSL_E_INVALID, "%s: chain %d has no fixed node (rank-deficient system)", fn, status - 1);
+  return COSL_OK;
+}
+
+// ---- general graphs: prepare (validation, numbering, plan, CSR lists, layout, packing) and enqueue (copies,
+// assembly, two tile solves, finish), shared by cosl_posegraph_solve and cosl_posegraph_solver_submit.
+struct PgSlab {  // offsets of the slab's sections; [0, in) is the packed input, uploaded in one copy
+  size_t R, t, eR, et, fixed, id1, id2, sc, freeNode, freeOf, nodeOff, nodeEdges, colOff, colEdges, pair, unitPos,
+      items, itemOff, diag, order, blkCam0, blkRows, tasks, bwd, sum, cnt, in;
+  size_t rhs, tiles, rhsS, Linv, y, x, x1, out, bytes;
+};
+
+struct PgJob {
+  int N = 0, nScale = 0, nF = 0;  // nF == 0: no free node, answered on the host (fixed nodes are copied)
+  BaPlan P;
+  int nA = 0;
+  size_t nCnt = 0, nOut = 0;  // counters of the tile solve; doubles of the output region
+  PgSlab o = {};
+};
+
 int pg_find(std::vector<int>& parent, int a) {
   while (parent[a] != a) a = parent[a] = parent[parent[a]];
   return a;
 }
 
-}  // namespace
-
-extern "C" double cosl_posegraph_last_host_ms(void) { return g_pgHostMs; }
-
-extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const double* R, const double* t,
-                                    int nEdges, const int* id1, const int* id2, const double* eR,
-                                    const double* et, const int* scaleCol, int nScale, double* newR,
-                                    double* newt, double* scale, int device) {
-  const auto tHost0 = std::chrono::steady_clock::now();
-  g_pgHostMs = 0.0;
-  const char* fn = "cosl_posegraph_solve";
+// outs: the synchronous call's {newR, newt, scale}, checked with the inputs; nullptr for a submit.
+int pg_prepare(const char* fn, int nNodes, const uint8_t* fixed, const double* R, const double* t, int nEdges,
+               const int* id1, const int* id2, const double* eR, const double* et, const int* scaleCol, int nScale,
+               const void* const* outs, const StageFn& stage, PgJob& j) {
+  j = PgJob();
   if (nNodes < 0 || nEdges < 0 || nScale < 0) return set_error(COSL_E_INVALID, "%s: negative count", fn);
-  if (nNodes > 0 && (!fixed || !R || !t || !newR || !newt)) return set_error(COSL_E_INVALID, "%s: null node array", fn);
+  if (nNodes > 0 && (!fixed || !R || !t || (outs && (!outs[0] || !outs[1]))))
+    return set_error(COSL_E_INVALID, "%s: null node array", fn);
   if (nEdges > 0 && (!id1 || !id2 || !eR || !et)) return set_error(COSL_E_INVALID, "%s: null edge array", fn);
-  if (nScale > 0 && !scale) return set_error(COSL_E_INVALID, "%s: null scale array", fn);
+  if (outs && nScale > 0 && !outs[2]) return set_error(COSL_E_INVALID, "%s: null scale array", fn);
   const int N = nNodes, E = nEdges;
+  j.N = N;
+  j.nScale = nScale;
   // ---- validation: indices, self-loops, rows of the scale columns, components without a fixed node
   std::vector<int> parent(N), colRows(nScale, 0);
   for (int k = 0; k < N; ++k) parent[k] = k;
   for (int e = 0; e < E; ++e) {
-    const int i = id1[e], j = id2[e], c = scaleCol ? scaleCol[e] : -1;
-    if (i < 0 || i >= N || j < 0 || j >= N)
-      return set_error(COSL_E_INVALID, "%s: edge %d joins node %d to node %d (%d nodes)", fn, e, i, j, N);
-    if (i == j) return set_error(COSL_E_INVALID, "%s: edge %d is a self-loop on node %d", fn, e, i);
+    const int i = id1[e], j2 = id2[e], c = scaleCol ? scaleCol[e] : -1;
+    if (i < 0 || i >= N || j2 < 0 || j2 >= N)
+      return set_error(COSL_E_INVALID, "%s: edge %d joins node %d to node %d (%d nodes)", fn, e, i, j2, N);
+    if (i == j2) return set_error(COSL_E_INVALID, "%s: edge %d is a self-loop on node %d", fn, e, i);
     if (c < -1 || c >= nScale)
       return set_error(COSL_E_INVALID, "%s: edge %d has scale column %d (%d columns)", fn, e, c, nScale);
-    if (fixed[i] && fixed[j]) continue;  // no rows (:59, :368)
+    if (fixed[i] && fixed[j2]) continue;  // no rows (:59, :368)
     if (c >= 0) ++colRows[c];
-    const int a = pg_find(parent, i), b = pg_find(parent, j);
+    const int a = pg_find(parent, i), b = pg_find(parent, j2);
     if (a != b) parent[std::max(a, b)] = std::min(a, b);
   }
   for (int c = 0; c < nScale; ++c)
@@ -696,19 +766,16 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
       freeNode.push_back(k);
     }
   const int nF = (int)freeNode.size();
-  if (nF == 0) {  // nothing to solve (and no scale column can have a row): fixed nodes are copied
-    std::memcpy(newR, R, sizeof(double) * 9 * (size_t)N);
-    std::memcpy(newt, t, sizeof(double) * 3 * (size_t)N);
-    return COSL_OK;
-  }
+  if (nF == 0) return COSL_OK;  // nothing to solve (and no scale column can have a row)
+  j.nF = nF;
   const int nG = (nScale + 5) / 6, mf = 2 * nF + nG;
   // ---- CSR lists in edge order: per free node, per scale column, per node pair
   std::vector<int> nodeOff(nF + 1, 0), colOff(nScale + 1, 0);
   for (int e = 0; e < E; ++e) {
-    const int i = id1[e], j = id2[e], c = scaleCol ? scaleCol[e] : -1;
-    if (fixed[i] && fixed[j]) continue;
+    const int i = id1[e], j2 = id2[e], c = scaleCol ? scaleCol[e] : -1;
+    if (fixed[i] && fixed[j2]) continue;
     if (!fixed[i]) ++nodeOff[freeOf[i] + 1];
-    if (!fixed[j]) ++nodeOff[freeOf[j] + 1];
+    if (!fixed[j2]) ++nodeOff[freeOf[j2] + 1];
     if (c >= 0) ++colOff[c + 1];
   }
   for (int f = 0; f < nF; ++f) nodeOff[f + 1] += nodeOff[f];
@@ -719,16 +786,17 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
   {
     std::vector<int> nf(nodeOff.begin(), nodeOff.end() - 1), cf(colOff.begin(), colOff.end() - 1);
     for (int e = 0; e < E; ++e) {
-      const int i = id1[e], j = id2[e], c = scaleCol ? scaleCol[e] : -1;
-      if (fixed[i] && fixed[j]) continue;
+      const int i = id1[e], j2 = id2[e], c = scaleCol ? scaleCol[e] : -1;
+      if (fixed[i] && fixed[j2]) continue;
       if (!fixed[i]) nodeEdges[nf[freeOf[i]]++] = e;
-      if (!fixed[j]) nodeEdges[nf[freeOf[j]]++] = e;
+      if (!fixed[j2]) nodeEdges[nf[freeOf[j2]]++] = e;
       if (c >= 0) {
         colEdges[cf[c]++] = e;
         if (!fixed[i]) scaleAdj.push_back({c / 6, freeOf[i]});
-        if (!fixed[j]) scaleAdj.push_back({c / 6, freeOf[j]});
+        if (!fixed[j2]) scaleAdj.push_back({c / 6, freeOf[j2]});
       }
-      if (!fixed[i] && !fixed[j]) pairs[{std::min(freeOf[i], freeOf[j]), std::max(freeOf[i], freeOf[j])}].push_back(e);
+      if (!fixed[i] && !fixed[j2])
+        pairs[{std::min(freeOf[i], freeOf[j2]), std::max(freeOf[i], freeOf[j2])}].push_back(e);
     }
     std::sort(scaleAdj.begin(), scaleAdj.end());
     scaleAdj.erase(std::unique(scaleAdj.begin(), scaleAdj.end()), scaleAdj.end());
@@ -744,10 +812,11 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
     link(2 * pr.first.first + 1, 2 * pr.first.second + 1);
   }
   for (const auto& sa : scaleAdj) link(2 * nF + sa.first, 2 * sa.second + 1);
-  const BaPlan P = ba_make_plan(mf, adj);
+  j.P = ba_make_plan(mf, adj);
+  const BaPlan& P = j.P;
   if (P.nb <= 0) return set_error(COSL_E_NUMERIC, "%s: planning the solve failed", fn);
   std::vector<BaTask> tasks;
-  const int nA = tile_task_order(P, tasks);
+  j.nA = tile_task_order(P, tasks);
   // ---- items: every structurally non-zero 6x6 block of the lower triangle, grouped by tile
   std::vector<int> unitPos(mf);
   for (int u = 0; u < mf; ++u) unitPos[u] = P.camBlk[u] * 64 + P.camOff[u];
@@ -782,118 +851,117 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
   std::vector<int> sc(E);
   for (int e = 0; e < E; ++e) sc[e] = scaleCol ? scaleCol[e] : -1;
   // ---- one slab: inputs (uploaded in one copy, counters included as zeros), work, outputs
-  const size_t nTilesAll = (size_t)nTiles + P.nScratch, nCnt = (size_t)P.nCounters + 2 + tasks.size();
+  const size_t nTilesAll = (size_t)nTiles + P.nScratch;
+  j.nCnt = (size_t)P.nCounters + 2 + tasks.size();
   SlabLayout L;
   auto put = [&](size_t bytes) { return L.take(std::max<size_t>(bytes, 8)); };
-  const size_t oR = put(72 * (size_t)N), ot = put(24 * (size_t)N), oeR = put(72 * (size_t)E), oet = put(24 * (size_t)E);
-  const size_t oFixed = put(N), oId1 = put(4 * (size_t)E), oId2 = put(4 * (size_t)E), oSc = put(4 * (size_t)E);
-  const size_t oFreeNode = put(4 * (size_t)nF), oFreeOf = put(4 * (size_t)N);
-  const size_t oNodeOff = put(4 * nodeOff.size()), oNodeEdges = put(4 * nodeEdges.size());
-  const size_t oColOff = put(4 * colOff.size()), oColEdges = put(4 * colEdges.size());
-  const size_t oPair = put(4 * pairEdges.size()), oUnitPos = put(4 * (size_t)mf);
-  const size_t oItems = put(sizeof(PgItem) * items.size()), oItemOff = put(4 * itemOff.size());
-  const size_t oDiag = put(4 * (size_t)nTiles), oOrder = put(4 * (size_t)mf), oBlkCam0 = put(4 * (size_t)(nb + 1));
-  const size_t oBlkRows = put(4 * (size_t)nb), oTasks = put(sizeof(BaTask) * tasks.size());
-  const size_t oBwd = put(sizeof(BaBwdEntry) * P.bwdList.size()), oSum = put(sizeof(BaSumEntry) * P.sumList.size());
-  const size_t oCnt = put(4 * nCnt);
-  const size_t inputBytes = L.bytes;
-  const size_t oRhs = put(8 * (size_t)nb * 64), oTiles = put(8 * nTilesAll * 4096);
-  const size_t oRhsS = put(8 * (size_t)std::max(1, P.nScratch) * 64), oLinv = put(8 * (size_t)nb * 4096);
-  const size_t oY = put(8 * (size_t)nb * 64), oX = put(8 * (size_t)nb * 64), oX1 = put(8 * (size_t)nb * 64);
+  PgSlab& o = j.o;
+  o.R = put(72 * (size_t)N), o.t = put(24 * (size_t)N), o.eR = put(72 * (size_t)E), o.et = put(24 * (size_t)E);
+  o.fixed = put(N), o.id1 = put(4 * (size_t)E), o.id2 = put(4 * (size_t)E), o.sc = put(4 * (size_t)E);
+  o.freeNode = put(4 * (size_t)nF), o.freeOf = put(4 * (size_t)N);
+  o.nodeOff = put(4 * nodeOff.size()), o.nodeEdges = put(4 * nodeEdges.size());
+  o.colOff = put(4 * colOff.size()), o.colEdges = put(4 * colEdges.size());
+  o.pair = put(4 * pairEdges.size()), o.unitPos = put(4 * (size_t)mf);
+  o.items = put(sizeof(PgItem) * items.size()), o.itemOff = put(4 * itemOff.size());
+  o.diag = put(4 * (size_t)nTiles), o.order = put(4 * (size_t)mf), o.blkCam0 = put(4 * (size_t)(nb + 1));
+  o.blkRows = put(4 * (size_t)nb), o.tasks = put(sizeof(BaTask) * tasks.size());
+  o.bwd = put(sizeof(BaBwdEntry) * P.bwdList.size()), o.sum = put(sizeof(BaSumEntry) * P.sumList.size());
+  o.cnt = put(4 * j.nCnt);
+  o.in = L.bytes;
+  o.rhs = put(8 * (size_t)nb * 64), o.tiles = put(8 * nTilesAll * 4096);
+  o.rhsS = put(8 * (size_t)std::max(1, P.nScratch) * 64), o.Linv = put(8 * (size_t)nb * 4096);
+  o.y = put(8 * (size_t)nb * 64), o.x = put(8 * (size_t)nb * 64), o.x1 = put(8 * (size_t)nb * 64);
   // outputs, contiguous: [newR 9N | newt 3N | scale | pivot failure | non-finite]
-  const size_t nOut = 12 * (size_t)N + nScale + 2;
-  const size_t oOut = put(8 * nOut);
-  std::vector<char> host(inputBytes, 0);
-  auto stage = [&](size_t off, const void* src, size_t bytes) {
-    if (bytes) std::memcpy(host.data() + off, src, bytes);
+  j.nOut = 12 * (size_t)N + nScale + 2;
+  o.out = put(8 * j.nOut);
+  o.bytes = L.bytes;
+  char* h = nullptr;
+  COSL_TRY(stage(o.in, &h));
+  std::memset(h, 0, o.in);
+  auto pack = [&](size_t off, const void* src, size_t bytes) {
+    if (bytes) std::memcpy(h + off, src, bytes);
   };
-  stage(oR, R, 72 * (size_t)N);
-  stage(ot, t, 24 * (size_t)N);
-  stage(oeR, eR, 72 * (size_t)E);
-  stage(oet, et, 24 * (size_t)E);
-  stage(oFixed, fixed, N);
-  stage(oId1, id1, 4 * (size_t)E);
-  stage(oId2, id2, 4 * (size_t)E);
-  stage(oSc, sc.data(), 4 * (size_t)E);
-  stage(oFreeNode, freeNode.data(), 4 * (size_t)nF);
-  stage(oFreeOf, freeOf.data(), 4 * (size_t)N);
-  stage(oNodeOff, nodeOff.data(), 4 * nodeOff.size());
-  stage(oNodeEdges, nodeEdges.data(), 4 * nodeEdges.size());
-  stage(oColOff, colOff.data(), 4 * colOff.size());
-  stage(oColEdges, colEdges.data(), 4 * colEdges.size());
-  stage(oPair, pairEdges.data(), 4 * pairEdges.size());
-  stage(oUnitPos, unitPos.data(), 4 * (size_t)mf);
-  stage(oItems, items.data(), sizeof(PgItem) * items.size());
-  stage(oItemOff, itemOff.data(), 4 * itemOff.size());
-  stage(oDiag, diagBlk.data(), 4 * (size_t)nTiles);
-  stage(oOrder, P.order.data(), 4 * (size_t)mf);
-  stage(oBlkCam0, P.blkCam0.data(), 4 * (size_t)(nb + 1));
-  stage(oBlkRows, P.blkRows.data(), 4 * (size_t)nb);
-  stage(oTasks, tasks.data(), sizeof(BaTask) * tasks.size());
-  stage(oBwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
-  stage(oSum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
-  g_pgHostMs = 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - tHost0).count();
-  // ---- device
-  COSL_CUDA(cudaSetDevice(device));
-  keep_pool(device);
-  cudaStream_t s = cudaStreamPerThread;
-  char* slab = nullptr;
-  {
-    const cudaError_t e = cudaMallocAsync(&slab, L.bytes, s);
-    if (e == cudaErrorMemoryAllocation) {
-      cudaGetLastError();
-      return set_error(COSL_E_NOMEM, "%s: device allocation of %zu bytes failed", fn, L.bytes);
-    }
-    if (e != cudaSuccess) return set_error(COSL_E_CUDA, "%s: cudaMallocAsync: %s", fn, cudaGetErrorString(e));
-  }
+  pack(o.R, R, 72 * (size_t)N);
+  pack(o.t, t, 24 * (size_t)N);
+  pack(o.eR, eR, 72 * (size_t)E);
+  pack(o.et, et, 24 * (size_t)E);
+  pack(o.fixed, fixed, N);
+  pack(o.id1, id1, 4 * (size_t)E);
+  pack(o.id2, id2, 4 * (size_t)E);
+  pack(o.sc, sc.data(), 4 * (size_t)E);
+  pack(o.freeNode, freeNode.data(), 4 * (size_t)nF);
+  pack(o.freeOf, freeOf.data(), 4 * (size_t)N);
+  pack(o.nodeOff, nodeOff.data(), 4 * nodeOff.size());
+  pack(o.nodeEdges, nodeEdges.data(), 4 * nodeEdges.size());
+  pack(o.colOff, colOff.data(), 4 * colOff.size());
+  pack(o.colEdges, colEdges.data(), 4 * colEdges.size());
+  pack(o.pair, pairEdges.data(), 4 * pairEdges.size());
+  pack(o.unitPos, unitPos.data(), 4 * (size_t)mf);
+  pack(o.items, items.data(), sizeof(PgItem) * items.size());
+  pack(o.itemOff, itemOff.data(), 4 * itemOff.size());
+  pack(o.diag, diagBlk.data(), 4 * (size_t)nTiles);
+  pack(o.order, P.order.data(), 4 * (size_t)mf);
+  pack(o.blkCam0, P.blkCam0.data(), 4 * (size_t)(nb + 1));
+  pack(o.blkRows, P.blkRows.data(), 4 * (size_t)nb);
+  pack(o.tasks, tasks.data(), sizeof(BaTask) * tasks.size());
+  pack(o.bwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
+  pack(o.sum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
+  return COSL_OK;
+}
+
+// The solve (j.nF > 0) on `s` into `slab` (j.o.bytes): the packed inputs in one copy, assembly and tile solve
+// twice, pg_finish, and the output region (j.nOut doubles) in one copy into hostOut.
+int pg_enqueue(const char* fn, const PgJob& j, char* slab, const char* staged, double* hostOut, int device,
+               cudaStream_t s) {
+  const PgSlab& o = j.o;
+  const int N = j.N, nScale = j.nScale, nb = j.P.nb;
   auto at = [&](size_t off) { return slab + off; };
   PgDev d;
-  d.R = reinterpret_cast<const double*>(at(oR));
-  d.t = reinterpret_cast<const double*>(at(ot));
-  d.eR = reinterpret_cast<const double*>(at(oeR));
-  d.et = reinterpret_cast<const double*>(at(oet));
-  d.fixed = reinterpret_cast<const unsigned char*>(at(oFixed));
-  d.id1 = reinterpret_cast<const int*>(at(oId1));
-  d.id2 = reinterpret_cast<const int*>(at(oId2));
-  d.scaleCol = reinterpret_cast<const int*>(at(oSc));
-  d.freeNode = reinterpret_cast<const int*>(at(oFreeNode));
-  d.freeOf = reinterpret_cast<const int*>(at(oFreeOf));
-  d.nodeOff = reinterpret_cast<const int*>(at(oNodeOff));
-  d.nodeEdges = reinterpret_cast<const int*>(at(oNodeEdges));
-  d.colOff = reinterpret_cast<const int*>(at(oColOff));
-  d.colEdges = reinterpret_cast<const int*>(at(oColEdges));
-  d.pairEdges = reinterpret_cast<const int*>(at(oPair));
-  d.unitPos = reinterpret_cast<const int*>(at(oUnitPos));
-  d.items = reinterpret_cast<const PgItem*>(at(oItems));
-  d.itemOff = reinterpret_cast<const int*>(at(oItemOff));
-  d.diagBlk = reinterpret_cast<const int*>(at(oDiag));
-  d.order = reinterpret_cast<const int*>(at(oOrder));
-  d.blkCam0 = reinterpret_cast<const int*>(at(oBlkCam0));
-  d.blkRows = reinterpret_cast<const int*>(at(oBlkRows));
-  d.nF = nF;
+  d.R = reinterpret_cast<const double*>(at(o.R));
+  d.t = reinterpret_cast<const double*>(at(o.t));
+  d.eR = reinterpret_cast<const double*>(at(o.eR));
+  d.et = reinterpret_cast<const double*>(at(o.et));
+  d.fixed = reinterpret_cast<const unsigned char*>(at(o.fixed));
+  d.id1 = reinterpret_cast<const int*>(at(o.id1));
+  d.id2 = reinterpret_cast<const int*>(at(o.id2));
+  d.scaleCol = reinterpret_cast<const int*>(at(o.sc));
+  d.freeNode = reinterpret_cast<const int*>(at(o.freeNode));
+  d.freeOf = reinterpret_cast<const int*>(at(o.freeOf));
+  d.nodeOff = reinterpret_cast<const int*>(at(o.nodeOff));
+  d.nodeEdges = reinterpret_cast<const int*>(at(o.nodeEdges));
+  d.colOff = reinterpret_cast<const int*>(at(o.colOff));
+  d.colEdges = reinterpret_cast<const int*>(at(o.colEdges));
+  d.pairEdges = reinterpret_cast<const int*>(at(o.pair));
+  d.unitPos = reinterpret_cast<const int*>(at(o.unitPos));
+  d.items = reinterpret_cast<const PgItem*>(at(o.items));
+  d.itemOff = reinterpret_cast<const int*>(at(o.itemOff));
+  d.diagBlk = reinterpret_cast<const int*>(at(o.diag));
+  d.order = reinterpret_cast<const int*>(at(o.order));
+  d.blkCam0 = reinterpret_cast<const int*>(at(o.blkCam0));
+  d.blkRows = reinterpret_cast<const int*>(at(o.blkRows));
+  d.nF = j.nF;
   d.nScale = nScale;
-  double* out = reinterpret_cast<double*>(at(oOut));
+  double* out = reinterpret_cast<double*>(at(o.out));
   TileSolveBufs b;
-  b.rhs = reinterpret_cast<double*>(at(oRhs));
-  b.tiles = reinterpret_cast<double*>(at(oTiles));
-  b.rhsS = reinterpret_cast<double*>(at(oRhsS));
-  b.Linv = reinterpret_cast<double*>(at(oLinv));
-  b.y = reinterpret_cast<double*>(at(oY));
-  b.x = reinterpret_cast<double*>(at(oX));
-  b.cnt = reinterpret_cast<int*>(at(oCnt));
-  b.tasks = reinterpret_cast<const BaTask*>(at(oTasks));
-  b.bwd = reinterpret_cast<const BaBwdEntry*>(at(oBwd));
-  b.sum = reinterpret_cast<const BaSumEntry*>(at(oSum));
+  b.rhs = reinterpret_cast<double*>(at(o.rhs));
+  b.tiles = reinterpret_cast<double*>(at(o.tiles));
+  b.rhsS = reinterpret_cast<double*>(at(o.rhsS));
+  b.Linv = reinterpret_cast<double*>(at(o.Linv));
+  b.y = reinterpret_cast<double*>(at(o.y));
+  b.x = reinterpret_cast<double*>(at(o.x));
+  b.cnt = reinterpret_cast<int*>(at(o.cnt));
+  b.tasks = reinterpret_cast<const BaTask*>(at(o.tasks));
+  b.bwd = reinterpret_cast<const BaBwdEntry*>(at(o.bwd));
+  b.sum = reinterpret_cast<const BaSumEntry*>(at(o.sum));
   b.blkRows = d.blkRows;
   b.fail = out + 12 * (size_t)N + nScale;
-  double* x1 = reinterpret_cast<double*>(at(oX1));
-  std::vector<double> hout(nOut);
+  double* x1 = reinterpret_cast<double*>(at(o.x1));
   int rc = COSL_OK;
   auto cuda_step = [&](cudaError_t e, const char* what) {
     if (rc == COSL_OK && e != cudaSuccess)
       rc = set_error(COSL_E_CUDA, "%s: %s: %s", fn, what, cudaGetErrorString(e));
   };
-  cuda_step(cudaMemcpyAsync(slab, host.data(), inputBytes, cudaMemcpyHostToDevice, s), "H2D");
+  cuda_step(cudaMemcpyAsync(slab, staged, o.in, cudaMemcpyHostToDevice, s), "H2D");
   cuda_step(cudaMemsetAsync(b.fail, 0, 16, s), "memset");
   // Normal equations square the condition number (chains of n free nodes: ~n^2), so the solve is
   // followed by one refinement step: assemble again with the residual A^T (b - A x1) as rhs, solve,
@@ -901,12 +969,12 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
   for (int pass = 0; pass < 2 && rc == COSL_OK; ++pass) {
     if (pass == 1) {
       cuda_step(cudaMemcpyAsync(x1, b.x, 8 * (size_t)nb * 64, cudaMemcpyDeviceToDevice, s), "D2D");
-      cuda_step(cudaMemsetAsync(b.cnt, 0, 4 * nCnt, s), "memset");
+      cuda_step(cudaMemsetAsync(b.cnt, 0, 4 * j.nCnt, s), "memset");
     }
     if (rc != COSL_OK) break;
-    COSL_LAUNCH(pg_assemble, nTiles, 256, 0, s, d, pass ? x1 : nullptr, b.tiles, b.rhs);
+    COSL_LAUNCH(pg_assemble, j.P.nTiles, 256, 0, s, d, pass ? x1 : nullptr, b.tiles, b.rhs);
     cuda_step(cudaGetLastError(), "pg_assemble");
-    if (rc == COSL_OK) rc = tile_solve_launch(P, nA, b, device, s);
+    if (rc == COSL_OK) rc = tile_solve_launch(j.P, j.nA, b, device, s);
   }
   if (rc == COSL_OK) {
     const int nThr = std::max(N, nScale);
@@ -914,15 +982,313 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
                 out + 12 * (size_t)N, out + 12 * (size_t)N + nScale + 1);
     cuda_step(cudaGetLastError(), "pg_finish");
   }
-  cuda_step(cudaMemcpyAsync(hout.data(), out, 8 * nOut, cudaMemcpyDeviceToHost, s), "D2H");
-  cuda_step(cudaStreamSynchronize(s), "sync");
-  cudaFreeAsync(slab, s);
-  if (rc != COSL_OK) return rc;
-  if (hout[12 * (size_t)N + nScale] != 0.0)
+  cuda_step(cudaMemcpyAsync(hostOut, out, 8 * j.nOut, cudaMemcpyDeviceToHost, s), "D2H");
+  return rc;
+}
+
+// The flags pg_finish and the tile solve leave in the output region, then newR, newt and the scales.
+int pg_result(const char* fn, int N, int nScale, const double* out, double* newR, double* newt, double* scale) {
+  if (out[12 * (size_t)N + nScale] != 0.0)
     return set_error(COSL_E_NUMERIC, "%s: non-positive pivot in the normal equations", fn);
-  if (hout[12 * (size_t)N + nScale + 1] != 0.0) return set_error(COSL_E_NUMERIC, "%s: non-finite result", fn);
-  std::memcpy(newR, hout.data(), sizeof(double) * 9 * (size_t)N);
-  std::memcpy(newt, hout.data() + 9 * (size_t)N, sizeof(double) * 3 * (size_t)N);
-  if (nScale) std::memcpy(scale, hout.data() + 12 * (size_t)N, sizeof(double) * nScale);
+  if (out[12 * (size_t)N + nScale + 1] != 0.0) return set_error(COSL_E_NUMERIC, "%s: non-finite result", fn);
+  std::memcpy(newR, out, sizeof(double) * 9 * (size_t)N);
+  std::memcpy(newt, out + 9 * (size_t)N, sizeof(double) * 3 * (size_t)N);
+  if (nScale) std::memcpy(scale, out + 12 * (size_t)N, sizeof(double) * nScale);
   return COSL_OK;
 }
+
+}  // namespace
+}  // namespace coslam
+
+using namespace coslam;
+
+extern "C" int cosl_posegraph_spread_chains(int nChains, const int* chainOff, const uint8_t* fixed,
+                                            const double* R, const double* t, const double* eR,
+                                            const double* et, double* newR, double* newt, int device) {
+  const char* fn = "cosl_posegraph_spread_chains";
+  const double* outs[2] = {newR, newt};
+  ChainJob j;
+  COSL_TRY(chain_prepare(fn, nChains, chainOff, fixed, R, t, eR, et, outs, StageFn(), j));
+  if (j.N == 0) return COSL_OK;
+  COSL_CUDA(cudaSetDevice(device));
+  keep_pool(device);
+  cudaStream_t s = cudaStreamPerThread;
+  char* slab = nullptr;
+  COSL_CUDA(cudaMallocAsync(&slab, j.bytes, s));
+  int status = 0;
+  int rc = chain_enqueue(fn, j, slab, s, nullptr, newR, newt, &status);
+  const cudaError_t e = cudaStreamSynchronize(s);
+  if (rc == COSL_OK && e != cudaSuccess) rc = set_error(COSL_E_CUDA, "%s: sync: %s", fn, cudaGetErrorString(e));
+  cudaFreeAsync(slab, s);
+  if (rc != COSL_OK) return rc;
+  return chain_status(fn, status);
+}
+
+extern "C" double cosl_posegraph_last_host_ms(void) { return g_pgHostMs; }
+
+extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const double* R, const double* t,
+                                    int nEdges, const int* id1, const int* id2, const double* eR,
+                                    const double* et, const int* scaleCol, int nScale, double* newR,
+                                    double* newt, double* scale, int device) {
+  const auto tHost0 = std::chrono::steady_clock::now();
+  g_pgHostMs = 0.0;
+  const char* fn = "cosl_posegraph_solve";
+  const void* outs[3] = {newR, newt, scale};
+  std::vector<char> host;
+  auto stage = [&](size_t bytes, char** buf) {
+    host.resize(bytes);
+    *buf = host.data();
+    return (int)COSL_OK;
+  };
+  PgJob j;
+  COSL_TRY(pg_prepare(fn, nNodes, fixed, R, t, nEdges, id1, id2, eR, et, scaleCol, nScale, outs, stage, j));
+  const int N = j.N;
+  if (j.nF == 0) {  // fixed nodes are copied
+    std::memcpy(newR, R, sizeof(double) * 9 * (size_t)N);
+    std::memcpy(newt, t, sizeof(double) * 3 * (size_t)N);
+    return COSL_OK;
+  }
+  g_pgHostMs = 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - tHost0).count();
+  // ---- device
+  COSL_CUDA(cudaSetDevice(device));
+  keep_pool(device);
+  cudaStream_t s = cudaStreamPerThread;
+  char* slab = nullptr;
+  {
+    const cudaError_t e = cudaMallocAsync(&slab, j.o.bytes, s);
+    if (e == cudaErrorMemoryAllocation) {
+      cudaGetLastError();
+      return set_error(COSL_E_NOMEM, "%s: device allocation of %zu bytes failed", fn, j.o.bytes);
+    }
+    if (e != cudaSuccess) return set_error(COSL_E_CUDA, "%s: cudaMallocAsync: %s", fn, cudaGetErrorString(e));
+  }
+  std::vector<double> hout(j.nOut);
+  int rc = pg_enqueue(fn, j, slab, host.data(), hout.data(), device, s);
+  const cudaError_t e = cudaStreamSynchronize(s);
+  if (rc == COSL_OK && e != cudaSuccess) rc = set_error(COSL_E_CUDA, "%s: sync: %s", fn, cudaGetErrorString(e));
+  cudaFreeAsync(slab, s);
+  if (rc != COSL_OK) return rc;
+  return pg_result(fn, N, nScale, hout.data(), newR, newt, scale);
+}
+
+// A pose-graph solver handle.  One request in flight at a time, of either kind; the device slab and the
+// pinned staging buffers serve both kinds and grow when a request does not fit.
+struct cosl_posegraph_solver {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  cudaEvent_t evStart = nullptr, evDone = nullptr;
+  char* slab = nullptr;  // from the device's stream-ordered pool, on `stream`
+  char* h_in = nullptr;  // pinned: the packed inputs
+  char* h_out = nullptr; // pinned: the output region of the slab
+  size_t slabBytes = 0, inBytes = 0, outBytes = 0;
+  bool inFlight = false, chains = false;  // the request in flight: a chain spread or a general solve
+  int N = 0, nScale = 0;                  // its nodes (0: nothing to write) and scale columns
+};
+
+namespace {
+
+void free_pg_solver(cosl_posegraph_solver* s) {
+  cudaSetDevice(s->device);
+  if (s->stream) {
+    cudaStreamSynchronize(s->stream);  // a request in flight reads and writes the buffers below
+    if (s->slab) cudaFreeAsync(s->slab, s->stream);
+    cudaStreamSynchronize(s->stream);
+  }
+  if (s->evStart) cudaEventDestroy(s->evStart);
+  if (s->evDone) cudaEventDestroy(s->evDone);
+  if (s->h_in) cudaFreeHost(s->h_in);
+  if (s->h_out) cudaFreeHost(s->h_out);
+  if (s->stream) cudaStreamDestroy(s->stream);
+  delete s;
+}
+
+// Grows a pinned buffer to `need` bytes.  Only called with nothing in flight, so no copy reads the old one.
+int grow_pinned(const char* fn, char** buf, size_t* cap, size_t need) {
+  if (need <= *cap) return COSL_OK;
+  if (*buf) cudaFreeHost(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  const cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(buf), need, cudaHostAllocPortable);
+  if (e != cudaSuccess) {
+    *buf = nullptr;
+    cudaGetLastError();
+    return set_error(e == cudaErrorMemoryAllocation ? COSL_E_NOMEM : COSL_E_CUDA,
+                     "%s: pinned allocation of %zu bytes failed: %s", fn, need, cudaGetErrorString(e));
+  }
+  *cap = need;
+  return COSL_OK;
+}
+
+// Grows the device slab in stream order: the old slab goes back to the pool behind the work already on
+// the handle's stream, and the new one comes out of it without a device synchronisation.
+int grow_slab(const char* fn, cosl_posegraph_solver* s, size_t need) {
+  if (need <= s->slabBytes) return COSL_OK;
+  if (s->slab) cudaFreeAsync(s->slab, s->stream);
+  s->slab = nullptr;
+  s->slabBytes = 0;
+  const cudaError_t e = cudaMallocAsync(&s->slab, need, s->stream);
+  if (e != cudaSuccess) {
+    s->slab = nullptr;
+    cudaGetLastError();
+    return set_error(e == cudaErrorMemoryAllocation ? COSL_E_NOMEM : COSL_E_CUDA,
+                     "%s: device allocation of %zu bytes failed: %s", fn, need, cudaGetErrorString(e));
+  }
+  s->slabBytes = need;
+  return COSL_OK;
+}
+
+StageFn stage_pinned(const char* fn, cosl_posegraph_solver* s) {
+  return [fn, s](size_t bytes, char** buf) {
+    COSL_TRY(grow_pinned(fn, &s->h_in, &s->inBytes, bytes));
+    *buf = s->h_in;
+    return (int)COSL_OK;
+  };
+}
+
+// Records the start event, runs `enqueue`, records the end event.  On a failure the stream is drained (a copy
+// that was enqueued may still read the staging buffer) and nothing is in flight.
+template <class F>
+int submit_timed(cosl_posegraph_solver* s, F enqueue) {
+  int rc = COSL_OK;
+  cudaError_t e = cudaEventRecord(s->evStart, s->stream);
+  if (e == cudaSuccess) {
+    rc = enqueue();
+    if (rc == COSL_OK) e = cudaEventRecord(s->evDone, s->stream);
+  }
+  if (rc == COSL_OK && e != cudaSuccess)
+    rc = set_error(COSL_E_CUDA, "cosl_posegraph_solver: cudaEventRecord: %s", cudaGetErrorString(e));
+  if (rc != COSL_OK) cudaStreamSynchronize(s->stream);
+  else s->inFlight = true;
+  return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cosl_posegraph_solver_create(int device, cosl_posegraph_solver** out) {
+  if (!out || device < 0) return set_error(COSL_E_INVALID, "cosl_posegraph_solver_create: bad argument");
+  *out = nullptr;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device >= ndev)
+    return set_error(COSL_E_CUDA, "CUDA device %d not available", device);
+  cosl_posegraph_solver* s = new (std::nothrow) cosl_posegraph_solver;
+  if (!s) return set_error(COSL_E_NOMEM, "cosl_posegraph_solver_create: out of host memory");
+  s->device = device;
+  auto init = [&]() {
+    COSL_CUDA(cudaSetDevice(device));
+    keep_pool(device);
+    COSL_CUDA(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
+    COSL_CUDA(cudaEventCreate(&s->evStart));
+    COSL_CUDA(cudaEventCreate(&s->evDone));
+    return (int)COSL_OK;
+  };
+  const int rc = init();
+  if (rc != COSL_OK) {
+    free_pg_solver(s);
+    return rc;
+  }
+  *out = s;
+  return COSL_OK;
+}
+
+int cosl_posegraph_solver_destroy(cosl_posegraph_solver* s) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
+  free_pg_solver(s);
+  return COSL_OK;
+}
+
+int cosl_posegraph_solver_submit_chains(cosl_posegraph_solver* s, int nChains, const int* chainOff,
+                                        const uint8_t* fixed, const double* R, const double* t,
+                                        const double* eR, const double* et) {
+  const char* fn = "cosl_posegraph_solver_submit_chains";
+  if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
+  if (s->inFlight) return set_error(COSL_E_STATE, "%s: a submitted solve is not collected yet", fn);
+  COSL_CUDA(cudaSetDevice(s->device));
+  ChainJob j;
+  COSL_TRY(chain_prepare(fn, nChains, chainOff, fixed, R, t, eR, et, nullptr, stage_pinned(fn, s), j));
+  if (j.N > 0) {
+    COSL_TRY(grow_pinned(fn, &s->h_out, &s->outBytes, chain_out_bytes(j.N)));
+    COSL_TRY(grow_slab(fn, s, j.bytes));
+  }
+  s->chains = true;
+  s->N = j.N;
+  s->nScale = 0;
+  return submit_timed(s, [&]() {
+    return j.N > 0 ? chain_enqueue(fn, j, s->slab, s->stream, s->h_out, nullptr, nullptr, nullptr) : (int)COSL_OK;
+  });
+}
+
+int cosl_posegraph_solver_submit(cosl_posegraph_solver* s, int nNodes, const uint8_t* fixed, const double* R,
+                                 const double* t, int nEdges, const int* id1, const int* id2, const double* eR,
+                                 const double* et, const int* scaleCol, int nScale) {
+  const char* fn = "cosl_posegraph_solver_submit";
+  if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
+  if (s->inFlight) return set_error(COSL_E_STATE, "%s: a submitted solve is not collected yet", fn);
+  COSL_CUDA(cudaSetDevice(s->device));
+  PgJob j;
+  COSL_TRY(pg_prepare(fn, nNodes, fixed, R, t, nEdges, id1, id2, eR, et, scaleCol, nScale, nullptr,
+                      stage_pinned(fn, s), j));
+  const int N = j.N;
+  COSL_TRY(grow_pinned(fn, &s->h_out, &s->outBytes, 8 * (12 * (size_t)N + nScale + 2)));
+  if (j.nF == 0) {  // answered on the host, as the synchronous call does: the fixed nodes are copied
+    double* out = reinterpret_cast<double*>(s->h_out);
+    std::memcpy(out, R, sizeof(double) * 9 * (size_t)N);
+    std::memcpy(out + 9 * (size_t)N, t, sizeof(double) * 3 * (size_t)N);
+    out[12 * (size_t)N] = out[12 * (size_t)N + 1] = 0.0;  // no failure flags (nScale is 0)
+  } else {
+    COSL_TRY(grow_slab(fn, s, j.o.bytes));
+  }
+  s->chains = false;
+  s->N = N;
+  s->nScale = nScale;
+  return submit_timed(s, [&]() {
+    return j.nF > 0 ? pg_enqueue(fn, j, s->slab, s->h_in, reinterpret_cast<double*>(s->h_out), s->device, s->stream)
+                    : (int)COSL_OK;
+  });
+}
+
+int cosl_posegraph_solver_query(cosl_posegraph_solver* s, int* done) {
+  if (!s || !done) return set_error(COSL_E_INVALID, "cosl_posegraph_solver_query: null argument");
+  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_posegraph_solver_query: nothing submitted");
+  COSL_CUDA(cudaSetDevice(s->device));
+  const cudaError_t e = cudaEventQuery(s->evDone);
+  if (e == cudaErrorNotReady) {
+    *done = 0;
+    return COSL_OK;
+  }
+  COSL_CUDA(e);
+  *done = 1;
+  return COSL_OK;
+}
+
+int cosl_posegraph_solver_collect(cosl_posegraph_solver* s, double* newR, double* newt, double* scale,
+                                  double* device_ms) {
+  const char* fn = "cosl_posegraph_solver_collect";
+  if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
+  if (!s->inFlight) return set_error(COSL_E_STATE, "%s: nothing submitted", fn);
+  if ((s->N > 0 && (!newR || !newt)) || (s->nScale > 0 && !scale))
+    return set_error(COSL_E_INVALID, "%s: null output array", fn);
+  COSL_CUDA(cudaSetDevice(s->device));
+  s->inFlight = false;
+  COSL_CUDA(cudaEventSynchronize(s->evDone));
+  if (device_ms) {
+    float ms = 0.f;
+    COSL_CUDA(cudaEventElapsedTime(&ms, s->evStart, s->evDone));
+    *device_ms = ms;
+  }
+  const int N = s->N;
+  if (!s->chains) return pg_result(fn, N, s->nScale, reinterpret_cast<const double*>(s->h_out), newR, newt, scale);
+  if (N == 0) return COSL_OK;
+  const double* out = reinterpret_cast<const double*>(s->h_out);
+  int status = 0;
+  std::memcpy(&status, out + 12 * (size_t)N, sizeof(int));
+  COSL_TRY(chain_status(fn, status));
+  std::memcpy(newR, out, sizeof(double) * 9 * (size_t)N);
+  std::memcpy(newt, out + 9 * (size_t)N, sizeof(double) * 3 * (size_t)N);
+  return COSL_OK;
+}
+
+void* cosl_posegraph_solver_stream(cosl_posegraph_solver* s) { return s ? (void*)s->stream : nullptr; }
+
+}  // extern "C"

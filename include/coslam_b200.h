@@ -580,6 +580,60 @@ int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const double* R, cons
  * cosl_posegraph_solve call. */
 double cosl_posegraph_last_host_ms(void);
 
+/* ================= pose-graph solver handle =================
+ * The two calls above without blocking the calling thread.  It serves the reference's two pose-graph call
+ * sites, both run with the BA lock held:
+ *   - RobustBundleRTS::output (app/SL_CoSLAMRobustBA.cpp:273-316) after every local BA, and again after a
+ *     camera-group merge (app/SL_MergeCameraGroup.cpp:1107): submit_chains after the key-pose write-back
+ *     (:279-296), the map-point write-back (:297-310) and other host work, then collect and the non-key
+ *     write-back of updateNonKeyCameraPoses;
+ *   - MergeCameraGroup::recomputeKeyCamPoses (app/SL_MergeCameraGroup.cpp:1083-1086): submit, collect.
+ * A handle owns a non-blocking stream, two timing events, a device buffer from the device's stream-ordered
+ * memory pool and pinned buffers for the inputs and the results.  create makes the stream and the events;
+ * without a usable device it gives COSL_E_CUDA (there is no CPU path).  The buffers are sized by the first
+ * submit and kept while later requests fit; a request that does not fit grows them.  A submit that fits
+ * allocates nothing; one that grows them may wait for the device (cudaHostAlloc / cudaFreeHost).
+ *
+ * submit_chains takes the arguments of cosl_posegraph_spread_chains, submit those of cosl_posegraph_solve,
+ * less the outputs and the device.  Each runs the checks and host work of its synchronous call on the
+ * calling thread (for submit: validation, numbering, the plan, the CSR lists) and returns that call's code
+ * and message for a malformed request (COSL_E_INVALID, COSL_E_NUMERIC when planning fails, COSL_E_NOMEM);
+ * the handle stays usable.  It packs the inputs into pinned memory, so the caller may reuse its arrays when
+ * it returns, enqueues one host-to-device copy, the synchronous call's kernels with the same launch shapes
+ * and one device-to-host copy into pinned memory on the handle's stream, and returns without waiting for
+ * the device.  A request the synchronous call answers without the device (a general graph without free
+ * nodes, an empty chain table) is in flight all the same, and its collect writes what that call writes
+ * (copies of the fixed nodes; nothing).
+ *
+ * query sets *done = 1 once the request has finished, without waiting.  collect waits for it and writes
+ * newR[9N], newt[3N] and, for a general solve, scale[nScale] (nullable when nScale == 0; newR / newt are
+ * nullable when N == 0) exactly as the synchronous call does for the same inputs, bit for bit.  It returns
+ * the errors only the device detects with the synchronous call's code and message: COSL_E_INVALID for a
+ * chain without a fixed node, COSL_E_NUMERIC for a non-positive pivot or a non-finite result; then nothing
+ * is written.  *device_ms (nullable) is the device time of the copies and kernels, from CUDA events.
+ *
+ * One request may be in flight per handle, of either kind: a second submit gives COSL_E_STATE, and so do
+ * query and collect with nothing in flight.  destroy waits for a request in flight.  A handle is not
+ * re-entrant; different handles, on any threads and devices, share no lock.  Every call makes the handle's
+ * device current on the calling thread.  The synchronous calls keep their own per-call buffers and
+ * cudaStreamPerThread: threads that call them at the same time do not take turns. */
+typedef struct cosl_posegraph_solver cosl_posegraph_solver;
+int cosl_posegraph_solver_create(int device, cosl_posegraph_solver** out);
+int cosl_posegraph_solver_destroy(cosl_posegraph_solver* s);
+int cosl_posegraph_solver_submit_chains(cosl_posegraph_solver* s, int nChains, const int* chainOff,
+                                        const uint8_t* fixed, const double* R, const double* t,
+                                        const double* eR, const double* et);
+int cosl_posegraph_solver_submit(cosl_posegraph_solver* s, int nNodes, const uint8_t* fixed,
+                                 const double* R, const double* t, int nEdges, const int* id1,
+                                 const int* id2, const double* eR, const double* et,
+                                 const int* scaleCol, int nScale);
+int cosl_posegraph_solver_query(cosl_posegraph_solver* s, int* done);
+int cosl_posegraph_solver_collect(cosl_posegraph_solver* s, double* newR, double* newt,
+                                  double* scale, double* device_ms);
+/* CUDA stream (cudaStream_t as void*) the handle's requests run on; work enqueued there after a submit
+ * runs after that request. */
+void* cosl_posegraph_solver_stream(cosl_posegraph_solver* s);
+
 #ifdef __cplusplus
 }
 #endif
