@@ -23,6 +23,7 @@
 // The second half of the file solves GENERAL graphs with shared unknown scales (cosl_posegraph_solve,
 // the camera-group merge): normal equations on the BA's tile Cholesky, see the comment above PgItem.
 #include <algorithm>
+#include <cfloat>
 #include <chrono>
 #include <cmath>
 #include <functional>
@@ -117,6 +118,50 @@ __device__ void nearest_rotation(const double* M, double* Rout) {
     const double inv = s > 0 ? 1.0 / s : 0.0;
 #pragma unroll
     for (int i = 0; i < 3; ++i) U[3 * i + j] = A[3 * i + j] * inv;
+  }
+  // A singular value that is zero or at roundoff level next to the largest (M of rank < 3) leaves its column
+  // of U zero, or -- when the Jacobi sweeps cannot orthogonalise a vanishing column (its squared norm falls
+  // under the 1e-300 floor of `rel`) -- parallel to another one, and Q below would not be orthogonal.  Such
+  // a direction does not enter ||R - M|| beyond roundoff, so U is completed to a right-handed orthonormal
+  // basis instead: any completion is a nearest rotation, and det(U) = det(W) = 1.  Outputs with every
+  // singular value above 16 eps of the largest keep the plain path.
+  // (Every index below is a constant after unrolling: U stays in registers.)
+  const double sTiny = 16.0 * DBL_EPSILON * fmax(S[0], fmax(S[1], S[2]));
+  bool zero[3] = {S[0] <= sTiny, S[1] <= sTiny, S[2] <= sTiny};
+  const int nZero = zero[0] + zero[1] + zero[2];
+  if (nZero == 3) {
+#pragma unroll
+    for (int i = 0; i < 9; ++i) U[i] = W[i];
+  } else if (nZero > 0) {
+    if (nZero == 2) {  // a unit vector orthogonal to the remaining column u, into the first zero column
+      double u[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) u[i] = !zero[0] ? U[3 * i] : (!zero[1] ? U[3 * i + 1] : U[3 * i + 2]);
+      // the coordinate axis least aligned with u, minus its component along u
+      const int m = (fabs(u[0]) <= fabs(u[1]) && fabs(u[0]) <= fabs(u[2])) ? 0 : (fabs(u[1]) <= fabs(u[2]) ? 1 : 2);
+      const double um = m == 0 ? u[0] : (m == 1 ? u[1] : u[2]);
+      double v[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) v[i] = (i == m ? 1.0 : 0.0) - um * u[i];
+      const double inv = 1.0 / sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+      const int z = zero[0] ? 0 : 1;
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (j == z) {
+#pragma unroll
+          for (int i = 0; i < 3; ++i) U[3 * i + j] = v[i] * inv;
+          zero[j] = false;  // the cross product below fills the last one
+        }
+    }
+    // the zero column z = (column z+1) x (column z+2): det(U) = +1
+#pragma unroll
+    for (int z = 0; z < 3; ++z)
+      if (zero[z]) {
+        const int p = (z + 1) % 3, q = (z + 2) % 3;
+        U[z] = U[3 + p] * U[6 + q] - U[6 + p] * U[3 + q];
+        U[3 + z] = U[6 + p] * U[q] - U[p] * U[6 + q];
+        U[6 + z] = U[p] * U[3 + q] - U[3 + p] * U[q];
+      }
   }
   double Q[9];
 #pragma unroll
