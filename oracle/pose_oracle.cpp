@@ -16,7 +16,8 @@
  *   weighted_lm        intraCamWeightedLMProc       :475-549
  *   orc_pose_intracam  intraCamEstimate             :626-709
  * Choices: matInv(6) = Gauss-Jordan with partial pivoting; R_tmp/t_tmp (read uninitialised by the
- * reference when the very first LM steps all fail, :540-543) start at R0/t0.
+ * reference when the very first LM steps all fail, :540-543) start at R0/t0, and so do R_opt/t_opt
+ * (never written by the reference when maxIterRW = 0 or maxIterLM = 0).
  *
  * Compiled with -ffp-contract=off so the forward differences (eps = 1e-8) see the same roundings
  * as the CUDA kernel, which uses explicit non-fused fp64 operations for them.
@@ -252,6 +253,10 @@ extern "C" int orc_pose_intracam(const double K[9], const double R0[9], const do
   double R[9], t[3];
   std::memcpy(R, R0, sizeof(R));
   std::memcpy(t, t0, sizeof(t));
+  // the reference leaves R_opt / t_opt unwritten with maxIterRW = 0 and, with maxIterLM = 0, reads them
+  // back as the next round's pose; like the kernel, they start at R0 / t0
+  std::memcpy(R_opt, R0, sizeof(R));
+  std::memcpy(t_opt, t0, sizeof(t));
   bool ret = true;
   int k = 0;
   opt->errRW = -1;
