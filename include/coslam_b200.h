@@ -390,17 +390,21 @@ void* cosl_pose_solver_stream(cosl_pose_solver* s);
 /* Flat form of the arguments of
  *   bundleAdjustRobust(nCamsCon, Ks, Rs, Ts, nPtsCon, pts, meas, maxErr, maxIter, nInnerMaxIter)
  * (LibVisualSLAM geometry/SL_BundleAdjust.h; call app/SL_CoSLAMRobustBA.cpp:174-175).
- * Observations are CSR by point: point i owns obs [ptr[i], ptr[i+1]), sorted by camera index,
- * exactly the order of vector<vector<Meas2D>> built at app/SL_CoSLAMRobustBA.cpp:109-165.
- * ptr[0] = 0, and a camera observes a point at most once (as sba's vmask); a problem with a
- * repeated (point, camera) pair is refused with COSL_E_INVALID. */
+ * Observations are CSR by point: point i owns obs [ptr[i], ptr[i+1]), usually sorted by camera
+ * index, the order of vector<vector<Meas2D>> built at app/SL_CoSLAMRobustBA.cpp:109-165; any
+ * other order gives the same solution up to the order of the device's floating-point sums.
+ * ptr[0] = 0, and a point may have no observation (it is left unchanged).  Moreover,
+ * a camera observes a point at most once (as sba's vmask): a problem with a repeated
+ * (point, camera) pair is refused with COSL_E_INVALID. */
 typedef struct cosl_ba_problem {
   int m;              /* cameras (poses)                                   */
   int n;              /* points                                            */
   int64_t nobs;       /* observations                                      */
   int m_con;          /* first m_con cameras fixed (nCamsCon)              */
   int n_con;          /* first n_con points fixed  (nPtsCon)               */
-  double* K;          /* [m][9] row-major intrinsics, read only            */
+  double* K;          /* [m][9] row-major intrinsics [fx s cx; 0 fy cy; 0 0 1], read only:
+                         K[3], K[6], K[7] are taken as 0 and K[8] as 1 (BundleRTS packs
+                         them so), only K[0], K[1], K[2], K[4], K[5] are read          */
   double* R;          /* [m][9] row-major, x_cam = R X + t; updated in place */
   double* t;          /* [m][3] updated in place                           */
   double* X;          /* [n][3] updated in place                           */

@@ -10,6 +10,24 @@ from coslam_b200 import synth
 from coslam_b200.ctypes_defs import COSL_KLT_COMPAT_ITER5, KltConfig
 
 
+def ba_same_decisions(want, got, prob):
+    """Two BA solves of `prob` (each (info, downloaded problem)) took the same decisions: info[5..10]
+    (iterations, stop, nfev, njev, nlss, total trials) and [13] (outliers) equal; the solutions equal up to
+    the order of the device's atomic sums; fixed parameters untouched; the second reports its device time."""
+    (iw, pw), (ig, pg) = want, got
+    assert np.array_equal(iw[5:11], ig[5:11]), (iw[:14], ig[:14])
+    assert iw[13] == ig[13]
+    assert np.array_equal(pw.outlier, pg.outlier)
+    assert abs(iw[12] - ig[12]) <= 1e-9 * iw[12] + 1e-12
+    assert np.abs(pw.R - pg.R).max() < 1e-9 and np.abs(pw.t - pg.t).max() < 1e-9
+    if prob.n:
+        assert np.abs(pw.X - pg.X).max() < 1e-8
+    assert np.array_equal(pg.R[:prob.m_con], prob.R[:prob.m_con])
+    assert np.array_equal(pg.t[:prob.m_con], prob.t[:prob.m_con])
+    assert np.array_equal(pg.X[:prob.n_con], prob.X[:prob.n_con])
+    assert ig[11] > 0
+
+
 def live_cfg(gain=True, min_corner=3000.0):
     c = KltConfig.coslam_live(with_gain=gain)
     c.minCornerness = min_corner

@@ -14,7 +14,7 @@ import pytest
 
 from coslam_b200 import synth
 from coslam_b200.ctypes_defs import BaOptions
-from helpers import live_cfg, seq
+from helpers import ba_same_decisions, live_cfg, seq
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 COSL_E_INVALID, COSL_E_CUDA, COSL_E_STATE = -1, -2, -6
@@ -69,22 +69,6 @@ def _submitted(api, prob, opt):
     return info, p
 
 
-def _same_decisions(want, got, prob):
-    """info[5..10] (iterations, stop, nfev, njev, nlss, total trials) and [13] (outliers) equal; the
-    solutions equal up to the order of the device's atomic sums; fixed parameters untouched"""
-    (iw, pw), (ig, pg) = want, got
-    assert np.array_equal(iw[5:11], ig[5:11]), (iw[:14], ig[:14])
-    assert iw[13] == ig[13]
-    assert np.array_equal(pw.outlier, pg.outlier)
-    assert abs(iw[12] - ig[12]) <= 1e-9 * iw[12] + 1e-12
-    assert np.abs(pw.R - pg.R).max() < 1e-9 and np.abs(pw.t - pg.t).max() < 1e-9
-    assert np.abs(pw.X - pg.X).max() < 1e-8
-    assert np.array_equal(pg.R[:prob.m_con], prob.R[:prob.m_con])
-    assert np.array_equal(pg.t[:prob.m_con], prob.t[:prob.m_con])
-    assert np.array_equal(pg.X[:prob.n_con], prob.X[:prob.n_con])
-    assert ig[11] > 0
-
-
 def _oracle_close(orc, prob, opt, got):
     """the tolerances of test_gpu_pose_ba._ba_compare"""
     ig, pg = got
@@ -102,7 +86,7 @@ def test_submit_matches_run_and_oracle(api, orc, name):
     prob = make()
     want = _run(api, prob, opt)
     got = _submitted(api, prob, opt)
-    _same_decisions(want, got, prob)
+    ba_same_decisions(want, got, prob)
     _oracle_close(orc, prob, opt, got)
 
 
@@ -145,7 +129,7 @@ def test_edge_shapes_and_stop_reasons(api, name):
     prob = make()
     want = _run(api, prob, opt)
     got = _submitted(api, prob, opt)
-    _same_decisions(want, got, prob)
+    ba_same_decisions(want, got, prob)
     s = api.BaSolver(prob.copy(), opt)
     plan, ns = s.plan_info(), s.stats()["ns"]
     s.close()
@@ -187,7 +171,7 @@ def test_submit_returns_before_the_device_runs_it(api):
     assert dt < 0.25, dt
     assert not s.done()
     info = s.collect()
-    _same_decisions(want, (info, s.download()), prob)
+    ba_same_decisions(want, (info, s.download()), prob)
     s.close()
 
 
@@ -207,7 +191,7 @@ def test_reuse_and_mixing_with_run(api):
             while not s.done() and time.perf_counter() < deadline:
                 time.sleep(1e-4)
             info = s.collect()
-        _same_decisions(want, (info, s.download()), prob)
+        ba_same_decisions(want, (info, s.download()), prob)
     s.close()
 
 
@@ -317,7 +301,7 @@ def test_concurrent_with_klt_tracking(api, orc):
     for k, ((fw, nw), (fg, ng)) in enumerate(zip(want, got)):
         assert np.array_equal(nw, ng), k
         assert fw.tobytes() == fg.tobytes(), k
-    _same_decisions(want_ba, got_ba, prob)
+    ba_same_decisions(want_ba, got_ba, prob)
     _oracle_close(orc, prob, opt, got_ba)
 
 

@@ -15,6 +15,7 @@ import pytest
 from coslam_b200 import synth
 from coslam_b200.ctypes_defs import BaOptions
 from coslam_b200.problem import BAProblem
+from helpers import ba_same_decisions
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 COSL_E_INVALID, COSL_E_CUDA, COSL_E_STATE = -1, -2, -6
@@ -79,21 +80,6 @@ def _fresh(api, prob, opt):
     return (info, p), st, plan
 
 
-def _same_decisions(want, got, prob):
-    """as test_gpu_ba_async._same_decisions"""
-    (iw, pw), (ig, pg) = want, got
-    assert np.array_equal(iw[5:11], ig[5:11]), (iw[:14], ig[:14])
-    assert iw[13] == ig[13]
-    assert np.array_equal(pw.outlier, pg.outlier)
-    assert abs(iw[12] - ig[12]) <= 1e-9 * iw[12] + 1e-12
-    assert np.abs(pw.R - pg.R).max() < 1e-9 and np.abs(pw.t - pg.t).max() < 1e-9
-    if prob.n:
-        assert np.abs(pw.X - pg.X).max() < 1e-8
-    assert np.array_equal(pg.R[:prob.m_con], prob.R[:prob.m_con])
-    assert np.array_equal(pg.t[:prob.m_con], prob.t[:prob.m_con])
-    assert np.array_equal(pg.X[:prob.n_con], prob.X[:prob.n_con])
-
-
 def _oracle_close(orc, prob, opt, got):
     """the tolerances of test_gpu_pose_ba._ba_compare"""
     ig, pg = got
@@ -120,7 +106,7 @@ def test_one_handle_loads_every_shape_like_a_fresh_one(api, orc):
         s.submit()
         got_sub = (s.collect(), s.download(prob.copy()))
         for got in (got_run, got_sub):
-            _same_decisions(want, got, prob)
+            ba_same_decisions(want, got, prob)
         assert got_sub[0][11] > 0, name
         if prob.n:
             _oracle_close(orc, prob, opt, got_sub)
@@ -158,7 +144,7 @@ def test_load_and_submit_return_before_the_device_runs_them(api):
         assert dt < 0.25, dt
         assert not s.done()
         info = s.collect()
-        _same_decisions(want, (info, s.download(prob.copy())), prob)
+        ba_same_decisions(want, (info, s.download(prob.copy())), prob)
     s.close()
 
 
@@ -178,7 +164,7 @@ def test_load_copies_its_input(api):
         a[:] = np.nan
     s.submit()
     got = (s.collect(), s.download(c3.copy()))
-    _same_decisions(want, got, c3)
+    ba_same_decisions(want, got, c3)
     s.close()
 
 
@@ -211,7 +197,7 @@ def test_malformed_problem_keeps_the_loaded_one(api):
     for name, bad in _malformed(c3).items():
         assert L.cosl_ba_solver_load(s.h, C.byref(bad.struct())) == COSL_E_INVALID, name
         assert L.cosl_ba_solver_load(s.h, None) == COSL_E_INVALID
-        _same_decisions(want, (s.run(), s.download(c3.copy())), c3)
+        ba_same_decisions(want, (s.run(), s.download(c3.copy())), c3)
         s.reset(c3.copy())
     s.close()
 
@@ -228,7 +214,7 @@ def test_load_while_a_submit_is_in_flight(api):
     s.submit()
     assert L.cosl_ba_solver_load(s.h, C.byref(c3.struct())) == COSL_E_STATE
     info = s.collect()
-    _same_decisions(want, (info, s.download(c2.copy())), c2)
+    ba_same_decisions(want, (info, s.download(c2.copy())), c2)
     s.close()
 
 

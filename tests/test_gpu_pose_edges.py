@@ -196,3 +196,29 @@ def test_batch_cameras_are_independent(api):
     for c in range(len(cams)):
         assert same_bits(opt_vector(opts2[c]), opt_vector(opts[c])) and opts2[c].npts == opts[c].npts, c
     print(f"{len(cams)} cameras, {sum(len(c[3]) for c in cams)} points, {int(ok.sum())} ok")
+
+
+def test_batch_with_per_camera_intrinsics(api, orc):
+    """The three cameras of a rig with their own K (fx 350 / 800 / 1400, fy = 0.92 / 1 / 1.07 fx, skew -4 / 0 /
+    3.5 px, principal points off-centre; tests/ba_dense.py) in one batch: each equals the oracle and the
+    dense restatement."""
+    import ba_dense
+    prob = ba_dense.rig_intrinsics()
+    pt = ba_dense.point_of(prob)
+    rng = np.random.default_rng(8)
+    Ks, R0s, t0s, Mss, mss = [], [], [], [], []
+    for j in (3, 4, 5):
+        o = prob.cam == j
+        Ks.append(prob.K[j].reshape(3, 3))
+        R0s.append(ba_dense.rot(rng.normal(size=3), 0.5) @ prob.R[j].reshape(3, 3))
+        t0s.append(prob.t[j] + rng.normal(0, 0.01, 3))
+        Mss.append(prob.X[pt[o]])
+        mss.append(prob.xy[o])
+    assert len({K[0, 0] for K in Ks}) == 3 and any(K[0, 1] != 0 for K in Ks)
+    ok, R, t, _ = api.pose_intracam_batch(Ks, R0s, t0s, Mss, mss, 10.0)
+    for c in range(3):
+        ok_o, R_o, t_o, _ = orc.pose_intracam(Ks[c], R0s[c], t0s[c], Mss[c], mss[c], 10.0)
+        ok_d, R_d, t_d, _ = pd.estimate(Ks[c], R0s[c], t0s[c], Mss[c], mss[c], 10.0)
+        assert ok[c] == ok_o == ok_d
+        assert np.abs(R[c] - R_o).max() < 1e-8 and np.abs(t[c] - t_o).max() < 1e-8, c
+        assert np.abs(R[c] - R_d).max() < 1e-8 and np.abs(t[c] - t_d).max() < 1e-8, c
