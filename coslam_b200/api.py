@@ -538,9 +538,36 @@ def pose_intracam_batch(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opt
     return ok.astype(bool), R.reshape(Cn, 3, 3), t, opts
 
 
-class PoseSolver:
+class _SolverHandle:
+    """A solver handle of the C-ABI with one request in flight at a time: close, done and stream call
+    <_prefix>_destroy, _query and _stream on self.h."""
+
+    _prefix = None
+
+    def close(self):
+        """destroy: waits for a request in flight."""
+        if getattr(self, "h", None):
+            getattr(LIB, self._prefix + "_destroy")(self.h)
+            self.h = None
+
+    def __del__(self):
+        self.close()
+
+    def done(self):
+        """query: True once the submitted request has finished (never waits)."""
+        d = C.c_int(0)
+        _ck(getattr(LIB, self._prefix + "_query")(self.h, C.byref(d)))
+        return bool(d.value)
+
+    def stream(self):
+        return getattr(LIB, self._prefix + "_stream")(self.h)
+
+
+class PoseSolver(_SolverHandle):
     """cosl_pose_solver: pose_intracam_batch without blocking, on a stream and buffers of its own for at
     most max_cams cameras and max_pts points (all cameras together) per submit."""
+
+    _prefix = "cosl_pose_solver"
 
     def __init__(self, device, max_cams, max_pts):
         h = C.c_void_p()
@@ -548,27 +575,12 @@ class PoseSolver:
         self.h, self.device, self.max_cams, self.max_pts = h, device, max_cams, max_pts
         self._opts = None
 
-    def close(self):
-        """cosl_pose_solver_destroy: waits for a solve in flight."""
-        if getattr(self, "h", None):
-            LIB.cosl_pose_solver_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        self.close()
-
     def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None):
         """cosl_pose_solver_submit: enqueue pose_intracam_batch's solve and return at once; the input arrays
         may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills."""
         args, opts, _keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
         _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
         self._opts = opts
-
-    def done(self):
-        """cosl_pose_solver_query: True once the submitted solve has finished (never waits)."""
-        d = C.c_int(0)
-        _ck(LIB.cosl_pose_solver_query(self.h, C.byref(d)))
-        return bool(d.value)
 
     def collect(self):
         """cosl_pose_solver_collect: wait for the submitted solve.  Returns (ok, R, t, opts) as
@@ -579,9 +591,6 @@ class PoseSolver:
         _ck(LIB.cosl_pose_solver_collect(self.h, _ptr(R), _ptr(t), opts, _ptr(ok), C.byref(ms)))
         self._opts = None
         return ok.astype(bool), R.reshape(Cn, 3, 3), t, opts, ms.value
-
-    def stream(self):
-        return LIB.cosl_pose_solver_stream(self.h)
 
 
 def ba_solve(prob, opt):
@@ -679,24 +688,17 @@ def posegraph_solve(fixed, R, t, id1, id2, eR, et, scale_col=None, n_scale=0, de
     return nR, nt, s[:int(n_scale)]
 
 
-class PoseGraphSolver:
+class PoseGraphSolver(_SolverHandle):
     """cosl_posegraph_solver: posegraph_spread_chains and posegraph_solve without blocking, on a stream and
     buffers of its own that grow with the largest request."""
+
+    _prefix = "cosl_posegraph_solver"
 
     def __init__(self, device):
         h = C.c_void_p()
         _ck(LIB.cosl_posegraph_solver_create(int(device), C.byref(h)))
         self.h, self.device = h, device
         self._shape = None  # (nodes, scale columns or None for a chain spread) of the request in flight
-
-    def close(self):
-        """cosl_posegraph_solver_destroy: waits for a request in flight."""
-        if getattr(self, "h", None):
-            LIB.cosl_posegraph_solver_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        self.close()
 
     def submit_chains(self, chain_off, fixed, R, t, eR, et):
         """cosl_posegraph_solver_submit_chains: enqueue posegraph_spread_chains' spread and return at once; the
@@ -712,12 +714,6 @@ class PoseGraphSolver:
         _ck(LIB.cosl_posegraph_solver_submit(self.h, *args))
         self._shape = (n, int(n_scale))
 
-    def done(self):
-        """cosl_posegraph_solver_query: True once the submitted request has finished (never waits)."""
-        d = C.c_int(0)
-        _ck(LIB.cosl_posegraph_solver_query(self.h, C.byref(d)))
-        return bool(d.value)
-
     def collect(self):
         """cosl_posegraph_solver_collect: wait for the submitted request.  Returns (newR, newt, scale, device_ms):
         what posegraph_spread_chains (scale None) or posegraph_solve returns, then the device time of the
@@ -728,9 +724,6 @@ class PoseGraphSolver:
         self._shape = None  # a collect that reports an error consumes the request as well
         _ck(LIB.cosl_posegraph_solver_collect(self.h, _ptr(nR), _ptr(nt), _ptr(s), C.byref(ms)))
         return nR, nt, (None if ns is None else s[:ns]), ms.value
-
-    def stream(self):
-        return LIB.cosl_posegraph_solver_stream(self.h)
 
 
 def posegraph_last_host_ms():
@@ -757,8 +750,10 @@ class BaComm:
             self.h = None
 
 
-class BaSolver:
+class BaSolver(_SolverHandle):
     """Problem resident on the device (this rank's shard of points when `comm` is given)."""
+
+    _prefix = "cosl_ba_solver"
 
     def __init__(self, prob, opt, comm=None):
         self.prob, self.opt = prob, opt
@@ -767,14 +762,6 @@ class BaSolver:
         _ck(LIB.cosl_ba_solver_create(C.byref(self._s), C.byref(opt), comm.h if comm else None,
                                       C.byref(h)))
         self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            LIB.cosl_ba_solver_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        self.close()
 
     def reset(self, prob=None):
         if prob is not None:
@@ -803,12 +790,6 @@ class BaSolver:
         """cosl_ba_solver_submit: enqueue run()'s robust loop on the solver's stream and return at once."""
         _ck(LIB.cosl_ba_solver_submit(self.h))
 
-    def done(self):
-        """cosl_ba_solver_query: True once the submitted loop has finished (never waits)."""
-        d = C.c_int(0)
-        _ck(LIB.cosl_ba_solver_query(self.h, C.byref(d)))
-        return bool(d.value)
-
     def collect(self):
         """cosl_ba_solver_collect: wait for the submitted loop; the info vector of run()."""
         info = np.zeros(COSL_BA_INFOSZ)
@@ -823,9 +804,6 @@ class BaSolver:
         s = into.struct()
         _ck(LIB.cosl_ba_solver_download(self.h, C.byref(s)))
         return into
-
-    def stream(self):
-        return LIB.cosl_ba_solver_stream(self.h)
 
     def stats(self):
         out = (C.c_double * 8)()

@@ -162,7 +162,7 @@ struct cosl_ba_solver {
   cosl_ba_options opt;
   cosl_ba_comm* comm = nullptr;
   int device = 0;
-  cudaStream_t stream = nullptr;
+  RequestStream rq;  // the solver's stream: every call enqueues there, cosl_ba_solver_submit as one request
   BaDev d;
   // host copies needed for write-back
   int m = 0, n = 0, mcon = 0, ncon = 0, mf = 0, ns = 0;
@@ -226,14 +226,12 @@ struct cosl_ba_solver {
   int secLin = 0, secSchur = 0, secSolve = 0, secBack = 0, secCost = 0, secComm = 0;
   // statistics
   int nfev = 0, njev = 0, nlss = 0;
-  // submitted robust loop (cosl_ba_solver_submit): the graph with the device-side LM control, the
-  // parameter buffers it was built for, and the events that time and mark one submission
+  // submitted robust loop (cosl_ba_solver_submit): the graph with the device-side LM control and the
+  // parameter buffers it was built for
   BaCtl* d_ctl = nullptr;
   cudaGraphExec_t graphExec = nullptr;
   bool graphStale = false;  // a load changed the problem since the graph was built
   const double *graphPa = nullptr, *graphNa = nullptr, *graphPb = nullptr, *graphNb = nullptr;
-  cudaEvent_t evSubmit = nullptr, evDone = nullptr;
-  bool inFlight = false;
 };
 
 namespace {
@@ -294,22 +292,6 @@ void quat_mul(const double a[4], const double b[4], double p[4]) {
   p[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
   p[2] = a[0] * b[2] - a[1] * b[3] + a[2] * b[0] + a[3] * b[1];
   p[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
-}
-
-// Solver buffers come from the device's stream-ordered memory pool with an unlimited release
-// threshold: cosl_ba_solve creates and destroys a solver per call, and after the first call the
-// ~30 buffers (0.7 GB at c4) are handed out again without touching the driver's allocator.
-static void pool_keep(int device) {
-  static std::mutex mu;
-  static bool done[64] = {};
-  std::lock_guard<std::mutex> lk(mu);
-  if (device < 0 || device >= 64 || done[device]) return;
-  done[device] = true;
-  cudaMemPool_t pool;
-  if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
-    unsigned long long keep = ~0ull;
-    cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-  }
 }
 
 // Pinned 128-byte slots for the per-trial scalar read-back.  cudaMallocHost / cudaFreeHost cost
@@ -462,11 +444,11 @@ int grow(cosl_ba_solver* s, T** p, size_t count) {
     auto it = s->cap.find((void*)*p);
     if (it != s->cap.end() && it->second >= bytes) return COSL_OK;
     s->cap.erase((void*)*p);
-    COSL_CUDA(cudaFreeAsync((void*)*p, s->stream));
+    COSL_CUDA(cudaFreeAsync((void*)*p, s->rq.stream));
     *p = nullptr;
   }
   const size_t want = bytes + bytes / 4;
-  COSL_CUDA(cudaMallocAsync((void**)p, want, s->stream));
+  COSL_CUDA(cudaMallocAsync((void**)p, want, s->rq.stream));
   s->cap[(void*)*p] = want;
   return COSL_OK;
 }
@@ -491,27 +473,24 @@ int upload_params(cosl_ba_solver* s, const cosl_ba_problem* p) {
     }
   }
   if (s->n) std::memcpy(X, p->X, sizeof(double) * 3 * (size_t)s->n);
-  COSL_CUDA(cudaMemcpyAsync(s->d_camR0, R0, sizeof(double) * 9 * m, cudaMemcpyHostToDevice, s->stream));
-  COSL_CUDA(cudaMemcpyAsync(s->d_pa, pa, sizeof(double) * 6 * m, cudaMemcpyHostToDevice, s->stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_camR0, R0, sizeof(double) * 9 * m, cudaMemcpyHostToDevice, s->rq.stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_pa, pa, sizeof(double) * 6 * m, cudaMemcpyHostToDevice, s->rq.stream));
   if (s->n)
-    COSL_CUDA(cudaMemcpyAsync(s->d_pb, X, sizeof(double) * 3 * (size_t)s->n, cudaMemcpyHostToDevice, s->stream));
+    COSL_CUDA(cudaMemcpyAsync(s->d_pb, X, sizeof(double) * 3 * (size_t)s->n, cudaMemcpyHostToDevice, s->rq.stream));
   return COSL_OK;
 }
 
 void free_solver(cosl_ba_solver* s) {
   if (!s) return;
   cudaSetDevice(s->device);
-  if (s->stream) cudaStreamSynchronize(s->stream);
+  if (s->rq.stream) cudaStreamSynchronize(s->rq.stream);
   s->timer.destroy();
   if (s->graphExec) cudaGraphExecDestroy(s->graphExec);
-  if (s->evSubmit) cudaEventDestroy(s->evSubmit);
-  if (s->evDone) cudaEventDestroy(s->evDone);
   if (s->evStaged) cudaEventDestroy(s->evStaged);
-  for (const auto& b : s->cap) cudaFreeAsync(b.first, s->stream);
-  if (s->stream) cudaStreamSynchronize(s->stream);
+  for (const auto& b : s->cap) cudaFreeAsync(b.first, s->rq.stream);
+  s->rq.destroy();  // waits for the frees above
   if (s->h_sc) pinned_slots().put(s->h_sc);
   pinned_staging().put(s->h_stage, s->stageBytes);
-  if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
 
@@ -632,14 +611,14 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
     for (int jb = ja; jb < mf; ++jb)
       if (x.poff[(size_t)ja * mf + jb + 1] > x.poff[(size_t)ja * mf + jb]) adj[(size_t)ja * mf + jb] = adj[(size_t)jb * mf + ja] = 1;
   if (multi(s) && mf > 0) {
-    TmpDeviceBufs tmp(s->stream);
+    TmpDeviceBufs tmp(s->rq.stream);
     uint8_t* d_adj = nullptr;
     COSL_TRY(tmp.alloc(&d_adj, adj.size()));
-    COSL_CUDA(cudaMemcpyAsync(d_adj, adj.data(), adj.size(), cudaMemcpyHostToDevice, s->stream));
-    const int rc = nccl().AllReduce(d_adj, d_adj, adj.size(), ncclUint8, ncclMax, s->comm->comm, s->stream);
+    COSL_CUDA(cudaMemcpyAsync(d_adj, adj.data(), adj.size(), cudaMemcpyHostToDevice, s->rq.stream));
+    const int rc = nccl().AllReduce(d_adj, d_adj, adj.size(), ncclUint8, ncclMax, s->comm->comm, s->rq.stream);
     if (rc != 0) return set_error(COSL_E_NCCL, "ncclAllReduce (co-visibility) failed (%d)", rc);
-    COSL_CUDA(cudaMemcpyAsync(adj.data(), d_adj, adj.size(), cudaMemcpyDeviceToHost, s->stream));
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
+    COSL_CUDA(cudaMemcpyAsync(adj.data(), d_adj, adj.size(), cudaMemcpyDeviceToHost, s->rq.stream));
+    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   }
   const double tPlan0 = now_s();
   BaPlan P = ba_make_plan(mf, adj);
@@ -756,7 +735,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   s->factorFlops = PL.flops;
   s->graphStale = true;
   COSL_TRY(grow(s, &s->d_in, inBytes));
-  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_stage + parBytes, inBytes, cudaMemcpyHostToDevice, s->stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_stage + parBytes, inBytes, cudaMemcpyHostToDevice, s->rq.stream));
   s->d_ptr = reinterpret_cast<const long long*>(s->d_in + oPtr);
   s->d_cam = reinterpret_cast<const int*>(s->d_in + oCam);
   s->d_xy = reinterpret_cast<const double*>(s->d_in + oXy);
@@ -800,19 +779,19 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   COSL_TRY(grow(s, &s->d_Vinv, (size_t)n * 6));
   COSL_TRY(grow(s, &s->d_entries, (size_t)nEntries));
   COSL_TRY(upload_params(s, p));
-  COSL_CUDA(cudaEventRecord(s->evStaged, s->stream));
+  COSL_CUDA(cudaEventRecord(s->evStaged, s->rq.stream));
   // observation index lists and Schur pair entries
-  if (n) COSL_LAUNCH(ba_index_points, div_up(n, 256), 256, 0, s->stream, s->d_ptr, n, s->d_pt);
+  if (n) COSL_LAUNCH(ba_index_points, div_up(n, 256), 256, 0, s->rq.stream, s->d_ptr, n, s->d_pt);
   if (Nc) {
     const int chunk = (int)std::max<long long>(256, 32 * div_up64(div_up64(N, 256), 32));
     const int nChunks = (int)div_up64(N, chunk);
     COSL_TRY(grow(s, &s->d_hist, (size_t)nChunks * mf));
-    COSL_CUDA(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * (size_t)nChunks * mf, s->stream));
+    COSL_CUDA(cudaMemsetAsync(s->d_hist, 0, sizeof(unsigned) * (size_t)nChunks * mf, s->rq.stream));
     const unsigned gW = (unsigned)div_up64(32LL * nChunks, 256);
-    COSL_LAUNCH(ba_index_cams<false>, gW, 256, 0, s->stream, s->d_cam, N, mcon, mf, chunk, s->d_hist, s->d_cobs,
+    COSL_LAUNCH(ba_index_cams<false>, gW, 256, 0, s->rq.stream, s->d_cam, N, mcon, mf, chunk, s->d_hist, s->d_cobs,
                 s->d_ccam);
-    COSL_LAUNCH(ba_index_cam_base, div_up(mf, 256), 256, 0, s->stream, s->d_hist, nChunks, mf, d_camStart);
-    COSL_LAUNCH(ba_index_cams<true>, gW, 256, 0, s->stream, s->d_cam, N, mcon, mf, chunk, s->d_hist, s->d_cobs,
+    COSL_LAUNCH(ba_index_cam_base, div_up(mf, 256), 256, 0, s->rq.stream, s->d_hist, nChunks, mf, d_camStart);
+    COSL_LAUNCH(ba_index_cams<true>, gW, 256, 0, s->rq.stream, s->d_cam, N, mcon, mf, chunk, s->d_hist, s->d_cobs,
                 s->d_ccam);
   }
   BaDev& d = s->d;
@@ -844,8 +823,8 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   d.sc = s->d_sc;
   if (nEntries) {
     COSL_TRY(grow(s, &s->d_pcnt, nBuckets + 1));
-    COSL_CUDA(cudaMemsetAsync(s->d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->stream));
-    COSL_LAUNCH(ba_pairs_build<true>, (unsigned)div_up64(Nc, 256), 256, 0, s->stream, d, s->d_pcnt, d_poff,
+    COSL_CUDA(cudaMemsetAsync(s->d_pcnt, 0, sizeof(unsigned) * (nBuckets + 1), s->rq.stream));
+    COSL_LAUNCH(ba_pairs_build<true>, (unsigned)div_up64(Nc, 256), 256, 0, s->rq.stream, d, s->d_pcnt, d_poff,
                 s->d_entries);
   }
   COSL_CUDA(cudaGetLastError());
@@ -897,20 +876,17 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   return COSL_OK;
 }
 
-// A solver handle without a problem: stream, scalar slots, the kernel attributes of the solve
+// A solver handle without a problem on the current device: stream, scalar slots, the kernel attributes of the
+// solve.  *out is set once the handle exists, also when a later step fails.
 int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver** out) {
   cosl_ba_solver* s = new (std::nothrow) cosl_ba_solver();
   if (!s) return set_error(COSL_E_NOMEM, "host allocation failed");
   s->opt = *opt;
   s->comm = comm;
   s->device = opt->device;
-  cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) {
-    delete s;
-    return set_error(COSL_E_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e));
-  }
   *out = s;
-  pool_keep(opt->device);
+  COSL_TRY(s->rq.create());
+  keep_pool(opt->device);
   static_assert(SC_NTOT <= 16, "pinned slot size");
   s->h_sc = pinned_slots().get();
   if (!s->h_sc) return set_error(COSL_E_NOMEM, "pinned host allocation failed");
@@ -937,9 +913,9 @@ int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver**
 
 int allreduce(cosl_ba_solver* s, double* buf, size_t count, int op) {
   if (!multi(s)) return COSL_OK;
-  s->timer.begin(s->secComm, s->stream);
-  const int rc = nccl().AllReduce(buf, buf, count, ncclFloat64, op, s->comm->comm, s->stream);
-  s->timer.end(s->stream);
+  s->timer.begin(s->secComm, s->rq.stream);
+  const int rc = nccl().AllReduce(buf, buf, count, ncclFloat64, op, s->comm->comm, s->rq.stream);
+  s->timer.end(s->rq.stream);
   if (rc != 0)
     return set_error(COSL_E_NCCL, "ncclAllReduce: %s",
                      nccl().GetErrorString ? nccl().GetErrorString(rc) : "?");
@@ -947,7 +923,7 @@ int allreduce(cosl_ba_solver* s, double* buf, size_t count, int op) {
 }
 
 int zero_sc(cosl_ba_solver* s, int first, int count) {
-  COSL_CUDA(cudaMemsetAsync(s->d_sc + first, 0, sizeof(double) * count, s->stream));
+  COSL_CUDA(cudaMemsetAsync(s->d_sc + first, 0, sizeof(double) * count, s->rq.stream));
   return COSL_OK;
 }
 
@@ -972,16 +948,16 @@ int read_sc(cosl_ba_solver* s) {
   const bool crowded = multi(s) && host_threads_all() < 3 * s->comm->nranks;
   if (crowded) {
     COSL_CUDA(cudaMemcpyAsync(s->h_sc, s->d_sc, sizeof(double) * SC_NTOT, cudaMemcpyDeviceToHost,
-                              s->stream));
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
+                              s->rq.stream));
+    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
     return COSL_OK;
   }
   const unsigned long long seq = ++s->scSeq;
-  COSL_LAUNCH(ba_publish_sc, 1, 32, 0, s->stream, s->d_sc, s->h_sc, seq);
+  COSL_LAUNCH(ba_publish_sc, 1, 32, 0, s->rq.stream, s->d_sc, s->h_sc, seq);
   volatile unsigned long long* flag = reinterpret_cast<volatile unsigned long long*>(s->h_sc + SC_NTOT);
   for (long long spin = 0; *flag != seq; ++spin) {
     if ((spin & 0xfff) == 0xfff) {
-      const cudaError_t q = cudaStreamQuery(s->stream);
+      const cudaError_t q = cudaStreamQuery(s->rq.stream);
       if (q == cudaSuccess) break;  // everything ran: the stores are visible after the query
       if (q != cudaErrorNotReady)
         return set_error(COSL_E_CUDA, "scalar read-back: %s", cudaGetErrorString(q));
@@ -989,7 +965,7 @@ int read_sc(cosl_ba_solver* s) {
   }
   std::atomic_thread_fence(std::memory_order_acquire);
   if (*flag != seq) {  // left through the query: make sure the stores have landed
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
+    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
     if (*flag != seq) return set_error(COSL_E_CUDA, "scalar read-back: flag missing after synchronise");
   }
   return COSL_OK;
@@ -1000,11 +976,11 @@ int eval_cost(cosl_ba_solver* s, const double* pa, const double* pb, double* out
   ++s->nfev;
   COSL_TRY(zero_sc(s, SC_COST, 1));
   COSL_TRY(zero_sc(s, SC_NONFINITE, 1));
-  s->timer.begin(s->secCost, s->stream);
+  s->timer.begin(s->secCost, s->rq.stream);
   if (s->N)
-    COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d, pa, pb,
+    COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, pa, pb,
                 0, 0.0, nullptr);
-  s->timer.end(s->stream);
+  s->timer.end(s->rq.stream);
   COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
   COSL_TRY(read_sc(s));
   *out = s->h_sc[SC_COST];
@@ -1015,13 +991,13 @@ int eval_cost(cosl_ba_solver* s, const double* pa, const double* pb, double* out
 int compute_weights(cosl_ba_solver* s) {
   if (s->opt.max_err > 0) {
     if (s->N)
-      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d,
+      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d,
                   s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
   } else {
     std::vector<double> ones((size_t)s->N, 1.0);
     COSL_CUDA(cudaMemcpyAsync(s->d_wgt, ones.data(), sizeof(double) * (size_t)s->N,
-                              cudaMemcpyHostToDevice, s->stream));
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
+                              cudaMemcpyHostToDevice, s->rq.stream));
+    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   }
   return COSL_OK;
 }
@@ -1031,20 +1007,20 @@ int compute_weights(cosl_ba_solver* s) {
 // computed by the prep kernel of the next trial (solve_trial) and arrive with that trial's scalars
 int linearize(cosl_ba_solver* s, bool statsNow, bool statsLater) {
   ++s->njev;
-  s->timer.begin(s->secLin, s->stream);
-  COSL_CUDA(cudaMemsetAsync(s->d_V, 0, sizeof(double) * (9 * (size_t)s->n + 27 * (size_t)s->m), s->stream));
+  s->timer.begin(s->secLin, s->rq.stream);
+  COSL_CUDA(cudaMemsetAsync(s->d_V, 0, sizeof(double) * (9 * (size_t)s->n + 27 * (size_t)s->m), s->rq.stream));
   if (s->N)
-    COSL_LAUNCH(ba_linearize_points, (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d,
+    COSL_LAUNCH(ba_linearize_points, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d,
                 s->d_pa, s->d_pb);
   if (s->Nc)
-    COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, s->stream, s->d,
+    COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, s->rq.stream, s->d,
                 s->d_pa, s->d_pb);
-  s->timer.end(s->stream);
+  s->timer.end(s->rq.stream);
   COSL_TRY(allreduce(s, s->d_Uea, (size_t)27 * s->m, ncclSum));
   if (!s->N) COSL_TRY(zero_sc(s, SC_GINF, 2));  // otherwise ba_linearize_points cleared them
   s->statsPending = false;
   if (statsNow || (statsLater && !s->ns)) {
-    COSL_LAUNCH(ba_stats_kernel, (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->stream,
+    COSL_LAUNCH(ba_stats_kernel, (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->rq.stream,
                 s->d);
     COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
   } else if (statsLater) {
@@ -1058,13 +1034,13 @@ int linearize(cosl_ba_solver* s, bool statsNow, bool statsLater) {
 int dense_solve(cosl_ba_solver* s) {
   const int ns = s->ns;
   if (ns == 0) return COSL_OK;
-  s->timer.begin(s->secSolve, s->stream);
+  s->timer.begin(s->secSolve, s->rq.stream);
   if (s->twoSolve) {
-    COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s->stream, s->td, s->two00, s->two10, s->two11);
+    COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s->rq.stream, s->td, s->two00, s->two10, s->two11);
   } else {
-    COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, s->stream, s->td);
+    COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, s->rq.stream, s->td);
   }
-  s->timer.end(s->stream);
+  s->timer.end(s->rq.stream);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
@@ -1083,27 +1059,27 @@ int solve_trial(cosl_ba_solver* s, double mu, bool* solved) {
   }
   static const bool fineSchur = std::getenv("COSL_BA_TIMING_FINE") != nullptr;  // diagnostic: init / contraction apart
   const int secInit = fineSchur ? s->timer.section("ba_schur_init") : s->secSchur;
-  s->timer.begin(secInit, s->stream);
+  s->timer.begin(secInit, s->rq.stream);
   if (ns) {
     // also clears the scalars of this trial (|dp|^2, dL, |p|^2, fail, cost, non-finite) and the task
     // counters of the solve: five memset nodes less per trial
     const int nTilesInit = std::max(1, s->plan.nTiles);
     const bool doStats = s->statsPending;
     s->statsPending = false;
-    COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->stream, s->d,
+    COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->rq.stream, s->d,
                 mu, r0 ? 1 : 0, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt,
                 s->td.nCounters + 2 + s->td.nTasks, nTilesInit, s->d_Vinv, doStats ? 1 : 0,
                 s->d_dpb, 3LL * s->n);
     if (doStats) COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
     if (fineSchur) {
-      s->timer.end(s->stream);
-      s->timer.begin(s->secSchur, s->stream);
+      s->timer.end(s->rq.stream);
+      s->timer.begin(s->secSchur, s->rq.stream);
     }
     if (s->nItems)
-      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, s->stream,
+      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, s->rq.stream,
                   s->d, s->d_items, s->nItems, s->d_entries, s->d_Vinv);
   }
-  s->timer.end(s->stream);
+  s->timer.end(s->rq.stream);
   // the one exchange of an LM trial: [rhs | Schur-structure tiles] is contiguous, no packing
   if (ns && multi(s)) COSL_TRY(allreduce(s, s->d_S, (size_t)s->reduceCount, ncclSum));
   COSL_TRY(dense_solve(s));
@@ -1112,30 +1088,30 @@ int solve_trial(cosl_ba_solver* s, double mu, bool* solved) {
     // back substitution + trial cost in two launches (ba_kernels.cuh): the accumulator d_dpb was zeroed by the
     // prep kernel, V*^-1 is the one the Schur contraction used
     const int nCamBlocks = div_up(6 * s->m, 256);
-    s->timer.begin(s->secBack, s->stream);
-    COSL_LAUNCH(ba_back_cams_points, nCamBlocks + (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d, s->d_pa,
+    s->timer.begin(s->secBack, s->rq.stream);
+    COSL_LAUNCH(ba_back_cams_points, nCamBlocks + (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, s->d_pa,
                 s->d_x, s->d_dpa, s->d_na, mu, r0 ? 1 : 0, nCamBlocks, s->d_dpb);
-    s->timer.end(s->stream);
-    s->timer.begin(s->secCost, s->stream);
-    COSL_LAUNCH(ba_finish_cost, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, s->stream, s->d, s->d_na,
+    s->timer.end(s->rq.stream);
+    s->timer.begin(s->secCost, s->rq.stream);
+    COSL_LAUNCH(ba_finish_cost, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, s->rq.stream, s->d, s->d_na,
                 s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu);
-    s->timer.end(s->stream);
+    s->timer.end(s->rq.stream);
     s->costDone = true;
     COSL_CUDA(cudaGetLastError());
     *solved = true;
     return COSL_OK;
   }
-  s->timer.begin(s->secBack, s->stream);
+  s->timer.begin(s->secBack, s->rq.stream);
   // (also zeroes the accumulator of the point back-substitution, d_nb)
   COSL_LAUNCH(ba_cam_update, std::max(div_up(6 * s->m, 256), (int)std::min<long long>(s->numSM, div_up64(3LL * s->n, 1024))),
-              256, 0, s->stream, s->d, s->d_pa, s->d_x, s->d_dpa, s->d_na, mu, r0 ? 1 : 0, s->d_nb, 3LL * s->n);
+              256, 0, s->rq.stream, s->d, s->d_pa, s->d_x, s->d_dpa, s->d_na, mu, r0 ? 1 : 0, s->d_nb, 3LL * s->n);
   if (s->N)
-    COSL_LAUNCH(ba_back_subst, (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d, s->d_dpa,
+    COSL_LAUNCH(ba_back_subst, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, s->d_dpa,
                 s->d_nb);
   if (s->n)
-    COSL_LAUNCH(ba_back_finish, (unsigned)div_up64(s->n, 256), 256, 0, s->stream, s->d, s->d_pb,
+    COSL_LAUNCH(ba_back_finish, (unsigned)div_up64(s->n, 256), 256, 0, s->rq.stream, s->d, s->d_pb,
                 s->d_nb, s->d_dpb, mu);
-  s->timer.end(s->stream);
+  s->timer.end(s->rq.stream);
   COSL_CUDA(cudaGetLastError());
   // the scalar all-reduce of this trial is merged with the cost evaluation by the caller
   *solved = true;
@@ -1183,11 +1159,11 @@ int levmar(cosl_ba_solver* s, int itmax, const double opts[5], double info[10], 
       // trial cost, merged scalar all-reduce
       ++s->nfev;  // (cost / non-finite scalars were cleared by solve_trial)
       if (!s->costDone) {
-        s->timer.begin(s->secCost, s->stream);
+        s->timer.begin(s->secCost, s->rq.stream);
         if (s->N)
-          COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d,
+          COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d,
                       s->d_na, s->d_nb, 0, 0.0, nullptr);
-        s->timer.end(s->stream);
+        s->timer.end(s->rq.stream);
       }
       COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
       COSL_TRY(read_sc(s));
@@ -1275,7 +1251,7 @@ int run_robust(cosl_ba_solver* s, int fixed_trials, double info[COSL_BA_INFOSZ])
   double sinfo[10] = {0};
   double first_e0 = -1;
   int total_trials = 0;
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   const auto t0 = std::chrono::steady_clock::now();
   const int rounds = fixed_trials ? 1 : std::max(1, s->opt.outer_iters);
   for (int r = 0; r < rounds; ++r) {
@@ -1289,14 +1265,14 @@ int run_robust(cosl_ba_solver* s, int fixed_trials, double info[COSL_BA_INFOSZ])
   if (s->opt.max_err > 0) {  // the same branch on every rank (options are global): collective inside
     COSL_TRY(zero_sc(s, SC_COST, 1));
     if (s->N)
-      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->stream, s->d, s->d_pa,
+      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, s->d_pa,
                   s->d_pb, 2, s->opt.max_err, s->d_outlier);
     COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
     COSL_TRY(read_sc(s));
     nout = s->h_sc[SC_COST];  // outliers over ALL ranks' observations
   } else {
-    COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, s->stream));
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
+    COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, s->rq.stream));
+    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   }
   const auto t1 = std::chrono::steady_clock::now();
   if (info) {
@@ -1315,14 +1291,14 @@ int download(cosl_ba_solver* s, cosl_ba_problem* p) {
   const int m = s->m;
   std::vector<double> pa((size_t)m * 6);
   COSL_CUDA(cudaMemcpyAsync(pa.data(), s->d_pa, sizeof(double) * 6 * m, cudaMemcpyDeviceToHost,
-                            s->stream));
+                            s->rq.stream));
   std::vector<double> X((size_t)s->n * 3);
   COSL_CUDA(cudaMemcpyAsync(X.data(), s->d_pb, sizeof(double) * 3 * (size_t)s->n,
-                            cudaMemcpyDeviceToHost, s->stream));
+                            cudaMemcpyDeviceToHost, s->rq.stream));
   if (p->outlier && s->N)
     COSL_CUDA(cudaMemcpyAsync(p->outlier, s->d_outlier, (size_t)s->N, cudaMemcpyDeviceToHost,
-                              s->stream));
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
+                              s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   for (int j = s->mcon; j < m; ++j) {
     const double* v = &pa[6 * j];
     const double dq[4] = {std::sqrt(1.0 - (v[0] * v[0] + v[1] * v[1] + v[2] * v[2])), v[0], v[1],
@@ -1592,14 +1568,12 @@ int cosl_ba_solver_create(const cosl_ba_problem* prob, const cosl_ba_options* op
   BaIndex x;
   COSL_TRY(index_problem(prob, x));
   if (ba_timing()) std::fprintf(stderr, "[ba timing] index %.2f ms\n", 1e3 * (now_s() - t0));
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || opt->device < 0 || opt->device >= ndev)
-    return set_error(COSL_E_CUDA, "CUDA device %d not available", opt->device);
+  COSL_TRY(check_device(opt->device));
   COSL_CUDA(cudaSetDevice(opt->device));
   cosl_ba_solver* s = nullptr;
   int rc = make_handle(opt, comm, &s);
   if (rc == COSL_OK) rc = load_problem(s, prob, x);
-  if (rc == COSL_OK && cudaStreamSynchronize(s->stream) != cudaSuccess)
+  if (rc == COSL_OK && cudaStreamSynchronize(s->rq.stream) != cudaSuccess)
     rc = set_error(COSL_E_CUDA, "cosl_ba_solver_create: %s", cudaGetErrorString(cudaGetLastError()));
   if (rc != COSL_OK) {
     free_solver(s);
@@ -1613,19 +1587,16 @@ int cosl_ba_solver_create(const cosl_ba_problem* prob, const cosl_ba_options* op
   if (!(s)) return set_error(COSL_E_INVALID, "null solver handle"); \
   COSL_CUDA(cudaSetDevice((s)->device));
 
-#define BA_IDLE(s, what) \
-  if ((s)->inFlight) return set_error(COSL_E_STATE, what ": a submitted solve is not collected yet");
-
 int cosl_ba_solver_reset(cosl_ba_solver* s, const cosl_ba_problem* prob) {
   BA_ENTER(s)
-  BA_IDLE(s, "cosl_ba_solver_reset")
+  COSL_TRY(s->rq.idle("cosl_ba_solver_reset"));
   if (!prob || prob->m != s->m || prob->n != s->n)
     return set_error(COSL_E_INVALID, "cosl_ba_solver_reset: problem shape changed");
   s->timer.reset();
   COSL_CUDA(cudaEventSynchronize(s->evStaged));
   COSL_TRY(upload_params(s, prob));
-  COSL_CUDA(cudaEventRecord(s->evStaged, s->stream));
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  COSL_CUDA(cudaEventRecord(s->evStaged, s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   return COSL_OK;
 }
 
@@ -1633,7 +1604,7 @@ int cosl_ba_solver_load(cosl_ba_solver* s, const cosl_ba_problem* prob) {
   BA_ENTER(s)
   if (multi(s))
     return set_error(COSL_E_INVALID, "cosl_ba_solver_load: a multi-rank solver plans over all ranks; create one");
-  BA_IDLE(s, "cosl_ba_solver_load")
+  COSL_TRY(s->rq.idle("cosl_ba_solver_load"));
   COSL_TRY(check_problem(prob, "cosl_ba_solver_load"));
   BaIndex x;
   COSL_TRY(index_problem(prob, x));
@@ -1643,19 +1614,19 @@ int cosl_ba_solver_load(cosl_ba_solver* s, const cosl_ba_problem* prob) {
 
 int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
-  BA_IDLE(s, "cosl_ba_solver_run")
+  COSL_TRY(s->rq.idle("cosl_ba_solver_run"));
   return run_robust(s, 0, info);
 }
 
 int cosl_ba_solver_run_fixed(cosl_ba_solver* s, int trials, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
-  BA_IDLE(s, "cosl_ba_solver_run_fixed")
+  COSL_TRY(s->rq.idle("cosl_ba_solver_run_fixed"));
   return run_robust(s, trials < 1 ? 1 : trials, info);
 }
 
 int cosl_ba_solver_download(cosl_ba_solver* s, cosl_ba_problem* prob) {
   BA_ENTER(s)
-  BA_IDLE(s, "cosl_ba_solver_download")
+  COSL_TRY(s->rq.idle("cosl_ba_solver_download"));
   if (!prob || prob->m != s->m || prob->n != s->n)
     return set_error(COSL_E_INVALID, "cosl_ba_solver_download: problem shape changed");
   return download(s, prob);
@@ -1667,47 +1638,35 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
     return set_error(COSL_E_INVALID,
                      "cosl_ba_solver_submit: a multi-rank solver exchanges over NCCL between host-ordered steps; "
                      "use cosl_ba_solver_run");
-  BA_IDLE(s, "cosl_ba_solver_submit")
+  COSL_TRY(s->rq.idle("cosl_ba_solver_submit"));
   // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
   if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
       s->graphNb != s->d_nb)
     COSL_TRY(build_graph(s));
-  if (!s->evSubmit) COSL_CUDA(cudaEventCreate(&s->evSubmit));
-  if (!s->evDone) COSL_CUDA(cudaEventCreate(&s->evDone));
-  COSL_CUDA(cudaEventRecord(s->evSubmit, s->stream));
-  COSL_CUDA(cudaGraphLaunch(s->graphExec, s->stream));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  COSL_CUDA(cudaEventRecord(s->evDone, s->stream));
-  s->inFlight = true;
-  return COSL_OK;
+  return s->rq.submit("cosl_ba_solver_submit", [&]() {
+    COSL_CUDA(cudaGraphLaunch(s->graphExec, s->rq.stream));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return (int)COSL_OK;
+  });
 }
 
 int cosl_ba_solver_query(cosl_ba_solver* s, int* done) {
   BA_ENTER(s)
   if (!done) return set_error(COSL_E_INVALID, "cosl_ba_solver_query: null argument");
-  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_ba_solver_query: nothing submitted");
-  const cudaError_t e = cudaEventQuery(s->evDone);
-  if (e == cudaErrorNotReady) {
-    *done = 0;
-    return COSL_OK;
-  }
-  COSL_CUDA(e);
-  *done = 1;
-  return COSL_OK;
+  COSL_TRY(s->rq.pending("cosl_ba_solver_query"));
+  return s->rq.query(done);
 }
 
 int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
-  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_ba_solver_collect: nothing submitted");
-  s->inFlight = false;
-  COSL_CUDA(cudaEventSynchronize(s->evDone));
+  COSL_TRY(s->rq.pending("cosl_ba_solver_collect"));
+  double ms = 0;
+  COSL_TRY(s->rq.wait(&ms));
   BaCtl c;
   double nout = 0;
-  COSL_CUDA(cudaMemcpyAsync(&c, s->d_ctl, sizeof(c), cudaMemcpyDeviceToHost, s->stream));
-  COSL_CUDA(cudaMemcpyAsync(&nout, s->d_sc + SC_COST, sizeof(double), cudaMemcpyDeviceToHost, s->stream));
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
-  float ms = 0.f;
-  COSL_CUDA(cudaEventElapsedTime(&ms, s->evSubmit, s->evDone));
+  COSL_CUDA(cudaMemcpyAsync(&c, s->d_ctl, sizeof(c), cudaMemcpyDeviceToHost, s->rq.stream));
+  COSL_CUDA(cudaMemcpyAsync(&nout, s->d_sc + SC_COST, sizeof(double), cudaMemcpyDeviceToHost, s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   if (info) {  // the fields of run_robust
     for (int k = 0; k < COSL_BA_INFOSZ; ++k) info[k] = 0;
     info[0] = c.first_e0;
@@ -1733,7 +1692,7 @@ int cosl_ba_solver_destroy(cosl_ba_solver* s) {
   return COSL_OK;
 }
 
-void* cosl_ba_solver_stream(cosl_ba_solver* s) { return s ? (void*)s->stream : nullptr; }
+void* cosl_ba_solver_stream(cosl_ba_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
 
 int cosl_ba_solver_stats(cosl_ba_solver* s, double out[8]) {
   if (!s || !out) return set_error(COSL_E_INVALID, "cosl_ba_solver_stats: null argument");
@@ -1770,14 +1729,14 @@ int cosl_ba_solver_trace(cosl_ba_solver* s, int enable, uint64_t* out, int32_t* 
   const int nt = (int)s->plan.tasks.size();
   if (enable) {
     COSL_TRY(grow(s, &s->d_trace, (size_t)std::max(1, nt) * 8));
-    COSL_CUDA(cudaMemsetAsync(s->d_trace, 0, sizeof(unsigned long long) * 8 * std::max(1, nt), s->stream));
+    COSL_CUDA(cudaMemsetAsync(s->d_trace, 0, sizeof(unsigned long long) * 8 * std::max(1, nt), s->rq.stream));
     s->td.trace = s->d_trace;
     return nt;
   }
   if (out && s->d_trace) {
     const int n = std::min(cap, nt);
-    COSL_CUDA(cudaMemcpyAsync(out, s->d_trace, sizeof(uint64_t) * 8 * n, cudaMemcpyDeviceToHost, s->stream));
-    COSL_CUDA(cudaStreamSynchronize(s->stream));
+    COSL_CUDA(cudaMemcpyAsync(out, s->d_trace, sizeof(uint64_t) * 8 * n, cudaMemcpyDeviceToHost, s->rq.stream));
+    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
     if (meta)
       for (int t = 0; t < n; ++t) {
         meta[3 * t] = s->taskOrder[t].type;
@@ -1905,7 +1864,7 @@ int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const dou
 
 int cosl_ba_solver_profile_enable(cosl_ba_solver* s, int on) {
   BA_ENTER(s)
-  COSL_CUDA(cudaStreamSynchronize(s->stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   s->timer.reset();
   s->timer.enabled = on != 0;
   return COSL_OK;
@@ -1914,7 +1873,7 @@ int cosl_ba_solver_profile_enable(cosl_ba_solver* s, int on) {
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls) {
   if (!s || idx < 0 || idx >= s->timer.nsec) return nullptr;
   cudaSetDevice(s->device);
-  cudaStreamSynchronize(s->stream);
+  cudaStreamSynchronize(s->rq.stream);
   s->timer.flush();
   if (ms) *ms = s->timer.ms[idx];
   if (calls) *calls = s->timer.calls[idx];

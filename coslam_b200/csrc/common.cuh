@@ -65,6 +65,48 @@ extern std::atomic<uint64_t> g_launches;
 inline int div_up(int a, int b) { return (a + b - 1) / b; }
 inline int64_t div_up64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// COSL_E_CUDA unless `device` is the ordinal of a visible CUDA device.
+int check_device(int device);
+
+// Gives the device's default memory pool an unlimited release threshold, once per device: after the first
+// request, cudaMallocAsync hands out buffers again without a device synchronisation or a trip to the driver's
+// allocator (cudaMalloc / cudaFree cost more than the kernels; cosl_ba_solve makes ~30 buffers, 0.7 GB at c4,
+// per call).
+void keep_pool(int device);
+
+// One request in flight on a handle's own non-blocking stream: the pose, pose-graph and BA solver handles.
+// evStart and evDone bracket the request's work.  The caller makes the handle's device current before
+// create / destroy / submit / query / wait, and calls idle / pending where its checks put the state check.
+struct RequestStream {
+  cudaStream_t stream = nullptr;
+  cudaEvent_t evStart = nullptr, evDone = nullptr;
+  bool inFlight = false;
+
+  int create();    // on the current device; destroy() cleans up after a failure
+  void destroy();  // waits for the stream first: a request in flight uses the handle's buffers
+  int idle(const char* fn) const;     // COSL_E_STATE while a request is in flight
+  int pending(const char* fn) const;  // COSL_E_STATE with nothing in flight
+  int query(int* done);               // *done = 1 once the request has finished, without waiting
+  int wait(double* device_ms);        // nothing is in flight afterwards; device_ms (nullable): evStart -> evDone
+
+  // Records evStart, runs `enqueue` (a COSL_ status), records evDone.  On a failure the stream is drained (a
+  // copy that was enqueued may still read a staging buffer) and nothing is in flight.
+  template <class F>
+  int submit(const char* fn, F enqueue) {
+    int rc = COSL_OK;
+    cudaError_t e = cudaEventRecord(evStart, stream);
+    if (e == cudaSuccess) {
+      rc = enqueue();
+      if (rc == COSL_OK) e = cudaEventRecord(evDone, stream);
+    }
+    if (rc == COSL_OK && e != cudaSuccess)
+      rc = set_error(COSL_E_CUDA, "%s: cudaEventRecord: %s", fn, cudaGetErrorString(e));
+    if (rc != COSL_OK) cudaStreamSynchronize(stream);
+    else inFlight = true;
+    return rc;
+  }
+};
+
 // simple per-stream section timer (CUDA events), used to report per-kernel-class device time
 struct SectionTimer {
   static const int kMaxSections = 16;

@@ -1206,9 +1206,7 @@ int cosl_klt_group_create_sizes(const cosl_klt_config* cfg, int nCams, const int
   if (cfg->windowWidth < 1 || cfg->windowWidth > 31 || cfg->minDistance < 1 ||
       cfg->minDistance > 32 || cfg->nIterations < 1)
     return set_error(COSL_E_INVALID, "bad tracker config");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
-    return set_error(COSL_E_CUDA, "CUDA device %d not available (%d devices)", device, ndev);
+  COSL_TRY(check_device(device));
   COSL_CUDA(cudaSetDevice(device));
   cosl_klt* g = new (std::nothrow) cosl_klt();
   if (!g) return set_error(COSL_E_NOMEM, "host allocation failed");

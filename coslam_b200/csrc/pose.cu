@@ -400,15 +400,13 @@ int check_cameras(const char* fn, int C, const int* npts, const double* const* M
 // pinned memory.  Capacity is fixed at create: everything is allocated once.
 struct cosl_pose_solver {
   int device = 0, maxCams = 0, maxPts = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t evStart = nullptr, evDone = nullptr;
+  RequestStream rq;
   unsigned char* h_in = nullptr;
   unsigned char* d_in = nullptr;
   double* d_W = nullptr;
   PoseOut* d_out = nullptr;
   PoseOut* h_out = nullptr;
   int C = 0;  // cameras of the solve in flight
-  bool inFlight = false;
 };
 
 namespace {
@@ -417,23 +415,18 @@ size_t input_bytes(int C, long long tot) { return sizeof(PoseCam) * C + sizeof(d
 
 void free_pose_solver(cosl_pose_solver* s) {
   cudaSetDevice(s->device);
-  if (s->stream) cudaStreamSynchronize(s->stream);  // a solve in flight reads and writes the buffers below
-  if (s->evStart) cudaEventDestroy(s->evStart);
-  if (s->evDone) cudaEventDestroy(s->evDone);
+  s->rq.destroy();
   if (s->h_in) cudaFreeHost(s->h_in);
   if (s->h_out) cudaFreeHost(s->h_out);
   cudaFree(s->d_in);
   cudaFree(s->d_W);
   cudaFree(s->d_out);
-  if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
 
 int alloc_pose_solver(cosl_pose_solver* s) {
   COSL_CUDA(cudaSetDevice(s->device));
-  COSL_CUDA(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
-  COSL_CUDA(cudaEventCreate(&s->evStart));
-  COSL_CUDA(cudaEventCreate(&s->evDone));
+  COSL_TRY(s->rq.create());
   const size_t in = input_bytes(s->maxCams, s->maxPts);
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
   COSL_CUDA(cudaHostAlloc(&s->h_out, sizeof(PoseOut) * s->maxCams, cudaHostAllocPortable));
@@ -443,18 +436,17 @@ int alloc_pose_solver(cosl_pose_solver* s) {
   return COSL_OK;
 }
 
-// The staged inputs of C cameras and tot points: copy, kernel, read-back, between the two events.
+// The staged inputs of C cameras and tot points: copy, kernel, read-back.
 int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg) {
   const PoseCam* d_cams = reinterpret_cast<const PoseCam*>(s->d_in);
   const double* d_M = reinterpret_cast<const double*>(s->d_in + sizeof(PoseCam) * C);
   const double* d_m = d_M + 3 * tot;
   const double* d_p = d_m + 2 * tot;
-  COSL_CUDA(cudaEventRecord(s->evStart, s->stream));
-  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, input_bytes(C, tot), cudaMemcpyHostToDevice, s->stream));
-  COSL_LAUNCH(pose_intracam_kernel, C, POSE_THREADS, 0, s->stream, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out);
+  cudaStream_t st = s->rq.stream;
+  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, input_bytes(C, tot), cudaMemcpyHostToDevice, st));
+  COSL_LAUNCH(pose_intracam_kernel, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out);
   COSL_CUDA(cudaGetLastError());
-  COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, s->stream));
-  COSL_CUDA(cudaEventRecord(s->evDone, s->stream));
+  COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, st));
   return COSL_OK;
 }
 
@@ -477,9 +469,7 @@ int cosl_pose_solver_create(int device, int maxCams, int maxPts, cosl_pose_solve
   if (!out || device < 0 || maxCams < 1 || maxPts < 0)
     return set_error(COSL_E_INVALID, "cosl_pose_solver_create: bad argument");
   *out = nullptr;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device >= ndev)
-    return set_error(COSL_E_CUDA, "CUDA device %d not available", device);
+  COSL_TRY(check_device(device));
   cosl_pose_solver* s = new (std::nothrow) cosl_pose_solver;
   if (!s) return set_error(COSL_E_NOMEM, "cosl_pose_solver_create: out of host memory");
   s->device = device;
@@ -504,7 +494,7 @@ int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const 
                             const int* npts, const double* const* Ms, const double* const* ms,
                             const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
   if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
-  if (s->inFlight) return set_error(COSL_E_STATE, "cosl_pose_solver_submit: a submitted solve is not collected yet");
+  COSL_TRY(s->rq.idle("cosl_pose_solver_submit"));
   if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !opts)
     return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: null argument");
   if (C > s->maxCams)
@@ -543,43 +533,24 @@ int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const 
   cfg.epsRW = opts[0].epsErrorChangeRW;
   cfg.lambda0 = opts[0].lambda0;
   cfg.tau = tau;
-  const int rc = enqueue_solve(s, C, tot, cfg);
-  if (rc != COSL_OK) {
-    cudaStreamSynchronize(s->stream);  // a copy that was enqueued may still read the staging buffer
-    return rc;
-  }
   s->C = C;
-  s->inFlight = true;
-  return COSL_OK;
+  return s->rq.submit("cosl_pose_solver_submit", [&]() { return enqueue_solve(s, C, tot, cfg); });
 }
 
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done) {
   if (!s || !done) return set_error(COSL_E_INVALID, "cosl_pose_solver_query: null argument");
-  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_pose_solver_query: nothing submitted");
+  COSL_TRY(s->rq.pending("cosl_pose_solver_query"));
   COSL_CUDA(cudaSetDevice(s->device));
-  const cudaError_t e = cudaEventQuery(s->evDone);
-  if (e == cudaErrorNotReady) {
-    *done = 0;
-    return COSL_OK;
-  }
-  COSL_CUDA(e);
-  *done = 1;
-  return COSL_OK;
+  return s->rq.query(done);
 }
 
 int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, cosl_pose_opt* opts, int* ok,
                              double* device_ms) {
   if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
-  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_pose_solver_collect: nothing submitted");
+  COSL_TRY(s->rq.pending("cosl_pose_solver_collect"));
   if (!R_opt || !t_opt || !opts) return set_error(COSL_E_INVALID, "cosl_pose_solver_collect: null argument");
   COSL_CUDA(cudaSetDevice(s->device));
-  s->inFlight = false;
-  COSL_CUDA(cudaEventSynchronize(s->evDone));
-  if (device_ms) {
-    float ms = 0.f;
-    COSL_CUDA(cudaEventElapsedTime(&ms, s->evStart, s->evDone));
-    *device_ms = ms;
-  }
+  COSL_TRY(s->rq.wait(device_ms));
   const PoseOut* outs = s->h_out;
   for (int c = 0; c < s->C; ++c) {
     std::memcpy(R_opt + 9 * c, outs[c].R, sizeof(double) * 9);
@@ -598,7 +569,7 @@ int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, 
   return COSL_OK;
 }
 
-void* cosl_pose_solver_stream(cosl_pose_solver* s) { return s ? (void*)s->stream : nullptr; }
+void* cosl_pose_solver_stream(cosl_pose_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
 
 int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const double* t0,
                              const int* npts, const double* const* Ms, const double* const* ms,
@@ -606,9 +577,7 @@ int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const do
                              double* t_opt, cosl_pose_opt* opts, int* ok, int device) {
   if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !R_opt || !t_opt || !opts)
     return set_error(COSL_E_INVALID, "cosl_pose_intracam_batch: null argument");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
-    return set_error(COSL_E_CUDA, "CUDA device %d not available", device);
+  COSL_TRY(check_device(device));
   long long tot = 0;
   COSL_TRY(check_cameras("cosl_pose_intracam_batch", C, npts, Ms, ms, opts, &tot));
   // one library-owned handle per device, reused across calls (the solve is latency-bound: an allocation per

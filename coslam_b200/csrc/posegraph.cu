@@ -28,7 +28,6 @@
 #include <cmath>
 #include <functional>
 #include <map>
-#include <mutex>
 #include <new>
 #include <utility>
 #include <vector>
@@ -368,22 +367,6 @@ posegraph_chain_kernel(const int* __restrict__ chainOff, const unsigned char* __
     for (int i = 0; i < 9; ++i) newR[9 * (size_t)g + i] = R[9 * (size_t)g + i];
 #pragma unroll
     for (int i = 0; i < 3; ++i) newt[3 * (size_t)g + i] = t[3 * (size_t)g + i];
-  }
-}
-
-// Stream-ordered allocation from the device's default pool: after the first call a slab comes out of
-// the pool without a device synchronisation (cudaMalloc / cudaFree cost more than the kernels).
-void keep_pool(int device) {
-  static std::mutex mu;
-  static bool kept[64] = {};
-  std::lock_guard<std::mutex> lk(mu);
-  if (device >= 0 && device < 64 && !kept[device]) {
-    kept[device] = true;
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
-      unsigned long long keep = ~0ull;
-      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-    }
   }
 }
 
@@ -1120,30 +1103,23 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
 // pinned staging buffers serve both kinds and grow when a request does not fit.
 struct cosl_posegraph_solver {
   int device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t evStart = nullptr, evDone = nullptr;
-  char* slab = nullptr;  // from the device's stream-ordered pool, on `stream`
+  RequestStream rq;
+  char* slab = nullptr;  // from the device's stream-ordered pool, on rq.stream
   char* h_in = nullptr;  // pinned: the packed inputs
   char* h_out = nullptr; // pinned: the output region of the slab
   size_t slabBytes = 0, inBytes = 0, outBytes = 0;
-  bool inFlight = false, chains = false;  // the request in flight: a chain spread or a general solve
-  int N = 0, nScale = 0;                  // its nodes (0: nothing to write) and scale columns
+  bool chains = false;    // the request in flight: a chain spread or a general solve
+  int N = 0, nScale = 0;  // its nodes (0: nothing to write) and scale columns
 };
 
 namespace {
 
 void free_pg_solver(cosl_posegraph_solver* s) {
   cudaSetDevice(s->device);
-  if (s->stream) {
-    cudaStreamSynchronize(s->stream);  // a request in flight reads and writes the buffers below
-    if (s->slab) cudaFreeAsync(s->slab, s->stream);
-    cudaStreamSynchronize(s->stream);
-  }
-  if (s->evStart) cudaEventDestroy(s->evStart);
-  if (s->evDone) cudaEventDestroy(s->evDone);
+  if (s->slab) cudaFreeAsync(s->slab, s->rq.stream);
+  s->rq.destroy();
   if (s->h_in) cudaFreeHost(s->h_in);
   if (s->h_out) cudaFreeHost(s->h_out);
-  if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
 
@@ -1168,10 +1144,10 @@ int grow_pinned(const char* fn, char** buf, size_t* cap, size_t need) {
 // the handle's stream, and the new one comes out of it without a device synchronisation.
 int grow_slab(const char* fn, cosl_posegraph_solver* s, size_t need) {
   if (need <= s->slabBytes) return COSL_OK;
-  if (s->slab) cudaFreeAsync(s->slab, s->stream);
+  if (s->slab) cudaFreeAsync(s->slab, s->rq.stream);
   s->slab = nullptr;
   s->slabBytes = 0;
-  const cudaError_t e = cudaMallocAsync(&s->slab, need, s->stream);
+  const cudaError_t e = cudaMallocAsync(&s->slab, need, s->rq.stream);
   if (e != cudaSuccess) {
     s->slab = nullptr;
     cudaGetLastError();
@@ -1190,23 +1166,6 @@ StageFn stage_pinned(const char* fn, cosl_posegraph_solver* s) {
   };
 }
 
-// Records the start event, runs `enqueue`, records the end event.  On a failure the stream is drained (a copy
-// that was enqueued may still read the staging buffer) and nothing is in flight.
-template <class F>
-int submit_timed(cosl_posegraph_solver* s, F enqueue) {
-  int rc = COSL_OK;
-  cudaError_t e = cudaEventRecord(s->evStart, s->stream);
-  if (e == cudaSuccess) {
-    rc = enqueue();
-    if (rc == COSL_OK) e = cudaEventRecord(s->evDone, s->stream);
-  }
-  if (rc == COSL_OK && e != cudaSuccess)
-    rc = set_error(COSL_E_CUDA, "cosl_posegraph_solver: cudaEventRecord: %s", cudaGetErrorString(e));
-  if (rc != COSL_OK) cudaStreamSynchronize(s->stream);
-  else s->inFlight = true;
-  return rc;
-}
-
 }  // namespace
 
 extern "C" {
@@ -1214,19 +1173,14 @@ extern "C" {
 int cosl_posegraph_solver_create(int device, cosl_posegraph_solver** out) {
   if (!out || device < 0) return set_error(COSL_E_INVALID, "cosl_posegraph_solver_create: bad argument");
   *out = nullptr;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device >= ndev)
-    return set_error(COSL_E_CUDA, "CUDA device %d not available", device);
+  COSL_TRY(check_device(device));
   cosl_posegraph_solver* s = new (std::nothrow) cosl_posegraph_solver;
   if (!s) return set_error(COSL_E_NOMEM, "cosl_posegraph_solver_create: out of host memory");
   s->device = device;
   auto init = [&]() {
     COSL_CUDA(cudaSetDevice(device));
     keep_pool(device);
-    COSL_CUDA(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
-    COSL_CUDA(cudaEventCreate(&s->evStart));
-    COSL_CUDA(cudaEventCreate(&s->evDone));
-    return (int)COSL_OK;
+    return s->rq.create();
   };
   const int rc = init();
   if (rc != COSL_OK) {
@@ -1248,7 +1202,7 @@ int cosl_posegraph_solver_submit_chains(cosl_posegraph_solver* s, int nChains, c
                                         const double* eR, const double* et) {
   const char* fn = "cosl_posegraph_solver_submit_chains";
   if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
-  if (s->inFlight) return set_error(COSL_E_STATE, "%s: a submitted solve is not collected yet", fn);
+  COSL_TRY(s->rq.idle(fn));
   COSL_CUDA(cudaSetDevice(s->device));
   ChainJob j;
   COSL_TRY(chain_prepare(fn, nChains, chainOff, fixed, R, t, eR, et, nullptr, stage_pinned(fn, s), j));
@@ -1259,8 +1213,8 @@ int cosl_posegraph_solver_submit_chains(cosl_posegraph_solver* s, int nChains, c
   s->chains = true;
   s->N = j.N;
   s->nScale = 0;
-  return submit_timed(s, [&]() {
-    return j.N > 0 ? chain_enqueue(fn, j, s->slab, s->stream, s->h_out, nullptr, nullptr, nullptr) : (int)COSL_OK;
+  return s->rq.submit(fn, [&]() {
+    return j.N > 0 ? chain_enqueue(fn, j, s->slab, s->rq.stream, s->h_out, nullptr, nullptr, nullptr) : (int)COSL_OK;
   });
 }
 
@@ -1269,7 +1223,7 @@ int cosl_posegraph_solver_submit(cosl_posegraph_solver* s, int nNodes, const uin
                                  const double* et, const int* scaleCol, int nScale) {
   const char* fn = "cosl_posegraph_solver_submit";
   if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
-  if (s->inFlight) return set_error(COSL_E_STATE, "%s: a submitted solve is not collected yet", fn);
+  COSL_TRY(s->rq.idle(fn));
   COSL_CUDA(cudaSetDevice(s->device));
   PgJob j;
   COSL_TRY(pg_prepare(fn, nNodes, fixed, R, t, nEdges, id1, id2, eR, et, scaleCol, nScale, nullptr,
@@ -1287,41 +1241,28 @@ int cosl_posegraph_solver_submit(cosl_posegraph_solver* s, int nNodes, const uin
   s->chains = false;
   s->N = N;
   s->nScale = nScale;
-  return submit_timed(s, [&]() {
-    return j.nF > 0 ? pg_enqueue(fn, j, s->slab, s->h_in, reinterpret_cast<double*>(s->h_out), s->device, s->stream)
+  return s->rq.submit(fn, [&]() {
+    return j.nF > 0 ? pg_enqueue(fn, j, s->slab, s->h_in, reinterpret_cast<double*>(s->h_out), s->device, s->rq.stream)
                     : (int)COSL_OK;
   });
 }
 
 int cosl_posegraph_solver_query(cosl_posegraph_solver* s, int* done) {
   if (!s || !done) return set_error(COSL_E_INVALID, "cosl_posegraph_solver_query: null argument");
-  if (!s->inFlight) return set_error(COSL_E_STATE, "cosl_posegraph_solver_query: nothing submitted");
+  COSL_TRY(s->rq.pending("cosl_posegraph_solver_query"));
   COSL_CUDA(cudaSetDevice(s->device));
-  const cudaError_t e = cudaEventQuery(s->evDone);
-  if (e == cudaErrorNotReady) {
-    *done = 0;
-    return COSL_OK;
-  }
-  COSL_CUDA(e);
-  *done = 1;
-  return COSL_OK;
+  return s->rq.query(done);
 }
 
 int cosl_posegraph_solver_collect(cosl_posegraph_solver* s, double* newR, double* newt, double* scale,
                                   double* device_ms) {
   const char* fn = "cosl_posegraph_solver_collect";
   if (!s) return set_error(COSL_E_INVALID, "null pose-graph solver handle");
-  if (!s->inFlight) return set_error(COSL_E_STATE, "%s: nothing submitted", fn);
+  COSL_TRY(s->rq.pending(fn));
   if ((s->N > 0 && (!newR || !newt)) || (s->nScale > 0 && !scale))
     return set_error(COSL_E_INVALID, "%s: null output array", fn);
   COSL_CUDA(cudaSetDevice(s->device));
-  s->inFlight = false;
-  COSL_CUDA(cudaEventSynchronize(s->evDone));
-  if (device_ms) {
-    float ms = 0.f;
-    COSL_CUDA(cudaEventElapsedTime(&ms, s->evStart, s->evDone));
-    *device_ms = ms;
-  }
+  COSL_TRY(s->rq.wait(device_ms));
   const int N = s->N;
   if (!s->chains) return pg_result(fn, N, s->nScale, reinterpret_cast<const double*>(s->h_out), newR, newt, scale);
   if (N == 0) return COSL_OK;
@@ -1334,6 +1275,6 @@ int cosl_posegraph_solver_collect(cosl_posegraph_solver* s, double* newR, double
   return COSL_OK;
 }
 
-void* cosl_posegraph_solver_stream(cosl_posegraph_solver* s) { return s ? (void*)s->stream : nullptr; }
+void* cosl_posegraph_solver_stream(cosl_posegraph_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
 
 }  // extern "C"
