@@ -98,6 +98,8 @@ def _load():
     L.cosl_ba_solver_submit.argtypes = [vp]
     L.cosl_ba_solver_query.argtypes = [vp, pint]
     L.cosl_ba_solver_collect.argtypes = [vp, vp]
+    L.cosl_ba_solver_stop.argtypes = [vp]
+    L.cosl_ba_solver_progress.argtypes = [vp, C.POINTER(cd)]
     L.cosl_ba_solver_download.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_destroy.argtypes = [vp]
     L.cosl_ba_solver_stream.argtypes = [vp]
@@ -795,6 +797,18 @@ class BaSolver(_SolverHandle):
         info = np.zeros(COSL_BA_INFOSZ)
         _ck(LIB.cosl_ba_solver_collect(self.h, _ptr(info)))
         return info
+
+    def stop(self):
+        """cosl_ba_solver_stop: ask the running or submitted BA to end at its next decision point (stop
+        reason 8); returns at once.  May be called from another thread while one is inside run / collect."""
+        _ck(LIB.cosl_ba_solver_stop(self.h))
+
+    def progress(self):
+        """cosl_ba_solver_progress: where the running or last BA is, without waiting for it."""
+        out = (C.c_double * 8)()
+        _ck(LIB.cosl_ba_solver_progress(self.h, out))
+        return {"running": bool(out[0]), "round": int(out[1]), "iteration": int(out[2]), "trials": int(out[3]),
+                "cost": out[4], "init_cost": out[5], "mu": out[6], "stop_requested": bool(out[7])}
 
     def download(self, into=None):
         """Current cameras and points into the solver's problem, or into `into` (same shape)."""

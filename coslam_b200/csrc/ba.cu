@@ -232,6 +232,18 @@ struct cosl_ba_solver {
   cudaGraphExec_t graphExec = nullptr;
   bool graphStale = false;  // a load changed the problem since the graph was built
   const double *graphPa = nullptr, *graphNa = nullptr, *graphPb = nullptr, *graphNb = nullptr;
+  // stop / progress (cosl_ba_solver_stop / _progress), the calls another thread may make while one is inside
+  // run / submit / collect.  Every run and submit takes the next request number; a stop names the current one.
+  BaCtlLink* d_link = nullptr;        // request number, stop word and progress record of the submitted loop
+  cudaStream_t sideStream = nullptr;  // the copies of stop and progress
+  std::mutex sideMu;                  // the side stream and its pinned slots (h_sc + BA_PIN_*)
+  std::atomic<unsigned long long> reqNo{0}, stopReq{0};
+  std::atomic<int> reqKind{0};     // of the last request: 0 none, 1 run (host loop), 2 submit (graph)
+  std::atomic<int> hostRunning{0}, submitted{0};
+  unsigned long long loopReq = 0;  // the request the host loop runs; 0: not stoppable (run_fixed, cosl_ba_solve)
+  std::mutex hostProgMu;
+  BaProgress hostProg = {};        // the host loop's progress record
+  int hpRound = 0, hpTrials0 = 0;  // round (1-based) and the trials of earlier rounds, for levmar's record
 };
 
 namespace {
@@ -294,8 +306,15 @@ void quat_mul(const double a[4], const double b[4], double p[4]) {
   p[3] = a[0] * b[3] + a[1] * b[2] - a[2] * b[1] + a[3] * b[0];
 }
 
-// Pinned 128-byte slots for the per-trial scalar read-back.  cudaMallocHost / cudaFreeHost cost
-// milliseconds each; a drop-in call creates and destroys a solver, so the slots are pooled.
+// Pinned slots for the per-trial scalar read-back.  cudaMallocHost / cudaFreeHost cost milliseconds
+// each; a drop-in call creates and destroys a solver, so the slots are pooled.
+enum {
+  BA_PIN_REQ = 20,   // the request number the submit copies to the device
+  BA_PIN_STOP = 24,  // the stop word cosl_ba_solver_stop copies to the device
+  BA_PIN_PROG = 32,  // two copies of the progress record (8 doubles each)
+  BA_PIN_SLOT = 48   // doubles per slot
+};
+static_assert(sizeof(BaProgress) == 8 * sizeof(double), "progress record size");
 struct PinnedSlots {
   std::mutex mu;
   std::vector<double*> free_;
@@ -308,10 +327,11 @@ struct PinnedSlots {
     }
     double* p = nullptr;
     // 16 scalars + the sequence flag of ba_publish_sc; mapped + portable: every device of the process writes
-    // its scalars straight into this host memory (UVA: the host pointer is the device pointer)
-    if (cudaHostAlloc(&p, sizeof(double) * 32, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess)
+    // its scalars straight into this host memory (UVA: the host pointer is the device pointer).  Then the
+    // sources and targets of the request-number, stop and progress copies (BA_PIN_*).
+    if (cudaHostAlloc(&p, sizeof(double) * BA_PIN_SLOT, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess)
       return nullptr;
-    std::memset(p, 0, sizeof(double) * 32);
+    std::memset(p, 0, sizeof(double) * BA_PIN_SLOT);
     return p;
   }
   void put(double* p) {
@@ -484,6 +504,10 @@ void free_solver(cosl_ba_solver* s) {
   if (!s) return;
   cudaSetDevice(s->device);
   if (s->rq.stream) cudaStreamSynchronize(s->rq.stream);
+  if (s->sideStream) {
+    cudaStreamSynchronize(s->sideStream);
+    cudaStreamDestroy(s->sideStream);
+  }
   s->timer.destroy();
   if (s->graphExec) cudaGraphExecDestroy(s->graphExec);
   if (s->evStaged) cudaEventDestroy(s->evStaged);
@@ -894,6 +918,9 @@ int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver**
   s->scSeq = 0;
   COSL_CUDA(cudaEventCreateWithFlags(&s->evStaged, cudaEventDisableTiming));
   COSL_TRY(grow(s, &s->d_sc, (size_t)SC_NTOT));
+  COSL_CUDA(cudaStreamCreateWithFlags(&s->sideStream, cudaStreamNonBlocking));
+  COSL_TRY(grow(s, &s->d_link, 1));
+  COSL_CUDA(cudaMemsetAsync(s->d_link, 0, sizeof(BaCtlLink), s->rq.stream));  // request numbers start at 1
   COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_schur_pairs_st, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_ST_SMEM));
@@ -1118,7 +1145,29 @@ int solve_trial(cosl_ba_solver* s, double mu, bool* solved) {
   return COSL_OK;
 }
 
-/* Weighted SBA LM, control flow identical to oracle/ba_oracle.cpp:levmar */
+// The host loop's stop test (ba_ctl_stop_asked of the submitted loop): only a run through the handle stops.
+bool host_stop_asked(const cosl_ba_solver* s) {
+  return s->loopReq && s->stopReq.load(std::memory_order_relaxed) == s->loopReq;
+}
+
+// The host loop's progress record (ba_ctl_publish of the submitted loop)
+void host_publish(cosl_ba_solver* s, int round, int itno, int trials, double p_eL2, double init_eL2, double mu) {
+  if (!s->loopReq) return;
+  std::lock_guard<std::mutex> lk(s->hostProgMu);
+  BaProgress& g = s->hostProg;
+  g.seq0 = g.seq1 = g.seq1 + 1;
+  g.req = s->loopReq;
+  g.round = round;
+  g.itno = itno;
+  g.trials = trials;
+  g.p_eL2 = p_eL2;
+  g.init_eL2 = init_eL2;
+  g.mu = mu;
+}
+
+/* Weighted SBA LM, control flow identical to oracle/ba_oracle.cpp:levmar.  Through the handle
+ * (s->loopReq) it also ends the round with reason 8 when the caller asks to stop, at the points where the
+ * submitted loop checks (ba_ctl.cuh), and keeps the progress record. */
 int levmar(cosl_ba_solver* s, int itmax, const double opts[5], double info[10], int fixed_trials) {
   const double tau = opts[0], eps1 = opts[1], eps2 = opts[2], eps2_sq = opts[2] * opts[2],
                eps3 = opts[3], eps4 = opts[4];
@@ -1132,6 +1181,7 @@ int levmar(cosl_ba_solver* s, int itmax, const double opts[5], double info[10], 
   const double init_eL2 = p_eL2;
   double ginf = 0, maxdiag = 0, dp_L2 = 0;
   if (!finite) stop = 7;
+  host_publish(s, s->hpRound, 0, s->hpTrials0, p_eL2, init_eL2, mu);
   for (itno = 0; itno < itmax && !stop; ++itno) {
     COSL_TRY(linearize(s, itno == 0, itno > 0 && !fixed_trials));
     // ginf / maxdiag are needed on the host for mu0 (first iteration) and for the eps1 stop test.  After
@@ -1152,6 +1202,11 @@ int levmar(cosl_ba_solver* s, int itmax, const double opts[5], double info[10], 
       break;
     }
     if (itno == 0) mu = tau * maxdiag;
+    if (host_stop_asked(s)) {  // into the first trial of the iteration: it is not counted
+      stop = BA_STOP_CALLER;
+      break;
+    }
+    host_publish(s, s->hpRound, itno, s->hpTrials0 + s->nlss, p_eL2, init_eL2, mu);
     bool lateStop = false;
     while (true) {
       bool solved = false, accepted = false;
@@ -1227,9 +1282,17 @@ int levmar(cosl_ba_solver* s, int itmax, const double opts[5], double info[10], 
         break;
       }
       nu = nu2;
+      host_publish(s, s->hpRound, itno, s->hpTrials0 + s->nlss, p_eL2, init_eL2, mu);
+      if (host_stop_asked(s)) {  // into the next trial: the iteration is not counted
+        stop = BA_STOP_CALLER;
+        lateStop = true;
+        break;
+      }
     }
     if (lateStop) break;
     if (!fixed_trials && p_eL2 <= eps3) stop = 3;
+    if (itno + 1 < itmax && !stop && host_stop_asked(s)) stop = BA_STOP_CALLER;  // into the next linearisation
+    host_publish(s, s->hpRound, itno + 1, s->hpTrials0 + s->nlss, p_eL2, init_eL2, mu);
   }
   if (itno >= itmax && !stop) stop = 3;
   if (info) {
@@ -1254,13 +1317,24 @@ int run_robust(cosl_ba_solver* s, int fixed_trials, double info[COSL_BA_INFOSZ])
   COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   const auto t0 = std::chrono::steady_clock::now();
   const int rounds = fixed_trials ? 1 : std::max(1, s->opt.outer_iters);
+  int ran = 0;
   for (int r = 0; r < rounds; ++r) {
+    if (r > 0 && host_stop_asked(s)) {  // into the next round: the round that ended reports the stop
+      sinfo[6] = BA_STOP_CALLER;
+      break;
+    }
+    s->hpRound = r + 1;
+    s->hpTrials0 = total_trials;
     COSL_TRY(compute_weights(s));
     COSL_TRY(levmar(s, fixed_trials ? (1 << 30) : s->opt.inner_iters, s->opt.opts, sinfo,
                     fixed_trials));
     if (first_e0 < 0) first_e0 = sinfo[0];
     total_trials += (int)sinfo[9];
+    ++ran;
+    if (sinfo[6] == BA_STOP_CALLER) break;
   }
+  // the final record: what info reports (mu as levmar last left it; only this thread writes the record)
+  host_publish(s, ran, (int)sinfo[5], total_trials, sinfo[1], sinfo[0], s->hostProg.mu);
   double nout = 0;
   if (s->opt.max_err > 0) {  // the same branch on every rank (options are global): collective inside
     COSL_TRY(zero_sc(s, SC_COST, 1));
@@ -1420,6 +1494,7 @@ int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
   P.ns = s->ns;
   P.hasObs = s->N > 0;
   P.outliers = s->opt.max_err > 0;
+  P.link = s->d_link;
   COSL_CUDA(cudaGraphConditionalHandleCreate(&P.hLoop, g, 1, cudaGraphCondAssignDefault));
   for (int k = 0; k < BA_NSTAGES; ++k)
     COSL_CUDA(cudaGraphConditionalHandleCreate(&P.hStage[k], g, k == BA_STAGE_ROUND ? 1 : 0, cudaGraphCondAssignDefault));
@@ -1615,7 +1690,14 @@ int cosl_ba_solver_load(cosl_ba_solver* s, const cosl_ba_problem* prob) {
 int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
   COSL_TRY(s->rq.idle("cosl_ba_solver_run"));
-  return run_robust(s, 0, info);
+  s->loopReq = s->reqNo.load() + 1;
+  s->reqKind.store(1);
+  s->hostRunning.store(1);
+  s->reqNo.store(s->loopReq);
+  const int rc = run_robust(s, 0, info);
+  s->hostRunning.store(0);
+  s->loopReq = 0;
+  return rc;
 }
 
 int cosl_ba_solver_run_fixed(cosl_ba_solver* s, int trials, double info[COSL_BA_INFOSZ]) {
@@ -1643,11 +1725,21 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
   if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
       s->graphNb != s->d_nb)
     COSL_TRY(build_graph(s));
-  return s->rq.submit("cosl_ba_solver_submit", [&]() {
+  // the request number goes to the device ahead of the graph, on the solver's stream: a stop made before the
+  // graph starts names it too (the pinned source is not rewritten before this request is collected)
+  const unsigned long long req = s->reqNo.load() + 1;
+  *reinterpret_cast<volatile unsigned long long*>(s->h_sc + BA_PIN_REQ) = req;
+  COSL_CUDA(cudaMemcpyAsync(&s->d_link->req, s->h_sc + BA_PIN_REQ, sizeof(req), cudaMemcpyHostToDevice,
+                            s->rq.stream));
+  s->reqKind.store(2);
+  s->reqNo.store(req);
+  const int rc = s->rq.submit("cosl_ba_solver_submit", [&]() {
     COSL_CUDA(cudaGraphLaunch(s->graphExec, s->rq.stream));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return (int)COSL_OK;
   });
+  if (rc == COSL_OK) s->submitted.store(1);
+  return rc;
 }
 
 int cosl_ba_solver_query(cosl_ba_solver* s, int* done) {
@@ -1661,7 +1753,9 @@ int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
   COSL_TRY(s->rq.pending("cosl_ba_solver_collect"));
   double ms = 0;
-  COSL_TRY(s->rq.wait(&ms));
+  const int waited = s->rq.wait(&ms);
+  s->submitted.store(0);
+  COSL_TRY(waited);
   BaCtl c;
   double nout = 0;
   COSL_CUDA(cudaMemcpyAsync(&c, s->d_ctl, sizeof(c), cudaMemcpyDeviceToHost, s->rq.stream));
@@ -1684,6 +1778,70 @@ int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
     info[12] = c.p_eL2;
     info[13] = s->opt.max_err > 0 ? nout : 0.0;
   }
+  return COSL_OK;
+}
+
+int cosl_ba_solver_stop(cosl_ba_solver* s) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_stop: each rank of a multi-rank solver would stop at a "
+                     "different trial");
+  std::lock_guard<std::mutex> lk(s->sideMu);
+  const unsigned long long req = s->reqNo.load();
+  s->stopReq.store(req);  // the host loop's stop word
+  if (!req) return COSL_OK;
+  // the submitted loop's: a copy on the side stream, never behind the solver's stream.  A copy still queued
+  // from an earlier stop reads the newer number, which names a request that was asked to stop as well.
+  *reinterpret_cast<volatile unsigned long long*>(s->h_sc + BA_PIN_STOP) = req;
+  COSL_CUDA(cudaMemcpyAsync(&s->d_link->stop, s->h_sc + BA_PIN_STOP, sizeof(req), cudaMemcpyHostToDevice,
+                            s->sideStream));
+  return COSL_OK;
+}
+
+int cosl_ba_solver_progress(cosl_ba_solver* s, double out[8]) {
+  BA_ENTER(s)
+  if (!out) return set_error(COSL_E_INVALID, "cosl_ba_solver_progress: null argument");
+  const int kind = s->reqKind.load();
+  const unsigned long long req = s->reqNo.load();
+  BaProgress g = {};
+  int running = 0;
+  if (kind == 1) {
+    std::lock_guard<std::mutex> lk(s->hostProgMu);
+    g = s->hostProg;
+    running = s->hostRunning.load();
+  } else if (kind == 2) {
+    if (s->submitted.load()) {
+      const cudaError_t q = cudaEventQuery(s->rq.evDone);
+      if (q != cudaSuccess && q != cudaErrorNotReady)
+        return set_error(COSL_E_CUDA, "cosl_ba_solver_progress: %s", cudaGetErrorString(q));
+      running = q == cudaErrorNotReady;
+    }
+    // two copies of the record, one after the other: taken when both agree and neither raced a write
+    std::lock_guard<std::mutex> lk(s->sideMu);
+    BaProgress* h = reinterpret_cast<BaProgress*>(s->h_sc + BA_PIN_PROG);
+    for (int attempt = 0;; ++attempt) {
+      COSL_CUDA(cudaMemcpyAsync(h, &s->d_link->prog, sizeof(BaProgress), cudaMemcpyDeviceToHost,
+                                s->sideStream));
+      COSL_CUDA(cudaMemcpyAsync(h + 1, &s->d_link->prog, sizeof(BaProgress), cudaMemcpyDeviceToHost,
+                                s->sideStream));
+      COSL_CUDA(cudaStreamSynchronize(s->sideStream));
+      if (h[0].seq0 == h[0].seq1 && !std::memcmp(&h[0], &h[1], sizeof(BaProgress))) break;
+      if (attempt == 1000)
+        return set_error(COSL_E_CUDA, "cosl_ba_solver_progress: no consistent copy of the progress record");
+    }
+    g = h[0];
+  }
+  for (int k = 0; k < 8; ++k) out[k] = 0.0;
+  out[0] = running;
+  if (kind && g.req == req) {  // otherwise the request has not reached its first decision
+    out[1] = g.round;
+    out[2] = g.itno;
+    out[3] = g.trials;
+    out[4] = g.p_eL2;
+    out[5] = g.init_eL2;
+    out[6] = g.mu;
+  }
+  out[7] = (req && s->stopReq.load() == req) ? 1.0 : 0.0;
   return COSL_OK;
 }
 

@@ -25,11 +25,36 @@ struct BaCtl {
   int done;
 };
 
+// stop reason of a loop ended by cosl_ba_solver_stop
+enum { BA_STOP_CALLER = 8 };
+
+// What ba_ctl_step publishes after every decision (cosl_ba_solver_progress).  seq0 is written first and
+// seq1 last, each with a fence, so a copy with seq0 != seq1 raced a write.
+struct BaProgress {
+  unsigned long long seq0, req;  // req: the request the record belongs to
+  double p_eL2, init_eL2, mu;
+  int round;   // rounds started (the rounds run once the loop has ended)
+  int itno;    // counted iterations of the round
+  int trials;  // LM trials over all rounds
+  int pad;
+  unsigned long long seq1;
+};
+
+// Device memory shared by the solver's stream and the side stream of stop / progress (one per solver):
+// req is the number of the submitted request, written on the solver's stream before its graph; stop is
+// the number of the request the caller asked to stop, written on the side stream.  They match only while
+// the request that was asked to stop runs.
+struct BaCtlLink {
+  unsigned long long req, stop;
+  BaProgress prog;
+};
+
 // fixed for the life of a graph (the options of a solver do not change)
 struct BaCtlParams {
   double tau, eps1, eps2, eps3, eps4;
   int rounds, itmax, ns, hasObs, outliers;
   cudaGraphConditionalHandle hLoop, hStage[BA_NSTAGES];
+  BaCtlLink* link;
 };
 
 __global__ void ba_fill_f64(double* __restrict__ p, long long n, double v) {
@@ -139,14 +164,25 @@ __device__ void ba_ctl_goto(BaCtl* c, double* sc, const BaCtlParams& P, int next
   }
 }
 
+// Has the caller asked to stop this request?  Read at every transition into a further stage: LIN after a
+// finished iteration, TRIAL after a linearisation or a rejected trial, ROUND for the next round.  The stop
+// word is written by a copy on another stream while the loop runs, hence the volatile load.
+__device__ bool ba_ctl_stop_asked(const BaCtlParams& P) {
+  const volatile unsigned long long* w = &P.link->req;
+  return w[1] == w[0];
+}
+
 // end of a robust round (after levmar returned): run_robust's bookkeeping, then the next round or the end
 __device__ void ba_ctl_end_round(BaCtl* c, double* sc, const BaCtlParams& P) {
   if (c->itno >= P.itmax && !c->stop) c->stop = 3;
   if (c->first_e0 < 0) c->first_e0 = c->init_eL2;
   c->totalTrials += c->nlss;
-  if (++c->round < P.rounds) {
-    ba_ctl_goto(c, sc, P, BA_STAGE_ROUND);
-    return;
+  if (++c->round < P.rounds && c->stop != BA_STOP_CALLER) {
+    if (!ba_ctl_stop_asked(P)) {
+      ba_ctl_goto(c, sc, P, BA_STAGE_ROUND);
+      return;
+    }
+    c->stop = BA_STOP_CALLER;  // no further round: the round that ended reports the stop
   }
   c->done = 1;
   c->stage = -1;
@@ -160,10 +196,40 @@ __device__ void ba_ctl_end_round(BaCtl* c, double* sc, const BaCtlParams& P) {
 __device__ void ba_ctl_end_iter(BaCtl* c, double* sc, const BaCtlParams& P) {
   if (c->p_eL2 <= P.eps3) c->stop = 3;
   ++c->itno;
+  if (c->itno < P.itmax && !c->stop && ba_ctl_stop_asked(P)) c->stop = BA_STOP_CALLER;
   if (c->itno < P.itmax && !c->stop)
     ba_ctl_goto(c, sc, P, BA_STAGE_LIN);
   else
     ba_ctl_end_round(c, sc, P);
+}
+
+// Into TRIAL after a linearisation or a rejected trial, unless the caller asked to stop: then the round
+// ends without counting the unfinished iteration (as the late eps1 test does).
+__device__ void ba_ctl_to_trial(BaCtl* c, double* sc, const BaCtlParams& P) {
+  if (ba_ctl_stop_asked(P)) {
+    c->stop = BA_STOP_CALLER;
+    ba_ctl_end_round(c, sc, P);
+  } else {
+    ba_ctl_goto(c, sc, P, BA_STAGE_TRIAL);
+  }
+}
+
+// the progress record of the decision just taken
+__device__ void ba_ctl_publish(const BaCtl* c, BaCtlLink* L) {
+  volatile BaProgress* g = &L->prog;
+  const unsigned long long k = g->seq1 + 1;
+  g->seq0 = k;
+  __threadfence();
+  g->req = L->req;
+  g->round = c->done ? c->round : c->round + 1;
+  g->itno = c->itno;
+  // end_round has added the round's trials; the ROUND stage clears nlss
+  g->trials = c->totalTrials + ((c->done || c->stage == BA_STAGE_ROUND) ? 0 : c->nlss);
+  g->p_eL2 = c->p_eL2;
+  g->init_eL2 = c->init_eL2;
+  g->mu = c->mu;
+  __threadfence();
+  g->seq1 = k;
 }
 
 __global__ void ba_ctl_init(BaCtl* __restrict__ c, double* __restrict__ sc) {
@@ -177,8 +243,7 @@ __global__ void ba_ctl_init(BaCtl* __restrict__ c, double* __restrict__ sc) {
   sc[SC_NONFINITE] = 0.0;
 }
 
-__global__ void ba_ctl_step(BaCtl* __restrict__ c, double* __restrict__ sc, BaCtlParams P) {
-  if (threadIdx.x != 0) return;
+__device__ void ba_ctl_decide(BaCtl* __restrict__ c, double* __restrict__ sc, const BaCtlParams& P) {
   const double EPS_SQ = 1e-24;
   c->copy = 0;
   switch (c->stage) {
@@ -217,7 +282,7 @@ __global__ void ba_ctl_step(BaCtl* __restrict__ c, double* __restrict__ sc, BaCt
       } else {
         c->ginfPending = 1;
       }
-      ba_ctl_goto(c, sc, P, BA_STAGE_TRIAL);
+      ba_ctl_to_trial(c, sc, P);
       return;
     }
     case BA_STAGE_TRIAL: {
@@ -279,12 +344,18 @@ __global__ void ba_ctl_step(BaCtl* __restrict__ c, double* __restrict__ sc, BaCt
         return;
       }
       c->nu = nu2;
-      ba_ctl_goto(c, sc, P, BA_STAGE_TRIAL);
+      ba_ctl_to_trial(c, sc, P);
       return;
     }
     default:
       return;
   }
+}
+
+__global__ void ba_ctl_step(BaCtl* __restrict__ c, double* __restrict__ sc, BaCtlParams P) {
+  if (threadIdx.x != 0) return;
+  ba_ctl_decide(c, sc, P);
+  ba_ctl_publish(c, P.link);
 }
 
 // accepted trial: pa <- na, pb <- nb (the host path swaps the pointers instead; the graph keeps its own)

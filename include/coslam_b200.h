@@ -498,6 +498,28 @@ void* cosl_ba_solver_stream(cosl_ba_solver* s);
 int cosl_ba_solver_submit(cosl_ba_solver* s);
 int cosl_ba_solver_query(cosl_ba_solver* s, int* done);
 int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]);
+/* Ask the BA running on `s` to end at its next decision point.  It may be a submitted BA, or
+ * cosl_ba_solver_run executing on another thread.  Returns at once and never waits for the device.
+ * A stop applies only to the request that is running or submitted when it is made.  With nothing
+ * running it has no effect: it returns COSL_OK and does not stop the next request.  COSL_E_INVALID
+ * for a NULL handle or a multi-rank solver (each rank would stop at a different trial, and the
+ * per-trial all-reduce would no longer match).
+ * The loop checks at every transition into a further stage: into the next linearisation after a
+ * finished iteration, into a trial after a linearisation or a rejected trial, and into the next
+ * robust round.  The round then ends with stop reason 8 in info[6]; an unfinished iteration is not
+ * counted, no further round starts, and the outlier pass still runs on the last accepted iterate, so
+ * collect returns COSL_OK and download returns parameters and outlier flags that belong together.
+ * run_fixed ignores stops. */
+int cosl_ba_solver_stop(cosl_ba_solver* s);
+/* Snapshot of the running or last BA (run or submit), without waiting for it:
+ * out = {running (0/1), round, iteration in the round, LM trials over all rounds,
+ *        cost of the accepted iterate (p_eL2), initial cost of the round, mu, stop requested (0/1)}.
+ * The fields come from one decision step, never a mix of two; before the request's first decision
+ * fields 1-6 are 0.  After collect (or run) returns, they equal what info reports: round count,
+ * info[5], info[10], info[12] / info[1].
+ * stop and progress are the only calls that may be made on a handle while another thread is inside
+ * run / submit / collect on it. */
+int cosl_ba_solver_progress(cosl_ba_solver* s, double out[8]);
 /* Per-kernel accumulated device time in ms since create/reset, by name (NULL-terminated list via
  * index): returns name or NULL when idx is out of range. */
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls);
