@@ -100,6 +100,8 @@ def _load():
     L.cosl_ba_solver_collect.argtypes = [vp, vp]
     L.cosl_ba_solver_stop.argtypes = [vp]
     L.cosl_ba_solver_progress.argtypes = [vp, C.POINTER(cd)]
+    L.cosl_ba_solver_set_covariance.argtypes = [vp, cd]
+    L.cosl_ba_solver_download_covariance.argtypes = [vp, vp, vp, C.POINTER(cd)]
     L.cosl_ba_solver_download.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_destroy.argtypes = [vp]
     L.cosl_ba_solver_stream.argtypes = [vp]
@@ -112,6 +114,7 @@ def _load():
     L.cosl_ba_solver_trace.argtypes = [vp, ci, vp, vp, ci]
     L.cosl_ba_solver_tasks.argtypes = [vp, vp, ci, vp, ci]
     L.cosl_ba_debug_tile_solve.argtypes = [ci, vp, ci, vp, vp, vp, pint, pint]
+    L.cosl_ba_debug_tile_selinv.argtypes = [ci, vp, ci, vp, vp, pint, pint]
     L.cosl_posegraph_spread_chains.argtypes = [ci, vp, vp, vp, vp, vp, vp, vp, vp, ci]
     L.cosl_posegraph_solve.argtypes = [ci, vp, vp, vp, ci, vp, vp, vp, vp, vp, ci, vp, vp, vp, ci]
     L.cosl_posegraph_last_host_ms.restype = cd
@@ -633,6 +636,25 @@ def ba_debug_tile_solve(S, b, adj, nd_depth=-1):
     return x, fail.value, dict(zip(PLAN_INFO_KEYS, [int(v) for v in out]))
 
 
+SELINV_INFO_KEYS = ("blocks", "tiles_schur", "tiles", "selinv_tasks", "nd_depth", "steps", "grid", "small_solve")
+
+
+def ba_debug_tile_selinv(S, adj, nd_depth=-1):
+    """cosl_ba_debug_tile_selinv: Z = S^-1 on the tile pattern of the BA's reduced-system factorisation (S dense
+    6mf x 6mf, lower triangle read; adj the mf x mf block pattern).  Returns (Z with the pattern's blocks (a, c),
+    a >= c, zero elsewhere; fail flag; info dict)."""
+    adj = np.ascontiguousarray(adj, np.uint8)
+    mf = adj.shape[0]
+    assert adj.shape == (mf, mf)
+    S = np.ascontiguousarray(S, np.float64)
+    assert S.shape == (6 * mf, 6 * mf)
+    Z = np.empty((6 * mf, 6 * mf))
+    fail = C.c_int(0)
+    out = (C.c_int * 8)()
+    _ck(LIB.cosl_ba_debug_tile_selinv(mf, _ptr(adj), int(nd_depth), _ptr(S), _ptr(Z), C.byref(fail), out))
+    return Z, fail.value, dict(zip(SELINV_INFO_KEYS, [int(v) for v in out]))
+
+
 def _chain_args(chain_off, fixed, R, t, eR, et):
     """C-ABI arguments of a chain spread from nChains on, and N.  The arrays behind the pointers live in the
     returned tuple."""
@@ -809,6 +831,21 @@ class BaSolver(_SolverHandle):
         _ck(LIB.cosl_ba_solver_progress(self.h, out))
         return {"running": bool(out[0]), "round": int(out[1]), "iteration": int(out[2]), "trials": int(out[3]),
                 "cost": out[4], "init_cost": out[5], "mu": out[6], "stop_requested": bool(out[7])}
+
+    def set_covariance(self, pixel_var):
+        """cosl_ba_solver_set_covariance: pixel_var > 0 makes every later run() and submit() end with the
+        covariance stage; 0 turns it off."""
+        _ck(LIB.cosl_ba_solver_set_covariance(self.h, float(pixel_var)))
+
+    def download_covariance(self):
+        """cosl_ba_solver_download_covariance: (camCov [m, 6, 6] for (w, t), ptCov [n, 3, 3], info dict) of the
+        last armed run or collect."""
+        cam = np.empty((self.prob.m, 6, 6))
+        pt = np.empty((self.prob.n, 3, 3))
+        out = (C.c_double * 8)()
+        _ck(LIB.cosl_ba_solver_download_covariance(self.h, _ptr(cam), _ptr(pt), out))
+        return cam, pt, {"pixel_var": out[0], "sigma2_hat": out[1], "dof": out[2], "unconstrained": int(out[3]),
+                         "device_ms": out[4], "min_pivot": out[5]}
 
     def download(self, into=None):
         """Current cameras and points into the solver's problem, or into `into` (same shape)."""

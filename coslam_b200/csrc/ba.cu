@@ -110,6 +110,56 @@ int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int devic
   return COSL_OK;
 }
 
+// Z = S^-1 on the tile pattern of P (S in td.tiles; the dataflow factorisation leaves its factor there).
+// Systems of one or two blocks: one resident CTA (ba_selinv_two).  Otherwise the diagonal of S is kept for
+// the pivot test, ba_tile_solve factors (its substitutions run on whatever rhs holds), then X_k = L_kk^-T for
+// every block and one launch per step of the plan.  Pivot break-down lands in td.sc[td.scFail], the blocks'
+// minimum relative pivots in sd.piv.  sd.cnt must be zero.
+int selinv_launch(const BaPlan& P, const BaSelPlan& SP, const BaTileDev& td, int grid, const BaSelDev& sd,
+                  cudaStream_t st) {
+  if (P.nb <= 0) return COSL_OK;
+  const int t00 = P.tileIdx[0];
+  const int t10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
+  const int t11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
+  if (P.nb <= 2 && t00 >= 0 && (P.nb == 1 || t11 >= 0)) {
+    COSL_LAUNCH(ba_selinv_two, 1, BA_NTHREADS, BA_SEL2_SMEM, st, td.tiles, td.blkRows, t00, t10, t11, sd.Z, sd.piv,
+                td.sc + td.scFail);
+  } else {
+    COSL_LAUNCH(ba_cov_sdiag, P.nb, BA_TB, 0, st, td.tiles, sd.diagTile, sd.sdiag);
+    COSL_LAUNCH(ba_tile_solve, grid, BA_NTHREADS, BA_TILE_SMEM, st, td);
+    COSL_LAUNCH(ba_selinv_xinv, P.nb, BA_NTHREADS, BA_SELX_SMEM, st, sd);
+    for (int q = 0; q + 1 < (int)SP.stepBegin.size(); ++q) {
+      const int t0 = SP.stepBegin[q], nOff = SP.stepBegin[q + 1] - t0 - 1;
+      COSL_LAUNCH(ba_selinv_step, std::max(1, nOff), BA_NTHREADS, BA_SELS_SMEM, st, sd, q, t0, nOff);
+    }
+  }
+  COSL_CUDA(cudaGetLastError());
+  return COSL_OK;
+}
+
+int selinv_attributes() {
+  COSL_CUDA(cudaFuncSetAttribute(ba_selinv_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SEL2_SMEM));
+  COSL_CUDA(cudaFuncSetAttribute(ba_selinv_xinv, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SELX_SMEM));
+  COSL_CUDA(cudaFuncSetAttribute(ba_selinv_step, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SELS_SMEM));
+  return COSL_OK;
+}
+
+// The device copy of a selected-inversion plan and the block -> diagonal tile map: [diagTile | tasks | ops]
+std::vector<unsigned char> selinv_index(const BaPlan& P, const BaSelPlan& SP, size_t* oTasks, size_t* oOps) {
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t nd = sizeof(int) * std::max(1, P.nb);
+  *oTasks = al(nd);
+  *oOps = *oTasks + al(sizeof(BaSelTask) * std::max<size_t>(1, SP.tasks.size()));
+  std::vector<unsigned char> h(*oOps + al(sizeof(BaSelOp) * std::max<size_t>(1, SP.ops.size())), 0);
+  for (int k = 0; k < P.nb; ++k) {
+    const int t = P.tileIdx[(size_t)k * P.nb + k];
+    std::memcpy(h.data() + sizeof(int) * k, &t, sizeof(int));
+  }
+  if (!SP.tasks.empty()) std::memcpy(h.data() + *oTasks, SP.tasks.data(), sizeof(BaSelTask) * SP.tasks.size());
+  if (!SP.ops.empty()) std::memcpy(h.data() + *oOps, SP.ops.data(), sizeof(BaSelOp) * SP.ops.size());
+  return h;
+}
+
 }  // namespace coslam
 
 /* ---------------------------------------------------------------- NCCL through dlopen */
@@ -244,6 +294,17 @@ struct cosl_ba_solver {
   std::mutex hostProgMu;
   BaProgress hostProg = {};        // the host loop's progress record
   int hpRound = 0, hpTrials0 = 0;  // round (1-based) and the trials of earlier rounds, for levmar's record
+  // covariance stage (cosl_ba_solver_set_covariance, DESIGN.md 4.6)
+  double covVar = 0.0;       // pixel variance; 0: disarmed
+  bool covReady = false;     // the selected-inversion plan and the stage's buffers exist for the loaded problem
+  bool covValid = false;     // the stage ran on the resident parameters
+  double graphCovVar = 0.0;  // covVar the submitted graph was built with
+  BaSelPlan sel;
+  BaSelDev sdev = {};
+  double *d_covWgt = nullptr, *d_covZ = nullptr, *d_covX = nullptr, *d_covSdiag = nullptr, *d_covPiv = nullptr;
+  double *d_covT = nullptr, *d_covCam = nullptr, *d_covPt = nullptr, *d_covSc = nullptr;
+  unsigned char *d_covUnc = nullptr, *d_covIdx = nullptr;
+  int* d_covCnt = nullptr;
 };
 
 namespace {
@@ -616,6 +677,8 @@ int index_problem(const cosl_ba_problem* p, BaIndex& x) {
   return COSL_OK;
 }
 
+int cov_prepare(cosl_ba_solver* s);
+
 // Replace the solver's problem with `p` (validated by check_problem, indexed by index_problem).  The
 // host plans the reduced-system solve and the Schur work items from the bucket counts, copies everything
 // the device needs into the staging buffer and enqueues the rest on the solver's stream: the upload, the
@@ -894,6 +957,8 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
     const int nsp = std::min(24, std::max(1, s->solveGrid / 6));
     td.nSpecial = std::max(1, std::min(nsp, s->solveGrid - 1));
   }
+  s->covReady = s->covValid = false;
+  if (s->covVar > 0) COSL_TRY(cov_prepare(s));
   if (ba_timing())
     std::fprintf(stderr, "[ba timing] load: host %.2f ms (%lld pair entries, %d items)\n", 1e3 * (now_s() - tLoad0),
                  nEntries, s->nItems);
@@ -924,6 +989,7 @@ int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver**
   COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_schur_pairs_st, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_ST_SMEM));
+  COSL_TRY(selinv_attributes());
   int nsm = 0;
   COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, s->device));
   s->numSM = std::max(1, nsm);
@@ -1389,6 +1455,106 @@ int download(cosl_ba_solver* s, cosl_ba_problem* p) {
   return COSL_OK;
 }
 
+/* ---------------------------------------------------------------- covariance stage (DESIGN.md 4.6) */
+// The selected-inversion plan of the loaded problem and the stage's buffers (arming, or a load while armed:
+// never inside run / submit).  Z has the factor's tile layout.
+int cov_prepare(cosl_ba_solver* s) {
+  const BaPlan& P = s->plan;
+  s->sel = ba_make_selinv_plan(P);
+  size_t oTasks = 0, oOps = 0;
+  const std::vector<unsigned char> idx = selinv_index(P, s->sel, &oTasks, &oOps);
+  const size_t nb = (size_t)std::max(1, P.nb), n = (size_t)s->n, m = (size_t)s->m;
+  COSL_TRY(grow(s, &s->d_covIdx, idx.size()));
+  COSL_TRY(grow(s, &s->d_covWgt, (size_t)s->N));
+  COSL_TRY(grow(s, &s->d_covZ, (size_t)std::max(1, P.nTiles) * BA_TILE));
+  COSL_TRY(grow(s, &s->d_covX, nb * BA_TILE));
+  COSL_TRY(grow(s, &s->d_covSdiag, nb * BA_TB));
+  COSL_TRY(grow(s, &s->d_covPiv, nb));
+  COSL_TRY(grow(s, &s->d_covCnt, nb));
+  COSL_TRY(grow(s, &s->d_covT, 6 * n));
+  COSL_TRY(grow(s, &s->d_covUnc, n));
+  COSL_TRY(grow(s, &s->d_covCam, 36 * m));
+  COSL_TRY(grow(s, &s->d_covPt, 9 * n));
+  COSL_TRY(grow(s, &s->d_covSc, (size_t)COV_NTOT));
+  // from pageable memory: the call returns once the source has been staged
+  COSL_CUDA(cudaMemcpyAsync(s->d_covIdx, idx.data(), idx.size(), cudaMemcpyHostToDevice, s->rq.stream));
+  BaSelDev& sd = s->sdev;
+  sd.L = s->d.tiles;
+  sd.Linv = s->d_Linv;
+  sd.sdiag = s->d_covSdiag;
+  sd.Z = s->d_covZ;
+  sd.X = s->d_covX;
+  sd.piv = s->d_covPiv;
+  sd.diagTile = reinterpret_cast<const int*>(s->d_covIdx);
+  sd.tasks = reinterpret_cast<const BaSelTask*>(s->d_covIdx + oTasks);
+  sd.ops = reinterpret_cast<const BaSelOp*>(s->d_covIdx + oOps);
+  sd.blkRows = s->d_blkRows;
+  sd.cnt = s->d_covCnt;
+  s->covReady = true;
+  return COSL_OK;
+}
+
+// The covariance stage at the resident parameters (d_pa, d_pb), enqueued on st (the solver's stream, or the
+// capture of the submitted graph): undamped re-linearisation with Tukey weights at those parameters through
+// the LM loop's kernels, Schur contraction, factorisation + selected inversion, camera and point blocks,
+// scalars.  Its weights and scalars are its own; the other buffers it writes (W, V, U, S, V^-1, the factor
+// work space) are rebuilt by the LM loop before it reads them.
+int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
+  BaDev cd = s->d;
+  cd.wgt = s->d_covWgt;
+  cd.sc = s->d_covSc;
+  BaTileDev td = s->td;
+  td.sc = s->d_covSc;
+  td.scFail = (int)SC_FAIL;
+  td.trace = nullptr;
+  const unsigned gN = (unsigned)div_up64(s->N, 256);
+  const int n = s->n, m = s->m, nb = std::max(0, s->plan.nb);
+  const double var = s->covVar;
+  COSL_LAUNCH(ba_cov_begin, (unsigned)std::max<long long>(1, std::min<long long>(1024, div_up64(6LL * n, 256))), 256,
+              0, st, s->d_covSc, s->d_covT, 6LL * n, s->d_covCnt, nb);
+  if (s->N) {
+    if (s->opt.max_err > 0)
+      COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+    else
+      COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_covWgt, s->N, 1.0);
+  }
+  if (n) COSL_LAUNCH(ba_cov_mask, div_up(n, 256), 256, 0, st, cd, s->d_covUnc);
+  const long long nV = 9LL * n + 27LL * m;
+  COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, st, s->d_V, nV, 0.0);
+  if (s->N) COSL_LAUNCH(ba_linearize_points, gN, 256, 0, st, cd, s->d_pa, s->d_pb);
+  if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, st, cd, s->d_pa, s->d_pb);
+  // mu = 0: S and V^-1 of the undamped system (and the cleared scalars and task counters)
+  const int nTilesInit = std::max(1, s->plan.nTiles);
+  COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)n + m, 256), 256, 0, st, cd, 0.0, 1,
+              s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks, nTilesInit,
+              s->d_Vinv, 0, nullptr, 0LL);
+  if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 0, 0.0, nullptr);
+  if (n) COSL_LAUNCH(ba_cov_vfix, div_up(n, 256), 256, 0, st, s->d_covUnc, s->d_Vinv, n);
+  if (s->ns) {
+    if (s->nItems)
+      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, st, cd, s->d_items,
+                  s->nItems, s->d_entries, s->d_Vinv);
+    COSL_TRY(selinv_launch(s->plan, s->sel, td, s->solveGrid, s->sdev, st));
+  }
+  COSL_LAUNCH(ba_cov_cams, div_up(m, 128), 128, 0, st, cd, s->d_pa, s->d_covZ, s->sdev.diagTile, var, s->d_covCam);
+  if (s->ns && s->nItems)
+    COSL_LAUNCH(ba_cov_pairs, div_up(s->nItems, 4), 128, 0, st, cd, s->d_items, s->nItems, s->d_entries, s->d_covZ,
+                s->d_covT);
+  if (n) COSL_LAUNCH(ba_cov_points, div_up(n, 256), 256, 0, st, n, s->ncon, s->d_Vinv, s->d_covT, s->d_covUnc, var,
+                     s->d_covPt);
+  COSL_LAUNCH(ba_cov_end, 1, 32, 0, st, s->d_covSc, s->d_covPiv, nb, s->mf, var);
+  COSL_CUDA(cudaGetLastError());
+  return COSL_OK;
+}
+
+// run's covariance stage: after the robust loop, on the solver's stream, waited for
+int run_cov(cosl_ba_solver* s) {
+  COSL_TRY(enqueue_cov(s, s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
+  s->covValid = true;
+  return COSL_OK;
+}
+
 /* ---------------------------------------------------------------- submitted robust loop (ba_ctl.cuh) */
 // Add a conditional node after the current capture position of `cs`; the capture continues behind it.
 int capture_conditional(cudaStream_t cs, cudaGraphConditionalHandle h, cudaGraphConditionalNodeType type,
@@ -1480,7 +1646,7 @@ int capture_into(cudaStream_t cs, cudaGraph_t g, F&& enqueue) {
 
 // The graph of the submitted robust loop:
 //   ba_ctl_init -> WHILE(loop) { IF(round) -> IF(lin0) -> IF(lin) -> IF(trial) -> ba_ctl_step -> ba_ctl_accept }
-//   -> outlier pass
+//   -> outlier pass -> covariance stage (when armed)
 int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
   BaCtlParams P = {};
   const double* o = s->opt.opts;
@@ -1509,6 +1675,7 @@ int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
     } else {
       COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, cs));
     }
+    if (s->covVar > 0) COSL_TRY(enqueue_cov(s, cs));
     COSL_CUDA(cudaGetLastError());
     return COSL_OK;
   }));
@@ -1571,6 +1738,7 @@ int build_graph(cosl_ba_solver* s) {
   s->graphNa = s->d_na;
   s->graphPb = s->d_pb;
   s->graphNb = s->d_nb;
+  s->graphCovVar = s->covVar;
   return COSL_OK;
 }
 
@@ -1668,6 +1836,7 @@ int cosl_ba_solver_reset(cosl_ba_solver* s, const cosl_ba_problem* prob) {
   if (!prob || prob->m != s->m || prob->n != s->n)
     return set_error(COSL_E_INVALID, "cosl_ba_solver_reset: problem shape changed");
   s->timer.reset();
+  s->covValid = false;
   COSL_CUDA(cudaEventSynchronize(s->evStaged));
   COSL_TRY(upload_params(s, prob));
   COSL_CUDA(cudaEventRecord(s->evStaged, s->rq.stream));
@@ -1694,7 +1863,9 @@ int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   s->reqKind.store(1);
   s->hostRunning.store(1);
   s->reqNo.store(s->loopReq);
-  const int rc = run_robust(s, 0, info);
+  s->covValid = false;
+  int rc = run_robust(s, 0, info);
+  if (rc == COSL_OK && s->covVar > 0) rc = run_cov(s);
   s->hostRunning.store(0);
   s->loopReq = 0;
   return rc;
@@ -1703,6 +1874,7 @@ int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
 int cosl_ba_solver_run_fixed(cosl_ba_solver* s, int trials, double info[COSL_BA_INFOSZ]) {
   BA_ENTER(s)
   COSL_TRY(s->rq.idle("cosl_ba_solver_run_fixed"));
+  s->covValid = false;
   return run_robust(s, trials < 1 ? 1 : trials, info);
 }
 
@@ -1723,7 +1895,7 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
   COSL_TRY(s->rq.idle("cosl_ba_solver_submit"));
   // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
   if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
-      s->graphNb != s->d_nb)
+      s->graphNb != s->d_nb || s->graphCovVar != s->covVar)
     COSL_TRY(build_graph(s));
   // the request number goes to the device ahead of the graph, on the solver's stream: a stop made before the
   // graph starts names it too (the pinned source is not rewritten before this request is collected)
@@ -1739,6 +1911,7 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
     return (int)COSL_OK;
   });
   if (rc == COSL_OK) s->submitted.store(1);
+  s->covValid = rc == COSL_OK && s->covVar > 0;  // readable once collected
   return rc;
 }
 
@@ -1755,6 +1928,7 @@ int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   double ms = 0;
   const int waited = s->rq.wait(&ms);
   s->submitted.store(0);
+  if (waited != COSL_OK) s->covValid = false;
   COSL_TRY(waited);
   BaCtl c;
   double nout = 0;
@@ -1842,6 +2016,45 @@ int cosl_ba_solver_progress(cosl_ba_solver* s, double out[8]) {
     out[6] = g.mu;
   }
   out[7] = (req && s->stopReq.load() == req) ? 1.0 : 0.0;
+  return COSL_OK;
+}
+
+int cosl_ba_solver_set_covariance(cosl_ba_solver* s, double pixel_var) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_set_covariance: the multi-rank solver has no covariance stage");
+  if (!(pixel_var >= 0.0) || !std::isfinite(pixel_var))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_set_covariance: pixel_var must be finite and >= 0");
+  COSL_TRY(s->rq.idle("cosl_ba_solver_set_covariance"));
+  if (pixel_var > 0 && !s->covReady) COSL_TRY(cov_prepare(s));
+  s->covVar = pixel_var;
+  return COSL_OK;
+}
+
+int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double* ptCov, double out[8]) {
+  BA_ENTER(s)
+  COSL_TRY(s->rq.idle("cosl_ba_solver_download_covariance"));
+  if (!s->covValid)
+    return set_error(COSL_E_STATE, "cosl_ba_solver_download_covariance: no covariance for the resident parameters "
+                     "(no armed run or collect since the last create, load, reset, run_fixed or unarmed BA)");
+  double sc[COV_NTOT];
+  COSL_CUDA(cudaMemcpyAsync(sc, s->d_covSc, sizeof(sc), cudaMemcpyDeviceToHost, s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
+  if (sc[COV_SING] != 0.0)
+    return set_error(COSL_E_NUMERIC,
+                     "cosl_ba_solver_download_covariance: the information matrix is singular in the gauge (%s; "
+                     "smallest relative pivot %.3e, threshold %.0e): fix cameras or points, or drop free cameras "
+                     "without weighted observations",
+                     sc[SC_FAIL] != 0.0 ? "pivot break-down" : "small pivot", sc[COV_OUT + 5], BA_COV_MIN_PIVOT);
+  if (camCov && s->m)
+    COSL_CUDA(cudaMemcpyAsync(camCov, s->d_covCam, sizeof(double) * 36 * (size_t)s->m, cudaMemcpyDeviceToHost,
+                              s->rq.stream));
+  if (ptCov && s->n)
+    COSL_CUDA(cudaMemcpyAsync(ptCov, s->d_covPt, sizeof(double) * 9 * (size_t)s->n, cudaMemcpyDeviceToHost,
+                              s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
+  if (out)
+    for (int k = 0; k < 8; ++k) out[k] = sc[COV_OUT + k];
   return COSL_OK;
 }
 
@@ -2017,6 +2230,151 @@ int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const dou
   out[5] = P.criticalPathTasks;
   out[6] = grid;
   out[7] = grid == 1 ? 1 : 0;
+  return COSL_OK;
+}
+
+// diagnostic: Z = S^-1 on the tile pattern with the covariance stage's factorisation and selected inversion
+int cosl_ba_debug_tile_selinv(int mf, const uint8_t* adj, int nd_depth, const double* S, double* Z, int* fail,
+                              int out[8]) {
+  if (mf < 1 || !adj || !S || !Z || !fail || !out)
+    return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_selinv: bad argument");
+  const BaPlan P = ba_make_plan(mf, std::vector<uint8_t>(adj, adj + (size_t)mf * mf), nd_depth);
+  if (P.nb <= 0) return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_selinv: planning failed");
+  const BaSelPlan SP = ba_make_selinv_plan(P);
+  std::vector<BaTask> tasks;
+  const int nA = tile_task_order(P, tasks);
+  const int nb = P.nb;
+  const size_t ns = 6 * (size_t)mf, nScratch = (size_t)std::max(1, P.nScratch);
+  const size_t nCnt = (size_t)P.nCounters + 2 + tasks.size();
+  std::vector<double> hTiles((size_t)P.nTiles * BA_TILE, 0.0);  // placed as cosl_ba_debug_tile_solve places them
+  for (int a = 0; a < mf; ++a)
+    for (int c = 0; c < mf; ++c) {
+      if (a != c && !adj[(size_t)a * mf + c] && !adj[(size_t)c * mf + a]) continue;
+      const int bA = P.camBlk[a], bC = P.camBlk[c];
+      if (bA < bC || (bA == bC && P.camOff[a] < P.camOff[c])) continue;
+      double* T = &hTiles[(size_t)P.tileIdx[(size_t)bA * nb + bC] * BA_TILE];
+      for (int r = 0; r < 6; ++r)
+        for (int q = 0; q < 6; ++q) {
+          if (a == c && q > r) continue;
+          const size_t i = 6 * (size_t)a + r, j = 6 * (size_t)c + q;
+          T[(size_t)(P.camOff[c] + q) * BA_TB + P.camOff[a] + r] = i >= j ? S[i * ns + j] : S[j * ns + i];
+        }
+    }
+  size_t oTasks = 0, oOps = 0;
+  const std::vector<unsigned char> idx = selinv_index(P, SP, &oTasks, &oOps);
+  int device = 0;
+  COSL_CUDA(cudaGetDevice(&device));
+  COSL_TRY(selinv_attributes());
+  COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+  cudaStream_t s = cudaStreamPerThread;
+  TmpDeviceBufs tmp(s);
+  double *dRhs, *dTiles, *dRhsS, *dLinv, *dY, *dX, *dSc, *dZ, *dXk, *dSdiag, *dPiv;
+  int *dCnt, *dBlkRows, *dSelCnt;
+  unsigned char* dIdx;
+  BaTask* dTasks;
+  BaBwdEntry* dBwd;
+  BaSumEntry* dSum;
+  COSL_TRY(tmp.alloc(&dRhs, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dTiles, ((size_t)P.nTiles + P.nScratch) * BA_TILE));
+  COSL_TRY(tmp.alloc(&dRhsS, nScratch * BA_TB));
+  COSL_TRY(tmp.alloc(&dLinv, (size_t)nb * BA_TILE));
+  COSL_TRY(tmp.alloc(&dY, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dX, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dSc, 1));
+  COSL_TRY(tmp.alloc(&dZ, (size_t)P.nTiles * BA_TILE));
+  COSL_TRY(tmp.alloc(&dXk, (size_t)nb * BA_TILE));
+  COSL_TRY(tmp.alloc(&dSdiag, (size_t)nb * BA_TB));
+  COSL_TRY(tmp.alloc(&dPiv, (size_t)nb));
+  COSL_TRY(tmp.alloc(&dCnt, nCnt));
+  COSL_TRY(tmp.alloc(&dBlkRows, (size_t)nb));
+  COSL_TRY(tmp.alloc(&dSelCnt, (size_t)nb));
+  COSL_TRY(tmp.alloc(&dIdx, idx.size()));
+  COSL_TRY(tmp.alloc(&dTasks, tasks.size()));
+  COSL_TRY(tmp.alloc(&dBwd, P.bwdList.size()));
+  COSL_TRY(tmp.alloc(&dSum, P.sumList.size()));
+  COSL_CUDA(cudaMemsetAsync(dRhs, 0, 8 * (size_t)nb * BA_TB, s));
+  COSL_CUDA(cudaMemcpyAsync(dTiles, hTiles.data(), 8 * hTiles.size(), cudaMemcpyHostToDevice, s));
+  COSL_CUDA(cudaMemsetAsync(dTiles + (size_t)P.nTiles * BA_TILE, 0xff, 8 * (size_t)P.nScratch * BA_TILE, s));
+  COSL_CUDA(cudaMemsetAsync(dRhsS, 0xff, 8 * nScratch * BA_TB, s));
+  COSL_CUDA(cudaMemsetAsync(dCnt, 0, 4 * nCnt, s));
+  COSL_CUDA(cudaMemsetAsync(dSelCnt, 0, 4 * (size_t)nb, s));
+  COSL_CUDA(cudaMemsetAsync(dSc, 0, 8, s));
+  COSL_CUDA(cudaMemcpyAsync(dBlkRows, P.blkRows.data(), 4 * (size_t)nb, cudaMemcpyHostToDevice, s));
+  COSL_CUDA(cudaMemcpyAsync(dIdx, idx.data(), idx.size(), cudaMemcpyHostToDevice, s));
+  COSL_CUDA(cudaMemcpyAsync(dTasks, tasks.data(), sizeof(BaTask) * tasks.size(), cudaMemcpyHostToDevice, s));
+  if (!P.bwdList.empty())
+    COSL_CUDA(cudaMemcpyAsync(dBwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size(), cudaMemcpyHostToDevice, s));
+  if (!P.sumList.empty())
+    COSL_CUDA(cudaMemcpyAsync(dSum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size(), cudaMemcpyHostToDevice, s));
+  BaTileDev td = {};
+  td.rhs = dRhs;
+  td.tiles = dTiles;
+  td.rhsS = dRhsS;
+  td.Linv = dLinv;
+  td.y = dY;
+  td.x = dX;
+  td.cnt = dCnt;
+  td.tasks = dTasks;
+  td.bwd = dBwd;
+  td.sum = dSum;
+  td.blkRows = dBlkRows;
+  td.nTasks = (int)tasks.size();
+  td.nA = nA;
+  td.nb = nb;
+  td.nTiles = P.nTiles;
+  td.nCounters = P.nCounters;
+  td.xdoneBase = P.nTiles + P.nScratch;
+  td.sc = dSc;
+  td.scFail = 0;
+  int nsm = 0;
+  COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+  const int grid = std::max(2, std::min(std::max(1, nsm), td.nTasks + 1));  // as tile_solve_launch
+  td.nSpecial = std::max(1, std::min(std::min(24, std::max(1, grid / 6)), grid - 1));
+  BaSelDev sd = {};
+  sd.L = dTiles;
+  sd.Linv = dLinv;
+  sd.sdiag = dSdiag;
+  sd.Z = dZ;
+  sd.X = dXk;
+  sd.piv = dPiv;
+  sd.diagTile = reinterpret_cast<const int*>(dIdx);
+  sd.tasks = reinterpret_cast<const BaSelTask*>(dIdx + oTasks);
+  sd.ops = reinterpret_cast<const BaSelOp*>(dIdx + oOps);
+  sd.blkRows = dBlkRows;
+  sd.cnt = dSelCnt;
+  COSL_TRY(selinv_launch(P, SP, td, grid, sd, s));
+  std::vector<double> hZ((size_t)P.nTiles * BA_TILE), hPiv(nb);
+  double hFail = 0.0;
+  COSL_CUDA(cudaMemcpyAsync(hZ.data(), dZ, 8 * hZ.size(), cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(hPiv.data(), dPiv, 8 * (size_t)nb, cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(&hFail, dSc, 8, cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaStreamSynchronize(s));
+  double minPiv = 1e300;
+  for (double v : hPiv) minPiv = std::min(minPiv, v);
+  *fail = (hFail != 0.0 || !(minPiv >= BA_COV_MIN_PIVOT)) ? 1 : 0;
+  // the lower camera blocks (a >= c) whose tile is in the pattern
+  std::memset(Z, 0, sizeof(double) * ns * ns);
+  for (int a = 0; a < mf; ++a)
+    for (int c = 0; c <= a; ++c) {
+      const int bA = P.camBlk[a], bC = P.camBlk[c];
+      const int t = bA >= bC ? P.tileIdx[(size_t)bA * nb + bC] : P.tileIdx[(size_t)bC * nb + bA];
+      if (t < 0) continue;
+      const double* T = &hZ[(size_t)t * BA_TILE];
+      for (int r = 0; r < 6; ++r)
+        for (int q = 0; q < 6; ++q) {
+          const int ra = P.camOff[a] + r, qc = P.camOff[c] + q;
+          // element (row of a, column of c) of the lower tile: transposed when c's block comes later
+          Z[(6 * (size_t)a + r) * ns + 6 * (size_t)c + q] = bA >= bC ? T[(size_t)qc * BA_TB + ra] : T[(size_t)ra * BA_TB + qc];
+        }
+    }
+  out[0] = P.nb;
+  out[1] = P.nTilesOrig;
+  out[2] = P.nTiles;
+  out[3] = (int)SP.tasks.size();
+  out[4] = P.ndDepth;
+  out[5] = (int)SP.stepBegin.size() - 1;
+  out[6] = P.nb <= 2 ? 1 : grid;
+  out[7] = P.nb <= 2 ? 1 : 0;
   return COSL_OK;
 }
 

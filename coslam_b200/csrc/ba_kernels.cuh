@@ -974,4 +974,208 @@ ba_finish_cost(BaDev d, const double* __restrict__ na, const double* __restrict_
   ba_finish_cost_body(d, na, pb, nb, acc3, Vinv, mu);
 }
 
+// ------------------------------------------------------------------------------------------
+// Covariance stage (cosl_ba_solver_set_covariance, DESIGN.md 4.6).  It re-linearises with the kernels above
+// through a BaDev of its own (weights, scalars), so nothing the LM loop keeps between calls changes.  Its
+// scalars: [0, SC_NTOT) those of that BaDev, then the slots below.
+// ------------------------------------------------------------------------------------------
+enum BaCovScalar {
+  COV_T0 = SC_NTOT,   // globaltimer at the start of the stage (bits of a uint64)
+  COV_NOBS = 17,      // observations with w > 0 that enter H
+  COV_NPTS = 18,      // free points with a covariance
+  COV_NUNC = 19,      // free points with fewer than two observations of non-zero weight
+  COV_SING = 20,      // 1: the reduced system is singular in the gauge
+  COV_OUT = 24,       // [8]: the out vector of cosl_ba_solver_download_covariance
+  COV_NTOT = 32
+};
+constexpr double BA_COV_MIN_PIVOT = 1e-12;  // smallest relative pivot L_ii^2 / S_ii of a regular system
+
+__global__ void __launch_bounds__(256)
+ba_cov_begin(double* __restrict__ sc, double* __restrict__ T, long long nT, int* __restrict__ cnt, int nCnt) {
+  const long long q0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, st = (long long)gridDim.x * blockDim.x;
+  for (long long q = q0; q < nT; q += st) T[q] = 0.0;
+  for (long long q = q0; q < nCnt; q += st) cnt[q] = 0;
+  if (q0 < COV_NTOT - COV_T0) sc[COV_T0 + q0] = 0.0;
+  __syncthreads();
+  if (q0 == 0) {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    *reinterpret_cast<unsigned long long*>(sc + COV_T0) = t;
+  }
+}
+
+// One thread per point: free points with fewer than two observations of non-zero weight are left out of H
+// (their weights are zeroed, unc[i] = 1); counts of the observations and points that enter H.
+__global__ void __launch_bounds__(256) ba_cov_mask(BaDev d, unsigned char* __restrict__ unc) {
+  __shared__ double s_red[8];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  double nobs = 0, npts = 0, nunc = 0;
+  if (i < d.n) {
+    int k = 0;
+    for (long long o = d.ptr[i]; o < d.ptr[i + 1]; ++o) k += d.wgt[o] > 0.0 ? 1 : 0;
+    const bool u = i >= d.ncon && k < 2;
+    unc[i] = u ? 1 : 0;
+    if (u) {
+      for (long long o = d.ptr[i]; o < d.ptr[i + 1]; ++o) d.wgt[o] = 0.0;
+      nunc = 1;
+    } else {
+      nobs = k;
+      npts = i >= d.ncon ? 1 : 0;
+    }
+  }
+  double t = block_sum_1(nobs, s_red);
+  if (threadIdx.x == 0 && t != 0) atomicAdd(&d.sc[COV_NOBS], t);
+  t = block_sum_1(npts, s_red);
+  if (threadIdx.x == 0 && t != 0) atomicAdd(&d.sc[COV_NPTS], t);
+  t = block_sum_1(nunc, s_red);
+  if (threadIdx.x == 0 && t != 0) atomicAdd(&d.sc[COV_NUNC], t);
+}
+
+// V^-1 of a point left out of H is 0, not the inverse of its zero V (the Schur contraction reads it)
+__global__ void __launch_bounds__(256)
+ba_cov_vfix(const unsigned char* __restrict__ unc, double* __restrict__ Vinv, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && unc[i])
+    for (int k = 0; k < 6; ++k) Vinv[6 * (size_t)i + k] = 0.0;
+}
+
+// diagonal of S before the factorisation overwrites it (relative pivots); one CTA of 64 per block
+__global__ void ba_cov_sdiag(const double* __restrict__ tiles, const int* __restrict__ diagTile,
+                             double* __restrict__ sdiag) {
+  const int k = blockIdx.x, r = threadIdx.x;
+  sdiag[(size_t)k * 64 + r] = tiles[(size_t)diagTile[k] * 4096 + (size_t)r * 65];
+}
+
+// Camera blocks: Z_jj in the solver's chart (v, t), R = R(q(v)) R0, turned into (w, t) with
+// R' = exp([w]x) R: w = J dv, J = 2 (w_q I + [v]x + v v^T / w_q), w_q = sqrt(1 - |v|^2).  camCov[j] =
+// var * T Z_jj T^T with T = diag(J, I), row-major 6x6; zeros for the fixed cameras.
+__global__ void __launch_bounds__(128)
+ba_cov_cams(BaDev d, const double* __restrict__ pa, const double* __restrict__ Z, const int* __restrict__ diagTile,
+            double var, double* __restrict__ camCov) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= d.m) return;
+  double* out = camCov + 36 * (size_t)j;
+  if (j < d.mcon) {
+    for (int k = 0; k < 36; ++k) out[k] = 0.0;
+    return;
+  }
+  const int si = d.solIdx[j - d.mcon], off = si & 63;
+  const double* Zt = Z + (size_t)diagTile[si >> 6] * 4096;
+  const double v0 = pa[6 * (size_t)j], v1 = pa[6 * (size_t)j + 1], v2 = pa[6 * (size_t)j + 2];
+  const double wq = sqrt(1.0 - (v0 * v0 + v1 * v1 + v2 * v2));
+  const double v[3] = {v0, v1, v2};
+  const double vx[9] = {0.0, -v2, v1, v2, 0.0, -v0, -v1, v0, 0.0};
+  double Tm[36];
+  for (int k = 0; k < 36; ++k) Tm[k] = 0.0;
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) Tm[6 * r + c] = 2.0 * ((r == c ? wq : 0.0) + vx[3 * r + c] + v[r] * v[c] / wq);
+    Tm[6 * (r + 3) + r + 3] = 1.0;
+  }
+  double M[36];  // T Z
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) {
+      double s = 0;
+      for (int p = 0; p < 6; ++p) s += Tm[6 * r + p] * Zt[(size_t)(off + c) * 64 + off + p];
+      M[6 * r + c] = s;
+    }
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) {
+      double s = 0;
+      for (int p = 0; p < 6; ++p) s += M[6 * r + p] * Tm[6 * c + p];
+      out[6 * r + c] = var * s;
+    }
+}
+
+// One pass over the Schur pair entries, one warp per work item: T_i += W_a^T Z_ab W_b (+ its transpose when
+// a != b), Z_ab read through the item's destination in the tile layout (ba_schur_pairs_st writes S there).
+// T: [n][6] packed symmetric (00, 01, 02, 11, 12, 22), zeroed by ba_cov_begin.
+__global__ void __launch_bounds__(128)
+ba_cov_pairs(BaDev d, const BaPairItem* __restrict__ items, int nItems, const int4* __restrict__ entries,
+             const double* __restrict__ Z, double* __restrict__ T) {
+  __shared__ double s_z[4][36];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int item = blockIdx.x * 4 + w;
+  if (item >= nItems) return;
+  const BaPairItem it = items[item];
+  for (int k = lane; k < 36; k += 32) {
+    const int r = k / 6, c = k - 6 * r;
+    s_z[w][k] = Z[(size_t)it.dst + (size_t)(it.cOff + (it.trans ? c : r)) * 64 + it.rOff + (it.trans ? r : c)];
+  }
+  __syncwarp();
+  const double* Zb = s_z[w];
+  for (int e = it.begin + lane; e < it.end; e += 32) {
+    const int4 en = entries[e];
+    const double* Wa = d.W + 18 * (size_t)en.x;
+    const double* Wb = d.W + 18 * (size_t)en.y;
+    double M[18];  // Z_ab W_b (6x3)
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 3; ++c) {
+        double s = 0;
+        for (int q = 0; q < 6; ++q) s += Zb[6 * r + q] * Wb[3 * q + c];
+        M[3 * r + c] = s;
+      }
+    double X[9];  // W_a^T M
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) {
+        double s = 0;
+        for (int q = 0; q < 6; ++q) s += Wa[3 * q + r] * M[3 * q + c];
+        X[3 * r + c] = s;
+      }
+    const double f = (en.x != en.y) ? 1.0 : 0.5;  // X + X^T, or the symmetric part of a diagonal term
+    double* Ti = T + 6 * (size_t)en.z;
+    atomicAdd(Ti + 0, 2.0 * f * X[0]);
+    atomicAdd(Ti + 1, f * (X[1] + X[3]));
+    atomicAdd(Ti + 2, f * (X[2] + X[6]));
+    atomicAdd(Ti + 3, 2.0 * f * X[4]);
+    atomicAdd(Ti + 4, f * (X[5] + X[7]));
+    atomicAdd(Ti + 5, 2.0 * f * X[8]);
+  }
+}
+
+// Point blocks: ptCov[i] = var (V_i^-1 + V_i^-1 T_i V_i^-1) (row-major 3x3); zeros for the fixed points, NaN for
+// the points left out of H.
+__global__ void __launch_bounds__(256)
+ba_cov_points(int n, int ncon, const double* __restrict__ Vinv, const double* __restrict__ T,
+              const unsigned char* __restrict__ unc, double var, double* __restrict__ ptCov) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double* out = ptCov + 9 * (size_t)i;
+  if (i < ncon || unc[i]) {
+    const double f = i < ncon ? 0.0 : __longlong_as_double(0x7ff8000000000000LL);
+    for (int k = 0; k < 9; ++k) out[k] = f;
+    return;
+  }
+  const int sym[9] = {0, 1, 2, 1, 3, 4, 2, 4, 5};
+  double Iv[9], Tm[9], A[9];
+  for (int k = 0; k < 9; ++k) {
+    Iv[k] = Vinv[6 * (size_t)i + sym[k]];
+    Tm[k] = T[6 * (size_t)i + sym[k]];
+  }
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) A[3 * r + c] = Iv[3 * r] * Tm[c] + Iv[3 * r + 1] * Tm[3 + c] + Iv[3 * r + 2] * Tm[6 + c];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c)
+      out[3 * r + c] = var * (Iv[3 * r + c] + A[3 * r] * Iv[c] + A[3 * r + 1] * Iv[3 + c] + A[3 * r + 2] * Iv[6 + c]);
+}
+
+// The stage's scalars: sigma^2-hat, dof, the minimum relative pivot over the nb blocks, singularity, time
+__global__ void ba_cov_end(double* __restrict__ sc, const double* __restrict__ piv, int nb, int mf, double var) {
+  if (threadIdx.x != 0) return;
+  double mp = __longlong_as_double(0x7ff0000000000000LL);  // +inf: no free camera, no pivot
+  for (int k = 0; k < nb; ++k) mp = fmin(mp, piv[k]);
+  const double dof = 2.0 * sc[COV_NOBS] - 6.0 * mf - 3.0 * sc[COV_NPTS];
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  const unsigned long long t0 = *reinterpret_cast<const unsigned long long*>(sc + COV_T0);
+  sc[COV_SING] = (sc[SC_FAIL] != 0.0 || !(mp >= BA_COV_MIN_PIVOT)) ? 1.0 : 0.0;
+  double* out = sc + COV_OUT;
+  out[0] = var;
+  out[1] = dof > 0 ? sc[SC_COST] / dof : __longlong_as_double(0x7ff8000000000000LL);
+  out[2] = dof;
+  out[3] = sc[COV_NUNC];
+  out[4] = 1e-6 * (double)(t - t0);
+  out[5] = mp;
+  out[6] = out[7] = 0.0;
+}
+
 }  // namespace coslam

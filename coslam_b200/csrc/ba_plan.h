@@ -497,4 +497,54 @@ inline BaPlan ba_make_plan(int mf, const std::vector<uint8_t>& adj, int ndDepthO
   return P;
 }
 
+// ---- selected inversion Z = S^-1 on the factor's tile pattern (covariance of the BA, DESIGN.md 4.6) ----
+// The Takahashi recurrences, walking the pivots from the last block to the first, with s = struct(k) =
+// the blocks i > k that own a tile (i, k) of the factor (fill included):
+//   Z_ik = -(sum_{j in s} Z_ij L_jk) L_kk^-1                  for every i in s
+//   Z_kk = L_kk^-T (L_kk^-1 - sum_{i in s} L_ik^T Z_ik)
+// Z_ij (i, j in s) is a tile of the pattern: the fill of pivot k joins every pair of s.  Every block of s is
+// eliminated after k, so all those tiles are final when step k runs: one step per pivot, its off-diagonal
+// tasks independent of each other, its diagonal task after them.  The order of the tasks of a step and of
+// the operands of a task is fixed (ascending block), so the sums are deterministic.
+struct BaSelTask {   // Z_ik (i > k), or Z_kk (i == k: the last task of its step)
+  int k, i, tOut;    // tOut = tile index of (i, k), in the factor's layout
+  int opBegin, opEnd;  // range in BaSelPlan::ops
+};
+
+struct BaSelOp {
+  // off-diagonal task: Z_ij (tile tZ, read transposed when zT: the tile stores Z_ji) times L_jk (tile tL);
+  // diagonal task: L_jk^T (tile tL) times Z_jk (tile tZ == tL)
+  int tZ, zT, tL, j;
+};
+
+struct BaSelPlan {
+  std::vector<int> stepBegin;  // step q (pivot k = nb - 1 - q): tasks [stepBegin[q], stepBegin[q + 1])
+  std::vector<BaSelTask> tasks;
+  std::vector<BaSelOp> ops;
+};
+
+inline BaSelPlan ba_make_selinv_plan(const BaPlan& P) {
+  BaSelPlan S;
+  const int nb = P.nb;
+  auto T = [&](int i, int j) { return P.tileIdx[(size_t)i * nb + j]; };
+  for (int k = nb - 1; k >= 0; --k) {
+    S.stepBegin.push_back((int)S.tasks.size());
+    std::vector<int> s;
+    for (int i = k + 1; i < nb; ++i)
+      if (T(i, k) >= 0) s.push_back(i);
+    for (int i : s) {
+      BaSelTask t{k, i, T(i, k), (int)S.ops.size(), 0};
+      for (int j : s) S.ops.push_back({i >= j ? T(i, j) : T(j, i), i < j ? 1 : 0, T(j, k), j});
+      t.opEnd = (int)S.ops.size();
+      S.tasks.push_back(t);
+    }
+    BaSelTask d{k, k, T(k, k), (int)S.ops.size(), 0};
+    for (int j : s) S.ops.push_back({T(j, k), 0, T(j, k), j});
+    d.opEnd = (int)S.ops.size();
+    S.tasks.push_back(d);
+  }
+  S.stepBegin.push_back((int)S.tasks.size());
+  return S;
+}
+
 }  // namespace coslam

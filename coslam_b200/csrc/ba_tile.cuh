@@ -843,4 +843,325 @@ __global__ void __launch_bounds__(BA_NTHREADS, 1) ba_tile_two(BaTileDev d, int t
   if (tid == 0 && s_fail) d.sc[d.scFail] = 1.0;
 }
 
+// =============================================================================================
+// Selected inversion Z = S^-1 on the factor's tile pattern (the covariance stage of the BA, DESIGN.md 4.6;
+// task plan: ba_make_selinv_plan in ba_plan.h).  Z has the factor's tile layout; its padding rows and columns
+// are zero and its diagonal tiles are stored in full (both triangles).
+// =============================================================================================
+
+// acc(r, c) += sum_{p < kk} opA(r, p) opB(p, c) with the DMMA fragments of tile_gemm_dmma.  Both tiles are
+// staged column-major (element (r, c) at c * BA_LDS + r); TA: opA = A^T (else A), TB: opB = B (else B^T).
+template <bool TA, bool TB>
+__device__ __forceinline__ void tile_gemm_acc(const double* __restrict__ sA, const double* __restrict__ sB,
+                                              int kk, int tid, TileAcc& acc) {
+  const int lane = tid & 31, w = tid >> 5;
+  const int mB = (w & 3) * 16 + (lane >> 2), nB = (w >> 2) * 32 + (lane >> 2), kl = lane & 3;
+  for (int p0 = 0; p0 < kk; p0 += 4) {
+    const int p = p0 + kl;
+    double a[2], b[4];
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi) a[mi] = TA ? sA[(mB + 8 * mi) * BA_LDS + p] : sA[p * BA_LDS + mB + 8 * mi];
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni) b[ni] = TB ? sB[(nB + 8 * ni) * BA_LDS + p] : sB[p * BA_LDS + nB + 8 * ni];
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+      for (int ni = 0; ni < 4; ++ni) dmma884(acc.c[mi][ni][0], acc.c[mi][ni][1], a[mi], b[ni]);
+  }
+}
+
+__device__ __forceinline__ void tile_acc_zero(TileAcc& acc) {
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni) acc.c[mi][ni][0] = acc.c[mi][ni][1] = 0.0;
+}
+
+// s(r, c) = scale * acc(r, c) inside rows x cols, 0 outside (shared, column-major)
+__device__ __forceinline__ void tile_acc_store(const TileAcc& acc, double* __restrict__ s, double scale, int rows,
+                                               int cols, int tid) {
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        int r, c;
+        tile_acc_rc(tid, mi, ni, e, r, c);
+        s[c * BA_LDS + r] = (r < rows && c < cols) ? scale * acc.c[mi][ni][e] : 0.0;
+      }
+}
+
+// shared tile -> global tile; sym: the symmetric part (diagonal tiles of Z)
+__device__ __forceinline__ void tile_store(const double* __restrict__ s, double* __restrict__ g, bool sym, int tid) {
+  for (int e = tid; e < BA_TILE; e += BA_NTHREADS) {
+    const int c = e >> 6, r = e & 63;
+    g[e] = sym ? 0.5 * (s[c * BA_LDS + r] + s[r * BA_LDS + c]) : s[c * BA_LDS + r];
+  }
+}
+
+// X = L_kk^-T in sX (zero outside bk x bk) from L_kk staged in sL (identity padding) and its 8x8 diagonal
+// inverses sM: X L^T = I by tile_trsm2.  Ends with a CTA barrier.
+__device__ __forceinline__ void tile_inv_t(const double* __restrict__ sL, const double* __restrict__ sM,
+                                          double* __restrict__ sX, int bk, int tid) {
+  for (int e = tid; e < BA_TILE; e += BA_NTHREADS) {
+    const int c = e >> 6, r = e & 63;
+    sX[c * BA_LDS + r] = (r == c) ? 1.0 : 0.0;
+  }
+  __syncthreads();
+  tile_trsm2(sX, sL, sM, (bk + 7) >> 3, tid);
+  __syncthreads();
+  for (int e = tid; e < BA_TILE; e += BA_NTHREADS) {
+    const int c = e >> 6, r = e & 63;
+    if (r >= bk || c >= bk) sX[c * BA_LDS + r] = 0.0;
+  }
+  __syncthreads();
+}
+
+// min over the rows of a block of L_ii^2 / S_ii (0 where S_ii is not positive or the pivot not finite)
+__device__ __forceinline__ double rel_pivot(double l, double s) {
+  const double q = l * l / s;
+  return (s > 0.0 && q >= 0.0 && q < 1e300) ? q : 0.0;
+}
+
+struct BaSelDev {
+  const double* L;        // factor tiles (lower; diagonal tiles: identity padding)
+  const double* Linv;     // [nb][512]: the 8x8 diagonal inverses of every L_kk (ba_tile_solve's POTRF)
+  double* sdiag;          // [nb][64]: diagonal of S before the factorisation (ba_cov_sdiag)
+  double* Z;              // Z tiles, the factor's layout
+  double* X;              // [nb][4096]: X_k = L_kk^-T
+  double* piv;            // [nb]: minimum relative pivot of block k
+  const BaSelTask* tasks;
+  const BaSelOp* ops;
+  const int* blkRows;
+  const int* diagTile;    // [nb]: tile index of (k, k)
+  int* cnt;               // [nb]: finished off-diagonal tasks of step q
+};
+
+constexpr int BA_SELX_SMEM = (2 * BA_TB * BA_LDS + 8 * BA_TB) * (int)sizeof(double);
+constexpr int BA_SELS_SMEM = 2 * BA_TB * BA_LDS * (int)sizeof(double);
+
+// One CTA per block: X_k = L_kk^-T and the block's minimum relative pivot.
+__global__ void __launch_bounds__(BA_NTHREADS, 1) ba_selinv_xinv(BaSelDev d) {
+  extern __shared__ double smem[];
+  double* sL = smem;
+  double* sX = sL + BA_TB * BA_LDS;
+  double* sM = sX + BA_TB * BA_LDS;
+  __shared__ double s_red[BA_TB];
+  const int tid = threadIdx.x, k = blockIdx.x, bk = d.blkRows[k];
+  tile_stage_diag(d.L + (size_t)d.diagTile[k] * BA_TILE, sL, bk, tid);
+  sM[tid] = __ldcg(d.Linv + (size_t)k * BA_TILE + tid);
+  sM[tid + BA_NTHREADS] = __ldcg(d.Linv + (size_t)k * BA_TILE + tid + BA_NTHREADS);
+  __syncthreads();
+  if (tid < BA_TB) s_red[tid] = tid < bk ? rel_pivot(sL[tid * BA_LDS + tid], d.sdiag[(size_t)k * BA_TB + tid]) : 1e300;
+  tile_inv_t(sL, sM, sX, bk, tid);
+  double* g = d.X + (size_t)k * BA_TILE;
+  for (int e = tid; e < BA_TILE; e += BA_NTHREADS) g[e] = sX[(e >> 6) * BA_LDS + (e & 63)];
+  if (tid == 0) {
+    double m = 1e300;
+    for (int r = 0; r < bk; ++r) m = fmin(m, s_red[r]);
+    d.piv[k] = m;
+  }
+}
+
+// Z_kk of the diagonal task t (the Z_jk of its step are final): X_k (X_k^T - sum_j L_jk^T Z_jk)
+__device__ __forceinline__ void selinv_diag(const BaSelDev& d, const BaSelTask& t, double* sA, double* sB, int tid) {
+  const int bk = d.blkRows[t.k];
+  TileAcc acc;
+  tile_acc_zero(acc);
+  for (int o = t.opBegin; o < t.opEnd; ++o) {
+    const BaSelOp op = d.ops[o];
+    __syncthreads();
+    tile_load<BA_LDS>(d.L + (size_t)op.tL * BA_TILE, sA, tid);
+    tile_load<BA_LDS>(d.Z + (size_t)op.tZ * BA_TILE, sB, tid);
+    __syncthreads();
+    tile_gemm_acc<true, true>(sA, sB, (d.blkRows[op.j] + 3) & ~3, tid, acc);  // P += L_jk^T Z_jk
+  }
+  __syncthreads();
+  tile_load<BA_LDS>(d.X + (size_t)t.k * BA_TILE, sB, tid);
+  __syncthreads();
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        int r, c;
+        tile_acc_rc(tid, mi, ni, e, r, c);
+        sA[c * BA_LDS + r] = sB[r * BA_LDS + c] - acc.c[mi][ni][e];  // Q = X^T - P
+      }
+  __syncthreads();
+  tile_acc_zero(acc);
+  tile_gemm_acc<false, true>(sB, sA, (bk + 3) & ~3, tid, acc);  // X Q
+  __syncthreads();
+  tile_acc_store(acc, sA, 1.0, bk, bk, tid);
+  __syncthreads();
+  tile_store(sA, d.Z + (size_t)t.tOut * BA_TILE, true, tid);
+}
+
+// One step of the recurrence (pivot k): CTA b < nOff computes Z_ik of task t0 + b; the CTA that finishes
+// last computes Z_kk (task t0 + nOff).  nOff == 0: one CTA, Z_kk = X_k X_k^T.
+__global__ void __launch_bounds__(BA_NTHREADS, 1) ba_selinv_step(BaSelDev d, int q, int t0, int nOff) {
+  extern __shared__ double smem[];
+  double* sA = smem;
+  double* sB = sA + BA_TB * BA_LDS;
+  __shared__ int s_last;
+  const int tid = threadIdx.x;
+  if (nOff > 0) {
+    const BaSelTask t = d.tasks[t0 + blockIdx.x];
+    const int bi = d.blkRows[t.i], bk = d.blkRows[t.k];
+    TileAcc acc;
+    tile_acc_zero(acc);
+    for (int o = t.opBegin; o < t.opEnd; ++o) {
+      const BaSelOp op = d.ops[o];
+      __syncthreads();
+      tile_load<BA_LDS>(d.Z + (size_t)op.tZ * BA_TILE, sA, tid);
+      tile_load<BA_LDS>(d.L + (size_t)op.tL * BA_TILE, sB, tid);
+      __syncthreads();
+      const int kk = (d.blkRows[op.j] + 3) & ~3;
+      if (op.zT)
+        tile_gemm_acc<true, true>(sA, sB, kk, tid, acc);  // G += Z_ji^T L_jk
+      else
+        tile_gemm_acc<false, true>(sA, sB, kk, tid, acc);  // G += Z_ij L_jk
+    }
+    __syncthreads();
+    tile_acc_store(acc, sA, 1.0, bi, bk, tid);
+    tile_load<BA_LDS>(d.X + (size_t)t.k * BA_TILE, sB, tid);
+    __syncthreads();
+    tile_acc_zero(acc);
+    tile_gemm_acc<false, false>(sA, sB, (bk + 3) & ~3, tid, acc);  // G X_k^T = G L_kk^-1
+    __syncthreads();
+    tile_acc_store(acc, sA, -1.0, bi, bk, tid);
+    __syncthreads();
+    tile_store(sA, d.Z + (size_t)t.tOut * BA_TILE, false, tid);
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(d.cnt + q, 1) == nOff - 1;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+  }
+  selinv_diag(d, d.tasks[t0 + nOff], sA, sB, tid);
+}
+
+// Systems of one or two blocks (every local BA): factorisation and selected inversion in ONE CTA with the
+// tiles resident in shared memory.  ba_tile_two keeps its factor in shared memory and never stores it, so
+// this kernel factors S again with the same primitives (tile_potrf2, tile_trsm2) before inverting.
+// Tiles t00 / t10 / t11 as ba_tile_two; S is read from tiles, Z written with the same indices.
+constexpr int BA_SEL2_SMEM = (5 * BA_TB * BA_LDS + 16 * BA_TB + 2 * BA_TB + 96 + 2 * BA_TB) * (int)sizeof(double);
+
+__global__ void __launch_bounds__(BA_NTHREADS, 1)
+ba_selinv_two(const double* __restrict__ tiles, const int* __restrict__ blkRows, int t00, int t10, int t11,
+              double* __restrict__ Z, double* __restrict__ piv, double* __restrict__ failFlag) {
+  extern __shared__ double smem[];
+  double* sA = smem;                   // S00 -> L00
+  double* sB = sA + BA_TB * BA_LDS;    // S10 -> L10 -> (Z11 L10)
+  double* sC = sB + BA_TB * BA_LDS;    // S11 -> L11 -> Z11 -> Q
+  double* sX0 = sC + BA_TB * BA_LDS;   // L00^-T
+  double* sX1 = sX0 + BA_TB * BA_LDS;  // L11^-T -> G -> Z10
+  double* sM0 = sX1 + BA_TB * BA_LDS;
+  double* sM1 = sM0 + 8 * BA_TB;
+  double* sV = sM1 + 8 * BA_TB;        // zero right-hand side
+  double* sY = sV + BA_TB;
+  double* sD = sY + BA_TB;
+  double* sdg = sD + 96;               // diagonal of S00 | S11
+  __shared__ int s_fail;
+  const int tid = threadIdx.x;
+  const int bk0 = blkRows[0];
+  const bool two = t11 >= 0;
+  const int bk1 = two ? blkRows[1] : 0;
+  if (tid == 0) s_fail = 0;
+  tile_stage_diag(tiles + (size_t)t00 * BA_TILE, sA, bk0, tid);
+  if (two) {
+    tile_stage_diag(tiles + (size_t)t11 * BA_TILE, sC, bk1, tid);
+    if (t10 >= 0) tile_load<BA_LDS>(tiles + (size_t)t10 * BA_TILE, sB, tid);
+  }
+  if (tid < BA_TB) sV[tid] = 0.0;
+  __syncthreads();
+  if (tid < BA_TB) {
+    sdg[tid] = sA[tid * BA_LDS + tid];
+    sdg[BA_TB + tid] = two ? sC[tid * BA_LDS + tid] : 1.0;
+  }
+  __syncthreads();
+  tile_potrf2(sA, sV, sY, sM0, sD, tid, &s_fail, (bk0 + 7) >> 3);
+  if (two) {
+    if (t10 >= 0) {
+      tile_trsm2(sB, sA, sM0, (bk0 + 7) >> 3, tid);  // L10 = S10 L00^-T
+      __syncthreads();
+      TileAcc acc;
+      tile_gemm_dmma(sB, sB, (bk0 + 3) & ~3, tid, acc);
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            int r, c;
+            tile_acc_rc(tid, mi, ni, e, r, c);
+            sC[c * BA_LDS + r] -= acc.c[mi][ni][e];
+          }
+    }
+    __syncthreads();
+    tile_potrf2(sC, sV, sY, sM1, sD, tid, &s_fail, (bk1 + 7) >> 3);
+  }
+  if (tid == 0) {
+    double m0 = 1e300, m1 = 1e300;
+    for (int r = 0; r < bk0; ++r) m0 = fmin(m0, rel_pivot(sA[r * BA_LDS + r], sdg[r]));
+    for (int r = 0; r < bk1; ++r) m1 = fmin(m1, rel_pivot(sC[r * BA_LDS + r], sdg[BA_TB + r]));
+    piv[0] = m0;
+    if (two) piv[1] = m1;
+    if (s_fail) *failFlag = 1.0;
+  }
+  tile_inv_t(sA, sM0, sX0, bk0, tid);
+  TileAcc acc;
+  if (!two) {
+    tile_acc_zero(acc);
+    tile_gemm_acc<false, false>(sX0, sX0, (bk0 + 3) & ~3, tid, acc);  // X0 X0^T
+    tile_acc_store(acc, sA, 1.0, bk0, bk0, tid);
+    __syncthreads();
+    tile_store(sA, Z + (size_t)t00 * BA_TILE, true, tid);
+    return;
+  }
+  tile_inv_t(sC, sM1, sX1, bk1, tid);
+  tile_acc_zero(acc);
+  tile_gemm_acc<false, false>(sX1, sX1, (bk1 + 3) & ~3, tid, acc);  // Z11 = X1 X1^T
+  __syncthreads();
+  tile_acc_store(acc, sC, 1.0, bk1, bk1, tid);
+  __syncthreads();
+  tile_store(sC, Z + (size_t)t11 * BA_TILE, true, tid);
+  tile_acc_zero(acc);
+  if (t10 >= 0) {
+    tile_gemm_acc<false, true>(sC, sB, (bk1 + 3) & ~3, tid, acc);  // G = Z11 L10
+    __syncthreads();
+    tile_acc_store(acc, sX1, 1.0, bk1, bk0, tid);
+    __syncthreads();
+    tile_acc_zero(acc);
+    tile_gemm_acc<false, false>(sX1, sX0, (bk0 + 3) & ~3, tid, acc);  // G X0^T
+    __syncthreads();
+    tile_acc_store(acc, sX1, -1.0, bk1, bk0, tid);                      // Z10
+    __syncthreads();
+    tile_store(sX1, Z + (size_t)t10 * BA_TILE, false, tid);
+    tile_acc_zero(acc);
+    tile_gemm_acc<true, true>(sB, sX1, (bk1 + 3) & ~3, tid, acc);      // P = L10^T Z10
+  }
+  __syncthreads();
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        int r, c;
+        tile_acc_rc(tid, mi, ni, e, r, c);
+        sC[c * BA_LDS + r] = sX0[r * BA_LDS + c] - acc.c[mi][ni][e];  // Q = X0^T - P
+      }
+  __syncthreads();
+  tile_acc_zero(acc);
+  tile_gemm_acc<false, true>(sX0, sC, (bk0 + 3) & ~3, tid, acc);  // Z00 = X0 Q
+  __syncthreads();
+  tile_acc_store(acc, sA, 1.0, bk0, bk0, tid);
+  __syncthreads();
+  tile_store(sA, Z + (size_t)t00 * BA_TILE, true, tid);
+}
+
 }  // namespace coslam

@@ -520,6 +520,32 @@ int cosl_ba_solver_stop(cosl_ba_solver* s);
  * stop and progress are the only calls that may be made on a handle while another thread is inside
  * run / submit / collect on it. */
 int cosl_ba_solver_progress(cosl_ba_solver* s, double out[8]);
+/* Marginal covariances of the adjusted cameras and points (an extension: the reference recomputes point
+ * covariances by triangulation instead).  At the parameters download returns, with Tukey weights
+ * w = (1 - (e / max_err)^2)^2 (0 for e >= max_err; 1 when max_err <= 0) evaluated there, the stage forms
+ * H = sum_obs w J^T J over the free parameters and returns diagonal blocks of pixel_var H^-1:
+ *   camCov[j]: 6x6, row-major, for (w, t) with R' = exp([w]x) R, t' = t + dt (x_cam = R X + t);
+ *   ptCov[i]:  3x3, row-major, for X_i in world coordinates.
+ * Fixed cameras and points get zeros.  A free point with fewer than two observations of non-zero weight is
+ * left out of H and gets NaN.
+ * pixel_var > 0 arms: every later cosl_ba_solver_run and cosl_ba_solver_submit ends with the covariance
+ * stage on the solver's stream (inside the submitted graph for submit, whose collect then reports its time
+ * in info[11] too; not run_fixed).  0 disarms.  Arming allocates the stage's buffers (and so does a load
+ * while armed).  COSL_E_INVALID for a multi-rank solver or pixel_var < 0 (or not finite); COSL_E_STATE
+ * while a submit is in flight. */
+int cosl_ba_solver_set_covariance(cosl_ba_solver* s, double pixel_var);
+/* After run / collect of an armed BA: camCov[m][36], ptCov[n][9] (each nullable);
+ * out = {pixel_var, sigma2_hat, dof, unconstrained points, device ms of the stage, min relative pivot, 0, 0}.
+ * sigma2_hat = sum w |e|^2 / dof over the observations that enter H, dof = 2 #(those with w > 0) -
+ * 6 (free cameras) - 3 (points with a covariance); NaN when dof <= 0: the caller may rescale by
+ * sigma2_hat / pixel_var.  The relative pivots are L_ii^2 / S_ii of the Cholesky factor of the reduced
+ * camera system (+inf without free cameras).
+ * COSL_E_STATE with no covariance for the resident parameters (none armed yet, or load / reset /
+ * run_fixed / an unarmed run or submit since) or while a submit is in flight;
+ * COSL_E_NUMERIC (nothing written) when the stage found the system singular in the gauge: a pivot
+ * break-down or a relative pivot below 1e-12 (e.g. no fixed camera and too few fixed points, or a free
+ * camera without an observation of non-zero weight).  The BA itself still returned COSL_OK. */
+int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double* ptCov, double out[8]);
 /* Per-kernel accumulated device time in ms since create/reset, by name (NULL-terminated list via
  * index): returns name or NULL when idx is out of range. */
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls);
@@ -554,6 +580,14 @@ int cosl_ba_solver_tasks(cosl_ba_solver* s, int32_t* tasks, int cap, int32_t* li
  * COSL_E_*. */
 int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const double* S,
                              const double* b, double* x, int* fail, int out[8]);
+/* Diagnostic, like cosl_ba_debug_tile_solve: Z = S^-1 on the tile pattern of adj (fill included) with the
+ * covariance stage's factorisation and selected inversion, returned dense (6mf x 6mf, row-major): the
+ * blocks (a, c), a >= c, whose tile is in the pattern; zero elsewhere.  *fail = 1 when the factorisation
+ * broke down or a relative pivot L_ii^2 / S_ii fell below 1e-12 (Z is then meaningless).
+ * out = {blocks, Schur-structure tiles, tiles incl. fill, selected-inversion tasks, nested-dissection
+ * depth, steps (one launch each), CTAs of the factorisation, small-solve}. */
+int cosl_ba_debug_tile_selinv(int mf, const uint8_t* adj, int nd_depth, const double* S, double* Z,
+                              int* fail, int out[8]);
 
 /* ================= post-BA pose-graph spreading (SURVEY.md 8f-2) =================
  * Replaces, for chain graphs, GlobalPoseGraph::computeNewCameraRotations
