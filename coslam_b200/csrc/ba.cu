@@ -1,7 +1,7 @@
 // ba.cu -- host side of the bundle-adjustment solver + its C-ABI (see include/coslam_b200.h).
 // Replaces bundleAdjustRobust (LibVisualSLAM, call app/SL_CoSLAMRobustBA.cpp:174) and
-// sba_motstr_levmar_x (sba-1.6, call app/SL_CoSLAMBA.cpp:360-363).  The LM control flow mirrors
-// oracle/ba_oracle.cpp:levmar line by line; every arithmetic step runs in the kernels of
+// sba_motstr_levmar_x (sba-1.6, call app/SL_CoSLAMBA.cpp:360-363).  The LM control flow (ba_lm.cuh)
+// mirrors oracle/ba_oracle.cpp:levmar line by line; every arithmetic step runs in the kernels of
 // ba_kernels.cuh.  Multi-GPU: points (with all their observations) are sharded over the ranks,
 // cameras are replicated; per LM trial one NCCL all-reduce (sum) of the packed buffer
 // [S | rhs] and one of a handful of scalars; per linearisation one of [U | ea] and one max-reduce.
@@ -263,8 +263,6 @@ struct cosl_ba_solver {
   unsigned char* d_outlier = nullptr;
   const BaPairItem* d_items = nullptr;
   double* d_Vinv = nullptr;
-  bool costDone = false;         // solve_trial already evaluated the trial cost (ba_finish_cost)
-  bool statsPending = false;     // |g|_inf / max diag of the last linearisation still to be computed (prep kernel)
   unsigned long long scSeq = 0;  // sequence number of the last scalar read-back (ba_publish_sc)
   int4* d_entries = nullptr;
   int nItems = 0;
@@ -274,8 +272,6 @@ struct cosl_ba_solver {
   int two00 = -1, two10 = -1, two11 = -1;
   SectionTimer timer;
   int secLin = 0, secSchur = 0, secSolve = 0, secBack = 0, secCost = 0, secComm = 0;
-  // statistics
-  int nfev = 0, njev = 0, nlss = 0;
   // submitted robust loop (cosl_ba_solver_submit): the graph with the device-side LM control and the
   // parameter buffers it was built for
   BaCtl* d_ctl = nullptr;
@@ -292,8 +288,7 @@ struct cosl_ba_solver {
   std::atomic<int> hostRunning{0}, submitted{0};
   unsigned long long loopReq = 0;  // the request the host loop runs; 0: not stoppable (run_fixed, cosl_ba_solve)
   std::mutex hostProgMu;
-  BaProgress hostProg = {};        // the host loop's progress record
-  int hpRound = 0, hpTrials0 = 0;  // round (1-based) and the trials of earlier rounds, for levmar's record
+  BaProgress hostProg = {};  // the host driver's progress record
   // covariance stage (cosl_ba_solver_set_covariance, DESIGN.md 4.6)
   double covVar = 0.0;       // pixel variance; 0: disarmed
   bool covReady = false;     // the selected-inversion plan and the stage's buffers exist for the loaded problem
@@ -1015,8 +1010,15 @@ int allreduce(cosl_ba_solver* s, double* buf, size_t count, int op) {
   return COSL_OK;
 }
 
-int zero_sc(cosl_ba_solver* s, int first, int count) {
-  COSL_CUDA(cudaMemsetAsync(s->d_sc + first, 0, sizeof(double) * count, s->rq.stream));
+// clear the scalar slots of `mask` (ba_lm_cleared): one memset per run of adjacent slots
+int clear_sc(cosl_ba_solver* s, unsigned mask) {
+  for (int k = 0; k < SC_NTOT; ++k) {
+    if (!(mask >> k & 1u)) continue;
+    int e = k + 1;
+    while (e < SC_NTOT && (mask >> e & 1u)) ++e;
+    COSL_CUDA(cudaMemsetAsync(s->d_sc + k, 0, sizeof(double) * (e - k), s->rq.stream));
+    k = e;
+  }
   return COSL_OK;
 }
 
@@ -1064,366 +1066,182 @@ int read_sc(cosl_ba_solver* s) {
   return COSL_OK;
 }
 
-// weighted cost of a parameter set -> *out (all ranks)
-int eval_cost(cosl_ba_solver* s, const double* pa, const double* pb, double* out, bool* finite) {
-  ++s->nfev;
-  COSL_TRY(zero_sc(s, SC_COST, 1));
-  COSL_TRY(zero_sc(s, SC_NONFINITE, 1));
-  s->timer.begin(s->secCost, s->rq.stream);
-  if (s->N)
-    COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, pa, pb,
-                0, 0.0, nullptr);
-  s->timer.end(s->rq.stream);
-  COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
-  COSL_TRY(read_sc(s));
-  *out = s->h_sc[SC_COST];
-  *finite = std::isfinite(*out) && s->h_sc[SC_NONFINITE] == 0.0;
+// The kernels of one stage of the robust loop, enqueued on st (the solver's stream, or the capture of the
+// submitted graph), with the stage's multi-rank all-reduces.  dctl: the control block of the submitted loop,
+// from which the trial kernels read mu (and the prep kernel doStats) when they run; without it they take mu
+// and doStats from the host driver.  doStats: the stage computes |g|_inf / max diag for the eps1 test
+// (BaCtl::statsPending).
+int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dctl, double mu, int doStats) {
+  const unsigned gN = (unsigned)div_up64(s->N, 256);
+  const int r0 = rank_of(s) == 0 ? 1 : 0;
+  SectionTimer& T = s->timer;
+  if (stage == BA_STAGE_ROUND) {  // the round's Tukey weights, then its initial cost
+    if (s->N) {
+      if (s->opt.max_err > 0)
+        COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+      else
+        COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_wgt, s->N, 1.0);
+    }
+    T.begin(s->secCost, st);
+    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 0, 0.0, nullptr);
+    T.end(st);
+  } else if (stage == BA_STAGE_LIN0 || stage == BA_STAGE_LIN) {  // Jacobians, U, V, W, ea, eb at (pa, pb)
+    const long long nV = 9LL * s->n + 27LL * s->m;  // [V | eb | U | ea]
+    T.begin(s->secLin, st);
+    COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, st, s->d_V, nV, 0.0);
+    if (s->N) COSL_LAUNCH(ba_linearize_points, gN, 256, 0, st, s->d, s->d_pa, s->d_pb);
+    if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, st, s->d, s->d_pa, s->d_pb);
+    T.end(st);
+    COSL_TRY(allreduce(s, s->d_Uea, (size_t)27 * s->m, ncclSum));
+    // at itno > 0 the prep kernel of the next trial computes the statistics, unless there is none
+    if (stage == BA_STAGE_LIN0 || (!s->ns && doStats)) {
+      COSL_LAUNCH(ba_stats_kernel, (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, st, s->d);
+      COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
+    }
+  } else if (s->ns) {  // a trial: Schur complement + dense solve + back substitution for mu, and its cost
+    const int nTilesInit = std::max(1, s->plan.nTiles);
+    T.begin(s->secSchur, st);
+    // also clears the scalars of this trial (|dp|^2, dL, |p|^2, fail, cost, non-finite), the task counters
+    // of the solve and the accumulator of the point back-substitution (d_dpb)
+    COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, st, s->d, dctl,
+                mu, r0, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks,
+                nTilesInit, s->d_Vinv, doStats, s->d_dpb, 3LL * s->n);
+    if (doStats) COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
+    if (s->nItems)
+      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, st, s->d,
+                  s->d_items, s->nItems, s->d_entries, s->d_Vinv);
+    T.end(st);
+    // the one exchange of an LM trial: [rhs | Schur-structure tiles] is contiguous, no packing
+    COSL_TRY(allreduce(s, s->d_S, (size_t)s->reduceCount, ncclSum));
+    T.begin(s->secSolve, st);  // reduced camera system -> d_x (block padded, permuted)
+    if (s->twoSolve)
+      COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, st, s->td, s->two00, s->two10, s->two11);
+    else
+      COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, st, s->td);
+    T.end(st);
+    // back substitution + trial cost in two launches (ba_kernels.cuh); V*^-1 is the one the contraction used
+    const int nCamBlocks = div_up(6 * s->m, 256);
+    T.begin(s->secBack, st);
+    COSL_LAUNCH(ba_back_cams_points, nCamBlocks + gN, 256, 0, st, s->d, dctl, s->d_pa, s->d_x, s->d_dpa, s->d_na, mu,
+                r0, nCamBlocks, s->d_dpb);
+    T.end(st);
+    T.begin(s->secCost, st);
+    if (s->N + s->n)  // a problem without points never reaches a trial (|g| = 0 stops it), but is captured
+      COSL_LAUNCH(ba_finish_cost, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, st, s->d, dctl, s->d_na,
+                  s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu);
+    T.end(st);
+  } else {  // a trial without free cameras
+    T.begin(s->secBack, st);
+    // (also zeroes the accumulator of the point back-substitution, d_nb)
+    COSL_LAUNCH(ba_cam_update,
+                std::max(div_up(6 * s->m, 256), (int)std::min<long long>(s->numSM, div_up64(3LL * s->n, 1024))), 256,
+                0, st, s->d, dctl, s->d_pa, s->d_x, s->d_dpa, s->d_na, mu, r0, s->d_nb, 3LL * s->n);
+    if (s->N) COSL_LAUNCH(ba_back_subst, gN, 256, 0, st, s->d, s->d_dpa, s->d_nb);
+    if (s->n)
+      COSL_LAUNCH(ba_back_finish, (unsigned)div_up64(s->n, 256), 256, 0, st, s->d, dctl, s->d_pb, s->d_nb, s->d_dpb,
+                  mu);
+    T.end(st);
+    T.begin(s->secCost, st);
+    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, s->d, s->d_na, s->d_nb, 0, 0.0, nullptr);
+    T.end(st);
+  }
+  if (stage == BA_STAGE_ROUND || stage == BA_STAGE_TRIAL) COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
+  COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
 
-int compute_weights(cosl_ba_solver* s) {
+// The outlier pass after the loop, at its final parameters: the flags, and their number over all ranks in
+// sc[SC_COST] (cleared by the loop's last decision).  The same branch on every rank (options are global).
+int enqueue_outliers(cosl_ba_solver* s, cudaStream_t st) {
   if (s->opt.max_err > 0) {
     if (s->N)
-      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d,
-                  s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, st, s->d, s->d_pa, s->d_pb, 2,
+                  s->opt.max_err, s->d_outlier);
+    COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
   } else {
-    std::vector<double> ones((size_t)s->N, 1.0);
-    COSL_CUDA(cudaMemcpyAsync(s->d_wgt, ones.data(), sizeof(double) * (size_t)s->N,
-                              cudaMemcpyHostToDevice, s->rq.stream));
-    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
-  }
-  return COSL_OK;
-}
-
-// Jacobians, U, V, W, ea, eb at (pa, pb); ginf / maxdiag land in h_sc
-// statsNow: |g|_inf / max diag are wanted before the next solve (first iteration: mu0); otherwise they are
-// computed by the prep kernel of the next trial (solve_trial) and arrive with that trial's scalars
-int linearize(cosl_ba_solver* s, bool statsNow, bool statsLater) {
-  ++s->njev;
-  s->timer.begin(s->secLin, s->rq.stream);
-  COSL_CUDA(cudaMemsetAsync(s->d_V, 0, sizeof(double) * (9 * (size_t)s->n + 27 * (size_t)s->m), s->rq.stream));
-  if (s->N)
-    COSL_LAUNCH(ba_linearize_points, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d,
-                s->d_pa, s->d_pb);
-  if (s->Nc)
-    COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, s->rq.stream, s->d,
-                s->d_pa, s->d_pb);
-  s->timer.end(s->rq.stream);
-  COSL_TRY(allreduce(s, s->d_Uea, (size_t)27 * s->m, ncclSum));
-  if (!s->N) COSL_TRY(zero_sc(s, SC_GINF, 2));  // otherwise ba_linearize_points cleared them
-  s->statsPending = false;
-  if (statsNow || (statsLater && !s->ns)) {
-    COSL_LAUNCH(ba_stats_kernel, (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->rq.stream,
-                s->d);
-    COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
-  } else if (statsLater) {
-    s->statsPending = true;
+    COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, st));
   }
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
 
-// reduced camera system -> d_x (block padded, permuted): one persistent dataflow launch
-int dense_solve(cosl_ba_solver* s) {
-  const int ns = s->ns;
-  if (ns == 0) return COSL_OK;
-  s->timer.begin(s->secSolve, s->rq.stream);
-  if (s->twoSolve) {
-    COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s->rq.stream, s->td, s->two00, s->two10, s->two11);
-  } else {
-    COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, s->rq.stream, s->td);
-  }
-  s->timer.end(s->rq.stream);
-  COSL_CUDA(cudaGetLastError());
-  return COSL_OK;
+// fixedTrials > 0: cosl_ba_solver_run_fixed (one round of that many trials)
+BaLmParams lm_params(const cosl_ba_solver* s, int fixedTrials) {
+  BaLmParams P = {};
+  const double* o = s->opt.opts;
+  P.tau = o[0];
+  P.eps1 = o[1];
+  P.eps2 = o[2];
+  P.eps3 = o[3];
+  P.eps4 = o[4];
+  P.rounds = fixedTrials ? 1 : std::max(1, s->opt.outer_iters);
+  P.itmax = fixedTrials ? (1 << 30) : s->opt.inner_iters;
+  P.ns = s->ns;
+  P.hasObs = s->N > 0;
+  P.outliers = s->opt.max_err > 0;
+  P.fixedTrials = fixedTrials;
+  return P;
 }
 
-// Schur complement + dense solve + back substitution for damping mu; trial parameters -> na, nb;
-// scalars (dp_L2, dL, p_L2, fail) -> h_sc
-int solve_trial(cosl_ba_solver* s, double mu, bool* solved) {
-  ++s->nlss;
-  const bool r0 = rank_of(s) == 0;
-  const long long ns = s->ns;
-  if (!ns) {  // no free camera: nothing launches ba_tile_init, which clears the trial's scalars otherwise
-    COSL_TRY(zero_sc(s, SC_DP_L2, 3));
-    COSL_TRY(zero_sc(s, SC_FAIL, 1));
-    COSL_TRY(zero_sc(s, SC_COST, 1));
-    COSL_TRY(zero_sc(s, SC_NONFINITE, 1));
-  }
-  static const bool fineSchur = std::getenv("COSL_BA_TIMING_FINE") != nullptr;  // diagnostic: init / contraction apart
-  const int secInit = fineSchur ? s->timer.section("ba_schur_init") : s->secSchur;
-  s->timer.begin(secInit, s->rq.stream);
-  if (ns) {
-    // also clears the scalars of this trial (|dp|^2, dL, |p|^2, fail, cost, non-finite) and the task
-    // counters of the solve: five memset nodes less per trial
-    const int nTilesInit = std::max(1, s->plan.nTiles);
-    const bool doStats = s->statsPending;
-    s->statsPending = false;
-    COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, s->rq.stream, s->d,
-                mu, r0 ? 1 : 0, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt,
-                s->td.nCounters + 2 + s->td.nTasks, nTilesInit, s->d_Vinv, doStats ? 1 : 0,
-                s->d_dpb, 3LL * s->n);
-    if (doStats) COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
-    if (fineSchur) {
-      s->timer.end(s->rq.stream);
-      s->timer.begin(s->secSchur, s->rq.stream);
-    }
-    if (s->nItems)
-      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, s->rq.stream,
-                  s->d, s->d_items, s->nItems, s->d_entries, s->d_Vinv);
-  }
-  s->timer.end(s->rq.stream);
-  // the one exchange of an LM trial: [rhs | Schur-structure tiles] is contiguous, no packing
-  if (ns && multi(s)) COSL_TRY(allreduce(s, s->d_S, (size_t)s->reduceCount, ncclSum));
-  COSL_TRY(dense_solve(s));
-  s->costDone = false;
-  if (ns) {
-    // back substitution + trial cost in two launches (ba_kernels.cuh): the accumulator d_dpb was zeroed by the
-    // prep kernel, V*^-1 is the one the Schur contraction used
-    const int nCamBlocks = div_up(6 * s->m, 256);
-    s->timer.begin(s->secBack, s->rq.stream);
-    COSL_LAUNCH(ba_back_cams_points, nCamBlocks + (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, s->d_pa,
-                s->d_x, s->d_dpa, s->d_na, mu, r0 ? 1 : 0, nCamBlocks, s->d_dpb);
-    s->timer.end(s->rq.stream);
-    s->timer.begin(s->secCost, s->rq.stream);
-    COSL_LAUNCH(ba_finish_cost, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, s->rq.stream, s->d, s->d_na,
-                s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu);
-    s->timer.end(s->rq.stream);
-    s->costDone = true;
-    COSL_CUDA(cudaGetLastError());
-    *solved = true;
-    return COSL_OK;
-  }
-  s->timer.begin(s->secBack, s->rq.stream);
-  // (also zeroes the accumulator of the point back-substitution, d_nb)
-  COSL_LAUNCH(ba_cam_update, std::max(div_up(6 * s->m, 256), (int)std::min<long long>(s->numSM, div_up64(3LL * s->n, 1024))),
-              256, 0, s->rq.stream, s->d, s->d_pa, s->d_x, s->d_dpa, s->d_na, mu, r0 ? 1 : 0, s->d_nb, 3LL * s->n);
-  if (s->N)
-    COSL_LAUNCH(ba_back_subst, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, s->d_dpa,
-                s->d_nb);
-  if (s->n)
-    COSL_LAUNCH(ba_back_finish, (unsigned)div_up64(s->n, 256), 256, 0, s->rq.stream, s->d, s->d_pb,
-                s->d_nb, s->d_dpb, mu);
-  s->timer.end(s->rq.stream);
-  COSL_CUDA(cudaGetLastError());
-  // the scalar all-reduce of this trial is merged with the cost evaluation by the caller
-  *solved = true;
-  return COSL_OK;
+// info[] of a finished loop (include/coslam_b200.h): the levmar fields of its last round, the first round's
+// initial cost, the trials of all rounds, the time it took and the outliers of the pass after it
+void fill_info(double info[COSL_BA_INFOSZ], const BaCtl& c, double seconds, double nout, bool outliers) {
+  if (!info) return;
+  for (int k = 0; k < COSL_BA_INFOSZ; ++k) info[k] = 0;
+  info[0] = c.first_e0;
+  info[1] = c.p_eL2;
+  info[2] = c.ginf;
+  info[3] = c.dp_L2;
+  info[4] = c.maxdiag > 0 ? c.mu / c.maxdiag : 0;
+  info[5] = c.itno;
+  info[6] = c.stop;
+  info[7] = c.nfev;
+  info[8] = c.njev;
+  info[9] = c.nlss;
+  info[10] = c.totalTrials;
+  info[11] = seconds;
+  info[12] = c.p_eL2;
+  info[13] = outliers ? nout : 0.0;
 }
 
-// The host loop's stop test (ba_ctl_stop_asked of the submitted loop): only a run through the handle stops.
-bool host_stop_asked(const cosl_ba_solver* s) {
-  return s->loopReq && s->stopReq.load(std::memory_order_relaxed) == s->loopReq;
-}
-
-// The host loop's progress record (ba_ctl_publish of the submitted loop)
-void host_publish(cosl_ba_solver* s, int round, int itno, int trials, double p_eL2, double init_eL2, double mu) {
-  if (!s->loopReq) return;
-  std::lock_guard<std::mutex> lk(s->hostProgMu);
-  BaProgress& g = s->hostProg;
-  g.seq0 = g.seq1 = g.seq1 + 1;
-  g.req = s->loopReq;
-  g.round = round;
-  g.itno = itno;
-  g.trials = trials;
-  g.p_eL2 = p_eL2;
-  g.init_eL2 = init_eL2;
-  g.mu = mu;
-}
-
-/* Weighted SBA LM, control flow identical to oracle/ba_oracle.cpp:levmar.  Through the handle
- * (s->loopReq) it also ends the round with reason 8 when the caller asks to stop, at the points where the
- * submitted loop checks (ba_ctl.cuh), and keeps the progress record. */
-int levmar(cosl_ba_solver* s, int itmax, const double opts[5], double info[10], int fixed_trials) {
-  const double tau = opts[0], eps1 = opts[1], eps2 = opts[2], eps2_sq = opts[2] * opts[2],
-               eps3 = opts[3], eps4 = opts[4];
-  const double EPS_SQ = 1e-24;
-  double mu = 0, nu = 2;
-  int stop = 0, itno = 0;
-  s->nfev = s->njev = s->nlss = 0;
-  double p_eL2 = 0;
-  bool finite = true;
-  COSL_TRY(eval_cost(s, s->d_pa, s->d_pb, &p_eL2, &finite));
-  const double init_eL2 = p_eL2;
-  double ginf = 0, maxdiag = 0, dp_L2 = 0;
-  if (!finite) stop = 7;
-  host_publish(s, s->hpRound, 0, s->hpTrials0, p_eL2, init_eL2, mu);
-  for (itno = 0; itno < itmax && !stop; ++itno) {
-    COSL_TRY(linearize(s, itno == 0, itno > 0 && !fixed_trials));
-    // ginf / maxdiag are needed on the host for mu0 (first iteration) and for the eps1 stop test.  After
-    // the first iteration the test is evaluated one read-back LATE: the scalars stay in d_sc (nothing
-    // below touches SC_GINF / SC_MAXDIAG) and arrive with the read-back of the next trial, which is
-    // discarded if the test fires -- it only wrote the trial buffers.  Same decisions and counters as
-    // the oracle, one host synchronisation less per LM iteration.
-    bool ginfPending = false;
-    if (itno == 0) {
-      COSL_TRY(read_sc(s));
-      ginf = s->h_sc[SC_GINF];
-      maxdiag = s->h_sc[SC_MAXDIAG];
-    } else if (!fixed_trials) {
-      ginfPending = true;
-    }
-    if (!fixed_trials && !ginfPending && ginf <= eps1) {
-      stop = 1;
-      break;
-    }
-    if (itno == 0) mu = tau * maxdiag;
-    if (host_stop_asked(s)) {  // into the first trial of the iteration: it is not counted
-      stop = BA_STOP_CALLER;
-      break;
-    }
-    host_publish(s, s->hpRound, itno, s->hpTrials0 + s->nlss, p_eL2, init_eL2, mu);
-    bool lateStop = false;
-    while (true) {
-      bool solved = false, accepted = false;
-      COSL_TRY(solve_trial(s, mu, &solved));
-      // trial cost, merged scalar all-reduce
-      ++s->nfev;  // (cost / non-finite scalars were cleared by solve_trial)
-      if (!s->costDone) {
-        s->timer.begin(s->secCost, s->rq.stream);
-        if (s->N)
-          COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d,
-                      s->d_na, s->d_nb, 0, 0.0, nullptr);
-        s->timer.end(s->rq.stream);
-      }
-      COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
-      COSL_TRY(read_sc(s));
-      if (ginfPending) {
-        ginfPending = false;
-        ginf = s->h_sc[SC_GINF];
-        maxdiag = s->h_sc[SC_MAXDIAG];
-        if (ginf <= eps1) {  // the eps1 test of this iteration: the trial just run never happened
-          --s->nlss;
-          --s->nfev;
-          stop = 1;
-          lateStop = true;
-          break;
-        }
-      }
-      solved = (s->h_sc[SC_FAIL] == 0.0);
-      if (solved) {
-        dp_L2 = s->h_sc[SC_DP_L2];
-        const double dL = s->h_sc[SC_DL], p_L2 = s->h_sc[SC_P_L2];
-        if (!fixed_trials) {
-          if (dp_L2 <= eps2_sq * p_L2) {
-            stop = 2;
-            break;
-          }
-          if (dp_L2 >= (p_L2 + eps2) / EPS_SQ) {
-            stop = 4;
-            break;
-          }
-        }
-        const double pdp_eL2 = s->h_sc[SC_COST];
-        if (!std::isfinite(pdp_eL2) || s->h_sc[SC_NONFINITE] != 0.0) {
-          stop = 7;
-          break;
-        }
-        const double dF = p_eL2 - pdp_eL2;
-        if (s->opt.verbose && rank_of(s) == 0)
-          std::printf("  [gpu LM %d] mu %.3e cost %.9g -> %.9g dL %.3e\n", itno, mu, p_eL2, pdp_eL2,
-                      dL);
-        if (dF > 0 && dL > 0) {
-          double tmp = 2 * dF / dL - 1;
-          tmp = 1 - tmp * tmp * tmp;
-          mu = mu * std::max(tmp, 1.0 / 3.0);
-          nu = 2;
-          if (!fixed_trials && (std::sqrt(p_eL2) - std::sqrt(pdp_eL2)) < eps4 * std::sqrt(p_eL2))
-            stop = 6;
-          std::swap(s->d_pa, s->d_na);
-          std::swap(s->d_pb, s->d_nb);
-          p_eL2 = pdp_eL2;
-          accepted = true;
-        }
-      }
-      if (fixed_trials && s->nlss >= fixed_trials) {
-        stop = 3;
-        break;
-      }
-      if (accepted) break;
-      mu *= nu;
-      const double nu2 = nu * 2;
-      if (!(nu2 > nu) || !std::isfinite(mu)) {
-        stop = 5;
-        break;
-      }
-      nu = nu2;
-      host_publish(s, s->hpRound, itno, s->hpTrials0 + s->nlss, p_eL2, init_eL2, mu);
-      if (host_stop_asked(s)) {  // into the next trial: the iteration is not counted
-        stop = BA_STOP_CALLER;
-        lateStop = true;
-        break;
-      }
-    }
-    if (lateStop) break;
-    if (!fixed_trials && p_eL2 <= eps3) stop = 3;
-    if (itno + 1 < itmax && !stop && host_stop_asked(s)) stop = BA_STOP_CALLER;  // into the next linearisation
-    host_publish(s, s->hpRound, itno + 1, s->hpTrials0 + s->nlss, p_eL2, init_eL2, mu);
-  }
-  if (itno >= itmax && !stop) stop = 3;
-  if (info) {
-    info[0] = init_eL2;
-    info[1] = p_eL2;
-    info[2] = ginf;
-    info[3] = dp_L2;
-    info[4] = maxdiag > 0 ? mu / maxdiag : 0;
-    info[5] = itno;
-    info[6] = stop;
-    info[7] = s->nfev;
-    info[8] = s->njev;
-    info[9] = s->nlss;
-  }
-  return COSL_OK;
-}
-
-int run_robust(cosl_ba_solver* s, int fixed_trials, double info[COSL_BA_INFOSZ]) {
-  double sinfo[10] = {0};
-  double first_e0 = -1;
-  int total_trials = 0;
+// The host driver of the robust loop (run, run_fixed and the handle-less entry points): after each stage the
+// scalars it needs are read back and ba_lm_decide picks the next stage, the decisions ba_ctl_step takes on the
+// device for submit.  Through the handle (s->loopReq) it stops when the caller asks and keeps the progress
+// record.  info[11]: wall time.
+int run_host(cosl_ba_solver* s, int fixedTrials, double info[COSL_BA_INFOSZ]) {
+  const BaLmParams P = lm_params(s, fixedTrials);
   COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
   const auto t0 = std::chrono::steady_clock::now();
-  const int rounds = fixed_trials ? 1 : std::max(1, s->opt.outer_iters);
-  int ran = 0;
-  for (int r = 0; r < rounds; ++r) {
-    if (r > 0 && host_stop_asked(s)) {  // into the next round: the round that ended reports the stop
-      sinfo[6] = BA_STOP_CALLER;
-      break;
+  BaCtl c;
+  ba_lm_start(c);
+  while (true) {
+    COSL_TRY(clear_sc(s, ba_lm_cleared(c, P)));
+    if (c.done) break;
+    const int stage = c.stage, itno = c.itno;
+    const double mu = c.mu, p_eL2 = c.p_eL2;
+    COSL_TRY(enqueue_stage(s, s->rq.stream, stage, nullptr, mu, c.statsPending));
+    // a linearisation at itno > 0 is decided without its statistics: they arrive with the next trial's
+    if (stage != BA_STAGE_LIN) COSL_TRY(read_sc(s));
+    ba_lm_decide(c, s->h_sc, P, s->loopReq && s->stopReq.load(std::memory_order_relaxed) == s->loopReq);
+    if (c.rated && s->opt.verbose && rank_of(s) == 0)
+      std::printf("  [gpu LM %d] mu %.3e cost %.9g -> %.9g dL %.3e\n", itno, mu, p_eL2, s->h_sc[SC_COST],
+                  s->h_sc[SC_DL]);
+    if (c.copy) {
+      std::swap(s->d_pa, s->d_na);
+      std::swap(s->d_pb, s->d_nb);
     }
-    s->hpRound = r + 1;
-    s->hpTrials0 = total_trials;
-    COSL_TRY(compute_weights(s));
-    COSL_TRY(levmar(s, fixed_trials ? (1 << 30) : s->opt.inner_iters, s->opt.opts, sinfo,
-                    fixed_trials));
-    if (first_e0 < 0) first_e0 = sinfo[0];
-    total_trials += (int)sinfo[9];
-    ++ran;
-    if (sinfo[6] == BA_STOP_CALLER) break;
+    if (s->loopReq) {
+      std::lock_guard<std::mutex> lk(s->hostProgMu);
+      BaProgress& g = s->hostProg;
+      g.seq0 = g.seq1 = g.seq1 + 1;
+      g.req = s->loopReq;
+      ba_lm_progress(c, g);
+    }
   }
-  // the final record: what info reports (mu as levmar last left it; only this thread writes the record)
-  host_publish(s, ran, (int)sinfo[5], total_trials, sinfo[1], sinfo[0], s->hostProg.mu);
-  double nout = 0;
-  if (s->opt.max_err > 0) {  // the same branch on every rank (options are global): collective inside
-    COSL_TRY(zero_sc(s, SC_COST, 1));
-    if (s->N)
-      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d, s->d_pa,
-                  s->d_pb, 2, s->opt.max_err, s->d_outlier);
-    COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
-    COSL_TRY(read_sc(s));
-    nout = s->h_sc[SC_COST];  // outliers over ALL ranks' observations
-  } else {
-    COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, s->rq.stream));
-    COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
-  }
-  const auto t1 = std::chrono::steady_clock::now();
-  if (info) {
-    for (int k = 0; k < COSL_BA_INFOSZ; ++k) info[k] = 0;
-    for (int k = 0; k < 10; ++k) info[k] = sinfo[k];
-    info[0] = first_e0;
-    info[10] = total_trials;
-    info[11] = std::chrono::duration<double>(t1 - t0).count();
-    info[12] = sinfo[1];
-    info[13] = nout;
-  }
+  COSL_TRY(enqueue_outliers(s, s->rq.stream));
+  COSL_TRY(read_sc(s));
+  const double seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  fill_info(info, c, seconds, s->h_sc[SC_COST], P.outliers);
   return COSL_OK;
 }
 
@@ -1525,7 +1343,7 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
   if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, st, cd, s->d_pa, s->d_pb);
   // mu = 0: S and V^-1 of the undamped system (and the cleared scalars and task counters)
   const int nTilesInit = std::max(1, s->plan.nTiles);
-  COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)n + m, 256), 256, 0, st, cd, 0.0, 1,
+  COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)n + m, 256), 256, 0, st, cd, nullptr, 0.0, 1,
               s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks, nTilesInit,
               s->d_Vinv, 0, nullptr, 0LL);
   if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 0, 0.0, nullptr);
@@ -1576,56 +1394,6 @@ int capture_conditional(cudaStream_t cs, cudaGraphConditionalHandle h, cudaGraph
   return COSL_OK;
 }
 
-// the kernels of one stage of the loop body, enqueued on the capturing stream cs
-int enqueue_stage(cosl_ba_solver* s, cudaStream_t cs, int stage) {
-  const unsigned gN = (unsigned)div_up64(s->N, 256);
-  if (stage == BA_STAGE_ROUND) {  // compute_weights + levmar's initial cost
-    if (s->opt.max_err > 0) {
-      if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, cs, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
-    } else if (s->N) {
-      COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, cs, s->d_wgt, s->N, 1.0);
-    }
-    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, cs, s->d, s->d_pa, s->d_pb, 0, 0.0, nullptr);
-  } else if (stage == BA_STAGE_LIN0 || stage == BA_STAGE_LIN) {  // linearize()
-    const long long nV = 9LL * s->n + 27LL * s->m;
-    COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, cs, s->d_V, nV, 0.0);
-    if (s->N) COSL_LAUNCH(ba_linearize_points, gN, 256, 0, cs, s->d, s->d_pa, s->d_pb);
-    if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, cs, s->d, s->d_pa, s->d_pb);
-    // at itno > 0 the prep kernel of the next trial computes the statistics, unless there is none
-    if (stage == BA_STAGE_LIN0 || !s->ns)
-      COSL_LAUNCH(ba_stats_kernel, (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, cs, s->d);
-  } else if (s->ns) {  // solve_trial + the trial cost, free cameras
-    const int nTilesInit = std::max(1, s->plan.nTiles);
-    COSL_LAUNCH(ba_prep_kernel_ctl, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, cs, s->d,
-                s->d_ctl, 1, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks,
-                nTilesInit, s->d_Vinv, s->d_dpb, 3LL * s->n);
-    if (s->nItems)
-      COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, cs, s->d,
-                  s->d_items, s->nItems, s->d_entries, s->d_Vinv);
-    if (s->twoSolve)
-      COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, cs, s->td, s->two00, s->two10, s->two11);
-    else
-      COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, cs, s->td);
-    const int nCamBlocks = div_up(6 * s->m, 256);
-    COSL_LAUNCH(ba_back_cams_points_ctl, nCamBlocks + gN, 256, 0, cs, s->d, s->d_ctl, s->d_pa, s->d_x, s->d_dpa,
-                s->d_na, 1, nCamBlocks, s->d_dpb);
-    if (s->N + s->n)  // a problem without points never reaches a trial (|g| = 0 stops it), but is captured
-      COSL_LAUNCH(ba_finish_cost_ctl, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, cs, s->d, s->d_ctl,
-                  s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv);
-  } else {  // solve_trial + the trial cost, no free camera
-    COSL_LAUNCH(ba_cam_update_ctl,
-                std::max(div_up(6 * s->m, 256), (int)std::min<long long>(s->numSM, div_up64(3LL * s->n, 1024))), 256,
-                0, cs, s->d, s->d_ctl, s->d_pa, s->d_x, s->d_dpa, s->d_na, 1, s->d_nb, 3LL * s->n);
-    if (s->N) COSL_LAUNCH(ba_back_subst, gN, 256, 0, cs, s->d, s->d_dpa, s->d_nb);
-    if (s->n)
-      COSL_LAUNCH(ba_back_finish_ctl, (unsigned)div_up64(s->n, 256), 256, 0, cs, s->d, s->d_ctl, s->d_pb, s->d_nb,
-                  s->d_dpb);
-    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, cs, s->d, s->d_na, s->d_nb, 0, 0.0, nullptr);
-  }
-  COSL_CUDA(cudaGetLastError());
-  return COSL_OK;
-}
-
 // capture into `g` on cs, leaving an empty node in a body that has no kernel (e.g. no observations)
 template <typename F>
 int capture_into(cudaStream_t cs, cudaGraph_t g, F&& enqueue) {
@@ -1649,32 +1417,16 @@ int capture_into(cudaStream_t cs, cudaGraph_t g, F&& enqueue) {
 //   -> outlier pass -> covariance stage (when armed)
 int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
   BaCtlParams P = {};
-  const double* o = s->opt.opts;
-  P.tau = o[0];
-  P.eps1 = o[1];
-  P.eps2 = o[2];
-  P.eps3 = o[3];
-  P.eps4 = o[4];
-  P.rounds = std::max(1, s->opt.outer_iters);
-  P.itmax = s->opt.inner_iters;
-  P.ns = s->ns;
-  P.hasObs = s->N > 0;
-  P.outliers = s->opt.max_err > 0;
+  P.lm = lm_params(s, 0);
   P.link = s->d_link;
   COSL_CUDA(cudaGraphConditionalHandleCreate(&P.hLoop, g, 1, cudaGraphCondAssignDefault));
   for (int k = 0; k < BA_NSTAGES; ++k)
     COSL_CUDA(cudaGraphConditionalHandleCreate(&P.hStage[k], g, k == BA_STAGE_ROUND ? 1 : 0, cudaGraphCondAssignDefault));
   cudaGraph_t loopBody = nullptr, stageBody[BA_NSTAGES] = {};
   COSL_TRY(capture_into(cs, g, [&]() -> int {
-    COSL_LAUNCH(ba_ctl_init, 1, 32, 0, cs, s->d_ctl, s->d_sc);
+    COSL_LAUNCH(ba_ctl_init, 1, 32, 0, cs, s->d_ctl, s->d_sc, P.lm);
     COSL_TRY(capture_conditional(cs, P.hLoop, cudaGraphCondTypeWhile, &loopBody));
-    if (s->opt.max_err > 0) {  // the outlier pass of run_robust; ba_ctl_step cleared the count
-      if (s->N)
-        COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, cs, s->d, s->d_pa, s->d_pb, 2,
-                    s->opt.max_err, s->d_outlier);
-    } else {
-      COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, cs));
-    }
+    COSL_TRY(enqueue_outliers(s, cs));
     if (s->covVar > 0) COSL_TRY(enqueue_cov(s, cs));
     COSL_CUDA(cudaGetLastError());
     return COSL_OK;
@@ -1688,7 +1440,9 @@ int build_graph_nodes(cosl_ba_solver* s, cudaStream_t cs, cudaGraph_t g) {
     COSL_CUDA(cudaGetLastError());
     return COSL_OK;
   }));
-  for (int k = 0; k < BA_NSTAGES; ++k) COSL_TRY(capture_into(cs, stageBody[k], [&]() { return enqueue_stage(s, cs, k); }));
+  // the trial kernels read mu and doStats from the control block; a submitted loop always wants the statistics
+  for (int k = 0; k < BA_NSTAGES; ++k)
+    COSL_TRY(capture_into(cs, stageBody[k], [&]() { return enqueue_stage(s, cs, k, s->d_ctl, 0.0, 1); }));
   return COSL_OK;
 }
 
@@ -1708,7 +1462,10 @@ int build_graph(cosl_ba_solver* s) {
   COSL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaGraphCreate(&g, 0);
+  const bool timing = s->timer.enabled;
+  s->timer.enabled = false;  // the section timers time the host driver's stages, not a capture
   int rc = e == cudaSuccess ? build_graph_nodes(s, cs, g) : set_error(COSL_E_CUDA, "cudaGraphCreate: %s", cudaGetErrorString(e));
+  s->timer.enabled = timing;
   const double t1 = now_s();
   bool updated = false;
   if (rc == COSL_OK && s->graphExec) {
@@ -1864,7 +1621,7 @@ int cosl_ba_solver_run(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   s->hostRunning.store(1);
   s->reqNo.store(s->loopReq);
   s->covValid = false;
-  int rc = run_robust(s, 0, info);
+  int rc = run_host(s, 0, info);
   if (rc == COSL_OK && s->covVar > 0) rc = run_cov(s);
   s->hostRunning.store(0);
   s->loopReq = 0;
@@ -1875,7 +1632,7 @@ int cosl_ba_solver_run_fixed(cosl_ba_solver* s, int trials, double info[COSL_BA_
   BA_ENTER(s)
   COSL_TRY(s->rq.idle("cosl_ba_solver_run_fixed"));
   s->covValid = false;
-  return run_robust(s, trials < 1 ? 1 : trials, info);
+  return run_host(s, trials < 1 ? 1 : trials, info);
 }
 
 int cosl_ba_solver_download(cosl_ba_solver* s, cosl_ba_problem* prob) {
@@ -1935,23 +1692,7 @@ int cosl_ba_solver_collect(cosl_ba_solver* s, double info[COSL_BA_INFOSZ]) {
   COSL_CUDA(cudaMemcpyAsync(&c, s->d_ctl, sizeof(c), cudaMemcpyDeviceToHost, s->rq.stream));
   COSL_CUDA(cudaMemcpyAsync(&nout, s->d_sc + SC_COST, sizeof(double), cudaMemcpyDeviceToHost, s->rq.stream));
   COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
-  if (info) {  // the fields of run_robust
-    for (int k = 0; k < COSL_BA_INFOSZ; ++k) info[k] = 0;
-    info[0] = c.first_e0;
-    info[1] = c.p_eL2;
-    info[2] = c.ginf;
-    info[3] = c.dp_L2;
-    info[4] = c.maxdiag > 0 ? c.mu / c.maxdiag : 0;
-    info[5] = c.itno;
-    info[6] = c.stop;
-    info[7] = c.nfev;
-    info[8] = c.njev;
-    info[9] = c.nlss;
-    info[10] = c.totalTrials;
-    info[11] = 1e-3 * ms;
-    info[12] = c.p_eL2;
-    info[13] = s->opt.max_err > 0 ? nout : 0.0;
-  }
+  fill_info(info, c, 1e-3 * ms, nout, s->opt.max_err > 0);
   return COSL_OK;
 }
 
@@ -2402,7 +2143,7 @@ int cosl_ba_solve(cosl_ba_problem* prob, const cosl_ba_options* opt,
   const double t0 = now_s();
   COSL_TRY(cosl_ba_solver_create(prob, opt, nullptr, &s));
   const double t1 = now_s();
-  int rc = run_robust(s, 0, info);
+  int rc = run_host(s, 0, info);
   const double t2 = now_s();
   if (rc == COSL_OK) rc = download(s, prob);
   const double t3 = now_s();

@@ -21,6 +21,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ba_lm.cuh"
+
 namespace coslam {
 
 struct BaDev {
@@ -44,19 +46,6 @@ struct BaDev {
   double* rhs;        // block padded: block k at rhs + 64 k
   const int* solIdx;  // per free camera: index of its first row in rhs / x
   double* sc;         // scalars, see BaScalar
-};
-
-enum BaScalar {
-  SC_COST = 0,     // sum w |e|^2 of the evaluated parameter set
-  SC_DP_L2 = 1,    // |dp|^2
-  SC_DL = 2,       // dp . (mu dp + g)
-  SC_P_L2 = 3,     // |p|^2 over free parameters
-  SC_NONFINITE = 4,
-  SC_NSUM = 8,     // [0, SC_NSUM) are sums (all-reduce sum)
-  SC_GINF = 8,     // |g|_inf                 (all-reduce max)
-  SC_MAXDIAG = 9,  // max diag(U, V)
-  SC_FAIL = 10,    // Cholesky break-down flag
-  SC_NTOT = 16
 };
 
 __device__ __forceinline__ void atomic_max_nonneg(double* addr, double v) {
@@ -421,11 +410,17 @@ __device__ __forceinline__ void inv3sym_mu(const double* __restrict__ V, double 
 // (ba_tile_init_body), the following blocks compute the damped inverses V*_i^-1 (one point per thread) and --
 // when a linearisation preceded this trial (doStats) -- the gradient / diagonal statistics |g|_inf and
 // max diag(U, V) that the host needs for the eps1 test (it reads them with the trial's scalars).  Block 0
-// also clears the scalars of the trial and the grid clears the task counters of the solve.
+// also clears the scalars of the trial and the grid clears the task counters of the solve.  ctl (the submitted
+// loop): mu and doStats come from the control block.
 __global__ void __launch_bounds__(256)
-ba_prep_kernel(BaDev d, double mu, int addU, const int* __restrict__ diagBlk, const int* __restrict__ blkCam0,
-               const int* __restrict__ order, int* __restrict__ cnt, int nCnt, int nTiles,
-               double* __restrict__ Vinv, int doStats, double* __restrict__ zeroBuf, long long zeroCount) {
+ba_prep_kernel(BaDev d, const BaCtl* __restrict__ ctl, double mu, int addU, const int* __restrict__ diagBlk,
+               const int* __restrict__ blkCam0, const int* __restrict__ order, int* __restrict__ cnt, int nCnt,
+               int nTiles, double* __restrict__ Vinv, int doStats, double* __restrict__ zeroBuf,
+               long long zeroCount) {
+  if (ctl) {
+    mu = ctl->mu;
+    doStats = ctl->statsPending;
+  }
   for (int q = blockIdx.x * 256 + threadIdx.x; q < nCnt; q += gridDim.x * 256) cnt[q] = 0;
   // accumulator of the point back-substitution (ba_back_cams_points)
   for (long long q = (long long)blockIdx.x * 256 + threadIdx.x; q < zeroCount; q += (long long)gridDim.x * 256)
@@ -745,8 +740,11 @@ ba_back_subst(BaDev d, const double* __restrict__ dpa, double* __restrict__ acc3
 
 // Back substitution, step 2, one point per thread: nb holds t_i on entry; db_i = V*_i^-1 (eb_i - t_i),
 // nb <- pb + db, plus the point-side parts of |dp|^2, dL, |p|^2.
-__device__ __forceinline__ void ba_back_finish_body(const BaDev& d, const double* __restrict__ pb,
-                                                    double* __restrict__ nb, double* __restrict__ dpb, double mu) {
+// ctl (the submitted loop): mu comes from the control block.
+__global__ void __launch_bounds__(256)
+ba_back_finish(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__ pb, double* __restrict__ nb,
+               double* __restrict__ dpb, double mu) {
+  if (ctl) mu = ctl->mu;
   __shared__ double s_red[8];
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double dp2 = 0, dl = 0, p2 = 0;
@@ -782,18 +780,13 @@ __device__ __forceinline__ void ba_back_finish_body(const BaDev& d, const double
   if (threadIdx.x == 0 && t != 0) atomicAdd(&d.sc[SC_P_L2], t);
 }
 
-__global__ void __launch_bounds__(256)
-ba_back_finish(BaDev d, const double* __restrict__ pb, double* __restrict__ nb,
-               double* __restrict__ dpb, double mu) {
-  ba_back_finish_body(d, pb, nb, dpb, mu);
-}
-
 // Trial camera parameters na = pa + dpa and the camera-side parts of |dp|^2, dL, |p|^2.
-// addSums: only one rank contributes the (replicated) camera-side sums.
-__device__ __forceinline__ void ba_cam_update_body(const BaDev& d, const double* __restrict__ pa,
-                                                   const double* __restrict__ sol, double* __restrict__ dpa,
-                                                   double* __restrict__ na, double mu, int addSums,
-                                                   double* __restrict__ zeroBuf, long long zeroCount) {
+// addSums: only one rank contributes the (replicated) camera-side sums.  ctl: mu from the control block.
+__global__ void __launch_bounds__(256)
+ba_cam_update(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__ pa, const double* __restrict__ sol,
+              double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums, double* __restrict__ zeroBuf,
+              long long zeroCount) {
+  if (ctl) mu = ctl->mu;
   __shared__ double s_red[8];
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   for (long long q = t; q < zeroCount; q += (long long)gridDim.x * blockDim.x) zeroBuf[q] = 0.0;
@@ -818,13 +811,6 @@ __device__ __forceinline__ void ba_cam_update_body(const BaDev& d, const double*
   if (threadIdx.x == 0 && addSums && s != 0) atomicAdd(&d.sc[SC_P_L2], s);
 }
 
-__global__ void __launch_bounds__(256)
-ba_cam_update(BaDev d, const double* __restrict__ pa, const double* __restrict__ sol,
-              double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums,
-              double* __restrict__ zeroBuf, long long zeroCount) {
-  ba_cam_update_body(d, pa, sol, dpa, na, mu, addSums, zeroBuf, zeroCount);
-}
-
 // ------------------------------------------------------------------------------------------
 // Back substitution in two launches (instead of cam update | memset | point accumulate | point finish | cost):
 //  ba_back_cams_points: blocks [0, nCamBlocks) form the trial camera parameters na = pa + da and the camera-side
@@ -835,13 +821,15 @@ ba_cam_update(BaDev d, const double* __restrict__ pa, const double* __restrict__
 //    accumulator (read-only here; the FIRST observation of a point stores nb_i = pb_i + db_i and adds the
 //    point-side sums), then the weighted squared residual at (na, nb_i) -> cost.  Extra threads finish the
 //    points that have no observation.
+// Both take mu from ctl, the control block of the submitted loop, when it is set.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ba_back_cams_points_body(const BaDev& d, const double* __restrict__ pa,
-                                                         const double* __restrict__ sol, double* __restrict__ dpa,
-                                                         double* __restrict__ na, double mu, int addSums,
-                                                         int nCamBlocks, double* __restrict__ acc3) {
+__global__ void __launch_bounds__(256)
+ba_back_cams_points(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__ pa,
+                    const double* __restrict__ sol, double* __restrict__ dpa, double* __restrict__ na, double mu,
+                    int addSums, int nCamBlocks, double* __restrict__ acc3) {
   __shared__ double s_red[8];
   if ((int)blockIdx.x < nCamBlocks) {
+    if (ctl) mu = ctl->mu;
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     double dp2 = 0, dl = 0, p2 = 0;
     if (t < 6 * d.m) {
@@ -893,16 +881,9 @@ __device__ __forceinline__ void ba_back_cams_points_body(const BaDev& d, const d
 }
 
 __global__ void __launch_bounds__(256)
-ba_back_cams_points(BaDev d, const double* __restrict__ pa, const double* __restrict__ sol,
-                    double* __restrict__ dpa, double* __restrict__ na, double mu, int addSums, int nCamBlocks,
-                    double* __restrict__ acc3) {
-  ba_back_cams_points_body(d, pa, sol, dpa, na, mu, addSums, nCamBlocks, acc3);
-}
-
-__device__ __forceinline__ void ba_finish_cost_body(const BaDev& d, const double* __restrict__ na,
-                                                    const double* __restrict__ pb, double* __restrict__ nb,
-                                                    const double* __restrict__ acc3,
-                                                    const double* __restrict__ Vinv, double mu) {
+ba_finish_cost(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__ na, const double* __restrict__ pb,
+               double* __restrict__ nb, const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu) {
+  if (ctl) mu = ctl->mu;
   __shared__ double s_red[8];
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double dp2 = 0, dl = 0, p2 = 0, c = 0;
@@ -966,12 +947,6 @@ __device__ __forceinline__ void ba_finish_cost_body(const BaDev& d, const double
   if (threadIdx.x == 0 && s != 0) atomicAdd(&d.sc[SC_DL], s);
   s = block_sum_1(p2, s_red);
   if (threadIdx.x == 0 && s != 0) atomicAdd(&d.sc[SC_P_L2], s);
-}
-
-__global__ void __launch_bounds__(256)
-ba_finish_cost(BaDev d, const double* __restrict__ na, const double* __restrict__ pb, double* __restrict__ nb,
-               const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu) {
-  ba_finish_cost_body(d, na, pb, nb, acc3, Vinv, mu);
 }
 
 // ------------------------------------------------------------------------------------------
