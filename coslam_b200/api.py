@@ -82,6 +82,8 @@ def _load():
     L.cosl_pose_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
     L.cosl_pose_solver_stream.argtypes = [vp]
     L.cosl_pose_solver_stream.restype = vp
+    L.cosl_pose_solver_set_covariance.argtypes = [vp, cd]
+    L.cosl_pose_solver_download_covariance.argtypes = [vp, vp, vp, vp]
     L.cosl_ba_options_default.argtypes = [C.POINTER(BaOptions)]
     L.cosl_ba_solve.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp]
     L.cosl_ba_solve_multi.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), ci, vp, vp]
@@ -579,13 +581,15 @@ class PoseSolver(_SolverHandle):
         _ck(LIB.cosl_pose_solver_create(int(device), int(max_cams), int(max_pts), C.byref(h)))
         self.h, self.device, self.max_cams, self.max_pts = h, device, max_cams, max_pts
         self._opts = None
+        self._npts = []  # points per camera of the last accepted submit: the shapes download_covariance returns
 
     def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None):
         """cosl_pose_solver_submit: enqueue pose_intracam_batch's solve and return at once; the input arrays
         may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills."""
-        args, opts, _keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
+        args, opts, keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
         _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
         self._opts = opts
+        self._npts = [len(a) for a in keep[3]]
 
     def collect(self):
         """cosl_pose_solver_collect: wait for the submitted solve.  Returns (ok, R, t, opts) as
@@ -596,6 +600,21 @@ class PoseSolver(_SolverHandle):
         _ck(LIB.cosl_pose_solver_collect(self.h, _ptr(R), _ptr(t), opts, _ptr(ok), C.byref(ms)))
         self._opts = None
         return ok.astype(bool), R.reshape(Cn, 3, 3), t, opts, ms.value
+
+    def set_covariance(self, pixel_var):
+        """cosl_pose_solver_set_covariance: pixel_var > 0 makes every later submit() end with the covariance
+        stage; 0 turns it off."""
+        _ck(LIB.cosl_pose_solver_set_covariance(self.h, float(pixel_var)))
+
+    def download_covariance(self):
+        """cosl_pose_solver_download_covariance after collect() of an armed solve: (cov [C, 6, 6] for (w, dt),
+        err: per camera the residuals of its points in px, stats [C, 4] = sigma2_hat, dof, smallest relative
+        pivot, valid)."""
+        npts = self._npts
+        cov, stats = np.empty((len(npts), 6, 6)), np.empty((len(npts), 4))
+        err = np.empty(sum(npts))
+        _ck(LIB.cosl_pose_solver_download_covariance(self.h, _ptr(cov), _ptr(err), _ptr(stats)))
+        return cov, np.split(err, np.cumsum(npts)[:-1]), stats
 
 
 def ba_solve(prob, opt):

@@ -8,6 +8,9 @@
 // The Jacobian is the reference's forward difference (eps = 1e-8, :43-117) evaluated with non-fused
 // fp64 operations (this file is compiled with -fmad=false) so that the differences see the same
 // roundings as the oracle.
+//
+// An armed pose solver handle (cosl_pose_solver_set_covariance) follows the solve with pose_cov_kernel, the
+// covariance of each refined pose with the analytic Jacobian (an extension, not reference parity).
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -370,6 +373,141 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
   }
 }
 
+// Per-camera layout of the covariance stage's results: cov[36] | sigma2_hat, dof, min relative pivot, valid.
+constexpr int POSE_COV_STRIDE = 40;
+
+// Covariance of the refined pose (an extension: the reference reports none).  One CTA per camera, at the
+// (R_opt, t_opt) that pose_intracam_kernel wrote into outs, in the solver's own chart R' = R exp([w]x),
+// t' = t + dt, order (w, dt):
+//   e_i = |project(K, R_opt, t_opt, M_i) - m_i|, w_i = tukey(e_i, tau), H = sum_i w_i J_i^T J_i with the
+//   analytic 2x6 Jacobian J_i of project, cov = pixel_var H^-1 by Cholesky.
+// res[c] gets cov | {sigma2_hat = sum w e^2 / dof (NaN for dof <= 0), dof = 2 #(w > 0) - 6, the smallest
+// relative pivot L_kk^2 / H_kk (0 when the factorisation breaks down), valid}; a break-down or a relative pivot
+// below 1e-12 gives a NaN covariance and valid = 0.  errAll gets e_i of every point, in the packed order.
+__global__ void __launch_bounds__(POSE_THREADS)
+pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
+                const double* __restrict__ msAll, const PoseOut* __restrict__ outs, double tau, double pixel_var,
+                double* __restrict__ res, double* __restrict__ errAll) {
+  __shared__ double s_red[(POSE_THREADS / 32) * 23];
+  const PoseCam& cam = cams[blockIdx.x];
+  const int n = cam.npts;
+  const double* Ms = MsAll + 3 * cam.off;
+  const double* ms = msAll + 2 * cam.off;
+  double K[9], R[9], t[3];
+  for (int k = 0; k < 9; ++k) {
+    K[k] = cam.K[k];
+    R[k] = outs[blockIdx.x].R[k];
+  }
+  for (int k = 0; k < 3; ++k) t[k] = outs[blockIdx.x].t[k];
+  double acc[23];  // 21 upper-triangle entries of H, sum w e^2, #(w > 0)
+#pragma unroll
+  for (int k = 0; k < 23; ++k) acc[k] = 0;
+  for (int i = threadIdx.x; i < n; i += POSE_THREADS) {
+    const double* M = Ms + 3 * i;
+    double rm[2];
+    project(K, R, t, M, rm);
+    const double dx = rm[0] - ms[2 * i], dy = rm[1] - ms[2 * i + 1];
+    const double e = sqrt(dx * dx + dy * dy);
+    errAll[cam.off + i] = e;
+    const double w = tukey(e, tau);
+    if (w > 0) {
+      // x = K c, c = R M + t; m = x_{0,1} / x_2.  dm/dc rows a, b; dc/dt = I; dc/dw_k = R (e_k x M), so
+      // dm_0/dw = M x (R^T a) and dm_1/dw = M x (R^T b)
+      const double c0 = R[0] * M[0] + R[1] * M[1] + R[2] * M[2] + t[0];
+      const double c1 = R[3] * M[0] + R[4] * M[1] + R[5] * M[2] + t[1];
+      const double c2 = R[6] * M[0] + R[7] * M[1] + R[8] * M[2] + t[2];
+      const double z = K[6] * c0 + K[7] * c1 + K[8] * c2;
+      double J[12];  // rows u, v; columns w0 w1 w2 t0 t1 t2
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        J[3 + k] = (K[k] - rm[0] * K[6 + k]) / z;
+        J[9 + k] = (K[3 + k] - rm[1] * K[6 + k]) / z;
+      }
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const double* a = J + 6 * r + 3;
+        const double q0 = R[0] * a[0] + R[3] * a[1] + R[6] * a[2];
+        const double q1 = R[1] * a[0] + R[4] * a[1] + R[7] * a[2];
+        const double q2 = R[2] * a[0] + R[5] * a[1] + R[8] * a[2];
+        J[6 * r + 0] = M[1] * q2 - M[2] * q1;
+        J[6 * r + 1] = M[2] * q0 - M[0] * q2;
+        J[6 * r + 2] = M[0] * q1 - M[1] * q0;
+      }
+      int q = 0;
+#pragma unroll
+      for (int a = 0; a < 6; ++a) {
+#pragma unroll
+        for (int b = a; b < 6; ++b) acc[q++] += w * (J[a] * J[b] + J[6 + a] * J[6 + b]);
+      }
+      acc[21] += w * (e * e);
+      acc[22] += 1;
+    }
+  }
+  block_sum<23>(acc, s_red);
+  if (threadIdx.x != 0) return;
+  // Cholesky H = L L^T in packed lower storage, L(i, j) at i (i + 1) / 2 + j
+  double L[21];
+  double minPiv = INFINITY;
+  bool valid = true;
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    const int jj = j * (j + 1) / 2;
+    const double h = acc[6 * j - j * (j - 1) / 2];  // H(j, j) in the upper-triangle order of acc
+    double d = h;
+#pragma unroll
+    for (int k = 0; k < j; ++k) d -= L[jj + k] * L[jj + k];
+    if (!(d > 0)) {
+      valid = false;
+      minPiv = 0;
+      d = 1;  // keeps the remaining arithmetic finite; the covariance is discarded
+    } else {
+      minPiv = fmin(minPiv, d / h);
+    }
+    const double ljj = sqrt(d);
+    L[jj + j] = ljj;
+#pragma unroll
+    for (int i = j + 1; i < 6; ++i) {
+      const int ii = i * (i + 1) / 2;
+      double s = acc[6 * j - j * (j - 1) / 2 + (i - j)];  // H(j, i), i > j
+#pragma unroll
+      for (int k = 0; k < j; ++k) s -= L[ii + k] * L[jj + k];
+      L[ii + j] = s / ljj;
+    }
+  }
+  if (minPiv < 1e-12) valid = false;
+  // X = L^-1 (lower triangular, packed as L), then cov = pixel_var X^T X
+  double X[21];
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    X[j * (j + 1) / 2 + j] = 1.0 / L[j * (j + 1) / 2 + j];
+#pragma unroll
+    for (int i = j + 1; i < 6; ++i) {
+      const int ii = i * (i + 1) / 2;
+      double s = 0;
+#pragma unroll
+      for (int k = j; k < i; ++k) s += L[ii + k] * X[k * (k + 1) / 2 + j];
+      X[ii + j] = -s / L[ii + i];
+    }
+  }
+  double* r = res + POSE_COV_STRIDE * blockIdx.x;
+#pragma unroll
+  for (int i = 0; i < 6; ++i)
+#pragma unroll
+    for (int j = i; j < 6; ++j) {
+      double s = 0;
+#pragma unroll
+      for (int k = j; k < 6; ++k) s += X[k * (k + 1) / 2 + i] * X[k * (k + 1) / 2 + j];
+      const double v = valid ? pixel_var * s : NAN;
+      r[6 * i + j] = v;
+      r[6 * j + i] = v;
+    }
+  const double dof = 2 * acc[22] - 6;
+  r[36] = dof > 0 ? acc[21] / dof : NAN;
+  r[37] = dof;
+  r[38] = minPiv;
+  r[39] = valid ? 1.0 : 0.0;
+}
+
 // Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
 // cameras.
 int check_cameras(const char* fn, int C, const int* npts, const double* const* Ms, const double* const* ms,
@@ -397,7 +535,8 @@ int check_cameras(const char* fn, int C, const int* npts, const double* const* M
 
 // A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out as
 // PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] (tot = points of the solve); the PoseOuts come back into
-// pinned memory.  Capacity is fixed at create: everything is allocated once.
+// pinned memory.  Capacity is fixed at create: everything is allocated once, the covariance stage's buffers
+// (laid out as res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed.
 struct cosl_pose_solver {
   int device = 0, maxCams = 0, maxPts = 0;
   RequestStream rq;
@@ -406,7 +545,12 @@ struct cosl_pose_solver {
   double* d_W = nullptr;
   PoseOut* d_out = nullptr;
   PoseOut* h_out = nullptr;
-  int C = 0;  // cameras of the solve in flight
+  int C = 0;           // cameras of the solve in flight
+  long long tot = 0;   // points of the solve in flight
+  double pixelVar = 0; // > 0: armed
+  double* d_cov = nullptr;
+  double* h_cov = nullptr;
+  bool covReady = false;  // the last submitted solve was armed
 };
 
 namespace {
@@ -418,11 +562,15 @@ void free_pose_solver(cosl_pose_solver* s) {
   s->rq.destroy();
   if (s->h_in) cudaFreeHost(s->h_in);
   if (s->h_out) cudaFreeHost(s->h_out);
+  if (s->h_cov) cudaFreeHost(s->h_cov);
   cudaFree(s->d_in);
   cudaFree(s->d_W);
   cudaFree(s->d_out);
+  cudaFree(s->d_cov);
   delete s;
 }
+
+size_t cov_doubles(int C, long long tot) { return (size_t)POSE_COV_STRIDE * C + tot; }
 
 int alloc_pose_solver(cosl_pose_solver* s) {
   COSL_CUDA(cudaSetDevice(s->device));
@@ -447,6 +595,12 @@ int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg)
   COSL_LAUNCH(pose_intracam_kernel, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out);
   COSL_CUDA(cudaGetLastError());
   COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, st));
+  if (s->pixelVar > 0) {
+    COSL_LAUNCH(pose_cov_kernel, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar, s->d_cov,
+                s->d_cov + POSE_COV_STRIDE * C);
+    COSL_CUDA(cudaGetLastError());
+    COSL_CUDA(cudaMemcpyAsync(s->h_cov, s->d_cov, sizeof(double) * cov_doubles(C, tot), cudaMemcpyDeviceToHost, st));
+  }
   return COSL_OK;
 }
 
@@ -534,7 +688,11 @@ int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const 
   cfg.lambda0 = opts[0].lambda0;
   cfg.tau = tau;
   s->C = C;
-  return s->rq.submit("cosl_pose_solver_submit", [&]() { return enqueue_solve(s, C, tot, cfg); });
+  s->tot = tot;
+  s->covReady = false;
+  COSL_TRY(s->rq.submit("cosl_pose_solver_submit", [&]() { return enqueue_solve(s, C, tot, cfg); }));
+  s->covReady = s->pixelVar > 0;
+  return COSL_OK;
 }
 
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done) {
@@ -570,6 +728,37 @@ int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, 
 }
 
 void* cosl_pose_solver_stream(cosl_pose_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
+
+int cosl_pose_solver_set_covariance(cosl_pose_solver* s, double pixel_var) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  if (!(pixel_var >= 0) || !std::isfinite(pixel_var))
+    return set_error(COSL_E_INVALID, "cosl_pose_solver_set_covariance: pixel_var %g is not a finite value >= 0",
+                     pixel_var);
+  COSL_TRY(s->rq.idle("cosl_pose_solver_set_covariance"));
+  if (pixel_var > 0) {
+    COSL_CUDA(cudaSetDevice(s->device));
+    const size_t n = cov_doubles(s->maxCams, s->maxPts);
+    if (!s->h_cov) COSL_CUDA(cudaHostAlloc(&s->h_cov, sizeof(double) * n, cudaHostAllocPortable));
+    if (!s->d_cov) COSL_CUDA(cudaMalloc(&s->d_cov, sizeof(double) * n));
+  }
+  s->pixelVar = pixel_var;
+  return COSL_OK;
+}
+
+int cosl_pose_solver_download_covariance(cosl_pose_solver* s, double* cov, double* err, double* out) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  COSL_TRY(s->rq.idle("cosl_pose_solver_download_covariance"));
+  if (!out) return set_error(COSL_E_INVALID, "cosl_pose_solver_download_covariance: null out");
+  if (!s->covReady)
+    return set_error(COSL_E_STATE, "cosl_pose_solver_download_covariance: the last solve was not armed");
+  for (int c = 0; c < s->C; ++c) {
+    const double* r = s->h_cov + POSE_COV_STRIDE * c;
+    if (cov) std::memcpy(cov + 36 * c, r, sizeof(double) * 36);
+    std::memcpy(out + 4 * c, r + 36, sizeof(double) * 4);
+  }
+  if (err) std::memcpy(err, s->h_cov + POSE_COV_STRIDE * s->C, sizeof(double) * s->tot);
+  return COSL_OK;
+}
 
 int cosl_pose_intracam_batch(int C, const double* K9, const double* R0, const double* t0,
                              const int* npts, const double* const* Ms, const double* const* ms,

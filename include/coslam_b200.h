@@ -384,6 +384,29 @@ int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, 
 /* CUDA stream (cudaStream_t as void*) the handle's solves run on; work enqueued there after a
  * submit runs after that solve. */
 void* cosl_pose_solver_stream(cosl_pose_solver* s);
+/* Covariance of each refined pose and the residuals of its points (an extension: the reference
+ * reports no uncertainty for this step).  Per camera, at the R_opt, t_opt collect returns (whatever
+ * ok says), in the solver's own chart R' = R exp([w]x), t' = t + dt, order (w, dt):
+ *   e_i = |pi(K, R_opt, t_opt, M_i) - m_i| in pixels, pi the projection of the solve;
+ *   w_i = (1 - (e_i / tau)^2)^2, 0 for e_i >= tau;
+ *   H = sum_i w_i J_i^T J_i with the analytic 2x6 Jacobian J_i of pi, in fp64;
+ *   cov = pixel_var H^-1, 6x6 row-major, by Cholesky.
+ * A camera whose factorisation breaks down, or whose smallest relative pivot L_kk^2 / H_kk is below
+ * 1e-12 (fewer than 3 weighted points, every point beyond tau), is singular: its covariance is NaN.
+ * Every camera is solved on its own: the others of the same submit are unaffected.
+ * pixel_var > 0 arms the handle: every later submit ends with the stage on the handle's stream and
+ * collect's device_ms includes it.  0 disarms.  Arming allocates the stage's buffers, once, for
+ * maxCams and maxPts; destroy frees them.  COSL_E_INVALID for a NULL handle or a pixel_var that is
+ * negative or not finite; COSL_E_STATE while a solve is in flight. */
+int cosl_pose_solver_set_covariance(cosl_pose_solver* s, double pixel_var);
+/* After collect of an armed solve: cov[C][36] (nullable); err[tot] (nullable), e_i of every point in
+ * submit order, camera-major; out[C][4] = {sigma2_hat, dof, smallest relative pivot, 1 if the
+ * covariance is valid else 0}, with dof = 2 #(w_i > 0) - 6, sigma2_hat = sum w_i e_i^2 / dof (NaN
+ * when dof <= 0) and the smallest relative pivot 0 when the factorisation broke down.  COSL_OK also
+ * when some cameras are singular (flagged in out).  COSL_E_INVALID for a NULL handle or out;
+ * COSL_E_STATE while a solve is in flight, before any armed solve, or after an unarmed submit since
+ * (a disarmed handle keeps the last armed result until its next submit). */
+int cosl_pose_solver_download_covariance(cosl_pose_solver* s, double* cov, double* err, double* out);
 
 /* ================================================================ bundle adjustment */
 
