@@ -9,7 +9,7 @@ Three restatements that must agree with each other:
     rotation v at v = 0, where R(q(v)) = exp([2 v]x) to first order: dx/dw = dx/dv / 2, so Sigma_w = 4 Sigma_v);
   - cov_full(jac=expmap_jacobian): the same with J by complex steps straight through exp([w]x) (Rodrigues);
   - cov_schur: the Schur form the device computes (reduced camera system S = U - W V^-1 W^T, Z = S^-1, point blocks
-    V^-1 + V^-1 (sum W^T Z W) V^-1), with S dense and the points one by one."""
+    V^-1 + V^-1 (sum W^T Z W) V^-1), with S dense and the points' terms batched over observations."""
 import numpy as np
 
 from ba_dense import (H_CS, K_of, _finish, cancellation, layout, local_jacobian, point_of, residuals, rot,
@@ -114,44 +114,50 @@ def cov_full(prob, max_err, pixel_var, jac=omega_jacobian):
     return cam, pt, _info(prob, e, w, unc, pixel_var), H
 
 
+def _pairs(prob, keep):
+    """(oa, ob): every ordered pair of observations of one point that has keep[point], both by free cameras."""
+    cnt = np.diff(prob.ptr)
+    oa, ob = [], []
+    for da in range(int(cnt.max(initial=0))):
+        for db in range(int(cnt.max(initial=0))):
+            i = np.nonzero(keep & (cnt > max(da, db)))[0]
+            a, b = prob.ptr[i] + da, prob.ptr[i] + db
+            free = (prob.cam[a] >= prob.m_con) & (prob.cam[b] >= prob.m_con)
+            oa.append(a[free])
+            ob.append(b[free])
+    return np.concatenate(oa).astype(np.int64), np.concatenate(ob).astype(np.int64)
+
+
 def cov_schur(prob, max_err, pixel_var):
-    """(camCov, ptCov, info) by the Schur form: S dense, points one at a time."""
+    """(camCov, ptCov, info) by the Schur form: S dense, the points' V, W and T batched over observations."""
     e, w, unc = weights(prob, max_err)
     J = omega_jacobian(prob) * np.sqrt(w)[:, None, None]
     A, B = J[:, :, :6], J[:, :, 6:]
     m, n, mcon, ncon = prob.m, prob.n, prob.m_con, prob.n_con
     mf = m - mcon
     pt_of, cam_of = point_of(prob), prob.cam
-    S = np.zeros((6 * mf, 6 * mf))
-    for o in range(prob.nobs):
-        j = cam_of[o] - mcon
-        if j >= 0:
-            S[6 * j:6 * j + 6, 6 * j:6 * j + 6] += A[o].T @ A[o]
-    Vinv, Ws = {}, {}
-    for i in range(ncon, n):
-        if unc[i]:
-            continue
-        obs = np.arange(prob.ptr[i], prob.ptr[i + 1])
-        V = sum(B[o].T @ B[o] for o in obs)
-        Vinv[i] = np.linalg.inv(V)
-        Ws[i] = [(cam_of[o] - mcon, A[o].T @ B[o]) for o in obs if cam_of[o] >= mcon]
-        for ja, Wa in Ws[i]:
-            for jb, Wb in Ws[i]:
-                S[6 * ja:6 * ja + 6, 6 * jb:6 * jb + 6] -= Wa @ Vinv[i] @ Wb.T
+    keep = (np.arange(n) >= ncon) & ~unc
+    Sb = np.zeros((mf, mf, 6, 6))
+    fo = np.nonzero(cam_of >= mcon)[0]
+    np.add.at(Sb, (cam_of[fo] - mcon, cam_of[fo] - mcon), np.einsum("nia,nib->nab", A[fo], A[fo]))
+    V = np.zeros((n, 3, 3))
+    np.add.at(V, pt_of, np.einsum("nia,nib->nab", B, B))
+    Vinv = np.zeros((n, 3, 3))
+    Vinv[keep] = np.linalg.inv(V[keep])
+    W = np.einsum("nia,nib->nab", A, B)  # A^T B per observation
+    oa, ob = _pairs(prob, keep)
+    ja, jb, Vi = cam_of[oa] - mcon, cam_of[ob] - mcon, Vinv[pt_of[oa]]
+    np.add.at(Sb, (ja, jb), -np.einsum("nab,nbc,ndc->nad", W[oa], Vi, W[ob]))
+    S = Sb.transpose(0, 2, 1, 3).reshape(6 * mf, 6 * mf)
     Z = np.linalg.inv(S) if mf else np.zeros((0, 0))
+    Zb = Z.reshape(mf, 6, mf, 6).transpose(0, 2, 1, 3)
     cam = np.zeros((m, 6, 6))
-    for j in range(mf):
-        cam[mcon + j] = pixel_var * Z[6 * j:6 * j + 6, 6 * j:6 * j + 6]
+    cam[mcon:] = pixel_var * Zb[np.arange(mf), np.arange(mf)]
+    T = np.zeros((n, 3, 3))
+    np.add.at(T, pt_of[oa], np.einsum("nba,nbc,ncd->nad", W[oa], Zb[ja, jb], W[ob]))
     pt = np.zeros((n, 3, 3))
-    for i in range(ncon, n):
-        if unc[i]:
-            pt[i] = np.nan
-            continue
-        T = np.zeros((3, 3))
-        for ja, Wa in Ws[i]:
-            for jb, Wb in Ws[i]:
-                T += Wa.T @ Z[6 * ja:6 * ja + 6, 6 * jb:6 * jb + 6] @ Wb
-        pt[i] = pixel_var * (Vinv[i] + Vinv[i] @ T @ Vinv[i])
+    pt[keep] = pixel_var * (Vinv[keep] + Vinv[keep] @ T[keep] @ Vinv[keep])
+    pt[(np.arange(n) >= ncon) & unc] = np.nan
     return cam, pt, _info(prob, e, w, unc, pixel_var)
 
 
@@ -252,3 +258,98 @@ def make(name):
     import ba_dense as bd
     f, max_err = cov_rows()[name]
     return f(), bd.options(max_err)
+
+
+# ---------------------------------------------------------------- edge scenes of the covariance stage
+# Built with the scene() / random_vis() of tests/test_gpu_ba_edges.py (camera 0 at the origin, cameras 0.25 apart
+# along x, points 4-7 in front).  One fixed camera and no fixed point leave the scale free, so every regular row
+# fixes it with a second fixed camera or with fixed points.
+def groups(k, g, blind_group=None, seed=7):
+    """Camera 0 fixed, then k groups of g free cameras that share no point; every third point of a group is also
+    seen by camera 0, and the first three points of every group are fixed: they fix its scale.  The reduced camera
+    system is block-diagonal over the groups.  In `blind_group` the middle camera sees no point: its rows of S are
+    exactly zero, a singular block.  (A group without fixed points is singular in its scale too, but only through
+    the cancellation of S = U - W V^-1 W^T, which leaves that pivot at rounding noise, 1e-13 to 1e-8 relative:
+    not a reliable singular case.)"""
+    import test_gpu_ba_edges as te
+    rng = np.random.default_rng(seed)
+    fixed, rest = [], []
+    for q in range(k):
+        cams = [c for c in range(1 + q * g, 1 + (q + 1) * g) if q != blind_group or c != 1 + q * g + g // 2]
+        vis = te.random_vis(rng, 6 * g, cams, 2, 5)
+        vis = [v + [0] if i % 3 == 0 else v for i, v in enumerate(vis)]
+        fixed += vis[:3]
+        rest += vis[3:]
+    return te.scene(fixed + rest, k * g + 1, 1, len(fixed), seed)
+
+
+def _edge(name):
+    import test_gpu_ba_edges as te
+    rng = np.random.default_rng(sum(map(ord, name)))
+    if name in ("structure_only", "motion_only", "free_camera_sees_only_fixed_points",
+                "points_seen_only_by_fixed_cameras"):
+        return te.make(name)
+    if name == "single_observation_points_fixed":  # 10 points seen once, 8 of them by free cameras
+        return te.scene(te.random_vis(rng, 50, range(6)) + [[1 + k % 5] for k in range(10)], 6, 2, 0, 6)
+    if name == "weight_dropped_points":  # 10 two-observation points: one observation 5 max_err off in y (across
+        # the epipolar lines of cameras displaced along x), the other 0.3 px off at the start
+        from ba_dense import project
+        prob = te.scene(te.random_vis(rng, 50, range(6)) + [[2 + k % 4, 2 + (k + 1) % 4] for k in range(10)],
+                        6, 2, 0, 9)
+        o = prob.ptr[50:60]
+        xy = project(prob)[0]
+        prob.xy[o] = xy[o] + [0.0, 5.0 * te.MAX_ERR]
+        prob.xy[o + 1] = xy[o + 1] + rng.normal(0, 0.3, (10, 2))
+        return prob
+    if name == "one_long_pair_fixed":  # free cameras 2 and 3 share 532 = 4 x 128 + 20 free points
+        return te.scene([[0, 1, 2, 3]] * 532, 4, 2, 0, 8)
+    if name.startswith("groups_"):  # groups_<k>x<g>[_blind<q>]
+        f = name.split("_")
+        k, g = map(int, f[1].split("x"))
+        return groups(k, g, int(f[2][5:]) if len(f) > 2 else None)
+    if name == "points_fix_gauge":  # m_con = 0: four fixed points fix the gauge
+        return te.scene(te.random_vis(rng, 60, range(5), 2, 4), 5, 0, 4, 10)
+    if name == "many_points":  # 6n > 1024 x 256: ba_cov_begin clears T in more than one grid-stride pass
+        return te.scene(te.random_vis(rng, 50000, range(8), 2, 4), 8, 2, 0, 11)
+    raise KeyError(name)
+
+
+# name -> max_err.  motion_only takes 30 px: at 6 px its cameras 3 and 5 have no observation of non-zero weight
+# at the start, so they never move and stay singular.
+EDGE_ROWS = {
+    "structure_only": 6.0, "motion_only": 30.0, "free_camera_sees_only_fixed_points": 6.0,
+    "points_seen_only_by_fixed_cameras": 6.0, "single_observation_points_fixed": 6.0,
+    "weight_dropped_points": 6.0, "one_long_pair_fixed": 6.0,
+    "groups_2x6": 6.0, "groups_2x10": 6.0, "groups_3x10": 6.0, "groups_5x5": 6.0,
+    "points_fix_gauge": 6.0, "many_points": 6.0,
+}
+# the singular block first, in the middle, last
+SINGULAR_EDGE_ROWS = {"groups_3x10_blind0": 6.0, "groups_3x10_blind1": 6.0, "groups_3x10_blind2": 6.0}
+LARGE = ("many_points",)  # beyond cov_full: H has 150 000 rows
+
+
+def make_edge(name):
+    import ba_dense as bd
+    return _edge(name), bd.options({**EDGE_ROWS, **SINGULAR_EDGE_ROWS}[name])
+
+
+def reference(prob, max_err, pixel_var):
+    """(camCov, ptCov, info, H or None): cov_full, or cov_schur where H is too large to invert whole."""
+    if prob.nobs > 20000:
+        return (*cov_schur(prob, max_err, pixel_var), None)
+    return cov_full(prob, max_err, pixel_var)
+
+
+def decision_margin(prob, max_err):
+    """min over the observations of ||e| - max_err| / max_err: how far every Tukey decision is from its tie."""
+    e = residuals(prob)
+    return float((np.abs(np.sqrt((e * e).sum(1)) - max_err) / max_err).min())
+
+
+def min_relative_pivot(H):
+    """smallest L_kk^2 / H_kk of the Cholesky factor of H, 0 when the factorisation breaks down"""
+    try:
+        L = np.linalg.cholesky(H)
+    except np.linalg.LinAlgError:
+        return 0.0
+    return float((np.diag(L) ** 2 / np.diag(H)).min())

@@ -37,6 +37,7 @@ int main(int argc, char** argv) {
       if (pat == "band") on = on || (b - a) <= (int)param;
       if (pat == "dense") on = true;
       if (pat == "random") on = on || (std::abs(U(rng)) < param) || (b - a) <= 2;
+      if (pat == "split") on = on || ((b - a) <= (int)param && (a < mf / 2) == (b < mf / 2));  // two components
       adj[(size_t)a * mf + b] = adj[(size_t)b * mf + a] = on ? 1 : 0;
     }
   const int ns = 6 * mf;

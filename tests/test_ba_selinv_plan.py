@@ -39,6 +39,10 @@ def block_errors(Z, Sinv, mask):
     (100, "random", 0.05), (150, "random", 0.01),
     (200, "band", 20), (200, "band", 20, 0), (200, "band", 20, 2),
     (396, "band", 35), (396, "band", 35, 3),
+    # block-diagonal S (every step without an operation, separator blocks of 6 rows at mf = 100) and two
+    # connected components
+    (12, "band", 0), (20, "band", 0), (25, "band", 0), (30, "band", 0), (61, "band", 0), (100, "band", 0),
+    (100, "band", 0, 2), (40, "split", 3), (41, "split", 2, 1),
 ])
 def test_selinv_plan_matches_the_dense_inverse(emul, tmp_path, args):
     out = subprocess.run([emul, str(tmp_path), *map(str, args)], capture_output=True, text=True, timeout=900)
@@ -50,6 +54,8 @@ def test_selinv_plan_matches_the_dense_inverse(emul, tmp_path, args):
     Z = np.fromfile(tmp_path / "Z.bin").reshape(ns, ns)
     mask = np.fromfile(tmp_path / "mask.bin", np.uint8).reshape(mf, mf)
     assert st["steps"] == st["nb"] and st["tasks"] >= st["nb"]
+    if args[1:3] == ("band", 0):
+        assert st["ops"] == 0 and st["tasks"] == st["nb"], st
     assert np.array_equal(mask, mask.T) and mask.diagonal().all()
     err = block_errors(Z, np.linalg.inv(S), mask)
     assert err.max() < 1e-10, (st, float(err.max()))

@@ -111,7 +111,8 @@ def _spd(mf, pat, param, rng):
     for a in range(mf):
         for b in range(a + 1, mf):
             on = pat == "dense" or (pat == "band" and b - a <= param) or (
-                pat == "random" and (rng.random() < param or b - a <= 2))
+                pat == "random" and (rng.random() < param or b - a <= 2)) or (
+                pat == "split" and b - a <= param and (a < mf // 2) == (b < mf // 2))
             adj[a, b] = adj[b, a] = on
     ns = 6 * mf
     S = rng.uniform(-1, 1, (ns, ns)) * np.kron(adj, np.ones((6, 6)))
@@ -123,7 +124,11 @@ def _spd(mf, pat, param, rng):
 @gpu
 @pytest.mark.parametrize("args", [(1, "dense", 0), (7, "band", 2), (12, "dense", 0), (40, "dense", 0),
                                   (29, "dense", 0), (100, "random", 0.05), (200, "band", 20, 2),
-                                  (396, "band", 35, 3)])
+                                  (396, "band", 35, 3),
+                                  # block-diagonal (no operation in any step) and two connected components
+                                  (12, "band", 0), (20, "band", 0), (25, "band", 0), (30, "band", 0),
+                                  (61, "band", 0), (100, "band", 0), (100, "band", 0, 2), (40, "split", 3),
+                                  (41, "split", 2, 1)])
 def test_debug_selinv_matches_the_inverse(api, args):
     mf, pat, param = args[:3]
     depth = args[3] if len(args) > 3 else -1
@@ -143,6 +148,9 @@ def test_debug_selinv_matches_the_inverse(api, args):
                 worst = max(worst, np.linalg.norm(z - B(Sinv, a, c)) / np.sqrt(dn[a] * dn[c]))
     assert worst < 1e-10, (info, worst)
     assert not np.triu(Z, 6).any()
+    if pat == "band" and param == 0:  # block-diagonal: no tile off the diagonal, one task per block
+        assert info["tiles"] == info["blocks"] and info["selinv_tasks"] == info["blocks"], info
+    print(f"{args}: {info}, worst block error {worst:.2g}")
 
 
 @gpu

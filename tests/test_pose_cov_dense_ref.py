@@ -85,6 +85,27 @@ def test_statistics():
     assert ref["valid"] and 1e-12 <= ref["min_pivot"] <= 1.0
 
 
+def test_points_with_non_finite_residuals_are_left_out():
+    """x_depth0 of tests/pose_edge_cases.py at R0: its last point has depth 0, e = inf and weight 0.  The
+    covariance is the one of the other 128 points alone (0 * inf must not make H NaN), and e stays inf.  A NaN
+    residual (a point at the camera centre) likewise has a NaN weight and is left out."""
+    import pose_edge_cases as pc
+    K, R0, t0, Ms, ms, tau, _, _ = pc.case_inputs(pc.row("x_depth0"))
+    ref = cd.cov_stage(K, R0, t0, Ms, ms, tau, 1.0)
+    rest = cd.cov_stage(K, R0, t0, Ms[:-1], ms[:-1], tau, 1.0)
+    assert np.isinf(ref["e"][-1]) and ref["w"][-1] == 0 and np.isfinite(ref["e"][:-1]).all()
+    assert rest["valid"] and ref["valid"]
+    assert np.array_equal(ref["H"], rest["H"]) and np.array_equal(ref["cov"], rest["cov"])
+    assert ref["dof"] == rest["dof"] and ref["sigma2_hat"] == rest["sigma2_hat"]
+    assert cd.residual_error(ref["e"], rest["e"].tolist() + [np.inf]) == 0.0
+    assert cd.residual_error(ref["e"], rest["e"].tolist() + [np.nan]) == np.inf
+    Mn = Ms.copy()
+    Mn[-1] = -R0.T @ t0  # the camera centre: 0 / 0
+    with np.errstate(invalid="ignore", divide="ignore"):
+        nan = cd.cov_stage(K, R0, t0, Mn, ms, tau, 1.0)
+    assert np.isnan(nan["e"][-1]) and np.array_equal(nan["cov"], rest["cov"])
+
+
 def test_singular_cameras():
     K, R, t, Ms, ms = _case(9, 40)
     two = cd.cov_stage(K, R, t, Ms[:2], ms[:2], TAU, 1.0)
