@@ -88,6 +88,7 @@ def _load():
     L.cosl_ba_solve.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp]
     L.cosl_ba_solve_multi.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), ci, vp, vp]
     L.cosl_sba_motstr_levmar_x.argtypes = [ci] * 4 + [vp, vp, ci, ci, vp, ci, vp, ci, ci, vp, vp, ci]
+    L.cosl_sba_motstr_levmar_x_cov.argtypes = [ci] * 4 + [vp, vp, ci, ci, vp, vp, ci, vp, ci, ci, vp, vp, ci]
     L.cosl_nccl_unique_id.argtypes = [vp]
     L.cosl_ba_comm_create.argtypes = [vp, ci, ci, ci, C.POINTER(vp)]
     L.cosl_ba_comm_destroy.argtypes = [vp]
@@ -104,6 +105,7 @@ def _load():
     L.cosl_ba_solver_progress.argtypes = [vp, C.POINTER(cd)]
     L.cosl_ba_solver_set_covariance.argtypes = [vp, cd]
     L.cosl_ba_solver_download_covariance.argtypes = [vp, vp, vp, C.POINTER(cd)]
+    L.cosl_ba_solver_set_obs_cov.argtypes = [vp, vp]
     L.cosl_ba_solver_download.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_destroy.argtypes = [vp]
     L.cosl_ba_solver_stream.argtypes = [vp]
@@ -634,6 +636,35 @@ def ba_solve_multi(prob, opt, n_gpus, devices=None):
     return info
 
 
+def _obs_cov(covx, nobs):
+    """covx as the C-ABI's contiguous [nobs][4] float64 array (None stays None)"""
+    if covx is None:
+        return None
+    c = np.ascontiguousarray(covx, np.float64).reshape(-1, 4)
+    if len(c) != nobs:
+        raise ValueError(f"covx has {len(c)} covariances for {nobs} observations")
+    return c
+
+
+def sba_motstr_levmar_x(p, rot0, vmask, x, itmax, opts, n_con=0, m_con=0, covx=None, verbose=0, device=0):
+    """cosl_sba_motstr_levmar_x (cnp = 11, pnp = 3, mnp = 2), or cosl_sba_motstr_levmar_x_cov with covx [nobs, 2, 2]
+    (px^2) in x's point-major order.  p [11 m + 3 n] is updated in place; returns (iterations, info [10])."""
+    vmask = np.ascontiguousarray(vmask, np.int8)
+    n, m = vmask.shape
+    assert p.dtype == np.float64 and p.flags.c_contiguous and p.size == 11 * m + 3 * n
+    x = np.ascontiguousarray(x, np.float64)
+    rot0 = np.ascontiguousarray(rot0, np.float64)
+    opts = np.ascontiguousarray(opts, np.float64)
+    c = _obs_cov(covx, int(np.count_nonzero(vmask)))
+    info = np.zeros(10)
+    rc = LIB.cosl_sba_motstr_levmar_x_cov(n, int(n_con), m, int(m_con), _ptr(vmask), _ptr(p), 11, 3, _ptr(x), _ptr(c),
+                                          2, _ptr(rot0), int(itmax), int(verbose), _ptr(opts), _ptr(info),
+                                          int(device))
+    if rc < 0:
+        _ck(rc)
+    return rc, info
+
+
 PLAN_INFO_KEYS = ("blocks", "tiles_schur", "tiles", "tasks", "nd_depth", "critical_tasks", "grid",
                   "small_solve")
 
@@ -855,6 +886,13 @@ class BaSolver(_SolverHandle):
         """cosl_ba_solver_set_covariance: pixel_var > 0 makes every later run() and submit() end with the
         covariance stage; 0 turns it off."""
         _ck(LIB.cosl_ba_solver_set_covariance(self.h, float(pixel_var)))
+
+    def set_obs_cov(self, covx):
+        """cosl_ba_solver_set_obs_cov: covx [nobs, 2, 2] (px^2, in the order of the problem's xy) weights every
+        observation by its inverse covariance in every later run / run_fixed / submit; None clears.  load() clears
+        it, reset() keeps it."""
+        c = _obs_cov(covx, int(self.prob.nobs))
+        _ck(LIB.cosl_ba_solver_set_obs_cov(self.h, _ptr(c)))
 
     def download_covariance(self):
         """cosl_ba_solver_download_covariance: (camCov [m, 6, 6] for (w, t), ptCov [n, 3, 3], info dict) of the

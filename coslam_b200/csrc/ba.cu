@@ -300,6 +300,10 @@ struct cosl_ba_solver {
   double *d_covT = nullptr, *d_covCam = nullptr, *d_covPt = nullptr, *d_covSc = nullptr;
   unsigned char *d_covUnc = nullptr, *d_covIdx = nullptr;
   int* d_covCnt = nullptr;
+  // measurement covariances (cosl_ba_solver_set_obs_cov, DESIGN.md 4.7): d.obsL is d_obsL while they are set and
+  // nullptr otherwise; the kernels that read it are launched as their OBSCOV instantiations then
+  double* d_obsL = nullptr;
+  const double* graphObsL = nullptr;  // d.obsL the submitted graph was built with
 };
 
 namespace {
@@ -603,6 +607,48 @@ int check_problem(const cosl_ba_problem* prob, const char* what) {
   return check_observations(prob);
 }
 
+// Measurement covariances covx[N][2][2] (px^2, row-major): finite, symmetric to 1e-12 relative and positive
+// definite.  On success L[N][3] holds (s00, s01, s11) for ba_obscov_factor; otherwise the first bad observation is
+// named.
+int check_obs_cov(const double* covx, long long N, std::vector<double>& L, const char* what) {
+  L.resize(3 * (size_t)N);
+  for (long long o = 0; o < N; ++o) {
+    const double* c = covx + 4 * (size_t)o;
+    const double a = c[0], b = c[1], b2 = c[2], d = c[3];
+    if (!std::isfinite(a) || !std::isfinite(b) || !std::isfinite(b2) || !std::isfinite(d))
+      return set_error(COSL_E_INVALID, "%s: covariance of observation %lld is not finite", what, o);
+    if (std::fabs(b - b2) > 1e-12 * std::max(std::fabs(a), std::fabs(d)))
+      return set_error(COSL_E_INVALID, "%s: covariance of observation %lld is not symmetric (%.17g, %.17g)", what, o,
+                       b, b2);
+    const double s01 = 0.5 * (b + b2), det = a * d - s01 * s01;
+    if (!(a > 0.0) || !(d > 0.0) || !(det > 0.0) || !std::isfinite(d / det))
+      return set_error(COSL_E_INVALID, "%s: covariance of observation %lld is not positive definite", what, o);
+    L[3 * (size_t)o] = a;
+    L[3 * (size_t)o + 1] = s01;
+    L[3 * (size_t)o + 2] = d;
+  }
+  return COSL_OK;
+}
+
+// Sets (covx != NULL, checked by check_obs_cov into L) or clears the measurement covariances of the loaded problem:
+// the upload and the factorisation are enqueued on the solver's stream, nothing is waited for.
+int set_obs_cov(cosl_ba_solver* s, const std::vector<double>* L) {
+  if (!L) {
+    s->d.obsL = nullptr;
+    return COSL_OK;
+  }
+  COSL_TRY(grow(s, &s->d_obsL, 3 * (size_t)s->N));
+  // from pageable memory: the call returns once the source has been staged
+  if (s->N) {
+    COSL_CUDA(cudaMemcpyAsync(s->d_obsL, L->data(), sizeof(double) * 3 * (size_t)s->N, cudaMemcpyHostToDevice,
+                              s->rq.stream));
+    COSL_LAUNCH(ba_obscov_factor, (unsigned)div_up64(s->N, 256), 256, 0, s->rq.stream, s->d_obsL, s->N);
+    COSL_CUDA(cudaGetLastError());
+  }
+  s->d.obsL = s->d_obsL;
+  return COSL_OK;
+}
+
 // What the host derives from the observation lists (validated by check_problem) to plan a problem
 // without a device round trip: the start of each free camera in the camera-major list and the start of
 // each camera-pair bucket (ja <= jb, row-major over mf x mf) in the Schur pair entries.
@@ -891,6 +937,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   d.pt = s->d_pt;
   d.xy = s->d_xy;
   d.wgt = s->d_wgt;
+  d.obsL = nullptr;  // a new problem has new observations: its covariances are unset
   d.ptr = s->d_ptr;
   d.cobs = s->d_cobs;
   d.ccam = s->d_ccam;
@@ -1066,6 +1113,28 @@ int read_sc(cosl_ba_solver* s) {
   return COSL_OK;
 }
 
+// sum w |e|^2 (w |L e|^2 with measurement covariances) at (pa, pb) into d.sc[SC_COST]
+int launch_cost(const BaDev& d, const double* pa, const double* pb, unsigned gN, cudaStream_t st) {
+  if (d.obsL)
+    COSL_LAUNCH(ba_residual_kernel<true>, gN, 256, 0, st, d, pa, pb, 0, 0.0, nullptr);
+  else
+    COSL_LAUNCH(ba_residual_kernel<false>, gN, 256, 0, st, d, pa, pb, 0, 0.0, nullptr);
+  return COSL_OK;
+}
+
+// the two linearisation kernels at (d_pa, d_pb) into d's V, eb, W, U, ea (zeroed before)
+int launch_linearize(const cosl_ba_solver* s, const BaDev& d, cudaStream_t st) {
+  const unsigned gN = (unsigned)div_up64(s->N, 256), gC = (unsigned)div_up64(s->Nc, 128);
+  if (d.obsL) {
+    if (s->N) COSL_LAUNCH(ba_linearize_points<true>, gN, 256, 0, st, d, s->d_pa, s->d_pb);
+    if (s->Nc) COSL_LAUNCH(ba_linearize_cams<true>, gC, 128, 0, st, d, s->d_pa, s->d_pb);
+  } else {
+    if (s->N) COSL_LAUNCH(ba_linearize_points<false>, gN, 256, 0, st, d, s->d_pa, s->d_pb);
+    if (s->Nc) COSL_LAUNCH(ba_linearize_cams<false>, gC, 128, 0, st, d, s->d_pa, s->d_pb);
+  }
+  return COSL_OK;
+}
+
 // The kernels of one stage of the robust loop, enqueued on st (the solver's stream, or the capture of the
 // submitted graph), with the stage's multi-rank all-reduces.  dctl: the control block of the submitted loop,
 // from which the trial kernels read mu (and the prep kernel doStats) when they run; without it they take mu
@@ -1074,23 +1143,23 @@ int read_sc(cosl_ba_solver* s) {
 int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dctl, double mu, int doStats) {
   const unsigned gN = (unsigned)div_up64(s->N, 256);
   const int r0 = rank_of(s) == 0 ? 1 : 0;
+  const bool oc = s->d.obsL != nullptr;
   SectionTimer& T = s->timer;
-  if (stage == BA_STAGE_ROUND) {  // the round's Tukey weights, then its initial cost
+  if (stage == BA_STAGE_ROUND) {  // the round's Tukey weights (on the pixel distance), then its initial cost
     if (s->N) {
       if (s->opt.max_err > 0)
-        COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+        COSL_LAUNCH(ba_residual_kernel<false>, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
       else
         COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_wgt, s->N, 1.0);
     }
     T.begin(s->secCost, st);
-    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 0, 0.0, nullptr);
+    if (s->N) COSL_TRY(launch_cost(s->d, s->d_pa, s->d_pb, gN, st));
     T.end(st);
   } else if (stage == BA_STAGE_LIN0 || stage == BA_STAGE_LIN) {  // Jacobians, U, V, W, ea, eb at (pa, pb)
     const long long nV = 9LL * s->n + 27LL * s->m;  // [V | eb | U | ea]
     T.begin(s->secLin, st);
     COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, st, s->d_V, nV, 0.0);
-    if (s->N) COSL_LAUNCH(ba_linearize_points, gN, 256, 0, st, s->d, s->d_pa, s->d_pb);
-    if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, st, s->d, s->d_pa, s->d_pb);
+    COSL_TRY(launch_linearize(s, s->d, st));
     T.end(st);
     COSL_TRY(allreduce(s, s->d_Uea, (size_t)27 * s->m, ncclSum));
     // at itno > 0 the prep kernel of the next trial computes the statistics, unless there is none
@@ -1126,9 +1195,14 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
                 r0, nCamBlocks, s->d_dpb);
     T.end(st);
     T.begin(s->secCost, st);
-    if (s->N + s->n)  // a problem without points never reaches a trial (|g| = 0 stops it), but is captured
-      COSL_LAUNCH(ba_finish_cost, (unsigned)div_up64(s->N + (long long)s->n, 256), 256, 0, st, s->d, dctl, s->d_na,
-                  s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu);
+    if (s->N + s->n) {  // a problem without points never reaches a trial (|g| = 0 stops it), but is captured
+      const unsigned gF = (unsigned)div_up64(s->N + (long long)s->n, 256);
+      if (oc)
+        COSL_LAUNCH(ba_finish_cost<true>, gF, 256, 0, st, s->d, dctl, s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu);
+      else
+        COSL_LAUNCH(ba_finish_cost<false>, gF, 256, 0, st, s->d, dctl, s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv,
+                    mu);
+    }
     T.end(st);
   } else {  // a trial without free cameras
     T.begin(s->secBack, st);
@@ -1142,7 +1216,7 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
                   mu);
     T.end(st);
     T.begin(s->secCost, st);
-    if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, s->d, s->d_na, s->d_nb, 0, 0.0, nullptr);
+    if (s->N) COSL_TRY(launch_cost(s->d, s->d_na, s->d_nb, gN, st));
     T.end(st);
   }
   if (stage == BA_STAGE_ROUND || stage == BA_STAGE_TRIAL) COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
@@ -1155,7 +1229,7 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
 int enqueue_outliers(cosl_ba_solver* s, cudaStream_t st) {
   if (s->opt.max_err > 0) {
     if (s->N)
-      COSL_LAUNCH(ba_residual_kernel, (unsigned)div_up64(s->N, 256), 256, 0, st, s->d, s->d_pa, s->d_pb, 2,
+      COSL_LAUNCH(ba_residual_kernel<false>, (unsigned)div_up64(s->N, 256), 256, 0, st, s->d, s->d_pa, s->d_pb, 2,
                   s->opt.max_err, s->d_outlier);
     COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
   } else {
@@ -1332,21 +1406,20 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
               0, st, s->d_covSc, s->d_covT, 6LL * n, s->d_covCnt, nb);
   if (s->N) {
     if (s->opt.max_err > 0)
-      COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+      COSL_LAUNCH(ba_residual_kernel<false>, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
     else
       COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_covWgt, s->N, 1.0);
   }
   if (n) COSL_LAUNCH(ba_cov_mask, div_up(n, 256), 256, 0, st, cd, s->d_covUnc);
   const long long nV = 9LL * n + 27LL * m;
   COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, st, s->d_V, nV, 0.0);
-  if (s->N) COSL_LAUNCH(ba_linearize_points, gN, 256, 0, st, cd, s->d_pa, s->d_pb);
-  if (s->Nc) COSL_LAUNCH(ba_linearize_cams, (unsigned)div_up64(s->Nc, 128), 128, 0, st, cd, s->d_pa, s->d_pb);
+  COSL_TRY(launch_linearize(s, cd, st));
   // mu = 0: S and V^-1 of the undamped system (and the cleared scalars and task counters)
   const int nTilesInit = std::max(1, s->plan.nTiles);
   COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)n + m, 256), 256, 0, st, cd, nullptr, 0.0, 1,
               s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks, nTilesInit,
               s->d_Vinv, 0, nullptr, 0LL);
-  if (s->N) COSL_LAUNCH(ba_residual_kernel, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 0, 0.0, nullptr);
+  if (s->N) COSL_TRY(launch_cost(cd, s->d_pa, s->d_pb, gN, st));
   if (n) COSL_LAUNCH(ba_cov_vfix, div_up(n, 256), 256, 0, st, s->d_covUnc, s->d_Vinv, n);
   if (s->ns) {
     if (s->nItems)
@@ -1496,6 +1569,7 @@ int build_graph(cosl_ba_solver* s) {
   s->graphPb = s->d_pb;
   s->graphNb = s->d_nb;
   s->graphCovVar = s->covVar;
+  s->graphObsL = s->d.obsL;
   return COSL_OK;
 }
 
@@ -1652,7 +1726,7 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
   COSL_TRY(s->rq.idle("cosl_ba_solver_submit"));
   // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
   if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
-      s->graphNb != s->d_nb || s->graphCovVar != s->covVar)
+      s->graphNb != s->d_nb || s->graphCovVar != s->covVar || s->graphObsL != s->d.obsL)
     COSL_TRY(build_graph(s));
   // the request number goes to the device ahead of the graph, on the solver's stream: a stop made before the
   // graph starts names it too (the pinned source is not rewritten before this request is collected)
@@ -1770,6 +1844,17 @@ int cosl_ba_solver_set_covariance(cosl_ba_solver* s, double pixel_var) {
   if (pixel_var > 0 && !s->covReady) COSL_TRY(cov_prepare(s));
   s->covVar = pixel_var;
   return COSL_OK;
+}
+
+int cosl_ba_solver_set_obs_cov(cosl_ba_solver* s, const double* covx) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_set_obs_cov: a multi-rank solver has no measurement covariances");
+  COSL_TRY(s->rq.idle("cosl_ba_solver_set_obs_cov"));
+  if (!covx) return set_obs_cov(s, nullptr);
+  std::vector<double> L;
+  COSL_TRY(check_obs_cov(covx, s->N, L, "cosl_ba_solver_set_obs_cov"));
+  return set_obs_cov(s, &L);
 }
 
 int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double* ptCov, double out[8]) {
@@ -2137,13 +2222,18 @@ const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* ca
   return s->timer.names[idx];
 }
 
-int cosl_ba_solve(cosl_ba_problem* prob, const cosl_ba_options* opt,
-                  double info[COSL_BA_INFOSZ]) {
+}  // extern "C"
+
+namespace {
+// cosl_ba_solve, with the measurement covariances L (check_obs_cov's output) when it is given
+int solve_once(cosl_ba_problem* prob, const cosl_ba_options* opt, const std::vector<double>* L,
+               double info[COSL_BA_INFOSZ]) {
   cosl_ba_solver* s = nullptr;
   const double t0 = now_s();
   COSL_TRY(cosl_ba_solver_create(prob, opt, nullptr, &s));
   const double t1 = now_s();
-  int rc = run_host(s, 0, info);
+  int rc = L ? set_obs_cov(s, L) : COSL_OK;
+  if (rc == COSL_OK) rc = run_host(s, 0, info);
   const double t2 = now_s();
   if (rc == COSL_OK) rc = download(s, prob);
   const double t3 = now_s();
@@ -2157,6 +2247,13 @@ int cosl_ba_solve(cosl_ba_problem* prob, const cosl_ba_options* opt,
     std::fprintf(stderr, "[ba timing] cosl_ba_solve: create %.1f  run %.1f  download %.1f  destroy %.1f ms\n",
                  1e3 * (t1 - t0), 1e3 * (t2 - t1), 1e3 * (t3 - t2), 1e3 * (now_s() - t3));
   return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int cosl_ba_solve(cosl_ba_problem* prob, const cosl_ba_options* opt, double info[COSL_BA_INFOSZ]) {
+  return solve_once(prob, opt, nullptr, info);
 }
 
 // Single-process multi-GPU drop-in (SURVEY.md 8b: the reference's BA pthread is ONE process,
@@ -2252,6 +2349,14 @@ int cosl_sba_motstr_levmar_x(int n, int ncon, int m, int mcon, const char* vmask
                              int cnp, int pnp, const double* x, int mnp,
                              const double* rot0params, int itmax, int verbose,
                              const double opts[5], double info[10], int device) {
+  return cosl_sba_motstr_levmar_x_cov(n, ncon, m, mcon, vmask, p, cnp, pnp, x, nullptr, mnp, rot0params, itmax,
+                                      verbose, opts, info, device);
+}
+
+int cosl_sba_motstr_levmar_x_cov(int n, int ncon, int m, int mcon, const char* vmask, double* p,
+                                 int cnp, int pnp, const double* x, const double* covx, int mnp,
+                                 const double* rot0params, int itmax, int verbose,
+                                 const double opts[5], double info[10], int device) {
   if (cnp != 11 || pnp != 3 || mnp != 2 || !vmask || !p || !x || !rot0params || !opts)
     return set_error(COSL_E_INVALID, "cosl_sba_motstr_levmar_x: only cnp=11, pnp=3, mnp=2");
   std::vector<double> K((size_t)m * 9, 0.0), R((size_t)m * 9), t((size_t)m * 3), X((size_t)n * 3);
@@ -2293,6 +2398,9 @@ int cosl_sba_motstr_levmar_x(int n, int ncon, int m, int mcon, const char* vmask
   pr.ptr = ptr.data();
   pr.cam = cam.data();
   pr.xy = x;
+  // covx follows x: sba's point-major measurement order, which is the order of cam above
+  std::vector<double> L;
+  if (covx) COSL_TRY(check_obs_cov(covx, pr.nobs, L, "cosl_sba_motstr_levmar_x_cov"));
   cosl_ba_options o;
   cosl_ba_options_default(&o);
   o.max_err = 0;
@@ -2302,7 +2410,7 @@ int cosl_sba_motstr_levmar_x(int n, int ncon, int m, int mcon, const char* vmask
   o.verbose = verbose;
   o.device = device;
   double inf[COSL_BA_INFOSZ];
-  COSL_TRY(cosl_ba_solve(&pr, &o, inf));
+  COSL_TRY(solve_once(&pr, &o, covx ? &L : nullptr, inf));
   if (info)
     for (int k = 0; k < 10; ++k) info[k] = inf[k];
   for (int j = mcon; j < m; ++j) {

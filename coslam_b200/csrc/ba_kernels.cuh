@@ -5,7 +5,8 @@
 // Data layout in HBM (per solver / per rank):
 //   cameras (replicated): camK[m][5] (K0,K1,K2,K4,K5), camR0[m][9] (rotation of q0), pa[m][6] (v,t)
 //   points  (this rank's shard): pb[n][3]
-//   observations, point-major CSR: cam[N], pt[N], xy[N][2], wgt[N]
+//   observations, point-major CSR: cam[N], pt[N], xy[N][2], wgt[N]; with measurement covariances set
+//   (cosl_ba_solver_set_obs_cov), obsL[N][3]: the whitening factor L of each observation (DESIGN.md 4.7)
 //   camera-major permutation of the free-camera observations: cobs[Nc], ccam[Nc]
 //   W[N][18]   W_ij = A_ij^T B_ij (6x3 row-major) of the current linearisation
 //   V[n][6], eb[n][3], U[m][21] (packed upper), ea[m][6]
@@ -34,6 +35,7 @@ struct BaDev {
   const int* pt;
   const double* xy;
   double* wgt;
+  const double* obsL;  // [N][3] (l00, l01, l11) with L^T L = Sigma^-1; read by the OBSCOV instantiations only
   const long long* ptr;
   const int* cobs;
   const int* ccam;
@@ -167,11 +169,42 @@ __device__ __forceinline__ double tukey_w(double e, double s) {
   return e * e;
 }
 
+// Measurement covariances (DESIGN.md 4.7).  The kernels that form residuals and Jacobians take a template flag
+// OBSCOV: with it they multiply the residual (and the Jacobian rows) of observation o by its upper-triangular L,
+// L^T L = Sigma_o^-1, so that |L e|^2 = e^T Sigma^-1 e.  Without it they are the unweighted kernels, unchanged.
+template <int NC>
+__device__ __forceinline__ void ba_whiten(const double* __restrict__ L, double* r0, double* r1) {
+  const double l00 = L[0], l01 = L[1], l11 = L[2];
+#pragma unroll
+  for (int k = 0; k < NC; ++k) {
+    const double a = r0[k], b = r1[k];
+    r0[k] = l00 * a + l01 * b;
+    r1[k] = l11 * b;
+  }
+}
+
+// In place, one observation per thread: (s00, s01, s11) of Sigma -> (l00, l01, l11) of the upper-triangular L with
+// L^T L = Sigma^-1.  Sigma^-1 = [s11 -s01; -s01 s00] / det, so l00 = sqrt(s11 / det), l01 = -s01 / sqrt(s11 det),
+// l11 = 1 / sqrt(s11): Sigma = I gives L = I and Sigma = s^2 I gives L = I / s exactly.  The host checked that
+// every Sigma is positive definite.
+__global__ void __launch_bounds__(256) ba_obscov_factor(double* __restrict__ L, long long N) {
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= N) return;
+  double* q = L + 3 * (size_t)o;
+  const double a = q[0], b = q[1], c = q[2];
+  const double det = a * c - b * b;
+  q[0] = sqrt(c / det);
+  q[1] = -b / sqrt(c * det);
+  q[2] = 1.0 / sqrt(c);
+}
+
 // ------------------------------------------------------------------------------------------
 // cost / weights / outliers: one observation per thread
 // mode 0: sc[SC_COST] += w |e|^2 ; mode 1: wgt = tukey(|e|, maxErr) ; mode 2: outlier = |e|>=maxErr,
-// sc[SC_COST] += number of outliers
+// sc[SC_COST] += number of outliers.  OBSCOV: mode 0 sums w |L e|^2; modes 1 and 2 stay on the pixel distance |e|
+// (they are launched without it).
 // ------------------------------------------------------------------------------------------
+template <bool OBSCOV>
 __global__ void __launch_bounds__(256)
 ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb, int mode,
                    double maxErr, unsigned char* __restrict__ outlier) {
@@ -183,7 +216,8 @@ ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restr
     const double X[3] = {pb[3 * (size_t)i], pb[3 * (size_t)i + 1], pb[3 * (size_t)i + 2]};
     double h[2];
     ba_project<false, false>(d.camK + 5 * j, d.camR0 + 9 * j, pa + 6 * j, X, h, nullptr, nullptr);
-    const double dx = d.xy[2 * o] - h[0], dy = d.xy[2 * o + 1] - h[1];
+    double dx = d.xy[2 * o] - h[0], dy = d.xy[2 * o + 1] - h[1];
+    if (OBSCOV && mode == 0) ba_whiten<1>(d.obsL + 3 * (size_t)o, &dx, &dy);
     const double e2 = dx * dx + dy * dy;
     if (mode == 0) {
       c = d.wgt[o] * e2;
@@ -211,9 +245,10 @@ ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restr
 }
 
 // ------------------------------------------------------------------------------------------
-// Linearisation, point-major: per observation e, A (2x6), B (2x3) (scaled by sqrt(w)); stores
-// W_ij = A^T B; collapses V_i = sum B^T B and eb_i = sum B^T e per point with segmented shuffles.
+// Linearisation, point-major: per observation e, A (2x6), B (2x3) (whitened by L with OBSCOV, scaled by
+// sqrt(w)); stores W_ij = A^T B; collapses V_i = sum B^T B and eb_i = sum B^T e per point with segmented shuffles.
 // ------------------------------------------------------------------------------------------
+template <bool OBSCOV>
 __global__ void __launch_bounds__(256, 2)
 ba_linearize_points(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb) {
   if (blockIdx.x == 0 && threadIdx.x < 2) d.sc[SC_GINF + threadIdx.x] = 0.0;  // |g|_inf, max diag: set by ba_stats_kernel
@@ -229,8 +264,15 @@ ba_linearize_points(BaDev d, const double* __restrict__ pa, const double* __rest
     const double X[3] = {pb[3 * (size_t)i], pb[3 * (size_t)i + 1], pb[3 * (size_t)i + 2]};
     double h[2], A[12], B[6];
     ba_project<true, true>(d.camK + 5 * j, d.camR0 + 9 * j, pa + 6 * j, X, h, A, B);
+    double r0 = d.xy[2 * o] - h[0], r1 = d.xy[2 * o + 1] - h[1];
+    if (OBSCOV) {
+      const double* L = d.obsL + 3 * (size_t)o;
+      ba_whiten<1>(L, &r0, &r1);
+      ba_whiten<3>(L, B, B + 3);
+      ba_whiten<6>(L, A, A + 6);
+    }
     const double sw = sqrt(d.wgt[o]);
-    const double e0 = (d.xy[2 * o] - h[0]) * sw, e1 = (d.xy[2 * o + 1] - h[1]) * sw;
+    const double e0 = r0 * sw, e1 = r1 * sw;
 #pragma unroll
     for (int k = 0; k < 6; ++k) B[k] *= sw;
     if (i >= d.ncon) {
@@ -266,7 +308,8 @@ ba_linearize_points(BaDev d, const double* __restrict__ pa, const double* __rest
 }
 
 // Linearisation, camera-major over the free-camera observations: U_j = sum A^T A (packed upper,
-// 21) and ea_j = sum A^T e (6), collapsed per camera with segmented shuffles.
+// 21) and ea_j = sum A^T e (6), collapsed per camera with segmented shuffles.  OBSCOV: A and e whitened by L.
+template <bool OBSCOV>
 __global__ void __launch_bounds__(128)
 ba_linearize_cams(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb) {
   const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -281,8 +324,14 @@ ba_linearize_cams(BaDev d, const double* __restrict__ pa, const double* __restri
     const double X[3] = {pb[3 * (size_t)i], pb[3 * (size_t)i + 1], pb[3 * (size_t)i + 2]};
     double h[2], A[12];
     ba_project<true, false>(d.camK + 5 * j, d.camR0 + 9 * j, pa + 6 * j, X, h, A, nullptr);
+    double r0 = d.xy[2 * (size_t)o] - h[0], r1 = d.xy[2 * (size_t)o + 1] - h[1];
+    if (OBSCOV) {
+      const double* L = d.obsL + 3 * (size_t)o;
+      ba_whiten<1>(L, &r0, &r1);
+      ba_whiten<6>(L, A, A + 6);
+    }
     const double sw = sqrt(d.wgt[o]);
-    const double e0 = (d.xy[2 * (size_t)o] - h[0]) * sw, e1 = (d.xy[2 * (size_t)o + 1] - h[1]) * sw;
+    const double e0 = r0 * sw, e1 = r1 * sw;
 #pragma unroll
     for (int k = 0; k < 12; ++k) A[k] *= sw;
     int t = 0;
@@ -819,8 +868,8 @@ ba_cam_update(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__
 //    reading da straight from the solution vector;
 //  ba_finish_cost: one observation per thread: db_i = V*_i^-1 (e_b,i - t_i) recomputed from the point's
 //    accumulator (read-only here; the FIRST observation of a point stores nb_i = pb_i + db_i and adds the
-//    point-side sums), then the weighted squared residual at (na, nb_i) -> cost.  Extra threads finish the
-//    points that have no observation.
+//    point-side sums), then the weighted squared residual at (na, nb_i) -> cost (whitened with OBSCOV).  Extra
+//    threads finish the points that have no observation.
 // Both take mu from ctl, the control block of the submitted loop, when it is set.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -880,6 +929,7 @@ ba_back_cams_points(BaDev d, const BaCtl* __restrict__ ctl, const double* __rest
   }
 }
 
+template <bool OBSCOV>
 __global__ void __launch_bounds__(256)
 ba_finish_cost(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__ na, const double* __restrict__ pb,
                double* __restrict__ nb, const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu) {
@@ -929,7 +979,8 @@ ba_finish_cost(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict_
       const int j = d.cam[o];
       double h[2];
       ba_project<false, false>(d.camK + 5 * j, d.camR0 + 9 * j, na + 6 * j, x, h, nullptr, nullptr);
-      const double dx = d.xy[2 * o] - h[0], dy = d.xy[2 * o + 1] - h[1];
+      double dx = d.xy[2 * o] - h[0], dy = d.xy[2 * o + 1] - h[1];
+      if (OBSCOV) ba_whiten<1>(d.obsL + 3 * (size_t)o, &dx, &dy);
       c = d.wgt[o] * (dx * dx + dy * dy);
     }
   }

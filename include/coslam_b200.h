@@ -475,6 +475,15 @@ int cosl_sba_motstr_levmar_x(int n, int ncon, int m, int mcon, const char* vmask
                              int cnp, int pnp, const double* x, int mnp,
                              const double* rot0params, int itmax, int verbose,
                              const double opts[5], double info[10], int device);
+/* The same with sba's covx (an extension of this C-ABI, which had dropped it): covx[k] is the 2x2 covariance
+ * (px^2, row-major) of measurement k of x, in x's point-major order; NULL is cosl_sba_motstr_levmar_x.  The
+ * least-squares term of measurement k becomes e_k^T covx[k]^-1 e_k, and info[0], info[1] are those sums.  Every
+ * covx[k] must be finite, symmetric and positive definite: otherwise COSL_E_INVALID names the first bad one
+ * (checked before any device work).  mnp must be 2. */
+int cosl_sba_motstr_levmar_x_cov(int n, int ncon, int m, int mcon, const char* vmask, double* p,
+                                 int cnp, int pnp, const double* x, const double* covx, int mnp,
+                                 const double* rot0params, int itmax, int verbose,
+                                 const double opts[5], double info[10], int device);
 
 /* ---- multi-GPU (points sharded across ranks, cameras replicated; one NCCL all-reduce of the
  * packed reduced camera system per LM trial + one small all-reduce of scalars). ---- */
@@ -569,6 +578,18 @@ int cosl_ba_solver_set_covariance(cosl_ba_solver* s, double pixel_var);
  * break-down or a relative pivot below 1e-12 (e.g. no fixed camera and too few fixed points, or a free
  * camera without an observation of non-zero weight).  The BA itself still returned COSL_OK. */
 int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double* ptCov, double out[8]);
+/* Measurement covariances of the loaded problem (an extension: sba's covx, DESIGN.md 4.7).  covx[nobs][4]: the
+ * 2x2 covariance of each observation in px^2, row-major, in the order of the problem's xy.  The least-squares
+ * term of observation k becomes w_k e_k^T covx[k]^-1 e_k: the kernels whiten residual and Jacobian rows by L_k with
+ * L_k^T L_k = covx[k]^-1.  The Tukey weights w and the outlier flags stay on the pixel distance |e_k| against
+ * max_err.  The costs in info (initial, final, weighted) and the covariance stage's sigma2_hat are whitened; the
+ * stage returns pixel_var (J^T W Lambda J)^-1, so with covariances in px^2 pass pixel_var = 1.
+ * Validates on the calling thread (every entry finite, symmetric to 1e-12 relative, positive definite): otherwise
+ * COSL_E_INVALID names the first bad observation and the handle keeps what it had.  Copies covx (the caller may
+ * reuse it on return), enqueues the upload and the factorisation on the solver's stream and returns without
+ * waiting.  NULL clears.  The covariances apply to every later run, run_fixed and submit; reset keeps them, load
+ * clears them.  COSL_E_STATE while a submit is in flight; COSL_E_INVALID for a NULL handle or a multi-rank solver. */
+int cosl_ba_solver_set_obs_cov(cosl_ba_solver* s, const double* covx);
 /* Per-kernel accumulated device time in ms since create/reset, by name (NULL-terminated list via
  * index): returns name or NULL when idx is out of range. */
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls);
