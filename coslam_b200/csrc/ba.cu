@@ -29,15 +29,16 @@
 
 using namespace coslam;
 
-/* ---------------------------------------------------------------- the tile solve for other callers */
+/* ---------------------------------------------------------------- tile solve set-up and launch (tile_solve.h) */
 namespace coslam {
 
-int tile_task_order(const BaPlan& P, std::vector<BaTask>& order) {
+TileLaunch tile_launch_plan(const BaPlan& P) {
+  TileLaunch L;
+  std::vector<BaTask>& order = L.order;
   // two ticket lists (each keeps the critical-path-first order, hence stays topological)
-  order.clear();
   for (const BaTask& t : P.tasks)
     if (t.type == BA_T_POTRF || t.type == BA_T_BWD) order.push_back(t);
-  const int nA = (int)order.size();
+  L.nA = (int)order.size();
   for (const BaTask& t : P.tasks)
     if (!(t.type == BA_T_POTRF || t.type == BA_T_BWD)) order.push_back(t);
   // hot successors of every POTRF(k): TRSM(j, k) and the diagonal UPD(j, j, k) of j = first block
@@ -60,74 +61,134 @@ int tile_task_order(const BaPlan& P, std::vector<BaTask>& order) {
       k.l0 = firstTrsm[k.k];
       k.l1 = diagUpd[k.k];
     }
-  return nA;
+  // Systems of one or two blocks (local BA) are solved by one resident CTA: for the 72 x 72 system of
+  // the c3 local BA, ba_tile_two needs 26 us per LM trial and the task kernel 42 us (H100 80GB HBM3, 400 W).
+  if (P.nb >= 1 && P.nb <= 2) {
+    L.t00 = P.tileIdx[0];
+    L.t10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
+    L.t11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
+    L.two = L.t00 >= 0 && (P.nb == 1 || L.t11 >= 0);
+  }
+  return L;
 }
 
-int tile_solve_launch(const BaPlan& P, int nA, const TileSolveBufs& b, int device, cudaStream_t s, int* gridOut) {
-  if (gridOut) *gridOut = 0;
-  if (P.nb <= 0) return COSL_OK;
+int tile_launch_device(TileLaunch& L) {
+  static std::mutex mu;
+  static std::vector<int> smCount;  // per device, 0 until the attributes are set there
+  int device = 0, nsm = 0;
+  COSL_CUDA(cudaGetDevice(&device));
+  {
+    std::lock_guard<std::mutex> lk(mu);
+    if ((int)smCount.size() <= device) smCount.resize(device + 1, 0);
+    if (!smCount[device]) {
+      COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+      COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+      COSL_CUDA(cudaFuncSetAttribute(ba_selinv_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SEL2_SMEM));
+      COSL_CUDA(cudaFuncSetAttribute(ba_selinv_xinv, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SELX_SMEM));
+      COSL_CUDA(cudaFuncSetAttribute(ba_selinv_step, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SELS_SMEM));
+      int perSm = 0;
+      COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+      COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS, BA_TILE_SMEM));
+      if (perSm < 1) return set_error(COSL_E_CUDA, "tile solve: the kernel does not fit on a multiprocessor");
+      smCount[device] = std::max(1, nsm);
+    }
+    nsm = smCount[device];
+  }
+  // one CTA per multiprocessor, at most one per task plus one
+  L.grid = std::max(2, std::min(nsm, (int)L.order.size() + 1));
+  L.nSpecial = std::max(1, std::min(std::min(24, std::max(1, L.grid / 6)), L.grid - 1));
+  return COSL_OK;
+}
+
+TileImage tile_image(const BaPlan& P, const TileLaunch& L) {
+  TileImage I;
+  SlabLayout S;
+  auto put = [&](size_t bytes) { return S.take(std::max<size_t>(bytes, 1)); };
+  I.tasks = put(sizeof(BaTask) * L.order.size());
+  I.bwd = put(sizeof(BaBwdEntry) * P.bwdList.size());
+  I.sum = put(sizeof(BaSumEntry) * P.sumList.size());
+  I.blkRows = put(sizeof(int) * P.blkRows.size());
+  I.blkCam0 = put(sizeof(int) * P.blkCam0.size());
+  I.order = put(sizeof(int) * P.order.size());
+  I.diagBlk = put(sizeof(int) * std::max(1, P.nTiles));
+  I.diagTile = put(sizeof(int) * std::max(1, P.nb));
+  I.bytes = S.bytes;
+  return I;
+}
+
+void tile_image_write(const BaPlan& P, const TileLaunch& L, const TileImage& I, unsigned char* dst) {
+  std::vector<int> diagBlk(std::max(1, P.nTiles), -1), diagTile(std::max(1, P.nb), 0);
+  for (int k = 0; k < P.nb; ++k) {
+    diagTile[k] = P.tileIdx[(size_t)k * P.nb + k];
+    diagBlk[diagTile[k]] = k;
+  }
+  auto pack = [&](size_t off, const void* src, size_t bytes) {
+    if (bytes) std::memcpy(dst + off, src, bytes);
+  };
+  pack(I.tasks, L.order.data(), sizeof(BaTask) * L.order.size());
+  pack(I.bwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
+  pack(I.sum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
+  pack(I.blkRows, P.blkRows.data(), sizeof(int) * P.blkRows.size());
+  pack(I.blkCam0, P.blkCam0.data(), sizeof(int) * P.blkCam0.size());
+  pack(I.order, P.order.data(), sizeof(int) * P.order.size());
+  pack(I.diagBlk, diagBlk.data(), sizeof(int) * diagBlk.size());
+  pack(I.diagTile, diagTile.data(), sizeof(int) * diagTile.size());
+}
+
+TileLists tile_lists(const TileImage& I, const void* base) {
+  const unsigned char* b = static_cast<const unsigned char*>(base);
+  TileLists t;
+  t.tasks = reinterpret_cast<const BaTask*>(b + I.tasks);
+  t.bwd = reinterpret_cast<const BaBwdEntry*>(b + I.bwd);
+  t.sum = reinterpret_cast<const BaSumEntry*>(b + I.sum);
+  t.blkRows = reinterpret_cast<const int*>(b + I.blkRows);
+  t.blkCam0 = reinterpret_cast<const int*>(b + I.blkCam0);
+  t.order = reinterpret_cast<const int*>(b + I.order);
+  t.diagBlk = reinterpret_cast<const int*>(b + I.diagBlk);
+  t.diagTile = reinterpret_cast<const int*>(b + I.diagTile);
+  return t;
+}
+
+BaTileDev tile_dev(const BaPlan& P, const TileLaunch& L, const TileLists& lists) {
   BaTileDev td = {};
-  td.rhs = b.rhs;
-  td.tiles = b.tiles;
-  td.rhsS = b.rhsS;
-  td.Linv = b.Linv;
-  td.y = b.y;
-  td.x = b.x;
-  td.cnt = b.cnt;
-  td.tasks = b.tasks;
-  td.bwd = b.bwd;
-  td.sum = b.sum;
-  td.blkRows = b.blkRows;
-  td.nTasks = (int)P.tasks.size();
-  td.nA = nA;
+  td.tasks = lists.tasks;
+  td.bwd = lists.bwd;
+  td.sum = lists.sum;
+  td.blkRows = lists.blkRows;
+  td.nTasks = (int)L.order.size();
+  td.nA = L.nA;
   td.nb = P.nb;
   td.nTiles = P.nTiles;
   td.nCounters = P.nCounters;
+  td.nSpecial = L.nSpecial;
   td.xdoneBase = P.nTiles + P.nScratch;
-  td.sc = b.fail;
-  td.scFail = 0;
-  td.trace = nullptr;
-  const int t00 = P.tileIdx[0];
-  const int t10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
-  const int t11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
-  if (P.nb <= 2 && t00 >= 0 && (P.nb == 1 || t11 >= 0)) {
-    COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
-    COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s, td, t00, t10, t11);
-    if (gridOut) *gridOut = 1;
-  } else {
-    // same grid rule as the BA solver: never more CTAs than can be co-resident (the tickets spin)
-    COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
-    int nsm = 0, perSm = 0;
-    COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
-    COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS, BA_TILE_SMEM));
-    if (perSm < 1) return set_error(COSL_E_CUDA, "tile solve: the kernel does not fit on a multiprocessor");
-    const int grid = std::max(2, std::min(std::max(1, nsm), td.nTasks + 1));
-    td.nSpecial = std::max(1, std::min(std::min(24, std::max(1, grid / 6)), grid - 1));
-    COSL_LAUNCH(ba_tile_solve, grid, BA_NTHREADS, BA_TILE_SMEM, s, td);
-    if (gridOut) *gridOut = grid;
-  }
+  return td;
+}
+
+int tile_solve_enqueue(const TileLaunch& L, const BaTileDev& td, cudaStream_t s) {
+  if (L.two)
+    COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, s, td, L.t00, L.t10, L.t11);
+  else
+    COSL_LAUNCH(ba_tile_solve, L.grid, BA_NTHREADS, BA_TILE_SMEM, s, td);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
 
-// Z = S^-1 on the tile pattern of P (S in td.tiles; the dataflow factorisation leaves its factor there).
-// Systems of one or two blocks: one resident CTA (ba_selinv_two).  Otherwise the diagonal of S is kept for
-// the pivot test, ba_tile_solve factors (its substitutions run on whatever rhs holds), then X_k = L_kk^-T for
-// every block and one launch per step of the plan.  Pivot break-down lands in td.sc[td.scFail], the blocks'
-// minimum relative pivots in sd.piv.  sd.cnt must be zero.
-int selinv_launch(const BaPlan& P, const BaSelPlan& SP, const BaTileDev& td, int grid, const BaSelDev& sd,
+// Z = S^-1 on the tile pattern of the plan (S in td.tiles; the dataflow factorisation leaves its factor there).
+// Systems of one or two blocks: one resident CTA (ba_selinv_two).  Otherwise the diagonal of S is kept for the
+// pivot test, ba_tile_solve factors (its substitutions run on whatever rhs holds), then X_k = L_kk^-T for every
+// block and one launch per step of the plan.  Pivot break-down lands in td.sc[td.scFail], the blocks' minimum
+// relative pivots in sd.piv.  sd.cnt must be zero.
+int selinv_launch(const TileLaunch& L, const BaSelPlan& SP, const BaTileDev& td, const BaSelDev& sd,
                   cudaStream_t st) {
-  if (P.nb <= 0) return COSL_OK;
-  const int t00 = P.tileIdx[0];
-  const int t10 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 0] : -1;
-  const int t11 = P.nb == 2 ? P.tileIdx[(size_t)1 * P.nb + 1] : -1;
-  if (P.nb <= 2 && t00 >= 0 && (P.nb == 1 || t11 >= 0)) {
-    COSL_LAUNCH(ba_selinv_two, 1, BA_NTHREADS, BA_SEL2_SMEM, st, td.tiles, td.blkRows, t00, t10, t11, sd.Z, sd.piv,
-                td.sc + td.scFail);
+  if (td.nb <= 0) return COSL_OK;
+  if (L.two) {
+    COSL_LAUNCH(ba_selinv_two, 1, BA_NTHREADS, BA_SEL2_SMEM, st, td.tiles, td.blkRows, L.t00, L.t10, L.t11, sd.Z,
+                sd.piv, td.sc + td.scFail);
   } else {
-    COSL_LAUNCH(ba_cov_sdiag, P.nb, BA_TB, 0, st, td.tiles, sd.diagTile, sd.sdiag);
-    COSL_LAUNCH(ba_tile_solve, grid, BA_NTHREADS, BA_TILE_SMEM, st, td);
-    COSL_LAUNCH(ba_selinv_xinv, P.nb, BA_NTHREADS, BA_SELX_SMEM, st, sd);
+    COSL_LAUNCH(ba_cov_sdiag, td.nb, BA_TB, 0, st, td.tiles, sd.diagTile, sd.sdiag);
+    COSL_LAUNCH(ba_tile_solve, L.grid, BA_NTHREADS, BA_TILE_SMEM, st, td);
+    COSL_LAUNCH(ba_selinv_xinv, td.nb, BA_NTHREADS, BA_SELX_SMEM, st, sd);
     for (int q = 0; q + 1 < (int)SP.stepBegin.size(); ++q) {
       const int t0 = SP.stepBegin[q], nOff = SP.stepBegin[q + 1] - t0 - 1;
       COSL_LAUNCH(ba_selinv_step, std::max(1, nOff), BA_NTHREADS, BA_SELS_SMEM, st, sd, q, t0, nOff);
@@ -137,25 +198,13 @@ int selinv_launch(const BaPlan& P, const BaSelPlan& SP, const BaTileDev& td, int
   return COSL_OK;
 }
 
-int selinv_attributes() {
-  COSL_CUDA(cudaFuncSetAttribute(ba_selinv_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SEL2_SMEM));
-  COSL_CUDA(cudaFuncSetAttribute(ba_selinv_xinv, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SELX_SMEM));
-  COSL_CUDA(cudaFuncSetAttribute(ba_selinv_step, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_SELS_SMEM));
-  return COSL_OK;
-}
-
-// The device copy of a selected-inversion plan and the block -> diagonal tile map: [diagTile | tasks | ops]
-std::vector<unsigned char> selinv_index(const BaPlan& P, const BaSelPlan& SP, size_t* oTasks, size_t* oOps) {
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  const size_t nd = sizeof(int) * std::max(1, P.nb);
-  *oTasks = al(nd);
-  *oOps = *oTasks + al(sizeof(BaSelTask) * std::max<size_t>(1, SP.tasks.size()));
-  std::vector<unsigned char> h(*oOps + al(sizeof(BaSelOp) * std::max<size_t>(1, SP.ops.size())), 0);
-  for (int k = 0; k < P.nb; ++k) {
-    const int t = P.tileIdx[(size_t)k * P.nb + k];
-    std::memcpy(h.data() + sizeof(int) * k, &t, sizeof(int));
-  }
-  if (!SP.tasks.empty()) std::memcpy(h.data() + *oTasks, SP.tasks.data(), sizeof(BaSelTask) * SP.tasks.size());
+// The device copy of a selected-inversion plan: [tasks | ops]
+std::vector<unsigned char> selinv_index(const BaSelPlan& SP, size_t* oOps) {
+  SlabLayout S;
+  S.take(sizeof(BaSelTask) * std::max<size_t>(1, SP.tasks.size()));
+  *oOps = S.take(sizeof(BaSelOp) * std::max<size_t>(1, SP.ops.size()));
+  std::vector<unsigned char> h(S.bytes, 0);
+  if (!SP.tasks.empty()) std::memcpy(h.data(), SP.tasks.data(), sizeof(BaSelTask) * SP.tasks.size());
   if (!SP.ops.empty()) std::memcpy(h.data() + *oOps, SP.ops.data(), sizeof(BaSelOp) * SP.ops.size());
   return h;
 }
@@ -247,16 +296,12 @@ struct cosl_ba_solver {
   long long reduceCount = 0;  // doubles in the all-reduce payload
   double *d_Linv = nullptr, *d_y = nullptr, *d_x = nullptr;
   int* d_cnt = nullptr;
-  const BaTask* d_tasks = nullptr;
-  const BaBwdEntry* d_bwd = nullptr;
-  const BaSumEntry* d_sum = nullptr;
   double* d_rhsS = nullptr;
-  const int *d_blkRows = nullptr, *d_diagBlk = nullptr, *d_blkCam0 = nullptr, *d_order = nullptr,
-            *d_solIdx = nullptr;
+  const int* d_solIdx = nullptr;
+  TileLaunch tile;  // of the loaded plan
+  TileLists tl;     // the plan's lists in d_in
   BaTileDev td;
-  std::vector<BaTask> taskOrder;  // as uploaded: [POTRF / BACKWARD | TRSM / UPDATE / SUM]
   unsigned long long* d_trace = nullptr;
-  int solveGrid = 1;
   int numSM = 1;  // of the solver's device
   double factorFlops = 0.0;
   double* d_sc = nullptr;
@@ -268,8 +313,6 @@ struct cosl_ba_solver {
   int nItems = 0;
   long long nEntries = 0;
   double* h_sc = nullptr;  // pinned
-  bool twoSolve = false;  // <= 2 blocks: single-CTA resident solve (ba_tile_two)
-  int two00 = -1, two10 = -1, two11 = -1;
   SectionTimer timer;
   int secLin = 0, secSchur = 0, secSolve = 0, secBack = 0, secCost = 0, secComm = 0;
   // submitted robust loop (cosl_ba_solver_submit): the graph with the device-side LM control and the
@@ -789,11 +832,11 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
         items.push_back(it);
       }
     }
-  std::vector<BaTask> taskOrder;
-  const int nA = tile_task_order(P, taskOrder);
+  TileLaunch tile = tile_launch_plan(P);
+  COSL_TRY(tile_launch_device(tile));
+  const TileImage img = tile_image(P, tile);
   const int nb = std::max(1, P.nb), nTiles = std::max(1, P.nTiles);
-  std::vector<int> h_diagBlk(nTiles, -1), h_solIdx(std::max(1, mf), 0);
-  for (int k = 0; k < P.nb; ++k) h_diagBlk[P.tileIdx[(size_t)k * P.nb + k]] = k;
+  std::vector<int> h_solIdx(std::max(1, mf), 0);
   for (int j = 0; j < mf; ++j) h_solIdx[j] = P.camBlk[j] * BA_TB + P.camOff[j];
   // intrinsics: only K0,K1,K2,K4,K5 are used (as BundleRTS packs them, app/SL_CoSLAMBA.cpp:337-343)
   std::vector<double> camK((size_t)m * 5);
@@ -823,13 +866,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   const size_t oXy = sec(p->xy, sizeof(double) * 2 * (size_t)N);
   const size_t oK = sec(camK.data(), sizeof(double) * camK.size());
   const size_t oItems = sec(items.data(), sizeof(BaPairItem) * items.size());
-  const size_t oTasks = sec(taskOrder.data(), sizeof(BaTask) * taskOrder.size());
-  const size_t oBwd = sec(P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
-  const size_t oSum = sec(P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
-  const size_t oBlkRows = sec(P.blkRows.data(), sizeof(int) * P.nb);
-  const size_t oBlkCam0 = sec(P.blkCam0.data(), P.nb ? sizeof(int) * (P.nb + 1) : 0);
-  const size_t oOrder = sec(P.order.data(), P.nb ? sizeof(int) * mf : 0);
-  const size_t oDiag = sec(h_diagBlk.data(), sizeof(int) * h_diagBlk.size());
+  const size_t oPlan = sec(nullptr, img.bytes);  // tile_image_write
   const size_t oSol = sec(h_solIdx.data(), sizeof(int) * h_solIdx.size());
   const size_t oCamStart = sec(x.camStart.data(), sizeof(unsigned) * x.camStart.size());
   const size_t oPoff = sec(x.poff.data(), sizeof(unsigned) * x.poff.size());
@@ -844,7 +881,8 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
     COSL_TRY(pinned_staging().get(parBytes + inBytes, &s->h_stage, &s->stageBytes));
   }
   for (const Sec& q : secs)
-    if (q.bytes) std::memcpy(s->h_stage + parBytes + q.off, q.src, q.bytes);
+    if (q.src && q.bytes) std::memcpy(s->h_stage + parBytes + q.off, q.src, q.bytes);
+  tile_image_write(P, tile, img, s->h_stage + parBytes + oPlan);
   // from here on the handle holds the new problem
   s->m = m;
   s->n = n;
@@ -857,7 +895,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   s->nEntries = nEntries;
   s->nItems = (int)items.size();
   s->plan = std::move(P);
-  s->taskOrder = std::move(taskOrder);
+  s->tile = std::move(tile);
   const BaPlan& PL = s->plan;
   s->reduceCount = (long long)nb * BA_TB + (long long)PL.nTilesOrig * BA_TILE;
   s->factorFlops = PL.flops;
@@ -869,13 +907,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   s->d_xy = reinterpret_cast<const double*>(s->d_in + oXy);
   s->d_camK = reinterpret_cast<const double*>(s->d_in + oK);
   s->d_items = reinterpret_cast<const BaPairItem*>(s->d_in + oItems);
-  s->d_tasks = reinterpret_cast<const BaTask*>(s->d_in + oTasks);
-  s->d_bwd = reinterpret_cast<const BaBwdEntry*>(s->d_in + oBwd);
-  s->d_sum = reinterpret_cast<const BaSumEntry*>(s->d_in + oSum);
-  s->d_blkRows = reinterpret_cast<const int*>(s->d_in + oBlkRows);
-  s->d_blkCam0 = reinterpret_cast<const int*>(s->d_in + oBlkCam0);
-  s->d_order = reinterpret_cast<const int*>(s->d_in + oOrder);
-  s->d_diagBlk = reinterpret_cast<const int*>(s->d_in + oDiag);
+  s->tl = tile_lists(img, s->d_in + oPlan);
   s->d_solIdx = reinterpret_cast<const int*>(s->d_in + oSol);
   const unsigned* d_camStart = reinterpret_cast<const unsigned*>(s->d_in + oCamStart);
   const unsigned* d_poff = reinterpret_cast<const unsigned*>(s->d_in + oPoff);
@@ -958,47 +990,16 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   }
   COSL_CUDA(cudaGetLastError());
   BaTileDev& td = s->td;
+  td = tile_dev(PL, s->tile, s->tl);
   td.rhs = d.rhs;
   td.tiles = d.tiles;
+  td.rhsS = s->d_rhsS;
   td.Linv = s->d_Linv;
   td.y = s->d_y;
   td.x = s->d_x;
   td.cnt = s->d_cnt;
-  td.tasks = s->d_tasks;
-  td.bwd = s->d_bwd;
-  td.sum = s->d_sum;
-  td.rhsS = s->d_rhsS;
-  td.xdoneBase = PL.nTiles + PL.nScratch;
-  td.blkRows = s->d_blkRows;
-  td.nTasks = (int)PL.tasks.size();
-  td.nA = nA;
-  td.nb = PL.nb;
-  td.nTiles = PL.nTiles;
-  td.nCounters = PL.nCounters;
   td.sc = s->d_sc;
   td.scFail = (int)SC_FAIL;
-  td.trace = nullptr;
-  // Systems of one or two blocks (local BA) are solved by one resident CTA: for the 72 x 72 system of
-  // the c3 local BA, ba_tile_two needs 26 us per LM trial and the task kernel 42 us (H100 80GB HBM3, 400 W).
-  s->twoSolve = false;
-  s->two00 = s->two10 = s->two11 = -1;
-  if (PL.nb >= 1 && PL.nb <= 2) {
-    s->twoSolve = true;
-    s->two00 = PL.tileIdx[0];
-    s->two10 = PL.nb == 2 ? PL.tileIdx[(size_t)1 * PL.nb + 0] : -1;
-    s->two11 = PL.nb == 2 ? PL.tileIdx[(size_t)1 * PL.nb + 1] : -1;
-    if (s->two00 < 0 || (PL.nb == 2 && s->two11 < 0)) s->twoSolve = false;
-  }
-  {
-    // persistent grid: never more CTAs than can be co-resident (the ticket scheduler spins)
-    int perSm = 0;
-    COSL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, ba_tile_solve, BA_NTHREADS, BA_TILE_SMEM));
-    const int grid = s->numSM * std::max(1, std::min(perSm, 1));
-    s->solveGrid = std::max(2, std::min(grid, td.nTasks + 1));
-    // CTAs that only ever run the diagonal-block tasks (see BaTileDev::nSpecial)
-    const int nsp = std::min(24, std::max(1, s->solveGrid / 6));
-    td.nSpecial = std::max(1, std::min(nsp, s->solveGrid - 1));
-  }
   s->covReady = s->covValid = false;
   if (s->covVar > 0) COSL_TRY(cov_prepare(s));
   if (ba_timing())
@@ -1007,8 +1008,8 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   return COSL_OK;
 }
 
-// A solver handle without a problem on the current device: stream, scalar slots, the kernel attributes of the
-// solve.  *out is set once the handle exists, also when a later step fails.
+// A solver handle without a problem on the current device: stream, scalar slots, the kernel attribute of the
+// Schur contraction.  *out is set once the handle exists, also when a later step fails.
 int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver** out) {
   cosl_ba_solver* s = new (std::nothrow) cosl_ba_solver();
   if (!s) return set_error(COSL_E_NOMEM, "host allocation failed");
@@ -1028,10 +1029,7 @@ int make_handle(const cosl_ba_options* opt, cosl_ba_comm* comm, cosl_ba_solver**
   COSL_CUDA(cudaStreamCreateWithFlags(&s->sideStream, cudaStreamNonBlocking));
   COSL_TRY(grow(s, &s->d_link, 1));
   COSL_CUDA(cudaMemsetAsync(s->d_link, 0, sizeof(BaCtlLink), s->rq.stream));  // request numbers start at 1
-  COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
-  COSL_CUDA(cudaFuncSetAttribute(ba_tile_two, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
   COSL_CUDA(cudaFuncSetAttribute(ba_schur_pairs_st, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_ST_SMEM));
-  COSL_TRY(selinv_attributes());
   int nsm = 0;
   COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, s->device));
   s->numSM = std::max(1, nsm);
@@ -1173,7 +1171,7 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
     // also clears the scalars of this trial (|dp|^2, dL, |p|^2, fail, cost, non-finite), the task counters
     // of the solve and the accumulator of the point back-substitution (d_dpb)
     COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)s->n + s->m, 256), 256, 0, st, s->d, dctl,
-                mu, r0, s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks,
+                mu, r0, s->tl.diagBlk, s->tl.blkCam0, s->tl.order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks,
                 nTilesInit, s->d_Vinv, doStats, s->d_dpb, 3LL * s->n);
     if (doStats) COSL_TRY(allreduce(s, s->d_sc + SC_NSUM, 2, ncclMax));
     if (s->nItems)
@@ -1183,10 +1181,7 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
     // the one exchange of an LM trial: [rhs | Schur-structure tiles] is contiguous, no packing
     COSL_TRY(allreduce(s, s->d_S, (size_t)s->reduceCount, ncclSum));
     T.begin(s->secSolve, st);  // reduced camera system -> d_x (block padded, permuted)
-    if (s->twoSolve)
-      COSL_LAUNCH(ba_tile_two, 1, BA_NTHREADS, BA_TILE_SMEM, st, s->td, s->two00, s->two10, s->two11);
-    else
-      COSL_LAUNCH(ba_tile_solve, s->solveGrid, BA_NTHREADS, BA_TILE_SMEM, st, s->td);
+    COSL_TRY(tile_solve_enqueue(s->tile, s->td, st));
     T.end(st);
     // back substitution + trial cost in two launches (ba_kernels.cuh); V*^-1 is the one the contraction used
     const int nCamBlocks = div_up(6 * s->m, 256);
@@ -1353,8 +1348,8 @@ int download(cosl_ba_solver* s, cosl_ba_problem* p) {
 int cov_prepare(cosl_ba_solver* s) {
   const BaPlan& P = s->plan;
   s->sel = ba_make_selinv_plan(P);
-  size_t oTasks = 0, oOps = 0;
-  const std::vector<unsigned char> idx = selinv_index(P, s->sel, &oTasks, &oOps);
+  size_t oOps = 0;
+  const std::vector<unsigned char> idx = selinv_index(s->sel, &oOps);
   const size_t nb = (size_t)std::max(1, P.nb), n = (size_t)s->n, m = (size_t)s->m;
   COSL_TRY(grow(s, &s->d_covIdx, idx.size()));
   COSL_TRY(grow(s, &s->d_covWgt, (size_t)s->N));
@@ -1377,10 +1372,10 @@ int cov_prepare(cosl_ba_solver* s) {
   sd.Z = s->d_covZ;
   sd.X = s->d_covX;
   sd.piv = s->d_covPiv;
-  sd.diagTile = reinterpret_cast<const int*>(s->d_covIdx);
-  sd.tasks = reinterpret_cast<const BaSelTask*>(s->d_covIdx + oTasks);
+  sd.diagTile = s->tl.diagTile;
+  sd.tasks = reinterpret_cast<const BaSelTask*>(s->d_covIdx);
   sd.ops = reinterpret_cast<const BaSelOp*>(s->d_covIdx + oOps);
-  sd.blkRows = s->d_blkRows;
+  sd.blkRows = s->tl.blkRows;
   sd.cnt = s->d_covCnt;
   s->covReady = true;
   return COSL_OK;
@@ -1417,7 +1412,7 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
   // mu = 0: S and V^-1 of the undamped system (and the cleared scalars and task counters)
   const int nTilesInit = std::max(1, s->plan.nTiles);
   COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)n + m, 256), 256, 0, st, cd, nullptr, 0.0, 1,
-              s->d_diagBlk, s->d_blkCam0, s->d_order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks, nTilesInit,
+              s->tl.diagBlk, s->tl.blkCam0, s->tl.order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks, nTilesInit,
               s->d_Vinv, 0, nullptr, 0LL);
   if (s->N) COSL_TRY(launch_cost(cd, s->d_pa, s->d_pb, gN, st));
   if (n) COSL_LAUNCH(ba_cov_vfix, div_up(n, 256), 256, 0, st, s->d_covUnc, s->d_Vinv, n);
@@ -1425,7 +1420,7 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
     if (s->nItems)
       COSL_LAUNCH(ba_schur_pairs_st, div_up(s->nItems, BA_ST_WARPS), 32 * BA_ST_WARPS, BA_ST_SMEM, st, cd, s->d_items,
                   s->nItems, s->d_entries, s->d_Vinv);
-    COSL_TRY(selinv_launch(s->plan, s->sel, td, s->solveGrid, s->sdev, st));
+    COSL_TRY(selinv_launch(s->tile, s->sel, td, s->sdev, st));
   }
   COSL_LAUNCH(ba_cov_cams, div_up(m, 128), 128, 0, st, cd, s->d_pa, s->d_covZ, s->sdev.diagTile, var, s->d_covCam);
   if (s->ns && s->nItems)
@@ -1570,6 +1565,67 @@ int build_graph(cosl_ba_solver* s) {
   s->graphNb = s->d_nb;
   s->graphCovVar = s->covVar;
   s->graphObsL = s->d.obsL;
+  return COSL_OK;
+}
+
+/* ---------------------------------------------------------------- debug entry points */
+// The device side of a debug solve of the dense SPD system S (6 mf x 6 mf) in one block from `tmp`, enqueued on
+// `st`: the lower triangle of S placed as load_problem's pair_dst places the Schur blocks (the camera later in
+// the elimination order owns the rows; fill and padding stay zero), b or zeros as the block-padded rhs, the
+// plan's lists, the solve's work buffers (scratch tiles and their rhs parts start as NaN: their first update must
+// overwrite them), zeroed counters and failure flag (td.sc[0]), and `extraBytes` more at *extra.
+int debug_tile_setup(const BaPlan& P, const TileLaunch& L, int mf, const uint8_t* adj, const double* S,
+                     const double* b, size_t extraBytes, TmpDeviceBufs& tmp, cudaStream_t st, BaTileDev& td,
+                     TileLists& tl, unsigned char** extra) {
+  const int nb = P.nb;
+  const size_t ns = 6 * (size_t)mf, nScratch = (size_t)std::max(1, P.nScratch);
+  const size_t nCnt = (size_t)P.nCounters + 2 + L.order.size();
+  std::vector<double> hTiles((size_t)P.nTiles * BA_TILE, 0.0), hRhs((size_t)nb * BA_TB, 0.0);
+  for (int a = 0; a < mf; ++a)
+    for (int c = 0; c < mf; ++c) {
+      if (a != c && !adj[(size_t)a * mf + c] && !adj[(size_t)c * mf + a]) continue;
+      const int bA = P.camBlk[a], bC = P.camBlk[c];
+      if (bA < bC || (bA == bC && P.camOff[a] < P.camOff[c])) continue;
+      double* T = &hTiles[(size_t)P.tileIdx[(size_t)bA * nb + bC] * BA_TILE];
+      for (int r = 0; r < 6; ++r)
+        for (int q = 0; q < 6; ++q) {
+          if (a == c && q > r) continue;
+          const size_t i = 6 * (size_t)a + r, j = 6 * (size_t)c + q;
+          T[(size_t)(P.camOff[c] + q) * BA_TB + P.camOff[a] + r] = i >= j ? S[i * ns + j] : S[j * ns + i];
+        }
+    }
+  if (b)
+    for (int a = 0; a < mf; ++a)
+      for (int r = 0; r < 6; ++r) hRhs[(size_t)P.camBlk[a] * BA_TB + P.camOff[a] + r] = b[6 * a + r];
+  const TileImage img = tile_image(P, L);
+  SlabLayout W;
+  const size_t oImg = W.take(img.bytes), oRhs = W.take(8 * hRhs.size());
+  const size_t oTiles = W.take(8 * ((size_t)P.nTiles + P.nScratch) * BA_TILE), oRhsS = W.take(8 * nScratch * BA_TB);
+  const size_t oLinv = W.take(8 * (size_t)nb * BA_TILE), oY = W.take(8 * hRhs.size()), oX = W.take(8 * hRhs.size());
+  const size_t oSc = W.take(8), oCnt = W.take(4 * nCnt), oExtra = W.take(extraBytes);
+  unsigned char* d = nullptr;
+  COSL_TRY(tmp.alloc(&d, W.bytes));
+  tl = tile_lists(img, d + oImg);
+  td = tile_dev(P, L, tl);
+  td.rhs = reinterpret_cast<double*>(d + oRhs);
+  td.tiles = reinterpret_cast<double*>(d + oTiles);
+  td.rhsS = reinterpret_cast<double*>(d + oRhsS);
+  td.Linv = reinterpret_cast<double*>(d + oLinv);
+  td.y = reinterpret_cast<double*>(d + oY);
+  td.x = reinterpret_cast<double*>(d + oX);
+  td.cnt = reinterpret_cast<int*>(d + oCnt);
+  td.sc = reinterpret_cast<double*>(d + oSc);
+  td.scFail = 0;
+  *extra = d + oExtra;
+  std::vector<unsigned char> hImg(img.bytes);
+  tile_image_write(P, L, img, hImg.data());
+  COSL_CUDA(cudaMemcpyAsync(d + oImg, hImg.data(), hImg.size(), cudaMemcpyHostToDevice, st));
+  COSL_CUDA(cudaMemcpyAsync(td.rhs, hRhs.data(), 8 * hRhs.size(), cudaMemcpyHostToDevice, st));
+  COSL_CUDA(cudaMemcpyAsync(td.tiles, hTiles.data(), 8 * hTiles.size(), cudaMemcpyHostToDevice, st));
+  COSL_CUDA(cudaMemsetAsync(td.tiles + hTiles.size(), 0xff, 8 * (size_t)P.nScratch * BA_TILE, st));
+  COSL_CUDA(cudaMemsetAsync(td.rhsS, 0xff, 8 * nScratch * BA_TB, st));
+  COSL_CUDA(cudaMemsetAsync(td.cnt, 0, 4 * nCnt, st));
+  COSL_CUDA(cudaMemsetAsync(td.sc, 0, 8, st));
   return COSL_OK;
 }
 
@@ -1913,8 +1969,8 @@ int cosl_ba_solver_plan_info(cosl_ba_solver* s, int out[8]) {
   out[3] = (int)s->plan.tasks.size();
   out[4] = s->plan.ndDepth;
   out[5] = s->plan.criticalPathTasks;
-  out[6] = s->solveGrid;
-  out[7] = s->twoSolve ? 1 : 0;
+  out[6] = s->tile.grid;
+  out[7] = s->tile.two ? 1 : 0;
   return COSL_OK;
 }
 
@@ -1936,9 +1992,9 @@ int cosl_ba_solver_trace(cosl_ba_solver* s, int enable, uint64_t* out, int32_t* 
     COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
     if (meta)
       for (int t = 0; t < n; ++t) {
-        meta[3 * t] = s->taskOrder[t].type;
-        meta[3 * t + 1] = s->taskOrder[t].k;
-        meta[3 * t + 2] = s->taskOrder[t].i;
+        meta[3 * t] = s->tile.order[t].type;
+        meta[3 * t + 1] = s->tile.order[t].k;
+        meta[3 * t + 2] = s->tile.order[t].i;
       }
   }
   s->td.trace = nullptr;
@@ -1954,7 +2010,7 @@ int cosl_ba_solver_tasks(cosl_ba_solver* s, int32_t* tasks, int cap, int32_t* li
   const int nt = (int)P.tasks.size();
   int nl = 0;
   for (int t = 0; t < nt && t < cap; ++t) {
-    BaTask k = s->taskOrder[t];
+    BaTask k = s->tile.order[t];
     if (k.type == BA_T_BWD || k.type == BA_T_SUM) {
       const int l0 = nl;
       for (int e = k.l0; e < k.l1; ++e) {
@@ -1980,70 +2036,19 @@ int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const dou
     return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_solve: bad argument");
   const BaPlan P = ba_make_plan(mf, std::vector<uint8_t>(adj, adj + (size_t)mf * mf), nd_depth);
   if (P.nb <= 0) return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_solve: planning failed");
-  std::vector<BaTask> tasks;
-  const int nA = tile_task_order(P, tasks);
-  const int nb = P.nb;
-  const size_t ns = 6 * (size_t)mf, nScratch = (size_t)std::max(1, P.nScratch);
-  const size_t nCnt = (size_t)P.nCounters + 2 + tasks.size();
-  // the lower triangle of the permuted system, placed as build_solver's pair_dst places the Schur
-  // blocks: the camera later in the elimination order owns the rows; fill and padding stay zero
-  std::vector<double> hTiles((size_t)P.nTiles * BA_TILE, 0.0), hRhs((size_t)nb * BA_TB, 0.0);
-  for (int a = 0; a < mf; ++a)
-    for (int c = 0; c < mf; ++c) {
-      if (a != c && !adj[(size_t)a * mf + c] && !adj[(size_t)c * mf + a]) continue;
-      const int bA = P.camBlk[a], bC = P.camBlk[c];
-      if (bA < bC || (bA == bC && P.camOff[a] < P.camOff[c])) continue;
-      double* T = &hTiles[(size_t)P.tileIdx[(size_t)bA * nb + bC] * BA_TILE];
-      for (int r = 0; r < 6; ++r)
-        for (int q = 0; q < 6; ++q) {
-          if (a == c && q > r) continue;
-          const size_t i = 6 * (size_t)a + r, j = 6 * (size_t)c + q;
-          T[(size_t)(P.camOff[c] + q) * BA_TB + P.camOff[a] + r] = i >= j ? S[i * ns + j] : S[j * ns + i];
-        }
-    }
-  for (int a = 0; a < mf; ++a)
-    for (int r = 0; r < 6; ++r) hRhs[(size_t)P.camBlk[a] * BA_TB + P.camOff[a] + r] = b[6 * a + r];
-  int device = 0;
-  COSL_CUDA(cudaGetDevice(&device));
+  TileLaunch L = tile_launch_plan(P);
+  COSL_TRY(tile_launch_device(L));
   cudaStream_t s = cudaStreamPerThread;
   TmpDeviceBufs tmp(s);
-  double *dRhs, *dTiles, *dRhsS, *dLinv, *dY, *dX, *dFail;
-  int *dCnt, *dBlkRows;
-  BaTask* dTasks;
-  BaBwdEntry* dBwd;
-  BaSumEntry* dSum;
-  COSL_TRY(tmp.alloc(&dRhs, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dTiles, ((size_t)P.nTiles + P.nScratch) * BA_TILE));
-  COSL_TRY(tmp.alloc(&dRhsS, nScratch * BA_TB));
-  COSL_TRY(tmp.alloc(&dLinv, (size_t)nb * BA_TILE));
-  COSL_TRY(tmp.alloc(&dY, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dX, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dFail, 1));
-  COSL_TRY(tmp.alloc(&dCnt, nCnt));
-  COSL_TRY(tmp.alloc(&dBlkRows, (size_t)nb));
-  COSL_TRY(tmp.alloc(&dTasks, tasks.size()));
-  COSL_TRY(tmp.alloc(&dBwd, P.bwdList.size()));
-  COSL_TRY(tmp.alloc(&dSum, P.sumList.size()));
-  COSL_CUDA(cudaMemcpyAsync(dRhs, hRhs.data(), 8 * hRhs.size(), cudaMemcpyHostToDevice, s));
-  COSL_CUDA(cudaMemcpyAsync(dTiles, hTiles.data(), 8 * hTiles.size(), cudaMemcpyHostToDevice, s));
-  // scratch tiles and their rhs parts start as NaN: their first update must overwrite them
-  COSL_CUDA(cudaMemsetAsync(dTiles + (size_t)P.nTiles * BA_TILE, 0xff, 8 * (size_t)P.nScratch * BA_TILE, s));
-  COSL_CUDA(cudaMemsetAsync(dRhsS, 0xff, 8 * nScratch * BA_TB, s));
-  COSL_CUDA(cudaMemsetAsync(dCnt, 0, 4 * nCnt, s));
-  COSL_CUDA(cudaMemsetAsync(dFail, 0, 8, s));
-  COSL_CUDA(cudaMemcpyAsync(dBlkRows, P.blkRows.data(), 4 * (size_t)nb, cudaMemcpyHostToDevice, s));
-  COSL_CUDA(cudaMemcpyAsync(dTasks, tasks.data(), sizeof(BaTask) * tasks.size(), cudaMemcpyHostToDevice, s));
-  if (!P.bwdList.empty())
-    COSL_CUDA(cudaMemcpyAsync(dBwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size(), cudaMemcpyHostToDevice, s));
-  if (!P.sumList.empty())
-    COSL_CUDA(cudaMemcpyAsync(dSum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size(), cudaMemcpyHostToDevice, s));
-  const TileSolveBufs tb = {dRhs, dTiles, dRhsS, dLinv, dY, dX, dCnt, dTasks, dBwd, dSum, dBlkRows, dFail};
-  int grid = 0;
-  COSL_TRY(tile_solve_launch(P, nA, tb, device, s, &grid));
-  std::vector<double> hX((size_t)nb * BA_TB);
+  BaTileDev td;
+  TileLists tl;
+  unsigned char* extra = nullptr;
+  COSL_TRY(debug_tile_setup(P, L, mf, adj, S, b, 0, tmp, s, td, tl, &extra));
+  COSL_TRY(tile_solve_enqueue(L, td, s));
+  std::vector<double> hX((size_t)P.nb * BA_TB);
   double hFail = 0.0;
-  COSL_CUDA(cudaMemcpyAsync(hX.data(), dX, 8 * hX.size(), cudaMemcpyDeviceToHost, s));
-  COSL_CUDA(cudaMemcpyAsync(&hFail, dFail, 8, cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(hX.data(), td.x, 8 * hX.size(), cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(&hFail, td.sc, 8, cudaMemcpyDeviceToHost, s));
   COSL_CUDA(cudaStreamSynchronize(s));
   for (int a = 0; a < mf; ++a)
     for (int r = 0; r < 6; ++r) x[6 * a + r] = hX[(size_t)P.camBlk[a] * BA_TB + P.camOff[a] + r];
@@ -2054,8 +2059,8 @@ int cosl_ba_debug_tile_solve(int mf, const uint8_t* adj, int nd_depth, const dou
   out[3] = (int)P.tasks.size();
   out[4] = P.ndDepth;
   out[5] = P.criticalPathTasks;
-  out[6] = grid;
-  out[7] = grid == 1 ? 1 : 0;
+  out[6] = L.two ? 1 : L.grid;
+  out[7] = L.two ? 1 : 0;
   return COSL_OK;
 }
 
@@ -2067,113 +2072,43 @@ int cosl_ba_debug_tile_selinv(int mf, const uint8_t* adj, int nd_depth, const do
   const BaPlan P = ba_make_plan(mf, std::vector<uint8_t>(adj, adj + (size_t)mf * mf), nd_depth);
   if (P.nb <= 0) return set_error(COSL_E_INVALID, "cosl_ba_debug_tile_selinv: planning failed");
   const BaSelPlan SP = ba_make_selinv_plan(P);
-  std::vector<BaTask> tasks;
-  const int nA = tile_task_order(P, tasks);
+  TileLaunch L = tile_launch_plan(P);
+  COSL_TRY(tile_launch_device(L));
   const int nb = P.nb;
-  const size_t ns = 6 * (size_t)mf, nScratch = (size_t)std::max(1, P.nScratch);
-  const size_t nCnt = (size_t)P.nCounters + 2 + tasks.size();
-  std::vector<double> hTiles((size_t)P.nTiles * BA_TILE, 0.0);  // placed as cosl_ba_debug_tile_solve places them
-  for (int a = 0; a < mf; ++a)
-    for (int c = 0; c < mf; ++c) {
-      if (a != c && !adj[(size_t)a * mf + c] && !adj[(size_t)c * mf + a]) continue;
-      const int bA = P.camBlk[a], bC = P.camBlk[c];
-      if (bA < bC || (bA == bC && P.camOff[a] < P.camOff[c])) continue;
-      double* T = &hTiles[(size_t)P.tileIdx[(size_t)bA * nb + bC] * BA_TILE];
-      for (int r = 0; r < 6; ++r)
-        for (int q = 0; q < 6; ++q) {
-          if (a == c && q > r) continue;
-          const size_t i = 6 * (size_t)a + r, j = 6 * (size_t)c + q;
-          T[(size_t)(P.camOff[c] + q) * BA_TB + P.camOff[a] + r] = i >= j ? S[i * ns + j] : S[j * ns + i];
-        }
-    }
-  size_t oTasks = 0, oOps = 0;
-  const std::vector<unsigned char> idx = selinv_index(P, SP, &oTasks, &oOps);
-  int device = 0;
-  COSL_CUDA(cudaGetDevice(&device));
-  COSL_TRY(selinv_attributes());
-  COSL_CUDA(cudaFuncSetAttribute(ba_tile_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, BA_TILE_SMEM));
+  const size_t ns = 6 * (size_t)mf;
+  size_t oOps = 0;
+  const std::vector<unsigned char> idx = selinv_index(SP, &oOps);
+  // the stage's buffers: [plan | Z | X | sdiag | piv | cnt]
+  SlabLayout E;
+  const size_t oIdx = E.take(idx.size()), oZ = E.take(8 * (size_t)P.nTiles * BA_TILE);
+  const size_t oXk = E.take(8 * (size_t)nb * BA_TILE), oSdiag = E.take(8 * (size_t)nb * BA_TB);
+  const size_t oPiv = E.take(8 * (size_t)nb), oCnt = E.take(4 * (size_t)nb);
   cudaStream_t s = cudaStreamPerThread;
   TmpDeviceBufs tmp(s);
-  double *dRhs, *dTiles, *dRhsS, *dLinv, *dY, *dX, *dSc, *dZ, *dXk, *dSdiag, *dPiv;
-  int *dCnt, *dBlkRows, *dSelCnt;
-  unsigned char* dIdx;
-  BaTask* dTasks;
-  BaBwdEntry* dBwd;
-  BaSumEntry* dSum;
-  COSL_TRY(tmp.alloc(&dRhs, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dTiles, ((size_t)P.nTiles + P.nScratch) * BA_TILE));
-  COSL_TRY(tmp.alloc(&dRhsS, nScratch * BA_TB));
-  COSL_TRY(tmp.alloc(&dLinv, (size_t)nb * BA_TILE));
-  COSL_TRY(tmp.alloc(&dY, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dX, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dSc, 1));
-  COSL_TRY(tmp.alloc(&dZ, (size_t)P.nTiles * BA_TILE));
-  COSL_TRY(tmp.alloc(&dXk, (size_t)nb * BA_TILE));
-  COSL_TRY(tmp.alloc(&dSdiag, (size_t)nb * BA_TB));
-  COSL_TRY(tmp.alloc(&dPiv, (size_t)nb));
-  COSL_TRY(tmp.alloc(&dCnt, nCnt));
-  COSL_TRY(tmp.alloc(&dBlkRows, (size_t)nb));
-  COSL_TRY(tmp.alloc(&dSelCnt, (size_t)nb));
-  COSL_TRY(tmp.alloc(&dIdx, idx.size()));
-  COSL_TRY(tmp.alloc(&dTasks, tasks.size()));
-  COSL_TRY(tmp.alloc(&dBwd, P.bwdList.size()));
-  COSL_TRY(tmp.alloc(&dSum, P.sumList.size()));
-  COSL_CUDA(cudaMemsetAsync(dRhs, 0, 8 * (size_t)nb * BA_TB, s));
-  COSL_CUDA(cudaMemcpyAsync(dTiles, hTiles.data(), 8 * hTiles.size(), cudaMemcpyHostToDevice, s));
-  COSL_CUDA(cudaMemsetAsync(dTiles + (size_t)P.nTiles * BA_TILE, 0xff, 8 * (size_t)P.nScratch * BA_TILE, s));
-  COSL_CUDA(cudaMemsetAsync(dRhsS, 0xff, 8 * nScratch * BA_TB, s));
-  COSL_CUDA(cudaMemsetAsync(dCnt, 0, 4 * nCnt, s));
-  COSL_CUDA(cudaMemsetAsync(dSelCnt, 0, 4 * (size_t)nb, s));
-  COSL_CUDA(cudaMemsetAsync(dSc, 0, 8, s));
-  COSL_CUDA(cudaMemcpyAsync(dBlkRows, P.blkRows.data(), 4 * (size_t)nb, cudaMemcpyHostToDevice, s));
-  COSL_CUDA(cudaMemcpyAsync(dIdx, idx.data(), idx.size(), cudaMemcpyHostToDevice, s));
-  COSL_CUDA(cudaMemcpyAsync(dTasks, tasks.data(), sizeof(BaTask) * tasks.size(), cudaMemcpyHostToDevice, s));
-  if (!P.bwdList.empty())
-    COSL_CUDA(cudaMemcpyAsync(dBwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size(), cudaMemcpyHostToDevice, s));
-  if (!P.sumList.empty())
-    COSL_CUDA(cudaMemcpyAsync(dSum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size(), cudaMemcpyHostToDevice, s));
-  BaTileDev td = {};
-  td.rhs = dRhs;
-  td.tiles = dTiles;
-  td.rhsS = dRhsS;
-  td.Linv = dLinv;
-  td.y = dY;
-  td.x = dX;
-  td.cnt = dCnt;
-  td.tasks = dTasks;
-  td.bwd = dBwd;
-  td.sum = dSum;
-  td.blkRows = dBlkRows;
-  td.nTasks = (int)tasks.size();
-  td.nA = nA;
-  td.nb = nb;
-  td.nTiles = P.nTiles;
-  td.nCounters = P.nCounters;
-  td.xdoneBase = P.nTiles + P.nScratch;
-  td.sc = dSc;
-  td.scFail = 0;
-  int nsm = 0;
-  COSL_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
-  const int grid = std::max(2, std::min(std::max(1, nsm), td.nTasks + 1));  // as tile_solve_launch
-  td.nSpecial = std::max(1, std::min(std::min(24, std::max(1, grid / 6)), grid - 1));
+  BaTileDev td;
+  TileLists tl;
+  unsigned char* e = nullptr;
+  COSL_TRY(debug_tile_setup(P, L, mf, adj, S, nullptr, E.bytes, tmp, s, td, tl, &e));
   BaSelDev sd = {};
-  sd.L = dTiles;
-  sd.Linv = dLinv;
-  sd.sdiag = dSdiag;
-  sd.Z = dZ;
-  sd.X = dXk;
-  sd.piv = dPiv;
-  sd.diagTile = reinterpret_cast<const int*>(dIdx);
-  sd.tasks = reinterpret_cast<const BaSelTask*>(dIdx + oTasks);
-  sd.ops = reinterpret_cast<const BaSelOp*>(dIdx + oOps);
-  sd.blkRows = dBlkRows;
-  sd.cnt = dSelCnt;
-  COSL_TRY(selinv_launch(P, SP, td, grid, sd, s));
+  sd.L = td.tiles;
+  sd.Linv = td.Linv;
+  sd.sdiag = reinterpret_cast<double*>(e + oSdiag);
+  sd.Z = reinterpret_cast<double*>(e + oZ);
+  sd.X = reinterpret_cast<double*>(e + oXk);
+  sd.piv = reinterpret_cast<double*>(e + oPiv);
+  sd.diagTile = tl.diagTile;
+  sd.tasks = reinterpret_cast<const BaSelTask*>(e + oIdx);
+  sd.ops = reinterpret_cast<const BaSelOp*>(e + oIdx + oOps);
+  sd.blkRows = tl.blkRows;
+  sd.cnt = reinterpret_cast<int*>(e + oCnt);
+  COSL_CUDA(cudaMemcpyAsync(e + oIdx, idx.data(), idx.size(), cudaMemcpyHostToDevice, s));
+  COSL_CUDA(cudaMemsetAsync(sd.cnt, 0, 4 * (size_t)nb, s));
+  COSL_TRY(selinv_launch(L, SP, td, sd, s));
   std::vector<double> hZ((size_t)P.nTiles * BA_TILE), hPiv(nb);
   double hFail = 0.0;
-  COSL_CUDA(cudaMemcpyAsync(hZ.data(), dZ, 8 * hZ.size(), cudaMemcpyDeviceToHost, s));
-  COSL_CUDA(cudaMemcpyAsync(hPiv.data(), dPiv, 8 * (size_t)nb, cudaMemcpyDeviceToHost, s));
-  COSL_CUDA(cudaMemcpyAsync(&hFail, dSc, 8, cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(hZ.data(), sd.Z, 8 * hZ.size(), cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(hPiv.data(), sd.piv, 8 * (size_t)nb, cudaMemcpyDeviceToHost, s));
+  COSL_CUDA(cudaMemcpyAsync(&hFail, td.sc, 8, cudaMemcpyDeviceToHost, s));
   COSL_CUDA(cudaStreamSynchronize(s));
   double minPiv = 1e300;
   for (double v : hPiv) minPiv = std::min(minPiv, v);
@@ -2199,8 +2134,8 @@ int cosl_ba_debug_tile_selinv(int mf, const uint8_t* adj, int nd_depth, const do
   out[3] = (int)SP.tasks.size();
   out[4] = P.ndDepth;
   out[5] = (int)SP.stepBegin.size() - 1;
-  out[6] = P.nb <= 2 ? 1 : grid;
-  out[7] = P.nb <= 2 ? 1 : 0;
+  out[6] = L.two ? 1 : L.grid;
+  out[7] = L.two ? 1 : 0;
   return COSL_OK;
 }
 

@@ -20,29 +20,9 @@
 #include <stdint.h>
 
 #include "ba_plan.h"
+#include "tile_solve.h"  // BaTileDev
 
 namespace coslam {
-
-struct BaTileDev {
-  double* rhs;    // [nb*64]
-  double* tiles;  // [nTiles + nScratch][4096]  (scratch tiles: see ba_plan.h)
-  double* rhsS;   // [nScratch*64] rhs parts that travel with the scratch tiles of diagonal tiles
-  double* Linv;   // [nb][4096]
-  double* y;      // [nb*64]
-  double* x;      // [nb*64]
-  int* cnt;       // [nCounters + 2 + nTasks]: counters, the two task tickets of the CTA roles, claim flags
-  const BaTask* tasks;
-  const BaBwdEntry* bwd;
-  const BaSumEntry* sum;
-  const int* blkRows;
-  int nTasks, nb, nTiles, nCounters;
-  int nA;        // tasks [0, nA) = POTRF / BACKWARD (specialist CTAs), [nA, nTasks) = TRSM / UPDATE / SUM
-  int nSpecial;  // CTAs [0, nSpecial) serve the first list: code working sets stay inside the I-cache
-  int xdoneBase;  // counter index of "x_0 done" (= nTiles + nScratch)
-  double* sc;
-  int scFail;
-  unsigned long long* trace;  // optional [nTasks][8]: sm id, ns at ticket / ready / done, 4 phase stamps
-};
 
 constexpr int BA_LDS = 68;                                   // smem leading dimension of a staged tile
 constexpr int BA_TILE_SMEM_DOUBLES = 3 * BA_TB * BA_LDS + 8 * BA_TB + 8 * BA_TB + 2 * BA_TB + 96;

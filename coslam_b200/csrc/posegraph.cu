@@ -594,16 +594,6 @@ pg_finish(PgDev d, int nNodes, const double* __restrict__ x1, const double* __re
 
 thread_local double g_pgHostMs = 0.0;
 
-// aligned bump layout of one device slab (the same offsets index the host staging buffers)
-struct SlabLayout {
-  size_t bytes = 0;
-  size_t take(size_t n) {
-    const size_t at = (bytes + 255) & ~(size_t)255;
-    bytes = at + n;
-    return at;
-  }
-};
-
 // Where a prepare step packs a request's inputs: stage(bytes, &buf) points buf at a host buffer of at least
 // `bytes` bytes (pageable for the synchronous calls, the handle's pinned buffer for a submit) or returns an
 // error code.
@@ -729,14 +719,15 @@ int chain_status(const char* fn, int status) {
 // assembly, two tile solves, finish), shared by cosl_posegraph_solve and cosl_posegraph_solver_submit.
 struct PgSlab {  // offsets of the slab's sections; [0, in) is the packed input, uploaded in one copy
   size_t R, t, eR, et, fixed, id1, id2, sc, freeNode, freeOf, nodeOff, nodeEdges, colOff, colEdges, pair, unitPos,
-      items, itemOff, diag, order, blkCam0, blkRows, tasks, bwd, sum, cnt, in;
+      items, itemOff, plan, cnt, in;
   size_t rhs, tiles, rhsS, Linv, y, x, x1, out, bytes;
 };
 
 struct PgJob {
   int N = 0, nScale = 0, nF = 0;  // nF == 0: no free node, answered on the host (fixed nodes are copied)
   BaPlan P;
-  int nA = 0;
+  TileLaunch tile;
+  TileImage img;  // layout of the plan's lists, at o.plan
   size_t nCnt = 0, nOut = 0;  // counters of the tile solve; doubles of the output region
   PgSlab o = {};
 };
@@ -843,8 +834,8 @@ int pg_prepare(const char* fn, int nNodes, const uint8_t* fixed, const double* R
   j.P = ba_make_plan(mf, adj);
   const BaPlan& P = j.P;
   if (P.nb <= 0) return set_error(COSL_E_NUMERIC, "%s: planning the solve failed", fn);
-  std::vector<BaTask> tasks;
-  j.nA = tile_task_order(P, tasks);
+  j.tile = tile_launch_plan(P);
+  j.img = tile_image(P, j.tile);
   // ---- items: every structurally non-zero 6x6 block of the lower triangle, grouped by tile
   std::vector<int> unitPos(mf);
   for (int u = 0; u < mf; ++u) unitPos[u] = P.camBlk[u] * 64 + P.camOff[u];
@@ -867,7 +858,7 @@ int pg_prepare(const char* fn, int nNodes, const uint8_t* fixed, const double* R
   if (pairEdges.empty()) pairEdges.push_back(0);
   const int nTiles = P.nTiles, nb = P.nb;
   auto tileOf = [&](const PgItem& it) { return P.tileIdx[(size_t)P.camBlk[it.uR] * nb + P.camBlk[it.uC]]; };
-  std::vector<int> itemOff(nTiles + 1, 0), diagBlk(nTiles, -1);
+  std::vector<int> itemOff(nTiles + 1, 0);
   for (const PgItem& it : raw) ++itemOff[tileOf(it) + 1];
   for (int q = 0; q < nTiles; ++q) itemOff[q + 1] += itemOff[q];
   std::vector<PgItem> items(raw.size());
@@ -875,12 +866,11 @@ int pg_prepare(const char* fn, int nNodes, const uint8_t* fixed, const double* R
     std::vector<int> fill(itemOff.begin(), itemOff.end() - 1);
     for (const PgItem& it : raw) items[fill[tileOf(it)]++] = it;
   }
-  for (int k = 0; k < nb; ++k) diagBlk[P.tileIdx[(size_t)k * nb + k]] = k;
   std::vector<int> sc(E);
   for (int e = 0; e < E; ++e) sc[e] = scaleCol ? scaleCol[e] : -1;
   // ---- one slab: inputs (uploaded in one copy, counters included as zeros), work, outputs
   const size_t nTilesAll = (size_t)nTiles + P.nScratch;
-  j.nCnt = (size_t)P.nCounters + 2 + tasks.size();
+  j.nCnt = (size_t)P.nCounters + 2 + j.tile.order.size();
   SlabLayout L;
   auto put = [&](size_t bytes) { return L.take(std::max<size_t>(bytes, 8)); };
   PgSlab& o = j.o;
@@ -891,10 +881,7 @@ int pg_prepare(const char* fn, int nNodes, const uint8_t* fixed, const double* R
   o.colOff = put(4 * colOff.size()), o.colEdges = put(4 * colEdges.size());
   o.pair = put(4 * pairEdges.size()), o.unitPos = put(4 * (size_t)mf);
   o.items = put(sizeof(PgItem) * items.size()), o.itemOff = put(4 * itemOff.size());
-  o.diag = put(4 * (size_t)nTiles), o.order = put(4 * (size_t)mf), o.blkCam0 = put(4 * (size_t)(nb + 1));
-  o.blkRows = put(4 * (size_t)nb), o.tasks = put(sizeof(BaTask) * tasks.size());
-  o.bwd = put(sizeof(BaBwdEntry) * P.bwdList.size()), o.sum = put(sizeof(BaSumEntry) * P.sumList.size());
-  o.cnt = put(4 * j.nCnt);
+  o.plan = put(j.img.bytes), o.cnt = put(4 * j.nCnt);
   o.in = L.bytes;
   o.rhs = put(8 * (size_t)nb * 64), o.tiles = put(8 * nTilesAll * 4096);
   o.rhsS = put(8 * (size_t)std::max(1, P.nScratch) * 64), o.Linv = put(8 * (size_t)nb * 4096);
@@ -927,20 +914,14 @@ int pg_prepare(const char* fn, int nNodes, const uint8_t* fixed, const double* R
   pack(o.unitPos, unitPos.data(), 4 * (size_t)mf);
   pack(o.items, items.data(), sizeof(PgItem) * items.size());
   pack(o.itemOff, itemOff.data(), 4 * itemOff.size());
-  pack(o.diag, diagBlk.data(), 4 * (size_t)nTiles);
-  pack(o.order, P.order.data(), 4 * (size_t)mf);
-  pack(o.blkCam0, P.blkCam0.data(), 4 * (size_t)(nb + 1));
-  pack(o.blkRows, P.blkRows.data(), 4 * (size_t)nb);
-  pack(o.tasks, tasks.data(), sizeof(BaTask) * tasks.size());
-  pack(o.bwd, P.bwdList.data(), sizeof(BaBwdEntry) * P.bwdList.size());
-  pack(o.sum, P.sumList.data(), sizeof(BaSumEntry) * P.sumList.size());
+  tile_image_write(P, j.tile, j.img, reinterpret_cast<unsigned char*>(h + o.plan));
   return COSL_OK;
 }
 
 // The solve (j.nF > 0) on `s` into `slab` (j.o.bytes): the packed inputs in one copy, assembly and tile solve
 // twice, pg_finish, and the output region (j.nOut doubles) in one copy into hostOut.
-int pg_enqueue(const char* fn, const PgJob& j, char* slab, const char* staged, double* hostOut, int device,
-               cudaStream_t s) {
+int pg_enqueue(const char* fn, PgJob& j, char* slab, const char* staged, double* hostOut, cudaStream_t s) {
+  COSL_TRY(tile_launch_device(j.tile));
   const PgSlab& o = j.o;
   const int N = j.N, nScale = j.nScale, nb = j.P.nb;
   auto at = [&](size_t off) { return slab + off; };
@@ -963,14 +944,15 @@ int pg_enqueue(const char* fn, const PgJob& j, char* slab, const char* staged, d
   d.unitPos = reinterpret_cast<const int*>(at(o.unitPos));
   d.items = reinterpret_cast<const PgItem*>(at(o.items));
   d.itemOff = reinterpret_cast<const int*>(at(o.itemOff));
-  d.diagBlk = reinterpret_cast<const int*>(at(o.diag));
-  d.order = reinterpret_cast<const int*>(at(o.order));
-  d.blkCam0 = reinterpret_cast<const int*>(at(o.blkCam0));
-  d.blkRows = reinterpret_cast<const int*>(at(o.blkRows));
+  const TileLists tl = tile_lists(j.img, at(o.plan));
+  d.diagBlk = tl.diagBlk;
+  d.order = tl.order;
+  d.blkCam0 = tl.blkCam0;
+  d.blkRows = tl.blkRows;
   d.nF = j.nF;
   d.nScale = nScale;
   double* out = reinterpret_cast<double*>(at(o.out));
-  TileSolveBufs b;
+  BaTileDev b = tile_dev(j.P, j.tile, tl);
   b.rhs = reinterpret_cast<double*>(at(o.rhs));
   b.tiles = reinterpret_cast<double*>(at(o.tiles));
   b.rhsS = reinterpret_cast<double*>(at(o.rhsS));
@@ -978,11 +960,7 @@ int pg_enqueue(const char* fn, const PgJob& j, char* slab, const char* staged, d
   b.y = reinterpret_cast<double*>(at(o.y));
   b.x = reinterpret_cast<double*>(at(o.x));
   b.cnt = reinterpret_cast<int*>(at(o.cnt));
-  b.tasks = reinterpret_cast<const BaTask*>(at(o.tasks));
-  b.bwd = reinterpret_cast<const BaBwdEntry*>(at(o.bwd));
-  b.sum = reinterpret_cast<const BaSumEntry*>(at(o.sum));
-  b.blkRows = d.blkRows;
-  b.fail = out + 12 * (size_t)N + nScale;
+  b.sc = out + 12 * (size_t)N + nScale;  // the pivot-failure flag
   double* x1 = reinterpret_cast<double*>(at(o.x1));
   int rc = COSL_OK;
   auto cuda_step = [&](cudaError_t e, const char* what) {
@@ -990,7 +968,7 @@ int pg_enqueue(const char* fn, const PgJob& j, char* slab, const char* staged, d
       rc = set_error(COSL_E_CUDA, "%s: %s: %s", fn, what, cudaGetErrorString(e));
   };
   cuda_step(cudaMemcpyAsync(slab, staged, o.in, cudaMemcpyHostToDevice, s), "H2D");
-  cuda_step(cudaMemsetAsync(b.fail, 0, 16, s), "memset");
+  cuda_step(cudaMemsetAsync(b.sc, 0, 16, s), "memset");
   // Normal equations square the condition number (chains of n free nodes: ~n^2), so the solve is
   // followed by one refinement step: assemble again with the residual A^T (b - A x1) as rhs, solve,
   // x = x1 + x2 (the same step as oracle/posegraph_general_oracle.cpp).
@@ -1002,7 +980,7 @@ int pg_enqueue(const char* fn, const PgJob& j, char* slab, const char* staged, d
     if (rc != COSL_OK) break;
     COSL_LAUNCH(pg_assemble, j.P.nTiles, 256, 0, s, d, pass ? x1 : nullptr, b.tiles, b.rhs);
     cuda_step(cudaGetLastError(), "pg_assemble");
-    if (rc == COSL_OK) rc = tile_solve_launch(j.P, j.nA, b, device, s);
+    if (rc == COSL_OK) rc = tile_solve_enqueue(j.tile, b, s);
   }
   if (rc == COSL_OK) {
     const int nThr = std::max(N, nScale);
@@ -1091,7 +1069,7 @@ extern "C" int cosl_posegraph_solve(int nNodes, const uint8_t* fixed, const doub
     if (e != cudaSuccess) return set_error(COSL_E_CUDA, "%s: cudaMallocAsync: %s", fn, cudaGetErrorString(e));
   }
   std::vector<double> hout(j.nOut);
-  int rc = pg_enqueue(fn, j, slab, host.data(), hout.data(), device, s);
+  int rc = pg_enqueue(fn, j, slab, host.data(), hout.data(), s);
   const cudaError_t e = cudaStreamSynchronize(s);
   if (rc == COSL_OK && e != cudaSuccess) rc = set_error(COSL_E_CUDA, "%s: sync: %s", fn, cudaGetErrorString(e));
   cudaFreeAsync(slab, s);
@@ -1242,7 +1220,7 @@ int cosl_posegraph_solver_submit(cosl_posegraph_solver* s, int nNodes, const uin
   s->N = N;
   s->nScale = nScale;
   return s->rq.submit(fn, [&]() {
-    return j.nF > 0 ? pg_enqueue(fn, j, s->slab, s->h_in, reinterpret_cast<double*>(s->h_out), s->device, s->rq.stream)
+    return j.nF > 0 ? pg_enqueue(fn, j, s->slab, s->h_in, reinterpret_cast<double*>(s->h_out), s->rq.stream)
                     : (int)COSL_OK;
   });
 }
