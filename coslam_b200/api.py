@@ -42,8 +42,9 @@ def _load():
     L.cosl_klt_track.argtypes = [vp, vp, C.c_size_t, vp, pint]
     L.cosl_klt_feed.argtypes = [vp, ci, vp, vp, pint]
     L.cosl_klt_advance.argtypes = [vp]
-    for f in (L.cosl_klt_set_margin, L.cosl_klt_set_conv, L.cosl_klt_set_ssd):
+    for f in (L.cosl_klt_set_margin, L.cosl_klt_set_conv, L.cosl_klt_set_ssd, L.cosl_klt_set_covariance):
         f.argtypes = [vp, cf]
+    L.cosl_klt_group_download_covariance.argtypes = [vp, vp]
     L.cosl_klt_group_next.argtypes = [vp, vp, C.c_size_t, vp, vp]
     L.cosl_klt_group_first.argtypes = [vp, vp, C.c_size_t, vp, vp]
     L.cosl_klt_group_first_present.argtypes = [vp, vp, C.c_size_t, vp, vp, vp, vp]
@@ -488,6 +489,20 @@ class KltGroup:
                 break
             out[name.decode()] = (ms.value, calls.value)
             i += 1
+        return out
+
+    def set_covariance(self, noise_var=0.0):
+        """cosl_klt_set_covariance: arm the position covariance of every tracked slot for the frames
+        enqueued from now on (noise_var > 0: that residual variance; 0: estimated per slot) or disarm
+        it (noise_var < 0)."""
+        _ck(LIB.cosl_klt_set_covariance(self.h, noise_var))
+
+    def download_covariance(self):
+        """cosl_klt_group_download_covariance: (C, F, 3) float32 (xx, xy, yy) in level-0 pixels^2 of
+        the last frame handed out; NaN where no slot was tracked."""
+        out = np.empty((self.C, self.F, 3), np.float32)
+        ptrs = (C.c_void_p * self.C)(*[out[c].ctypes.data for c in range(self.C)])
+        _ck(LIB.cosl_klt_group_download_covariance(self.h, ptrs))
         return out
 
     def pyramid(self, cam, which, level):

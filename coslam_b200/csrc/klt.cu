@@ -13,6 +13,7 @@
 #include "klt_track.cuh"
 #include "klt_front.cuh"
 #include "klt_pyr_tma.cuh"
+#include "klt_cov.cuh"
 
 using namespace coslam;
 
@@ -159,6 +160,19 @@ struct cosl_klt {
   int nInFlight = 0;
   bool havePrev = false;
   KltPrefetch pf;
+  // position covariances of the tracked slots (cosl_klt_set_covariance, klt_cov.cuh).  covNoise < 0:
+  // disarmed, nothing below is allocated or launched.  d_cov [C][F][3] holds the last frame run_frame
+  // computed it for (covFrame); it is read back with the feature table, into h_cov for the synchronous
+  // calls and into h_covQ[slot] for a submitted frame (covQ[slot]: that frame was armed), and copy_out
+  // hands the addressed cameras' entries to covOut, what cosl_klt_group_download_covariance returns
+  // (covHanded: the last frame handed out was armed)
+  float covNoise = -1.f;
+  bool covFrame = false, covHanded = false;
+  bool covQ[2] = {false, false};
+  float* d_cov = nullptr;
+  float* h_cov = nullptr;
+  float* h_covQ[2] = {nullptr, nullptr};
+  std::vector<float> covOut;
   // persistent fused gain tracker (klt_gain_fused)
   float4* d_state = nullptr;             // [C*F]
   unsigned long long* d_ver = nullptr;   // [2][C*F] (pass << 32 | beta bits)
@@ -477,7 +491,10 @@ void free_group(cosl_klt* g) {
     if (g->h_featQ[i]) cudaFreeHost(g->h_featQ[i]);
     if (g->h_cntQ[i]) cudaFreeHost(g->h_cntQ[i]);
     if (g->evDone[i]) cudaEventDestroy(g->evDone[i]);
+    if (g->h_covQ[i]) cudaFreeHost(g->h_covQ[i]);
   }
+  cudaFree(g->d_cov);
+  if (g->h_cov) cudaFreeHost(g->h_cov);
   if (g->stream) cudaStreamDestroy(g->stream);
   delete g;
 }
@@ -728,6 +745,26 @@ int run_tracker(cosl_klt* g, const FramePlan& p) {
   return COSL_OK;
 }
 
+// The position covariances of an armed frame (klt_cov.cuh) into d_cov.  After a tracker it reads the
+// pyramids, the start table d_src and the result d_res that tracker read and wrote, at its last level,
+// so it runs before the fences of p0 / p1 (it is their last reader), before a step's exchange of
+// their slices and before provide or the refill rewrite d_src.  A frame without a tracker leaves
+// every camera NaN.
+static int run_covariance(cosl_klt* g, const FramePlan& p) {
+  if (!p.tracked) {
+    COSL_CUDA(cudaMemsetAsync(g->d_cov, 0xff, sizeof(float) * 3 * g->F * g->C, g->stream));  // NaN
+    return COSL_OK;
+  }
+  const KltLevels LV = tracker_levels(g, false);
+  const int li = LV.n - 1;
+  const KltTrackParams P = track_params(g, true);
+  COSL_LAUNCH(klt_cov, dim3(div_up(g->F, 8), g->C), 256, 0, g->stream, g->d_pyr[g->p0], g->d_pyr[g->p1],
+              g->pyrStride, LV.off[li], LV.w[li], LV.level[li], p.cams, g->d_src, g->d_res, g->d_cov, g->F,
+              g->halfWidth, g->cfg.trackWithGain ? 1 : 0, P.lambda, P.delta, g->covNoise);
+  COSL_CUDA(cudaGetLastError());
+  return COSL_OK;
+}
+
 // KLT_Detector::detectCorners + extractCorners (v3d_gpuklt.cpp:423-588) and the slot logic of
 // detect/redetect (:651-805) on the cornerness map klt_front produced for this frame.  p.detectMode
 // 0: detect (present = the external points of upload_present, p.maxPresent = the longest list),
@@ -772,6 +809,9 @@ int fetch_results(cosl_klt* g) {
                             cudaMemcpyDeviceToHost, g->stream));
   COSL_CUDA(cudaMemcpyAsync(g->h_counters, g->d_counters[g->par], sizeof(int) * 8 * g->C,
                             cudaMemcpyDeviceToHost, g->stream));
+  if (g->covFrame)
+    COSL_CUDA(cudaMemcpyAsync(g->h_cov, g->d_cov, sizeof(float) * 3 * g->F * g->C, cudaMemcpyDeviceToHost,
+                              g->stream));
   COSL_CUDA(cudaStreamSynchronize(g->stream));
   return COSL_OK;
 }
@@ -1052,8 +1092,10 @@ int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_
     if (!p.ops || p.ops[c] != COSL_KLT_OP_SKIP) g->lv0Stored[g->nxt][c] = p.lv0[c];
   g->p1 = g->nxt;
   COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
+  g->covFrame = g->covNoise >= 0.f;
   if (p.tracked) {
     COSL_TRY(run_tracker(g, p));
+    if (g->covFrame) COSL_TRY(run_covariance(g, p));
     if (p.exchangeLate.n) {
       COSL_TRY(exchange_slices(g, p.exchangeLate, 0));
     } else {
@@ -1066,6 +1108,8 @@ int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_
       dim3 grid(div_up(g->F, 256), g->C);
       COSL_LAUNCH(status, grid, 256, 0, g->stream, g->d_res, g->d_feat, counters, g->F, p.cams);
     }
+  } else if (g->covFrame) {
+    COSL_TRY(run_covariance(g, p));
   }
   // provide: the tracked set becomes the feature table of the next frame
   if (p.provideAll) {
@@ -1154,16 +1198,27 @@ static int drop_prefetch(cosl_klt* g) {
 // Camera c's table of `feat` -> dest[c] and its count counters[8c + 2] -> n[c], each where given.
 // ops: the step the tables come from (nullptr: a frame of one kind for every camera): the addressed
 // cameras only, a tracked-only camera's count being its live tracks (counters[8c + 0], what track()
-// returns).
-void copy_out(const cosl_klt* g, const cosl_klt_feature* feat, const int* counters, const uint8_t* ops,
-              cosl_klt_feature* const* dest, int* n) {
+// returns).  cov: the frame's covariances (nullptr: it was not armed), which the addressed cameras'
+// entries of covOut take, as dest[c] takes the table.
+void copy_out(cosl_klt* g, const cosl_klt_feature* feat, const int* counters, const float* cov,
+              const uint8_t* ops, cosl_klt_feature* const* dest, int* n) {
+  bool any = false;
   for (int c = 0; c < g->C; ++c) {
     const int op = ops ? ops[c] : COSL_KLT_OP_NEXT;
     if (op == COSL_KLT_OP_SKIP) continue;
+    any = true;
     if (dest && dest[c]) std::memcpy(dest[c], feat + (size_t)c * g->F, sizeof(cosl_klt_feature) * g->F);
     if (n) n[c] = counters[8 * c + (op == COSL_KLT_OP_TRACK ? 0 : 2)];
+    if (cov) {
+      const size_t o = (size_t)3 * c * g->F;
+      std::memcpy(g->covOut.data() + o, cov + o, sizeof(float) * 3 * g->F);
+    }
   }
+  if (any) g->covHanded = cov != nullptr;
 }
+
+// the synchronous calls' covariances (fetch_results): those of the last frame run, if it was armed
+const float* sync_cov(const cosl_klt* g) { return g->covFrame ? g->h_cov : nullptr; }
 
 }  // namespace
 
@@ -1300,7 +1355,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_DETECT, maxPresent, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nDetected);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, &dest, nDetected);
   return COSL_OK;
 }
 
@@ -1313,7 +1368,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nNewFeatures);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, &dest, nNewFeatures);
   return COSL_OK;
 }
 
@@ -1326,7 +1381,7 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_TRACK, 0, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, nullptr, &dest, nullptr);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, &dest, nullptr);
   *nPresent = h->h_counters[0];
   return COSL_OK;
 }
@@ -1363,6 +1418,33 @@ int cosl_klt_set_ssd(cosl_klt* h, float t) {
   return COSL_OK;
 }
 
+// The buffers are made on the first arming and kept when the group is disarmed.
+int cosl_klt_set_covariance(cosl_klt* h, float noise_var) {
+  KLT_ENTER(h)
+  if (!std::isfinite(noise_var)) return set_error(COSL_E_INVALID, "set_covariance: noise_var is not finite");
+  if (noise_var >= 0.f && !h->d_cov) {
+    const size_t n = (size_t)3 * h->F * h->C;
+    COSL_CUDA(cudaMalloc(&h->d_cov, sizeof(float) * n));
+    COSL_CUDA(cudaMallocHost(&h->h_cov, sizeof(float) * n));
+    for (int i = 0; i < 2; ++i) COSL_CUDA(cudaMallocHost(&h->h_covQ[i], sizeof(float) * n));
+    h->covOut.assign(n, std::nanf(""));
+  }
+  h->covNoise = noise_var >= 0.f ? noise_var : -1.f;
+  return COSL_OK;
+}
+
+int cosl_klt_group_download_covariance(cosl_klt* h, float* const* cov) {
+  KLT_ENTER(h)
+  if (!cov) return set_error(COSL_E_INVALID, "group_download_covariance: null argument");
+  if (!h->covHanded)
+    return set_error(COSL_E_STATE, "group_download_covariance: the last frame handed out was not armed "
+                                   "(cosl_klt_set_covariance)");
+  for (int c = 0; c < h->C; ++c)
+    if (cov[c])
+      std::memcpy(cov[c], h->covOut.data() + (size_t)3 * c * h->F, sizeof(float) * 3 * h->F);
+  return COSL_OK;
+}
+
 #define KLT_NOT_IN_FLIGHT(h, name) \
   if ((h)->nInFlight > 0) return set_error(COSL_E_STATE, name ": submitted frames not yet collected");
 
@@ -1374,7 +1456,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
   if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_DETECT, maxPresent, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, nullptr, dest, nDetected);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, dest, nDetected);
   return COSL_OK;
 }
 
@@ -1427,7 +1509,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, nullptr, dest, nNew);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, dest, nNew);
   return COSL_OK;
 }
 
@@ -1459,7 +1541,7 @@ int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* i
   COSL_TRY(check_step(h, ops, imgs, pitch, "group_step"));
   COSL_TRY(run_step(h, ops, imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, ops, dest, n);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), ops, dest, n);
   return COSL_OK;
 }
 
@@ -1474,7 +1556,7 @@ int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* cons
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, h->stepOpsValid ? h->stepOps : nullptr, dest, nNew);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), h->stepOpsValid ? h->stepOps : nullptr, dest, nNew);
   return COSL_OK;
 }
 
@@ -1510,6 +1592,10 @@ static int submit_readback(cosl_klt* h, int slot) {
     COSL_CUDA(cudaMemcpyAsync(h->h_cntQ[slot], h->d_counters[h->par], sizeof(int) * 8 * h->C,
                               cudaMemcpyDeviceToHost, h->stream));
   }
+  h->covQ[slot] = any && h->covFrame;
+  if (h->covQ[slot])
+    COSL_CUDA(cudaMemcpyAsync(h->h_covQ[slot], h->d_cov, sizeof(float) * 3 * h->F * h->C, cudaMemcpyDeviceToHost,
+                              h->stream));
   COSL_CUDA(cudaEventRecord(h->evDone[slot], h->stream));
   ++h->subSeq;
   ++h->nInFlight;
@@ -1548,7 +1634,8 @@ int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew
   const int slot = (int)((h->subSeq - (unsigned)h->nInFlight) & 1u);
   COSL_CUDA(cudaEventSynchronize(h->evDone[slot]));
   --h->nInFlight;
-  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], h->opsQ[slot], dest, nNew);
+  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], h->covQ[slot] ? h->h_covQ[slot] : nullptr, h->opsQ[slot], dest,
+           nNew);
   return COSL_OK;
 }
 
@@ -1596,7 +1683,7 @@ int cosl_klt_group_run_prefetched(cosl_klt* h, cosl_klt_feature* const* dest, in
   if (h->pf.step) KLT_NOT_IN_FLIGHT(h, "group_run_prefetched")
   COSL_TRY(consume_prefetch(h));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, h->pf.step ? h->pf.ops : nullptr, dest, n);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), h->pf.step ? h->pf.ops : nullptr, dest, n);
   return COSL_OK;
 }
 

@@ -150,6 +150,27 @@ int cosl_klt_advance(cosl_klt* h);
 int cosl_klt_set_margin(cosl_klt* h, float margin);
 int cosl_klt_set_conv(cosl_klt* h, float thr);
 int cosl_klt_set_ssd(cosl_klt* h, float thr);
+/* Extension: the 2x2 position covariance of every tracked feature (DESIGN.md section 3.4), the
+ * measurement covariance cosl_ba_solver_set_obs_cov / cosl_sba_motstr_levmar_x_cov take.  For each
+ * slot with status 0 in a frame where its camera ran the tracker, at the tracker's last level L:
+ *   M = J^T J of the tracker's window at the returned position and gain (the gain tracker's 3x3 system
+ *       with its gain prior, the neighbour gains fixed; the 2x2 tracker's data matrix),
+ *   sigma^2 = noise_var, or SSD / (npx - k) of the window residual when noise_var == 0 (k = 3 with
+ *       gain, 2 without; npx = window pixels),
+ *   cov = sigma^2 diag(W_c, H_c) [M^-1]_position diag(W_c, H_c), level-0 pixels^2 of camera c.
+ * noise_var > 0: fixed residual variance, in the pyramid's intensity units; 0: estimated per slot;
+ * < 0: disarmed (the default: nothing is computed and the group launches exactly what it launches
+ * without this call).  NaN or inf gives COSL_E_INVALID.  Like cosl_klt_set_ssd it applies to the
+ * frames enqueued after the call; a pending prefetch takes it when it is consumed.  An armed frame
+ * adds one kernel after the tracker and one D2H copy of C * featW * featH * 3 floats. */
+int cosl_klt_set_covariance(cosl_klt* h, float noise_var);
+/* The covariances of the last frame handed out (by next, step, track, redetect, detect, first*,
+ * run_prefetched, collect or fetch): cov[c] (may be NULL: not written) receives featW * featH
+ * (xx, xy, yy) float triples, slot-major.  NaN for a slot that is not tracked (status != 0), whose
+ * normal matrix is singular, and for every slot of a camera that frame addressed with FIRST / detect;
+ * a camera the frame skipped keeps the entries it had, as its dest[c] does.  COSL_E_STATE when the
+ * last frame handed out was not armed, or none was. */
+int cosl_klt_group_download_covariance(cosl_klt* h, float* const* cov);
 
 /* Extension (batched GPUKLT::next, tracking/GPUKLT.cpp:144-161): redetect + advanceFrame for all
  * cameras of the group.  imgs[c] are HOST pointers (pinned memory recommended); dest[c] has
