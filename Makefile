@@ -24,10 +24,12 @@ $(LIB): $(OBJS)
 oracle:
 	$(MAKE) -s -C oracle
 	$(MAKE) -s -C oracle -f Makefile.pg_general
+	$(MAKE) -s -C oracle -f Makefile.obscov
 
 clean:
 	rm -f $(CSRC)/*.o $(CSRC)/*.ptxas.log $(LIB)
 	$(MAKE) -C oracle clean
 	$(MAKE) -C oracle -f Makefile.pg_general clean
+	$(MAKE) -C oracle -f Makefile.obscov clean
 
 .PHONY: all oracle clean

@@ -79,6 +79,7 @@ def _load():
     L.cosl_pose_solver_create.argtypes = [ci, ci, ci, C.POINTER(vp)]
     L.cosl_pose_solver_destroy.argtypes = [vp]
     L.cosl_pose_solver_submit.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, cd, vp]
+    L.cosl_pose_solver_submit_cov.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, cd, vp]
     L.cosl_pose_solver_query.argtypes = [vp, pint]
     L.cosl_pose_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
     L.cosl_pose_solver_stream.argtypes = [vp]
@@ -600,11 +601,20 @@ class PoseSolver(_SolverHandle):
         self._opts = None
         self._npts = []  # points per camera of the last accepted submit: the shapes download_covariance returns
 
-    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None):
+    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, covx=None):
         """cosl_pose_solver_submit: enqueue pose_intracam_batch's solve and return at once; the input arrays
-        may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills."""
+        may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills.
+        covx, a list of per-camera [n, 2, 2] or [n, 4] measurement covariances (px^2, in the order of ms_list;
+        None entries for identity), weights the solve through cosl_pose_solver_submit_cov."""
         args, opts, keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
-        _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
+        if covx is None:
+            _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
+        else:
+            if len(covx) != args[0]:
+                raise ValueError(f"covx has {len(covx)} cameras for {args[0]}")
+            covx = [None if a is None else _obs_cov(a, len(keep[3][c])) for c, a in enumerate(covx)]
+            cp = (C.c_void_p * args[0])(*[None if a is None else a.ctypes.data for a in covx])
+            _ck(LIB.cosl_pose_solver_submit_cov(self.h, *args[:7], cp, *args[7:], opts))
         self._opts = opts
         self._npts = [len(a) for a in keep[3]]
 

@@ -152,23 +152,38 @@ __device__ bool inv6(const double A[36], double Ainv[36]) {
   return true;
 }
 
+// r <- L r with the upper-triangular whitening factor L = {l00, l01, l11} of a point's measurement covariance
+// (cosl_pose_solver_submit_cov).  With L = {1, -0, 1} and no fused multiply-add this is the identity, bit for bit.
+__device__ __forceinline__ void whiten(const double* L, double& r0, double& r1) {
+  r0 = L[0] * r0 + L[1] * r1;
+  r1 = L[2] * r1;
+}
+
+// The factor pointer of a pose_cov_kernel<true> launch, its one trailing argument.
+__device__ __forceinline__ const double* factors_arg() { return nullptr; }
+__device__ __forceinline__ const double* factors_arg(const double* L) { return L; }
+
+// intraCamWeightedCost (:439-456); OBSCOV whitens each residual by Ls (3 per point) before the weight
+template <bool OBSCOV>
 __device__ double weighted_cost(const double K[9], const double R[9], const double t[3], int n,
-                                const double* Ws, const double* Ms, const double* ms,
+                                const double* Ws, const double* Ms, const double* ms, const double* Ls,
                                 double* s_red) {
   double err[1] = {0};
   for (int i = threadIdx.x; i < n; i += POSE_THREADS) {
     double rm[2];
     project(K, R, t, Ms + 3 * i, rm);
-    const double dx = ms[2 * i] - rm[0], dy = ms[2 * i + 1] - rm[1];
+    double dx = ms[2 * i] - rm[0], dy = ms[2 * i + 1] - rm[1];
+    if (OBSCOV) whiten(Ls + 3 * i, dx, dy);
     err[0] += (dx * dx + dy * dy) * Ws[i];
   }
   block_sum<1>(err, s_red);
   return err[0];
 }
 
-// intraCamWeightedLMStep (:259-303)
+// intraCamWeightedLMStep (:259-303); OBSCOV whitens the residual and both Jacobian rows by Ls before the weight
+template <bool OBSCOV>
 __device__ void weighted_step(const double K[9], const double R[9], const double t[3], int n,
-                              const double* Ws, const double* Ms, const double* ms,
+                              const double* Ws, const double* Ms, const double* ms, const double* Ls,
                               double param[6], double lambda, const double dRk[3][9],
                               double* s_red) {
   const double eps = 1e-8;
@@ -195,11 +210,17 @@ __device__ void weighted_step(const double K[9], const double R[9], const double
       J[3 + k] = (rm[0] - rm0[0]) / eps;
       J[9 + k] = (rm[1] - rm0[1]) / eps;
     }
+    if (OBSCOV) {
+#pragma unroll
+      for (int k = 0; k < 6; ++k) whiten(Ls + 3 * i, J[k], J[6 + k]);
+    }
     const double w = Ws[i];
 #pragma unroll
     for (int k = 0; k < 12; ++k) J[k] = w * J[k];
-    const double r0 = (-rm0[0] + ms[2 * i]) * w;
-    const double r1 = (-rm0[1] + ms[2 * i + 1]) * w;
+    double r0 = -rm0[0] + ms[2 * i], r1 = -rm0[1] + ms[2 * i + 1];
+    if (OBSCOV) whiten(Ls + 3 * i, r0, r1);
+    r0 = r0 * w;
+    r1 = r1 * w;
     int q = 0;
 #pragma unroll
     for (int a = 0; a < 6; ++a) {
@@ -230,15 +251,20 @@ __device__ void weighted_step(const double K[9], const double R[9], const double
   }
 }
 
+// OBSCOV: every residual and Jacobian row is whitened by the factors LAll (3 per point, packed as the points;
+// cosl_pose_solver_submit_cov).  The false instantiation never reads LAll and is the unweighted solve.
+template <bool OBSCOV>
 __global__ void __launch_bounds__(POSE_THREADS)
 pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
                      const double* __restrict__ msAll, const double* __restrict__ prevAll,
-                     double* __restrict__ WsAll, PoseCfg cfg, PoseOut* __restrict__ outs) {
+                     double* __restrict__ WsAll, PoseCfg cfg, PoseOut* __restrict__ outs,
+                     const double* __restrict__ LAll) {
   __shared__ double s_red[(POSE_THREADS / 32) * 27];
   const PoseCam cam = cams[blockIdx.x];
   const int n = cam.npts;
   const double* Ms = MsAll + 3 * cam.off;
   const double* ms = msAll + 2 * cam.off;
+  const double* Ls = OBSCOV ? LAll + 3 * cam.off : nullptr;
   double* Ws = WsAll + cam.off;
   const double tau = cfg.tau;
   double K[9], R[9], t[3], R_opt[9], t_opt[3], R_tmp[9], t_tmp[3], Rlm[9], tlm[3];
@@ -269,7 +295,7 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
     // ---- intraCamWeightedLMProc (:475-549) from (R, t) ----
     double param[6];
     lambda = lambda0;
-    err0 = weighted_cost(K, R, t, n, Ws, Ms, ms, s_red);
+    err0 = weighted_cost<OBSCOV>(K, R, t, n, Ws, Ms, ms, Ls, s_red);
     errLM = err0;
     for (int q = 0; q < 9; ++q) {
       Rlm[q] = R[q];
@@ -283,7 +309,7 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
     int i = 0;
     double err = err0;
     for (; i < cfg.maxIterLM; ++i) {
-      weighted_step(K, Rlm, tlm, n, Ws, Ms, ms, param, lambda, dRk, s_red);
+      weighted_step<OBSCOV>(K, Rlm, tlm, n, Ws, Ms, ms, Ls, param, lambda, dRk, s_red);
       {  // intraCamUpdatePose (:367-380)
         double dR[9];
         so3_exp(param, dR);
@@ -300,7 +326,7 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
         retType = 0;
         break;
       }
-      err = weighted_cost(K, R_opt, t_opt, n, Ws, Ms, ms, s_red);
+      err = weighted_cost<OBSCOV>(K, R_opt, t_opt, n, Ws, Ms, ms, Ls, s_red);
       if (fabs(err - errLM) < cfg.epsErr) {
         retType = 0;
         break;
@@ -384,10 +410,16 @@ constexpr int POSE_COV_STRIDE = 40;
 // res[c] gets cov | {sigma2_hat = sum w e^2 / dof (NaN for dof <= 0), dof = 2 #(w > 0) - 6, the smallest
 // relative pivot L_kk^2 / H_kk (0 when the factorisation breaks down), valid}; a break-down or a relative pivot
 // below 1e-12 gives a NaN covariance and valid = 0.  errAll gets e_i of every point, in the packed order.
+// OBSCOV (cosl_pose_solver_submit_cov) whitens by the factors L_i of LAll: H = sum_i w_i (L_i J_i)^T (L_i J_i) and
+// sigma2_hat = sum w |L_i (project - m_i)|^2 / dof; e_i and w_i stay on the pixel distance.
+// The factors travel as a trailing argument of the OBSCOV launch only: the unweighted kernel keeps the parameter
+// list it had before measurement covariances, and with it its code (an unused parameter changes its registers).
+template <bool OBSCOV, typename... Factors>
 __global__ void __launch_bounds__(POSE_THREADS)
 pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
                 const double* __restrict__ msAll, const PoseOut* __restrict__ outs, double tau, double pixel_var,
-                double* __restrict__ res, double* __restrict__ errAll) {
+                double* __restrict__ res, double* __restrict__ errAll, Factors... LAll) {
+  static_assert(sizeof...(Factors) == (OBSCOV ? 1 : 0), "an OBSCOV launch passes the factors, no other does");
   __shared__ double s_red[(POSE_THREADS / 32) * 23];
   const PoseCam& cam = cams[blockIdx.x];
   const int n = cam.npts;
@@ -433,13 +465,22 @@ pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsA
         J[6 * r + 1] = M[2] * q0 - M[0] * q2;
         J[6 * r + 2] = M[0] * q1 - M[1] * q0;
       }
+      double ew = 0;  // |L (project - m)|, which is e bit for bit when L = I
+      if (OBSCOV) {
+        const double* L = factors_arg(LAll...) + 3 * (cam.off + i);
+        double r0 = dx, r1 = dy;
+        whiten(L, r0, r1);
+        ew = sqrt(r0 * r0 + r1 * r1);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) whiten(L, J[k], J[6 + k]);
+      }
       int q = 0;
 #pragma unroll
       for (int a = 0; a < 6; ++a) {
 #pragma unroll
         for (int b = a; b < 6; ++b) acc[q++] += w * (J[a] * J[b] + J[6 + a] * J[6 + b]);
       }
-      acc[21] += w * (e * e);
+      acc[21] += w * (OBSCOV ? ew * ew : e * e);
       acc[22] += 1;
     }
   }
@@ -508,6 +549,7 @@ pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsA
   r[39] = valid ? 1.0 : 0.0;
 }
 
+
 // Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
 // cameras.
 int check_cameras(const char* fn, int C, const int* npts, const double* const* Ms, const double* const* ms,
@@ -531,12 +573,45 @@ int check_cameras(const char* fn, int C, const int* npts, const double* const* M
   return COSL_OK;
 }
 
+// The whitening factor of one measurement covariance c = [a b; b c'] (row-major, px^2): the upper-triangular
+// L = {sqrt(c'/det), -b/sqrt(c' det), 1/sqrt(c')} with L^T L = c^-1, det = a c' - b^2.  False unless c is finite,
+// exactly symmetric, a > 0, det > 0 and L comes out finite.
+bool cov_factor(const double* c, double L[3]) {
+  if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !std::isfinite(c[2]) || !std::isfinite(c[3])) return false;
+  if (c[1] != c[2] || !(c[0] > 0)) return false;
+  const double det = c[0] * c[3] - c[1] * c[1];
+  if (!(det > 0)) return false;
+  L[0] = std::sqrt(c[3] / det);
+  L[1] = -c[1] / std::sqrt(c[3] * det);
+  L[2] = 1.0 / std::sqrt(c[3]);
+  return std::isfinite(L[0]) && std::isfinite(L[1]) && std::isfinite(L[2]) && L[0] > 0 && L[2] > 0;
+}
+
+// Checks every covariance of covx (nullable, as covx[c]) against cov_factor, naming the first bad one.
+int check_covx(const char* fn, int C, const int* npts, const double* const* covx) {
+  if (!covx) return COSL_OK;
+  for (int c = 0; c < C; ++c) {
+    if (!covx[c]) continue;
+    for (int i = 0; i < npts[c]; ++i) {
+      double L[3];
+      const double* v = covx[c] + 4 * (size_t)i;
+      if (!cov_factor(v, L))
+        return set_error(COSL_E_INVALID,
+                         "%s: covariance of camera %d point %d [%g %g; %g %g] is not finite, symmetric and positive "
+                         "definite",
+                         fn, c, i, v[0], v[1], v[2], v[3]);
+    }
+  }
+  return COSL_OK;
+}
+
 }  // namespace
 
 // A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out as
-// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] (tot = points of the solve); the PoseOuts come back into
-// pinned memory.  Capacity is fixed at create: everything is allocated once, the covariance stage's buffers
-// (laid out as res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed.
+// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] | L[3 tot] (tot = points of the solve; the whitening factors L
+// are staged and copied by cosl_pose_solver_submit_cov only); the PoseOuts come back into pinned memory.  Capacity
+// is fixed at create: everything is allocated once, the covariance stage's buffers (laid out as
+// res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed.
 struct cosl_pose_solver {
   int device = 0, maxCams = 0, maxPts = 0;
   RequestStream rq;
@@ -551,11 +626,14 @@ struct cosl_pose_solver {
   double* d_cov = nullptr;
   double* h_cov = nullptr;
   bool covReady = false;  // the last submitted solve was armed
+  bool obsCov = false;    // the solve in flight carries measurement covariances
 };
 
 namespace {
 
 size_t input_bytes(int C, long long tot) { return sizeof(PoseCam) * C + sizeof(double) * 6 * tot; }
+// the staged inputs followed by the whitening factors of cosl_pose_solver_submit_cov
+size_t input_bytes_cov(int C, long long tot) { return input_bytes(C, tot) + sizeof(double) * 3 * tot; }
 
 void free_pose_solver(cosl_pose_solver* s) {
   cudaSetDevice(s->device);
@@ -575,7 +653,7 @@ size_t cov_doubles(int C, long long tot) { return (size_t)POSE_COV_STRIDE * C + 
 int alloc_pose_solver(cosl_pose_solver* s) {
   COSL_CUDA(cudaSetDevice(s->device));
   COSL_TRY(s->rq.create());
-  const size_t in = input_bytes(s->maxCams, s->maxPts);
+  const size_t in = input_bytes_cov(s->maxCams, s->maxPts);
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
   COSL_CUDA(cudaHostAlloc(&s->h_out, sizeof(PoseOut) * s->maxCams, cudaHostAllocPortable));
   COSL_CUDA(cudaMalloc(&s->d_in, in));
@@ -584,23 +662,104 @@ int alloc_pose_solver(cosl_pose_solver* s) {
   return COSL_OK;
 }
 
-// The staged inputs of C cameras and tot points: copy, kernel, read-back.
+// The staged inputs of C cameras and tot points: copy, kernel, read-back.  s->obsCov selects the whitened
+// instantiations and copies the factors with the rest.
 int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg) {
   const PoseCam* d_cams = reinterpret_cast<const PoseCam*>(s->d_in);
   const double* d_M = reinterpret_cast<const double*>(s->d_in + sizeof(PoseCam) * C);
   const double* d_m = d_M + 3 * tot;
   const double* d_p = d_m + 2 * tot;
+  const double* d_L = d_p + tot;
   cudaStream_t st = s->rq.stream;
-  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, input_bytes(C, tot), cudaMemcpyHostToDevice, st));
-  COSL_LAUNCH(pose_intracam_kernel, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out);
+  const size_t bytes = s->obsCov ? input_bytes_cov(C, tot) : input_bytes(C, tot);
+  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, bytes, cudaMemcpyHostToDevice, st));
+  if (s->obsCov)
+    COSL_LAUNCH(pose_intracam_kernel<true>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out,
+                d_L);
+  else
+    COSL_LAUNCH(pose_intracam_kernel<false>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out,
+                nullptr);
   COSL_CUDA(cudaGetLastError());
   COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, st));
   if (s->pixelVar > 0) {
-    COSL_LAUNCH(pose_cov_kernel, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar, s->d_cov,
-                s->d_cov + POSE_COV_STRIDE * C);
+    double* d_res = s->d_cov;
+    double* d_err = s->d_cov + POSE_COV_STRIDE * C;
+    if (s->obsCov)
+      COSL_LAUNCH(pose_cov_kernel<true>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar,
+                  d_res, d_err, d_L);
+    else
+      COSL_LAUNCH(pose_cov_kernel<false>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar,
+                  d_res, d_err);
     COSL_CUDA(cudaGetLastError());
     COSL_CUDA(cudaMemcpyAsync(s->h_cov, s->d_cov, sizeof(double) * cov_doubles(C, tot), cudaMemcpyDeviceToHost, st));
   }
+  return COSL_OK;
+}
+
+// cosl_pose_solver_submit (covx == nullptr) and cosl_pose_solver_submit_cov; fn names the caller in messages.
+int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
+                 const int* npts, const double* const* Ms, const double* const* ms, const double* const* covx,
+                 const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  COSL_TRY(s->rq.idle(fn));
+  if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !opts)
+    return set_error(COSL_E_INVALID, "%s: null argument", fn);
+  if (C > s->maxCams)
+    return set_error(COSL_E_INVALID, "%s: %d cameras exceed the handle's %d", fn, C, s->maxCams);
+  long long tot = 0;
+  COSL_TRY(check_cameras(fn, C, npts, Ms, ms, opts, &tot));
+  if (tot > s->maxPts)
+    return set_error(COSL_E_INVALID, "%s: %lld points exceed the handle's %d", fn, tot, s->maxPts);
+  COSL_TRY(check_covx(fn, C, npts, covx));
+  COSL_CUDA(cudaSetDevice(s->device));
+  // nothing is in flight, so no copy reads the staging buffer any more
+  PoseCam* cams = reinterpret_cast<PoseCam*>(s->h_in);
+  double* hM = reinterpret_cast<double*>(s->h_in + sizeof(PoseCam) * C);
+  double* hm = hM + 3 * tot;
+  double* hp = hm + 2 * tot;
+  double* hL = hp + tot;
+  long long off = 0;
+  for (int c = 0; c < C; ++c) {
+    std::memcpy(cams[c].K, K9 + 9 * c, sizeof(double) * 9);
+    std::memcpy(cams[c].R0, R0 + 9 * c, sizeof(double) * 9);
+    std::memcpy(cams[c].t0, t0 + 3 * c, sizeof(double) * 3);
+    cams[c].npts = npts[c];
+    cams[c].hasPrev = (prevErrs && prevErrs[c]) ? 1 : 0;
+    cams[c].off = off;
+    if (npts[c]) {
+      std::memcpy(hM + 3 * off, Ms[c], sizeof(double) * 3 * npts[c]);
+      std::memcpy(hm + 2 * off, ms[c], sizeof(double) * 2 * npts[c]);
+      // a camera without prevErrs leaves its slice unset: the kernel does not read it
+      if (cams[c].hasPrev) std::memcpy(hp + off, prevErrs[c], sizeof(double) * npts[c]);
+      // a camera without covariances gets the identity factor {1, -0, 1}, whitening it bit for bit to nothing
+      if (covx)
+        for (int i = 0; i < npts[c]; ++i) {
+          double* L = hL + 3 * (off + i);
+          if (covx[c]) {
+            cov_factor(covx[c] + 4 * (size_t)i, L);
+          } else {
+            L[0] = 1.0;
+            L[1] = -0.0;
+            L[2] = 1.0;
+          }
+        }
+    }
+    off += npts[c];
+  }
+  PoseCfg cfg;
+  cfg.maxIterLM = opts[0].maxIterLM;
+  cfg.maxIterRW = opts[0].maxIterRW;
+  cfg.epsErr = opts[0].epsErrorChangeLM;
+  cfg.epsParam = opts[0].epsParamChangeLM;
+  cfg.epsRW = opts[0].epsErrorChangeRW;
+  cfg.lambda0 = opts[0].lambda0;
+  cfg.tau = tau;
+  s->C = C;
+  s->tot = tot;
+  s->covReady = false;
+  s->obsCov = covx != nullptr;
+  COSL_TRY(s->rq.submit(fn, [&]() { return enqueue_solve(s, C, tot, cfg); }));
+  s->covReady = s->pixelVar > 0;
   return COSL_OK;
 }
 
@@ -647,52 +806,14 @@ int cosl_pose_solver_destroy(cosl_pose_solver* s) {
 int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
                             const int* npts, const double* const* Ms, const double* const* ms,
                             const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
-  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
-  COSL_TRY(s->rq.idle("cosl_pose_solver_submit"));
-  if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !opts)
-    return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: null argument");
-  if (C > s->maxCams)
-    return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: %d cameras exceed the handle's %d", C, s->maxCams);
-  long long tot = 0;
-  COSL_TRY(check_cameras("cosl_pose_solver_submit", C, npts, Ms, ms, opts, &tot));
-  if (tot > s->maxPts)
-    return set_error(COSL_E_INVALID, "cosl_pose_solver_submit: %lld points exceed the handle's %d", tot, s->maxPts);
-  COSL_CUDA(cudaSetDevice(s->device));
-  // nothing is in flight, so no copy reads the staging buffer any more
-  PoseCam* cams = reinterpret_cast<PoseCam*>(s->h_in);
-  double* hM = reinterpret_cast<double*>(s->h_in + sizeof(PoseCam) * C);
-  double* hm = hM + 3 * tot;
-  double* hp = hm + 2 * tot;
-  long long off = 0;
-  for (int c = 0; c < C; ++c) {
-    std::memcpy(cams[c].K, K9 + 9 * c, sizeof(double) * 9);
-    std::memcpy(cams[c].R0, R0 + 9 * c, sizeof(double) * 9);
-    std::memcpy(cams[c].t0, t0 + 3 * c, sizeof(double) * 3);
-    cams[c].npts = npts[c];
-    cams[c].hasPrev = (prevErrs && prevErrs[c]) ? 1 : 0;
-    cams[c].off = off;
-    if (npts[c]) {
-      std::memcpy(hM + 3 * off, Ms[c], sizeof(double) * 3 * npts[c]);
-      std::memcpy(hm + 2 * off, ms[c], sizeof(double) * 2 * npts[c]);
-      // a camera without prevErrs leaves its slice unset: the kernel does not read it
-      if (cams[c].hasPrev) std::memcpy(hp + off, prevErrs[c], sizeof(double) * npts[c]);
-    }
-    off += npts[c];
-  }
-  PoseCfg cfg;
-  cfg.maxIterLM = opts[0].maxIterLM;
-  cfg.maxIterRW = opts[0].maxIterRW;
-  cfg.epsErr = opts[0].epsErrorChangeLM;
-  cfg.epsParam = opts[0].epsParamChangeLM;
-  cfg.epsRW = opts[0].epsErrorChangeRW;
-  cfg.lambda0 = opts[0].lambda0;
-  cfg.tau = tau;
-  s->C = C;
-  s->tot = tot;
-  s->covReady = false;
-  COSL_TRY(s->rq.submit("cosl_pose_solver_submit", [&]() { return enqueue_solve(s, C, tot, cfg); }));
-  s->covReady = s->pixelVar > 0;
-  return COSL_OK;
+  return submit_solve("cosl_pose_solver_submit", s, C, K9, R0, t0, npts, Ms, ms, nullptr, prevErrs, tau, opts);
+}
+
+int cosl_pose_solver_submit_cov(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
+                                const int* npts, const double* const* Ms, const double* const* ms,
+                                const double* const* covx, const double* const* prevErrs, double tau,
+                                const cosl_pose_opt* opts) {
+  return submit_solve("cosl_pose_solver_submit_cov", s, C, K9, R0, t0, npts, Ms, ms, covx, prevErrs, tau, opts);
 }
 
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done) {

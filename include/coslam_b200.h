@@ -399,6 +399,31 @@ int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const 
                             const double* t0, const int* npts, const double* const* Ms,
                             const double* const* ms, const double* const* prevErrs, double tau,
                             const cosl_pose_opt* opts);
+/* submit with 2x2 measurement covariances (an extension: the reference's covariance-weighted solve,
+ * intraCamCovEstimate, builds them from the map points instead; DESIGN.md 5.2).  covx[c] holds npts[c]
+ * row-major covariances [xx, xy, yx, yy] in px^2, in the order of ms[c]; covx == NULL or covx[c] == NULL
+ * means identity covariances for that camera.  Per point, with Sigma = [a b; b c] and det = ac - b^2,
+ * the upper-triangular whitening factor
+ *   L = [sqrt(c/det), -b/sqrt(c det); 0, 1/sqrt(c)],  L^T L = Sigma^-1,
+ * is computed on the calling thread (Sigma = I gives exactly L = I, Sigma = 4I exactly 0.5 I) and:
+ *   the residual is r~ = L (m - pi(K, R, t, M)) and the rows of the forward-difference Jacobian are
+ *   whitened by the same L; the cost is sum w |r~|^2; the LM step is that of cosl_pose_intracam_batch
+ *   (rows scaled by w) on the whitened rows, lambda added to the whitened system's diagonal;
+ *   the Tukey weights w (from prevErrs and from every re-weighting) stay on the Euclidean pixel
+ *   distance |m - pi| against tau;
+ *   opts[c].err0, err and errRW are whitened costs.
+ * An armed handle's covariance stage uses the same L: H = sum w (L J)^T (L J) with the analytic J,
+ * sigma2_hat = sum w |L e|^2 / dof, cov = pixel_var H^-1 (so covariances in px^2 arm with pixel_var
+ * = 1); download_covariance's err stays the pixel distance |e|.
+ * Every covariance must be finite with xy == yx exactly, xx > 0 and det > 0 (and a finite L), else
+ * COSL_E_INVALID naming the first bad camera and point, before anything is staged; the handle stays
+ * usable.  Everything else is cosl_pose_solver_submit's: its checks and codes, COSL_E_STATE while a
+ * solve is in flight, and query, collect and download_covariance.  cosl_pose_solver_submit is this
+ * call with covx = NULL, and runs the unweighted kernels. */
+int cosl_pose_solver_submit_cov(cosl_pose_solver* s, int C, const double* K9, const double* R0,
+                                const double* t0, const int* npts, const double* const* Ms,
+                                const double* const* ms, const double* const* covx,
+                                const double* const* prevErrs, double tau, const cosl_pose_opt* opts);
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done);
 int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, cosl_pose_opt* opts,
                              int* ok, double* device_ms);
