@@ -108,6 +108,7 @@ def _load():
     L.cosl_ba_solver_set_covariance.argtypes = [vp, cd]
     L.cosl_ba_solver_download_covariance.argtypes = [vp, vp, vp, C.POINTER(cd)]
     L.cosl_ba_solver_set_obs_cov.argtypes = [vp, vp]
+    L.cosl_ba_solver_set_cam_prior.argtypes = [vp, ci, vp, vp, vp, vp]
     L.cosl_ba_solver_download.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_destroy.argtypes = [vp]
     L.cosl_ba_solver_stream.argtypes = [vp]
@@ -919,6 +920,24 @@ class BaSolver(_SolverHandle):
         c = _obs_cov(covx, int(self.prob.nobs))
         _ck(LIB.cosl_ba_solver_set_obs_cov(self.h, _ptr(c)))
 
+    def set_cam_prior(self, cams, R=None, t=None, cov=None):
+        """cosl_ba_solver_set_cam_prior: Gaussian priors on free cameras cams [k] with means R [k, 3, 3], t [k, 3]
+        and covariances cov [k, 6, 6] for (w, t) in the chart of download_covariance's camCov, in the units of the
+        objective (a camCov of an earlier BA in px^2 as it stands; camCov / s2 for unweighted observations of
+        pixel variance s2).  They apply to every later run / run_fixed / submit; None (or no cameras) clears.
+        load() clears them, reset() keeps them."""
+        if cams is None or len(cams) == 0:
+            _ck(LIB.cosl_ba_solver_set_cam_prior(self.h, 0, None, None, None, None))
+            return
+        cams = np.ascontiguousarray(cams, np.int32).reshape(-1)
+        k = len(cams)
+        R = np.ascontiguousarray(R, np.float64).reshape(-1, 9)
+        t = np.ascontiguousarray(t, np.float64).reshape(-1, 3)
+        cov = np.ascontiguousarray(cov, np.float64).reshape(-1, 36)
+        if len(R) != k or len(t) != k or len(cov) != k:
+            raise ValueError(f"set_cam_prior: {k} cameras but {len(R)} R, {len(t)} t and {len(cov)} cov")
+        _ck(LIB.cosl_ba_solver_set_cam_prior(self.h, k, _ptr(cams), _ptr(R), _ptr(t), _ptr(cov)))
+
     def download_covariance(self):
         """cosl_ba_solver_download_covariance: (camCov [m, 6, 6] for (w, t), ptCov [n, 3, 3], info dict) of the
         last armed run or collect."""
@@ -927,7 +946,7 @@ class BaSolver(_SolverHandle):
         out = (C.c_double * 8)()
         _ck(LIB.cosl_ba_solver_download_covariance(self.h, _ptr(cam), _ptr(pt), out))
         return cam, pt, {"pixel_var": out[0], "sigma2_hat": out[1], "dof": out[2], "unconstrained": int(out[3]),
-                         "device_ms": out[4], "min_pivot": out[5]}
+                         "device_ms": out[4], "min_pivot": out[5], "priors": int(out[6])}
 
     def download(self, into=None):
         """Current cameras and points into the solver's problem, or into `into` (same shape)."""

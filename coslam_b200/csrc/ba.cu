@@ -347,6 +347,12 @@ struct cosl_ba_solver {
   // nullptr otherwise; the kernels that read it are launched as their OBSCOV instantiations then
   double* d_obsL = nullptr;
   const double* graphObsL = nullptr;  // d.obsL the submitted graph was built with
+  // camera priors (cosl_ba_solver_set_cam_prior, DESIGN.md 4.8): prior.n > 0 while they are set, and then the
+  // kernels that read them are launched as their PRIOR instantiations.  d_prior holds [n][BA_PRIOR_REC] doubles,
+  // then the n camera indices.
+  BaPriorDev prior = {};
+  unsigned char* d_prior = nullptr;
+  BaPriorDev graphPrior = {};  // prior the submitted graph was built with
 };
 
 namespace {
@@ -692,6 +698,108 @@ int set_obs_cov(cosl_ba_solver* s, const std::vector<double>* L) {
   return COSL_OK;
 }
 
+// Cholesky factor G (lower, row-major 6x6) of a symmetric A: false when a pivot is not positive and finite
+bool chol6(const double* A, double* G) {
+  for (int i = 0; i < 36; ++i) G[i] = 0.0;
+  for (int j = 0; j < 6; ++j) {
+    double dj = A[6 * j + j];
+    for (int k = 0; k < j; ++k) dj -= G[6 * j + k] * G[6 * j + k];
+    if (!(dj > 0.0) || !std::isfinite(dj)) return false;
+    G[6 * j + j] = std::sqrt(dj);
+    for (int i = j + 1; i < 6; ++i) {
+      double a = A[6 * i + j];
+      for (int k = 0; k < j; ++k) a -= G[6 * i + k] * G[6 * j + k];
+      G[6 * i + j] = a / G[6 * j + j];
+    }
+  }
+  return true;
+}
+
+// Camera priors (DESIGN.md 4.8): cams[n] distinct free cameras of an m-camera problem with m_con fixed ones, R[n][9]
+// rotations, t[n][3], cov[n][36] symmetric positive definite (row-major, (w, dt)).  On success rec holds
+// [n][BA_PRIOR_REC] records (the upper-triangular L with L^T L = cov^-1 packed by rows, R_p, t_p); otherwise the first
+// bad prior is named.
+int check_cam_prior(int n, const int32_t* cams, const double* R, const double* t, const double* cov, int m, int mcon,
+                    std::vector<double>& rec, const char* what) {
+  if (!R || !t || !cov) return set_error(COSL_E_INVALID, "%s: null R, t or cov", what);
+  rec.assign((size_t)n * BA_PRIOR_REC, 0.0);
+  std::vector<char> seen((size_t)m, 0);
+  for (int k = 0; k < n; ++k) {
+    const int j = cams[k];
+    if (j < mcon || j >= m)
+      return set_error(COSL_E_INVALID, "%s: prior %d is on camera %d, not a free camera [%d, %d)", what, k, j, mcon, m);
+    if (seen[j]) return set_error(COSL_E_INVALID, "%s: prior %d repeats camera %d", what, k, j);
+    seen[j] = 1;
+    const double *Rk = R + 9 * (size_t)k, *tk = t + 3 * (size_t)k, *P = cov + 36 * (size_t)k;
+    bool finite = true;
+    for (int i = 0; i < 9; ++i) finite = finite && std::isfinite(Rk[i]);
+    for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(tk[i]);
+    for (int i = 0; i < 36; ++i) finite = finite && std::isfinite(P[i]);
+    if (!finite) return set_error(COSL_E_INVALID, "%s: prior %d is not finite", what, k);
+    double orth = 0.0;
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) {
+        const double g = Rk[a] * Rk[b] + Rk[3 + a] * Rk[3 + b] + Rk[6 + a] * Rk[6 + b] - (a == b ? 1.0 : 0.0);
+        orth = std::max(orth, std::fabs(g));
+      }
+    const double det = Rk[0] * (Rk[4] * Rk[8] - Rk[5] * Rk[7]) - Rk[1] * (Rk[3] * Rk[8] - Rk[5] * Rk[6]) +
+                       Rk[2] * (Rk[3] * Rk[7] - Rk[4] * Rk[6]);
+    if (orth > 1e-9 || !(det > 0.0))
+      return set_error(COSL_E_INVALID, "%s: R of prior %d is not a rotation (|R^T R - I| %.3g, det %.17g)", what, k,
+                       orth, det);
+    double pmax = 0.0;
+    for (int i = 0; i < 6; ++i) pmax = std::max(pmax, std::fabs(P[7 * i]));
+    for (int a = 0; a < 6; ++a)
+      for (int b = a + 1; b < 6; ++b)
+        if (std::fabs(P[6 * a + b] - P[6 * b + a]) > 1e-12 * pmax)
+          return set_error(COSL_E_INVALID, "%s: cov of prior %d is not symmetric (%d, %d)", what, k, a, b);
+    // P = G G^T, P^-1 = G^-T G^-1 = C C^T and L = C^T
+    double S[36], G[36], Gi[36] = {}, Pi[36], C[36];
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) S[6 * a + b] = 0.5 * (P[6 * a + b] + P[6 * b + a]);
+    if (!chol6(S, G)) return set_error(COSL_E_INVALID, "%s: cov of prior %d is not positive definite", what, k);
+    for (int c = 0; c < 6; ++c)  // G^-1, lower, by forward substitution of the unit columns
+      for (int i = c; i < 6; ++i) {
+        double a = i == c ? 1.0 : 0.0;
+        for (int q = c; q < i; ++q) a -= G[6 * i + q] * Gi[6 * q + c];
+        Gi[6 * i + c] = a / G[6 * i + i];
+      }
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) {
+        double u = 0.0;
+        for (int q = std::max(a, b); q < 6; ++q) u += Gi[6 * q + a] * Gi[6 * q + b];
+        Pi[6 * a + b] = u;
+      }
+    if (!chol6(Pi, C)) return set_error(COSL_E_INVALID, "%s: cov of prior %d is not positive definite", what, k);
+    double* out = rec.data() + (size_t)k * BA_PRIOR_REC;
+    int q = 0;
+    for (int a = 0; a < 6; ++a)
+      for (int b = a; b < 6; ++b) out[q++] = C[6 * b + a];
+    for (int i = 0; i < 9; ++i) out[21 + i] = Rk[i];
+    for (int i = 0; i < 3; ++i) out[30 + i] = tk[i];
+  }
+  return COSL_OK;
+}
+
+// Sets (rec and cams of n > 0 priors, checked by check_cam_prior) or clears (n == 0) the camera priors of the loaded
+// problem: the upload is enqueued on the solver's stream, nothing is waited for.
+int set_cam_prior(cosl_ba_solver* s, int n, const int32_t* cams, const std::vector<double>& rec) {
+  if (!n) {
+    s->prior = {};
+    return COSL_OK;
+  }
+  const size_t recBytes = sizeof(double) * (size_t)n * BA_PRIOR_REC;
+  COSL_TRY(grow(s, &s->d_prior, recBytes + sizeof(int32_t) * (size_t)n));
+  // from pageable memory: the calls return once the sources have been staged
+  COSL_CUDA(cudaMemcpyAsync(s->d_prior, rec.data(), recBytes, cudaMemcpyHostToDevice, s->rq.stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_prior + recBytes, cams, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice,
+                            s->rq.stream));
+  s->prior.rec = reinterpret_cast<const double*>(s->d_prior);
+  s->prior.cam = reinterpret_cast<const int*>(s->d_prior + recBytes);
+  s->prior.n = n;
+  return COSL_OK;
+}
+
 // What the host derives from the observation lists (validated by check_problem) to plan a problem
 // without a device round trip: the start of each free camera in the camera-major list and the start of
 // each camera-pair bucket (ja <= jb, row-major over mf x mf) in the Schur pair entries.
@@ -970,6 +1078,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   d.xy = s->d_xy;
   d.wgt = s->d_wgt;
   d.obsL = nullptr;  // a new problem has new observations: its covariances are unset
+  s->prior = {};     // and new cameras: its priors are unset
   d.ptr = s->d_ptr;
   d.cobs = s->d_cobs;
   d.ccam = s->d_ccam;
@@ -1111,25 +1220,40 @@ int read_sc(cosl_ba_solver* s) {
   return COSL_OK;
 }
 
-// sum w |e|^2 (w |L e|^2 with measurement covariances) at (pa, pb) into d.sc[SC_COST]
-int launch_cost(const BaDev& d, const double* pa, const double* pb, unsigned gN, cudaStream_t st) {
-  if (d.obsL)
-    COSL_LAUNCH(ba_residual_kernel<true>, gN, 256, 0, st, d, pa, pb, 0, 0.0, nullptr);
-  else
-    COSL_LAUNCH(ba_residual_kernel<false>, gN, 256, 0, st, d, pa, pb, 0, 0.0, nullptr);
+// The residual kernel's weight (mode 1) and outlier (mode 2) passes: on the pixel distance, without priors
+constexpr auto ba_residual_pass = ba_residual_kernel<false, false>;
+
+// The instantiation of a kernel templated on <OBSCOV, PRIOR> that d and the priors select
+template <typename K>
+K pick(bool obscov, bool prior, K ff, K tf, K ft, K tt) {
+  return prior ? (obscov ? tt : ft) : (obscov ? tf : ff);
+}
+
+// sum w |e|^2 (w |L e|^2 with measurement covariances), plus the priors' |L r|^2, at (pa, pb) into d.sc[SC_COST]
+int launch_cost(const cosl_ba_solver* s, const BaDev& d, const double* pa, const double* pb, cudaStream_t st) {
+  const bool pr = s->prior.n > 0;
+  const unsigned g = (unsigned)(div_up64(s->N, 256) + (pr ? div_up(s->prior.n, 256) : 0));
+  if (!g) return COSL_OK;
+  const auto k = pick(d.obsL != nullptr, pr, ba_residual_kernel<false, false>, ba_residual_kernel<true, false>,
+                      ba_residual_kernel<false, true>, ba_residual_kernel<true, true>);
+  COSL_LAUNCH(k, g, 256, 0, st, d, pa, pb, 0, 0.0, nullptr, s->prior);
   return COSL_OK;
 }
 
-// the two linearisation kernels at (d_pa, d_pb) into d's V, eb, W, U, ea (zeroed before)
+// the two linearisation kernels at (d_pa, d_pb) into d's V, eb, W, U, ea (zeroed before); the camera kernel adds
+// the priors in CTAs after those of the observations
 int launch_linearize(const cosl_ba_solver* s, const BaDev& d, cudaStream_t st) {
-  const unsigned gN = (unsigned)div_up64(s->N, 256), gC = (unsigned)div_up64(s->Nc, 128);
+  const bool pr = s->prior.n > 0;
+  const unsigned gN = (unsigned)div_up64(s->N, 256);
+  const unsigned gC = (unsigned)(div_up64(s->Nc, 128) + (pr ? div_up(s->prior.n, 128) : 0));
   if (d.obsL) {
     if (s->N) COSL_LAUNCH(ba_linearize_points<true>, gN, 256, 0, st, d, s->d_pa, s->d_pb);
-    if (s->Nc) COSL_LAUNCH(ba_linearize_cams<true>, gC, 128, 0, st, d, s->d_pa, s->d_pb);
   } else {
     if (s->N) COSL_LAUNCH(ba_linearize_points<false>, gN, 256, 0, st, d, s->d_pa, s->d_pb);
-    if (s->Nc) COSL_LAUNCH(ba_linearize_cams<false>, gC, 128, 0, st, d, s->d_pa, s->d_pb);
   }
+  const auto k = pick(d.obsL != nullptr, pr, ba_linearize_cams<false, false>, ba_linearize_cams<true, false>,
+                      ba_linearize_cams<false, true>, ba_linearize_cams<true, true>);
+  if (gC) COSL_LAUNCH(k, gC, 128, 0, st, d, s->d_pa, s->d_pb, s->prior);
   return COSL_OK;
 }
 
@@ -1141,17 +1265,18 @@ int launch_linearize(const cosl_ba_solver* s, const BaDev& d, cudaStream_t st) {
 int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dctl, double mu, int doStats) {
   const unsigned gN = (unsigned)div_up64(s->N, 256);
   const int r0 = rank_of(s) == 0 ? 1 : 0;
-  const bool oc = s->d.obsL != nullptr;
+  const bool oc = s->d.obsL != nullptr, pr = s->prior.n > 0;
   SectionTimer& T = s->timer;
   if (stage == BA_STAGE_ROUND) {  // the round's Tukey weights (on the pixel distance), then its initial cost
     if (s->N) {
       if (s->opt.max_err > 0)
-        COSL_LAUNCH(ba_residual_kernel<false>, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+        COSL_LAUNCH(ba_residual_pass, gN, 256, 0, st, s->d, s->d_pa, s->d_pb, 1, s->opt.max_err,
+                    nullptr, BaPriorDev{});
       else
         COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_wgt, s->N, 1.0);
     }
     T.begin(s->secCost, st);
-    if (s->N) COSL_TRY(launch_cost(s->d, s->d_pa, s->d_pb, gN, st));
+    COSL_TRY(launch_cost(s, s->d, s->d_pa, s->d_pb, st));
     T.end(st);
   } else if (stage == BA_STAGE_LIN0 || stage == BA_STAGE_LIN) {  // Jacobians, U, V, W, ea, eb at (pa, pb)
     const long long nV = 9LL * s->n + 27LL * s->m;  // [V | eb | U | ea]
@@ -1190,13 +1315,13 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
                 r0, nCamBlocks, s->d_dpb);
     T.end(st);
     T.begin(s->secCost, st);
-    if (s->N + s->n) {  // a problem without points never reaches a trial (|g| = 0 stops it), but is captured
-      const unsigned gF = (unsigned)div_up64(s->N + (long long)s->n, 256);
-      if (oc)
-        COSL_LAUNCH(ba_finish_cost<true>, gF, 256, 0, st, s->d, dctl, s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu);
-      else
-        COSL_LAUNCH(ba_finish_cost<false>, gF, 256, 0, st, s->d, dctl, s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv,
-                    mu);
+    // a problem without points or priors never reaches a trial (|g| = 0 stops it), but is captured
+    const unsigned gF =
+        (unsigned)(div_up64(s->N + (long long)s->n, 256) + (pr ? div_up(s->prior.n, 256) : 0));
+    if (gF) {
+      const auto k = pick(oc, pr, ba_finish_cost<false, false>, ba_finish_cost<true, false>,
+                          ba_finish_cost<false, true>, ba_finish_cost<true, true>);
+      COSL_LAUNCH(k, gF, 256, 0, st, s->d, dctl, s->d_na, s->d_pb, s->d_nb, s->d_dpb, s->d_Vinv, mu, s->prior);
     }
     T.end(st);
   } else {  // a trial without free cameras
@@ -1211,7 +1336,7 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
                   mu);
     T.end(st);
     T.begin(s->secCost, st);
-    if (s->N) COSL_TRY(launch_cost(s->d, s->d_na, s->d_nb, gN, st));
+    COSL_TRY(launch_cost(s, s->d, s->d_na, s->d_nb, st));
     T.end(st);
   }
   if (stage == BA_STAGE_ROUND || stage == BA_STAGE_TRIAL) COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
@@ -1224,8 +1349,8 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
 int enqueue_outliers(cosl_ba_solver* s, cudaStream_t st) {
   if (s->opt.max_err > 0) {
     if (s->N)
-      COSL_LAUNCH(ba_residual_kernel<false>, (unsigned)div_up64(s->N, 256), 256, 0, st, s->d, s->d_pa, s->d_pb, 2,
-                  s->opt.max_err, s->d_outlier);
+      COSL_LAUNCH(ba_residual_pass, (unsigned)div_up64(s->N, 256), 256, 0, st, s->d, s->d_pa,
+                  s->d_pb, 2, s->opt.max_err, s->d_outlier, BaPriorDev{});
     COSL_TRY(allreduce(s, s->d_sc, SC_NSUM, ncclSum));
   } else {
     COSL_CUDA(cudaMemsetAsync(s->d_outlier, 0, (size_t)s->N ? (size_t)s->N : 1, st));
@@ -1401,7 +1526,8 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
               0, st, s->d_covSc, s->d_covT, 6LL * n, s->d_covCnt, nb);
   if (s->N) {
     if (s->opt.max_err > 0)
-      COSL_LAUNCH(ba_residual_kernel<false>, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr);
+      COSL_LAUNCH(ba_residual_pass, gN, 256, 0, st, cd, s->d_pa, s->d_pb, 1, s->opt.max_err, nullptr,
+                  BaPriorDev{});
     else
       COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_covWgt, s->N, 1.0);
   }
@@ -1414,7 +1540,7 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
   COSL_LAUNCH(ba_prep_kernel, nTilesInit + (unsigned)div_up64((long long)n + m, 256), 256, 0, st, cd, nullptr, 0.0, 1,
               s->tl.diagBlk, s->tl.blkCam0, s->tl.order, s->d_cnt, s->td.nCounters + 2 + s->td.nTasks, nTilesInit,
               s->d_Vinv, 0, nullptr, 0LL);
-  if (s->N) COSL_TRY(launch_cost(cd, s->d_pa, s->d_pb, gN, st));
+  COSL_TRY(launch_cost(s, cd, s->d_pa, s->d_pb, st));
   if (n) COSL_LAUNCH(ba_cov_vfix, div_up(n, 256), 256, 0, st, s->d_covUnc, s->d_Vinv, n);
   if (s->ns) {
     if (s->nItems)
@@ -1428,7 +1554,7 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
                 s->d_covT);
   if (n) COSL_LAUNCH(ba_cov_points, div_up(n, 256), 256, 0, st, n, s->ncon, s->d_Vinv, s->d_covT, s->d_covUnc, var,
                      s->d_covPt);
-  COSL_LAUNCH(ba_cov_end, 1, 32, 0, st, s->d_covSc, s->d_covPiv, nb, s->mf, var);
+  COSL_LAUNCH(ba_cov_end, 1, 32, 0, st, s->d_covSc, s->d_covPiv, nb, s->mf, var, s->prior.n);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
@@ -1565,6 +1691,7 @@ int build_graph(cosl_ba_solver* s) {
   s->graphNb = s->d_nb;
   s->graphCovVar = s->covVar;
   s->graphObsL = s->d.obsL;
+  s->graphPrior = s->prior;
   return COSL_OK;
 }
 
@@ -1782,7 +1909,8 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
   COSL_TRY(s->rq.idle("cosl_ba_solver_submit"));
   // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
   if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
-      s->graphNb != s->d_nb || s->graphCovVar != s->covVar || s->graphObsL != s->d.obsL)
+      s->graphNb != s->d_nb || s->graphCovVar != s->covVar || s->graphObsL != s->d.obsL ||
+      s->graphPrior.rec != s->prior.rec || s->graphPrior.n != s->prior.n)
     COSL_TRY(build_graph(s));
   // the request number goes to the device ahead of the graph, on the solver's stream: a stop made before the
   // graph starts names it too (the pinned source is not rewritten before this request is collected)
@@ -1911,6 +2039,19 @@ int cosl_ba_solver_set_obs_cov(cosl_ba_solver* s, const double* covx) {
   std::vector<double> L;
   COSL_TRY(check_obs_cov(covx, s->N, L, "cosl_ba_solver_set_obs_cov"));
   return set_obs_cov(s, &L);
+}
+
+int cosl_ba_solver_set_cam_prior(cosl_ba_solver* s, int nPrior, const int32_t* cams, const double* R,
+                                 const double* t, const double* cov) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_set_cam_prior: a multi-rank solver has no camera priors");
+  if (nPrior < 0) return set_error(COSL_E_INVALID, "cosl_ba_solver_set_cam_prior: nPrior %d < 0", nPrior);
+  COSL_TRY(s->rq.idle("cosl_ba_solver_set_cam_prior"));
+  std::vector<double> rec;
+  if (nPrior == 0 || !cams) return set_cam_prior(s, 0, nullptr, rec);
+  COSL_TRY(check_cam_prior(nPrior, cams, R, t, cov, s->m, s->mcon, rec, "cosl_ba_solver_set_cam_prior"));
+  return set_cam_prior(s, nPrior, cams, rec);
 }
 
 int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double* ptCov, double out[8]) {

@@ -198,16 +198,135 @@ __global__ void __launch_bounds__(256) ba_obscov_factor(double* __restrict__ L, 
   q[2] = 1.0 / sqrt(c);
 }
 
+// Gaussian camera priors (cosl_ba_solver_set_cam_prior, DESIGN.md 4.8).  Prior k on free camera cam[k] is
+// rec[k] = [L (21: the upper-triangular 6x6 factor with L^T L = P^-1, packed by rows) | R_p (9, row-major) | t_p (3)].
+// Its residual is r = [Log(R R_p^T); t - t_p] with R = R(q(v)) R0 and t of pa, so it follows a reset that re-anchors
+// R0.  The kernels that take a template flag PRIOR add |L r|^2 to the cost and (L J)^T (L J), -(L J)^T L r to U_j and
+// ea_j in CTAs beyond their observation range.  The priors are a kernel argument of their own rather than BaDev
+// fields, so the instantiations without PRIOR keep their parameter layout and code.
+struct BaPriorDev {
+  const double* rec;  // [n][BA_PRIOR_REC]
+  const int* cam;     // [n], distinct free cameras
+  int n;
+};
+constexpr int BA_PRIOR_REC = 33;
+
+// Whitened prior residual rw = L r of prior k at pa and, with WANT_J, Jw = L dr/d(v, t) (6x6 row-major).
+// Log(M) by atan2 with the axis from the skew part below 120 degrees and from the symmetric part above (exact to
+// roundoff up to pi); dr_w / dv = Jl^-1(r_w) J_q with the left-Jacobian inverse of SO(3),
+// Jl^-1(w) = I - [w]x / 2 + (1 - (th / 2) cot(th / 2)) / th^2 [w]x^2, and J_q = 2 (w_q I + [v]x + v v^T / w_q) the
+// chart factor of ba_cov_cams.
+template <bool WANT_J>
+__device__ __forceinline__ void ba_prior_eval(const BaDev& d, const BaPriorDev& pr, int k,
+                                              const double* __restrict__ pa, double rw[6], double Jw[36]) {
+  const int j = pr.cam[k];
+  const double* __restrict__ q = pr.rec + BA_PRIOR_REC * (size_t)k;
+  const double* __restrict__ R0 = d.camR0 + 9 * (size_t)j;
+  const double* __restrict__ p6 = pa + 6 * (size_t)j;
+  const double x = p6[0], y = p6[1], z = p6[2];
+  const double wq = sqrt(1.0 - (x * x + y * y + z * z));
+  const double Rd[9] = {wq * wq + x * x - y * y - z * z, 2 * (x * y - wq * z), 2 * (x * z + wq * y),
+                        2 * (x * y + wq * z), wq * wq - x * x + y * y - z * z, 2 * (y * z - wq * x),
+                        2 * (x * z - wq * y), 2 * (y * z + wq * x), wq * wq - x * x - y * y + z * z};
+  double R[9], M[9];  // R = R(q(v)) R0, M = R R_p^T
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) R[3 * a + b] = Rd[3 * a] * R0[b] + Rd[3 * a + 1] * R0[3 + b] + Rd[3 * a + 2] * R0[6 + b];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b)
+      M[3 * a + b] = R[3 * a] * q[21 + 3 * b] + R[3 * a + 1] * q[22 + 3 * b] + R[3 * a + 2] * q[23 + 3 * b];
+  const double s[3] = {0.5 * (M[7] - M[5]), 0.5 * (M[2] - M[6]), 0.5 * (M[3] - M[1])};
+  const double sn = sqrt(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]);
+  const double cs = 0.5 * (M[0] + M[4] + M[8] - 1.0);
+  const double th = atan2(sn, cs);
+  double r[6];
+  if (cs > -0.5) {
+    const double f = th < 1e-4 ? 1.0 + th * th / 6.0 : th / sn;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) r[a] = f * s[a];
+  } else {  // (M + M^T) / 2 - cos th I = (1 - cos th) a a^T: the column of the largest diagonal entry
+    const double S0 = M[0] - cs, S1 = M[4] - cs, S2 = M[8] - cs;
+    const double s01 = 0.5 * (M[1] + M[3]), s02 = 0.5 * (M[2] + M[6]), s12 = 0.5 * (M[5] + M[7]);
+    const int c = (S0 >= S1 && S0 >= S2) ? 0 : (S1 >= S2 ? 1 : 2);
+    const double col[3] = {c == 0 ? S0 : (c == 1 ? s01 : s02), c == 0 ? s01 : (c == 1 ? S1 : s12),
+                           c == 0 ? s02 : (c == 1 ? s12 : S2)};
+    const double f = th / sqrt((1.0 - cs) * (c == 0 ? S0 : (c == 1 ? S1 : S2)));
+    const double sg = (col[0] * s[0] + col[1] * s[1] + col[2] * s[2]) < 0.0 ? -f : f;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) r[a] = sg * col[a];
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) r[3 + a] = p6[3 + a] - q[30 + a];
+  // rw = L r, L packed by rows: row a holds L[a][a .. 5] from offset 6a - a(a-1)/2
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const int off = 6 * a - a * (a - 1) / 2;
+    double t = 0.0;
+#pragma unroll
+    for (int b = a; b < 6; ++b) t += q[off + b - a] * r[b];
+    rw[a] = t;
+  }
+  if (!WANT_J) return;
+  // cot(th / 2) = sin th / (1 - cos th) = sn / (|(sn, cs)| - cs): no trigonometric call, exact up to pi
+  const double c2 = th < 1e-2 ? 1.0 / 12.0 + th * th * (1.0 / 720.0 + th * th / 30240.0)
+                              : (1.0 - 0.5 * th * sn / (sqrt(sn * sn + cs * cs) - cs)) / (th * th);
+  const double wx[9] = {0.0, -r[2], r[1], r[2], 0.0, -r[0], -r[1], r[0], 0.0};
+  double Ji[9], Jq[9], Jo[9];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      const double w2 = wx[3 * a] * wx[b] + wx[3 * a + 1] * wx[3 + b] + wx[3 * a + 2] * wx[6 + b];
+      Ji[3 * a + b] = (a == b ? 1.0 : 0.0) - 0.5 * wx[3 * a + b] + c2 * w2;
+    }
+  const double v[3] = {x, y, z}, vx[9] = {0.0, -z, y, z, 0.0, -x, -y, x, 0.0};
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) Jq[3 * a + b] = 2.0 * ((a == b ? wq : 0.0) + vx[3 * a + b] + v[a] * v[b] / wq);
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) Jo[3 * a + b] = Ji[3 * a] * Jq[b] + Ji[3 * a + 1] * Jq[3 + b] + Ji[3 * a + 2] * Jq[6 + b];
+  // Jw = L diag(Jo, I)
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const int off = 6 * a - a * (a - 1) / 2;
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      double t = 0.0;
+#pragma unroll
+      for (int c = a; c < 3; ++c) t += q[off + c - a] * Jo[3 * c + b];
+      Jw[6 * a + b] = t;
+    }
+#pragma unroll
+    for (int b = 3; b < 6; ++b) Jw[6 * a + b] = b >= a ? q[off + b - a] : 0.0;
+  }
+}
+
+// sum over this CTA's priors (one per thread, from prior index k0) of |L r|^2 at pa
+__device__ __forceinline__ double ba_prior_cost(const BaDev& d, const BaPriorDev& pr, long long k0,
+                                                const double* __restrict__ pa) {
+  const long long k = k0 + threadIdx.x;
+  if (k >= pr.n) return 0.0;
+  double rw[6];
+  ba_prior_eval<false>(d, pr, (int)k, pa, rw, nullptr);
+  return rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2] + rw[3] * rw[3] + rw[4] * rw[4] + rw[5] * rw[5];
+}
+
 // ------------------------------------------------------------------------------------------
 // cost / weights / outliers: one observation per thread
 // mode 0: sc[SC_COST] += w |e|^2 ; mode 1: wgt = tukey(|e|, maxErr) ; mode 2: outlier = |e|>=maxErr,
 // sc[SC_COST] += number of outliers.  OBSCOV: mode 0 sums w |L e|^2; modes 1 and 2 stay on the pixel distance |e|
-// (they are launched without it).
+// (they are launched without it).  PRIOR (mode 0 only): the CTAs beyond the observations add the priors' |L r|^2.
 // ------------------------------------------------------------------------------------------
-template <bool OBSCOV>
+template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(256)
 ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb, int mode,
-                   double maxErr, unsigned char* __restrict__ outlier) {
+                   double maxErr, unsigned char* __restrict__ outlier, BaPriorDev pr) {
   __shared__ double s_red[8];
   const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double c = 0;
@@ -228,6 +347,10 @@ ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restr
       outlier[o] = (unsigned char)isOut;
       c = (double)isOut;
     }
+  }
+  if (PRIOR) {
+    const long long nb0 = (d.N + blockDim.x - 1) / blockDim.x;
+    if ((long long)blockIdx.x >= nb0) c = ba_prior_cost(d, pr, ((long long)blockIdx.x - nb0) * blockDim.x, pa);
   }
   if (mode == 2) {  // number of outliers -> sc[SC_COST] (info[13] of the solver entry points)
     const double t = block_sum_1(c, s_red);
@@ -309,9 +432,39 @@ ba_linearize_points(BaDev d, const double* __restrict__ pa, const double* __rest
 
 // Linearisation, camera-major over the free-camera observations: U_j = sum A^T A (packed upper,
 // 21) and ea_j = sum A^T e (6), collapsed per camera with segmented shuffles.  OBSCOV: A and e whitened by L.
-template <bool OBSCOV>
+// PRIOR: the CTAs beyond the observations add one prior per thread, U_j += Jw^T Jw and ea_j -= Jw^T rw (ea sums
+// A^T (x - h), and the prior's "x - h" is -r); a prior camera that no observation sees gets its U_j here.
+template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(128)
-ba_linearize_cams(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb) {
+ba_linearize_cams(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb, BaPriorDev pr) {
+  if (PRIOR) {
+    const long long nb0 = (d.Nc + blockDim.x - 1) / blockDim.x;
+    if ((long long)blockIdx.x >= nb0) {
+      const long long k = ((long long)blockIdx.x - nb0) * blockDim.x + threadIdx.x;
+      if (k >= pr.n) return;
+      double rw[6], Jw[36];
+      ba_prior_eval<true>(d, pr, (int)k, pa, rw, Jw);
+      const int j = pr.cam[k];
+      int t = 0;
+#pragma unroll
+      for (int a = 0; a < 6; ++a)
+#pragma unroll
+        for (int b = a; b < 6; ++b) {
+          double u = 0.0;
+#pragma unroll
+          for (int r = 0; r < 6; ++r) u += Jw[6 * r + a] * Jw[6 * r + b];
+          atomicAdd(&d.U[21 * (size_t)j + t++], u);
+        }
+#pragma unroll
+      for (int a = 0; a < 6; ++a) {
+        double g = 0.0;
+#pragma unroll
+        for (int r = 0; r < 6; ++r) g += Jw[6 * r + a] * rw[r];
+        atomicAdd(&d.ea[6 * (size_t)j + a], -g);
+      }
+      return;
+    }
+  }
   const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
   double acc[27];
@@ -869,7 +1022,8 @@ ba_cam_update(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__
 //  ba_finish_cost: one observation per thread: db_i = V*_i^-1 (e_b,i - t_i) recomputed from the point's
 //    accumulator (read-only here; the FIRST observation of a point stores nb_i = pb_i + db_i and adds the
 //    point-side sums), then the weighted squared residual at (na, nb_i) -> cost (whitened with OBSCOV).  Extra
-//    threads finish the points that have no observation.
+//    threads finish the points that have no observation; with PRIOR, the CTAs after those add the priors' |L r|^2
+//    at na.
 // Both take mu from ctl, the control block of the submitted loop, when it is set.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -929,10 +1083,11 @@ ba_back_cams_points(BaDev d, const BaCtl* __restrict__ ctl, const double* __rest
   }
 }
 
-template <bool OBSCOV>
+template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(256)
 ba_finish_cost(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__ na, const double* __restrict__ pb,
-               double* __restrict__ nb, const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu) {
+               double* __restrict__ nb, const double* __restrict__ acc3, const double* __restrict__ Vinv, double mu,
+               BaPriorDev pr) {
   if (ctl) mu = ctl->mu;
   __shared__ double s_red[8];
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -983,6 +1138,10 @@ ba_finish_cost(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict_
       if (OBSCOV) ba_whiten<1>(d.obsL + 3 * (size_t)o, &dx, &dy);
       c = d.wgt[o] * (dx * dx + dy * dy);
     }
+  }
+  if (PRIOR) {
+    const long long nb0 = (d.N + d.n + blockDim.x - 1) / blockDim.x;
+    if ((long long)blockIdx.x >= nb0) c = ba_prior_cost(d, pr, ((long long)blockIdx.x - nb0) * blockDim.x, na);
   }
   double s = block_sum_1(c, s_red);
   if (threadIdx.x == 0) {
@@ -1184,12 +1343,14 @@ ba_cov_points(int n, int ncon, const double* __restrict__ Vinv, const double* __
       out[3 * r + c] = var * (Iv[3 * r + c] + A[3 * r] * Iv[c] + A[3 * r + 1] * Iv[3 + c] + A[3 * r + 2] * Iv[6 + c]);
 }
 
-// The stage's scalars: sigma^2-hat, dof, the minimum relative pivot over the nb blocks, singularity, time
-__global__ void ba_cov_end(double* __restrict__ sc, const double* __restrict__ piv, int nb, int mf, double var) {
+// The stage's scalars: sigma^2-hat, dof, the minimum relative pivot over the nb blocks, singularity, time, the
+// number of camera priors (each counts as six measurements in dof; their |L r|^2 is in sc[SC_COST])
+__global__ void ba_cov_end(double* __restrict__ sc, const double* __restrict__ piv, int nb, int mf, double var,
+                           int nPrior) {
   if (threadIdx.x != 0) return;
   double mp = __longlong_as_double(0x7ff0000000000000LL);  // +inf: no free camera, no pivot
   for (int k = 0; k < nb; ++k) mp = fmin(mp, piv[k]);
-  const double dof = 2.0 * sc[COV_NOBS] - 6.0 * mf - 3.0 * sc[COV_NPTS];
+  const double dof = 2.0 * sc[COV_NOBS] - 6.0 * mf - 3.0 * sc[COV_NPTS] + 6.0 * nPrior;
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   const unsigned long long t0 = *reinterpret_cast<const unsigned long long*>(sc + COV_T0);
@@ -1201,7 +1362,8 @@ __global__ void ba_cov_end(double* __restrict__ sc, const double* __restrict__ p
   out[3] = sc[COV_NUNC];
   out[4] = 1e-6 * (double)(t - t0);
   out[5] = mp;
-  out[6] = out[7] = 0.0;
+  out[6] = nPrior;
+  out[7] = 0.0;
 }
 
 }  // namespace coslam

@@ -636,6 +636,24 @@ int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double
  * waiting.  NULL clears.  The covariances apply to every later run, run_fixed and submit; reset keeps them, load
  * clears them.  COSL_E_STATE while a submit is in flight; COSL_E_INVALID for a NULL handle or a multi-rank solver. */
 int cosl_ba_solver_set_obs_cov(cosl_ba_solver* s, const double* covx);
+/* Gaussian pose priors on free cameras of the loaded problem (an extension, DESIGN.md 4.8).  Prior k on camera
+ * cams[k] has the mean (R[k] row-major 3x3, t[k]) and the 6x6 covariance cov[k] (row-major) for (w, dt) in the chart
+ * of camCov: its residual is r = [Log(R R_p^T); t - t_p], and the objective becomes
+ *   sum_obs w e^T Lambda e + sum_priors r^T cov^-1 r.
+ * cov is in the units of the objective: a camCov of an earlier BA with covariances in px^2 (or with none and
+ * pixel_var = 1) is a valid cov as it stands; with unweighted observations of pixel variance s2, pass camCov / s2.
+ * Tukey weights and the outlier pass ignore priors.  The priors enter U and ea, every cost in info and progress, the
+ * statistics behind mu0, and the covariance stage, whose H gains sum cov^-1 (a problem singular in the gauge may
+ * become regular), whose sigma2_hat gains sum r^T cov^-1 r, and whose dof gains 6 per prior; out[6] of
+ * cosl_ba_solver_download_covariance is the number of priors.
+ * Validates on the calling thread: cams[k] in [m_con, m) and distinct, R[k] a rotation (|R^T R - I|_max <= 1e-9, det
+ * > 0), every value finite, cov[k] symmetric to 1e-12 relative and positive definite; otherwise COSL_E_INVALID names
+ * the first bad prior and the handle keeps what it had.  Copies the priors (the caller may reuse its arrays on
+ * return), enqueues the upload on the solver's stream and returns without waiting.  nPrior == 0 or cams == NULL
+ * clears.  The priors apply to every later run, run_fixed and submit; reset keeps them, load clears them.
+ * COSL_E_STATE while a submit is in flight; COSL_E_INVALID for a NULL handle, a multi-rank solver or nPrior < 0. */
+int cosl_ba_solver_set_cam_prior(cosl_ba_solver* s, int nPrior, const int32_t* cams, const double* R,
+                                 const double* t, const double* cov);
 /* Per-kernel accumulated device time in ms since create/reset, by name (NULL-terminated list via
  * index): returns name or NULL when idx is out of range. */
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls);
