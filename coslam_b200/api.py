@@ -109,6 +109,7 @@ def _load():
     L.cosl_ba_solver_download_covariance.argtypes = [vp, vp, vp, C.POINTER(cd)]
     L.cosl_ba_solver_set_obs_cov.argtypes = [vp, vp]
     L.cosl_ba_solver_set_cam_prior.argtypes = [vp, ci, vp, vp, vp, vp]
+    L.cosl_ba_solver_set_pt_prior.argtypes = [vp, ci, vp, vp, vp]
     L.cosl_ba_solver_download.argtypes = [vp, C.POINTER(BaProblem)]
     L.cosl_ba_solver_destroy.argtypes = [vp]
     L.cosl_ba_solver_stream.argtypes = [vp]
@@ -938,6 +939,23 @@ class BaSolver(_SolverHandle):
             raise ValueError(f"set_cam_prior: {k} cameras but {len(R)} R, {len(t)} t and {len(cov)} cov")
         _ck(LIB.cosl_ba_solver_set_cam_prior(self.h, k, _ptr(cams), _ptr(R), _ptr(t), _ptr(cov)))
 
+    def set_pt_prior(self, pts, X=None, cov=None):
+        """cosl_ba_solver_set_pt_prior: Gaussian priors on free points pts [k] with means X [k, 3] and covariances
+        cov [k, 3, 3] in world coordinates (the chart of download_covariance's ptCov), in the units of the objective
+        (a ptCov of an earlier BA in px^2 as it stands; ptCov / s2 for unweighted observations of pixel variance
+        s2).  They apply to every later run / run_fixed / submit; None (or no points) clears.  load() clears them,
+        reset() keeps them; camera priors may be set as well."""
+        if pts is None or len(pts) == 0:
+            _ck(LIB.cosl_ba_solver_set_pt_prior(self.h, 0, None, None, None))
+            return
+        pts = np.ascontiguousarray(pts, np.int32).reshape(-1)
+        k = len(pts)
+        X = np.ascontiguousarray(X, np.float64).reshape(-1, 3)
+        cov = np.ascontiguousarray(cov, np.float64).reshape(-1, 9)
+        if len(X) != k or len(cov) != k:
+            raise ValueError(f"set_pt_prior: {k} points but {len(X)} X and {len(cov)} cov")
+        _ck(LIB.cosl_ba_solver_set_pt_prior(self.h, k, _ptr(pts), _ptr(X), _ptr(cov)))
+
     def download_covariance(self):
         """cosl_ba_solver_download_covariance: (camCov [m, 6, 6] for (w, t), ptCov [n, 3, 3], info dict) of the
         last armed run or collect."""
@@ -946,7 +964,8 @@ class BaSolver(_SolverHandle):
         out = (C.c_double * 8)()
         _ck(LIB.cosl_ba_solver_download_covariance(self.h, _ptr(cam), _ptr(pt), out))
         return cam, pt, {"pixel_var": out[0], "sigma2_hat": out[1], "dof": out[2], "unconstrained": int(out[3]),
-                         "device_ms": out[4], "min_pivot": out[5], "priors": int(out[6])}
+                         "device_ms": out[4], "min_pivot": out[5], "priors": int(out[6]),
+                         "pt_priors": int(out[7])}
 
     def download(self, into=None):
         """Current cameras and points into the solver's problem, or into `into` (same shape)."""

@@ -350,8 +350,13 @@ struct cosl_ba_solver {
   // camera priors (cosl_ba_solver_set_cam_prior, DESIGN.md 4.8): prior.n > 0 while they are set, and then the
   // kernels that read them are launched as their PRIOR instantiations.  d_prior holds [n][BA_PRIOR_REC] doubles,
   // then the n camera indices.
+  // Point priors (cosl_ba_solver_set_pt_prior, DESIGN.md 4.9) are prior.np > 0 and the prec / pt / has fields, in
+  // d_ptPrior: [np][BA_PTPRIOR_REC] doubles, the np point indices, then one flag byte per point.  The PRIOR
+  // instantiations run while priors of either kind are set, ba_linearize_points<PRIOR> and ba_cov_mask<PRIOR>
+  // while point priors are.
   BaPriorDev prior = {};
   unsigned char* d_prior = nullptr;
+  unsigned char* d_ptPrior = nullptr;
   BaPriorDev graphPrior = {};  // prior the submitted graph was built with
 };
 
@@ -698,22 +703,25 @@ int set_obs_cov(cosl_ba_solver* s, const std::vector<double>* L) {
   return COSL_OK;
 }
 
-// Cholesky factor G (lower, row-major 6x6) of a symmetric A: false when a pivot is not positive and finite
-bool chol6(const double* A, double* G) {
-  for (int i = 0; i < 36; ++i) G[i] = 0.0;
-  for (int j = 0; j < 6; ++j) {
-    double dj = A[6 * j + j];
-    for (int k = 0; k < j; ++k) dj -= G[6 * j + k] * G[6 * j + k];
+// Cholesky factor G (lower, row-major NxN) of a symmetric A: false when a pivot is not positive and finite
+template <int N>
+bool chol(const double* A, double* G) {
+  for (int i = 0; i < N * N; ++i) G[i] = 0.0;
+  for (int j = 0; j < N; ++j) {
+    double dj = A[N * j + j];
+    for (int k = 0; k < j; ++k) dj -= G[N * j + k] * G[N * j + k];
     if (!(dj > 0.0) || !std::isfinite(dj)) return false;
-    G[6 * j + j] = std::sqrt(dj);
-    for (int i = j + 1; i < 6; ++i) {
-      double a = A[6 * i + j];
-      for (int k = 0; k < j; ++k) a -= G[6 * i + k] * G[6 * j + k];
-      G[6 * i + j] = a / G[6 * j + j];
+    G[N * j + j] = std::sqrt(dj);
+    for (int i = j + 1; i < N; ++i) {
+      double a = A[N * i + j];
+      for (int k = 0; k < j; ++k) a -= G[N * i + k] * G[N * j + k];
+      G[N * i + j] = a / G[N * j + j];
     }
   }
   return true;
 }
+constexpr auto chol6 = chol<6>;
+constexpr auto chol3 = chol<3>;
 
 // Camera priors (DESIGN.md 4.8): cams[n] distinct free cameras of an m-camera problem with m_con fixed ones, R[n][9]
 // rotations, t[n][3], cov[n][36] symmetric positive definite (row-major, (w, dt)).  On success rec holds
@@ -785,7 +793,9 @@ int check_cam_prior(int n, const int32_t* cams, const double* R, const double* t
 // problem: the upload is enqueued on the solver's stream, nothing is waited for.
 int set_cam_prior(cosl_ba_solver* s, int n, const int32_t* cams, const std::vector<double>& rec) {
   if (!n) {
-    s->prior = {};
+    s->prior.rec = nullptr;
+    s->prior.cam = nullptr;
+    s->prior.n = 0;
     return COSL_OK;
   }
   const size_t recBytes = sizeof(double) * (size_t)n * BA_PRIOR_REC;
@@ -797,6 +807,84 @@ int set_cam_prior(cosl_ba_solver* s, int n, const int32_t* cams, const std::vect
   s->prior.rec = reinterpret_cast<const double*>(s->d_prior);
   s->prior.cam = reinterpret_cast<const int*>(s->d_prior + recBytes);
   s->prior.n = n;
+  return COSL_OK;
+}
+
+// Point priors (DESIGN.md 4.9): pts[n] distinct free points of an np-point problem with ncon fixed ones, X[n][3],
+// cov[n][9] symmetric positive definite (row-major).  On success rec holds [n][BA_PTPRIOR_REC] records (the
+// upper-triangular L with L^T L = cov^-1 packed by rows, mu); otherwise the first bad prior is named.
+int check_pt_prior(int n, const int32_t* pts, const double* X, const double* cov, int np, int ncon,
+                   std::vector<double>& rec, const char* what) {
+  if (!X || !cov) return set_error(COSL_E_INVALID, "%s: null X or cov", what);
+  rec.assign((size_t)n * BA_PTPRIOR_REC, 0.0);
+  std::vector<char> seen((size_t)np, 0);
+  for (int k = 0; k < n; ++k) {
+    const int i = pts[k];
+    if (i < ncon || i >= np)
+      return set_error(COSL_E_INVALID, "%s: prior %d is on point %d, not a free point [%d, %d)", what, k, i, ncon, np);
+    if (seen[i]) return set_error(COSL_E_INVALID, "%s: prior %d repeats point %d", what, k, i);
+    seen[i] = 1;
+    const double *Xk = X + 3 * (size_t)k, *P = cov + 9 * (size_t)k;
+    bool finite = true;
+    for (int a = 0; a < 3; ++a) finite = finite && std::isfinite(Xk[a]);
+    for (int a = 0; a < 9; ++a) finite = finite && std::isfinite(P[a]);
+    if (!finite) return set_error(COSL_E_INVALID, "%s: prior %d is not finite", what, k);
+    const double pmax = std::max(std::fabs(P[0]), std::max(std::fabs(P[4]), std::fabs(P[8])));
+    for (int a = 0; a < 3; ++a)
+      for (int b = a + 1; b < 3; ++b)
+        if (std::fabs(P[3 * a + b] - P[3 * b + a]) > 1e-12 * pmax)
+          return set_error(COSL_E_INVALID, "%s: cov of prior %d is not symmetric (%d, %d)", what, k, a, b);
+    // P = G G^T, P^-1 = G^-T G^-1 = C C^T and L = C^T, as for the camera priors
+    double S[9], G[9], Gi[9] = {}, Pi[9], Cf[9];
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) S[3 * a + b] = 0.5 * (P[3 * a + b] + P[3 * b + a]);
+    if (!chol3(S, G)) return set_error(COSL_E_INVALID, "%s: cov of prior %d is not positive definite", what, k);
+    for (int c = 0; c < 3; ++c)
+      for (int i2 = c; i2 < 3; ++i2) {
+        double a = i2 == c ? 1.0 : 0.0;
+        for (int q = c; q < i2; ++q) a -= G[3 * i2 + q] * Gi[3 * q + c];
+        Gi[3 * i2 + c] = a / G[3 * i2 + i2];
+      }
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) {
+        double u = 0.0;
+        for (int q = std::max(a, b); q < 3; ++q) u += Gi[3 * q + a] * Gi[3 * q + b];
+        Pi[3 * a + b] = u;
+      }
+    if (!chol3(Pi, Cf)) return set_error(COSL_E_INVALID, "%s: cov of prior %d is not positive definite", what, k);
+    double* out = rec.data() + (size_t)k * BA_PTPRIOR_REC;
+    int q = 0;
+    for (int a = 0; a < 3; ++a)
+      for (int b = a; b < 3; ++b) out[q++] = Cf[3 * b + a];
+    for (int a = 0; a < 3; ++a) out[6 + a] = Xk[a];
+  }
+  return COSL_OK;
+}
+
+// Sets (rec and pts of n > 0 priors, checked by check_pt_prior) or clears (n == 0) the point priors of the loaded
+// problem: the upload (records, indices and the per-point flags) is enqueued on the solver's stream, nothing is
+// waited for.
+int set_pt_prior(cosl_ba_solver* s, int n, const int32_t* pts, const std::vector<double>& rec) {
+  if (!n) {
+    s->prior.np = 0;
+    s->prior.prec = nullptr;
+    s->prior.pt = nullptr;
+    s->prior.has = nullptr;
+    return COSL_OK;
+  }
+  const size_t recBytes = sizeof(double) * (size_t)n * BA_PTPRIOR_REC, ptBytes = sizeof(int32_t) * (size_t)n;
+  std::vector<unsigned char> has((size_t)s->n, 0);
+  for (int k = 0; k < n; ++k) has[pts[k]] = 1;
+  COSL_TRY(grow(s, &s->d_ptPrior, recBytes + ptBytes + has.size()));
+  // from pageable memory: the calls return once the sources have been staged
+  COSL_CUDA(cudaMemcpyAsync(s->d_ptPrior, rec.data(), recBytes, cudaMemcpyHostToDevice, s->rq.stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_ptPrior + recBytes, pts, ptBytes, cudaMemcpyHostToDevice, s->rq.stream));
+  COSL_CUDA(cudaMemcpyAsync(s->d_ptPrior + recBytes + ptBytes, has.data(), has.size(), cudaMemcpyHostToDevice,
+                            s->rq.stream));
+  s->prior.prec = reinterpret_cast<const double*>(s->d_ptPrior);
+  s->prior.pt = reinterpret_cast<const int*>(s->d_ptPrior + recBytes);
+  s->prior.has = s->d_ptPrior + recBytes + ptBytes;
+  s->prior.np = n;
   return COSL_OK;
 }
 
@@ -1078,7 +1166,7 @@ int load_problem(cosl_ba_solver* s, const cosl_ba_problem* p, const BaIndex& x) 
   d.xy = s->d_xy;
   d.wgt = s->d_wgt;
   d.obsL = nullptr;  // a new problem has new observations: its covariances are unset
-  s->prior = {};     // and new cameras: its priors are unset
+  s->prior = {};     // and new cameras and points: its priors of both kinds are unset
   d.ptr = s->d_ptr;
   d.cobs = s->d_cobs;
   d.ccam = s->d_ccam;
@@ -1231,8 +1319,9 @@ K pick(bool obscov, bool prior, K ff, K tf, K ft, K tt) {
 
 // sum w |e|^2 (w |L e|^2 with measurement covariances), plus the priors' |L r|^2, at (pa, pb) into d.sc[SC_COST]
 int launch_cost(const cosl_ba_solver* s, const BaDev& d, const double* pa, const double* pb, cudaStream_t st) {
-  const bool pr = s->prior.n > 0;
-  const unsigned g = (unsigned)(div_up64(s->N, 256) + (pr ? div_up(s->prior.n, 256) : 0));
+  const int nPr = s->prior.n + s->prior.np;
+  const bool pr = nPr > 0;
+  const unsigned g = (unsigned)(div_up64(s->N, 256) + (pr ? div_up(nPr, 256) : 0));
   if (!g) return COSL_OK;
   const auto k = pick(d.obsL != nullptr, pr, ba_residual_kernel<false, false>, ba_residual_kernel<true, false>,
                       ba_residual_kernel<false, true>, ba_residual_kernel<true, true>);
@@ -1240,17 +1329,15 @@ int launch_cost(const cosl_ba_solver* s, const BaDev& d, const double* pa, const
   return COSL_OK;
 }
 
-// the two linearisation kernels at (d_pa, d_pb) into d's V, eb, W, U, ea (zeroed before); the camera kernel adds
-// the priors in CTAs after those of the observations
+// the two linearisation kernels at (d_pa, d_pb) into d's V, eb, W, U, ea (zeroed before); each adds its kind of
+// prior in CTAs after those of the observations
 int launch_linearize(const cosl_ba_solver* s, const BaDev& d, cudaStream_t st) {
-  const bool pr = s->prior.n > 0;
-  const unsigned gN = (unsigned)div_up64(s->N, 256);
+  const bool pr = s->prior.n > 0, ppr = s->prior.np > 0;
+  const unsigned gN = (unsigned)(div_up64(s->N, 256) + (ppr ? div_up(s->prior.np, 256) : 0));
   const unsigned gC = (unsigned)(div_up64(s->Nc, 128) + (pr ? div_up(s->prior.n, 128) : 0));
-  if (d.obsL) {
-    if (s->N) COSL_LAUNCH(ba_linearize_points<true>, gN, 256, 0, st, d, s->d_pa, s->d_pb);
-  } else {
-    if (s->N) COSL_LAUNCH(ba_linearize_points<false>, gN, 256, 0, st, d, s->d_pa, s->d_pb);
-  }
+  const auto kp = pick(d.obsL != nullptr, ppr, ba_linearize_points<false, false>, ba_linearize_points<true, false>,
+                       ba_linearize_points<false, true>, ba_linearize_points<true, true>);
+  if (gN) COSL_LAUNCH(kp, gN, 256, 0, st, d, s->d_pa, s->d_pb, s->prior);
   const auto k = pick(d.obsL != nullptr, pr, ba_linearize_cams<false, false>, ba_linearize_cams<true, false>,
                       ba_linearize_cams<false, true>, ba_linearize_cams<true, true>);
   if (gC) COSL_LAUNCH(k, gC, 128, 0, st, d, s->d_pa, s->d_pb, s->prior);
@@ -1265,7 +1352,8 @@ int launch_linearize(const cosl_ba_solver* s, const BaDev& d, cudaStream_t st) {
 int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dctl, double mu, int doStats) {
   const unsigned gN = (unsigned)div_up64(s->N, 256);
   const int r0 = rank_of(s) == 0 ? 1 : 0;
-  const bool oc = s->d.obsL != nullptr, pr = s->prior.n > 0;
+  const int nPr = s->prior.n + s->prior.np;
+  const bool oc = s->d.obsL != nullptr, pr = nPr > 0;
   SectionTimer& T = s->timer;
   if (stage == BA_STAGE_ROUND) {  // the round's Tukey weights (on the pixel distance), then its initial cost
     if (s->N) {
@@ -1317,7 +1405,7 @@ int enqueue_stage(cosl_ba_solver* s, cudaStream_t st, int stage, const BaCtl* dc
     T.begin(s->secCost, st);
     // a problem without points or priors never reaches a trial (|g| = 0 stops it), but is captured
     const unsigned gF =
-        (unsigned)(div_up64(s->N + (long long)s->n, 256) + (pr ? div_up(s->prior.n, 256) : 0));
+        (unsigned)(div_up64(s->N + (long long)s->n, 256) + (pr ? div_up(nPr, 256) : 0));
     if (gF) {
       const auto k = pick(oc, pr, ba_finish_cost<false, false>, ba_finish_cost<true, false>,
                           ba_finish_cost<false, true>, ba_finish_cost<true, true>);
@@ -1531,7 +1619,12 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
     else
       COSL_LAUNCH(ba_fill_f64, std::min<unsigned>(gN, 1024), 256, 0, st, s->d_covWgt, s->N, 1.0);
   }
-  if (n) COSL_LAUNCH(ba_cov_mask, div_up(n, 256), 256, 0, st, cd, s->d_covUnc);
+  if (n) {
+    if (s->prior.np)
+      COSL_LAUNCH(ba_cov_mask<true>, div_up(n, 256), 256, 0, st, cd, s->d_covUnc, s->prior);
+    else
+      COSL_LAUNCH(ba_cov_mask<false>, div_up(n, 256), 256, 0, st, cd, s->d_covUnc, s->prior);
+  }
   const long long nV = 9LL * n + 27LL * m;
   COSL_LAUNCH(ba_fill_f64, (unsigned)std::min<long long>(div_up64(nV, 256), 1024), 256, 0, st, s->d_V, nV, 0.0);
   COSL_TRY(launch_linearize(s, cd, st));
@@ -1554,7 +1647,7 @@ int enqueue_cov(cosl_ba_solver* s, cudaStream_t st) {
                 s->d_covT);
   if (n) COSL_LAUNCH(ba_cov_points, div_up(n, 256), 256, 0, st, n, s->ncon, s->d_Vinv, s->d_covT, s->d_covUnc, var,
                      s->d_covPt);
-  COSL_LAUNCH(ba_cov_end, 1, 32, 0, st, s->d_covSc, s->d_covPiv, nb, s->mf, var, s->prior.n);
+  COSL_LAUNCH(ba_cov_end, 1, 32, 0, st, s->d_covSc, s->d_covPiv, nb, s->mf, var, s->prior.n, s->prior.np);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;
 }
@@ -1910,7 +2003,8 @@ int cosl_ba_solver_submit(cosl_ba_solver* s) {
   // the synchronous path swaps d_pa / d_na (d_pb / d_nb) on every accepted trial; the graph holds pointers
   if (!s->graphExec || s->graphStale || s->graphPa != s->d_pa || s->graphNa != s->d_na || s->graphPb != s->d_pb ||
       s->graphNb != s->d_nb || s->graphCovVar != s->covVar || s->graphObsL != s->d.obsL ||
-      s->graphPrior.rec != s->prior.rec || s->graphPrior.n != s->prior.n)
+      s->graphPrior.rec != s->prior.rec || s->graphPrior.n != s->prior.n || s->graphPrior.prec != s->prior.prec ||
+      s->graphPrior.np != s->prior.np)
     COSL_TRY(build_graph(s));
   // the request number goes to the device ahead of the graph, on the solver's stream: a stop made before the
   // graph starts names it too (the pinned source is not rewritten before this request is collected)
@@ -2052,6 +2146,19 @@ int cosl_ba_solver_set_cam_prior(cosl_ba_solver* s, int nPrior, const int32_t* c
   if (nPrior == 0 || !cams) return set_cam_prior(s, 0, nullptr, rec);
   COSL_TRY(check_cam_prior(nPrior, cams, R, t, cov, s->m, s->mcon, rec, "cosl_ba_solver_set_cam_prior"));
   return set_cam_prior(s, nPrior, cams, rec);
+}
+
+int cosl_ba_solver_set_pt_prior(cosl_ba_solver* s, int nPrior, const int32_t* pts, const double* X,
+                                const double* cov) {
+  BA_ENTER(s)
+  if (multi(s))
+    return set_error(COSL_E_INVALID, "cosl_ba_solver_set_pt_prior: a multi-rank solver has no point priors");
+  if (nPrior < 0) return set_error(COSL_E_INVALID, "cosl_ba_solver_set_pt_prior: nPrior %d < 0", nPrior);
+  COSL_TRY(s->rq.idle("cosl_ba_solver_set_pt_prior"));
+  std::vector<double> rec;
+  if (nPrior == 0 || !pts) return set_pt_prior(s, 0, nullptr, rec);
+  COSL_TRY(check_pt_prior(nPrior, pts, X, cov, s->n, s->ncon, rec, "cosl_ba_solver_set_pt_prior"));
+  return set_pt_prior(s, nPrior, pts, rec);
 }
 
 int cosl_ba_solver_download_covariance(cosl_ba_solver* s, double* camCov, double* ptCov, double out[8]) {

@@ -204,12 +204,22 @@ __global__ void __launch_bounds__(256) ba_obscov_factor(double* __restrict__ L, 
 // R0.  The kernels that take a template flag PRIOR add |L r|^2 to the cost and (L J)^T (L J), -(L J)^T L r to U_j and
 // ea_j in CTAs beyond their observation range.  The priors are a kernel argument of their own rather than BaDev
 // fields, so the instantiations without PRIOR keep their parameter layout and code.
+// Point priors (cosl_ba_solver_set_pt_prior, DESIGN.md 4.9) follow the camera ones in the same argument: prior k on
+// free point pt[k] is prec[k] = [L (6: the upper-triangular 3x3 factor with L^T L = P^-1, packed by rows) | mu (3)],
+// its residual r = X - mu.  The PRIOR instantiations of the residual and trial-cost kernels run one thread per prior
+// of either kind, cameras first; ba_linearize_points<PRIOR> adds L^T L and L^T L (mu - X) to V_i and eb_i, and
+// ba_cov_mask<PRIOR> keeps every point with a prior in H (has[i] != 0).
 struct BaPriorDev {
   const double* rec;  // [n][BA_PRIOR_REC]
   const int* cam;     // [n], distinct free cameras
   int n;
+  int np;                    // number of point priors
+  const double* prec;        // [np][BA_PTPRIOR_REC]
+  const int* pt;             // [np], distinct free points
+  const unsigned char* has;  // [n points]: 1 for a point with a prior
 };
 constexpr int BA_PRIOR_REC = 33;
+constexpr int BA_PTPRIOR_REC = 9;
 
 // Whitened prior residual rw = L r of prior k at pa and, with WANT_J, Jw = L dr/d(v, t) (6x6 row-major).
 // Log(M) by atan2 with the axis from the skew part below 120 degrees and from the symmetric part above (exact to
@@ -307,21 +317,48 @@ __device__ __forceinline__ void ba_prior_eval(const BaDev& d, const BaPriorDev& 
   }
 }
 
-// sum over this CTA's priors (one per thread, from prior index k0) of |L r|^2 at pa
-__device__ __forceinline__ double ba_prior_cost(const BaDev& d, const BaPriorDev& pr, long long k0,
+// |L r|^2 of camera prior k at pa
+__device__ __forceinline__ double ba_prior_cost(const BaDev& d, const BaPriorDev& pr, int k,
                                                 const double* __restrict__ pa) {
-  const long long k = k0 + threadIdx.x;
-  if (k >= pr.n) return 0.0;
   double rw[6];
-  ba_prior_eval<false>(d, pr, (int)k, pa, rw, nullptr);
+  ba_prior_eval<false>(d, pr, k, pa, rw, nullptr);
   return rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2] + rw[3] * rw[3] + rw[4] * rw[4] + rw[5] * rw[5];
+}
+
+// Whitened residual rw = L (X - mu) of point prior k
+__device__ __forceinline__ void ba_ptprior_eval(const BaPriorDev& pr, int k, const double X[3], double rw[3]) {
+  const double* __restrict__ q = pr.prec + BA_PTPRIOR_REC * (size_t)k;
+  const double r0 = X[0] - q[6], r1 = X[1] - q[7], r2 = X[2] - q[8];
+  rw[0] = q[0] * r0 + q[1] * r1 + q[2] * r2;
+  rw[1] = q[3] * r1 + q[4] * r2;
+  rw[2] = q[5] * r2;
+}
+
+// |L (X - mu)|^2 of point prior k
+__device__ __forceinline__ double ba_ptprior_cost(const BaPriorDev& pr, int k, const double X[3]) {
+  double rw[3];
+  ba_ptprior_eval(pr, k, X, rw);
+  return rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2];
+}
+
+// The priors' cost of thread k of the CTAs beyond the observations (cameras [0, n), then points [n, n + np)) at
+// (pa, pb)
+__device__ __forceinline__ double ba_priors_cost(const BaDev& d, const BaPriorDev& pr, long long k,
+                                                 const double* __restrict__ pa, const double* __restrict__ pb) {
+  if (k < pr.n) return ba_prior_cost(d, pr, (int)k, pa);
+  k -= pr.n;
+  if (k >= pr.np) return 0.0;
+  const int i = pr.pt[k];
+  const double X[3] = {pb[3 * (size_t)i], pb[3 * (size_t)i + 1], pb[3 * (size_t)i + 2]};
+  return ba_ptprior_cost(pr, (int)k, X);
 }
 
 // ------------------------------------------------------------------------------------------
 // cost / weights / outliers: one observation per thread
 // mode 0: sc[SC_COST] += w |e|^2 ; mode 1: wgt = tukey(|e|, maxErr) ; mode 2: outlier = |e|>=maxErr,
 // sc[SC_COST] += number of outliers.  OBSCOV: mode 0 sums w |L e|^2; modes 1 and 2 stay on the pixel distance |e|
-// (they are launched without it).  PRIOR (mode 0 only): the CTAs beyond the observations add the priors' |L r|^2.
+// (they are launched without it).  PRIOR (mode 0 only): the CTAs beyond the observations add the priors' |L r|^2,
+// one camera or point prior per thread.
 // ------------------------------------------------------------------------------------------
 template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(256)
@@ -350,7 +387,8 @@ ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restr
   }
   if (PRIOR) {
     const long long nb0 = (d.N + blockDim.x - 1) / blockDim.x;
-    if ((long long)blockIdx.x >= nb0) c = ba_prior_cost(d, pr, ((long long)blockIdx.x - nb0) * blockDim.x, pa);
+    if ((long long)blockIdx.x >= nb0)
+      c = ba_priors_cost(d, pr, ((long long)blockIdx.x - nb0) * blockDim.x + threadIdx.x, pa, pb);
   }
   if (mode == 2) {  // number of outliers -> sc[SC_COST] (info[13] of the solver entry points)
     const double t = block_sum_1(c, s_red);
@@ -370,11 +408,34 @@ ba_residual_kernel(BaDev d, const double* __restrict__ pa, const double* __restr
 // ------------------------------------------------------------------------------------------
 // Linearisation, point-major: per observation e, A (2x6), B (2x3) (whitened by L with OBSCOV, scaled by
 // sqrt(w)); stores W_ij = A^T B; collapses V_i = sum B^T B and eb_i = sum B^T e per point with segmented shuffles.
+// PRIOR: the CTAs beyond the observations add one point prior per thread, V_i += L^T L and eb_i += L^T L (mu - X)
+// (eb sums B^T (x - h), and the prior's "x - h" is -r); a prior point that no observation sees gets its V_i here.
 // ------------------------------------------------------------------------------------------
-template <bool OBSCOV>
+template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(256, 2)
-ba_linearize_points(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb) {
+ba_linearize_points(BaDev d, const double* __restrict__ pa, const double* __restrict__ pb, BaPriorDev pr) {
   if (blockIdx.x == 0 && threadIdx.x < 2) d.sc[SC_GINF + threadIdx.x] = 0.0;  // |g|_inf, max diag: set by ba_stats_kernel
+  if (PRIOR) {
+    const long long nb0 = (d.N + blockDim.x - 1) / blockDim.x;
+    if ((long long)blockIdx.x >= nb0) {
+      const long long k = ((long long)blockIdx.x - nb0) * blockDim.x + threadIdx.x;
+      if (k >= pr.np) return;
+      const int i = pr.pt[k];
+      const double* __restrict__ q = pr.prec + BA_PTPRIOR_REC * (size_t)k;
+      const double X[3] = {pb[3 * (size_t)i], pb[3 * (size_t)i + 1], pb[3 * (size_t)i + 2]};
+      double rw[3];
+      ba_ptprior_eval(pr, (int)k, X, rw);
+      const double l00 = q[0], l01 = q[1], l02 = q[2], l11 = q[3], l12 = q[4], l22 = q[5];
+      const double H[6] = {l00 * l00, l00 * l01, l00 * l02, l01 * l01 + l11 * l11, l01 * l02 + l11 * l12,
+                           l02 * l02 + l12 * l12 + l22 * l22};
+      const double g[3] = {l00 * rw[0], l01 * rw[0] + l11 * rw[1], l02 * rw[0] + l12 * rw[1] + l22 * rw[2]};
+#pragma unroll
+      for (int c = 0; c < 6; ++c) atomicAdd(&d.V[6 * (size_t)i + c], H[c]);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) atomicAdd(&d.eb[3 * (size_t)i + c], -g[c]);
+      return;
+    }
+  }
   const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
   double acc[9];
@@ -1022,8 +1083,9 @@ ba_cam_update(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict__
 //  ba_finish_cost: one observation per thread: db_i = V*_i^-1 (e_b,i - t_i) recomputed from the point's
 //    accumulator (read-only here; the FIRST observation of a point stores nb_i = pb_i + db_i and adds the
 //    point-side sums), then the weighted squared residual at (na, nb_i) -> cost (whitened with OBSCOV).  Extra
-//    threads finish the points that have no observation; with PRIOR, the CTAs after those add the priors' |L r|^2
-//    at na.
+//    threads finish the points that have no observation; with PRIOR, the CTAs after those add the priors' |L r|^2,
+//    a camera prior's at na, a point prior's at its trial point recomputed from the accumulator as above (nb is
+//    written by other threads of the launch).
 // Both take mu from ctl, the control block of the submitted loop, when it is set.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -1141,7 +1203,22 @@ ba_finish_cost(BaDev d, const BaCtl* __restrict__ ctl, const double* __restrict_
   }
   if (PRIOR) {
     const long long nb0 = (d.N + d.n + blockDim.x - 1) / blockDim.x;
-    if ((long long)blockIdx.x >= nb0) c = ba_prior_cost(d, pr, ((long long)blockIdx.x - nb0) * blockDim.x, na);
+    if ((long long)blockIdx.x >= nb0) {
+      const long long k = ((long long)blockIdx.x - nb0) * blockDim.x + threadIdx.x;
+      if (k < pr.n) {
+        c = ba_prior_cost(d, pr, (int)k, na);
+      } else if (k < pr.n + (long long)pr.np) {
+        const int kp = (int)(k - pr.n), ip = pr.pt[kp];
+        const double* Iv = Vinv + 6 * (size_t)ip;
+        const double* eb = d.eb + 3 * (size_t)ip;
+        const double t0 = eb[0] - acc3[3 * (size_t)ip], t1 = eb[1] - acc3[3 * (size_t)ip + 1],
+                     t2 = eb[2] - acc3[3 * (size_t)ip + 2];
+        const double X[3] = {pb[3 * (size_t)ip] + (Iv[0] * t0 + Iv[1] * t1 + Iv[2] * t2),
+                             pb[3 * (size_t)ip + 1] + (Iv[1] * t0 + Iv[3] * t1 + Iv[4] * t2),
+                             pb[3 * (size_t)ip + 2] + (Iv[2] * t0 + Iv[4] * t1 + Iv[5] * t2)};
+        c = ba_ptprior_cost(pr, kp, X);
+      }
+    }
   }
   double s = block_sum_1(c, s_red);
   if (threadIdx.x == 0) {
@@ -1190,15 +1267,17 @@ ba_cov_begin(double* __restrict__ sc, double* __restrict__ T, long long nT, int*
 }
 
 // One thread per point: free points with fewer than two observations of non-zero weight are left out of H
-// (their weights are zeroed, unc[i] = 1); counts of the observations and points that enter H.
-__global__ void __launch_bounds__(256) ba_cov_mask(BaDev d, unsigned char* __restrict__ unc) {
+// (their weights are zeroed, unc[i] = 1); counts of the observations and points that enter H.  PRIOR (point
+// priors set): a point with a prior always enters H, its V_i holds P^-1.
+template <bool PRIOR>
+__global__ void __launch_bounds__(256) ba_cov_mask(BaDev d, unsigned char* __restrict__ unc, BaPriorDev pr) {
   __shared__ double s_red[8];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double nobs = 0, npts = 0, nunc = 0;
   if (i < d.n) {
     int k = 0;
     for (long long o = d.ptr[i]; o < d.ptr[i + 1]; ++o) k += d.wgt[o] > 0.0 ? 1 : 0;
-    const bool u = i >= d.ncon && k < 2;
+    const bool u = i >= d.ncon && k < 2 && !(PRIOR && pr.has[i]);
     unc[i] = u ? 1 : 0;
     if (u) {
       for (long long o = d.ptr[i]; o < d.ptr[i + 1]; ++o) d.wgt[o] = 0.0;
@@ -1344,13 +1423,14 @@ ba_cov_points(int n, int ncon, const double* __restrict__ Vinv, const double* __
 }
 
 // The stage's scalars: sigma^2-hat, dof, the minimum relative pivot over the nb blocks, singularity, time, the
-// number of camera priors (each counts as six measurements in dof; their |L r|^2 is in sc[SC_COST])
+// numbers of camera and point priors (each counts as six, resp. three, measurements in dof; their |L r|^2 is in
+// sc[SC_COST])
 __global__ void ba_cov_end(double* __restrict__ sc, const double* __restrict__ piv, int nb, int mf, double var,
-                           int nPrior) {
+                           int nPrior, int nPtPrior) {
   if (threadIdx.x != 0) return;
   double mp = __longlong_as_double(0x7ff0000000000000LL);  // +inf: no free camera, no pivot
   for (int k = 0; k < nb; ++k) mp = fmin(mp, piv[k]);
-  const double dof = 2.0 * sc[COV_NOBS] - 6.0 * mf - 3.0 * sc[COV_NPTS] + 6.0 * nPrior;
+  const double dof = 2.0 * sc[COV_NOBS] - 6.0 * mf - 3.0 * sc[COV_NPTS] + 6.0 * nPrior + 3.0 * nPtPrior;
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   const unsigned long long t0 = *reinterpret_cast<const unsigned long long*>(sc + COV_T0);
@@ -1363,7 +1443,7 @@ __global__ void ba_cov_end(double* __restrict__ sc, const double* __restrict__ p
   out[4] = 1e-6 * (double)(t - t0);
   out[5] = mp;
   out[6] = nPrior;
-  out[7] = 0.0;
+  out[7] = nPtPrior;
 }
 
 }  // namespace coslam

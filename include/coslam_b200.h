@@ -604,8 +604,8 @@ int cosl_ba_solver_progress(cosl_ba_solver* s, double out[8]);
  * H = sum_obs w J^T J over the free parameters and returns diagonal blocks of pixel_var H^-1:
  *   camCov[j]: 6x6, row-major, for (w, t) with R' = exp([w]x) R, t' = t + dt (x_cam = R X + t);
  *   ptCov[i]:  3x3, row-major, for X_i in world coordinates.
- * Fixed cameras and points get zeros.  A free point with fewer than two observations of non-zero weight is
- * left out of H and gets NaN.
+ * Fixed cameras and points get zeros.  A free point with fewer than two observations of non-zero weight and no
+ * point prior (cosl_ba_solver_set_pt_prior) is left out of H and gets NaN; a point with a prior always enters H.
  * pixel_var > 0 arms: every later cosl_ba_solver_run and cosl_ba_solver_submit ends with the covariance
  * stage on the solver's stream (inside the submitted graph for submit, whose collect then reports its time
  * in info[11] too; not run_fixed).  0 disarms.  Arming allocates the stage's buffers (and so does a load
@@ -613,9 +613,11 @@ int cosl_ba_solver_progress(cosl_ba_solver* s, double out[8]);
  * while a submit is in flight. */
 int cosl_ba_solver_set_covariance(cosl_ba_solver* s, double pixel_var);
 /* After run / collect of an armed BA: camCov[m][36], ptCov[n][9] (each nullable);
- * out = {pixel_var, sigma2_hat, dof, unconstrained points, device ms of the stage, min relative pivot, 0, 0}.
+ * out = {pixel_var, sigma2_hat, dof, unconstrained points, device ms of the stage, min relative pivot, camera
+ * priors, point priors}: out[6] and out[7] are the numbers of priors set (0 without them).
  * sigma2_hat = sum w |e|^2 / dof over the observations that enter H, dof = 2 #(those with w > 0) -
- * 6 (free cameras) - 3 (points with a covariance); NaN when dof <= 0: the caller may rescale by
+ * 6 (free cameras) - 3 (points with a covariance); with priors, the numerator gains their sum r^T cov^-1 r and dof
+ * gains 6 per camera prior and 3 per point prior.  NaN when dof <= 0: the caller may rescale by
  * sigma2_hat / pixel_var.  The relative pivots are L_ii^2 / S_ii of the Cholesky factor of the reduced
  * camera system (+inf without free cameras).
  * COSL_E_STATE with no covariance for the resident parameters (none armed yet, or load / reset /
@@ -654,6 +656,26 @@ int cosl_ba_solver_set_obs_cov(cosl_ba_solver* s, const double* covx);
  * COSL_E_STATE while a submit is in flight; COSL_E_INVALID for a NULL handle, a multi-rank solver or nPrior < 0. */
 int cosl_ba_solver_set_cam_prior(cosl_ba_solver* s, int nPrior, const int32_t* cams, const double* R,
                                  const double* t, const double* cov);
+/* Gaussian position priors on free points of the loaded problem (an extension, DESIGN.md 4.9).  Prior k on point
+ * pts[k] has the mean X[k] (3) and the 3x3 covariance cov[k] (row-major) in world coordinates, the chart of ptCov:
+ * its residual is r = X - mu, and the objective gains sum_point_priors r^T cov^-1 r.  Units as for camera priors: a
+ * ptCov of an earlier BA with covariances in px^2 (or with none and pixel_var = 1) is a valid cov as it stands; with
+ * unweighted observations of pixel variance s2, pass ptCov / s2.  Camera and point priors may be set together.
+ * Tukey weights and the outlier pass ignore priors.  The priors enter V and eb, every cost in info and progress, the
+ * statistics behind mu0, and the covariance stage: H gains cov^-1 on the point blocks, a point with a prior always
+ * gets a finite ptCov (also with zero or one weighted observation; an unobserved one has ptCov = pixel_var cov at
+ * its mean), sigma2_hat gains sum r^T cov^-1 r, dof gains 3 per prior, and out[7] of
+ * cosl_ba_solver_download_covariance is the number of point priors.  Priors on three non-collinear points fix the
+ * gauge of a problem without fixed cameras or points.
+ * Validates on the calling thread: pts[k] in [n_con, n) and distinct, every value finite, cov[k] symmetric to 1e-12
+ * relative to its largest diagonal entry and positive definite; otherwise COSL_E_INVALID names the first bad prior
+ * and the handle keeps what it had.  Copies the priors (the caller may reuse its arrays on return), enqueues the
+ * upload on the solver's stream and returns without waiting.  nPrior == 0 or pts == NULL clears.  The priors apply
+ * to every later run, run_fixed and submit; reset keeps them, load clears them.  COSL_E_STATE while a submit is in
+ * flight; COSL_E_INVALID for a NULL handle, a multi-rank solver or nPrior < 0.  cosl_ba_solve(_multi) and the sba
+ * entry points take no priors. */
+int cosl_ba_solver_set_pt_prior(cosl_ba_solver* s, int nPrior, const int32_t* pts, const double* X,
+                                const double* cov);
 /* Per-kernel accumulated device time in ms since create/reset, by name (NULL-terminated list via
  * index): returns name or NULL when idx is out of range. */
 const char* cosl_ba_solver_timer(cosl_ba_solver* s, int idx, double* ms, int* calls);
