@@ -80,6 +80,7 @@ def _load():
     L.cosl_pose_solver_destroy.argtypes = [vp]
     L.cosl_pose_solver_submit.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, cd, vp]
     L.cosl_pose_solver_submit_cov.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, cd, vp]
+    L.cosl_pose_solver_submit_prior.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, cd, vp]
     L.cosl_pose_solver_query.argtypes = [vp, pint]
     L.cosl_pose_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
     L.cosl_pose_solver_stream.argtypes = [vp]
@@ -603,19 +604,30 @@ class PoseSolver(_SolverHandle):
         self._opts = None
         self._npts = []  # points per camera of the last accepted submit: the shapes download_covariance returns
 
-    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, covx=None):
+    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, covx=None, prior=None):
         """cosl_pose_solver_submit: enqueue pose_intracam_batch's solve and return at once; the input arrays
         may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills.
         covx, a list of per-camera [n, 2, 2] or [n, 4] measurement covariances (px^2, in the order of ms_list;
-        None entries for identity), weights the solve through cosl_pose_solver_submit_cov."""
+        None entries for identity), weights the solve through cosl_pose_solver_submit_cov.
+        prior, a list with one entry per camera, None or (R [3, 3], t [3], P [6, 6]): a Gaussian pose prior with
+        mean (R, t) and covariance P in the order (w, dt) of the solver's chart R = R_p exp([w]x), t = t_p + dt
+        (download_covariance's), through cosl_pose_solver_submit_prior."""
         args, opts, keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
-        if covx is None:
-            _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
-        else:
+        cp = None
+        if covx is not None:
             if len(covx) != args[0]:
                 raise ValueError(f"covx has {len(covx)} cameras for {args[0]}")
             covx = [None if a is None else _obs_cov(a, len(keep[3][c])) for c, a in enumerate(covx)]
             cp = (C.c_void_p * args[0])(*[None if a is None else a.ctypes.data for a in covx])
+        if prior is not None:
+            if len(prior) != args[0]:
+                raise ValueError(f"prior has {len(prior)} cameras for {args[0]}")
+            recs = [None if p is None else _pose_prior(*p) for p in prior]
+            pp = (C.c_void_p * args[0])(*[None if r is None else r.ctypes.data for r in recs])
+            _ck(LIB.cosl_pose_solver_submit_prior(self.h, *args[:7], cp, pp, *args[7:], opts))
+        elif covx is None:
+            _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
+        else:
             _ck(LIB.cosl_pose_solver_submit_cov(self.h, *args[:7], cp, *args[7:], opts))
         self._opts = opts
         self._npts = [len(a) for a in keep[3]]
@@ -644,6 +656,14 @@ class PoseSolver(_SolverHandle):
         err = np.empty(sum(npts))
         _ck(LIB.cosl_pose_solver_download_covariance(self.h, _ptr(cov), _ptr(err), _ptr(stats)))
         return cov, np.split(err, np.cumsum(npts)[:-1]), stats
+
+
+def _pose_prior(R, t, P):
+    """One prior record of cosl_pose_solver_submit_prior: R [3, 3], t [3], P [6, 6] as 48 contiguous doubles."""
+    R, t, P = (np.asarray(a, np.float64) for a in (R, t, P))
+    if R.size != 9 or t.size != 3 or P.size != 36:
+        raise ValueError(f"a pose prior is (R [3, 3], t [3], P [6, 6]), got sizes {R.size}, {t.size}, {P.size}")
+    return np.ascontiguousarray(np.concatenate([R.ravel(), t.ravel(), P.ravel()]))
 
 
 def ba_solve(prob, opt):

@@ -11,6 +11,8 @@
 //
 // An armed pose solver handle (cosl_pose_solver_set_covariance) follows the solve with pose_cov_kernel, the
 // covariance of each refined pose with the analytic Jacobian (an extension, not reference parity).
+// cosl_pose_solver_submit_prior anchors cameras with Gaussian pose priors (also an extension): the PRIOR
+// instantiations of both kernels add each prior's whitened residual to the costs, the LM step and the stage's H.
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -159,15 +161,142 @@ __device__ __forceinline__ void whiten(const double* L, double& r0, double& r1) 
   r1 = L[2] * r1;
 }
 
-// The factor pointer of a pose_cov_kernel<true> launch, its one trailing argument.
+// Gaussian pose priors (cosl_pose_solver_submit_prior, DESIGN.md 5.3).  Camera c has a prior when has[c] != 0; its
+// record is rec[c] = [L (21: the upper-triangular 6x6 factor with L^T L = P^-1, packed by rows) | R_p (9, row-major) |
+// t_p (3)], staged by the host.  The records reach the PRIOR instantiations as a trailing argument of their own, so
+// the other instantiations keep their parameter lists and code.
+struct PosePriorDev {
+  const double* rec;  // [C][POSE_PRIOR_REC]
+  const int* has;     // [C]
+};
+constexpr int POSE_PRIOR_REC = 33;
+
+// The trailing arguments of a launch: the factors of an OBSCOV launch (const double*), then the priors of a PRIOR one.
 __device__ __forceinline__ const double* factors_arg() { return nullptr; }
 __device__ __forceinline__ const double* factors_arg(const double* L) { return L; }
+__device__ __forceinline__ const double* factors_arg(PosePriorDev) { return nullptr; }
+__device__ __forceinline__ const double* factors_arg(const double* L, PosePriorDev) { return L; }
+__device__ __forceinline__ PosePriorDev prior_arg() { return PosePriorDev{nullptr, nullptr}; }
+__device__ __forceinline__ PosePriorDev prior_arg(const double*) { return PosePriorDev{nullptr, nullptr}; }
+__device__ __forceinline__ PosePriorDev prior_arg(PosePriorDev p) { return p; }
+__device__ __forceinline__ PosePriorDev prior_arg(const double*, PosePriorDev p) { return p; }
 
-// intraCamWeightedCost (:439-456); OBSCOV whitens each residual by Ls (3 per point) before the weight
-template <bool OBSCOV>
+// This CTA's prior record, or nullptr for a camera without a prior (uniform over the CTA)
+__device__ __forceinline__ const double* prior_record(const PosePriorDev& pr) {
+  return pr.has[blockIdx.x] ? pr.rec + POSE_PRIOR_REC * (size_t)blockIdx.x : nullptr;
+}
+
+// Whitened prior residual rw = L r at (R, t), r = [Log(R_p^T R); t - t_p], and with WANT_J, Jw = L dr/d(dw, dt)
+// (6x6 row-major) for the solver's update R' = R exp([dw]x), t' = t + dt.  Log(M) by atan2 with the axis from the
+// skew part below 120 degrees and from the symmetric part above (exact to roundoff up to pi).  dr_w / ddw =
+// Jr^-1(r_w), the inverse right Jacobian of SO(3), Jr^-1(w) = I + [w]x / 2 + (1 - (th / 2) cot(th / 2)) / th^2 [w]x^2,
+// and dr_t / ddt = I.  q is the record, read from global memory where it is used.
+template <bool WANT_J>
+__device__ __forceinline__ void prior_eval(const double* __restrict__ q, const double R[9], const double t[3],
+                                           double rw[6], double Jw[36]) {
+  double M[9];  // R_p^T R
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) M[3 * a + b] = q[21 + a] * R[b] + q[24 + a] * R[3 + b] + q[27 + a] * R[6 + b];
+  const double s[3] = {0.5 * (M[7] - M[5]), 0.5 * (M[2] - M[6]), 0.5 * (M[3] - M[1])};
+  const double sn = sqrt(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]);
+  const double cs = 0.5 * (M[0] + M[4] + M[8] - 1.0);
+  const double th = atan2(sn, cs);
+  double r[6];
+  if (cs > -0.5) {
+    const double f = th < 1e-4 ? 1.0 + th * th / 6.0 : th / sn;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) r[a] = f * s[a];
+  } else {  // (M + M^T) / 2 - cos th I = (1 - cos th) a a^T: the column of the largest diagonal entry
+    const double S0 = M[0] - cs, S1 = M[4] - cs, S2 = M[8] - cs;
+    const double s01 = 0.5 * (M[1] + M[3]), s02 = 0.5 * (M[2] + M[6]), s12 = 0.5 * (M[5] + M[7]);
+    const int c = (S0 >= S1 && S0 >= S2) ? 0 : (S1 >= S2 ? 1 : 2);
+    const double col[3] = {c == 0 ? S0 : (c == 1 ? s01 : s02), c == 0 ? s01 : (c == 1 ? S1 : s12),
+                           c == 0 ? s02 : (c == 1 ? s12 : S2)};
+    const double f = th / sqrt((1.0 - cs) * (c == 0 ? S0 : (c == 1 ? S1 : S2)));
+    const double sg = (col[0] * s[0] + col[1] * s[1] + col[2] * s[2]) < 0.0 ? -f : f;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) r[a] = sg * col[a];
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) r[3 + a] = t[a] - q[30 + a];
+  // rw = L r, L packed by rows: row a holds L[a][a .. 5] from offset 6a - a(a-1)/2
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const int off = 6 * a - a * (a - 1) / 2;
+    double v = 0.0;
+#pragma unroll
+    for (int b = a; b < 6; ++b) v += q[off + b - a] * r[b];
+    rw[a] = v;
+  }
+  if (!WANT_J) return;
+  // cot(th / 2) = sin th / (1 - cos th) = sn / (|(sn, cs)| - cs): no trigonometric call, exact up to pi
+  const double c2 = th < 1e-2 ? 1.0 / 12.0 + th * th * (1.0 / 720.0 + th * th / 30240.0)
+                              : (1.0 - 0.5 * th * sn / (sqrt(sn * sn + cs * cs) - cs)) / (th * th);
+  const double wx[9] = {0.0, -r[2], r[1], r[2], 0.0, -r[0], -r[1], r[0], 0.0};
+  double Ji[9];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      const double w2 = wx[3 * a] * wx[b] + wx[3 * a + 1] * wx[3 + b] + wx[3 * a + 2] * wx[6 + b];
+      Ji[3 * a + b] = (a == b ? 1.0 : 0.0) + 0.5 * wx[3 * a + b] + c2 * w2;
+    }
+  // Jw = L diag(Ji, I)
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const int off = 6 * a - a * (a - 1) / 2;
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      double v = 0.0;
+#pragma unroll
+      for (int c = a; c < 3; ++c) v += q[off + c - a] * Ji[3 * c + b];
+      Jw[6 * a + b] = v;
+    }
+#pragma unroll
+    for (int b = 3; b < 6; ++b) Jw[6 * a + b] = b >= a ? q[off + b - a] : 0.0;
+  }
+}
+
+// |L r|^2 of the prior record q at (R, t)
+__device__ __forceinline__ double prior_cost(const double* __restrict__ q, const double R[9], const double t[3]) {
+  double rw[6];
+  prior_eval<false>(q, R, t, rw, nullptr);
+  return rw[0] * rw[0] + rw[1] * rw[1] + rw[2] * rw[2] + rw[3] * rw[3] + rw[4] * rw[4] + rw[5] * rw[5];
+}
+
+// acc (21 upper-triangle entries of a 6x6 system, then its 6 right-hand-side entries) += the prior's rows at (R, t):
+// (L J)^T (L J) and -(L J)^T L r
+__device__ __forceinline__ void prior_normal(const double* __restrict__ q, const double R[9], const double t[3],
+                                             double acc[27]) {
+  double rw[6], Jw[36];
+  prior_eval<true>(q, R, t, rw, Jw);
+  int k = 0;
+#pragma unroll
+  for (int a = 0; a < 6; ++a)
+#pragma unroll
+    for (int b = a; b < 6; ++b) {
+      double v = 0.0;
+#pragma unroll
+      for (int c = 0; c < 6; ++c) v += Jw[6 * c + a] * Jw[6 * c + b];
+      acc[k++] += v;
+    }
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    double v = 0.0;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) v += Jw[6 * c + a] * rw[c];
+    acc[21 + a] -= v;
+  }
+}
+
+// intraCamWeightedCost (:439-456); OBSCOV whitens each residual by Ls (3 per point) before the weight; PRIOR adds
+// |L r|^2 of the prior record Pq when the camera has one (Pq != nullptr, uniform over the CTA)
+template <bool OBSCOV, bool PRIOR>
 __device__ double weighted_cost(const double K[9], const double R[9], const double t[3], int n,
                                 const double* Ws, const double* Ms, const double* ms, const double* Ls,
-                                double* s_red) {
+                                double* s_red, const double* Pq) {
   double err[1] = {0};
   for (int i = threadIdx.x; i < n; i += POSE_THREADS) {
     double rm[2];
@@ -177,15 +306,17 @@ __device__ double weighted_cost(const double K[9], const double R[9], const doub
     err[0] += (dx * dx + dy * dy) * Ws[i];
   }
   block_sum<1>(err, s_red);
+  if (PRIOR && Pq) err[0] += prior_cost(Pq, R, t);
   return err[0];
 }
 
-// intraCamWeightedLMStep (:259-303); OBSCOV whitens the residual and both Jacobian rows by Ls before the weight
-template <bool OBSCOV>
+// intraCamWeightedLMStep (:259-303); OBSCOV whitens the residual and both Jacobian rows by Ls before the weight;
+// PRIOR adds the rows of the prior record Pq (when not nullptr, uniform over the CTA) before lambda, unweighted
+template <bool OBSCOV, bool PRIOR>
 __device__ void weighted_step(const double K[9], const double R[9], const double t[3], int n,
                               const double* Ws, const double* Ms, const double* ms, const double* Ls,
                               double param[6], double lambda, const double dRk[3][9],
-                              double* s_red) {
+                              double* s_red, const double* Pq) {
   const double eps = 1e-8;
   double acc[27];  // 21 upper-triangle entries of J^T J + 6 of J^T r
 #pragma unroll
@@ -231,6 +362,7 @@ __device__ void weighted_step(const double K[9], const double R[9], const double
     for (int a = 0; a < 6; ++a) acc[21 + a] += J[a] * r0 + J[6 + a] * r1;
   }
   block_sum<27>(acc, s_red);
+  if (PRIOR && Pq) prior_normal(Pq, R, t, acc);
   double sA[36], inv[36];
   int q = 0;
   for (int a = 0; a < 6; ++a)
@@ -253,13 +385,18 @@ __device__ void weighted_step(const double K[9], const double R[9], const double
 
 // OBSCOV: every residual and Jacobian row is whitened by the factors LAll (3 per point, packed as the points;
 // cosl_pose_solver_submit_cov).  The false instantiation never reads LAll and is the unweighted solve.
-template <bool OBSCOV>
+// PRIOR (cosl_pose_solver_submit_prior): the one trailing argument holds the priors; a camera with one adds its
+// |L r|^2 to every cost and its rows to every LM step, a camera without one computes what the launch without PRIOR
+// computes.
+template <bool OBSCOV, bool PRIOR = false, typename... Priors>
 __global__ void __launch_bounds__(POSE_THREADS)
 pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
                      const double* __restrict__ msAll, const double* __restrict__ prevAll,
                      double* __restrict__ WsAll, PoseCfg cfg, PoseOut* __restrict__ outs,
-                     const double* __restrict__ LAll) {
+                     const double* __restrict__ LAll, Priors... prior) {
+  static_assert(sizeof...(Priors) == (PRIOR ? 1 : 0), "a PRIOR launch passes the priors, no other does");
   __shared__ double s_red[(POSE_THREADS / 32) * 27];
+  const double* Pq = PRIOR ? prior_record(prior_arg(prior...)) : nullptr;
   const PoseCam cam = cams[blockIdx.x];
   const int n = cam.npts;
   const double* Ms = MsAll + 3 * cam.off;
@@ -295,7 +432,7 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
     // ---- intraCamWeightedLMProc (:475-549) from (R, t) ----
     double param[6];
     lambda = lambda0;
-    err0 = weighted_cost<OBSCOV>(K, R, t, n, Ws, Ms, ms, Ls, s_red);
+    err0 = weighted_cost<OBSCOV, PRIOR>(K, R, t, n, Ws, Ms, ms, Ls, s_red, Pq);
     errLM = err0;
     for (int q = 0; q < 9; ++q) {
       Rlm[q] = R[q];
@@ -309,7 +446,7 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
     int i = 0;
     double err = err0;
     for (; i < cfg.maxIterLM; ++i) {
-      weighted_step<OBSCOV>(K, Rlm, tlm, n, Ws, Ms, ms, Ls, param, lambda, dRk, s_red);
+      weighted_step<OBSCOV, PRIOR>(K, Rlm, tlm, n, Ws, Ms, ms, Ls, param, lambda, dRk, s_red, Pq);
       {  // intraCamUpdatePose (:367-380)
         double dR[9];
         so3_exp(param, dR);
@@ -326,7 +463,7 @@ pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict_
         retType = 0;
         break;
       }
-      err = weighted_cost<OBSCOV>(K, R_opt, t_opt, n, Ws, Ms, ms, Ls, s_red);
+      err = weighted_cost<OBSCOV, PRIOR>(K, R_opt, t_opt, n, Ws, Ms, ms, Ls, s_red, Pq);
       if (fabs(err - errLM) < cfg.epsErr) {
         retType = 0;
         break;
@@ -414,12 +551,15 @@ constexpr int POSE_COV_STRIDE = 40;
 // sigma2_hat = sum w |L_i (project - m_i)|^2 / dof; e_i and w_i stay on the pixel distance.
 // The factors travel as a trailing argument of the OBSCOV launch only: the unweighted kernel keeps the parameter
 // list it had before measurement covariances, and with it its code (an unused parameter changes its registers).
-template <bool OBSCOV, typename... Factors>
+// PRIOR (cosl_pose_solver_submit_prior): the priors follow as the last trailing argument.  A camera with a prior adds
+// (L J_p)^T (L J_p) to H and |L r|^2 to sigma2_hat's numerator at (R_opt, t_opt), and 6 to dof.
+template <bool OBSCOV, bool PRIOR = false, typename... Extra>
 __global__ void __launch_bounds__(POSE_THREADS)
 pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
                 const double* __restrict__ msAll, const PoseOut* __restrict__ outs, double tau, double pixel_var,
-                double* __restrict__ res, double* __restrict__ errAll, Factors... LAll) {
-  static_assert(sizeof...(Factors) == (OBSCOV ? 1 : 0), "an OBSCOV launch passes the factors, no other does");
+                double* __restrict__ res, double* __restrict__ errAll, Extra... LAll) {
+  static_assert(sizeof...(Extra) == (OBSCOV ? 1 : 0) + (PRIOR ? 1 : 0),
+                "an OBSCOV launch passes the factors and a PRIOR launch the priors, no other does");
   __shared__ double s_red[(POSE_THREADS / 32) * 23];
   const PoseCam& cam = cams[blockIdx.x];
   const int n = cam.npts;
@@ -486,6 +626,19 @@ pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsA
   }
   block_sum<23>(acc, s_red);
   if (threadIdx.x != 0) return;
+  if constexpr (PRIOR) {  // discarded without PRIOR, so the other instantiations keep their code
+    const double* Pq = prior_record(prior_arg(LAll...));
+    if (Pq) {
+      double hb[27];  // the prior's 21 entries of H; its 6 right-hand-side entries are not needed here
+#pragma unroll
+      for (int k = 0; k < 27; ++k) hb[k] = 0;
+      prior_normal(Pq, R, t, hb);
+#pragma unroll
+      for (int k = 0; k < 21; ++k) acc[k] += hb[k];
+      acc[21] += prior_cost(Pq, R, t);
+      acc[22] += 3;  // six measurements: dof = 2 #(w > 0) - 6 + 6
+    }
+  }
   // Cholesky H = L L^T in packed lower storage, L(i, j) at i (i + 1) / 2 + j
   double L[21];
   double minPiv = INFINITY;
@@ -605,12 +758,96 @@ int check_covx(const char* fn, int C, const int* npts, const double* const* covx
   return COSL_OK;
 }
 
+// Cholesky A = G G^T of a symmetric positive definite 6x6 (row-major; G lower, row-major); false on a pivot that is
+// not positive and finite.
+bool chol6(const double* A, double* G) {
+  for (int i = 0; i < 36; ++i) G[i] = 0.0;
+  for (int j = 0; j < 6; ++j) {
+    double d = A[7 * j];
+    for (int k = 0; k < j; ++k) d -= G[6 * j + k] * G[6 * j + k];
+    if (!(d > 0.0) || !std::isfinite(d)) return false;
+    G[7 * j] = std::sqrt(d);
+    for (int i = j + 1; i < 6; ++i) {
+      double v = A[6 * i + j];
+      for (int k = 0; k < j; ++k) v -= G[6 * i + k] * G[6 * j + k];
+      G[6 * i + j] = v / G[7 * j];
+    }
+  }
+  return true;
+}
+
+// Checks camera c's prior record p (R_p[9] row-major | t_p[3] | P[36] row-major in the order (w, dt)) and, when out is
+// not nullptr, writes its POSE_PRIOR_REC doubles: the upper-triangular L with L^T L = P^-1 packed by rows, R_p, t_p.
+// R_p must be a rotation (|R_p^T R_p - I|_max <= 1e-9, det > 0), every value finite, P symmetric to 1e-12 of its
+// largest diagonal entry and positive definite; otherwise COSL_E_INVALID names camera c.
+int prior_factor(const char* fn, int c, const double* p, double* out) {
+  const double *Rp = p, *tp = p + 9, *P = p + 12;
+  for (int i = 0; i < 48; ++i)
+    if (!std::isfinite(p[i])) return set_error(COSL_E_INVALID, "%s: prior of camera %d is not finite", fn, c);
+  double orth = 0.0;
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) {
+      const double g = Rp[a] * Rp[b] + Rp[3 + a] * Rp[3 + b] + Rp[6 + a] * Rp[6 + b] - (a == b ? 1.0 : 0.0);
+      orth = std::max(orth, std::fabs(g));
+    }
+  const double det = Rp[0] * (Rp[4] * Rp[8] - Rp[5] * Rp[7]) - Rp[1] * (Rp[3] * Rp[8] - Rp[5] * Rp[6]) +
+                     Rp[2] * (Rp[3] * Rp[7] - Rp[4] * Rp[6]);
+  if (orth > 1e-9 || !(det > 0.0))
+    return set_error(COSL_E_INVALID, "%s: R of camera %d's prior is not a rotation (|R^T R - I| %.3g, det %.17g)", fn,
+                     c, orth, det);
+  double pmax = 0.0;
+  for (int i = 0; i < 6; ++i) pmax = std::max(pmax, std::fabs(P[7 * i]));
+  for (int a = 0; a < 6; ++a)
+    for (int b = a + 1; b < 6; ++b)
+      if (std::fabs(P[6 * a + b] - P[6 * b + a]) > 1e-12 * pmax)
+        return set_error(COSL_E_INVALID, "%s: P of camera %d's prior is not symmetric (%d, %d)", fn, c, a, b);
+  // P = G G^T, P^-1 = G^-T G^-1 = C C^T and L = C^T
+  double S[36], G[36], Gi[36] = {}, Pi[36], C[36];
+  for (int a = 0; a < 6; ++a)
+    for (int b = 0; b < 6; ++b) S[6 * a + b] = 0.5 * (P[6 * a + b] + P[6 * b + a]);
+  if (!chol6(S, G)) return set_error(COSL_E_INVALID, "%s: P of camera %d's prior is not positive definite", fn, c);
+  for (int k = 0; k < 6; ++k)  // G^-1, lower, by forward substitution of the unit columns
+    for (int i = k; i < 6; ++i) {
+      double a = i == k ? 1.0 : 0.0;
+      for (int q = k; q < i; ++q) a -= G[6 * i + q] * Gi[6 * q + k];
+      Gi[6 * i + k] = a / G[6 * i + i];
+    }
+  for (int a = 0; a < 6; ++a)
+    for (int b = 0; b < 6; ++b) {
+      double u = 0.0;
+      for (int q = std::max(a, b); q < 6; ++q) u += Gi[6 * q + a] * Gi[6 * q + b];
+      Pi[6 * a + b] = u;
+    }
+  if (!chol6(Pi, C)) return set_error(COSL_E_INVALID, "%s: P of camera %d's prior is not positive definite", fn, c);
+  if (!out) return COSL_OK;
+  int q = 0;
+  for (int a = 0; a < 6; ++a)
+    for (int b = a; b < 6; ++b) out[q++] = C[6 * b + a];
+  for (int i = 0; i < 9; ++i) out[21 + i] = Rp[i];
+  for (int i = 0; i < 3; ++i) out[30 + i] = tp[i];
+  return COSL_OK;
+}
+
+// Checks every prior of prior (nullable, as prior[c]) with prior_factor, naming the first bad camera; *any = some
+// camera has one.
+int check_priors(const char* fn, int C, const double* const* prior, bool* any) {
+  *any = false;
+  if (!prior) return COSL_OK;
+  for (int c = 0; c < C; ++c) {
+    if (!prior[c]) continue;
+    COSL_TRY(prior_factor(fn, c, prior[c], nullptr));
+    *any = true;
+  }
+  return COSL_OK;
+}
+
 }  // namespace
 
 // A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out as
-// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] | L[3 tot] (tot = points of the solve; the whitening factors L
-// are staged and copied by cosl_pose_solver_submit_cov only); the PoseOuts come back into pinned memory.  Capacity
-// is fixed at create: everything is allocated once, the covariance stage's buffers (laid out as
+// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] | L[3 tot] | prior[C][POSE_PRIOR_REC] | hasPrior[C] (tot =
+// points of the solve; the whitening factors L are staged and copied by the submits with covariances only, and the
+// priors, right after the last section copied, by a submit with some prior); the PoseOuts come back into pinned
+// memory.  Capacity is fixed at create: everything is allocated once, the covariance stage's buffers (laid out as
 // res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed.
 struct cosl_pose_solver {
   int device = 0, maxCams = 0, maxPts = 0;
@@ -627,6 +864,7 @@ struct cosl_pose_solver {
   double* h_cov = nullptr;
   bool covReady = false;  // the last submitted solve was armed
   bool obsCov = false;    // the solve in flight carries measurement covariances
+  bool prior = false;     // the solve in flight carries pose priors
 };
 
 namespace {
@@ -634,6 +872,11 @@ namespace {
 size_t input_bytes(int C, long long tot) { return sizeof(PoseCam) * C + sizeof(double) * 6 * tot; }
 // the staged inputs followed by the whitening factors of cosl_pose_solver_submit_cov
 size_t input_bytes_cov(int C, long long tot) { return input_bytes(C, tot) + sizeof(double) * 3 * tot; }
+// the prior records and flags of cosl_pose_solver_submit_prior, staged after the inputs
+size_t prior_bytes(int C) { return (sizeof(double) * POSE_PRIOR_REC + sizeof(int)) * C; }
+size_t prior_offset(int C, long long tot, bool obsCov) {
+  return obsCov ? input_bytes_cov(C, tot) : input_bytes(C, tot);
+}
 
 void free_pose_solver(cosl_pose_solver* s) {
   cudaSetDevice(s->device);
@@ -653,7 +896,7 @@ size_t cov_doubles(int C, long long tot) { return (size_t)POSE_COV_STRIDE * C + 
 int alloc_pose_solver(cosl_pose_solver* s) {
   COSL_CUDA(cudaSetDevice(s->device));
   COSL_TRY(s->rq.create());
-  const size_t in = input_bytes_cov(s->maxCams, s->maxPts);
+  const size_t in = input_bytes_cov(s->maxCams, s->maxPts) + prior_bytes(s->maxCams);
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
   COSL_CUDA(cudaHostAlloc(&s->h_out, sizeof(PoseOut) * s->maxCams, cudaHostAllocPortable));
   COSL_CUDA(cudaMalloc(&s->d_in, in));
@@ -662,18 +905,34 @@ int alloc_pose_solver(cosl_pose_solver* s) {
   return COSL_OK;
 }
 
+// The PRIOR instantiations, named: their template argument lists do not fit the launch macro
+constexpr auto pose_intracam_prior = pose_intracam_kernel<false, true, PosePriorDev>;
+constexpr auto pose_intracam_obscov_prior = pose_intracam_kernel<true, true, PosePriorDev>;
+constexpr auto pose_cov_prior = pose_cov_kernel<false, true, PosePriorDev>;
+constexpr auto pose_cov_obscov_prior = pose_cov_kernel<true, true, const double*, PosePriorDev>;
+
 // The staged inputs of C cameras and tot points: copy, kernel, read-back.  s->obsCov selects the whitened
-// instantiations and copies the factors with the rest.
+// instantiations and copies the factors with the rest; s->prior the PRIOR instantiations and the prior records.
 int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg) {
   const PoseCam* d_cams = reinterpret_cast<const PoseCam*>(s->d_in);
   const double* d_M = reinterpret_cast<const double*>(s->d_in + sizeof(PoseCam) * C);
   const double* d_m = d_M + 3 * tot;
   const double* d_p = d_m + 2 * tot;
   const double* d_L = d_p + tot;
+  const size_t poff = prior_offset(C, tot, s->obsCov);
+  PosePriorDev pr;
+  pr.rec = reinterpret_cast<const double*>(s->d_in + poff);
+  pr.has = reinterpret_cast<const int*>(s->d_in + poff + sizeof(double) * POSE_PRIOR_REC * C);
   cudaStream_t st = s->rq.stream;
-  const size_t bytes = s->obsCov ? input_bytes_cov(C, tot) : input_bytes(C, tot);
+  const size_t bytes = s->prior ? poff + prior_bytes(C) : poff;
   COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, bytes, cudaMemcpyHostToDevice, st));
-  if (s->obsCov)
+  if (s->prior && s->obsCov)
+    COSL_LAUNCH(pose_intracam_obscov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg,
+                s->d_out, d_L, pr);
+  else if (s->prior)
+    COSL_LAUNCH(pose_intracam_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg,
+                s->d_out, nullptr, pr);
+  else if (s->obsCov)
     COSL_LAUNCH(pose_intracam_kernel<true>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out,
                 d_L);
   else
@@ -684,7 +943,13 @@ int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg)
   if (s->pixelVar > 0) {
     double* d_res = s->d_cov;
     double* d_err = s->d_cov + POSE_COV_STRIDE * C;
-    if (s->obsCov)
+    if (s->prior && s->obsCov)
+      COSL_LAUNCH(pose_cov_obscov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau,
+                  s->pixelVar, d_res, d_err, d_L, pr);
+    else if (s->prior)
+      COSL_LAUNCH(pose_cov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau,
+                  s->pixelVar, d_res, d_err, pr);
+    else if (s->obsCov)
       COSL_LAUNCH(pose_cov_kernel<true>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar,
                   d_res, d_err, d_L);
     else
@@ -696,10 +961,11 @@ int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg)
   return COSL_OK;
 }
 
-// cosl_pose_solver_submit (covx == nullptr) and cosl_pose_solver_submit_cov; fn names the caller in messages.
+// cosl_pose_solver_submit (covx == prior == nullptr), cosl_pose_solver_submit_cov (prior == nullptr) and
+// cosl_pose_solver_submit_prior; fn names the caller in messages.
 int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
                  const int* npts, const double* const* Ms, const double* const* ms, const double* const* covx,
-                 const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
+                 const double* const* prior, const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
   if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
   COSL_TRY(s->rq.idle(fn));
   if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !opts)
@@ -711,6 +977,8 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   if (tot > s->maxPts)
     return set_error(COSL_E_INVALID, "%s: %lld points exceed the handle's %d", fn, tot, s->maxPts);
   COSL_TRY(check_covx(fn, C, npts, covx));
+  bool anyPrior = false;
+  COSL_TRY(check_priors(fn, C, prior, &anyPrior));
   COSL_CUDA(cudaSetDevice(s->device));
   // nothing is in flight, so no copy reads the staging buffer any more
   PoseCam* cams = reinterpret_cast<PoseCam*>(s->h_in);
@@ -746,6 +1014,16 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
     }
     off += npts[c];
   }
+  if (anyPrior) {
+    const size_t poff = prior_offset(C, tot, covx != nullptr);
+    double* hq = reinterpret_cast<double*>(s->h_in + poff);
+    int* hh = reinterpret_cast<int*>(s->h_in + poff + sizeof(double) * POSE_PRIOR_REC * C);
+    for (int c = 0; c < C; ++c) {
+      hh[c] = prior[c] ? 1 : 0;
+      // a camera without a prior leaves its record unset: the kernels do not read it
+      if (prior[c]) prior_factor(fn, c, prior[c], hq + POSE_PRIOR_REC * (size_t)c);
+    }
+  }
   PoseCfg cfg;
   cfg.maxIterLM = opts[0].maxIterLM;
   cfg.maxIterRW = opts[0].maxIterRW;
@@ -758,6 +1036,7 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   s->tot = tot;
   s->covReady = false;
   s->obsCov = covx != nullptr;
+  s->prior = anyPrior;
   COSL_TRY(s->rq.submit(fn, [&]() { return enqueue_solve(s, C, tot, cfg); }));
   s->covReady = s->pixelVar > 0;
   return COSL_OK;
@@ -806,14 +1085,24 @@ int cosl_pose_solver_destroy(cosl_pose_solver* s) {
 int cosl_pose_solver_submit(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
                             const int* npts, const double* const* Ms, const double* const* ms,
                             const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
-  return submit_solve("cosl_pose_solver_submit", s, C, K9, R0, t0, npts, Ms, ms, nullptr, prevErrs, tau, opts);
+  return submit_solve("cosl_pose_solver_submit", s, C, K9, R0, t0, npts, Ms, ms, nullptr, nullptr, prevErrs, tau,
+                      opts);
 }
 
 int cosl_pose_solver_submit_cov(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
                                 const int* npts, const double* const* Ms, const double* const* ms,
                                 const double* const* covx, const double* const* prevErrs, double tau,
                                 const cosl_pose_opt* opts) {
-  return submit_solve("cosl_pose_solver_submit_cov", s, C, K9, R0, t0, npts, Ms, ms, covx, prevErrs, tau, opts);
+  return submit_solve("cosl_pose_solver_submit_cov", s, C, K9, R0, t0, npts, Ms, ms, covx, nullptr, prevErrs, tau,
+                      opts);
+}
+
+int cosl_pose_solver_submit_prior(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
+                                  const int* npts, const double* const* Ms, const double* const* ms,
+                                  const double* const* covx, const double* const* prior,
+                                  const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
+  return submit_solve("cosl_pose_solver_submit_prior", s, C, K9, R0, t0, npts, Ms, ms, covx, prior, prevErrs, tau,
+                      opts);
 }
 
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done) {

@@ -424,6 +424,36 @@ int cosl_pose_solver_submit_cov(cosl_pose_solver* s, int C, const double* K9, co
                                 const double* t0, const int* npts, const double* const* Ms,
                                 const double* const* ms, const double* const* covx,
                                 const double* const* prevErrs, double tau, const cosl_pose_opt* opts);
+/* submit with Gaussian pose priors (an extension: intraCamEstimate solves every frame from the
+ * observations alone; DESIGN.md 5.3).  prior == NULL is cosl_pose_solver_submit_cov exactly; otherwise
+ * prior[c] is NULL (no prior on camera c) or 48 doubles: R_p[9] row-major, t_p[3], P[36] row-major, a
+ * mean (R_p, t_p) and a 6x6 covariance P in the order (w, dt) of the solver's own chart, the chart of
+ * download_covariance: R = R_p exp([w]x), t = t_p + dt.  So a download_covariance block is a valid P.
+ * With the upper-triangular L, L^T L = P^-1, computed on the calling thread:
+ *   the prior residual is r = [Log(R_p^T R); t - t_p] (Log exact to roundoff up to pi), and the
+ *   objective sum_i w_i |L_i (m_i - pi(K, R, t, M_i))|^2 + r^T P^-1 r (L_i = I without covx);
+ *   the observation rows are those of cosl_pose_solver_submit_cov; the prior adds the six rows L J_p,
+ *   residual L r, with J_p = diag(Jr^-1(r_w), I) for the update R' = R exp([dw]x), t' = t + dt
+ *   (Jr^-1 the inverse right Jacobian of SO(3)): (L J_p)^T (L J_p) joins the LM system and
+ *   -(L J_p)^T (L r) its right-hand side before lambda is added, with no Tukey weight;
+ *   every cost the loop evaluates gains |L r|^2, so opts[c].err0, err and errRW include it and
+ *   the LM and re-weighting tests see it; the Tukey weights, prevErrs and download_covariance's err
+ *   stay on the pixel distance.
+ * An armed handle's covariance stage adds J_p^T P^-1 J_p to H at the answer, 6 to dof and r^T P^-1 r
+ * to sigma2_hat's numerator: a camera with a prior and 0, 1 or 2 weighted points is regular, and an
+ * unobserved camera (npts 0) with a prior converges to its mean with cov = pixel_var P.  With covx
+ * in px^2 (or none and pixel_var = 1) a stored pose covariance is a valid P as it stands; with
+ * unweighted observations of pixel variance s2, pass cov / s2.
+ * Every prior is checked before anything is staged: |R_p^T R_p - I|_max <= 1e-9 and det R_p > 0,
+ * every value finite, P symmetric to 1e-12 of its largest diagonal entry and positive definite;
+ * else COSL_E_INVALID naming the first bad camera, and the handle stays usable.  Everything else is
+ * cosl_pose_solver_submit_cov's: covx (nullable per camera), its checks and codes, COSL_E_STATE
+ * while a solve is in flight, and query, collect and download_covariance. */
+int cosl_pose_solver_submit_prior(cosl_pose_solver* s, int C, const double* K9, const double* R0,
+                                  const double* t0, const int* npts, const double* const* Ms,
+                                  const double* const* ms, const double* const* covx,
+                                  const double* const* prior, const double* const* prevErrs, double tau,
+                                  const cosl_pose_opt* opts);
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done);
 int cosl_pose_solver_collect(cosl_pose_solver* s, double* R_opt, double* t_opt, cosl_pose_opt* opts,
                              int* ok, double* device_ms);
