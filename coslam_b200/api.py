@@ -87,6 +87,10 @@ def _load():
     L.cosl_pose_solver_stream.restype = vp
     L.cosl_pose_solver_set_covariance.argtypes = [vp, cd]
     L.cosl_pose_solver_download_covariance.argtypes = [vp, vp, vp, vp]
+    L.cosl_pose_solver_reserve_mappts.argtypes = [vp, ci]
+    L.cosl_pose_solver_submit_mappts.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, cd, vp,
+                                                 vp, vp, vp, vp, vp, cd]
+    L.cosl_pose_solver_download_mappts.argtypes = [vp, vp, vp, vp, vp]
     L.cosl_ba_options_default.argtypes = [C.POINTER(BaOptions)]
     L.cosl_ba_solve.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp]
     L.cosl_ba_solve_multi.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), ci, vp, vp]
@@ -603,17 +607,27 @@ class PoseSolver(_SolverHandle):
         self.h, self.device, self.max_cams, self.max_pts = h, device, max_cams, max_pts
         self._opts = None
         self._npts = []  # points per camera of the last accepted submit: the shapes download_covariance returns
+        self._nmap = []  # map points per camera of the last accepted submit_mappts
 
-    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, covx=None, prior=None):
+    def reserve_mappts(self, n):
+        """cosl_pose_solver_reserve_mappts: room for at most n map points per submit (all cameras); 0 frees it."""
+        _ck(LIB.cosl_pose_solver_reserve_mappts(self.h, int(n)))
+
+    def submit(self, Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list=None, opts=None, covx=None, prior=None,
+               mappts=None, gate=None):
         """cosl_pose_solver_submit: enqueue pose_intracam_batch's solve and return at once; the input arrays
         may be reused when it returns.  opts (C PoseOpts, defaults when None) is what collect() fills.
         covx, a list of per-camera [n, 2, 2] or [n, 4] measurement covariances (px^2, in the order of ms_list;
         None entries for identity), weights the solve through cosl_pose_solver_submit_cov.
         prior, a list with one entry per camera, None or (R [3, 3], t [3], P [6, 6]): a Gaussian pose prior with
         mean (R, t) and covariance P in the order (w, dt) of the solver's chart R = R_p exp([w]x), t = t_p + dt
-        (download_covariance's), through cosl_pose_solver_submit_prior."""
+        (download_covariance's), through cosl_pose_solver_submit_prior.
+        mappts, a list with one entry per camera, None (no map points) or (X [n, 3], P [n, 3, 3], m [n, 2]) or
+        (X, P, m, covm [n, 2, 2] or None): the map points the frame observes, gated at gate (a chi-square quantile
+        for 2 dof) and updated after the armed covariance stage through cosl_pose_solver_submit_mappts; read them
+        with download_mappts()."""
         args, opts, keep = _pose_batch_args(Ks, R0s, t0s, Ms_list, ms_list, tau, prev_list, opts)
-        cp = None
+        cp = pp = None
         if covx is not None:
             if len(covx) != args[0]:
                 raise ValueError(f"covx has {len(covx)} cameras for {args[0]}")
@@ -624,6 +638,22 @@ class PoseSolver(_SolverHandle):
                 raise ValueError(f"prior has {len(prior)} cameras for {args[0]}")
             recs = [None if p is None else _pose_prior(*p) for p in prior]
             pp = (C.c_void_p * args[0])(*[None if r is None else r.ctypes.data for r in recs])
+        if mappts is not None:
+            if gate is None:
+                raise ValueError("mappts needs a gate")
+            if len(mappts) != args[0]:
+                raise ValueError(f"mappts has {len(mappts)} cameras for {args[0]}")
+            mp = [_map_points(e) for e in mappts]
+            nmap = np.array([len(e[0]) for e in mp], np.int32)
+            ptrs = [(C.c_void_p * args[0])(*[None if len(e[0]) == 0 else e[k].ctypes.data for e in mp])
+                    for k in range(3)]
+            cm = None
+            if any(e[3] is not None for e in mp):
+                cm = (C.c_void_p * args[0])(*[None if e[3] is None else e[3].ctypes.data for e in mp])
+            _ck(LIB.cosl_pose_solver_submit_mappts(self.h, *args[:7], cp, pp, *args[7:], opts, _ptr(nmap), *ptrs, cm,
+                                                   float(gate)))
+            self._nmap = [int(n) for n in nmap]
+        elif prior is not None:
             _ck(LIB.cosl_pose_solver_submit_prior(self.h, *args[:7], cp, pp, *args[7:], opts))
         elif covx is None:
             _ck(LIB.cosl_pose_solver_submit(self.h, *args, opts))
@@ -656,6 +686,30 @@ class PoseSolver(_SolverHandle):
         err = np.empty(sum(npts))
         _ck(LIB.cosl_pose_solver_download_covariance(self.h, _ptr(cov), _ptr(err), _ptr(stats)))
         return cov, np.split(err, np.cumsum(npts)[:-1]), stats
+
+    def download_mappts(self):
+        """cosl_pose_solver_download_mappts after collect() of a submit with mappts: a dict of arrays over every map
+        point, camera-major in submit order: X [N, 3], P [N, 3, 3], d2_0 (the gate's Mahalanobis distance), d2_1 (at
+        the update, NaN unless updated), e0 (|m - pi(X0)| in px), status [N] (0 updated, 1 gated out, 2 not
+        updatable, 3 the camera's pose covariance invalid) and cam [N], each point's camera."""
+        n = sum(self._nmap)
+        X, P, st, status = np.empty((n, 3)), np.empty((n, 3, 3)), np.empty((n, 3)), np.empty(n, np.int32)
+        _ck(LIB.cosl_pose_solver_download_mappts(self.h, _ptr(X), _ptr(P), _ptr(st), _ptr(status)))
+        cam = np.repeat(np.arange(len(self._nmap), dtype=np.int32), self._nmap)
+        return dict(X=X, P=P, d2_0=st[:, 0].copy(), d2_1=st[:, 1].copy(), e0=st[:, 2].copy(), status=status, cam=cam)
+
+
+def _map_points(entry):
+    """One camera's map points of cosl_pose_solver_submit_mappts as contiguous float64 arrays (X [n, 3], P [n, 9],
+    m [n, 2], covm [n, 4] or None); None is no map points."""
+    if entry is None:
+        return np.empty((0, 3)), np.empty((0, 9)), np.empty((0, 2)), None
+    X, P, m = (np.ascontiguousarray(a, np.float64) for a in entry[:3])
+    X, P, m = X.reshape(-1, 3), P.reshape(-1, 9), m.reshape(-1, 2)
+    if not len(X) == len(P) == len(m):
+        raise ValueError(f"map points: {len(X)} X, {len(P)} P and {len(m)} m")
+    cm = entry[3] if len(entry) > 3 else None
+    return X, P, m, None if cm is None else _obs_cov(cm, len(X))
 
 
 def _pose_prior(R, t, P):

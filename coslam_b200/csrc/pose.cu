@@ -702,6 +702,280 @@ pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsA
   r[39] = valid ? 1.0 : 0.0;
 }
 
+// Map-point update of cosl_pose_solver_submit_mappts (DESIGN.md 5.4, an extension).  Per point, staged as
+// MAPPT_IN doubles: X0[3] | P0 (6: xx xy xz yy yz zz) | m[2] | Sigma_m (3: xx xy yy); results as MAPPT_OUT doubles:
+// X[3] | P (6, as P0) | d2_0, d2_1, e0 | status.
+constexpr int MAPPT_THREADS = 64;
+constexpr int MAPPT_IN = 14;
+constexpr int MAPPT_OUT = 13;
+constexpr int MAPPT_MAX_ITER = 8;
+
+// c = R X + t, m = x_{0,1} / x_2 of x = K c (x_2 into *x2), and the rows of dm/dX = (a; b) R, a and b the rows of
+// dm/dc (5.1), as ha = R^T a and hb = R^T b.  Returns c_2, the depth.
+__device__ __forceinline__ double mappt_project(const double* K, const double* R, const double* t, const double X[3],
+                                                double m[2], double a[3], double b[3], double ha[3], double hb[3],
+                                                double* x2) {
+  const double c0 = R[0] * X[0] + R[1] * X[1] + R[2] * X[2] + t[0];
+  const double c1 = R[3] * X[0] + R[4] * X[1] + R[5] * X[2] + t[1];
+  const double c2 = R[6] * X[0] + R[7] * X[1] + R[8] * X[2] + t[2];
+  const double u = K[0] * c0 + K[1] * c1 + K[2] * c2;
+  const double v = K[3] * c0 + K[4] * c1 + K[5] * c2;
+  const double w = K[6] * c0 + K[7] * c1 + K[8] * c2;
+  m[0] = u / w;
+  m[1] = v / w;
+  *x2 = w;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    a[k] = (K[k] - m[0] * K[6 + k]) / w;
+    b[k] = (K[3 + k] - m[1] * K[6 + k]) / w;
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    ha[k] = R[k] * a[0] + R[3 + k] * a[1] + R[6 + k] * a[2];
+    hb[k] = R[k] * b[0] + R[3 + k] * b[1] + R[6 + k] * b[2];
+  }
+  return c2;
+}
+
+// Cholesky A = L L^T of a symmetric 3x3 packed as (00 01 02 11 12 22); L lower packed as (00 10 11 20 21 22).
+// False on a pivot that is not positive and finite.
+__device__ __forceinline__ bool mappt_chol3(const double A[6], double L[6]) {
+  const double d0 = A[0];
+  if (!(d0 > 0) || !isfinite(d0)) return false;
+  L[0] = sqrt(d0);
+  L[1] = A[1] / L[0];
+  L[3] = A[2] / L[0];
+  const double d1 = A[3] - L[1] * L[1];
+  if (!(d1 > 0) || !isfinite(d1)) return false;
+  L[2] = sqrt(d1);
+  L[4] = (A[4] - L[3] * L[1]) / L[2];
+  const double d2 = A[5] - L[3] * L[3] - L[4] * L[4];
+  if (!(d2 > 0) || !isfinite(d2)) return false;
+  L[5] = sqrt(d2);
+  return true;
+}
+
+// A^-1 = L^-T L^-1 (packed as A) from the factor of mappt_chol3
+__device__ __forceinline__ void mappt_chol3_inv(const double L[6], double Ai[6]) {
+  const double i00 = 1.0 / L[0], i11 = 1.0 / L[2], i22 = 1.0 / L[5];
+  const double i10 = -L[1] * i00 * i11;
+  const double i21 = -L[4] * i11 * i22;
+  const double i20 = -(L[3] * i00 + L[4] * i10) * i22;
+  Ai[0] = i00 * i00 + i10 * i10 + i20 * i20;
+  Ai[1] = i10 * i11 + i20 * i21;
+  Ai[2] = i20 * i22;
+  Ai[3] = i11 * i11 + i21 * i21;
+  Ai[4] = i21 * i22;
+  Ai[5] = i22 * i22;
+}
+
+// r^T S^-1 r of a symmetric 2x2 S = (s00 s01 s11); false unless S is positive definite
+__device__ __forceinline__ bool mappt_quad2(const double S[3], const double r[2], double* q) {
+  const double det = S[0] * S[2] - S[1] * S[1];
+  if (!(S[0] > 0) || !(det > 0)) return false;
+  *q = (S[2] * r[0] * r[0] - 2.0 * S[1] * r[0] * r[1] + S[0] * r[1] * r[1]) / det;
+  return true;
+}
+
+// f(X + s) - f(X) of the update's objective f(X) = (X - X0)^T P0^-1 (X - X0) + (m - pi(X))^T Rf^-1 (m - pi(X)), from
+// differences: s^T P0^-1 (2 (X - X0) + s) - dpi^T Rf^-1 (2 nu - dpi), nu = m - pi(X), pm = pi(X) and
+// dpi = pi(X + s) - pi(X) = (dx_{0,1} - pm dx_2) / (x_2 + dx_2) with dx = K R s.  Near the minimum the two objectives
+// agree to their roundoff (m - pi cancels about 1e-13 px), and their difference would decide a step by noise.
+__device__ __forceinline__ double mappt_descent(const double* K, const double* R, const double L0[6], const double Rf[3],
+                                               const double X0[3], const double X[3], double w, const double pm[2],
+                                               const double nu[2], const double s[3]) {
+  const double dc0 = R[0] * s[0] + R[1] * s[1] + R[2] * s[2];
+  const double dc1 = R[3] * s[0] + R[4] * s[1] + R[5] * s[2];
+  const double dc2 = R[6] * s[0] + R[7] * s[1] + R[8] * s[2];
+  const double dx0 = K[0] * dc0 + K[1] * dc1 + K[2] * dc2;
+  const double dx1 = K[3] * dc0 + K[4] * dc1 + K[5] * dc2;
+  const double dx2 = K[6] * dc0 + K[7] * dc1 + K[8] * dc2;
+  const double wn = w + dx2;
+  const double dp0 = (dx0 - pm[0] * dx2) / wn, dp1 = (dx1 - pm[1] * dx2) / wn;
+  const double q0 = 2.0 * nu[0] - dp0, q1 = 2.0 * nu[1] - dp1;
+  const double det = Rf[0] * Rf[2] - Rf[1] * Rf[1];
+  const double meas = (Rf[2] * dp0 * q0 - Rf[1] * (dp0 * q1 + dp1 * q0) + Rf[0] * dp1 * q1) / det;
+  // s^T P0^-1 (2 d + s) = (L0^-1 s) . (L0^-1 (2 d + s)), d = X - X0
+  const double u0 = s[0] / L0[0];
+  const double u1 = (s[1] - L0[1] * u0) / L0[2];
+  const double u2 = (s[2] - L0[3] * u0 - L0[4] * u1) / L0[5];
+  const double e0 = 2.0 * (X[0] - X0[0]) + s[0], e1 = 2.0 * (X[1] - X0[1]) + s[1], e2 = 2.0 * (X[2] - X0[2]) + s[2];
+  const double v0 = e0 / L0[0];
+  const double v1 = (e1 - L0[1] * v0) / L0[2];
+  const double v2 = (e2 - L0[3] * v0 - L0[4] * v1) / L0[5];
+  return u0 * v0 + u1 * v1 + u2 * v2 - meas;
+}
+
+// S = H P H^T + Rf for H = (ha; hb) (2x3) and P packed as mappt_chol3's A; U = P H^T (3x2, row-major)
+__device__ __forceinline__ void mappt_innov(const double ha[3], const double hb[3], const double P[6],
+                                            const double Rf[3], double U[6], double S[3]) {
+  const double F[9] = {P[0], P[1], P[2], P[1], P[3], P[4], P[2], P[4], P[5]};
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    U[2 * i] = F[3 * i] * ha[0] + F[3 * i + 1] * ha[1] + F[3 * i + 2] * ha[2];
+    U[2 * i + 1] = F[3 * i] * hb[0] + F[3 * i + 1] * hb[1] + F[3 * i + 2] * hb[2];
+  }
+  S[0] = ha[0] * U[0] + ha[1] * U[2] + ha[2] * U[4] + Rf[0];
+  S[1] = ha[0] * U[1] + ha[1] * U[3] + ha[2] * U[5] + Rf[1];
+  S[2] = hb[0] * U[1] + hb[1] * U[3] + hb[2] * U[5] + Rf[2];
+}
+
+// One thread per map point; each CTA serves the points [first, end) of one camera, blk[blockIdx.x] = (camera,
+// first, end, -), staged by the host.  The camera's K, its refined (R, t) from outs and its stage covariance P_c
+// from res (pose_cov_kernel's, in the chart R' = R exp([w]x), t' = t + dt) go to shared memory.  Per point:
+//   R_eff = Sigma_m + H_c(X0) P_c H_c(X0)^T, H_c the analytic 2x6 Jacobian of 5.1, H_X = (a; b) R;
+//   gate: nu0 = m - pi(X0), S0 = H_X P0 H_X^T + R_eff, d2_0 = nu0^T S0^-1 nu0, update when d2_0 < gate;
+//   update: at most MAPPT_MAX_ITER Gauss-Newton steps in Kalman form on (X - X0)^T P0^-1 (X - X0) +
+//   (m - pi(X))^T R_eff^-1 (m - pi(X)), X' = X0 + P0 H^T (H P0 H^T + R_eff)^-1 (m - pi(X) + H (X - X0)) at X, taken
+//   only when it lowers that objective (mappt_descent < 0) and keeps the depth > 0, stopped once
+//   |X' - X| <= 1e-12 max(1, |X'|);
+//   P+ = (P0^-1 + H^T R_eff^-1 H)^-1 at X+ by Cholesky; d2_1 = nu1^T (H P+ H^T + R_eff)^-1 nu1 at X+.
+// status 0 updated, 1 gated out, 2 not updatable (depth <= 0, a non-finite value, S0 not positive definite), 3 the
+// camera's pose covariance is invalid; with status != 0, X0 and P0 come back as given and d2_1 (and d2_0 for 2 and
+// 3) is NaN.  e0 = |nu0| is reported as computed whatever the status.
+__global__ void __launch_bounds__(MAPPT_THREADS)
+pose_mappt_kernel(const int4* __restrict__ blk, const double* __restrict__ in, const PoseCam* __restrict__ cams,
+                  const PoseOut* __restrict__ outs, const double* __restrict__ res, double gate,
+                  double* __restrict__ out) {
+  __shared__ double s_K[9], s_R[9], s_t[3], s_P[36];
+  __shared__ int s_valid;
+  const int4 b = blk[blockIdx.x];
+  const int c = b.x;
+  if (threadIdx.x < 9) {
+    s_K[threadIdx.x] = cams[c].K[threadIdx.x];
+    s_R[threadIdx.x] = outs[c].R[threadIdx.x];
+  }
+  if (threadIdx.x < 3) s_t[threadIdx.x] = outs[c].t[threadIdx.x];
+  if (threadIdx.x < 36) s_P[threadIdx.x] = res[POSE_COV_STRIDE * c + threadIdx.x];
+  if (threadIdx.x == 0) s_valid = res[POSE_COV_STRIDE * c + 39] == 1.0;
+  __syncthreads();
+  const int j = b.y + threadIdx.x;
+  if (j >= b.z) return;
+  const double* q = in + (size_t)MAPPT_IN * j;
+  double* o = out + (size_t)MAPPT_OUT * j;
+  const double X0[3] = {q[0], q[1], q[2]};
+  double P0[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) P0[k] = q[3 + k];
+  const double mo[2] = {q[9], q[10]};
+  double pm[2], a[3], bb[3], ha[3], hb[3], w;
+  const double z0 = mappt_project(s_K, s_R, s_t, X0, pm, a, bb, ha, hb, &w);
+  double nu[2] = {mo[0] - pm[0], mo[1] - pm[1]};
+  const double e0 = sqrt(nu[0] * nu[0] + nu[1] * nu[1]);
+  int status = 2;
+  double d0 = NAN, d1 = NAN, X[3] = {X0[0], X0[1], X0[2]}, P[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) P[k] = P0[k];
+  if (!s_valid) {
+    status = 3;
+  } else if (z0 > 0 && isfinite(pm[0]) && isfinite(pm[1])) {
+    // R_eff = Sigma_m + H_c P_c H_c^T; H_c rows (X0 x ha, a) and (X0 x hb, b)
+    double Hc[12];
+    Hc[0] = X0[1] * ha[2] - X0[2] * ha[1];
+    Hc[1] = X0[2] * ha[0] - X0[0] * ha[2];
+    Hc[2] = X0[0] * ha[1] - X0[1] * ha[0];
+    Hc[6] = X0[1] * hb[2] - X0[2] * hb[1];
+    Hc[7] = X0[2] * hb[0] - X0[0] * hb[2];
+    Hc[8] = X0[0] * hb[1] - X0[1] * hb[0];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      Hc[3 + k] = a[k];
+      Hc[9 + k] = bb[k];
+    }
+    double Rf[3] = {q[11], q[12], q[13]};
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      double t0 = 0, t1 = 0;
+#pragma unroll
+      for (int l = 0; l < 6; ++l) {
+        t0 += Hc[l] * s_P[6 * l + k];
+        t1 += Hc[6 + l] * s_P[6 * l + k];
+      }
+      Rf[0] += t0 * Hc[k];
+      Rf[1] += t0 * Hc[6 + k];
+      Rf[2] += t1 * Hc[6 + k];
+    }
+    double U[6], S[3], L0[6], f0;  // f0: R_eff must be positive definite too
+    mappt_innov(ha, hb, P0, Rf, U, S);
+    if (mappt_quad2(S, nu, &d0) && isfinite(d0) && mappt_quad2(Rf, nu, &f0) && mappt_chol3(P0, L0)) {
+      status = d0 < gate ? 0 : 1;
+    } else {
+      d0 = NAN;
+    }
+    if (status == 0) {
+      for (int it = 0; it < MAPPT_MAX_ITER; ++it) {
+        // Gauss-Newton step from X (U, S, nu, ha, hb at X)
+        const double y0 = nu[0] + ha[0] * (X[0] - X0[0]) + ha[1] * (X[1] - X0[1]) + ha[2] * (X[2] - X0[2]);
+        const double y1 = nu[1] + hb[0] * (X[0] - X0[0]) + hb[1] * (X[1] - X0[1]) + hb[2] * (X[2] - X0[2]);
+        const double det = S[0] * S[2] - S[1] * S[1];
+        const double g0 = (S[2] * y0 - S[1] * y1) / det, g1 = (S[0] * y1 - S[1] * y0) / det;
+        double Xn[3], pn[2], an[3], bn[3], han[3], hbn[3], wn;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) Xn[k] = X0[k] + (U[2 * k] * g0 + U[2 * k + 1] * g1);
+        const double zn = mappt_project(s_K, s_R, s_t, Xn, pn, an, bn, han, hbn, &wn);
+        if (!(zn > 0)) break;
+        const double nun[2] = {mo[0] - pn[0], mo[1] - pn[1]};
+        const double st[3] = {Xn[0] - X[0], Xn[1] - X[1], Xn[2] - X[2]};
+        if (!(mappt_descent(s_K, s_R, L0, Rf, X0, X, w, pm, nu, st) < 0)) break;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          X[k] = Xn[k];
+          ha[k] = han[k];
+          hb[k] = hbn[k];
+        }
+        nu[0] = nun[0];
+        nu[1] = nun[1];
+        pm[0] = pn[0];
+        pm[1] = pn[1];
+        w = wn;
+        const double xn = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+        if (sqrt(st[0] * st[0] + st[1] * st[1] + st[2] * st[2]) <= 1e-12 * fmax(1.0, xn)) break;
+        mappt_innov(ha, hb, P0, Rf, U, S);
+      }
+      // P+ = (P0^-1 + H^T R_eff^-1 H)^-1 at X+
+      double Pi[6], Lp[6];
+      mappt_chol3_inv(L0, Pi);
+      const double det = Rf[0] * Rf[2] - Rf[1] * Rf[1];
+      const double w00 = Rf[2] / det, w01 = -Rf[1] / det, w11 = Rf[0] / det;
+      int k = 0;
+#pragma unroll
+      for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int s = r; s < 3; ++s) {
+          Pi[k] += ha[r] * (w00 * ha[s] + w01 * hb[s]) + hb[r] * (w01 * ha[s] + w11 * hb[s]);
+          ++k;
+        }
+      double Pp[6], Sp[3];
+      bool good = mappt_chol3(Pi, Lp);
+      if (good) {
+        mappt_chol3_inv(Lp, Pp);
+        mappt_innov(ha, hb, Pp, Rf, U, Sp);
+        good = mappt_quad2(Sp, nu, &d1) && isfinite(d1) && isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]);
+#pragma unroll
+        for (int r = 0; r < 6; ++r) good = good && isfinite(Pp[r]);
+      }
+      if (good) {
+#pragma unroll
+        for (int r = 0; r < 6; ++r) P[r] = Pp[r];
+      } else {
+        status = 2;
+        d0 = d1 = NAN;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) X[r] = X0[r];
+      }
+    }
+  }
+  if (status != 0) d1 = NAN;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) o[k] = X[k];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) o[3 + k] = P[k];
+  o[9] = d0;
+  o[10] = d1;
+  o[11] = e0;
+  o[12] = status;
+}
+
 
 // Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
 // cameras.
@@ -841,14 +1115,83 @@ int check_priors(const char* fn, int C, const double* const* prior, bool* any) {
   return COSL_OK;
 }
 
+// The map points of cosl_pose_solver_submit_mappts, as passed
+struct MapPtsArgs {
+  const int* n;
+  const double* const* X;
+  const double* const* P;
+  const double* const* m;
+  const double* const* cov;  // nullable, as cov[c]
+  double gate;
+};
+
+// True when the 3x3 covariance P (row-major) is finite, symmetric to 1e-12 of its largest diagonal entry and positive
+// definite; S gets its symmetrised upper triangle (xx xy xz yy yz zz).
+bool point_cov(const double* P, double S[6]) {
+  double pmax = 0.0;
+  for (int i = 0; i < 9; ++i)
+    if (!std::isfinite(P[i])) return false;
+  for (int i = 0; i < 3; ++i) pmax = std::max(pmax, std::fabs(P[4 * i]));
+  for (int a = 0; a < 3; ++a)
+    for (int b = a + 1; b < 3; ++b)
+      if (std::fabs(P[3 * a + b] - P[3 * b + a]) > 1e-12 * pmax) return false;
+  int k = 0;
+  for (int a = 0; a < 3; ++a)
+    for (int b = a; b < 3; ++b) S[k++] = 0.5 * (P[3 * a + b] + P[3 * b + a]);
+  // Cholesky pivots of S
+  const double d0 = S[0];
+  if (!(d0 > 0)) return false;
+  const double l10 = S[1] / std::sqrt(d0), l20 = S[2] / std::sqrt(d0);
+  const double d1 = S[3] - l10 * l10;
+  if (!(d1 > 0)) return false;
+  const double l21 = (S[4] - l20 * l10) / std::sqrt(d1);
+  const double d2 = S[5] - l20 * l20 - l21 * l21;
+  return d2 > 0 && std::isfinite(d2);
+}
+
+// Checks the map points of one submit, naming the first bad camera and point; *tot = map points over all cameras.
+int check_mappts(const char* fn, int C, int cap, const MapPtsArgs& mp, long long* tot) {
+  if (!mp.n || !mp.X || !mp.P || !mp.m) return set_error(COSL_E_INVALID, "%s: null map-point argument", fn);
+  if (!std::isfinite(mp.gate) || !(mp.gate > 0))
+    return set_error(COSL_E_INVALID, "%s: gate %g is not a finite value > 0", fn, mp.gate);
+  long long n = 0;
+  for (int c = 0; c < C; ++c) {
+    if (mp.n[c] < 0 || (mp.n[c] && (!mp.X[c] || !mp.P[c] || !mp.m[c])))
+      return set_error(COSL_E_INVALID, "%s: bad map points of camera %d", fn, c);
+    n += mp.n[c];
+  }
+  if (n > cap) return set_error(COSL_E_INVALID, "%s: %lld map points exceed the %d reserved", fn, n, cap);
+  for (int c = 0; c < C; ++c)
+    for (int i = 0; i < mp.n[c]; ++i) {
+      const double* X = mp.X[c] + 3 * (size_t)i;
+      const double* m = mp.m[c] + 2 * (size_t)i;
+      if (!std::isfinite(X[0]) || !std::isfinite(X[1]) || !std::isfinite(X[2]) || !std::isfinite(m[0]) ||
+          !std::isfinite(m[1]))
+        return set_error(COSL_E_INVALID, "%s: map point %d of camera %d: X or m is not finite", fn, i, c);
+      double S[6];
+      if (!point_cov(mp.P[c] + 9 * (size_t)i, S))
+        return set_error(COSL_E_INVALID,
+                         "%s: map point %d of camera %d: P is not finite, symmetric and positive definite", fn, i, c);
+      double L[3];
+      if (mp.cov && mp.cov[c] && !cov_factor(mp.cov[c] + 4 * (size_t)i, L))
+        return set_error(COSL_E_INVALID,
+                         "%s: map point %d of camera %d: covm is not finite, symmetric and positive definite", fn, i,
+                         c);
+    }
+  *tot = n;
+  return COSL_OK;
+}
+
 }  // namespace
 
 // A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out as
-// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] | L[3 tot] | prior[C][POSE_PRIOR_REC] | hasPrior[C] (tot =
-// points of the solve; the whitening factors L are staged and copied by the submits with covariances only, and the
-// priors, right after the last section copied, by a submit with some prior); the PoseOuts come back into pinned
-// memory.  Capacity is fixed at create: everything is allocated once, the covariance stage's buffers (laid out as
-// res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed.
+// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] | L[3 tot] | prior[C][POSE_PRIOR_REC] | hasPrior[C] |
+// map[nmap][MAPPT_IN] | blk[nblk] (tot = points of the solve; the whitening factors L are staged and copied by the
+// submits with covariances only, the priors, right after the last section copied, by a submit with some prior, and
+// the map points, 16-byte aligned after the last section copied, by cosl_pose_solver_submit_mappts); the PoseOuts
+// come back into pinned memory.  Capacity is fixed at create: everything is allocated once, the covariance stage's
+// buffers (laid out as res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed, and the map-point sections
+// and results (mres[nmap][MAPPT_OUT]) by cosl_pose_solver_reserve_mappts, which reallocates the staging buffers.
 struct cosl_pose_solver {
   int device = 0, maxCams = 0, maxPts = 0;
   RequestStream rq;
@@ -865,6 +1208,14 @@ struct cosl_pose_solver {
   bool covReady = false;  // the last submitted solve was armed
   bool obsCov = false;    // the solve in flight carries measurement covariances
   bool prior = false;     // the solve in flight carries pose priors
+  int maxMap = 0;         // map points reserved per submit
+  double* d_mres = nullptr;
+  double* h_mres = nullptr;
+  bool map = false;       // the solve in flight carries map points
+  bool mapReady = false;  // the last submit was a cosl_pose_solver_submit_mappts
+  long long nmap = 0;     // map points of that submit
+  int nblk = 0;           // CTAs of its pose_mappt_kernel
+  double gate = 0;
 };
 
 namespace {
@@ -877,6 +1228,21 @@ size_t prior_bytes(int C) { return (sizeof(double) * POSE_PRIOR_REC + sizeof(int
 size_t prior_offset(int C, long long tot, bool obsCov) {
   return obsCov ? input_bytes_cov(C, tot) : input_bytes(C, tot);
 }
+// the map points of cosl_pose_solver_submit_mappts, 16-byte aligned after the last section copied
+size_t mappt_offset(int C, long long tot, bool obsCov, bool prior) {
+  const size_t o = prior_offset(C, tot, obsCov) + (prior ? prior_bytes(C) : 0);
+  return (o + 15) & ~(size_t)15;
+}
+// nmap records and at most nblk CTAs of pose_mappt_kernel
+size_t mappt_bytes(long long nmap, int nblk) { return sizeof(double) * MAPPT_IN * nmap + sizeof(int4) * nblk; }
+// a bound on the CTAs of nmap map points over C cameras: sum_c ceil(n_c / MAPPT_THREADS)
+int mappt_max_blocks(int C, long long nmap) { return (int)(nmap / MAPPT_THREADS) + C; }
+// the staging buffers' size: every section at capacity
+size_t input_capacity(int maxCams, int maxPts, int maxMap) {
+  size_t in = input_bytes_cov(maxCams, maxPts) + prior_bytes(maxCams);
+  if (maxMap > 0) in += 16 + mappt_bytes(maxMap, mappt_max_blocks(maxCams, maxMap));
+  return in;
+}
 
 void free_pose_solver(cosl_pose_solver* s) {
   cudaSetDevice(s->device);
@@ -884,10 +1250,12 @@ void free_pose_solver(cosl_pose_solver* s) {
   if (s->h_in) cudaFreeHost(s->h_in);
   if (s->h_out) cudaFreeHost(s->h_out);
   if (s->h_cov) cudaFreeHost(s->h_cov);
+  if (s->h_mres) cudaFreeHost(s->h_mres);
   cudaFree(s->d_in);
   cudaFree(s->d_W);
   cudaFree(s->d_out);
   cudaFree(s->d_cov);
+  cudaFree(s->d_mres);
   delete s;
 }
 
@@ -896,7 +1264,7 @@ size_t cov_doubles(int C, long long tot) { return (size_t)POSE_COV_STRIDE * C + 
 int alloc_pose_solver(cosl_pose_solver* s) {
   COSL_CUDA(cudaSetDevice(s->device));
   COSL_TRY(s->rq.create());
-  const size_t in = input_bytes_cov(s->maxCams, s->maxPts) + prior_bytes(s->maxCams);
+  const size_t in = input_capacity(s->maxCams, s->maxPts, s->maxMap);
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
   COSL_CUDA(cudaHostAlloc(&s->h_out, sizeof(PoseOut) * s->maxCams, cudaHostAllocPortable));
   COSL_CUDA(cudaMalloc(&s->d_in, in));
@@ -924,7 +1292,8 @@ int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg)
   pr.rec = reinterpret_cast<const double*>(s->d_in + poff);
   pr.has = reinterpret_cast<const int*>(s->d_in + poff + sizeof(double) * POSE_PRIOR_REC * C);
   cudaStream_t st = s->rq.stream;
-  const size_t bytes = s->prior ? poff + prior_bytes(C) : poff;
+  const size_t moff = mappt_offset(C, tot, s->obsCov, s->prior);
+  const size_t bytes = s->map ? moff + mappt_bytes(s->nmap, s->nblk) : s->prior ? poff + prior_bytes(C) : poff;
   COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, bytes, cudaMemcpyHostToDevice, st));
   if (s->prior && s->obsCov)
     COSL_LAUNCH(pose_intracam_obscov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg,
@@ -957,15 +1326,25 @@ int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg)
                   d_res, d_err);
     COSL_CUDA(cudaGetLastError());
     COSL_CUDA(cudaMemcpyAsync(s->h_cov, s->d_cov, sizeof(double) * cov_doubles(C, tot), cudaMemcpyDeviceToHost, st));
+    if (s->map && s->nblk > 0) {  // submit_mappts requires an armed handle
+      const double* d_map = reinterpret_cast<const double*>(s->d_in + moff);
+      const int4* d_blk = reinterpret_cast<const int4*>(d_map + (size_t)MAPPT_IN * s->nmap);
+      COSL_LAUNCH(pose_mappt_kernel, s->nblk, MAPPT_THREADS, 0, st, d_blk, d_map, d_cams, s->d_out, d_res, s->gate,
+                  s->d_mres);
+      COSL_CUDA(cudaGetLastError());
+      COSL_CUDA(cudaMemcpyAsync(s->h_mres, s->d_mres, sizeof(double) * MAPPT_OUT * s->nmap, cudaMemcpyDeviceToHost,
+                                st));
+    }
   }
   return COSL_OK;
 }
 
-// cosl_pose_solver_submit (covx == prior == nullptr), cosl_pose_solver_submit_cov (prior == nullptr) and
-// cosl_pose_solver_submit_prior; fn names the caller in messages.
+// cosl_pose_solver_submit (covx == prior == mp == nullptr), cosl_pose_solver_submit_cov (prior == mp == nullptr),
+// cosl_pose_solver_submit_prior (mp == nullptr) and cosl_pose_solver_submit_mappts; fn names the caller in messages.
 int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
                  const int* npts, const double* const* Ms, const double* const* ms, const double* const* covx,
-                 const double* const* prior, const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
+                 const double* const* prior, const double* const* prevErrs, double tau, const cosl_pose_opt* opts,
+                 const MapPtsArgs* mp = nullptr) {
   if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
   COSL_TRY(s->rq.idle(fn));
   if (C < 1 || !K9 || !R0 || !t0 || !npts || !Ms || !ms || !opts)
@@ -979,6 +1358,12 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   COSL_TRY(check_covx(fn, C, npts, covx));
   bool anyPrior = false;
   COSL_TRY(check_priors(fn, C, prior, &anyPrior));
+  long long nmap = 0;
+  if (mp) {
+    if (!(s->pixelVar > 0)) return set_error(COSL_E_STATE, "%s: the handle is not armed (set_covariance)", fn);
+    if (s->maxMap < 1) return set_error(COSL_E_STATE, "%s: no map points reserved (reserve_mappts)", fn);
+    COSL_TRY(check_mappts(fn, C, s->maxMap, *mp, &nmap));
+  }
   COSL_CUDA(cudaSetDevice(s->device));
   // nothing is in flight, so no copy reads the staging buffer any more
   PoseCam* cams = reinterpret_cast<PoseCam*>(s->h_in);
@@ -1024,6 +1409,36 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
       if (prior[c]) prior_factor(fn, c, prior[c], hq + POSE_PRIOR_REC * (size_t)c);
     }
   }
+  int nblk = 0;
+  if (mp) {  // records camera-major, then one CTA per MAPPT_THREADS points of a camera
+    const size_t moff = mappt_offset(C, tot, covx != nullptr, anyPrior);
+    double* hr = reinterpret_cast<double*>(s->h_in + moff);
+    int4* hb = reinterpret_cast<int4*>(hr + (size_t)MAPPT_IN * nmap);
+    const double pv = s->pixelVar;
+    long long j = 0;
+    for (int c = 0; c < C; ++c) {
+      for (int i = 0; i < mp->n[c]; ++i) {
+        double* r = hr + (size_t)MAPPT_IN * (j + i);
+        std::memcpy(r, mp->X[c] + 3 * (size_t)i, sizeof(double) * 3);
+        const double* P = mp->P[c] + 9 * (size_t)i;  // symmetrised, as point_cov checked it
+        r[3] = P[0];
+        r[4] = 0.5 * (P[1] + P[3]);
+        r[5] = 0.5 * (P[2] + P[6]);
+        r[6] = P[4];
+        r[7] = 0.5 * (P[5] + P[7]);
+        r[8] = P[8];
+        std::memcpy(r + 9, mp->m[c] + 2 * (size_t)i, sizeof(double) * 2);
+        // Sigma_m = pixel_var I when the camera has no covm
+        const double* v = (mp->cov && mp->cov[c]) ? mp->cov[c] + 4 * (size_t)i : nullptr;
+        r[11] = v ? v[0] : pv;
+        r[12] = v ? v[1] : 0.0;
+        r[13] = v ? v[3] : pv;
+      }
+      for (int i = 0; i < mp->n[c]; i += MAPPT_THREADS)
+        hb[nblk++] = make_int4(c, (int)(j + i), (int)(j + std::min(i + MAPPT_THREADS, mp->n[c])), 0);
+      j += mp->n[c];
+    }
+  }
   PoseCfg cfg;
   cfg.maxIterLM = opts[0].maxIterLM;
   cfg.maxIterRW = opts[0].maxIterRW;
@@ -1037,8 +1452,14 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   s->covReady = false;
   s->obsCov = covx != nullptr;
   s->prior = anyPrior;
+  s->map = mp != nullptr;
+  s->mapReady = false;
+  s->nmap = nmap;
+  s->nblk = nblk;
+  s->gate = mp ? mp->gate : 0.0;
   COSL_TRY(s->rq.submit(fn, [&]() { return enqueue_solve(s, C, tot, cfg); }));
   s->covReady = s->pixelVar > 0;
+  s->mapReady = s->map;
   return COSL_OK;
 }
 
@@ -1103,6 +1524,76 @@ int cosl_pose_solver_submit_prior(cosl_pose_solver* s, int C, const double* K9, 
                                   const double* const* prevErrs, double tau, const cosl_pose_opt* opts) {
   return submit_solve("cosl_pose_solver_submit_prior", s, C, K9, R0, t0, npts, Ms, ms, covx, prior, prevErrs, tau,
                       opts);
+}
+
+int cosl_pose_solver_reserve_mappts(cosl_pose_solver* s, int maxMapPts) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  if (maxMapPts < 0) return set_error(COSL_E_INVALID, "cosl_pose_solver_reserve_mappts: maxMapPts %d < 0", maxMapPts);
+  COSL_TRY(s->rq.idle("cosl_pose_solver_reserve_mappts"));
+  if (maxMapPts == s->maxMap) return COSL_OK;
+  COSL_CUDA(cudaSetDevice(s->device));
+  // the new buffers first, so a failed allocation leaves the handle as it was
+  const size_t in = input_capacity(s->maxCams, s->maxPts, maxMapPts);
+  unsigned char *h_in = nullptr, *d_in = nullptr;
+  double *h_mres = nullptr, *d_mres = nullptr;
+  const size_t nres = sizeof(double) * MAPPT_OUT * (size_t)maxMapPts;
+  cudaError_t e = cudaHostAlloc(&h_in, in, cudaHostAllocPortable);
+  if (e == cudaSuccess) e = cudaMalloc(&d_in, in);
+  if (e == cudaSuccess && nres) e = cudaHostAlloc(&h_mres, nres, cudaHostAllocPortable);
+  if (e == cudaSuccess && nres) e = cudaMalloc(&d_mres, nres);
+  if (e != cudaSuccess) {
+    if (h_in) cudaFreeHost(h_in);
+    if (h_mres) cudaFreeHost(h_mres);
+    cudaFree(d_in);
+    cudaFree(d_mres);
+    return set_error(COSL_E_NOMEM, "cosl_pose_solver_reserve_mappts: %d map points: %s", maxMapPts,
+                     cudaGetErrorString(e));
+  }
+  cudaFreeHost(s->h_in);
+  cudaFree(s->d_in);
+  if (s->h_mres) cudaFreeHost(s->h_mres);
+  cudaFree(s->d_mres);
+  s->h_in = h_in;
+  s->d_in = d_in;
+  s->h_mres = h_mres;
+  s->d_mres = d_mres;
+  s->maxMap = maxMapPts;
+  s->mapReady = false;
+  return COSL_OK;
+}
+
+int cosl_pose_solver_submit_mappts(cosl_pose_solver* s, int C, const double* K9, const double* R0, const double* t0,
+                                   const int* npts, const double* const* Ms, const double* const* ms,
+                                   const double* const* covx, const double* const* prior,
+                                   const double* const* prevErrs, double tau, const cosl_pose_opt* opts,
+                                   const int* nmap, const double* const* Xmap, const double* const* Pmap,
+                                   const double* const* mmap, const double* const* covm, double gate) {
+  const MapPtsArgs mp{nmap, Xmap, Pmap, mmap, covm, gate};
+  return submit_solve("cosl_pose_solver_submit_mappts", s, C, K9, R0, t0, npts, Ms, ms, covx, prior, prevErrs, tau,
+                      opts, &mp);
+}
+
+int cosl_pose_solver_download_mappts(cosl_pose_solver* s, double* X, double* P, double* stat, int* status) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  COSL_TRY(s->rq.idle("cosl_pose_solver_download_mappts"));
+  if (!s->mapReady)
+    return set_error(COSL_E_STATE, "cosl_pose_solver_download_mappts: the last submit was not a submit_mappts");
+  for (long long j = 0; j < s->nmap; ++j) {
+    const double* r = s->h_mres + (size_t)MAPPT_OUT * j;
+    if (X) std::memcpy(X + 3 * j, r, sizeof(double) * 3);
+    if (P) {
+      double* p = P + 9 * j;
+      p[0] = r[3];
+      p[1] = p[3] = r[4];
+      p[2] = p[6] = r[5];
+      p[4] = r[6];
+      p[5] = p[7] = r[7];
+      p[8] = r[8];
+    }
+    if (stat) std::memcpy(stat + 3 * j, r + 9, sizeof(double) * 3);
+    if (status) status[j] = (int)r[12];
+  }
+  return COSL_OK;
 }
 
 int cosl_pose_solver_query(cosl_pose_solver* s, int* done) {

@@ -483,6 +483,45 @@ int cosl_pose_solver_set_covariance(cosl_pose_solver* s, double pixel_var);
  * COSL_E_STATE while a solve is in flight, before any armed solve, or after an unarmed submit since
  * (a disarmed handle keeps the last armed result until its next submit). */
 int cosl_pose_solver_download_covariance(cosl_pose_solver* s, double* cov, double* err, double* out);
+/* Gate and update the map points a frame observes (an extension: poseUpdate3D's point loop after
+ * intraCamEstimate; DESIGN.md 5.4).  reserve_mappts allocates, once, the pinned and device buffers for
+ * at most maxMapPts map points per submit (all cameras together); 0 frees them.  No submit allocates.
+ * COSL_E_INVALID for a NULL handle or maxMapPts < 0, COSL_E_STATE while a solve is in flight. */
+int cosl_pose_solver_reserve_mappts(cosl_pose_solver* s, int maxMapPts);
+/* cosl_pose_solver_submit_prior plus the map points of each camera: nmap[c] points, Xmap[c] 3 n means
+ * (world), Pmap[c] 9 n row-major 3x3 covariances (world, MapPoint::cov's layout), mmap[c] 2 n
+ * observations in px, covm[c] 4 n row-major 2x2 covariances [xx, xy, yx, yy] in px^2 (covm and covm[c]
+ * nullable: Sigma_m = pixel_var I).  The solve, collect and download_covariance are those of
+ * submit_prior with the same arguments, bit for bit.  After the covariance stage, per point j of camera c,
+ * at the (R, t) collect returns and its stage covariance P_c (chart R' = R exp([w]x), t' = t + dt):
+ *   H_X = d pi / dX = (a; b) R, H_c the stage's analytic 2x6 Jacobian at X0,
+ *   R_eff = Sigma_m + H_c P_c H_c^T (the pose uncertainty as measurement noise, linearised at X0);
+ *   gate: nu0 = m - pi(X0), S0 = H_X P0 H_X^T + R_eff, d2_0 = nu0^T S0^-1 nu0, e0 = |nu0| in px;
+ *   d2_0 < gate (strict): at most 8 fp64 Gauss-Newton steps on (X - X0)^T P0^-1 (X - X0) +
+ *   (m - pi(X))^T R_eff^-1 (m - pi(X)), each taken only when it lowers that objective and keeps the
+ *   depth (R X + t)_z > 0, stopping at |dX| <= 1e-12 max(1, |X|); the first is the EKF update
+ *   X0 + P0 H_X^T S0^-1 nu0.  Then P+ = (P0^-1 + H_X^T R_eff^-1 H_X)^-1 at X+, symmetric, and
+ *   d2_1 = nu1^T (H_X P+ H_X^T + R_eff)^-1 nu1 at X+ (reported only).
+ *   status 0 updated; 1 gated out; 2 not updatable (depth <= 0 at X0, a non-finite value, S0 not
+ *   positive definite), d2_0 NaN; 3 the camera's stage covariance is invalid, d2_0 NaN.  With status
+ *   != 0, X and P come back as given (P symmetrised) and d2_1 is NaN.  ok[c] does not change the update.
+ * It needs an armed handle (set_covariance) and reserved capacity, else COSL_E_STATE; more map points
+ * than reserved, a NULL nmap, Xmap, Pmap or mmap (or entry of a camera with points), a non-finite X or
+ * m, a P not symmetric to 1e-12 of its largest diagonal entry or not positive definite, a bad covm
+ * (submit_cov's rules) or a gate that is not finite and > 0 give COSL_E_INVALID naming the first bad
+ * camera and point, before anything is staged; the handle stays usable.  The update's kernel runs after
+ * the covariance stage on the handle's stream, and collect's device_ms includes it. */
+int cosl_pose_solver_submit_mappts(cosl_pose_solver* s, int C, const double* K9, const double* R0,
+                                   const double* t0, const int* npts, const double* const* Ms,
+                                   const double* const* ms, const double* const* covx,
+                                   const double* const* prior, const double* const* prevErrs, double tau,
+                                   const cosl_pose_opt* opts, const int* nmap, const double* const* Xmap,
+                                   const double* const* Pmap, const double* const* mmap,
+                                   const double* const* covm, double gate);
+/* After collect of a submit_mappts, camera-major in submit order: X[3 n], P[9 n] row-major,
+ * stat[3 n] = {d2_0, d2_1, e0} and status[n]; every output nullable.  COSL_E_STATE while a solve is in
+ * flight, or when the last submit was not a submit_mappts. */
+int cosl_pose_solver_download_mappts(cosl_pose_solver* s, double* X, double* P, double* stat, int* status);
 
 /* ================================================================ bundle adjustment */
 
