@@ -91,6 +91,13 @@ def _load():
     L.cosl_pose_solver_submit_mappts.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, cd, vp,
                                                  vp, vp, vp, vp, vp, cd]
     L.cosl_pose_solver_download_mappts.argtypes = [vp, vp, vp, vp, vp]
+    L.cosl_tri_solver_create.argtypes = [ci, ci, ci, ci, C.POINTER(vp)]
+    L.cosl_tri_solver_destroy.argtypes = [vp]
+    L.cosl_tri_solver_submit.argtypes = [vp, ci, vp, vp, vp, vp, ci, vp, vp, vp, vp, cd, cd]
+    L.cosl_tri_solver_query.argtypes = [vp, pint]
+    L.cosl_tri_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.cosl_tri_solver_stream.argtypes = [vp]
+    L.cosl_tri_solver_stream.restype = vp
     L.cosl_ba_options_default.argtypes = [C.POINTER(BaOptions)]
     L.cosl_ba_solve.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp]
     L.cosl_ba_solve_multi.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), ci, vp, vp]
@@ -697,6 +704,57 @@ class PoseSolver(_SolverHandle):
         _ck(LIB.cosl_pose_solver_download_mappts(self.h, _ptr(X), _ptr(P), _ptr(st), _ptr(status)))
         cam = np.repeat(np.arange(len(self._nmap), dtype=np.int32), self._nmap)
         return dict(X=X, P=P, d2_0=st[:, 0].copy(), d2_1=st[:, 1].copy(), e0=st[:, 2].copy(), status=status, cam=cam)
+
+
+class TriSolver(_SolverHandle):
+    """cosl_tri_solver: batched multi-view triangulation of points with their 3x3 covariance, on a stream and buffers
+    of its own for at most max_cams camera entries, max_pts points and max_views views (all points) per submit."""
+
+    _prefix = "cosl_tri_solver"
+
+    def __init__(self, device, max_cams, max_pts, max_views):
+        h = C.c_void_p()
+        _ck(LIB.cosl_tri_solver_create(int(device), int(max_cams), int(max_pts), int(max_views), C.byref(h)))
+        self.h, self.device = h, device
+        self.max_cams, self.max_pts, self.max_views = max_cams, max_pts, max_views
+        self._n = 0
+
+    def submit(self, K, R, t, view_off, view_cam, m, covm=None, cam_cov=None, pixel_var=1.0, max_err=float("inf")):
+        """cosl_tri_solver_submit: enqueue the triangulation and return at once; the input arrays may be reused when
+        it returns.  The camera table is K [C, 3, 3], R [C, 3, 3] (world to camera) and t [C, 3], with cam_cov a list
+        of C entries, None or a 6x6 pose covariance in the pose solver's chart (download_covariance's).  Point j has
+        the views view_off[j]:view_off[j + 1] (2 to 32 of them, the current frame last), each with a camera entry
+        view_cam [V], an observation m [V, 2] in px and, with covm [V, 2, 2] (px^2), its covariance; without covm,
+        pixel_var I.  A point with e_max >= max_err gets status 3."""
+        K = np.ascontiguousarray(K, np.float64).reshape(-1, 9)
+        Cn = len(K)
+        R = np.ascontiguousarray(R, np.float64).reshape(Cn, 9)
+        t = np.ascontiguousarray(t, np.float64).reshape(Cn, 3)
+        off = np.ascontiguousarray(view_off, np.int32).ravel()
+        vc = np.ascontiguousarray(view_cam, np.int32).ravel()
+        m = np.ascontiguousarray(m, np.float64).reshape(-1, 2)
+        if len(off) < 1 or len(vc) != len(m):
+            raise ValueError(f"view_off has {len(off)} entries, view_cam {len(vc)} and m {len(m)}")
+        cm = None if covm is None else _obs_cov(covm, len(m))
+        cp = keep = None
+        if cam_cov is not None:
+            if len(cam_cov) != Cn:
+                raise ValueError(f"cam_cov has {len(cam_cov)} entries for {Cn} cameras")
+            keep = [None if P is None else np.ascontiguousarray(P, np.float64).reshape(36) for P in cam_cov]
+            cp = (C.c_void_p * Cn)(*[None if P is None else P.ctypes.data for P in keep])
+        _ck(LIB.cosl_tri_solver_submit(self.h, Cn, _ptr(K), _ptr(R), _ptr(t), cp, len(off) - 1, _ptr(off), _ptr(vc),
+                                       _ptr(m), _ptr(cm), float(pixel_var), float(max_err)))
+        self._n = len(off) - 1
+
+    def collect(self):
+        """cosl_tri_solver_collect: wait for the submitted triangulation.  A dict of X [N, 3], P [N, 3, 3], stat [N, 4]
+        (f, e_max in px, parallax in radians, rho), status [N] (0 good, 1 behind a camera, 2 too uncertain, 3 e_max >=
+        max_err, 4 degenerate) and device_ms, the device time of its copies and kernel."""
+        n = self._n
+        X, P, st, status, ms = np.empty((n, 3)), np.empty((n, 3, 3)), np.empty((n, 4)), np.empty(n, np.int32), \
+            C.c_double(0)
+        _ck(LIB.cosl_tri_solver_collect(self.h, _ptr(X), _ptr(P), _ptr(st), _ptr(status), C.byref(ms)))
+        return dict(X=X, P=P, stat=st, status=status, device_ms=ms.value)
 
 
 def _map_points(entry):

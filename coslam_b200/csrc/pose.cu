@@ -13,6 +13,8 @@
 // covariance of each refined pose with the analytic Jacobian (an extension, not reference parity).
 // cosl_pose_solver_submit_prior anchors cameras with Gaussian pose priors (also an extension): the PRIOR
 // instantiations of both kernels add each prior's whitened residual to the costs, the LM step and the stage's H.
+// A triangulation handle (cosl_tri_solver, also an extension) runs tri_kernel, which shares the map-point update's
+// projection, Jacobians and 3x3 Cholesky.
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -976,6 +978,313 @@ pose_mappt_kernel(const int4* __restrict__ blk, const double* __restrict__ in, c
   o[12] = status;
 }
 
+// Multi-view triangulation of cosl_tri_solver_submit (DESIGN.md 5.5, an extension).  The camera table is staged as
+// TriCam records; per view, TRI_VIEW doubles m[2] | Sigma_m (xx xy yy); per point, TRI_OUT doubles come back:
+// X[3] | P (6: xx xy xz yy yz zz) | f, e_max, parallax, rho | status.  The per-view scratch holds TRI_SCRATCH doubles:
+// R_v^-1 (xx xy yy) | the unit ray from X+ to the camera centre.
+constexpr int TRI_THREADS = 64;
+constexpr int TRI_MAX_VIEWS = 32;
+constexpr int TRI_MAX_ITER = 10;
+constexpr int TRI_HALVINGS = 4;
+constexpr int TRI_VIEW = 5;
+constexpr int TRI_OUT = 14;
+constexpr int TRI_SCRATCH = 6;
+
+struct TriCam {
+  double K[9], Ki[9], R[9], t[3];  // Ki = K^-1, computed by the host
+  double P[36];                    // the pose covariance, read only when hasP
+  int hasP, pad;
+};
+
+// K, R and t of a camera record through the read-only path
+__device__ __forceinline__ void tri_cam(const TriCam* __restrict__ c, double K[9], double R[9], double t[3]) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    K[k] = __ldg(c->K + k);
+    R[k] = __ldg(c->R + k);
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) t[k] = __ldg(c->t + k);
+}
+
+// The camera centre -R^T t
+__device__ __forceinline__ void tri_centre(const double R[9], const double t[3], double C[3]) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k) C[k] = -(R[k] * t[0] + R[3 + k] * t[1] + R[6 + k] * t[2]);
+}
+
+// Rf += H_c P_c H_c^T: a camera's pose covariance P_c (6x6 row-major, chart R' = R exp([w]x), t' = t + dt) as noise of
+// the projection of X.  H_c is the analytic 2x6 Jacobian of 5.1 with rows (X x ha, a) and (X x hb, b), a, b, ha, hb as
+// mappt_project returns them at X: pose_mappt_kernel's R_eff arithmetic, which keeps its own inline copy (as a call it
+// compiles to a different register allocation).
+__device__ __forceinline__ void tri_pose_noise(const double X[3], const double a[3], const double b[3],
+                                               const double ha[3], const double hb[3], const double* Pc,
+                                               double Rf[3]) {
+  double Hc[12];
+  Hc[0] = X[1] * ha[2] - X[2] * ha[1];
+  Hc[1] = X[2] * ha[0] - X[0] * ha[2];
+  Hc[2] = X[0] * ha[1] - X[1] * ha[0];
+  Hc[6] = X[1] * hb[2] - X[2] * hb[1];
+  Hc[7] = X[2] * hb[0] - X[0] * hb[2];
+  Hc[8] = X[0] * hb[1] - X[1] * hb[0];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    Hc[3 + k] = a[k];
+    Hc[9 + k] = b[k];
+  }
+#pragma unroll
+  for (int k = 0; k < 6; ++k) {
+    double t0 = 0, t1 = 0;
+#pragma unroll
+    for (int l = 0; l < 6; ++l) {
+      t0 += Hc[l] * Pc[6 * l + k];
+      t1 += Hc[6 + l] * Pc[6 * l + k];
+    }
+    Rf[0] += t0 * Hc[k];
+    Rf[1] += t0 * Hc[6 + k];
+    Rf[2] += t1 * Hc[6 + k];
+  }
+}
+
+// mappt_chol3 of A with a smallest relative pivot L_kk^2 / A_kk of at least 1e-12: the positive-definiteness test of
+// every 3x3 this stage factors (A of the rays, N of the Gauss-Newton steps and of the covariance).  A point running
+// off to infinity leaves N singular to roundoff, where a plain Cholesky may still pass.
+__device__ __forceinline__ bool tri_chol3(const double A[6], double L[6]) {
+  return mappt_chol3(A, L) && fmin(fmin(L[0] * L[0] / A[0], L[2] * L[2] / A[3]), L[5] * L[5] / A[5]) >= 1e-12;
+}
+
+// One thread per point, over its views [off[j], off[j + 1]) (camera vcam[v], observation views[v]):
+//   1. X_lin = A^-1 b, A = sum (I - d d^T), b = sum (I - d d^T) C, d = normalize(R^T K^-1 [m; 1]), C = -R^T t, by
+//      Cholesky; a smallest relative pivot L_kk^2 / A_kk below 1e-12 (parallel rays) gives status 4;
+//   2. R_v = Sigma_m + H_c P_c H_c^T at X_lin (Sigma_m alone without P_c); R_v^-1 goes to the scratch; a non-positive
+//      definite R_v gives status 4;
+//   3. from X_lin in front of every camera, at most TRI_MAX_ITER Gauss-Newton steps s = N^-1 sum H_X^T R_v^-1 nu_v,
+//      N = sum H_X^T R_v^-1 H_X, each taken when it lowers f = sum nu^T R_v^-1 nu (the change formed from differences,
+//      as mappt_descent) and keeps every depth > 0, else halved at most TRI_HALVINGS times, and stopped at
+//      |s| <= 1e-12 max(1, |X|) or when N is not positive definite (tri_chol3);
+//   4. P = N^-1 at X+ by Cholesky, status 4 when N is not positive definite (tri_chol3);
+//   5. f, e_max = max |nu_v|, the largest angle between two rays X+ -> C_v, rho = sqrt(trace P) / |X+ - C_last|;
+//   6. status 4 degenerate (also any non-finite output), 1 a depth <= 0 at X_lin or X+, 2 rho > 1, 3 e_max >= max_err,
+//      else 0; with status 1 or 4 X, P and the statistics are NaN.
+// The view loops stay rolled: a point has up to TRI_MAX_VIEWS views.  __maxnreg__ instead of __launch_bounds__
+// (TRI_THREADS-thread CTAs either way): under the launch bounds ptxas stopped at 128 registers and spilled.
+__global__ void __maxnreg__(168)
+tri_kernel(const TriCam* __restrict__ cams, const double* __restrict__ views, const int* __restrict__ off,
+           const int* __restrict__ vcam, int nPts, double max_err, double* __restrict__ scratch,
+           double* __restrict__ out) {
+  const int j = blockIdx.x * TRI_THREADS + threadIdx.x;
+  if (j >= nPts) return;
+  const int o = off[j], n = off[j + 1] - o;
+  const double* q = views + (size_t)TRI_VIEW * o;
+  const int* vc = vcam + o;
+  double* W = scratch + (size_t)TRI_SCRATCH * o;
+  double* r = out + (size_t)TRI_OUT * j;
+  double K[9], R[9], t[3];
+  // 1. the point closest to every ray
+  double A[6] = {0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0};
+#pragma unroll 1
+  for (int v = 0; v < n; ++v) {
+    const TriCam* c = cams + vc[v];
+    tri_cam(c, K, R, t);
+    const double m0 = q[TRI_VIEW * v], m1 = q[TRI_VIEW * v + 1];
+    double x[3], d[3], C[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      x[k] = __ldg(c->Ki + 3 * k) * m0 + __ldg(c->Ki + 3 * k + 1) * m1 + __ldg(c->Ki + 3 * k + 2);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) d[k] = R[k] * x[0] + R[3 + k] * x[1] + R[6 + k] * x[2];
+    const double dn = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) d[k] /= dn;
+    tri_centre(R, t, C);
+    const double dc = d[0] * C[0] + d[1] * C[1] + d[2] * C[2];
+    A[0] += 1.0 - d[0] * d[0];
+    A[1] -= d[0] * d[1];
+    A[2] -= d[0] * d[2];
+    A[3] += 1.0 - d[1] * d[1];
+    A[4] -= d[1] * d[2];
+    A[5] += 1.0 - d[2] * d[2];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) b[k] += C[k] - d[k] * dc;
+  }
+  double L[6], Ai[6], X[3];
+  bool good = tri_chol3(A, L);
+  if (good) {
+    mappt_chol3_inv(L, Ai);
+    X[0] = Ai[0] * b[0] + Ai[1] * b[1] + Ai[2] * b[2];
+    X[1] = Ai[1] * b[0] + Ai[3] * b[1] + Ai[4] * b[2];
+    X[2] = Ai[2] * b[0] + Ai[4] * b[1] + Ai[5] * b[2];
+    good = isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]);
+  }
+  // 2. the noise of each view, fixed at X_lin
+  bool behind = false;
+#pragma unroll 1
+  for (int v = 0; good && v < n; ++v) {
+    const TriCam* c = cams + vc[v];
+    tri_cam(c, K, R, t);
+    double pm[2], a[3], bb[3], ha[3], hb[3], w;
+    behind |= !(mappt_project(K, R, t, X, pm, a, bb, ha, hb, &w) > 0);
+    double Rf[3] = {q[TRI_VIEW * v + 2], q[TRI_VIEW * v + 3], q[TRI_VIEW * v + 4]};
+    if (__ldg(&c->hasP)) tri_pose_noise(X, a, bb, ha, hb, c->P, Rf);
+    const double det = Rf[0] * Rf[2] - Rf[1] * Rf[1];
+    good = Rf[0] > 0 && det > 0 && isfinite(det) && isfinite(Rf[1]);
+    W[TRI_SCRATCH * v] = Rf[2] / det;
+    W[TRI_SCRATCH * v + 1] = -Rf[1] / det;
+    W[TRI_SCRATCH * v + 2] = Rf[0] / det;
+  }
+  if (!good) {
+#pragma unroll
+    for (int k = 0; k < 13; ++k) r[k] = NAN;
+    r[13] = 4;
+    return;
+  }
+  // 3. Gauss-Newton from X_lin
+#pragma unroll 1
+  for (int it = 0; !behind && it < TRI_MAX_ITER; ++it) {
+    double N[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0};
+#pragma unroll 1
+    for (int v = 0; v < n; ++v) {
+      tri_cam(cams + vc[v], K, R, t);
+      double pm[2], a[3], bb[3], ha[3], hb[3], w;
+      mappt_project(K, R, t, X, pm, a, bb, ha, hb, &w);
+      const double nu0 = q[TRI_VIEW * v] - pm[0], nu1 = q[TRI_VIEW * v + 1] - pm[1];
+      const double w00 = W[TRI_SCRATCH * v], w01 = W[TRI_SCRATCH * v + 1], w11 = W[TRI_SCRATCH * v + 2];
+      double wa[3], wb[3];  // rows of R_v^-1 H_X
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        wa[k] = w00 * ha[k] + w01 * hb[k];
+        wb[k] = w01 * ha[k] + w11 * hb[k];
+      }
+      int k = 0;
+#pragma unroll
+      for (int a0 = 0; a0 < 3; ++a0) {
+#pragma unroll
+        for (int a1 = a0; a1 < 3; ++a1) N[k++] += ha[a0] * wa[a1] + hb[a0] * wb[a1];
+        g[a0] += wa[a0] * nu0 + wb[a0] * nu1;
+      }
+    }
+    double Ln[6], Ni[6], s[3];
+    if (!tri_chol3(N, Ln)) break;
+    mappt_chol3_inv(Ln, Ni);
+    s[0] = Ni[0] * g[0] + Ni[1] * g[1] + Ni[2] * g[2];
+    s[1] = Ni[1] * g[0] + Ni[3] * g[1] + Ni[4] * g[2];
+    s[2] = Ni[2] * g[0] + Ni[4] * g[1] + Ni[5] * g[2];
+    bool taken = false;
+    double Xn[3];
+#pragma unroll 1
+    for (int h = 0; !taken && h <= TRI_HALVINGS; ++h) {
+      if (h) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) s[k] *= 0.5;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) Xn[k] = X[k] + s[k];
+      // f(X + s) - f(X) = -sum dpi^T R_v^-1 (2 nu - dpi), dpi = (dx_{0,1} - pi dx_2) / (x_2 + dx_2), dx = K R s
+      bool front = true;
+      double meas = 0;
+#pragma unroll 1
+      for (int v = 0; front && v < n; ++v) {
+        tri_cam(cams + vc[v], K, R, t);
+        double c[3], x[3], dc[3], dx[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          c[k] = R[3 * k] * X[0] + R[3 * k + 1] * X[1] + R[3 * k + 2] * X[2] + t[k];
+          dc[k] = R[3 * k] * s[0] + R[3 * k + 1] * s[1] + R[3 * k + 2] * s[2];
+        }
+        front = R[6] * Xn[0] + R[7] * Xn[1] + R[8] * Xn[2] + t[2] > 0;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          x[k] = K[3 * k] * c[0] + K[3 * k + 1] * c[1] + K[3 * k + 2] * c[2];
+          dx[k] = K[3 * k] * dc[0] + K[3 * k + 1] * dc[1] + K[3 * k + 2] * dc[2];
+        }
+        const double p0 = x[0] / x[2], p1 = x[1] / x[2];
+        const double wn = x[2] + dx[2];
+        const double dp0 = (dx[0] - p0 * dx[2]) / wn, dp1 = (dx[1] - p1 * dx[2]) / wn;
+        const double q0 = 2.0 * (q[TRI_VIEW * v] - p0) - dp0, q1 = 2.0 * (q[TRI_VIEW * v + 1] - p1) - dp1;
+        meas += W[TRI_SCRATCH * v] * dp0 * q0 + W[TRI_SCRATCH * v + 1] * (dp0 * q1 + dp1 * q0) +
+                W[TRI_SCRATCH * v + 2] * dp1 * q1;
+      }
+      taken = front && -meas < 0;
+    }
+    if (!taken) break;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) X[k] = Xn[k];
+    const double xn = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+    if (sqrt(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]) <= 1e-12 * fmax(1.0, xn)) break;
+  }
+  // 4.-5. covariance and statistics at X+
+  double N[6] = {0, 0, 0, 0, 0, 0}, f = 0, emax = 0, dlast = 0;
+#pragma unroll 1
+  for (int v = 0; v < n; ++v) {
+    tri_cam(cams + vc[v], K, R, t);
+    double pm[2], a[3], bb[3], ha[3], hb[3], w, C[3];
+    behind |= !(mappt_project(K, R, t, X, pm, a, bb, ha, hb, &w) > 0);
+    const double nu0 = q[TRI_VIEW * v] - pm[0], nu1 = q[TRI_VIEW * v + 1] - pm[1];
+    const double w00 = W[TRI_SCRATCH * v], w01 = W[TRI_SCRATCH * v + 1], w11 = W[TRI_SCRATCH * v + 2];
+    f += w00 * nu0 * nu0 + 2.0 * w01 * nu0 * nu1 + w11 * nu1 * nu1;
+    const double e = sqrt(nu0 * nu0 + nu1 * nu1);
+    emax = e > emax ? e : emax;
+    double wa[3], wb[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      wa[k] = w00 * ha[k] + w01 * hb[k];
+      wb[k] = w01 * ha[k] + w11 * hb[k];
+    }
+    int k = 0;
+#pragma unroll
+    for (int a0 = 0; a0 < 3; ++a0)
+#pragma unroll
+      for (int a1 = a0; a1 < 3; ++a1) N[k++] += ha[a0] * wa[a1] + hb[a0] * wb[a1];
+    tri_centre(R, t, C);
+    const double u0 = C[0] - X[0], u1 = C[1] - X[1], u2 = C[2] - X[2];
+    const double un = sqrt(u0 * u0 + u1 * u1 + u2 * u2);
+    W[TRI_SCRATCH * v + 3] = u0 / un;
+    W[TRI_SCRATCH * v + 4] = u1 / un;
+    W[TRI_SCRATCH * v + 5] = u2 / un;
+    dlast = un;
+  }
+  double Ln[6], P[6];
+  good = tri_chol3(N, Ln);
+  if (good) mappt_chol3_inv(Ln, P);
+  double par = 0;  // atan2(|u x w|, u . w) is accurate at small angles, where acos is not
+#pragma unroll 1
+  for (int v = 1; v < n; ++v) {
+    const double u0 = W[TRI_SCRATCH * v + 3], u1 = W[TRI_SCRATCH * v + 4], u2 = W[TRI_SCRATCH * v + 5];
+#pragma unroll 1
+    for (int i = 0; i < v; ++i) {
+      const double w0 = W[TRI_SCRATCH * i + 3], w1 = W[TRI_SCRATCH * i + 4], w2 = W[TRI_SCRATCH * i + 5];
+      const double x0 = u1 * w2 - u2 * w1, x1 = u2 * w0 - u0 * w2, x2 = u0 * w1 - u1 * w0;
+      const double ang = atan2(sqrt(x0 * x0 + x1 * x1 + x2 * x2), u0 * w0 + u1 * w1 + u2 * w2);
+      par = ang > par ? ang : par;
+    }
+  }
+  int status = 4;
+  if (good) {
+    const double rho = sqrt(P[0] + P[3] + P[5]) / dlast;
+    const double st[4] = {f, emax, par, rho};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) good = good && isfinite(X[k]);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) good = good && isfinite(P[k]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) good = good && isfinite(st[k]);
+    status = !good ? 4 : behind ? 1 : rho > 1.0 ? 2 : emax >= max_err ? 3 : 0;
+    if (status != 1 && status != 4) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) r[k] = X[k];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) r[3 + k] = P[k];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) r[9 + k] = st[k];
+    }
+  }
+  if (status == 1 || status == 4) {
+#pragma unroll
+    for (int k = 0; k < 13; ++k) r[k] = NAN;
+  }
+  r[13] = status;
+}
+
 
 // Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
 // cameras.
@@ -1465,6 +1774,165 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
 
 }  // namespace
 
+// A triangulation handle (cosl_tri_solver).  The inputs of one submit travel in one copy from a pinned staging buffer
+// laid out as TriCam[nCams] | views[nViews][TRI_VIEW] | viewOff[nPts + 1] | viewCam[nViews]; TRI_OUT doubles per
+// point come back into pinned memory.  Everything, the per-view scratch included, is allocated by create for at most
+// maxCams camera entries, maxPts points and maxViews views per submit.
+struct cosl_tri_solver {
+  int device = 0, maxCams = 0, maxPts = 0, maxViews = 0;
+  RequestStream rq;
+  unsigned char* h_in = nullptr;
+  unsigned char* d_in = nullptr;
+  double* d_scratch = nullptr;
+  double* d_out = nullptr;
+  double* h_out = nullptr;
+  int* seen = nullptr;  // [maxCams]: the last point that used each camera entry, for the repeated-camera check
+  int nPts = 0;         // points of the submit in flight or last collected
+};
+
+namespace {
+
+size_t tri_bytes(int nCams, int nPts, int nViews) {
+  return sizeof(TriCam) * nCams + sizeof(double) * TRI_VIEW * nViews + sizeof(int) * ((size_t)nPts + 1 + nViews);
+}
+
+void free_tri_solver(cosl_tri_solver* s) {
+  cudaSetDevice(s->device);
+  s->rq.destroy();
+  if (s->h_in) cudaFreeHost(s->h_in);
+  if (s->h_out) cudaFreeHost(s->h_out);
+  cudaFree(s->d_in);
+  cudaFree(s->d_scratch);
+  cudaFree(s->d_out);
+  delete[] s->seen;
+  delete s;
+}
+
+int alloc_tri_solver(cosl_tri_solver* s) {
+  s->seen = new (std::nothrow) int[s->maxCams];
+  if (!s->seen) return set_error(COSL_E_NOMEM, "cosl_tri_solver_create: out of host memory");
+  COSL_CUDA(cudaSetDevice(s->device));
+  COSL_TRY(s->rq.create());
+  const size_t in = tri_bytes(s->maxCams, s->maxPts, s->maxViews);
+  const size_t outb = sizeof(double) * TRI_OUT * s->maxPts;
+  COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
+  COSL_CUDA(cudaHostAlloc(&s->h_out, outb, cudaHostAllocPortable));
+  COSL_CUDA(cudaMalloc(&s->d_in, in));
+  COSL_CUDA(cudaMalloc(&s->d_scratch, sizeof(double) * TRI_SCRATCH * s->maxViews));
+  COSL_CUDA(cudaMalloc(&s->d_out, outb));
+  return COSL_OK;
+}
+
+// Checks one submit on the calling thread, naming the first bad camera, point or view.
+int check_tri(const char* fn, cosl_tri_solver* s, int nCams, const double* K9, const double* R, const double* t,
+              const double* const* camCov, int nPts, const int* viewOff, const int* viewCam, const double* m,
+              const double* covm, double pixel_var, double max_err) {
+  if (nCams < 0 || nPts < 0) return set_error(COSL_E_INVALID, "%s: nCams %d or nPts %d < 0", fn, nCams, nPts);
+  if (nCams > s->maxCams)
+    return set_error(COSL_E_INVALID, "%s: %d cameras exceed the handle's %d", fn, nCams, s->maxCams);
+  if (nPts > s->maxPts)
+    return set_error(COSL_E_INVALID, "%s: %d points exceed the handle's %d", fn, nPts, s->maxPts);
+  if (!viewOff || (nCams > 0 && (!K9 || !R || !t)) || (nPts > 0 && (!viewCam || !m)))
+    return set_error(COSL_E_INVALID, "%s: null argument", fn);
+  if (!std::isfinite(pixel_var) || !(pixel_var > 0))
+    return set_error(COSL_E_INVALID, "%s: pixel_var %g is not a finite value > 0", fn, pixel_var);
+  if (!(max_err > 0)) return set_error(COSL_E_INVALID, "%s: max_err %g is not > 0", fn, max_err);
+  for (int c = 0; c < nCams; ++c) {
+    for (int k = 0; k < 9; ++k)
+      if (!std::isfinite(K9[9 * c + k]) || !std::isfinite(R[9 * c + k]) || (k < 3 && !std::isfinite(t[3 * c + k])))
+        return set_error(COSL_E_INVALID, "%s: K, R or t of camera %d is not finite", fn, c);
+    // R a rotation and camCov symmetric and positive definite: the rules of a pose prior (R, t, P)
+    double rec[48] = {};
+    std::memcpy(rec, R + 9 * c, sizeof(double) * 9);
+    std::memcpy(rec + 9, t + 3 * c, sizeof(double) * 3);
+    if (camCov && camCov[c]) std::memcpy(rec + 12, camCov[c], sizeof(double) * 36);
+    else for (int k = 0; k < 6; ++k) rec[12 + 7 * k] = 1.0;
+    COSL_TRY(prior_factor(fn, c, rec, nullptr));
+  }
+  if (viewOff[0] != 0) return set_error(COSL_E_INVALID, "%s: viewOff[0] = %d is not 0", fn, viewOff[0]);
+  for (int c = 0; c < nCams; ++c) s->seen[c] = -1;
+  for (int j = 0; j < nPts; ++j) {
+    const int n = viewOff[j + 1] - viewOff[j];
+    if (viewOff[j + 1] < viewOff[j] || n < 2 || n > TRI_MAX_VIEWS)
+      return set_error(COSL_E_INVALID, "%s: point %d has %d views, not 2 to %d", fn, j, n, TRI_MAX_VIEWS);
+    if (viewOff[j + 1] > s->maxViews)
+      return set_error(COSL_E_INVALID, "%s: point %d: %d views exceed the handle's %d", fn, j, viewOff[j + 1],
+                       s->maxViews);
+    for (int v = viewOff[j]; v < viewOff[j + 1]; ++v) {
+      const int c = viewCam[v];
+      if (c < 0 || c >= nCams)
+        return set_error(COSL_E_INVALID, "%s: view %d of point %d: camera %d is not in [0, %d)", fn, v, j, c, nCams);
+      if (s->seen[c] == j)
+        return set_error(COSL_E_INVALID, "%s: view %d of point %d: camera %d is used twice", fn, v, j, c);
+      s->seen[c] = j;
+      if (!std::isfinite(m[2 * (size_t)v]) || !std::isfinite(m[2 * (size_t)v + 1]))
+        return set_error(COSL_E_INVALID, "%s: view %d of point %d: m is not finite", fn, v, j);
+      double L[3];
+      if (covm && !cov_factor(covm + 4 * (size_t)v, L))
+        return set_error(COSL_E_INVALID, "%s: view %d of point %d: covm is not finite, symmetric and positive definite",
+                         fn, v, j);
+    }
+  }
+  return COSL_OK;
+}
+
+// Stages a checked submit and enqueues the copy, tri_kernel and the read-back.
+int stage_tri(cosl_tri_solver* s, int nCams, const double* K9, const double* R, const double* t,
+              const double* const* camCov, int nPts, const int* viewOff, const int* viewCam, const double* m,
+              const double* covm, double pixel_var, double max_err) {
+  const int nViews = viewOff[nPts];
+  TriCam* hc = reinterpret_cast<TriCam*>(s->h_in);
+  double* hv = reinterpret_cast<double*>(s->h_in + sizeof(TriCam) * nCams);
+  int* ho = reinterpret_cast<int*>(hv + (size_t)TRI_VIEW * nViews);
+  for (int c = 0; c < nCams; ++c) {
+    TriCam& e = hc[c];
+    const double* k = K9 + 9 * c;
+    std::memcpy(e.K, k, sizeof(double) * 9);
+    std::memcpy(e.R, R + 9 * c, sizeof(double) * 9);
+    std::memcpy(e.t, t + 3 * c, sizeof(double) * 3);
+    // K^-1 by the adjugate; a singular K gives non-finite rays and status 4
+    const double det = k[0] * (k[4] * k[8] - k[5] * k[7]) - k[1] * (k[3] * k[8] - k[5] * k[6]) +
+                       k[2] * (k[3] * k[7] - k[4] * k[6]);
+    const double adj[9] = {k[4] * k[8] - k[5] * k[7], k[2] * k[7] - k[1] * k[8], k[1] * k[5] - k[2] * k[4],
+                           k[5] * k[6] - k[3] * k[8], k[0] * k[8] - k[2] * k[6], k[2] * k[3] - k[0] * k[5],
+                           k[3] * k[7] - k[4] * k[6], k[1] * k[6] - k[0] * k[7], k[0] * k[4] - k[1] * k[3]};
+    for (int i = 0; i < 9; ++i) e.Ki[i] = adj[i] / det;
+    e.hasP = camCov && camCov[c] ? 1 : 0;
+    e.pad = 0;
+    if (e.hasP)  // symmetrised, as prior_factor checked it
+      for (int a = 0; a < 6; ++a)
+        for (int b = 0; b < 6; ++b) e.P[6 * a + b] = 0.5 * (camCov[c][6 * a + b] + camCov[c][6 * b + a]);
+  }
+  for (int v = 0; v < nViews; ++v) {
+    double* q = hv + (size_t)TRI_VIEW * v;
+    q[0] = m[2 * (size_t)v];
+    q[1] = m[2 * (size_t)v + 1];
+    const double* cv = covm ? covm + 4 * (size_t)v : nullptr;  // Sigma_m = pixel_var I without covm
+    q[2] = cv ? cv[0] : pixel_var;
+    q[3] = cv ? cv[1] : 0.0;
+    q[4] = cv ? cv[3] : pixel_var;
+  }
+  std::memcpy(ho, viewOff, sizeof(int) * ((size_t)nPts + 1));
+  if (nViews) std::memcpy(ho + nPts + 1, viewCam, sizeof(int) * (size_t)nViews);
+  s->nPts = nPts;
+  cudaStream_t st = s->rq.stream;
+  return s->rq.submit("cosl_tri_solver_submit", [&]() -> int {
+    COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, tri_bytes(nCams, nPts, nViews), cudaMemcpyHostToDevice, st));
+    if (nPts > 0) {
+      const TriCam* d_cams = reinterpret_cast<const TriCam*>(s->d_in);
+      const double* d_views = reinterpret_cast<const double*>(s->d_in + sizeof(TriCam) * nCams);
+      const int* d_off = reinterpret_cast<const int*>(d_views + (size_t)TRI_VIEW * nViews);
+      COSL_LAUNCH(tri_kernel, div_up(nPts, TRI_THREADS), TRI_THREADS, 0, st, d_cams, d_views, d_off,
+                  d_off + nPts + 1, nPts, max_err, s->d_scratch, s->d_out);
+      COSL_CUDA(cudaGetLastError());
+      COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * TRI_OUT * nPts, cudaMemcpyDeviceToHost, st));
+    }
+    return COSL_OK;
+  });
+}
+
+}  // namespace
+
 extern "C" {
 
 void cosl_pose_opt_default(cosl_pose_opt* o) {
@@ -1699,5 +2167,74 @@ int cosl_pose_intracam(const double K[9], const double R0[9], const double t0[3]
   return cosl_pose_intracam_batch(1, K, R0, t0, &npts, Msp, msp, prevErrs ? pep : nullptr, tau,
                                   R_opt, t_opt, opt, ok, device);
 }
+
+int cosl_tri_solver_create(int device, int maxCams, int maxPts, int maxViews, cosl_tri_solver** out) {
+  if (!out || device < 0 || maxCams < 1 || maxPts < 1 || maxViews < 2)
+    return set_error(COSL_E_INVALID, "cosl_tri_solver_create: bad argument");
+  *out = nullptr;
+  COSL_TRY(check_device(device));
+  cosl_tri_solver* s = new (std::nothrow) cosl_tri_solver;
+  if (!s) return set_error(COSL_E_NOMEM, "cosl_tri_solver_create: out of host memory");
+  s->device = device;
+  s->maxCams = maxCams;
+  s->maxPts = maxPts;
+  s->maxViews = maxViews;
+  const int rc = alloc_tri_solver(s);
+  if (rc != COSL_OK) {
+    free_tri_solver(s);
+    return rc;
+  }
+  *out = s;
+  return COSL_OK;
+}
+
+int cosl_tri_solver_destroy(cosl_tri_solver* s) {
+  if (!s) return set_error(COSL_E_INVALID, "null triangulation handle");
+  free_tri_solver(s);
+  return COSL_OK;
+}
+
+int cosl_tri_solver_submit(cosl_tri_solver* s, int nCams, const double* K9, const double* R, const double* t,
+                           const double* const* camCov, int nPts, const int* viewOff, const int* viewCam,
+                           const double* m, const double* covm, double pixel_var, double max_err) {
+  const char* fn = "cosl_tri_solver_submit";
+  if (!s) return set_error(COSL_E_INVALID, "null triangulation handle");
+  COSL_TRY(s->rq.idle(fn));
+  COSL_TRY(check_tri(fn, s, nCams, K9, R, t, camCov, nPts, viewOff, viewCam, m, covm, pixel_var, max_err));
+  COSL_CUDA(cudaSetDevice(s->device));
+  return stage_tri(s, nCams, K9, R, t, camCov, nPts, viewOff, viewCam, m, covm, pixel_var, max_err);
+}
+
+int cosl_tri_solver_query(cosl_tri_solver* s, int* done) {
+  if (!s || !done) return set_error(COSL_E_INVALID, "cosl_tri_solver_query: null argument");
+  COSL_TRY(s->rq.pending("cosl_tri_solver_query"));
+  COSL_CUDA(cudaSetDevice(s->device));
+  return s->rq.query(done);
+}
+
+int cosl_tri_solver_collect(cosl_tri_solver* s, double* X, double* P, double* stat, int* status, double* device_ms) {
+  if (!s) return set_error(COSL_E_INVALID, "null triangulation handle");
+  COSL_TRY(s->rq.pending("cosl_tri_solver_collect"));
+  COSL_CUDA(cudaSetDevice(s->device));
+  COSL_TRY(s->rq.wait(device_ms));
+  for (int j = 0; j < s->nPts; ++j) {
+    const double* r = s->h_out + (size_t)TRI_OUT * j;
+    if (X) std::memcpy(X + 3 * (size_t)j, r, sizeof(double) * 3);
+    if (P) {
+      double* p = P + 9 * (size_t)j;
+      p[0] = r[3];
+      p[1] = p[3] = r[4];
+      p[2] = p[6] = r[5];
+      p[4] = r[6];
+      p[5] = p[7] = r[7];
+      p[8] = r[8];
+    }
+    if (stat) std::memcpy(stat + 4 * (size_t)j, r + 9, sizeof(double) * 4);
+    if (status) status[j] = (int)r[13];
+  }
+  return COSL_OK;
+}
+
+void* cosl_tri_solver_stream(cosl_tri_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
 
 }  // extern "C"

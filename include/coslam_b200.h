@@ -523,6 +523,71 @@ int cosl_pose_solver_submit_mappts(cosl_pose_solver* s, int C, const double* K9,
  * flight, or when the last submit was not a submit_mappts. */
 int cosl_pose_solver_download_mappts(cosl_pose_solver* s, double* X, double* P, double* stat, int* status);
 
+/* A triangulation handle: batched multi-view triangulation of map points with their 3x3 covariance (an
+ * extension: the birth of a MapPoint's M and cov in SingleSLAM::newMapPoints, updateStaticPointPosition and
+ * NewMapPointsInterCam, whose triangulation functions are not in this tree; DESIGN.md 5.5).  A handle owns
+ * a non-blocking stream, a pinned staging buffer, device buffers, a per-view scratch and a pinned result
+ * buffer, all allocated by create for at most maxCams camera entries, maxPts points and maxViews views (all
+ * points together) per submit; no submit allocates.  Without a usable device create gives COSL_E_CUDA; there
+ * is no CPU path.  COSL_E_INVALID for maxCams < 1, maxPts < 1 or maxViews < 2.
+ *
+ * submit: a camera table of nCams entries, K9[9 nCams], R[9 nCams] (row-major, world to camera) and
+ * t[3 nCams], and camCov (nullable, as camCov[c]): the entry's 6x6 pose covariance, row-major, in the pose
+ * solver's chart R' = R exp([w]x), t' = t + dt, order (w, dt), so a download_covariance block is valid as it
+ * stands (a BA camCov, in the chart exp([w]x) R, converts as blockdiag(R^T, I) P blockdiag(R, I)).  nPts
+ * points in CSR form: point j has the views [viewOff[j], viewOff[j + 1]), 2 to 32 of them, viewOff[0] = 0;
+ * view v has the camera entry viewCam[v], the observation m[2 v] in px and covm[4 v] (covm nullable), its
+ * row-major 2x2 covariance [xx, xy, yx, yy] in px^2; without covm, Sigma_m = pixel_var I.  A point uses a
+ * camera entry at most once; pass the current frame's view last (rho below).  Per point, in fp64, with pi
+ * the pose solver's projection, H_X = (a; b) R its Jacobian in X and H_c the covariance stage's 2x6 one:
+ *   1. X_lin = A^-1 b, A = sum (I - d d^T), b = sum (I - d d^T) C, d = normalize(R^T K^-1 [m; 1]) and
+ *      C = -R^T t per view: the point closest to every ray, by Cholesky;
+ *   2. R_v = Sigma_m + H_c(X_lin) P_c H_c(X_lin)^T (Sigma_m without camCov), fixed from here on;
+ *   3. from X_lin, at most 10 Gauss-Newton steps s = (sum H_X^T R_v^-1 H_X)^-1 sum H_X^T R_v^-1 nu_v on
+ *      f(X) = sum nu_v^T R_v^-1 nu_v, nu_v = m_v - pi_v(X), each taken only when it lowers f and keeps
+ *      every depth > 0, else halved at most 4 times; stopped at |s| <= 1e-12 max(1, |X|).  No step is
+ *      taken from an X_lin behind a camera;
+ *   4. P = (sum H_X^T R_v^-1 H_X)^-1 at X+, by Cholesky, symmetric.  Every 3x3 here counts as positive
+ *      definite only with a smallest relative Cholesky pivot L_kk^2 / A_kk of at least 1e-12, and the
+ *      Gauss-Newton loop also stops at an information matrix that is not;
+ *   5. stat[4] = {f(X+), e_max = max |nu_v| in px, the parallax (the largest angle at X+ between two
+ *      rays X+ -> C_v, in radians), rho = sqrt(trace P) / |X+ - C_last|, C_last the point's last view};
+ *   6. status 4 degenerate (a smallest relative pivot L_kk^2 / A_kk below 1e-12, i.e. parallel rays; a
+ *      non-finite value; R_v or the information matrix not positive definite), else 1 a depth <= 0 at
+ *      X_lin or X+, else 2 rho > 1, else 3 e_max >= max_err, else 0.  With status 0, 2 or 3, X, P and
+ *      stat are as computed; with 1 or 4 they are NaN.
+ * Each point is solved on its own, so a point's output does not depend on the others of the submit.
+ * submit checks everything on the calling thread before anything is staged, and gives COSL_E_INVALID
+ * naming the first bad camera, point or view (the handle stays usable) for: counts above the reserved
+ * sizes; a NULL required array; a non-finite K, R, t or m; an R that is not a rotation (|R^T R - I|_max
+ * <= 1e-9, det > 0) or a camCov that is not symmetric to 1e-12 of its largest diagonal entry or not
+ * positive definite (the rules of a pose prior, and the message names the entry as a camera's prior); a
+ * covm failing submit_cov's rules; a view camera out of range or used twice in one point; a point with
+ * fewer than 2 or more than 32 views or a viewOff that is not monotone; a pixel_var that is not finite
+ * and > 0; a max_err that is not > 0 (+inf accepts every e_max).  It packs the inputs into pinned memory,
+ * so the caller may reuse its arrays when it returns, enqueues one host-to-device copy, tri_kernel and
+ * one device-to-host copy on the handle's stream, and returns without waiting for the device.
+ *
+ * query sets *done = 1 once the request has finished, without waiting.  collect waits for it and writes,
+ * per point in submit order, X[3 n], P[9 n] (row-major), stat[4 n] and status[n], every output nullable;
+ * *device_ms (nullable) is the device time of the copies and the kernel, from CUDA events.  One request
+ * may be in flight per handle: a second submit gives COSL_E_STATE, and so do query and collect with
+ * nothing in flight.  destroy waits for a request in flight.  A handle is not re-entrant; different
+ * handles share no lock.  Every call makes the handle's device current on the calling thread. */
+typedef struct cosl_tri_solver cosl_tri_solver;
+int cosl_tri_solver_create(int device, int maxCams, int maxPts, int maxViews, cosl_tri_solver** out);
+int cosl_tri_solver_destroy(cosl_tri_solver* s);
+int cosl_tri_solver_submit(cosl_tri_solver* s, int nCams, const double* K9, const double* R,
+                           const double* t, const double* const* camCov, int nPts, const int* viewOff,
+                           const int* viewCam, const double* m, const double* covm, double pixel_var,
+                           double max_err);
+int cosl_tri_solver_query(cosl_tri_solver* s, int* done);
+int cosl_tri_solver_collect(cosl_tri_solver* s, double* X, double* P, double* stat, int* status,
+                            double* device_ms);
+/* CUDA stream (cudaStream_t as void*) the handle's requests run on; work enqueued there after a submit
+ * runs after that request. */
+void* cosl_tri_solver_stream(cosl_tri_solver* s);
+
 /* ================================================================ bundle adjustment */
 
 /* Flat form of the arguments of
