@@ -98,6 +98,14 @@ def _load():
     L.cosl_tri_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
     L.cosl_tri_solver_stream.argtypes = [vp]
     L.cosl_tri_solver_stream.restype = vp
+    L.cosl_assoc_solver_create.argtypes = [ci, ci, ci, ci, ci, ci, C.POINTER(vp)]
+    L.cosl_assoc_solver_destroy.argtypes = [vp]
+    L.cosl_assoc_solver_submit.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp,
+                                           cd, cd, cd]
+    L.cosl_assoc_solver_query.argtypes = [vp, pint]
+    L.cosl_assoc_solver_collect.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.cosl_assoc_solver_stream.argtypes = [vp]
+    L.cosl_assoc_solver_stream.restype = vp
     L.cosl_ba_options_default.argtypes = [C.POINTER(BaOptions)]
     L.cosl_ba_solve.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), vp]
     L.cosl_ba_solve_multi.argtypes = [C.POINTER(BaProblem), C.POINTER(BaOptions), ci, vp, vp]
@@ -755,6 +763,70 @@ class TriSolver(_SolverHandle):
             C.c_double(0)
         _ck(LIB.cosl_tri_solver_collect(self.h, _ptr(X), _ptr(P), _ptr(st), _ptr(status), C.byref(ms)))
         return dict(X=X, P=P, stat=st, status=status, device_ms=ms.value)
+
+
+class AssocSolver(_SolverHandle):
+    """cosl_assoc_solver: batched Mahalanobis nearest-feature search of map points in the current frame's features, on
+    a stream and buffers of its own for at most max_cams camera entries, max_pts points, max_queries query pairs,
+    max_feats features and max_track_obs track observations per submit."""
+
+    _prefix = "cosl_assoc_solver"
+
+    def __init__(self, device, max_cams, max_pts, max_queries, max_feats, max_track_obs=0):
+        h = C.c_void_p()
+        _ck(LIB.cosl_assoc_solver_create(int(device), int(max_cams), int(max_pts), int(max_queries), int(max_feats),
+                                         int(max_track_obs), C.byref(h)))
+        self.h, self.device = h, device
+        self._n = 0
+
+    def submit(self, K, R, t, wh, feat_off, mf, X, P, q_off, q_cam, covf=None, owned=None, cam_cov=None,
+               trk_off=None, trk_cam=None, trk_m=None, pixel_var=1.0, gate=9.21, track_gate=float("inf")):
+        """cosl_assoc_solver_submit: enqueue the search and return at once; the input arrays may be reused when it
+        returns.  The camera table is K [C, 3, 3], R [C, 3, 3] (world to camera), t [C, 3], wh [C, 2] (image width
+        and height in px) and cam_cov, a list of C entries, None or a 6x6 pose covariance in the pose solver's chart.
+        Entry c has the features feat_off[c]:feat_off[c + 1] of mf [F, 2] (undistorted px), with covf [F, 2, 2]
+        (px^2; pixel_var I without it), owned [F] (0 or 1) and the track trk_off[f]:trk_off[f + 1] of trk_cam [T] and
+        trk_m [T, 2].  Point j, X [N, 3] and P [N, 3, 3], searches the entries q_cam[q_off[j]:q_off[j + 1]]."""
+        K = np.ascontiguousarray(K, np.float64).reshape(-1, 9)
+        Cn = len(K)
+        R = np.ascontiguousarray(R, np.float64).reshape(Cn, 9)
+        t = np.ascontiguousarray(t, np.float64).reshape(Cn, 3)
+        wh = np.ascontiguousarray(wh, np.int32).reshape(Cn, 2)
+        fo = np.ascontiguousarray(feat_off, np.int32).ravel()
+        mf = np.ascontiguousarray(mf, np.float64).reshape(-1, 2)
+        X = np.ascontiguousarray(X, np.float64).reshape(-1, 3)
+        P = np.ascontiguousarray(P, np.float64).reshape(-1, 9)
+        qo = np.ascontiguousarray(q_off, np.int32).ravel()
+        qc = np.ascontiguousarray(q_cam, np.int32).ravel()
+        if len(fo) != Cn + 1 or len(qo) != len(X) + 1 or len(P) != len(X):
+            raise ValueError(f"feat_off has {len(fo)} entries for {Cn} cameras, q_off {len(qo)} and P {len(P)} for "
+                             f"{len(X)} points")
+        cf = None if covf is None else _obs_cov(covf, len(mf))
+        ow = None if owned is None else np.ascontiguousarray(owned, np.int32).ravel()
+        to = None if trk_off is None else np.ascontiguousarray(trk_off, np.int32).ravel()
+        tc = None if trk_cam is None else np.ascontiguousarray(trk_cam, np.int32).ravel()
+        tm = None if trk_m is None else np.ascontiguousarray(trk_m, np.float64).reshape(-1, 2)
+        cp = keep = None
+        if cam_cov is not None:
+            if len(cam_cov) != Cn:
+                raise ValueError(f"cam_cov has {len(cam_cov)} entries for {Cn} cameras")
+            keep = [None if Pc is None else np.ascontiguousarray(Pc, np.float64).reshape(36) for Pc in cam_cov]
+            cp = (C.c_void_p * Cn)(*[None if Pc is None else Pc.ctypes.data for Pc in keep])
+        _ck(LIB.cosl_assoc_solver_submit(self.h, Cn, _ptr(K), _ptr(R), _ptr(t), cp, _ptr(wh), _ptr(fo), _ptr(mf),
+                                         _ptr(cf), _ptr(ow), _ptr(to), _ptr(tc), _ptr(tm), len(X), _ptr(X), _ptr(P),
+                                         _ptr(qo), _ptr(qc), float(pixel_var), float(gate), float(track_gate)))
+        self._n = int(qo[-1])
+
+    def collect(self):
+        """cosl_assoc_solver_collect: wait for the submitted search.  A dict of status [Q] (0 registered, 1 behind the
+        camera, 2 outside the image, 3 no feature in the gate, 4 owned, 5 the track disagrees, 6 claimed by another
+        point, 7 non-finite), feat [Q] (-1 without one), d2 [Q, 2] (d2 of feat and the second least in the gate),
+        pred [Q, 5] (m_hat, S xx xy yy) and device_ms, the device time of its copies and kernels."""
+        n = self._n
+        st, ft, d2, pr, ms = np.empty(n, np.int32), np.empty(n, np.int32), np.empty((n, 2)), np.empty((n, 5)), \
+            C.c_double(0)
+        _ck(LIB.cosl_assoc_solver_collect(self.h, _ptr(st), _ptr(ft), _ptr(d2), _ptr(pr), C.byref(ms)))
+        return dict(status=st, feat=ft, d2=d2, pred=pr, device_ms=ms.value)
 
 
 def _map_points(entry):

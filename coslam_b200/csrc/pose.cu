@@ -15,6 +15,8 @@
 // instantiations of both kernels add each prior's whitened residual to the costs, the LM step and the stage's H.
 // A triangulation handle (cosl_tri_solver, also an extension) runs tri_kernel, which shares the map-point update's
 // projection, Jacobians and 3x3 Cholesky.
+// A registration handle (cosl_assoc_solver, also an extension) bins each entry's features into a uniform grid and
+// runs one search thread per (map point, camera entry) pair on the same projection and Jacobians.
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -1285,6 +1287,232 @@ tri_kernel(const TriCam* __restrict__ cams, const double* __restrict__ views, co
   r[13] = status;
 }
 
+// Map-point registration of cosl_assoc_solver_submit (DESIGN.md 5.6, an extension).  The camera table is staged as
+// AssocCam records; per point ASSOC_PT doubles X[3] | P_X (6: xx xy xz yy yz zz); per feature ASSOC_FEAT doubles
+// m_f[2] | Sigma_f (xx xy yy) and its cell (an int, cell0 of its entry + cy nx + cx, cx = clamp(floor(x / ASSOC_CELL),
+// 0, nx - 1), likewise cy); per track observation 2 doubles m_k.  Per query pair, ASSOC_OUT doubles come back:
+// status | feat | d2, d2_2 | pred (m_hat[2], S xx xy yy).
+constexpr int ASSOC_THREADS = 64;
+constexpr int ASSOC_BIN_THREADS = 256;
+constexpr int ASSOC_SCAN_THREADS = 1024;
+constexpr int ASSOC_CELL = 32;          // px, the side of a grid cell
+constexpr int ASSOC_MAX_SIDE = 4096;    // px, the largest image width or height an entry may have
+constexpr int ASSOC_MAX_CELLS = (ASSOC_MAX_SIDE / ASSOC_CELL) * (ASSOC_MAX_SIDE / ASSOC_CELL);  // per entry
+constexpr int ASSOC_MAX_QUERIES = 32;   // per point
+constexpr int ASSOC_PT = 9;
+constexpr int ASSOC_FEAT = 5;
+constexpr int ASSOC_OUT = 9;
+
+struct AssocCam {
+  double K[9], R[9], t[3];
+  double P[36];    // the pose covariance, read only when hasP
+  double lam;      // the largest lambda_max(Sigma_f) over the entry's features, from the host
+  double W, H;     // image size, px
+  int hasP, nx, ny, cell0;  // the entry's grid: nx x ny cells from cell0 on
+};
+
+// d2 = |L^-1 nu|^2 with L L^T = A (a symmetric 2x2, xx xy yy): never negative; NaN unless A is positive definite
+__device__ __forceinline__ double assoc_d2(const double A[3], double nu0, double nu1) {
+  const double l00 = sqrt(A[0]);
+  const double l10 = A[1] / l00;
+  const double l11 = sqrt(A[2] - l10 * l10);
+  const double z0 = nu0 / l00;
+  const double z1 = (nu1 - l10 * z0) / l11;
+  return z0 * z0 + z1 * z1;
+}
+
+// The projection m_hat of X in entry c and S = H_X P_X H_X^T (+ H_c P_c H_c^T with the entry's P_c) + add I; returns
+// the depth.
+__device__ __forceinline__ double assoc_predict(const AssocCam* __restrict__ c, const double X[3], const double PX[6],
+                                                double add, double m[2], double S[3]) {
+  double K[9], R[9], t[3];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    K[k] = __ldg(c->K + k);
+    R[k] = __ldg(c->R + k);
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) t[k] = __ldg(c->t + k);
+  double a[3], b[3], ha[3], hb[3], w, U[6];
+  const double z = mappt_project(K, R, t, X, m, a, b, ha, hb, &w);
+  double Rf[3] = {add, 0.0, add};
+  if (__ldg(&c->hasP)) tri_pose_noise(X, a, b, ha, hb, c->P, Rf);
+  mappt_innov(ha, hb, PX, Rf, U, S);
+  return z;
+}
+
+// Count the features of every cell; cell[f] was staged by the host.
+__global__ void __launch_bounds__(ASSOC_BIN_THREADS)
+assoc_count_kernel(const int* __restrict__ cell, int nFeats, int* __restrict__ count) {
+  const int f = blockIdx.x * ASSOC_BIN_THREADS + threadIdx.x;
+  if (f < nFeats) atomicAdd(count + cell[f], 1);
+}
+
+// One CTA per entry: start[cell0 + i] = featOff[e] + the exclusive scan of the entry's cell counts, and the counts
+// zeroed for the scatter's cursors.  The last entry also writes start[cells] = featOff[nCams], so that every cell's
+// features are [start[i], start[i + 1]).
+__global__ void __launch_bounds__(ASSOC_SCAN_THREADS)
+assoc_scan_kernel(const AssocCam* __restrict__ cams, const int* __restrict__ featOff, int nCams,
+                  int* __restrict__ count, int* __restrict__ start) {
+  __shared__ int s_warp[ASSOC_SCAN_THREADS / 32];
+  const int e = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c0 = cams[e].cell0, n = cams[e].nx * cams[e].ny;
+  int carry = featOff[e];
+  for (int base = 0; base < n; base += ASSOC_SCAN_THREADS) {
+    const int i = base + threadIdx.x;
+    const int v = i < n ? count[c0 + i] : 0;
+    int x = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, x, d);
+      if (lane >= d) x += y;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      int w = s_warp[lane];
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, w, d);
+        if (lane >= d) w += y;
+      }
+      s_warp[lane] = w;
+    }
+    __syncthreads();
+    if (i < n) {
+      start[c0 + i] = carry + x - v + (warp ? s_warp[warp - 1] : 0);
+      count[c0 + i] = 0;
+    }
+    carry += s_warp[ASSOC_SCAN_THREADS / 32 - 1];
+    __syncthreads();
+  }
+  if (e == nCams - 1 && threadIdx.x == 0) start[c0 + n] = featOff[nCams];
+}
+
+// Scatter every feature index into its cell's range of sorted; the order inside a cell is whatever the atomics give.
+__global__ void __launch_bounds__(ASSOC_BIN_THREADS)
+assoc_scatter_kernel(const int* __restrict__ cell, int nFeats, const int* __restrict__ start, int* __restrict__ cursor,
+                     int* __restrict__ sorted) {
+  const int f = blockIdx.x * ASSOC_BIN_THREADS + threadIdx.x;
+  if (f < nFeats) {
+    const int c = cell[f];
+    sorted[start[c] + atomicAdd(cursor + c, 1)] = f;
+  }
+}
+
+// One thread per query pair q (point qPt[q], entry qCam[q]):
+//   1. x = R X + t, m_hat = pi(X), S = H_X P_X H_X^T + H_c P_c H_c^T (the second term with the entry's P_c only);
+//      status 7 unless depth, m_hat and S are finite, 1 depth <= 0, 2 m_hat outside [0, W) x [0, H);
+//   2. over the features of the cells the box |dx| <= sqrt(gate (S + lam I)_xx), |dy| <= sqrt(gate (S + lam I)_yy)
+//      covers (widened by 1e-6 relative; lam >= lambda_max(Sigma_f) of every feature of the entry, so the box holds
+//      every gate ellipse): d2_f = |L^-1 (m_f - m_hat)|^2, L L^T = S + Sigma_f; f* the least (d2, f) with d2 < gate,
+//      d2_2 the second least d2 (+inf without one); status 3 without f*;
+//   3. status 4 when f* is owned;
+//   4. with a finite track_gate, status 5 when an earlier observation k of f* (entry trkCam[k], m_k) has depth <= 0
+//      or not d2_k < track_gate, d2_k = |L^-1 (m_k - pi_k(X))|^2, L L^T = H_X P_X H_X^T + H_c P_c H_c^T + pixel_var I;
+//   5. a pair still at status 0 enters the claims: pass one of the claim resolution, key[f*] = min bits of d2.
+// The record gets status (0 for a claimant, resolved by assoc_claim_kernel and assoc_final_kernel), feat (-1 for 1, 2,
+// 3 and 7), d2 and d2_2 (NaN for 1, 2 and 7; +inf for 3) and pred (NaN for 1 and 7).
+__global__ void __launch_bounds__(ASSOC_THREADS)
+assoc_search_kernel(const AssocCam* __restrict__ cams, const double* __restrict__ pts,
+                    const double* __restrict__ feats, const int* __restrict__ owned,
+                    const int* __restrict__ trkOff, const int* __restrict__ trkCam, const double* __restrict__ trkM,
+                    const int* __restrict__ qPt, const int* __restrict__ qCam, int nQ,
+                    const int* __restrict__ start, const int* __restrict__ sorted, double pixel_var, double gate,
+                    double track_gate, unsigned long long* __restrict__ key, double* __restrict__ out) {
+  const int q = blockIdx.x * ASSOC_THREADS + threadIdx.x;
+  if (q >= nQ) return;
+  double* r = out + (size_t)ASSOC_OUT * q;
+  const double* pj = pts + (size_t)ASSOC_PT * qPt[q];
+  const double X[3] = {pj[0], pj[1], pj[2]};
+  const double PX[6] = {pj[3], pj[4], pj[5], pj[6], pj[7], pj[8]};
+  const AssocCam* c = cams + qCam[q];
+  double m[2], S[3];
+  const double z = assoc_predict(c, X, PX, 0.0, m, S);
+  int status = !(isfinite(z) && isfinite(m[0]) && isfinite(m[1]) && isfinite(S[0]) && isfinite(S[1]) &&
+                 isfinite(S[2])) ? 7
+               : !(z > 0) ? 1
+               : !(m[0] >= 0 && m[0] < __ldg(&c->W) && m[1] >= 0 && m[1] < __ldg(&c->H)) ? 2 : 0;
+  double best = INFINITY, second = INFINITY;
+  int fs = -1;
+  if (status == 0) {
+    const double lam = __ldg(&c->lam);
+    const int nx = __ldg(&c->nx), ny = __ldg(&c->ny), c0 = __ldg(&c->cell0);
+    const double hx = sqrt(gate * (S[0] + lam)) * (1.0 + 1e-6), hy = sqrt(gate * (S[2] + lam)) * (1.0 + 1e-6);
+    const double inv = 1.0 / ASSOC_CELL;
+    const int x0 = (int)fmax(0.0, fmin(nx - 1.0, floor((m[0] - hx) * inv)));
+    const int x1 = (int)fmax(0.0, fmin(nx - 1.0, floor((m[0] + hx) * inv)));
+    const int y0 = (int)fmax(0.0, fmin(ny - 1.0, floor((m[1] - hy) * inv)));
+    const int y1 = (int)fmax(0.0, fmin(ny - 1.0, floor((m[1] + hy) * inv)));
+#pragma unroll 1
+    for (int cy = y0; cy <= y1; ++cy) {
+      const int row = c0 + cy * nx;
+      const int i1 = start[row + x1 + 1];
+#pragma unroll 1
+      for (int i = start[row + x0]; i < i1; ++i) {
+        const int f = sorted[i];
+        const double* ff = feats + (size_t)ASSOC_FEAT * f;
+        const double A[3] = {S[0] + ff[2], S[1] + ff[3], S[2] + ff[4]};
+        const double d2 = assoc_d2(A, ff[0] - m[0], ff[1] - m[1]);
+        if (!(d2 < gate)) continue;
+        if (d2 < best || (d2 == best && f < fs)) {
+          second = best;
+          best = d2;
+          fs = f;
+        } else if (d2 < second) {
+          second = d2;
+        }
+      }
+    }
+    if (fs < 0) status = 3;
+    else if (owned[fs]) status = 4;
+    else if (track_gate < INFINITY) {
+#pragma unroll 1
+      for (int k = trkOff[fs]; status == 0 && k < trkOff[fs + 1]; ++k) {
+        double mk[2], Sk[3];
+        const double zk = assoc_predict(cams + trkCam[k], X, PX, pixel_var, mk, Sk);
+        const double d2k = assoc_d2(Sk, trkM[2 * (size_t)k] - mk[0], trkM[2 * (size_t)k + 1] - mk[1]);
+        if (!(zk > 0) || !(d2k < track_gate)) status = 5;
+      }
+    }
+    if (status == 0) atomicMin(key + fs, (unsigned long long)__double_as_longlong(best));
+  }
+  r[0] = status;
+  r[1] = fs;
+  r[2] = status == 1 || status == 2 || status == 7 ? NAN : best;
+  r[3] = status == 1 || status == 2 || status == 7 ? NAN : second;
+  const bool pred = status != 1 && status != 7;
+  r[4] = pred ? m[0] : NAN;
+  r[5] = pred ? m[1] : NAN;
+  r[6] = pred ? S[0] : NAN;
+  r[7] = pred ? S[1] : NAN;
+  r[8] = pred ? S[2] : NAN;
+}
+
+// Pass two of the claim resolution: among the claimants of f* whose d2 is key[f*], win[f*] = the least point index.
+__global__ void __launch_bounds__(ASSOC_BIN_THREADS)
+assoc_claim_kernel(const int* __restrict__ qPt, int nQ, const unsigned long long* __restrict__ key,
+                   unsigned int* __restrict__ win, const double* __restrict__ out) {
+  const int q = blockIdx.x * ASSOC_BIN_THREADS + threadIdx.x;
+  if (q >= nQ) return;
+  const double* r = out + (size_t)ASSOC_OUT * q;
+  if (r[0] != 0) return;
+  const int f = (int)r[1];
+  if ((unsigned long long)__double_as_longlong(r[2]) == key[f]) atomicMin(win + f, (unsigned int)qPt[q]);
+}
+
+// The claimants that lost their feature get status 6.
+__global__ void __launch_bounds__(ASSOC_BIN_THREADS)
+assoc_final_kernel(const int* __restrict__ qPt, int nQ, const unsigned long long* __restrict__ key,
+                   const unsigned int* __restrict__ win, double* __restrict__ out) {
+  const int q = blockIdx.x * ASSOC_BIN_THREADS + threadIdx.x;
+  if (q >= nQ) return;
+  double* r = out + (size_t)ASSOC_OUT * q;
+  if (r[0] != 0) return;
+  const int f = (int)r[1];
+  if ((unsigned long long)__double_as_longlong(r[2]) != key[f] || win[f] != (unsigned int)qPt[q]) r[0] = 6;
+}
+
 
 // Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
 // cameras.
@@ -1823,6 +2051,26 @@ int alloc_tri_solver(cosl_tri_solver* s) {
   return COSL_OK;
 }
 
+// Checks a camera table of the triangulation and registration handles: K, R and t finite, R a rotation and camCov[c]
+// (nullable, as camCov[c]) symmetric and positive definite, the rules of a pose prior (R, t, P), naming the first bad
+// camera.
+int check_cam_table(const char* fn, int nCams, const double* K9, const double* R, const double* t,
+                    const double* const* camCov) {
+  for (int c = 0; c < nCams; ++c) {
+    for (int k = 0; k < 9; ++k)
+      if (!std::isfinite(K9[9 * c + k]) || !std::isfinite(R[9 * c + k]) || (k < 3 && !std::isfinite(t[3 * c + k])))
+        return set_error(COSL_E_INVALID, "%s: K, R or t of camera %d is not finite", fn, c);
+    // R a rotation and camCov symmetric and positive definite: the rules of a pose prior (R, t, P)
+    double rec[48] = {};
+    std::memcpy(rec, R + 9 * c, sizeof(double) * 9);
+    std::memcpy(rec + 9, t + 3 * c, sizeof(double) * 3);
+    if (camCov && camCov[c]) std::memcpy(rec + 12, camCov[c], sizeof(double) * 36);
+    else for (int k = 0; k < 6; ++k) rec[12 + 7 * k] = 1.0;
+    COSL_TRY(prior_factor(fn, c, rec, nullptr));
+  }
+  return COSL_OK;
+}
+
 // Checks one submit on the calling thread, naming the first bad camera, point or view.
 int check_tri(const char* fn, cosl_tri_solver* s, int nCams, const double* K9, const double* R, const double* t,
               const double* const* camCov, int nPts, const int* viewOff, const int* viewCam, const double* m,
@@ -1837,18 +2085,7 @@ int check_tri(const char* fn, cosl_tri_solver* s, int nCams, const double* K9, c
   if (!std::isfinite(pixel_var) || !(pixel_var > 0))
     return set_error(COSL_E_INVALID, "%s: pixel_var %g is not a finite value > 0", fn, pixel_var);
   if (!(max_err > 0)) return set_error(COSL_E_INVALID, "%s: max_err %g is not > 0", fn, max_err);
-  for (int c = 0; c < nCams; ++c) {
-    for (int k = 0; k < 9; ++k)
-      if (!std::isfinite(K9[9 * c + k]) || !std::isfinite(R[9 * c + k]) || (k < 3 && !std::isfinite(t[3 * c + k])))
-        return set_error(COSL_E_INVALID, "%s: K, R or t of camera %d is not finite", fn, c);
-    // R a rotation and camCov symmetric and positive definite: the rules of a pose prior (R, t, P)
-    double rec[48] = {};
-    std::memcpy(rec, R + 9 * c, sizeof(double) * 9);
-    std::memcpy(rec + 9, t + 3 * c, sizeof(double) * 3);
-    if (camCov && camCov[c]) std::memcpy(rec + 12, camCov[c], sizeof(double) * 36);
-    else for (int k = 0; k < 6; ++k) rec[12 + 7 * k] = 1.0;
-    COSL_TRY(prior_factor(fn, c, rec, nullptr));
-  }
+  COSL_TRY(check_cam_table(fn, nCams, K9, R, t, camCov));
   if (viewOff[0] != 0) return set_error(COSL_E_INVALID, "%s: viewOff[0] = %d is not 0", fn, viewOff[0]);
   for (int c = 0; c < nCams; ++c) s->seen[c] = -1;
   for (int j = 0; j < nPts; ++j) {
@@ -1927,6 +2164,281 @@ int stage_tri(cosl_tri_solver* s, int nCams, const double* K9, const double* R, 
       COSL_CUDA(cudaGetLastError());
       COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * TRI_OUT * nPts, cudaMemcpyDeviceToHost, st));
     }
+    return COSL_OK;
+  });
+}
+
+}  // namespace
+
+// A registration handle (cosl_assoc_solver).  The inputs of one submit travel in one copy from a pinned staging buffer
+// laid out as AssocCam[nCams] | pts[nPts][ASSOC_PT] | feats[nFeats][ASSOC_FEAT] | trkM[nTrk][2] | featOff[nCams + 1] |
+// cell[nFeats] | owned[nFeats] | trkOff[nFeats + 1] | trkCam[nTrk] | qPt[nQ] | qCam[nQ]; ASSOC_OUT doubles per query
+// pair come back into pinned memory.  The grid (count and start per cell, the features sorted by cell) and the claim
+// keys live on the device only.  Everything is allocated by create for at most maxCams camera entries, maxPts points,
+// maxQueries query pairs, maxFeats features and maxTrackObs track observations per submit.
+struct cosl_assoc_solver {
+  int device = 0, maxCams = 0, maxPts = 0, maxQueries = 0, maxFeats = 0, maxTrackObs = 0;
+  RequestStream rq;
+  unsigned char* h_in = nullptr;
+  unsigned char* d_in = nullptr;
+  int* d_count = nullptr;   // [maxCams * ASSOC_MAX_CELLS]
+  int* d_start = nullptr;   // [maxCams * ASSOC_MAX_CELLS + 1]
+  int* d_sorted = nullptr;  // [maxFeats]
+  unsigned long long* d_key = nullptr;  // [maxFeats]: pass one of the claims, the least d2 bits per feature
+  unsigned int* d_win = nullptr;        // [maxFeats]: pass two, the least point index among those holding it
+  double* d_out = nullptr;
+  double* h_out = nullptr;
+  int* seen = nullptr;  // [maxCams]: the last point that queried each camera entry, for the repeated-entry check
+  int nQ = 0;           // query pairs of the submit in flight or last collected
+};
+
+namespace {
+
+size_t assoc_bytes(int nCams, int nPts, int nFeats, int nTrk, int nQ) {
+  return sizeof(AssocCam) * nCams +
+         sizeof(double) * ((size_t)ASSOC_PT * nPts + (size_t)ASSOC_FEAT * nFeats + 2 * (size_t)nTrk) +
+         sizeof(int) * ((size_t)nCams + 1 + 3 * (size_t)nFeats + 1 + nTrk + 2 * (size_t)nQ);
+}
+
+void free_assoc_solver(cosl_assoc_solver* s) {
+  cudaSetDevice(s->device);
+  s->rq.destroy();
+  if (s->h_in) cudaFreeHost(s->h_in);
+  if (s->h_out) cudaFreeHost(s->h_out);
+  cudaFree(s->d_in);
+  cudaFree(s->d_count);
+  cudaFree(s->d_start);
+  cudaFree(s->d_sorted);
+  cudaFree(s->d_key);
+  cudaFree(s->d_win);
+  cudaFree(s->d_out);
+  delete[] s->seen;
+  delete s;
+}
+
+int alloc_assoc_solver(cosl_assoc_solver* s) {
+  s->seen = new (std::nothrow) int[s->maxCams];
+  if (!s->seen) return set_error(COSL_E_NOMEM, "cosl_assoc_solver_create: out of host memory");
+  COSL_CUDA(cudaSetDevice(s->device));
+  COSL_TRY(s->rq.create());
+  const size_t in = assoc_bytes(s->maxCams, s->maxPts, s->maxFeats, s->maxTrackObs, s->maxQueries);
+  const size_t outb = sizeof(double) * ASSOC_OUT * s->maxQueries;
+  const size_t cells = (size_t)s->maxCams * ASSOC_MAX_CELLS;
+  COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
+  COSL_CUDA(cudaHostAlloc(&s->h_out, outb, cudaHostAllocPortable));
+  COSL_CUDA(cudaMalloc(&s->d_in, in));
+  COSL_CUDA(cudaMalloc(&s->d_count, sizeof(int) * cells));
+  COSL_CUDA(cudaMalloc(&s->d_start, sizeof(int) * (cells + 1)));
+  COSL_CUDA(cudaMalloc(&s->d_sorted, sizeof(int) * s->maxFeats));
+  COSL_CUDA(cudaMalloc(&s->d_key, sizeof(unsigned long long) * s->maxFeats));
+  COSL_CUDA(cudaMalloc(&s->d_win, sizeof(unsigned int) * s->maxFeats));
+  COSL_CUDA(cudaMalloc(&s->d_out, outb));
+  return COSL_OK;
+}
+
+// The arguments of one cosl_assoc_solver_submit
+struct AssocArgs {
+  int nCams;
+  const double *K9, *R, *t;
+  const double* const* camCov;
+  const int* wh;
+  const int* featOff;
+  const double *mf, *covf;
+  const int* owned;
+  const int *trkOff, *trkCam;
+  const double* trkM;
+  int nPts;
+  const double *X, *PX;
+  const int *qOff, *qCam;
+  double pixel_var, gate, track_gate;
+};
+
+// Checks one submit on the calling thread, naming the first bad camera, feature, track observation, point or query.
+int check_assoc(const char* fn, cosl_assoc_solver* s, const AssocArgs& a) {
+  const int nCams = a.nCams, nPts = a.nPts;
+  if (nCams < 0 || nPts < 0) return set_error(COSL_E_INVALID, "%s: nCams %d or nPts %d < 0", fn, nCams, nPts);
+  if (nCams > s->maxCams)
+    return set_error(COSL_E_INVALID, "%s: %d cameras exceed the handle's %d", fn, nCams, s->maxCams);
+  if (nPts > s->maxPts)
+    return set_error(COSL_E_INVALID, "%s: %d points exceed the handle's %d", fn, nPts, s->maxPts);
+  if (!a.featOff || !a.qOff || (nCams > 0 && (!a.K9 || !a.R || !a.t || !a.wh)) || (nPts > 0 && (!a.X || !a.PX)))
+    return set_error(COSL_E_INVALID, "%s: null argument", fn);
+  if (!std::isfinite(a.pixel_var) || !(a.pixel_var > 0))
+    return set_error(COSL_E_INVALID, "%s: pixel_var %g is not a finite value > 0", fn, a.pixel_var);
+  if (!(a.gate > 0)) return set_error(COSL_E_INVALID, "%s: gate %g is not > 0", fn, a.gate);
+  if (!(a.track_gate > 0)) return set_error(COSL_E_INVALID, "%s: track_gate %g is not > 0", fn, a.track_gate);
+  COSL_TRY(check_cam_table(fn, nCams, a.K9, a.R, a.t, a.camCov));
+  for (int c = 0; c < nCams; ++c)
+    if (a.wh[2 * c] < 1 || a.wh[2 * c] > ASSOC_MAX_SIDE || a.wh[2 * c + 1] < 1 || a.wh[2 * c + 1] > ASSOC_MAX_SIDE)
+      return set_error(COSL_E_INVALID, "%s: image size %d x %d of camera %d is not in [1, %d]", fn, a.wh[2 * c],
+                       a.wh[2 * c + 1], c, ASSOC_MAX_SIDE);
+  if (a.featOff[0] != 0) return set_error(COSL_E_INVALID, "%s: featOff[0] = %d is not 0", fn, a.featOff[0]);
+  for (int c = 0; c < nCams; ++c)
+    if (a.featOff[c + 1] < a.featOff[c])
+      return set_error(COSL_E_INVALID, "%s: camera %d has %d features", fn, c, a.featOff[c + 1] - a.featOff[c]);
+  const int nF = a.featOff[nCams];
+  if (nF > s->maxFeats)
+    return set_error(COSL_E_INVALID, "%s: %d features exceed the handle's %d", fn, nF, s->maxFeats);
+  if (nF > 0 && !a.mf) return set_error(COSL_E_INVALID, "%s: null argument", fn);
+  if (a.trkOff) {
+    if (a.trkOff[0] != 0) return set_error(COSL_E_INVALID, "%s: trkOff[0] = %d is not 0", fn, a.trkOff[0]);
+    for (int f = 0; f < nF; ++f)
+      if (a.trkOff[f + 1] < a.trkOff[f])
+        return set_error(COSL_E_INVALID, "%s: feature %d has %d track observations", fn, f,
+                         a.trkOff[f + 1] - a.trkOff[f]);
+    if (a.trkOff[nF] > s->maxTrackObs)
+      return set_error(COSL_E_INVALID, "%s: %d track observations exceed the handle's %d", fn, a.trkOff[nF],
+                       s->maxTrackObs);
+    if (a.trkOff[nF] > 0 && (!a.trkCam || !a.trkM)) return set_error(COSL_E_INVALID, "%s: null argument", fn);
+  }
+  for (int f = 0; f < nF; ++f) {
+    if (!std::isfinite(a.mf[2 * (size_t)f]) || !std::isfinite(a.mf[2 * (size_t)f + 1]))
+      return set_error(COSL_E_INVALID, "%s: feature %d: m is not finite", fn, f);
+    double L[3];
+    if (a.covf && !cov_factor(a.covf + 4 * (size_t)f, L))
+      return set_error(COSL_E_INVALID, "%s: feature %d: covf is not finite, symmetric and positive definite", fn, f);
+    if (a.owned && a.owned[f] != 0 && a.owned[f] != 1)
+      return set_error(COSL_E_INVALID, "%s: feature %d: owned %d is not 0 or 1", fn, f, a.owned[f]);
+    for (int k = a.trkOff ? a.trkOff[f] : 0; a.trkOff && k < a.trkOff[f + 1]; ++k) {
+      const int c = a.trkCam[k];
+      if (c < 0 || c >= nCams)
+        return set_error(COSL_E_INVALID, "%s: track observation %d of feature %d: camera %d is not in [0, %d)", fn,
+                         k, f, c, nCams);
+      if (!std::isfinite(a.trkM[2 * (size_t)k]) || !std::isfinite(a.trkM[2 * (size_t)k + 1]))
+        return set_error(COSL_E_INVALID, "%s: track observation %d of feature %d: m is not finite", fn, k, f);
+    }
+  }
+  for (int j = 0; j < nPts; ++j) {
+    const double* X = a.X + 3 * (size_t)j;
+    if (!std::isfinite(X[0]) || !std::isfinite(X[1]) || !std::isfinite(X[2]))
+      return set_error(COSL_E_INVALID, "%s: point %d: X is not finite", fn, j);
+    double S[6];
+    if (!point_cov(a.PX + 9 * (size_t)j, S))
+      return set_error(COSL_E_INVALID, "%s: point %d: P is not finite, symmetric and positive definite", fn, j);
+  }
+  if (a.qOff[0] != 0) return set_error(COSL_E_INVALID, "%s: qOff[0] = %d is not 0", fn, a.qOff[0]);
+  for (int c = 0; c < nCams; ++c) s->seen[c] = -1;
+  for (int j = 0; j < nPts; ++j) {
+    const int n = a.qOff[j + 1] - a.qOff[j];
+    if (a.qOff[j + 1] < a.qOff[j] || n > ASSOC_MAX_QUERIES)
+      return set_error(COSL_E_INVALID, "%s: point %d has %d queries, not 0 to %d", fn, j, n, ASSOC_MAX_QUERIES);
+    if (a.qOff[j + 1] > s->maxQueries)
+      return set_error(COSL_E_INVALID, "%s: point %d: %d queries exceed the handle's %d", fn, j, a.qOff[j + 1],
+                       s->maxQueries);
+    if (n > 0 && !a.qCam) return set_error(COSL_E_INVALID, "%s: null argument", fn);
+    for (int q = a.qOff[j]; q < a.qOff[j + 1]; ++q) {
+      const int c = a.qCam[q];
+      if (c < 0 || c >= nCams)
+        return set_error(COSL_E_INVALID, "%s: query %d of point %d: camera %d is not in [0, %d)", fn, q, j, c, nCams);
+      if (s->seen[c] == j)
+        return set_error(COSL_E_INVALID, "%s: query %d of point %d: camera %d is queried twice", fn, q, j, c);
+      s->seen[c] = j;
+    }
+  }
+  return COSL_OK;
+}
+
+// Stages a checked submit and enqueues the copy, the binning, the search, the claims and the read-back.
+int stage_assoc(cosl_assoc_solver* s, const AssocArgs& a) {
+  const int nCams = a.nCams, nPts = a.nPts, nF = a.featOff[nCams];
+  const int nTrk = a.trkOff ? a.trkOff[nF] : 0, nQ = a.qOff[nPts];
+  AssocCam* hc = reinterpret_cast<AssocCam*>(s->h_in);
+  double* hp = reinterpret_cast<double*>(hc + nCams);
+  double* hf = hp + (size_t)ASSOC_PT * nPts;
+  double* hm = hf + (size_t)ASSOC_FEAT * nF;
+  int* hoff = reinterpret_cast<int*>(hm + 2 * (size_t)nTrk);
+  int* hcell = hoff + nCams + 1;
+  int* hown = hcell + nF;
+  int* htoff = hown + nF;
+  int* htcam = htoff + nF + 1;
+  int* hqpt = htcam + nTrk;
+  int* hqcam = hqpt + nQ;
+  int cells = 0;
+  for (int c = 0; c < nCams; ++c) {
+    AssocCam& e = hc[c];
+    std::memcpy(e.K, a.K9 + 9 * c, sizeof(double) * 9);
+    std::memcpy(e.R, a.R + 9 * c, sizeof(double) * 9);
+    std::memcpy(e.t, a.t + 3 * c, sizeof(double) * 3);
+    e.hasP = a.camCov && a.camCov[c] ? 1 : 0;
+    if (e.hasP)  // symmetrised, as prior_factor checked it
+      for (int i = 0; i < 6; ++i)
+        for (int k = 0; k < 6; ++k) e.P[6 * i + k] = 0.5 * (a.camCov[c][6 * i + k] + a.camCov[c][6 * k + i]);
+    e.W = a.wh[2 * c];
+    e.H = a.wh[2 * c + 1];
+    e.nx = (a.wh[2 * c] + ASSOC_CELL - 1) / ASSOC_CELL;
+    e.ny = (a.wh[2 * c + 1] + ASSOC_CELL - 1) / ASSOC_CELL;
+    e.cell0 = cells;
+    cells += e.nx * e.ny;
+    // the features: m_f, Sigma_f (pixel_var I without covf), the cell and lam = the largest lambda_max(Sigma_f)
+    double lam = 0.0;
+    for (int f = a.featOff[c]; f < a.featOff[c + 1]; ++f) {
+      double* q = hf + (size_t)ASSOC_FEAT * f;
+      const double* cv = a.covf ? a.covf + 4 * (size_t)f : nullptr;
+      q[0] = a.mf[2 * (size_t)f];
+      q[1] = a.mf[2 * (size_t)f + 1];
+      q[2] = cv ? cv[0] : a.pixel_var;
+      q[3] = cv ? cv[1] : 0.0;
+      q[4] = cv ? cv[3] : a.pixel_var;
+      const double h = 0.5 * (q[2] - q[4]);
+      lam = std::max(lam, 0.5 * (q[2] + q[4]) + std::sqrt(h * h + q[3] * q[3]));
+      const double cx = std::max(0.0, std::min(e.nx - 1.0, std::floor(q[0] / ASSOC_CELL)));
+      const double cy = std::max(0.0, std::min(e.ny - 1.0, std::floor(q[1] / ASSOC_CELL)));
+      hcell[f] = e.cell0 + (int)cy * e.nx + (int)cx;
+    }
+    e.lam = lam;
+  }
+  for (int j = 0; j < nPts; ++j) {
+    double* p = hp + (size_t)ASSOC_PT * j;
+    std::memcpy(p, a.X + 3 * (size_t)j, sizeof(double) * 3);
+    point_cov(a.PX + 9 * (size_t)j, p + 3);  // symmetrised, as check_assoc accepted it
+    for (int q = a.qOff[j]; q < a.qOff[j + 1]; ++q) hqpt[q] = j;
+  }
+  if (nTrk) std::memcpy(hm, a.trkM, sizeof(double) * 2 * (size_t)nTrk);
+  std::memcpy(hoff, a.featOff, sizeof(int) * ((size_t)nCams + 1));
+  for (int f = 0; f < nF; ++f) hown[f] = a.owned ? a.owned[f] : 0;
+  if (a.trkOff) std::memcpy(htoff, a.trkOff, sizeof(int) * ((size_t)nF + 1));
+  else std::fill(htoff, htoff + nF + 1, 0);
+  if (nTrk) std::memcpy(htcam, a.trkCam, sizeof(int) * (size_t)nTrk);
+  if (nQ) std::memcpy(hqcam, a.qCam, sizeof(int) * (size_t)nQ);
+  s->nQ = nQ;
+  cudaStream_t st = s->rq.stream;
+  const double pv = a.pixel_var, gate = a.gate, tg = a.track_gate;
+  return s->rq.submit("cosl_assoc_solver_submit", [&]() -> int {
+    COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, assoc_bytes(nCams, nPts, nF, nTrk, nQ), cudaMemcpyHostToDevice, st));
+    if (nQ == 0) return COSL_OK;
+    const AssocCam* d_cams = reinterpret_cast<const AssocCam*>(s->d_in);
+    const double* d_pts = reinterpret_cast<const double*>(d_cams + nCams);
+    const double* d_feats = d_pts + (size_t)ASSOC_PT * nPts;
+    const double* d_trkM = d_feats + (size_t)ASSOC_FEAT * nF;
+    const int* d_off = reinterpret_cast<const int*>(d_trkM + 2 * (size_t)nTrk);
+    const int* d_cell = d_off + nCams + 1;
+    const int* d_own = d_cell + nF;
+    const int* d_toff = d_own + nF;
+    const int* d_tcam = d_toff + nF + 1;
+    const int* d_qpt = d_tcam + nTrk;
+    const int* d_qcam = d_qpt + nQ;
+    // the grid: count, a per-entry exclusive scan, scatter
+    COSL_CUDA(cudaMemsetAsync(s->d_count, 0, sizeof(int) * (size_t)cells, st));
+    if (nF) COSL_LAUNCH(assoc_count_kernel, div_up(nF, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_cell, nF,
+                        s->d_count);
+    COSL_LAUNCH(assoc_scan_kernel, nCams, ASSOC_SCAN_THREADS, 0, st, d_cams, d_off, nCams, s->d_count, s->d_start);
+    if (nF) {
+      COSL_LAUNCH(assoc_scatter_kernel, div_up(nF, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_cell, nF,
+                  s->d_start, s->d_count, s->d_sorted);
+      COSL_CUDA(cudaMemsetAsync(s->d_key, 0xff, sizeof(unsigned long long) * (size_t)nF, st));
+      COSL_CUDA(cudaMemsetAsync(s->d_win, 0xff, sizeof(unsigned int) * (size_t)nF, st));
+    }
+    // the search with pass one of the claims, pass two, and the statuses
+    COSL_LAUNCH(assoc_search_kernel, div_up(nQ, ASSOC_THREADS), ASSOC_THREADS, 0, st, d_cams, d_pts, d_feats, d_own,
+                d_toff, d_tcam, d_trkM, d_qpt, d_qcam, nQ, s->d_start, s->d_sorted, pv, gate, tg, s->d_key,
+                s->d_out);
+    COSL_LAUNCH(assoc_claim_kernel, div_up(nQ, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_qpt, nQ, s->d_key,
+                s->d_win, s->d_out);
+    COSL_LAUNCH(assoc_final_kernel, div_up(nQ, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_qpt, nQ, s->d_key,
+                s->d_win, s->d_out);
+    COSL_CUDA(cudaGetLastError());
+    COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * ASSOC_OUT * (size_t)nQ, cudaMemcpyDeviceToHost,
+                              st));
     return COSL_OK;
   });
 }
@@ -2236,5 +2748,74 @@ int cosl_tri_solver_collect(cosl_tri_solver* s, double* X, double* P, double* st
 }
 
 void* cosl_tri_solver_stream(cosl_tri_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
+
+int cosl_assoc_solver_create(int device, int maxCams, int maxPts, int maxQueries, int maxFeats, int maxTrackObs,
+                             cosl_assoc_solver** out) {
+  if (!out || device < 0 || maxCams < 1 || maxPts < 1 || maxQueries < 1 || maxFeats < 1 || maxTrackObs < 0)
+    return set_error(COSL_E_INVALID, "cosl_assoc_solver_create: bad argument");
+  *out = nullptr;
+  COSL_TRY(check_device(device));
+  cosl_assoc_solver* s = new (std::nothrow) cosl_assoc_solver;
+  if (!s) return set_error(COSL_E_NOMEM, "cosl_assoc_solver_create: out of host memory");
+  s->device = device;
+  s->maxCams = maxCams;
+  s->maxPts = maxPts;
+  s->maxQueries = maxQueries;
+  s->maxFeats = maxFeats;
+  s->maxTrackObs = maxTrackObs;
+  const int rc = alloc_assoc_solver(s);
+  if (rc != COSL_OK) {
+    free_assoc_solver(s);
+    return rc;
+  }
+  *out = s;
+  return COSL_OK;
+}
+
+int cosl_assoc_solver_destroy(cosl_assoc_solver* s) {
+  if (!s) return set_error(COSL_E_INVALID, "null registration handle");
+  free_assoc_solver(s);
+  return COSL_OK;
+}
+
+int cosl_assoc_solver_submit(cosl_assoc_solver* s, int nCams, const double* K9, const double* R, const double* t,
+                             const double* const* camCov, const int* wh, const int* featOff, const double* mf,
+                             const double* covf, const int* owned, const int* trkOff, const int* trkCam,
+                             const double* trkM, int nPts, const double* X, const double* PX, const int* qOff,
+                             const int* qCam, double pixel_var, double gate, double track_gate) {
+  const char* fn = "cosl_assoc_solver_submit";
+  if (!s) return set_error(COSL_E_INVALID, "null registration handle");
+  COSL_TRY(s->rq.idle(fn));
+  const AssocArgs a{nCams, K9, R, t, camCov, wh, featOff, mf, covf, owned, trkOff, trkCam, trkM, nPts, X, PX, qOff,
+                    qCam, pixel_var, gate, track_gate};
+  COSL_TRY(check_assoc(fn, s, a));
+  COSL_CUDA(cudaSetDevice(s->device));
+  return stage_assoc(s, a);
+}
+
+int cosl_assoc_solver_query(cosl_assoc_solver* s, int* done) {
+  if (!s || !done) return set_error(COSL_E_INVALID, "cosl_assoc_solver_query: null argument");
+  COSL_TRY(s->rq.pending("cosl_assoc_solver_query"));
+  COSL_CUDA(cudaSetDevice(s->device));
+  return s->rq.query(done);
+}
+
+int cosl_assoc_solver_collect(cosl_assoc_solver* s, int* status, int* feat, double* d2, double* pred,
+                              double* device_ms) {
+  if (!s) return set_error(COSL_E_INVALID, "null registration handle");
+  COSL_TRY(s->rq.pending("cosl_assoc_solver_collect"));
+  COSL_CUDA(cudaSetDevice(s->device));
+  COSL_TRY(s->rq.wait(device_ms));
+  for (int q = 0; q < s->nQ; ++q) {
+    const double* r = s->h_out + (size_t)ASSOC_OUT * q;
+    if (status) status[q] = (int)r[0];
+    if (feat) feat[q] = (int)r[1];
+    if (d2) std::memcpy(d2 + 2 * (size_t)q, r + 2, sizeof(double) * 2);
+    if (pred) std::memcpy(pred + 5 * (size_t)q, r + 4, sizeof(double) * 5);
+  }
+  return COSL_OK;
+}
+
+void* cosl_assoc_solver_stream(cosl_assoc_solver* s) { return s ? (void*)s->rq.stream : nullptr; }
 
 }  // extern "C"

@@ -588,6 +588,71 @@ int cosl_tri_solver_collect(cosl_tri_solver* s, double* X, double* P, double* st
  * runs after that request. */
 void* cosl_tri_solver_stream(cosl_tri_solver* s);
 
+/* A registration handle: batched Mahalanobis nearest-feature search of map points in the current frame's
+ * features (an extension: the geometric half of CoSLAM::activeMapPointRegisterInGroup and
+ * curStaticPointRegInGroup, whose getProjectionCovMat is not in this tree; DESIGN.md 5.6).  A handle owns a
+ * non-blocking stream, a pinned staging buffer, device buffers (the feature grid and the claim keys among
+ * them) and a pinned result buffer, all allocated by create for at most maxCams camera entries, maxPts
+ * points, maxQueries query pairs, maxFeats features and maxTrackObs track observations (all points or
+ * features together) per submit; no submit allocates.  Without a usable device create gives COSL_E_CUDA;
+ * there is no CPU path.  COSL_E_INVALID for maxCams, maxPts, maxQueries or maxFeats < 1 or maxTrackObs < 0.
+ *
+ * submit: a camera table of nCams entries as cosl_tri_solver_submit's (K9, R, t, camCov in the pose solver's
+ * chart, nullable as camCov[c]) with wh[2 nCams], each entry's image width and height in px (1 to 4096).
+ * Features in CSR form over the entries: entry c has the features [featOff[c], featOff[c + 1]),
+ * featOff[0] = 0; feature f has an undistorted position mf[2 f] (px), covf[4 f] (nullable), its row-major
+ * 2x2 covariance Sigma_f in px^2 (pixel_var I without covf), owned[f] (nullable; 0 or 1, 1 when a map point
+ * already holds it) and the earlier observations of its track (trkOff nullable: none), [trkOff[f],
+ * trkOff[f + 1]), each with a camera entry trkCam[k] and a position trkM[2 k] (px, noise pixel_var I).  nPts
+ * points, X[3 j] and PX[9 j] (row-major 3x3, symmetric and positive definite), each with the query entries
+ * [qOff[j], qOff[j + 1]) of qCam, at most 32 and each entry at most once per point.  Per query pair (j, c),
+ * in fp64, with pi the pose solver's projection, H_X = (a; b) R its Jacobian in X and H_c the covariance
+ * stage's 2x6 one:
+ *   1. m_hat = pi_c(X_j), S = H_X P_X H_X^T + H_c P_c H_c^T (the second term with the entry's camCov only);
+ *   2. d2_f = |L^-1 (m_f - m_hat)|^2 with L L^T = S + Sigma_f over the features of entry c; f* the least
+ *      (d2, f) with d2 < gate (+inf allowed: the plain nearest feature), d2_2 the second least such d2;
+ *   3. with a finite track_gate, every earlier observation k of f* must have depth > 0 and
+ *      d2_k = nu_k^T (H_X P_X H_X^T + H_c P_c H_c^T + pixel_var I)^-1 nu_k < track_gate at its entry;
+ *   4. several pairs that hold one feature: the least (d2, point index) keeps it.
+ * status, in this order: 7 a non-finite depth, m_hat or S; 1 depth <= 0; 2 m_hat outside [0, W) x [0, H);
+ * 3 no feature inside the gate; 4 f* owned; 5 the track check failed; 6 another pair kept f*; else 0,
+ * registered.  The result does not depend on the order of points or queries.
+ * submit checks everything on the calling thread before anything is staged, and gives COSL_E_INVALID
+ * naming the first bad camera, feature, track observation, point or query (the handle stays usable) for:
+ * counts above the reserved sizes; a NULL required array; tri's camera-table rules, with its messages; an
+ * image size outside [1, 4096]; a featOff, trkOff or qOff that does not start at 0 or is not monotone; a
+ * non-finite mf or trkM; a covf failing submit_cov's rules; an owned other than 0 or 1; a track or query
+ * camera out of range; an entry queried twice by one point or more than 32 queries; a non-finite X or a P
+ * failing the BA point prior's rules; a pixel_var that is not finite and > 0; a gate or track_gate that is
+ * not > 0.  It packs the inputs into pinned memory, so the caller may reuse its arrays when it returns,
+ * enqueues one host-to-device copy, the binning, search and claim kernels and one device-to-host copy on
+ * the handle's stream, and returns without waiting for the device.
+ *
+ * query sets *done = 1 once the request has finished, without waiting.  collect waits for it and writes,
+ * per query pair in submit order, status[Q], feat[Q] (the global feature index f*, -1 for status 1, 2, 3
+ * and 7), d2[2 Q] (d2 of f* and d2_2; NaN for 1, 2 and 7, +inf without a feature in the gate) and pred[5 Q]
+ * (m_hat and S as xx, xy, yy; NaN for 1 and 7), every output nullable; *device_ms (nullable) is the device
+ * time of the copies and the kernels, from CUDA events.  One request may be in flight per handle: a second
+ * submit gives COSL_E_STATE, and so do query and collect with nothing in flight.  destroy waits for a
+ * request in flight.  A handle is not re-entrant; different handles share no lock.  Every call makes the
+ * handle's device current on the calling thread. */
+typedef struct cosl_assoc_solver cosl_assoc_solver;
+int cosl_assoc_solver_create(int device, int maxCams, int maxPts, int maxQueries, int maxFeats,
+                             int maxTrackObs, cosl_assoc_solver** out);
+int cosl_assoc_solver_destroy(cosl_assoc_solver* s);
+int cosl_assoc_solver_submit(cosl_assoc_solver* s, int nCams, const double* K9, const double* R,
+                             const double* t, const double* const* camCov, const int* wh,
+                             const int* featOff, const double* mf, const double* covf, const int* owned,
+                             const int* trkOff, const int* trkCam, const double* trkM, int nPts,
+                             const double* X, const double* PX, const int* qOff, const int* qCam,
+                             double pixel_var, double gate, double track_gate);
+int cosl_assoc_solver_query(cosl_assoc_solver* s, int* done);
+int cosl_assoc_solver_collect(cosl_assoc_solver* s, int* status, int* feat, double* d2, double* pred,
+                              double* device_ms);
+/* CUDA stream (cudaStream_t as void*) the handle's requests run on; work enqueued there after a submit
+ * runs after that request. */
+void* cosl_assoc_solver_stream(cosl_assoc_solver* s);
+
 /* ================================================================ bundle adjustment */
 
 /* Flat form of the arguments of
