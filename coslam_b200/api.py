@@ -45,6 +45,8 @@ def _load():
     for f in (L.cosl_klt_set_margin, L.cosl_klt_set_conv, L.cosl_klt_set_ssd, L.cosl_klt_set_covariance):
         f.argtypes = [vp, cf]
     L.cosl_klt_group_download_covariance.argtypes = [vp, vp]
+    L.cosl_klt_set_undistortion.argtypes = [vp, vp, vp]
+    L.cosl_klt_group_download_undistorted.argtypes = [vp, vp, vp]
     L.cosl_klt_group_next.argtypes = [vp, vp, C.c_size_t, vp, vp]
     L.cosl_klt_group_first.argtypes = [vp, vp, C.c_size_t, vp, vp]
     L.cosl_klt_group_first_present.argtypes = [vp, vp, C.c_size_t, vp, vp, vp, vp]
@@ -527,6 +529,31 @@ class KltGroup:
         ptrs = (C.c_void_p * self.C)(*[out[c].ctypes.data for c in range(self.C)])
         _ck(LIB.cosl_klt_group_download_covariance(self.h, ptrs))
         return out
+
+    def set_undistortion(self, K, kc):
+        """cosl_klt_set_undistortion: arm the undistorted position (and, with set_covariance, covariance) of
+        every slot for the frames enqueued from now on.  K: [C, 3, 3] camera matrices, kc: [C, 5] Bouguet
+        distortion vectors (k1, k2, p1, p2, k3); K None disarms."""
+        if K is None:
+            _ck(LIB.cosl_klt_set_undistortion(self.h, None, None))
+            return
+        K = np.ascontiguousarray(K, np.float64)
+        kc = np.ascontiguousarray(kc, np.float64)
+        assert K.shape == (self.C, 3, 3) and kc.shape == (self.C, 5)
+        _ck(LIB.cosl_klt_set_undistortion(self.h, _ptr(K), _ptr(kc)))
+
+    def download_undistorted(self):
+        """cosl_klt_group_download_undistorted of the last frame handed out: (pos [C, F, 2] float64 undistorted
+        pixels, cov [C, F, 3] float32 (xx, xy, yy) in undistorted pixels^2, or None when that frame had no
+        position covariances); NaN where a slot has none."""
+        pos = np.empty((self.C, self.F, 2), np.float64)
+        cov = np.empty((self.C, self.F, 3), np.float32)
+        pp = (C.c_void_p * self.C)(*[pos[c].ctypes.data for c in range(self.C)])
+        cp = (C.c_void_p * self.C)(*[cov[c].ctypes.data for c in range(self.C)])
+        if LIB.cosl_klt_group_download_undistorted(self.h, pp, cp) == 0:
+            return pos, cov
+        _ck(LIB.cosl_klt_group_download_undistorted(self.h, pp, None))  # armed without covariances?
+        return pos, None
 
     def pyramid(self, cam, which, level):
         w, h = self.sizes[cam][0] >> level, self.sizes[cam][1] >> level

@@ -14,6 +14,7 @@
 #include "klt_front.cuh"
 #include "klt_pyr_tma.cuh"
 #include "klt_cov.cuh"
+#include "klt_undist.cuh"
 
 using namespace coslam;
 
@@ -173,6 +174,24 @@ struct cosl_klt {
   float* h_cov = nullptr;
   float* h_covQ[2] = {nullptr, nullptr};
   std::vector<float> covOut;
+  // undistorted positions and covariances of every slot (cosl_klt_set_undistortion, klt_undist.cuh).
+  // undArmed false: disarmed, nothing below is allocated or launched.  d_undCams holds the lenses, written
+  // on `stream` by the set call; d_undPos [C][F][2] / d_undCov [C][F][3] hold the last frame run_frame
+  // computed them for (undFrame; the covariances only when that frame also had covFrame).  They are read
+  // back with the feature table as the covariances are (h_und*, h_und*Q[slot], undQ[slot]), and copy_out
+  // hands the addressed cameras' entries to undPosOut / undCovOut, what
+  // cosl_klt_group_download_undistorted returns (undHanded, undCovHanded: of the last frame handed out)
+  bool undArmed = false, undFrame = false, undHanded = false, undCovHanded = false;
+  bool undQ[2] = {false, false};
+  KltUndistCam* d_undCams = nullptr;
+  double* d_undPos = nullptr;
+  float* d_undCov = nullptr;
+  double* h_undPos = nullptr;
+  float* h_undCov = nullptr;
+  double* h_undPosQ[2] = {nullptr, nullptr};
+  float* h_undCovQ[2] = {nullptr, nullptr};
+  std::vector<double> undPosOut;
+  std::vector<float> undCovOut;
   // persistent fused gain tracker (klt_gain_fused)
   float4* d_state = nullptr;             // [C*F]
   unsigned long long* d_ver = nullptr;   // [2][C*F] (pass << 32 | beta bits)
@@ -492,9 +511,16 @@ void free_group(cosl_klt* g) {
     if (g->h_cntQ[i]) cudaFreeHost(g->h_cntQ[i]);
     if (g->evDone[i]) cudaEventDestroy(g->evDone[i]);
     if (g->h_covQ[i]) cudaFreeHost(g->h_covQ[i]);
+    if (g->h_undPosQ[i]) cudaFreeHost(g->h_undPosQ[i]);
+    if (g->h_undCovQ[i]) cudaFreeHost(g->h_undCovQ[i]);
   }
   cudaFree(g->d_cov);
   if (g->h_cov) cudaFreeHost(g->h_cov);
+  cudaFree(g->d_undCams);
+  cudaFree(g->d_undPos);
+  cudaFree(g->d_undCov);
+  if (g->h_undPos) cudaFreeHost(g->h_undPos);
+  if (g->h_undCov) cudaFreeHost(g->h_undCov);
   if (g->stream) cudaStreamDestroy(g->stream);
   delete g;
 }
@@ -765,6 +791,16 @@ static int run_covariance(cosl_klt* g, const FramePlan& p) {
   return COSL_OK;
 }
 
+// The undistorted positions of an armed frame (klt_undist.cuh) into d_undPos and, when the frame's
+// covariances were computed, d_undCov.  It reads the final feature table, so it follows the table's last
+// writer: the refill of run_detector, or klt_status (the fused tracker) on a frame without a detector.
+static int run_undistortion(cosl_klt* g) {
+  COSL_LAUNCH(klt_undistort, dim3(div_up(g->F, 128), g->C), 128, 0, g->stream, g->d_feat,
+              g->covFrame ? g->d_cov : (const float*)nullptr, g->d_undCams, g->d_undPos, g->d_undCov, g->F);
+  COSL_CUDA(cudaGetLastError());
+  return COSL_OK;
+}
+
 // KLT_Detector::detectCorners + extractCorners (v3d_gpuklt.cpp:423-588) and the slot logic of
 // detect/redetect (:651-805) on the cornerness map klt_front produced for this frame.  p.detectMode
 // 0: detect (present = the external points of upload_present, p.maxPresent = the longest list),
@@ -804,6 +840,17 @@ int run_detector(cosl_klt* g, const FramePlan& p) {
   return COSL_OK;
 }
 
+// The read-back of the last frame's undistorted positions into pos and, when that frame had covariances,
+// of their covariances into cov, on `stream`; nothing when it was not armed (armed false).
+static int read_undistorted(cosl_klt* g, double* pos, float* cov, bool armed) {
+  if (!armed) return COSL_OK;
+  const size_t n = (size_t)g->F * g->C;
+  COSL_CUDA(cudaMemcpyAsync(pos, g->d_undPos, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, g->stream));
+  if (g->covFrame)
+    COSL_CUDA(cudaMemcpyAsync(cov, g->d_undCov, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, g->stream));
+  return COSL_OK;
+}
+
 int fetch_results(cosl_klt* g) {
   COSL_CUDA(cudaMemcpyAsync(g->h_feat, g->d_feat, sizeof(cosl_klt_feature) * (size_t)g->F * g->C,
                             cudaMemcpyDeviceToHost, g->stream));
@@ -812,6 +859,7 @@ int fetch_results(cosl_klt* g) {
   if (g->covFrame)
     COSL_CUDA(cudaMemcpyAsync(g->h_cov, g->d_cov, sizeof(float) * 3 * g->F * g->C, cudaMemcpyDeviceToHost,
                               g->stream));
+  COSL_TRY(read_undistorted(g, g->h_undPos, g->h_undCov, g->undFrame));
   COSL_CUDA(cudaStreamSynchronize(g->stream));
   return COSL_OK;
 }
@@ -1093,6 +1141,7 @@ int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_
   g->p1 = g->nxt;
   COSL_CUDA(cudaStreamWaitEvent(g->stream, g->evTail, 0));
   g->covFrame = g->covNoise >= 0.f;
+  g->undFrame = g->undArmed;
   if (p.tracked) {
     COSL_TRY(run_tracker(g, p));
     if (g->covFrame) COSL_TRY(run_covariance(g, p));
@@ -1120,6 +1169,7 @@ int run_frame(cosl_klt* g, const FramePlan& p, const uint8_t* const* imgs, size_
     COSL_LAUNCH(klt_provide_cams, dim3(div_up(g->F, 256), p.provide.n), 256, 0, g->stream, g->d_res, g->d_dst,
                 g->d_src, g->F, p.provide);
   if (p.wantCorn) COSL_TRY(run_detector(g, p));
+  if (g->undFrame) COSL_TRY(run_undistortion(g));
   if (!p.tracked) COSL_TRY(exchange_slices(g, p.exchangeLate, 0));
   if (p.tab >= 0) COSL_CUDA(cudaEventRecord(g->evStepFence[p.tab], g->stream));
   if (p.intoP1) {
@@ -1199,8 +1249,13 @@ static int drop_prefetch(cosl_klt* g) {
 // ops: the step the tables come from (nullptr: a frame of one kind for every camera): the addressed
 // cameras only, a tracked-only camera's count being its live tracks (counters[8c + 0], what track()
 // returns).  cov: the frame's covariances (nullptr: it was not armed), which the addressed cameras'
-// entries of covOut take, as dest[c] takes the table.
-void copy_out(cosl_klt* g, const cosl_klt_feature* feat, const int* counters, const float* cov,
+// entries of covOut take, as dest[c] takes the table; und: its undistorted positions and their
+// covariances (either nullptr: not computed), likewise for undPosOut and undCovOut.
+struct UndOut {
+  const double* pos;
+  const float* cov;
+};
+void copy_out(cosl_klt* g, const cosl_klt_feature* feat, const int* counters, const float* cov, UndOut und,
               const uint8_t* ops, cosl_klt_feature* const* dest, int* n) {
   bool any = false;
   for (int c = 0; c < g->C; ++c) {
@@ -1213,12 +1268,28 @@ void copy_out(cosl_klt* g, const cosl_klt_feature* feat, const int* counters, co
       const size_t o = (size_t)3 * c * g->F;
       std::memcpy(g->covOut.data() + o, cov + o, sizeof(float) * 3 * g->F);
     }
+    if (und.pos) {
+      const size_t o = (size_t)2 * c * g->F;
+      std::memcpy(g->undPosOut.data() + o, und.pos + o, sizeof(double) * 2 * g->F);
+    }
+    if (und.cov) {
+      const size_t o = (size_t)3 * c * g->F;
+      std::memcpy(g->undCovOut.data() + o, und.cov + o, sizeof(float) * 3 * g->F);
+    }
   }
-  if (any) g->covHanded = cov != nullptr;
+  if (any) {
+    g->covHanded = cov != nullptr;
+    g->undHanded = und.pos != nullptr;
+    g->undCovHanded = und.cov != nullptr;
+  }
 }
 
-// the synchronous calls' covariances (fetch_results): those of the last frame run, if it was armed
+// the synchronous calls' covariances and undistorted positions (fetch_results): those of the last frame
+// run, if it was armed
 const float* sync_cov(const cosl_klt* g) { return g->covFrame ? g->h_cov : nullptr; }
+UndOut sync_und(const cosl_klt* g) {
+  return {g->undFrame ? g->h_undPos : nullptr, g->undFrame && g->covFrame ? g->h_undCov : nullptr};
+}
 
 }  // namespace
 
@@ -1355,7 +1426,7 @@ int cosl_klt_detect(cosl_klt* h, const uint8_t* img, size_t pitch, int nPresent,
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_DETECT, maxPresent, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, &dest, nDetected);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), nullptr, &dest, nDetected);
   return COSL_OK;
 }
 
@@ -1368,7 +1439,7 @@ int cosl_klt_redetect(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_fe
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, &dest, nNewFeatures);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), nullptr, &dest, nNewFeatures);
   return COSL_OK;
 }
 
@@ -1381,7 +1452,7 @@ int cosl_klt_track(cosl_klt* h, const uint8_t* img, size_t pitch, cosl_klt_featu
   const uint8_t* imgs[1] = {img};
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_TRACK, 0, false), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, &dest, nullptr);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), nullptr, &dest, nullptr);
   *nPresent = h->h_counters[0];
   return COSL_OK;
 }
@@ -1445,6 +1516,72 @@ int cosl_klt_group_download_covariance(cosl_klt* h, float* const* cov) {
   return COSL_OK;
 }
 
+// Every lens is checked before anything changes, so a refused call leaves the group as it was.  The
+// buffers are made on the first arming and kept when the group is disarmed.  The table goes to the
+// device on `stream` from pageable memory (staged before the call returns), so the frames enqueued
+// before the call read the old lenses and those after it the new ones.
+int cosl_klt_set_undistortion(cosl_klt* h, const double* K, const double* kc) {
+  KLT_ENTER(h)
+  if (!K) {
+    h->undArmed = false;
+    return COSL_OK;
+  }
+  if (!kc) return set_error(COSL_E_INVALID, "set_undistortion: K given without kc");
+  std::vector<KltUndistCam> cams(h->C);
+  for (int c = 0; c < h->C; ++c) {
+    const double* k = K + 9 * c;
+    const double* d = kc + 5 * c;
+    for (int i = 0; i < 9; ++i)
+      if (!std::isfinite(k[i])) return set_error(COSL_E_INVALID, "set_undistortion: K of camera %d is not finite", c);
+    for (int i = 0; i < 5; ++i)
+      if (!std::isfinite(d[i])) return set_error(COSL_E_INVALID, "set_undistortion: kc of camera %d is not finite", c);
+    if (!(k[0] > 0.0) || !(k[4] > 0.0))
+      return set_error(COSL_E_INVALID, "set_undistortion: K of camera %d has fx %g, fy %g (both must be > 0)", c,
+                       k[0], k[4]);
+    if (k[3] != 0.0 || k[6] != 0.0 || k[7] != 0.0 || k[8] != 1.0)
+      return set_error(COSL_E_INVALID,
+                       "set_undistortion: K of camera %d is not upper triangular with K[8] = 1 (K[3] %g, last row "
+                       "%g %g %g)",
+                       c, k[3], k[6], k[7], k[8]);
+    cams[c] = {k[0], k[1], k[2], k[4], k[5], d[0], d[1], d[2], d[3], d[4], h->hcam[c].W, h->hcam[c].H};
+  }
+  if (!h->d_undCams) {
+    const size_t n = (size_t)h->F * h->C;
+    COSL_CUDA(cudaMalloc(&h->d_undCams, sizeof(KltUndistCam) * h->C));
+    COSL_CUDA(cudaMalloc(&h->d_undPos, sizeof(double) * 2 * n));
+    COSL_CUDA(cudaMalloc(&h->d_undCov, sizeof(float) * 3 * n));
+    COSL_CUDA(cudaMallocHost(&h->h_undPos, sizeof(double) * 2 * n));
+    COSL_CUDA(cudaMallocHost(&h->h_undCov, sizeof(float) * 3 * n));
+    for (int i = 0; i < 2; ++i) {
+      COSL_CUDA(cudaMallocHost(&h->h_undPosQ[i], sizeof(double) * 2 * n));
+      COSL_CUDA(cudaMallocHost(&h->h_undCovQ[i], sizeof(float) * 3 * n));
+    }
+    h->undPosOut.assign(2 * n, std::nan(""));
+    h->undCovOut.assign(3 * n, std::nanf(""));
+  }
+  COSL_CUDA(cudaMemcpyAsync(h->d_undCams, cams.data(), sizeof(KltUndistCam) * h->C, cudaMemcpyHostToDevice,
+                            h->stream));
+  h->undArmed = true;
+  return COSL_OK;
+}
+
+int cosl_klt_group_download_undistorted(cosl_klt* h, double* const* pos, float* const* cov) {
+  KLT_ENTER(h)
+  if (!h->undHanded)
+    return set_error(COSL_E_STATE, "group_download_undistorted: the last frame handed out was not armed "
+                                   "(cosl_klt_set_undistortion)");
+  if (cov && !h->undCovHanded)
+    return set_error(COSL_E_STATE, "group_download_undistorted: the last frame handed out had no position "
+                                   "covariances (cosl_klt_set_covariance)");
+  for (int c = 0; c < h->C; ++c) {
+    if (pos && pos[c])
+      std::memcpy(pos[c], h->undPosOut.data() + (size_t)2 * c * h->F, sizeof(double) * 2 * h->F);
+    if (cov && cov[c])
+      std::memcpy(cov[c], h->undCovOut.data() + (size_t)3 * c * h->F, sizeof(float) * 3 * h->F);
+  }
+  return COSL_OK;
+}
+
 #define KLT_NOT_IN_FLIGHT(h, name) \
   if ((h)->nInFlight > 0) return set_error(COSL_E_STATE, name ": submitted frames not yet collected");
 
@@ -1456,7 +1593,7 @@ static int group_first(cosl_klt* h, const uint8_t* const* imgs, size_t pitch, co
   if (nPresent) COSL_TRY(upload_present(h, nPresent, present3, &maxPresent));
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_DETECT, maxPresent, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, dest, nDetected);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), nullptr, dest, nDetected);
   return COSL_OK;
 }
 
@@ -1509,7 +1646,7 @@ int cosl_klt_group_next(cosl_klt* h, const uint8_t* const* imgs, size_t pitch,
   if (!imgs || !pitch_ok(h, pitch)) return set_error(COSL_E_INVALID, "group_next: bad argument");
   COSL_TRY(run_frame(h, plan_frame(h, FRAME_REDETECT, 0, true), imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), nullptr, dest, nNew);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), nullptr, dest, nNew);
   return COSL_OK;
 }
 
@@ -1541,7 +1678,7 @@ int cosl_klt_group_step(cosl_klt* h, const uint8_t* ops, const uint8_t* const* i
   COSL_TRY(check_step(h, ops, imgs, pitch, "group_step"));
   COSL_TRY(run_step(h, ops, imgs, pitch, cudaMemcpyHostToDevice));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), ops, dest, n);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), ops, dest, n);
   return COSL_OK;
 }
 
@@ -1556,7 +1693,8 @@ int cosl_klt_group_step_dev(cosl_klt* h, const uint8_t* ops, const uint8_t* cons
 int cosl_klt_group_fetch(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew) {
   KLT_ENTER(h)
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), h->stepOpsValid ? h->stepOps : nullptr, dest, nNew);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), h->stepOpsValid ? h->stepOps : nullptr, dest,
+           nNew);
   return COSL_OK;
 }
 
@@ -1596,6 +1734,8 @@ static int submit_readback(cosl_klt* h, int slot) {
   if (h->covQ[slot])
     COSL_CUDA(cudaMemcpyAsync(h->h_covQ[slot], h->d_cov, sizeof(float) * 3 * h->F * h->C, cudaMemcpyDeviceToHost,
                               h->stream));
+  h->undQ[slot] = any && h->undFrame;
+  COSL_TRY(read_undistorted(h, h->h_undPosQ[slot], h->h_undCovQ[slot], h->undQ[slot]));
   COSL_CUDA(cudaEventRecord(h->evDone[slot], h->stream));
   ++h->subSeq;
   ++h->nInFlight;
@@ -1634,8 +1774,10 @@ int cosl_klt_group_collect(cosl_klt* h, cosl_klt_feature* const* dest, int* nNew
   const int slot = (int)((h->subSeq - (unsigned)h->nInFlight) & 1u);
   COSL_CUDA(cudaEventSynchronize(h->evDone[slot]));
   --h->nInFlight;
-  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], h->covQ[slot] ? h->h_covQ[slot] : nullptr, h->opsQ[slot], dest,
-           nNew);
+  const UndOut und = {h->undQ[slot] ? h->h_undPosQ[slot] : nullptr,
+                      h->undQ[slot] && h->covQ[slot] ? h->h_undCovQ[slot] : nullptr};
+  copy_out(h, h->h_featQ[slot], h->h_cntQ[slot], h->covQ[slot] ? h->h_covQ[slot] : nullptr, und, h->opsQ[slot],
+           dest, nNew);
   return COSL_OK;
 }
 
@@ -1683,7 +1825,7 @@ int cosl_klt_group_run_prefetched(cosl_klt* h, cosl_klt_feature* const* dest, in
   if (h->pf.step) KLT_NOT_IN_FLIGHT(h, "group_run_prefetched")
   COSL_TRY(consume_prefetch(h));
   COSL_TRY(fetch_results(h));
-  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), h->pf.step ? h->pf.ops : nullptr, dest, n);
+  copy_out(h, h->h_feat, h->h_counters, sync_cov(h), sync_und(h), h->pf.step ? h->pf.ops : nullptr, dest, n);
   return COSL_OK;
 }
 

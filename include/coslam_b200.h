@@ -171,6 +171,32 @@ int cosl_klt_set_covariance(cosl_klt* h, float noise_var);
  * a camera the frame skipped keeps the entries it had, as its dest[c] does.  COSL_E_STATE when the
  * last frame handed out was not armed, or none was. */
 int cosl_klt_group_download_covariance(cosl_klt* h, float* const* cov);
+/* Extension: the undistorted pixel position of every slot and, where the frame has position
+ * covariances, their covariance in the undistorted image (DESIGN.md section 3.5).  K: C row-major
+ * 3x3 camera matrices (C * 9 doubles; K[3] = K[6] = K[7] = 0, K[8] = 1, fx = K[0] > 0, fy = K[4] > 0,
+ * skew K[1]); kc: C Bouguet 5-vectors (k1, k2, p1, p2, k3), the forward model OpenCV's projectPoints
+ * applies.  For slot i of camera c (W_c x H_c):
+ *   u_d = pos[0] W_c, v_d = pos[1] H_c (texel centres at i + 0.5), x_d = K2^-1 (u_d - cx, v_d - cy),
+ *       K2 = [[fx, s], [0, fy]];
+ *   x* solves d(x*) = x_d by at most 20 Newton steps from x_d, stopping once |K2 (d(x) - x_d)|_inf
+ *       <= 1e-9 px; (u, v) = K2 x* + (cx, cy), fp64;
+ *   cov = A Sigma_d A^T, A = K2 J(x*)^-1 K2^-1 (J = dd/dx), from the slot's cosl_klt_set_covariance
+ *       entry Sigma_d, computed in fp64 and stored as float (xx, xy, yy).
+ * NaN for a slot with status < 0 and where the inverse fails (the tolerance is not met, det J <= 0 at an
+ * iterate or at the answer, a non-finite value); cov also where Sigma_d is NaN.  With kc = 0 the stage
+ * is the identity to roundoff.  K == NULL disarms (the default: nothing is computed, and the group
+ * launches exactly what it launches without this call).  COSL_E_INVALID, naming the first bad camera,
+ * for a non-finite K or kc, fx <= 0 or fy <= 0, or a malformed K; nothing changes then.  Like
+ * cosl_klt_set_covariance it applies to the frames enqueued after the call; a pending prefetch takes
+ * it when it is consumed.  An armed frame adds one kernel after the last writer of the feature table and
+ * a D2H copy of C * featW * featH * 2 doubles (and * 3 floats with covariances). */
+int cosl_klt_set_undistortion(cosl_klt* h, const double* K, const double* kc);
+/* Of the last frame handed out (by next, step, track, redetect, detect, first*, run_prefetched, collect
+ * or fetch): pos[c] receives featW * featH (u, v) doubles, cov[c] featW * featH (xx, xy, yy) floats,
+ * slot-major.  Either array, or any entry of it, may be NULL: not written.  A camera the frame skipped
+ * keeps the entries it had, as its dest[c] does.  COSL_E_STATE when the last frame handed out was not
+ * armed (or none was), and when cov is given and that frame had no position covariances. */
+int cosl_klt_group_download_undistorted(cosl_klt* h, double* const* pos, float* const* cov);
 
 /* Extension (batched GPUKLT::next, tracking/GPUKLT.cpp:144-161): redetect + advanceFrame for all
  * cameras of the group.  imgs[c] are HOST pointers (pinned memory recommended); dest[c] has
