@@ -93,6 +93,9 @@ def _load():
     L.cosl_pose_solver_submit_mappts.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, cd, vp,
                                                  vp, vp, vp, vp, vp, cd]
     L.cosl_pose_solver_download_mappts.argtypes = [vp, vp, vp, vp, vp]
+    L.cosl_pose_solver_set_ransac.argtypes = [vp, ci, vp, ci, cd, ci, C.c_uint64]
+    L.cosl_pose_solver_download_ransac.argtypes = [vp, vp, vp, vp, vp]
+    L.cosl_pose_solver_download_ransac_hyps.argtypes = [vp, ci, vp, vp, vp, vp, vp]
     L.cosl_tri_solver_create.argtypes = [ci, ci, ci, ci, C.POINTER(vp)]
     L.cosl_tri_solver_destroy.argtypes = [vp]
     L.cosl_tri_solver_submit.argtypes = [vp, ci, vp, vp, vp, vp, ci, vp, vp, vp, vp, cd, cd]
@@ -739,6 +742,41 @@ class PoseSolver(_SolverHandle):
         _ck(LIB.cosl_pose_solver_download_mappts(self.h, _ptr(X), _ptr(P), _ptr(st), _ptr(status)))
         cam = np.repeat(np.arange(len(self._nmap), dtype=np.int32), self._nmap)
         return dict(X=X, P=P, d2_0=st[:, 0].copy(), d2_1=st[:, 1].copy(), e0=st[:, 2].copy(), status=status, cam=cam)
+
+    def set_ransac(self, use, n_hyp, err_thres, min_inliers=6, seed=0):
+        """cosl_pose_solver_set_ransac: use, one flag per camera of the submits that follow (None disarms), selects
+        the cameras whose R0, t0 a PnP RANSAC of n_hyp 5-point EPnP hypotheses may replace before the solve; a point
+        is an inlier within err_thres px.  Read the outcome with download_ransac()."""
+        if use is None:
+            _ck(LIB.cosl_pose_solver_set_ransac(self.h, 0, None, 0, 0.0, 0, 0))
+            return
+        u = np.ascontiguousarray(np.asarray(use).astype(bool).astype(np.uint8))
+        _ck(LIB.cosl_pose_solver_set_ransac(self.h, len(u), _ptr(u), int(n_hyp), float(err_thres), int(min_inliers),
+                                            int(seed) & ((1 << 64) - 1)))
+
+    def download_ransac(self):
+        """cosl_pose_solver_download_ransac after collect() of an armed submit: a dict with R [C, 3, 3], t [C, 3] (the
+        start pose of the solve), status, inliers, sse and h [C] (status 0 replaced, 1 fewer than 5 points, 2 too few
+        inliers, 3 not selected, 4 R0 kept; h = -1 for R0), and inl, per camera the inlier flags of its points."""
+        npts = self._npts
+        Cn = len(npts)
+        R, t, st, inl = np.empty((Cn, 9)), np.empty((Cn, 3)), np.empty((Cn, 4)), np.empty(sum(npts), np.uint8)
+        _ck(LIB.cosl_pose_solver_download_ransac(self.h, _ptr(R), _ptr(t), _ptr(st), _ptr(inl)))
+        return dict(R=R.reshape(Cn, 3, 3), t=t, status=st[:, 0].astype(np.int32), inliers=st[:, 1].astype(np.int64),
+                    sse=st[:, 2].copy(), h=st[:, 3].astype(np.int64),
+                    inl=[a.astype(bool) for a in np.split(inl, np.cumsum(npts)[:-1])])
+
+    def download_ransac_hyps(self):
+        """cosl_pose_solver_download_ransac_hyps: per camera and hypothesis of the last armed submit, idx [C, H, 5],
+        pose [C, H, 12] (R | t), inliers [C, H] (-1 degenerate) and sse [C, H], H the hypotheses that submit drew
+        (asked of the handle, so a later set_ransac does not change the shapes)."""
+        Cn, nh = len(self._npts), C.c_int(0)
+        _ck(LIB.cosl_pose_solver_download_ransac_hyps(self.h, 0, C.byref(nh), None, None, None, None))
+        H = nh.value
+        idx, pose = np.empty((Cn, H, 5), np.int32), np.empty((Cn, H, 12))
+        cnt, sse = np.empty((Cn, H), np.int32), np.empty((Cn, H))
+        _ck(LIB.cosl_pose_solver_download_ransac_hyps(self.h, H, None, _ptr(idx), _ptr(pose), _ptr(cnt), _ptr(sse)))
+        return dict(idx=idx, pose=pose, inliers=cnt, sse=sse)
 
 
 class TriSolver(_SolverHandle):

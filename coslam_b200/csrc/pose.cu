@@ -24,6 +24,8 @@
 #include <mutex>
 #include <new>
 
+#include <math_constants.h>
+
 #include "common.cuh"
 
 using namespace coslam;
@@ -1513,6 +1515,645 @@ assoc_final_kernel(const int* __restrict__ qPt, int nQ, const unsigned long long
   if ((unsigned long long)__double_as_longlong(r[2]) != key[f] || win[f] != (unsigned int)qPt[q]) r[0] = 6;
 }
 
+// PnP RANSAC of an armed pose solver handle (cosl_pose_solver_set_ransac, DESIGN.md 5.7, an extension).  Before the
+// solve, ransac_hyp_kernel draws and solves nHyp 5-point EPnP hypotheses per selected camera, ransac_score_kernel
+// scores them and the caller's R0, t0 over the camera's points, and ransac_select_kernel picks one per camera and
+// rewrites the record's R0, t0 when it replaces them.  tests/pnp_dense.py restates all of it operation for operation.
+constexpr int RANSAC_HYP_THREADS = 32;
+constexpr int RANSAC_SCORE_THREADS = 128;
+constexpr int RANSAC_SEL_THREADS = 128;
+constexpr int RANSAC_HYP = 13;   // per hypothesis: R[9] | t[3] | ok
+constexpr int RANSAC_RES = 16;   // per camera: R[9] | t[3] | status | inliers | sse | h
+constexpr int RANSAC_NDRAW = 256;
+constexpr int RANSAC_SWEEPS3 = 12, RANSAC_SWEEPS12 = 16, RANSAC_GN = 5;
+constexpr double RANSAC_JACOBI_TOL = 1e-30;
+constexpr double RANSAC_PCA_MIN = 1e-12;
+// per-thread scratch of ransac_hyp_kernel, in doubles: 12x12 MtM | its eigenvectors | alphas | world points |
+// pixels | rho | camera points | K | the best candidate's R, t.  After the 12x12 solve the MtM section holds the
+// beta stage (RS_L...).  Little stays in registers across the eigensolver and least-squares calls.
+constexpr int RS_A = 0, RS_V = 144, RS_AL = 288, RS_PW = 308, RS_PX = 323, RS_RHO = 333, RS_PC = 339, RS_K = 354,
+              RS_BEST = 363, RS_N = 375;
+constexpr int RS_L = 0, RS_LSA = 60, RS_LSB = 90, RS_LSX = 96, RS_KA = 101, RS_KS = 110, RS_KV = 119, RS_CC = 128;
+
+// One thread's scratch in shared memory, element i at p[i * RANSAC_HYP_THREADS]: the threads of a warp read
+// consecutive doubles, and every index may be computed at run time without local memory.
+struct Scr {
+  double* p;
+  __device__ __forceinline__ double& operator[](int i) const { return p[i * RANSAC_HYP_THREADS]; }
+  __device__ __forceinline__ Scr operator+(int o) const { return Scr{p + o * RANSAC_HYP_THREADS}; }
+};
+
+__device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
+  unsigned long long z = x + 0x9e3779b97f4a7c15ull;
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+
+__device__ __forceinline__ bool finite_all(const double* x, int n) {
+  bool f = true;
+  for (int i = 0; i < n; ++i) f &= isfinite(x[i]);
+  return f;
+}
+
+// Cyclic Jacobi on the symmetric n x n A (row-major): A = V diag(A_kk) V^T afterwards.  Sweeps over (p, q), p < q,
+// row by row; each rotation theta = (a_qq - a_pp) / (2 a_pq), t = sign(theta) / (|theta| + sqrt(theta^2 + 1)),
+// c = 1 / sqrt(t^2 + 1), s = t c goes to the columns p, q, then the rows p, q, then a_pq = a_qp = 0, and to V's
+// columns; a_pq = 0 skips.  A sweep starts only while sum_{p<q} a_pq^2 > RANSAC_JACOBI_TOL sum_p a_pp^2.
+__device__ __noinline__ void jacobi_sym(Scr A, Scr V, int n, int sweeps) {
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < n; ++j) V[n * i + j] = i == j ? 1.0 : 0.0;
+  for (int sw = 0; sw < sweeps; ++sw) {
+    double off = 0, dia = 0;
+    for (int p = 0; p < n; ++p) {
+      dia = dia + A[n * p + p] * A[n * p + p];
+      for (int q = p + 1; q < n; ++q) off = off + A[n * p + q] * A[n * p + q];
+    }
+    if (off <= RANSAC_JACOBI_TOL * dia) break;
+    for (int p = 0; p < n - 1; ++p)
+      for (int q = p + 1; q < n; ++q) {
+        const double apq = A[n * p + q];
+        if (apq == 0) continue;
+        const double theta = (A[n * q + q] - A[n * p + p]) / (2.0 * apq);
+        double t = 1.0 / (fabs(theta) + sqrt(theta * theta + 1.0));
+        if (theta < 0) t = -t;
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < n; ++k) {
+          const double xp = A[n * k + p], xq = A[n * k + q];
+          A[n * k + p] = c * xp - s * xq;
+          A[n * k + q] = s * xp + c * xq;
+        }
+        for (int k = 0; k < n; ++k) {
+          const double xp = A[n * p + k], xq = A[n * q + k];
+          A[n * p + k] = c * xp - s * xq;
+          A[n * q + k] = s * xp + c * xq;
+        }
+        A[n * p + q] = 0.0;
+        A[n * q + p] = 0.0;
+        for (int k = 0; k < n; ++k) {
+          const double xp = V[n * k + p], xq = V[n * k + q];
+          V[n * k + p] = c * xp - s * xq;
+          V[n * k + q] = s * xp + c * xq;
+        }
+      }
+  }
+}
+
+// min |A x - b| for A 6 x n (row-major, n <= 5) by Householder QR; A and b are overwritten, x gets n values.
+__device__ __noinline__ void lstsq6(Scr A, Scr b, Scr x, int n) {
+  for (int k = 0; k < n; ++k) {
+    double nrm2 = 0;
+    for (int i = k; i < 6; ++i) nrm2 = nrm2 + A[n * i + k] * A[n * i + k];
+    const double alpha = A[n * k + k] > 0 ? -sqrt(nrm2) : sqrt(nrm2);
+    double v[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) v[i] = i < k ? 0.0 : i == k ? A[n * i + k] - alpha : A[n * i + k];
+    double vv = 0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+      if (i >= k) vv = vv + v[i] * v[i];
+    for (int j = k; j < n; ++j) {
+      double f = 0;
+#pragma unroll
+      for (int i = 0; i < 6; ++i)
+        if (i >= k) f = f + v[i] * A[n * i + j];
+      f = 2.0 * f / vv;
+#pragma unroll
+      for (int i = 0; i < 6; ++i)
+        if (i >= k) A[n * i + j] = A[n * i + j] - f * v[i];
+    }
+    double f = 0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+      if (i >= k) f = f + v[i] * b[i];
+    f = 2.0 * f / vv;
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+      if (i >= k) b[i] = b[i] - f * v[i];
+  }
+  for (int k = n - 1; k >= 0; --k) {
+    double a = b[k];
+    for (int j = k + 1; j < n; ++j) a = a - A[n * k + j] * x[j];
+    x[k] = a / A[n * k + k];
+  }
+}
+
+// The first n columns of L (6 x 10) over the betas {B11 B12 B13 B14} (n = 4: columns 0, 1, 3, 6) or {B11 B12 B22
+// B13 B23} (n = 3 or 5: columns 0 to n - 1) into the least-squares matrix, rho into its right-hand side, and the solve.
+__device__ __forceinline__ void betas_lstsq(Scr s, int n) {
+  for (int i = 0; i < 6; ++i) {
+    for (int j = 0; j < n; ++j) s[RS_LSA + n * i + j] = s[RS_L + 10 * i + (n == 4 ? (j * (j + 1)) / 2 : j)];
+    s[RS_LSB + i] = s[RS_RHO + i];
+  }
+  lstsq6(s + RS_LSA, s + RS_LSB, s + RS_LSX, n);
+}
+
+// The pose of the betas b: camera-frame control points sum_k b_k v_k (v_k = column ev[k] of V), the sample's camera
+// points, the sign fix and the absolute orientation (pnp_dense.pose_from_betas).  Returns the summed reprojection
+// error over the sample in px, +inf when anything is not finite.
+__device__ double epnp_pose(Scr s, const int ev[4], const double b[4], double R[9], double t[3]) {
+  for (int j = 0; j < 4; ++j)
+    for (int k = 0; k < 3; ++k) {
+      const int r = 3 * j + k;
+      s[RS_CC + r] = b[0] * s[RS_V + 12 * r + ev[0]] + b[1] * s[RS_V + 12 * r + ev[1]] +
+                     b[2] * s[RS_V + 12 * r + ev[2]] + b[3] * s[RS_V + 12 * r + ev[3]];
+    }
+  for (int i = 0; i < 5; ++i)
+    for (int k = 0; k < 3; ++k)
+      s[RS_PC + 3 * i + k] = s[RS_AL + 4 * i] * s[RS_CC + k] + s[RS_AL + 4 * i + 1] * s[RS_CC + 3 + k] +
+                             s[RS_AL + 4 * i + 2] * s[RS_CC + 6 + k] + s[RS_AL + 4 * i + 3] * s[RS_CC + 9 + k];
+  if (s[RS_PC + 2] < 0)
+    for (int i = 0; i < 15; ++i) s[RS_PC + i] = -s[RS_PC + i];
+  double pc0[3], pw0[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    double a = s[RS_PC + k], w = s[RS_PW + k];
+    for (int i = 1; i < 5; ++i) {
+      a = a + s[RS_PC + 3 * i + k];
+      w = w + s[RS_PW + 3 * i + k];
+    }
+    pc0[k] = a / 5.0;
+    pw0[k] = w / 5.0;
+  }
+  double A[9];
+#pragma unroll
+  for (int q = 0; q < 9; ++q) A[q] = 0.0;
+  for (int i = 0; i < 5; ++i) {
+    double dc[3], dw[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      dc[k] = s[RS_PC + 3 * i + k] - pc0[k];
+      dw[k] = s[RS_PW + 3 * i + k] - pw0[k];
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) A[3 * a + c] += dc[a] * dw[c];
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s[RS_KS + 3 * a + c] = A[a] * A[c] + A[3 + a] * A[3 + c] + A[6 + a] * A[6 + c];
+  jacobi_sym(s + RS_KS, s + RS_KV, 3, RANSAC_SWEEPS3);
+  // columns of V by decreasing eigenvalue, ties to the lower index
+  const double l0 = s[RS_KS], l1 = s[RS_KS + 4], l2 = s[RS_KS + 8];
+  int o[3];
+  o[0] = (l0 >= l1 && l0 >= l2) ? 0 : (l1 >= l2 ? 1 : 2);
+  {
+    const int a = o[0] == 0 ? 1 : 0, c = o[0] == 2 ? 1 : 2;
+    const double la = a == 0 ? l0 : l1, lc = c == 1 ? l1 : l2;
+    o[1] = la >= lc ? a : c;
+    o[2] = la >= lc ? c : a;
+  }
+  double v1[3], v2[3], v3[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    v1[k] = s[RS_KV + 3 * k + o[0]];
+    v2[k] = s[RS_KV + 3 * k + o[1]];
+    v3[k] = s[RS_KV + 3 * k + o[2]];
+  }
+  double u1[3], u2[3], u3[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    u1[i] = A[3 * i] * v1[0] + A[3 * i + 1] * v1[1] + A[3 * i + 2] * v1[2];
+    u2[i] = A[3 * i] * v2[0] + A[3 * i + 1] * v2[1] + A[3 * i + 2] * v2[2];
+  }
+  const double n1 = sqrt(u1[0] * u1[0] + u1[1] * u1[1] + u1[2] * u1[2]);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) u1[i] = u1[i] / n1;
+  const double d12 = u1[0] * u2[0] + u1[1] * u2[1] + u1[2] * u2[2];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) u2[i] = u2[i] - d12 * u1[i];
+  const double n2 = sqrt(u2[0] * u2[0] + u2[1] * u2[1] + u2[2] * u2[2]);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) u2[i] = u2[i] / n2;
+  u3[0] = u1[1] * u2[2] - u1[2] * u2[1];
+  u3[1] = u1[2] * u2[0] - u1[0] * u2[2];
+  u3[2] = u1[0] * u2[1] - u1[1] * u2[0];
+  const double detV = v1[0] * (v2[1] * v3[2] - v2[2] * v3[1]) - v2[0] * (v1[1] * v3[2] - v1[2] * v3[1]) +
+                      v3[0] * (v1[1] * v2[2] - v1[2] * v2[1]);
+  const double sgn = detV < 0 ? -1.0 : 1.0;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) R[3 * i + j] = u1[i] * v1[j] + u2[i] * v2[j] + sgn * u3[i] * v3[j];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) t[i] = pc0[i] - (R[3 * i] * pw0[0] + R[3 * i + 1] * pw0[1] + R[3 * i + 2] * pw0[2]);
+  double K[9];
+#pragma unroll
+  for (int q = 0; q < 9; ++q) K[q] = s[RS_K + q];
+  double err = 0;
+  for (int i = 0; i < 5; ++i) {
+    const double M[3] = {s[RS_PW + 3 * i], s[RS_PW + 3 * i + 1], s[RS_PW + 3 * i + 2]};
+    double m[2];
+    project(K, R, t, M, m);
+    const double du = s[RS_PX + 2 * i] - m[0], dv = s[RS_PX + 2 * i + 1] - m[1];
+    err = err + sqrt(du * du + dv * dv);
+  }
+  return (isfinite(err) && finite_all(R, 9) && finite_all(t, 3)) ? err : CUDART_INF;
+}
+
+// One hypothesis per thread: the sampler, then EPnP on the sample (DESIGN.md 5.7).  hyp[c][h] gets R | t | ok and
+// smp[c][h] the 5 indices (-1 without 5 distinct ones); a camera that is not selected or has fewer than 5 points gets
+// ok = 0 and indices -1.
+__global__ void __launch_bounds__(RANSAC_HYP_THREADS)
+ransac_hyp_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll, const double* __restrict__ msAll,
+                  const unsigned char* __restrict__ use, int nHyp, unsigned long long seed, double* __restrict__ hyp,
+                  int* __restrict__ smp) {
+  extern __shared__ double s_scr[];
+  const int c = blockIdx.y;
+  const int h = blockIdx.x * RANSAC_HYP_THREADS + threadIdx.x;
+  if (h >= nHyp) return;
+  const Scr s{s_scr + threadIdx.x};
+  const PoseCam& cam = cams[c];
+  const int n = cam.npts;
+  double* out = hyp + RANSAC_HYP * ((size_t)c * nHyp + h);
+  int* idx = smp + 5 * ((size_t)c * nHyp + h);
+  out[12] = 0.0;
+  int i0 = -1, i1 = -1, i2 = -1, i3 = -1, i4 = -1, cnt = 0;
+  if (use[c] && n >= 5) {
+    const unsigned long long base = seed ^ (((unsigned long long)c << 40) | ((unsigned long long)h << 8));
+    for (int j = 0; j < RANSAC_NDRAW && cnt < 5; ++j) {
+      const int v = (int)(splitmix64(base ^ (unsigned long long)j) % (unsigned long long)n);
+      if (v == i0 || v == i1 || v == i2 || v == i3) continue;
+      if (cnt == 0) i0 = v;
+      else if (cnt == 1) i1 = v;
+      else if (cnt == 2) i2 = v;
+      else if (cnt == 3) i3 = v;
+      else i4 = v;
+      ++cnt;
+    }
+  }
+  if (cnt < 5) i0 = i1 = i2 = i3 = i4 = -1;
+  idx[0] = i0;
+  idx[1] = i1;
+  idx[2] = i2;
+  idx[3] = i3;
+  idx[4] = i4;
+  if (cnt < 5) return;
+  const double* Ms = MsAll + 3 * cam.off;
+  const double* ms = msAll + 2 * cam.off;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) s[RS_K + k] = cam.K[k];
+  const int sel[5] = {i0, i1, i2, i3, i4};
+#pragma unroll
+  for (int i = 0; i < 5; ++i) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) s[RS_PW + 3 * i + k] = Ms[3 * sel[i] + k];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) s[RS_PX + 2 * i + k] = ms[2 * sel[i] + k];
+  }
+  // control points: the centroid and the principal axes
+  double c0[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    double a = s[RS_PW + k];
+    for (int i = 1; i < 5; ++i) a = a + s[RS_PW + 3 * i + k];
+    c0[k] = a / 5.0;
+  }
+  {
+    double Cv[9];
+#pragma unroll
+    for (int q = 0; q < 9; ++q) Cv[q] = 0.0;
+    for (int i = 0; i < 5; ++i) {
+      double D[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) D[k] = s[RS_PW + 3 * i + k] - c0[k];
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) Cv[3 * a + b] += D[a] * D[b];
+    }
+#pragma unroll
+    for (int q = 0; q < 9; ++q) s[RS_A + q] = Cv[q];
+  }
+  jacobi_sym(s + RS_A, s + RS_V, 3, RANSAC_SWEEPS3);
+  const double l0 = s[RS_A], l1 = s[RS_A + 4], l2 = s[RS_A + 8];
+  int o[3];
+  o[0] = (l0 >= l1 && l0 >= l2) ? 0 : (l1 >= l2 ? 1 : 2);
+  {
+    const int a = o[0] == 0 ? 1 : 0, b = o[0] == 2 ? 1 : 2;
+    const double la = a == 0 ? l0 : l1, lb = b == 1 ? l1 : l2;
+    o[1] = la >= lb ? a : b;
+    o[2] = la >= lb ? b : a;
+  }
+  double lam[3], E[9];  // E[3 k + j]: component k of axis j
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    lam[j] = o[j] == 0 ? l0 : o[j] == 1 ? l1 : l2;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) E[3 * k + j] = s[RS_V + 3 * k + o[j]];
+  }
+  if (!finite_all(lam, 3) || !(lam[2] >= RANSAC_PCA_MIN * lam[0]) || !(lam[0] > 0)) return;
+  double sc[3], cw[12];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) sc[j] = sqrt(lam[j] / 5.0);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    cw[k] = c0[k];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) cw[3 * (j + 1) + k] = c0[k] + sc[j] * E[3 * k + j];
+  }
+  for (int i = 0; i < 5; ++i) {
+    const double D0 = s[RS_PW + 3 * i] - c0[0], D1 = s[RS_PW + 3 * i + 1] - c0[1], D2 = s[RS_PW + 3 * i + 2] - c0[2];
+    double a[4];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) a[j + 1] = (D0 * E[j] + D1 * E[3 + j] + D2 * E[6 + j]) / sc[j];
+    a[0] = 1.0 - a[1] - a[2] - a[3];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s[RS_AL + 4 * i + j] = a[j];
+  }
+  {
+    const int pa[6] = {0, 0, 0, 1, 1, 2}, pb[6] = {1, 2, 3, 2, 3, 3};
+#pragma unroll
+    for (int r = 0; r < 6; ++r) {
+      const double d0 = cw[3 * pa[r]] - cw[3 * pb[r]], d1 = cw[3 * pa[r] + 1] - cw[3 * pb[r] + 1],
+                   d2 = cw[3 * pa[r] + 2] - cw[3 * pb[r] + 2];
+      s[RS_RHO + r] = d0 * d0 + d1 * d1 + d2 * d2;
+    }
+  }
+  // M^T M of the 10 x 12 M, rows accumulated in order
+  for (int q = 0; q < 144; ++q) s[RS_A + q] = 0.0;
+  for (int i = 0; i < 5; ++i)
+    for (int r = 0; r < 2; ++r) {
+      const double x = s[RS_PX + 2 * i + r];
+      double row[12];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) row[3 * j + k] = s[RS_AL + 4 * i + j] * (s[RS_K + 3 * r + k] - x * s[RS_K + 6 + k]);
+#pragma unroll
+      for (int b = 0; b < 12; ++b) s[RS_PC + b] = row[b];  // the camera-point section is free until the betas
+#pragma unroll
+      for (int a = 0; a < 12; ++a)
+#pragma unroll 1
+        for (int b = 0; b < 12; ++b) s[RS_A + 12 * a + b] = s[RS_A + 12 * a + b] + row[a] * s[RS_PC + b];
+    }
+  jacobi_sym(s + RS_A, s + RS_V, 12, RANSAC_SWEEPS12);
+  // the eigenvectors of the 4 smallest eigenvalues, ties to the lower index
+  int ev[4];
+  {
+    unsigned taken = 0;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      int best = -1;
+      double bv = 0;
+      for (int k = 0; k < 12; ++k) {
+        const double d = s[RS_A + 13 * k];
+        if (!isfinite(d)) return;
+        if (!(taken >> k & 1u) && (best < 0 || d < bv)) {
+          best = k;
+          bv = d;
+        }
+      }
+      taken |= 1u << best;
+      ev[r] = best;
+    }
+  }
+  // L_6x10 (the MtM section is free now)
+  {
+    const int pa[6] = {0, 0, 0, 1, 1, 2}, pb[6] = {1, 2, 3, 2, 3, 3};
+    for (int r = 0; r < 6; ++r) {
+      double dv[4][3];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+          dv[i][k] = s[RS_V + 12 * (3 * pa[r] + k) + ev[i]] - s[RS_V + 12 * (3 * pb[r] + k) + ev[i]];
+#define RDOT(a, b) (dv[a][0] * dv[b][0] + dv[a][1] * dv[b][1] + dv[a][2] * dv[b][2])
+      s[RS_L + 10 * r + 0] = RDOT(0, 0);
+      s[RS_L + 10 * r + 1] = 2.0 * RDOT(0, 1);
+      s[RS_L + 10 * r + 2] = RDOT(1, 1);
+      s[RS_L + 10 * r + 3] = 2.0 * RDOT(0, 2);
+      s[RS_L + 10 * r + 4] = 2.0 * RDOT(1, 2);
+      s[RS_L + 10 * r + 5] = RDOT(2, 2);
+      s[RS_L + 10 * r + 6] = 2.0 * RDOT(0, 3);
+      s[RS_L + 10 * r + 7] = 2.0 * RDOT(1, 3);
+      s[RS_L + 10 * r + 8] = 2.0 * RDOT(2, 3);
+      s[RS_L + 10 * r + 9] = RDOT(3, 3);
+#undef RDOT
+    }
+  }
+  double bestErr = CUDART_INF;
+#pragma unroll 1
+  for (int N = 1; N <= 3; ++N) {
+    double b[4] = {0, 0, 0, 0};
+    if (N == 1) {
+      betas_lstsq(s, 4);
+      const double x0 = s[RS_LSX];
+      const bool neg = x0 < 0;
+      b[0] = sqrt(neg ? -x0 : x0);
+      for (int k = 1; k < 4; ++k) b[k] = (neg ? -s[RS_LSX + k] : s[RS_LSX + k]) / b[0];
+    } else {
+      betas_lstsq(s, N == 2 ? 3 : 5);
+      const double x0 = s[RS_LSX], x1 = s[RS_LSX + 1], x2 = s[RS_LSX + 2];
+      if (x0 < 0) {
+        b[0] = sqrt(-x0);
+        b[1] = x2 < 0 ? sqrt(-x2) : 0.0;
+      } else {
+        b[0] = sqrt(x0);
+        b[1] = x2 > 0 ? sqrt(x2) : 0.0;
+      }
+      if (x1 < 0) b[0] = -b[0];
+      if (N == 3) b[2] = s[RS_LSX + 3] / b[0];
+    }
+    for (int it = 0; it < RANSAC_GN; ++it) {  // Gauss-Newton on the 4 betas
+      for (int i = 0; i < 6; ++i) {
+        double l[10];
+#pragma unroll
+        for (int q = 0; q < 10; ++q) l[q] = s[RS_L + 10 * i + q];
+        s[RS_LSA + 4 * i + 0] = 2.0 * l[0] * b[0] + l[1] * b[1] + l[3] * b[2] + l[6] * b[3];
+        s[RS_LSA + 4 * i + 1] = l[1] * b[0] + 2.0 * l[2] * b[1] + l[4] * b[2] + l[7] * b[3];
+        s[RS_LSA + 4 * i + 2] = l[3] * b[0] + l[4] * b[1] + 2.0 * l[5] * b[2] + l[8] * b[3];
+        s[RS_LSA + 4 * i + 3] = l[6] * b[0] + l[7] * b[1] + l[8] * b[2] + 2.0 * l[9] * b[3];
+        s[RS_LSB + i] = s[RS_RHO + i] - (l[0] * b[0] * b[0] + l[1] * b[0] * b[1] + l[2] * b[1] * b[1] +
+                                         l[3] * b[0] * b[2] + l[4] * b[1] * b[2] + l[5] * b[2] * b[2] +
+                                         l[6] * b[0] * b[3] + l[7] * b[1] * b[3] + l[8] * b[2] * b[3] +
+                                         l[9] * b[3] * b[3]);
+      }
+      lstsq6(s + RS_LSA, s + RS_LSB, s + RS_LSX, 4);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) b[k] = b[k] + s[RS_LSX + k];
+    }
+    double R[9], t[3];
+    const double err = epnp_pose(s, ev, b, R, t);
+    if (err < bestErr) {
+      bestErr = err;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) s[RS_BEST + k] = R[k];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) s[RS_BEST + 9 + k] = t[k];
+    }
+  }
+  if (!isfinite(bestErr)) return;
+  for (int k = 0; k < 12; ++k) out[k] = s[RS_BEST + k];
+  out[12] = 1.0;
+}
+
+// Inlier count and sum of squared errors of pose (R, t) at one point: depth > 0 and sqrt(du^2 + dv^2) < thr.
+__device__ __forceinline__ void ransac_point(const double K[9], const double R[9], const double t[3], const double* M,
+                                            const double* m, double thr, bool& inl, double& e2) {
+  const double c0 = R[0] * M[0] + R[1] * M[1] + R[2] * M[2] + t[0];
+  const double c1 = R[3] * M[0] + R[4] * M[1] + R[5] * M[2] + t[1];
+  const double c2 = R[6] * M[0] + R[7] * M[1] + R[8] * M[2] + t[2];
+  const double u = K[0] * c0 + K[1] * c1 + K[2] * c2;
+  const double v = K[3] * c0 + K[4] * c1 + K[5] * c2;
+  const double w = K[6] * c0 + K[7] * c1 + K[8] * c2;
+  const double du = m[0] - u / w, dv = m[1] - v / w;
+  e2 = du * du + dv * dv;
+  inl = c2 > 0 && sqrt(e2) < thr;
+}
+
+// Slot k of camera c (blockIdx.y) is the caller's R0, t0 for k = 0 and hypothesis k - 1 after; each thread scores
+// one slot over the camera's points, staged through shared memory in tiles.  cnt = -1 (sse 0) for a degenerate
+// hypothesis and for every hypothesis of a camera that draws none.
+__global__ void __launch_bounds__(RANSAC_SCORE_THREADS)
+ransac_score_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
+                    const double* __restrict__ msAll, const unsigned char* __restrict__ use, int nHyp,
+                    const double* __restrict__ hyp, double thr, int* __restrict__ cnt, double* __restrict__ sse) {
+  __shared__ double s_pt[RANSAC_SCORE_THREADS * 5];
+  const int c = blockIdx.y;
+  const int k = blockIdx.x * RANSAC_SCORE_THREADS + threadIdx.x;
+  const PoseCam& cam = cams[c];
+  const int n = cam.npts;
+  const bool draws = use[c] && n >= 5;
+  int* oc = cnt + (size_t)c * (nHyp + 1);
+  double* os = sse + (size_t)c * (nHyp + 1);
+  if (!draws && blockIdx.x > 0) {  // uniform over the CTA
+    if (k <= nHyp) {
+      oc[k] = -1;
+      os[k] = 0.0;
+    }
+    return;
+  }
+  double K[9], R[9], t[3];
+  bool live = k <= nHyp;
+#pragma unroll
+  for (int q = 0; q < 9; ++q) K[q] = cam.K[q];
+  if (k == 0) {
+#pragma unroll
+    for (int q = 0; q < 9; ++q) R[q] = cam.R0[q];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) t[q] = cam.t0[q];
+  } else if (live) {
+    const double* r = hyp + RANSAC_HYP * ((size_t)c * nHyp + (k - 1));
+    live = draws && r[12] != 0.0;
+#pragma unroll
+    for (int q = 0; q < 9; ++q) R[q] = r[q];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) t[q] = r[9 + q];
+  }
+  const double* Ms = MsAll + 3 * cam.off;
+  const double* ms = msAll + 2 * cam.off;
+  int ni = 0;
+  double acc = 0.0;
+  for (int i0 = 0; i0 < n; i0 += RANSAC_SCORE_THREADS) {
+    const int m = min(RANSAC_SCORE_THREADS, n - i0);
+    __syncthreads();
+    for (int q = threadIdx.x; q < 3 * m; q += RANSAC_SCORE_THREADS) s_pt[q] = Ms[3 * i0 + q];
+    for (int q = threadIdx.x; q < 2 * m; q += RANSAC_SCORE_THREADS) s_pt[3 * RANSAC_SCORE_THREADS + q] = ms[2 * i0 + q];
+    __syncthreads();
+    if (live)
+      for (int i = 0; i < m; ++i) {
+        bool inl;
+        double e2;
+        ransac_point(K, R, t, s_pt + 3 * i, s_pt + 3 * RANSAC_SCORE_THREADS + 2 * i, thr, inl, e2);
+        if (inl) {
+          ++ni;
+          acc = acc + e2;
+        }
+      }
+  }
+  if (k <= nHyp) {
+    oc[k] = live ? ni : -1;
+    os[k] = live ? acc : 0.0;
+  }
+}
+
+// Slot a ranks before slot b: more inliers, then less sse, then the lower slot (slot 0, R0, is h = -1).
+__device__ __forceinline__ bool ransac_before(int ca, double sa, int a, int cb, double sb, int b) {
+  if (ca != cb) return ca > cb;
+  if (sa != sb) return sa < sb;
+  return a < b;
+}
+
+// One CTA per camera: the best slot by a reduction over a total order (so the result does not depend on thread
+// order), the status, the start pose (written into the record when a hypothesis replaces R0, t0), the result record
+// res[c] and the start pose's inlier flag of every point.
+__global__ void __launch_bounds__(RANSAC_SEL_THREADS)
+ransac_select_kernel(PoseCam* __restrict__ cams, const double* __restrict__ MsAll, const double* __restrict__ msAll,
+                     const unsigned char* __restrict__ use, int nHyp, const double* __restrict__ hyp,
+                     const int* __restrict__ cnt, const double* __restrict__ sse, double thr, int minInl,
+                     double* __restrict__ res, unsigned char* __restrict__ inl) {
+  __shared__ int s_k[RANSAC_SEL_THREADS], s_c[RANSAC_SEL_THREADS];
+  __shared__ double s_s[RANSAC_SEL_THREADS];
+  __shared__ double s_pose[12];
+  const int c = blockIdx.x;
+  PoseCam& cam = cams[c];
+  const int n = cam.npts;
+  const bool draws = use[c] && n >= 5;
+  const int slots = draws ? nHyp + 1 : 1;
+  const int* oc = cnt + (size_t)c * (nHyp + 1);
+  const double* os = sse + (size_t)c * (nHyp + 1);
+  int bk = 0, bc = oc[0];
+  double bs = os[0];
+  for (int k = threadIdx.x; k < slots; k += RANSAC_SEL_THREADS)
+    if (ransac_before(oc[k], os[k], k, bc, bs, bk)) {
+      bk = k;
+      bc = oc[k];
+      bs = os[k];
+    }
+  s_k[threadIdx.x] = bk;
+  s_c[threadIdx.x] = bc;
+  s_s[threadIdx.x] = bs;
+  __syncthreads();
+  for (int w = RANSAC_SEL_THREADS / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) {
+      const int o = threadIdx.x + w;
+      if (ransac_before(s_c[o], s_s[o], s_k[o], s_c[threadIdx.x], s_s[threadIdx.x], s_k[threadIdx.x])) {
+        s_k[threadIdx.x] = s_k[o];
+        s_c[threadIdx.x] = s_c[o];
+        s_s[threadIdx.x] = s_s[o];
+      }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    bk = s_k[0];
+    const int status = !use[c] ? 3 : n < 5 ? 1 : bk == 0 ? 4 : s_c[0] < minInl ? 2 : 0;
+    const double* src = status == 0 ? hyp + RANSAC_HYP * ((size_t)c * nHyp + (bk - 1)) : nullptr;
+    double* r = res + RANSAC_RES * (size_t)c;
+    for (int q = 0; q < 9; ++q) s_pose[q] = src ? src[q] : cam.R0[q];
+    for (int q = 0; q < 3; ++q) s_pose[9 + q] = src ? src[9 + q] : cam.t0[q];
+    for (int q = 0; q < 12; ++q) r[q] = s_pose[q];
+    r[12] = status;
+    r[13] = s_c[0];
+    r[14] = s_s[0];
+    r[15] = bk - 1;
+    if (status == 0) {
+      for (int q = 0; q < 9; ++q) cam.R0[q] = s_pose[q];
+      for (int q = 0; q < 3; ++q) cam.t0[q] = s_pose[9 + q];
+    }
+  }
+  __syncthreads();
+  double K[9], R[9], t[3];
+#pragma unroll
+  for (int q = 0; q < 9; ++q) {
+    K[q] = cam.K[q];
+    R[q] = s_pose[q];
+  }
+#pragma unroll
+  for (int q = 0; q < 3; ++q) t[q] = s_pose[9 + q];
+  const double* Ms = MsAll + 3 * cam.off;
+  const double* ms = msAll + 2 * cam.off;
+  for (int i = threadIdx.x; i < n; i += RANSAC_SEL_THREADS) {
+    bool f;
+    double e2;
+    ransac_point(K, R, t, Ms + 3 * i, ms + 2 * i, thr, f, e2);
+    inl[cam.off + i] = f ? 1 : 0;
+  }
+}
+
 
 // Checks of one solve's inputs shared by the batch call and cosl_pose_solver_submit; *tot = points over all
 // cameras.
@@ -1753,6 +2394,23 @@ struct cosl_pose_solver {
   long long nmap = 0;     // map points of that submit
   int nblk = 0;           // CTAs of its pose_mappt_kernel
   double gate = 0;
+  // PnP RANSAC (cosl_pose_solver_set_ransac): the armed setting (rC = 0: disarmed), its buffers, allocated by
+  // set_ransac for rCap hypotheses per camera and laid out as hyp[maxCams][rCap][RANSAC_HYP], smp[maxCams][rCap][5],
+  // cnt and sse[maxCams][rCap + 1], and the results res[C][RANSAC_RES] | inl[tot], copied back in one piece
+  int rC = 0, rHyp = 0, rMinInl = 0, rCap = 0;
+  double rThr = 0;
+  unsigned long long rSeed = 0;
+  unsigned char* d_ruse = nullptr;
+  double* d_rhyp = nullptr;
+  int* d_rsmp = nullptr;
+  int* d_rcnt = nullptr;
+  double* d_rsse = nullptr;
+  unsigned char* d_rres = nullptr;
+  unsigned char* h_rres = nullptr;
+  bool ransac = false;       // the solve in flight runs RANSAC
+  bool ransacReady = false;  // the last submit ran it
+  bool ransacHyps = false;   // the hypothesis buffers still hold the last submit's
+  int rHypRun = 0;           // nHyp of the last submit that ran it
 };
 
 namespace {
@@ -1793,6 +2451,13 @@ void free_pose_solver(cosl_pose_solver* s) {
   cudaFree(s->d_out);
   cudaFree(s->d_cov);
   cudaFree(s->d_mres);
+  if (s->h_rres) cudaFreeHost(s->h_rres);
+  cudaFree(s->d_ruse);
+  cudaFree(s->d_rhyp);
+  cudaFree(s->d_rsmp);
+  cudaFree(s->d_rcnt);
+  cudaFree(s->d_rsse);
+  cudaFree(s->d_rres);
   delete s;
 }
 
@@ -1816,6 +2481,30 @@ constexpr auto pose_intracam_obscov_prior = pose_intracam_kernel<true, true, Pos
 constexpr auto pose_cov_prior = pose_cov_kernel<false, true, PosePriorDev>;
 constexpr auto pose_cov_obscov_prior = pose_cov_kernel<true, true, const double*, PosePriorDev>;
 
+size_t ransac_res_bytes(int C, long long tot) { return sizeof(double) * RANSAC_RES * C + tot; }
+size_t ransac_hyp_smem() { return sizeof(double) * RS_N * RANSAC_HYP_THREADS; }
+
+// PnP RANSAC of the armed cameras on the staged inputs: hypotheses, scores, selection (which rewrites the records'
+// R0, t0 it replaces), and the results' read-back.  Enqueued after the inputs' copy and before the solve.
+int enqueue_ransac(cosl_pose_solver* s, int C, long long tot, const double* d_M, const double* d_m) {
+  PoseCam* d_cams = reinterpret_cast<PoseCam*>(s->d_in);
+  cudaStream_t st = s->rq.stream;
+  const int nh = s->rHyp;
+  double* d_res = reinterpret_cast<double*>(s->d_rres);
+  unsigned char* d_inl = s->d_rres + sizeof(double) * RANSAC_RES * C;
+  COSL_LAUNCH(ransac_hyp_kernel, dim3((nh + RANSAC_HYP_THREADS - 1) / RANSAC_HYP_THREADS, C), RANSAC_HYP_THREADS,
+              ransac_hyp_smem(), st, d_cams, d_M, d_m, s->d_ruse, nh, s->rSeed, s->d_rhyp, s->d_rsmp);
+  COSL_CUDA(cudaGetLastError());
+  COSL_LAUNCH(ransac_score_kernel, dim3(nh / RANSAC_SCORE_THREADS + 1, C), RANSAC_SCORE_THREADS, 0, st, d_cams, d_M,
+              d_m, s->d_ruse, nh, s->d_rhyp, s->rThr, s->d_rcnt, s->d_rsse);
+  COSL_CUDA(cudaGetLastError());
+  COSL_LAUNCH(ransac_select_kernel, C, RANSAC_SEL_THREADS, 0, st, d_cams, d_M, d_m, s->d_ruse, nh, s->d_rhyp,
+              s->d_rcnt, s->d_rsse, s->rThr, s->rMinInl, d_res, d_inl);
+  COSL_CUDA(cudaGetLastError());
+  COSL_CUDA(cudaMemcpyAsync(s->h_rres, s->d_rres, ransac_res_bytes(C, tot), cudaMemcpyDeviceToHost, st));
+  return COSL_OK;
+}
+
 // The staged inputs of C cameras and tot points: copy, kernel, read-back.  s->obsCov selects the whitened
 // instantiations and copies the factors with the rest; s->prior the PRIOR instantiations and the prior records.
 int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg) {
@@ -1832,6 +2521,7 @@ int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg)
   const size_t moff = mappt_offset(C, tot, s->obsCov, s->prior);
   const size_t bytes = s->map ? moff + mappt_bytes(s->nmap, s->nblk) : s->prior ? poff + prior_bytes(C) : poff;
   COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, bytes, cudaMemcpyHostToDevice, st));
+  if (s->ransac) COSL_TRY(enqueue_ransac(s, C, tot, d_M, d_m));
   if (s->prior && s->obsCov)
     COSL_LAUNCH(pose_intracam_obscov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg,
                 s->d_out, d_L, pr);
@@ -1889,6 +2579,8 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   if (C > s->maxCams)
     return set_error(COSL_E_INVALID, "%s: %d cameras exceed the handle's %d", fn, C, s->maxCams);
   long long tot = 0;
+  if (s->rC > 0 && C != s->rC)
+    return set_error(COSL_E_INVALID, "%s: %d cameras, but RANSAC is armed for %d (set_ransac)", fn, C, s->rC);
   COSL_TRY(check_cameras(fn, C, npts, Ms, ms, opts, &tot));
   if (tot > s->maxPts)
     return set_error(COSL_E_INVALID, "%s: %lld points exceed the handle's %d", fn, tot, s->maxPts);
@@ -1994,9 +2686,16 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   s->nmap = nmap;
   s->nblk = nblk;
   s->gate = mp ? mp->gate : 0.0;
+  s->ransac = s->rC > 0;
+  s->ransacReady = false;
+  if (s->ransac) {
+    s->ransacHyps = true;
+    s->rHypRun = s->rHyp;
+  }
   COSL_TRY(s->rq.submit(fn, [&]() { return enqueue_solve(s, C, tot, cfg); }));
   s->covReady = s->pixelVar > 0;
   s->mapReady = s->map;
+  s->ransacReady = s->ransac;
   return COSL_OK;
 }
 
@@ -2573,6 +3272,124 @@ int cosl_pose_solver_download_mappts(cosl_pose_solver* s, double* X, double* P, 
     if (stat) std::memcpy(stat + 3 * j, r + 9, sizeof(double) * 3);
     if (status) status[j] = (int)r[12];
   }
+  return COSL_OK;
+}
+
+int cosl_pose_solver_set_ransac(cosl_pose_solver* s, int C, const uint8_t* use, int nHyp, double err_thres,
+                                int min_inliers, uint64_t seed) {
+  static const char* fn = "cosl_pose_solver_set_ransac";
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  COSL_TRY(s->rq.idle(fn));
+  if (!use) {
+    s->rC = 0;
+    return COSL_OK;
+  }
+  if (C < 1 || C > s->maxCams)
+    return set_error(COSL_E_INVALID, "%s: %d cameras, the handle takes 1 to %d", fn, C, s->maxCams);
+  if (nHyp < 1 || nHyp > (1 << 20)) return set_error(COSL_E_INVALID, "%s: nHyp %d is not in [1, 2^20]", fn, nHyp);
+  if (!std::isfinite(err_thres) || !(err_thres > 0))
+    return set_error(COSL_E_INVALID, "%s: err_thres %g is not a finite value > 0", fn, err_thres);
+  if (min_inliers < 5) return set_error(COSL_E_INVALID, "%s: min_inliers %d < 5", fn, min_inliers);
+  COSL_CUDA(cudaSetDevice(s->device));
+  if (!s->d_rres) {  // the first arming: all of it or nothing, as below
+    COSL_CUDA(cudaFuncSetAttribute(ransac_hyp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)ransac_hyp_smem()));
+    const size_t nres = ransac_res_bytes(s->maxCams, s->maxPts);
+    unsigned char *ruse = nullptr, *h_res = nullptr, *d_res = nullptr;
+    cudaError_t e = cudaMalloc(&ruse, s->maxCams);
+    if (e == cudaSuccess) e = cudaHostAlloc(&h_res, nres, cudaHostAllocPortable);
+    if (e == cudaSuccess) e = cudaMalloc(&d_res, nres);
+    if (e != cudaSuccess) {
+      cudaFree(ruse);
+      if (h_res) cudaFreeHost(h_res);
+      cudaFree(d_res);
+      return set_error(COSL_E_NOMEM, "%s: result buffers for %d cameras and %d points: %s", fn, s->maxCams,
+                       s->maxPts, cudaGetErrorString(e));
+    }
+    s->d_ruse = ruse;
+    s->h_rres = h_res;
+    s->d_rres = d_res;
+  }
+  if (nHyp > s->rCap) {  // the new buffers first, so a failed allocation leaves the handle as it was
+    const size_t nc = (size_t)s->maxCams;
+    double *hyp = nullptr, *sse = nullptr;
+    int *smp = nullptr, *cnt = nullptr;
+    cudaError_t e = cudaMalloc(&hyp, sizeof(double) * RANSAC_HYP * nc * nHyp);
+    if (e == cudaSuccess) e = cudaMalloc(&smp, sizeof(int) * 5 * nc * nHyp);
+    if (e == cudaSuccess) e = cudaMalloc(&cnt, sizeof(int) * nc * (nHyp + 1));
+    if (e == cudaSuccess) e = cudaMalloc(&sse, sizeof(double) * nc * (nHyp + 1));
+    if (e != cudaSuccess) {
+      cudaFree(hyp);
+      cudaFree(smp);
+      cudaFree(cnt);
+      cudaFree(sse);
+      return set_error(COSL_E_NOMEM, "%s: %d hypotheses for %d cameras: %s", fn, nHyp, s->maxCams,
+                       cudaGetErrorString(e));
+    }
+    cudaFree(s->d_rhyp);
+    cudaFree(s->d_rsmp);
+    cudaFree(s->d_rcnt);
+    cudaFree(s->d_rsse);
+    s->d_rhyp = hyp;
+    s->d_rsmp = smp;
+    s->d_rcnt = cnt;
+    s->d_rsse = sse;
+    s->rCap = nHyp;
+    s->ransacHyps = false;
+  }
+  COSL_CUDA(cudaMemcpyAsync(s->d_ruse, use, C, cudaMemcpyHostToDevice, s->rq.stream));
+  COSL_CUDA(cudaStreamSynchronize(s->rq.stream));
+  s->rC = C;
+  s->rHyp = nHyp;
+  s->rThr = err_thres;
+  s->rMinInl = min_inliers;
+  s->rSeed = seed;
+  return COSL_OK;
+}
+
+int cosl_pose_solver_download_ransac(cosl_pose_solver* s, double* R, double* t, double* stat, uint8_t* inl) {
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  COSL_TRY(s->rq.idle("cosl_pose_solver_download_ransac"));
+  if (!s->ransacReady)
+    return set_error(COSL_E_STATE, "cosl_pose_solver_download_ransac: the last submit did not run RANSAC");
+  const double* res = reinterpret_cast<const double*>(s->h_rres);
+  for (int c = 0; c < s->C; ++c) {
+    const double* r = res + RANSAC_RES * c;
+    if (R) std::memcpy(R + 9 * c, r, sizeof(double) * 9);
+    if (t) std::memcpy(t + 3 * c, r + 9, sizeof(double) * 3);
+    if (stat) std::memcpy(stat + 4 * c, r + 12, sizeof(double) * 4);
+  }
+  if (inl) std::memcpy(inl, s->h_rres + sizeof(double) * RANSAC_RES * s->C, s->tot);
+  return COSL_OK;
+}
+
+int cosl_pose_solver_download_ransac_hyps(cosl_pose_solver* s, int maxHyp, int* nHyp, int* idx, double* pose,
+                                          int* inliers, double* sse) {
+  static const char* fn = "cosl_pose_solver_download_ransac_hyps";
+  if (!s) return set_error(COSL_E_INVALID, "null pose solver handle");
+  COSL_TRY(s->rq.idle(fn));
+  if (!s->ransacReady || !s->ransacHyps)
+    return set_error(COSL_E_STATE, "%s: the buffers do not hold the last submit's hypotheses", fn);
+  const int nh = s->rHypRun;
+  if (nHyp) *nHyp = nh;
+  if (!idx && !pose && !inliers && !sse) return COSL_OK;
+  if (maxHyp < nh)
+    return set_error(COSL_E_INVALID, "%s: room for %d hypotheses per camera, the last submit drew %d", fn, maxHyp, nh);
+  COSL_CUDA(cudaSetDevice(s->device));
+  const size_t C = s->C, cap = (size_t)maxHyp, n = (size_t)nh;
+  if (idx)
+    COSL_CUDA(cudaMemcpy2D(idx, sizeof(int) * 5 * cap, s->d_rsmp, sizeof(int) * 5 * n, sizeof(int) * 5 * n, C,
+                           cudaMemcpyDeviceToHost));
+  if (pose)
+    for (size_t c = 0; c < C; ++c)
+      COSL_CUDA(cudaMemcpy2D(pose + 12 * cap * c, sizeof(double) * 12, s->d_rhyp + RANSAC_HYP * n * c,
+                             sizeof(double) * RANSAC_HYP, sizeof(double) * 12, n, cudaMemcpyDeviceToHost));
+  if (inliers)
+    COSL_CUDA(cudaMemcpy2D(inliers, sizeof(int) * cap, s->d_rcnt + 1, sizeof(int) * (n + 1), sizeof(int) * n, C,
+                           cudaMemcpyDeviceToHost));
+  if (sse)
+    COSL_CUDA(cudaMemcpy2D(sse, sizeof(double) * cap, s->d_rsse + 1, sizeof(double) * (n + 1), sizeof(double) * n, C,
+                           cudaMemcpyDeviceToHost));
   return COSL_OK;
 }
 

@@ -548,6 +548,45 @@ int cosl_pose_solver_submit_mappts(cosl_pose_solver* s, int C, const double* K9,
  * stat[3 n] = {d2_0, d2_1, e0} and status[n]; every output nullable.  COSL_E_STATE while a solve is in
  * flight, or when the last submit was not a submit_mappts. */
 int cosl_pose_solver_download_mappts(cosl_pose_solver* s, double* X, double* P, double* stat, int* status);
+/* PnP RANSAC before the solve (an extension: a robust start where R0, t0 is poor, after solvePnPRobust's EPnP-then-
+ * refine pattern; DESIGN.md 5.7).  use[c] != 0 selects camera c of the C cameras of every later submit, of every
+ * kind, until the next call; use == NULL disarms.  Per selected camera with n = npts[c] points, in fp64 on the
+ * handle's stream between the inputs' copy and the solve:
+ *   samples: hypothesis h in [0, nHyp) takes the first 5 distinct idx = u_j mod n of u_j = splitmix64(seed ^
+ *   ((c << 40) | (h << 8) | j)), j = 0 .. 255 (splitmix64(x): z = x + 0x9e3779b97f4a7c15, then the standard
+ *   SplitMix64 finaliser); none within 256 draws is degenerate;
+ *   EPnP (Lepetit et al. 2009) on the 5 points: PCA control points (degenerate when the smallest eigenvalue is below
+ *   1e-12 of the largest), the 12x12 M^T M by cyclic Jacobi, betas for N = 1, 2, 3 each refined by 5 Gauss-Newton
+ *   steps, absolute orientation with the reflection fix, and of the three the least summed reprojection error over
+ *   the sample; a non-finite value is degenerate;
+ *   score: point i is an inlier of (R, t) when its depth (R M_i + t)_z > 0 and |m_i - pi(K, R, t, M_i)| < err_thres
+ *   (px, Euclidean); a hypothesis scores (inliers, sum over inliers of |e|^2), a degenerate one (-1, 0); covx,
+ *   prevErrs and priors do not enter;
+ *   select: most inliers, then least sum, then lowest h; the caller's R0, t0 is scored as h = -1 and wins ties.
+ * The status of camera c, tested in this order: 3 not selected; 1 n < 5, no hypotheses drawn; 4 R0, t0 kept, no
+ * hypothesis beat it; 2 the best hypothesis has fewer than min_inliers inliers, R0, t0 kept; 0 the hypothesis
+ * replaced R0, t0.  The solve then starts from that pose and runs unchanged on the same points.  The result does not
+ * depend on thread order.  An unarmed handle launches exactly what it did before this call existed.
+ * Allocates the hypothesis buffers for nHyp x maxCams once (a later call with a larger nHyp reallocates); no submit
+ * allocates.  COSL_E_INVALID for a NULL handle, C not in [1, maxCams], nHyp not in [1, 2^20], err_thres not finite
+ * and > 0, or min_inliers < 5, keeping the old setting; COSL_E_STATE while a solve is in flight.  A later submit
+ * whose C differs from the armed C gives COSL_E_INVALID. */
+int cosl_pose_solver_set_ransac(cosl_pose_solver* s, int C, const uint8_t* use, int nHyp, double err_thres,
+                                int min_inliers, uint64_t seed);
+/* After collect of a submit that ran RANSAC, per camera: R[9] and t[3], the start pose the solve used; stat[4] =
+ * {status, inliers, sum |e|^2, h} of the selection's winner (R0, t0's with h = -1 for status 1, 3 and 4); and
+ * inl[tot], camera-major in submit order, 1 where the point is an inlier of the start pose.  Every output
+ * nullable.  COSL_E_STATE while a solve is in flight, or when the last submit did not run RANSAC. */
+int cosl_pose_solver_download_ransac(cosl_pose_solver* s, double* R, double* t, double* stat, uint8_t* inl);
+/* Diagnostics of the same submit, per camera and hypothesis.  *nHyp (nullable) gets the number of hypotheses that
+ * submit drew per camera.  The outputs have room for maxHyp hypotheses per camera, camera-major, and each camera's
+ * first *nHyp entries are written: idx[5] (-1 where none were drawn or 5 distinct were not found), pose[12] = R | t
+ * (unset when degenerate), inliers (-1 when degenerate or not drawn) and sse.  Every output nullable; with all four
+ * NULL the call only reports *nHyp.  COSL_E_INVALID when an output is given and maxHyp is below *nHyp, before
+ * anything is written; COSL_E_STATE as download_ransac, and also after a set_ransac that reallocated the hypothesis
+ * buffers.  A synchronous copy from the device. */
+int cosl_pose_solver_download_ransac_hyps(cosl_pose_solver* s, int maxHyp, int* nHyp, int* idx, double* pose,
+                                          int* inliers, double* sse);
 
 /* A triangulation handle: batched multi-view triangulation of map points with their 3x3 covariance (an
  * extension: the birth of a MapPoint's M and cov in SingleSLAM::newMapPoints, updateStaticPointPosition and
