@@ -111,7 +111,7 @@ struct cosl_klt {
   long long lvOff[8];
   long long pyrStride = 0;  // float4 elements per camera
   size_t imgPitch = 0, imgStride = 0;
-  int candCap = 0, smemKeys = 0;
+  int candCap = 0, smemKeys = 0, selectSmem = 0;  // selectSmem: klt_select_refill's dynamic shared memory
   // device memory
   uint8_t* d_img = nullptr;
   // Three pyramid buffers.  p0 holds the previous frame's pyramid (the tracker's P0) and p1 the
@@ -328,7 +328,12 @@ int alloc_group(cosl_klt* g) {
   int cap = 1024;
   while (cap < maxCand) cap <<= 1;
   g->candCap = cap;
-  g->smemKeys = std::min(cap, KLT_MAX_SMEM_KEYS);
+  // klt_select_refill keeps in shared memory the keys it sorts: every candidate for
+  // COSL_KLT_COMPAT_HISTOPYR, else at most one per slot
+  int slotKeys = 1;
+  while (slotKeys < F) slotKeys <<= 1;
+  g->smemKeys = std::min((g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? cap : slotKeys, KLT_MAX_SMEM_KEYS);
+  g->selectSmem = g->smemKeys * (int)sizeof(unsigned long long) + (int)sizeof(int) * div_up(F, 32);
   COSL_CUDA(cudaMalloc(&g->d_img, g->imgStride * C));
   std::fill(&g->lv0Stored[0][0], &g->lv0Stored[0][0] + 3 * 64, true);
   for (int b = 0; b < 3; ++b) {
@@ -445,9 +450,13 @@ int alloc_group(cosl_klt* g) {
   }
   // dynamic shared memory opt-in: the attribute belongs to the kernel, not to this group, so it is
   // the largest any group uses (a group created later must not lower it below an earlier one's)
-  for (const bool mixed : {false, true})
-    COSL_CUDA(cudaFuncSetAttribute(KLT_SIZED(mixed, klt_select_refill), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   KLT_MAX_SMEM_KEYS * (int)sizeof(unsigned long long)));
+  for (const bool mixed : {false, true}) {
+    cudaFuncAttributes fa;
+    COSL_CUDA(cudaFuncGetAttributes(&fa, KLT_SIZED(mixed, klt_select_refill)));
+    if (fa.maxDynamicSharedSizeBytes < g->selectSmem)
+      COSL_CUDA(cudaFuncSetAttribute(KLT_SIZED(mixed, klt_select_refill), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     g->selectSmem));
+  }
   COSL_TRY(update_cameras(g));
   g->secPyr = g->timer.section("klt_pyramid");
   g->secTrack = g->timer.section("klt_track");
@@ -826,15 +835,20 @@ int run_detector(cosl_klt* g, const FramePlan& p) {
   else
     launch_prefilter(g, g->stream, p.mixed, p.cams);
   dim3 gv(2 * g->numSM, g->C);
-  COSL_LAUNCH(KLT_SIZED(p.mixed, klt_nm_verify), gv, 256, 0, g->stream, corn, g->W, cs, p.cams, g->W, g->H, r,
-              g->d_prelim[g->par], g->prelimCap, g->d_cand, g->candCap, counters);
+  // Verify and select are programmatic dependent launches (both kernels wait before they read what the
+  // kernel ahead of them wrote).  The profile timer's events, when enabled, sit between the launches;
+  // disabled, it enqueues nothing.
+  COSL_LAUNCH_PDL(KLT_SIZED(p.mixed, klt_nm_verify), gv, dim3(256), 0, g->stream, (const float*)corn, g->W, cs,
+                  (const KltCam*)p.cams, g->W, g->H, r, (const unsigned*)g->d_prelim[g->par], g->prelimCap, g->d_cand,
+                  g->candCap, counters);
   g->timer.end(g->stream);
   g->timer.begin(g->secSelect, g->stream);
-  COSL_LAUNCH(KLT_SIZED(p.mixed, klt_select_refill), g->C, 1024, g->smemKeys * sizeof(unsigned long long), g->stream,
-              g->d_cand, g->candCap, g->plCap, counters, g->d_feat, g->d_dst,
-              p.foldAdvance ? g->d_src : (float4*)nullptr, g->d_present,
-              maxPresent > 0 ? g->d_nPresent : (const int*)nullptr, g->F, p.cams, g->W, g->H, mode,
-              g->cfg.trackWithGain ? 1 : 0, g->smemKeys, (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
+  COSL_LAUNCH_PDL(KLT_SIZED(p.mixed, klt_select_refill), dim3(g->C), dim3(1024), (size_t)g->selectSmem, g->stream,
+                  g->d_cand, g->candCap, g->plCap, counters, g->d_feat, g->d_dst,
+                  p.foldAdvance ? g->d_src : (float4*)nullptr, (const float4*)g->d_present,
+                  maxPresent > 0 ? (const int*)g->d_nPresent : (const int*)nullptr, g->F, (const KltCam*)p.cams, g->W,
+                  g->H, mode, g->cfg.trackWithGain ? 1 : 0, g->smemKeys,
+                  (g->cfg.compat & COSL_KLT_COMPAT_HISTOPYR) ? 1 : 0);
   g->timer.end(g->stream);
   COSL_CUDA(cudaGetLastError());
   return COSL_OK;

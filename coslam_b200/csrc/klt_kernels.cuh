@@ -396,6 +396,16 @@ klt_nm_verify(const float* __restrict__ corn, int pitch, long long cornStride,
     W = __ldg(&cams[cam].W);
     H = __ldg(&cams[cam].H);
   }
+  // Launched as a programmatic dependent of the kernel ahead of it on the group's stream: the
+  // prefilter on a detect frame, the tracker or klt_suppress on a re-detect frame.  Above, only the
+  // camera table is read, which work ahead of that kernel wrote.  The prelim list, its count and
+  // the cornerness map (its centre values and windows marked by the tracker) are read after the
+  // wait, which returns once that grid has completed and its stores are visible.  The trigger
+  // follows the wait, so klt_select_refill, which reads the tracker's feature table before its own
+  // wait, starts only after a wait here has returned.  A CTA of a camera outside the detector stage
+  // exits above, which counts as a trigger; its camera's select CTA exits before it reads anything.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   const float* cm = corn + (size_t)cam * cornStride;
   const int lane = threadIdx.x & 31;
   const int warp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -443,9 +453,93 @@ klt_nm_verify(const float* __restrict__ corn, int pitch, long long cornStride,
   }
 }
 
+constexpr int KLT_MAX_SMEM_KEYS = 16384;  // keys sorted in shared memory; more sort in global memory
+
+// Exclusive prefix over the block of v (one value per thread), and the block's sum in total.  s_w
+// holds 33 ints; it is free again when the call returns.
+__device__ __forceinline__ int klt_block_excl_scan(int v, int* s_w, int& total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) s_w[wid] = inc;
+  __syncthreads();
+  if (wid == 0) {
+    const int w = (lane < (int)(blockDim.x >> 5)) ? s_w[lane] : 0;
+    int wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += t;
+    }
+    s_w[lane] = wi - w;  // exclusive prefix of the warp totals
+    if (lane == 31) s_w[32] = wi;
+  }
+  __syncthreads();
+  const int r = s_w[wid] + inc - v;
+  total = s_w[32];
+  __syncthreads();
+  return r;
+}
+
+// The largest key T such that exactly k of the n distinct keys ck[0..n) are <= T (1 <= k < n): a
+// radix select from the most significant byte down.  Each pass histograms the byte below the prefix
+// found so far over the keys that carry that prefix; the bin holding the k-th key becomes the new
+// prefix, and the select ends at the first pass where the k-th key is the last of its bin, so T is the
+// largest key with that prefix.  The keys are distinct, so that happens at the last byte at the latest.
+// s_hist holds 256 ints, s_sel 3.
+__device__ __forceinline__ unsigned long long klt_select_threshold(const unsigned long long* __restrict__ ck, int n, int k,
+                                                   int* s_hist, int* s_sel) {
+  const int lane = threadIdx.x & 31;
+  unsigned long long prefix = 0, pmask = 0;
+  for (int shift = 56;; shift -= 8) {
+    if (threadIdx.x < 256) s_hist[threadIdx.x] = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const unsigned long long key = ck[i];
+      if ((key & pmask) == prefix) atomicAdd(&s_hist[(unsigned)(key >> shift) & 255u], 1);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {  // warp 0: lane l owns bins 8l .. 8l+7
+      int h[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        h[j] = s_hist[8 * lane + j];
+        sum += h[j];
+      }
+      int inc = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+      }
+      int before = inc - sum;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        if (before < k && k <= before + h[j]) {  // exactly one bin of one lane
+          s_sel[0] = 8 * lane + j;
+          s_sel[1] = k - before;
+          s_sel[2] = (k - before) == h[j];
+        }
+        before += h[j];
+      }
+    }
+    __syncthreads();
+    const int digit = s_sel[0], kr = s_sel[1], closes = s_sel[2];
+    prefix |= (unsigned long long)digit << shift;
+    pmask |= 0xffull << shift;
+    if (closes) return prefix | ~pmask;  // the k-th key is the last of its bin
+    k = kr;
+    // s_sel and s_hist are rewritten only after the next pass's first barrier
+  }
+}
+
 // ------------------------------------------------------------------------------------------
-// Single-CTA per camera: sort the candidate keys (bitonic, shared memory when they fit), then do
-// the slot logic of KLT_SequenceTracker::{detect, redetect} (v3d_gpuklt.cpp:651-805) on the device:
+// Single-CTA per camera: the strongest candidates in increasing key order, then the slot logic of
+// KLT_SequenceTracker::{detect, redetect} (v3d_gpuklt.cpp:651-805) on the device:
 //   mode 0 (detect):   slots [0, nDet) <- strongest corners, [nDet, nDet+nPresent) <- present pts
 //                      (nPresent = nPresentExt[cam], 0 when nPresentExt is null)
 //   mode 1 (redetect): dead slots, in increasing slot index, <- strongest corners
@@ -453,6 +547,15 @@ klt_nm_verify(const float* __restrict__ corn, int pitch, long long cornStride,
 //                      (cosl_klt_group_step; the cameras outside the detector stage exit)
 // and "provide" the new feature table (dst buffer).  counters[cam*8+2] = returned count
 // (nDetected / nNewFeatures as the reference defines them), [3] = raw candidate count.
+//
+// Only the first nSel = min(nCand, plCap, free slots) keys of the sorted list are used.  The keys
+// (~cornerness | y | x) are distinct, so those are one set in one order: a radix select finds the
+// nSel-th key, the keys at or below it are compacted into shared memory and only they are sorted
+// (bitonic, next_pow2(nSel) <= next_pow2(F) keys).  Only a group with more than KLT_MAX_SMEM_KEYS
+// slots can have more winners than shared memory holds; it sorts every key in global memory.
+// COSL_KLT_COMPAT_HISTOPYR needs the whole candidate list in Morton order and sorts all of it.
+//
+// Dynamic shared memory: smemKeys keys, then one int per 32 slots (the dead slots ahead of them).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void bitonic_sort(unsigned long long* k, int n2) {
   for (int size = 2; size <= n2; size <<= 1) {
@@ -493,10 +596,9 @@ __device__ __forceinline__ unsigned klt_compact1by1(unsigned v) {
   return v;
 }
 
-constexpr int KLT_MAX_SMEM_KEYS = 16384;  // keys sorted in shared memory; more sort in global memory
-
+// (1024, 1): with the block count left open ptxas kept the kernel at 32 registers, and it spilled
 template <bool MIXED>
-__global__ void __launch_bounds__(1024)
+__global__ void __launch_bounds__(1024, 1)
 klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
                   int* __restrict__ counters, cosl_klt_feature* __restrict__ dest,
                   float4* __restrict__ dstbuf, float4* __restrict__ alsoSrc,
@@ -504,40 +606,75 @@ klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
                   int F, const KltCam* __restrict__ cams, int W, int H, int mode, int withGain,
                   int smemKeys, int histo) {
   extern __shared__ unsigned long long s_keys[];
-  __shared__ int s_scan[1024];
-  __shared__ int s_base;
+  __shared__ int s_w[33];
+  __shared__ int s_hist[256];
+  __shared__ int s_sel[3];
+  __shared__ int s_nWin, s_nDead;
   const int cam = blockIdx.x;
   if (MIXED) {
     const int stages = __ldg(&cams[cam].stages);
     if (!(stages & KLT_STAGE_DETECT)) return;
     if (mode == 2) mode = (stages & KLT_STAGE_TRACK) ? 1 : 0;  // per camera: re-detect after a track
-    W = __ldg(&cams[cam].W);
-    H = __ldg(&cams[cam].H);
   }
-  const int nPresentExt = (mode == 0 && nPresentPer) ? nPresentPer[cam] : 0;
+  const int lane = threadIdx.x & 31;
+  cosl_klt_feature* d = dest + (size_t)cam * F;
+  int* s_dead = reinterpret_cast<int*>(s_keys + smemKeys);  // dead slots ahead of each 32-slot group
+  if (mode == 1) {
+    // Launched as a programmatic dependent of klt_nm_verify, whose CTAs trigger only after their own
+    // griddepcontrol.wait returned, i.e. after the grid ahead of verify completed.  That is the
+    // tracker (the fused gain tracker writes the feature table itself), klt_status or klt_suppress,
+    // each behind the table's last writer on the same stream, so the table read here is complete
+    // and visible.  Nothing this CTA reads or writes in global memory before its own wait is touched
+    // by verify.  This scan is what the refill would do after the wait: dead slots get ranks in
+    // increasing slot index.
+    const int nGroups = (F + 31) >> 5;
+    for (int gi = threadIdx.x >> 5; gi < nGroups; gi += blockDim.x >> 5) {
+      const int i = gi * 32 + lane;
+      const unsigned bal = __ballot_sync(0xffffffffu, i < F && d[i].status < 0);
+      if (lane == 0) s_dead[gi] = __popc(bal);
+    }
+    __syncthreads();
+    int nDead = 0;
+    for (int s = 0; s < nGroups; s += blockDim.x) {
+      const int gi = s + threadIdx.x;
+      int tot;
+      const int ex = klt_block_excl_scan(gi < nGroups ? s_dead[gi] : 0, s_w, tot);
+      if (gi < nGroups) s_dead[gi] = nDead + ex;
+      nDead += tot;
+    }
+    if (threadIdx.x == 0) s_nDead = nDead;  // read by the same thread after the wait
+  }
+  // Everything below reads what verify (the candidate keys and their count) or the work ahead of it
+  // wrote.  Triggering after the wait lets the stream's next kernel, if it is a programmatic launch,
+  // be placed while this one runs; it waits for this grid to complete before it reads.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   int* cnt = counters + cam * 8;
   unsigned long long* ck = cand + (size_t)cam * candCap;
-  const int nCandRaw = cnt[1];
-  const int nCand = min(nCandRaw, candCap);
-  int n2 = 1;
-  while (n2 < nCand) n2 <<= 1;
-  unsigned long long* keys;
-  if (n2 <= smemKeys) {
-    keys = s_keys;
-    for (int i = threadIdx.x; i < n2; i += blockDim.x) keys[i] = (i < nCand) ? ck[i] : ~0ull;
-  } else {
-    keys = ck;  // sort in place in global memory (candCap is a power of two >= n2)
-    for (int i = nCand + threadIdx.x; i < n2; i += blockDim.x) keys[i] = ~0ull;
-  }
-  __syncthreads();
-  int nCandEff = nCand;
-  bool wantSort = true;
+  const int nCand = min(cnt[1], candCap);
+  // the present counts are read again after the selection, so that they are not live across it
+  const int freeSlots = F - ((mode == 0) ? (nPresentPer ? nPresentPer[cam] : 0) : cnt[0]);
+  unsigned long long* keys = s_keys;
+  int nSel;
   if (histo) {
     // COSL_KLT_COMPAT_HISTOPYR: the reference's candidate list.  (1) the discriminator pass covers W/2 x H/2
     // texels of 2x2 pixels (v3d_gpuklt.cpp:519-523): a last odd row / column is never seen; (2) the first
     // plCap candidates in HistoPyramid extraction order (= Morton order) are read back (:752-757);
     // (3) only if they exceed the free slots they are ordered by cornerness (:759-768), else they fill
     // the slots in extraction order.
+    if (MIXED) {
+      W = __ldg(&cams[cam].W);
+      H = __ldg(&cams[cam].H);
+    }
+    int n2 = 1;
+    while (n2 < nCand) n2 <<= 1;
+    if (n2 <= smemKeys) {
+      for (int i = threadIdx.x; i < n2; i += blockDim.x) keys[i] = (i < nCand) ? ck[i] : ~0ull;
+    } else {
+      keys = ck;  // sort in place in global memory (candCap is a power of two >= n2)
+      for (int i = nCand + threadIdx.x; i < n2; i += blockDim.x) keys[i] = ~0ull;
+    }
+    __syncthreads();
     __shared__ int s_nvalid;
     const unsigned Wc = 2u * (unsigned)(W / 2), Hc = 2u * (unsigned)(H / 2);
     if (threadIdx.x == 0) s_nvalid = 0;
@@ -557,9 +694,8 @@ klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
     for (int i = threadIdx.x; i < n2; i += blockDim.x)
       if (keys[i] != ~0ull && (i + 1 == n2 || keys[i + 1] == ~0ull)) s_nvalid = i + 1;
     __syncthreads();
-    nCandEff = min(s_nvalid, plCap);
-    const int freeSlots = (mode == 0) ? F - nPresentExt : F - cnt[0];
-    wantSort = nCandEff > freeSlots;
+    const int nCandEff = min(s_nvalid, plCap);
+    const bool wantSort = nCandEff > freeSlots;
     for (int i = threadIdx.x; i < n2; i += blockDim.x) {
       unsigned long long k = keys[i];
       if (i < nCandEff) {
@@ -572,14 +708,58 @@ klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
       keys[i] = k;
     }
     __syncthreads();
+    if (nCand > 1 && wantSort) bitonic_sort(keys, n2);
+    nSel = max(0, min(nCandEff, freeSlots));
+  } else {
+    nSel = max(0, min(min(nCand, plCap), freeSlots));
+    int n2 = 1;
+    while (n2 < nSel) n2 <<= 1;
+    if (n2 <= smemKeys) {
+      if (nSel > 0) {
+        const unsigned long long T = (nSel < nCand) ? klt_select_threshold(ck, nCand, nSel, s_hist, s_sel) : ~0ull;
+        if (threadIdx.x == 0) s_nWin = 0;
+        __syncthreads();
+        // exactly nSel keys are <= T; one shared-memory atomic per warp and round
+        for (int s = 0; s < nCand; s += blockDim.x) {
+          const int i = s + threadIdx.x;
+          const unsigned long long key = (i < nCand) ? ck[i] : ~0ull;
+          const bool win = (i < nCand) && key <= T;
+          const unsigned bal = __ballot_sync(0xffffffffu, win);
+          int base = 0;
+          if (lane == 0 && bal) base = atomicAdd(&s_nWin, __popc(bal));
+          base = __shfl_sync(0xffffffffu, base, 0);
+          if (win) keys[base + __popc(bal & ((1u << lane) - 1))] = key;
+        }
+      }
+      for (int i = nSel + threadIdx.x; i < n2; i += blockDim.x) keys[i] = ~0ull;
+      __syncthreads();
+      if (nSel > 1) bitonic_sort(keys, n2);
+    } else {
+      // more winners than shared memory holds (more than KLT_MAX_SMEM_KEYS slots): sort every key in place
+      n2 = 1;
+      while (n2 < nCand) n2 <<= 1;
+      keys = ck;
+      for (int i = nCand + threadIdx.x; i < n2; i += blockDim.x) keys[i] = ~0ull;
+      __syncthreads();
+      if (nCand > 1) bitonic_sort(keys, n2);
+    }
   }
-  if (nCand > 1 && wantSort) bitonic_sort(keys, n2);
+  const int nPresentExt = (mode == 0 && nPresentPer) ? nPresentPer[cam] : 0;
+  // written ahead of the refill so that no count stays live across it
+  if (threadIdx.x == 0) {
+    const int nCandRaw = cnt[1];
+    cnt[2] = (mode == 0) ? nSel + nPresentExt : min(nSel, s_nDead) + cnt[0];
+    cnt[3] = nCandRaw;
+  }
+  if (MIXED) {  // read here rather than at the top, so that they are not live across the selection
+    W = __ldg(&cams[cam].W);
+    H = __ldg(&cams[cam].H);
+  }
   const float Wf = (float)W, Hf = (float)H;
-  cosl_klt_feature* d = dest + (size_t)cam * F;
   float4* pb = dstbuf + (size_t)cam * F;
   float4* ps = alsoSrc ? alsoSrc + (size_t)cam * F : nullptr;  // advanceFrame copy folded in
   if (mode == 0) {
-    const int nDet = max(0, min(min(nCandEff, plCap), F - nPresentExt));
+    const int nDet = nSel;
     for (int i = threadIdx.x; i < F; i += blockDim.x) {
       cosl_klt_feature f;
       float4 p;
@@ -612,41 +792,19 @@ klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
       pb[i] = p;
       if (ps) ps[i] = p;
     }
-    if (threadIdx.x == 0) {
-      cnt[2] = nDet + nPresentExt;
-      cnt[3] = nCandRaw;
-    }
   } else {
-    const int nPresent = cnt[0];
-    const int nNew = max(0, min(min(nCandEff, plCap), F - nPresent));
-    if (threadIdx.x == 0) s_base = 0;
-    __syncthreads();
-    // dead slots in increasing index get corner k = rank among dead slots
-    for (int start = 0; start < F; start += blockDim.x) {
-      const int i = start + threadIdx.x;
+    const int nNew = nSel;
+    // dead slot i gets corner k = its rank among the dead slots (the scan before the wait); a warp
+    // covers one 32-slot group per round (blockDim.x is a multiple of 32), so the round's ballot
+    // gives the rank within the group
+    for (int s = 0; s < F; s += blockDim.x) {
+      const int i = s + threadIdx.x;
       const bool dead = (i < F) && (d[i].status < 0);
-      // block-wide exclusive scan of `dead`
       const unsigned bal = __ballot_sync(0xffffffffu, dead);
-      const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-      const int inwarp = __popc(bal & ((1u << lane) - 1));
-      if (lane == 0) s_scan[wid] = __popc(bal);
-      __syncthreads();
-      if (wid == 0) {
-        int v = (lane < (int)(blockDim.x >> 5)) ? s_scan[lane] : 0;
-        int inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int t = __shfl_up_sync(0xffffffffu, inc, o);
-          if (lane >= o) inc += t;
-        }
-        s_scan[lane] = inc - v;                  // exclusive prefix of warp totals
-        if (lane == 31) s_scan[32] = inc;        // block total
-      }
-      __syncthreads();
-      const int rank = s_base + s_scan[wid] + inwarp;
       if (i < F) {
         float4 p;
         if (dead) {
+          const int rank = s_dead[i >> 5] + __popc(bal & ((1u << lane) - 1));
           if (rank < nNew) {
             const unsigned long long key = keys[rank];
             const float c = __uint_as_float(~(unsigned)(key >> 32));
@@ -669,13 +827,6 @@ klt_select_refill(unsigned long long* __restrict__ cand, int candCap, int plCap,
         pb[i] = p;
         if (ps) ps[i] = p;
       }
-      __syncthreads();
-      if (threadIdx.x == 0) s_base += s_scan[32];
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-      cnt[2] = min(nNew, s_base) + nPresent;
-      cnt[3] = nCandRaw;
     }
   }
 }
