@@ -65,6 +65,16 @@ extern std::atomic<uint64_t> g_launches;
 inline int div_up(int a, int b) { return (a + b - 1) / b; }
 inline int64_t div_up64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// aligned bump layout of one device block (the same offsets index its host image)
+struct SlabLayout {
+  size_t bytes = 0;
+  size_t take(size_t n) {
+    const size_t at = (bytes + 255) & ~(size_t)255;
+    bytes = at + n;
+    return at;
+  }
+};
+
 // COSL_E_CUDA unless `device` is the ordinal of a visible CUDA device.
 int check_device(int device);
 

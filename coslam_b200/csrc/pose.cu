@@ -17,6 +17,9 @@
 // projection, Jacobians and 3x3 Cholesky.
 // A registration handle (cosl_assoc_solver, also an extension) bins each entry's features into a uniform grid and
 // runs one search thread per (map point, camera entry) pair on the same projection and Jacobians.
+// Each handle stages a submit's inputs in one pinned buffer of 256-byte-aligned SlabLayout sections, placed by one
+// layout function per handle (pose_layout, tri_layout, assoc_layout) whose offsets index the host buffer and its
+// device copy alike and, at the handle's maxima, size both.
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -169,23 +172,13 @@ __device__ __forceinline__ void whiten(const double* L, double& r0, double& r1) 
 
 // Gaussian pose priors (cosl_pose_solver_submit_prior, DESIGN.md 5.3).  Camera c has a prior when has[c] != 0; its
 // record is rec[c] = [L (21: the upper-triangular 6x6 factor with L^T L = P^-1, packed by rows) | R_p (9, row-major) |
-// t_p (3)], staged by the host.  The records reach the PRIOR instantiations as a trailing argument of their own, so
-// the other instantiations keep their parameter lists and code.
+// t_p (3)], staged by the host.  Every instantiation of both pose kernels takes the records as its last parameter;
+// only the PRIOR ones read them.
 struct PosePriorDev {
   const double* rec;  // [C][POSE_PRIOR_REC]
   const int* has;     // [C]
 };
 constexpr int POSE_PRIOR_REC = 33;
-
-// The trailing arguments of a launch: the factors of an OBSCOV launch (const double*), then the priors of a PRIOR one.
-__device__ __forceinline__ const double* factors_arg() { return nullptr; }
-__device__ __forceinline__ const double* factors_arg(const double* L) { return L; }
-__device__ __forceinline__ const double* factors_arg(PosePriorDev) { return nullptr; }
-__device__ __forceinline__ const double* factors_arg(const double* L, PosePriorDev) { return L; }
-__device__ __forceinline__ PosePriorDev prior_arg() { return PosePriorDev{nullptr, nullptr}; }
-__device__ __forceinline__ PosePriorDev prior_arg(const double*) { return PosePriorDev{nullptr, nullptr}; }
-__device__ __forceinline__ PosePriorDev prior_arg(PosePriorDev p) { return p; }
-__device__ __forceinline__ PosePriorDev prior_arg(const double*, PosePriorDev p) { return p; }
 
 // This CTA's prior record, or nullptr for a camera without a prior (uniform over the CTA)
 __device__ __forceinline__ const double* prior_record(const PosePriorDev& pr) {
@@ -391,18 +384,17 @@ __device__ void weighted_step(const double K[9], const double R[9], const double
 
 // OBSCOV: every residual and Jacobian row is whitened by the factors LAll (3 per point, packed as the points;
 // cosl_pose_solver_submit_cov).  The false instantiation never reads LAll and is the unweighted solve.
-// PRIOR (cosl_pose_solver_submit_prior): the one trailing argument holds the priors; a camera with one adds its
-// |L r|^2 to every cost and its rows to every LM step, a camera without one computes what the launch without PRIOR
-// computes.
-template <bool OBSCOV, bool PRIOR = false, typename... Priors>
+// PRIOR (cosl_pose_solver_submit_prior): a camera with a prior in `prior` adds its |L r|^2 to every cost and its rows
+// to every LM step, a camera without one computes what the launch without PRIOR computes.  The false instantiation
+// never reads `prior`.
+template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(POSE_THREADS)
 pose_intracam_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
                      const double* __restrict__ msAll, const double* __restrict__ prevAll,
                      double* __restrict__ WsAll, PoseCfg cfg, PoseOut* __restrict__ outs,
-                     const double* __restrict__ LAll, Priors... prior) {
-  static_assert(sizeof...(Priors) == (PRIOR ? 1 : 0), "a PRIOR launch passes the priors, no other does");
+                     const double* __restrict__ LAll, PosePriorDev prior) {
   __shared__ double s_red[(POSE_THREADS / 32) * 27];
-  const double* Pq = PRIOR ? prior_record(prior_arg(prior...)) : nullptr;
+  const double* Pq = PRIOR ? prior_record(prior) : nullptr;
   const PoseCam cam = cams[blockIdx.x];
   const int n = cam.npts;
   const double* Ms = MsAll + 3 * cam.off;
@@ -555,17 +547,15 @@ constexpr int POSE_COV_STRIDE = 40;
 // below 1e-12 gives a NaN covariance and valid = 0.  errAll gets e_i of every point, in the packed order.
 // OBSCOV (cosl_pose_solver_submit_cov) whitens by the factors L_i of LAll: H = sum_i w_i (L_i J_i)^T (L_i J_i) and
 // sigma2_hat = sum w |L_i (project - m_i)|^2 / dof; e_i and w_i stay on the pixel distance.
-// The factors travel as a trailing argument of the OBSCOV launch only: the unweighted kernel keeps the parameter
-// list it had before measurement covariances, and with it its code (an unused parameter changes its registers).
-// PRIOR (cosl_pose_solver_submit_prior): the priors follow as the last trailing argument.  A camera with a prior adds
-// (L J_p)^T (L J_p) to H and |L r|^2 to sigma2_hat's numerator at (R_opt, t_opt), and 6 to dof.
-template <bool OBSCOV, bool PRIOR = false, typename... Extra>
+// PRIOR (cosl_pose_solver_submit_prior): a camera with a prior in `prior` adds (L J_p)^T (L J_p) to H and |L r|^2 to
+// sigma2_hat's numerator at (R_opt, t_opt), and 6 to dof.
+// Every instantiation takes both LAll and `prior`; the false ones never read them.  LAll is not __restrict__: that
+// turns its loads into constant-cache loads and changes the OBSCOV instantiation's code.
+template <bool OBSCOV, bool PRIOR>
 __global__ void __launch_bounds__(POSE_THREADS)
 pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsAll,
                 const double* __restrict__ msAll, const PoseOut* __restrict__ outs, double tau, double pixel_var,
-                double* __restrict__ res, double* __restrict__ errAll, Extra... LAll) {
-  static_assert(sizeof...(Extra) == (OBSCOV ? 1 : 0) + (PRIOR ? 1 : 0),
-                "an OBSCOV launch passes the factors and a PRIOR launch the priors, no other does");
+                double* __restrict__ res, double* __restrict__ errAll, const double* LAll, PosePriorDev prior) {
   __shared__ double s_red[(POSE_THREADS / 32) * 23];
   const PoseCam& cam = cams[blockIdx.x];
   const int n = cam.npts;
@@ -613,7 +603,7 @@ pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsA
       }
       double ew = 0;  // |L (project - m)|, which is e bit for bit when L = I
       if (OBSCOV) {
-        const double* L = factors_arg(LAll...) + 3 * (cam.off + i);
+        const double* L = LAll + 3 * (cam.off + i);
         double r0 = dx, r1 = dy;
         whiten(L, r0, r1);
         ew = sqrt(r0 * r0 + r1 * r1);
@@ -633,7 +623,7 @@ pose_cov_kernel(const PoseCam* __restrict__ cams, const double* __restrict__ MsA
   block_sum<23>(acc, s_red);
   if (threadIdx.x != 0) return;
   if constexpr (PRIOR) {  // discarded without PRIOR, so the other instantiations keep their code
-    const double* Pq = prior_record(prior_arg(LAll...));
+    const double* Pq = prior_record(prior);
     if (Pq) {
       double hb[27];  // the prior's 21 entries of H; its 6 right-hand-side entries are not needed here
 #pragma unroll
@@ -2192,6 +2182,14 @@ bool cov_factor(const double* c, double L[3]) {
   return std::isfinite(L[0]) && std::isfinite(L[1]) && std::isfinite(L[2]) && L[0] > 0 && L[2] > 0;
 }
 
+// A measurement covariance c (row-major 2x2, nullable) as staged for the devices: (xx, xy, yy), or pixel_var I when c
+// is nullptr.
+void pack_cov2(const double* c, double pixel_var, double out[3]) {
+  out[0] = c ? c[0] : pixel_var;
+  out[1] = c ? c[1] : 0.0;
+  out[2] = c ? c[3] : pixel_var;
+}
+
 // Checks every covariance of covx (nullable, as covx[c]) against cov_factor, naming the first bad one.
 int check_covx(const char* fn, int C, const int* npts, const double* const* covx) {
   if (!covx) return COSL_OK;
@@ -2228,6 +2226,12 @@ bool chol6(const double* A, double* G) {
   return true;
 }
 
+// S = 0.5 (P + P^T) of a 6x6 P (row-major)
+void sym6(const double* P, double S[36]) {
+  for (int a = 0; a < 6; ++a)
+    for (int b = 0; b < 6; ++b) S[6 * a + b] = 0.5 * (P[6 * a + b] + P[6 * b + a]);
+}
+
 // Checks camera c's prior record p (R_p[9] row-major | t_p[3] | P[36] row-major in the order (w, dt)) and, when out is
 // not nullptr, writes its POSE_PRIOR_REC doubles: the upper-triangular L with L^T L = P^-1 packed by rows, R_p, t_p.
 // R_p must be a rotation (|R_p^T R_p - I|_max <= 1e-9, det > 0), every value finite, P symmetric to 1e-12 of its
@@ -2255,8 +2259,7 @@ int prior_factor(const char* fn, int c, const double* p, double* out) {
         return set_error(COSL_E_INVALID, "%s: P of camera %d's prior is not symmetric (%d, %d)", fn, c, a, b);
   // P = G G^T, P^-1 = G^-T G^-1 = C C^T and L = C^T
   double S[36], G[36], Gi[36] = {}, Pi[36], C[36];
-  for (int a = 0; a < 6; ++a)
-    for (int b = 0; b < 6; ++b) S[6 * a + b] = 0.5 * (P[6 * a + b] + P[6 * b + a]);
+  sym6(P, S);
   if (!chol6(S, G)) return set_error(COSL_E_INVALID, "%s: P of camera %d's prior is not positive definite", fn, c);
   for (int k = 0; k < 6; ++k)  // G^-1, lower, by forward substitution of the unit columns
     for (int i = k; i < 6; ++i) {
@@ -2327,6 +2330,16 @@ bool point_cov(const double* P, double S[6]) {
   return d2 > 0 && std::isfinite(d2);
 }
 
+// A symmetric 3x3 packed as (xx xy xz yy yz zz), unpacked into P (row-major)
+void unpack_sym3(const double* S, double P[9]) {
+  P[0] = S[0];
+  P[1] = P[3] = S[1];
+  P[2] = P[6] = S[2];
+  P[4] = S[3];
+  P[5] = P[7] = S[4];
+  P[8] = S[5];
+}
+
 // Checks the map points of one submit, naming the first bad camera and point; *tot = map points over all cameras.
 int check_mappts(const char* fn, int C, int cap, const MapPtsArgs& mp, long long* tot) {
   if (!mp.n || !mp.X || !mp.P || !mp.m) return set_error(COSL_E_INVALID, "%s: null map-point argument", fn);
@@ -2360,16 +2373,44 @@ int check_mappts(const char* fn, int C, int cap, const MapPtsArgs& mp, long long
   return COSL_OK;
 }
 
+// The section at byte offset `off` of a staging buffer or of its device copy
+template <class T>
+T* section(unsigned char* base, size_t off) {
+  return reinterpret_cast<T*>(base + off);
+}
+
+// The sections of a pose solve's staging buffer and its device copy: PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot]
+// | L[3 tot] | prior[C][POSE_PRIOR_REC] | hasPrior[C] | map[nmap][MAPPT_IN] | blk[nblk] (tot = points of the solve).
+// The whitening factors L are carried by the submits with covariances, the priors by a submit with some prior, and
+// the map points and the CTA table of pose_mappt_kernel by cosl_pose_solver_submit_mappts.  A section a submit does
+// not carry takes 0 bytes, so its one copy of `bytes` stops within 255 bytes of the end of the last one it carries.
+struct PoseLayout {
+  size_t cams, M, m, prev, L, rec, has, map, blk, bytes;
+};
+
+PoseLayout pose_layout(int C, long long tot, bool obsCov, bool prior, long long nmap, int nblk) {
+  SlabLayout S;
+  PoseLayout o;
+  o.cams = S.take(sizeof(PoseCam) * C);
+  o.M = S.take(sizeof(double) * 3 * tot);
+  o.m = S.take(sizeof(double) * 2 * tot);
+  o.prev = S.take(sizeof(double) * tot);
+  o.L = S.take(obsCov ? sizeof(double) * 3 * tot : 0);
+  o.rec = S.take(prior ? sizeof(double) * POSE_PRIOR_REC * C : 0);
+  o.has = S.take(prior ? sizeof(int) * C : 0);
+  o.map = S.take(sizeof(double) * MAPPT_IN * nmap);
+  o.blk = S.take(sizeof(int4) * nblk);
+  o.bytes = S.bytes;
+  return o;
+}
+
 }  // namespace
 
-// A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out as
-// PoseCam[C] | M[3 tot] | m[2 tot] | prevErrs[tot] | L[3 tot] | prior[C][POSE_PRIOR_REC] | hasPrior[C] |
-// map[nmap][MAPPT_IN] | blk[nblk] (tot = points of the solve; the whitening factors L are staged and copied by the
-// submits with covariances only, the priors, right after the last section copied, by a submit with some prior, and
-// the map points, 16-byte aligned after the last section copied, by cosl_pose_solver_submit_mappts); the PoseOuts
-// come back into pinned memory.  Capacity is fixed at create: everything is allocated once, the covariance stage's
-// buffers (laid out as res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed, and the map-point sections
-// and results (mres[nmap][MAPPT_OUT]) by cosl_pose_solver_reserve_mappts, which reallocates the staging buffers.
+// A pose solver handle.  The inputs of one solve travel in one copy from a pinned staging buffer laid out by
+// pose_layout; the PoseOuts come back into pinned memory.  Capacity is fixed at create: everything is allocated once,
+// the covariance stage's buffers (laid out as res[C][POSE_COV_STRIDE] | err[tot]) when the handle is first armed, and
+// the map-point sections and results (mres[nmap][MAPPT_OUT]) by cosl_pose_solver_reserve_mappts, which reallocates the
+// staging buffers.
 struct cosl_pose_solver {
   int device = 0, maxCams = 0, maxPts = 0;
   RequestStream rq;
@@ -2380,6 +2421,7 @@ struct cosl_pose_solver {
   PoseOut* h_out = nullptr;
   int C = 0;           // cameras of the solve in flight
   long long tot = 0;   // points of the solve in flight
+  PoseLayout lay = {}; // its staged sections
   double pixelVar = 0; // > 0: armed
   double* d_cov = nullptr;
   double* h_cov = nullptr;
@@ -2415,28 +2457,11 @@ struct cosl_pose_solver {
 
 namespace {
 
-size_t input_bytes(int C, long long tot) { return sizeof(PoseCam) * C + sizeof(double) * 6 * tot; }
-// the staged inputs followed by the whitening factors of cosl_pose_solver_submit_cov
-size_t input_bytes_cov(int C, long long tot) { return input_bytes(C, tot) + sizeof(double) * 3 * tot; }
-// the prior records and flags of cosl_pose_solver_submit_prior, staged after the inputs
-size_t prior_bytes(int C) { return (sizeof(double) * POSE_PRIOR_REC + sizeof(int)) * C; }
-size_t prior_offset(int C, long long tot, bool obsCov) {
-  return obsCov ? input_bytes_cov(C, tot) : input_bytes(C, tot);
-}
-// the map points of cosl_pose_solver_submit_mappts, 16-byte aligned after the last section copied
-size_t mappt_offset(int C, long long tot, bool obsCov, bool prior) {
-  const size_t o = prior_offset(C, tot, obsCov) + (prior ? prior_bytes(C) : 0);
-  return (o + 15) & ~(size_t)15;
-}
-// nmap records and at most nblk CTAs of pose_mappt_kernel
-size_t mappt_bytes(long long nmap, int nblk) { return sizeof(double) * MAPPT_IN * nmap + sizeof(int4) * nblk; }
-// a bound on the CTAs of nmap map points over C cameras: sum_c ceil(n_c / MAPPT_THREADS)
-int mappt_max_blocks(int C, long long nmap) { return (int)(nmap / MAPPT_THREADS) + C; }
-// the staging buffers' size: every section at capacity
-size_t input_capacity(int maxCams, int maxPts, int maxMap) {
-  size_t in = input_bytes_cov(maxCams, maxPts) + prior_bytes(maxCams);
-  if (maxMap > 0) in += 16 + mappt_bytes(maxMap, mappt_max_blocks(maxCams, maxMap));
-  return in;
+// the staging buffers' size: every section at the handle's maxima, with maxMap map points and a bound on their CTAs
+// (sum_c ceil(n_c / MAPPT_THREADS), none without points)
+size_t pose_capacity(const cosl_pose_solver* s, int maxMap) {
+  const int maxBlk = (int)std::min<long long>(maxMap, maxMap / MAPPT_THREADS + s->maxCams);
+  return pose_layout(s->maxCams, s->maxPts, true, true, maxMap, maxBlk).bytes;
 }
 
 void free_pose_solver(cosl_pose_solver* s) {
@@ -2466,7 +2491,7 @@ size_t cov_doubles(int C, long long tot) { return (size_t)POSE_COV_STRIDE * C + 
 int alloc_pose_solver(cosl_pose_solver* s) {
   COSL_CUDA(cudaSetDevice(s->device));
   COSL_TRY(s->rq.create());
-  const size_t in = input_capacity(s->maxCams, s->maxPts, s->maxMap);
+  const size_t in = pose_capacity(s, s->maxMap);
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
   COSL_CUDA(cudaHostAlloc(&s->h_out, sizeof(PoseOut) * s->maxCams, cudaHostAllocPortable));
   COSL_CUDA(cudaMalloc(&s->d_in, in));
@@ -2475,19 +2500,15 @@ int alloc_pose_solver(cosl_pose_solver* s) {
   return COSL_OK;
 }
 
-// The PRIOR instantiations, named: their template argument lists do not fit the launch macro
-constexpr auto pose_intracam_prior = pose_intracam_kernel<false, true, PosePriorDev>;
-constexpr auto pose_intracam_obscov_prior = pose_intracam_kernel<true, true, PosePriorDev>;
-constexpr auto pose_cov_prior = pose_cov_kernel<false, true, PosePriorDev>;
-constexpr auto pose_cov_obscov_prior = pose_cov_kernel<true, true, const double*, PosePriorDev>;
-
 size_t ransac_res_bytes(int C, long long tot) { return sizeof(double) * RANSAC_RES * C + tot; }
 size_t ransac_hyp_smem() { return sizeof(double) * RS_N * RANSAC_HYP_THREADS; }
 
 // PnP RANSAC of the armed cameras on the staged inputs: hypotheses, scores, selection (which rewrites the records'
 // R0, t0 it replaces), and the results' read-back.  Enqueued after the inputs' copy and before the solve.
-int enqueue_ransac(cosl_pose_solver* s, int C, long long tot, const double* d_M, const double* d_m) {
-  PoseCam* d_cams = reinterpret_cast<PoseCam*>(s->d_in);
+int enqueue_ransac(cosl_pose_solver* s, int C, long long tot) {
+  PoseCam* d_cams = section<PoseCam>(s->d_in, s->lay.cams);
+  const double* d_M = section<const double>(s->d_in, s->lay.M);
+  const double* d_m = section<const double>(s->d_in, s->lay.m);
   cudaStream_t st = s->rq.stream;
   const int nh = s->rHyp;
   double* d_res = reinterpret_cast<double*>(s->d_rres);
@@ -2505,59 +2526,36 @@ int enqueue_ransac(cosl_pose_solver* s, int C, long long tot, const double* d_M,
   return COSL_OK;
 }
 
-// The staged inputs of C cameras and tot points: copy, kernel, read-back.  s->obsCov selects the whitened
-// instantiations and copies the factors with the rest; s->prior the PRIOR instantiations and the prior records.
+// The staged inputs of C cameras and tot points (the sections of s->lay): copy, kernels, read-backs.  s->obsCov
+// selects the whitened instantiations, s->prior the PRIOR ones.
 int enqueue_solve(cosl_pose_solver* s, int C, long long tot, const PoseCfg& cfg) {
-  const PoseCam* d_cams = reinterpret_cast<const PoseCam*>(s->d_in);
-  const double* d_M = reinterpret_cast<const double*>(s->d_in + sizeof(PoseCam) * C);
-  const double* d_m = d_M + 3 * tot;
-  const double* d_p = d_m + 2 * tot;
-  const double* d_L = d_p + tot;
-  const size_t poff = prior_offset(C, tot, s->obsCov);
-  PosePriorDev pr;
-  pr.rec = reinterpret_cast<const double*>(s->d_in + poff);
-  pr.has = reinterpret_cast<const int*>(s->d_in + poff + sizeof(double) * POSE_PRIOR_REC * C);
+  const PoseLayout& lay = s->lay;
+  const PoseCam* d_cams = section<const PoseCam>(s->d_in, lay.cams);
+  const double* d_M = section<const double>(s->d_in, lay.M);
+  const double* d_m = section<const double>(s->d_in, lay.m);
+  const double* d_p = section<const double>(s->d_in, lay.prev);
+  const double* d_L = section<const double>(s->d_in, lay.L);
+  const PosePriorDev pr{section<const double>(s->d_in, lay.rec), section<const int>(s->d_in, lay.has)};
   cudaStream_t st = s->rq.stream;
-  const size_t moff = mappt_offset(C, tot, s->obsCov, s->prior);
-  const size_t bytes = s->map ? moff + mappt_bytes(s->nmap, s->nblk) : s->prior ? poff + prior_bytes(C) : poff;
-  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, bytes, cudaMemcpyHostToDevice, st));
-  if (s->ransac) COSL_TRY(enqueue_ransac(s, C, tot, d_M, d_m));
-  if (s->prior && s->obsCov)
-    COSL_LAUNCH(pose_intracam_obscov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg,
-                s->d_out, d_L, pr);
-  else if (s->prior)
-    COSL_LAUNCH(pose_intracam_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg,
-                s->d_out, nullptr, pr);
-  else if (s->obsCov)
-    COSL_LAUNCH(pose_intracam_kernel<true>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out,
-                d_L);
-  else
-    COSL_LAUNCH(pose_intracam_kernel<false>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out,
-                nullptr);
+  COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, lay.bytes, cudaMemcpyHostToDevice, st));
+  if (s->ransac) COSL_TRY(enqueue_ransac(s, C, tot));
+  const auto solve = s->obsCov ? (s->prior ? pose_intracam_kernel<true, true> : pose_intracam_kernel<true, false>)
+                               : (s->prior ? pose_intracam_kernel<false, true> : pose_intracam_kernel<false, false>);
+  COSL_LAUNCH(solve, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, d_p, s->d_W, cfg, s->d_out, d_L, pr);
   COSL_CUDA(cudaGetLastError());
   COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(PoseOut) * C, cudaMemcpyDeviceToHost, st));
   if (s->pixelVar > 0) {
     double* d_res = s->d_cov;
     double* d_err = s->d_cov + POSE_COV_STRIDE * C;
-    if (s->prior && s->obsCov)
-      COSL_LAUNCH(pose_cov_obscov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau,
-                  s->pixelVar, d_res, d_err, d_L, pr);
-    else if (s->prior)
-      COSL_LAUNCH(pose_cov_prior, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau,
-                  s->pixelVar, d_res, d_err, pr);
-    else if (s->obsCov)
-      COSL_LAUNCH(pose_cov_kernel<true>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar,
-                  d_res, d_err, d_L);
-    else
-      COSL_LAUNCH(pose_cov_kernel<false>, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar,
-                  d_res, d_err);
+    const auto stage = s->obsCov ? (s->prior ? pose_cov_kernel<true, true> : pose_cov_kernel<true, false>)
+                                 : (s->prior ? pose_cov_kernel<false, true> : pose_cov_kernel<false, false>);
+    COSL_LAUNCH(stage, C, POSE_THREADS, 0, st, d_cams, d_M, d_m, s->d_out, cfg.tau, s->pixelVar, d_res, d_err, d_L,
+                pr);
     COSL_CUDA(cudaGetLastError());
     COSL_CUDA(cudaMemcpyAsync(s->h_cov, s->d_cov, sizeof(double) * cov_doubles(C, tot), cudaMemcpyDeviceToHost, st));
     if (s->map && s->nblk > 0) {  // submit_mappts requires an armed handle
-      const double* d_map = reinterpret_cast<const double*>(s->d_in + moff);
-      const int4* d_blk = reinterpret_cast<const int4*>(d_map + (size_t)MAPPT_IN * s->nmap);
-      COSL_LAUNCH(pose_mappt_kernel, s->nblk, MAPPT_THREADS, 0, st, d_blk, d_map, d_cams, s->d_out, d_res, s->gate,
-                  s->d_mres);
+      COSL_LAUNCH(pose_mappt_kernel, s->nblk, MAPPT_THREADS, 0, st, section<const int4>(s->d_in, lay.blk),
+                  section<const double>(s->d_in, lay.map), d_cams, s->d_out, d_res, s->gate, s->d_mres);
       COSL_CUDA(cudaGetLastError());
       COSL_CUDA(cudaMemcpyAsync(s->h_mres, s->d_mres, sizeof(double) * MAPPT_OUT * s->nmap, cudaMemcpyDeviceToHost,
                                 st));
@@ -2594,12 +2592,16 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
     COSL_TRY(check_mappts(fn, C, s->maxMap, *mp, &nmap));
   }
   COSL_CUDA(cudaSetDevice(s->device));
+  int nblk = 0;  // one CTA of pose_mappt_kernel per MAPPT_THREADS map points of a camera
+  if (mp)
+    for (int c = 0; c < C; ++c) nblk += div_up(mp->n[c], MAPPT_THREADS);
+  const PoseLayout lay = pose_layout(C, tot, covx != nullptr, anyPrior, nmap, nblk);
   // nothing is in flight, so no copy reads the staging buffer any more
-  PoseCam* cams = reinterpret_cast<PoseCam*>(s->h_in);
-  double* hM = reinterpret_cast<double*>(s->h_in + sizeof(PoseCam) * C);
-  double* hm = hM + 3 * tot;
-  double* hp = hm + 2 * tot;
-  double* hL = hp + tot;
+  PoseCam* cams = section<PoseCam>(s->h_in, lay.cams);
+  double* hM = section<double>(s->h_in, lay.M);
+  double* hm = section<double>(s->h_in, lay.m);
+  double* hp = section<double>(s->h_in, lay.prev);
+  double* hL = section<double>(s->h_in, lay.L);
   long long off = 0;
   for (int c = 0; c < C; ++c) {
     std::memcpy(cams[c].K, K9 + 9 * c, sizeof(double) * 9);
@@ -2629,22 +2631,19 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
     off += npts[c];
   }
   if (anyPrior) {
-    const size_t poff = prior_offset(C, tot, covx != nullptr);
-    double* hq = reinterpret_cast<double*>(s->h_in + poff);
-    int* hh = reinterpret_cast<int*>(s->h_in + poff + sizeof(double) * POSE_PRIOR_REC * C);
+    double* hq = section<double>(s->h_in, lay.rec);
+    int* hh = section<int>(s->h_in, lay.has);
     for (int c = 0; c < C; ++c) {
       hh[c] = prior[c] ? 1 : 0;
       // a camera without a prior leaves its record unset: the kernels do not read it
       if (prior[c]) prior_factor(fn, c, prior[c], hq + POSE_PRIOR_REC * (size_t)c);
     }
   }
-  int nblk = 0;
-  if (mp) {  // records camera-major, then one CTA per MAPPT_THREADS points of a camera
-    const size_t moff = mappt_offset(C, tot, covx != nullptr, anyPrior);
-    double* hr = reinterpret_cast<double*>(s->h_in + moff);
-    int4* hb = reinterpret_cast<int4*>(hr + (size_t)MAPPT_IN * nmap);
-    const double pv = s->pixelVar;
+  if (mp) {  // records camera-major, then the CTA table
+    double* hr = section<double>(s->h_in, lay.map);
+    int4* hb = section<int4>(s->h_in, lay.blk);
     long long j = 0;
+    int b = 0;
     for (int c = 0; c < C; ++c) {
       for (int i = 0; i < mp->n[c]; ++i) {
         double* r = hr + (size_t)MAPPT_IN * (j + i);
@@ -2657,14 +2656,10 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
         r[7] = 0.5 * (P[5] + P[7]);
         r[8] = P[8];
         std::memcpy(r + 9, mp->m[c] + 2 * (size_t)i, sizeof(double) * 2);
-        // Sigma_m = pixel_var I when the camera has no covm
-        const double* v = (mp->cov && mp->cov[c]) ? mp->cov[c] + 4 * (size_t)i : nullptr;
-        r[11] = v ? v[0] : pv;
-        r[12] = v ? v[1] : 0.0;
-        r[13] = v ? v[3] : pv;
+        pack_cov2((mp->cov && mp->cov[c]) ? mp->cov[c] + 4 * (size_t)i : nullptr, s->pixelVar, r + 11);
       }
       for (int i = 0; i < mp->n[c]; i += MAPPT_THREADS)
-        hb[nblk++] = make_int4(c, (int)(j + i), (int)(j + std::min(i + MAPPT_THREADS, mp->n[c])), 0);
+        hb[b++] = make_int4(c, (int)(j + i), (int)(j + std::min(i + MAPPT_THREADS, mp->n[c])), 0);
       j += mp->n[c];
     }
   }
@@ -2678,6 +2673,7 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
   cfg.tau = tau;
   s->C = C;
   s->tot = tot;
+  s->lay = lay;
   s->covReady = false;
   s->obsCov = covx != nullptr;
   s->prior = anyPrior;
@@ -2702,9 +2698,9 @@ int submit_solve(const char* fn, cosl_pose_solver* s, int C, const double* K9, c
 }  // namespace
 
 // A triangulation handle (cosl_tri_solver).  The inputs of one submit travel in one copy from a pinned staging buffer
-// laid out as TriCam[nCams] | views[nViews][TRI_VIEW] | viewOff[nPts + 1] | viewCam[nViews]; TRI_OUT doubles per
-// point come back into pinned memory.  Everything, the per-view scratch included, is allocated by create for at most
-// maxCams camera entries, maxPts points and maxViews views per submit.
+// in the sections of tri_layout, TriCam[nCams] | views[nViews][TRI_VIEW] | viewOff[nPts + 1] | viewCam[nViews];
+// TRI_OUT doubles per point come back into pinned memory.  Everything, the per-view scratch included, is allocated by
+// create for at most maxCams camera entries, maxPts points and maxViews views per submit.
 struct cosl_tri_solver {
   int device = 0, maxCams = 0, maxPts = 0, maxViews = 0;
   RequestStream rq;
@@ -2719,8 +2715,20 @@ struct cosl_tri_solver {
 
 namespace {
 
-size_t tri_bytes(int nCams, int nPts, int nViews) {
-  return sizeof(TriCam) * nCams + sizeof(double) * TRI_VIEW * nViews + sizeof(int) * ((size_t)nPts + 1 + nViews);
+// The sections of a triangulation submit's staging buffer and its device copy
+struct TriLayout {
+  size_t cams, views, viewOff, viewCam, bytes;
+};
+
+TriLayout tri_layout(int nCams, int nPts, int nViews) {
+  SlabLayout S;
+  TriLayout o;
+  o.cams = S.take(sizeof(TriCam) * nCams);
+  o.views = S.take(sizeof(double) * TRI_VIEW * nViews);
+  o.viewOff = S.take(sizeof(int) * ((size_t)nPts + 1));
+  o.viewCam = S.take(sizeof(int) * (size_t)nViews);
+  o.bytes = S.bytes;
+  return o;
 }
 
 void free_tri_solver(cosl_tri_solver* s) {
@@ -2740,7 +2748,7 @@ int alloc_tri_solver(cosl_tri_solver* s) {
   if (!s->seen) return set_error(COSL_E_NOMEM, "cosl_tri_solver_create: out of host memory");
   COSL_CUDA(cudaSetDevice(s->device));
   COSL_TRY(s->rq.create());
-  const size_t in = tri_bytes(s->maxCams, s->maxPts, s->maxViews);
+  const size_t in = tri_layout(s->maxCams, s->maxPts, s->maxViews).bytes;
   const size_t outb = sizeof(double) * TRI_OUT * s->maxPts;
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
   COSL_CUDA(cudaHostAlloc(&s->h_out, outb, cudaHostAllocPortable));
@@ -2817,9 +2825,9 @@ int stage_tri(cosl_tri_solver* s, int nCams, const double* K9, const double* R, 
               const double* const* camCov, int nPts, const int* viewOff, const int* viewCam, const double* m,
               const double* covm, double pixel_var, double max_err) {
   const int nViews = viewOff[nPts];
-  TriCam* hc = reinterpret_cast<TriCam*>(s->h_in);
-  double* hv = reinterpret_cast<double*>(s->h_in + sizeof(TriCam) * nCams);
-  int* ho = reinterpret_cast<int*>(hv + (size_t)TRI_VIEW * nViews);
+  const TriLayout lay = tri_layout(nCams, nPts, nViews);
+  TriCam* hc = section<TriCam>(s->h_in, lay.cams);
+  double* hv = section<double>(s->h_in, lay.views);
   for (int c = 0; c < nCams; ++c) {
     TriCam& e = hc[c];
     const double* k = K9 + 9 * c;
@@ -2835,31 +2843,24 @@ int stage_tri(cosl_tri_solver* s, int nCams, const double* K9, const double* R, 
     for (int i = 0; i < 9; ++i) e.Ki[i] = adj[i] / det;
     e.hasP = camCov && camCov[c] ? 1 : 0;
     e.pad = 0;
-    if (e.hasP)  // symmetrised, as prior_factor checked it
-      for (int a = 0; a < 6; ++a)
-        for (int b = 0; b < 6; ++b) e.P[6 * a + b] = 0.5 * (camCov[c][6 * a + b] + camCov[c][6 * b + a]);
+    if (e.hasP) sym6(camCov[c], e.P);  // symmetrised, as prior_factor checked it
   }
   for (int v = 0; v < nViews; ++v) {
     double* q = hv + (size_t)TRI_VIEW * v;
     q[0] = m[2 * (size_t)v];
     q[1] = m[2 * (size_t)v + 1];
-    const double* cv = covm ? covm + 4 * (size_t)v : nullptr;  // Sigma_m = pixel_var I without covm
-    q[2] = cv ? cv[0] : pixel_var;
-    q[3] = cv ? cv[1] : 0.0;
-    q[4] = cv ? cv[3] : pixel_var;
+    pack_cov2(covm ? covm + 4 * (size_t)v : nullptr, pixel_var, q + 2);
   }
-  std::memcpy(ho, viewOff, sizeof(int) * ((size_t)nPts + 1));
-  if (nViews) std::memcpy(ho + nPts + 1, viewCam, sizeof(int) * (size_t)nViews);
+  std::memcpy(section<int>(s->h_in, lay.viewOff), viewOff, sizeof(int) * ((size_t)nPts + 1));
+  if (nViews) std::memcpy(section<int>(s->h_in, lay.viewCam), viewCam, sizeof(int) * (size_t)nViews);
   s->nPts = nPts;
   cudaStream_t st = s->rq.stream;
   return s->rq.submit("cosl_tri_solver_submit", [&]() -> int {
-    COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, tri_bytes(nCams, nPts, nViews), cudaMemcpyHostToDevice, st));
+    COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, lay.bytes, cudaMemcpyHostToDevice, st));
     if (nPts > 0) {
-      const TriCam* d_cams = reinterpret_cast<const TriCam*>(s->d_in);
-      const double* d_views = reinterpret_cast<const double*>(s->d_in + sizeof(TriCam) * nCams);
-      const int* d_off = reinterpret_cast<const int*>(d_views + (size_t)TRI_VIEW * nViews);
-      COSL_LAUNCH(tri_kernel, div_up(nPts, TRI_THREADS), TRI_THREADS, 0, st, d_cams, d_views, d_off,
-                  d_off + nPts + 1, nPts, max_err, s->d_scratch, s->d_out);
+      COSL_LAUNCH(tri_kernel, div_up(nPts, TRI_THREADS), TRI_THREADS, 0, st, section<const TriCam>(s->d_in, lay.cams),
+                  section<const double>(s->d_in, lay.views), section<const int>(s->d_in, lay.viewOff),
+                  section<const int>(s->d_in, lay.viewCam), nPts, max_err, s->d_scratch, s->d_out);
       COSL_CUDA(cudaGetLastError());
       COSL_CUDA(cudaMemcpyAsync(s->h_out, s->d_out, sizeof(double) * TRI_OUT * nPts, cudaMemcpyDeviceToHost, st));
     }
@@ -2870,11 +2871,12 @@ int stage_tri(cosl_tri_solver* s, int nCams, const double* K9, const double* R, 
 }  // namespace
 
 // A registration handle (cosl_assoc_solver).  The inputs of one submit travel in one copy from a pinned staging buffer
-// laid out as AssocCam[nCams] | pts[nPts][ASSOC_PT] | feats[nFeats][ASSOC_FEAT] | trkM[nTrk][2] | featOff[nCams + 1] |
-// cell[nFeats] | owned[nFeats] | trkOff[nFeats + 1] | trkCam[nTrk] | qPt[nQ] | qCam[nQ]; ASSOC_OUT doubles per query
-// pair come back into pinned memory.  The grid (count and start per cell, the features sorted by cell) and the claim
-// keys live on the device only.  Everything is allocated by create for at most maxCams camera entries, maxPts points,
-// maxQueries query pairs, maxFeats features and maxTrackObs track observations per submit.
+// in the sections of assoc_layout, AssocCam[nCams] | pts[nPts][ASSOC_PT] | feats[nFeats][ASSOC_FEAT] | trkM[nTrk][2] |
+// featOff[nCams + 1] | cell[nFeats] | owned[nFeats] | trkOff[nFeats + 1] | trkCam[nTrk] | qPt[nQ] | qCam[nQ];
+// ASSOC_OUT doubles per query pair come back into pinned memory.  The grid (count and start per cell, the features
+// sorted by cell) and the claim keys live on the device only.  Everything is allocated by create for at most maxCams
+// camera entries, maxPts points, maxQueries query pairs, maxFeats features and maxTrackObs track observations per
+// submit.
 struct cosl_assoc_solver {
   int device = 0, maxCams = 0, maxPts = 0, maxQueries = 0, maxFeats = 0, maxTrackObs = 0;
   RequestStream rq;
@@ -2893,10 +2895,27 @@ struct cosl_assoc_solver {
 
 namespace {
 
-size_t assoc_bytes(int nCams, int nPts, int nFeats, int nTrk, int nQ) {
-  return sizeof(AssocCam) * nCams +
-         sizeof(double) * ((size_t)ASSOC_PT * nPts + (size_t)ASSOC_FEAT * nFeats + 2 * (size_t)nTrk) +
-         sizeof(int) * ((size_t)nCams + 1 + 3 * (size_t)nFeats + 1 + nTrk + 2 * (size_t)nQ);
+// The sections of a registration submit's staging buffer and its device copy
+struct AssocLayout {
+  size_t cams, pts, feats, trkM, featOff, cell, owned, trkOff, trkCam, qPt, qCam, bytes;
+};
+
+AssocLayout assoc_layout(int nCams, int nPts, int nFeats, int nTrk, int nQ) {
+  SlabLayout S;
+  AssocLayout o;
+  o.cams = S.take(sizeof(AssocCam) * nCams);
+  o.pts = S.take(sizeof(double) * ASSOC_PT * nPts);
+  o.feats = S.take(sizeof(double) * ASSOC_FEAT * nFeats);
+  o.trkM = S.take(sizeof(double) * 2 * nTrk);
+  o.featOff = S.take(sizeof(int) * ((size_t)nCams + 1));
+  o.cell = S.take(sizeof(int) * nFeats);
+  o.owned = S.take(sizeof(int) * nFeats);
+  o.trkOff = S.take(sizeof(int) * ((size_t)nFeats + 1));
+  o.trkCam = S.take(sizeof(int) * nTrk);
+  o.qPt = S.take(sizeof(int) * nQ);
+  o.qCam = S.take(sizeof(int) * nQ);
+  o.bytes = S.bytes;
+  return o;
 }
 
 void free_assoc_solver(cosl_assoc_solver* s) {
@@ -2920,7 +2939,7 @@ int alloc_assoc_solver(cosl_assoc_solver* s) {
   if (!s->seen) return set_error(COSL_E_NOMEM, "cosl_assoc_solver_create: out of host memory");
   COSL_CUDA(cudaSetDevice(s->device));
   COSL_TRY(s->rq.create());
-  const size_t in = assoc_bytes(s->maxCams, s->maxPts, s->maxFeats, s->maxTrackObs, s->maxQueries);
+  const size_t in = assoc_layout(s->maxCams, s->maxPts, s->maxFeats, s->maxTrackObs, s->maxQueries).bytes;
   const size_t outb = sizeof(double) * ASSOC_OUT * s->maxQueries;
   const size_t cells = (size_t)s->maxCams * ASSOC_MAX_CELLS;
   COSL_CUDA(cudaHostAlloc(&s->h_in, in, cudaHostAllocPortable));
@@ -3041,17 +3060,14 @@ int check_assoc(const char* fn, cosl_assoc_solver* s, const AssocArgs& a) {
 int stage_assoc(cosl_assoc_solver* s, const AssocArgs& a) {
   const int nCams = a.nCams, nPts = a.nPts, nF = a.featOff[nCams];
   const int nTrk = a.trkOff ? a.trkOff[nF] : 0, nQ = a.qOff[nPts];
-  AssocCam* hc = reinterpret_cast<AssocCam*>(s->h_in);
-  double* hp = reinterpret_cast<double*>(hc + nCams);
-  double* hf = hp + (size_t)ASSOC_PT * nPts;
-  double* hm = hf + (size_t)ASSOC_FEAT * nF;
-  int* hoff = reinterpret_cast<int*>(hm + 2 * (size_t)nTrk);
-  int* hcell = hoff + nCams + 1;
-  int* hown = hcell + nF;
-  int* htoff = hown + nF;
-  int* htcam = htoff + nF + 1;
-  int* hqpt = htcam + nTrk;
-  int* hqcam = hqpt + nQ;
+  const AssocLayout lay = assoc_layout(nCams, nPts, nF, nTrk, nQ);
+  AssocCam* hc = section<AssocCam>(s->h_in, lay.cams);
+  double* hp = section<double>(s->h_in, lay.pts);
+  double* hf = section<double>(s->h_in, lay.feats);
+  int* hcell = section<int>(s->h_in, lay.cell);
+  int* hown = section<int>(s->h_in, lay.owned);
+  int* htoff = section<int>(s->h_in, lay.trkOff);
+  int* hqpt = section<int>(s->h_in, lay.qPt);
   int cells = 0;
   for (int c = 0; c < nCams; ++c) {
     AssocCam& e = hc[c];
@@ -3059,9 +3075,7 @@ int stage_assoc(cosl_assoc_solver* s, const AssocArgs& a) {
     std::memcpy(e.R, a.R + 9 * c, sizeof(double) * 9);
     std::memcpy(e.t, a.t + 3 * c, sizeof(double) * 3);
     e.hasP = a.camCov && a.camCov[c] ? 1 : 0;
-    if (e.hasP)  // symmetrised, as prior_factor checked it
-      for (int i = 0; i < 6; ++i)
-        for (int k = 0; k < 6; ++k) e.P[6 * i + k] = 0.5 * (a.camCov[c][6 * i + k] + a.camCov[c][6 * k + i]);
+    if (e.hasP) sym6(a.camCov[c], e.P);  // symmetrised, as prior_factor checked it
     e.W = a.wh[2 * c];
     e.H = a.wh[2 * c + 1];
     e.nx = (a.wh[2 * c] + ASSOC_CELL - 1) / ASSOC_CELL;
@@ -3072,12 +3086,9 @@ int stage_assoc(cosl_assoc_solver* s, const AssocArgs& a) {
     double lam = 0.0;
     for (int f = a.featOff[c]; f < a.featOff[c + 1]; ++f) {
       double* q = hf + (size_t)ASSOC_FEAT * f;
-      const double* cv = a.covf ? a.covf + 4 * (size_t)f : nullptr;
       q[0] = a.mf[2 * (size_t)f];
       q[1] = a.mf[2 * (size_t)f + 1];
-      q[2] = cv ? cv[0] : a.pixel_var;
-      q[3] = cv ? cv[1] : 0.0;
-      q[4] = cv ? cv[3] : a.pixel_var;
+      pack_cov2(a.covf ? a.covf + 4 * (size_t)f : nullptr, a.pixel_var, q + 2);
       const double h = 0.5 * (q[2] - q[4]);
       lam = std::max(lam, 0.5 * (q[2] + q[4]) + std::sqrt(h * h + q[3] * q[3]));
       const double cx = std::max(0.0, std::min(e.nx - 1.0, std::floor(q[0] / ASSOC_CELL)));
@@ -3092,35 +3103,28 @@ int stage_assoc(cosl_assoc_solver* s, const AssocArgs& a) {
     point_cov(a.PX + 9 * (size_t)j, p + 3);  // symmetrised, as check_assoc accepted it
     for (int q = a.qOff[j]; q < a.qOff[j + 1]; ++q) hqpt[q] = j;
   }
-  if (nTrk) std::memcpy(hm, a.trkM, sizeof(double) * 2 * (size_t)nTrk);
-  std::memcpy(hoff, a.featOff, sizeof(int) * ((size_t)nCams + 1));
+  if (nTrk) std::memcpy(section<double>(s->h_in, lay.trkM), a.trkM, sizeof(double) * 2 * (size_t)nTrk);
+  std::memcpy(section<int>(s->h_in, lay.featOff), a.featOff, sizeof(int) * ((size_t)nCams + 1));
   for (int f = 0; f < nF; ++f) hown[f] = a.owned ? a.owned[f] : 0;
   if (a.trkOff) std::memcpy(htoff, a.trkOff, sizeof(int) * ((size_t)nF + 1));
   else std::fill(htoff, htoff + nF + 1, 0);
-  if (nTrk) std::memcpy(htcam, a.trkCam, sizeof(int) * (size_t)nTrk);
-  if (nQ) std::memcpy(hqcam, a.qCam, sizeof(int) * (size_t)nQ);
+  if (nTrk) std::memcpy(section<int>(s->h_in, lay.trkCam), a.trkCam, sizeof(int) * (size_t)nTrk);
+  if (nQ) std::memcpy(section<int>(s->h_in, lay.qCam), a.qCam, sizeof(int) * (size_t)nQ);
   s->nQ = nQ;
   cudaStream_t st = s->rq.stream;
   const double pv = a.pixel_var, gate = a.gate, tg = a.track_gate;
   return s->rq.submit("cosl_assoc_solver_submit", [&]() -> int {
-    COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, assoc_bytes(nCams, nPts, nF, nTrk, nQ), cudaMemcpyHostToDevice, st));
+    COSL_CUDA(cudaMemcpyAsync(s->d_in, s->h_in, lay.bytes, cudaMemcpyHostToDevice, st));
     if (nQ == 0) return COSL_OK;
-    const AssocCam* d_cams = reinterpret_cast<const AssocCam*>(s->d_in);
-    const double* d_pts = reinterpret_cast<const double*>(d_cams + nCams);
-    const double* d_feats = d_pts + (size_t)ASSOC_PT * nPts;
-    const double* d_trkM = d_feats + (size_t)ASSOC_FEAT * nF;
-    const int* d_off = reinterpret_cast<const int*>(d_trkM + 2 * (size_t)nTrk);
-    const int* d_cell = d_off + nCams + 1;
-    const int* d_own = d_cell + nF;
-    const int* d_toff = d_own + nF;
-    const int* d_tcam = d_toff + nF + 1;
-    const int* d_qpt = d_tcam + nTrk;
-    const int* d_qcam = d_qpt + nQ;
+    const AssocCam* d_cams = section<const AssocCam>(s->d_in, lay.cams);
+    const int* d_cell = section<const int>(s->d_in, lay.cell);
+    const int* d_qpt = section<const int>(s->d_in, lay.qPt);
     // the grid: count, a per-entry exclusive scan, scatter
     COSL_CUDA(cudaMemsetAsync(s->d_count, 0, sizeof(int) * (size_t)cells, st));
     if (nF) COSL_LAUNCH(assoc_count_kernel, div_up(nF, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_cell, nF,
                         s->d_count);
-    COSL_LAUNCH(assoc_scan_kernel, nCams, ASSOC_SCAN_THREADS, 0, st, d_cams, d_off, nCams, s->d_count, s->d_start);
+    COSL_LAUNCH(assoc_scan_kernel, nCams, ASSOC_SCAN_THREADS, 0, st, d_cams, section<const int>(s->d_in, lay.featOff),
+                nCams, s->d_count, s->d_start);
     if (nF) {
       COSL_LAUNCH(assoc_scatter_kernel, div_up(nF, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_cell, nF,
                   s->d_start, s->d_count, s->d_sorted);
@@ -3128,9 +3132,11 @@ int stage_assoc(cosl_assoc_solver* s, const AssocArgs& a) {
       COSL_CUDA(cudaMemsetAsync(s->d_win, 0xff, sizeof(unsigned int) * (size_t)nF, st));
     }
     // the search with pass one of the claims, pass two, and the statuses
-    COSL_LAUNCH(assoc_search_kernel, div_up(nQ, ASSOC_THREADS), ASSOC_THREADS, 0, st, d_cams, d_pts, d_feats, d_own,
-                d_toff, d_tcam, d_trkM, d_qpt, d_qcam, nQ, s->d_start, s->d_sorted, pv, gate, tg, s->d_key,
-                s->d_out);
+    COSL_LAUNCH(assoc_search_kernel, div_up(nQ, ASSOC_THREADS), ASSOC_THREADS, 0, st, d_cams,
+                section<const double>(s->d_in, lay.pts), section<const double>(s->d_in, lay.feats),
+                section<const int>(s->d_in, lay.owned), section<const int>(s->d_in, lay.trkOff),
+                section<const int>(s->d_in, lay.trkCam), section<const double>(s->d_in, lay.trkM), d_qpt,
+                section<const int>(s->d_in, lay.qCam), nQ, s->d_start, s->d_sorted, pv, gate, tg, s->d_key, s->d_out);
     COSL_LAUNCH(assoc_claim_kernel, div_up(nQ, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_qpt, nQ, s->d_key,
                 s->d_win, s->d_out);
     COSL_LAUNCH(assoc_final_kernel, div_up(nQ, ASSOC_BIN_THREADS), ASSOC_BIN_THREADS, 0, st, d_qpt, nQ, s->d_key,
@@ -3212,7 +3218,7 @@ int cosl_pose_solver_reserve_mappts(cosl_pose_solver* s, int maxMapPts) {
   if (maxMapPts == s->maxMap) return COSL_OK;
   COSL_CUDA(cudaSetDevice(s->device));
   // the new buffers first, so a failed allocation leaves the handle as it was
-  const size_t in = input_capacity(s->maxCams, s->maxPts, maxMapPts);
+  const size_t in = pose_capacity(s, maxMapPts);
   unsigned char *h_in = nullptr, *d_in = nullptr;
   double *h_mres = nullptr, *d_mres = nullptr;
   const size_t nres = sizeof(double) * MAPPT_OUT * (size_t)maxMapPts;
@@ -3260,15 +3266,7 @@ int cosl_pose_solver_download_mappts(cosl_pose_solver* s, double* X, double* P, 
   for (long long j = 0; j < s->nmap; ++j) {
     const double* r = s->h_mres + (size_t)MAPPT_OUT * j;
     if (X) std::memcpy(X + 3 * j, r, sizeof(double) * 3);
-    if (P) {
-      double* p = P + 9 * j;
-      p[0] = r[3];
-      p[1] = p[3] = r[4];
-      p[2] = p[6] = r[5];
-      p[4] = r[6];
-      p[5] = p[7] = r[7];
-      p[8] = r[8];
-    }
+    if (P) unpack_sym3(r + 3, P + 9 * j);
     if (stat) std::memcpy(stat + 3 * j, r + 9, sizeof(double) * 3);
     if (status) status[j] = (int)r[12];
   }
@@ -3549,15 +3547,7 @@ int cosl_tri_solver_collect(cosl_tri_solver* s, double* X, double* P, double* st
   for (int j = 0; j < s->nPts; ++j) {
     const double* r = s->h_out + (size_t)TRI_OUT * j;
     if (X) std::memcpy(X + 3 * (size_t)j, r, sizeof(double) * 3);
-    if (P) {
-      double* p = P + 9 * (size_t)j;
-      p[0] = r[3];
-      p[1] = p[3] = r[4];
-      p[2] = p[6] = r[5];
-      p[4] = r[6];
-      p[5] = p[7] = r[7];
-      p[8] = r[8];
-    }
+    if (P) unpack_sym3(r + 3, P + 9 * (size_t)j);
     if (stat) std::memcpy(stat + 4 * (size_t)j, r + 9, sizeof(double) * 4);
     if (status) status[j] = (int)r[13];
   }

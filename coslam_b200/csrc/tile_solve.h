@@ -35,16 +35,6 @@ struct BaTileDev {
   unsigned long long* trace;  // optional [nTasks][8]: sm id, ns at ticket / ready / done, 4 phase stamps
 };
 
-// aligned bump layout of one device block (the same offsets index its host image)
-struct SlabLayout {
-  size_t bytes = 0;
-  size_t take(size_t n) {
-    const size_t at = (bytes + 255) & ~(size_t)255;
-    bytes = at + n;
-    return at;
-  }
-};
-
 // How the solve of one plan is launched.
 struct TileLaunch {
   // The plan's tasks in the order the persistent kernel takes them: POTRF / BWD first (served by the
